@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the dense-LA hot path on N B200s of one node.
+"""bench.py -- headline benchmark of the dense-LA hot path on N H100s of one node.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     torchrun --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 ... bench.py --gpus N ...
 
 A "step" is one pass of the hot path over one batch of synthetic input: one bf16 matmul 8192^3 per GPU (BASELINE
@@ -13,6 +13,10 @@ both operands + D2H of the result inside the timed region, every step).
 Secondary objects on the same JSON line cover the other BASELINE configs: `reduce` (f32 sum of 2^28, weak + strong
 sharding with an NCCL all-reduce), `matmul_f32_4096`, `batched_bf16_4096`, `reference_equivalent` (what CubeCL's own
 wmma / vec4 kernels reach on this GPU), plus `roofline`, `roofline_reduce`, `cpu_baseline`, `clocks`.
+
+--dump-outputs DIR writes what the timed headline matmul returned in its last step, as DIR/<name>.npy (float32): a fixed,
+seeded sample of 512 output rows (16 MiB).  The inputs are seeded, so two builds run with the same arguments can be compared
+output for output.
 
 --impl reference times the reference's CPU semantics (the oracle port; the Rust reference cannot be built here) on the
 host cores, on a bounded sample of the same workload; rank 0 only.
@@ -42,7 +46,8 @@ N_MM = 8192                      # BASELINE config 3
 FLOPS_MM = 2.0 * N_MM ** 3
 N_RED = 1 << 28                  # BASELINE config 4
 BYTES_RED = N_RED * 4
-FALLBACK_PEAKS = {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0}
+# NVIDIA H100 SXM data sheet (700 W): HBM3 3.35 TB/s, dense bf16 989 TFLOP/s -- used when no measured peaks are supplied
+FALLBACK_PEAKS = {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}
 
 
 def peaks():
@@ -51,13 +56,7 @@ def peaks():
         d = json.loads(p.read_text())
         return {"hbm_gbs": float(d["hbm_gbs"]), "bf16_tflops": float(d["bf16_tflops"]),
                 "bf16_tflops_sustained": float(d.get("bf16_tflops_sustained", d["bf16_tflops"])), "source": "measured"}
-    return dict(FALLBACK_PEAKS, bf16_tflops_sustained=1400.0, source="fallback")
-
-
-def ncu_traffic():
-    """Per-launch DRAM traffic of the dominant kernels, from the committed ncu summary of this round (or None)."""
-    p = ROOT / "profiles" / "traffic.json"
-    return json.loads(p.read_text()) if p.exists() else {}
+    return dict(FALLBACK_PEAKS, bf16_tflops_sustained=FALLBACK_PEAKS["bf16_tflops"], source="data sheet")
 
 
 # ---------------------------------------------------------------------------------------------------- clocks
@@ -371,6 +370,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--quick", action="store_true", help="headline + reduce only")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write a fixed sample of the timed matmul's last output to DIR/<name>.npy (float32)")
     args = ap.parse_args()
     args.warmup = max(3, args.warmup)
     if args.impl == "reference":
@@ -445,7 +446,13 @@ def main():
     value = world * FLOPS_MM * args.steps / (ms * 1e-3) / 1e12
     per_launch_ms = ms / args.steps
     per_gpu_tflops = FLOPS_MM / (per_launch_ms * 1e-3) / 1e12
-    traffic = ncu_traffic()
+    if args.dump_outputs:
+        # the timed path's result of its last step, before any secondary row reuses `o`: 512 seeded rows of C, widened to f32
+        rows = np.sort(np.random.default_rng(20240611).choice(N_MM, size=512, replace=False))
+        got = synth.bf16_bits_to_f32(o.to_numpy(c))[rows]
+        out_dir = Path(args.dump_outputs)
+        out_dir.mkdir(parents=True, exist_ok=True)
+        np.save(out_dir / f"matmul_bf16_8192_rank{e.rank}_rows512.npy", got.astype(np.float32))
 
     line = {
         "metric": "bf16_matmul_tflops", "value": value, "unit": "TFLOP/s", "n_gpus": world, "steps": args.steps,
@@ -453,12 +460,11 @@ def main():
         "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
         "config": {"workload": f"bf16 matmul 8192x8192x8192 per GPU (f32 accumulate, bf16 out), batch [{world},8192,8192] sharded over the batch axis",
                    "parallelism": f"batch-shard x{world}, no data-path collective",
-                   "l2": "inputs_larger_than_L2 (A+B+C = 384 MiB per GPU vs 126 MB L2)", "rhs_layout": "row-major [K,N]"},
+                   "l2": "inputs_larger_than_L2 (A+B+C = 384 MiB per GPU vs 50 MB L2)", "rhs_layout": "row-major [K,N]"},
         "gpu_launches": launches * world,
         "roofline": {"bound": "tensor", "achieved": per_gpu_tflops, "peak": pk["bf16_tflops"], "unit": "TFLOP/s",
-                     "frac": per_gpu_tflops / pk["bf16_tflops"], "traffic": traffic.get("gemm_bf16_8192_dram_bytes"),
-                     "traffic_source": "static: dram__bytes_read+write of this kernel from the committed ncu --set full capture (profiles/traffic.json), not observed by this run",
-                     "peak_source": pk["source"] + " (cuBLAS bf16 burst)", "kernel": mm_kernel,
+                     "frac": per_gpu_tflops / pk["bf16_tflops"],
+                     "peak_source": pk["source"] + (" (cuBLAS bf16 burst)" if pk["source"] == "measured" else " (H100 SXM, dense bf16)"), "kernel": mm_kernel,
                      "algorithmic_flops_per_launch": FLOPS_MM},
         "clocks": clocks,
     }
@@ -524,7 +530,7 @@ def main():
             ms_ = D.max_over_ranks(ms_, dist, tdev)
         return ms_
 
-    e2e_steps = max(4, min(args.steps, 20))
+    e2e_steps = args.steps
     e2e_run(3)                                        # warm-up
     ms_e2e = e2e_run(e2e_steps)
     assert hc.view(np.uint16)[0] == 0x4600, "e2e result check failed"  # 8192 = sum of 8192 ones, exact in bf16
@@ -578,7 +584,7 @@ def main():
 
     # ------------------------------------------------------------------ reduce: f32 sum of 2^28 (1 GiB), weak + strong
     red = {"metric": "f32_reduce_sum_gbs", "unit": "GB/s", "elements": N_RED}
-    nbuf = 3                                                 # rotate 3 x 1 GiB so nothing survives in the 126 MB L2
+    nbuf = 3                                                 # rotate 3 x 1 GiB so nothing survives in the 50 MB L2
     xs = [TensorHandle.empty_contiguous(c, [N_RED], "f32") for _ in range(nbuf)]
     for i, x in enumerate(xs):
         c.fill_uniform(x.handle, "f32", N_RED, 5 + i + 10 * e.rank, 0.0, 1.0)
@@ -593,15 +599,13 @@ def main():
         k[0] += 1
         reduce.launch(c, xs[k[0] % nbuf], r_out, None, "sum")
 
-    rsteps = max(args.steps, 20)
+    rsteps = args.steps
     ms_r, _ = timed(red_local, rsteps, args.warmup)
     red_kernel = c.last_kernel()
     gbs = BYTES_RED / (ms_r / rsteps * 1e-3) / 1e9
     red["kernel_only_per_gpu"] = gbs
     line["roofline_reduce"] = {"bound": "hbm", "achieved": gbs, "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": gbs / pk["hbm_gbs"],
-                               "traffic": traffic.get("reduce_sum_2p28_dram_bytes"),
-                               "traffic_source": "static: committed ncu --set full capture (profiles/traffic.json)",
-                               "peak_source": pk["source"] + " (copy, read+write)",
+                               "peak_source": pk["source"] + (" (copy, read+write)" if pk["source"] == "measured" else " (H100 SXM HBM3)"),
                                "kernel": red_kernel, "algorithmic_bytes_per_launch": BYTES_RED,
                                "note": "3 rotating 1 GiB inputs (nothing served from L2); consecutive launches on the stream overlap through "
                                        "programmatic dependent launch (the next launch streams while this one's last block finishes) -- "
@@ -617,7 +621,7 @@ def main():
     arg_kernel = c.last_kernel()
     gbs_a = BYTES_RED / (ms_a / rsteps * 1e-3) / 1e9
     line["roofline_argmax"] = {"bound": "hbm", "achieved": gbs_a, "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": gbs_a / pk["hbm_gbs"],
-                               "traffic": None, "peak_source": pk["source"] + " (copy, read+write)", "kernel": arg_kernel,
+                               "peak_source": pk["source"] + (" (copy, read+write)" if pk["source"] == "measured" else " (H100 SXM HBM3)"), "kernel": arg_kernel,
                                "algorithmic_bytes_per_launch": BYTES_RED, "config": "argmax of 2^28 f32 (1 GiB), 3 rotating buffers"}
     parity = {}
     # exact-integer check of the headline reduce on every rank (BASELINE config 4 pattern: sum of i % 8 = 939,524,096)
@@ -715,7 +719,7 @@ def main():
     # ------------------------------------------------------------------ other BASELINE configs (N-independent per GPU)
     def other_configs():
         if not args.quick:
-            extra_steps = max(5, min(args.steps, 10))
+            extra_steps = args.steps
             n4 = 4096
             # config 5: batched bf16, 8 x 4096^3 per GPU (B = 8N sharded over the batch axis)
             ab = TensorHandle.empty_contiguous(c, [8, n4, n4], "bf16")
@@ -755,7 +759,7 @@ def main():
             parity["matmul_f32_4096"] = {"ok": bool(f32err["hybrid"] <= 1e-5 and f32err["3xtf32"] <= 1e-5 and f32err["tf32"] <= 1e-3),
                                          "worst_scaled_err": f32err}
             del af, bf, of
-            # widening row (SURVEY 8f-4): fp8 e4m3 8192^3 -> bf16 on the same kernel (kind::f8f6f4)
+            # widening row (SURVEY 8f-4): fp8 e4m3 8192^3 -> bf16 on the same kernel template (fp8 wgmma)
             a8 = TensorHandle.empty_contiguous(c, [N_MM, N_MM], "f8e4m3")
             b8 = TensorHandle.empty_contiguous(c, [N_MM, N_MM], "f8e4m3")
             c.fill_uniform(a8.handle, "f8e4m3", N_MM * N_MM, 8, -1.0, 1.0)
@@ -763,24 +767,23 @@ def main():
             ms_8, _ = timed(lambda: matmul.launch(c, a8, b8, o), extra_steps, 3)
             line["matmul_fp8_8192"] = {"value": world * FLOPS_MM * extra_steps / (ms_8 * 1e-3) / 1e12, "unit": "TFLOP/s",
                                        "config": "fp8 e4m3 x e4m3 -> bf16, f32 accumulate, 8192^3 per GPU"}
-            # same box, same operands: the 512x256 pair tile vs the 256x256 double-accumulator tile (bf16: auto picks the
-            # former; fp8: forced, to decide its default)
+            # same box, same operands: the 256x256 cluster tile forced (auto chooses by the wave model)
             c.set_option("gemm.variant", "2sm_n256")
             ms_bn, _ = timed(mm_step, extra_steps, 3)
             ms_8n, _ = timed(lambda: matmul.launch(c, a8, b8, o), extra_steps, 3)
             c.set_option("gemm.variant", "auto")
             line["tile_variants_8192"] = {"unit": "TFLOP/s", "bf16_2sm_n256": world * FLOPS_MM * extra_steps / (ms_bn * 1e-3) / 1e12,
                                           "fp8_2sm_n256": world * FLOPS_MM * extra_steps / (ms_8n * 1e-3) / 1e12,
-                                          "note": "gemm.variant forced to the 256x256 double-accumulator tile; the headline and matmul_fp8_8192 (auto) run the 512x256 pair tile 2sm_m512"}
-            # widening row (SURVEY 8f-4): block-scaled MX formats -- tcgen05 kind::mxf8f6f4 / kind::mxf4, ue8m0 scale per 32 K,
-            # row-major scales as the reference's scaled MMA takes them (the two packing passes run inside the timed call)
+                                          "note": "gemm.variant forced to the 256x256 cluster tile 2sm_n256; the headline and matmul_fp8_8192 run the wave model's choice"}
+            # widening row (SURVEY 8f-4): block-scaled MX formats, ue8m0 scale per 32 K, row-major scales as the reference's
+            # scaled MMA takes them; each operand is expanded to bf16 x * scale inside the timed call, then the bf16 wgmma GEMM runs
             import numpy as _np
             sc = TensorHandle.from_numpy(c, _np.full((N_MM, N_MM // 32), 127, _np.uint8), "ue8m0")
             ms_m8, _ = timed(lambda: matmul.launch_scaled(c, a8, b8, sc, sc, o), extra_steps, 3)
             a4 = TensorHandle(a8.handle, [N_MM, N_MM // 2], [N_MM // 2, 1], "f4e2m1x2")   # the same bytes read as packed e2m1
             b4 = TensorHandle(b8.handle, [N_MM, N_MM // 2], [N_MM // 2, 1], "f4e2m1x2")
             ms_m4, _ = timed(lambda: matmul.launch_scaled(c, a4, b4, sc, sc, o), extra_steps, 3)
-            # NVFP4: the same packed e2m1 operands with an e4m3 scale byte per 16 elements of K (kind::mxf4nvf4)
+            # NVFP4: the same packed e2m1 operands with an e4m3 scale byte per 16 elements of K
             sc16 = TensorHandle.from_numpy(c, _np.full((N_MM, N_MM // 16), 0x38, _np.uint8), "f8e4m3")
             ms_nv, _ = timed(lambda: matmul.launch_scaled(c, a4, b4, sc16, sc16, o, scale_block=16), extra_steps, 3)
             line["matmul_block_scaled_8192"] = {
@@ -789,7 +792,7 @@ def main():
                 "nvfp4_e2m1": world * FLOPS_MM * extra_steps / (ms_nv * 1e-3) / 1e12,
                 "kernel": c.last_kernel(),
                 "config": "8192^3 per GPU -> bf16, row-major scales for both operands (ue8m0 per 32 elements of K; nvfp4: e4m3 per 16), the two "
-                          "scale-packing passes run inside the timed call; scale atoms reach TMEM through the dedicated copy thread"}
+                          "dequantize-to-bf16 passes run inside the timed call"}
             del a8, b8, a4, b4, sc, sc16
             # what CubeCL's own kernels reach on this GPU (hand-written from its emit rules; SURVEY 8d)
             if world == 1:
@@ -809,10 +812,10 @@ def main():
                 buf = c.empty(512 << 20)
                 c.fill_modulo(buf, "f32", (512 << 20) // 4, 8)
                 ms_m, _ = timed(lambda: c.probe_memread(buf, 512 << 20, scratch), 10, 2)
-                line["tcgen05_probe_tflops"] = uops[0] * 5 / (ms_u * 1e-3) / 1e12
+                line["wgmma_probe_tflops"] = uops[0] * 5 / (ms_u * 1e-3) / 1e12
                 line["reference_equivalent"] = {"wmma_bf16_probe_tflops": ops[0] * 5 / (ms_p * 1e-3) / 1e12,
                                                 "vec4_read_probe_gbs": (512 << 20) * 10 / (ms_m * 1e-3) / 1e9,
-                                                "note": "compute_cmma.rs / memory_read.rs kernels as CubeCL would JIT them for sm_100a (wmma, 128-bit loads)"}
+                                                "note": "compute_cmma.rs / memory_read.rs kernels as CubeCL would JIT them for sm_90a (wmma, 128-bit loads)"}
                 del buf
 
     try:

@@ -1,7 +1,7 @@
-"""cubecl_b200: B200-native (sm_100a) implementation of CubeCL's dense linear-algebra hot path.
+"""cubecl_b200: H100-native (sm_90a) implementation of CubeCL's dense linear-algebra hot path.
 
   matmul.launch / reduce.launch over ComputeClient + TensorHandle  ->  C ABI (include/cubecl_b200.h)
-  ->  prebuilt sm_100a cubins: tcgen05/TMA GEMM (csrc/gemm_tcgen05.cu), HBM-bound reductions (csrc/reduce.cu).
+  ->  prebuilt sm_90a cubins: wgmma/TMA GEMM (csrc/gemm_wgmma.cu), HBM-bound reductions (csrc/reduce.cu).
 
 There is no CPU implementation in this package; the CPU oracle lives in /oracle and is test infrastructure only.
 """

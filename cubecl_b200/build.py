@@ -1,6 +1,6 @@
 """In-tree build of the native pieces (no JIT cache, no pip install):
 
-  csrc/*.cu  --nvcc -cubin, sm_100a-->  build/*.cubin  --.incbin-->  lib/libcubecl_b200.so  (host: g++, dlopen's libcuda)
+  csrc/*.cu  --nvcc -cubin, sm_90a-->  build/*.cubin  --.incbin-->  lib/libcubecl_b200.so  (host: g++, dlopen's libcuda)
 
 The cubins are PREBUILT images loaded with cuModuleLoadData at b200_init(); nothing is compiled at run time
 (the reference's NVRTC step, crates/cubecl-cuda/src/compute/context.rs:141-317, is what this replaces).
@@ -23,11 +23,10 @@ BUILD = PKG / "build"
 LIBDIR = PKG / "lib"
 LIB = LIBDIR / "libcubecl_b200.so"
 
-# tag -> (source, extra nvcc flags); the GEMM source is split in two cubins so the halves compile in parallel
-CUBINS = {"gemm": ("gemm_tcgen05.cu", ["-DGEMM_PART=0"]), "gemm_b": ("gemm_tcgen05.cu", ["-DGEMM_PART=2"]),
-          "gemm_c": ("gemm_tcgen05.cu", ["-DGEMM_PART=3"]), "gemm_mx": ("gemm_tcgen05.cu", ["-DGEMM_PART=1"]),
-          "reduce": ("reduce.cu", []), "aux": ("aux_kernels.cu", [])}
-NVCC_FLAGS = ["-cubin", "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17"]
+# tag -> (source, extra nvcc flags); the GEMM source is split in three cubins so the parts compile in parallel
+CUBINS = {"gemm": ("gemm_wgmma.cu", ["-DGEMM_PART=0"]), "gemm_b": ("gemm_wgmma.cu", ["-DGEMM_PART=1"]),
+          "gemm_c": ("gemm_wgmma.cu", ["-DGEMM_PART=2"]), "reduce": ("reduce.cu", []), "aux": ("aux_kernels.cu", [])}
+NVCC_FLAGS = ["-cubin", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17"]
 
 
 def _nvcc() -> str:

@@ -335,7 +335,7 @@ class ComputeClient:
         return ops.value
 
     def probe_umma_kind(self, dtype: str, block_scaled: bool, n_iter: int, scratch: Handle) -> float:
-        """tcgen05 peak probe for fp8 (plain / block-scaled) and block-scaled fp4 operands; returns the op count of the launch."""
+        """wgmma peak probe for bf16 or fp8 e4m3 operands (block-scaled kinds raise: sm_90 has no block-scaled MMA); returns the op count of the launch."""
         ops = C.c_double()
         _ffi.check(self._lib.b200_probe_umma_kind(self._ctx, None, DTYPES[dtype], int(bool(block_scaled)), int(n_iter),
                                                   C.c_uint64(scratch.ptr), C.byref(ops)))

@@ -1,4 +1,4 @@
-// Auxiliary sm_100a kernels (cubin):
+// Auxiliary sm_90a kernels (cubin):
 //  * counter-hash generators so host (numpy) and device produce bit-identical synthetic operands without PCIe traffic
 //  * a strided SIMT matmul for operands whose strides/alignment TMA cannot describe (still a CUDA path, never a CPU one);
 //    it accumulates in f32 over increasing k with separate mul/add roundings, i.e. exactly the reference's CPU order
@@ -148,7 +148,6 @@ struct PackScalesParams {
 extern "C" __global__ void __launch_bounds__(256) pack_scales(const __grid_constant__ PackScalesParams p) {
   // one 32-bit word = the 4 scales (one k atom) of one row.  Threads walk (chunk, row, atom) with the atom fastest, so the
   // row-major input is read coalesced (whole words when the rows allow it); the scattered side is the 4-byte stores
-  // (round 1 walked the OUTPUT order and gathered single bytes from rows 32 apart: 20 us per 2 MB operand at 8192 x 8192)
   const uint64_t words = static_cast<uint64_t>(p.batch) * p.tiles * p.atoms * 128;
   const uint8_t* in = reinterpret_cast<const uint8_t*>(p.in);
   uint32_t* out = reinterpret_cast<uint32_t*>(p.out);
@@ -158,8 +157,7 @@ extern "C" __global__ void __launch_bounds__(256) pack_scales(const __grid_const
     // Rows of whole 32-byte groups (K a multiple of 1024 / 512 elements): one warp per (chunk, 8 atoms), lane = row % 32.
     // Each lane reads the 32 bytes (8 atoms) of its four rows r, r + 32, r + 64, r + 96 -- whole sectors -- and the warp writes
     // each atom as one contiguous 512-byte chunk (lane r: the 16 bytes {row group 0..3} of that atom).  The word-per-thread
-    // form below scatters 4-byte stores 512 bytes apart (every 32-byte sector assembled from eight far-apart writes): 8 us per
-    // 2 MB mxfp operand, 65 us per 4 MB nvfp4 operand at 8192 x 8192 (profiles/r02b_block_scaled_sweep.log).
+    // form below scatters 4-byte stores 512 bytes apart (every 32-byte sector assembled from eight far-apart writes).
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t groups = p.atoms / 8;
     const uint64_t n_warps = static_cast<uint64_t>(p.batch) * p.tiles * groups;
@@ -235,7 +233,7 @@ __device__ __forceinline__ float mx_elem_to_f32(uint64_t base, uint64_t idx, uin
 
 // Reference-order block-scaled matmul (the expected-value loop of test_cmma_scaled, cmma.rs:1572-1590):
 //   out[m,n] = sum over l, increasing, in f32 with separately rounded operations, of ((a[m,l] * sa[m,l/32]) * b[n,l]) * sb[n,l/32]
-// One thread per output element; the path for shapes TMA cannot describe, and the on-device cross-check of the tcgen05 path.
+// One thread per output element; the path for shapes TMA cannot describe, and the on-device cross-check of the wgmma path.
 struct ScaledSimtParams {
   uint64_t a, b, sa, sb, out;
   uint32_t batch, M, N, K;       // K in elements
@@ -264,6 +262,47 @@ extern "C" __global__ void __launch_bounds__(256) gemm_scaled_simt(const __grid_
   }
 }
 
+// Block-scaled operand -> bf16 [rows, K]: x * scale per element, for the wgmma GEMM (Hopper's tensor cores take no scale
+// factors).  Exact: an e2m1 / e4m3 / e5m2 value times a ue8m0 power of two, or e2m1 times a ue4m3 scale (at most 6
+// significant bits), fits bf16's 8-bit significand; bf16 products are exact in the f32 accumulators.  Scales are the
+// reference's row-major [rows, K / scale_block] layout, or the packed 128-row atom layout of pack_scales when `packed`.
+struct DequantParams {
+  uint64_t in, scales, out;
+  uint32_t rows_per_batch, batch, K, dtype;     // K in elements; dtype 10 e4m3, 11 e5m2, 12 packed e2m1
+  uint32_t scale_block, scale_ue4m3, packed, atoms;
+};
+
+extern "C" __global__ void __launch_bounds__(256) dequant_scaled_bf16(const __grid_constant__ DequantParams p) {
+  const uint32_t n_scales = p.K / p.scale_block;
+  const uint64_t groups = static_cast<uint64_t>(p.batch) * p.rows_per_batch * (p.K / 8);   // 8 outputs (16 B) per thread
+  const uint8_t* sc = reinterpret_cast<const uint8_t*>(p.scales);
+  for (uint64_t g = blockIdx.x * static_cast<uint64_t>(blockDim.x) + threadIdx.x; g < groups; g += static_cast<uint64_t>(gridDim.x) * blockDim.x) {
+    const uint64_t row = g / (p.K / 8);
+    const uint32_t k0 = static_cast<uint32_t>(g % (p.K / 8)) * 8u;
+    const uint32_t si = k0 / p.scale_block;   // scale_block is 16 or 32: one scale per group of 8
+    uint64_t sidx;
+    if (p.packed) {
+      const uint64_t b = row / p.rows_per_batch;
+      const uint32_t r = static_cast<uint32_t>(row % p.rows_per_batch);
+      const uint64_t tiles = (p.rows_per_batch + 127) / 128;
+      const uint32_t lr = r % 128;
+      sidx = ((b * tiles + r / 128) * p.atoms + si / 4) * 512 + (lr % 32) * 16 + (lr / 32) * 4 + si % 4;
+    } else {
+      sidx = row * n_scales + si;
+    }
+    const float s = p.scale_ue4m3 ? fabsf(load_as_f32(p.scales, sidx, 10)) : ue8m0_to_f32(sc[sidx]);
+    uint32_t w[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float lo = mx_elem_to_f32(p.in, row * p.K + k0 + 2 * j, p.dtype) * s;
+      const float hi = mx_elem_to_f32(p.in, row * p.K + k0 + 2 * j + 1, p.dtype) * s;
+      __nv_bfloat162 h = __floats2bfloat162_rn(lo, hi);
+      w[j] = *reinterpret_cast<uint32_t*>(&h);
+    }
+    reinterpret_cast<uint4*>(p.out)[g] = make_uint4(w[0], w[1], w[2], w[3]);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ 3xTF32 split
 // lo = x - hi, hi = x with the low 13 mantissa bits cleared: the tf32 datapath ignores those bits of an f32 operand, so
 // the ORIGINAL tensor already acts as "hi" and only `lo` (exact in f32) is materialised, with the input's own strides
@@ -287,7 +326,7 @@ extern "C" __global__ void __launch_bounds__(256) split_tf32_lo(const __grid_con
   const bool vec = (p.cols % 4 == 0) && (p.in_rs % 4 == 0) && (p.in_bs % 4 == 0) && (p.in % 16 == 0) && (p.out % 16 == 0);
   if (vec && p.in_rs == p.cols && p.out_rs == p.cols && (p.batch == 1 || p.in_bs == p.rows * p.cols)) {
     // compact input and output (the common case): one flat stream of 128-bit vectors, no index arithmetic -- this pass runs in
-    // front of every 3xTF32 GEMM and at 4096^2 the scalar, divide-per-element form cost 68 us per operand against ~20 us of traffic
+    // front of every 3xTF32 GEMM, where a scalar, divide-per-element form costs several times its traffic time
     const uint64_t nv = p.batch * p.rows * p.cols / 4;
     const float4* in = reinterpret_cast<const float4*>(p.in);
     float4* out = reinterpret_cast<float4*>(p.out);
@@ -478,6 +517,38 @@ extern "C" __global__ void __launch_bounds__(256) gather_strided(const __grid_co
 // Copy a strided [batch, rows, cols] operand into a pitched buffer TMA can describe (pitch a multiple of 16 bytes): one
 // 16-byte output vector per thread, gathered element by element from the (possibly misaligned) input rows.  Only in front
 // of the tensor-core GEMM for operands whose own pitch / base is not 16-byte aligned (bf16 with K = 4097, odd sub-views).
+// fp8 (e4m3 / e5m2) operand -> f16, exactly (f16 holds every e4m3 and e5m2 value), with the operand's own strides compacted to
+// [batch, rows, out_pitch].  wgmma accumulates fp8 products with less than f32 precision, so fp8 matmuls run on the f16 kernels.
+struct ConvertF16Params {
+  uint64_t in, out;
+  uint64_t batch, rows, cols;        // logical [batch, rows, cols], cols innermost in the OUTPUT
+  uint64_t in_sb, in_sr, in_sc;      // input strides in elements
+  uint64_t out_pitch;                // output row pitch in elements (multiple of 8)
+  uint32_t dtype, pad;               // 10 = e4m3, 11 = e5m2
+};
+extern "C" __global__ void __launch_bounds__(256) convert_fp8_f16(const __grid_constant__ ConvertF16Params p) {
+  const uint64_t vpr = p.out_pitch / 8;                  // 16-byte output vectors per row
+  const uint64_t total = p.batch * p.rows * vpr;
+  const uint8_t* in = reinterpret_cast<const uint8_t*>(p.in);
+  for (uint64_t v = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; v < total;
+       v += static_cast<uint64_t>(gridDim.x) * blockDim.x) {
+    const uint64_t row = v / vpr, cv = v - row * vpr;
+    const uint64_t b = row / p.rows, r = row - b * p.rows;
+    const uint64_t c0 = cv * 8;
+    const uint64_t src = b * p.in_sb + r * p.in_sr;
+    uint32_t w[4] = {0u, 0u, 0u, 0u};                    // padding columns are written as zeros
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      if (c0 + j < p.cols) {
+        const __nv_fp8_storage_t x = in[src + (c0 + j) * p.in_sc];
+        const __half_raw h = __nv_cvt_fp8_to_halfraw(x, p.dtype == 11 ? __NV_E5M2 : __NV_E4M3);
+        w[j >> 1] |= static_cast<uint32_t>(h.x) << (16 * (j & 1));
+      }
+    }
+    reinterpret_cast<uint4*>(p.out)[row * vpr + cv] = make_uint4(w[0], w[1], w[2], w[3]);
+  }
+}
+
 struct RepitchParams {
   uint64_t in, out;
   uint64_t batch, rows, cols;

@@ -1,9 +1,9 @@
 // Host side of the C ABI declared in include/cubecl_b200.h.
 //
-// What this file is: the B200-native stand-in for the pieces of cubecl-cuda that sit between `ComputeClient::launch` and
+// What this file is: the H100-native stand-in for the pieces of cubecl-cuda that sit between `ComputeClient::launch` and
 // `cuLaunchKernel` on the dense-LA hot path -- minus NVRTC.  It loads libcuda (and, lazily, libnccl) with dlopen exactly
 // like cudarc's dynamic loading does (reference Cargo.toml:179-187), retains the device's primary context, loads the
-// PREBUILT sm_100a cubins embedded in this library with cuModuleLoadData (the call the reference makes with NVRTC's PTX at
+// PREBUILT sm_90a cubins embedded in this library with cuModuleLoadData (the call the reference makes with NVRTC's PTX at
 // crates/cubecl-cuda/src/compute/context.rs:293), keeps a small exclusive-page memory pool + pinned staging
 // (semantics of crates/cubecl-runtime/src/memory_management, crates/cubecl-cuda/src/compute/storage/gpu.rs:174-207),
 // encodes TMA descriptors (same cuTensorMapEncodeTiled call as crates/cubecl-cuda/src/compute/server.rs:1210-1224) and
@@ -34,8 +34,6 @@ extern const unsigned char b200_cubin_gemm_b[];
 extern const unsigned char b200_cubin_gemm_b_end[];
 extern const unsigned char b200_cubin_gemm_c[];
 extern const unsigned char b200_cubin_gemm_c_end[];
-extern const unsigned char b200_cubin_gemm_mx[];
-extern const unsigned char b200_cubin_gemm_mx_end[];
 extern const unsigned char b200_cubin_reduce[];
 extern const unsigned char b200_cubin_reduce_end[];
 extern const unsigned char b200_cubin_aux[];
@@ -208,7 +206,7 @@ static int ensure_nccl() {
   } while (0)
 
 // ================================================================================================ kernel parameter blocks
-// (layouts mirror the structs in gemm_tcgen05.cu / reduce.cu / aux_kernels.cu)
+// (layouts mirror the structs in gemm_wgmma.cu / reduce.cu / aux_kernels.cu)
 struct GemmParams {
   uint64_t out, out_row_stride, out_batch_stride;
   uint32_t M, N, K, batch;
@@ -218,12 +216,23 @@ struct GemmParams {
   uint64_t bias;
   float alpha;
   uint32_t epi_on;
-  uint32_t full_tiles, sk_tiles, sk_ranges, sk_umax;  // stream-K head, see gemm_tcgen05.cu
+  uint32_t full_tiles, sk_tiles, sk_ranges, sk_umax;  // stream-K head, see gemm_wgmma.cu
   uint64_t split_ws, split_tickets;
-  uint32_t sf_fmt_a, sf_fmt_b, sf_tiles_a, sf_tiles_b;  // block-scaled kinds; operand formats of a mixed 8-bit pair
-  uint32_t tma_store, fmt_mixed;
-  uint32_t hyb, hyb_nba, hyb_nbb;  // hybrid f32 schedule: tf32 main product + two bf16 cross terms (gemm_tcgen05.cu)
-  uint32_t sf_flags;               // block-scaled kinds: bit 0 = scale copies by the MMA thread (gemm.sf_copy=mma)
+  uint32_t fmt_b, fmt_mixed;       // rhs format of a mixed 8-bit pair
+  uint32_t hyb, hyb_nba, hyb_nbb;  // hybrid f32 schedule: tf32 main product + two bf16 cross terms (gemm_wgmma.cu)
+  uint32_t tma_store;              // whole tiles leave through shared-memory staging and TMA stores
+};
+struct ConvertF16Params {
+  uint64_t in, out;
+  uint64_t batch, rows, cols;
+  uint64_t in_sb, in_sr, in_sc;
+  uint64_t out_pitch;
+  uint32_t dtype, pad;
+};
+struct DequantParams {
+  uint64_t in, scales, out;
+  uint32_t rows_per_batch, batch, K, dtype;
+  uint32_t scale_block, scale_ue4m3, packed, atoms;
 };
 struct PackScalesParams {
   uint64_t in, out;
@@ -377,7 +386,7 @@ static int load_module(b200_ctx* c, const unsigned char* begin, const unsigned c
   CUmodule m;
   CUresult r = g_drv.cuModuleLoadData_p(&m, begin);
   if (r != CUDA_SUCCESS)
-    return fail(B200_ERR_COMPILATION, "cuModuleLoadData(%s) failed: %s -- the cubins are sm_100a only", what, cu_err(r));
+    return fail(B200_ERR_COMPILATION, "cuModuleLoadData(%s) failed: %s -- the cubins are sm_90a only", what, cu_err(r));
   c->modules.push_back(m);
   return B200_OK;
 }
@@ -387,17 +396,14 @@ static int get_func(b200_ctx* c, const std::string& name, CUfunction* out) {
   if (c->dry) { c->pending_kernel = name; *out = nullptr; return B200_OK; }
   auto it = c->funcs.find(name);
   if (it != c->funcs.end()) { *out = it->second; return B200_OK; }
-  // modules are loaded in the order gemm, reduce, aux, gemm_mx, gemm_b, gemm_c; the kernel name says where a kernel lives (no
+  // modules are loaded in the order gemm, reduce, aux, gemm_b, gemm_c; the kernel name says where a kernel lives (no
   // failing lookups, which API-level tools such as compute-sanitizer would report)
   auto starts = [&](const char* pfx) { return name.rfind(pfx, 0) == 0; };
   auto has = [&](const char* part) { return name.find(part) != std::string::npos; };
-  const bool mx = starts("gemm_mxf8_") || starts("gemm_mxf4_") || starts("gemm_nvf4_") || starts("umma_probe_e4m3") ||
-                  starts("umma_probe_mxf8") || starts("umma_probe_mxf4");
   const bool tc_gemm = starts("gemm_") && name != "gemm_simt_strided" && name != "gemm_scaled_simt";
-  const size_t home = mx ? 3
-                      : tc_gemm && has("_2sm_m512_") ? 5
-                      : tc_gemm && (has("_2sm_n128_") || has("_1sm_n128_")) ? 4
-                      : tc_gemm || starts("umma_") ? 0
+  const size_t home = tc_gemm && (has("_2sm_n128_") || has("_2sm_n224_")) ? 3
+                      : tc_gemm && (has("_1sm_n128_") || has("_2sm_m512_")) ? 4
+                      : tc_gemm || starts("wgmma_probe_") ? 0
                       : starts("reduce_") ? 1 : 2;
   if (home < c->modules.size()) {
     CUfunction f;
@@ -416,10 +422,9 @@ extern "C" int b200_get_cubin(const char* name, const void** image, size_t* size
   if (!strcmp(name, "gemm")) { b = b200_cubin_gemm; e = b200_cubin_gemm_end; }
   else if (!strcmp(name, "reduce")) { b = b200_cubin_reduce; e = b200_cubin_reduce_end; }
   else if (!strcmp(name, "aux")) { b = b200_cubin_aux; e = b200_cubin_aux_end; }
-  else if (!strcmp(name, "gemm_mx")) { b = b200_cubin_gemm_mx; e = b200_cubin_gemm_mx_end; }
   else if (!strcmp(name, "gemm_b")) { b = b200_cubin_gemm_b; e = b200_cubin_gemm_b_end; }
   else if (!strcmp(name, "gemm_c")) { b = b200_cubin_gemm_c; e = b200_cubin_gemm_c_end; }
-  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|gemm_mx|reduce|aux)", name);
+  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux)", name);
   *image = b;
   *size = static_cast<size_t>(e - b);
   return B200_OK;
@@ -462,15 +467,14 @@ extern "C" int b200_init(int device, b200_ctx** out) {
   g_drv.cuDeviceTotalMem_p(&total, c->dev);
   c->props.total_mem = total;
   g_drv.cuDeviceGetName_p(c->props.name, sizeof(c->props.name), c->dev);
-  if (c->props.cc_major != 10) {
+  if (c->props.cc_major != 9 || c->props.cc_minor != 0) {
     g_drv.cuDevicePrimaryCtxRelease_p(c->dev);
-    return bail(fail(B200_ERR_NO_DEVICE, "device %d is sm_%d%d; this library ships sm_100a cubins only (B200)", device,
+    return bail(fail(B200_ERR_NO_DEVICE, "device %d is sm_%d%d; this library ships sm_90a cubins only (H100)", device,
                      c->props.cc_major, c->props.cc_minor));
   }
   if ((rc = load_module(c, b200_cubin_gemm, b200_cubin_gemm_end, "gemm")) ||
       (rc = load_module(c, b200_cubin_reduce, b200_cubin_reduce_end, "reduce")) ||
       (rc = load_module(c, b200_cubin_aux, b200_cubin_aux_end, "aux")) ||
-      (rc = load_module(c, b200_cubin_gemm_mx, b200_cubin_gemm_mx_end, "gemm_mx")) ||
       (rc = load_module(c, b200_cubin_gemm_b, b200_cubin_gemm_b_end, "gemm_b")) ||
       (rc = load_module(c, b200_cubin_gemm_c, b200_cubin_gemm_c_end, "gemm_c"))) {
     for (CUmodule m : c->modules) g_drv.cuModuleUnload_p(m);
@@ -480,7 +484,7 @@ extern "C" int b200_init(int device, b200_ctx** out) {
   if ((r = g_drv.cuStreamCreate_p(&c->stream, CU_STREAM_NON_BLOCKING)) != CUDA_SUCCESS ||
       (r = g_drv.cuStreamCreate_p(&c->comm_stream, CU_STREAM_NON_BLOCKING)) != CUDA_SUCCESS ||
       (r = g_drv.cuEventCreate_p(&c->comm_event, CU_EVENT_DISABLE_TIMING)) != CUDA_SUCCESS) {
-    // release what exists: streams created so far, the four loaded modules, the retained primary context
+    // release what exists: streams created so far, the loaded modules, the retained primary context
     if (c->comm_stream) g_drv.cuStreamDestroy_p(c->comm_stream);
     if (c->stream) g_drv.cuStreamDestroy_p(c->stream);
     for (CUmodule m : c->modules) g_drv.cuModuleUnload_p(m);
@@ -523,7 +527,7 @@ extern "C" int b200_plan_begin(int num_sms, b200_ctx** out) {
   c->dry = true;
   c->device = 0;
   c->props.num_sms = num_sms;
-  c->props.cc_major = 10;
+  c->props.cc_major = 9;
   c->props.plane_size = 32;
   snprintf(c->props.name, sizeof(c->props.name), "dry-run (%d SMs)", num_sms);
   *out = c;
@@ -550,7 +554,7 @@ extern "C" int b200_get_props(b200_ctx* c, b200_props* out) {
 
 extern "C" int b200_set_option(b200_ctx* c, const char* key, const char* value) {
   if (!c || !key || !value) return fail(B200_ERR_INVALID_ARG, "null argument");
-  static const char* known[] = {"gemm.variant", "gemm.f32", "gemm.group_m", "gemm.split_k", "gemm.epilogue", "gemm.l2_promotion", "gemm.stage", "gemm.sf_copy", "reduce.variant", "reduce.threads",
+  static const char* known[] = {"gemm.variant", "gemm.f32", "gemm.group_m", "gemm.split_k", "gemm.epilogue", "gemm.l2_promotion", "gemm.stage", "reduce.variant", "reduce.threads",
                                 "reduce.blocks_per_sm", "reduce.rows_vpt", "reduce.rows_blocks_per_sm", "reduce.cols_blocks_per_sm",
                                 "reduce.debug", "reduce.pdl", "reduce.tma_stages", "reduce.tma_ctas_per_sm", "reduce.cols_split_target", "reduce.cols_loads", "reduce.cols_fused"};
   for (const char* k : known)
@@ -856,53 +860,18 @@ static size_t dtype_size(int dt) {
 struct GemmVariant {
   const char* tag;  // suffix in the kernel name
   int cg, block_n, stages;
-  double eff;       // measured MMA-pipe efficiency relative to 2sm_n256 (8192^3, B200): the N=128 shapes need
-                    // 128 B/cycle/SM of operand reads from shared memory and are smem-bandwidth bound.
+  double eff;       // MMA-pipe efficiency assumed relative to 2sm_n256 (not measured on H100): the 128-wide tiles issue
+                    // m64n128 wgmma, which moves twice the shared-memory operand bytes per FLOP of m64n256.
                     // 0 = never chosen automatically (gemm.variant=<tag> only)
-  int mt;           // 128-row sub-tiles of M per CTA: the pair tile is (128 * cg * mt) x block_n
+  int mt;           // 128-row sub-tiles of M per CTA: the tile is (128 * cg * mt) x block_n
 };
-static const GemmVariant kVariants[] = {{"2sm_n256", 2, 256, 6, 1.0, 1}, {"2sm_n128", 2, 128, 8, 0.66, 1}, {"1sm_n128", 1, 128, 6, 0.59, 1},
-                                        // 512 x 256 pair tile, one accumulator stage, 384 threads (gemm_tcgen05.cu, MT = 2).  Measured
-                                        // bf16 8192^3, same box, power state equalised (profiles/r01_pair_tile_ab.log): x1.059 of
-                                        // 2sm_n256 in a 50-launch burst and x1.058 held for 1 s (25 % less L2->SM operand traffic
-                                        // -> 1.53 instead of 1.45 GHz under the power cap), 0.98 of cuBLAS; fp8 e4m3 8192^3: x1.04
-                                        // (3223 vs 3098 TFLOP/s, profiles/r01_bench_n1.json tile_variants_8192)
-                                        {"2sm_m512", 2, 256, 4, 1.06, 2},
-                                        // block-scaled kinds only: 256 x 224 tile -- two accumulator stages and the scale columns fit
-                                        // the 512 TMEM columns, so the epilogue hides behind the next tile (the 256-wide scaled tiles
-                                        // hold ONE stage).  Needs the B scales packed per 224-row tile, i.e. row-major scales.
-                                        // MEASURED SLOWER (profiles/r02_block_scaled_sweep.log, 8192^3 -> bf16): mxfp8 2046 vs 2448 TFLOP/s,
-                                        // mxfp4 3798 vs 3866 -- UMMA N = 224 issues at the N = 256 rate, which costs more than the hidden
-                                        // epilogue returns.  eff 0: never chosen automatically (gemm.variant=2sm_n224 only).
-                                        {"2sm_n224", 2, 224, 6, 0.0, 1},
-                                        // diagnostic: 256 x 256 tile with ONE accumulator stage (bf16 -> bf16, K-major lhs only)
-                                        {"2sm_n256a1", 2, 256, 6, 0.0, 1}};
-static bool variant_has_dtype(const GemmVariant& v, int in_dtype) {
-  if (!strcmp(v.tag, "2sm_n224")) return false;   // block-scaled kinds only
-  const bool bits8 = (in_dtype == B200_F8E4M3 || in_dtype == B200_F8E5M2 || in_dtype == B200_U8 || in_dtype == B200_I8);
-  if (!strcmp(v.tag, "2sm_m512")) return in_dtype == B200_BF16 || in_dtype == B200_F16 || in_dtype == B200_F8E4M3 || in_dtype == B200_F8E5M2;
-  if (!strcmp(v.tag, "2sm_n256a1")) return in_dtype == B200_BF16 || in_dtype == B200_F8E4M3;
-  if (bits8) return !strcmp(v.tag, "2sm_n256") || !strcmp(v.tag, "1sm_n128");
-  return true;
-}
-
-// mx_kind: 0 = unscaled, 1 = mxf8 (one 512-byte scale chunk per 128 rows per k-block), 2 = mxf4 (two), 3 = nvfp4 (four)
-static unsigned mx_atoms(int mx_kind) { return mx_kind == 3 ? 4u : (unsigned)mx_kind; }
-// scale atoms of one stage (512 bytes each: A rows of the CTA, B rows of the whole tile), padded to the 1 KB stage alignment
-static unsigned gemm_sf_stage_bytes(const GemmVariant& v, int mx_kind) {
-  if (!mx_kind) return 0;
-  return (512u * mx_atoms(mx_kind) * (1 + (v.block_n + 127) / 128) + 1023u) / 1024u * 1024u;
-}
-// block-scaled kinds: as many stages as fit 227 KB, eight at most (mirror of mx_stages() in gemm_tcgen05.cu)
-static int gemm_stages(const GemmVariant& v, int mx_kind) {
-  if (!mx_kind) return v.stages;
-  const int stage = 16384 + (v.block_n / v.cg) * 128 + (int)gemm_sf_stage_bytes(v, mx_kind);
-  return std::min(8, (232448 - 1024 - 1024 - 16384) / stage);
-}
-// alignment slack + operand ring (+ scale chunks) + barrier block + epilogue staging (4 * mt warps x [32 rows x 128 B])
-static unsigned gemm_smem_bytes(const GemmVariant& v, int mx_kind = 0) {
-  return 1024 + gemm_stages(v, mx_kind) * (16384 * v.mt + (v.block_n / v.cg) * 128 + gemm_sf_stage_bytes(v, mx_kind)) + 1024 + 16384 * v.mt;
-}
+static const GemmVariant kVariants[] = {{"2sm_n256", 2, 256, 4, 1.0, 1}, {"2sm_n128", 2, 128, 6, 0.9, 1}, {"1sm_n128", 1, 128, 6, 0.85, 1},
+                                        // 512 x 128 pair tile (256 rows per CTA), 16-bit kinds; opt-in until measured
+                                        {"2sm_m512", 2, 128, 4, 0.0, 2},
+                                        // block-scaled kinds only: 256 x 224 pair tile; opt-in until measured
+                                        {"2sm_n224", 2, 224, 4, 0.0, 1}};
+// alignment slack + operand ring (A: 128 * mt rows, B: block_n rows, 128 B of K each) + barrier block + TMA-store staging
+static unsigned gemm_smem_bytes(const GemmVariant& v) { return 1024 + v.stages * (16384 * v.mt + v.block_n * 128) + 1024 + 16384; }
 
 static int encode_tmap(b200_ctx* c, CUtensorMap* out, CUtensorMapDataType dt, size_t esz, uint64_t base, uint64_t d0,
                        uint64_t d1, uint64_t d2, uint64_t s1_elems, uint64_t s2_elems, uint32_t b0, uint32_t b1,
@@ -947,41 +916,13 @@ static int encode_tmap(b200_ctx* c, CUtensorMap* out, CUtensorMapDataType dt, si
   return B200_OK;
 }
 
-// Scale-factor tensor map: the packed tensor [tiles][k atoms][512 B] viewed as (one 512-byte atom = 128 words, k atoms, tiles);
-// a box of (128, atoms, tiles) lands in shared memory as [tile][atom][512 B].  Whole atoms are the box rows: round 2 used
-// (16 B, 32 rows x atoms, tiles) boxes, whose 16-byte rows cost the TMA unit far more per byte.
-static int encode_sf_tmap(b200_ctx* c, CUtensorMap* out, uint64_t base, uint64_t k_atoms, uint64_t tiles, uint32_t box_atoms, uint32_t box_tiles) {
-  char key[256];
-  snprintf(key, sizeof(key), "sf|%llx|%llu|%llu|%u|%u", (unsigned long long)base, (unsigned long long)k_atoms, (unsigned long long)tiles, box_atoms, box_tiles);
-  if (c->dry) {
-    char line[256];
-    snprintf(line, sizeof(line), "tmap scales esz=4 dims=(128,%llu,%llu) strides=(512,%llu) box=(128,%u,%u)\n", (unsigned long long)k_atoms,
-             (unsigned long long)tiles, (unsigned long long)(512 * k_atoms), box_atoms, box_tiles);
-    c->plan += line;
-    memset(out, 0, sizeof(*out));
-    return B200_OK;
-  }
-  auto it = c->tmap_cache.find(key);
-  if (it != c->tmap_cache.end()) { *out = it->second; return B200_OK; }
-  cuuint64_t dims[3] = {128, k_atoms, tiles};
-  cuuint64_t strides[2] = {512, 512 * k_atoms};
-  cuuint32_t box[3] = {128, box_atoms, box_tiles};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = g_drv.cuTensorMapEncodeTiled_p(out, CU_TENSOR_MAP_DATA_TYPE_UINT32, 3, reinterpret_cast<void*>(base), dims, strides, box, estr,
-                                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(B200_ERR_INVALID_ARG, "cuTensorMapEncodeTiled (scales) failed: %s", cu_err(r));
-  if (c->tmap_cache.size() > 512) c->tmap_cache.clear();
-  c->tmap_cache[key] = *out;
-  return B200_OK;
-}
-
 // One batched problem with LINEAR batch strides (0 = broadcast).  Strides in elements.
 struct GemmProblem {
   int in_dtype, out_dtype;
   int rhs_dtype = -1;           // >= 0: a mixed 8-bit pair (fp8 e4m3 x e5m2, u8 x i8); in_dtype is then the lhs format
   uint64_t a, b, out;
   uint64_t a_lo = 0, b_lo = 0;  // 3xTF32: compact low parts (same logical layout class as a / b), 0 otherwise
+  bool mx = false;              // block-scaled operands expanded to bf16: the gemm_mx_* kernels (promoted accumulation)
   bool hybrid = false;          // a_lo / b_lo are bf16 PAIR buffers [2][entries][rows][pitch]: bf16(x) planes, then bf16(x - trunc_tf32(x))
   uint64_t bias = 0;            // fused epilogue: out = act(alpha * acc + bias[n])
   float alpha = 1.0f;
@@ -990,14 +931,13 @@ struct GemmProblem {
   uint64_t a_sm, a_sk, a_sb;
   uint64_t b_sk, b_sn, b_sb;
   uint64_t o_sm, o_sn, o_sb;
-  // block-scaled (MX) problems: in_dtype is a 1-byte marker, K / a_sm / b_sn count BYTES of K-major packed operands
-  int mx_kind = 0;                 // 0 unscaled, 1 mxf8 (e4m3 / e5m2), 2 mxf4 (packed e2m1, ue8m0 / 32), 3 nvfp4 (packed e2m1, ue4m3 / 16)
-  uint32_t fmt_a = 0, fmt_b = 0;   // instruction-descriptor operand formats
-  uint64_t sfa = 0, sfb = 0;       // packed scale tensors [batch * tiles][atoms][512 B]
-  uint64_t sf_atoms = 0;           // 4-scale atoms along K
-  int sfb_tile_rows = 128;         // how the rhs scales are packed: per 128-row chunk, or per 224-row GEMM tile (2sm_n224 only)
-  bool sfb_any_layout = false;     // planning pass: the caller packs the scales AFTER the variant is known
 };
+
+static bool variant_has(const GemmVariant& v, const GemmProblem& g) {
+  if (!strcmp(v.tag, "2sm_n224")) return g.mx;
+  if (!strcmp(v.tag, "2sm_m512")) return !g.mx && (g.in_dtype == B200_BF16 || g.in_dtype == B200_F16);
+  return true;
+}
 
 static int launch_simt(b200_ctx* c, CUstream st, const GemmProblem& g) {
   CUfunction f;
@@ -1039,17 +979,16 @@ static bool tma_ok(const GemmProblem& g, bool* a_mn, bool* b_mn) {
 
 static int reduce_workspace(b200_ctx* c, CUstream st, CUdeviceptr* out);
 
-// Stream-K head plan for `tiles` tiles on `clusters` CTA pairs (gemm_tcgen05.cu, GemmParams): the rem = tiles % clusters
+// Stream-K head plan for `tiles` tiles on `clusters` clusters (gemm_wgmma.cu, GemmParams): the rem = tiles % clusters
 // tiles that would form a partial last wave are instead cut along K into `ranges` equal ranges processed FIRST, so all
-// pairs stay busy and the slab exchange runs under the whole tiles that follow.
+// clusters stay busy and the slab exchange runs under the whole tiles that follow.
 //   time (in tile-times) without: full_waves + 1.
 //   with: full_waves + 1.4 * head + overhead / num_kb, head = ceil(ranges / clusters) * share / num_kb.
-// Measured (profiles/r02_split_sweep.log): while the head runs, S pairs stream the operands of ONE tile, so the phase needs
-// S times the operand bandwidth of a normal wave with less panel sharing in L2 -- it runs ~1.4x longer than its MMA time
-// (bf16 4096^3: 92.0 us with S = 2 against 94.6 us for two waves of pair tiles; tf32 4096^3: 179 against 186 us).  Equal
-// parts (ranges = rem * S) beat the even cut over all pairs whenever they fit (fp8 4096^3: 54.6 against 72.3 us), so S =
-// floor(clusters / rem) when that is >= 2.  The exchange itself is hidden when whole tiles follow (~4 k-block times) and
-// exposed, (14 + 8 parts) k-block times, when the head is the whole problem (round 1 measurement).
+// While the head runs, S clusters stream the operands of ONE tile, so the phase needs S times the operand bandwidth of a
+// normal wave with less panel sharing in L2; the model charges it 1.4x its MMA time.  Equal parts (ranges = rem * S) are
+// preferred to an even cut over all clusters whenever they fit, so S = floor(clusters / rem) when that is >= 2.  The
+// exchange is modelled as hidden when whole tiles follow (~4 k-block times) and exposed, (14 + 8 parts) k-block times, when
+// the head is the whole problem.  These constants are not measured on H100.
 // gemm.split_k: auto (only when the model gains >= 4 %), off, on (whenever rem != 0), or N = 1..8 (N ranges per tile).
 struct SkPlan {
   double time = 0;           // modelled time in tile-times
@@ -1129,22 +1068,14 @@ static const GemmVariant* pick_variant(b200_ctx* c, const GemmProblem& g, SkPlan
   for (const GemmVariant& v : kVariants) {
     if (forced != "auto" && forced != v.tag) continue;
     if (forced == "auto" && v.eff <= 0.0) continue;
-    if (!g.mx_kind && !variant_has_dtype(v, g.in_dtype)) continue;
+    if (!variant_has(v, g)) continue;
     if (forced == "auto" && v.cg == 2 && g.M <= 128) continue;  // a CTA pair would idle its second half: one CTA per tile
-    if (g.mx_kind && v.mt != 1) continue;                       // block-scaled kinds have no two-unit instantiation
-    if (g.mx_kind == 3 && v.block_n == 224) continue;           // NVFP4: 448 accumulator columns leave room for one scale buffer only
-    if (v.block_n == 224 && !(g.mx_kind && (g.sfb_any_layout || g.sfb_tile_rows == 224))) continue;
-    if (v.block_n != 224 && g.mx_kind && !g.sfb_any_layout && g.sfb_tile_rows == 224) continue;   // scales already packed for 224-row tiles
-    // the two-unit tile hides its epilogue only on the packed-register path (16-bit outputs); f32 outputs stay on 2sm_n256
-    if (forced == "auto" && v.mt == 2 && !(g.out_dtype == B200_BF16 || g.out_dtype == B200_F16)) continue;
     const uint64_t tile_m = 128ull * v.cg * v.mt;
     const uint64_t tm = (g.M + tile_m - 1) / tile_m, tn = (g.N + v.block_n - 1) / v.block_n;
     const uint64_t tiles = tm * tn * g.batch;
     const uint64_t clusters = std::max(1, c->props.num_sms / v.cg);
-    // the slab exchange is a per-128-row-CTA-tile protocol with f32 accumulators: not for the pair tile, not for integers
+    // the slab exchange is a per-128-row-CTA-tile protocol with f32 accumulators: not for the 512-row tile, not for integers
     const SkPlan sk = sk_plan(tiles, clusters, num_kb, split_opt, float_acc && v.mt == 1);
-    // block-scaled kinds: measured 8192^3 ratios to the 256-wide tile are 0.63 (2sm_n128) and 0.61 (1sm_n128) for mxfp8,
-    // 0.63 / 0.66 for mxfp4 -- the same ordering as the unscaled table, so it is reused
     const double eff = v.eff > 0 ? v.eff : 1.0;
     const double cost = sk.time * (128.0 * v.mt * v.block_n) / eff;  // per-SM MMA time
     if (!best || cost < best_cost * 0.999) { best = &v; best_cost = cost; *sk_out = sk; }
@@ -1152,10 +1083,9 @@ static const GemmVariant* pick_variant(b200_ctx* c, const GemmProblem& g, SkPlan
   return best;
 }
 
-static int launch_tcgen05(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_mn, bool b_mn) {
+static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_mn, bool b_mn) {
   const size_t esz = dtype_size(g.in_dtype), osz = dtype_size(g.out_dtype);
-  const char* in_tag = g.mx_kind == 1 ? "mxf8" : g.mx_kind == 2 ? "mxf4" : g.mx_kind == 3 ? "nvf4"
-                       : g.in_dtype == B200_BF16 ? "bf16" : g.in_dtype == B200_F16 ? "f16" : g.in_dtype == B200_F8E4M3 ? "e4m3"
+  const char* in_tag = g.mx ? "mx" : g.in_dtype == B200_BF16 ? "bf16" : g.in_dtype == B200_F16 ? "f16" : g.in_dtype == B200_F8E4M3 ? "e4m3"
                        : g.in_dtype == B200_F8E5M2 ? "e5m2" : g.in_dtype == B200_U8 ? "u8" : g.in_dtype == B200_I8 ? "s8" : "tf32";
   const char* out_tag = g.out_dtype == B200_BF16 ? "bf16" : g.out_dtype == B200_F16 ? "f16" : g.out_dtype == B200_I32 ? "i32" : "f32";
   const uint32_t block_k = static_cast<uint32_t>(128 / esz);
@@ -1163,7 +1093,7 @@ static int launch_tcgen05(b200_ctx* c, CUstream st, const GemmProblem& g, bool a
   const uint64_t k_segments = (g.a_lo != 0 && g.b_lo != 0) ? 3 : 1;
   SkPlan best_sk;
   const GemmVariant* best = pick_variant(c, g, &best_sk);
-  if (!best) return fail(B200_ERR_INVALID_ARG, "gemm.variant '%s' is not a tcgen05 variant for this dtype", forced.c_str());
+  if (!best) return fail(B200_ERR_INVALID_ARG, "gemm.variant '%s' is not a wgmma variant", forced.c_str());
   if (best_sk.bad_option) return fail(B200_ERR_INVALID_ARG, "gemm.split_k must be auto, off, on or 1..8");
   const GemmVariant& v = *best;
 
@@ -1171,7 +1101,7 @@ static int launch_tcgen05(b200_ctx* c, CUstream st, const GemmProblem& g, bool a
   CUfunction f;
   int rc = get_func(c, name, &f);
   if (rc) return rc;
-  const unsigned smem = gemm_smem_bytes(v, g.mx_kind);
+  const unsigned smem = gemm_smem_bytes(v);
   if (!c->dry) CU_CHECK(g_drv.cuFuncSetAttribute_p(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem));
 
   const CUtensorMapDataType dt = g.in_dtype == B200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
@@ -1181,27 +1111,25 @@ static int launch_tcgen05(b200_ctx* c, CUstream st, const GemmProblem& g, bool a
   const bool a_bcast = (g.a_sb == 0 || g.batch == 1), b_bcast = (g.b_sb == 0 || g.batch == 1);
   CUtensorMap ta, tb;
   auto pad16 = [&](uint64_t elems) { const uint64_t q = 16 / esz; return (elems + q - 1) / q * q; };
-  const uint32_t chunk = static_cast<uint32_t>(128 / esz);  // MN-major operands: elements per 128-byte row
-  const CUtensorMapSwizzle mn_swz = esz == 4 ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B;
+  const uint32_t chunk = static_cast<uint32_t>(128 / esz);  // MN-major operands (16-bit): elements per 128-byte row
   if (!a_mn) {
     const uint64_t a_sm = g.M > 1 ? g.a_sm : pad16(g.K);
     rc = encode_tmap(c, &ta, dt, esz, g.a, g.K, g.M, a_bcast ? 1 : g.batch, a_sm, a_bcast ? a_sm * g.M : g.a_sb, block_k, 128);
   } else {
     const uint64_t a_sk = g.K > 1 ? g.a_sk : pad16(g.M);
-    rc = encode_tmap(c, &ta, dt, esz, g.a, g.M, g.K, a_bcast ? 1 : g.batch, a_sk, a_bcast ? a_sk * g.K : g.a_sb, chunk, block_k, mn_swz);
+    rc = encode_tmap(c, &ta, dt, esz, g.a, g.M, g.K, a_bcast ? 1 : g.batch, a_sk, a_bcast ? a_sk * g.K : g.a_sb, chunk, block_k);
   }
   if (rc) return rc;
-  const uint32_t n_local = v.block_n / v.cg;
+  const uint32_t n_local = v.block_n / v.cg;   // B rows each CTA of a pair loads (multicast to both)
   if (!b_mn) {
     const uint64_t b_sn = g.N > 1 ? g.b_sn : pad16(g.K);
     rc = encode_tmap(c, &tb, dt, esz, g.b, g.K, g.N, b_bcast ? 1 : g.batch, b_sn, b_bcast ? b_sn * g.N : g.b_sb, block_k, n_local);
   } else {
     const uint64_t b_sk = g.K > 1 ? g.b_sk : pad16(g.N);
-    // MN-major 32-bit operands: 32-byte swizzle atoms (matches the SWIZZLE_128B_BASE32B smem descriptor)
-    rc = encode_tmap(c, &tb, dt, esz, g.b, g.N, g.K, b_bcast ? 1 : g.batch, b_sk, b_bcast ? b_sk * g.K : g.b_sb, chunk, block_k, mn_swz);
+    rc = encode_tmap(c, &tb, dt, esz, g.b, g.N, g.K, b_bcast ? 1 : g.batch, b_sk, b_bcast ? b_sk * g.K : g.b_sb, chunk, block_k);
   }
   if (rc) return rc;
-  // 3xTF32: compact low parts, same operand-major class as the originals (K-major: [rows, K]; MN-major: [K, cols])
+  // 3xTF32: compact low parts (K-major: [rows, K]); hybrid: bf16 pair buffers
   CUtensorMap ta_lo = ta, tb_lo = tb;
   const bool split = (g.a_lo != 0 && g.b_lo != 0);
   if (split && g.hybrid) {
@@ -1209,45 +1137,23 @@ static int launch_tcgen05(b200_ctx* c, CUstream st, const GemmProblem& g, bool a
     const uint64_t ab = a_bcast ? 1 : g.batch, bb = b_bcast ? 1 : g.batch;
     auto pad8 = [](uint64_t e) { return (e + 7) / 8 * 8; };
     const CUtensorMapDataType d16 = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-    rc = !a_mn ? encode_tmap(c, &ta_lo, d16, 2, g.a_lo, g.K, g.M, 2 * ab, pad8(g.K), pad8(g.K) * g.M, 64, 128)
-               : encode_tmap(c, &ta_lo, d16, 2, g.a_lo, g.M, g.K, 2 * ab, pad8(g.M), pad8(g.M) * g.K, 64, 64);
+    rc = encode_tmap(c, &ta_lo, d16, 2, g.a_lo, g.K, g.M, 2 * ab, pad8(g.K), pad8(g.K) * g.M, 64, 128);
     if (rc) return rc;
-    rc = !b_mn ? encode_tmap(c, &tb_lo, d16, 2, g.b_lo, g.K, g.N, 2 * bb, pad8(g.K), pad8(g.K) * g.N, 64, n_local)
-               : encode_tmap(c, &tb_lo, d16, 2, g.b_lo, g.N, g.K, 2 * bb, pad8(g.N), pad8(g.N) * g.K, 64, 64);
+    rc = encode_tmap(c, &tb_lo, d16, 2, g.b_lo, g.K, g.N, 2 * bb, pad8(g.K), pad8(g.K) * g.N, 64, n_local);
     if (rc) return rc;
   } else if (split) {
     const uint64_t ab = a_bcast ? 1 : g.batch, bb = b_bcast ? 1 : g.batch;
-    rc = !a_mn ? encode_tmap(c, &ta_lo, dt, esz, g.a_lo, g.K, g.M, ab, pad16(g.K), pad16(g.K) * g.M, block_k, 128)
-               : encode_tmap(c, &ta_lo, dt, esz, g.a_lo, g.M, g.K, ab, pad16(g.M), pad16(g.M) * g.K, chunk, block_k, mn_swz);
+    rc = encode_tmap(c, &ta_lo, dt, esz, g.a_lo, g.K, g.M, ab, pad16(g.K), pad16(g.K) * g.M, block_k, 128);
     if (rc) return rc;
-    rc = !b_mn ? encode_tmap(c, &tb_lo, dt, esz, g.b_lo, g.K, g.N, bb, pad16(g.K), pad16(g.K) * g.N, block_k, n_local)
-               : encode_tmap(c, &tb_lo, dt, esz, g.b_lo, g.N, g.K, bb, pad16(g.N), pad16(g.N) * g.K, chunk, block_k, mn_swz);
+    rc = encode_tmap(c, &tb_lo, dt, esz, g.b_lo, g.K, g.N, bb, pad16(g.K), pad16(g.K) * g.N, block_k, n_local);
     if (rc) return rc;
   }
 
   GemmParams p;
   memset(&p, 0, sizeof(p));
-  if (g.mx_kind) {
-    // packed scale tensors viewed as (16 B, 32 rows x atoms, 128-row tiles); one box = the chunks of one k-block
-    // 128-row chunks per batch entry; the rhs scales packed per 224-row tile take two chunks per tile (see pack_scales)
-    const uint64_t tiles_a = (g.M + 127) / 128;
-    const uint64_t tiles_b = g.sfb_tile_rows == 224 ? 2 * ((g.N + 223) / 224) : (g.N + 127) / 128;
-    const uint64_t ab = a_bcast ? 1 : g.batch, bb = b_bcast ? 1 : g.batch;
-    rc = encode_sf_tmap(c, &ta_lo, g.sfa, g.sf_atoms, tiles_a * ab, mx_atoms(g.mx_kind), 1);
-    if (rc) return rc;
-    rc = encode_sf_tmap(c, &tb_lo, g.sfb, g.sf_atoms, tiles_b * bb, mx_atoms(g.mx_kind), (v.block_n + 127) / 128);
-    if (rc) return rc;
-    {  // who issues the scale copies: one copy thread (default), two copy threads in different warps, or the MMA thread (A/B reference)
-      const std::string sfc = opt(c, "gemm.sf_copy", "thread");
-      if (sfc != "thread" && sfc != "thread2" && sfc != "mma") return fail(B200_ERR_INVALID_ARG, "gemm.sf_copy must be thread, thread2 or mma");
-      p.sf_flags = sfc == "mma" ? 1u : sfc == "thread2" ? 2u : 0u;
-    }
-    p.sf_fmt_a = g.fmt_a; p.sf_fmt_b = g.fmt_b;
-    p.sf_tiles_a = (uint32_t)tiles_a; p.sf_tiles_b = (uint32_t)tiles_b;
-  }
-  if (!g.mx_kind && g.rhs_dtype >= 0 && g.rhs_dtype != g.in_dtype) {
-    auto fmt8 = [](int dt) { return (dt == B200_F8E5M2 || dt == B200_I8) ? 1u : 0u; };   // kind::f8f6f4: e4m3 0 / e5m2 1; kind::i8: u8 0 / s8 1
-    p.sf_fmt_a = fmt8(g.in_dtype); p.sf_fmt_b = fmt8(g.rhs_dtype); p.fmt_mixed = 1;
+  if (g.rhs_dtype >= 0 && g.rhs_dtype != g.in_dtype) {
+    p.fmt_b = (g.rhs_dtype == B200_F8E5M2 || g.rhs_dtype == B200_I8) ? 1u : 0u;   // 0 = e4m3 / u8, 1 = e5m2 / s8
+    p.fmt_mixed = 1;
   }
   p.k_segments = (uint32_t)k_segments;
   if (split && g.hybrid) {
@@ -1267,15 +1173,17 @@ static int launch_tcgen05(b200_ctx* c, CUstream st, const GemmProblem& g, bool a
   p.a_bmul = a_bcast ? 0 : 1;
   p.b_bmul = b_bcast ? 0 : 1;
   p.vec_store = (g.out % 16 == 0 && (g.o_sm * osz) % 16 == 0 && (g.o_sb * osz) % 16 == 0) ? 1 : 0;
-  // whole tiles leave through swizzled staging tiles and TMA stores when `out` is describable: (N, M, batch), 128-byte boxes
+  // whole tiles leave through swizzled staging tiles and TMA stores when `out` is describable: (N, M, batch), [128 B x 64 rows] boxes
+  const std::string epi = opt(c, "gemm.epilogue", "tma");
+  if (epi != "tma" && epi != "direct") return fail(B200_ERR_INVALID_ARG, "gemm.epilogue must be tma or direct");
   CUtensorMap tout;
   memset(&tout, 0, sizeof(tout));
   const uint64_t lim40 = 1ull << 40;
-  if (p.vec_store && opt(c, "gemm.epilogue", "tma") == "tma" && g.o_sm * osz < lim40 && g.o_sb * osz < lim40 && (g.M == 1 || g.o_sm >= g.N)) {
+  if (p.vec_store && epi == "tma" && g.o_sm * osz < lim40 && g.o_sb * osz < lim40 && (g.M == 1 || g.o_sm >= g.N)) {
     const uint64_t o_sm = g.M > 1 ? g.o_sm : (g.N + 15) / 16 * 16;
     const uint64_t o_sb = g.batch > 1 ? g.o_sb : o_sm * g.M;
     rc = encode_tmap(c, &tout, osz == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_UINT16, osz, g.out, g.N, g.M, g.batch,
-                     o_sm, o_sb, static_cast<uint32_t>(128 / osz), 32);
+                     o_sm, o_sb, static_cast<uint32_t>(128 / osz), 64);
     if (rc) return rc;
     p.tma_store = 1;
   }
@@ -1302,7 +1210,7 @@ static int launch_tcgen05(b200_ctx* c, CUstream st, const GemmProblem& g, bool a
     p.sk_umax = (uint32_t)best_sk.umax;
     p.split_ws = slabs;
     p.split_tickets = ws + kWsGemmTicketOffset;
-    // the head's ranges are dealt to pairs 0 .. ranges-1 (mod the grid); whole tiles to every pair
+    // the head's ranges are dealt to clusters 0 .. ranges-1 (mod the grid); whole tiles to every cluster
     clusters = (unsigned)std::min<uint64_t>(std::max<uint64_t>(p.full_tiles, best_sk.ranges), max_clusters);
     if (c->dry) {
       char line[200];
@@ -1312,8 +1220,7 @@ static int launch_tcgen05(b200_ctx* c, CUstream st, const GemmProblem& g, bool a
     }
   }
   void* args[] = {&ta, &tb, &ta_lo, &tb_lo, &tout, &p};
-  // block-scaled kernels carry one more warp (the optional second scale-copy thread)
-  rc = launch(c, f, clusters * v.cg, 1, 1, 256 + 128 * (v.mt - 1) + (g.mx_kind ? 32 : 0), smem, v.cg, st, args);
+  rc = launch(c, f, clusters * v.cg, 1, 1, 384, smem, v.cg, st, args);
   if (slabs) pool_free(c, slabs, st);  // stream-ordered: reusable by later work once this launch has drained
   return rc;
 }
@@ -1359,7 +1266,8 @@ struct RepitchParams {
 // buffer it can: [batch, rows, pitch] with the operand's own contiguous dimension innermost when it has one.
 static int stage_operand(b200_ctx* c, CUstream st, size_t esz, uint64_t ptr, uint64_t batch, uint64_t mn, uint64_t K, uint64_t s_mn, uint64_t s_k,
                          uint64_t s_b, CUdeviceptr* out, uint64_t* o_smn, uint64_t* o_sk, uint64_t* o_sb) {
-  const bool keep_mn_major = (s_mn == 1 && s_k != 1);          // rows of the M / N extent: keep them (coalesced both ways)
+  // rows of the M / N extent are kept (coalesced both ways) where wgmma reads them: 16-bit operands
+  const bool keep_mn_major = (s_mn == 1 && s_k != 1) && esz == 2;
   const uint64_t rows = keep_mn_major ? K : mn, cols = keep_mn_major ? mn : K;
   const uint64_t q = 16 / esz, pitch = (cols + q - 1) / q * q;
   const uint64_t nb = (s_b == 0) ? 1 : batch;                  // a broadcast operand is staged once
@@ -1383,19 +1291,72 @@ static int stage_operand(b200_ctx* c, CUstream st, size_t esz, uint64_t ptr, uin
 }
 
 static int run_gemm_staged(b200_ctx* c, CUstream st, const GemmProblem& g);
+static int run_gemm(b200_ctx* c, CUstream st, const GemmProblem& g);
+
+// An fp8 operand widened to f16 (exact) in a pooled [batch, rows, pitch] buffer that keeps the operand's own contiguous
+// dimension innermost when it has one (wgmma reads 16-bit operands in either major).
+static int widen_fp8_operand(b200_ctx* c, CUstream st, int dtype, uint64_t ptr, uint64_t batch, uint64_t mn, uint64_t K, uint64_t s_mn,
+                             uint64_t s_k, uint64_t s_b, CUdeviceptr* out, uint64_t* o_smn, uint64_t* o_sk, uint64_t* o_sb) {
+  const bool keep_mn_major = (s_mn == 1 && s_k != 1);
+  const uint64_t rows = keep_mn_major ? K : mn, cols = keep_mn_major ? mn : K;
+  const uint64_t pitch = (cols + 7) / 8 * 8;
+  const uint64_t nb = (s_b == 0) ? 1 : batch;
+  CUdeviceptr buf;
+  int rc = pool_alloc(c, nb * rows * pitch * 2, &buf, st);
+  if (rc) return rc;
+  CUfunction f;
+  rc = get_func(c, "convert_fp8_f16", &f);
+  if (rc) { pool_free(c, buf, st); return rc; }
+  ConvertF16Params p{ptr, buf, nb, rows, cols, s_b, keep_mn_major ? s_k : s_mn, keep_mn_major ? s_mn : s_k, pitch, (uint32_t)dtype, 0};
+  const uint64_t vecs = nb * rows * (pitch / 8);
+  const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((vecs + 255) / 256, (uint64_t)c->props.num_sms * 16));
+  void* args[] = {&p};
+  rc = launch(c, f, grid, 1, 1, 256, 0, 1, st, args);
+  if (rc) { pool_free(c, buf, st); return rc; }
+  *out = buf;
+  *o_smn = keep_mn_major ? 1 : pitch;
+  *o_sk = keep_mn_major ? pitch : 1;
+  *o_sb = (s_b == 0) ? 0 : rows * pitch;
+  return B200_OK;
+}
+
+// fp8 products accumulate with less than f32 precision in wgmma; the reference's expectation is an f32 sum of exact products.
+// Both operands are widened to f16 (exact for e4m3 and e5m2, mixed pairs included) and the f16 kernels accumulate in f32.
+static int run_gemm_fp8_as_f16(b200_ctx* c, CUstream st, const GemmProblem& g) {
+  const int rdt = g.rhs_dtype >= 0 ? g.rhs_dtype : g.in_dtype;
+  GemmProblem h = g;
+  h.in_dtype = B200_F16;
+  h.rhs_dtype = -1;
+  CUdeviceptr wa = 0, wb = 0;
+  int rc = widen_fp8_operand(c, st, g.in_dtype, g.a, g.batch, g.M, g.K, g.a_sm, g.a_sk, g.a_sb, &wa, &h.a_sm, &h.a_sk, &h.a_sb);
+  if (!rc) rc = widen_fp8_operand(c, st, rdt, g.b, g.batch, g.N, g.K, g.b_sn, g.b_sk, g.b_sb, &wb, &h.b_sn, &h.b_sk, &h.b_sb);
+  if (!rc) {
+    h.a = wa;
+    h.b = wb;
+    rc = run_gemm(c, st, h);
+  }
+  if (wa) pool_free(c, wa, st);
+  if (wb) pool_free(c, wb, st);
+  return rc;
+}
 
 static int run_gemm(b200_ctx* c, CUstream st, const GemmProblem& g) {
   if (g.M == 0 || g.N == 0 || g.batch == 0) return B200_OK;
   const std::string forced = opt(c, "gemm.variant", "auto");
   bool a_mn = false, b_mn = false;
   const bool tma = g.K > 0 && tma_ok(g, &a_mn, &b_mn);
+  const bool big = g.M * g.N * g.K * g.batch >= (1ull << 21);
+  const bool fp8 = (g.in_dtype == B200_F8E4M3 || g.in_dtype == B200_F8E5M2);
+  if (fp8 && forced != "simt" && g.K > 0 && extents_tma_ok(g) && (tma || (forced == "auto" && big && opt(c, "gemm.stage", "on") == "on")))
+    return run_gemm_fp8_as_f16(c, st, g);
+  // wgmma reads MN-major operands for 16-bit types only: tf32 / 8-bit operands in that layout are staged K-major first
+  if (tma && forced != "simt" && dtype_size(g.in_dtype) != 2 && (a_mn || b_mn)) return run_gemm_staged(c, st, g);
   if (forced == "simt" || !tma) {
     if (forced != "simt" && forced != "auto")
       return fail(B200_ERR_UNSUPPORTED, "gemm.variant=%s forced but operands are not TMA-describable", forced.c_str());
     // Operands whose pitch / base TMA cannot describe (bf16 with K = 4097, an odd sub-view): one staging pass into an
     // aligned pooled copy, then the tensor-core kernel -- the strided SIMT kernel is kept for tiny problems and for
     // outputs without a unit inner stride.  gemm.stage=off keeps the SIMT path (reference-order arithmetic) for everything.
-    const bool big = g.M * g.N * g.K * g.batch >= (1ull << 21);
     if (forced == "auto" && g.K > 0 && big && extents_tma_ok(g) && opt(c, "gemm.stage", "on") == "on") return run_gemm_staged(c, st, g);
     return launch_simt(c, st, g);
   }
@@ -1421,7 +1382,7 @@ static int run_gemm(b200_ctx* c, CUstream st, const GemmProblem& g) {
       h.a_lo = a_p;
       h.b_lo = b_p;
       h.hybrid = true;
-      rc = launch_tcgen05(c, st, h, a_mn, b_mn);
+      rc = launch_wgmma(c, st, h, a_mn, b_mn);
     }
     pool_free(c, a_p, st);
     pool_free(c, b_p, st);
@@ -1444,27 +1405,27 @@ static int run_gemm(b200_ctx* c, CUstream st, const GemmProblem& g) {
       GemmProblem h = g;
       h.a_lo = a_lo;
       h.b_lo = b_lo;
-      rc = launch_tcgen05(c, st, h, a_mn, b_mn);
+      rc = launch_wgmma(c, st, h, a_mn, b_mn);
     }
     // stream-ordered reuse: the pool hands these pages out again only to later work on this context
     pool_free(c, a_lo, st);
     pool_free(c, b_lo, st);
     return rc;
   }
-  return launch_tcgen05(c, st, g, a_mn, b_mn);
+  return launch_wgmma(c, st, g, a_mn, b_mn);
 }
 
 static int run_gemm_staged(b200_ctx* c, CUstream st, const GemmProblem& g) {
   const size_t esz = dtype_size(g.in_dtype);
   GemmProblem h = g;
   CUdeviceptr sa = 0, sb = 0;
-  bool mn;
+  bool mn = false;
   int rc = B200_OK;
-  if (!operand_tma_ok(g.a, esz, g.M, g.K, g.a_sm, g.a_sk, g.a_sb, &mn)) {
+  if (!operand_tma_ok(g.a, esz, g.M, g.K, g.a_sm, g.a_sk, g.a_sb, &mn) || (mn && esz != 2)) {
     rc = stage_operand(c, st, esz, g.a, g.batch, g.M, g.K, g.a_sm, g.a_sk, g.a_sb, &sa, &h.a_sm, &h.a_sk, &h.a_sb);
     if (!rc) h.a = sa;
   }
-  if (!rc && !operand_tma_ok(g.b, esz, g.N, g.K, g.b_sn, g.b_sk, g.b_sb, &mn)) {
+  if (!rc && (!operand_tma_ok(g.b, esz, g.N, g.K, g.b_sn, g.b_sk, g.b_sb, &mn) || (mn && esz != 2))) {
     rc = stage_operand(c, st, esz, g.b, g.batch, g.N, g.K, g.b_sn, g.b_sk, g.b_sb, &sb, &h.b_sn, &h.b_sk, &h.b_sb);
     if (!rc) h.b = sb;
   }
@@ -1592,55 +1553,47 @@ extern "C" int b200_matmul_scaled(b200_ctx* c, b200_stream s, b200_dtype lhs_dty
     void* args[] = {&p};
     return launch(c, f, std::max(1u, grid), 1, 1, 256, 0, 1, st, args);
   }
-  // the problem as the GEMM sees it (operands described to TMA as bytes); the tile variant is chosen BEFORE the scales are
-  // packed, because the 256 x 224 variant wants the rhs scales packed per 224-row tile
-  GemmProblem g{};
-  g.in_dtype = B200_F8E4M3;  // 1-byte marker
-  g.out_dtype = out_dtype;
-  g.a = lhs; g.b = rhs; g.out = out;
-  g.M = M; g.N = N; g.K = k_bytes; g.batch = batch;
-  g.a_sm = k_bytes; g.a_sk = 1; g.a_sb = batch > 1 ? M * k_bytes : 0;
-  g.b_sn = k_bytes; g.b_sk = 1; g.b_sb = batch > 1 ? N * k_bytes : 0;
-  g.o_sm = N; g.o_sn = 1; g.o_sb = batch > 1 ? M * N : 0;
-  g.mx_kind = nvf4 ? 3 : fp4 ? 2 : 1;
-  g.fmt_a = fp4 ? 1u : (lhs_dtype == B200_F8E5M2 ? 1u : 0u);
-  g.fmt_b = fp4 ? 1u : (rhs_dtype == B200_F8E5M2 ? 1u : 0u);
-  g.sf_atoms = atoms;
-  g.sfb_any_layout = !scales_packed;           // pre-packed scales are in the plain 128-row layout
-  SkPlan sk_unused;
-  const GemmVariant* v = pick_variant(c, g, &sk_unused);
-  if (!v) return fail(B200_ERR_INVALID_ARG, "gemm.variant '%s' is not a tcgen05 variant for block-scaled operands%s", forced.c_str(),
-                      scales_packed ? " with pre-packed scales" : "");
-  g.sfb_any_layout = false;
-  g.sfb_tile_rows = (v->block_n == 224) ? 224 : 128;
-  // scales -> the tensor core's packed chunks (skipped when the caller already holds them in that form)
-  const uint64_t tiles_a = (M + 127) / 128;
-  const uint64_t tiles_b = g.sfb_tile_rows == 224 ? 2 * ((N + 223) / 224) : (N + 127) / 128;
-  if (batch * tiles_a >= (1ull << 31) || batch * tiles_b >= (1ull << 31) || atoms * 32 >= (1ull << 31))
-    return fail(B200_ERR_UNSUPPORTED, "matmul_scaled: scale tensor too large for 32-bit TMA coordinates");
-  CUdeviceptr sfa = lhs_scales, sfb = rhs_scales;
-  int rc = B200_OK;
-  if (!scales_packed) {
-    sfa = sfb = 0;
-    rc = pool_alloc(c, batch * tiles_a * atoms * 512, &sfa, st);
-    if (rc) return rc;
-    rc = pool_alloc(c, batch * tiles_b * atoms * 512, &sfb, st);
-    if (rc) { pool_free(c, sfa, st); return rc; }
-    const uint32_t one = nvf4 ? 0x38u : 127u;
-    rc = launch_pack_scales(c, st, lhs_scales, sfa, batch, M, n_scales, tiles_a, atoms, one);
-    if (!rc) rc = launch_pack_scales(c, st, rhs_scales, sfb, batch, N, n_scales, tiles_b, atoms, one, (uint32_t)g.sfb_tile_rows);
-  }
+  // Hopper's tensor cores take no scale factors: each operand is expanded once to bf16 x * scale (exact, see
+  // dequant_scaled_bf16) and the bf16 wgmma GEMM accumulates the products in f32
+  const uint64_t ab = batch * M, bb = batch * N;
+  CUdeviceptr da = 0, db = 0;
+  int rc = pool_alloc(c, ab * K * 2, &da, st);
+  if (rc) return rc;
+  rc = pool_alloc(c, bb * K * 2, &db, st);
+  if (rc) { pool_free(c, da, st); return rc; }
+  auto dequant = [&](uint64_t in, uint64_t scales, CUdeviceptr out_bf16, uint64_t rows, int dtype) {
+    CUfunction f;
+    int r = get_func(c, "dequant_scaled_bf16", &f);
+    if (r) return r;
+    DequantParams p{in, scales, out_bf16, (uint32_t)rows, (uint32_t)batch, (uint32_t)K, fp4 ? 12u : (uint32_t)dtype,
+                    (uint32_t)scale_block, nvf4 ? 1u : 0u, scales_packed ? 1u : 0u, (uint32_t)atoms};
+    const uint64_t groups = batch * rows * (K / 8);
+    const unsigned grid = (unsigned)std::min<uint64_t>((groups + 255) / 256, (uint64_t)c->props.num_sms * 16);
+    void* args[] = {&p};
+    return launch(c, f, std::max(1u, grid), 1, 1, 256, 0, 1, st, args);
+  };
+  rc = dequant(lhs, lhs_scales, da, M, lhs_dtype);
+  if (!rc) rc = dequant(rhs, rhs_scales, db, N, rhs_dtype);
   if (!rc) {
-    g.sfa = sfa; g.sfb = sfb;
-    rc = launch_tcgen05(c, st, g, false, false);
+    GemmProblem g{};
+    g.in_dtype = B200_BF16;
+    g.out_dtype = out_dtype;
+    g.a = da; g.b = db; g.out = out;
+    g.M = M; g.N = N; g.K = K; g.batch = batch;
+    g.a_sm = K; g.a_sk = 1; g.a_sb = batch > 1 ? M * K : 0;
+    g.b_sn = K; g.b_sk = 1; g.b_sb = batch > 1 ? N * K : 0;
+    g.o_sm = N; g.o_sn = 1; g.o_sb = batch > 1 ? M * N : 0;
+    g.mx = true;
+    rc = launch_wgmma(c, st, g, false, false);
   }
-  if (!scales_packed) { pool_free(c, sfa, st); pool_free(c, sfb, st); }
+  pool_free(c, da, st);
+  pool_free(c, db, st);
   return rc;
 }
 
 // Mixed 8-bit operand formats (the cartesian products the reference instantiates for its manual MMA,
 // crates/cubecl-cpp/src/cuda/mma/manual.rs:151-166 i8 x u8 / u8 x i8 and :170-186 fp8 pairs): same kernels, the two format
-// fields of the tcgen05 instruction descriptor differ.
+// operand types of the wgmma instruction differ.
 extern "C" int b200_matmul_mixed(b200_ctx* c, b200_stream s, b200_dtype lhs_dtype, b200_dtype rhs_dtype, b200_dtype out_dtype, b200_dptr lhs,
                                  b200_dptr rhs, b200_dptr out, int rank, const uint64_t* shape_lhs, const uint64_t* strides_lhs,
                                  const uint64_t* shape_rhs, const uint64_t* strides_rhs, const uint64_t* shape_out,
@@ -1765,8 +1718,7 @@ static int launch_reduce_all(b200_ctx* c, CUstream st, int op, int dt, const RVi
   bool bulk = false;
   if (!pitched && !arg) {
     // variants: the plain 128-bit streaming kernel, its tuning forms (f32 sum only) and the bulk-copy staged kernel
-    // auto = the bulk-copy staged kernel once the input is big enough to fill a ring on every SM (measured, 1 GiB f32 sum:
-    // 7.08 TB/s against 6.92 for the best plain-load form, profiles/r02_reduce_sweep.log); plain loads below that
+    // auto = the bulk-copy staged kernel once the input is big enough to fill a ring on every SM; plain loads below that
     const std::string var = opt(c, "reduce.variant", "auto");
     if (var == "tma" || var == "auto") {
       bulk = n * esz >= (var == "tma" ? 64ull * 16384 : (uint64_t)c->props.num_sms * 8 * 16384);
@@ -1779,7 +1731,7 @@ static int launch_reduce_all(b200_ctx* c, CUstream st, int op, int dt, const RVi
   if (bulk) {
     name += "_tma";
     threads = 256 + 32;                       // eight consumer warps + one producer warp
-    stages = opt_uint(c, "reduce.tma_stages", 6, 2, 8);   // measured: 6 x 16 KB 145.4 us, 8 x 16 KB 147.3 us, 4 x 16 KB 150.0 us (1 GiB f32)
+    stages = opt_uint(c, "reduce.tma_stages", 6, 2, 8);   // 6 x 16 KB ring stages (1 GiB f32)
     smem = stages * 16384 + 128;
     const uint64_t tiles = n * esz / 16384;
     const unsigned per_sm = stages <= 6 ? opt_uint(c, "reduce.tma_ctas_per_sm", 1, 1, 2) : 1;
@@ -1824,10 +1776,9 @@ static int launch_rows_kernel(b200_ctx* c, CUstream st, int op, int dt, const RV
   const uint64_t vec = 16 / esz;
   const uint64_t nseg = ceil_div(v.len, seg_len), items = v.outer * nseg;
   // Threads per item (power of two): about `vpt` 128-bit vectors per thread, so a 32 KB row is one 256-thread block and the
-  // grid has many more blocks than resident slots (the hardware scheduler balances the tail block by block -- a warp per
-  // 32 KB row left the last, nearly empty wave running at a third of the bandwidth: ncu, round 1).
-  // measured (profiles/r02_reduce_sweep.log): 16 vectors per thread for inputs that stream from HBM for a while ([9000,16384]
-  // 6.38 vs 6.09 TB/s, argmax [8192,8192] 5.65 vs 4.90), 8 for small launch-bound inputs ([512,8192] 7.1 vs 8.6 us)
+  // grid has many more blocks than resident slots (the hardware scheduler balances the tail block by block; a warp per
+  // 32 KB row would leave a last, nearly empty wave).
+  // 16 vectors per thread for inputs that stream from HBM for a while, 8 for small launch-bound inputs
   const bool big = v.outer * v.len * esz >= (128ull << 20);
   const unsigned vpt = opt_uint(c, "reduce.rows_vpt", big ? 16 : 8, 1, 64);
   const uint64_t nv = ceil_div(std::min(seg_len, v.len), vec);
@@ -1931,8 +1882,8 @@ static int reduce_axis_view(b200_ctx* c, CUstream st, int op, int dt, const RVie
     const uint64_t tiles = ceil_div(units, std::min<uint64_t>(units, 32));
     const unsigned bps = opt_uint(c, "reduce.cols_blocks_per_sm", 4, 1, 64);
     if (v.outer * tiles < sms * bps && v.len >= 256) {
-      // ~8 blocks per SM (two resident waves of big blocks) measured best on average for value ops (eight loads in flight per
-      // thread) and arg ops (four) alike -- profiles/r02_cols_sweep.log.  Target 0: exactly one resident wave (4 blocks per SM).
+      // ~8 blocks per SM (two resident waves of big blocks) for value ops (eight loads in flight per thread) and arg ops (four)
+      // alike.  Target 0: exactly one resident wave (4 blocks per SM).
       const unsigned tgt = opt_uint(c, "reduce.cols_split_target", 8, 0, 256);
       uint64_t nseg;
       if (tgt == 0) nseg = std::max<uint64_t>(1, (sms * 4) / (v.outer * tiles));
@@ -2383,41 +2334,34 @@ extern "C" int b200_probe_wmma(b200_ctx* c, b200_stream s, b200_dtype dtype, uin
   return rc;
 }
 
-extern "C" int b200_probe_umma(b200_ctx* c, b200_stream s, uint32_t n_iter, b200_dptr scratch, double* ops) {
-  CTX_ENTER_DEVICE(c);
+// Tensor-core peak probe (wgmma_probe_* in gemm_wgmma.cu): one CTA per SM, two warpgroups each issuing 4 m64n256 wgmma per
+// iteration on shared-memory operands.  K per instruction: 16 (bf16), 32 (e4m3).
+static int probe_wgmma(b200_ctx* c, b200_stream s, const char* name, double k_per_instr, uint32_t n_iter, b200_dptr scratch, double* ops) {
   CUfunction f;
-  int rc = get_func(c, "umma_probe_bf16_2sm", &f);
+  int rc = get_func(c, name, &f);
   if (rc) return rc;
-  const unsigned smem = 32768 + 1024 + 64;
+  const unsigned smem = 16384 + 32768 + 1024;
   CU_CHECK(g_drv.cuFuncSetAttribute_p(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem));
-  const unsigned clusters = (unsigned)std::max(1, c->props.num_sms / 2);
+  const unsigned grid = (unsigned)std::max(1, c->props.num_sms);
   uint64_t sp = scratch;
   void* args[] = {&sp, &n_iter};
-  rc = launch(c, f, clusters * 2, 1, 1, 256, smem, 2, resolve_stream(c, s), args);
-  if (!rc && ops) *ops = static_cast<double>(clusters) * n_iter * 4.0 * 2.0 * 256 * 256 * 16;
+  rc = launch(c, f, grid, 1, 1, 384, smem, 1, resolve_stream(c, s), args);
+  if (!rc && ops) *ops = static_cast<double>(grid) * 2 * n_iter * 4.0 * 2.0 * 64 * 256 * k_per_instr;
   return rc;
+}
+
+extern "C" int b200_probe_umma(b200_ctx* c, b200_stream s, uint32_t n_iter, b200_dptr scratch, double* ops) {
+  CTX_ENTER_DEVICE(c);
+  return probe_wgmma(c, s, "wgmma_probe_bf16", 16.0, n_iter, scratch, ops);
 }
 
 extern "C" int b200_probe_umma_kind(b200_ctx* c, b200_stream s, b200_dtype dtype, int block_scaled, uint32_t n_iter, b200_dptr scratch,
                                     double* ops) {
   CTX_ENTER_DEVICE(c);
-  if (dtype == B200_BF16 && !block_scaled) return b200_probe_umma(c, s, n_iter, scratch, ops);
-  const char* name = (dtype == B200_F8E4M3 && !block_scaled) ? "umma_probe_e4m3_2sm"
-                     : (dtype == B200_F8E4M3 && block_scaled) ? "umma_probe_mxf8_2sm"
-                     : (dtype == B200_F4E2M1X2 && block_scaled) ? "umma_probe_mxf4_2sm" : nullptr;
-  if (!name) return fail(B200_ERR_UNSUPPORTED, "probe_umma_kind: bf16, f8e4m3 (plain or block-scaled) or block-scaled f4e2m1x2");
-  CUfunction f;
-  int rc = get_func(c, name, &f);
-  if (rc) return rc;
-  const unsigned smem = 32768 + 2048 + 1024 + 64;
-  CU_CHECK(g_drv.cuFuncSetAttribute_p(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem));
-  const unsigned clusters = (unsigned)std::max(1, c->props.num_sms / 2);
-  uint64_t sp = scratch;
-  void* args[] = {&sp, &n_iter};
-  rc = launch(c, f, clusters * 2, 1, 1, 256, smem, 2, resolve_stream(c, s), args);
-  const double k_per_instr = dtype == B200_F4E2M1X2 ? 64.0 : 32.0;
-  if (!rc && ops) *ops = static_cast<double>(clusters) * n_iter * 4.0 * 2.0 * 256 * 256 * k_per_instr;
-  return rc;
+  if (block_scaled) return fail(B200_ERR_UNSUPPORTED, "probe_umma_kind: sm_90 tensor cores have no block-scaled MMA");
+  if (dtype == B200_BF16) return probe_wgmma(c, s, "wgmma_probe_bf16", 16.0, n_iter, scratch, ops);
+  if (dtype == B200_F8E4M3) return probe_wgmma(c, s, "wgmma_probe_e4m3", 32.0, n_iter, scratch, ops);
+  return fail(B200_ERR_UNSUPPORTED, "probe_umma_kind: bf16 or f8e4m3");
 }
 
 extern "C" int b200_probe_memread(b200_ctx* c, b200_stream s, b200_dptr buf, uint64_t bytes, b200_dptr scratch) {

@@ -1,0 +1,676 @@
+// Hand-written sm_90a GEMM: TMA -> 128B-swizzled smem ring -> wgmma (accumulators in registers) -> direct stores.
+// Persistent, warp-specialised: warpgroup 0 is the producer (one thread issues the TMA loads), warpgroups 1 and 2 each
+// run wgmma on 64 rows of the CTA's 128-row tile.  Optional 2-CTA cluster (CG = 2, "2sm" tiles of 256 x BLOCK_N): each
+// CTA computes its own 128 rows and loads half of the B tile, multicast into both CTAs, so a pair reads B from L2 once.
+//
+// Replaces: the (out-of-tree, cubek) `matmul::launch` kernel bodies that CubeCL lowers to nvcuda::wmma / mma.sync
+// through crates/cubecl-cpp/src/shared/mma.rs:48-174 and crates/cubecl-cpp/src/cuda/ptx/mma.rs:30-61.
+// Semantics follow the reference's CPU expectation `test_simple_cube_expected`
+// (crates/cubecl-core/src/runtime_tests/cmma.rs:695-721): inputs widened to f32, f32 accumulate over increasing k.
+// Shape / batch-broadcast rule: crates/cubecl-zspace/src/shape.rs:489-517 (resolved on the host, see capi.cpp).
+//
+// Compiled to a cubin (no host code here): nvcc -cubin -gencode arch=compute_90a,code=sm_90a
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+
+#include "ptx.cuh"
+
+using namespace b200;
+
+struct GemmParams {
+  uint64_t out;               // device pointer of out[batch, M, N]
+  uint64_t out_row_stride;    // in elements
+  uint64_t out_batch_stride;  // in elements
+  uint32_t M, N, K, batch;
+  uint32_t tiles_m, tiles_n;  // tile grid per batch; a tile is (128*CG) x BLOCK_N
+  uint32_t group_m;           // rasterisation: tiles are walked in column strips of `group_m` tile-rows (L2 reuse)
+  uint32_t a_bmul, b_bmul;    // 0 = operand broadcast over batch (tensor map has batch extent 1), 1 = batched
+  uint32_t vec_store;         // 1 when every output row start is 16-byte aligned
+  uint32_t k_segments;        // 1, or 3 for the 3xTF32 schedule: the K loop runs three times over (A,B), (A,B_lo), (A_lo,B)
+  uint32_t epi_act;           // fused epilogue (float accumulators only): 0 = none, 1 = relu, 2 = gelu (erf form)
+  uint64_t bias;              // f32[N] added per output column, or 0
+  float alpha;                // out = act(alpha * acc + bias[n]); the epilogue is skipped when alpha == 1, bias == 0, act == 0
+  uint32_t epi_on;
+  // Stream-K head (deterministic, replaces a mostly empty LAST wave): tiles [0, full_tiles) are whole "data-parallel" tiles;
+  // the k-blocks of the remaining `sk_tiles` tiles form one linear space of sk_tiles * num_kb k-blocks that is cut into
+  // `sk_ranges` equal ranges; cluster c works through ranges c, c + C, ... FIRST (a range may cover the end of one tile and
+  // the start of the next: one work unit per tile it touches), then through its whole tiles c, c + C, ....  A unit that
+  // covers only part of a tile's K stores its f32 accumulators to its own slab and takes a ticket for the tile; whoever
+  // completes the tile adds the slabs in k order (so the result does not depend on who came last) and writes the output --
+  // under the MMAs of the following whole tiles, which is why the partial tiles go first.  sk_tiles == 0 disables it.
+  uint32_t full_tiles, sk_tiles, sk_ranges, sk_umax;  // sk_umax: slabs reserved per range (max tiles a range can touch)
+  uint64_t split_ws;          // slabs: [sk_ranges][sk_umax][CG] x (128 x BLOCK_N f32, in accumulator-fragment order)
+  uint64_t split_tickets;     // u32 [sk_tiles][CG], zero on entry, left zero on exit
+  // 8-bit kinds: a MIXED pair (e4m3 x e5m2, u8 x s8 ..., the reference's manual-MMA cartesian products,
+  // crates/cubecl-cpp/src/cuda/mma/manual.rs:151-186) when fmt_mixed != 0; fmt_b is then the rhs format (0 = e4m3 / u8,
+  // 1 = e5m2 / s8).  The lhs format is the kernel's own.
+  uint32_t fmt_b, fmt_mixed;
+  // Hybrid f32 schedule (tf32 kernels, k_segments == 3): segment 0 is the tf32 product of the ORIGINAL operands (their top
+  // 19 bits); segments 1 and 2 are the cross terms A*B_lo and A_lo*B on bf16 copies at twice the tensor rate -- bf16
+  // wgmma into the same f32 accumulators, 64 elements of K per stage instead of 32.  tma_a_lo / tma_b_lo then describe
+  // bf16 PAIR buffers [2 * entries][rows][pitch]: entries [0, hyb_nba) hold bf16(x), entries [hyb_nba, 2 hyb_nba) hold
+  // bf16(x - trunc_tf32(x)).  Two tensor passes' worth of time instead of 3xTF32's three.
+  uint32_t hyb, hyb_nba, hyb_nbb;
+  // 1: whole tiles leave through swizzled shared-memory staging and TMA stores (tma_out describes `out` as (N, M, batch),
+  // [128 B x 64 rows] boxes); needs a 16-byte aligned base and row / batch pitches.  0: each thread stores its own fragment.
+  uint32_t tma_store;
+};
+
+enum : int { KIND_F16 = 0, KIND_BF16 = 1, KIND_TF32 = 2, KIND_E4M3 = 3, KIND_E5M2 = 4, KIND_U8 = 5, KIND_S8 = 6 };
+enum : int { OUT_F16 = 0, OUT_BF16 = 1, OUT_F32 = 2 };  // OUT_F32 is a raw 32-bit store: it also carries the s32 accumulators of the int kinds
+
+constexpr int kNumThreads = 384;  // warpgroup 0: TMA producer, warpgroups 1-2: wgmma + epilogue (64 rows each)
+
+#include <type_traits>
+struct TileCoord {
+  uint32_t b, m_blk, n_blk;
+};
+
+__device__ __forceinline__ TileCoord tile_coord(uint32_t t, const GemmParams& p) {
+  const uint32_t per_batch = p.tiles_m * p.tiles_n;
+  TileCoord c;
+  c.b = t / per_batch;
+  uint32_t r = t - c.b * per_batch;
+  const uint32_t strip = p.group_m * p.tiles_n;
+  const uint32_t g = r / strip;
+  const uint32_t first_m = g * p.group_m;
+  const uint32_t gsize = min(p.group_m, p.tiles_m - first_m);
+  const uint32_t in = r - g * strip;
+  c.m_blk = first_m + in % gsize;
+  c.n_blk = in / gsize;
+  return c;
+}
+
+struct WorkUnit {
+  uint32_t tile, kb0, kb1;
+  uint32_t slab;   // partial units: slab index (range * sk_umax + unit within the range)
+  bool partial;
+};
+
+// The sequence of work units of one CTA pair: stream-K ranges first, whole tiles after (see GemmParams).  Every role of the
+// CTA (TMA producers, MMA issuer, epilogue warps) walks the same sequence with its own copy of this iterator.
+struct UnitIter {
+  uint32_t c, C, num_kb;
+  uint32_t r;          // current stream-K range (c, c + C, ...), >= sk_ranges once the head is done
+  uint32_t u;          // unit index inside the current range
+  uint64_t pos, hi;    // unconsumed part [pos, hi) of the current range, in linear k-blocks
+  uint32_t next_tile;  // next whole tile
+  bool open;           // [pos, hi) of range r has been set up
+};
+
+__device__ __forceinline__ UnitIter unit_iter(uint32_t cluster, uint32_t n_clusters, uint32_t num_kb) {
+  UnitIter it;
+  it.c = cluster; it.C = n_clusters; it.num_kb = num_kb;
+  it.r = cluster; it.u = 0; it.pos = 0; it.hi = 0; it.next_tile = cluster; it.open = false;
+  return it;
+}
+
+__device__ __forceinline__ uint64_t sk_range_lo(uint32_t r, const GemmParams& p, uint32_t num_kb) {
+  return (static_cast<uint64_t>(r) * p.sk_tiles * num_kb) / p.sk_ranges;
+}
+// range that owns linear k-block x: the largest r with sk_range_lo(r) <= x (ranges are non-empty: sk_ranges <= sk_tiles * num_kb)
+__device__ __forceinline__ uint32_t sk_owner(uint64_t x, const GemmParams& p, uint32_t num_kb) {
+  return static_cast<uint32_t>(((x + 1) * p.sk_ranges - 1) / (static_cast<uint64_t>(p.sk_tiles) * num_kb));
+}
+
+__device__ __forceinline__ bool next_unit(UnitIter& it, const GemmParams& p, WorkUnit& w) {
+  while (p.sk_tiles != 0 && it.r < p.sk_ranges) {
+    if (!it.open) {
+      it.pos = sk_range_lo(it.r, p, it.num_kb);
+      it.hi = sk_range_lo(it.r + 1, p, it.num_kb);
+      it.u = 0;
+      it.open = true;
+    }
+    if (it.pos < it.hi) {
+      const uint32_t tau = static_cast<uint32_t>(it.pos / it.num_kb);
+      const uint64_t t0 = static_cast<uint64_t>(tau) * it.num_kb;
+      const uint64_t end = (it.hi < t0 + it.num_kb) ? it.hi : t0 + it.num_kb;
+      w.tile = p.full_tiles + tau;
+      w.kb0 = static_cast<uint32_t>(it.pos - t0);
+      w.kb1 = static_cast<uint32_t>(end - t0);
+      w.partial = !(w.kb0 == 0 && w.kb1 == it.num_kb);
+      w.slab = it.r * p.sk_umax + it.u;
+      it.pos = end;
+      ++it.u;
+      return true;
+    }
+    it.r += it.C;
+    it.open = false;
+  }
+  if (it.next_tile < p.full_tiles) {
+    w.tile = it.next_tile; w.kb0 = 0; w.kb1 = it.num_kb; w.slab = 0; w.partial = false;
+    it.next_tile += it.C;
+    return true;
+  }
+  return false;
+}
+
+
+// Stores of one accumulator fragment pair: columns n, n + 1 of one output row.
+template <int OUT>
+__device__ __forceinline__ void store_pair(uint64_t row_ptr, uint32_t n, uint32_t N, bool vec, uint32_t v0, uint32_t v1) {
+  if constexpr (OUT == OUT_F32) {
+    uint32_t* dst = reinterpret_cast<uint32_t*>(row_ptr) + n;
+    if (vec && n + 1 < N) *reinterpret_cast<uint2*>(dst) = make_uint2(v0, v1);
+    else { if (n < N) dst[0] = v0; if (n + 1 < N) dst[1] = v1; }
+  } else {
+    uint16_t* dst = reinterpret_cast<uint16_t*>(row_ptr) + n;
+    uint32_t packed;   // cvt packs (hi, lo): lo lands in the low half, the lower address
+    if constexpr (OUT == OUT_BF16) asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(packed) : "r"(v1), "r"(v0));
+    else asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(packed) : "r"(v1), "r"(v0));
+    if (vec && n + 1 < N) *reinterpret_cast<uint32_t*>(dst) = packed;
+    else { if (n < N) dst[0] = static_cast<uint16_t>(packed & 0xFFFFu); if (n + 1 < N) dst[1] = static_cast<uint16_t>(packed >> 16); }
+  }
+}
+
+__device__ __forceinline__ uint32_t acc_bits(float x) { return __float_as_uint(x); }
+__device__ __forceinline__ uint32_t acc_bits(uint32_t x) { return x; }
+
+// PROMOTE (the block-scaled kernels): every k-block is summed by wgmma into a fresh register partial (one 128- or 112-column
+// part of the tile at a time), which is then added to the f32 accumulators with round-to-nearest adds.  wgmma truncates as it
+// accumulates; promoting per 64 elements of K keeps that error to one k-block instead of letting it build up over K.
+// MT: 128-row sub-tiles of M per CTA.  MT = 2 (the 2sm_m512 pair tile, 512 x BLOCK_N per CTA pair) gives each consumer
+// warpgroup two m64 row blocks that share every B stage: per FLOP the pair reads a third less operand data from L2 than the
+// 256 x 256 tile at the same accumulator count per thread.
+template <int CG, int BLOCK_N, bool A_MN, bool B_MN, int KIND, int OUT, int STAGES, bool PROMOTE = false, int MT = 1>
+__device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUtensorMap* tma_b_hi, const CUtensorMap* tma_a_lo,
+                                          const CUtensorMap* tma_b_lo, const CUtensorMap* tma_out, const GemmParams& p) {
+  constexpr bool INT_ACC = (KIND == KIND_U8 || KIND == KIND_S8);
+  constexpr int ESZ = (KIND == KIND_TF32) ? 4 : (KIND >= KIND_E4M3) ? 1 : 2;
+  static_assert(ESZ == 2 || (!A_MN && !B_MN), "wgmma reads MN-major operands for 16-bit kinds only");
+  constexpr int BLOCK_K = 128 / ESZ;  // one 128-byte swizzle row of K per stage
+  constexpr int MMA_K = 32 / ESZ;     // K per wgmma instruction: 32 bytes
+  constexpr int N_LOCAL = BLOCK_N / CG;  // rows of the B tile this CTA loads (multicast to the pair)
+  constexpr uint32_t A_SUB_BYTES = 128 * 128;       // one 128-row sub-tile of A: 128 rows x 128 B
+  constexpr uint32_t A_BYTES = MT * A_SUB_BYTES;
+  constexpr uint32_t B_BYTES = BLOCK_N * 128;
+  constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
+  constexpr int CHUNK_N = 64;                        // MN-major operand (16-bit): M/N elements per 128-byte row
+  constexpr uint32_t CHUNK_BYTES = BLOCK_K * 128;    // MN-major operand: one [BLOCK_K x 128 B] chunk
+  constexpr int NUM_CHUNKS = N_LOCAL / CHUNK_N;      // B chunks this CTA loads
+  constexpr int NACC = BLOCK_N / 2;                  // accumulator registers per thread (m64 x BLOCK_N per warpgroup)
+  static_assert(STAGE_BYTES % 1024 == 0, "stages must keep 1024-byte alignment for SWIZZLE_128B");
+  using Acc = typename std::conditional<INT_ACC, uint32_t, float>::type;
+  static_assert(!PROMOTE || (KIND == KIND_BF16 && !A_MN && !B_MN && MT == 1), "promoted accumulation: bf16, K-major operands");
+  static_assert(MT == 1 || (MT == 2 && ESZ == 2), "two M sub-tiles per CTA: 16-bit kinds");
+  constexpr int PH = (BLOCK_N % 128 == 0) ? 128 : 112;   // promoted partial: columns per wgmma (N = 224 -> two of 112)
+  static_assert(!PROMOTE || BLOCK_N % PH == 0, "promoted partials tile BLOCK_N");
+  constexpr int CW = (OUT == OUT_F32) ? 32 : 64;         // TMA-store staging: columns per 128-byte staging row
+
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t bar_base = smem_base + STAGES * STAGE_BYTES;
+  auto full_bar = [&](int s) { return bar_base + 8u * s; };
+  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
+  const uint32_t split_flag = bar_base + 16u * STAGES;  // "this CTA reduces the slabs" broadcast among the consumer threads
+  const uint32_t epi_base = bar_base + 1024u;            // TMA-store staging: one [64 rows x 128 B] tile per consumer warpgroup
+
+  const uint32_t wg = threadIdx.x >> 7;
+  const uint32_t rank = (CG == 2) ? cluster_ctarank() : 0u;
+  const uint32_t cluster_id = (CG == 2) ? cluster_id_x() : blockIdx.x;
+  const uint32_t n_clusters = (CG == 2) ? num_clusters_x() : gridDim.x;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(tma_a_hi);
+    tma_prefetch_desc(tma_b_hi);
+    if (p.k_segments > 1) { tma_prefetch_desc(tma_a_lo); tma_prefetch_desc(tma_b_lo); }
+    if (p.tma_store) tma_prefetch_desc(tma_out);
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(full_bar(s), 1);        // one arrive.expect_tx by this CTA's producer; the peer's multicast bytes counted too
+      mbar_init(empty_bar(s), 2 * CG);  // one arrive per consumer warpgroup of every CTA that writes into this stage
+    }
+    fence_mbar_init();
+  }
+  if constexpr (CG == 2) cluster_sync_all(); else __syncthreads();
+
+  // 3xTF32: x = hi + lo with hi = the top 19 bits of x (exactly what the tf32 datapath reads from an f32 operand, so the
+  // ORIGINAL tensors serve as "hi") and lo = x - hi materialised once.  A*B ~= hi*hi + hi*lo + lo*hi is accumulated by
+  // running the K loop over three segments with the operand tensor maps swapped per segment.
+  const uint32_t seg_kb = (p.K + BLOCK_K - 1) / BLOCK_K;
+  // hybrid schedule: the two bf16 segments cover K in 64-element stages (half as many k-blocks as the tf32 segment)
+  const bool hyb = (KIND == KIND_TF32) && p.hyb != 0 && p.k_segments == 3;
+  const uint32_t seg_kb1 = hyb ? (p.K + 63u) / 64u : seg_kb;
+  const uint32_t num_kb = (p.k_segments == 3) ? seg_kb + 2u * seg_kb1 : seg_kb * p.k_segments;
+  // (segment, k-block within it) of linear k-block kb
+  auto seg_of = [&](uint32_t kb, uint32_t& seg, uint32_t& kk) {
+    seg = 0; kk = kb;
+    if (kk >= seg_kb) { kk -= seg_kb; seg = 1u + kk / seg_kb1; kk -= (seg - 1u) * seg_kb1; }
+  };
+
+  if (wg == 0) {
+    // ===================================================================== TMA producer (one thread)
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      uint32_t s = 0, ph = 0;
+      UnitIter it = unit_iter(cluster_id, n_clusters, num_kb);
+      WorkUnit wu;
+      while (next_unit(it, p, wu)) {
+        const TileCoord tc = tile_coord(wu.tile, p);
+        const int m0 = static_cast<int>((tc.m_blk * CG + rank) * (128 * MT));
+        const int nb0 = static_cast<int>(tc.n_blk * BLOCK_N);
+        const int ba = static_cast<int>(tc.b * p.a_bmul), bb = static_cast<int>(tc.b * p.b_bmul);
+        uint32_t seg, kk;  // segment (0 unless k_segments == 3), k-block within it
+        seg_of(wu.kb0, seg, kk);
+        for (uint32_t kb = wu.kb0; kb < wu.kb1; ++kb) {
+          mbar_wait(empty_bar(s), ph ^ 1);   // every consumer of the pair has released the stage
+          const uint32_t sa = smem_base + s * STAGE_BYTES;
+          const uint32_t sb = sa + A_BYTES;
+          const uint32_t fb = full_bar(s);
+          mbar_arrive_expect_tx(fb, STAGE_BYTES);
+          // B rows [rank * N_LOCAL, (rank + 1) * N_LOCAL) of the tile land at the same offset in both CTAs of a pair
+          auto load_b = [&](uint32_t dst, const CUtensorMap* m, int c0, int c1, int c2) {
+            if constexpr (CG == 2) tma_load_3d_mc(dst, m, fb, static_cast<uint16_t>(3), c0, c1, c2);
+            else tma_load_3d(dst, m, fb, c0, c1, c2);
+          };
+          bool h16 = false;
+          if constexpr (KIND == KIND_TF32) h16 = hyb && seg != 0;
+          if (h16) {
+            // bf16 stage of the hybrid schedule (K-major operands): the same bytes per stage, 64 elements of K
+            const int k0 = static_cast<int>(kk * 64u);
+            const int ea = ba + static_cast<int>(seg == 2 ? p.hyb_nba : 0u), eb = bb + static_cast<int>(seg == 1 ? p.hyb_nbb : 0u);
+            tma_load_3d(sa, tma_a_lo, fb, k0, m0, ea);
+            load_b(sb + rank * N_LOCAL * 128u, tma_b_lo, k0, nb0 + static_cast<int>(rank * N_LOCAL), eb);
+          } else {
+            const int k0 = static_cast<int>(kk * BLOCK_K);
+            const CUtensorMap* tma_a = (seg == 2) ? tma_a_lo : tma_a_hi;
+            const CUtensorMap* tma_b = (seg == 1) ? tma_b_lo : tma_b_hi;
+            if constexpr (A_MN) {
+#pragma unroll
+              for (int c = 0; c < MT * 128 / CHUNK_N; ++c) tma_load_3d(sa + c * CHUNK_BYTES, tma_a, fb, m0 + c * CHUNK_N, k0, ba);
+            } else {
+#pragma unroll
+              for (int mt = 0; mt < MT; ++mt) tma_load_3d(sa + mt * A_SUB_BYTES, tma_a, fb, k0, m0 + mt * 128, ba);
+            }
+            if constexpr (B_MN) {
+#pragma unroll
+              for (int c = 0; c < NUM_CHUNKS; ++c) {
+                const int ci = static_cast<int>(rank) * NUM_CHUNKS + c;
+                load_b(sb + ci * CHUNK_BYTES, tma_b, nb0 + ci * CHUNK_N, k0, bb);
+              }
+            } else {
+              load_b(sb + rank * N_LOCAL * 128u, tma_b, k0, nb0 + static_cast<int>(rank * N_LOCAL), bb);
+            }
+          }
+          if (++kk == (seg == 0 ? seg_kb : seg_kb1)) { kk = 0; ++seg; }
+          if (++s == STAGES) { s = 0; ph ^= 1; }
+        }
+      }
+    }
+  } else {
+    // ===================================================================== wgmma consumers (64 rows of each sub-tile) + epilogue
+    setmaxnreg_inc<232>();
+    const uint32_t cw = wg - 1;                    // 64-row half of each 128-row sub-tile
+    const uint32_t ct = threadIdx.x - 128;         // consumer thread 0..255
+    const uint32_t t = threadIdx.x & 127;          // thread in the warpgroup
+    const uint32_t lane = t & 31, wq = t >> 5;
+    const uint32_t peer_empty0 = (CG == 2) ? mapa_shared(empty_bar(0), rank ^ 1u) : 0u;
+    const bool elected = (t == 0);
+    auto release = [&](uint32_t st) {
+      if (elected) {
+        mbar_arrive(empty_bar(st));
+        if constexpr (CG == 2) mbar_arrive_cluster(peer_empty0 + 8u * st);
+      }
+    };
+    // 8-bit kinds: the rhs format of a mixed pair is chosen at run time (same smem layout, another instruction)
+    const bool mixed = (ESZ == 1) && p.fmt_mixed != 0 && p.fmt_b != ((KIND == KIND_E5M2 || KIND == KIND_S8) ? 1u : 0u);
+    constexpr int KIND_OTHER = (KIND == KIND_E4M3) ? KIND_E5M2 : (KIND == KIND_E5M2) ? KIND_E4M3 : (KIND == KIND_U8) ? KIND_S8
+                               : (KIND == KIND_S8) ? KIND_U8 : KIND;
+    const uint32_t osz = (OUT == OUT_F32) ? 4 : 2;
+    Acc acc[MT][NACC];
+    uint32_t s = 0, ph = 0;
+    UnitIter it = unit_iter(cluster_id, n_clusters, num_kb);
+    WorkUnit wu;
+    while (next_unit(it, p, wu)) {
+      const TileCoord tc = tile_coord(wu.tile, p);
+      uint32_t seg = 0, kk = 0;
+      if constexpr (KIND == KIND_TF32) seg_of(wu.kb0, seg, kk);
+      uint32_t prev = 0;
+      if constexpr (PROMOTE) {
+#pragma unroll
+        for (int i = 0; i < NACC; ++i) acc[0][i] = 0.f;
+      }
+      for (uint32_t kb = wu.kb0; kb < wu.kb1; ++kb) {
+        mbar_wait(full_bar(s), ph);
+        const uint32_t sa = smem_base + s * STAGE_BYTES;
+        const uint32_t sb = sa + A_BYTES;
+        // A rows of (sub-tile mt, half cw): K-major 128-byte rows, or the (2 mt + cw)-th 64-element MN-major chunk
+        auto a_desc_of = [&](int mt) {
+          return A_MN ? make_smem_desc_sw128(sa + (2u * mt + cw) * CHUNK_BYTES, CHUNK_BYTES, 1024)
+                      : make_smem_desc_sw128(sa + mt * A_SUB_BYTES + cw * 64u * 128u, 16, 1024);
+        };
+        const uint64_t a_desc = a_desc_of(0);
+        const uint64_t b_desc = B_MN ? make_smem_desc_sw128(sb, CHUNK_BYTES, 1024) : make_smem_desc_sw128(sb, 16, 1024);
+        if constexpr (PROMOTE) {
+          float part[PH / 2];
+#pragma unroll
+          for (int h = 0; h < BLOCK_N / PH; ++h) {
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+              wgmma_ss<PH, KIND_BF16, KIND_BF16, 0, 0>(part, a_desc + 2 * k, b_desc + ((h * PH * 128u) >> 4) + 2 * k, k != 0 ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_operands(part);
+#pragma unroll
+            for (int i = 0; i < PH / 2; ++i) acc[0][PH / 2 * h + i] += part[i];
+          }
+          release(s);
+        } else {
+  #pragma unroll
+          for (int mt = 0; mt < MT; ++mt) wgmma_fence_operands(acc[mt]);
+          wgmma_fence();
+          bool h16 = false;
+          if constexpr (KIND == KIND_TF32) {
+            h16 = hyb && seg != 0;
+            if (++kk == (seg == 0 ? seg_kb : seg_kb1)) { kk = 0; ++seg; }
+          }
+          if (h16) {
+            // bf16 stage of the hybrid schedule: 16 elements of K (32 bytes) per instruction, K-major operands
+            if constexpr (KIND == KIND_TF32) {
+  #pragma unroll
+              for (int k = 0; k < 4; ++k)
+                wgmma_ss<BLOCK_N, KIND_BF16, KIND_BF16, 0, 0>(acc[0], a_desc + 2 * k, b_desc + 2 * k, (kb != wu.kb0 || k != 0) ? 1u : 0u);
+            }
+          } else if (mixed) {
+            if constexpr (ESZ == 1) {
+  #pragma unroll
+              for (int k = 0; k < BLOCK_K / MMA_K; ++k)
+                wgmma_ss<BLOCK_N, KIND, KIND_OTHER, 0, 0>(acc[0], a_desc + 2 * k, b_desc + 2 * k, (kb != wu.kb0 || k != 0) ? 1u : 0u);
+            }
+          } else {
+  #pragma unroll
+            for (int k = 0; k < BLOCK_K / MMA_K; ++k) {
+              const uint64_t b_k = b_desc + static_cast<uint64_t>(B_MN ? ((k * MMA_K * 128) >> 4) : 2 * k);
+  #pragma unroll
+              for (int mt = 0; mt < MT; ++mt) {
+                const uint64_t a_k = a_desc_of(mt) + static_cast<uint64_t>(A_MN ? ((k * MMA_K * 128) >> 4) : 2 * k);
+                wgmma_ss<BLOCK_N, KIND, KIND, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc[mt], a_k, b_k, (kb != wu.kb0 || k != 0) ? 1u : 0u);
+              }
+            }
+          }
+          wgmma_commit();
+          if (kb != wu.kb0) {
+            wgmma_wait<1>();   // the previous k-block's MMAs have retired: its stage may be refilled
+            release(prev);
+          }
+  #pragma unroll
+          for (int mt = 0; mt < MT; ++mt) wgmma_fence_operands(acc[mt]);   // after the wait: fencing the accumulators of the group still in flight would retire it first
+          prev = s;
+        }
+        if (++s == STAGES) { s = 0; ph ^= 1; }
+      }
+      if constexpr (!PROMOTE) {
+        wgmma_wait<0>();
+#pragma unroll
+        for (int mt = 0; mt < MT; ++mt) wgmma_fence_operands(acc[mt]);
+        release(prev);
+      }
+
+      // fragment of m64nNk*: thread (warp wq, lane) holds rows 16 wq + lane / 4 (+8) and column pairs 8 j + 2 (lane % 4)
+      const uint32_t m_cta = (tc.m_blk * CG + rank) * (128u * MT);
+      const uint32_t c0 = tc.n_blk * BLOCK_N + 2u * (lane & 3u);
+      // fused epilogue of fragment group j: v = {(r, n), (r, n + 1), (r + 8, n), (r + 8, n + 1)}
+      auto epilogue = [&](uint32_t n, uint32_t (&v)[4]) {
+        if (!INT_ACC && p.epi_on) {
+          const float* bias = reinterpret_cast<const float*>(p.bias);
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const uint32_t col = n + (e & 1);
+            float x = __uint_as_float(v[e]) * p.alpha;
+            if (bias != nullptr && col < p.N) x += __ldg(bias + col);
+            if (p.epi_act == 1) x = fmaxf(x, 0.f);
+            else if (p.epi_act == 2) x = 0.5f * x * (1.f + erff(x * 0.70710678118654752f));
+            v[e] = __float_as_uint(x);
+          }
+        }
+      };
+      // direct stores of fragment group j of sub-tile mt
+      auto store_group = [&](int mt, int j, uint32_t (&v)[4]) {
+        const uint32_t n = c0 + 8u * j;
+        if (n >= p.N) return;
+        epilogue(n, v);
+        const uint32_t r0 = m_cta + mt * 128u + cw * 64u + wq * 16u + (lane >> 2);
+        const uint64_t row0 = p.out + (static_cast<uint64_t>(tc.b) * p.out_batch_stride + static_cast<uint64_t>(r0) * p.out_row_stride) * osz;
+        if (r0 < p.M) store_pair<OUT>(row0, n, p.N, p.vec_store != 0, v[0], v[1]);
+        if (r0 + 8 < p.M) store_pair<OUT>(row0 + static_cast<uint64_t>(8) * p.out_row_stride * osz, n, p.N, p.vec_store != 0, v[2], v[3]);
+      };
+      auto frag = [&](int mt, int j, uint32_t (&v)[4]) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) v[e] = acc_bits(acc[mt][4 * j + e]);
+      };
+      const bool partial = (MT == 1) && !INT_ACC && wu.partial;   // the host plans no stream-K head for these
+
+      if (!partial && p.tma_store) {
+        // fragments -> (epilogue, convert) -> 128B-swizzled [64 rows x 128 B] staging tile -> one TMA store per 128-byte column
+        // group; the TMA unit clips ragged edges.  A direct store writes 16 bytes per row per instruction, 8 rows apart.
+        const uint32_t stage_smem = epi_base + cw * 8192u;
+        const uint32_t rl = wq * 16u + (lane >> 2);   // row of the first fragment value inside the staging tile
+#pragma unroll
+        for (int mt = 0; mt < MT; ++mt) {
+          const int m_row0 = static_cast<int>(m_cta + mt * 128u + cw * 64u);
+#pragma unroll   // fully: a run-time chunk index would index the accumulators dynamically and move them to local memory
+          for (int c = 0; c < BLOCK_N / CW; ++c) {
+            const uint32_t n0 = tc.n_blk * BLOCK_N + c * CW;
+            if (t == 0) tma_store_wait_read<0>();   // the previous store has finished reading the staging tile
+            asm volatile("bar.sync %0, 128;" ::"r"(2u + cw) : "memory");
+#pragma unroll
+            for (int jj = 0; jj < CW / 8; ++jj) {
+              const int j = c * (CW / 8) + jj;
+              uint32_t v[4];
+              frag(mt, j, v);
+              epilogue(c0 + 8u * j, v);
+              const uint32_t cb = (8u * jj + 2u * (lane & 3u)) * osz;   // byte of the pair inside the 128-byte row
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const uint32_t r = rl + 8u * h;
+                const uint32_t addr = stage_smem + r * 128u + ((((cb >> 4) ^ (r & 7u)) << 4) | (cb & 15u));
+                if constexpr (OUT == OUT_F32) {
+                  asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(addr), "r"(v[2 * h]), "r"(v[2 * h + 1]) : "memory");
+                } else {
+                  uint32_t packed;
+                  if constexpr (OUT == OUT_BF16) asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(packed) : "r"(v[2 * h + 1]), "r"(v[2 * h]));
+                  else asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(packed) : "r"(v[2 * h + 1]), "r"(v[2 * h]));
+                  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(packed) : "memory");
+                }
+              }
+            }
+            fence_proxy_async_smem();   // generic-proxy writes -> visible to the TMA unit
+            asm volatile("bar.sync %0, 128;" ::"r"(2u + cw) : "memory");
+            if (t == 0 && m_row0 < static_cast<int>(p.M) && n0 < p.N) {
+              tma_store_3d(tma_out, stage_smem, static_cast<int>(n0), m_row0, static_cast<int>(tc.b));
+              tma_store_commit();
+            }
+          }
+          // 224-wide tiles with 16-bit outputs: the last 32 columns are half a staging row; a 64-wide box would spill into the
+          // neighbouring tile, so they leave through direct stores
+#pragma unroll
+          for (int j = BLOCK_N / CW * CW / 8; j < NACC / 4; ++j) {
+            uint32_t v[4];
+            frag(mt, j, v);
+            store_group(mt, j, v);
+          }
+        }
+      } else if (!partial) {
+#pragma unroll
+        for (int mt = 0; mt < MT; ++mt) {
+#pragma unroll
+          for (int j = 0; j < NACC / 4; ++j) {
+            uint32_t v[4];
+            frag(mt, j, v);
+            store_group(mt, j, v);
+          }
+        }
+      } else {
+        // part of a stream-K tile's K range: raw f32 accumulators -> this unit's slab, [j][consumer thread] x 16 B (one warp
+        // store covers 512 contiguous bytes); the reduction reads them back in the same fragment order
+        const uint64_t cta_slab_bytes = static_cast<uint64_t>(128) * BLOCK_N * 4;
+        uint4* dst = reinterpret_cast<uint4*>(p.split_ws + (static_cast<uint64_t>(wu.slab) * CG + rank) * cta_slab_bytes) + ct;
+#pragma unroll
+        for (int j = 0; j < NACC / 4; ++j)
+          __stcg(dst + j * 256, make_uint4(acc_bits(acc[0][4 * j]), acc_bits(acc[0][4 * j + 1]), acc_bits(acc[0][4 * j + 2]), acc_bits(acc[0][4 * j + 3])));
+        // publish the slab, take a ticket for (tile, CTA rank); whoever completes the tile's set of parts reduces them in k order
+        const uint32_t tau = wu.tile - p.full_tiles;
+        const uint32_t first = sk_owner(static_cast<uint64_t>(tau) * num_kb, p, num_kb);               // range holding the tile's k-block 0
+        const uint32_t parts = sk_owner(static_cast<uint64_t>(tau + 1) * num_kb - 1, p, num_kb) - first + 1;
+        __threadfence();
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        if (ct == 0) {
+          unsigned int* ticket = reinterpret_cast<unsigned int*>(p.split_tickets) + tau * CG + rank;
+          const unsigned int old = atomicAdd(ticket, 1u);
+          const uint32_t last = (old == parts - 1) ? 1u : 0u;
+          if (last) *ticket = 0;  // every part has arrived: leave the ticket ready for the next launch
+          asm volatile("st.shared.u32 [%0], %1;" ::"r"(split_flag), "r"(last) : "memory");
+        }
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        uint32_t last;
+        asm volatile("ld.shared.u32 %0, [%1];" : "=r"(last) : "r"(split_flag) : "memory");
+        if (last) {
+          __threadfence();
+          // slab of part j of this tile: range first + j; the tile is that range's (tau - first tile of the range)-th unit
+          auto part_slab = [&](uint32_t j) {
+            const uint32_t r = first + j;
+            const uint32_t u = tau - static_cast<uint32_t>(sk_range_lo(r, p, num_kb) / num_kb);
+            return reinterpret_cast<const float4*>(p.split_ws + ((static_cast<uint64_t>(r) * p.sk_umax + u) * CG + rank) * cta_slab_bytes) + ct;
+          };
+          // parts are ADDED in k order (bit-reproducible whoever arrived last), one fragment group at a time: the accumulators
+          // are not written here (writing them on this data-dependent path makes ptxas serialise every wgmma of the kernel)
+#pragma unroll 1
+          for (int j = 0; j < NACC / 4; ++j) {
+            float4 sum = make_float4(0.f, 0.f, 0.f, 0.f);
+            for (uint32_t sl = 0; sl < parts; ++sl) {
+              const float4 x = __ldcg(part_slab(sl) + j * 256);
+              sum.x += x.x; sum.y += x.y; sum.z += x.z; sum.w += x.w;
+            }
+            uint32_t v[4] = {__float_as_uint(sum.x), __float_as_uint(sum.y), __float_as_uint(sum.z), __float_as_uint(sum.w)};
+            store_group(0, j, v);
+          }
+        }
+        asm volatile("bar.sync 1, 256;" ::: "memory");  // the flag word is reused by the next partial unit
+      }
+    }
+    if (t == 0) tma_store_wait<0>();   // outstanding TMA stores read this CTA's shared memory: finish before teardown
+  }
+
+  // a CTA of a pair must not exit while its peer may still multicast into its shared memory or arrive on its barriers
+  if constexpr (CG == 2) cluster_sync_all(); else __syncthreads();
+}
+
+// Dynamic shared memory a variant needs (host mirrors this in capi.cpp: gemm_smem_bytes()).
+//   1024 (alignment slack) + STAGES * (MT * 16384 + BLOCK_N * 128) + 1024 (barriers) + 16384 (TMA-store staging)
+
+#define GEMM_KERNEL_PM(NAME, CG, BN, AMN, BMN, KIND, OUT, STAGES, PROMOTE, MT)                                     \
+  extern "C" __global__ void __launch_bounds__(kNumThreads, 1)                                                     \
+      NAME(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,                  \
+           const __grid_constant__ CUtensorMap tma_a_lo, const __grid_constant__ CUtensorMap tma_b_lo,            \
+           const __grid_constant__ CUtensorMap tma_out, const __grid_constant__ GemmParams p) {                    \
+    gemm_body<CG, BN, AMN, BMN, KIND, OUT, STAGES, PROMOTE, MT>(&tma_a, &tma_b, &tma_a_lo, &tma_b_lo, &tma_out, p); \
+  }
+#define GEMM_KERNEL_P(NAME, CG, BN, AMN, BMN, KIND, OUT, STAGES, PROMOTE) GEMM_KERNEL_PM(NAME, CG, BN, AMN, BMN, KIND, OUT, STAGES, PROMOTE, 1)
+#define GEMM_KERNEL(NAME, CG, BN, AMN, BMN, KIND, OUT, STAGES) GEMM_KERNEL_P(NAME, CG, BN, AMN, BMN, KIND, OUT, STAGES, false)
+
+// name: gemm_<in>_<out>_<cg>sm_n<BLOCK_N>_<a><b>
+//   a: k = lhs stored [M,K] row-major (K-major), m = lhs stored [K,M] (transposed view, M contiguous)
+//   b: n = rhs stored [K,N] row-major (N contiguous), k = rhs stored [N,K] (transposed view, K contiguous)
+// wgmma reads MN-major shared-memory operands for 16-bit kinds only: tf32 and 8-bit kinds have the `kk` layout alone (the
+// host stages other layouts K-major first).
+#define GEMM_LAYOUTS(PFX, CG, BN, KIND, OUT, STAGES)           \
+  GEMM_KERNEL(PFX##_kn, CG, BN, false, true, KIND, OUT, STAGES)  \
+  GEMM_KERNEL(PFX##_kk, CG, BN, false, false, KIND, OUT, STAGES) \
+  GEMM_KERNEL(PFX##_mn, CG, BN, true, true, KIND, OUT, STAGES)   \
+  GEMM_KERNEL(PFX##_mk, CG, BN, true, false, KIND, OUT, STAGES)
+#define GEMM_DTYPES(TILE, CG, BN, STAGES)                                                  \
+  GEMM_LAYOUTS(gemm_bf16_bf16_##TILE, CG, BN, KIND_BF16, OUT_BF16, STAGES)                  \
+  GEMM_LAYOUTS(gemm_bf16_f32_##TILE, CG, BN, KIND_BF16, OUT_F32, STAGES)                    \
+  GEMM_LAYOUTS(gemm_f16_f16_##TILE, CG, BN, KIND_F16, OUT_F16, STAGES)                      \
+  GEMM_LAYOUTS(gemm_f16_f32_##TILE, CG, BN, KIND_F16, OUT_F32, STAGES)                      \
+  GEMM_LAYOUTS(gemm_f16_bf16_##TILE, CG, BN, KIND_F16, OUT_BF16, STAGES)                    \
+  GEMM_KERNEL(gemm_tf32_f32_##TILE##_kk, CG, BN, false, false, KIND_TF32, OUT_F32, STAGES)
+// 8-bit integer inputs: u8 / s8 (s32 accumulate, exact): 128 elements of K per 128-byte row.  fp8 inputs run on the f16
+// kernels after an exact widening pass (capi.cpp: run_gemm_fp8_as_f16): wgmma accumulates fp8 products with less than f32
+// precision.
+#define GEMM_INT8(TILE, CG, BN, STAGES)                                                      \
+  GEMM_KERNEL(gemm_u8_i32_##TILE##_kk, CG, BN, false, false, KIND_U8, OUT_F32, STAGES)        \
+  GEMM_KERNEL(gemm_s8_i32_##TILE##_kk, CG, BN, false, false, KIND_S8, OUT_F32, STAGES)
+// block-scaled kinds: operands expanded to bf16 x * scale (capi.cpp: b200_matmul_scaled), promoted accumulation
+#define GEMM_MX(TILE, CG, BN, STAGES)                                                                     \
+  GEMM_KERNEL_P(gemm_mx_bf16_##TILE##_kk, CG, BN, false, false, KIND_BF16, OUT_BF16, STAGES, true)         \
+  GEMM_KERNEL_P(gemm_mx_f16_##TILE##_kk, CG, BN, false, false, KIND_BF16, OUT_F16, STAGES, true)           \
+  GEMM_KERNEL_P(gemm_mx_f32_##TILE##_kk, CG, BN, false, false, KIND_BF16, OUT_F32, STAGES, true)
+
+// The kernels are built as three cubins from this one source (cubecl_b200/build.py compiles them in parallel):
+//   GEMM_PART 0 ("gemm")    256 x 256 pair tiles (2-CTA cluster, 128 x 256 per CTA) and the bf16 peak probe
+//   GEMM_PART 1 ("gemm_b")  256 x 128 pair tiles, 256 x 224 block-scaled pair tiles
+//   GEMM_PART 2 ("gemm_c")  128 x 128 single-CTA tiles, 512 x 128 pair tiles
+#ifndef GEMM_PART
+#define GEMM_PART 0
+#endif
+
+#if GEMM_PART == 0
+// 128 x 256 per CTA: 48 KB/stage -> 4 stages = 192 KB
+GEMM_DTYPES(2sm_n256, 2, 256, 4)
+GEMM_INT8(2sm_n256, 2, 256, 4)
+GEMM_MX(2sm_n256, 2, 256, 4)
+#endif
+#if GEMM_PART == 1
+// 128 x 128 per CTA: 32 KB/stage -> 6 stages = 192 KB
+GEMM_DTYPES(2sm_n128, 2, 128, 6)
+GEMM_INT8(2sm_n128, 2, 128, 6)
+GEMM_MX(2sm_n128, 2, 128, 6)
+// block-scaled kinds: 224 columns per tile (two promoted partials of 112), 4 x 44 KB stages
+GEMM_MX(2sm_n224, 2, 224, 4)
+#endif
+#if GEMM_PART == 2
+// single CTA, 128 x 128 tiles (small problems; also the bring-up path)
+GEMM_DTYPES(1sm_n128, 1, 128, 6)
+GEMM_INT8(1sm_n128, 1, 128, 6)
+GEMM_MX(1sm_n128, 1, 128, 6)
+// 512 x 128 pair tiles (MT = 2: 256 rows per CTA, two m64 blocks per consumer warpgroup), 16-bit kinds: 4 x 48 KB stages
+#define GEMM_M512(PFX, KIND, OUT)                                                     \
+  GEMM_KERNEL_PM(PFX##_2sm_m512_kn, 2, 128, false, true, KIND, OUT, 4, false, 2)       \
+  GEMM_KERNEL_PM(PFX##_2sm_m512_kk, 2, 128, false, false, KIND, OUT, 4, false, 2)      \
+  GEMM_KERNEL_PM(PFX##_2sm_m512_mn, 2, 128, true, true, KIND, OUT, 4, false, 2)        \
+  GEMM_KERNEL_PM(PFX##_2sm_m512_mk, 2, 128, true, false, KIND, OUT, 4, false, 2)
+GEMM_M512(gemm_bf16_bf16, KIND_BF16, OUT_BF16)
+GEMM_M512(gemm_bf16_f32, KIND_BF16, OUT_F32)
+GEMM_M512(gemm_f16_f16, KIND_F16, OUT_F16)
+GEMM_M512(gemm_f16_f32, KIND_F16, OUT_F32)
+GEMM_M512(gemm_f16_bf16, KIND_F16, OUT_BF16)
+#endif
+
+#if GEMM_PART == 0
+// ---------------------------------------------------------------------------------------------------------------------
+// wgmma peak probe: the accounting of compute_cmma_throughput (crates/cubecl-std/src/throughput/runners/
+// compute_cmma.rs:16,41-42: ops = cubes * planes * 2mnk * n_iter) moved to Hopper's tensor cores -- each of the two
+// consumer warpgroups of every CTA issues n_iter x 4 back-to-back wgmma m64n256k(32 bytes) on operands resident in shared
+// memory (all ones), so it measures the MMA pipe with no TMA / HBM in the loop.  PK 0 = bf16 (K = 16 per instruction),
+// 1 = e4m3 (K = 32).  out[cta] = acc[0] = 64 * n_iter (bf16) or 128 * n_iter (e4m3).
+template <int PK>
+__device__ __forceinline__ void wgmma_probe_body(float* out, uint32_t n_iter) {
+  extern __shared__ uint8_t smem_probe_raw[];
+  const uint32_t smem_base = (smem_u32(smem_probe_raw) + 1023u) & ~1023u;
+  const uint32_t sa = smem_base, sb = smem_base + 16384;   // A: 128 x 128 B, B: 256 x 128 B
+  const uint32_t ones = PK == 0 ? 0x3F803F80u : 0x38383838u;  // bf16 1.0 pairs / e4m3 1.0 bytes
+  for (uint32_t i = threadIdx.x; i < (16384 + 32768) / 4; i += blockDim.x)
+    asm volatile("st.shared.u32 [%0], %1;" ::"r"(smem_base + 4 * i), "r"(ones) : "memory");
+  fence_proxy_async_smem();  // generic-proxy stores -> visible to the tensor core's async-proxy reads
+  __syncthreads();
+  const uint32_t wg = threadIdx.x >> 7;
+  if (wg == 0) return;
+  float acc[128];
+  const uint64_t a_desc = make_smem_desc_sw128(sa + (wg - 1) * 8192u, 16, 1024), b_desc = make_smem_desc_sw128(sb, 16, 1024);
+  for (uint32_t i = 0; i < n_iter; ++i) {
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      if constexpr (PK == 0) wgmma_ss<256, KIND_BF16, KIND_BF16, 0, 0>(acc, a_desc + 2 * k, b_desc + 2 * k, (i | k) != 0 ? 1u : 0u);
+      else wgmma_ss<256, KIND_E4M3, KIND_E4M3, 0, 0>(acc, a_desc + 2 * k, b_desc + 2 * k, (i | k) != 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+  }
+  wgmma_wait<0>();
+  wgmma_fence_operands(acc);
+  if (threadIdx.x == 128) out[blockIdx.x] = acc[0];
+}
+extern "C" __global__ void __launch_bounds__(384, 1) wgmma_probe_bf16(float* out, uint32_t n_iter) { wgmma_probe_body<0>(out, n_iter); }
+extern "C" __global__ void __launch_bounds__(384, 1) wgmma_probe_e4m3(float* out, uint32_t n_iter) { wgmma_probe_body<1>(out, n_iter); }
+#endif  // GEMM_PART == 0

@@ -1,10 +1,10 @@
-// Inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA / TMEM / commit),
+// Inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA from shared memory),
 // cluster primitives.  Everything here is device-only and header-only; compiled into the prebuilt cubins.
 //
 // These replace what the reference would have obtained from NVRTC-compiled generated C++:
 //   mbarrier  -> crates/cubecl-cpp/src/cuda/barrier.rs (reference emits cuda::barrier / mbarrier PTX)
 //   TMA       -> crates/cubecl-cpp/src/cuda/tma.rs:11-45
-//   MMA       -> crates/cubecl-cpp/src/shared/mma.rs:48-174 (wmma) -- here tcgen05, which the reference lacks
+//   MMA       -> crates/cubecl-cpp/src/shared/mma.rs:48-174 (wmma) -- here wgmma, which the reference lacks
 #pragma once
 #include <cstdint>
 #include <cuda.h>
@@ -67,9 +67,11 @@ __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 
-// Arrive on a barrier that lives in another CTA of the cluster (address from mapa_shared).
+// Arrive on a barrier that lives in another CTA of the cluster (address from mapa_shared).  Releases at CTA scope: the
+// arrive only says "this stage's shared memory may be overwritten", and the wgmma wait before it already ordered the reads
+// (a cluster-scope release costs a GPU-wide memory barrier per call).
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_bar) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar) : "memory");
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar) : "memory");
 }
 
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
@@ -139,17 +141,6 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* m, 
       : "memory");
 }
 
-// 3-D tiled load issued by one CTA of a cta_group::2 pair; `cluster_bar` may live in the peer (leader) CTA.
-__device__ __forceinline__ void tma_load_3d_2sm(uint32_t dst, const CUtensorMap* m, uint32_t cluster_bar, int c0, int c1,
-                                                int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5}], [%2];"
-      :
-      : "r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(cluster_bar), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-
 // Multicast 3-D load: the box lands at the same smem offset in every CTA of `mask`, each CTA's own barrier
 // (same offset) receives the complete_tx.
 __device__ __forceinline__ void tma_load_3d_mc(uint32_t dst, const CUtensorMap* m, uint32_t bar, uint16_t mask, int c0,
@@ -197,168 +188,98 @@ __device__ __forceinline__ void bulk_load_1d(uint32_t dst, const void* src, uint
       : "memory");
 }
 
-// ---------------------------------------------------------------------------------------------- tcgen05
-template <int CG>
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-  if constexpr (CG == 1)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols)
-                 : "memory");
-  else
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols)
-                 : "memory");
-}
-
-template <int CG>
-__device__ __forceinline__ void tmem_relinquish() {
-  if constexpr (CG == 1)
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  else
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-
-template <int CG>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  if constexpr (CG == 1)
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-  else
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-__device__ __forceinline__ void tcgen05_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-
-// D[tmem] (+)= A[smem] * B[smem].  KIND: 0/1 = kind::f16 (f16 / bf16 inputs), 2 = kind::tf32, 3/4 = kind::f8f6f4
-// (e4m3 / e5m2 inputs), 5/6 = kind::i8 (u8 / s8 inputs, s32 accumulate).  The operand formats themselves are encoded in
-// the instruction descriptor.
-#define B200_UMMA_ASM(CGS, KINDS)                                                                             \
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"                                            \
-               "tcgen05.mma.cta_group::" CGS ".kind::" KINDS " [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),       \
-               "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)                                          \
-               : "memory")
-template <int CG, int KIND>
-__device__ __forceinline__ void umma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                        uint32_t accumulate) {
-  if constexpr (KIND <= 1) {
-    if constexpr (CG == 1) B200_UMMA_ASM("1", "f16"); else B200_UMMA_ASM("2", "f16");
-  } else if constexpr (KIND == 2) {
-    if constexpr (CG == 1) B200_UMMA_ASM("1", "tf32"); else B200_UMMA_ASM("2", "tf32");
-  } else if constexpr (KIND <= 4) {
-    if constexpr (CG == 1) B200_UMMA_ASM("1", "f8f6f4"); else B200_UMMA_ASM("2", "f8f6f4");
-  } else {
-    if constexpr (CG == 1) B200_UMMA_ASM("1", "i8"); else B200_UMMA_ASM("2", "i8");
-  }
-}
-
-// Block-scaled forms (MX formats): D[tmem] (+)= (A * SFA) * (B * SFB) with one scale per row per 32 K elements, the scale
-// factors read from TMEM.  MXKIND 0 = kind::mxf8f6f4 (K = 32 per instruction, one scale per row: byte `sf_id` of the
-// 32-bit TMEM word, selected in the instruction descriptor), 1 = kind::mxf4 with scale_vec::2X (packed e2m1, K = 64 per
-// instruction, two scales per row: bytes sf_id, sf_id + 1), 2 = kind::mxf4nvf4 with scale_vec::4X (NVFP4: packed e2m1, K = 64,
-// four ue4m3 scales per row -- one per 16 elements -- the whole 32-bit word).
-#define B200_UMMA_SCALED_ASM(CGS, KINDS)                                                                          \
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"                                                \
-               "tcgen05.mma.cta_group::" CGS ".kind::" KINDS " [%0], %1, %2, %3, [%5], [%6], p;\n\t}" ::"r"(d_tmem), \
-               "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate), "r"(sfa_tmem), "r"(sfb_tmem)                \
-               : "memory")
-template <int CG, int MXKIND>
-__device__ __forceinline__ void umma_ss_scaled(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                               uint32_t sfa_tmem, uint32_t sfb_tmem, uint32_t accumulate) {
-  if constexpr (MXKIND == 0) {
-    if constexpr (CG == 1) B200_UMMA_SCALED_ASM("1", "mxf8f6f4.block_scale"); else B200_UMMA_SCALED_ASM("2", "mxf8f6f4.block_scale");
-  } else if constexpr (MXKIND == 1) {
-    if constexpr (CG == 1) B200_UMMA_SCALED_ASM("1", "mxf4.block_scale.scale_vec::2X");
-    else B200_UMMA_SCALED_ASM("2", "mxf4.block_scale.scale_vec::2X");
-  } else {
-    if constexpr (CG == 1) B200_UMMA_SCALED_ASM("1", "mxf4nvf4.block_scale.scale_vec::4X");
-    else B200_UMMA_SCALED_ASM("2", "mxf4nvf4.block_scale.scale_vec::4X");
-  }
-}
-
-// smem -> TMEM copy of one scale-factor chunk: 32 rows x 128 bits, broadcast to the four 32-lane sub-partitions
-// (columns [taddr, taddr + 4)).  Ordered with the tcgen05.mma instructions issued by the same thread.
-template <int CG>
-__device__ __forceinline__ void tmem_cp_32x128b_warpx4(uint32_t taddr, uint64_t smem_desc) {
-  if constexpr (CG == 1)
-    asm volatile("tcgen05.cp.cta_group::1.32x128b.warpx4 [%0], %1;" ::"r"(taddr), "l"(smem_desc) : "memory");
-  else
-    asm volatile("tcgen05.cp.cta_group::2.32x128b.warpx4 [%0], %1;" ::"r"(taddr), "l"(smem_desc) : "memory");
-}
-
-// Instruction descriptor of the block-scaled kinds (f32 accumulate, K-major operands); the scale-factor byte ids (bits
-// 29-30 for A, 4-5 for B) are OR-ed in per instruction.
-//   a_fmt/b_fmt: kind::mxf8f6f4 -> 0 = e4m3, 1 = e5m2; kind::mxf4 / mxf4nvf4 -> 1 = e2m1.  ue8m0: scale format bit (23).
-__host__ __device__ constexpr uint32_t make_idesc_scaled(uint32_t a_fmt, uint32_t b_fmt, uint32_t umma_m, uint32_t umma_n,
-                                                         uint32_t ue8m0 = 1) {
-  return (a_fmt << 7) | (b_fmt << 10) | ((umma_n >> 3) << 17) | (ue8m0 << 23) | ((umma_m >> 4) << 24);
-}
-
-// All previously issued tcgen05.mma of this thread arrive (once) on `bar` when they retire.
-// CG==2: the arrive is multicast to the barrier at the same smem offset in both CTAs of the pair.
-template <int CG>
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  if constexpr (CG == 1)
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-  else
-    asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-        "h"(static_cast<uint16_t>(3))
-        : "memory");
-}
-
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive 32-bit columns (thread t <- lane base+t).
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ---------------------------------------------------------------------------------------------- descriptors
-// Shared-memory matrix descriptor (sm_100 "version 1"), SWIZZLE_128B.  Offsets are byte values, multiples of 16.
+// ---------------------------------------------------------------------------------------------- wgmma
+// Shared-memory matrix descriptor (sm_90), SWIZZLE_128B.  Offsets are byte values, multiples of 16.
 //   bits [0,14)  start address >> 4        bits [16,30) leading-dim byte offset >> 4
-//   bits [32,46) stride-dim byte offset >> 4   bits [46,48) version = 1   bits [61,64) layout type
-//   layout: 2 = SWIZZLE_128B (16-byte swizzle atoms), 1 = SWIZZLE_128B_BASE32B (32-byte atoms; the only layout the
-//   hardware accepts for MN-major 32-bit (tf32) operands -- pairs with CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B)
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout) {
+//   bits [32,46) stride-dim byte offset >> 4   bits [62,64) layout type (1 = SWIZZLE_128B)
+// K-major operand: rows of 128 B along K, 8-row swizzle atoms SBO = 1024 B apart (LBO unused).
+// MN-major operand (16-bit types only): 128-byte rows run along M/N, 8 k-rows per atom (SBO = 1024), the next 64-element
+// M/N chunk LBO bytes further.
+__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(layout) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
-__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  return make_smem_desc(saddr, lbo_bytes, sbo_bytes, 2);
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// The accumulator registers are live across wgmma_commit / wgmma_wait: keep the compiler from moving their uses.
+template <int R>
+__device__ __forceinline__ void wgmma_fence_operands(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+template <int R>
+__device__ __forceinline__ void wgmma_fence_operands(uint32_t (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+r"(d[i])::"memory");
 }
 
-// Instruction descriptor for kind::f16 / kind::tf32, f32 accumulate.
-//   fmt: kind::f16 -> 0 = f16, 1 = bf16; kind::tf32 -> 2; kind::f8f6f4 -> 0 = e4m3, 1 = e5m2; kind::i8 -> 0 = u8, 1 = s8.
-//   *_mn: 0 = K-major operand, 1 = MN-major operand.
-__host__ __device__ constexpr uint32_t make_idesc(uint32_t fmt, uint32_t a_mn, uint32_t b_mn, uint32_t umma_m,
-                                                  uint32_t umma_n, uint32_t c_fmt = 1 /* 1 = f32, 2 = s32 */) {
-  return (c_fmt << 4)         // accumulator format
-         | (fmt << 7)         // A format
-         | (fmt << 10)        // B format
-         | (a_mn << 15)       // A major
-         | (b_mn << 16)       // B major
-         | ((umma_n >> 3) << 17) | ((umma_m >> 4) << 24);
-}
+// Register budget per warpgroup (producer warpgroups give registers to the wgmma warpgroups).
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
-__host__ __device__ constexpr uint32_t make_idesc_ab(uint32_t fmt_a, uint32_t fmt_b, uint32_t a_mn, uint32_t b_mn, uint32_t umma_m,
-                                                     uint32_t umma_n, uint32_t c_fmt) {
-  return (c_fmt << 4) | (fmt_a << 7) | (fmt_b << 10) | (a_mn << 15) | (b_mn << 16) | ((umma_n >> 3) << 17) | ((umma_m >> 4) << 24);
+// Register / operand lists of the m64nNk* accumulator fragments (N / 2 registers per thread).
+#define B200_WG_REGS_112 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55}"
+#define B200_WG_OPS_F112 "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55])
+#define B200_WG_OPS_R112 "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55])
+#define B200_WG_DA_112 "%56"
+#define B200_WG_DB_112 "%57"
+#define B200_WG_SC_112 "%58"
+#define B200_WG_REGS_128 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}"
+#define B200_WG_OPS_F128 "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+#define B200_WG_OPS_R128 "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+#define B200_WG_DA_128 "%64"
+#define B200_WG_DB_128 "%65"
+#define B200_WG_SC_128 "%66"
+#define B200_WG_REGS_256 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}"
+#define B200_WG_OPS_F256 "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+#define B200_WG_OPS_R256 "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63]), "+r"(d[64]), "+r"(d[65]), "+r"(d[66]), "+r"(d[67]), "+r"(d[68]), "+r"(d[69]), "+r"(d[70]), "+r"(d[71]), "+r"(d[72]), "+r"(d[73]), "+r"(d[74]), "+r"(d[75]), "+r"(d[76]), "+r"(d[77]), "+r"(d[78]), "+r"(d[79]), "+r"(d[80]), "+r"(d[81]), "+r"(d[82]), "+r"(d[83]), "+r"(d[84]), "+r"(d[85]), "+r"(d[86]), "+r"(d[87]), "+r"(d[88]), "+r"(d[89]), "+r"(d[90]), "+r"(d[91]), "+r"(d[92]), "+r"(d[93]), "+r"(d[94]), "+r"(d[95]), "+r"(d[96]), "+r"(d[97]), "+r"(d[98]), "+r"(d[99]), "+r"(d[100]), "+r"(d[101]), "+r"(d[102]), "+r"(d[103]), "+r"(d[104]), "+r"(d[105]), "+r"(d[106]), "+r"(d[107]), "+r"(d[108]), "+r"(d[109]), "+r"(d[110]), "+r"(d[111]), "+r"(d[112]), "+r"(d[113]), "+r"(d[114]), "+r"(d[115]), "+r"(d[116]), "+r"(d[117]), "+r"(d[118]), "+r"(d[119]), "+r"(d[120]), "+r"(d[121]), "+r"(d[122]), "+r"(d[123]), "+r"(d[124]), "+r"(d[125]), "+r"(d[126]), "+r"(d[127])
+#define B200_WG_DA_256 "%128"
+#define B200_WG_DB_256 "%129"
+#define B200_WG_SC_256 "%130"
+
+// D (+)= A[smem] * B[smem] for one warpgroup, m64 x N, f32 (F) or s32 (R) accumulators.  scale_d == 0: D = A * B.
+#define B200_WGMMA(N, C, KS, TYPES, TAIL)                                                                              \
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, " B200_WG_SC_##N ", 0;\n\t"                                   \
+               "wgmma.mma_async.sync.aligned.m64n" #N "k" #KS "." TYPES " " B200_WG_REGS_##N ", " B200_WG_DA_##N ", "  \
+               B200_WG_DB_##N ", p" TAIL ";\n\t}"                                                                      \
+               : B200_WG_OPS_##C##N                                                                                    \
+               : "l"(da), "l"(db), "r"(scale_d))
+
+// Operand kinds (the GEMM's KIND values): 0 f16, 1 bf16, 2 tf32, 3 e4m3, 4 e5m2, 5 u8, 6 s8.  TA / TB: 1 = MN-major
+// operand (16-bit kinds only).  8-bit kinds may pair different formats (KA != KB).
+#define B200_WGMMA_16(N, T)                                                       \
+  if constexpr (TA == 0 && TB == 0) B200_WGMMA(N, F, 16, "f32." T "." T, ", 1, 1, 0, 0"); \
+  else if constexpr (TA == 0) B200_WGMMA(N, F, 16, "f32." T "." T, ", 1, 1, 0, 1");        \
+  else if constexpr (TB == 0) B200_WGMMA(N, F, 16, "f32." T "." T, ", 1, 1, 1, 0");        \
+  else B200_WGMMA(N, F, 16, "f32." T "." T, ", 1, 1, 1, 1");
+#define B200_WGMMA_ALL(N)                                                                                     \
+  if constexpr (KA == 0) { B200_WGMMA_16(N, "f16") }                                                          \
+  else if constexpr (KA == 1) { B200_WGMMA_16(N, "bf16") }                                                    \
+  else if constexpr (KA == 2) B200_WGMMA(N, F, 8, "f32.tf32.tf32", ", 1, 1");                                 \
+  else if constexpr (KA == 3 && KB == 3) B200_WGMMA(N, F, 32, "f32.e4m3.e4m3", ", 1, 1");                     \
+  else if constexpr (KA == 3 && KB == 4) B200_WGMMA(N, F, 32, "f32.e4m3.e5m2", ", 1, 1");                     \
+  else if constexpr (KA == 4 && KB == 3) B200_WGMMA(N, F, 32, "f32.e5m2.e4m3", ", 1, 1");                     \
+  else if constexpr (KA == 4 && KB == 4) B200_WGMMA(N, F, 32, "f32.e5m2.e5m2", ", 1, 1");                     \
+  else if constexpr (KA == 5 && KB == 5) B200_WGMMA(N, R, 32, "s32.u8.u8", "");                               \
+  else if constexpr (KA == 5 && KB == 6) B200_WGMMA(N, R, 32, "s32.u8.s8", "");                               \
+  else if constexpr (KA == 6 && KB == 5) B200_WGMMA(N, R, 32, "s32.s8.u8", "");                               \
+  else B200_WGMMA(N, R, 32, "s32.s8.s8", "");
+
+template <int N, int KA, int KB, int TA, int TB, typename Acc>
+__device__ __forceinline__ void wgmma_ss(Acc (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d) {
+  static_assert(N == 112 || N == 128 || N == 256, "m64n112 / m64n128 / m64n256 only");
+  if constexpr (N == 112) { B200_WGMMA_ALL(112) } else if constexpr (N == 128) { B200_WGMMA_ALL(128) } else { B200_WGMMA_ALL(256) }
 }
 
 }  // namespace b200

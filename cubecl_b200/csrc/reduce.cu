@@ -1,4 +1,4 @@
-// Hand-written sm_100a reductions: sum / mean / prod / max / min / argmax / argmin over all elements, over the
+// Hand-written sm_90a reductions: sum / mean / prod / max / min / argmax / argmin over all elements, over the
 // innermost axis ("rows") or over an outer/middle axis ("columns").  HBM-bound: coalesced 128-bit (optionally 256-bit)
 // streaming loads -- or 16 KB bulk copies (cp.async.bulk, UBLKCP) into a shared-memory ring for the `_tma` variants --
 // many independent accumulators per thread, __shfl_down warp stage, smem block stage, and a last-block-done grid stage
@@ -18,7 +18,7 @@
 // Arg-reductions: ties -> lowest index; NaN compares as the extreme value (first NaN wins), i.e. numpy semantics.  They run
 // on a monotone integer key of the value packed with the complemented index, (key << 32) | ~index, so "better" is a plain
 // unsigned 64-bit max -- associative and commutative, hence independent of the reduction tree.
-// Compiled to a cubin: nvcc -cubin -gencode arch=compute_100a,code=sm_100a
+// Compiled to a cubin: nvcc -cubin -gencode arch=compute_90a,code=sm_90a
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cstdint>
@@ -138,9 +138,11 @@ struct ArgAcc {
 struct float8 {
   float4 lo, hi;
 };
+// sm_90 has no 256-bit loads: two adjacent 128-bit streaming loads
 __device__ __forceinline__ float8 ldg_stream_v8(const float* p) {
   float8 v;
-  asm volatile("ld.global.nc.L1::no_allocate.L2::evict_first.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+  asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0,%1,%2,%3}, [%8];\n\t"
+               "ld.global.nc.L1::no_allocate.v4.f32 {%4,%5,%6,%7}, [%8+16];"
                : "=f"(v.lo.x), "=f"(v.lo.y), "=f"(v.lo.z), "=f"(v.lo.w), "=f"(v.hi.x), "=f"(v.hi.y), "=f"(v.hi.z),
                  "=f"(v.hi.w)
                : "l"(p));

@@ -3,7 +3,7 @@ crates/cubecl-zspace/src/shape.rs:489-517, std-lib op convention `op::launch(cli
 crates/cubecl-std/src/tensor/identity.rs:39-83).
 
 out[..., m, n] = sum_k lhs[..., m, k] * rhs[..., k, n], f32 accumulation, batch dims broadcast.
-The kernel behind it is the hand-written tcgen05/TMA GEMM in csrc/gemm_tcgen05.cu.
+The kernel behind it is the hand-written wgmma/TMA GEMM in csrc/gemm_wgmma.cu.
 """
 from __future__ import annotations
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""examples/sum_things (reference: examples/sum_things/src/lib.rs:178-227) on the B200-native path.
+"""examples/sum_things (reference: examples/sum_things/src/lib.rs:178-227) on the H100-native path.
 
 The reference launches 4 kernel kinds over input [-1, 10, 1, 5] with one unit per element, every unit computing the full
 sum (15) -- or sum * input[unit] for the series kind -- and prints the output buffer after each.  Here the sum is the

@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""examples/throughput (reference: examples/throughput/src/lib.rs, README.md:28-34) on the B200-native path.
+"""examples/throughput (reference: examples/throughput/src/lib.rs, README.md:28-34) on the H100-native path.
 
 Prints the reference's table -- using its own sampling protocol (ThroughputBenchmarker: warm up to a plateau, min of N
 samples, host clock around launch+sync) -- for (a) the kernels CubeCL itself would JIT on this GPU (wmma probe, float_4
-read probe: "reference-equivalent") and (b) the hand-written sm_100a kernels that replace them.
+read probe: "reference-equivalent") and (b) the hand-written sm_90a kernels that replace them.
 """
 import sys
 from pathlib import Path
@@ -35,14 +35,14 @@ def run(device: int = 0, clock: str = "host") -> None:
         ops[0] = c.probe_umma(4096, scratch)
 
     v = bench.measure(device_sampler(c, umma, clock), 1)
-    rows.append(("compute-umma", "bf16→f32 256×256×16 (tcgen05, 2-CTA)", fmt(ops[0] / v.duration_s / 1e12, "TOPS/s")))
+    rows.append(("compute-wgmma", "bf16→f32 64×256×16 per warpgroup (wgmma)", fmt(ops[0] / v.duration_s / 1e12, "TOPS/s")))
 
     n = 8192
     a, b, o = (TensorHandle.empty_contiguous(c, [n, n], "bf16") for _ in range(3))
     c.fill_uniform(a.handle, "bf16", n * n, 3, -1, 1)
     c.fill_uniform(b.handle, "bf16", n * n, 4, -1, 1)
     v = bench.measure(device_sampler(c, lambda: matmul.launch(c, a, b, o), clock), int(2 * n ** 3))
-    rows.append(("matmul", "bf16 8192×8192×8192 (tcgen05 + TMA)", fmt(v.ops_per_s() / 1e12, "TOPS/s")))
+    rows.append(("matmul", "bf16 8192×8192×8192 (wgmma + TMA)", fmt(v.ops_per_s() / 1e12, "TOPS/s")))
     del a, b, o
 
     nbytes = 512 << 20   # the reference's buffer size (throughput/base.rs:9)

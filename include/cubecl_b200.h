@@ -1,4 +1,4 @@
-/* cubecl_b200.h -- C ABI of the B200-native dense linear-algebra hot path (tcgen05 matmul + HBM-bound reduction).
+/* cubecl_b200.h -- C ABI of the H100-native dense linear-algebra hot path (wgmma matmul + HBM-bound reduction).
  *
  * This is the drop-in boundary a CubeCL maintainer binds from Rust (see INTEGRATION.md for the `extern "C"` block and the
  * `CudaServer` hook).  Plain pointers and sizes only; no torch / C++ types.  All device pointers are CUdeviceptr values
@@ -14,7 +14,7 @@
  * from b200_last_error() on the calling thread.  Asynchronous device faults surface at the next b200_sync()/b200_read(),
  * like ServerError::ServerUnhealthy does at sync/read (crates/cubecl-cuda/src/compute/server.rs:981-1022).
  *
- * There is no CPU fallback anywhere behind this header: without a CUDA driver and an sm_100 device b200_init() fails.
+ * There is no CPU fallback anywhere behind this header: without a CUDA driver and an sm_90 device b200_init() fails.
  */
 #ifndef CUBECL_B200_H
 #define CUBECL_B200_H
@@ -43,7 +43,7 @@ typedef enum b200_status {
   B200_ERR_IO = 5,                 /* LaunchError::IoError / IoError::* */
   B200_ERR_INVALID_ARG = 6,        /* shape/stride/dtype validation failed before launch */
   B200_ERR_UNSUPPORTED = 7,        /* feature absent (dtype/layout not implemented) -- callers self-skip like runtime_tests do */
-  B200_ERR_NO_DEVICE = 8,          /* no driver / no sm_100 device: fail loudly, never fall back */
+  B200_ERR_NO_DEVICE = 8,          /* no driver / no sm_90 device: fail loudly, never fall back */
   B200_ERR_COMM = 9,               /* NCCL failure -> ServerError::Generic (server.rs:773-776) */
   B200_ERR_UNHEALTHY = 10          /* deferred device fault surfaced at sync -> ServerError::ServerUnhealthy */
 } b200_status;
@@ -82,10 +82,10 @@ typedef struct b200_props {
 /* ---- lifecycle: R::client(device) -> DeviceService::init (cubecl-cuda/src/runtime.rs:52-350) ------------------------ */
 int b200_abi_version(void);
 int b200_device_count(int* count);
-/* The embedded prebuilt sm_100a images ("gemm" | "gemm_b" | "gemm_c" | "gemm_mx" | "reduce" | "aux"), for a host that prefers to cuModuleLoadData them into
+/* The embedded prebuilt sm_90a images ("gemm" | "gemm_b" | "gemm_c" | "reduce" | "aux"), for a host that prefers to cuModuleLoadData them into
  * its own module cache (CudaContext::modules, crates/cubecl-cuda/src/compute/context.rs:38-62,293). No GPU needed. */
 int b200_get_cubin(const char* name, const void** image, size_t* size);
-int b200_init(int device, b200_ctx** out);   /* cuInit, primary ctx retain, load the embedded sm_100a cubins (context.rs:293) */
+int b200_init(int device, b200_ctx** out);   /* cuInit, primary ctx retain, load the embedded sm_90a cubins (context.rs:293) */
 int b200_destroy(b200_ctx* ctx);
 int b200_get_props(b200_ctx* ctx, b200_props* out);
 /* Dry-run planning context (DryRun, crates/cubecl-runtime/src/dry_run.rs:45,88,121): needs no driver and no device.  Ops
@@ -95,14 +95,15 @@ int b200_get_props(b200_ctx* ctx, b200_props* out);
 int b200_plan_begin(int num_sms, b200_ctx** out);
 int b200_plan_text(b200_ctx* ctx, char* buf, size_t capacity, size_t* needed);
 /* Runtime knobs, string-typed like cubecl.toml keys (config/base.rs:18-120).  Keys: "gemm.variant"
- * (auto|2sm_m512|2sm_n256|2sm_n128|1sm_n128|simt; 2sm_n256a1 = single-accumulator diagnostic), "gemm.f32" (hybrid|3xtf32|tf32: f32 inputs as one
- * tf32 pass + two bf16 cross-term passes in ONE launch (default, ~2^-20 of the product), three tf32 passes, or one), "gemm.sf_copy" (thread|thread2|mma:
- * block-scaled kinds, who issues the scale-factor copies to TMEM -- the dedicated copy thread, two of them, or the MMA thread for an A/B), "gemm.group_m",
+ * (auto|2sm_n256|2sm_n128|1sm_n128|simt; opt-in: 2sm_m512 = 512 x 128 pair tile for 16-bit kinds, 2sm_n224 = 256 x 224 pair tile
+ * for block-scaled kinds), "gemm.f32" (hybrid|3xtf32|tf32: f32 inputs as one
+ * tf32 pass + two bf16 cross-term passes in ONE launch (default, ~2^-20 of the product), three tf32 passes, or one), "gemm.group_m",
  * "gemm.l2_promotion" (256|128|64|0: TMA L2 promotion bytes of the operand tensor maps), "gemm.split_k" (auto|off|on|1..8:
  * deterministic stream-K head -- the tiles of a partial last wave are cut along K into equal ranges that run FIRST, slabs
- * added in k order; N = ranges per tile), "gemm.epilogue" (tma|direct), "gemm.stage" (on|off: operands TMA cannot describe --
+ * added in k order; N = ranges per tile), "gemm.epilogue" (tma|direct: whole tiles leave through shared-memory staging and
+ * TMA stores, or each thread stores its own fragment), "gemm.stage" (on|off: operands TMA cannot describe --
  * unaligned row pitch / base -- are first copied into an aligned pooled buffer and run on the tensor cores; off = strided SIMT kernel), "reduce.variant"
- * (auto|u2|u4|u8|u16|b4|b8|w2|w4: load-unroll / blocked / 256-bit forms of the all-elements kernel; tma: 16 KB bulk copies
+ * (auto|u2|u4|u8|u16|b4|b8|w2|w4: load-unroll / blocked / 2 x 128-bit forms of the all-elements kernel; tma: 16 KB bulk copies
  * into a shared-memory ring), "reduce.threads", "reduce.blocks_per_sm" (all-elements kernel), "reduce.rows_vpt" (128-bit
  * vectors per thread that size the threads-per-row of the row kernel), "reduce.rows_blocks_per_sm" /
  * "reduce.cols_blocks_per_sm" (below this many blocks per SM a long reduced axis is cut into segments: two passes),
@@ -161,8 +162,8 @@ int b200_matmul(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b200_dtype ou
                 const uint64_t* shape_out, const uint64_t* strides_out);
 /* The same product with DIFFERENT 8-bit formats for the two operands -- the pairs the reference instantiates for its manual
  * MMA: i8 x u8 / u8 x i8 -> i32 (crates/cubecl-cpp/src/cuda/mma/manual.rs:151-166) and fp8 e4m3 x e5m2 / e5m2 x e4m3
- * (:170-186).  Same tcgen05 kernels (kind::i8 / kind::f8f6f4 take one format field per operand in the instruction
- * descriptor); equal formats behave exactly like b200_matmul.  Other combinations: B200_ERR_UNSUPPORTED. */
+ * (:170-186).  Same wgmma kernels (the instruction names the type of each operand); equal formats behave exactly like
+ * b200_matmul.  Other combinations: B200_ERR_UNSUPPORTED. */
 int b200_matmul_mixed(b200_ctx* ctx, b200_stream s, b200_dtype lhs_dtype, b200_dtype rhs_dtype, b200_dtype out_dtype,
                       b200_dptr lhs, b200_dptr rhs, b200_dptr out, int rank,
                       const uint64_t* shape_lhs, const uint64_t* strides_lhs,
@@ -170,7 +171,7 @@ int b200_matmul_mixed(b200_ctx* ctx, b200_stream s, b200_dtype lhs_dtype, b200_d
                       const uint64_t* shape_out, const uint64_t* strides_out);
 
 /* Fused epilogue (SURVEY 8f-4): out = act(alpha * (lhs @ rhs) + bias[n]) applied to the f32 accumulators inside the GEMM
- * epilogue (TMEM -> registers -> here -> store), no extra pass over the output.  bias: f32[N] device pointer or 0.
+ * epilogue (accumulator registers -> here -> staging / store), no extra pass over the output.  bias: f32[N] device pointer or 0.
  * activation: 0 none, 1 relu, 2 gelu (erf form).  Float inputs only. */
 typedef struct b200_epilogue {
   float alpha;
@@ -186,14 +187,15 @@ int b200_matmul_fused(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b200_dt
 /* Block-scaled (MX) matmul: out[b,m,n] = sum_k (lhs[b,m,k] * lhs_scales[b,m,k/32]) * (rhs[b,n,k] * rhs_scales[b,n,k/32]),
  * f32 accumulation.  Replaces MmaDefinition::new_scaled / execute_scaled (crates/cubecl-core/src/frontend/cmma.rs:438-460,
  * 798-840), the ScaledMmaConfig feature rows (crates/cubecl-ir/src/features.rs:190-211; on CUDA the reference offers them
- * for sm_120 only, cubecl-cpp/src/cuda/mma/manual.rs:201-255 -- sm_100 needs tcgen05 kind::mxf8f6f4 / kind::mxf4) and is
+ * for sm_120 only, cubecl-cpp/src/cuda/mma/manual.rs:201-255 -- sm_90 tensor cores take no scales: each operand is expanded
+ * once to bf16 x * scale, exactly, and multiplied by the bf16 wgmma GEMM) and is
  * pinned by test_cmma_scaled / test_cmma_scaled_fp4 (crates/cubecl-core/src/runtime_tests/cmma.rs:1476-1700).
  * Layouts follow those tests: lhs [batch, m, k] and rhs [batch, n, k] K-contiguous ("col-major" rhs), dtypes B200_F8E4M3 /
  * B200_F8E5M2 (mixable) or both B200_F4E2M1X2 (k / 2 bytes per row); scales are B200_UE8M0 bytes [batch, rows, k / 32]
- * row-major (scales_packed = 0) or already in the tensor core's packed form [batch * ceil(rows/128)][ceil(k/128)][512 B],
+ * row-major (scales_packed = 0) or in the packed form of pack_scales [batch * ceil(rows/128)][ceil(k/128)][512 B],
  * byte (r % 32) * 16 + (r / 32) * 4 + s (scales_packed = 1).  out [batch, m, n] contiguous, f32 / bf16 / f16.
  * scale_block = 32: ue8m0 scales (MXFP8 / MXFP4).  scale_block = 16: NVFP4 -- packed e2m1 operands with e4m3 scale bytes
- * [batch, rows, k / 16] whose sign is ignored (the third ScaledMmaConfig row of manual.rs:241-250; kind::mxf4nvf4).
+ * [batch, rows, k / 16] whose sign is ignored (the third ScaledMmaConfig row of manual.rs:241-250).
  * k must be a multiple of 32.  Operands that TMA cannot describe take the reference-order SIMT path. */
 int b200_matmul_scaled(b200_ctx* ctx, b200_stream stream, b200_dtype lhs_dtype, b200_dtype rhs_dtype, b200_dtype out_dtype,
                        b200_dptr lhs, b200_dptr rhs, b200_dptr lhs_scales, b200_dptr rhs_scales, b200_dptr out,
@@ -267,13 +269,13 @@ int b200_fill_modulo(b200_ctx* ctx, b200_stream s, b200_dtype dtype, b200_dptr o
 /* compute_cmma_throughput as CubeCL would JIT it today (wmma 16x16x16): launches grid = SMs*32, block = 256, `n_iter`
  * dependent mma_sync per plane; *ops = cubes * planes * 2*m*n*k * n_iter (compute_cmma.rs:16,41-42). dtype F16 or BF16. */
 int b200_probe_wmma(b200_ctx* ctx, b200_stream s, b200_dtype dtype, uint32_t n_iter, b200_dptr scratch_1k, double* ops);
-/* The same accounting on the 5th-gen tensor cores: every CTA pair issues n_iter x 4 dependent UMMA 256x256x16 (bf16->f32,
- * TMEM accumulator) on smem-resident operands; *ops = pairs * n_iter * 4 * 2*256*256*16.  scratch: >= 4 * num_sms/2 bytes;
- * scratch[pair] = 64 * n_iter afterwards. */
+/* The same accounting on the Hopper tensor cores: one CTA per SM, whose two warpgroups each issue n_iter x 4 dependent wgmma
+ * m64n256k16 (bf16->f32, register accumulators) on smem-resident operands; *ops = SMs * 2 * n_iter * 4 * 2*64*256*16.
+ * scratch: >= 4 * num_sms bytes; scratch[cta] = 64 * n_iter afterwards. */
 int b200_probe_umma(b200_ctx* ctx, b200_stream s, uint32_t n_iter, b200_dptr scratch, double* ops);
-/* The same probe for the other operand kinds: dtype B200_BF16 (as above), B200_F8E4M3 (kind::f8f6f4, or kind::mxf8f6f4
- * block-scaled when block_scaled != 0) or B200_F4E2M1X2 (kind::mxf4, block_scaled only).  UMMA 256x256xK with K = 16 / 32 /
- * 64 elements; *ops = pairs * n_iter * 4 * 2*256*256*K; scratch[pair] = 4 * K * n_iter afterwards. */
+/* The same probe for the other operand kinds: dtype B200_BF16 (as above) or B200_F8E4M3 (wgmma m64n256k32); block_scaled != 0
+ * is B200_ERR_UNSUPPORTED (sm_90 has no block-scaled MMA).  *ops = SMs * 2 * n_iter * 4 * 2*64*256*K with K = 16 / 32;
+ * scratch[cta] = 4 * K * n_iter afterwards. */
 int b200_probe_umma_kind(b200_ctx* ctx, b200_stream s, b200_dtype dtype, int block_scaled, uint32_t n_iter, b200_dptr scratch,
                          double* ops);
 /* memory_read_throughput with float_4 lines over `bytes` of `buf` (memory_read.rs:68-154): grid = SMs*32, block = 256. */

@@ -400,7 +400,7 @@ impl Drop for Context {
     }
 }
 
-/// The embedded prebuilt sm_100a image `name` ("gemm" | "gemm_mx" | "reduce" | "aux") for a host that prefers to
+/// The embedded prebuilt sm_90a image `name` ("gemm" | "gemm_b" | "gemm_c" | "reduce" | "aux") for a host that prefers to
 /// `cuModuleLoadData` it into its own module cache (CudaContext::modules, cubecl-cuda/src/compute/context.rs:38-62,293).
 pub fn cubin(name: &str) -> Result<&'static [u8], Error> {
     let n = CString::new(name).map_err(|_| Error { status: Status::InvalidArg as i32, message: "NUL in name".into() })?;

@@ -1,7 +1,7 @@
 """Extract the golden vectors the reference's own tests hold for the dense-LA path into reference_golden.json.
 
-Run in the authoring container only (reads /root/reference, which does not exist on the GPU box):
-    python tests/golden/make_golden.py
+Needs a checkout of the reference (tracel-ai/cubecl @ 4057f39e); the stored JSON is what the tests read:
+    python tests/golden/make_golden.py <path to the cubecl checkout>
 The reference cannot be executed here (Rust, no toolchain), so the goldens are the LITERAL expected arrays and input
 generators written in its test sources; this script parses them so nothing is transcribed by hand.
 """
@@ -9,9 +9,10 @@ from __future__ import annotations
 
 import json
 import re
+import sys
 from pathlib import Path
 
-REF = Path("/root/reference")
+REF = Path(sys.argv[1]) if len(sys.argv) > 1 else None
 OUT = Path(__file__).resolve().parent / "reference_golden.json"
 NUM = r"-?\d+(?:\.\d*)?"
 
@@ -83,4 +84,6 @@ def main() -> None:
 
 
 if __name__ == "__main__":
+    if REF is None:
+        raise SystemExit("usage: make_golden.py <path to the cubecl checkout>")
     main()

@@ -1,4 +1,4 @@
-"""CPU: numerics model of the f32 matmul schedules (csrc/gemm_tcgen05.cu, run_gemm in capi.cpp) -- what each split leaves out, in
+"""CPU: numerics model of the f32 matmul schedules (csrc/gemm_wgmma.cu, run_gemm in capi.cpp) -- what each split leaves out, in
 exact arithmetic (numpy f64 sums of the exactly representable partial products), so the accuracy claims in DESIGN.md are pinned:
 
   tf32     : hi(a) . hi(b)                                        hi = the top 19 bits of the f32 (what the tf32 datapath reads)

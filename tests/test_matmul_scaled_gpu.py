@@ -1,4 +1,4 @@
-"""GPU parity: block-scaled (MX) matmul through the C ABI -- tcgen05 kind::mxf8f6f4 / kind::mxf4 with ue8m0 scales in TMEM --
+"""GPU parity: block-scaled (MX) matmul through the C ABI -- operands expanded exactly to bf16 x * scale, then the bf16 wgmma GEMM --
 against the oracle's restatement of the reference's expected loops (test_cmma_scaled / test_cmma_scaled_fp4,
 crates/cubecl-core/src/runtime_tests/cmma.rs:1476-1700)."""
 import numpy as np
@@ -17,7 +17,6 @@ def _reset_options(client):
     yield
     client.set_option("gemm.variant", "auto")
     client.set_option("gemm.split_k", "auto")
-    client.set_option("gemm.sf_copy", "thread")
 
 
 def quantise(vals, dtype):
@@ -143,21 +142,6 @@ def test_prepacked_scales_and_batches(client, dtype):
         check(plain[i], a[i], b[i], sa[i], sb[i], 2e-6)
 
 
-@pytest.mark.parametrize("dtype,K", [("f8e4m3", 1024), ("f4e2m1x2", 2048)])
-def test_scale_copy_schemes_agree_bit_for_bit(client, dtype, K):
-    # who copies the scale atoms to TMEM (the dedicated copy thread, or two of them) changes the schedule, never the arithmetic:
-    # identical bits, and parity with the oracle, on a multi-tile problem with ragged edges.  (gemm.sf_copy=mma, the round-2 scheme,
-    # is kept as a TIMING reference for tools/perf_sweep.py scaledab only.)
-    M, N = 300, 520
-    a_dev, a, b_dev, b, sa, sb = random_problem(M, N, K, dtype, dtype, seed=31)
-    outs = {}
-    for scheme in ("thread", "thread2"):
-        client.set_option("gemm.sf_copy", scheme)
-        outs[scheme] = run_scaled(client, a_dev, b_dev, sa, sb, dtype, dtype, "f32")
-    check(outs["thread"], a, b, sa, sb, 2e-6)
-    assert np.array_equal(outs["thread"], outs["thread2"])
-
-
 # ------------------------------------------------------------------------------------------------ NVFP4 (ue4m3 scale per 16)
 def nvfp4_problem(M, N, K, seed, batch=()):
     """packed e2m1 operands + e4m3 scale bytes per 16 elements; some scale bytes carry a sign bit, which the hardware ignores
@@ -180,8 +164,7 @@ def check_nvfp4(got, a, b, sa, sb, tol):
     return o32
 
 
-# (no 256 x 224 NVFP4 tile: its two accumulator stages leave TMEM room for ONE 48-column scale buffer, the copy thread needs two)
-@pytest.mark.parametrize("variant", ["simt"] + [v for v in TC_VARIANTS if v != "2sm_n224"])
+@pytest.mark.parametrize("variant", ["simt"] + TC_VARIANTS)
 @pytest.mark.parametrize("out_dtype,tol", [("f32", 2e-6), ("bf16", 1e-2)])
 @pytest.mark.parametrize("M,N,K", [(16, 8, 64), (300, 520, 1024), (128, 256, 96), (257, 129, 2048)])
 def test_parity_nvfp4(client, variant, out_dtype, tol, M, N, K):

@@ -11,7 +11,7 @@ pytestmark = pytest.mark.gpu
 
 def test_props_and_pool(client):
     p = client.properties
-    assert p["cc"][0] == 10 and p["num_streaming_multiprocessors"] >= 100 and p["plane_size_min"] == 32
+    assert p["cc"] == (9, 0) and p["num_streaming_multiprocessors"] >= 100 and p["plane_size_min"] == 32
     before = client.memory_usage()
     h = client.empty(1 << 20)
     mid = client.memory_usage()
@@ -42,7 +42,7 @@ def test_error_paths_are_loud(client):
     bad = C.c_void_p()
     assert client._lib.b200_init(99, C.byref(bad)) == 8                            # no such device
     with pytest.raises(B200Error):
-        client.set_option("gemm.variant", "2sm_n128")
+        client.set_option("gemm.variant", "2sm_n512")
         try:
             a = TensorHandle.empty_contiguous(client, [64, 128], "f8e4m3")
             b = TensorHandle.empty_contiguous(client, [128, 64], "f8e4m3")
@@ -50,7 +50,7 @@ def test_error_paths_are_loud(client):
             _ffi.check(client._lib.b200_matmul(client._ctx, None, 10, 0, C.c_uint64(a.handle.ptr), C.c_uint64(b.handle.ptr),
                                                C.c_uint64(o.handle.ptr), 2, _ffi.u64_array([64, 128]), _ffi.u64_array([128, 1]),
                                                _ffi.u64_array([128, 64]), _ffi.u64_array([64, 1]), _ffi.u64_array([64, 64]),
-                                               _ffi.u64_array([64, 1])))       # no fp8 2sm_n128 variant exists
+                                               _ffi.u64_array([64, 1])))       # no 2sm_n512 variant exists
         finally:
             client.set_option("gemm.variant", "auto")
 
@@ -141,18 +141,21 @@ def test_reference_probes_run(client):
     client.sync()
     assert ops == client.properties["num_streaming_multiprocessors"] * 32 * 8 * 2 * 16 ** 3 * 4
     assert np.all(np.frombuffer(client.read_one(scratch), dtype=np.float16)[:256] == 64.0)
-    # the same accounting on tcgen05: 4 UMMAs of K=16 per iteration on all-ones operands -> acc = 64 * n_iter
+    # the same accounting on wgmma: per CTA two warpgroups x 4 m64n256k16 per iteration on all-ones operands -> acc = 64 * n_iter
+    from cubecl_b200 import B200Error
     ops = client.probe_umma(16, scratch)
     client.sync()
-    pairs = client.properties["num_streaming_multiprocessors"] // 2
-    assert ops == pairs * 16 * 4 * 2 * 256 * 256 * 16
-    assert np.all(np.frombuffer(client.read_one(scratch), dtype=np.float32)[:pairs] == 1024.0)
-    # fp8, block-scaled fp8 and block-scaled fp4 peaks: K = 32 / 32 / 64 per UMMA, scales = 1.0 -> acc = 4 * K * n_iter
-    for dtype, scaled, kk in (("f8e4m3", False, 32), ("f8e4m3", True, 32), ("f4e2m1x2", True, 64)):
-        ops = client.probe_umma_kind(dtype, scaled, 16, scratch)
-        client.sync()
-        assert ops == pairs * 16 * 4 * 2 * 256 * 256 * kk
-        assert np.all(np.frombuffer(client.read_one(scratch), dtype=np.float32)[:pairs] == 4.0 * kk * 16)
+    ctas = client.properties["num_streaming_multiprocessors"]
+    assert ops == ctas * 2 * 16 * 4 * 2 * 64 * 256 * 16
+    assert np.all(np.frombuffer(client.read_one(scratch), dtype=np.float32)[:ctas] == 1024.0)
+    # fp8 peak: K = 32 per wgmma -> acc = 4 * K * n_iter; sm_90 has no block-scaled MMA to probe
+    ops = client.probe_umma_kind("f8e4m3", False, 16, scratch)
+    client.sync()
+    assert ops == ctas * 2 * 16 * 4 * 2 * 64 * 256 * 32
+    assert np.all(np.frombuffer(client.read_one(scratch), dtype=np.float32)[:ctas] == 4.0 * 32 * 16)
+    for dtype in ("f8e4m3", "f4e2m1x2"):
+        with pytest.raises(B200Error):
+            client.probe_umma_kind(dtype, True, 16, scratch)
     buf = client.empty(1 << 24)
     client.fill_modulo(buf, "f32", 1 << 22, 2)
     client.probe_memread(buf, 1 << 24, scratch)

@@ -1,5 +1,5 @@
 """CPU model of the GEMM's stream-K head (deterministic split-K of what would be a partial last wave): a Python transcription
-of `next_unit`, `sk_range_lo`, `sk_owner` and of the slab / ticket exchange in cubecl_b200/csrc/gemm_tcgen05.cu, checked for
+of `next_unit`, `sk_range_lo`, `sk_owner` and of the slab / ticket exchange in cubecl_b200/csrc/gemm_wgmma.cu, checked for
 the invariants the kernel relies on -- every (tile, k-block) is computed exactly once, every unit is non-empty, the number of
 partial units of a tile equals the `parts` the ticket waits for, the slab a finishing CTA reads for part j is the slab the unit
 that computed part j wrote, and the reduced tile does not depend on which part arrives last."""

@@ -1,4 +1,4 @@
-"""Same-box, same-protocol comparison of the tcgen05 GEMM with cuBLAS (torch.matmul) on bf16 8192^3.
+"""Same-box, same-protocol comparison of the wgmma GEMM with cuBLAS (torch.matmul) on bf16 8192^3.
 
 MEASURED_PEAKS.json's bf16 figure is cuBLAS "best of 10" single launches (burst) and a 4 s back-to-back run (sustained);
 bench.py reports the MEAN of K back-to-back launches.  This tool times BOTH kernels BOTH ways on identical U[-1,1) data so
