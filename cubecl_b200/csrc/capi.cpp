@@ -259,6 +259,15 @@ struct ArgCombineParams {
   uint64_t keys, idx, out;
   uint64_t outer, nseg, inner;
 };
+struct ScanParams {
+  uint64_t in, out, carry;       // carry: f32 [outer, nseg, inner] start value of every segment (0: the identity)
+  uint64_t outer, len, inner;
+  uint64_t s_outer, s_len;
+  uint64_t row_len, row_pitch;
+  uint64_t seg_len;
+  uint32_t nseg;
+  uint32_t flags;                // 1: exclusive, 2: column kernel uses vector units
+};
 struct FillParams {
   uint64_t out, n, seed;
   float lo, scale;
@@ -404,7 +413,7 @@ static int get_func(b200_ctx* c, const std::string& name, CUfunction* out) {
   const size_t home = tc_gemm && (has("_2sm_n128_") || has("_2sm_n224_")) ? 3
                       : tc_gemm && (has("_1sm_n128_") || has("_2sm_m512_")) ? 4
                       : tc_gemm || starts("wgmma_probe_") ? 0
-                      : starts("reduce_") ? 1 : 2;
+                      : starts("reduce_") || starts("scan_") ? 1 : 2;
   if (home < c->modules.size()) {
     CUfunction f;
     if (g_drv.cuModuleGetFunction_p(&f, c->modules[home], name.c_str()) == CUDA_SUCCESS) {
@@ -2040,6 +2049,175 @@ extern "C" int b200_reduce_strided(b200_ctx* c, b200_stream s, b200_reduce_op op
                                    int rank, const uint64_t* shape, const uint64_t* strides, int axis) {
   CTX_ENTER(c);
   return reduce_impl(c, s, op, in_dtype, in, out, rank, shape, strides, axis);
+}
+
+// ================================================================================================ scan
+// Scan tile geometry (csrc/reduce.cu): a row-kernel thread owns kScanElems consecutive elements per tile; a column-kernel
+// block owns up to kScanColUnits column units.
+static constexpr uint64_t kScanElems = 16;
+static constexpr uint64_t kScanColUnits = 256;
+
+static std::string scan_name(const char* family, int op, int dt, int odt) {
+  std::string n = std::string(family) + op_tag(op) + "_" + dt_tag(dt);
+  if (odt != B200_F32) n += std::string("_") + dt_tag(odt);
+  return n;
+}
+
+// Column units of the view: 128-bit vectors of consecutive inner elements when the layout allows it, else elements.
+static bool scan_cols_vector(const RView& v, size_t esz) {
+  const uint64_t vec = 16 / esz;
+  return v.inner % vec == 0 && v.row_len % vec == 0 && v.in % 16 == 0 && (v.s_len * esz) % 16 == 0 && (v.s_outer * esz) % 16 == 0 &&
+         (v.row_pitch * esz) % 16 == 0;
+}
+static uint64_t scan_cols_ctu(uint64_t units) { return std::min<uint64_t>(kScanColUnits, std::max<uint64_t>(32, pow2_ceil(units))); }
+
+// One launch of scan_rows over items (row, segment): TPR threads per item sized so every thread walks about four tiles.
+static int launch_scan_rows(b200_ctx* c, CUstream st, int op, int dt, int odt, const RView& v, uint64_t seg_len, uint64_t out,
+                            uint64_t carry, bool exclusive, bool pdl) {
+  CUfunction f;
+  int rc = get_func(c, scan_name("scan_rows_", op, dt, odt), &f);
+  if (rc) return rc;
+  const uint64_t nseg = ceil_div(v.len, seg_len), items = v.outer * nseg;
+  const uint64_t chunks = ceil_div(std::min(seg_len, v.len), kScanElems);
+  const uint64_t tpr = std::min<uint64_t>(512, pow2_ceil(ceil_div(chunks, 4)));
+  int tpr_log2 = 0;
+  while ((1ull << tpr_log2) < tpr) ++tpr_log2;
+  const unsigned threads = tpr > 32 ? (unsigned)tpr : 256;   // a multi-warp item owns its block
+  const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(ceil_div(items, threads / tpr), 0x7FFFFFFFull));
+  ScanParams p{};
+  p.in = v.in; p.out = out; p.carry = carry;
+  p.outer = v.outer; p.len = v.len; p.inner = 1;
+  p.s_outer = v.s_outer; p.s_len = 1;
+  p.row_len = 1; p.row_pitch = 1;
+  p.seg_len = seg_len; p.nseg = (uint32_t)nseg;
+  p.flags = exclusive ? 1u : 0u;
+  void* args[] = {&p, &tpr_log2};
+  return launch(c, f, grid, 1, 1, threads, 0, 1, st, args, pdl);
+}
+
+// One launch of scan_cols over items (outer, segment, tile of column units).
+static int launch_scan_cols(b200_ctx* c, CUstream st, int op, int dt, int odt, const RView& v, uint64_t seg_len, uint64_t out,
+                            uint64_t carry, bool exclusive, bool pdl) {
+  CUfunction f;
+  int rc = get_func(c, scan_name("scan_cols_", op, dt, odt), &f);
+  if (rc) return rc;
+  const size_t esz = dtype_size(dt);
+  const bool vector = scan_cols_vector(v, esz);
+  const uint64_t units = vector ? v.inner / (16 / esz) : v.inner;
+  const uint64_t ctu = scan_cols_ctu(units);
+  const uint64_t nseg = ceil_div(v.len, seg_len);
+  const uint64_t items = v.outer * nseg * ceil_div(units, ctu);
+  const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(items, 0x7FFFFFFFull));
+  ScanParams p{};
+  p.in = v.in; p.out = out; p.carry = carry;
+  p.outer = v.outer; p.len = v.len; p.inner = v.inner;
+  p.s_outer = v.s_outer; p.s_len = v.s_len;
+  p.row_len = v.row_len; p.row_pitch = v.row_pitch;
+  p.seg_len = seg_len; p.nseg = (uint32_t)nseg;
+  p.flags = (exclusive ? 1u : 0u) | (vector ? 2u : 0u);
+  void* args[] = {&p};
+  return launch(c, f, grid, 1, 1, (unsigned)ctu, 0, 1, st, args, pdl);
+}
+
+static int launch_scan(b200_ctx* c, CUstream st, int op, int dt, int odt, const RView& v, uint64_t seg_len, uint64_t out, uint64_t carry,
+                       bool exclusive, bool pdl) {
+  return v.inner == 1 ? launch_scan_rows(c, st, op, dt, odt, v, seg_len, out, carry, exclusive, pdl)
+                      : launch_scan_cols(c, st, op, dt, odt, v, seg_len, out, carry, exclusive, pdl);
+}
+
+// Scan the `len` axis of the view into the compact output.  Whole items (rows, or tiles of columns) are scanned in one
+// launch; when they cannot fill the machine, the axis is cut into segments and scanned in three stream-ordered launches:
+// the reduce first pass (one partial per segment), an exclusive scan of the partials (the carries), and the scan of every
+// segment from its carry.  That path reads the input twice.  The segmentation follows reduce_axis_view's policy.
+static int scan_axis_view(b200_ctx* c, CUstream st, int op, int dt, int odt, const RView& v, uint64_t out, bool exclusive) {
+  const uint64_t sms = c->props.num_sms;
+  const size_t esz = dtype_size(dt);
+  uint64_t seg_len = v.len;
+  if (v.inner == 1) {
+    // fewer than 4 rows per SM, a long axis and >= 32 MB: ~16 segments per SM, each >= 4096 elements, 512-element aligned
+    if (v.outer < sms * 4 && v.len >= 16384 && v.outer * v.len * esz >= (32ull << 20)) {
+      const uint64_t nseg = std::min<uint64_t>(ceil_div(sms * 16, v.outer), v.len / 4096);
+      if (nseg > 1) seg_len = ceil_div(ceil_div(v.len, nseg), 512) * 512;
+    }
+  } else {
+    // fewer than 4 column blocks per SM on an axis of >= 256 rows: ~8 blocks per SM, every segment >= 64 rows
+    const uint64_t units = scan_cols_vector(v, esz) ? v.inner / (16 / esz) : v.inner;
+    const uint64_t blocks = v.outer * ceil_div(units, scan_cols_ctu(units));
+    if (blocks < sms * 4 && v.len >= 256) {
+      const uint64_t nseg = std::min<uint64_t>(ceil_div(sms * 8, blocks), v.len / 64);
+      if (nseg > 1) seg_len = ceil_div(v.len, nseg);
+    }
+  }
+  const uint64_t nseg = ceil_div(v.len, seg_len);
+  if (nseg == 1) return launch_scan(c, st, op, dt, odt, v, v.len, out, 0, exclusive, false);
+  const uint64_t count = v.outer * nseg * v.inner;
+  CUdeviceptr partials = 0, carries = 0;
+  int rc = pool_alloc(c, count * 4, &partials, st);
+  if (rc) return rc;
+  rc = pool_alloc(c, count * 4, &carries, st);
+  if (rc) { pool_free(c, partials, st); return rc; }
+  rc = v.inner == 1 ? launch_rows_kernel(c, st, op, dt, v, seg_len, partials, 0, 1.0f)
+                    : launch_cols_kernel(c, st, op, dt, v, seg_len, partials, 0, 1.0f);
+  if (!rc) {
+    RView t;
+    t.in = partials; t.outer = v.outer; t.len = nseg; t.inner = v.inner;
+    t.s_outer = nseg * v.inner; t.s_len = v.inner; t.row_len = v.inner; t.row_pitch = v.inner;
+    rc = launch_scan(c, st, op, B200_F32, B200_F32, t, nseg, carries, 0, true, true);
+  }
+  if (!rc) rc = launch_scan(c, st, op, dt, odt, v, seg_len, out, carries, exclusive, true);
+  pool_free(c, partials, st);
+  pool_free(c, carries, st);
+  return rc;
+}
+
+static int scan_impl(b200_ctx* c, b200_stream s, b200_reduce_op op, int exclusive, b200_dtype in_dtype, b200_dtype out_dtype,
+                     b200_dptr in, b200_dptr out, int rank, const uint64_t* shape, const uint64_t* strides, int axis) {
+  if (op == B200_REDUCE_ARGMAX || op == B200_REDUCE_ARGMIN || op == B200_REDUCE_MEAN)
+    return fail(B200_ERR_UNSUPPORTED, "scan: op %d has no scan (sum, prod, max, min)", (int)op);
+  if (!op_tag(op)) return fail(B200_ERR_INVALID_ARG, "scan: unknown op %d", (int)op);
+  if (!dt_tag(in_dtype)) return fail(B200_ERR_UNSUPPORTED, "scan: input dtype %d unsupported (f32, f16, bf16)", (int)in_dtype);
+  if (out_dtype != B200_F32 && out_dtype != in_dtype)
+    return fail(B200_ERR_INVALID_ARG, "scan: output dtype %d must be f32 or the input dtype", (int)out_dtype);
+  if (rank < 1 || rank > 8 || !shape) return fail(B200_ERR_INVALID_ARG, "scan: bad rank/shape");
+  if (axis < 0 || axis >= rank) return fail(B200_ERR_INVALID_ARG, "scan: axis %d out of range for rank %d", axis, rank);
+  uint64_t n = 1;
+  for (int i = 0; i < rank; ++i) n *= shape[i];
+  if (n == 0) return B200_OK;
+  if (!in || !out) return fail(B200_ERR_INVALID_ARG, "scan: null device pointer");
+  if (in % dtype_size(in_dtype) || out % dtype_size(out_dtype))
+    return fail(B200_ERR_INVALID_ARG, "scan: a pointer is not aligned to its element size");
+  CUstream st = resolve_stream(c, s);
+  // The output is logical row-major, so the input is read in place only when its dimensions lie in memory in their logical
+  // order (contiguous, or pitched rows): then the view keeps the scanned axis at its logical position.
+  bool in_order = true;
+  if (strides) {
+    int prev = -1;
+    for (int i = 0; i < rank; ++i) {
+      if (shape[i] == 1) continue;
+      if (prev >= 0 && strides[prev] <= strides[i]) in_order = false;
+      prev = i;
+    }
+  }
+  RView v;
+  if (in_order && plan_view(rank, shape, strides, axis, false, in, &v)) return scan_axis_view(c, st, op, in_dtype, out_dtype, v, out, exclusive != 0);
+  // any other view: gather into a compact temporary first (into_contiguous), then scan that
+  CUdeviceptr tmp;
+  int rc = pool_alloc(c, n * dtype_size(in_dtype), &tmp, st);
+  if (rc) return rc;
+  rc = b200_into_contiguous(c, s, in_dtype, in, tmp, rank, shape, strides);
+  if (!rc) {
+    RView w;
+    rc = !plan_view(rank, shape, nullptr, axis, false, tmp, &w) ? fail(B200_ERR_UNKNOWN, "scan: contiguous plan failed")
+                                                                : scan_axis_view(c, st, op, in_dtype, out_dtype, w, out, exclusive != 0);
+  }
+  pool_free(c, tmp, st);
+  return rc;
+}
+
+extern "C" int b200_scan(b200_ctx* c, b200_stream s, b200_reduce_op op, int exclusive, b200_dtype in_dtype, b200_dtype out_dtype,
+                         b200_dptr in, b200_dptr out, int rank, const uint64_t* shape, const uint64_t* strides, int axis) {
+  CTX_ENTER(c);
+  return scan_impl(c, s, op, exclusive, in_dtype, out_dtype, in, out, rank, shape, strides, axis);
 }
 
 // Stage timings (ns) of the most recent fused reduce + exchange launched with option reduce.debug=1 on stream `s`:

@@ -1186,3 +1186,305 @@ REDUCE_ALL(reduce_all_sum_f32_w2, OP_SUM, DT_F32, 2, true)
 REDUCE_ALL(reduce_all_sum_f32_w4, OP_SUM, DT_F32, 4, true)
 // the arg-reduction with more loads in flight (tuning variant)
 REDUCE_ALL(reduce_all_argmax_f32_u8, OP_ARGMAX, DT_F32, 8, false)
+
+// ================================================================================================ scans along an axis
+// cumsum / cumprod / cummax / cummin of the view [outer, len, inner] into a COMPACT row-major output of the same shape:
+// inclusive out[l] = x[0] (+) ... (+) x[l], exclusive out[0] = identity, out[l] = x[0] (+) ... (+) x[l-1].  The device-wide
+// form of the reference's plane scans (crates/cubecl-core/src/runtime_tests/plane.rs:191-405).  f32 running values; a
+// 16-bit output is the running value rounded to nearest-even once, at the store.
+//
+// A long axis with few items is cut into nseg segments: the reduce first pass writes one partial per segment, an exclusive
+// scan of the partials (f32 -> f32, these kernels) turns them into per-segment carries, and the final scan starts every
+// segment from its carry (`carry` != 0).  Every combination order is fixed by the launch geometry: results are bitwise
+// reproducible for a given shape and SM count.
+struct ScanParams {
+  uint64_t in;        // input view, element (o, l, i) at in + (o * s_outer + l * s_len + inner_off(i)) elements
+  uint64_t out;       // compact [outer, len, inner] output
+  uint64_t carry;     // f32 [outer, nseg, inner]: the value every segment starts from (0: the identity)
+  uint64_t outer, len, inner;
+  uint64_t s_outer, s_len;
+  uint64_t row_len, row_pitch;  // as ReduceParams
+  uint64_t seg_len;
+  uint32_t nseg;
+  uint32_t flags;     // bit 0: exclusive; bit 1: column kernel uses vector units
+};
+
+template <int ODT>
+struct OutElem;
+template <>
+struct OutElem<DT_F32> {
+  using T = float;
+  static constexpr int VEC = 4;
+  static __device__ __forceinline__ void put(void* base, uint64_t i, float v) { reinterpret_cast<float*>(base)[i] = v; }
+  static __device__ __forceinline__ uint4 pack(const float* f) {
+    return make_uint4(__float_as_uint(f[0]), __float_as_uint(f[1]), __float_as_uint(f[2]), __float_as_uint(f[3]));
+  }
+};
+template <>
+struct OutElem<DT_F16> {
+  using T = __half;
+  static constexpr int VEC = 8;
+  static __device__ __forceinline__ void put(void* base, uint64_t i, float v) { reinterpret_cast<__half*>(base)[i] = __float2half_rn(v); }
+  static __device__ __forceinline__ uint4 pack(const float* f) {
+    uint32_t w[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const __half2 h = __floats2half2_rn(f[2 * j], f[2 * j + 1]);
+      w[j] = *reinterpret_cast<const uint32_t*>(&h);
+    }
+    return make_uint4(w[0], w[1], w[2], w[3]);
+  }
+};
+template <>
+struct OutElem<DT_BF16> {
+  using T = __nv_bfloat16;
+  static constexpr int VEC = 8;
+  static __device__ __forceinline__ void put(void* base, uint64_t i, float v) {
+    reinterpret_cast<__nv_bfloat16*>(base)[i] = __float2bfloat16_rn(v);
+  }
+  static __device__ __forceinline__ uint4 pack(const float* f) {
+    uint32_t w[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const __nv_bfloat162 h = __floats2bfloat162_rn(f[2 * j], f[2 * j + 1]);
+      w[j] = *reinterpret_cast<const uint32_t*>(&h);
+    }
+    return make_uint4(w[0], w[1], w[2], w[3]);
+  }
+};
+
+__device__ __forceinline__ void stg_stream_u4(void* p, uint4 v) {
+  asm volatile("st.global.cs.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
+
+// ------------------------------------------------------------------------------------------------ rows: the axis is innermost
+// Work items q in [0, outer * nseg) as in reduce_rows_body, TPR threads per item (TPR <= 32: a sub-warp group, TPR > 32: the
+// whole block, blockDim == TPR).  An item is walked in tiles of TPR x kScanElems elements: each thread loads its
+// kScanElems consecutive elements (128-bit loads), scans them serially in registers, the group scans the thread totals
+// (shfl_up, width min(TPR, 32), then a shared-memory stage across warps), and the running carry of the item joins in front.
+// A base that is not 16-byte aligned costs one scalar head tile; outputs leave as 128-bit stores when their address allows.
+constexpr int kScanElems = 16;
+
+template <int OP, int DT, int ODT>
+__device__ __forceinline__ void scan_rows_body(const ScanParams& p, int tpr_log2) {
+  using E = Elem<DT>;
+  using T = typename E::T;
+  using O = OutElem<ODT>;
+  using OT = typename O::T;
+  using V = ValOp<OP>;
+  constexpr int VEC = E::VEC, OVEC = O::VEC, NE = kScanElems;
+  static_assert(NE % VEC == 0 && NE % OVEC == 0, "tile chunk must be whole vectors");
+  __shared__ float s_warp[kMaxWarps];
+  pdl_wait();   // launches 2 and 3 of a segmented scan read what the previous launch wrote
+  const uint32_t tpr = 1u << tpr_log2;
+  const uint32_t per_block = blockDim.x >> tpr_log2;
+  const uint32_t sub = threadIdx.x >> tpr_log2, t = threadIdx.x & (tpr - 1);
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const uint32_t gw = tpr < 32 ? tpr : 32;                     // shuffle width
+  const uint32_t gl = lane & (gw - 1);                          // lane within the shuffle segment
+  const uint32_t gmask = tpr >= 32 ? 0xffffffffu : (((1u << tpr) - 1u) << (lane & ~(tpr - 1)));
+  const bool excl = (p.flags & 1u) != 0;
+  const uint64_t items = p.outer * p.nseg;
+  const uint64_t qstride = static_cast<uint64_t>(gridDim.x) * per_block;
+
+  for (uint64_t q = static_cast<uint64_t>(blockIdx.x) * per_block + sub; q < items; q += qstride) {
+    const uint64_t o = q / p.nseg, s = q - o * p.nseg;
+    const uint64_t l0 = s * p.seg_len;
+    const uint64_t L = (p.len - l0 < p.seg_len) ? p.len - l0 : p.seg_len;
+    const char* ib = reinterpret_cast<const char*>(p.in) + (o * p.s_outer + l0) * sizeof(T);
+    char* ob = reinterpret_cast<char*>(p.out) + (o * p.len + l0) * sizeof(OT);
+    float carry = p.carry ? reinterpret_cast<const float*>(p.carry)[q] : V::identity();
+    const uint32_t mis = static_cast<uint32_t>(reinterpret_cast<uint64_t>(ib)) & 15u;
+    uint64_t head = mis ? (16u - mis) / sizeof(T) : 0;
+    if (head > L) head = L;
+    const bool ovec = ((reinterpret_cast<uint64_t>(ob) + head * sizeof(OT)) & 15u) == 0;
+
+    for (uint64_t pos = 0; pos < L;) {
+      const bool head_tile = (pos == 0 && head != 0);
+      const uint64_t cnt = head_tile ? head : ((L - pos < static_cast<uint64_t>(tpr) * NE) ? L - pos : static_cast<uint64_t>(tpr) * NE);
+      const uint64_t c0 = static_cast<uint64_t>(t) * NE;   // this thread's chunk within the tile
+      float v[NE];
+#pragma unroll
+      for (int u = 0; u < NE / VEC; ++u) {
+        const uint64_t e = c0 + u * VEC;
+        if (!head_tile && e + VEC <= cnt) {
+          float f[VEC];
+          E::unpack(ldg_stream_u4(ib + (pos + e) * sizeof(T)), f);
+#pragma unroll
+          for (int j = 0; j < VEC; ++j) v[u * VEC + j] = f[j];
+        } else {
+#pragma unroll
+          for (int j = 0; j < VEC; ++j) v[u * VEC + j] = (e + j < cnt) ? E::get(ib, pos + e + j) : V::identity();
+        }
+      }
+      // serial inclusive scan of the chunk
+#pragma unroll
+      for (int j = 1; j < NE; ++j) v[j] = V::apply(v[j - 1], v[j]);
+      // scan of the chunk totals over the item's threads
+      float incl = v[NE - 1];
+#pragma unroll
+      for (uint32_t off = 1; off < 32; off <<= 1) {
+        if (off < gw) {
+          const float y = __shfl_up_sync(gmask, incl, off, gw);
+          if (gl >= off) incl = V::apply(y, incl);
+        }
+      }
+      float before = __shfl_up_sync(gmask, incl, 1, gw);
+      if (gl == 0) before = V::identity();
+      float tile_total;
+      if (tpr > 32) {   // one item per block: combine the warps through shared memory, in warp order
+        if (lane == 31) s_warp[warp] = incl;
+        __syncthreads();
+        float pre = V::identity();
+        tile_total = V::identity();
+        const uint32_t nw = tpr >> 5;
+        for (uint32_t w = 0; w < nw; ++w) {
+          const float x = s_warp[w];
+          if (w < warp) pre = V::apply(pre, x);
+          tile_total = V::apply(tile_total, x);
+        }
+        __syncthreads();   // the slots are reused by the next tile
+        before = V::apply(pre, before);
+      } else {
+        tile_total = __shfl_sync(gmask, incl, gw - 1, gw);
+      }
+      const float prefix = V::apply(carry, before);
+      carry = V::apply(carry, tile_total);
+      float r[NE];
+      r[0] = excl ? prefix : V::apply(prefix, v[0]);
+#pragma unroll
+      for (int j = 1; j < NE; ++j) r[j] = V::apply(prefix, excl ? v[j - 1] : v[j]);
+#pragma unroll
+      for (int u = 0; u < NE / OVEC; ++u) {
+        const uint64_t e = c0 + u * OVEC;
+        if (!head_tile && ovec && e + OVEC <= cnt) {
+          stg_stream_u4(ob + (pos + e) * sizeof(OT), O::pack(&r[u * OVEC]));
+        } else {
+#pragma unroll
+          for (int j = 0; j < OVEC; ++j)
+            if (e + j < cnt) O::put(ob, pos + e + j, r[u * OVEC + j]);
+        }
+      }
+      pos += cnt;
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ columns: any other axis
+// Each thread owns one column UNIT (a 128-bit vector of consecutive inner elements when the layout allows it, else one
+// element) and walks the item's segment of the axis serially with the running value in registers, kScanColLoads rows of
+// loads in flight; consecutive threads own consecutive units, so loads and stores are coalesced.  Work items = (outer x
+// segment) x tiles of blockDim units.  Per column this is the serial f32 order exactly.
+constexpr int kScanColLoads = 8;
+
+template <int OP, int DT, int ODT, bool VECTOR>
+__device__ __forceinline__ void scan_cols_tiles(const ScanParams& p) {
+  using E = Elem<DT>;
+  using T = typename E::T;
+  using O = OutElem<ODT>;
+  using OT = typename O::T;
+  using V = ValOp<OP>;
+  constexpr int UV = VECTOR ? E::VEC : 1;
+  constexpr int NL = kScanColLoads;
+  static_assert(!VECTOR || UV % O::VEC == 0, "a vector unit stores whole 128-bit output vectors");
+  const uint64_t units = p.inner / UV;
+  const uint32_t ctu = blockDim.x;
+  const uint64_t tiles = (units + ctu - 1) / ctu;
+  const uint64_t items = p.outer * p.nseg * tiles;
+  const bool excl = (p.flags & 1u) != 0;
+  const bool ovec = VECTOR && (p.out % 16) == 0;
+  const char* base = reinterpret_cast<const char*>(p.in);
+
+  for (uint64_t item = blockIdx.x; item < items; item += gridDim.x) {
+    const uint64_t q = item / tiles, tile = item - q * tiles;
+    const uint64_t o = q / p.nseg, s = q - o * p.nseg;
+    const uint64_t unit = tile * ctu + threadIdx.x;
+    if (unit >= units) continue;
+    const uint64_t l0 = s * p.seg_len;
+    const uint64_t L = (p.len - l0 < p.seg_len) ? p.len - l0 : p.seg_len;
+    const uint64_t i0 = unit * UV;
+    uint64_t ioff = i0;
+    if (p.row_len != p.inner) { const uint64_t rr = i0 / p.row_len; ioff = rr * p.row_pitch + (i0 - rr * p.row_len); }
+    const char* cb = base + (o * p.s_outer + l0 * p.s_len + ioff) * sizeof(T);
+    const uint64_t lstep = p.s_len * sizeof(T);
+    char* ob = reinterpret_cast<char*>(p.out) + ((o * p.len + l0) * p.inner + i0) * sizeof(OT);
+    const uint64_t ostep = p.inner * sizeof(OT);
+    float run[UV];
+#pragma unroll
+    for (int j = 0; j < UV; ++j) run[j] = p.carry ? reinterpret_cast<const float*>(p.carry)[q * p.inner + i0 + j] : V::identity();
+
+    auto emit = [&](const float (&f)[UV], uint64_t l) {
+      float r[UV];
+#pragma unroll
+      for (int j = 0; j < UV; ++j) {
+        const float nxt = V::apply(run[j], f[j]);
+        r[j] = excl ? run[j] : nxt;
+        run[j] = nxt;
+      }
+      char* dst = ob + l * ostep;
+      if (ovec) {
+#pragma unroll
+        for (int k = 0; k < UV / O::VEC; ++k) stg_stream_u4(dst + k * 16, O::pack(&r[k * O::VEC]));
+      } else {
+#pragma unroll
+        for (int j = 0; j < UV; ++j) O::put(dst, j, r[j]);
+      }
+    };
+
+    uint64_t l = 0;
+    for (; l + NL <= L; l += NL) {
+      float f[NL][UV];
+      if constexpr (VECTOR) {
+        uint4 r[NL];
+#pragma unroll
+        for (int u = 0; u < NL; ++u) r[u] = ldg_stream_u4(cb + (l + u) * lstep);
+#pragma unroll
+        for (int u = 0; u < NL; ++u) E::unpack(r[u], f[u]);
+      } else {
+#pragma unroll
+        for (int u = 0; u < NL; ++u) f[u][0] = E::get(cb + (l + u) * lstep, 0);
+      }
+#pragma unroll
+      for (int u = 0; u < NL; ++u) emit(f[u], l + u);
+    }
+    for (; l < L; ++l) {
+      float f[UV];
+      if constexpr (VECTOR) E::unpack(ldg_stream_u4(cb + l * lstep), f);
+      else f[0] = E::get(cb + l * lstep, 0);
+      emit(f, l);
+    }
+  }
+}
+
+template <int OP, int DT, int ODT>
+__device__ __forceinline__ void scan_cols_body(const ScanParams& p) {
+  using E = Elem<DT>;
+  using T = typename E::T;
+  pdl_wait();
+  const uint64_t esz = sizeof(T);
+  const bool vec_ok = (p.flags & 2u) != 0 &&  // the host counted vector units
+                      (p.inner % E::VEC) == 0 && (p.row_len % E::VEC) == 0 && (p.in % 16) == 0 && ((p.s_len * esz) % 16) == 0 &&
+                      ((p.s_outer * esz) % 16) == 0 && ((p.row_pitch * esz) % 16) == 0;
+  if (vec_ok) scan_cols_tiles<OP, DT, ODT, true>(p);
+  else scan_cols_tiles<OP, DT, ODT, false>(p);
+}
+
+#define SCAN_KERNELS(NAME_SFX, OP, DT, ODT)                                                                              \
+  extern "C" __global__ void __launch_bounds__(512) scan_rows_##NAME_SFX(const __grid_constant__ ScanParams p, int tpr_log2) { \
+    scan_rows_body<OP, DT, ODT>(p, tpr_log2);                                                                          \
+  }                                                                                                                    \
+  extern "C" __global__ void __launch_bounds__(256) scan_cols_##NAME_SFX(const __grid_constant__ ScanParams p) {         \
+    scan_cols_body<OP, DT, ODT>(p);                                                                                    \
+  }
+// output f32 for every input dtype; a 16-bit input may also keep its own dtype (suffix _<out dtype>)
+#define SCAN_DTYPES(OPN, OP)                                 \
+  SCAN_KERNELS(OPN##_f32, OP, DT_F32, DT_F32)                \
+  SCAN_KERNELS(OPN##_f16, OP, DT_F16, DT_F32)                \
+  SCAN_KERNELS(OPN##_f16_f16, OP, DT_F16, DT_F16)            \
+  SCAN_KERNELS(OPN##_bf16, OP, DT_BF16, DT_F32)              \
+  SCAN_KERNELS(OPN##_bf16_bf16, OP, DT_BF16, DT_BF16)
+
+SCAN_DTYPES(sum, OP_SUM)
+SCAN_DTYPES(prod, OP_PROD)
+SCAN_DTYPES(max, OP_MAX)
+SCAN_DTYPES(min, OP_MIN)

@@ -226,6 +226,21 @@ int b200_reduce_debug(b200_ctx* ctx, b200_stream s, uint64_t* words4);
 int b200_into_contiguous(b200_ctx* ctx, b200_stream s, b200_dtype dtype, b200_dptr in, b200_dptr out, int rank,
                          const uint64_t* shape, const uint64_t* strides);
 
+/* ---- scans along an axis: the device-wide form of the plane scans plane_inclusive_sum / plane_exclusive_sum /
+ * plane_inclusive_prod / plane_exclusive_prod (crates/cubecl-core/src/runtime_tests/plane.rs:191-405) ---------------------
+ * cumsum / cumprod / cummax / cummin of `axis` (0..rank-1): inclusive out[.., l, ..] = x[0] op ... op x[l]; exclusive
+ * (exclusive != 0) out[.., 0, ..] = identity (0, 1, -inf, +inf) and out[.., l, ..] = x[0] op ... op x[l-1].  op is SUM, PROD,
+ * MAX or MIN (ARGMAX / ARGMIN / MEAN: B200_ERR_UNSUPPORTED); max / min follow b200_reduce's rule (a NaN makes every later
+ * output NaN).  Input F32 / F16 / BF16, f32 running values; out_dtype F32 or the input dtype (a 16-bit output is the running
+ * value rounded to nearest-even once), anything else B200_ERR_INVALID_ARG.  out is compact row-major with the input's
+ * shape.  Contiguous inputs and pitched rows are read in place (any element-aligned base); other views (strides != NULL)
+ * are first gathered with b200_into_contiguous.  An extent of 0 is a no-op.  One launch when whole rows / column tiles fill
+ * the GPU, else three (segment partials, their exclusive scan, the segments from their carries): bitwise reproducible for
+ * the same shape, dtypes and SM count.  Stream-ordered, no host sync, temporaries from the pool. */
+int b200_scan(b200_ctx* ctx, b200_stream s, b200_reduce_op op, int exclusive, b200_dtype in_dtype, b200_dtype out_dtype,
+              b200_dptr in, b200_dptr out, int rank, const uint64_t* shape, const uint64_t* strides /* NULL = contiguous */,
+              int axis);
+
 /* ---- collectives: ServerCommunication (server/base.rs:632-739), CUDA impl cubecl-cuda/src/compute/server.rs:666-926 -- */
 #define B200_UNIQUE_ID_BYTES 128
 int b200_comm_get_unique_id(b200_ctx* ctx, void* id128);            /* ncclGetUniqueId (communication.rs:11-25 holds it per device set) */

@@ -223,4 +223,17 @@ inline void launch(ComputeClient& client, const TensorHandle& input, const Tenso
 }
 }  // namespace reduce
 
+namespace scan {
+/// Inclusive (or exclusive) cumulative sum / prod / max / min along `axis` into a compact output of the input's shape;
+/// output dtype F32 or the input's. Errors deferred.
+inline void launch(ComputeClient& client, const TensorHandle& input, const TensorHandle& output, int axis, reduce::Op op,
+                   bool exclusive = false) {
+  const int rc = b200_scan(client.raw(), nullptr, static_cast<b200_reduce_op>(op), exclusive ? 1 : 0,
+                           static_cast<b200_dtype>(input.dtype), static_cast<b200_dtype>(output.dtype), input.handle.ptr(),
+                           output.handle.ptr(), static_cast<int>(input.shape.size()), input.shape.data(), input.strides.data(),
+                           axis);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+}  // namespace scan
+
 }  // namespace cubecl

@@ -161,3 +161,25 @@ pub mod reduce {
         ctx.reduce(stream, op, input.dtype, &input.view(), output.ptr, axis)
     }
 }
+
+pub mod scan {
+    use super::*;
+
+    /// `scan::launch(client, input, output, axis, op, exclusive)`: cumulative sum / prod / max / min along `axis`;
+    /// `output` is contiguous with the input's shape, F32 or the input's dtype.
+    ///
+    /// # Safety
+    /// As [`super::matmul::launch`].
+    pub unsafe fn launch(
+        ctx: &mut Context, stream: b200_stream, input: &TensorHandle, output: &TensorHandle, axis: usize, op: ReduceOp,
+        exclusive: bool,
+    ) -> Result<(), Error> {
+        if output.shape != input.shape {
+            return Err(invalid("scan: output shape differs from the input's".to_string()));
+        }
+        if axis >= input.shape.len() {
+            return Err(invalid(format!("axis {} out of range for rank {}", axis, input.shape.len())));
+        }
+        ctx.scan(stream, op, exclusive, input.dtype, output.dtype, &input.view(), output.ptr, axis)
+    }
+}

@@ -335,6 +335,23 @@ impl Context {
         ))
     }
 
+    /// Inclusive (or exclusive) cumulative sum / prod / max / min of `axis` into the compact row-major `out` of the input's
+    /// shape; `out_dtype` F32 or the input's (the device-wide form of the plane scans, runtime_tests/plane.rs:191-405).
+    ///
+    /// # Safety
+    /// Same contract as [`Context::matmul`].
+    #[allow(clippy::too_many_arguments)]
+    pub unsafe fn scan(
+        &mut self, stream: b200_stream, op: ReduceOp, exclusive: bool, in_dtype: DType, out_dtype: DType, input: &TensorView,
+        out: b200_dptr, axis: usize,
+    ) -> Result<(), Error> {
+        assert!(input.strides.len() == input.shape.len());
+        check(sys::b200_scan(
+            self.0, stream, op as c_int, exclusive as c_int, in_dtype as c_int, out_dtype as c_int, input.ptr, out,
+            input.shape.len() as c_int, input.shape.as_ptr(), input.strides.as_ptr(), axis as c_int,
+        ))
+    }
+
     /// out (compact row-major) = gather of the strided tensor `input` (into_contiguous, cubecl-std/src/tensor/contiguous.rs).
     ///
     /// # Safety
