@@ -18,6 +18,7 @@ HEADER_PATH = PKG.parent / "include" / "cubecl_b200.h"
 F32, F16, BF16, U32, I32, F64, I64, U64, U8, I8, F8E4M3, F8E5M2, F4E2M1X2, UE8M0 = range(14)
 REDUCE_SUM, REDUCE_PROD, REDUCE_MAX, REDUCE_MIN, REDUCE_ARGMAX, REDUCE_ARGMIN, REDUCE_MEAN = range(7)
 COMM_SUM, COMM_MEAN = 0, 1
+QV_Q8F, QV_E5M2, QV_E4M3, QV_Q4F, QV_E2M1, QV_Q2F, QV_Q8S, QV_Q4S, QV_Q2S = range(9)
 UNIQUE_ID_BYTES = 128
 IPC_HANDLE_BYTES = 64
 
@@ -38,6 +39,11 @@ class B200Error(RuntimeError):
 
 class Epilogue(C.Structure):
     _fields_ = [("alpha", C.c_float), ("activation", C.c_int32), ("bias", C.c_uint64)]
+
+
+class QuantScheme(C.Structure):
+    """b200_quant_scheme: value (b200_quant_value), block, block_scale (b200_dtype), tensor_scale (0 / 1)."""
+    _fields_ = [("value", C.c_int32), ("block", C.c_int32), ("block_scale", C.c_int32), ("tensor_scale", C.c_int32)]
 
 
 class Props(C.Structure):
@@ -97,6 +103,10 @@ SIGNATURES = {
     "b200_reduce_debug": (C.c_int, [_vp, _vp, _u64p]),
     "b200_into_contiguous": (C.c_int, [_vp, _vp, C.c_int, C.c_uint64, C.c_uint64, C.c_int, _u64p, _u64p]),
     "b200_scan": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint64, C.c_uint64, C.c_int, _u64p, _u64p, C.c_int]),
+    "b200_quantize": (C.c_int, [_vp, _vp, C.POINTER(QuantScheme), C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64,
+                                C.c_int, _u64p, _u64p]),
+    "b200_dequantize": (C.c_int, [_vp, _vp, C.POINTER(QuantScheme), C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64,
+                                  C.c_int, _u64p]),
     "b200_comm_get_unique_id": (C.c_int, [_vp, _vp]),
     "b200_comm_init": (C.c_int, [_vp, _intp, C.c_int, _vp]),
     "b200_all_reduce": (C.c_int, [_vp, _vp, C.c_uint64, C.c_uint64, C.c_size_t, C.c_int, C.c_int, _intp, C.c_int]),

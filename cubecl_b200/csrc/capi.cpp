@@ -38,6 +38,8 @@ extern const unsigned char b200_cubin_reduce[];
 extern const unsigned char b200_cubin_reduce_end[];
 extern const unsigned char b200_cubin_aux[];
 extern const unsigned char b200_cubin_aux_end[];
+extern const unsigned char b200_cubin_quant[];
+extern const unsigned char b200_cubin_quant_end[];
 }
 
 // ================================================================================================ errors
@@ -405,12 +407,13 @@ static int get_func(b200_ctx* c, const std::string& name, CUfunction* out) {
   if (c->dry) { c->pending_kernel = name; *out = nullptr; return B200_OK; }
   auto it = c->funcs.find(name);
   if (it != c->funcs.end()) { *out = it->second; return B200_OK; }
-  // modules are loaded in the order gemm, reduce, aux, gemm_b, gemm_c; the kernel name says where a kernel lives (no
+  // modules are loaded in the order gemm, reduce, aux, gemm_b, gemm_c, quant; the kernel name says where a kernel lives (no
   // failing lookups, which API-level tools such as compute-sanitizer would report)
   auto starts = [&](const char* pfx) { return name.rfind(pfx, 0) == 0; };
   auto has = [&](const char* part) { return name.find(part) != std::string::npos; };
   const bool tc_gemm = starts("gemm_") && name != "gemm_simt_strided" && name != "gemm_scaled_simt";
-  const size_t home = tc_gemm && (has("_2sm_n128_") || has("_2sm_n224_")) ? 3
+  const size_t home = starts("quant_") ? 5
+                      : tc_gemm && (has("_2sm_n128_") || has("_2sm_n224_")) ? 3
                       : tc_gemm && (has("_1sm_n128_") || has("_2sm_m512_")) ? 4
                       : tc_gemm || starts("wgmma_probe_") ? 0
                       : starts("reduce_") || starts("scan_") ? 1 : 2;
@@ -433,7 +436,8 @@ extern "C" int b200_get_cubin(const char* name, const void** image, size_t* size
   else if (!strcmp(name, "aux")) { b = b200_cubin_aux; e = b200_cubin_aux_end; }
   else if (!strcmp(name, "gemm_b")) { b = b200_cubin_gemm_b; e = b200_cubin_gemm_b_end; }
   else if (!strcmp(name, "gemm_c")) { b = b200_cubin_gemm_c; e = b200_cubin_gemm_c_end; }
-  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux)", name);
+  else if (!strcmp(name, "quant")) { b = b200_cubin_quant; e = b200_cubin_quant_end; }
+  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant)", name);
   *image = b;
   *size = static_cast<size_t>(e - b);
   return B200_OK;
@@ -485,7 +489,8 @@ extern "C" int b200_init(int device, b200_ctx** out) {
       (rc = load_module(c, b200_cubin_reduce, b200_cubin_reduce_end, "reduce")) ||
       (rc = load_module(c, b200_cubin_aux, b200_cubin_aux_end, "aux")) ||
       (rc = load_module(c, b200_cubin_gemm_b, b200_cubin_gemm_b_end, "gemm_b")) ||
-      (rc = load_module(c, b200_cubin_gemm_c, b200_cubin_gemm_c_end, "gemm_c"))) {
+      (rc = load_module(c, b200_cubin_gemm_c, b200_cubin_gemm_c_end, "gemm_c")) ||
+      (rc = load_module(c, b200_cubin_quant, b200_cubin_quant_end, "quant"))) {
     for (CUmodule m : c->modules) g_drv.cuModuleUnload_p(m);
     g_drv.cuDevicePrimaryCtxRelease_p(c->dev);
     return bail(rc);
@@ -2218,6 +2223,219 @@ extern "C" int b200_scan(b200_ctx* c, b200_stream s, b200_reduce_op op, int excl
                          b200_dptr in, b200_dptr out, int rank, const uint64_t* shape, const uint64_t* strides, int axis) {
   CTX_ENTER(c);
   return scan_impl(c, s, op, exclusive, in_dtype, out_dtype, in, out, rank, shape, strides, axis);
+}
+
+// ================================================================================================ quantize / dequantize
+// Kernels in csrc/quant.cu (parameter blocks mirrored there).
+struct QuantParams {
+  uint64_t in, values, block_scales, tensor_scale, amax;
+  uint64_t rows, K, pitch;
+  uint32_t value, block, scale_dt, block_log2;
+};
+struct QuantDecodeParams {
+  uint64_t values, block_scales, tensor_scale, out;
+  uint64_t n;
+  uint32_t value, block, scale_dt, flags;
+  uint32_t block_log2, pad;
+};
+
+static uint32_t log2_u32(uint32_t v) {
+  uint32_t l = 0;
+  while (v > 1) { v >>= 1; ++l; }
+  return l;
+}
+
+static constexpr unsigned kQuantThreads = 256;
+
+// Bits of a b200_quant_value (QuantValue::size_bits, scheme.rs:381-387); 0 for a value outside the enum.
+static uint32_t quant_bits(int32_t v) {
+  switch (v) {
+    case B200_QV_Q8F: case B200_QV_E5M2: case B200_QV_E4M3: case B200_QV_Q8S: return 8;
+    case B200_QV_Q4F: case B200_QV_E2M1: case B200_QV_Q4S: return 4;
+    case B200_QV_Q2F: case B200_QV_Q2S: return 2;
+    default: return 0;
+  }
+}
+static size_t scale_dtype_size(int32_t dt) {
+  switch (dt) {
+    case B200_F32: return 4;
+    case B200_F16: case B200_BF16: return 2;
+    case B200_UE8M0: case B200_F8E4M3: return 1;
+    default: return 0;
+  }
+}
+
+// A device-side memset that a dry-run planning context records as one line.
+static int memset32_async(b200_ctx* c, CUstream st, CUdeviceptr dst, uint32_t value, size_t words) {
+  if (c->dry) {
+    char line[64];
+    snprintf(line, sizeof(line), "memset32 %zu\n", words);
+    c->plan += line;
+    return B200_OK;
+  }
+  CU_CHECK(g_drv.cuMemsetD32Async_p(dst, value, words, st));
+  return B200_OK;
+}
+
+// The checks both directions share: the scheme's fields, the shape, and which pointers its levels need.  block_scale is
+// read only when the scheme has a block level (block > 0); with block == 0 it is ignored, whatever it holds.  `what` names the
+// call in messages.  On success *n is the element count and *K the innermost extent.
+static int quant_check(const char* what, const b200_quant_scheme* q, int rank, const uint64_t* shape, b200_dptr block_scales,
+                       b200_dptr tensor_scale, uint64_t* n, uint64_t* K) {
+  if (!q) return fail(B200_ERR_INVALID_ARG, "%s: null scheme", what);
+  const uint32_t bits = quant_bits(q->value);
+  if (!bits) return fail(B200_ERR_INVALID_ARG, "%s: unknown quant value %d", what, (int)q->value);
+  if (q->tensor_scale != 0 && q->tensor_scale != 1) return fail(B200_ERR_INVALID_ARG, "%s: tensor_scale must be 0 or 1", what);
+  if (q->block < 0) return fail(B200_ERR_INVALID_ARG, "%s: negative block %d", what, (int)q->block);
+  if (q->block == 0 && !q->tensor_scale)
+    return fail(B200_ERR_INVALID_ARG, "%s: a scheme without a block level needs the tensor level (per-tensor f32)", what);
+  if (q->block > 0 && !scale_dtype_size(q->block_scale))
+    return fail(B200_ERR_INVALID_ARG, "%s: block-scale dtype %d is not F32, F16, BF16, UE8M0 or F8E4M3", what, (int)q->block_scale);
+  if (q->block != 0 && q->block != 8 && q->block != 16 && q->block != 32 && q->block != 64 && q->block != 128)
+    return fail(B200_ERR_UNSUPPORTED, "%s: block %d (0, 8, 16, 32, 64, 128)", what, (int)q->block);
+  if (rank < 1 || rank > 8 || !shape) return fail(B200_ERR_INVALID_ARG, "%s: bad rank/shape", what);
+  *n = 1;
+  for (int i = 0; i < rank; ++i) *n *= shape[i];
+  *K = shape[rank - 1];
+  if (q->block > 0 && *K % (uint64_t)q->block)
+    return fail(B200_ERR_INVALID_ARG, "%s: innermost extent %llu is not a multiple of the block %d", what, (unsigned long long)*K,
+                (int)q->block);
+  if (*K * bits % 8) return fail(B200_ERR_INVALID_ARG, "%s: a row of %llu %u-bit values is not a whole number of bytes", what,
+                                 (unsigned long long)*K, bits);
+  if (*n == 0) return B200_OK;
+  if ((q->block > 0) != (block_scales != 0))
+    return fail(B200_ERR_INVALID_ARG, "%s: block_scales must be non-null exactly when the scheme has a block level", what);
+  if ((q->tensor_scale != 0) != (tensor_scale != 0))
+    return fail(B200_ERR_INVALID_ARG, "%s: tensor_scale must be non-null exactly when the scheme has a tensor level", what);
+  if ((q->block > 0 && block_scales % scale_dtype_size(q->block_scale)) || tensor_scale % 4)
+    return fail(B200_ERR_INVALID_ARG, "%s: a scale pointer is not aligned to its element size", what);
+  return B200_OK;
+}
+
+// The input as rows of K elements `pitch` apart, read in place when base and rows are 16-byte aligned.  A per-tensor scheme
+// on a contiguous input runs as one row (scales do not care about rows there).
+static bool quant_rows_view(int rank, const uint64_t* shape, const uint64_t* strides, uint64_t n, size_t esz, bool per_tensor,
+                            uint64_t in, uint64_t* rows, uint64_t* K, uint64_t* pitch) {
+  *K = shape[rank - 1];
+  *rows = n / *K;
+  *pitch = *K;
+  if (strides) {
+    // innermost unit-stride (or extent 1); every other non-unit dimension nests at its successor's extent; the first
+    // non-unit leading dimension sets the row pitch
+    uint64_t expect = 0;
+    bool first = true;
+    if (*K > 1 && strides[rank - 1] != 1) return false;
+    for (int i = rank - 2; i >= 0; --i) {
+      if (shape[i] == 1) continue;
+      if (first) {
+        if (strides[i] < *K) return false;
+        *pitch = strides[i];
+        first = false;
+      } else if (strides[i] != expect) {
+        return false;
+      }
+      expect = strides[i] * shape[i];
+    }
+  }
+  if (per_tensor && *pitch == *K) { *rows = 1; *K = n; *pitch = n; }
+  return in % 16 == 0 && (*rows == 1 || (*pitch * esz) % 16 == 0);
+}
+
+static int quant_impl(b200_ctx* c, b200_stream s, const b200_quant_scheme* q, b200_dtype in_dtype, b200_dptr in, b200_dptr values,
+                      b200_dptr block_scales, b200_dptr tensor_scale, int rank, const uint64_t* shape, const uint64_t* strides) {
+  uint64_t n = 0, K = 0;
+  int rc = quant_check("quantize", q, rank, shape, block_scales, tensor_scale, &n, &K);
+  if (rc) return rc;
+  if (q->block > 0 && q->tensor_scale && q->block_scale != B200_F16 && q->block_scale != B200_F8E4M3)
+    return fail(B200_ERR_UNSUPPORTED, "quantize: two-level schemes take F16 or F8E4M3 (ue4m3) block scales, not dtype %d",
+                (int)q->block_scale);
+  if (!dt_tag(in_dtype)) return fail(B200_ERR_INVALID_ARG, "quantize: input dtype %d is not F32, F16 or BF16", (int)in_dtype);
+  if (n == 0) return B200_OK;
+  if (!in || !values) return fail(B200_ERR_INVALID_ARG, "quantize: null device pointer");
+  const size_t esz = dtype_size(in_dtype);
+  if (in % esz) return fail(B200_ERR_INVALID_ARG, "quantize: input pointer is not aligned to its element size");
+  CUstream st = resolve_stream(c, s);
+  QuantParams p{};
+  p.values = values; p.block_scales = block_scales; p.tensor_scale = tensor_scale;
+  p.value = (uint32_t)q->value; p.block = (uint32_t)q->block; p.scale_dt = q->block > 0 ? (uint32_t)q->block_scale : B200_F32;
+  p.block_log2 = log2_u32(p.block);
+  CUdeviceptr tmp = 0, amax = 0;
+  uint64_t rows, pitch;
+  if (quant_rows_view(rank, shape, strides, n, esz, q->block == 0, in, &rows, &K, &pitch)) {
+    p.in = in;
+  } else {
+    // any other view (or an unaligned base / row): gather into a compact pooled temporary first
+    rc = pool_alloc(c, n * esz, &tmp, st);
+    if (rc) return rc;
+    std::vector<uint64_t> cs(rank);
+    uint64_t acc = 1;
+    for (int i = rank - 1; i >= 0; --i) { cs[i] = acc; acc *= shape[i]; }
+    rc = b200_into_contiguous(c, s, in_dtype, in, tmp, rank, shape, strides ? strides : cs.data());
+    quant_rows_view(rank, shape, nullptr, n, esz, q->block == 0, tmp, &rows, &K, &pitch);
+    p.in = tmp;
+  }
+  p.rows = rows; p.K = K; p.pitch = pitch;
+  const uint64_t vec = 16 / esz, chunks = rows * ((K + vec - 1) / vec);
+  if (!rc && q->tensor_scale) {
+    // the tensor level first: the finite |x| max of the whole tensor, atomicMax'ed as u32 bits into a pooled word
+    rc = pool_alloc(c, 4, &amax, st);
+    if (!rc) rc = memset32_async(c, st, amax, 0, 1);
+    CUfunction f;
+    if (!rc) rc = get_func(c, std::string("quant_absmax_") + dt_tag(in_dtype), &f);
+    if (!rc) {
+      p.amax = amax;
+      const uint64_t want = ceil_div(chunks, (uint64_t)kQuantThreads * 4);
+      const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(want, (uint64_t)c->props.num_sms * 8));
+      void* args[] = {&p};
+      rc = launch(c, f, grid, 1, 1, kQuantThreads, 0, 1, st, args);
+    }
+  }
+  if (!rc) {
+    CUfunction f;
+    rc = get_func(c, std::string("quant_encode_") + dt_tag(in_dtype), &f);
+    if (!rc) {
+      const uint64_t grid = std::max<uint64_t>(1, ceil_div(chunks, (uint64_t)kQuantThreads));
+      if (grid > 0x7FFFFFFFull) rc = fail(B200_ERR_TOO_MANY_RESOURCES, "quantize: %llu chunks exceed one launch", (unsigned long long)chunks);
+      void* args[] = {&p};
+      if (!rc) rc = launch(c, f, (unsigned)grid, 1, 1, kQuantThreads, 0, 1, st, args);
+    }
+  }
+  if (amax) pool_free(c, amax, st);
+  if (tmp) pool_free(c, tmp, st);
+  return rc;
+}
+
+extern "C" int b200_quantize(b200_ctx* c, b200_stream s, const b200_quant_scheme* scheme, b200_dtype in_dtype, b200_dptr in,
+                             b200_dptr values, b200_dptr block_scales, b200_dptr tensor_scale, int rank, const uint64_t* shape,
+                             const uint64_t* strides) {
+  CTX_ENTER(c);
+  return quant_impl(c, s, scheme, in_dtype, in, values, block_scales, tensor_scale, rank, shape, strides);
+}
+
+extern "C" int b200_dequantize(b200_ctx* c, b200_stream s, const b200_quant_scheme* scheme, b200_dtype out_dtype, b200_dptr values,
+                               b200_dptr block_scales, b200_dptr tensor_scale, b200_dptr out, int rank, const uint64_t* shape) {
+  CTX_ENTER(c);
+  uint64_t n = 0, K = 0;
+  int rc = quant_check("dequantize", scheme, rank, shape, block_scales, tensor_scale, &n, &K);
+  if (rc) return rc;
+  if (!dt_tag(out_dtype)) return fail(B200_ERR_INVALID_ARG, "dequantize: output dtype %d is not F32, F16 or BF16", (int)out_dtype);
+  if (n == 0) return B200_OK;
+  if (!values || !out) return fail(B200_ERR_INVALID_ARG, "dequantize: null device pointer");
+  if (out % dtype_size(out_dtype)) return fail(B200_ERR_INVALID_ARG, "dequantize: output pointer is not aligned to its element size");
+  CUfunction f;
+  rc = get_func(c, std::string("quant_decode_") + dt_tag(out_dtype), &f);
+  if (rc) return rc;
+  QuantDecodeParams p{};
+  p.values = values; p.block_scales = block_scales; p.tensor_scale = tensor_scale; p.out = out; p.n = n;
+  p.value = (uint32_t)scheme->value; p.block = (uint32_t)scheme->block;
+  p.scale_dt = scheme->block > 0 ? (uint32_t)scheme->block_scale : B200_F32;
+  p.flags = (values % 16 == 0 && out % 16 == 0) ? 1u : 0u;
+  p.block_log2 = log2_u32(p.block);
+  const uint64_t threads = ceil_div(n * quant_bits(scheme->value) / 8, (uint64_t)16);
+  const uint64_t grid = std::max<uint64_t>(1, ceil_div(threads, (uint64_t)kQuantThreads));
+  if (grid > 0x7FFFFFFFull) return fail(B200_ERR_TOO_MANY_RESOURCES, "dequantize: %llu elements exceed one launch", (unsigned long long)n);
+  void* args[] = {&p};
+  return launch(c, f, (unsigned)grid, 1, 1, kQuantThreads, 0, 1, resolve_stream(c, s), args);
 }
 
 // Stage timings (ns) of the most recent fused reduce + exchange launched with option reduce.debug=1 on stream `s`:

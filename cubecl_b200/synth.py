@@ -71,7 +71,8 @@ def fp8_bits_to_f32(bits: np.ndarray, kind: str) -> np.ndarray:
 
 
 def f32_to_fp8_bits(x: np.ndarray, kind: str) -> np.ndarray:
-    """Round-to-nearest-even, saturating to the largest finite value (mirrors __nv_cvt_float_to_fp8(.., __NV_SATFINITE, ..))."""
+    """Round-to-nearest-even, saturating to the largest finite value (mirrors __nv_cvt_float_to_fp8(.., __NV_SATFINITE, ..));
+    +-inf saturates with its sign, NaN of either sign gives 0x7F."""
     table = _fp8_table(kind).astype(np.float64)
     pos_codes = np.array([c for c in range(128) if np.isfinite(table[c])], dtype=np.int64)   # ascending magnitudes
     pos_vals = table[pos_codes]
@@ -83,9 +84,8 @@ def f32_to_fp8_bits(x: np.ndarray, kind: str) -> np.ndarray:
     pick_hi = (d_hi < d_lo) | ((d_hi == d_lo) & (pos_codes[hi] % 2 == 0))   # ties -> even mantissa
     code = np.where(pick_hi, pos_codes[hi], pos_codes[lo])
     code = np.where(a >= pos_vals[-1], pos_codes[-1], code)                     # saturate (incl. inf)
-    code = np.where(np.isnan(a), 0x7F, code)
     sign = np.signbit(xf).astype(np.int64) << 7
-    return (code | sign).astype(np.uint8)
+    return np.where(np.isnan(a), 0x7F, code | sign).astype(np.uint8)
 
 
 # ---- MX formats (block-scaled matmul): e2m1 (fp4) packed two per byte, ue8m0 scales
@@ -99,14 +99,14 @@ def e2m1_codes_to_f32(codes: np.ndarray) -> np.ndarray:
 
 
 def f32_to_e2m1_codes(x: np.ndarray) -> np.ndarray:
-    """Round to nearest (ties to the even code), saturating at +-6."""
+    """Round to nearest (ties to the even code), saturating at +-6 (+-inf included); NaN gives code 0."""
     xf = np.ascontiguousarray(x, dtype=np.float32)
     a = np.minimum(np.abs(xf.astype(np.float64)), 6.0)
     hi = np.clip(np.searchsorted(E2M1_VALUES.astype(np.float64), a, side="left"), 0, 7)
     lo = np.clip(hi - 1, 0, 7)
     d_lo, d_hi = np.abs(a - E2M1_VALUES[lo]), np.abs(E2M1_VALUES[hi] - a)
     code = np.where((d_hi < d_lo) | ((d_hi == d_lo) & (hi % 2 == 0)), hi, lo)
-    return (code | (np.signbit(xf).astype(np.int64) << 3)).astype(np.uint8)
+    return np.where(np.isnan(xf), 0, code | (np.signbit(xf).astype(np.int64) << 3)).astype(np.uint8)
 
 
 def pack_e2m1x2(codes: np.ndarray) -> np.ndarray:

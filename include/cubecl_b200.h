@@ -82,7 +82,7 @@ typedef struct b200_props {
 /* ---- lifecycle: R::client(device) -> DeviceService::init (cubecl-cuda/src/runtime.rs:52-350) ------------------------ */
 int b200_abi_version(void);
 int b200_device_count(int* count);
-/* The embedded prebuilt sm_90a images ("gemm" | "gemm_b" | "gemm_c" | "reduce" | "aux"), for a host that prefers to cuModuleLoadData them into
+/* The embedded prebuilt sm_90a images ("gemm" | "gemm_b" | "gemm_c" | "reduce" | "aux" | "quant"), for a host that prefers to cuModuleLoadData them into
  * its own module cache (CudaContext::modules, crates/cubecl-cuda/src/compute/context.rs:38-62,293). No GPU needed. */
 int b200_get_cubin(const char* name, const void** image, size_t* size);
 int b200_init(int device, b200_ctx** out);   /* cuInit, primary ctx retain, load the embedded sm_90a cubins (context.rs:293) */
@@ -240,6 +240,50 @@ int b200_into_contiguous(b200_ctx* ctx, b200_stream s, b200_dtype dtype, b200_dp
 int b200_scan(b200_ctx* ctx, b200_stream s, b200_reduce_op op, int exclusive, b200_dtype in_dtype, b200_dtype out_dtype,
               b200_dptr in, b200_dptr out, int rank, const uint64_t* shape, const uint64_t* strides /* NULL = contiguous */,
               int axis);
+
+/* ---- quantize / dequantize along the innermost axis: CubeCL's QuantScheme (crates/cubecl-common/src/quant/scheme.rs) -----
+ * Layout.  x is [..., K] (rank >= 1).  Codes are one compact row-major byte stream [..., K * bits / 8]: field i of a row sits
+ * at bit offset i * bits, from the low bits upward (8-bit values are bytes; two e2m1 per byte, element 2i in the low nibble,
+ * as B200_F4E2M1X2).  Read as little-endian u32 words this stream is the reference's PackedU32(0) store, and it is also its
+ * Native / PackedNative(0) store, so the scheme has no store field: K * bits must be a multiple of 8.  Block scales are compact
+ * [..., K / block] in the block-scale dtype (for MXFP8 / MXFP4 the row-major scales of b200_matmul_scaled, scales_packed = 0;
+ * for E2M1 / 16 / F8E4M3 its scale_block = 16 layout); the tensor scale is one f32.
+ * Schemes.  block in {0, 8, 16, 32, 64, 128} (other sizes: B200_ERR_UNSUPPORTED) with K % block == 0; block == 0 is per-tensor
+ * f32 only and needs tensor_scale = 1 (a level-less scheme resolves to it, scheme.rs:94-104).  block > 0 with tensor_scale = 1
+ * is two-level: b200_quantize takes F16 or F8E4M3 (ue4m3) block scales only (F32 / UE8M0 gain nothing and BF16 drives the
+ * global scale subnormal, scheme.rs:200-207: B200_ERR_UNSUPPORTED); b200_dequantize takes every block-scale dtype.
+ * Scale rule.  range_max = the positive end of QuantValue::range() (127, 7, 1, 448, 57344, 6); amax = max |x| over FINITE x.
+ * One level: s = round_up(amax / range_max) in the scale dtype.  Two levels: g = (amax_tensor / range_max) /
+ * max_representable(block dtype), s_b = round_up((amax_b / range_max) / g) (0 for a block whose amax is 0), effective scale
+ * g * f32(s_b) rounded once in f32.  round_up is ScaleDtype::round_up bit for bit for F32 / F16 / BF16 / UE4M3; UE8M0, which the
+ * reference leaves unimplemented, takes the smallest power of two >= s, clamped to codes 0..254 (unlike the OCP MX recipe
+ * floor(log2 amax) - emax, it never clips the block maximum).  IEEE f32 throughout, division by `/`.
+ * Encoding.  q = x / eff; integers: round half to even, clamp to range(); e4m3 / e5m2: round to nearest even, satfinite;
+ * e2m1: round to nearest, ties to the even code, saturating at +-6.  A zero scale gives code 0; +-inf saturates to the range
+ * end; NaN gives code 0 (integers, e2m1) or 0x7F (fp8).
+ * Dequantize.  out = RNE(f32(q) * eff) in F32 / F16 / BF16, compact.  Integer fields are sign-extended; ue8m0 scales are
+ * 2^(b-127) (255 = NaN); e4m3 scales are read with the sign ignored.
+ * Malformed input is B200_ERR_INVALID_ARG: K not divisible, a sub-byte row, a null pointer for a present level or a non-null
+ * one for an absent level, a dtype or value outside the lists (block_scale is only read when block > 0).  An extent of 0 is a no-op.  Stream-ordered, no host sync,
+ * temporaries from the pool.  Inputs F32 / F16 / BF16: contiguous tensors and pitched rows with 16-byte aligned base and rows
+ * are read in place, any other view is first gathered with b200_into_contiguous.  A scheme with a tensor level runs a
+ * memset, an absmax pass and the encode pass; a block-only scheme is one launch; dequantize is one launch. */
+typedef enum b200_quant_value {            /* QuantValue, scheme.rs:358-377, in its order */
+  B200_QV_Q8F = 0, B200_QV_E5M2 = 1, B200_QV_E4M3 = 2, B200_QV_Q4F = 3, B200_QV_E2M1 = 4,
+  B200_QV_Q2F = 5, B200_QV_Q8S = 6, B200_QV_Q4S = 7, B200_QV_Q2S = 8
+} b200_quant_value;
+typedef struct b200_quant_scheme {
+  int32_t value;         /* b200_quant_value */
+  int32_t block;         /* values per block scale along the innermost axis; 0 = no block level */
+  int32_t block_scale;   /* b200_dtype: F32, F16, BF16, UE8M0, F8E4M3 (= ue4m3: written with the sign clear); ignored when block == 0 */
+  int32_t tensor_scale;  /* 1 = one f32 per-tensor scale (the only level, or the global level over the blocks) */
+} b200_quant_scheme;
+int b200_quantize(b200_ctx* ctx, b200_stream s, const b200_quant_scheme* scheme, b200_dtype in_dtype, b200_dptr in,
+                  b200_dptr values, b200_dptr block_scales, b200_dptr tensor_scale,
+                  int rank, const uint64_t* shape, const uint64_t* strides /* NULL = contiguous */);
+int b200_dequantize(b200_ctx* ctx, b200_stream s, const b200_quant_scheme* scheme, b200_dtype out_dtype,
+                    b200_dptr values, b200_dptr block_scales, b200_dptr tensor_scale, b200_dptr out,
+                    int rank, const uint64_t* shape);
 
 /* ---- collectives: ServerCommunication (server/base.rs:632-739), CUDA impl cubecl-cuda/src/compute/server.rs:666-926 -- */
 #define B200_UNIQUE_ID_BYTES 128

@@ -236,4 +236,25 @@ inline void launch(ComputeClient& client, const TensorHandle& input, const Tenso
 }
 }  // namespace scan
 
+namespace quant {
+/// QuantScheme (value, block level, per-tensor level); see b200_quantize in cubecl_b200.h for the contract.
+using Scheme = b200_quant_scheme;
+/// Codes [..., K * bits / 8], block scales [..., K / block] and the f32 tensor scale of `input` (any strides) along its
+/// innermost axis; pass 0 for an absent level. Errors deferred.
+inline void quantize(ComputeClient& client, const TensorHandle& input, const Scheme& scheme, b200_dptr values,
+                     b200_dptr block_scales, b200_dptr tensor_scale) {
+  const int rc = b200_quantize(client.raw(), nullptr, &scheme, static_cast<b200_dtype>(input.dtype), input.handle.ptr(), values,
+                               block_scales, tensor_scale, static_cast<int>(input.shape.size()), input.shape.data(),
+                               input.strides.data());
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+/// output (contiguous F32 / F16 / BF16, the quantized tensor's shape) = the dequantized values. Errors deferred.
+inline void dequantize(ComputeClient& client, const Scheme& scheme, b200_dptr values, b200_dptr block_scales, b200_dptr tensor_scale,
+                       const TensorHandle& output) {
+  const int rc = b200_dequantize(client.raw(), nullptr, &scheme, static_cast<b200_dtype>(output.dtype), values, block_scales,
+                                 tensor_scale, output.handle.ptr(), static_cast<int>(output.shape.size()), output.shape.data());
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+}  // namespace quant
+
 }  // namespace cubecl

@@ -6,7 +6,7 @@
 //! Inside cubecl-cuda the `Context` is owned by `CudaServer` and `TensorHandle::ptr` is what `BufferBinding` resolves to
 //! on the runner thread (INTEGRATION.md section 3); standalone, it is a pointer from `Context::alloc`.
 
-use crate::{b200_dptr, b200_stream, Context, DType, Error, Epilogue, ReduceOp, Status, TensorView};
+use crate::{b200_dptr, b200_stream, Context, DType, Error, Epilogue, QuantScheme, ReduceOp, Status, TensorView};
 
 /// Buffer + shape + strides (in ELEMENTS) + dtype: `TensorHandle<R>` of crates/cubecl-std/src/tensor/handle.rs:13-23
 /// with the `Handle` already resolved to a device pointer.
@@ -181,5 +181,39 @@ pub mod scan {
             return Err(invalid(format!("axis {} out of range for rank {}", axis, input.shape.len())));
         }
         ctx.scan(stream, op, exclusive, input.dtype, output.dtype, &input.view(), output.ptr, axis)
+    }
+}
+
+pub mod quant {
+    use super::*;
+
+    /// `quant::quantize(client, input, scheme, values, block_scales, tensor_scale)`: codes, block scales and tensor scale
+    /// of `input` along its innermost axis (`block_scales` / `tensor_scale` are `None` for an absent level).
+    ///
+    /// # Safety
+    /// As [`super::matmul::launch`].
+    pub unsafe fn quantize(
+        ctx: &mut Context, stream: b200_stream, input: &TensorHandle, scheme: &QuantScheme, values: &TensorHandle,
+        block_scales: Option<&TensorHandle>, tensor_scale: Option<&TensorHandle>,
+    ) -> Result<(), Error> {
+        ctx.quantize(
+            stream, scheme, input.dtype, &input.view(), values.ptr, block_scales.map_or(0, |t| t.ptr),
+            tensor_scale.map_or(0, |t| t.ptr),
+        )
+    }
+
+    /// `quant::dequantize(client, values, block_scales, tensor_scale, scheme, output)`: `output` is contiguous, F32 / F16 /
+    /// BF16, with the logical shape of the quantized tensor.
+    ///
+    /// # Safety
+    /// As [`super::matmul::launch`].
+    pub unsafe fn dequantize(
+        ctx: &mut Context, stream: b200_stream, values: &TensorHandle, block_scales: Option<&TensorHandle>,
+        tensor_scale: Option<&TensorHandle>, scheme: &QuantScheme, output: &TensorHandle,
+    ) -> Result<(), Error> {
+        ctx.dequantize(
+            stream, scheme, output.dtype, values.ptr, block_scales.map_or(0, |t| t.ptr), tensor_scale.map_or(0, |t| t.ptr),
+            output.ptr, &output.shape,
+        )
     }
 }

@@ -75,6 +75,42 @@ pub enum CommOp {
     Mean = 1,
 }
 
+/// `b200_quant_value` = QuantValue (crates/cubecl-common/src/quant/scheme.rs:358-377), in its order.
+#[repr(i32)]
+#[derive(Clone, Copy, Debug, PartialEq, Eq)]
+pub enum QuantValue {
+    Q8F = 0,
+    E5M2 = 1,
+    E4M3 = 2,
+    Q4F = 3,
+    E2M1 = 4,
+    Q2F = 5,
+    Q8S = 6,
+    Q4S = 7,
+    Q2S = 8,
+}
+
+/// `b200_quant_scheme`: the value type, an optional block level (`block` values per scale stored as `block_scale`, one of
+/// F32 / F16 / BF16 / UE8M0 / F8E4M3 = ue4m3) and an optional per-tensor f32 level.
+#[derive(Clone, Copy, Debug, PartialEq, Eq)]
+pub struct QuantScheme {
+    pub value: QuantValue,
+    pub block: u32,
+    pub block_scale: DType,
+    pub tensor_scale: bool,
+}
+
+impl QuantScheme {
+    fn raw(&self) -> sys::b200_quant_scheme {
+        sys::b200_quant_scheme {
+            value: self.value as i32,
+            block: self.block as i32,
+            block_scale: self.block_scale as i32,
+            tensor_scale: self.tensor_scale as i32,
+        }
+    }
+}
+
 /// Activation of the fused GEMM epilogue (`b200_epilogue.activation`).
 #[repr(i32)]
 #[derive(Clone, Copy, Debug, PartialEq, Eq)]
@@ -349,6 +385,41 @@ impl Context {
         check(sys::b200_scan(
             self.0, stream, op as c_int, exclusive as c_int, in_dtype as c_int, out_dtype as c_int, input.ptr, out,
             input.shape.len() as c_int, input.shape.as_ptr(), input.strides.as_ptr(), axis as c_int,
+        ))
+    }
+
+    /// Quantize `input` ([..., K], F32 / F16 / BF16, any strides) along its innermost axis under `scheme` into compact
+    /// codes [..., K * bits / 8], block scales [..., K / block] and the f32 tensor scale (0 for an absent level); the
+    /// contract is `b200_quantize`'s in include/cubecl_b200.h.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::matmul`].
+    #[allow(clippy::too_many_arguments)]
+    pub unsafe fn quantize(
+        &mut self, stream: b200_stream, scheme: &QuantScheme, in_dtype: DType, input: &TensorView, values: b200_dptr,
+        block_scales: b200_dptr, tensor_scale: b200_dptr,
+    ) -> Result<(), Error> {
+        assert!(input.strides.len() == input.shape.len());
+        let raw = scheme.raw();
+        check(sys::b200_quantize(
+            self.0, stream, &raw, in_dtype as c_int, input.ptr, values, block_scales, tensor_scale, input.shape.len() as c_int,
+            input.shape.as_ptr(), input.strides.as_ptr(),
+        ))
+    }
+
+    /// out (compact, F32 / F16 / BF16) = the values of quantized codes of `shape` under `scheme` (`b200_dequantize`).
+    ///
+    /// # Safety
+    /// Same contract as [`Context::matmul`].
+    #[allow(clippy::too_many_arguments)]
+    pub unsafe fn dequantize(
+        &mut self, stream: b200_stream, scheme: &QuantScheme, out_dtype: DType, values: b200_dptr, block_scales: b200_dptr,
+        tensor_scale: b200_dptr, out: b200_dptr, shape: &[u64],
+    ) -> Result<(), Error> {
+        let raw = scheme.raw();
+        check(sys::b200_dequantize(
+            self.0, stream, &raw, out_dtype as c_int, values, block_scales, tensor_scale, out, shape.len() as c_int,
+            shape.as_ptr(),
         ))
     }
 
