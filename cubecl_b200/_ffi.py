@@ -54,6 +54,11 @@ class Props(C.Structure):
     ]
 
 
+class QuantOperand(C.Structure):
+    """b200_quant_operand: a quantized matmul operand (scheme, codes, block scales, device tensor scale)."""
+    _fields_ = [("scheme", QuantScheme), ("values", C.c_uint64), ("block_scales", C.c_uint64), ("tensor_scale", C.c_uint64)]
+
+
 _u64p = C.POINTER(C.c_uint64)
 _intp = C.POINTER(C.c_int)
 _vp = C.c_void_p
@@ -98,6 +103,8 @@ SIGNATURES = {
                                     _u64p, _u64p, _u64p, _u64p, _u64p, _u64p, C.POINTER(Epilogue)]),
     "b200_matmul_scaled": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64,
                                      C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64, C.c_int, C.c_int]),
+    "b200_matmul_quantized": (C.c_int, [_vp, _vp, C.POINTER(QuantOperand), C.POINTER(QuantOperand), C.c_int, C.c_uint64,
+                                        C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64]),
     "b200_reduce": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, C.c_uint64, C.c_int, _u64p, C.c_int]),
     "b200_reduce_strided": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, C.c_uint64, C.c_int, _u64p, _u64p, C.c_int]),
     "b200_reduce_debug": (C.c_int, [_vp, _vp, _u64p]),

@@ -40,6 +40,10 @@ extern const unsigned char b200_cubin_aux[];
 extern const unsigned char b200_cubin_aux_end[];
 extern const unsigned char b200_cubin_quant[];
 extern const unsigned char b200_cubin_quant_end[];
+extern const unsigned char b200_cubin_gemm_q[];
+extern const unsigned char b200_cubin_gemm_q_end[];
+extern const unsigned char b200_cubin_quant_mm[];
+extern const unsigned char b200_cubin_quant_mm_end[];
 }
 
 // ================================================================================================ errors
@@ -223,6 +227,8 @@ struct GemmParams {
   uint32_t fmt_b, fmt_mixed;       // rhs format of a mixed 8-bit pair
   uint32_t hyb, hyb_nba, hyb_nbb;  // hybrid f32 schedule: tf32 main product + two bf16 cross terms (gemm_wgmma.cu)
   uint32_t tma_store;              // whole tiles leave through shared-memory staging and TMA stores
+  uint32_t q_nsub, q_pad;          // quantized operands: scale blocks per 128-element stage (per-block kernels)
+  uint64_t q_ga, q_gb;             // quantized operands: device pointers of the two f32 tensor scales (per-tensor kernels)
 };
 struct ConvertF16Params {
   uint64_t in, out;
@@ -407,12 +413,14 @@ static int get_func(b200_ctx* c, const std::string& name, CUfunction* out) {
   if (c->dry) { c->pending_kernel = name; *out = nullptr; return B200_OK; }
   auto it = c->funcs.find(name);
   if (it != c->funcs.end()) { *out = it->second; return B200_OK; }
-  // modules are loaded in the order gemm, reduce, aux, gemm_b, gemm_c, quant; the kernel name says where a kernel lives (no
-  // failing lookups, which API-level tools such as compute-sanitizer would report)
+  // modules are loaded in the order gemm, reduce, aux, gemm_b, gemm_c, quant, gemm_q, quant_mm; the kernel name says where a
+  // kernel lives (no failing lookups, which API-level tools such as compute-sanitizer would report)
   auto starts = [&](const char* pfx) { return name.rfind(pfx, 0) == 0; };
   auto has = [&](const char* part) { return name.find(part) != std::string::npos; };
   const bool tc_gemm = starts("gemm_") && name != "gemm_simt_strided" && name != "gemm_scaled_simt";
-  const size_t home = starts("quant_") ? 5
+  const size_t home = starts("gemm_q8") ? 6
+                      : starts("quant_scales_") || starts("quant_widen_") ? 7
+                      : starts("quant_") ? 5
                       : tc_gemm && (has("_2sm_n128_") || has("_2sm_n224_")) ? 3
                       : tc_gemm && (has("_1sm_n128_") || has("_2sm_m512_")) ? 4
                       : tc_gemm || starts("wgmma_probe_") ? 0
@@ -437,7 +445,9 @@ extern "C" int b200_get_cubin(const char* name, const void** image, size_t* size
   else if (!strcmp(name, "gemm_b")) { b = b200_cubin_gemm_b; e = b200_cubin_gemm_b_end; }
   else if (!strcmp(name, "gemm_c")) { b = b200_cubin_gemm_c; e = b200_cubin_gemm_c_end; }
   else if (!strcmp(name, "quant")) { b = b200_cubin_quant; e = b200_cubin_quant_end; }
-  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant)", name);
+  else if (!strcmp(name, "gemm_q")) { b = b200_cubin_gemm_q; e = b200_cubin_gemm_q_end; }
+  else if (!strcmp(name, "quant_mm")) { b = b200_cubin_quant_mm; e = b200_cubin_quant_mm_end; }
+  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm)", name);
   *image = b;
   *size = static_cast<size_t>(e - b);
   return B200_OK;
@@ -490,7 +500,9 @@ extern "C" int b200_init(int device, b200_ctx** out) {
       (rc = load_module(c, b200_cubin_aux, b200_cubin_aux_end, "aux")) ||
       (rc = load_module(c, b200_cubin_gemm_b, b200_cubin_gemm_b_end, "gemm_b")) ||
       (rc = load_module(c, b200_cubin_gemm_c, b200_cubin_gemm_c_end, "gemm_c")) ||
-      (rc = load_module(c, b200_cubin_quant, b200_cubin_quant_end, "quant"))) {
+      (rc = load_module(c, b200_cubin_quant, b200_cubin_quant_end, "quant")) ||
+      (rc = load_module(c, b200_cubin_gemm_q, b200_cubin_gemm_q_end, "gemm_q")) ||
+      (rc = load_module(c, b200_cubin_quant_mm, b200_cubin_quant_mm_end, "quant_mm"))) {
     for (CUmodule m : c->modules) g_drv.cuModuleUnload_p(m);
     g_drv.cuDevicePrimaryCtxRelease_p(c->dev);
     return bail(rc);
@@ -886,6 +898,12 @@ static const GemmVariant kVariants[] = {{"2sm_n256", 2, 256, 4, 1.0, 1}, {"2sm_n
                                         {"2sm_n224", 2, 224, 4, 0.0, 1}};
 // alignment slack + operand ring (A: 128 * mt rows, B: block_n rows, 128 B of K each) + barrier block + TMA-store staging
 static unsigned gemm_smem_bytes(const GemmVariant& v) { return 1024 + v.stages * (16384 * v.mt + v.block_n * 128) + 1024 + 16384; }
+// The per-block quantized kernels (gemm_q8_*) add f32 scale tiles for (128 + block_n) rows x 4 blocks to every stage and run
+// the largest stage count that fits 227 KB (gemm_wgmma.cu: GEMM_Q).
+static int gemm_q8_stages(const GemmVariant& v) { return v.block_n == 256 ? 3 : 5; }
+static unsigned gemm_q8_smem_bytes(const GemmVariant& v) {
+  return 1024 + gemm_q8_stages(v) * (16384 + v.block_n * 128 + (128 + v.block_n) * 16) + 1024 + 16384;
+}
 
 static int encode_tmap(b200_ctx* c, CUtensorMap* out, CUtensorMapDataType dt, size_t esz, uint64_t base, uint64_t d0,
                        uint64_t d1, uint64_t d2, uint64_t s1_elems, uint64_t s2_elems, uint32_t b0, uint32_t b1,
@@ -945,9 +963,16 @@ struct GemmProblem {
   uint64_t a_sm, a_sk, a_sb;
   uint64_t b_sk, b_sn, b_sb;
   uint64_t o_sm, o_sn, o_sb;
+  // integer-quantized operands (b200_matmul_quantized): s8 codes, K-major.  q = 1: per-block scales folded per Bk block of K
+  // from the f32 effective-scale buffers sa_q / sb_q ([batch][K / Bk][rows padded to 4]); q = 2: per-tensor scales g_a, g_b
+  // read from the device in the epilogue
+  int q = 0;
+  uint32_t q_bk = 0;
+  uint64_t q_sa = 0, q_sb = 0, q_ga = 0, q_gb = 0;
 };
 
 static bool variant_has(const GemmVariant& v, const GemmProblem& g) {
+  if (g.q == 1 && v.block_n == 256) return false;   // the per-block fold has 128-wide tiles only (gemm_wgmma.cu: GEMM_Q)
   if (!strcmp(v.tag, "2sm_n224")) return g.mx;
   if (!strcmp(v.tag, "2sm_m512")) return !g.mx && (g.in_dtype == B200_BF16 || g.in_dtype == B200_F16);
   return true;
@@ -1099,7 +1124,7 @@ static const GemmVariant* pick_variant(b200_ctx* c, const GemmProblem& g, SkPlan
 
 static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_mn, bool b_mn) {
   const size_t esz = dtype_size(g.in_dtype), osz = dtype_size(g.out_dtype);
-  const char* in_tag = g.mx ? "mx" : g.in_dtype == B200_BF16 ? "bf16" : g.in_dtype == B200_F16 ? "f16" : g.in_dtype == B200_F8E4M3 ? "e4m3"
+  const char* in_tag = g.q == 1 ? "q8" : g.q == 2 ? "q8t" : g.mx ? "mx" : g.in_dtype == B200_BF16 ? "bf16" : g.in_dtype == B200_F16 ? "f16" : g.in_dtype == B200_F8E4M3 ? "e4m3"
                        : g.in_dtype == B200_F8E5M2 ? "e5m2" : g.in_dtype == B200_U8 ? "u8" : g.in_dtype == B200_I8 ? "s8" : "tf32";
   const char* out_tag = g.out_dtype == B200_BF16 ? "bf16" : g.out_dtype == B200_F16 ? "f16" : g.out_dtype == B200_I32 ? "i32" : "f32";
   const uint32_t block_k = static_cast<uint32_t>(128 / esz);
@@ -1115,7 +1140,7 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
   CUfunction f;
   int rc = get_func(c, name, &f);
   if (rc) return rc;
-  const unsigned smem = gemm_smem_bytes(v);
+  const unsigned smem = g.q == 1 ? gemm_q8_smem_bytes(v) : gemm_smem_bytes(v);
   if (!c->dry) CU_CHECK(g_drv.cuFuncSetAttribute_p(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem));
 
   const CUtensorMapDataType dt = g.in_dtype == B200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
@@ -1161,6 +1186,16 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
     if (rc) return rc;
     rc = encode_tmap(c, &tb_lo, dt, esz, g.b_lo, g.K, g.N, bb, pad16(g.K), pad16(g.K) * g.N, block_k, n_local);
     if (rc) return rc;
+  } else if (g.q == 1) {
+    // effective-scale tiles of one stage: [128 / Bk blocks][128 rows] of A, [128 / Bk][block_n] of B (no swizzle)
+    const uint64_t nblk = g.K / g.q_bk, ra = (g.M + 3) / 4 * 4, rb = (g.N + 3) / 4 * 4;
+    const uint32_t nsub = 128u / g.q_bk;
+    rc = encode_tmap(c, &ta_lo, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, g.q_sa, ra, nblk, a_bcast ? 1 : g.batch, ra, ra * nblk, 128, nsub,
+                     CU_TENSOR_MAP_SWIZZLE_NONE);
+    if (rc) return rc;
+    rc = encode_tmap(c, &tb_lo, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, g.q_sb, rb, nblk, b_bcast ? 1 : g.batch, rb, rb * nblk,
+                     (uint32_t)v.block_n, nsub, CU_TENSOR_MAP_SWIZZLE_NONE);
+    if (rc) return rc;
   }
 
   GemmParams p;
@@ -1175,6 +1210,8 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
     p.hyb_nba = a_bcast ? 1u : (uint32_t)g.batch;
     p.hyb_nbb = b_bcast ? 1u : (uint32_t)g.batch;
   }
+  if (g.q == 1) p.q_nsub = 128u / g.q_bk;
+  p.q_ga = g.q_ga; p.q_gb = g.q_gb;
   p.alpha = g.alpha; p.bias = g.bias; p.epi_act = g.act;
   p.epi_on = (g.alpha != 1.0f || g.bias != 0 || g.act != 0) ? 1u : 0u;
   p.out = g.out;
@@ -2436,6 +2473,134 @@ extern "C" int b200_dequantize(b200_ctx* c, b200_stream s, const b200_quant_sche
   if (grid > 0x7FFFFFFFull) return fail(B200_ERR_TOO_MANY_RESOURCES, "dequantize: %llu elements exceed one launch", (unsigned long long)n);
   void* args[] = {&p};
   return launch(c, f, (unsigned)grid, 1, 1, kQuantThreads, 0, 1, resolve_stream(c, s), args);
+}
+
+// ------------------------------------------------------------------------------------------------ quantized matmul
+// Kernels: csrc/quant.cu (QUANT_PART 1, parameter blocks mirrored there) and csrc/gemm_wgmma.cu (gemm_q8_*, gemm_q8t_*).
+struct QuantScalesParams {
+  uint64_t block_scales, tensor_scale, out;
+  uint64_t batch, rows, rows_pad, nblk;
+  uint32_t rep, pad;
+};
+struct QuantWidenParams {
+  uint64_t in, out;
+  uint64_t rows, K, pitch;
+  uint32_t bits, pad;
+};
+
+static const char* quant_scale_tag(int32_t dt) {
+  switch (dt) {
+    case B200_F32: return "f32";
+    case B200_F16: return "f16";
+    case B200_BF16: return "bf16";
+    case B200_UE8M0: return "ue8m0";
+    default: return "ue4m3";
+  }
+}
+
+// The codes of one operand as s8 rows TMA can read: Q8 codes in place (16-byte aligned base, K % 16 == 0) or through the
+// staging pass; Q4 / Q2 codes widened exactly to one s8 per element.  *tmp is the pooled buffer, if any.
+static int qmm_codes(b200_ctx* c, CUstream st, const b200_quant_operand* o, uint64_t batch, uint64_t rows, uint64_t K,
+                     CUdeviceptr* tmp, uint64_t* ptr, uint64_t* pitch) {
+  const uint32_t bits = quant_bits(o->scheme.value);
+  if (bits == 8) {
+    if (o->values % 16 == 0 && K % 16 == 0) { *ptr = o->values; *pitch = K; return B200_OK; }
+    uint64_t s_mn, s_k, s_b;
+    int rc = stage_operand(c, st, 1, o->values, batch, rows, K, K, 1, rows * K, tmp, &s_mn, &s_k, &s_b);
+    *ptr = *tmp; *pitch = s_mn;
+    return rc;
+  }
+  const uint64_t total_rows = batch * rows, pch = (K + 15) / 16 * 16;
+  int rc = pool_alloc(c, total_rows * pch, tmp, st);
+  if (rc) return rc;
+  CUfunction f;
+  rc = get_func(c, "quant_widen_s8", &f);
+  if (rc) return rc;
+  QuantWidenParams p{o->values, *tmp, total_rows, K, pch, bits, 0};
+  const uint64_t vecs = total_rows * (pch / 16);
+  const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(ceil_div(vecs, (uint64_t)kQuantThreads), (uint64_t)c->props.num_sms * 16));
+  void* args[] = {&p};
+  *ptr = *tmp; *pitch = pch;
+  return launch(c, f, grid, 1, 1, kQuantThreads, 0, 1, st, args);
+}
+
+// The f32 effective scales of one operand per GEMM block of bk elements, block-major [batch][K / bk][rows padded to 4].
+static int qmm_scales(b200_ctx* c, CUstream st, const b200_quant_operand* o, uint64_t batch, uint64_t rows, uint64_t K, uint32_t bk,
+                      CUdeviceptr* out) {
+  const uint64_t rows_pad = (rows + 3) / 4 * 4, nblk = K / bk, total = batch * nblk * rows_pad;
+  int rc = pool_alloc(c, total * 4, out, st);
+  if (rc) return rc;
+  const int32_t block = o->scheme.block;
+  CUfunction f;
+  rc = get_func(c, std::string("quant_scales_f32_") + (block ? quant_scale_tag(o->scheme.block_scale) : "tensor"), &f);
+  if (rc) return rc;
+  QuantScalesParams p{block ? o->block_scales : 0, o->tensor_scale, *out, batch, rows, rows_pad, nblk, block ? (uint32_t)block / bk : 1u, 0};
+  const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(ceil_div(total, (uint64_t)kQuantThreads), (uint64_t)c->props.num_sms * 16));
+  void* args[] = {&p};
+  return launch(c, f, grid, 1, 1, kQuantThreads, 0, 1, st, args);
+}
+
+extern "C" int b200_matmul_quantized(b200_ctx* c, b200_stream s, const b200_quant_operand* lhs, const b200_quant_operand* rhs,
+                                     b200_dtype out_dtype, b200_dptr out, uint64_t batch, uint64_t m, uint64_t n, uint64_t k) {
+  CTX_ENTER(c);
+  if (!lhs || !rhs) return fail(B200_ERR_INVALID_ARG, "matmul_quantized: null operand");
+  const bool empty = (batch == 0 || m == 0 || n == 0);
+  const b200_quant_operand* ops[2] = {lhs, rhs};
+  const uint64_t rows[2] = {m, n};
+  for (int i = 0; i < 2; ++i) {
+    const char* what = i == 0 ? "matmul_quantized (lhs)" : "matmul_quantized (rhs)";
+    const uint64_t shape[2] = {empty ? 0 : batch * rows[i], k};
+    uint64_t nel = 0, K = 0;
+    int rc = quant_check(what, &ops[i]->scheme, 2, shape, ops[i]->block_scales, ops[i]->tensor_scale, &nel, &K);
+    if (rc) return rc;
+    const int32_t v = ops[i]->scheme.value;
+    if (v == B200_QV_E4M3 || v == B200_QV_E5M2 || v == B200_QV_E2M1)
+      return fail(B200_ERR_UNSUPPORTED, "%s: minifloat values (e4m3 / e5m2 / e2m1) with block scales run through b200_matmul_scaled", what);
+    if (ops[i]->scheme.block == 8 || ops[i]->scheme.block == 16)
+      return fail(B200_ERR_UNSUPPORTED, "%s: block %d (32, 64 or 128: s8 wgmma consumes K in steps of 32)", what, (int)ops[i]->scheme.block);
+  }
+  if (out_dtype != B200_F32 && out_dtype != B200_BF16 && out_dtype != B200_F16)
+    return fail(B200_ERR_INVALID_ARG, "matmul_quantized: output dtype %d is not F32, BF16 or F16", (int)out_dtype);
+  if (empty) return B200_OK;
+  if (k == 0) return fail(B200_ERR_INVALID_ARG, "matmul_quantized: K must be positive");
+  const bool per_tensor = lhs->scheme.block == 0 && rhs->scheme.block == 0;
+  // |q| <= 128 on either side: one product is at most 2^14, so the exact s32 dot product over K needs K * 2^14 < 2^31
+  if (per_tensor && k >= (1ull << 17))
+    return fail(B200_ERR_UNSUPPORTED, "matmul_quantized: per-tensor x per-tensor needs K < 131072 (exact s32 dot products), K = %llu",
+                (unsigned long long)k);
+  if (!out || !lhs->values || !rhs->values) return fail(B200_ERR_INVALID_ARG, "matmul_quantized: null device pointer");
+  const size_t osz = dtype_size(out_dtype);
+  if (out % osz) return fail(B200_ERR_INVALID_ARG, "matmul_quantized: output pointer is not aligned to its element size");
+  if (m >= (1ull << 31) || n >= (1ull << 31) || k >= (1ull << 31) || batch >= (1ull << 20))
+    return fail(B200_ERR_UNSUPPORTED, "matmul_quantized: extent too large");
+  CUstream st = resolve_stream(c, s);
+  CUdeviceptr tmp[4] = {0, 0, 0, 0};   // lhs codes, rhs codes, lhs scales, rhs scales
+  uint64_t pa = 0, pb = 0, pitch_a = 0, pitch_b = 0;
+  int rc = qmm_codes(c, st, lhs, batch, m, k, &tmp[0], &pa, &pitch_a);
+  if (!rc) rc = qmm_codes(c, st, rhs, batch, n, k, &tmp[1], &pb, &pitch_b);
+  GemmProblem g{};
+  g.in_dtype = B200_I8; g.out_dtype = out_dtype;
+  g.a = pa; g.b = pb; g.out = out;
+  g.M = m; g.N = n; g.K = k; g.batch = batch;
+  g.a_sm = pitch_a; g.a_sk = 1; g.a_sb = batch > 1 ? m * pitch_a : 0;
+  g.b_sn = pitch_b; g.b_sk = 1; g.b_sb = batch > 1 ? n * pitch_b : 0;
+  g.o_sm = n; g.o_sn = 1; g.o_sb = batch > 1 ? m * n : 0;
+  if (per_tensor) {
+    g.q = 2;
+    g.q_ga = lhs->tensor_scale; g.q_gb = rhs->tensor_scale;
+  } else {
+    // kernel block: the finer of the present block levels; a coarser block repeats its scale, a per-tensor side uses g
+    const int32_t ba = lhs->scheme.block, bb = rhs->scheme.block;
+    g.q = 1;
+    g.q_bk = (uint32_t)(ba == 0 ? bb : bb == 0 ? ba : std::min(ba, bb));
+    if (!rc) rc = qmm_scales(c, st, lhs, batch, m, k, g.q_bk, &tmp[2]);
+    if (!rc) rc = qmm_scales(c, st, rhs, batch, n, k, g.q_bk, &tmp[3]);
+    g.q_sa = tmp[2]; g.q_sb = tmp[3];
+  }
+  if (!rc) rc = launch_wgmma(c, st, g, false, false);
+  for (CUdeviceptr t : tmp)
+    if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMM has drained
+  return rc;
 }
 
 // Stage timings (ns) of the most recent fused reduce + exchange launched with option reduce.debug=1 on stream `s`:

@@ -54,6 +54,10 @@ struct GemmParams {
   // 1: whole tiles leave through swizzled shared-memory staging and TMA stores (tma_out describes `out` as (N, M, batch),
   // [128 B x 64 rows] boxes); needs a 16-byte aligned base and row / batch pitches.  0: each thread stores its own fragment.
   uint32_t tma_store;
+  // Quantized operands (QM != 0, see gemm_body): q_nsub = 128 / Bk scale blocks per 128-element stage of K (per-block
+  // kernels); q_ga / q_gb = device pointers of the two f32 tensor scales (per-tensor kernels).
+  uint32_t q_nsub, q_pad;
+  uint64_t q_ga, q_gb;
 };
 
 enum : int { KIND_F16 = 0, KIND_BF16 = 1, KIND_TF32 = 2, KIND_E4M3 = 3, KIND_E5M2 = 4, KIND_U8 = 5, KIND_S8 = 6 };
@@ -172,10 +176,21 @@ __device__ __forceinline__ uint32_t acc_bits(uint32_t x) { return x; }
 // MT: 128-row sub-tiles of M per CTA.  MT = 2 (the 2sm_m512 pair tile, 512 x BLOCK_N per CTA pair) gives each consumer
 // warpgroup two m64 row blocks that share every B stage: per FLOP the pair reads a third less operand data from L2 than the
 // 256 x 256 tile at the same accumulator count per thread.
-template <int CG, int BLOCK_N, bool A_MN, bool B_MN, int KIND, int OUT, int STAGES, bool PROMOTE = false, int MT = 1>
+// QM (integer-quantized operands, s8 codes, K-major; capi.cpp: b200_matmul_quantized):
+//   QM_BLOCK   per-block scales.  Each Bk-element block j of K is summed exactly by wgmma into a fresh s32 partial, which is
+//              folded into f32 accumulators as acc = fma(f32(D_j), rn(eff_a[m, j] * eff_b[n, j]), acc) in increasing j.  The
+//              producer also loads the stage's f32 effective-scale tiles ([128/Bk][rows] boxes of a block-major buffer) through
+//              tma_a_lo / tma_b_lo into a region after the operand ring.
+//   QM_TENSOR  one f32 scale per side: the s8 mainloop into s32 accumulators; the epilogue stores rn(f32(D) * rn(g_a * g_b)).
+enum : int { QM_NONE = 0, QM_BLOCK = 1, QM_TENSOR = 2 };
+template <int CG, int BLOCK_N, bool A_MN, bool B_MN, int KIND, int OUT, int STAGES, bool PROMOTE = false, int MT = 1, int QM = QM_NONE>
 __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUtensorMap* tma_b_hi, const CUtensorMap* tma_a_lo,
                                           const CUtensorMap* tma_b_lo, const CUtensorMap* tma_out, const GemmParams& p) {
-  constexpr bool INT_ACC = (KIND == KIND_U8 || KIND == KIND_S8);
+  constexpr bool INT_ACC = (KIND == KIND_U8 || KIND == KIND_S8) && QM != QM_BLOCK;
+  static_assert(QM == QM_NONE || (KIND == KIND_S8 && !A_MN && !B_MN && !PROMOTE && MT == 1), "quantized operands: s8, K-major");
+  // per-block scale tiles of one stage, sized for the finest block (Bk = 32: four blocks per 128-element stage)
+  constexpr uint32_t SC_A_BYTES = (QM == QM_BLOCK) ? 128u * 4u * 4u : 0u;
+  constexpr uint32_t SC_STAGE_BYTES = (QM == QM_BLOCK) ? SC_A_BYTES + BLOCK_N * 4u * 4u : 0u;
   constexpr int ESZ = (KIND == KIND_TF32) ? 4 : (KIND >= KIND_E4M3) ? 1 : 2;
   static_assert(ESZ == 2 || (!A_MN && !B_MN), "wgmma reads MN-major operands for 16-bit kinds only");
   constexpr int BLOCK_K = 128 / ESZ;  // one 128-byte swizzle row of K per stage
@@ -199,7 +214,8 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bar_base = smem_base + STAGES * STAGE_BYTES;
+  const uint32_t sc_base = smem_base + STAGES * STAGE_BYTES;   // QM_BLOCK: per-stage [A scales | B scales]
+  const uint32_t bar_base = sc_base + STAGES * SC_STAGE_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
   const uint32_t split_flag = bar_base + 16u * STAGES;  // "this CTA reduces the slabs" broadcast among the consumer threads
@@ -214,6 +230,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
     tma_prefetch_desc(tma_a_hi);
     tma_prefetch_desc(tma_b_hi);
     if (p.k_segments > 1) { tma_prefetch_desc(tma_a_lo); tma_prefetch_desc(tma_b_lo); }
+    if constexpr (QM == QM_BLOCK) { tma_prefetch_desc(tma_a_lo); tma_prefetch_desc(tma_b_lo); }
     if (p.tma_store) tma_prefetch_desc(tma_out);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);        // one arrive.expect_tx by this CTA's producer; the peer's multicast bytes counted too
@@ -256,7 +273,17 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
           const uint32_t sa = smem_base + s * STAGE_BYTES;
           const uint32_t sb = sa + A_BYTES;
           const uint32_t fb = full_bar(s);
-          mbar_arrive_expect_tx(fb, STAGE_BYTES);
+          if constexpr (QM == QM_BLOCK) {
+            // the scale tiles of this stage: A rows of this CTA, and every column of the B tile (each CTA of a pair loads
+            // its own copy, no multicast)
+            mbar_arrive_expect_tx(fb, STAGE_BYTES + (128u + BLOCK_N) * 4u * p.q_nsub);
+            const uint32_t sc = sc_base + s * SC_STAGE_BYTES;
+            const int j0 = static_cast<int>(kk * p.q_nsub);
+            tma_load_3d(sc, tma_a_lo, fb, m0, j0, ba);
+            tma_load_3d(sc + SC_A_BYTES, tma_b_lo, fb, nb0, j0, bb);
+          } else {
+            mbar_arrive_expect_tx(fb, STAGE_BYTES);
+          }
           // B rows [rank * N_LOCAL, (rank + 1) * N_LOCAL) of the tile land at the same offset in both CTAs of a pair
           auto load_b = [&](uint32_t dst, const CUtensorMap* m, int c0, int c1, int c2) {
             if constexpr (CG == 2) tma_load_3d_mc(dst, m, fb, static_cast<uint16_t>(3), c0, c1, c2);
@@ -316,6 +343,8 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
     constexpr int KIND_OTHER = (KIND == KIND_E4M3) ? KIND_E5M2 : (KIND == KIND_E5M2) ? KIND_E4M3 : (KIND == KIND_U8) ? KIND_S8
                                : (KIND == KIND_S8) ? KIND_U8 : KIND;
     const uint32_t osz = (OUT == OUT_F32) ? 4 : 2;
+    float gab = 0.f;   // QM_TENSOR: rn(g_a * g_b), read once per CTA from the device
+    if constexpr (QM == QM_TENSOR) gab = __fmul_rn(__ldg(reinterpret_cast<const float*>(p.q_ga)), __ldg(reinterpret_cast<const float*>(p.q_gb)));
     Acc acc[MT][NACC];
     uint32_t s = 0, ph = 0;
     UnitIter it = unit_iter(cluster_id, n_clusters, num_kb);
@@ -325,7 +354,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
       uint32_t seg = 0, kk = 0;
       if constexpr (KIND == KIND_TF32) seg_of(wu.kb0, seg, kk);
       uint32_t prev = 0;
-      if constexpr (PROMOTE) {
+      if constexpr (PROMOTE || QM == QM_BLOCK) {
 #pragma unroll
         for (int i = 0; i < NACC; ++i) acc[0][i] = 0.f;
       }
@@ -354,6 +383,52 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
 #pragma unroll
             for (int i = 0; i < PH / 2; ++i) acc[0][PH / 2 * h + i] += part[i];
           }
+          release(s);
+        } else if constexpr (QM == QM_BLOCK) {
+          // per scale block j of the stage (K = 128 / nsub elements, 4 / nsub wgmma of K = 32), per 64-column part h:
+          // exact s32 partial, then the fold.  Rows r, r + 8 of the fragment and column pairs n, n + 1 read their scales
+          // from the stage's tiles ([nsub][128] row scales, [nsub][BLOCK_N] column scales).
+          const uint32_t sc = sc_base + s * SC_STAGE_BYTES;
+          const uint32_t row = cw * 64u + wq * 16u + (lane >> 2);
+          // straight-line code per block size (a run-time trip count around wgmma costs registers and spills)
+          auto fold_stage = [&](auto ns) {
+            constexpr uint32_t NSUB = decltype(ns)::value, KPER = 4u / NSUB;
+#pragma unroll
+            for (uint32_t j = 0; j < NSUB; ++j) {
+              float ra0, ra1;
+              asm volatile("ld.shared.f32 %0, [%1];" : "=f"(ra0) : "r"(sc + (j * 128u + row) * 4u) : "memory");
+              asm volatile("ld.shared.f32 %0, [%1];" : "=f"(ra1) : "r"(sc + (j * 128u + row + 8u) * 4u) : "memory");
+              const uint32_t scb = sc + SC_A_BYTES + (j * BLOCK_N + 2u * (lane & 3u)) * 4u;
+#pragma unroll
+              for (int h = 0; h < BLOCK_N / 64; ++h) {
+                uint32_t part[32];   // 64-column partials: 64 accumulators + 32 partials stay within the register budget
+                wgmma_fence();
+#pragma unroll
+                for (uint32_t k = 0; k < KPER; ++k) {
+                  const uint32_t kk2 = 2u * (j * KPER + k);
+                  wgmma_ss<64, KIND_S8, KIND_S8, 0, 0>(part, a_desc + kk2, b_desc + ((h * 64u * 128u) >> 4) + kk2, k != 0 ? 1u : 0u);
+                }
+                wgmma_commit();
+                wgmma_wait<0>();
+                wgmma_fence_operands(part);
+#pragma unroll
+                for (int g = 0; g < 8; ++g) {
+                  float cb0, cb1;
+                  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(cb0), "=f"(cb1) : "r"(scb + (h * 64u + 8u * g) * 4u) : "memory");
+                  const float sc4[4] = {__fmul_rn(ra0, cb0), __fmul_rn(ra0, cb1), __fmul_rn(ra1, cb0), __fmul_rn(ra1, cb1)};
+#pragma unroll
+                  for (int e = 0; e < 4; ++e) {
+                    // |D_j| < 2^22: the magic-number conversion is exact (s32 -> f32 in an integer add and an f32 subtract)
+                    const float d = __fsub_rn(__int_as_float(static_cast<int>(part[4 * g + e]) + 0x4B400000), 12582912.f);
+                    acc[0][32 * h + 4 * g + e] = __fmaf_rn(d, sc4[e], acc[0][32 * h + 4 * g + e]);
+                  }
+                }
+              }
+            }
+          };
+          if (p.q_nsub == 4) fold_stage(std::integral_constant<uint32_t, 4>{});
+          else if (p.q_nsub == 2) fold_stage(std::integral_constant<uint32_t, 2>{});
+          else fold_stage(std::integral_constant<uint32_t, 1>{});
           release(s);
         } else {
   #pragma unroll
@@ -399,7 +474,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
         }
         if (++s == STAGES) { s = 0; ph ^= 1; }
       }
-      if constexpr (!PROMOTE) {
+      if constexpr (!PROMOTE && QM != QM_BLOCK) {
         wgmma_wait<0>();
 #pragma unroll
         for (int mt = 0; mt < MT; ++mt) wgmma_fence_operands(acc[mt]);
@@ -411,7 +486,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
       const uint32_t c0 = tc.n_blk * BLOCK_N + 2u * (lane & 3u);
       // fused epilogue of fragment group j: v = {(r, n), (r, n + 1), (r + 8, n), (r + 8, n + 1)}
       auto epilogue = [&](uint32_t n, uint32_t (&v)[4]) {
-        if (!INT_ACC && p.epi_on) {
+        if (!INT_ACC && QM == QM_NONE && p.epi_on) {
           const float* bias = reinterpret_cast<const float*>(p.bias);
 #pragma unroll
           for (int e = 0; e < 4; ++e) {
@@ -436,9 +511,12 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
       };
       auto frag = [&](int mt, int j, uint32_t (&v)[4]) {
 #pragma unroll
-        for (int e = 0; e < 4; ++e) v[e] = acc_bits(acc[mt][4 * j + e]);
+        for (int e = 0; e < 4; ++e) {
+          if constexpr (QM == QM_TENSOR) v[e] = __float_as_uint(__fmul_rn(__int2float_rn(static_cast<int>(acc[mt][4 * j + e])), gab));
+          else v[e] = acc_bits(acc[mt][4 * j + e]);
+        }
       };
-      const bool partial = (MT == 1) && !INT_ACC && wu.partial;   // the host plans no stream-K head for these
+      const bool partial = (MT == 1) && !INT_ACC && QM == QM_NONE && wu.partial;   // the host plans no stream-K head for these
 
       if (!partial && p.tma_store) {
         // fragments -> (epilogue, convert) -> 128B-swizzled [64 rows x 128 B] staging tile -> one TMA store per 128-byte column
@@ -597,10 +675,30 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
   GEMM_KERNEL_P(gemm_mx_f16_##TILE##_kk, CG, BN, false, false, KIND_BF16, OUT_F16, STAGES, true)           \
   GEMM_KERNEL_P(gemm_mx_f32_##TILE##_kk, CG, BN, false, false, KIND_BF16, OUT_F32, STAGES, true)
 
-// The kernels are built as three cubins from this one source (cubecl_b200/build.py compiles them in parallel):
+// integer-quantized operands (s8 codes, capi.cpp: b200_matmul_quantized): gemm_q8_* fold per-block scales (QSTAGES stages
+// hold the scale tiles too), gemm_q8t_* apply two per-tensor scales in the epilogue
+#define GEMM_KERNEL_Q(NAME, CG, BN, OUT, STAGES, QM)                                                                  \
+  extern "C" __global__ void __launch_bounds__(kNumThreads, 1)                                                     \
+      NAME(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,                  \
+           const __grid_constant__ CUtensorMap tma_a_sc, const __grid_constant__ CUtensorMap tma_b_sc,            \
+           const __grid_constant__ CUtensorMap tma_out, const __grid_constant__ GemmParams p) {                    \
+    gemm_body<CG, BN, false, false, KIND_S8, OUT, STAGES, false, 1, QM>(&tma_a, &tma_b, &tma_a_sc, &tma_b_sc, &tma_out, p); \
+  }
+#define GEMM_Q8T(TILE, CG, BN, STAGES)                                                     \
+  GEMM_KERNEL_Q(gemm_q8t_bf16_##TILE##_kk, CG, BN, OUT_BF16, STAGES, QM_TENSOR)            \
+  GEMM_KERNEL_Q(gemm_q8t_f16_##TILE##_kk, CG, BN, OUT_F16, STAGES, QM_TENSOR)              \
+  GEMM_KERNEL_Q(gemm_q8t_f32_##TILE##_kk, CG, BN, OUT_F32, STAGES, QM_TENSOR)
+#define GEMM_Q(TILE, CG, BN, STAGES, QSTAGES)                                              \
+  GEMM_KERNEL_Q(gemm_q8_bf16_##TILE##_kk, CG, BN, OUT_BF16, QSTAGES, QM_BLOCK)             \
+  GEMM_KERNEL_Q(gemm_q8_f16_##TILE##_kk, CG, BN, OUT_F16, QSTAGES, QM_BLOCK)               \
+  GEMM_KERNEL_Q(gemm_q8_f32_##TILE##_kk, CG, BN, OUT_F32, QSTAGES, QM_BLOCK)               \
+  GEMM_Q8T(TILE, CG, BN, STAGES)
+
+// The kernels are built as four cubins from this one source (cubecl_b200/build.py compiles them in parallel):
 //   GEMM_PART 0 ("gemm")    256 x 256 pair tiles (2-CTA cluster, 128 x 256 per CTA) and the bf16 peak probe
 //   GEMM_PART 1 ("gemm_b")  256 x 128 pair tiles, 256 x 224 block-scaled pair tiles
 //   GEMM_PART 2 ("gemm_c")  128 x 128 single-CTA tiles, 512 x 128 pair tiles
+//   GEMM_PART 3 ("gemm_q")  the quantized-operand kernels of every tile
 #ifndef GEMM_PART
 #define GEMM_PART 0
 #endif
@@ -635,6 +733,14 @@ GEMM_M512(gemm_bf16_f32, KIND_BF16, OUT_F32)
 GEMM_M512(gemm_f16_f16, KIND_F16, OUT_F16)
 GEMM_M512(gemm_f16_f32, KIND_F16, OUT_F32)
 GEMM_M512(gemm_f16_bf16, KIND_F16, OUT_BF16)
+#endif
+#if GEMM_PART == 3
+// per-block stages carry (128 + BLOCK_N) x 16 B of scales: the largest count that fits 227 KB (capi.cpp: gemm_smem_bytes)
+// 2sm_n256 has the per-tensor kernels only: its 128 f32 accumulators and a partial exceed the 168 registers a thread of a
+// 384-thread CTA gets, and the per-block fold would spill
+GEMM_Q8T(2sm_n256, 2, 256, 4)
+GEMM_Q(2sm_n128, 2, 128, 6, 5)
+GEMM_Q(1sm_n128, 1, 128, 6, 5)
 #endif
 
 #if GEMM_PART == 0

@@ -472,10 +472,97 @@ __device__ __forceinline__ void decode_dispatch(const QuantDecodeParams& p) {
   else decode_body<ODT, 2>(p);
 }
 
-#define QUANT_KERNELS(tag, DT)                                                                                        \
+// Two cubins come from this source (cubecl_b200/build.py): QUANT_PART 0 ("quant") quantize / dequantize, QUANT_PART 1
+// ("quant_mm") the operand preparation of the quantized matmul.
+#ifndef QUANT_PART
+#define QUANT_PART 0
+#endif
+
+#if QUANT_PART == 1
+// ------------------------------------------------------------------------------------------------ quantized-matmul operands
+// (capi.cpp: b200_matmul_quantized, gemm_wgmma.cu: QM_BLOCK)
+struct QuantScalesParams {
+  uint64_t block_scales;  // [batch, rows, nblk / rep] in the block-scale dtype; unused by the per-tensor kernel
+  uint64_t tensor_scale;  // f32 [1] on the device, or 0
+  uint64_t out;           // f32 [batch][nblk][rows_pad], block-major: one TMA box per GEMM stage
+  uint64_t batch, rows, rows_pad, nblk;
+  uint32_t rep;           // GEMM blocks per stored block (this side's block / the GEMM's Bk)
+  uint32_t pad;
+};
+
+// The effective scale of GEMM block j of row r, as b200_dequantize defines it: f32(s), rn(g * f32(s)) with a tensor level,
+// or g for a per-tensor side.  A coarser block repeats its scale `rep` times; rows [rows, rows_pad) are written as 0.
+template <int DT>   // block-scale dtype, or -1 for a per-tensor side
+__device__ __forceinline__ void scales_body(const QuantScalesParams& p) {
+  const uint64_t total = p.batch * p.nblk * p.rows_pad;
+  const float g = p.tensor_scale ? __ldg(reinterpret_cast<const float*>(p.tensor_scale)) : 0.f;
+  for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += static_cast<uint64_t>(gridDim.x) * blockDim.x) {
+    const uint64_t r = i % p.rows_pad, t = i / p.rows_pad;
+    const uint64_t j = t % p.nblk, b = t / p.nblk;
+    float eff = 0.f;
+    if (r < p.rows) {
+      if constexpr (DT < 0) {
+        eff = g;
+      } else {
+        const uint64_t per_row = p.nblk / p.rep;
+        const float s = load_scale(p.block_scales, (b * p.rows + r) * per_row + j / p.rep, DT);
+        eff = p.tensor_scale ? __fmul_rn(g, s) : s;
+      }
+    }
+    reinterpret_cast<float*>(p.out)[i] = eff;
+  }
+}
+
+struct QuantWidenParams {
+  uint64_t in, out;       // in: compact code rows of K * bits / 8 bytes; out: s8 rows `pitch` bytes apart (16-byte multiple)
+  uint64_t rows, K, pitch;
+  uint32_t bits, pad;
+};
+
+// 4- and 2-bit code streams widened exactly to one s8 per element (sign extension, as b200_dequantize reads a field);
+// one thread writes 16 output bytes, the pitch padding as 0.
+__device__ __forceinline__ void widen_body(const QuantWidenParams& p) {
+  const uint64_t vpr = p.pitch / 16, total = p.rows * vpr;
+  const uint32_t bits = p.bits, sb = 1u << (bits - 1), mask = (1u << bits) - 1u;
+  const uint64_t row_bytes = p.K * bits / 8;
+  for (uint64_t t = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; t < total; t += static_cast<uint64_t>(gridDim.x) * blockDim.x) {
+    const uint64_t r = t / vpr, c0 = (t - r * vpr) * 16;
+    const uint64_t src = p.in + r * row_bytes + c0 * bits / 8;
+    const uint32_t nbytes = 2u * bits;   // 16 fields
+    uint64_t word = 0;
+    if (c0 + 16 <= p.K && (src & (nbytes - 1)) == 0) {
+      word = bits == 4 ? __ldg(reinterpret_cast<const unsigned long long*>(src)) : __ldg(reinterpret_cast<const unsigned int*>(src));
+    } else {
+      const uint64_t left = c0 < p.K ? (p.K - c0) * bits / 8 : 0;
+      for (uint32_t b = 0; b < nbytes; ++b)
+        if (b < left) word |= static_cast<uint64_t>(__ldg(reinterpret_cast<const unsigned char*>(src) + b)) << (8 * b);
+    }
+    uint32_t w[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+    for (int e = 0; e < 16; ++e) {
+      const uint32_t f = static_cast<uint32_t>(word >> (e * bits)) & mask;
+      const uint32_t s8 = c0 + e < p.K ? ((f ^ sb) - sb) & 0xFFu : 0u;
+      w[e / 4] |= s8 << (8 * (e % 4));
+    }
+    *reinterpret_cast<uint4*>(p.out + r * p.pitch + c0) = make_uint4(w[0], w[1], w[2], w[3]);
+  }
+}
+
+extern "C" __global__ void __launch_bounds__(256) quant_scales_f32_f32(const QuantScalesParams p) { scales_body<DT_F32>(p); }
+extern "C" __global__ void __launch_bounds__(256) quant_scales_f32_f16(const QuantScalesParams p) { scales_body<DT_F16>(p); }
+extern "C" __global__ void __launch_bounds__(256) quant_scales_f32_bf16(const QuantScalesParams p) { scales_body<DT_BF16>(p); }
+extern "C" __global__ void __launch_bounds__(256) quant_scales_f32_ue8m0(const QuantScalesParams p) { scales_body<DT_UE8M0>(p); }
+extern "C" __global__ void __launch_bounds__(256) quant_scales_f32_ue4m3(const QuantScalesParams p) { scales_body<DT_F8E4M3>(p); }
+extern "C" __global__ void __launch_bounds__(256) quant_scales_f32_tensor(const QuantScalesParams p) { scales_body<-1>(p); }
+extern "C" __global__ void __launch_bounds__(256) quant_widen_s8(const QuantWidenParams p) { widen_body(p); }
+#endif  // QUANT_PART == 1
+
+#if QUANT_PART == 0
+#define QUANT_KERNELS(tag, DT)                                                                                     \
   extern "C" __global__ void __launch_bounds__(256) quant_absmax_##tag(const QuantParams p) { absmax_body<DT>(p); }  \
   extern "C" __global__ void __launch_bounds__(256) quant_encode_##tag(const QuantParams p) { encode_body<DT>(p); }  \
   extern "C" __global__ void __launch_bounds__(256) quant_decode_##tag(const QuantDecodeParams p) { decode_dispatch<DT>(p); }
 QUANT_KERNELS(f32, DT_F32)
 QUANT_KERNELS(f16, DT_F16)
 QUANT_KERNELS(bf16, DT_BF16)
+#endif  // QUANT_PART == 0

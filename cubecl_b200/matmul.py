@@ -133,6 +133,36 @@ def launch_scaled(client: ComputeClient, lhs: TensorHandle, rhs: TensorHandle, l
         client._defer(e)
 
 
+def launch_quantized(client: ComputeClient, lhs, rhs, out: TensorHandle, stream=None) -> None:
+    """Matmul of two integer-quantized tensors (cubecl_b200.quant.QuantizedTensor) on the s8 tensor cores, scales applied
+    inside the GEMM: lhs [..., M, K] (activations) and rhs [..., N, K] (weights), both quantized along K with equal leading
+    dims (flattened into one batch); out [..., M, N] contiguous f32 / bf16 / f16 = sum_k deq(lhs)[.., m, k] * deq(rhs)[.., n, k].
+    Values q8f / q8s / q4f / q4s / q2f / q2s; per-tensor, per-block (32, 64, 128) or two-level scales on either side.  The
+    bit-exact arithmetic is stated in include/cubecl_b200.h (b200_matmul_quantized).  Errors are deferred to client.sync()."""
+    try:
+        ls, rs = list(lhs.shape), list(rhs.shape)
+        if len(ls) < 2 or len(ls) != len(rs) or ls[:-2] != rs[:-2]:
+            raise B200Error(6, f"matmul_quantized: lhs {ls} and rhs {rs} need rank >= 2 and equal leading dims")
+        if ls[-1] != rs[-1]:
+            raise B200Error(6, f"matmul_quantized: K mismatch (lhs {ls[-1]}, rhs {rs[-1]})")
+        M, N, K = ls[-2], rs[-2], ls[-1]
+        if list(out.shape) != ls[:-2] + [M, N] or not out.is_contiguous():
+            raise B200Error(6, f"matmul_quantized: out must be contiguous with shape {ls[:-2] + [M, N]}")
+        batch = int(np.prod(ls[:-2])) if len(ls) > 2 else 1
+        ops = []
+        for q in (lhs, rhs):
+            for t in (q.values, q.block_scales, q.tensor_scale):
+                if t is not None:
+                    t.handle.used_on(stream)
+            ops.append(_ffi.QuantOperand(q.scheme.to_c(), *(t.handle.ptr if t is not None else 0
+                                                              for t in (q.values, q.block_scales, q.tensor_scale))))
+        out.handle.used_on(stream)
+        _ffi.check(client._lib.b200_matmul_quantized(client._ctx, stream, C.byref(ops[0]), C.byref(ops[1]), DTYPES[out.dtype],
+                                                     C.c_uint64(out.handle.ptr), batch, M, N, K))
+    except B200Error as e:
+        client._defer(e)
+
+
 def launch_alloc(client: ComputeClient, lhs: TensorHandle, rhs: TensorHandle, out_dtype: str | None = None) -> TensorHandle:
     """Convenience: allocate `out` with the reference's shape rule, then launch."""
     shape = calculate_matmul_output(lhs.shape, rhs.shape)

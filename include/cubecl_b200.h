@@ -82,7 +82,7 @@ typedef struct b200_props {
 /* ---- lifecycle: R::client(device) -> DeviceService::init (cubecl-cuda/src/runtime.rs:52-350) ------------------------ */
 int b200_abi_version(void);
 int b200_device_count(int* count);
-/* The embedded prebuilt sm_90a images ("gemm" | "gemm_b" | "gemm_c" | "reduce" | "aux" | "quant"), for a host that prefers to cuModuleLoadData them into
+/* The embedded prebuilt sm_90a images ("gemm" | "gemm_b" | "gemm_c" | "reduce" | "aux" | "quant" | "gemm_q" | "quant_mm"), for a host that prefers to cuModuleLoadData them into
  * its own module cache (CudaContext::modules, crates/cubecl-cuda/src/compute/context.rs:38-62,293). No GPU needed. */
 int b200_get_cubin(const char* name, const void** image, size_t* size);
 int b200_init(int device, b200_ctx** out);   /* cuInit, primary ctx retain, load the embedded sm_90a cubins (context.rs:293) */
@@ -284,6 +284,34 @@ int b200_quantize(b200_ctx* ctx, b200_stream s, const b200_quant_scheme* scheme,
 int b200_dequantize(b200_ctx* ctx, b200_stream s, const b200_quant_scheme* scheme, b200_dtype out_dtype,
                     b200_dptr values, b200_dptr block_scales, b200_dptr tensor_scale, b200_dptr out,
                     int rank, const uint64_t* shape);
+
+/* ---- matmul of integer-quantized operands on the s8 tensor cores, scales applied inside the GEMM ----------------------------
+ * out[b, m, n] = sum_k deq(lhs)[b, m, k] * deq(rhs)[b, n, k]; lhs holds codes [batch, M, K], rhs [batch, N, K], both quantized
+ * along K exactly as b200_quantize writes them (values, block_scales, tensor_scale as there); out is [batch, M, N] contiguous
+ * in F32 / BF16 / F16.  Values Q8F / Q8S / Q4F / Q4S / Q2F / Q2S, independently per side (Q8 bytes feed the tensor cores, Q4 / Q2
+ * codes are first widened exactly to one s8 per element); per-tensor, per-block (32, 64, 128) or two-level on either side, every
+ * block-scale dtype b200_dequantize reads.  Tensor scales are read on the device: no host sync, b200_quantize and this call
+ * may be enqueued back to back.
+ * Arithmetic (bit-exact; integer fields sign-extended as b200_dequantize reads them).  eff_x[b, r, j] is the effective scale of
+ * block j of row r as b200_dequantize defines it: f32(s), rn(g * f32(s)) with two levels, g for a per-tensor side.
+ *   Per-block (either side has a block level): Bk = the smaller present block; a coarser block repeats its scale and a
+ *   per-tensor side uses g for every block.  D_j = the exact integer dot product over block j (|D_j| <= 2^21).  Blocks fold in
+ *   increasing j: acc_0 = 0, acc_{j+1} = fma(f32(D_j), rn(eff_a[m, j] * eff_b[n, j]), acc_j); out = RNE(acc_J).
+ *   Per-tensor x per-tensor: D = the exact s32 dot product over K (needs K < 131072); out = RNE(rn(rn(f32(D)) * rn(g_a * g_b))).
+ *   NaN and inf scales propagate as IEEE says.  No stream-K head runs: every output is one serial fold, reproducible bit for bit.
+ * Errors: B200_ERR_INVALID_ARG for K not divisible by a block, a null pointer for a present level or a non-null one for an absent
+ * level, an unknown value or dtype, K == 0 with a non-empty output; B200_ERR_UNSUPPORTED for minifloat values (use
+ * b200_matmul_scaled), blocks of 8 or 16, and per-tensor x per-tensor with K >= 131072.  batch, M or N of 0 is a no-op.
+ * Launches: per-tensor x per-tensor 1; per-block 2 scale passes + 1 GEMM; +1 per Q4 / Q2 operand (widening) and per Q8 operand
+ * TMA cannot read in place (base not 16-byte aligned or K % 16 != 0: staging).  Temporaries come from the pool, stream-ordered. */
+typedef struct b200_quant_operand {
+  b200_quant_scheme scheme;   /* as passed to b200_quantize */
+  b200_dptr values;           /* codes [batch, rows, K * bits / 8], the compact bit stream b200_quantize writes */
+  b200_dptr block_scales;     /* [batch, rows, K / block] in scheme.block_scale, or 0 when block == 0 */
+  b200_dptr tensor_scale;     /* f32[1] ON THE DEVICE, or 0 when the scheme has no tensor level */
+} b200_quant_operand;
+int b200_matmul_quantized(b200_ctx* ctx, b200_stream s, const b200_quant_operand* lhs, const b200_quant_operand* rhs,
+                          b200_dtype out_dtype, b200_dptr out, uint64_t batch, uint64_t m, uint64_t n, uint64_t k);
 
 /* ---- collectives: ServerCommunication (server/base.rs:632-739), CUDA impl cubecl-cuda/src/compute/server.rs:666-926 -- */
 #define B200_UNIQUE_ID_BYTES 128

@@ -210,6 +210,14 @@ inline void launch_scaled(ComputeClient& client, const TensorHandle& lhs, const 
                                     scales_packed ? 1 : 0);
   if (rc != B200_OK) client.defer(b200_last_error());
 }
+/// out (contiguous [batch, m, n], F32 / BF16 / F16) = deq(lhs) x deq(rhs)^T of two integer-quantized operands on the s8 tensor
+/// cores, scales applied inside the GEMM; see b200_matmul_quantized in cubecl_b200.h for the contract. Errors deferred.
+inline void launch_quantized(ComputeClient& client, const b200_quant_operand& lhs, const b200_quant_operand& rhs, const TensorHandle& out,
+                             uint64_t batch, uint64_t m, uint64_t n, uint64_t k) {
+  const int rc = b200_matmul_quantized(client.raw(), nullptr, &lhs, &rhs, static_cast<b200_dtype>(out.dtype), out.handle.ptr(),
+                                       batch, m, n, k);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
 }  // namespace matmul
 
 namespace reduce {

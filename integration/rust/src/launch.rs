@@ -6,7 +6,7 @@
 //! Inside cubecl-cuda the `Context` is owned by `CudaServer` and `TensorHandle::ptr` is what `BufferBinding` resolves to
 //! on the runner thread (INTEGRATION.md section 3); standalone, it is a pointer from `Context::alloc`.
 
-use crate::{b200_dptr, b200_stream, Context, DType, Error, Epilogue, QuantScheme, ReduceOp, Status, TensorView};
+use crate::{b200_dptr, b200_stream, Context, DType, Error, Epilogue, QuantOperand, QuantScheme, ReduceOp, Status, TensorView};
 
 /// Buffer + shape + strides (in ELEMENTS) + dtype: `TensorHandle<R>` of crates/cubecl-std/src/tensor/handle.rs:13-23
 /// with the `Handle` already resolved to a device pointer.
@@ -114,6 +114,37 @@ pub mod matmul {
             return Err(invalid(format!("out shape {:?} != {:?}", out.shape, expect)));
         }
         ctx.matmul_fused(stream, lhs.dtype, out.dtype, &lhs.view(), &rhs.view(), &out.view(), epilogue)
+    }
+
+    /// One integer-quantized matmul operand: codes [.., rows, K * bits / 8] and its scales (`None` for an absent level).
+    pub struct QuantizedTensor<'a> {
+        pub scheme: &'a QuantScheme,
+        pub values: &'a TensorHandle,
+        pub block_scales: Option<&'a TensorHandle>,
+        pub tensor_scale: Option<&'a TensorHandle>,
+    }
+
+    /// `matmul::launch_quantized(client, lhs, rhs, out)`: lhs [.., M, K] and rhs [.., N, K] quantized along K (K elements:
+    /// `k`), equal leading dims flattened into one batch; out [.., M, N] contiguous F32 / BF16 / F16.
+    ///
+    /// # Safety
+    /// As [`launch`].
+    pub unsafe fn launch_quantized(
+        ctx: &mut Context, stream: b200_stream, lhs: &QuantizedTensor, rhs: &QuantizedTensor, out: &TensorHandle, k: u64,
+    ) -> Result<(), Error> {
+        let r = out.shape.len();
+        if r < 2 || lhs.values.shape.len() != r || rhs.values.shape.len() != r || lhs.values.shape[..r - 2] != rhs.values.shape[..r - 2] {
+            return Err(invalid("lhs [.., M, K] and rhs [.., N, K] need the rank of out and equal leading dims".to_string()));
+        }
+        let (m, n) = (lhs.values.shape[r - 2], rhs.values.shape[r - 2]);
+        let batch: u64 = out.shape[..r - 2].iter().product();
+        let op = |q: &QuantizedTensor| QuantOperand {
+            scheme: *q.scheme,
+            values: q.values.ptr,
+            block_scales: q.block_scales.map_or(0, |t| t.ptr),
+            tensor_scale: q.tensor_scale.map_or(0, |t| t.ptr),
+        };
+        ctx.matmul_quantized(stream, &op(lhs), &op(rhs), out.dtype, out.ptr, batch, m, n, k)
     }
 }
 

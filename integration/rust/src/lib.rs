@@ -111,6 +111,27 @@ impl QuantScheme {
     }
 }
 
+/// `b200_quant_operand`: one operand of [`Context::matmul_quantized`], its codes and scales as `b200_quantize` wrote them
+/// (0 for an absent level; the tensor scale stays on the device).
+#[derive(Clone, Copy, Debug)]
+pub struct QuantOperand {
+    pub scheme: QuantScheme,
+    pub values: b200_dptr,
+    pub block_scales: b200_dptr,
+    pub tensor_scale: b200_dptr,
+}
+
+impl QuantOperand {
+    fn raw(&self) -> sys::b200_quant_operand {
+        sys::b200_quant_operand {
+            scheme: self.scheme.raw(),
+            values: self.values,
+            block_scales: self.block_scales,
+            tensor_scale: self.tensor_scale,
+        }
+    }
+}
+
 /// Activation of the fused GEMM epilogue (`b200_epilogue.activation`).
 #[repr(i32)]
 #[derive(Clone, Copy, Debug, PartialEq, Eq)]
@@ -421,6 +442,21 @@ impl Context {
             self.0, stream, &raw, out_dtype as c_int, values, block_scales, tensor_scale, out, shape.len() as c_int,
             shape.as_ptr(),
         ))
+    }
+
+    /// out [batch, m, n] (contiguous, F32 / BF16 / F16) = deq(lhs) x deq(rhs)^T of two integer-quantized operands, codes
+    /// [batch, m | n, k] quantized along k, on the s8 tensor cores with the scales applied inside the GEMM; the bit-exact
+    /// contract is `b200_matmul_quantized`'s in include/cubecl_b200.h.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::matmul`].
+    #[allow(clippy::too_many_arguments)]
+    pub unsafe fn matmul_quantized(
+        &mut self, stream: b200_stream, lhs: &QuantOperand, rhs: &QuantOperand, out_dtype: DType, out: b200_dptr, batch: u64,
+        m: u64, n: u64, k: u64,
+    ) -> Result<(), Error> {
+        let (a, b) = (lhs.raw(), rhs.raw());
+        check(sys::b200_matmul_quantized(self.0, stream, &a, &b, out_dtype as c_int, out, batch, m, n, k))
     }
 
     /// out (compact row-major) = gather of the strided tensor `input` (into_contiguous, cubecl-std/src/tensor/contiguous.rs).
