@@ -72,11 +72,11 @@ def build(force: bool = False, verbose: bool = False) -> Path:
         return LIB
     nvcc = _nvcc()
 
-    # every cubin is rebuilt only when ITS inputs changed (source, the shared PTX header, the flags): editing reduce.cu does not
+    # every cubin is rebuilt only when ITS inputs changed (source, the shared headers, the flags): editing reduce.cu does not
     # cost the five minutes of ptxas the GEMM instantiations take
     def inputs_digest(src, extra):
         h = hashlib.sha256(" ".join(NVCC_FLAGS + list(extra)).encode())
-        for f in (CSRC / src, CSRC / "ptx.cuh"):
+        for f in (CSRC / src, CSRC / "ptx.cuh", CSRC / "kernel_params.h", ROOT / "include" / "cubecl_b200.h"):
             h.update(f.read_bytes())
         return h.hexdigest()
 
@@ -106,7 +106,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     asm.append('.section .note.GNU-stack,"",@progbits\n')
     embed = BUILD / "embed.S"
     embed.write_text("".join(asm))
-    _run(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-Wall", "-Wno-unused-function", "-I", _cuda_include(),
+    _run(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-Wall", "-I", _cuda_include(),
           str(CSRC / "capi.cpp"), str(embed), "-ldl", "-lpthread", "-o", str(LIB)])
     # C++ host-layer example (include/cubecl_b200.hpp): compiled here so the header cannot rot; run on the GPU box by
     # tests/test_cpp_host_gpu.py

@@ -14,6 +14,8 @@
 #include <mma.h>
 #include <cstdint>
 
+#include "kernel_params.h"
+
 // ------------------------------------------------------------------------------------------------ generators
 // splitmix64 finaliser over (seed, index); the numpy mirror lives in cubecl_b200/synth.py.
 __device__ __forceinline__ uint32_t hash_u32(uint64_t seed, uint64_t i) {
@@ -29,54 +31,33 @@ __device__ __forceinline__ float hash_uniform(uint64_t seed, uint64_t i, float l
   return __fadd_rn(lo, __fmul_rn(u, scale));
 }
 
-struct FillParams {
-  uint64_t out, n, seed;
-  float lo, scale;     // value = lo + u * scale
-  uint32_t dtype;      // b200_dtype: 0 f32, 1 f16, 2 bf16, 10 fp8 e4m3, 11 fp8 e5m2
-  uint32_t mode;       // 0 uniform hash, 1 (i % modulus) as a number
-  uint32_t modulus, pad;
-};
-
 extern "C" __global__ void __launch_bounds__(256) fill_kernel(const __grid_constant__ FillParams p) {
   for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < p.n;
        i += static_cast<uint64_t>(gridDim.x) * blockDim.x) {
     const float v = (p.mode == 0) ? hash_uniform(p.seed, i, p.lo, p.scale) : static_cast<float>(i % p.modulus);
-    if (p.dtype == 0) reinterpret_cast<float*>(p.out)[i] = v;
-    else if (p.dtype == 1) reinterpret_cast<__half*>(p.out)[i] = __float2half_rn(v);
-    else if (p.dtype == 2) reinterpret_cast<__nv_bfloat16*>(p.out)[i] = __float2bfloat16_rn(v);
-    else reinterpret_cast<uint8_t*>(p.out)[i] = __nv_cvt_float_to_fp8(v, __NV_SATFINITE, p.dtype == 10 ? __NV_E4M3 : __NV_E5M2);
+    if (p.dtype == B200_F32) reinterpret_cast<float*>(p.out)[i] = v;
+    else if (p.dtype == B200_F16) reinterpret_cast<__half*>(p.out)[i] = __float2half_rn(v);
+    else if (p.dtype == B200_BF16) reinterpret_cast<__nv_bfloat16*>(p.out)[i] = __float2bfloat16_rn(v);
+    else reinterpret_cast<uint8_t*>(p.out)[i] = __nv_cvt_float_to_fp8(v, __NV_SATFINITE, p.dtype == B200_F8E4M3 ? __NV_E4M3 : __NV_E5M2);
   }
 }
 
 // ------------------------------------------------------------------------------------------------ strided SIMT matmul
-struct SimtGemmParams {
-  uint64_t a, b, out;
-  uint64_t a_sb, a_sm, a_sk;  // strides in elements: batch, m, k
-  uint64_t b_sb, b_sk, b_sn;
-  uint64_t o_sb, o_sm, o_sn;
-  uint32_t M, N, K, batch;
-  uint32_t in_dtype, out_dtype;  // b200_dtype: 0 f32, 1 f16, 2 bf16; inputs also 10 fp8 e4m3, 11 fp8 e5m2
-  uint64_t bias;                 // fused epilogue, same meaning as GemmParams
-  float alpha;
-  uint32_t epi_act, epi_on;
-  uint32_t b_dtype_p1;           // rhs dtype + 1 when it differs from in_dtype (mixed fp8 / int8 pairs), 0 = same as lhs
-};
-
 __device__ __forceinline__ float load_as_f32(uint64_t base, uint64_t idx, uint32_t dt) {
-  if (dt == 0) return reinterpret_cast<const float*>(base)[idx];
-  if (dt == 1) return __half2float(reinterpret_cast<const __half*>(base)[idx]);
-  if (dt == 2) return __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(base)[idx]);
-  const __half_raw h = __nv_cvt_fp8_to_halfraw(reinterpret_cast<const uint8_t*>(base)[idx], dt == 10 ? __NV_E4M3 : __NV_E5M2);
+  if (dt == B200_F32) return reinterpret_cast<const float*>(base)[idx];
+  if (dt == B200_F16) return __half2float(reinterpret_cast<const __half*>(base)[idx]);
+  if (dt == B200_BF16) return __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(base)[idx]);
+  const __half_raw h = __nv_cvt_fp8_to_halfraw(reinterpret_cast<const uint8_t*>(base)[idx], dt == B200_F8E4M3 ? __NV_E4M3 : __NV_E5M2);
   return __half2float(__half(h));
 }
 __device__ __forceinline__ void store_from_f32(uint64_t base, uint64_t idx, uint32_t dt, float v) {
-  if (dt == 0) reinterpret_cast<float*>(base)[idx] = v;
-  else if (dt == 1) reinterpret_cast<__half*>(base)[idx] = __float2half_rn(v);
+  if (dt == B200_F32) reinterpret_cast<float*>(base)[idx] = v;
+  else if (dt == B200_F16) reinterpret_cast<__half*>(base)[idx] = __float2half_rn(v);
   else reinterpret_cast<__nv_bfloat16*>(base)[idx] = __float2bfloat16_rn(v);
 }
 
 __device__ __forceinline__ int load_as_i32(uint64_t base, uint64_t idx, uint32_t dt) {
-  return dt == 8 ? static_cast<int>(reinterpret_cast<const uint8_t*>(base)[idx]) : static_cast<int>(reinterpret_cast<const int8_t*>(base)[idx]);
+  return dt == B200_U8 ? static_cast<int>(reinterpret_cast<const uint8_t*>(base)[idx]) : static_cast<int>(reinterpret_cast<const int8_t*>(base)[idx]);
 }
 
 extern "C" __global__ void __launch_bounds__(256) gemm_simt_strided(const __grid_constant__ SimtGemmParams p) {
@@ -84,7 +65,7 @@ extern "C" __global__ void __launch_bounds__(256) gemm_simt_strided(const __grid
   __shared__ float sb[16][17];
   const uint32_t tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
   const uint32_t n = blockIdx.x * 16 + tx, bz = blockIdx.z;
-  const bool integer = (p.in_dtype == 8 || p.in_dtype == 9);  // u8 / i8 -> exact s32 accumulation
+  const bool integer = (p.in_dtype == B200_U8 || p.in_dtype == B200_I8);  // exact s32 accumulation
   // 16-row tiles of M are walked with a stride of gridDim.y (the y extent of a grid stops at 65535)
   for (uint64_t mt = blockIdx.y; mt * 16 < p.M; mt += gridDim.y) {
   const uint32_t m = static_cast<uint32_t>(mt * 16) + ty;
@@ -131,97 +112,13 @@ extern "C" __global__ void __launch_bounds__(256) gemm_simt_strided(const __grid
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Block-scaled (MX) support.
-//
-// pack_scales: ue8m0 scales in the reference's layout -- [batch, rows, n_scales] row-major, one scale per row per 32 K
-// elements (test_cmma_scaled: crates/cubecl-core/src/runtime_tests/cmma.rs:1518-1533) -- to the tensor core's packed form:
-// [batch * tiles][atoms][512 B], tile = 128 rows, atom = 4 consecutive scales, byte (r % 32) * 16 + (r / 32) * 4 + s.
-// Rows / scales beyond the tensor are written as 1.0 (127 / 0x38), so padded K blocks multiply TMA's zero fill by a finite value.
-struct PackScalesParams {
-  uint64_t in, out;
-  uint32_t batch, rows, n_scales, tiles, atoms, pad_value;  // pad_value: the scale byte that means 1.0 (127 ue8m0, 0x38 ue4m3)
-  // `tiles` counts 128-row CHUNKS per batch entry.  A GEMM tile of `tile_rows` rows owns `chunks_per_tile` consecutive chunks
-  // (128 / 1: the plain layout; 224 / 2 for the 256 x 224 variant: chunk 2t holds rows [224 t, 224 t + 128), chunk 2t + 1 rows
-  // [224 t + 128, 224 t + 224) and padding), so a tile's 32-row groups always start a chunk.
-  uint32_t tile_rows, chunks_per_tile;
-};
-
-extern "C" __global__ void __launch_bounds__(256) pack_scales(const __grid_constant__ PackScalesParams p) {
-  // one 32-bit word = the 4 scales (one k atom) of one row.  Threads walk (chunk, row, atom) with the atom fastest, so the
-  // row-major input is read coalesced (whole words when the rows allow it); the scattered side is the 4-byte stores
-  const uint64_t words = static_cast<uint64_t>(p.batch) * p.tiles * p.atoms * 128;
-  const uint8_t* in = reinterpret_cast<const uint8_t*>(p.in);
-  uint32_t* out = reinterpret_cast<uint32_t*>(p.out);
-  const bool word_rows = (p.n_scales % 4 == 0) && (p.in % 4 == 0);
-  const uint32_t pad_word = p.pad_value * 0x01010101u;
-  if ((p.n_scales % 32 == 0) && (p.in % 16 == 0) && (p.atoms % 8 == 0) && (p.out % 16 == 0)) {
-    // Rows of whole 32-byte groups (K a multiple of 1024 / 512 elements): one warp per (chunk, 8 atoms), lane = row % 32.
-    // Each lane reads the 32 bytes (8 atoms) of its four rows r, r + 32, r + 64, r + 96 -- whole sectors -- and the warp writes
-    // each atom as one contiguous 512-byte chunk (lane r: the 16 bytes {row group 0..3} of that atom).  The word-per-thread
-    // form below scatters 4-byte stores 512 bytes apart (every 32-byte sector assembled from eight far-apart writes).
-    const uint32_t lane = threadIdx.x & 31;
-    const uint32_t groups = p.atoms / 8;
-    const uint64_t n_warps = static_cast<uint64_t>(p.batch) * p.tiles * groups;
-    const uint64_t warp0 = (blockIdx.x * static_cast<uint64_t>(blockDim.x) + threadIdx.x) >> 5, wstep = (static_cast<uint64_t>(gridDim.x) * blockDim.x) >> 5;
-    for (uint64_t w = warp0; w < n_warps; w += wstep) {
-      const uint32_t group = static_cast<uint32_t>(w % groups);
-      const uint64_t t2 = w / groups;
-      const uint32_t tile = static_cast<uint32_t>(t2 % p.tiles), b = static_cast<uint32_t>(t2 / p.tiles);
-      uint32_t wd[4][8];
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        const uint32_t lr = lane + 32u * g;
-        const uint32_t local = (tile % p.chunks_per_tile) * 128 + lr;
-        const uint32_t row = (tile / p.chunks_per_tile) * p.tile_rows + local;
-        if (local < p.tile_rows && row < p.rows && group * 32u < p.n_scales) {
-          const uint4* src = reinterpret_cast<const uint4*>(in + (static_cast<uint64_t>(b) * p.rows + row) * p.n_scales + group * 32ull);
-          const uint4 x = __ldg(src), y = __ldg(src + 1);
-          wd[g][0] = x.x; wd[g][1] = x.y; wd[g][2] = x.z; wd[g][3] = x.w;
-          wd[g][4] = y.x; wd[g][5] = y.y; wd[g][6] = y.z; wd[g][7] = y.w;
-        } else {
-#pragma unroll
-          for (int a = 0; a < 8; ++a) wd[g][a] = pad_word;
-        }
-      }
-      uint4* dst = reinterpret_cast<uint4*>(out) + ((static_cast<uint64_t>(b) * p.tiles + tile) * p.atoms + group * 8ull) * 32 + lane;
-#pragma unroll
-      for (int a = 0; a < 8; ++a) dst[a * 32] = make_uint4(wd[0][a], wd[1][a], wd[2][a], wd[3][a]);
-    }
-    return;
-  }
-  for (uint64_t w = blockIdx.x * static_cast<uint64_t>(blockDim.x) + threadIdx.x; w < words; w += static_cast<uint64_t>(gridDim.x) * blockDim.x) {
-    const uint32_t atom = static_cast<uint32_t>(w % p.atoms);
-    const uint64_t t1 = w / p.atoms;
-    const uint32_t lr = static_cast<uint32_t>(t1 % 128);                        // row inside the 128-row chunk
-    const uint64_t t2 = t1 / 128;
-    const uint32_t tile = static_cast<uint32_t>(t2 % p.tiles), b = static_cast<uint32_t>(t2 / p.tiles);
-    const uint32_t local = (tile % p.chunks_per_tile) * 128 + lr;               // row inside the GEMM tile
-    const uint32_t row = (tile / p.chunks_per_tile) * p.tile_rows + local;
-    uint32_t word = pad_word;
-    if (local < p.tile_rows && row < p.rows) {
-      const uint64_t base = (static_cast<uint64_t>(b) * p.rows + row) * p.n_scales + atom * 4ull;
-      if (word_rows && atom * 4u + 3u < p.n_scales) {
-        word = *reinterpret_cast<const uint32_t*>(in + base);
-      } else {
-        word = 0;
-#pragma unroll
-        for (uint32_t sidx = 0; sidx < 4; ++sidx) {
-          const uint32_t ks = atom * 4 + sidx;
-          const uint32_t v = (ks < p.n_scales) ? in[base + sidx] : p.pad_value;
-          word |= v << (8 * sidx);
-        }
-      }
-    }
-    out[((static_cast<uint64_t>(b) * p.tiles + tile) * p.atoms + atom) * 128 + (lr % 32) * 4 + lr / 32] = word;
-  }
-}
-
 __device__ __forceinline__ float ue8m0_to_f32(uint32_t bits) {
   if (bits == 255u) return __uint_as_float(0x7FC00000u);      // NaN
   if (bits == 0u) return __uint_as_float(0x00400000u);        // 2^-127 (an f32 subnormal)
   return __uint_as_float(bits << 23);
 }
 __device__ __forceinline__ float mx_elem_to_f32(uint64_t base, uint64_t idx, uint32_t dt) {
-  if (dt == 12) {  // packed e2m1: element 2i in the low nibble of byte i (e2m1x2::from_f32_slice, cubecl-common/src/float/fp4.rs:204-216)
+  if (dt == B200_F4E2M1X2) {  // packed e2m1: element 2i in the low nibble of byte i (e2m1x2::from_f32_slice, cubecl-common/src/float/fp4.rs:204-216)
     const uint32_t byte = reinterpret_cast<const uint8_t*>(base)[idx >> 1];
     const uint32_t nib = (idx & 1) ? (byte >> 4) : (byte & 0xFu);
     const float mag[8] = {0.f, 0.5f, 1.f, 1.5f, 2.f, 3.f, 4.f, 6.f};
@@ -234,13 +131,6 @@ __device__ __forceinline__ float mx_elem_to_f32(uint64_t base, uint64_t idx, uin
 // Reference-order block-scaled matmul (the expected-value loop of test_cmma_scaled, cmma.rs:1572-1590):
 //   out[m,n] = sum over l, increasing, in f32 with separately rounded operations, of ((a[m,l] * sa[m,l/32]) * b[n,l]) * sb[n,l/32]
 // One thread per output element; the path for shapes TMA cannot describe, and the on-device cross-check of the wgmma path.
-struct ScaledSimtParams {
-  uint64_t a, b, sa, sb, out;
-  uint32_t batch, M, N, K;       // K in elements
-  uint32_t a_dtype, b_dtype, out_dtype, scale_block;
-  uint32_t a_bmul, b_bmul, scale_ue4m3, pad1;   // scale_ue4m3: scales are |e4m3| (NVFP4: the sign bit is ignored) instead of ue8m0
-};
-
 extern "C" __global__ void __launch_bounds__(256) gemm_scaled_simt(const __grid_constant__ ScaledSimtParams p) {
   const uint64_t total = static_cast<uint64_t>(p.batch) * p.M * p.N;
   const uint32_t n_scales = (p.K + p.scale_block - 1) / p.scale_block;
@@ -254,8 +144,8 @@ extern "C" __global__ void __launch_bounds__(256) gemm_scaled_simt(const __grid_
     float acc = 0.f;
     for (uint32_t l = 0; l < p.K; ++l) {
       const float av = mx_elem_to_f32(p.a, arow * p.K + l, p.a_dtype), bv = mx_elem_to_f32(p.b, brow * p.K + l, p.b_dtype);
-      const float as = p.scale_ue4m3 ? fabsf(load_as_f32(reinterpret_cast<uint64_t>(sa), l / p.scale_block, 10)) : ue8m0_to_f32(sa[l / p.scale_block]);
-      const float bs = p.scale_ue4m3 ? fabsf(load_as_f32(reinterpret_cast<uint64_t>(sb), l / p.scale_block, 10)) : ue8m0_to_f32(sb[l / p.scale_block]);
+      const float as = p.scale_ue4m3 ? fabsf(load_as_f32(reinterpret_cast<uint64_t>(sa), l / p.scale_block, B200_F8E4M3)) : ue8m0_to_f32(sa[l / p.scale_block]);
+      const float bs = p.scale_ue4m3 ? fabsf(load_as_f32(reinterpret_cast<uint64_t>(sb), l / p.scale_block, B200_F8E4M3)) : ue8m0_to_f32(sb[l / p.scale_block]);
       acc = __fadd_rn(acc, __fmul_rn(__fmul_rn(__fmul_rn(av, as), bv), bs));
     }
     store_from_f32(p.out, i, p.out_dtype, acc);
@@ -265,13 +155,7 @@ extern "C" __global__ void __launch_bounds__(256) gemm_scaled_simt(const __grid_
 // Block-scaled operand -> bf16 [rows, K]: x * scale per element, for the wgmma GEMM (Hopper's tensor cores take no scale
 // factors).  Exact: an e2m1 / e4m3 / e5m2 value times a ue8m0 power of two, or e2m1 times a ue4m3 scale (at most 6
 // significant bits), fits bf16's 8-bit significand; bf16 products are exact in the f32 accumulators.  Scales are the
-// reference's row-major [rows, K / scale_block] layout, or the packed 128-row atom layout of pack_scales when `packed`.
-struct DequantParams {
-  uint64_t in, scales, out;
-  uint32_t rows_per_batch, batch, K, dtype;     // K in elements; dtype 10 e4m3, 11 e5m2, 12 packed e2m1
-  uint32_t scale_block, scale_ue4m3, packed, atoms;
-};
-
+// reference's row-major [rows, K / scale_block] layout, or the packed 128-row chunk layout when `packed`.
 extern "C" __global__ void __launch_bounds__(256) dequant_scaled_bf16(const __grid_constant__ DequantParams p) {
   const uint32_t n_scales = p.K / p.scale_block;
   const uint64_t groups = static_cast<uint64_t>(p.batch) * p.rows_per_batch * (p.K / 8);   // 8 outputs (16 B) per thread
@@ -290,7 +174,7 @@ extern "C" __global__ void __launch_bounds__(256) dequant_scaled_bf16(const __gr
     } else {
       sidx = row * n_scales + si;
     }
-    const float s = p.scale_ue4m3 ? fabsf(load_as_f32(p.scales, sidx, 10)) : ue8m0_to_f32(sc[sidx]);
+    const float s = p.scale_ue4m3 ? fabsf(load_as_f32(p.scales, sidx, B200_F8E4M3)) : ue8m0_to_f32(sc[sidx]);
     uint32_t w[4];
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
@@ -308,12 +192,6 @@ extern "C" __global__ void __launch_bounds__(256) dequant_scaled_bf16(const __gr
 // the ORIGINAL tensor already acts as "hi" and only `lo` (exact in f32) is materialised, with the input's own strides
 // compacted to a [batch, rows, out_rs] copy (rows padded to 16 bytes).  The GEMM then accumulates hi*hi + hi*lo + lo*hi in one launch
 // (GemmParams::k_segments == 3).
-struct SplitParams {
-  uint64_t in, out;
-  uint64_t batch, rows, cols;   // logical [batch, rows, cols], cols innermost (stride 1)
-  uint64_t in_bs, in_rs;        // input strides in elements
-  uint64_t out_rs;              // output row pitch in elements (>= cols, multiple of 4 so rows stay 16-byte aligned for TMA)
-};
 // (a non-finite x has no low part: inf - inf would turn an infinite product into NaN)
 __device__ __forceinline__ float tf32_lo(float x) {
   const float lo = x - __uint_as_float(__float_as_uint(x) & 0xFFFFE000u);
@@ -490,11 +368,6 @@ extern "C" __global__ void __launch_bounds__(256) memcopy_probe_vec4(const float
 // Gather a strided rank<=8 tensor into a compact row-major buffer (crates/cubecl-std/src/tensor/contiguous.rs is the
 // reference's generic version).  Only used in front of kernels that need contiguous input (reduce) when the caller
 // hands in a pitched / permuted TensorHandle; element size 1, 2, 4 or 8 bytes.
-struct GatherParams {
-  uint64_t in, out, n;
-  uint64_t shape[8], strides[8];
-  uint32_t rank, esz;
-};
 extern "C" __global__ void __launch_bounds__(256) gather_strided(const __grid_constant__ GatherParams p) {
   for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < p.n;
        i += static_cast<uint64_t>(gridDim.x) * blockDim.x) {
@@ -519,13 +392,6 @@ extern "C" __global__ void __launch_bounds__(256) gather_strided(const __grid_co
 // of the tensor-core GEMM for operands whose own pitch / base is not 16-byte aligned (bf16 with K = 4097, odd sub-views).
 // fp8 (e4m3 / e5m2) operand -> f16, exactly (f16 holds every e4m3 and e5m2 value), with the operand's own strides compacted to
 // [batch, rows, out_pitch].  wgmma accumulates fp8 products with less than f32 precision, so fp8 matmuls run on the f16 kernels.
-struct ConvertF16Params {
-  uint64_t in, out;
-  uint64_t batch, rows, cols;        // logical [batch, rows, cols], cols innermost in the OUTPUT
-  uint64_t in_sb, in_sr, in_sc;      // input strides in elements
-  uint64_t out_pitch;                // output row pitch in elements (multiple of 8)
-  uint32_t dtype, pad;               // 10 = e4m3, 11 = e5m2
-};
 extern "C" __global__ void __launch_bounds__(256) convert_fp8_f16(const __grid_constant__ ConvertF16Params p) {
   const uint64_t vpr = p.out_pitch / 8;                  // 16-byte output vectors per row
   const uint64_t total = p.batch * p.rows * vpr;
@@ -541,7 +407,7 @@ extern "C" __global__ void __launch_bounds__(256) convert_fp8_f16(const __grid_c
     for (int j = 0; j < 8; ++j) {
       if (c0 + j < p.cols) {
         const __nv_fp8_storage_t x = in[src + (c0 + j) * p.in_sc];
-        const __half_raw h = __nv_cvt_fp8_to_halfraw(x, p.dtype == 11 ? __NV_E5M2 : __NV_E4M3);
+        const __half_raw h = __nv_cvt_fp8_to_halfraw(x, p.dtype == B200_F8E5M2 ? __NV_E5M2 : __NV_E4M3);
         w[j >> 1] |= static_cast<uint32_t>(h.x) << (16 * (j & 1));
       }
     }
@@ -549,13 +415,6 @@ extern "C" __global__ void __launch_bounds__(256) convert_fp8_f16(const __grid_c
   }
 }
 
-struct RepitchParams {
-  uint64_t in, out;
-  uint64_t batch, rows, cols;
-  uint64_t in_sb, in_sr, in_sc;
-  uint64_t out_pitch;
-  uint32_t esz, pad;
-};
 extern "C" __global__ void __launch_bounds__(256) repitch_rows(const __grid_constant__ RepitchParams p) {
   const uint32_t per = 16 / p.esz;                       // elements per output vector
   const uint64_t vpr = p.out_pitch / per;                // vectors per output row

@@ -9,6 +9,7 @@
 // encodes TMA descriptors (same cuTensorMapEncodeTiled call as crates/cubecl-cuda/src/compute/server.rs:1210-1224) and
 // launches.  No kernels are generated, compiled or autotuned at run time and nothing here can run without a GPU.
 #include "../../include/cubecl_b200.h"
+#include "kernel_params.h"
 
 #include <cuda.h>
 #include <dlfcn.h>
@@ -210,105 +211,6 @@ static int ensure_nccl() {
     int _r = (call);                                                                                          \
     if (_r != ncclSuccess) return fail(B200_ERR_COMM, "%s failed: %s", #call, g_nccl.GetErrorString(_r));     \
   } while (0)
-
-// ================================================================================================ kernel parameter blocks
-// (layouts mirror the structs in gemm_wgmma.cu / reduce.cu / aux_kernels.cu)
-struct GemmParams {
-  uint64_t out, out_row_stride, out_batch_stride;
-  uint32_t M, N, K, batch;
-  uint32_t tiles_m, tiles_n, group_m;
-  uint32_t a_bmul, b_bmul, vec_store;
-  uint32_t k_segments, epi_act;
-  uint64_t bias;
-  float alpha;
-  uint32_t epi_on;
-  uint32_t full_tiles, sk_tiles, sk_ranges, sk_umax;  // stream-K head, see gemm_wgmma.cu
-  uint64_t split_ws, split_tickets;
-  uint32_t fmt_b, fmt_mixed;       // rhs format of a mixed 8-bit pair
-  uint32_t hyb, hyb_nba, hyb_nbb;  // hybrid f32 schedule: tf32 main product + two bf16 cross terms (gemm_wgmma.cu)
-  uint32_t tma_store;              // whole tiles leave through shared-memory staging and TMA stores
-  uint32_t q_nsub, q_pad;          // quantized operands: scale blocks per 128-element stage (per-block kernels)
-  uint64_t q_ga, q_gb;             // quantized operands: device pointers of the two f32 tensor scales (per-tensor kernels)
-};
-struct ConvertF16Params {
-  uint64_t in, out;
-  uint64_t batch, rows, cols;
-  uint64_t in_sb, in_sr, in_sc;
-  uint64_t out_pitch;
-  uint32_t dtype, pad;
-};
-struct DequantParams {
-  uint64_t in, scales, out;
-  uint32_t rows_per_batch, batch, K, dtype;
-  uint32_t scale_block, scale_ue4m3, packed, atoms;
-};
-struct PackScalesParams {
-  uint64_t in, out;
-  uint32_t batch, rows, n_scales, tiles, atoms, pad_value;
-  uint32_t tile_rows, chunks_per_tile;
-};
-struct ScaledSimtParams {
-  uint64_t a, b, sa, sb, out;
-  uint32_t batch, M, N, K;
-  uint32_t a_dtype, b_dtype, out_dtype, scale_block;
-  uint32_t a_bmul, b_bmul, scale_ue4m3, pad1;
-};
-struct ReduceParams {
-  uint64_t in, out, out2, final_out, ws;
-  uint64_t outer, len, inner;
-  uint64_t s_outer, s_len;       // element strides of the outer and the reduced axis
-  uint64_t row_len, row_pitch;   // inner offset i -> (i / row_len) * row_pitch + i % row_len (row_len == inner: no pitch)
-  uint64_t seg_len;              // the reduced axis is cut into nseg segments (first pass of a two-pass reduction)
-  uint32_t nseg, ctu;
-  float scale;
-  uint32_t flags;                // 1: record stage timings in the workspace debug words, 2: column kernels use vector units
-};
-struct ArgCombineParams {
-  uint64_t keys, idx, out;
-  uint64_t outer, nseg, inner;
-};
-struct ScanParams {
-  uint64_t in, out, carry;       // carry: f32 [outer, nseg, inner] start value of every segment (0: the identity)
-  uint64_t outer, len, inner;
-  uint64_t s_outer, s_len;
-  uint64_t row_len, row_pitch;
-  uint64_t seg_len;
-  uint32_t nseg;
-  uint32_t flags;                // 1: exclusive, 2: column kernel uses vector units
-};
-struct FillParams {
-  uint64_t out, n, seed;
-  float lo, scale;
-  uint32_t dtype, mode, modulus, pad;
-};
-struct SimtGemmParams {
-  uint64_t a, b, out;
-  uint64_t a_sb, a_sm, a_sk, b_sb, b_sk, b_sn, o_sb, o_sm, o_sn;
-  uint32_t M, N, K, batch, in_dtype, out_dtype;
-  uint64_t bias;
-  float alpha;
-  uint32_t epi_act, epi_on, b_dtype_p1;
-};
-struct SplitParams {
-  uint64_t in, out, batch, rows, cols, in_bs, in_rs, out_rs;
-};
-struct XgpuParams {
-  uint64_t mailbox[8];
-  uint32_t rank, nranks, epoch, pad;
-  uint64_t index_offset;
-};
-// One 256-byte slot block (value + index words, two epoch parities, eight source ranks) per DEVICE SET, addressed by the
-// set's device bitmask: overlapping sets ({0,1} and {0,1,2,3}) never share slots, and every rank derives the same offset.
-static constexpr size_t kMailboxSetBytes = 256;
-static constexpr size_t kMailboxBytes = 256 * kMailboxSetBytes;
-static constexpr uint32_t kWsMaxBlocks = 4096;
-static constexpr uint32_t kWsTicketOffset = kWsMaxBlocks * 4 + kWsMaxBlocks * 8;
-static constexpr uint32_t kWsDebugOffset = kWsTicketOffset + 64;         // four u64 words written by the reduce grid stage on request
-static constexpr uint32_t kWsGemmTicketOffset = kWsTicketOffset + 256;  // u32 per (tail tile, CTA rank) of a split GEMM
-static constexpr uint32_t kWsGemmTickets = 1024;                             // u32 entries
-static constexpr uint32_t kWsColTicketOffset = kWsGemmTicketOffset + kWsGemmTickets * 4;  // u32[1024]: one per (outer, column tile) of a fused split column reduction
-static constexpr uint32_t kWsColTickets = 1024;
-static constexpr size_t kWsBytes = kWsColTicketOffset + kWsColTickets * 4;
 
 // ================================================================================================ context
 struct PoolBlock {
@@ -1305,14 +1207,6 @@ static int launch_split_pair(b200_ctx* c, CUstream st, uint64_t in, uint64_t out
   return launch(c, f, std::max(1u, grid), 1, 1, 256, 0, 1, st, args);
 }
 
-struct RepitchParams {
-  uint64_t in, out;
-  uint64_t batch, rows, cols;        // logical [batch, rows, cols] of the copy, cols innermost in the OUTPUT
-  uint64_t in_sb, in_sr, in_sc;      // input strides in elements
-  uint64_t out_pitch;                // output row pitch in elements (16-byte multiple)
-  uint32_t esz, pad;
-};
-
 // One pass that copies an operand TMA cannot describe (row pitch or base not 16-byte aligned, no unit stride) into a pooled
 // buffer it can: [batch, rows, pitch] with the operand's own contiguous dimension innermost when it has one.
 static int stage_operand(b200_ctx* c, CUstream st, size_t esz, uint64_t ptr, uint64_t batch, uint64_t mn, uint64_t K, uint64_t s_mn, uint64_t s_k,
@@ -1554,19 +1448,6 @@ extern "C" int b200_matmul_fused(b200_ctx* c, b200_stream s, b200_dtype in_dtype
 }
 
 // ------------------------------------------------------------------------------------------------ block-scaled matmul
-static int launch_pack_scales(b200_ctx* c, CUstream st, uint64_t in, uint64_t out, uint64_t batch, uint64_t rows,
-                              uint64_t n_scales, uint64_t tiles, uint64_t atoms, uint32_t pad_value, uint32_t tile_rows = 128) {
-  CUfunction f;
-  int rc = get_func(c, "pack_scales", &f);
-  if (rc) return rc;
-  PackScalesParams p{in, out, (uint32_t)batch, (uint32_t)rows, (uint32_t)n_scales, (uint32_t)tiles, (uint32_t)atoms, pad_value,
-                     tile_rows, tile_rows == 224 ? 2u : 1u};
-  const uint64_t words = batch * tiles * atoms * 128;
-  const unsigned grid = (unsigned)std::min<uint64_t>((words + 255) / 256, (uint64_t)c->props.num_sms * 8);
-  void* args[] = {&p};
-  return launch(c, f, std::max(1u, grid), 1, 1, 256, 0, 1, st, args);
-}
-
 extern "C" int b200_matmul_scaled(b200_ctx* c, b200_stream s, b200_dtype lhs_dtype, b200_dtype rhs_dtype, b200_dtype out_dtype,
                                   b200_dptr lhs, b200_dptr rhs, b200_dptr lhs_scales, b200_dptr rhs_scales, b200_dptr out,
                                   uint64_t batch, uint64_t M, uint64_t N, uint64_t K, int scale_block, int scales_packed) {
@@ -1616,7 +1497,7 @@ extern "C" int b200_matmul_scaled(b200_ctx* c, b200_stream s, b200_dtype lhs_dty
     CUfunction f;
     int r = get_func(c, "dequant_scaled_bf16", &f);
     if (r) return r;
-    DequantParams p{in, scales, out_bf16, (uint32_t)rows, (uint32_t)batch, (uint32_t)K, fp4 ? 12u : (uint32_t)dtype,
+    DequantParams p{in, scales, out_bf16, (uint32_t)rows, (uint32_t)batch, (uint32_t)K, fp4 ? (uint32_t)B200_F4E2M1X2 : (uint32_t)dtype,
                     (uint32_t)scale_block, nvf4 ? 1u : 0u, scales_packed ? 1u : 0u, (uint32_t)atoms};
     const uint64_t groups = batch * rows * (K / 8);
     const unsigned grid = (unsigned)std::min<uint64_t>((groups + 255) / 256, (uint64_t)c->props.num_sms * 16);
@@ -1772,7 +1653,7 @@ static int launch_reduce_all(b200_ctx* c, CUstream st, int op, int dt, const RVi
     // auto = the bulk-copy staged kernel once the input is big enough to fill a ring on every SM; plain loads below that
     const std::string var = opt(c, "reduce.variant", "auto");
     if (var == "tma" || var == "auto") {
-      bulk = n * esz >= (var == "tma" ? 64ull * 16384 : (uint64_t)c->props.num_sms * 8 * 16384);
+      bulk = n * esz >= (var == "tma" ? 64ull * kBulkStageBytes : (uint64_t)c->props.num_sms * 8 * kBulkStageBytes);
     } else if (var != "u8") {
       if (std::string(op_tag(op)) == "sum" && dt == B200_F32) name += "_" + var;
     }
@@ -1781,10 +1662,10 @@ static int launch_reduce_all(b200_ctx* c, CUstream st, int op, int dt, const RVi
   unsigned grid;
   if (bulk) {
     name += "_tma";
-    threads = 256 + 32;                       // eight consumer warps + one producer warp
+    threads = kBulkConsumers + 32;            // consumer warps + one producer warp
     stages = opt_uint(c, "reduce.tma_stages", 6, 2, 8);   // 6 x 16 KB ring stages (1 GiB f32)
-    smem = stages * 16384 + 128;
-    const uint64_t tiles = n * esz / 16384;
+    smem = stages * kBulkStageBytes + 128;
+    const uint64_t tiles = n * esz / kBulkStageBytes;
     const unsigned per_sm = stages <= 6 ? opt_uint(c, "reduce.tma_ctas_per_sm", 1, 1, 2) : 1;
     grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(tiles, (uint64_t)c->props.num_sms * per_sm));
   } else {
@@ -1869,12 +1750,12 @@ static int launch_cols_kernel(b200_ctx* c, CUstream st, int op, int dt, const RV
   const uint64_t units = vector ? v.inner / vec : v.inner;
   const uint64_t nseg = ceil_div(v.len, seg_len);
   const uint64_t seg = std::min(seg_len, v.len);
-  // tile shape: RL row lanes x ctu column units per 256-thread block.  A warp's worth of units (512 contiguous bytes per row
+  // tile shape: RL row lanes x ctu column units per kColsThreads-thread block.  A warp's worth of units (512 contiguous bytes per row
   // in vector mode) keeps the loads coalesced; the rest of the block goes to row lanes as long as every lane still has ~4 rows
   const uint64_t ctu_min = std::min<uint64_t>(units, 32);
-  const uint64_t rl_max = 256 / ctu_min;
+  const uint64_t rl_max = kColsThreads / ctu_min;
   const uint64_t rl = std::min<uint64_t>(rl_max, std::max<uint64_t>(1, pow2_floor(std::max<uint64_t>(1, seg / 4))));
-  const uint64_t ctu = std::min<uint64_t>(units, 256 / rl);
+  const uint64_t ctu = std::min<uint64_t>(units, kColsThreads / rl);
   const uint64_t tiles = ceil_div(units, ctu);
   const uint64_t items = v.outer * nseg * tiles;
   const unsigned bps = 8;
@@ -1898,7 +1779,7 @@ static int launch_cols_kernel(b200_ctx* c, CUstream st, int op, int dt, const RV
   }
   if (nseg > 1 && !(p.flags & 4u)) p.scale = 1.0f;   // first pass of a two-launch reduction: the scale (mean) belongs to the second
   void* args[] = {&p};
-  return launch(c, f, grid, 1, 1, 256, 0, 1, st, args, pdl);
+  return launch(c, f, grid, 1, 1, kColsThreads, 0, 1, st, args, pdl);
 }
 
 static int launch_argcombine(b200_ctx* c, CUstream st, uint64_t keys, uint64_t idx, uint64_t out, uint64_t outer, uint64_t nseg, uint64_t inner) {
@@ -2094,11 +1975,6 @@ extern "C" int b200_reduce_strided(b200_ctx* c, b200_stream s, b200_reduce_op op
 }
 
 // ================================================================================================ scan
-// Scan tile geometry (csrc/reduce.cu): a row-kernel thread owns kScanElems consecutive elements per tile; a column-kernel
-// block owns up to kScanColUnits column units.
-static constexpr uint64_t kScanElems = 16;
-static constexpr uint64_t kScanColUnits = 256;
-
 static std::string scan_name(const char* family, int op, int dt, int odt) {
   std::string n = std::string(family) + op_tag(op) + "_" + dt_tag(dt);
   if (odt != B200_F32) n += std::string("_") + dt_tag(odt);
@@ -2263,19 +2139,7 @@ extern "C" int b200_scan(b200_ctx* c, b200_stream s, b200_reduce_op op, int excl
 }
 
 // ================================================================================================ quantize / dequantize
-// Kernels in csrc/quant.cu (parameter blocks mirrored there).
-struct QuantParams {
-  uint64_t in, values, block_scales, tensor_scale, amax;
-  uint64_t rows, K, pitch;
-  uint32_t value, block, scale_dt, block_log2;
-};
-struct QuantDecodeParams {
-  uint64_t values, block_scales, tensor_scale, out;
-  uint64_t n;
-  uint32_t value, block, scale_dt, flags;
-  uint32_t block_log2, pad;
-};
-
+// Kernels in csrc/quant.cu.
 static uint32_t log2_u32(uint32_t v) {
   uint32_t l = 0;
   while (v > 1) { v >>= 1; ++l; }
@@ -2476,18 +2340,7 @@ extern "C" int b200_dequantize(b200_ctx* c, b200_stream s, const b200_quant_sche
 }
 
 // ------------------------------------------------------------------------------------------------ quantized matmul
-// Kernels: csrc/quant.cu (QUANT_PART 1, parameter blocks mirrored there) and csrc/gemm_wgmma.cu (gemm_q8_*, gemm_q8t_*).
-struct QuantScalesParams {
-  uint64_t block_scales, tensor_scale, out;
-  uint64_t batch, rows, rows_pad, nblk;
-  uint32_t rep, pad;
-};
-struct QuantWidenParams {
-  uint64_t in, out;
-  uint64_t rows, K, pitch;
-  uint32_t bits, pad;
-};
-
+// Kernels: csrc/quant.cu (QUANT_PART 1) and csrc/gemm_wgmma.cu (gemm_q8_*, gemm_q8t_*).
 static const char* quant_scale_tag(int32_t dt) {
   switch (dt) {
     case B200_F32: return "f32";
@@ -2616,12 +2469,6 @@ extern "C" int b200_reduce_debug(b200_ctx* c, b200_stream s, uint64_t* words4) {
   CU_CHECK(g_drv.cuStreamSynchronize_p(st));
   return B200_OK;
 }
-
-struct GatherParams {
-  uint64_t in, out, n;
-  uint64_t shape[8], strides[8];
-  uint32_t rank, esz;
-};
 
 extern "C" int b200_into_contiguous(b200_ctx* c, b200_stream s, b200_dtype dtype, b200_dptr in, b200_dptr out, int rank,
                                     const uint64_t* shape, const uint64_t* strides) {

@@ -13,52 +13,10 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
+#include "kernel_params.h"
 #include "ptx.cuh"
 
 using namespace b200;
-
-struct GemmParams {
-  uint64_t out;               // device pointer of out[batch, M, N]
-  uint64_t out_row_stride;    // in elements
-  uint64_t out_batch_stride;  // in elements
-  uint32_t M, N, K, batch;
-  uint32_t tiles_m, tiles_n;  // tile grid per batch; a tile is (128*CG) x BLOCK_N
-  uint32_t group_m;           // rasterisation: tiles are walked in column strips of `group_m` tile-rows (L2 reuse)
-  uint32_t a_bmul, b_bmul;    // 0 = operand broadcast over batch (tensor map has batch extent 1), 1 = batched
-  uint32_t vec_store;         // 1 when every output row start is 16-byte aligned
-  uint32_t k_segments;        // 1, or 3 for the 3xTF32 schedule: the K loop runs three times over (A,B), (A,B_lo), (A_lo,B)
-  uint32_t epi_act;           // fused epilogue (float accumulators only): 0 = none, 1 = relu, 2 = gelu (erf form)
-  uint64_t bias;              // f32[N] added per output column, or 0
-  float alpha;                // out = act(alpha * acc + bias[n]); the epilogue is skipped when alpha == 1, bias == 0, act == 0
-  uint32_t epi_on;
-  // Stream-K head (deterministic, replaces a mostly empty LAST wave): tiles [0, full_tiles) are whole "data-parallel" tiles;
-  // the k-blocks of the remaining `sk_tiles` tiles form one linear space of sk_tiles * num_kb k-blocks that is cut into
-  // `sk_ranges` equal ranges; cluster c works through ranges c, c + C, ... FIRST (a range may cover the end of one tile and
-  // the start of the next: one work unit per tile it touches), then through its whole tiles c, c + C, ....  A unit that
-  // covers only part of a tile's K stores its f32 accumulators to its own slab and takes a ticket for the tile; whoever
-  // completes the tile adds the slabs in k order (so the result does not depend on who came last) and writes the output --
-  // under the MMAs of the following whole tiles, which is why the partial tiles go first.  sk_tiles == 0 disables it.
-  uint32_t full_tiles, sk_tiles, sk_ranges, sk_umax;  // sk_umax: slabs reserved per range (max tiles a range can touch)
-  uint64_t split_ws;          // slabs: [sk_ranges][sk_umax][CG] x (128 x BLOCK_N f32, in accumulator-fragment order)
-  uint64_t split_tickets;     // u32 [sk_tiles][CG], zero on entry, left zero on exit
-  // 8-bit kinds: a MIXED pair (e4m3 x e5m2, u8 x s8 ..., the reference's manual-MMA cartesian products,
-  // crates/cubecl-cpp/src/cuda/mma/manual.rs:151-186) when fmt_mixed != 0; fmt_b is then the rhs format (0 = e4m3 / u8,
-  // 1 = e5m2 / s8).  The lhs format is the kernel's own.
-  uint32_t fmt_b, fmt_mixed;
-  // Hybrid f32 schedule (tf32 kernels, k_segments == 3): segment 0 is the tf32 product of the ORIGINAL operands (their top
-  // 19 bits); segments 1 and 2 are the cross terms A*B_lo and A_lo*B on bf16 copies at twice the tensor rate -- bf16
-  // wgmma into the same f32 accumulators, 64 elements of K per stage instead of 32.  tma_a_lo / tma_b_lo then describe
-  // bf16 PAIR buffers [2 * entries][rows][pitch]: entries [0, hyb_nba) hold bf16(x), entries [hyb_nba, 2 hyb_nba) hold
-  // bf16(x - trunc_tf32(x)).  Two tensor passes' worth of time instead of 3xTF32's three.
-  uint32_t hyb, hyb_nba, hyb_nbb;
-  // 1: whole tiles leave through swizzled shared-memory staging and TMA stores (tma_out describes `out` as (N, M, batch),
-  // [128 B x 64 rows] boxes); needs a 16-byte aligned base and row / batch pitches.  0: each thread stores its own fragment.
-  uint32_t tma_store;
-  // Quantized operands (QM != 0, see gemm_body): q_nsub = 128 / Bk scale blocks per 128-element stage of K (per-block
-  // kernels); q_ga / q_gb = device pointers of the two f32 tensor scales (per-tensor kernels).
-  uint32_t q_nsub, q_pad;
-  uint64_t q_ga, q_gb;
-};
 
 enum : int { KIND_F16 = 0, KIND_BF16 = 1, KIND_TF32 = 2, KIND_E4M3 = 3, KIND_E5M2 = 4, KIND_U8 = 5, KIND_S8 = 6 };
 enum : int { OUT_F16 = 0, OUT_BF16 = 1, OUT_F32 = 2 };  // OUT_F32 is a raw 32-bit store: it also carries the s32 accumulators of the int kinds

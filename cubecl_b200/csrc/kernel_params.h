@@ -1,0 +1,232 @@
+// The host-kernel interface: every parameter block the kernels take as a __grid_constant__ argument, and the layout
+// constants both sides rely on.  capi.cpp (g++) fills these structs and hands their address to cuLaunchKernel; the .cu
+// files (nvcc) read them.  One definition serves both, so a field added here moves on both sides at once.  Plain C++17,
+// no CUDA types.  Dtype and quant-value fields carry the public codes of include/cubecl_b200.h (b200_dtype,
+// b200_quant_value).
+#pragma once
+#include <cstdint>
+
+#include "../../include/cubecl_b200.h"
+
+// ================================================================================================ gemm_wgmma.cu
+struct GemmParams {
+  uint64_t out;               // device pointer of out[batch, M, N]
+  uint64_t out_row_stride;    // in elements
+  uint64_t out_batch_stride;  // in elements
+  uint32_t M, N, K, batch;
+  uint32_t tiles_m, tiles_n;  // tile grid per batch; a tile is (128*CG) x BLOCK_N
+  uint32_t group_m;           // rasterisation: tiles are walked in column strips of `group_m` tile-rows (L2 reuse)
+  uint32_t a_bmul, b_bmul;    // 0 = operand broadcast over batch (tensor map has batch extent 1), 1 = batched
+  uint32_t vec_store;         // 1 when every output row start is 16-byte aligned
+  uint32_t k_segments;        // 1, or 3 for the 3xTF32 schedule: the K loop runs three times over (A,B), (A,B_lo), (A_lo,B)
+  uint32_t epi_act;           // fused epilogue (float accumulators only): 0 = none, 1 = relu, 2 = gelu (erf form)
+  uint64_t bias;              // f32[N] added per output column, or 0
+  float alpha;                // out = act(alpha * acc + bias[n]); the epilogue is skipped when alpha == 1, bias == 0, act == 0
+  uint32_t epi_on;
+  // Stream-K head (deterministic, replaces a mostly empty LAST wave): tiles [0, full_tiles) are whole "data-parallel" tiles;
+  // the k-blocks of the remaining `sk_tiles` tiles form one linear space of sk_tiles * num_kb k-blocks that is cut into
+  // `sk_ranges` equal ranges; cluster c works through ranges c, c + C, ... FIRST (a range may cover the end of one tile and
+  // the start of the next: one work unit per tile it touches), then through its whole tiles c, c + C, ....  A unit that
+  // covers only part of a tile's K stores its f32 accumulators to its own slab and takes a ticket for the tile; whoever
+  // completes the tile adds the slabs in k order (so the result does not depend on who came last) and writes the output --
+  // under the MMAs of the following whole tiles, which is why the partial tiles go first.  sk_tiles == 0 disables it.
+  uint32_t full_tiles, sk_tiles, sk_ranges, sk_umax;  // sk_umax: slabs reserved per range (max tiles a range can touch)
+  uint64_t split_ws;          // slabs: [sk_ranges][sk_umax][CG] x (128 x BLOCK_N f32, in accumulator-fragment order)
+  uint64_t split_tickets;     // u32 [sk_tiles][CG] in the reduce workspace (kWsGemmTicketOffset), zero on entry and on exit
+  // 8-bit kinds: a MIXED pair (e4m3 x e5m2, u8 x s8 ..., the reference's manual-MMA cartesian products,
+  // crates/cubecl-cpp/src/cuda/mma/manual.rs:151-186) when fmt_mixed != 0; fmt_b is then the rhs format (0 = e4m3 / u8,
+  // 1 = e5m2 / s8).  The lhs format is the kernel's own.
+  uint32_t fmt_b, fmt_mixed;
+  // Hybrid f32 schedule (tf32 kernels, k_segments == 3): segment 0 is the tf32 product of the ORIGINAL operands (their top
+  // 19 bits); segments 1 and 2 are the cross terms A*B_lo and A_lo*B on bf16 copies at twice the tensor rate -- bf16
+  // wgmma into the same f32 accumulators, 64 elements of K per stage instead of 32.  tma_a_lo / tma_b_lo then describe
+  // bf16 PAIR buffers [2 * entries][rows][pitch]: entries [0, hyb_nba) hold bf16(x), entries [hyb_nba, 2 hyb_nba) hold
+  // bf16(x - trunc_tf32(x)).  Two tensor passes' worth of time instead of 3xTF32's three.
+  uint32_t hyb, hyb_nba, hyb_nbb;
+  // 1: whole tiles leave through swizzled shared-memory staging and TMA stores (tma_out describes `out` as (N, M, batch),
+  // [128 B x 64 rows] boxes); needs a 16-byte aligned base and row / batch pitches.  0: each thread stores its own fragment.
+  uint32_t tma_store;
+  // Quantized operands (QM != 0, see gemm_body): q_nsub = 128 / Bk scale blocks per 128-element stage of K (per-block
+  // kernels); q_ga / q_gb = device pointers of the two f32 tensor scales (per-tensor kernels).
+  uint32_t q_nsub, q_pad;
+  uint64_t q_ga, q_gb;
+};
+
+// ================================================================================================ aux_kernels.cu
+struct FillParams {
+  uint64_t out, n, seed;
+  float lo, scale;     // value = lo + u * scale
+  uint32_t dtype;      // b200_dtype: F32, F16, BF16, F8E4M3, F8E5M2
+  uint32_t mode;       // 0 uniform hash, 1 (i % modulus) as a number
+  uint32_t modulus, pad;
+};
+
+struct SimtGemmParams {
+  uint64_t a, b, out;
+  uint64_t a_sb, a_sm, a_sk;  // strides in elements: batch, m, k
+  uint64_t b_sb, b_sk, b_sn;
+  uint64_t o_sb, o_sm, o_sn;
+  uint32_t M, N, K, batch;
+  uint32_t in_dtype, out_dtype;  // b200_dtype: F32, F16, BF16; inputs also F8E4M3, F8E5M2, U8, I8
+  uint64_t bias;                 // fused epilogue, same meaning as GemmParams
+  float alpha;
+  uint32_t epi_act, epi_on;
+  uint32_t b_dtype_p1;           // rhs dtype + 1 when it differs from in_dtype (mixed fp8 / int8 pairs), 0 = same as lhs
+};
+
+struct ScaledSimtParams {
+  uint64_t a, b, sa, sb, out;
+  uint32_t batch, M, N, K;       // K in elements
+  uint32_t a_dtype, b_dtype, out_dtype, scale_block;
+  uint32_t a_bmul, b_bmul, scale_ue4m3, pad1;   // scale_ue4m3: scales are |e4m3| (NVFP4: the sign bit is ignored) instead of ue8m0
+};
+
+// Scales are the reference's row-major [rows, K / scale_block] layout, or (packed) the 128-row chunk layout
+// b200_matmul_scaled takes with scales_packed = 1.
+struct DequantParams {
+  uint64_t in, scales, out;
+  uint32_t rows_per_batch, batch, K, dtype;     // K in elements; dtype F8E4M3, F8E5M2 or F4E2M1X2
+  uint32_t scale_block, scale_ue4m3, packed, atoms;
+};
+
+struct SplitParams {
+  uint64_t in, out;
+  uint64_t batch, rows, cols;   // logical [batch, rows, cols], cols innermost (stride 1)
+  uint64_t in_bs, in_rs;        // input strides in elements
+  uint64_t out_rs;              // output row pitch in elements (>= cols, multiple of 4 so rows stay 16-byte aligned for TMA)
+};
+
+struct GatherParams {
+  uint64_t in, out, n;
+  uint64_t shape[8], strides[8];
+  uint32_t rank, esz;
+};
+
+struct ConvertF16Params {
+  uint64_t in, out;
+  uint64_t batch, rows, cols;        // logical [batch, rows, cols], cols innermost in the OUTPUT
+  uint64_t in_sb, in_sr, in_sc;      // input strides in elements
+  uint64_t out_pitch;                // output row pitch in elements (multiple of 8)
+  uint32_t dtype, pad;               // F8E4M3 or F8E5M2
+};
+
+struct RepitchParams {
+  uint64_t in, out;
+  uint64_t batch, rows, cols;        // logical [batch, rows, cols] of the copy, cols innermost in the OUTPUT
+  uint64_t in_sb, in_sr, in_sc;      // input strides in elements
+  uint64_t out_pitch;                // output row pitch in elements (16-byte multiple)
+  uint32_t esz, pad;
+};
+
+// ================================================================================================ reduce.cu
+struct ReduceParams {
+  uint64_t in;        // input view, element (o, l, i) at in + (o * s_outer + l * s_len + inner_off(i)) elements
+  uint64_t out;       // output [outer (* segments), inner]: f32 values, u32 indices (arg ops), or u32 keys (arg ops, split pass)
+  uint64_t out2;      // arg ops, split pass: u32 indices along the reduced axis; 0 otherwise
+  uint64_t final_out; // column kernels, split pass with a fused finish (flags bit 2): the real output [outer, inner]; the block
+                      // that completes a column tile's last segment (ticket) combines the partials in `out` / `out2` itself
+  uint64_t ws;        // the per-stream reduce workspace (layout below)
+  uint64_t outer, len, inner;
+  uint64_t s_outer, s_len;      // element strides of the outer and the reduced axis
+  uint64_t row_len, row_pitch;  // inner_off(i) = (i / row_len) * row_pitch + i % row_len; row_len == inner (or len, for
+                                // reductions over all elements, where i is the flat index): no pitch
+  uint64_t seg_len;   // the reduced axis is cut into nseg = ceil(len / seg_len) segments reduced independently (first pass of
+  uint32_t nseg;      // a two-pass reduction); nseg == 1: whole axis
+  uint32_t ctu;       // column kernels: column units (one 128-bit vector, or one element) per block tile; bulk-copy kernels:
+                      // ring depth in stages
+  float scale;        // applied to the final value (mean = 1/len, sum = 1)
+  uint32_t flags;     // bit 0: record stage timings in the workspace debug words; bit 1: column kernels use vector units;
+                      // bit 2: fused finish of a split column reduction (see final_out)
+};
+
+// Reduce workspace, one per stream, zeroed once at allocation (every ticket is left at zero by the kernel that used it).
+constexpr uint32_t kWsMaxBlocks = 4096;                                    // grid cap of the all-elements reduction
+constexpr uint32_t kWsIdxOffset = kWsMaxBlocks * 4;                        // after f32 partials[kWsMaxBlocks]: u64 packed pairs
+constexpr uint32_t kWsTicketOffset = kWsIdxOffset + kWsMaxBlocks * 8;      // u32 last-block ticket of the grid stage
+constexpr uint32_t kWsDebugOffset = kWsTicketOffset + 64;                  // four u64 words: stage timings (ReduceParams::flags bit 0)
+constexpr uint32_t kWsGemmTicketOffset = kWsTicketOffset + 256;            // u32 per (stream-K head tile, CTA rank) of a GEMM
+static_assert(kWsDebugOffset + 4 * 8 <= kWsGemmTicketOffset, "debug words overlap the GEMM tickets");
+constexpr uint32_t kWsGemmTickets = 1024;
+constexpr uint32_t kWsColTicketOffset = kWsGemmTicketOffset + kWsGemmTickets * 4;  // u32 per (outer, column tile) of a fused
+constexpr uint32_t kWsColTickets = 1024;                                            // split column reduction
+constexpr uint32_t kWsBytes = kWsColTicketOffset + kWsColTickets * 4;
+
+// Cross-GPU exchange fused into the grid stage (one kernel = local reduce + all-reduce of the scalar over NVLink peer
+// memory).  Every rank owns a mailbox its peers can write; an entry is (epoch << 32) | 32 payload bits, stored with ONE
+// 64-bit system-scope store so value and flag arrive together.
+struct XgpuParams {
+  uint64_t mailbox[8];   // device pointers of every rank's slot set (own included), indexed by rank
+  uint32_t rank, nranks, epoch, pad;
+  uint64_t index_offset; // arg ops: global index of this rank's element 0 (outer-axis shard offset)
+};
+// A slot set is value slots u64[2][8] (epoch parity x source rank), then index slots u64[2][8] (arg ops: the second word,
+// same epoch tag).  The mailbox holds one set per DEVICE SET, addressed by the set's device bitmask: overlapping sets
+// ({0,1} and {0,1,2,3}) never share slots, and every rank derives the same offset.
+constexpr uint32_t kMailboxIndexOffset = 2 * 8 * 8;
+constexpr uint32_t kMailboxSetBytes = 2 * kMailboxIndexOffset;
+constexpr uint32_t kMailboxBytes = 256 * kMailboxSetBytes;
+
+// Bulk-copy all-elements kernels (_tma): kBulkConsumers consumer threads plus one producer warp, kBulkStageBytes per ring stage.
+constexpr uint32_t kBulkStageBytes = 16384;
+constexpr int kBulkConsumers = 256;
+// Column kernels: threads per block (row lanes x column units).
+constexpr int kColsThreads = 256;
+
+struct ArgCombineParams {
+  uint64_t keys, idx, out;      // u32 keys and u32 indices [outer, nseg, inner] -> u32 indices [outer, inner]
+  uint64_t outer, nseg, inner;
+};
+
+struct ScanParams {
+  uint64_t in;        // input view, element (o, l, i) at in + (o * s_outer + l * s_len + inner_off(i)) elements
+  uint64_t out;       // compact [outer, len, inner] output
+  uint64_t carry;     // f32 [outer, nseg, inner]: the value every segment starts from (0: the identity)
+  uint64_t outer, len, inner;
+  uint64_t s_outer, s_len;
+  uint64_t row_len, row_pitch;  // as ReduceParams
+  uint64_t seg_len;
+  uint32_t nseg;
+  uint32_t flags;     // bit 0: exclusive; bit 1: column kernel uses vector units
+};
+// Scans: a row-kernel thread owns kScanElems consecutive elements per tile; a column-kernel block owns at most kScanColUnits
+// column units (one per thread).
+constexpr int kScanElems = 16;
+constexpr int kScanColUnits = 256;
+
+// ================================================================================================ quant.cu
+struct QuantParams {
+  uint64_t in;            // input rows: element (r, k) at in + (r * pitch + k) elements; 16-byte aligned base and rows
+  uint64_t values;        // codes, compact [rows, K * bits / 8] bytes
+  uint64_t block_scales;  // compact [rows, K / block] in scale_dt; 0 without a block level
+  uint64_t tensor_scale;  // f32 [1]; 0 without a tensor level
+  uint64_t amax;          // u32 [1]: bits of the finite |x| max of the tensor (quant_absmax); 0 without a tensor level
+  uint64_t rows, K, pitch;
+  uint32_t value;         // b200_quant_value
+  uint32_t block;         // values per block scale; 0 = per-tensor only
+  uint32_t scale_dt;      // block-scale dtype (b200_dtype)
+  uint32_t block_log2;    // log2(block) (blocks are powers of two)
+};
+
+struct QuantDecodeParams {
+  uint64_t values, block_scales, tensor_scale, out;
+  uint64_t n;             // elements
+  uint32_t value, block, scale_dt;
+  uint32_t flags;         // bit 0: values and out are 16-byte aligned (vector loads and stores)
+  uint32_t block_log2, pad;
+};
+
+// Quantized-matmul operands (b200_matmul_quantized)
+struct QuantScalesParams {
+  uint64_t block_scales;  // [batch, rows, nblk / rep] in the block-scale dtype; unused by the per-tensor kernel
+  uint64_t tensor_scale;  // f32 [1] on the device, or 0
+  uint64_t out;           // f32 [batch][nblk][rows_pad], block-major: one TMA box per GEMM stage
+  uint64_t batch, rows, rows_pad, nblk;
+  uint32_t rep;           // GEMM blocks per stored block (this side's block / the GEMM's Bk)
+  uint32_t pad;
+};
+
+struct QuantWidenParams {
+  uint64_t in, out;       // in: compact code rows of K * bits / 8 bytes; out: s8 rows `pitch` bytes apart (16-byte multiple)
+  uint64_t rows, K, pitch;
+  uint32_t bits, pad;
+};

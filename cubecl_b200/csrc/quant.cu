@@ -22,56 +22,33 @@
 #include <cuda_fp16.h>
 #include <cstdint>
 
-enum : int { DT_F32 = 0, DT_F16 = 1, DT_BF16 = 2, DT_F8E4M3 = 10, DT_UE8M0 = 13 };
-// QuantValue, scheme.rs:358-377, in its order (b200_quant_value)
-enum : uint32_t { QV_Q8F = 0, QV_E5M2 = 1, QV_E4M3 = 2, QV_Q4F = 3, QV_E2M1 = 4, QV_Q2F = 5, QV_Q8S = 6, QV_Q4S = 7, QV_Q2S = 8 };
-
-struct QuantParams {
-  uint64_t in;            // input rows: element (r, k) at in + (r * pitch + k) elements; 16-byte aligned base and rows
-  uint64_t values;        // codes, compact [rows, K * bits / 8] bytes
-  uint64_t block_scales;  // compact [rows, K / block] in scale_dt; 0 without a block level
-  uint64_t tensor_scale;  // f32 [1]; 0 without a tensor level
-  uint64_t amax;          // u32 [1]: bits of the finite |x| max of the tensor (quant_absmax); 0 without a tensor level
-  uint64_t rows, K, pitch;
-  uint32_t value;         // b200_quant_value
-  uint32_t block;         // values per block scale; 0 = per-tensor only
-  uint32_t scale_dt;      // block-scale dtype (b200_dtype)
-  uint32_t block_log2;    // log2(block) (blocks are powers of two)
-};
-
-struct QuantDecodeParams {
-  uint64_t values, block_scales, tensor_scale, out;
-  uint64_t n;             // elements
-  uint32_t value, block, scale_dt;
-  uint32_t flags;         // bit 0: values and out are 16-byte aligned (vector loads and stores)
-  uint32_t block_log2, pad;
-};
+#include "kernel_params.h"
 
 // ------------------------------------------------------------------------------------------------ value types
 __device__ __forceinline__ uint32_t qv_bits(uint32_t v) {
-  return (v == QV_Q4F || v == QV_Q4S || v == QV_E2M1) ? 4u : (v == QV_Q2F || v == QV_Q2S) ? 2u : 8u;
+  return (v == B200_QV_Q4F || v == B200_QV_Q4S || v == B200_QV_E2M1) ? 4u : (v == B200_QV_Q2F || v == B200_QV_Q2S) ? 2u : 8u;
 }
 // QuantValue::range() (scheme.rs:399-411)
 __device__ __forceinline__ float qv_lo(uint32_t v) {
   switch (v) {
-    case QV_Q8F: return -128.f;
-    case QV_Q4F: return -8.f;
-    case QV_Q2F: return -2.f;
-    case QV_Q8S: return -127.f;
-    case QV_Q4S: return -7.f;
-    case QV_Q2S: return -1.f;
-    case QV_E4M3: return -448.f;
-    case QV_E5M2: return -57344.f;
+    case B200_QV_Q8F: return -128.f;
+    case B200_QV_Q4F: return -8.f;
+    case B200_QV_Q2F: return -2.f;
+    case B200_QV_Q8S: return -127.f;
+    case B200_QV_Q4S: return -7.f;
+    case B200_QV_Q2S: return -1.f;
+    case B200_QV_E4M3: return -448.f;
+    case B200_QV_E5M2: return -57344.f;
     default: return -6.f;
   }
 }
 __device__ __forceinline__ float qv_hi(uint32_t v) {
   switch (v) {
-    case QV_Q8F: case QV_Q8S: return 127.f;
-    case QV_Q4F: case QV_Q4S: return 7.f;
-    case QV_Q2F: case QV_Q2S: return 1.f;
-    case QV_E4M3: return 448.f;
-    case QV_E5M2: return 57344.f;
+    case B200_QV_Q8F: case B200_QV_Q8S: return 127.f;
+    case B200_QV_Q4F: case B200_QV_Q4S: return 7.f;
+    case B200_QV_Q2F: case B200_QV_Q2S: return 1.f;
+    case B200_QV_E4M3: return 448.f;
+    case B200_QV_E5M2: return 57344.f;
     default: return 6.f;
   }
 }
@@ -80,10 +57,10 @@ __device__ __forceinline__ float qv_hi(uint32_t v) {
 // ScaleDtype::max_representable (scheme.rs:208-218)
 __device__ __forceinline__ float scale_max(uint32_t dt) {
   switch (dt) {
-    case DT_F16: return 65504.f;
-    case DT_BF16: return __uint_as_float(0x7F7F0000u);
-    case DT_UE8M0: return __uint_as_float(0x7F000000u);   // 2^127
-    case DT_F8E4M3: return 448.f;
+    case B200_F16: return 65504.f;
+    case B200_BF16: return __uint_as_float(0x7F7F0000u);
+    case B200_UE8M0: return __uint_as_float(0x7F000000u);   // 2^127
+    case B200_F8E4M3: return 448.f;
     default: return __uint_as_float(0x7F7FFFFFu);
   }
 }
@@ -102,14 +79,14 @@ __device__ __forceinline__ float ue8m0_value(uint32_t c) {
 
 // ScaleDtype::round_up (scheme.rs:235-270) / round_up_to_dtype (cubecl-std/src/quant/round.rs), bit for bit; UE8M0 above.
 __device__ __forceinline__ float round_up_scale(float s, uint32_t dt) {
-  if (dt == DT_F32) return s;
-  if (dt == DT_UE8M0) return ue8m0_value(ue8m0_code(s));
+  if (dt == B200_F32) return s;
+  if (dt == B200_UE8M0) return ue8m0_value(ue8m0_code(s));
   if (s != s) return s;
   const float mx = scale_max(dt);
   if (s >= mx) return mx;
-  if (dt == DT_F16 && s < 6.103515625e-05f) return ceilf(s / 5.9604644775390625e-08f) * 5.9604644775390625e-08f;
-  if (dt == DT_F8E4M3 && s < 0.015625f) return ceilf(s / 0.001953125f) * 0.001953125f;
-  const uint32_t step = dt == DT_F16 ? (1u << 13) : dt == DT_BF16 ? (1u << 16) : (1u << 20);
+  if (dt == B200_F16 && s < 6.103515625e-05f) return ceilf(s / 5.9604644775390625e-08f) * 5.9604644775390625e-08f;
+  if (dt == B200_F8E4M3 && s < 0.015625f) return ceilf(s / 0.001953125f) * 0.001953125f;
+  const uint32_t step = dt == B200_F16 ? (1u << 13) : dt == B200_BF16 ? (1u << 16) : (1u << 20);
   return __uint_as_float((__float_as_uint(s) + (step - 1)) & ~(step - 1));
 }
 
@@ -137,20 +114,20 @@ __device__ __forceinline__ float e5m2_to_f32(uint32_t b) {
 // The stored bits of a scale already on the dtype's grid (round_up_scale's result): every conversion here is exact.
 __device__ __forceinline__ uint32_t scale_bits(float s, uint32_t dt) {
   switch (dt) {
-    case DT_F16: return __half_as_ushort(__float2half_rn(s));
-    case DT_BF16: return __float_as_uint(s) >> 16;
-    case DT_F8E4M3: return f32_to_e4m3(s) & 0x7Fu;
-    case DT_UE8M0: return ue8m0_code(s);
+    case B200_F16: return __half_as_ushort(__float2half_rn(s));
+    case B200_BF16: return __float_as_uint(s) >> 16;
+    case B200_F8E4M3: return f32_to_e4m3(s) & 0x7Fu;
+    case B200_UE8M0: return ue8m0_code(s);
     default: return __float_as_uint(s);
   }
 }
 // A stored block scale read back as f32; e4m3 scales are read with the sign ignored, as b200_matmul_scaled reads them.
 __device__ __forceinline__ float load_scale(uint64_t base, uint64_t i, uint32_t dt) {
   switch (dt) {
-    case DT_F16: return __half2float(__ushort_as_half(__ldg(reinterpret_cast<const unsigned short*>(base) + i)));
-    case DT_BF16: return __uint_as_float(static_cast<uint32_t>(__ldg(reinterpret_cast<const unsigned short*>(base) + i)) << 16);
-    case DT_F8E4M3: return e4m3_to_f32(__ldg(reinterpret_cast<const unsigned char*>(base) + i) & 0x7Fu);
-    case DT_UE8M0: return ue8m0_value(__ldg(reinterpret_cast<const unsigned char*>(base) + i));
+    case B200_F16: return __half2float(__ushort_as_half(__ldg(reinterpret_cast<const unsigned short*>(base) + i)));
+    case B200_BF16: return __uint_as_float(static_cast<uint32_t>(__ldg(reinterpret_cast<const unsigned short*>(base) + i)) << 16);
+    case B200_F8E4M3: return e4m3_to_f32(__ldg(reinterpret_cast<const unsigned char*>(base) + i) & 0x7Fu);
+    case B200_UE8M0: return ue8m0_value(__ldg(reinterpret_cast<const unsigned char*>(base) + i));
     default: return __ldg(reinterpret_cast<const float*>(base) + i);
   }
 }
@@ -163,11 +140,11 @@ __device__ __forceinline__ float load_scale(uint64_t base, uint64_t i, uint32_t 
 __device__ __forceinline__ uint32_t encode_one(float x, float eff, float rcp, bool pow2, uint32_t v, float lo, float hi) {
   if (eff == 0.f) return 0u;
   const float q = pow2 ? x * rcp : x / eff;
-  if (v == QV_E4M3 || v == QV_E5M2) {
+  if (v == B200_QV_E4M3 || v == B200_QV_E5M2) {
     if (q != q) return 0x7Fu;
-    return v == QV_E4M3 ? f32_to_e4m3(q) : f32_to_e5m2(q);
+    return v == B200_QV_E4M3 ? f32_to_e4m3(q) : f32_to_e5m2(q);
   }
-  if (v == QV_E2M1) {
+  if (v == B200_QV_E2M1) {
     if (q != q) return 0u;
     const float a = fabsf(q);
     const uint32_t c = a <= 0.25f ? 0u : a < 0.75f ? 1u : a <= 1.25f ? 2u : a < 1.75f ? 3u
@@ -181,9 +158,9 @@ __device__ __forceinline__ uint32_t encode_one(float x, float eff, float rcp, bo
 
 __device__ __forceinline__ float decode_one(uint32_t field, uint32_t v, uint32_t bits) {
   switch (v) {
-    case QV_E4M3: return e4m3_to_f32(field);
-    case QV_E5M2: return e5m2_to_f32(field);
-    case QV_E2M1: {
+    case B200_QV_E4M3: return e4m3_to_f32(field);
+    case B200_QV_E5M2: return e5m2_to_f32(field);
+    case B200_QV_E2M1: {
       const float m = (field & 4u) ? ((field & 2u) ? ((field & 1u) ? 6.f : 4.f) : ((field & 1u) ? 3.f : 2.f))
                                    : ((field & 2u) ? ((field & 1u) ? 1.5f : 1.f) : ((field & 1u) ? 0.5f : 0.f));
       return (field & 8u) ? -m : m;
@@ -199,7 +176,7 @@ __device__ __forceinline__ float decode_one(uint32_t field, uint32_t v, uint32_t
 template <int DT>
 struct In;
 template <>
-struct In<DT_F32> {
+struct In<B200_F32> {
   static constexpr int VEC = 4;
   static __device__ __forceinline__ float get(uint64_t base, uint64_t i) { return __ldg(reinterpret_cast<const float*>(base) + i); }
   static __device__ __forceinline__ void unpack(uint4 r, float (&f)[VEC]) {
@@ -207,7 +184,7 @@ struct In<DT_F32> {
   }
 };
 template <>
-struct In<DT_F16> {
+struct In<B200_F16> {
   static constexpr int VEC = 8;
   static __device__ __forceinline__ float get(uint64_t base, uint64_t i) {
     return __half2float(__ushort_as_half(__ldg(reinterpret_cast<const unsigned short*>(base) + i)));
@@ -222,7 +199,7 @@ struct In<DT_F16> {
   }
 };
 template <>
-struct In<DT_BF16> {
+struct In<B200_BF16> {
   static constexpr int VEC = 8;
   static __device__ __forceinline__ float get(uint64_t base, uint64_t i) {
     return __uint_as_float(static_cast<uint32_t>(__ldg(reinterpret_cast<const unsigned short*>(base) + i)) << 16);
@@ -262,7 +239,7 @@ __device__ __forceinline__ uint32_t load_chunk(const QuantParams& p, uint64_t cp
   }
   const uint32_t n = static_cast<uint32_t>(left < VEC ? left : VEC);
   if (n == VEC) {
-    In<DT>::unpack(ldg_stream_u4(p.in + e * (DT == DT_F32 ? 4 : 2)), x);
+    In<DT>::unpack(ldg_stream_u4(p.in + e * (DT == B200_F32 ? 4 : 2)), x);
   } else {
 #pragma unroll
     for (int j = 0; j < VEC; ++j) x[j] = j < static_cast<int>(n) ? In<DT>::get(p.in, e + j) : 0.f;
@@ -349,8 +326,8 @@ __device__ __forceinline__ void encode_chunk(const QuantParams& p, const float (
       const uint64_t si = f >> p.block_log2;
       const uint32_t sbits = scale_bits(s, p.scale_dt);
       switch (p.scale_dt) {
-        case DT_F32: reinterpret_cast<uint32_t*>(p.block_scales)[si] = sbits; break;
-        case DT_F16: case DT_BF16: reinterpret_cast<unsigned short*>(p.block_scales)[si] = static_cast<unsigned short>(sbits); break;
+        case B200_F32: reinterpret_cast<uint32_t*>(p.block_scales)[si] = sbits; break;
+        case B200_F16: case B200_BF16: reinterpret_cast<unsigned short*>(p.block_scales)[si] = static_cast<unsigned short>(sbits); break;
         default: reinterpret_cast<unsigned char*>(p.block_scales)[si] = static_cast<unsigned char>(sbits); break;
       }
     }
@@ -392,7 +369,7 @@ __device__ __forceinline__ void encode_body(const QuantParams& p) {
 // ------------------------------------------------------------------------------------------------ decode pass
 template <int ODT>
 __device__ __forceinline__ void store8(uint64_t out, uint64_t i, const float (&y)[8], uint32_t valid, bool vec) {
-  if (ODT == DT_F32) {
+  if (ODT == B200_F32) {
     float* o = reinterpret_cast<float*>(out) + i;
     if (vec && valid == 8) {
       reinterpret_cast<float4*>(o)[0] = make_float4(y[0], y[1], y[2], y[3]);
@@ -404,7 +381,7 @@ __device__ __forceinline__ void store8(uint64_t out, uint64_t i, const float (&y
     unsigned short h[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j)
-      h[j] = ODT == DT_F16 ? __half_as_ushort(__float2half_rn(y[j])) : __bfloat16_as_ushort(__float2bfloat16_rn(y[j]));
+      h[j] = ODT == B200_F16 ? __half_as_ushort(__float2half_rn(y[j])) : __bfloat16_as_ushort(__float2bfloat16_rn(y[j]));
     unsigned short* o = reinterpret_cast<unsigned short*>(out) + i;
     if (vec && valid == 8) {
       uint4 w;
@@ -481,15 +458,6 @@ __device__ __forceinline__ void decode_dispatch(const QuantDecodeParams& p) {
 #if QUANT_PART == 1
 // ------------------------------------------------------------------------------------------------ quantized-matmul operands
 // (capi.cpp: b200_matmul_quantized, gemm_wgmma.cu: QM_BLOCK)
-struct QuantScalesParams {
-  uint64_t block_scales;  // [batch, rows, nblk / rep] in the block-scale dtype; unused by the per-tensor kernel
-  uint64_t tensor_scale;  // f32 [1] on the device, or 0
-  uint64_t out;           // f32 [batch][nblk][rows_pad], block-major: one TMA box per GEMM stage
-  uint64_t batch, rows, rows_pad, nblk;
-  uint32_t rep;           // GEMM blocks per stored block (this side's block / the GEMM's Bk)
-  uint32_t pad;
-};
-
 // The effective scale of GEMM block j of row r, as b200_dequantize defines it: f32(s), rn(g * f32(s)) with a tensor level,
 // or g for a per-tensor side.  A coarser block repeats its scale `rep` times; rows [rows, rows_pad) are written as 0.
 template <int DT>   // block-scale dtype, or -1 for a per-tensor side
@@ -512,12 +480,6 @@ __device__ __forceinline__ void scales_body(const QuantScalesParams& p) {
     reinterpret_cast<float*>(p.out)[i] = eff;
   }
 }
-
-struct QuantWidenParams {
-  uint64_t in, out;       // in: compact code rows of K * bits / 8 bytes; out: s8 rows `pitch` bytes apart (16-byte multiple)
-  uint64_t rows, K, pitch;
-  uint32_t bits, pad;
-};
 
 // 4- and 2-bit code streams widened exactly to one s8 per element (sign extension, as b200_dequantize reads a field);
 // one thread writes 16 output bytes, the pitch padding as 0.
@@ -548,11 +510,11 @@ __device__ __forceinline__ void widen_body(const QuantWidenParams& p) {
   }
 }
 
-extern "C" __global__ void __launch_bounds__(256) quant_scales_f32_f32(const QuantScalesParams p) { scales_body<DT_F32>(p); }
-extern "C" __global__ void __launch_bounds__(256) quant_scales_f32_f16(const QuantScalesParams p) { scales_body<DT_F16>(p); }
-extern "C" __global__ void __launch_bounds__(256) quant_scales_f32_bf16(const QuantScalesParams p) { scales_body<DT_BF16>(p); }
-extern "C" __global__ void __launch_bounds__(256) quant_scales_f32_ue8m0(const QuantScalesParams p) { scales_body<DT_UE8M0>(p); }
-extern "C" __global__ void __launch_bounds__(256) quant_scales_f32_ue4m3(const QuantScalesParams p) { scales_body<DT_F8E4M3>(p); }
+extern "C" __global__ void __launch_bounds__(256) quant_scales_f32_f32(const QuantScalesParams p) { scales_body<B200_F32>(p); }
+extern "C" __global__ void __launch_bounds__(256) quant_scales_f32_f16(const QuantScalesParams p) { scales_body<B200_F16>(p); }
+extern "C" __global__ void __launch_bounds__(256) quant_scales_f32_bf16(const QuantScalesParams p) { scales_body<B200_BF16>(p); }
+extern "C" __global__ void __launch_bounds__(256) quant_scales_f32_ue8m0(const QuantScalesParams p) { scales_body<B200_UE8M0>(p); }
+extern "C" __global__ void __launch_bounds__(256) quant_scales_f32_ue4m3(const QuantScalesParams p) { scales_body<B200_F8E4M3>(p); }
 extern "C" __global__ void __launch_bounds__(256) quant_scales_f32_tensor(const QuantScalesParams p) { scales_body<-1>(p); }
 extern "C" __global__ void __launch_bounds__(256) quant_widen_s8(const QuantWidenParams p) { widen_body(p); }
 #endif  // QUANT_PART == 1
@@ -562,7 +524,7 @@ extern "C" __global__ void __launch_bounds__(256) quant_widen_s8(const QuantWide
   extern "C" __global__ void __launch_bounds__(256) quant_absmax_##tag(const QuantParams p) { absmax_body<DT>(p); }  \
   extern "C" __global__ void __launch_bounds__(256) quant_encode_##tag(const QuantParams p) { encode_body<DT>(p); }  \
   extern "C" __global__ void __launch_bounds__(256) quant_decode_##tag(const QuantDecodeParams p) { decode_dispatch<DT>(p); }
-QUANT_KERNELS(f32, DT_F32)
-QUANT_KERNELS(f16, DT_F16)
-QUANT_KERNELS(bf16, DT_BF16)
+QUANT_KERNELS(f32, B200_F32)
+QUANT_KERNELS(f16, B200_F16)
+QUANT_KERNELS(bf16, B200_BF16)
 #endif  // QUANT_PART == 0

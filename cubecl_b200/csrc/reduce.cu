@@ -23,50 +23,12 @@
 #include <cuda_fp16.h>
 #include <cstdint>
 
+#include "kernel_params.h"
 #include "ptx.cuh"
 
-struct ReduceParams {
-  uint64_t in;        // input view, element (o, l, i) at in + (o * s_outer + l * s_len + inner_off(i)) elements
-  uint64_t out;       // output [outer (* segments), inner]: f32 values, u32 indices (arg ops), or u32 keys (arg ops, split pass)
-  uint64_t out2;      // arg ops, split pass: u32 indices along the reduced axis; 0 otherwise
-  uint64_t final_out; // column kernels, split pass with a fused finish (flags bit 2): the real output [outer, inner]; the block
-                      // that completes a column tile's last segment (ticket) combines the partials in `out` / `out2` itself
-  uint64_t ws;        // workspace: partial values f32[grid] | partial packed pairs u64[grid] | u32 ticket | debug words
-  uint64_t outer, len, inner;
-  uint64_t s_outer, s_len;
-  uint64_t row_len, row_pitch;  // inner_off(i) = (i / row_len) * row_pitch + i % row_len; row_len == inner (or len, for
-                                // reductions over all elements, where i is the flat index): no pitch
-  uint64_t seg_len;   // the reduced axis is cut into nseg = ceil(len / seg_len) segments reduced independently (first pass of
-  uint32_t nseg;      // a two-pass reduction); nseg == 1: whole axis
-  uint32_t ctu;       // column kernels: column units (one 128-bit vector, or one element) per block tile
-  float scale;        // applied to the final value (mean = 1/len, sum = 1)
-  uint32_t flags;     // bit 0: record stage timings in the workspace debug words; bit 1: column kernels use vector units;
-                      // bit 2: fused finish of a split column reduction (see final_out)
-};
-
-// Cross-GPU exchange fused into the grid stage (one kernel = local reduce + all-reduce of the scalar over NVLink peer
-// memory).  Every rank owns a mailbox `uint64 slots[2][8]` (epoch parity x source rank) that its peers can write; an entry
-// is (epoch << 32) | 32 payload bits, stored with ONE 64-bit system-scope store so value and flag arrive together.
-struct XgpuParams {
-  uint64_t mailbox[8];   // device pointers of every rank's mailbox (own included), indexed by rank
-  uint32_t rank, nranks, epoch, pad;
-  uint64_t index_offset; // arg ops: global index of this rank's element 0 (outer-axis shard offset)
-};
-// mailbox layout: [0,128) value slots[2][8]; [128,256) index slots[2][8] (arg ops: second word, same epoch tag)
-constexpr uint32_t kMailboxIndexOffset = 128;
-
 enum : int { OP_SUM = 0, OP_PROD = 1, OP_MAX = 2, OP_MIN = 3, OP_ARGMAX = 4, OP_ARGMIN = 5 };
-enum : int { DT_F32 = 0, DT_F16 = 1, DT_BF16 = 2 };
 
 constexpr int kMaxWarps = 32;
-// workspace layout (host mirrors this): [0, 16 KiB) f32 partials, [16 KiB, 48 KiB) u64 partial pairs, then the ticket,
-// then four u64 debug words (exchange / grid-stage timings of the last launch that asked for them)
-constexpr uint32_t kWsMaxBlocks = 4096;
-constexpr uint32_t kWsIdxOffset = kWsMaxBlocks * 4;
-constexpr uint32_t kWsTicketOffset = kWsIdxOffset + kWsMaxBlocks * 8;
-constexpr uint32_t kWsDebugOffset = kWsTicketOffset + 64;
-constexpr uint32_t kWsColTicketOffset = kWsTicketOffset + 256 + 4096;   // after the GEMM's 1024 tickets: u32[1024], one per (outer, column tile)
-constexpr uint32_t kWsColTickets = 1024;
 
 // ------------------------------------------------------------------------------------------------ value ops
 template <int OP>
@@ -160,7 +122,7 @@ __device__ __forceinline__ uint4 ldg_stream_u4(const void* p) {
 template <int DT>
 struct Elem;
 template <>
-struct Elem<DT_F32> {
+struct Elem<B200_F32> {
   using T = float;
   static constexpr int VEC = 4;  // elements per 128-bit load
   static __device__ __forceinline__ float get(const void* base, uint64_t i) { return reinterpret_cast<const float*>(base)[i]; }
@@ -169,7 +131,7 @@ struct Elem<DT_F32> {
   }
 };
 template <>
-struct Elem<DT_F16> {
+struct Elem<B200_F16> {
   using T = __half;
   static constexpr int VEC = 8;
   static __device__ __forceinline__ float get(const void* base, uint64_t i) { return __half2float(reinterpret_cast<const __half*>(base)[i]); }
@@ -183,7 +145,7 @@ struct Elem<DT_F16> {
   }
 };
 template <>
-struct Elem<DT_BF16> {
+struct Elem<B200_BF16> {
   using T = __nv_bfloat16;
   static constexpr int VEC = 8;
   static __device__ __forceinline__ float get(const void* base, uint64_t i) { return __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(base)[i]); }
@@ -549,10 +511,8 @@ __device__ __forceinline__ void reduce_all_body(const ReduceParams& p, const Xgp
 // and accumulate.  One CTA per SM, tiles dealt round-robin over the grid, so at any instant the grid reads ONE contiguous
 // window of gridDim x 16 KB x (stages in flight); no register is spent on loads in flight and no address arithmetic per
 // 16 bytes.  Head (unaligned base) and tail (< one tile) elements go through plain loads.
-constexpr uint32_t kBulkStageBytes = 16384;
 constexpr int kBulkStages = 8;       // at most; the launch picks the ring depth (ReduceParams::ctu): 8 = one CTA per SM,
                                      // <= 6 lets two CTAs share an SM (the next launch's CTA can start under PDL)
-constexpr int kBulkConsumers = 256;  // threads; + one producer warp
 
 template <int OP, int DT>
 __device__ __forceinline__ void reduce_all_bulk_body(const ReduceParams& p) {
@@ -890,8 +850,6 @@ __device__ __forceinline__ void reduce_rows_body(const ReduceParams& p, int tpr_
 // l = rl, rl + RL, ... of its unit, four loads in flight, consecutive threads on consecutive units (coalesced); the RL
 // partial results per unit are combined through shared memory.  Work items = (outer x segment) x tiles over the grid.
 // Few columns with a long axis: small ctu -> many row lanes.  Many columns with a short axis: ctu = blockDim, one row lane.
-constexpr int kColsThreads = 256;
-
 template <int OP, int DT, bool VECTOR, int NL /* loads in flight per thread */>
 __device__ __forceinline__ void reduce_cols_tiles(const ReduceParams& p, uint64_t* s_raw) {
   using E = Elem<DT>;
@@ -1074,10 +1032,6 @@ __device__ __forceinline__ void reduce_cols_body(const ReduceParams& p) {
 
 // ================================================================================================ second pass of a split arg-reduction
 // keys / indices [outer, nseg, inner] (u32, u32) -> indices [outer, inner]: max of the packed pairs over the segments.
-struct ArgCombineParams {
-  uint64_t keys, idx, out;
-  uint64_t outer, nseg, inner;
-};
 extern "C" __global__ void __launch_bounds__(256) reduce_argcombine(const __grid_constant__ ArgCombineParams p) {
   const uint64_t total = p.outer * p.inner;
   const uint32_t* keys = reinterpret_cast<const uint32_t*>(p.keys);
@@ -1139,7 +1093,7 @@ extern "C" __global__ void __launch_bounds__(256) reduce_argcombine(const __grid
   }
 
 #define ALL_SHAPES(OPN, OP, DTN, DT)                                                \
-  REDUCE_ALL(reduce_all_##OPN##_##DTN, OP, DT, (DT == DT_F32 ? 8 : 4), false)       \
+  REDUCE_ALL(reduce_all_##OPN##_##DTN, OP, DT, (DT == B200_F32 ? 8 : 4), false)     \
   REDUCE_ALL_BULK(reduce_all_##OPN##_##DTN##_tma, OP, DT)                           \
   REDUCE_ALL_PITCHED(reduce_allp_##OPN##_##DTN, OP, DT)                             \
   REDUCE_ROWS(reduce_rows_##OPN##_##DTN, OP, DT)                                    \
@@ -1149,7 +1103,7 @@ extern "C" __global__ void __launch_bounds__(256) reduce_argcombine(const __grid
   REDUCE_ALL_PITCHED(reduce_allp_##OPN##_##DTN, OP, DT)                             \
   REDUCE_ROWS(reduce_rows_##OPN##_##DTN, OP, DT)                                    \
   REDUCE_COLS(reduce_cols_##OPN##_##DTN, OP, DT)
-#define ALL_DTYPES(M, OPN, OP) M(OPN, OP, f32, DT_F32) M(OPN, OP, f16, DT_F16) M(OPN, OP, bf16, DT_BF16)
+#define ALL_DTYPES(M, OPN, OP) M(OPN, OP, f32, B200_F32) M(OPN, OP, f16, B200_F16) M(OPN, OP, bf16, B200_BF16)
 
 ALL_DTYPES(ALL_SHAPES, sum, OP_SUM)
 ALL_DTYPES(ALL_SHAPES, prod, OP_PROD)
@@ -1161,31 +1115,31 @@ ALL_DTYPES(ALL_ARG_SHAPES, argmin, OP_ARGMIN)
 // local sum + cross-GPU all-reduce of the scalar in one launch (see XgpuParams)
 extern "C" __global__ void __launch_bounds__(512, 2) reduce_all_sum_f32_xgpu(const __grid_constant__ ReduceParams p,
                                                                           const __grid_constant__ XgpuParams xg) {
-  reduce_all_body<OP_SUM, DT_F32, 8, false, true>(p, &xg);
+  reduce_all_body<OP_SUM, B200_F32, 8, false, true>(p, &xg);
 }
 extern "C" __global__ void __launch_bounds__(512) reduce_all_argmax_f32_xgpu(const __grid_constant__ ReduceParams p,
                                                                              const __grid_constant__ XgpuParams xg) {
-  reduce_all_body<OP_ARGMAX, DT_F32, 4, false, true>(p, &xg);
+  reduce_all_body<OP_ARGMAX, B200_F32, 4, false, true>(p, &xg);
 }
 extern "C" __global__ void __launch_bounds__(512) reduce_all_argmin_f32_xgpu(const __grid_constant__ ReduceParams p,
                                                                              const __grid_constant__ XgpuParams xg) {
-  reduce_all_body<OP_ARGMIN, DT_F32, 4, false, true>(p, &xg);
+  reduce_all_body<OP_ARGMIN, B200_F32, 4, false, true>(p, &xg);
 }
 
 // tuning variants of the headline kernel (f32 sum over all elements); the host picks one by name.
 #define REDUCE_ALL_BLOCKED(NAME, UNROLL)                                                           \
   extern "C" __global__ void __launch_bounds__(512) NAME(const __grid_constant__ ReduceParams p) {  \
-    reduce_all_body<OP_SUM, DT_F32, UNROLL, false, false, true>(p);                                \
+    reduce_all_body<OP_SUM, B200_F32, UNROLL, false, false, true>(p);                              \
   }
 REDUCE_ALL_BLOCKED(reduce_all_sum_f32_b4, 4)
 REDUCE_ALL_BLOCKED(reduce_all_sum_f32_b8, 8)
-REDUCE_ALL(reduce_all_sum_f32_u2, OP_SUM, DT_F32, 2, false)
-REDUCE_ALL(reduce_all_sum_f32_u4, OP_SUM, DT_F32, 4, false)
-REDUCE_ALL(reduce_all_sum_f32_u16, OP_SUM, DT_F32, 16, false)
-REDUCE_ALL(reduce_all_sum_f32_w2, OP_SUM, DT_F32, 2, true)
-REDUCE_ALL(reduce_all_sum_f32_w4, OP_SUM, DT_F32, 4, true)
+REDUCE_ALL(reduce_all_sum_f32_u2, OP_SUM, B200_F32, 2, false)
+REDUCE_ALL(reduce_all_sum_f32_u4, OP_SUM, B200_F32, 4, false)
+REDUCE_ALL(reduce_all_sum_f32_u16, OP_SUM, B200_F32, 16, false)
+REDUCE_ALL(reduce_all_sum_f32_w2, OP_SUM, B200_F32, 2, true)
+REDUCE_ALL(reduce_all_sum_f32_w4, OP_SUM, B200_F32, 4, true)
 // the arg-reduction with more loads in flight (tuning variant)
-REDUCE_ALL(reduce_all_argmax_f32_u8, OP_ARGMAX, DT_F32, 8, false)
+REDUCE_ALL(reduce_all_argmax_f32_u8, OP_ARGMAX, B200_F32, 8, false)
 
 // ================================================================================================ scans along an axis
 // cumsum / cumprod / cummax / cummin of the view [outer, len, inner] into a COMPACT row-major output of the same shape:
@@ -1197,22 +1151,10 @@ REDUCE_ALL(reduce_all_argmax_f32_u8, OP_ARGMAX, DT_F32, 8, false)
 // scan of the partials (f32 -> f32, these kernels) turns them into per-segment carries, and the final scan starts every
 // segment from its carry (`carry` != 0).  Every combination order is fixed by the launch geometry: results are bitwise
 // reproducible for a given shape and SM count.
-struct ScanParams {
-  uint64_t in;        // input view, element (o, l, i) at in + (o * s_outer + l * s_len + inner_off(i)) elements
-  uint64_t out;       // compact [outer, len, inner] output
-  uint64_t carry;     // f32 [outer, nseg, inner]: the value every segment starts from (0: the identity)
-  uint64_t outer, len, inner;
-  uint64_t s_outer, s_len;
-  uint64_t row_len, row_pitch;  // as ReduceParams
-  uint64_t seg_len;
-  uint32_t nseg;
-  uint32_t flags;     // bit 0: exclusive; bit 1: column kernel uses vector units
-};
-
 template <int ODT>
 struct OutElem;
 template <>
-struct OutElem<DT_F32> {
+struct OutElem<B200_F32> {
   using T = float;
   static constexpr int VEC = 4;
   static __device__ __forceinline__ void put(void* base, uint64_t i, float v) { reinterpret_cast<float*>(base)[i] = v; }
@@ -1221,7 +1163,7 @@ struct OutElem<DT_F32> {
   }
 };
 template <>
-struct OutElem<DT_F16> {
+struct OutElem<B200_F16> {
   using T = __half;
   static constexpr int VEC = 8;
   static __device__ __forceinline__ void put(void* base, uint64_t i, float v) { reinterpret_cast<__half*>(base)[i] = __float2half_rn(v); }
@@ -1236,7 +1178,7 @@ struct OutElem<DT_F16> {
   }
 };
 template <>
-struct OutElem<DT_BF16> {
+struct OutElem<B200_BF16> {
   using T = __nv_bfloat16;
   static constexpr int VEC = 8;
   static __device__ __forceinline__ void put(void* base, uint64_t i, float v) {
@@ -1263,8 +1205,6 @@ __device__ __forceinline__ void stg_stream_u4(void* p, uint4 v) {
 // kScanElems consecutive elements (128-bit loads), scans them serially in registers, the group scans the thread totals
 // (shfl_up, width min(TPR, 32), then a shared-memory stage across warps), and the running carry of the item joins in front.
 // A base that is not 16-byte aligned costs one scalar head tile; outputs leave as 128-bit stores when their address allows.
-constexpr int kScanElems = 16;
-
 template <int OP, int DT, int ODT>
 __device__ __forceinline__ void scan_rows_body(const ScanParams& p, int tpr_log2) {
   using E = Elem<DT>;
@@ -1473,16 +1413,16 @@ __device__ __forceinline__ void scan_cols_body(const ScanParams& p) {
   extern "C" __global__ void __launch_bounds__(512) scan_rows_##NAME_SFX(const __grid_constant__ ScanParams p, int tpr_log2) { \
     scan_rows_body<OP, DT, ODT>(p, tpr_log2);                                                                          \
   }                                                                                                                    \
-  extern "C" __global__ void __launch_bounds__(256) scan_cols_##NAME_SFX(const __grid_constant__ ScanParams p) {         \
+  extern "C" __global__ void __launch_bounds__(kScanColUnits) scan_cols_##NAME_SFX(const __grid_constant__ ScanParams p) { \
     scan_cols_body<OP, DT, ODT>(p);                                                                                    \
   }
 // output f32 for every input dtype; a 16-bit input may also keep its own dtype (suffix _<out dtype>)
 #define SCAN_DTYPES(OPN, OP)                                 \
-  SCAN_KERNELS(OPN##_f32, OP, DT_F32, DT_F32)                \
-  SCAN_KERNELS(OPN##_f16, OP, DT_F16, DT_F32)                \
-  SCAN_KERNELS(OPN##_f16_f16, OP, DT_F16, DT_F16)            \
-  SCAN_KERNELS(OPN##_bf16, OP, DT_BF16, DT_F32)              \
-  SCAN_KERNELS(OPN##_bf16_bf16, OP, DT_BF16, DT_BF16)
+  SCAN_KERNELS(OPN##_f32, OP, B200_F32, B200_F32)            \
+  SCAN_KERNELS(OPN##_f16, OP, B200_F16, B200_F32)            \
+  SCAN_KERNELS(OPN##_f16_f16, OP, B200_F16, B200_F16)        \
+  SCAN_KERNELS(OPN##_bf16, OP, B200_BF16, B200_F32)          \
+  SCAN_KERNELS(OPN##_bf16_bf16, OP, B200_BF16, B200_BF16)
 
 SCAN_DTYPES(sum, OP_SUM)
 SCAN_DTYPES(prod, OP_PROD)

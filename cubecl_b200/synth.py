@@ -132,7 +132,8 @@ def ue8m0_to_f32(bits: np.ndarray) -> np.ndarray:
 
 def pack_scale_chunks(scales: np.ndarray, pad: int = 127) -> np.ndarray:
     """[rows, n_scales] scale bytes -> the tensor core's packed chunks [ceil(rows/128)][ceil(n_scales/4)][512]:
-    byte (r % 32) * 16 + (r / 32) * 4 + s; padding = 1.0 (127 for ue8m0, 0x38 for ue4m3).  Host mirror of the pack_scales kernel."""
+    byte (r % 32) * 16 + (r / 32) * 4 + s; padding = 1.0 (127 for ue8m0, 0x38 for ue4m3).  The scales_packed = 1 input layout
+    of b200_matmul_scaled."""
     scales = np.asarray(scales, dtype=np.uint8)
     rows, ns = scales.shape
     tiles, atoms = (rows + 127) // 128, (ns + 3) // 4

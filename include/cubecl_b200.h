@@ -192,7 +192,7 @@ int b200_matmul_fused(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b200_dt
  * pinned by test_cmma_scaled / test_cmma_scaled_fp4 (crates/cubecl-core/src/runtime_tests/cmma.rs:1476-1700).
  * Layouts follow those tests: lhs [batch, m, k] and rhs [batch, n, k] K-contiguous ("col-major" rhs), dtypes B200_F8E4M3 /
  * B200_F8E5M2 (mixable) or both B200_F4E2M1X2 (k / 2 bytes per row); scales are B200_UE8M0 bytes [batch, rows, k / 32]
- * row-major (scales_packed = 0) or in the packed form of pack_scales [batch * ceil(rows/128)][ceil(k/128)][512 B],
+ * row-major (scales_packed = 0) or in the packed 128-row chunk form [batch * ceil(rows/128)][ceil(k/128)][512 B],
  * byte (r % 32) * 16 + (r / 32) * 4 + s (scales_packed = 1).  out [batch, m, n] contiguous, f32 / bf16 / f16.
  * scale_block = 32: ue8m0 scales (MXFP8 / MXFP4).  scale_block = 16: NVFP4 -- packed e2m1 operands with e4m3 scale bytes
  * [batch, rows, k / 16] whose sign is ignored (the third ScaledMmaConfig row of manual.rs:241-250).
