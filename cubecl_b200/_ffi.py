@@ -41,6 +41,12 @@ class Epilogue(C.Structure):
     _fields_ = [("alpha", C.c_float), ("activation", C.c_int32), ("bias", C.c_uint64)]
 
 
+class Conv2dArgs(C.Structure):
+    """b200_conv2d_args: stride, padding and dilation per spatial axis (h, w)."""
+    _fields_ = [("stride_h", C.c_int32), ("stride_w", C.c_int32), ("pad_h", C.c_int32), ("pad_w", C.c_int32),
+                ("dilation_h", C.c_int32), ("dilation_w", C.c_int32)]
+
+
 class QuantScheme(C.Structure):
     """b200_quant_scheme: value (b200_quant_value), block, block_scale (b200_dtype), tensor_scale (0 / 1)."""
     _fields_ = [("value", C.c_int32), ("block", C.c_int32), ("block_scale", C.c_int32), ("tensor_scale", C.c_int32)]
@@ -105,6 +111,8 @@ SIGNATURES = {
                                      C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64, C.c_int, C.c_int]),
     "b200_matmul_quantized": (C.c_int, [_vp, _vp, C.POINTER(QuantOperand), C.POINTER(QuantOperand), C.c_int, C.c_uint64,
                                         C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64]),
+    "b200_conv2d": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, _u64p, _u64p, C.c_uint64, _u64p, _u64p, C.c_uint64, _u64p,
+                              _u64p, C.POINTER(Conv2dArgs), C.POINTER(Epilogue)]),
     "b200_reduce": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, C.c_uint64, C.c_int, _u64p, C.c_int]),
     "b200_reduce_strided": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, C.c_uint64, C.c_int, _u64p, _u64p, C.c_int]),
     "b200_reduce_debug": (C.c_int, [_vp, _vp, _u64p]),

@@ -1,0 +1,87 @@
+"""2-D convolution surface (cubek's convolution kernels are out of tree), in the std-lib op convention
+`op::launch(client, &TensorHandle...)` (crates/cubecl-std/src/tensor/identity.rs:39-83).
+
+out[n, oh, ow, co] = act(alpha * sum_{ky, kx, c} x[n, oh*sh - ph + ky*dh, ow*sw - pw + kx*dw, c] * w[co, ky, kx, c] + bias[co])
+
+x is NHWC [N, H, W, C], w is [Cout, KH, KW, C], out is NHWC [N, OH, OW, Cout]; input outside x reads as zero, f32
+accumulation.  The kernel behind it is the wgmma GEMM of csrc/gemm_wgmma.cu with its A tile loaded through a TMA im2col
+map (an implicit GEMM: M = N * OH * OW output pixels, N = Cout, K = KH * KW * C), see include/cubecl_b200.h (b200_conv2d).
+"""
+from __future__ import annotations
+
+import ctypes as C
+
+from . import _ffi
+from ._ffi import B200Error
+from .client import ComputeClient, DTYPES, TensorHandle
+from .matmul import ACTIVATIONS
+
+
+class ConvShapeError(ValueError):
+    """The output-shape rule does not hold: channel mismatch, rank, or an output extent < 1."""
+
+
+def _pair(v, what: str) -> tuple[int, int]:
+    if isinstance(v, int):
+        return int(v), int(v)
+    v = tuple(int(e) for e in v)
+    if len(v) != 2:
+        raise ValueError(f"{what} must be an int or a pair, got {v!r}")
+    return v
+
+
+def calculate_conv2d_output(x_shape, w_shape, stride=1, padding=0, dilation=1) -> list[int]:
+    """[N, OH, OW, Cout] of an NHWC input [N, H, W, C] and weights [Cout, KH, KW, C]; PyTorch's rule:
+    OH = floor((H + 2*ph - dh*(KH-1) - 1) / sh) + 1, OW likewise."""
+    x_shape, w_shape = [int(s) for s in x_shape], [int(s) for s in w_shape]
+    if len(x_shape) != 4 or len(w_shape) != 4:
+        raise ConvShapeError(f"conv2d needs rank-4 x [N,H,W,C] and w [Cout,KH,KW,C], got {x_shape} and {w_shape}")
+    (sh, sw), (ph, pw), (dh, dw) = _pair(stride, "stride"), _pair(padding, "padding"), _pair(dilation, "dilation")
+    n, h, w, c = x_shape
+    cout, kh, kw, c2 = w_shape
+    if c != c2:
+        raise ConvShapeError(f"channels differ: x has {c}, w has {c2}")
+    if sh < 1 or sw < 1 or dh < 1 or dw < 1 or ph < 0 or pw < 0:
+        raise ConvShapeError("strides and dilations must be >= 1 and padding >= 0")
+    nh, nw = h + 2 * ph - dh * (kh - 1) - 1, w + 2 * pw - dw * (kw - 1) - 1
+    if nh < 0 or nw < 0:
+        raise ConvShapeError(f"the dilated kernel {kh}x{kw} is larger than the padded input {h}x{w}")
+    return [n, nh // sh + 1, nw // sw + 1, cout]
+
+
+def launch(client: ComputeClient, x: TensorHandle, w: TensorHandle, out: TensorHandle, stride=1, padding=0, dilation=1,
+           alpha: float = 1.0, bias: TensorHandle | None = None, activation: str | None = None, stream=None) -> None:
+    """Enqueue the convolution on the client's stream.  stride / padding / dilation are ints or (h, w) pairs.  Optional fused
+    epilogue: out = activation(alpha * conv + bias[co]) with `bias` an f32 [Cout] tensor.  Never raises for launch problems:
+    errors are deferred to client.sync() / read_one() like matmul.launch."""
+    try:
+        if activation not in ACTIVATIONS:
+            raise B200Error(6, f"unknown activation {activation!r}")
+        if len(x.shape) != 4 or len(w.shape) != 4 or len(out.shape) != 4:
+            raise B200Error(6, "conv2d: x, w and out must have rank 4")
+        if x.dtype != w.dtype:
+            raise B200Error(6, f"conv2d: x dtype {x.dtype} != w dtype {w.dtype}")
+        if bias is not None and (bias.dtype != "f32" or not bias.is_contiguous() or bias.size() != w.shape[0]):
+            raise B200Error(6, "conv2d: bias must be a contiguous f32 tensor with Cout elements")
+        (sh, sw), (ph, pw), (dh, dw) = _pair(stride, "stride"), _pair(padding, "padding"), _pair(dilation, "dilation")
+        for t in (x, w, out) + ((bias,) if bias is not None else ()):
+            t.handle.used_on(stream)
+        args = _ffi.Conv2dArgs(sh, sw, ph, pw, dh, dw)
+        ep = None
+        if alpha != 1.0 or bias is not None or activation not in (None, "none"):
+            ep = C.byref(_ffi.Epilogue(float(alpha), ACTIVATIONS[activation], bias.handle.ptr if bias is not None else 0))
+        _ffi.check(client._lib.b200_conv2d(
+            client._ctx, stream, DTYPES[x.dtype], DTYPES[out.dtype],
+            C.c_uint64(x.handle.ptr), _ffi.u64_array(x.shape), _ffi.u64_array(x.strides),
+            C.c_uint64(w.handle.ptr), _ffi.u64_array(w.shape), _ffi.u64_array(w.strides),
+            C.c_uint64(out.handle.ptr), _ffi.u64_array(out.shape), _ffi.u64_array(out.strides), C.byref(args), ep))
+    except (B200Error, ValueError) as e:
+        client._defer(e if isinstance(e, B200Error) else B200Error(6, str(e)))
+
+
+def launch_alloc(client: ComputeClient, x: TensorHandle, w: TensorHandle, out_dtype: str | None = None, **kwargs) -> TensorHandle:
+    """Convenience: allocate a compact NHWC `out` with the output rule, then launch (keyword arguments as launch)."""
+    shape = calculate_conv2d_output(x.shape, w.shape, kwargs.get("stride", 1), kwargs.get("padding", 0), kwargs.get("dilation", 1))
+    out = TensorHandle.empty_contiguous(client, shape, out_dtype or x.dtype)
+    launch(client, x, w, out, **kwargs)
+    return out

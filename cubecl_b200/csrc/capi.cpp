@@ -45,6 +45,8 @@ extern const unsigned char b200_cubin_gemm_q[];
 extern const unsigned char b200_cubin_gemm_q_end[];
 extern const unsigned char b200_cubin_quant_mm[];
 extern const unsigned char b200_cubin_quant_mm_end[];
+extern const unsigned char b200_cubin_gemm_conv[];
+extern const unsigned char b200_cubin_gemm_conv_end[];
 }
 
 // ================================================================================================ errors
@@ -73,7 +75,7 @@ extern "C" int b200_abi_version(void) { return B200_ABI_VERSION; }
   X(cuMemcpyDtoDAsync) X(cuMemsetD32Async) X(cuMemGetInfo)                                                           \
   X(cuStreamCreate) X(cuStreamDestroy) X(cuStreamSynchronize) X(cuStreamWaitEvent)                                   \
   X(cuEventCreate) X(cuEventRecord) X(cuEventElapsedTime) X(cuEventDestroy) X(cuEventSynchronize) X(cuEventQuery)                    \
-  X(cuTensorMapEncodeTiled) X(cuGetErrorString) X(cuGetErrorName)                                                    \
+  X(cuTensorMapEncodeTiled) X(cuTensorMapEncodeIm2col) X(cuGetErrorString) X(cuGetErrorName)                                                    \
   X(cuIpcGetMemHandle) X(cuIpcOpenMemHandle) X(cuIpcCloseMemHandle) X(cuCtxEnablePeerAccess) X(cuDeviceCanAccessPeer)
 
 struct Driver {
@@ -315,12 +317,13 @@ static int get_func(b200_ctx* c, const std::string& name, CUfunction* out) {
   if (c->dry) { c->pending_kernel = name; *out = nullptr; return B200_OK; }
   auto it = c->funcs.find(name);
   if (it != c->funcs.end()) { *out = it->second; return B200_OK; }
-  // modules are loaded in the order gemm, reduce, aux, gemm_b, gemm_c, quant, gemm_q, quant_mm; the kernel name says where a
+  // modules are loaded in the order gemm, reduce, aux, gemm_b, gemm_c, quant, gemm_q, quant_mm, gemm_conv; the kernel name says where a
   // kernel lives (no failing lookups, which API-level tools such as compute-sanitizer would report)
   auto starts = [&](const char* pfx) { return name.rfind(pfx, 0) == 0; };
   auto has = [&](const char* part) { return name.find(part) != std::string::npos; };
   const bool tc_gemm = starts("gemm_") && name != "gemm_simt_strided" && name != "gemm_scaled_simt";
-  const size_t home = starts("gemm_q8") ? 6
+  const size_t home = starts("conv2d_") ? 8
+                      : starts("gemm_q8") ? 6
                       : starts("quant_scales_") || starts("quant_widen_") ? 7
                       : starts("quant_") ? 5
                       : tc_gemm && (has("_2sm_n128_") || has("_2sm_n224_")) ? 3
@@ -349,7 +352,8 @@ extern "C" int b200_get_cubin(const char* name, const void** image, size_t* size
   else if (!strcmp(name, "quant")) { b = b200_cubin_quant; e = b200_cubin_quant_end; }
   else if (!strcmp(name, "gemm_q")) { b = b200_cubin_gemm_q; e = b200_cubin_gemm_q_end; }
   else if (!strcmp(name, "quant_mm")) { b = b200_cubin_quant_mm; e = b200_cubin_quant_mm_end; }
-  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm)", name);
+  else if (!strcmp(name, "gemm_conv")) { b = b200_cubin_gemm_conv; e = b200_cubin_gemm_conv_end; }
+  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv)", name);
   *image = b;
   *size = static_cast<size_t>(e - b);
   return B200_OK;
@@ -404,7 +408,8 @@ extern "C" int b200_init(int device, b200_ctx** out) {
       (rc = load_module(c, b200_cubin_gemm_c, b200_cubin_gemm_c_end, "gemm_c")) ||
       (rc = load_module(c, b200_cubin_quant, b200_cubin_quant_end, "quant")) ||
       (rc = load_module(c, b200_cubin_gemm_q, b200_cubin_gemm_q_end, "gemm_q")) ||
-      (rc = load_module(c, b200_cubin_quant_mm, b200_cubin_quant_mm_end, "quant_mm"))) {
+      (rc = load_module(c, b200_cubin_quant_mm, b200_cubin_quant_mm_end, "quant_mm")) ||
+      (rc = load_module(c, b200_cubin_gemm_conv, b200_cubin_gemm_conv_end, "gemm_conv"))) {
     for (CUmodule m : c->modules) g_drv.cuModuleUnload_p(m);
     g_drv.cuDevicePrimaryCtxRelease_p(c->dev);
     return bail(rc);
@@ -850,6 +855,59 @@ static int encode_tmap(b200_ctx* c, CUtensorMap* out, CUtensorMapDataType dt, si
   return B200_OK;
 }
 
+// 4-D im2col map of an NHWC tensor (dims innermost first: C, W, H, N; strides of W, H, N in elements), SWIZZLE_128B, zero
+// out-of-bounds fill.  Corners (w, h) bound the pixels a load walks; estr_w / estr_h are the conv strides.  Same cache as
+// encode_tmap.
+static int encode_im2col(b200_ctx* c, CUtensorMap* out, CUtensorMapDataType dt, size_t esz, uint64_t base, const uint64_t dims[4],
+                         const uint64_t strides[3], const int lower[2], const int upper[2], uint32_t channels, uint32_t pixels,
+                         uint32_t estr_w, uint32_t estr_h) {
+  const int promo_bytes = atoi(opt(c, "gemm.l2_promotion", "256").c_str());
+  const CUtensorMapL2promotion promo = promo_bytes >= 256 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B
+                                       : promo_bytes >= 128 ? CU_TENSOR_MAP_L2_PROMOTION_L2_128B
+                                       : promo_bytes >= 64 ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B : CU_TENSOR_MAP_L2_PROMOTION_NONE;
+  char key[320];
+  snprintf(key, sizeof(key), "im2col|%d|%llx|%llu|%llu|%llu|%llu|%llu|%llu|%llu|%d|%d|%d|%d|%u|%u|%u|%u|%d", (int)dt,
+           (unsigned long long)base, (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)dims[2],
+           (unsigned long long)dims[3], (unsigned long long)strides[0], (unsigned long long)strides[1], (unsigned long long)strides[2],
+           lower[0], lower[1], upper[0], upper[1], channels, pixels, estr_w, estr_h, (int)promo);
+  if (c->dry) {
+    char line[320];
+    snprintf(line, sizeof(line),
+             "tmap im2col esz=%zu dims=(%llu,%llu,%llu,%llu) strides=(%llu,%llu,%llu) lower=(%d,%d) upper=(%d,%d) channels=%u pixels=%u "
+             "estrides=(1,%u,%u,1) swizzle=%d\n",
+             esz, (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)dims[2], (unsigned long long)dims[3],
+             (unsigned long long)(strides[0] * esz), (unsigned long long)(strides[1] * esz), (unsigned long long)(strides[2] * esz),
+             lower[0], lower[1], upper[0], upper[1], channels, pixels, estr_w, estr_h, (int)CU_TENSOR_MAP_SWIZZLE_128B);
+    c->plan += line;
+    memset(out, 0, sizeof(*out));
+    return B200_OK;
+  }
+  auto it = c->tmap_cache.find(key);
+  if (it != c->tmap_cache.end()) { *out = it->second; return B200_OK; }
+  cuuint64_t gdim[4] = {dims[0], dims[1], dims[2], dims[3]};
+  cuuint64_t gstr[3] = {strides[0] * esz, strides[1] * esz, strides[2] * esz};
+  cuuint32_t estr[4] = {1, estr_w, estr_h, 1};
+  CUresult r = g_drv.cuTensorMapEncodeIm2col_p(out, dt, 4, reinterpret_cast<void*>(base), gdim, gstr, lower, upper, channels, pixels, estr,
+                                               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, promo,
+                                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS)
+    return fail(B200_ERR_INVALID_ARG, "cuTensorMapEncodeIm2col failed: %s (dims %llu,%llu,%llu,%llu corners (%d,%d)..(%d,%d))", cu_err(r),
+                (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)dims[2], (unsigned long long)dims[3],
+                lower[0], lower[1], upper[0], upper[1]);
+  if (c->tmap_cache.size() > 512) c->tmap_cache.clear();
+  c->tmap_cache[key] = *out;
+  return B200_OK;
+}
+
+// Geometry of a 2-D convolution run as an implicit GEMM (b200_conv2d): x is NHWC with unit channel stride, w is
+// [Cout, KH * KW, C] with unit channel stride; strides in elements.
+struct ConvGeom {
+  uint64_t N, H, W, C, KH, KW, OH, OW, Cout;
+  int32_t sh, sw, ph, pw, dh, dw;
+  uint64_t x_sw, x_sh, x_sn;   // x: pixel (w), row (h) and image (n) strides
+  uint64_t w_sp, w_sco;        // w: kernel-position and output-channel strides
+};
+
 // One batched problem with LINEAR batch strides (0 = broadcast).  Strides in elements.
 struct GemmProblem {
   int in_dtype, out_dtype;
@@ -871,9 +929,12 @@ struct GemmProblem {
   int q = 0;
   uint32_t q_bk = 0;
   uint64_t q_sa = 0, q_sb = 0, q_ga = 0, q_gb = 0;
+  // 2-D convolution (b200_conv2d): a = x, b = w, M = N * OH * OW, N = Cout, K = KH * KW * (C padded to 64), batch 1
+  const ConvGeom* conv = nullptr;
 };
 
 static bool variant_has(const GemmVariant& v, const GemmProblem& g) {
+  if (g.conv) return !strcmp(v.tag, "2sm_n128") || !strcmp(v.tag, "1sm_n128");   // gemm_wgmma.cu: GEMM_PART 4
   if (g.q == 1 && v.block_n == 256) return false;   // the per-block fold has 128-wide tiles only (gemm_wgmma.cu: GEMM_Q)
   if (!strcmp(v.tag, "2sm_n224")) return g.mx;
   if (!strcmp(v.tag, "2sm_m512")) return !g.mx && (g.in_dtype == B200_BF16 || g.in_dtype == B200_F16);
@@ -1038,7 +1099,8 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
   if (best_sk.bad_option) return fail(B200_ERR_INVALID_ARG, "gemm.split_k must be auto, off, on or 1..8");
   const GemmVariant& v = *best;
 
-  const std::string name = std::string("gemm_") + in_tag + "_" + out_tag + "_" + v.tag + (a_mn ? "_m" : "_k") + (b_mn ? "n" : "k");
+  const std::string name = g.conv ? std::string("conv2d_") + in_tag + "_" + out_tag + "_" + v.tag
+                                  : std::string("gemm_") + in_tag + "_" + out_tag + "_" + v.tag + (a_mn ? "_m" : "_k") + (b_mn ? "n" : "k");
   CUfunction f;
   int rc = get_func(c, name, &f);
   if (rc) return rc;
@@ -1053,7 +1115,15 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
   CUtensorMap ta, tb;
   auto pad16 = [&](uint64_t elems) { const uint64_t q = 16 / esz; return (elems + q - 1) / q * q; };
   const uint32_t chunk = static_cast<uint32_t>(128 / esz);  // MN-major operands (16-bit): elements per 128-byte row
-  if (!a_mn) {
+  const uint32_t n_local = v.block_n / v.cg;   // B rows each CTA of a pair loads (multicast to both)
+  if (g.conv) {
+    // 128 output pixels x 64 channels per load, walking the input pixels the output grid reads at kernel position (0, 0)
+    const ConvGeom& cv = *g.conv;
+    const uint64_t dims[4] = {cv.C, cv.W, cv.H, cv.N}, strides[3] = {cv.x_sw, cv.x_sh, cv.x_sn};
+    const int lower[2] = {-cv.pw, -cv.ph};
+    const int upper[2] = {cv.pw - cv.dw * (int)(cv.KW - 1), cv.ph - cv.dh * (int)(cv.KH - 1)};
+    rc = encode_im2col(c, &ta, dt, esz, g.a, dims, strides, lower, upper, 64, 128, (uint32_t)cv.sw, (uint32_t)cv.sh);
+  } else if (!a_mn) {
     const uint64_t a_sm = g.M > 1 ? g.a_sm : pad16(g.K);
     rc = encode_tmap(c, &ta, dt, esz, g.a, g.K, g.M, a_bcast ? 1 : g.batch, a_sm, a_bcast ? a_sm * g.M : g.a_sb, block_k, 128);
   } else {
@@ -1061,8 +1131,11 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
     rc = encode_tmap(c, &ta, dt, esz, g.a, g.M, g.K, a_bcast ? 1 : g.batch, a_sk, a_bcast ? a_sk * g.K : g.a_sb, chunk, block_k);
   }
   if (rc) return rc;
-  const uint32_t n_local = v.block_n / v.cg;   // B rows each CTA of a pair loads (multicast to both)
-  if (!b_mn) {
+  if (g.conv) {
+    // [n_local output channels x 64 channels] of one kernel position
+    const ConvGeom& cv = *g.conv;
+    rc = encode_tmap(c, &tb, dt, esz, g.b, cv.C, cv.KH * cv.KW, cv.Cout, cv.w_sp, cv.w_sco, 64, 1, CU_TENSOR_MAP_SWIZZLE_128B, n_local);
+  } else if (!b_mn) {
     const uint64_t b_sn = g.N > 1 ? g.b_sn : pad16(g.K);
     rc = encode_tmap(c, &tb, dt, esz, g.b, g.K, g.N, b_bcast ? 1 : g.batch, b_sn, b_bcast ? b_sn * g.N : g.b_sb, block_k, n_local);
   } else {
@@ -1113,6 +1186,13 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
     p.hyb_nbb = b_bcast ? 1u : (uint32_t)g.batch;
   }
   if (g.q == 1) p.q_nsub = 128u / g.q_bk;
+  if (g.conv) {
+    const ConvGeom& cv = *g.conv;
+    p.cv_ohw = (uint32_t)(cv.OH * cv.OW); p.cv_ow = (uint32_t)cv.OW;
+    p.cv_cblk = (uint32_t)((cv.C + 63) / 64); p.cv_kw = (uint32_t)cv.KW;
+    p.cv_stride_h = cv.sh; p.cv_stride_w = cv.sw; p.cv_pad_h = cv.ph; p.cv_pad_w = cv.pw;
+    p.cv_dil_h = (uint32_t)cv.dh; p.cv_dil_w = (uint32_t)cv.dw;
+  }
   p.q_ga = g.q_ga; p.q_gb = g.q_gb;
   p.alpha = g.alpha; p.bias = g.bias; p.epi_act = g.act;
   p.epi_on = (g.alpha != 1.0f || g.bias != 0 || g.act != 0) ? 1u : 0u;
@@ -2451,6 +2531,166 @@ extern "C" int b200_matmul_quantized(b200_ctx* c, b200_stream s, const b200_quan
     g.q_sa = tmp[2]; g.q_sb = tmp[3];
   }
   if (!rc) rc = launch_wgmma(c, st, g, false, false);
+  for (CUdeviceptr t : tmp)
+    if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMM has drained
+  return rc;
+}
+
+// ------------------------------------------------------------------------------------------------ 2-D convolution
+// Strides of a rank-4 view with every extent-1 dimension given the stride a compact tensor would have there (the address of
+// its only index is unchanged), so layout tests do not trip over strides that are never used.
+static void conv_norm_strides(const uint64_t* shape, const uint64_t* strides, uint64_t* out) {
+  uint64_t inner = 1;
+  for (int d = 3; d >= 0; --d) {
+    out[d] = strides ? strides[d] : inner;
+    if (shape[d] == 1) out[d] = inner;
+    inner = out[d] * shape[d];
+  }
+}
+
+// Pooled copy of an operand seen as [batch, rows, C] (strides in elements) with C padded to `cp` zero channels (repitch_rows
+// writes the padding columns as zeros).
+static int conv_pad_channels(b200_ctx* c, CUstream st, uint64_t in, uint64_t batch, uint64_t rows, uint64_t C, uint64_t s_b,
+                             uint64_t s_r, uint64_t s_c, uint64_t cp, CUdeviceptr* out) {
+  CUdeviceptr buf;
+  int rc = pool_alloc(c, batch * rows * cp * 2, &buf, st);
+  if (rc) return rc;
+  CUfunction f;
+  rc = get_func(c, "repitch_rows", &f);
+  if (rc) { pool_free(c, buf, st); return rc; }
+  RepitchParams p{in, buf, batch, rows, C, s_b, s_r, s_c, cp, 2u, 0u};
+  const uint64_t vecs = batch * rows * (cp / 8);
+  const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((vecs + 255) / 256, 0x7FFFFFFFull));
+  void* args[] = {&p};
+  rc = launch(c, f, grid, 1, 1, 256, 0, 1, st, args);
+  if (rc) { pool_free(c, buf, st); return rc; }
+  *out = buf;
+  return B200_OK;
+}
+
+// A compact pooled copy of a rank-4 view (b200_into_contiguous).
+static int conv_gather(b200_ctx* c, CUstream st, b200_dtype dt, uint64_t in, const uint64_t* shape, const uint64_t* strides,
+                       CUdeviceptr* out) {
+  CUdeviceptr buf;
+  int rc = pool_alloc(c, shape[0] * shape[1] * shape[2] * shape[3] * 2, &buf, st);
+  if (rc) return rc;
+  rc = b200_into_contiguous(c, static_cast<b200_stream>(st), dt, in, buf, 4, shape, strides);
+  if (rc) { pool_free(c, buf, st); return rc; }
+  *out = buf;
+  return B200_OK;
+}
+
+extern "C" int b200_conv2d(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr x, const uint64_t* x_shape,
+                           const uint64_t* x_strides, b200_dptr w, const uint64_t* w_shape, const uint64_t* w_strides, b200_dptr out,
+                           const uint64_t* out_shape, const uint64_t* out_strides, const b200_conv2d_args* args, const b200_epilogue* ep) {
+  CTX_ENTER(c);
+  if (!x_shape || !w_shape || !out_shape || !args) return fail(B200_ERR_INVALID_ARG, "conv2d: null shape or args");
+  if (in_dtype != B200_F16 && in_dtype != B200_BF16)
+    return fail(B200_ERR_UNSUPPORTED, "conv2d: input dtype %d unsupported (f16, bf16)", (int)in_dtype);
+  if (out_dtype != in_dtype && out_dtype != B200_F32)
+    return fail(B200_ERR_UNSUPPORTED, "conv2d: output dtype must equal the input dtype or be f32");
+  if (ep && (ep->activation < 0 || ep->activation > 2)) return fail(B200_ERR_INVALID_ARG, "conv2d: unknown activation %d", ep->activation);
+  const b200_conv2d_args& a = *args;
+  if (a.stride_h < 1 || a.stride_w < 1 || a.dilation_h < 1 || a.dilation_w < 1 || a.pad_h < 0 || a.pad_w < 0)
+    return fail(B200_ERR_INVALID_ARG, "conv2d: strides and dilations must be >= 1 and padding >= 0");
+  const uint64_t N = x_shape[0], H = x_shape[1], W = x_shape[2], C = x_shape[3];
+  const uint64_t Cout = w_shape[0], KH = w_shape[1], KW = w_shape[2];
+  if (w_shape[3] != C)
+    return fail(B200_ERR_INVALID_ARG, "conv2d: weights have %llu channels, x has %llu", (unsigned long long)w_shape[3], (unsigned long long)C);
+  if (N == 0 || H == 0 || W == 0 || C == 0 || Cout == 0 || KH == 0 || KW == 0) return B200_OK;
+  const uint64_t lim = 1ull << 31;
+  if (N >= lim || H >= lim || W >= lim || C >= lim || Cout >= lim || KH >= lim || KW >= lim)
+    return fail(B200_ERR_UNSUPPORTED, "conv2d: extents must be < 2^31");
+  // PyTorch's output rule
+  const int64_t nh = (int64_t)H + 2 * (int64_t)a.pad_h - (int64_t)a.dilation_h * ((int64_t)KH - 1) - 1;
+  const int64_t nw = (int64_t)W + 2 * (int64_t)a.pad_w - (int64_t)a.dilation_w * ((int64_t)KW - 1) - 1;
+  if (nh < 0 || nw < 0) return fail(B200_ERR_INVALID_ARG, "conv2d: the dilated kernel is larger than the padded input (output extent < 1)");
+  const uint64_t OH = (uint64_t)(nh / a.stride_h) + 1, OW = (uint64_t)(nw / a.stride_w) + 1;
+  if (out_shape[0] != N || out_shape[1] != OH || out_shape[2] != OW || out_shape[3] != Cout)
+    return fail(B200_ERR_INVALID_ARG, "conv2d: out is [%llu,%llu,%llu,%llu], expected [%llu,%llu,%llu,%llu]", (unsigned long long)out_shape[0],
+                (unsigned long long)out_shape[1], (unsigned long long)out_shape[2], (unsigned long long)out_shape[3], (unsigned long long)N,
+                (unsigned long long)OH, (unsigned long long)OW, (unsigned long long)Cout);
+  // the 4-D im2col limits of the tensor map (cuda.h: cuTensorMapEncodeIm2col)
+  const int64_t corners[4] = {-(int64_t)a.pad_h, -(int64_t)a.pad_w, (int64_t)a.pad_h - (int64_t)a.dilation_h * ((int64_t)KH - 1),
+                              (int64_t)a.pad_w - (int64_t)a.dilation_w * ((int64_t)KW - 1)};
+  for (int64_t k : corners)
+    if (k < -128 || k > 127)
+      return fail(B200_ERR_UNSUPPORTED, "conv2d: im2col pixel-box corner %lld outside [-128, 127] (-pad and pad - dilation * (kernel - 1))", (long long)k);
+  if (a.stride_h > 8 || a.stride_w > 8) return fail(B200_ERR_UNSUPPORTED, "conv2d: im2col element stride (the conv stride) must be <= 8");
+  const uint64_t M = N * OH * OW;
+  if (M >= lim) return fail(B200_ERR_UNSUPPORTED, "conv2d: N * OH * OW = %llu must be < 2^31", (unsigned long long)M);
+  if (!x || !w || !out) return fail(B200_ERR_INVALID_ARG, "conv2d: null device pointer");
+  const size_t osz = dtype_size(out_dtype);
+  if (out % osz) return fail(B200_ERR_INVALID_ARG, "conv2d: output pointer is not aligned to its element size");
+  // out: unit channel stride, the three outer strides one pixel pitch >= Cout
+  uint64_t os[4];
+  conv_norm_strides(out_shape, out_strides, os);
+  if (os[3] != 1 || os[2] < Cout || os[1] != OW * os[2] || os[0] != OH * os[1])
+    return fail(B200_ERR_UNSUPPORTED, "conv2d: out must have unit channel stride and one pixel pitch >= Cout for N, OH, OW");
+  if (KH * KW * ((C + 63) / 64 * 64) >= lim) return fail(B200_ERR_UNSUPPORTED, "conv2d: KH * KW * C (C padded to 64) must be < 2^31");
+  CUstream st = resolve_stream(c, s);
+  uint64_t xs[4], ws[4];
+  conv_norm_strides(x_shape, x_strides, xs);
+  conv_norm_strides(w_shape, w_strides, ws);
+  // (KH, KW) as one kernel-position dimension: stride, or 0 when the view cannot be flattened
+  const uint64_t w_sp = (KW == 1) ? ws[1] : (KH == 1 || ws[1] == KW * ws[2]) ? ws[2] : 0;
+  const uint64_t x_spx = (W == 1) ? xs[1] : (H == 1 || xs[1] == W * xs[2]) ? xs[2] : 0;   // (H, W) as one pixel dimension
+  auto al = [](uint64_t e) { return e % 8 == 0 && e * 2 < (1ull << 40); };   // 16-byte multiple (16-bit elements)
+  ConvGeom g{};
+  g.N = N; g.H = H; g.W = W; g.KH = KH; g.KW = KW; g.OH = OH; g.OW = OW; g.Cout = Cout;
+  g.sh = a.stride_h; g.sw = a.stride_w; g.ph = a.pad_h; g.pw = a.pad_w; g.dh = a.dilation_h; g.dw = a.dilation_w;
+  CUdeviceptr tmp[4] = {0, 0, 0, 0};
+  uint64_t xa = x, wa = w;
+  int rc = B200_OK;
+  if (C % 8 == 0) {
+    g.C = C;
+    if (x % 16 == 0 && xs[3] == 1 && al(xs[0]) && al(xs[1]) && al(xs[2])) {
+      g.x_sw = xs[2]; g.x_sh = xs[1]; g.x_sn = xs[0];
+    } else {
+      rc = conv_gather(c, st, in_dtype, x, x_shape, xs, &tmp[0]);
+      xa = tmp[0];
+      g.x_sw = C; g.x_sh = W * C; g.x_sn = H * W * C;
+    }
+    if (!rc && w % 16 == 0 && ws[3] == 1 && w_sp != 0 && al(w_sp) && al(ws[0])) {
+      g.w_sp = w_sp; g.w_sco = ws[0];
+    } else if (!rc) {
+      rc = conv_gather(c, st, in_dtype, w, w_shape, ws, &tmp[1]);
+      wa = tmp[1];
+      g.w_sp = C; g.w_sco = KH * KW * C;
+    }
+  } else {
+    // rows of C * 2 bytes are not 16-byte multiples: TMA cannot describe them.  Both operands are copied with C padded to a
+    // multiple of 8 zero channels (first gathered when their spatial dimensions do not flatten into one strided dimension)
+    const uint64_t cp = (C + 7) / 8 * 8;
+    g.C = cp;
+    uint64_t xin = x, xsb = xs[0], xsp = x_spx, xsc = xs[3];
+    if (x_spx == 0) {
+      rc = conv_gather(c, st, in_dtype, x, x_shape, xs, &tmp[0]);
+      xin = tmp[0]; xsb = H * W * C; xsp = C; xsc = 1;
+    }
+    if (!rc) rc = conv_pad_channels(c, st, xin, N, H * W, C, xsb, xsp, xsc, cp, &tmp[2]);
+    xa = tmp[2];
+    g.x_sw = cp; g.x_sh = W * cp; g.x_sn = H * W * cp;
+    uint64_t win = w, wsb = ws[0], wsp = w_sp, wsc = ws[3];
+    if (!rc && w_sp == 0) {
+      rc = conv_gather(c, st, in_dtype, w, w_shape, ws, &tmp[1]);
+      win = tmp[1]; wsb = KH * KW * C; wsp = C; wsc = 1;
+    }
+    if (!rc) rc = conv_pad_channels(c, st, win, Cout, KH * KW, C, wsb, wsp, wsc, cp, &tmp[3]);
+    wa = tmp[3];
+    g.w_sp = cp; g.w_sco = KH * KW * cp;
+  }
+  if (!rc) {
+    GemmProblem gp{};
+    gp.in_dtype = in_dtype; gp.out_dtype = out_dtype;
+    gp.a = xa; gp.b = wa; gp.out = out;
+    gp.M = M; gp.N = Cout; gp.K = KH * KW * ((g.C + 63) / 64 * 64); gp.batch = 1;
+    gp.a_sm = gp.K; gp.a_sk = 1; gp.b_sn = gp.K; gp.b_sk = 1;
+    gp.o_sm = os[2]; gp.o_sn = 1; gp.o_sb = 0;
+    if (ep) { gp.alpha = ep->alpha; gp.bias = ep->bias; gp.act = (uint32_t)ep->activation; }
+    gp.conv = &g;
+    rc = launch_wgmma(c, st, gp, false, false);
+  }
   for (CUdeviceptr t : tmp)
     if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMM has drained
   return rc;

@@ -141,11 +141,18 @@ __device__ __forceinline__ uint32_t acc_bits(uint32_t x) { return x; }
 //              tma_a_lo / tma_b_lo into a region after the operand ring.
 //   QM_TENSOR  one f32 scale per side: the s8 mainloop into s32 accumulators; the epilogue stores rn(f32(D) * rn(g_a * g_b)).
 enum : int { QM_NONE = 0, QM_BLOCK = 1, QM_TENSOR = 2 };
-template <int CG, int BLOCK_N, bool A_MN, bool B_MN, int KIND, int OUT, int STAGES, bool PROMOTE = false, int MT = 1, int QM = QM_NONE>
+// CONV (2-D convolution as an implicit GEMM; capi.cpp: b200_conv2d): the A tile of k-block kb is one im2col load -- 128
+// consecutive output pixels x 64 channels of kernel position kb / cv_cblk, channel block kb % cv_cblk -- which TMA writes in
+// exactly the 128B-swizzled [128 rows x 128 B] layout of a K-major A tile; B is the weights' [n_local x 64 channels] box of
+// that (kernel position, channel block).  Channels past C read as zero on both sides.  Everything after the load is the GEMM.
+template <int CG, int BLOCK_N, bool A_MN, bool B_MN, int KIND, int OUT, int STAGES, bool PROMOTE = false, int MT = 1, int QM = QM_NONE,
+          bool CONV = false>
 __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUtensorMap* tma_b_hi, const CUtensorMap* tma_a_lo,
                                           const CUtensorMap* tma_b_lo, const CUtensorMap* tma_out, const GemmParams& p) {
   constexpr bool INT_ACC = (KIND == KIND_U8 || KIND == KIND_S8) && QM != QM_BLOCK;
   static_assert(QM == QM_NONE || (KIND == KIND_S8 && !A_MN && !B_MN && !PROMOTE && MT == 1), "quantized operands: s8, K-major");
+  static_assert(!CONV || ((KIND == KIND_BF16 || KIND == KIND_F16) && !A_MN && !B_MN && !PROMOTE && MT == 1 && QM == QM_NONE),
+                "convolution: 16-bit kinds, K-major operands");
   // per-block scale tiles of one stage, sized for the finest block (Bk = 32: four blocks per 128-element stage)
   constexpr uint32_t SC_A_BYTES = (QM == QM_BLOCK) ? 128u * 4u * 4u : 0u;
   constexpr uint32_t SC_STAGE_BYTES = (QM == QM_BLOCK) ? SC_A_BYTES + BLOCK_N * 4u * 4u : 0u;
@@ -226,11 +233,32 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
         const int ba = static_cast<int>(tc.b * p.a_bmul), bb = static_cast<int>(tc.b * p.b_bmul);
         uint32_t seg, kk;  // segment (0 unless k_segments == 3), k-block within it
         seg_of(wu.kb0, seg, kk);
+        // convolution: input pixel of the tile's first row (output pixel (n, oh, ow) at kernel position (0, 0)), once per tile
+        int cv_w = 0, cv_h = 0, cv_n = 0;
+        if constexpr (CONV) {
+          const uint32_t mu = static_cast<uint32_t>(m0), n = mu / p.cv_ohw, r = mu - n * p.cv_ohw, oh = r / p.cv_ow;
+          cv_n = static_cast<int>(n);
+          cv_h = static_cast<int>(oh) * p.cv_stride_h - p.cv_pad_h;
+          cv_w = static_cast<int>(r - oh * p.cv_ow) * p.cv_stride_w - p.cv_pad_w;
+        }
         for (uint32_t kb = wu.kb0; kb < wu.kb1; ++kb) {
           mbar_wait(empty_bar(s), ph ^ 1);   // every consumer of the pair has released the stage
           const uint32_t sa = smem_base + s * STAGE_BYTES;
           const uint32_t sb = sa + A_BYTES;
           const uint32_t fb = full_bar(s);
+          if constexpr (CONV) {
+            mbar_arrive_expect_tx(fb, STAGE_BYTES);
+            const uint32_t kpos = kb / p.cv_cblk, cb = kb - kpos * p.cv_cblk;
+            const uint32_t ky = kpos / p.cv_kw, kx = kpos - ky * p.cv_kw;
+            const int c0 = static_cast<int>(cb * 64u);
+            tma_load_im2col_4d(sa, tma_a_hi, fb, c0, cv_w, cv_h, cv_n, static_cast<uint16_t>(kx * p.cv_dil_w),
+                               static_cast<uint16_t>(ky * p.cv_dil_h));
+            const int n_row = nb0 + static_cast<int>(rank * N_LOCAL);
+            if constexpr (CG == 2) tma_load_3d_mc(sb + rank * N_LOCAL * 128u, tma_b_hi, fb, static_cast<uint16_t>(3), c0, static_cast<int>(kpos), n_row);
+            else tma_load_3d(sb, tma_b_hi, fb, c0, static_cast<int>(kpos), n_row);
+            if (++s == STAGES) { s = 0; ph ^= 1; }
+            continue;
+          }
           if constexpr (QM == QM_BLOCK) {
             // the scale tiles of this stage: A rows of this CTA, and every column of the B tile (each CTA of a pair loads
             // its own copy, no multicast)
@@ -652,11 +680,27 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
   GEMM_KERNEL_Q(gemm_q8_f32_##TILE##_kk, CG, BN, OUT_F32, QSTAGES, QM_BLOCK)               \
   GEMM_Q8T(TILE, CG, BN, STAGES)
 
-// The kernels are built as four cubins from this one source (cubecl_b200/build.py compiles them in parallel):
-//   GEMM_PART 0 ("gemm")    256 x 256 pair tiles (2-CTA cluster, 128 x 256 per CTA) and the bf16 peak probe
-//   GEMM_PART 1 ("gemm_b")  256 x 128 pair tiles, 256 x 224 block-scaled pair tiles
-//   GEMM_PART 2 ("gemm_c")  128 x 128 single-CTA tiles, 512 x 128 pair tiles
-//   GEMM_PART 3 ("gemm_q")  the quantized-operand kernels of every tile
+// 2-D convolution (implicit GEMM, CONV): tma_a = im2col map of x, tma_b = 3-D weight map; tma_a_lo / tma_b_lo are unused
+// name: conv2d_<in>_<out>_<tile>
+#define CONV_KERNEL(NAME, CG, BN, KIND, OUT, STAGES)                                                                \
+  extern "C" __global__ void __launch_bounds__(kNumThreads, 1)                                                     \
+      NAME(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,                  \
+           const __grid_constant__ CUtensorMap tma_a_lo, const __grid_constant__ CUtensorMap tma_b_lo,            \
+           const __grid_constant__ CUtensorMap tma_out, const __grid_constant__ GemmParams p) {                    \
+    gemm_body<CG, BN, false, false, KIND, OUT, STAGES, false, 1, QM_NONE, true>(&tma_a, &tma_b, &tma_a_lo, &tma_b_lo, &tma_out, p); \
+  }
+#define CONV_DTYPES(TILE, CG, BN, STAGES)                                  \
+  CONV_KERNEL(conv2d_bf16_bf16_##TILE, CG, BN, KIND_BF16, OUT_BF16, STAGES) \
+  CONV_KERNEL(conv2d_bf16_f32_##TILE, CG, BN, KIND_BF16, OUT_F32, STAGES)   \
+  CONV_KERNEL(conv2d_f16_f16_##TILE, CG, BN, KIND_F16, OUT_F16, STAGES)     \
+  CONV_KERNEL(conv2d_f16_f32_##TILE, CG, BN, KIND_F16, OUT_F32, STAGES)
+
+// The kernels are built as five cubins from this one source (cubecl_b200/build.py compiles them in parallel):
+//   GEMM_PART 0 ("gemm")       256 x 256 pair tiles (2-CTA cluster, 128 x 256 per CTA) and the bf16 peak probe
+//   GEMM_PART 1 ("gemm_b")     256 x 128 pair tiles, 256 x 224 block-scaled pair tiles
+//   GEMM_PART 2 ("gemm_c")     128 x 128 single-CTA tiles, 512 x 128 pair tiles
+//   GEMM_PART 3 ("gemm_q")     the quantized-operand kernels of every tile
+//   GEMM_PART 4 ("gemm_conv")  the 2-D convolution kernels of the 2sm_n128 and 1sm_n128 tiles
 #ifndef GEMM_PART
 #define GEMM_PART 0
 #endif
@@ -699,6 +743,12 @@ GEMM_M512(gemm_f16_bf16, KIND_F16, OUT_BF16)
 GEMM_Q8T(2sm_n256, 2, 256, 4)
 GEMM_Q(2sm_n128, 2, 128, 6, 5)
 GEMM_Q(1sm_n128, 1, 128, 6, 5)
+#endif
+#if GEMM_PART == 4
+// the stage counts of the GEMM tiles of the same shape.  No 256 x 256 tile: with 128 accumulators per thread its consumer
+// spills at the 168 registers a thread of a 384-thread CTA gets (as gemm_*_2sm_n256_kk does), and these kernels do not spill
+CONV_DTYPES(2sm_n128, 2, 128, 6)
+CONV_DTYPES(1sm_n128, 1, 128, 6)
 #endif
 
 #if GEMM_PART == 0

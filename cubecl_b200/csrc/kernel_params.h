@@ -50,6 +50,13 @@ struct GemmParams {
   // kernels); q_ga / q_gb = device pointers of the two f32 tensor scales (per-tensor kernels).
   uint32_t q_nsub, q_pad;
   uint64_t q_ga, q_gb;
+  // 2-D convolution as an implicit GEMM (conv2d_* kernels; capi.cpp: b200_conv2d): GEMM row m is output pixel
+  // (n, oh, ow) = (m / cv_ohw, (m % cv_ohw) / cv_ow, m % cv_ow), and K runs over (kernel position, 64-channel block) with
+  // cv_cblk channel blocks per position.  tma_a_hi is a 4-D im2col map of x (C, W, H, N); tma_b_hi a 3-D map of the weights
+  // (C, KH * KW, Cout).  K = KH * KW * cv_cblk * 64.
+  uint32_t cv_ohw, cv_ow, cv_cblk, cv_kw;
+  int32_t cv_stride_h, cv_stride_w, cv_pad_h, cv_pad_w;
+  uint32_t cv_dil_h, cv_dil_w;
 };
 
 // ================================================================================================ aux_kernels.cu

@@ -141,6 +141,19 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* m, 
       : "memory");
 }
 
+// 4-D im2col load of an NHWC tensor: `pixelsPerColumn` pixels x `channelsPerPixel` channels, starting at pixel (n, h, w)
+// and walking the map's pixel bounding box in W, then H, then N order (with the map's element strides); every pixel is
+// read at (h + off_h, w + off_w), channels from c.  Out-of-bounds elements are zero-filled.
+__device__ __forceinline__ void tma_load_im2col_4d(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c, int w, int h, int n,
+                                                   uint16_t off_w, uint16_t off_h) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes"
+      " [%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8};"
+      :
+      : "r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c), "r"(w), "r"(h), "r"(n), "h"(off_w), "h"(off_h)
+      : "memory");
+}
+
 // Multicast 3-D load: the box lands at the same smem offset in every CTA of `mask`, each CTA's own barrier
 // (same offset) receives the complete_tx.
 __device__ __forceinline__ void tma_load_3d_mc(uint32_t dst, const CUtensorMap* m, uint32_t bar, uint16_t mask, int c0,

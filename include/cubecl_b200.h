@@ -82,7 +82,7 @@ typedef struct b200_props {
 /* ---- lifecycle: R::client(device) -> DeviceService::init (cubecl-cuda/src/runtime.rs:52-350) ------------------------ */
 int b200_abi_version(void);
 int b200_device_count(int* count);
-/* The embedded prebuilt sm_90a images ("gemm" | "gemm_b" | "gemm_c" | "reduce" | "aux" | "quant" | "gemm_q" | "quant_mm"), for a host that prefers to cuModuleLoadData them into
+/* The embedded prebuilt sm_90a images ("gemm" | "gemm_b" | "gemm_c" | "reduce" | "aux" | "quant" | "gemm_q" | "quant_mm" | "gemm_conv"), for a host that prefers to cuModuleLoadData them into
  * its own module cache (CudaContext::modules, crates/cubecl-cuda/src/compute/context.rs:38-62,293). No GPU needed. */
 int b200_get_cubin(const char* name, const void** image, size_t* size);
 int b200_init(int device, b200_ctx** out);   /* cuInit, primary ctx retain, load the embedded sm_90a cubins (context.rs:293) */
@@ -312,6 +312,34 @@ typedef struct b200_quant_operand {
 } b200_quant_operand;
 int b200_matmul_quantized(b200_ctx* ctx, b200_stream s, const b200_quant_operand* lhs, const b200_quant_operand* rhs,
                           b200_dtype out_dtype, b200_dptr out, uint64_t batch, uint64_t m, uint64_t n, uint64_t k);
+
+/* ---- 2-D convolution (cubek's convolution kernels), an implicit GEMM on the wgmma kernel --------------------------------
+ * out[n, oh, ow, co] = act(alpha * sum_{ky, kx, c} x[n, oh*sh - ph + ky*dh, ow*sw - pw + kx*dw, c] * w[co, ky, kx, c] + bias[co]).
+ * Input outside x reads as zero; f32 accumulation; the epilogue is b200_epilogue (NULL = none).  x is [N, H, W, C] (NHWC), w is
+ * [Cout, KH, KW, C], out is [N, OH, OW, Cout] with OH = floor((H + 2*ph - dh*(KH-1) - 1) / sh) + 1 and OW likewise (PyTorch's
+ * rule).  Shapes and strides in elements; NULL strides = compact.
+ * Dtypes: F16 or BF16 inputs; out_dtype the input dtype or F32 (the rule of b200_matmul); anything else B200_ERR_UNSUPPORTED.
+ * Views: x with unit channel stride and 16-byte aligned base and strides, and w whose (KH, KW) flatten into one stride with
+ * the same alignment, are read in place (compact NHWC x and compact [Cout, KH, KW, C] w are); any other view (NCHW x, PyTorch's
+ * OIHW weights passed as a stride-permuted view) is first gathered with b200_into_contiguous.  out needs a unit channel
+ * stride and outer strides that flatten to one pixel pitch >= Cout (a channel slice of a wider NHWC tensor is fine).  When
+ * C * 2 bytes is not a multiple of 16 (e.g. an RGB stem, C = 3) both operands are copied with C padded to a multiple of 8
+ * zero channels.
+ * Errors: B200_ERR_INVALID_ARG for a channel mismatch, a wrong out_shape, OH or OW < 1, stride / dilation < 1, negative padding,
+ * an unknown activation or a null pointer; B200_ERR_UNSUPPORTED for shapes outside the 4-D im2col limits: pixel-box corners
+ * -p and p - d*(K-1) in [-128, 127], conv strides <= 8, N*OH*OW < 2^31.  An extent of 0 in x or w is a no-op.
+ * Launches: 1 (the GEMM) for in-place operands; +1 per gathered operand; when C * 2 % 16 != 0, +1 per operand (the channel
+ * padding copy) and +1 more for an operand whose spatial dimensions do not flatten into one stride.  Stream-ordered, no host
+ * sync, temporaries from the pool; bitwise reproducible for a fixed shape, dtypes and SM count.  The tile is chosen like
+ * b200_matmul's ("gemm.variant" 2sm_n128 | 1sm_n128, "gemm.split_k", "gemm.epilogue" apply). */
+typedef struct b200_conv2d_args {
+  int32_t stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w;
+} b200_conv2d_args;
+int b200_conv2d(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype,
+                b200_dptr x, const uint64_t* x_shape, const uint64_t* x_strides,
+                b200_dptr w, const uint64_t* w_shape, const uint64_t* w_strides,
+                b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides,
+                const b200_conv2d_args* args, const b200_epilogue* epilogue);
 
 /* ---- collectives: ServerCommunication (server/base.rs:632-739), CUDA impl cubecl-cuda/src/compute/server.rs:666-926 -- */
 #define B200_UNIQUE_ID_BYTES 128

@@ -220,6 +220,22 @@ inline void launch_quantized(ComputeClient& client, const b200_quant_operand& lh
 }
 }  // namespace matmul
 
+namespace conv {
+/// 2-D convolution: x [N, H, W, C] (NHWC), w [Cout, KH, KW, C], out [N, OH, OW, Cout]; f32 accumulation, optional fused epilogue
+/// (nullptr = none).  See b200_conv2d in cubecl_b200.h for the contract.  Errors are deferred to client.sync().
+inline void launch(ComputeClient& client, const TensorHandle& x, const TensorHandle& w, const TensorHandle& out,
+                   const b200_conv2d_args& args, const b200_epilogue* epilogue = nullptr) {
+  if (x.shape.size() != 4 || w.shape.size() != 4 || out.shape.size() != 4 || x.dtype != w.dtype) {
+    client.defer("InvalidArgument: conv2d needs rank-4 x, w and out, and x and w of one dtype");
+    return;
+  }
+  const int rc = b200_conv2d(client.raw(), nullptr, static_cast<b200_dtype>(x.dtype), static_cast<b200_dtype>(out.dtype),
+                             x.handle.ptr(), x.shape.data(), x.strides.data(), w.handle.ptr(), w.shape.data(), w.strides.data(),
+                             out.handle.ptr(), out.shape.data(), out.strides.data(), &args, epilogue);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+}  // namespace conv
+
 namespace reduce {
 enum class Op : int { Sum = B200_REDUCE_SUM, Prod = B200_REDUCE_PROD, Max = B200_REDUCE_MAX, Min = B200_REDUCE_MIN,
                       ArgMax = B200_REDUCE_ARGMAX, ArgMin = B200_REDUCE_ARGMIN, Mean = B200_REDUCE_MEAN };

@@ -248,3 +248,46 @@ pub mod quant {
         )
     }
 }
+
+pub mod conv {
+    use super::*;
+
+    /// [N, OH, OW, Cout] of x [N, H, W, C] and w [Cout, KH, KW, C]; PyTorch's rule
+    /// OH = (H + 2 pad_h - dilation_h (KH - 1) - 1) / stride_h + 1, OW likewise.  `args` as [`Context::conv2d`].
+    pub fn calculate_conv2d_output(x: &[u64], w: &[u64], args: [i32; 6]) -> Result<Vec<u64>, Error> {
+        if x.len() != 4 || w.len() != 4 {
+            return Err(invalid("conv2d needs rank-4 x [N, H, W, C] and w [Cout, KH, KW, C]".to_string()));
+        }
+        if x[3] != w[3] {
+            return Err(invalid(format!("channels differ: x has {}, w has {}", x[3], w[3])));
+        }
+        let [sh, sw, ph, pw, dh, dw] = args.map(i64::from);
+        if sh < 1 || sw < 1 || dh < 1 || dw < 1 || ph < 0 || pw < 0 {
+            return Err(invalid("strides and dilations must be >= 1 and padding >= 0".to_string()));
+        }
+        let nh = x[1] as i64 + 2 * ph - dh * (w[1] as i64 - 1) - 1;
+        let nw = x[2] as i64 + 2 * pw - dw * (w[2] as i64 - 1) - 1;
+        if nh < 0 || nw < 0 {
+            return Err(invalid("the dilated kernel is larger than the padded input".to_string()));
+        }
+        Ok(vec![x[0], (nh / sh + 1) as u64, (nw / sw + 1) as u64, w[0]])
+    }
+
+    /// `conv::launch(client, x, w, out, ...)`: NHWC 2-D convolution on the wgmma GEMM with the input loaded through TMA im2col.
+    ///
+    /// # Safety
+    /// As [`super::matmul::launch`]; `epilogue.bias` must be 0 or an f32[Cout] device allocation.
+    pub unsafe fn launch(
+        ctx: &mut Context, stream: b200_stream, x: &TensorHandle, w: &TensorHandle, out: &TensorHandle, args: [i32; 6],
+        epilogue: Option<&Epilogue>,
+    ) -> Result<(), Error> {
+        if x.dtype != w.dtype {
+            return Err(invalid("x and w dtypes differ".to_string()));
+        }
+        let expect = calculate_conv2d_output(&x.shape, &w.shape, args)?;
+        if expect != out.shape {
+            return Err(invalid(format!("out shape {:?} != {:?}", out.shape, expect)));
+        }
+        ctx.conv2d(stream, x.dtype, out.dtype, &x.view(), &w.view(), &out.view(), args, epilogue)
+    }
+}

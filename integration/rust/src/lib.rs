@@ -358,6 +358,28 @@ impl Context {
         ))
     }
 
+    /// 2-D convolution: x [N, H, W, C] (NHWC), w [Cout, KH, KW, C], out [N, OH, OW, Cout], f32 accumulation, optional fused
+    /// epilogue; `args` = (stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w).  See b200_conv2d in cubecl_b200.h.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::matmul`]; `epilogue.bias` must be 0 or an f32[Cout] device allocation.
+    pub unsafe fn conv2d(
+        &mut self, stream: b200_stream, in_dtype: DType, out_dtype: DType, x: &TensorView, w: &TensorView, out: &TensorView,
+        args: [i32; 6], epilogue: Option<&Epilogue>,
+    ) -> Result<(), Error> {
+        assert!(x.shape.len() == 4 && w.shape.len() == 4 && out.shape.len() == 4);
+        assert!(x.strides.len() == 4 && w.strides.len() == 4 && out.strides.len() == 4);
+        let a = sys::b200_conv2d_args {
+            stride_h: args[0], stride_w: args[1], pad_h: args[2], pad_w: args[3], dilation_h: args[4], dilation_w: args[5],
+        };
+        let e = epilogue.map(|e| sys::b200_epilogue { alpha: e.alpha, activation: e.activation as i32, bias: e.bias });
+        check(sys::b200_conv2d(
+            self.0, stream, in_dtype as c_int, out_dtype as c_int, x.ptr, x.shape.as_ptr(), x.strides.as_ptr(), w.ptr,
+            w.shape.as_ptr(), w.strides.as_ptr(), out.ptr, out.shape.as_ptr(), out.strides.as_ptr(), &a,
+            e.as_ref().map_or(std::ptr::null(), |e| e as *const sys::b200_epilogue),
+        ))
+    }
+
     /// Block-scaled (MX / NVFP4) matmul: lhs [batch, m, k], rhs [batch, n, k] K-contiguous, scales per `scale_block`
     /// (32: ue8m0, 16: e4m3) elements of K; replaces `MmaDefinition::new_scaled` / `execute_scaled` tiles
     /// (crates/cubecl-core/src/frontend/cmma.rs:438-460, 798-840) at GEMM level.
