@@ -6,6 +6,12 @@ out[n, oh, ow, co] = act(alpha * sum_{ky, kx, c} x[n, oh*sh - ph + ky*dh, ow*sw 
 x is NHWC [N, H, W, C], w is [Cout, KH, KW, C], out is NHWC [N, OH, OW, Cout]; input outside x reads as zero, f32
 accumulation.  The kernel behind it is the wgmma GEMM of csrc/gemm_wgmma.cu with its A tile loaded through a TMA im2col
 map (an implicit GEMM: M = N * OH * OW output pixels, N = Cout, K = KH * KW * C), see include/cubecl_b200.h (b200_conv2d).
+
+The gradients (b200_conv2d_backward_data / _weight) run on the same GEMM kernel:
+  dx = backward_data(dy, w):    stride 1: a convolution of dy with the flipped, channel-transposed weights; stride > 1: one such
+                                convolution per output phase (h % sh, w % sw), each storing its pixels straight into dx.
+  dw = backward_weight(x, dy):  M = Cout, N = KH * KW * C, K = N * OH * OW pixels, with x read through im2col loads.
+The bias gradient is reduce.launch(client, "sum", dy viewed as [N * OH * OW, Cout], axis=0): no separate entry point.
 """
 from __future__ import annotations
 
@@ -85,3 +91,68 @@ def launch_alloc(client: ComputeClient, x: TensorHandle, w: TensorHandle, out_dt
     out = TensorHandle.empty_contiguous(client, shape, out_dtype or x.dtype)
     launch(client, x, w, out, **kwargs)
     return out
+
+
+def _check_grad_operands(what: str, a: TensorHandle, b: TensorHandle, out: TensorHandle) -> None:
+    if len(a.shape) != 4 or len(b.shape) != 4 or len(out.shape) != 4:
+        raise B200Error(6, f"{what}: every operand must have rank 4")
+    if a.dtype != b.dtype:
+        raise B200Error(6, f"{what}: operand dtypes differ ({a.dtype}, {b.dtype})")
+
+
+def backward_data(client: ComputeClient, dy: TensorHandle, w: TensorHandle, dx: TensorHandle, stride=1, padding=0, dilation=1,
+                  stream=None) -> None:
+    """Enqueue dx = the gradient of conv2d with respect to its input: dy [N, OH, OW, Cout], w [Cout, KH, KW, C], dx
+    [N, H, W, C] (NHWC), with dy's shape the output rule of (dx, w).  Errors are deferred like launch."""
+    try:
+        _check_grad_operands("conv2d_backward_data", dy, w, dx)
+        (sh, sw), (ph, pw), (dh, dw) = _pair(stride, "stride"), _pair(padding, "padding"), _pair(dilation, "dilation")
+        for t in (dy, w, dx):
+            t.handle.used_on(stream)
+        args = _ffi.Conv2dArgs(sh, sw, ph, pw, dh, dw)
+        _ffi.check(client._lib.b200_conv2d_backward_data(
+            client._ctx, stream, DTYPES[dy.dtype], DTYPES[dx.dtype],
+            C.c_uint64(dy.handle.ptr), _ffi.u64_array(dy.shape), _ffi.u64_array(dy.strides),
+            C.c_uint64(w.handle.ptr), _ffi.u64_array(w.shape), _ffi.u64_array(w.strides),
+            C.c_uint64(dx.handle.ptr), _ffi.u64_array(dx.shape), _ffi.u64_array(dx.strides), C.byref(args)))
+    except (B200Error, ValueError) as e:
+        client._defer(e if isinstance(e, B200Error) else B200Error(6, str(e)))
+
+
+def backward_data_alloc(client: ComputeClient, dy: TensorHandle, w: TensorHandle, input_hw, out_dtype: str | None = None,
+                        **kwargs) -> TensorHandle:
+    """Convenience: allocate a compact NHWC dx [N, H, W, C] with (H, W) = input_hw (the forward input's extents; a stride > 1
+    convolution maps several H to one OH), then backward_data (keyword arguments as backward_data)."""
+    h, wd = _pair(input_hw, "input_hw")
+    dx = TensorHandle.empty_contiguous(client, [dy.shape[0], h, wd, w.shape[3]], out_dtype or dy.dtype)
+    backward_data(client, dy, w, dx, **kwargs)
+    return dx
+
+
+def backward_weight(client: ComputeClient, x: TensorHandle, dy: TensorHandle, dw: TensorHandle, stride=1, padding=0, dilation=1,
+                    stream=None) -> None:
+    """Enqueue dw = the gradient of conv2d with respect to its weights: x [N, H, W, C], dy [N, OH, OW, Cout], dw
+    [Cout, KH, KW, C], with dy's shape the output rule of (x, dw).  Errors are deferred like launch."""
+    try:
+        _check_grad_operands("conv2d_backward_weight", x, dy, dw)
+        (sh, sw), (ph, pw), (dh, dw_) = _pair(stride, "stride"), _pair(padding, "padding"), _pair(dilation, "dilation")
+        for t in (x, dy, dw):
+            t.handle.used_on(stream)
+        args = _ffi.Conv2dArgs(sh, sw, ph, pw, dh, dw_)
+        _ffi.check(client._lib.b200_conv2d_backward_weight(
+            client._ctx, stream, DTYPES[x.dtype], DTYPES[dw.dtype],
+            C.c_uint64(x.handle.ptr), _ffi.u64_array(x.shape), _ffi.u64_array(x.strides),
+            C.c_uint64(dy.handle.ptr), _ffi.u64_array(dy.shape), _ffi.u64_array(dy.strides),
+            C.c_uint64(dw.handle.ptr), _ffi.u64_array(dw.shape), _ffi.u64_array(dw.strides), C.byref(args)))
+    except (B200Error, ValueError) as e:
+        client._defer(e if isinstance(e, B200Error) else B200Error(6, str(e)))
+
+
+def backward_weight_alloc(client: ComputeClient, x: TensorHandle, dy: TensorHandle, kernel_hw, out_dtype: str | None = None,
+                          **kwargs) -> TensorHandle:
+    """Convenience: allocate a compact dw [Cout, KH, KW, C] with (KH, KW) = kernel_hw, then backward_weight (keyword arguments
+    as backward_weight)."""
+    kh, kw = _pair(kernel_hw, "kernel_hw")
+    dw = TensorHandle.empty_contiguous(client, [dy.shape[3], kh, kw, x.shape[3]], out_dtype or x.dtype)
+    backward_weight(client, x, dy, dw, **kwargs)
+    return dw

@@ -442,3 +442,31 @@ extern "C" __global__ void __launch_bounds__(256) repitch_rows(const __grid_cons
     reinterpret_cast<uint4*>(p.out)[row * vpr + cv] = make_uint4(w[0], w[1], w[2], w[3]);
   }
 }
+
+// ------------------------------------------------------------------------------------------------ convolution backward
+// Weights of every data-gradient phase (see ConvDgradWeightsParams): w'[c, th, tw, co] = w[co, ky, kx, c] with the taps of
+// each phase in ascending dy-offset order.  A block transposes one 32 (co) x 32 (c) tile of one kernel position through
+// shared memory, so both the reads (along c) and the writes (along co) are coalesced.  grid = (c tiles * co tiles, KH * KW).
+extern "C" __global__ void __launch_bounds__(256) conv_dgrad_weights(const __grid_constant__ ConvDgradWeightsParams p) {
+  __shared__ uint16_t tile[32][33];
+  const uint32_t kpos = blockIdx.y, ky = kpos / p.KW, kx = kpos - ky * p.KW;
+  const uint64_t c_tiles = (p.C + 31) / 32;
+  const uint64_t c0 = (blockIdx.x % c_tiles) * 32, co0 = (blockIdx.x / c_tiles) * 32;
+  const uint32_t tx = threadIdx.x & 31u, ty = threadIdx.x >> 5;
+  const uint16_t* w = reinterpret_cast<const uint16_t*>(p.w);
+  for (uint32_t r = ty; r < 32; r += 8) {
+    const uint64_t co = co0 + r, c = c0 + tx;
+    tile[r][tx] = (co < p.Cout && c < p.C) ? w[co * p.s_co + ky * p.s_ky + kx * p.s_kx + c * p.s_c] : static_cast<uint16_t>(0);
+  }
+  __syncthreads();
+  // phase of this kernel position and its tap index inside the phase
+  const uint32_t rh = (ky * p.dh + p.sh * p.ph - p.ph) % p.sh, rw = (kx * p.dw + p.sw * p.pw - p.pw) % p.sw;
+  const uint32_t th = (p.kmax_h[rh] - ky) / p.qh, tw = (p.kmax_w[rw] - kx) / p.qw;
+  const uint64_t base = p.off[rh * p.sw + rw] + (static_cast<uint64_t>(th) * p.taps_w[rw] + tw) * p.cp;
+  const uint64_t c_pitch = static_cast<uint64_t>(p.taps_h[rh]) * p.taps_w[rw] * p.cp;
+  uint16_t* out = reinterpret_cast<uint16_t*>(p.out);
+  for (uint32_t r = ty; r < 32; r += 8) {
+    const uint64_t c = c0 + r, co = co0 + tx;
+    if (c < p.C && co < p.cp) out[base + c * c_pitch + co] = tile[tx][r];
+  }
+}

@@ -47,6 +47,8 @@ extern const unsigned char b200_cubin_quant_mm[];
 extern const unsigned char b200_cubin_quant_mm_end[];
 extern const unsigned char b200_cubin_gemm_conv[];
 extern const unsigned char b200_cubin_gemm_conv_end[];
+extern const unsigned char b200_cubin_gemm_convbwd[];
+extern const unsigned char b200_cubin_gemm_convbwd_end[];
 }
 
 // ================================================================================================ errors
@@ -72,7 +74,7 @@ extern "C" int b200_abi_version(void) { return B200_ABI_VERSION; }
   X(cuModuleLoadData) X(cuModuleUnload) X(cuModuleGetFunction) X(cuFuncSetAttribute) X(cuFuncGetAttribute)           \
   X(cuLaunchKernelEx) X(cuLaunchKernel) X(cuOccupancyMaxActiveClusters)                                              \
   X(cuMemAlloc) X(cuMemFree) X(cuMemAllocHost) X(cuMemFreeHost) X(cuMemcpyHtoDAsync) X(cuMemcpyDtoHAsync)            \
-  X(cuMemcpyDtoDAsync) X(cuMemsetD32Async) X(cuMemGetInfo)                                                           \
+  X(cuMemcpyDtoDAsync) X(cuMemsetD32Async) X(cuMemsetD2D16Async) X(cuMemsetD2D32Async) X(cuMemGetInfo)                 \
   X(cuStreamCreate) X(cuStreamDestroy) X(cuStreamSynchronize) X(cuStreamWaitEvent)                                   \
   X(cuEventCreate) X(cuEventRecord) X(cuEventElapsedTime) X(cuEventDestroy) X(cuEventSynchronize) X(cuEventQuery)                    \
   X(cuTensorMapEncodeTiled) X(cuTensorMapEncodeIm2col) X(cuGetErrorString) X(cuGetErrorName)                                                    \
@@ -317,12 +319,14 @@ static int get_func(b200_ctx* c, const std::string& name, CUfunction* out) {
   if (c->dry) { c->pending_kernel = name; *out = nullptr; return B200_OK; }
   auto it = c->funcs.find(name);
   if (it != c->funcs.end()) { *out = it->second; return B200_OK; }
-  // modules are loaded in the order gemm, reduce, aux, gemm_b, gemm_c, quant, gemm_q, quant_mm, gemm_conv; the kernel name says where a
+  // modules are loaded in the order gemm, reduce, aux, gemm_b, gemm_c, quant, gemm_q, quant_mm, gemm_conv, gemm_convbwd; the kernel
+  // name says where a
   // kernel lives (no failing lookups, which API-level tools such as compute-sanitizer would report)
   auto starts = [&](const char* pfx) { return name.rfind(pfx, 0) == 0; };
   auto has = [&](const char* part) { return name.find(part) != std::string::npos; };
   const bool tc_gemm = starts("gemm_") && name != "gemm_simt_strided" && name != "gemm_scaled_simt";
-  const size_t home = starts("conv2d_") ? 8
+  const size_t home = starts("conv2d_dgrad_") || starts("conv2d_wgrad_") ? 9
+                      : starts("conv2d_") ? 8
                       : starts("gemm_q8") ? 6
                       : starts("quant_scales_") || starts("quant_widen_") ? 7
                       : starts("quant_") ? 5
@@ -353,7 +357,8 @@ extern "C" int b200_get_cubin(const char* name, const void** image, size_t* size
   else if (!strcmp(name, "gemm_q")) { b = b200_cubin_gemm_q; e = b200_cubin_gemm_q_end; }
   else if (!strcmp(name, "quant_mm")) { b = b200_cubin_quant_mm; e = b200_cubin_quant_mm_end; }
   else if (!strcmp(name, "gemm_conv")) { b = b200_cubin_gemm_conv; e = b200_cubin_gemm_conv_end; }
-  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv)", name);
+  else if (!strcmp(name, "gemm_convbwd")) { b = b200_cubin_gemm_convbwd; e = b200_cubin_gemm_convbwd_end; }
+  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd)", name);
   *image = b;
   *size = static_cast<size_t>(e - b);
   return B200_OK;
@@ -409,7 +414,8 @@ extern "C" int b200_init(int device, b200_ctx** out) {
       (rc = load_module(c, b200_cubin_quant, b200_cubin_quant_end, "quant")) ||
       (rc = load_module(c, b200_cubin_gemm_q, b200_cubin_gemm_q_end, "gemm_q")) ||
       (rc = load_module(c, b200_cubin_quant_mm, b200_cubin_quant_mm_end, "quant_mm")) ||
-      (rc = load_module(c, b200_cubin_gemm_conv, b200_cubin_gemm_conv_end, "gemm_conv"))) {
+      (rc = load_module(c, b200_cubin_gemm_conv, b200_cubin_gemm_conv_end, "gemm_conv")) ||
+      (rc = load_module(c, b200_cubin_gemm_convbwd, b200_cubin_gemm_convbwd_end, "gemm_convbwd"))) {
     for (CUmodule m : c->modules) g_drv.cuModuleUnload_p(m);
     g_drv.cuDevicePrimaryCtxRelease_p(c->dev);
     return bail(rc);
@@ -906,6 +912,15 @@ struct ConvGeom {
   int32_t sh, sw, ph, pw, dh, dw;
   uint64_t x_sw, x_sh, x_sn;   // x: pixel (w), row (h) and image (n) strides
   uint64_t w_sp, w_sco;        // w: kernel-position and output-channel strides
+  // An explicit, asymmetric pixel box (stride 1 only): the im2col walk covers OW x OH pixels from the lower corner
+  // (lo_w, lo_h) instead of the forward's (-pw, -ph) .. (pw - dw (KW - 1), ph - dh (KH - 1)).  A data-gradient phase.
+  bool box = false;
+  int32_t lo_h = 0, lo_w = 0;
+  // 0: the forward (conv2d_*); 1: a data-gradient phase with the phase-addressed epilogue (conv2d_dgrad_*, dx_* strides);
+  // 2: the weight gradient (conv2d_wgrad_*): A = dy [Cout x pixels], B = x through im2col, out = dw (dw_sp, dw_c)
+  int mode = 0;
+  uint64_t dx_sn = 0, dx_si = 0, dx_sj = 0;
+  uint64_t dw_sp = 0, dw_c = 0;
 };
 
 // One batched problem with LINEAR batch strides (0 = broadcast).  Strides in elements.
@@ -931,6 +946,7 @@ struct GemmProblem {
   uint64_t q_sa = 0, q_sb = 0, q_ga = 0, q_gb = 0;
   // 2-D convolution (b200_conv2d): a = x, b = w, M = N * OH * OW, N = Cout, K = KH * KW * (C padded to 64), batch 1
   const ConvGeom* conv = nullptr;
+  uint64_t sk_max_parts = 8;    // stream-K head: at most this many ranges per tile (sk_plan)
 };
 
 static bool variant_has(const GemmVariant& v, const GemmProblem& g) {
@@ -997,7 +1013,10 @@ struct SkPlan {
   uint64_t sk_tiles = 0, ranges = 0, umax = 0;
   bool bad_option = false;
 };
-static SkPlan sk_plan(uint64_t tiles, uint64_t clusters, uint64_t num_kb, const std::string& option, bool eligible) {
+// max_parts caps the ranges per tile of the automatic plan (8 for every GEMM but the convolution weight gradient, whose few
+// tiles have a very long K).
+static SkPlan sk_plan(uint64_t tiles, uint64_t clusters, uint64_t num_kb, const std::string& option, bool eligible,
+                      uint64_t max_parts = 8) {
   SkPlan pl;
   const uint64_t full_waves = tiles / clusters, rem = tiles % clusters;
   pl.time = static_cast<double>(full_waves + (rem ? 1 : 0));
@@ -1014,7 +1033,7 @@ static SkPlan sk_plan(uint64_t tiles, uint64_t clusters, uint64_t num_kb, const 
   bool force = false, even = true;
   if (option == "auto" || option == "on") {
     force = (option == "on");
-    const uint64_t s_fit = std::min<uint64_t>(clusters / rem, 8);
+    const uint64_t s_fit = std::min<uint64_t>(clusters / rem, max_parts);
     if (s_fit >= 2) {
       // equal parts; when whole tiles follow, as many as fit; when the head is everything, the S the model likes best
       uint64_t best_s = s_fit;
@@ -1077,7 +1096,7 @@ static const GemmVariant* pick_variant(b200_ctx* c, const GemmProblem& g, SkPlan
     const uint64_t tiles = tm * tn * g.batch;
     const uint64_t clusters = std::max(1, c->props.num_sms / v.cg);
     // the slab exchange is a per-128-row-CTA-tile protocol with f32 accumulators: not for the 512-row tile, not for integers
-    const SkPlan sk = sk_plan(tiles, clusters, num_kb, split_opt, float_acc && v.mt == 1);
+    const SkPlan sk = sk_plan(tiles, clusters, num_kb, split_opt, float_acc && v.mt == 1, g.sk_max_parts);
     const double eff = v.eff > 0 ? v.eff : 1.0;
     const double cost = sk.time * (128.0 * v.mt * v.block_n) / eff;  // per-SM MMA time
     if (!best || cost < best_cost * 0.999) { best = &v; best_cost = cost; *sk_out = sk; }
@@ -1099,7 +1118,8 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
   if (best_sk.bad_option) return fail(B200_ERR_INVALID_ARG, "gemm.split_k must be auto, off, on or 1..8");
   const GemmVariant& v = *best;
 
-  const std::string name = g.conv ? std::string("conv2d_") + in_tag + "_" + out_tag + "_" + v.tag
+  const int cmode = g.conv ? g.conv->mode : 0;
+  const std::string name = g.conv ? std::string(cmode == 1 ? "conv2d_dgrad_" : cmode == 2 ? "conv2d_wgrad_" : "conv2d_") + in_tag + "_" + out_tag + "_" + v.tag
                                   : std::string("gemm_") + in_tag + "_" + out_tag + "_" + v.tag + (a_mn ? "_m" : "_k") + (b_mn ? "n" : "k");
   CUfunction f;
   int rc = get_func(c, name, &f);
@@ -1116,13 +1136,21 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
   auto pad16 = [&](uint64_t elems) { const uint64_t q = 16 / esz; return (elems + q - 1) / q * q; };
   const uint32_t chunk = static_cast<uint32_t>(128 / esz);  // MN-major operands (16-bit): elements per 128-byte row
   const uint32_t n_local = v.block_n / v.cg;   // B rows each CTA of a pair loads (multicast to both)
-  if (g.conv) {
-    // 128 output pixels x 64 channels per load, walking the input pixels the output grid reads at kernel position (0, 0)
+  // im2col map of the convolution input: `pixels` output pixels x 64 channels per load, walking the input pixels the output
+  // grid reads at kernel position (0, 0)
+  auto conv_im2col = [&](CUtensorMap* m, uint64_t base, uint32_t pixels) {
     const ConvGeom& cv = *g.conv;
     const uint64_t dims[4] = {cv.C, cv.W, cv.H, cv.N}, strides[3] = {cv.x_sw, cv.x_sh, cv.x_sn};
-    const int lower[2] = {-cv.pw, -cv.ph};
-    const int upper[2] = {cv.pw - cv.dw * (int)(cv.KW - 1), cv.ph - cv.dh * (int)(cv.KH - 1)};
-    rc = encode_im2col(c, &ta, dt, esz, g.a, dims, strides, lower, upper, 64, 128, (uint32_t)cv.sw, (uint32_t)cv.sh);
+    int lower[2] = {-cv.pw, -cv.ph};
+    int upper[2] = {cv.pw - cv.dw * (int)(cv.KW - 1), cv.ph - cv.dh * (int)(cv.KH - 1)};
+    if (cv.box) {
+      lower[0] = cv.lo_w; lower[1] = cv.lo_h;
+      upper[0] = cv.lo_w + (int)cv.OW - (int)cv.W; upper[1] = cv.lo_h + (int)cv.OH - (int)cv.H;
+    }
+    return encode_im2col(c, m, dt, esz, base, dims, strides, lower, upper, 64, pixels, (uint32_t)cv.sw, (uint32_t)cv.sh);
+  };
+  if (g.conv && cmode != 2) {
+    rc = conv_im2col(&ta, g.a, 128);
   } else if (!a_mn) {
     const uint64_t a_sm = g.M > 1 ? g.a_sm : pad16(g.K);
     rc = encode_tmap(c, &ta, dt, esz, g.a, g.K, g.M, a_bcast ? 1 : g.batch, a_sm, a_bcast ? a_sm * g.M : g.a_sb, block_k, 128);
@@ -1131,7 +1159,10 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
     rc = encode_tmap(c, &ta, dt, esz, g.a, g.M, g.K, a_bcast ? 1 : g.batch, a_sk, a_bcast ? a_sk * g.K : g.a_sb, chunk, block_k);
   }
   if (rc) return rc;
-  if (g.conv) {
+  if (cmode == 2) {
+    // weight gradient: 64 pixels x 64 channels of x per MN-major B chunk
+    rc = conv_im2col(&tb, g.b, 64);
+  } else if (g.conv) {
     // [n_local output channels x 64 channels] of one kernel position
     const ConvGeom& cv = *g.conv;
     rc = encode_tmap(c, &tb, dt, esz, g.b, cv.C, cv.KH * cv.KW, cv.Cout, cv.w_sp, cv.w_sco, 64, 1, CU_TENSOR_MAP_SWIZZLE_128B, n_local);
@@ -1192,6 +1223,8 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
     p.cv_cblk = (uint32_t)((cv.C + 63) / 64); p.cv_kw = (uint32_t)cv.KW;
     p.cv_stride_h = cv.sh; p.cv_stride_w = cv.sw; p.cv_pad_h = cv.ph; p.cv_pad_w = cv.pw;
     p.cv_dil_h = (uint32_t)cv.dh; p.cv_dil_w = (uint32_t)cv.dw;
+    p.dx_sn = cv.dx_sn; p.dx_si = cv.dx_si; p.dx_sj = cv.dx_sj;
+    p.dw_sp = cv.dw_sp; p.dw_c = (uint32_t)cv.dw_c;
   }
   p.q_ga = g.q_ga; p.q_gb = g.q_gb;
   p.alpha = g.alpha; p.bias = g.bias; p.epi_act = g.act;
@@ -1206,13 +1239,22 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
   p.a_bmul = a_bcast ? 0 : 1;
   p.b_bmul = b_bcast ? 0 : 1;
   p.vec_store = (g.out % 16 == 0 && (g.o_sm * osz) % 16 == 0 && (g.o_sb * osz) % 16 == 0) ? 1 : 0;
+  if (cmode == 1 && ((p.dx_sn * osz) % 16 || (p.dx_si * osz) % 16 || (p.dx_sj * osz) % 16)) p.vec_store = 0;
+  if (cmode == 2 && (p.dw_sp * osz) % 16) p.vec_store = 0;
   // whole tiles leave through swizzled staging tiles and TMA stores when `out` is describable: (N, M, batch), [128 B x 64 rows] boxes
   const std::string epi = opt(c, "gemm.epilogue", "tma");
   if (epi != "tma" && epi != "direct") return fail(B200_ERR_INVALID_ARG, "gemm.epilogue must be tma or direct");
   CUtensorMap tout;
   memset(&tout, 0, sizeof(tout));
   const uint64_t lim40 = 1ull << 40;
-  if (p.vec_store && epi == "tma" && g.o_sm * osz < lim40 && g.o_sb * osz < lim40 && (g.M == 1 || g.o_sm >= g.N)) {
+  if (cmode == 2 && p.vec_store && epi == "tma" && g.o_sm * osz < lim40 && p.dw_sp * osz < lim40) {
+    // dw as (C, Cout, KH * KW): a staging tile of 64-column chunk (kpos, ch0) lands at (ch0, co, kpos), clipped at C
+    const ConvGeom& cv = *g.conv;
+    rc = encode_tmap(c, &tout, osz == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_UINT16, osz, g.out, cv.dw_c, g.M,
+                     cv.KH * cv.KW, g.o_sm, cv.dw_sp, static_cast<uint32_t>(128 / osz), 64);
+    if (rc) return rc;
+    p.tma_store = 1;
+  } else if (cmode == 0 && p.vec_store && epi == "tma" && g.o_sm * osz < lim40 && g.o_sb * osz < lim40 && (g.M == 1 || g.o_sm >= g.N)) {
     const uint64_t o_sm = g.M > 1 ? g.o_sm : (g.N + 15) / 16 * 16;
     const uint64_t o_sb = g.batch > 1 ? g.o_sb : o_sm * g.M;
     rc = encode_tmap(c, &tout, osz == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_UINT16, osz, g.out, g.N, g.M, g.batch,
@@ -2690,6 +2732,298 @@ extern "C" int b200_conv2d(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200
     if (ep) { gp.alpha = ep->alpha; gp.bias = ep->bias; gp.act = (uint32_t)ep->activation; }
     gp.conv = &g;
     rc = launch_wgmma(c, st, gp, false, false);
+  }
+  for (CUdeviceptr t : tmp)
+    if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMM has drained
+  return rc;
+}
+
+// ------------------------------------------------------------------------------------------------ convolution backward
+// Zeros written to `rows` rows of `cols` elements, `pitch` elements apart (a 2-D device memset; recorded as one plan line).
+static int memset2d_zero(b200_ctx* c, CUstream st, CUdeviceptr dst, size_t esz, uint64_t pitch, uint64_t cols, uint64_t rows) {
+  if (c->dry) {
+    char line[96];
+    snprintf(line, sizeof(line), "memset2d esz=%zu cols=%llu rows=%llu\n", esz, (unsigned long long)cols, (unsigned long long)rows);
+    c->plan += line;
+    return B200_OK;
+  }
+  if (esz == 4) CU_CHECK(g_drv.cuMemsetD2D32Async_p(dst, pitch * 4, 0u, cols, rows, st));
+  else CU_CHECK(g_drv.cuMemsetD2D16Async_p(dst, pitch * 2, 0, cols, rows, st));
+  return B200_OK;
+}
+
+// An NHWC operand [N, H, W, C] (normalised strides `ns`) as the convolution maps read it: unit channel stride, 16-byte
+// aligned base and pixel / row / image strides, channels a multiple of 8 -- the forward's rules.  A view that does not
+// qualify is gathered into a compact pooled copy; channel counts that are not multiples of 8 are copied with the channels
+// padded to 8 zeros.  one_pitch: the pixels must also form one strided dimension (the weight gradient reads dy as
+// [pixels, Cout]).  tmp[0] / tmp[1] receive the pooled copies (the caller frees them).
+struct NhwcOperand {
+  uint64_t ptr, C, s_w, s_h, s_n;
+};
+static int conv_prep_nhwc(b200_ctx* c, CUstream st, b200_dtype dt, uint64_t ptr, const uint64_t* shape, const uint64_t* ns, bool one_pitch,
+                          CUdeviceptr tmp[2], NhwcOperand* o) {
+  const uint64_t N = shape[0], H = shape[1], W = shape[2], C = shape[3];
+  auto al = [](uint64_t e) { return e % 8 == 0 && e * 2 < (1ull << 40); };   // 16-byte multiple (16-bit elements)
+  const bool pitch_ok = !one_pitch || (ns[1] == W * ns[2] && ns[0] == H * ns[1]);
+  int rc = B200_OK;
+  if (C % 8 == 0) {
+    if (ptr % 16 == 0 && ns[3] == 1 && al(ns[0]) && al(ns[1]) && al(ns[2]) && pitch_ok) {
+      *o = {ptr, C, ns[2], ns[1], ns[0]};
+      return B200_OK;
+    }
+    rc = conv_gather(c, st, dt, ptr, shape, ns, &tmp[0]);
+    *o = {tmp[0], C, C, W * C, H * W * C};
+    return rc;
+  }
+  const uint64_t cp = (C + 7) / 8 * 8;
+  const uint64_t spx = (W == 1) ? ns[1] : (H == 1 || ns[1] == W * ns[2]) ? ns[2] : 0;   // (H, W) as one pixel dimension
+  uint64_t in = ptr, sb = ns[0], sp = spx, sc = ns[3];
+  if (spx == 0) {
+    rc = conv_gather(c, st, dt, ptr, shape, ns, &tmp[0]);
+    in = tmp[0]; sb = H * W * C; sp = C; sc = 1;
+  }
+  if (!rc) rc = conv_pad_channels(c, st, in, N, H * W, C, sb, sp, sc, cp, &tmp[1]);
+  *o = {tmp[1], cp, cp, W * cp, H * W * cp};
+  return rc;
+}
+
+// Shared argument checks of the two gradients: dtypes, args, and dy's shape against the forward's output rule for the
+// input [N, H, W, C] and weights [Cout, KH, KW, C].  what: the entry point, for messages.
+static int conv_bwd_check(const char* what, b200_dtype in_dtype, b200_dtype out_dtype, const b200_conv2d_args& a, const uint64_t* in_shape,
+                          const uint64_t* w_shape, const uint64_t* dy_shape, uint64_t* OH, uint64_t* OW) {
+  if (in_dtype != B200_F16 && in_dtype != B200_BF16)
+    return fail(B200_ERR_UNSUPPORTED, "%s: input dtype %d unsupported (f16, bf16)", what, (int)in_dtype);
+  if (out_dtype != in_dtype && out_dtype != B200_F32)
+    return fail(B200_ERR_UNSUPPORTED, "%s: output dtype must equal the input dtype or be f32", what);
+  if (a.stride_h < 1 || a.stride_w < 1 || a.dilation_h < 1 || a.dilation_w < 1 || a.pad_h < 0 || a.pad_w < 0)
+    return fail(B200_ERR_INVALID_ARG, "%s: strides and dilations must be >= 1 and padding >= 0", what);
+  if (w_shape[3] != in_shape[3])
+    return fail(B200_ERR_INVALID_ARG, "%s: weights have %llu channels, the input has %llu", what, (unsigned long long)w_shape[3],
+                (unsigned long long)in_shape[3]);
+  const uint64_t lim = 1ull << 31;
+  for (int d = 0; d < 4; ++d)
+    if (in_shape[d] >= lim || w_shape[d] >= lim || dy_shape[d] >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: extents must be < 2^31", what);
+  const int64_t KH = (int64_t)w_shape[1], KW = (int64_t)w_shape[2];
+  if (KH == 0 || KW == 0) return B200_OK;   // an empty kernel: no output rule to check (the gradients are zero or empty)
+  const int64_t nh = (int64_t)in_shape[1] + 2 * (int64_t)a.pad_h - (int64_t)a.dilation_h * (KH - 1) - 1;
+  const int64_t nw = (int64_t)in_shape[2] + 2 * (int64_t)a.pad_w - (int64_t)a.dilation_w * (KW - 1) - 1;
+  if (nh < 0 || nw < 0)
+    return fail(B200_ERR_INVALID_ARG, "%s: the dilated kernel is larger than the padded input (output extent < 1)", what);
+  *OH = (uint64_t)(nh / a.stride_h) + 1;
+  *OW = (uint64_t)(nw / a.stride_w) + 1;
+  if (dy_shape[0] != in_shape[0] || dy_shape[1] != *OH || dy_shape[2] != *OW || dy_shape[3] != w_shape[0])
+    return fail(B200_ERR_INVALID_ARG, "%s: dy is [%llu,%llu,%llu,%llu], expected [%llu,%llu,%llu,%llu]", what, (unsigned long long)dy_shape[0],
+                (unsigned long long)dy_shape[1], (unsigned long long)dy_shape[2], (unsigned long long)dy_shape[3],
+                (unsigned long long)in_shape[0], (unsigned long long)*OH, (unsigned long long)*OW, (unsigned long long)w_shape[0]);
+  if (a.stride_h > kDgradMaxStride || a.stride_w > kDgradMaxStride)
+    return fail(B200_ERR_UNSUPPORTED, "%s: the conv stride must be <= %d", what, kDgradMaxStride);
+  return B200_OK;
+}
+
+// One dimension of the data gradient's phase decomposition.  Output index h = r + s * i (phase r, 0 <= r < s) receives
+// dy[i + e] * w[k] for the taps k with (r + p - k * d) % s == 0, e = (r + p - k * d) / s.  Sorted by e ascending (k
+// descending) the taps are an arithmetic progression: e_t = e0 + t * d', d' = d / gcd(s, d).
+struct DgradPhase1D {
+  uint32_t r, taps, kmax;   // kmax: the tap with the smallest e (t = 0); taps == 0: the phase receives nothing
+  int64_t e0;
+  uint32_t dil, step;       // tap t is k = kmax - t * step (step = s / gcd(s, d)) and reads dy offset e0 + t * dil
+  uint64_t extent;          // ceil((H - r) / s), 0 when r >= H
+};
+static DgradPhase1D dgrad_phase(uint64_t H, uint64_t K, int64_t s, int64_t p, int64_t d, uint32_t r) {
+  DgradPhase1D ph{};
+  ph.r = r;
+  int64_t g = s, b = d;
+  while (b) { const int64_t t = g % b; g = b; b = t; }
+  ph.dil = (uint32_t)(d / g);
+  ph.step = (uint32_t)(s / g);
+  ph.extent = r < H ? (H - r + s - 1) / s : 0;
+  for (int64_t k = (int64_t)K - 1; k >= 0; --k) {
+    const int64_t num = (int64_t)r + p - k * d;
+    if (((num % s) + s) % s != 0) continue;
+    if (ph.taps == 0) { ph.kmax = (uint32_t)k; ph.e0 = num / s; }
+    ++ph.taps;
+  }
+  return ph;
+}
+
+extern "C" int b200_conv2d_backward_data(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr dy,
+                                         const uint64_t* dy_shape, const uint64_t* dy_strides, b200_dptr w, const uint64_t* w_shape,
+                                         const uint64_t* w_strides, b200_dptr dx, const uint64_t* dx_shape, const uint64_t* dx_strides,
+                                         const b200_conv2d_args* args) {
+  CTX_ENTER(c);
+  const char* what = "conv2d_backward_data";
+  if (!dy_shape || !w_shape || !dx_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
+  const b200_conv2d_args& a = *args;
+  uint64_t OH = 0, OW = 0;
+  int rc = conv_bwd_check(what, in_dtype, out_dtype, a, dx_shape, w_shape, dy_shape, &OH, &OW);
+  if (rc) return rc;
+  const uint64_t N = dx_shape[0], H = dx_shape[1], W = dx_shape[2], C = dx_shape[3];
+  const uint64_t Cout = w_shape[0], KH = w_shape[1], KW = w_shape[2];
+  if (N == 0 || H == 0 || W == 0 || C == 0) return B200_OK;   // no dx
+  const uint64_t lim = 1ull << 31;
+  if (N * H * W >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * H * W = %llu must be < 2^31", what, (unsigned long long)(N * H * W));
+  if (KH * KW * ((Cout + 63) / 64 * 64) >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: KH * KW * Cout (Cout padded to 64) must be < 2^31", what);
+  // phases of each dimension, and the im2col limits of every phase that runs
+  std::vector<DgradPhase1D> phs, pws;
+  for (int r = 0; r < a.stride_h; ++r) phs.push_back(dgrad_phase(H, KH, a.stride_h, a.pad_h, a.dilation_h, (uint32_t)r));
+  for (int r = 0; r < a.stride_w; ++r) pws.push_back(dgrad_phase(W, KW, a.stride_w, a.pad_w, a.dilation_w, (uint32_t)r));
+  bool zero_phase = false;
+  for (const DgradPhase1D& ph : phs)
+    for (const DgradPhase1D& pw : pws) {
+      if (!ph.extent || !pw.extent) continue;
+      if (!ph.taps || !pw.taps || Cout == 0) { zero_phase = true; continue; }
+      const int64_t corners[4] = {ph.e0, pw.e0, ph.e0 + (int64_t)ph.extent - (int64_t)OH, pw.e0 + (int64_t)pw.extent - (int64_t)OW};
+      for (int64_t k : corners)
+        if (k < -128 || k > 127)
+          return fail(B200_ERR_UNSUPPORTED, "%s: im2col pixel-box corner %lld of phase (%u, %u) outside [-128, 127]", what, (long long)k, ph.r, pw.r);
+    }
+  if (!dy || !w || !dx) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
+  const size_t osz = dtype_size(out_dtype);
+  if (dx % osz) return fail(B200_ERR_INVALID_ARG, "%s: dx pointer is not aligned to its element size", what);
+  uint64_t os[4], ys[4], ws[4];
+  conv_norm_strides(dx_shape, dx_strides, os);
+  if (os[3] != 1 || os[2] < C || os[1] != W * os[2] || os[0] != H * os[1])
+    return fail(B200_ERR_UNSUPPORTED, "%s: dx must have unit channel stride and one pixel pitch >= C for N, H, W", what);
+  CUstream st = resolve_stream(c, s);
+  // dx pixels that no tap reaches are exact zeros: one memset of dx, before the phases that overwrite the rest
+  if (zero_phase) {
+    rc = memset2d_zero(c, st, dx, osz, os[2], C, N * H * W);
+    if (rc) return rc;
+  }
+  if (Cout == 0 || KH == 0 || KW == 0) return B200_OK;
+  conv_norm_strides(dy_shape, dy_strides, ys);
+  conv_norm_strides(w_shape, w_strides, ws);
+  CUdeviceptr tmp[3] = {0, 0, 0};
+  NhwcOperand y{};
+  rc = conv_prep_nhwc(c, st, in_dtype, dy, dy_shape, ys, false, tmp, &y);
+  // every phase's flipped, channel-transposed weights [C][Th][Tw][cp] in one pooled buffer of KH * KW * C * cp elements
+  const uint64_t cp = y.C;
+  ConvDgradWeightsParams wp;
+  memset(&wp, 0, sizeof(wp));
+  if (!rc) rc = pool_alloc(c, KH * KW * C * cp * 2, &tmp[2], st);
+  if (!rc) {
+    wp.w = w; wp.out = tmp[2];
+    wp.s_co = ws[0]; wp.s_ky = ws[1]; wp.s_kx = ws[2]; wp.s_c = ws[3];
+    wp.C = C; wp.Cout = Cout; wp.cp = cp;
+    wp.KH = (uint32_t)KH; wp.KW = (uint32_t)KW; wp.sh = (uint32_t)a.stride_h; wp.sw = (uint32_t)a.stride_w;
+    wp.dh = (uint32_t)a.dilation_h; wp.dw = (uint32_t)a.dilation_w; wp.ph = (uint32_t)a.pad_h; wp.pw = (uint32_t)a.pad_w;
+    wp.qh = phs[0].step; wp.qw = pws[0].step;
+    uint64_t off = 0;
+    for (const DgradPhase1D& ph : phs)
+      for (const DgradPhase1D& pw : pws) {
+        wp.off[ph.r * a.stride_w + pw.r] = off;
+        off += (uint64_t)ph.taps * pw.taps * C * cp;
+      }
+    for (const DgradPhase1D& ph : phs) { wp.kmax_h[ph.r] = ph.kmax; wp.taps_h[ph.r] = ph.taps; }
+    for (const DgradPhase1D& pw : pws) { wp.kmax_w[pw.r] = pw.kmax; wp.taps_w[pw.r] = pw.taps; }
+    CUfunction f;
+    rc = get_func(c, "conv_dgrad_weights", &f);
+    void* kargs[] = {&wp};
+    if (!rc) rc = launch(c, f, (unsigned)(((C + 31) / 32) * ((cp + 31) / 32)), (unsigned)(KH * KW), 1, 256, 0, 1, st, kargs);
+  }
+  // one stride-1 convolution of dy per phase that has taps and pixels
+  const bool stride1 = a.stride_h == 1 && a.stride_w == 1;
+  for (const DgradPhase1D& ph : phs)
+    for (const DgradPhase1D& pw : pws) {
+      if (rc) break;
+      if (!ph.extent || !pw.extent || !ph.taps || !pw.taps) continue;
+      ConvGeom g{};
+      g.N = N; g.H = OH; g.W = OW; g.C = cp; g.KH = ph.taps; g.KW = pw.taps; g.OH = ph.extent; g.OW = pw.extent; g.Cout = C;
+      g.sh = 1; g.sw = 1; g.ph = (int32_t)-ph.e0; g.pw = (int32_t)-pw.e0; g.dh = (int32_t)ph.dil; g.dw = (int32_t)pw.dil;
+      g.x_sw = y.s_w; g.x_sh = y.s_h; g.x_sn = y.s_n;
+      g.w_sp = cp; g.w_sco = (uint64_t)ph.taps * pw.taps * cp;
+      g.box = true; g.lo_h = (int32_t)ph.e0; g.lo_w = (int32_t)pw.e0;
+      g.mode = stride1 ? 0 : 1;
+      g.dx_sn = os[0]; g.dx_si = (uint64_t)a.stride_h * os[1]; g.dx_sj = (uint64_t)a.stride_w * os[2];
+      if (c->dry) {
+        std::string line = "conv dgrad phase r=(" + std::to_string(ph.r) + "," + std::to_string(pw.r) + ") taps_h=";
+        for (uint32_t t = 0; t < ph.taps; ++t) line += (t ? "," : "") + std::to_string(ph.kmax - t * ph.step);
+        line += " taps_w=";
+        for (uint32_t t = 0; t < pw.taps; ++t) line += (t ? "," : "") + std::to_string(pw.kmax - t * pw.step);
+        line += " dil=(" + std::to_string(ph.dil) + "," + std::to_string(pw.dil) + ") lower=(" + std::to_string(ph.e0) + "," +
+                std::to_string(pw.e0) + ") upper=(" + std::to_string(ph.e0 + (int64_t)ph.extent - (int64_t)OH) + "," +
+                std::to_string(pw.e0 + (int64_t)pw.extent - (int64_t)OW) + ") extent=(" + std::to_string(ph.extent) + "," +
+                std::to_string(pw.extent) + ")\n";
+        c->plan += line;
+      }
+      GemmProblem gp{};
+      gp.in_dtype = in_dtype; gp.out_dtype = out_dtype;
+      gp.a = y.ptr; gp.b = tmp[2] + wp.off[ph.r * a.stride_w + pw.r] * 2;
+      gp.out = dx + ((uint64_t)ph.r * os[1] + (uint64_t)pw.r * os[2]) * osz;
+      gp.M = N * ph.extent * pw.extent; gp.N = C; gp.K = (uint64_t)ph.taps * pw.taps * ((cp + 63) / 64 * 64); gp.batch = 1;
+      gp.a_sm = gp.K; gp.a_sk = 1; gp.b_sn = gp.K; gp.b_sk = 1;
+      gp.o_sm = os[2]; gp.o_sn = 1; gp.o_sb = 0;
+      gp.conv = &g;
+      rc = launch_wgmma(c, st, gp, false, false);
+    }
+  for (CUdeviceptr t : tmp)
+    if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMMs have drained
+  return rc;
+}
+
+extern "C" int b200_conv2d_backward_weight(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr x,
+                                           const uint64_t* x_shape, const uint64_t* x_strides, b200_dptr dy, const uint64_t* dy_shape,
+                                           const uint64_t* dy_strides, b200_dptr dw, const uint64_t* dw_shape, const uint64_t* dw_strides,
+                                           const b200_conv2d_args* args) {
+  CTX_ENTER(c);
+  const char* what = "conv2d_backward_weight";
+  if (!x_shape || !dy_shape || !dw_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
+  const b200_conv2d_args& a = *args;
+  uint64_t OH = 0, OW = 0;
+  int rc = conv_bwd_check(what, in_dtype, out_dtype, a, x_shape, dw_shape, dy_shape, &OH, &OW);
+  if (rc) return rc;
+  const uint64_t N = x_shape[0], H = x_shape[1], W = x_shape[2], C = x_shape[3];
+  const uint64_t Cout = dw_shape[0], KH = dw_shape[1], KW = dw_shape[2];
+  if (Cout == 0 || C == 0 || KH == 0 || KW == 0) return B200_OK;   // no dw
+  // the forward's 4-D im2col limits: x is read through the same map
+  const int64_t corners[4] = {-(int64_t)a.pad_h, -(int64_t)a.pad_w, (int64_t)a.pad_h - (int64_t)a.dilation_h * ((int64_t)KH - 1),
+                              (int64_t)a.pad_w - (int64_t)a.dilation_w * ((int64_t)KW - 1)};
+  for (int64_t k : corners)
+    if (k < -128 || k > 127)
+      return fail(B200_ERR_UNSUPPORTED, "%s: im2col pixel-box corner %lld outside [-128, 127] (-pad and pad - dilation * (kernel - 1))", what,
+                  (long long)k);
+  const uint64_t P = N * OH * OW, lim = 1ull << 31;
+  if (P >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * OH * OW = %llu must be < 2^31", what, (unsigned long long)P);
+  const uint64_t cx = (C + 7) / 8 * 8;
+  if (KH * KW * ((cx + 63) / 64 * 64) >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: KH * KW * C (C padded to 64) must be < 2^31", what);
+  if (!x || !dy || !dw) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
+  const size_t osz = dtype_size(out_dtype);
+  if (dw % osz) return fail(B200_ERR_INVALID_ARG, "%s: dw pointer is not aligned to its element size", what);
+  // dw: unit channel stride, (KH, KW) flattening into one kernel-position stride, and an output-channel stride
+  uint64_t ds[4], xs[4], ys[4];
+  conv_norm_strides(dw_shape, dw_strides, ds);
+  const uint64_t dw_sp = (KW == 1) ? ds[1] : (KH == 1 || ds[1] == KW * ds[2]) ? ds[2] : 0;
+  if (ds[3] != 1 || dw_sp == 0 || ds[0] * osz >= (1ull << 40) || dw_sp * osz >= (1ull << 40))
+    return fail(B200_ERR_UNSUPPORTED, "%s: dw must have unit channel stride and (KH, KW) flattening into one stride", what);
+  CUstream st = resolve_stream(c, s);
+  if (P == 0) {
+    // no pixels: dw is exactly zero
+    if (ds[0] == KH * KW * dw_sp) return memset2d_zero(c, st, dw, osz, dw_sp, C, Cout * KH * KW);
+    for (uint64_t co = 0; co < Cout && !rc; ++co) rc = memset2d_zero(c, st, dw + co * ds[0] * osz, osz, dw_sp, C, KH * KW);
+    return rc;
+  }
+  conv_norm_strides(x_shape, x_strides, xs);
+  conv_norm_strides(dy_shape, dy_strides, ys);
+  CUdeviceptr tmp[4] = {0, 0, 0, 0};
+  NhwcOperand xo{}, yo{};
+  rc = conv_prep_nhwc(c, st, in_dtype, x, x_shape, xs, false, &tmp[0], &xo);
+  if (!rc) rc = conv_prep_nhwc(c, st, in_dtype, dy, dy_shape, ys, true, &tmp[2], &yo);
+  if (!rc) {
+    ConvGeom g{};
+    g.N = N; g.H = H; g.W = W; g.C = xo.C; g.KH = KH; g.KW = KW; g.OH = OH; g.OW = OW; g.Cout = Cout;
+    g.sh = a.stride_h; g.sw = a.stride_w; g.ph = a.pad_h; g.pw = a.pad_w; g.dh = a.dilation_h; g.dw = a.dilation_w;
+    g.x_sw = xo.s_w; g.x_sh = xo.s_h; g.x_sn = xo.s_n;
+    g.mode = 2; g.dw_sp = dw_sp; g.dw_c = C;
+    GemmProblem gp{};
+    gp.in_dtype = in_dtype; gp.out_dtype = out_dtype;
+    gp.a = yo.ptr; gp.b = xo.ptr; gp.out = dw;
+    gp.M = Cout; gp.N = KH * KW * ((xo.C + 63) / 64 * 64); gp.K = P; gp.batch = 1;
+    gp.a_sm = 1; gp.a_sk = yo.s_w; gp.b_sn = 1; gp.b_sk = xo.s_w;
+    gp.o_sm = ds[0]; gp.o_sn = 1; gp.o_sb = 0;
+    gp.conv = &g;
+    // few tiles, a long K: the stream-K head may cut a tile into as many ranges as fill the SMs, each >= 8 k-blocks
+    gp.sk_max_parts = std::max<uint64_t>(8, (P + 63) / 64 / 8);
+    rc = launch_wgmma(c, st, gp, true, true);
   }
   for (CUdeviceptr t : tmp)
     if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMM has drained

@@ -145,14 +145,26 @@ enum : int { QM_NONE = 0, QM_BLOCK = 1, QM_TENSOR = 2 };
 // consecutive output pixels x 64 channels of kernel position kb / cv_cblk, channel block kb % cv_cblk -- which TMA writes in
 // exactly the 128B-swizzled [128 rows x 128 B] layout of a K-major A tile; B is the weights' [n_local x 64 channels] box of
 // that (kernel position, channel block).  Channels past C read as zero on both sides.  Everything after the load is the GEMM.
+// CB (convolution backward; capi.cpp: b200_conv2d_backward_data / _weight):
+//   CB_DGRAD  the CONV producer; the epilogue stores GEMM row (n, i, j) of one output phase at its dx pixel (GemmParams dx_*),
+//             with row addresses computed once per tile.  Direct stores only: a TMA store cannot describe that row mapping.
+//   CB_WGRAD  MN-major A (dy: 64 output channels x 64 pixels per chunk, tiled) and B: each 64-column chunk of the B tile is one
+//             im2col load of 64 pixels x 64 channels of x at one (kernel position, channel block), which TMA writes as
+//             [64 pixel rows x 128 B], exactly an MN-major B chunk.  Pixels past N * OH * OW read as zero on both sides (tiled
+//             out-of-bounds fill for dy; the im2col walk runs into image N for x).  The epilogue maps virtual column
+//             (kpos, ch) to dw's column and drops ch >= C, in the direct stores and in the TMA-store coordinate.
+enum : int { CB_NONE = 0, CB_DGRAD = 1, CB_WGRAD = 2 };
 template <int CG, int BLOCK_N, bool A_MN, bool B_MN, int KIND, int OUT, int STAGES, bool PROMOTE = false, int MT = 1, int QM = QM_NONE,
-          bool CONV = false>
+          bool CONV = false, int CB = CB_NONE>
 __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUtensorMap* tma_b_hi, const CUtensorMap* tma_a_lo,
                                           const CUtensorMap* tma_b_lo, const CUtensorMap* tma_out, const GemmParams& p) {
   constexpr bool INT_ACC = (KIND == KIND_U8 || KIND == KIND_S8) && QM != QM_BLOCK;
   static_assert(QM == QM_NONE || (KIND == KIND_S8 && !A_MN && !B_MN && !PROMOTE && MT == 1), "quantized operands: s8, K-major");
   static_assert(!CONV || ((KIND == KIND_BF16 || KIND == KIND_F16) && !A_MN && !B_MN && !PROMOTE && MT == 1 && QM == QM_NONE),
                 "convolution: 16-bit kinds, K-major operands");
+  static_assert(CB != CB_DGRAD || CONV, "data gradient: the convolution producer");
+  static_assert(CB != CB_WGRAD || (!CONV && A_MN && B_MN && (KIND == KIND_BF16 || KIND == KIND_F16) && !PROMOTE && MT == 1 && QM == QM_NONE),
+                "weight gradient: 16-bit kinds, MN-major operands");
   // per-block scale tiles of one stage, sized for the finest block (Bk = 32: four blocks per 128-element stage)
   constexpr uint32_t SC_A_BYTES = (QM == QM_BLOCK) ? 128u * 4u * 4u : 0u;
   constexpr uint32_t SC_STAGE_BYTES = (QM == QM_BLOCK) ? SC_A_BYTES + BLOCK_N * 4u * 4u : 0u;
@@ -294,7 +306,26 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
 #pragma unroll
               for (int mt = 0; mt < MT; ++mt) tma_load_3d(sa + mt * A_SUB_BYTES, tma_a, fb, k0, m0 + mt * 128, ba);
             }
-            if constexpr (B_MN) {
+            if constexpr (CB == CB_WGRAD) {
+              // input pixel of output pixel k0 = (n, oh, ow) at kernel position (0, 0)
+              const uint32_t px = static_cast<uint32_t>(k0), n = px / p.cv_ohw, r = px - n * p.cv_ohw, oh = r / p.cv_ow;
+              const int h = static_cast<int>(oh) * p.cv_stride_h - p.cv_pad_h;
+              const int w = static_cast<int>(r - oh * p.cv_ow) * p.cv_stride_w - p.cv_pad_w;
+#pragma unroll
+              for (int c = 0; c < NUM_CHUNKS; ++c) {
+                const int ci = static_cast<int>(rank) * NUM_CHUNKS + c;
+                // a chunk past N (odd chunk count) loads the last chunk again: its columns are never stored
+                const uint32_t col = min(static_cast<uint32_t>(nb0 + ci * CHUNK_N), p.N - CHUNK_N) / CHUNK_N;
+                const uint32_t kpos = col / p.cv_cblk, cb = col - kpos * p.cv_cblk;
+                const uint32_t ky = kpos / p.cv_kw, kx = kpos - ky * p.cv_kw;
+                const uint16_t ow_ = static_cast<uint16_t>(kx * p.cv_dil_w), oh_ = static_cast<uint16_t>(ky * p.cv_dil_h);
+                if constexpr (CG == 2)
+                  tma_load_im2col_4d_mc(sb + ci * CHUNK_BYTES, tma_b, fb, static_cast<uint16_t>(3), static_cast<int>(cb * 64u), w, h,
+                                        static_cast<int>(n), ow_, oh_);
+                else
+                  tma_load_im2col_4d(sb + ci * CHUNK_BYTES, tma_b, fb, static_cast<int>(cb * 64u), w, h, static_cast<int>(n), ow_, oh_);
+              }
+            } else if constexpr (B_MN) {
 #pragma unroll
               for (int c = 0; c < NUM_CHUNKS; ++c) {
                 const int ci = static_cast<int>(rank) * NUM_CHUNKS + c;
@@ -485,15 +516,37 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
           }
         }
       };
+      // data gradient: the dx addresses of this thread's two fragment rows, once per tile
+      uint64_t dg_row[2] = {0, 0};
+      if constexpr (CB == CB_DGRAD) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const uint32_t r = m_cta + cw * 64u + wq * 16u + (lane >> 2) + 8u * h;
+          const uint32_t n = r / p.cv_ohw, rr = r - n * p.cv_ohw, i = rr / p.cv_ow, j = rr - i * p.cv_ow;
+          dg_row[h] = p.out + (n * p.dx_sn + i * p.dx_si + j * p.dx_sj) * osz;
+        }
+      }
       // direct stores of fragment group j of sub-tile mt
       auto store_group = [&](int mt, int j, uint32_t (&v)[4]) {
         const uint32_t n = c0 + 8u * j;
         if (n >= p.N) return;
         epilogue(n, v);
         const uint32_t r0 = m_cta + mt * 128u + cw * 64u + wq * 16u + (lane >> 2);
-        const uint64_t row0 = p.out + (static_cast<uint64_t>(tc.b) * p.out_batch_stride + static_cast<uint64_t>(r0) * p.out_row_stride) * osz;
-        if (r0 < p.M) store_pair<OUT>(row0, n, p.N, p.vec_store != 0, v[0], v[1]);
-        if (r0 + 8 < p.M) store_pair<OUT>(row0 + static_cast<uint64_t>(8) * p.out_row_stride * osz, n, p.N, p.vec_store != 0, v[2], v[3]);
+        if constexpr (CB == CB_DGRAD) {
+          if (r0 < p.M) store_pair<OUT>(dg_row[0], n, p.N, p.vec_store != 0, v[0], v[1]);
+          if (r0 + 8 < p.M) store_pair<OUT>(dg_row[1], n, p.N, p.vec_store != 0, v[2], v[3]);
+        } else if constexpr (CB == CB_WGRAD) {
+          // virtual column n = (kpos, ch): dw row r0, element kpos * dw_sp + ch; channels ch >= C are dropped (a pair never
+          // straddles two kernel positions)
+          const uint32_t kpos = n / (p.cv_cblk * 64u), ch = n - kpos * p.cv_cblk * 64u;
+          const uint64_t row0 = p.out + (static_cast<uint64_t>(r0) * p.out_row_stride + kpos * p.dw_sp) * osz;
+          if (r0 < p.M) store_pair<OUT>(row0, ch, p.dw_c, p.vec_store != 0, v[0], v[1]);
+          if (r0 + 8 < p.M) store_pair<OUT>(row0 + static_cast<uint64_t>(8) * p.out_row_stride * osz, ch, p.dw_c, p.vec_store != 0, v[2], v[3]);
+        } else {
+          const uint64_t row0 = p.out + (static_cast<uint64_t>(tc.b) * p.out_batch_stride + static_cast<uint64_t>(r0) * p.out_row_stride) * osz;
+          if (r0 < p.M) store_pair<OUT>(row0, n, p.N, p.vec_store != 0, v[0], v[1]);
+          if (r0 + 8 < p.M) store_pair<OUT>(row0 + static_cast<uint64_t>(8) * p.out_row_stride * osz, n, p.N, p.vec_store != 0, v[2], v[3]);
+        }
       };
       auto frag = [&](int mt, int j, uint32_t (&v)[4]) {
 #pragma unroll
@@ -504,7 +557,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
       };
       const bool partial = (MT == 1) && !INT_ACC && QM == QM_NONE && wu.partial;   // the host plans no stream-K head for these
 
-      if (!partial && p.tma_store) {
+      if (CB != CB_DGRAD && !partial && p.tma_store) {
         // fragments -> (epilogue, convert) -> 128B-swizzled [64 rows x 128 B] staging tile -> one TMA store per 128-byte column
         // group; the TMA unit clips ragged edges.  A direct store writes 16 bytes per row per instruction, 8 rows apart.
         const uint32_t stage_smem = epi_base + cw * 8192u;
@@ -541,7 +594,13 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
             fence_proxy_async_smem();   // generic-proxy writes -> visible to the TMA unit
             asm volatile("bar.sync %0, 128;" ::"r"(2u + cw) : "memory");
             if (t == 0 && m_row0 < static_cast<int>(p.M) && n0 < p.N) {
-              tma_store_3d(tma_out, stage_smem, static_cast<int>(n0), m_row0, static_cast<int>(tc.b));
+              if constexpr (CB == CB_WGRAD) {
+                // tma_out describes dw as (C, Cout, KH * KW): the store clips channels past C
+                const uint32_t kpos = n0 / (p.cv_cblk * 64u);
+                tma_store_3d(tma_out, stage_smem, static_cast<int>(n0 - kpos * p.cv_cblk * 64u), m_row0, static_cast<int>(kpos));
+              } else {
+                tma_store_3d(tma_out, stage_smem, static_cast<int>(n0), m_row0, static_cast<int>(tc.b));
+              }
               tma_store_commit();
             }
           }
@@ -695,12 +754,32 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
   CONV_KERNEL(conv2d_f16_f16_##TILE, CG, BN, KIND_F16, OUT_F16, STAGES)     \
   CONV_KERNEL(conv2d_f16_f32_##TILE, CG, BN, KIND_F16, OUT_F32, STAGES)
 
-// The kernels are built as five cubins from this one source (cubecl_b200/build.py compiles them in parallel):
+// Convolution backward: conv2d_dgrad_* (tma_a = im2col map of dy, tma_b = 3-D map of one phase's flipped weights) and
+// conv2d_wgrad_* (tma_a = 3-D map of dy as (Cout, pixels), tma_b = im2col map of x, tma_out = (C, Cout, KH * KW) map of dw)
+#define CONV_BWD_KERNEL(NAME, CG, BN, AMN, KIND, OUT, STAGES, CONV, CB)                                            \
+  extern "C" __global__ void __launch_bounds__(kNumThreads, 1)                                                     \
+      NAME(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,                  \
+           const __grid_constant__ CUtensorMap tma_a_lo, const __grid_constant__ CUtensorMap tma_b_lo,            \
+           const __grid_constant__ CUtensorMap tma_out, const __grid_constant__ GemmParams p) {                    \
+    gemm_body<CG, BN, AMN, AMN, KIND, OUT, STAGES, false, 1, QM_NONE, CONV, CB>(&tma_a, &tma_b, &tma_a_lo, &tma_b_lo, &tma_out, p); \
+  }
+#define CONV_BWD_DTYPES(TILE, CG, BN, STAGES)                                                                  \
+  CONV_BWD_KERNEL(conv2d_dgrad_bf16_bf16_##TILE, CG, BN, false, KIND_BF16, OUT_BF16, STAGES, true, CB_DGRAD)   \
+  CONV_BWD_KERNEL(conv2d_dgrad_bf16_f32_##TILE, CG, BN, false, KIND_BF16, OUT_F32, STAGES, true, CB_DGRAD)     \
+  CONV_BWD_KERNEL(conv2d_dgrad_f16_f16_##TILE, CG, BN, false, KIND_F16, OUT_F16, STAGES, true, CB_DGRAD)       \
+  CONV_BWD_KERNEL(conv2d_dgrad_f16_f32_##TILE, CG, BN, false, KIND_F16, OUT_F32, STAGES, true, CB_DGRAD)       \
+  CONV_BWD_KERNEL(conv2d_wgrad_bf16_bf16_##TILE, CG, BN, true, KIND_BF16, OUT_BF16, STAGES, false, CB_WGRAD)   \
+  CONV_BWD_KERNEL(conv2d_wgrad_bf16_f32_##TILE, CG, BN, true, KIND_BF16, OUT_F32, STAGES, false, CB_WGRAD)     \
+  CONV_BWD_KERNEL(conv2d_wgrad_f16_f16_##TILE, CG, BN, true, KIND_F16, OUT_F16, STAGES, false, CB_WGRAD)       \
+  CONV_BWD_KERNEL(conv2d_wgrad_f16_f32_##TILE, CG, BN, true, KIND_F16, OUT_F32, STAGES, false, CB_WGRAD)
+
+// The kernels are built as six cubins from this one source (cubecl_b200/build.py compiles them in parallel):
 //   GEMM_PART 0 ("gemm")       256 x 256 pair tiles (2-CTA cluster, 128 x 256 per CTA) and the bf16 peak probe
 //   GEMM_PART 1 ("gemm_b")     256 x 128 pair tiles, 256 x 224 block-scaled pair tiles
 //   GEMM_PART 2 ("gemm_c")     128 x 128 single-CTA tiles, 512 x 128 pair tiles
 //   GEMM_PART 3 ("gemm_q")     the quantized-operand kernels of every tile
 //   GEMM_PART 4 ("gemm_conv")  the 2-D convolution kernels of the 2sm_n128 and 1sm_n128 tiles
+//   GEMM_PART 5 ("gemm_convbwd")  the convolution backward kernels (data and weight gradients) of the same two tiles
 #ifndef GEMM_PART
 #define GEMM_PART 0
 #endif
@@ -749,6 +828,10 @@ GEMM_Q(1sm_n128, 1, 128, 6, 5)
 // spills at the 168 registers a thread of a 384-thread CTA gets (as gemm_*_2sm_n256_kk does), and these kernels do not spill
 CONV_DTYPES(2sm_n128, 2, 128, 6)
 CONV_DTYPES(1sm_n128, 1, 128, 6)
+#endif
+#if GEMM_PART == 5
+CONV_BWD_DTYPES(2sm_n128, 2, 128, 6)
+CONV_BWD_DTYPES(1sm_n128, 1, 128, 6)
 #endif
 
 #if GEMM_PART == 0

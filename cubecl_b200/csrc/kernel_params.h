@@ -57,6 +57,16 @@ struct GemmParams {
   uint32_t cv_ohw, cv_ow, cv_cblk, cv_kw;
   int32_t cv_stride_h, cv_stride_w, cv_pad_h, cv_pad_w;
   uint32_t cv_dil_h, cv_dil_w;
+  // Convolution backward (capi.cpp: b200_conv2d_backward_data / _weight).
+  // Data gradient, stride > 1 (conv2d_dgrad_*): one output phase (h = rh + sh * i, w = rw + sw * j) run as a stride-1
+  // convolution of dy.  GEMM row m = (n, i, j) of the phase grid (the cv_ohw / cv_ow geometry above) is stored at
+  // out + n * dx_sn + i * dx_si + j * dx_sj elements; `out` already points at pixel (0, rh, rw).
+  uint64_t dx_sn, dx_si, dx_sj;
+  // Weight gradient (conv2d_wgrad_*): A = dy as [K = pixels, M = Cout] (MN-major), B = the im2col of x, 64 pixels x 64
+  // channels of one (kernel position, channel block) per load, K = N * OH * OW pixels.  Virtual column n = (kpos, ch) with
+  // kpos = n / (cv_cblk * 64) is dw's element kpos * dw_sp + ch of row co; columns with ch >= dw_c are dropped.
+  uint64_t dw_sp;
+  uint32_t dw_c, dw_pad;
 };
 
 // ================================================================================================ aux_kernels.cu
@@ -123,6 +133,20 @@ struct RepitchParams {
   uint64_t in_sb, in_sr, in_sc;      // input strides in elements
   uint64_t out_pitch;                // output row pitch in elements (16-byte multiple)
   uint32_t esz, pad;
+};
+
+// Convolution data gradient (conv_dgrad_weights): every output phase's flipped, channel-transposed weights in one pooled
+// buffer.  Phase (rh, rw) owns taps ky with (ky * dh - ph - rh) % sh == 0 (likewise kx); its block starts at element
+// off[rh * sw + rw] and is [C][Th][Tw][cp] with tap th = (kmax_h[rh] - ky) / qh (ascending dy offset), co innermost and
+// channels [Cout, cp) zero.  The phases partition the taps, so the blocks fill KH * KW * C * cp elements.
+constexpr int kDgradMaxStride = 8;
+struct ConvDgradWeightsParams {
+  uint64_t w, out;
+  uint64_t s_co, s_ky, s_kx, s_c;      // w [Cout, KH, KW, C] strides in elements
+  uint64_t C, Cout, cp;                // cp: output channel pitch (Cout padded to 8)
+  uint64_t off[kDgradMaxStride * kDgradMaxStride];
+  uint32_t KH, KW, sh, sw, dh, dw, ph, pw, qh, qw;
+  uint32_t kmax_h[kDgradMaxStride], kmax_w[kDgradMaxStride], taps_h[kDgradMaxStride], taps_w[kDgradMaxStride];
 };
 
 // ================================================================================================ reduce.cu

@@ -154,6 +154,18 @@ __device__ __forceinline__ void tma_load_im2col_4d(uint32_t dst, const CUtensorM
       : "memory");
 }
 
+// Multicast 4-D im2col load: as tma_load_im2col_4d, the box landing at the same smem offset in every CTA of `mask`, each
+// CTA's own barrier (same offset) receiving the complete_tx.
+__device__ __forceinline__ void tma_load_im2col_4d_mc(uint32_t dst, const CUtensorMap* m, uint32_t bar, uint16_t mask, int c, int w,
+                                                      int h, int n, uint16_t off_w, uint16_t off_h) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%4, %5, %6, %7}], [%2], {%8, %9}, %3;"
+      :
+      : "r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "h"(mask), "r"(c), "r"(w), "r"(h), "r"(n), "h"(off_w), "h"(off_h)
+      : "memory");
+}
+
 // Multicast 3-D load: the box lands at the same smem offset in every CTA of `mask`, each CTA's own barrier
 // (same offset) receives the complete_tx.
 __device__ __forceinline__ void tma_load_3d_mc(uint32_t dst, const CUtensorMap* m, uint32_t bar, uint16_t mask, int c0,

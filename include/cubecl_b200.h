@@ -341,6 +341,48 @@ int b200_conv2d(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b200_dtype ou
                 b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides,
                 const b200_conv2d_args* args, const b200_epilogue* epilogue);
 
+/* Gradients of b200_conv2d (same args, same NHWC / [Cout, KH, KW, C] layouts, f32 accumulation, no epilogue).
+ *   dx[n, h, w, c]    = sum over (oh, ow, ky, kx) with oh*sh - ph + ky*dh = h, ow*sw - pw + kx*dw = w of dy[n, oh, ow, co] * w[co, ky, kx, c]
+ *   dw[co, ky, kx, c] = sum over (n, oh, ow) of dy[n, oh, ow, co] * x[n, oh*sh - ph + ky*dh, ow*sw - pw + kx*dw, c]
+ * dy must have the shape b200_conv2d gives for (dx or x, w or dw, args): [N, OH, OW, Cout]; that admits every H and W that
+ * PyTorch's output_padding admits.  The bias gradient needs no entry point: it is b200_reduce (sum) over axis 0 of dy viewed as
+ * [N * OH * OW, Cout].
+ * Dtypes: F16 or BF16 dy / w / x; out_dtype the input dtype or F32.
+ * Views: dy and x follow b200_conv2d's input rules (gathered when not readable in place; C or Cout with C * 2 % 16 != 0 copied
+ * with the channels padded to 8 zeros); b200_conv2d_backward_weight also gathers a dy whose pixels do not share one pitch.
+ * backward_data reads w through any strides.  dx follows b200_conv2d's out rule (unit channel stride, one pixel pitch >= C).
+ * dw needs a unit channel stride, (KH, KW) flattening into one stride and any Cout stride; other dw views get
+ * B200_ERR_UNSUPPORTED.
+ * Errors: B200_ERR_INVALID_ARG for a channel mismatch, a dy shape that is not the output rule's, stride / dilation < 1, negative
+ * padding or a null pointer; B200_ERR_UNSUPPORTED for strides > 8, pixel-box corners outside [-128, 127] (backward_weight: the
+ * forward's corners; backward_data: per output phase, below), N*H*W or N*OH*OW >= 2^31.  An empty dx / dw is a no-op; when dy
+ * has no pixels (N = 0) dw is written as zeros, and when Cout = 0 dx is.
+ *
+ * backward_data: with stride 1, dx is a stride-1 convolution of dy with the flipped, channel-transposed weights
+ * w'[c, ky', kx', co] = w[co, KH-1-ky', KW-1-kx', c]: launches = 1 weight-prep kernel + 1 conv2d GEMM.  With stride > 1, dx
+ * splits into sh * sw phases (h = rh + sh*i, w = rw + sw*j); each phase is a stride-1 convolution of dy over the taps
+ * ky with (rh + ph - ky*dh) % sh == 0 (dilation dh / gcd(sh, dh)), one conv2d_dgrad GEMM per phase with taps and pixels, whose
+ * epilogue stores its rows straight into dx.  Its pixel-box corners are the first tap's dy offset and that offset + the
+ * phase extent - OH (likewise for w).  Phases no tap reaches (a 1x1 stride-2 layer has three) are exact zeros: one memset of
+ * dx, only when such a phase exists.  Temporaries: the prepared weights (|w| elements, Cout padded to 8) plus dy's copies.
+ * backward_weight: one conv2d_wgrad GEMM with M = Cout, N = KH * KW * pad64(C), K = N * OH * OW; dy is read as an MN-major
+ * [pixels, Cout] operand, x through a 64-pixel im2col load per (kernel position, 64-channel block).  K is long and the tiles are
+ * few, so the stream-K head ("gemm.split_k" auto) may cut a tile into more than 8 k-ranges (each >= 8 k-blocks of 64 pixels),
+ * reduced in k order.
+ * Both: stream-ordered, no host sync, temporaries from the pool, bitwise reproducible for a fixed shape, dtypes and SM count;
+ * "gemm.variant" (2sm_n128 | 1sm_n128), "gemm.split_k" and "gemm.epilogue" apply (backward_data's stride > 1 phases always
+ * store directly). */
+int b200_conv2d_backward_data(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype,
+                              b200_dptr dy, const uint64_t* dy_shape, const uint64_t* dy_strides,
+                              b200_dptr w, const uint64_t* w_shape, const uint64_t* w_strides,
+                              b200_dptr dx, const uint64_t* dx_shape, const uint64_t* dx_strides,
+                              const b200_conv2d_args* args);
+int b200_conv2d_backward_weight(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype,
+                                b200_dptr x, const uint64_t* x_shape, const uint64_t* x_strides,
+                                b200_dptr dy, const uint64_t* dy_shape, const uint64_t* dy_strides,
+                                b200_dptr dw, const uint64_t* dw_shape, const uint64_t* dw_strides,
+                                const b200_conv2d_args* args);
+
 /* ---- collectives: ServerCommunication (server/base.rs:632-739), CUDA impl cubecl-cuda/src/compute/server.rs:666-926 -- */
 #define B200_UNIQUE_ID_BYTES 128
 int b200_comm_get_unique_id(b200_ctx* ctx, void* id128);            /* ncclGetUniqueId (communication.rs:11-25 holds it per device set) */

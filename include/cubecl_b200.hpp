@@ -234,6 +234,34 @@ inline void launch(ComputeClient& client, const TensorHandle& x, const TensorHan
                              out.handle.ptr(), out.shape.data(), out.strides.data(), &args, epilogue);
   if (rc != B200_OK) client.defer(b200_last_error());
 }
+
+/// Input gradient: dy [N, OH, OW, Cout], w [Cout, KH, KW, C] -> dx [N, H, W, C].  See b200_conv2d_backward_data.  Errors are
+/// deferred to client.sync().
+inline void backward_data(ComputeClient& client, const TensorHandle& dy, const TensorHandle& w, const TensorHandle& dx,
+                          const b200_conv2d_args& args) {
+  if (dy.shape.size() != 4 || w.shape.size() != 4 || dx.shape.size() != 4 || dy.dtype != w.dtype) {
+    client.defer("InvalidArgument: conv2d_backward_data needs rank-4 dy, w and dx, and dy and w of one dtype");
+    return;
+  }
+  const int rc = b200_conv2d_backward_data(client.raw(), nullptr, static_cast<b200_dtype>(dy.dtype), static_cast<b200_dtype>(dx.dtype),
+                                           dy.handle.ptr(), dy.shape.data(), dy.strides.data(), w.handle.ptr(), w.shape.data(),
+                                           w.strides.data(), dx.handle.ptr(), dx.shape.data(), dx.strides.data(), &args);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+
+/// Weight gradient: x [N, H, W, C], dy [N, OH, OW, Cout] -> dw [Cout, KH, KW, C].  The bias gradient is reduce (sum) over
+/// axis 0 of dy viewed as [N * OH * OW, Cout].  See b200_conv2d_backward_weight.  Errors are deferred to client.sync().
+inline void backward_weight(ComputeClient& client, const TensorHandle& x, const TensorHandle& dy, const TensorHandle& dw,
+                            const b200_conv2d_args& args) {
+  if (x.shape.size() != 4 || dy.shape.size() != 4 || dw.shape.size() != 4 || x.dtype != dy.dtype) {
+    client.defer("InvalidArgument: conv2d_backward_weight needs rank-4 x, dy and dw, and x and dy of one dtype");
+    return;
+  }
+  const int rc = b200_conv2d_backward_weight(client.raw(), nullptr, static_cast<b200_dtype>(x.dtype), static_cast<b200_dtype>(dw.dtype),
+                                             x.handle.ptr(), x.shape.data(), x.strides.data(), dy.handle.ptr(), dy.shape.data(),
+                                             dy.strides.data(), dw.handle.ptr(), dw.shape.data(), dw.strides.data(), &args);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
 }  // namespace conv
 
 namespace reduce {
