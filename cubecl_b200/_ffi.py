@@ -117,6 +117,12 @@ SIGNATURES = {
                                             C.c_uint64, _u64p, _u64p, C.POINTER(Conv2dArgs)]),
     "b200_conv2d_backward_weight": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, _u64p, _u64p, C.c_uint64, _u64p, _u64p,
                                               C.c_uint64, _u64p, _u64p, C.POINTER(Conv2dArgs)]),
+    "b200_conv2d_grouped": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, _u64p, _u64p, C.c_uint64, _u64p, _u64p, C.c_uint64,
+                                      _u64p, _u64p, C.POINTER(Conv2dArgs), C.c_uint32, C.POINTER(Epilogue)]),
+    "b200_conv2d_grouped_backward_data": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, _u64p, _u64p, C.c_uint64, _u64p, _u64p,
+                                                    C.c_uint64, _u64p, _u64p, C.POINTER(Conv2dArgs), C.c_uint32]),
+    "b200_conv2d_grouped_backward_weight": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, _u64p, _u64p, C.c_uint64, _u64p, _u64p,
+                                                      C.c_uint64, _u64p, _u64p, C.POINTER(Conv2dArgs), C.c_uint32]),
     "b200_reduce": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, C.c_uint64, C.c_int, _u64p, C.c_int]),
     "b200_reduce_strided": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, C.c_uint64, C.c_int, _u64p, _u64p, C.c_int]),
     "b200_reduce_debug": (C.c_int, [_vp, _vp, _u64p]),

@@ -28,7 +28,7 @@ CUBINS = {"gemm": ("gemm_wgmma.cu", ["-DGEMM_PART=0"]), "gemm_b": ("gemm_wgmma.c
           "gemm_c": ("gemm_wgmma.cu", ["-DGEMM_PART=2"]), "reduce": ("reduce.cu", []), "aux": ("aux_kernels.cu", []),
           "quant": ("quant.cu", []), "gemm_q": ("gemm_wgmma.cu", ["-DGEMM_PART=3"]),
           "quant_mm": ("quant.cu", ["-DQUANT_PART=1"]), "gemm_conv": ("gemm_wgmma.cu", ["-DGEMM_PART=4"]),
-          "gemm_convbwd": ("gemm_wgmma.cu", ["-DGEMM_PART=5"])}
+          "gemm_convbwd": ("gemm_wgmma.cu", ["-DGEMM_PART=5"]), "conv_grouped": ("conv_grouped.cu", [])}
 NVCC_FLAGS = ["-cubin", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17"]
 
 
@@ -77,7 +77,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     # cost the five minutes of ptxas the GEMM instantiations take
     def inputs_digest(src, extra):
         h = hashlib.sha256(" ".join(NVCC_FLAGS + list(extra)).encode())
-        for f in (CSRC / src, CSRC / "ptx.cuh", CSRC / "kernel_params.h", ROOT / "include" / "cubecl_b200.h"):
+        for f in (CSRC / src, CSRC / "ptx.cuh", CSRC / "epilogue.cuh", CSRC / "kernel_params.h", ROOT / "include" / "cubecl_b200.h"):
             h.update(f.read_bytes())
         return h.hexdigest()
 

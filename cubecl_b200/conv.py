@@ -12,6 +12,10 @@ The gradients (b200_conv2d_backward_data / _weight) run on the same GEMM kernel:
                                 convolution per output phase (h % sh, w % sw), each storing its pixels straight into dx.
   dw = backward_weight(x, dy):  M = Cout, N = KH * KW * C, K = N * OH * OW pixels, with x read through im2col loads.
 The bias gradient is reduce.launch(client, "sum", dy viewed as [N * OH * OW, Cout], axis=0): no separate entry point.
+
+Grouped and depthwise convolution (groups > 1, b200_conv2d_grouped*): w and dw are [Cout, KH, KW, C / groups], group g maps
+input channels [g C/groups, (g+1) C/groups) to output channels [g Cout/groups, (g+1) Cout/groups).  Groups of >= 64 channels
+run one GEMM per group on channel slices; narrower groups run direct CUDA-core kernels.  groups=1 calls the plain entry points.
 """
 from __future__ import annotations
 
@@ -36,8 +40,8 @@ def _pair(v, what: str) -> tuple[int, int]:
     return v
 
 
-def calculate_conv2d_output(x_shape, w_shape, stride=1, padding=0, dilation=1) -> list[int]:
-    """[N, OH, OW, Cout] of an NHWC input [N, H, W, C] and weights [Cout, KH, KW, C]; PyTorch's rule:
+def calculate_conv2d_output(x_shape, w_shape, stride=1, padding=0, dilation=1, groups: int = 1) -> list[int]:
+    """[N, OH, OW, Cout] of an NHWC input [N, H, W, C] and weights [Cout, KH, KW, C / groups]; PyTorch's rule:
     OH = floor((H + 2*ph - dh*(KH-1) - 1) / sh) + 1, OW likewise."""
     x_shape, w_shape = [int(s) for s in x_shape], [int(s) for s in w_shape]
     if len(x_shape) != 4 or len(w_shape) != 4:
@@ -45,8 +49,10 @@ def calculate_conv2d_output(x_shape, w_shape, stride=1, padding=0, dilation=1) -
     (sh, sw), (ph, pw), (dh, dw) = _pair(stride, "stride"), _pair(padding, "padding"), _pair(dilation, "dilation")
     n, h, w, c = x_shape
     cout, kh, kw, c2 = w_shape
-    if c != c2:
-        raise ConvShapeError(f"channels differ: x has {c}, w has {c2}")
+    if groups < 1 or c % groups or cout % groups:
+        raise ConvShapeError(f"groups = {groups} must be >= 1 and divide C = {c} and Cout = {cout}")
+    if c // groups != c2:
+        raise ConvShapeError(f"channels differ: x has {c} in {groups} group(s), w has {c2} per group")
     if sh < 1 or sw < 1 or dh < 1 or dw < 1 or ph < 0 or pw < 0:
         raise ConvShapeError("strides and dilations must be >= 1 and padding >= 0")
     nh, nw = h + 2 * ph - dh * (kh - 1) - 1, w + 2 * pw - dw * (kw - 1) - 1
@@ -56,10 +62,11 @@ def calculate_conv2d_output(x_shape, w_shape, stride=1, padding=0, dilation=1) -
 
 
 def launch(client: ComputeClient, x: TensorHandle, w: TensorHandle, out: TensorHandle, stride=1, padding=0, dilation=1,
-           alpha: float = 1.0, bias: TensorHandle | None = None, activation: str | None = None, stream=None) -> None:
+           alpha: float = 1.0, bias: TensorHandle | None = None, activation: str | None = None, stream=None, groups: int = 1) -> None:
     """Enqueue the convolution on the client's stream.  stride / padding / dilation are ints or (h, w) pairs.  Optional fused
-    epilogue: out = activation(alpha * conv + bias[co]) with `bias` an f32 [Cout] tensor.  Never raises for launch problems:
-    errors are deferred to client.sync() / read_one() like matmul.launch."""
+    epilogue: out = activation(alpha * conv + bias[co]) with `bias` an f32 [Cout] tensor.  groups > 1: a grouped convolution
+    with w [Cout, KH, KW, C / groups].  Never raises for launch problems: errors are deferred to client.sync() / read_one()
+    like matmul.launch."""
     try:
         if activation not in ACTIVATIONS:
             raise B200Error(6, f"unknown activation {activation!r}")
@@ -76,21 +83,32 @@ def launch(client: ComputeClient, x: TensorHandle, w: TensorHandle, out: TensorH
         ep = None
         if alpha != 1.0 or bias is not None or activation not in (None, "none"):
             ep = C.byref(_ffi.Epilogue(float(alpha), ACTIVATIONS[activation], bias.handle.ptr if bias is not None else 0))
-        _ffi.check(client._lib.b200_conv2d(
-            client._ctx, stream, DTYPES[x.dtype], DTYPES[out.dtype],
-            C.c_uint64(x.handle.ptr), _ffi.u64_array(x.shape), _ffi.u64_array(x.strides),
-            C.c_uint64(w.handle.ptr), _ffi.u64_array(w.shape), _ffi.u64_array(w.strides),
-            C.c_uint64(out.handle.ptr), _ffi.u64_array(out.shape), _ffi.u64_array(out.strides), C.byref(args), ep))
+        operands = (client._ctx, stream, DTYPES[x.dtype], DTYPES[out.dtype],
+                    C.c_uint64(x.handle.ptr), _ffi.u64_array(x.shape), _ffi.u64_array(x.strides),
+                    C.c_uint64(w.handle.ptr), _ffi.u64_array(w.shape), _ffi.u64_array(w.strides),
+                    C.c_uint64(out.handle.ptr), _ffi.u64_array(out.shape), _ffi.u64_array(out.strides), C.byref(args))
+        if groups == 1:
+            _ffi.check(client._lib.b200_conv2d(*operands, ep))
+        else:
+            _ffi.check(client._lib.b200_conv2d_grouped(*operands, _groups(groups), ep))
     except (B200Error, ValueError) as e:
         client._defer(e if isinstance(e, B200Error) else B200Error(6, str(e)))
 
 
 def launch_alloc(client: ComputeClient, x: TensorHandle, w: TensorHandle, out_dtype: str | None = None, **kwargs) -> TensorHandle:
     """Convenience: allocate a compact NHWC `out` with the output rule, then launch (keyword arguments as launch)."""
-    shape = calculate_conv2d_output(x.shape, w.shape, kwargs.get("stride", 1), kwargs.get("padding", 0), kwargs.get("dilation", 1))
+    shape = calculate_conv2d_output(x.shape, w.shape, kwargs.get("stride", 1), kwargs.get("padding", 0), kwargs.get("dilation", 1),
+                                    kwargs.get("groups", 1))
     out = TensorHandle.empty_contiguous(client, shape, out_dtype or x.dtype)
     launch(client, x, w, out, **kwargs)
     return out
+
+
+def _groups(groups) -> C.c_uint32:
+    groups = int(groups)
+    if not 0 <= groups < 2 ** 32:
+        raise B200Error(6, f"conv2d: groups = {groups} out of range")
+    return C.c_uint32(groups)
 
 
 def _check_grad_operands(what: str, a: TensorHandle, b: TensorHandle, out: TensorHandle) -> None:
@@ -101,8 +119,8 @@ def _check_grad_operands(what: str, a: TensorHandle, b: TensorHandle, out: Tenso
 
 
 def backward_data(client: ComputeClient, dy: TensorHandle, w: TensorHandle, dx: TensorHandle, stride=1, padding=0, dilation=1,
-                  stream=None) -> None:
-    """Enqueue dx = the gradient of conv2d with respect to its input: dy [N, OH, OW, Cout], w [Cout, KH, KW, C], dx
+                  stream=None, groups: int = 1) -> None:
+    """Enqueue dx = the gradient of conv2d with respect to its input: dy [N, OH, OW, Cout], w [Cout, KH, KW, C / groups], dx
     [N, H, W, C] (NHWC), with dy's shape the output rule of (dx, w).  Errors are deferred like launch."""
     try:
         _check_grad_operands("conv2d_backward_data", dy, w, dx)
@@ -110,11 +128,14 @@ def backward_data(client: ComputeClient, dy: TensorHandle, w: TensorHandle, dx: 
         for t in (dy, w, dx):
             t.handle.used_on(stream)
         args = _ffi.Conv2dArgs(sh, sw, ph, pw, dh, dw)
-        _ffi.check(client._lib.b200_conv2d_backward_data(
-            client._ctx, stream, DTYPES[dy.dtype], DTYPES[dx.dtype],
-            C.c_uint64(dy.handle.ptr), _ffi.u64_array(dy.shape), _ffi.u64_array(dy.strides),
-            C.c_uint64(w.handle.ptr), _ffi.u64_array(w.shape), _ffi.u64_array(w.strides),
-            C.c_uint64(dx.handle.ptr), _ffi.u64_array(dx.shape), _ffi.u64_array(dx.strides), C.byref(args)))
+        operands = (client._ctx, stream, DTYPES[dy.dtype], DTYPES[dx.dtype],
+                    C.c_uint64(dy.handle.ptr), _ffi.u64_array(dy.shape), _ffi.u64_array(dy.strides),
+                    C.c_uint64(w.handle.ptr), _ffi.u64_array(w.shape), _ffi.u64_array(w.strides),
+                    C.c_uint64(dx.handle.ptr), _ffi.u64_array(dx.shape), _ffi.u64_array(dx.strides), C.byref(args))
+        if groups == 1:
+            _ffi.check(client._lib.b200_conv2d_backward_data(*operands))
+        else:
+            _ffi.check(client._lib.b200_conv2d_grouped_backward_data(*operands, _groups(groups)))
     except (B200Error, ValueError) as e:
         client._defer(e if isinstance(e, B200Error) else B200Error(6, str(e)))
 
@@ -122,37 +143,44 @@ def backward_data(client: ComputeClient, dy: TensorHandle, w: TensorHandle, dx: 
 def backward_data_alloc(client: ComputeClient, dy: TensorHandle, w: TensorHandle, input_hw, out_dtype: str | None = None,
                         **kwargs) -> TensorHandle:
     """Convenience: allocate a compact NHWC dx [N, H, W, C] with (H, W) = input_hw (the forward input's extents; a stride > 1
-    convolution maps several H to one OH), then backward_data (keyword arguments as backward_data)."""
+    convolution maps several H to one OH) and C = groups * w.shape[3], then backward_data (keyword arguments as
+    backward_data)."""
     h, wd = _pair(input_hw, "input_hw")
-    dx = TensorHandle.empty_contiguous(client, [dy.shape[0], h, wd, w.shape[3]], out_dtype or dy.dtype)
+    dx = TensorHandle.empty_contiguous(client, [dy.shape[0], h, wd, w.shape[3] * int(kwargs.get("groups", 1))], out_dtype or dy.dtype)
     backward_data(client, dy, w, dx, **kwargs)
     return dx
 
 
 def backward_weight(client: ComputeClient, x: TensorHandle, dy: TensorHandle, dw: TensorHandle, stride=1, padding=0, dilation=1,
-                    stream=None) -> None:
+                    stream=None, groups: int = 1) -> None:
     """Enqueue dw = the gradient of conv2d with respect to its weights: x [N, H, W, C], dy [N, OH, OW, Cout], dw
-    [Cout, KH, KW, C], with dy's shape the output rule of (x, dw).  Errors are deferred like launch."""
+    [Cout, KH, KW, C / groups], with dy's shape the output rule of (x, dw).  Errors are deferred like launch."""
     try:
         _check_grad_operands("conv2d_backward_weight", x, dy, dw)
         (sh, sw), (ph, pw), (dh, dw_) = _pair(stride, "stride"), _pair(padding, "padding"), _pair(dilation, "dilation")
         for t in (x, dy, dw):
             t.handle.used_on(stream)
         args = _ffi.Conv2dArgs(sh, sw, ph, pw, dh, dw_)
-        _ffi.check(client._lib.b200_conv2d_backward_weight(
-            client._ctx, stream, DTYPES[x.dtype], DTYPES[dw.dtype],
-            C.c_uint64(x.handle.ptr), _ffi.u64_array(x.shape), _ffi.u64_array(x.strides),
-            C.c_uint64(dy.handle.ptr), _ffi.u64_array(dy.shape), _ffi.u64_array(dy.strides),
-            C.c_uint64(dw.handle.ptr), _ffi.u64_array(dw.shape), _ffi.u64_array(dw.strides), C.byref(args)))
+        operands = (client._ctx, stream, DTYPES[x.dtype], DTYPES[dw.dtype],
+                    C.c_uint64(x.handle.ptr), _ffi.u64_array(x.shape), _ffi.u64_array(x.strides),
+                    C.c_uint64(dy.handle.ptr), _ffi.u64_array(dy.shape), _ffi.u64_array(dy.strides),
+                    C.c_uint64(dw.handle.ptr), _ffi.u64_array(dw.shape), _ffi.u64_array(dw.strides), C.byref(args))
+        if groups == 1:
+            _ffi.check(client._lib.b200_conv2d_backward_weight(*operands))
+        else:
+            _ffi.check(client._lib.b200_conv2d_grouped_backward_weight(*operands, _groups(groups)))
     except (B200Error, ValueError) as e:
         client._defer(e if isinstance(e, B200Error) else B200Error(6, str(e)))
 
 
 def backward_weight_alloc(client: ComputeClient, x: TensorHandle, dy: TensorHandle, kernel_hw, out_dtype: str | None = None,
                           **kwargs) -> TensorHandle:
-    """Convenience: allocate a compact dw [Cout, KH, KW, C] with (KH, KW) = kernel_hw, then backward_weight (keyword arguments
-    as backward_weight)."""
+    """Convenience: allocate a compact dw [Cout, KH, KW, C / groups] with (KH, KW) = kernel_hw, then backward_weight (keyword
+    arguments as backward_weight)."""
     kh, kw = _pair(kernel_hw, "kernel_hw")
-    dw = TensorHandle.empty_contiguous(client, [dy.shape[3], kh, kw, x.shape[3]], out_dtype or x.dtype)
+    groups = int(kwargs.get("groups", 1))
+    if groups < 1 or x.shape[3] % groups:
+        raise ValueError(f"groups = {groups} must be >= 1 and divide C = {x.shape[3]}")
+    dw = TensorHandle.empty_contiguous(client, [dy.shape[3], kh, kw, x.shape[3] // groups], out_dtype or x.dtype)
     backward_weight(client, x, dy, dw, **kwargs)
     return dw

@@ -49,6 +49,8 @@ extern const unsigned char b200_cubin_gemm_conv[];
 extern const unsigned char b200_cubin_gemm_conv_end[];
 extern const unsigned char b200_cubin_gemm_convbwd[];
 extern const unsigned char b200_cubin_gemm_convbwd_end[];
+extern const unsigned char b200_cubin_conv_grouped[];
+extern const unsigned char b200_cubin_conv_grouped_end[];
 }
 
 // ================================================================================================ errors
@@ -319,13 +321,15 @@ static int get_func(b200_ctx* c, const std::string& name, CUfunction* out) {
   if (c->dry) { c->pending_kernel = name; *out = nullptr; return B200_OK; }
   auto it = c->funcs.find(name);
   if (it != c->funcs.end()) { *out = it->second; return B200_OK; }
-  // modules are loaded in the order gemm, reduce, aux, gemm_b, gemm_c, quant, gemm_q, quant_mm, gemm_conv, gemm_convbwd; the kernel
+  // modules are loaded in the order gemm, reduce, aux, gemm_b, gemm_c, quant, gemm_q, quant_mm, gemm_conv, gemm_convbwd,
+  // conv_grouped; the kernel
   // name says where a
   // kernel lives (no failing lookups, which API-level tools such as compute-sanitizer would report)
   auto starts = [&](const char* pfx) { return name.rfind(pfx, 0) == 0; };
   auto has = [&](const char* part) { return name.find(part) != std::string::npos; };
   const bool tc_gemm = starts("gemm_") && name != "gemm_simt_strided" && name != "gemm_scaled_simt";
-  const size_t home = starts("conv2d_dgrad_") || starts("conv2d_wgrad_") ? 9
+  const size_t home = starts("conv2d_grp_") ? 10
+                      : starts("conv2d_dgrad_") || starts("conv2d_wgrad_") ? 9
                       : starts("conv2d_") ? 8
                       : starts("gemm_q8") ? 6
                       : starts("quant_scales_") || starts("quant_widen_") ? 7
@@ -358,7 +362,8 @@ extern "C" int b200_get_cubin(const char* name, const void** image, size_t* size
   else if (!strcmp(name, "quant_mm")) { b = b200_cubin_quant_mm; e = b200_cubin_quant_mm_end; }
   else if (!strcmp(name, "gemm_conv")) { b = b200_cubin_gemm_conv; e = b200_cubin_gemm_conv_end; }
   else if (!strcmp(name, "gemm_convbwd")) { b = b200_cubin_gemm_convbwd; e = b200_cubin_gemm_convbwd_end; }
-  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd)", name);
+  else if (!strcmp(name, "conv_grouped")) { b = b200_cubin_conv_grouped; e = b200_cubin_conv_grouped_end; }
+  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd|conv_grouped)", name);
   *image = b;
   *size = static_cast<size_t>(e - b);
   return B200_OK;
@@ -415,7 +420,8 @@ extern "C" int b200_init(int device, b200_ctx** out) {
       (rc = load_module(c, b200_cubin_gemm_q, b200_cubin_gemm_q_end, "gemm_q")) ||
       (rc = load_module(c, b200_cubin_quant_mm, b200_cubin_quant_mm_end, "quant_mm")) ||
       (rc = load_module(c, b200_cubin_gemm_conv, b200_cubin_gemm_conv_end, "gemm_conv")) ||
-      (rc = load_module(c, b200_cubin_gemm_convbwd, b200_cubin_gemm_convbwd_end, "gemm_convbwd"))) {
+      (rc = load_module(c, b200_cubin_gemm_convbwd, b200_cubin_gemm_convbwd_end, "gemm_convbwd")) ||
+      (rc = load_module(c, b200_cubin_conv_grouped, b200_cubin_conv_grouped_end, "conv_grouped"))) {
     for (CUmodule m : c->modules) g_drv.cuModuleUnload_p(m);
     g_drv.cuDevicePrimaryCtxRelease_p(c->dev);
     return bail(rc);
@@ -3027,6 +3033,318 @@ extern "C" int b200_conv2d_backward_weight(b200_ctx* c, b200_stream s, b200_dtyp
   }
   for (CUdeviceptr t : tmp)
     if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMM has drained
+  return rc;
+}
+
+// ------------------------------------------------------------------------------------------------ grouped convolution
+// Routing, from the shape alone: groups == 1 is the plain entry point; a group width Cg = C / groups of at least one
+// k-block (64 channels) runs one implicit GEMM per group on channel slices; narrower groups run the direct kernels of
+// conv_grouped.cu, for which the GEMM route would multiply mostly zero-padded k-blocks.
+constexpr uint64_t kGrpGemmMinCg = 64;
+
+static int grp_check(const char* what, uint32_t groups, uint64_t C, uint64_t Cout, uint64_t w_c) {
+  if (groups == 0) return fail(B200_ERR_INVALID_ARG, "%s: groups must be >= 1", what);
+  if (C % groups || Cout % groups)
+    return fail(B200_ERR_INVALID_ARG, "%s: groups = %u must divide C = %llu and Cout = %llu", what, groups, (unsigned long long)C,
+                (unsigned long long)Cout);
+  if (w_c != C / groups)
+    return fail(B200_ERR_INVALID_ARG, "%s: weights have %llu channels, C / groups = %llu", what, (unsigned long long)w_c,
+                (unsigned long long)(C / groups));
+  return B200_OK;
+}
+
+// The forward's limits on (args, kernel extent), applied to every direct-route kernel so both routes accept the same shapes.
+static int grp_limits(const char* what, const b200_conv2d_args& a, uint64_t KH, uint64_t KW) {
+  const int64_t corners[4] = {-(int64_t)a.pad_h, -(int64_t)a.pad_w, (int64_t)a.pad_h - (int64_t)a.dilation_h * ((int64_t)KH - 1),
+                              (int64_t)a.pad_w - (int64_t)a.dilation_w * ((int64_t)KW - 1)};
+  for (int64_t k : corners)
+    if (k < -128 || k > 127)
+      return fail(B200_ERR_UNSUPPORTED, "%s: pixel-box corner %lld outside [-128, 127] (-pad and pad - dilation * (kernel - 1))", what,
+                  (long long)k);
+  if (a.stride_h > 8 || a.stride_w > 8) return fail(B200_ERR_UNSUPPORTED, "%s: the conv stride must be <= 8", what);
+  return B200_OK;
+}
+
+// A rank-4 operand the direct kernels read through its strides: kept in place with a unit channel stride, else gathered
+// into a compact pooled copy (*tmp, freed by the caller).  s: the strides to read it with.
+static int grp_operand(b200_ctx* c, CUstream st, b200_dtype dt, uint64_t ptr, const uint64_t* shape, const uint64_t* ns,
+                       CUdeviceptr* tmp, uint64_t* out, uint64_t s[4]) {
+  if (ns[3] == 1) {
+    *out = ptr;
+    for (int d = 0; d < 4; ++d) s[d] = ns[d];
+    return B200_OK;
+  }
+  int rc = conv_gather(c, st, dt, ptr, shape, ns, tmp);
+  *out = *tmp;
+  s[3] = 1; s[2] = shape[3]; s[1] = shape[2] * shape[3]; s[0] = shape[1] * shape[2] * shape[3];
+  return rc;
+}
+
+static const char* grp_tag(b200_dtype dt) { return dt == B200_BF16 ? "bf16" : dt == B200_F16 ? "f16" : "f32"; }
+
+extern "C" int b200_conv2d_grouped(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr x,
+                                   const uint64_t* x_shape, const uint64_t* x_strides, b200_dptr w, const uint64_t* w_shape,
+                                   const uint64_t* w_strides, b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides,
+                                   const b200_conv2d_args* args, uint32_t groups, const b200_epilogue* ep) {
+  CTX_ENTER(c);
+  const char* what = "conv2d_grouped";
+  if (!x_shape || !w_shape || !out_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
+  if (groups == 1)
+    return b200_conv2d(c, s, in_dtype, out_dtype, x, x_shape, x_strides, w, w_shape, w_strides, out, out_shape, out_strides, args, ep);
+  const uint64_t N = x_shape[0], H = x_shape[1], W = x_shape[2], C = x_shape[3];
+  const uint64_t Cout = w_shape[0], KH = w_shape[1], KW = w_shape[2];
+  int rc = grp_check(what, groups, C, Cout, w_shape[3]);
+  if (rc) return rc;
+  if (in_dtype != B200_F16 && in_dtype != B200_BF16)
+    return fail(B200_ERR_UNSUPPORTED, "%s: input dtype %d unsupported (f16, bf16)", what, (int)in_dtype);
+  if (out_dtype != in_dtype && out_dtype != B200_F32)
+    return fail(B200_ERR_UNSUPPORTED, "%s: output dtype must equal the input dtype or be f32", what);
+  if (ep && (ep->activation < 0 || ep->activation > 2)) return fail(B200_ERR_INVALID_ARG, "%s: unknown activation %d", what, ep->activation);
+  const b200_conv2d_args& a = *args;
+  if (a.stride_h < 1 || a.stride_w < 1 || a.dilation_h < 1 || a.dilation_w < 1 || a.pad_h < 0 || a.pad_w < 0)
+    return fail(B200_ERR_INVALID_ARG, "%s: strides and dilations must be >= 1 and padding >= 0", what);
+  if (N == 0 || H == 0 || W == 0 || C == 0 || Cout == 0 || KH == 0 || KW == 0) return B200_OK;
+  const uint64_t lim = 1ull << 31;
+  if (N >= lim || H >= lim || W >= lim || C >= lim || Cout >= lim || KH >= lim || KW >= lim)
+    return fail(B200_ERR_UNSUPPORTED, "%s: extents must be < 2^31", what);
+  const int64_t nh = (int64_t)H + 2 * (int64_t)a.pad_h - (int64_t)a.dilation_h * ((int64_t)KH - 1) - 1;
+  const int64_t nw = (int64_t)W + 2 * (int64_t)a.pad_w - (int64_t)a.dilation_w * ((int64_t)KW - 1) - 1;
+  if (nh < 0 || nw < 0) return fail(B200_ERR_INVALID_ARG, "%s: the dilated kernel is larger than the padded input (output extent < 1)", what);
+  const uint64_t OH = (uint64_t)(nh / a.stride_h) + 1, OW = (uint64_t)(nw / a.stride_w) + 1;
+  if (out_shape[0] != N || out_shape[1] != OH || out_shape[2] != OW || out_shape[3] != Cout)
+    return fail(B200_ERR_INVALID_ARG, "%s: out is [%llu,%llu,%llu,%llu], expected [%llu,%llu,%llu,%llu]", what,
+                (unsigned long long)out_shape[0], (unsigned long long)out_shape[1], (unsigned long long)out_shape[2],
+                (unsigned long long)out_shape[3], (unsigned long long)N, (unsigned long long)OH, (unsigned long long)OW,
+                (unsigned long long)Cout);
+  if (!x || !w || !out) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
+  const size_t osz = dtype_size(out_dtype);
+  if (out % osz) return fail(B200_ERR_INVALID_ARG, "%s: output pointer is not aligned to its element size", what);
+  const uint64_t Cg = C / groups, Coutg = Cout / groups;
+  uint64_t xs[4], ws[4], os[4];
+  conv_norm_strides(x_shape, x_strides, xs);
+  conv_norm_strides(w_shape, w_strides, ws);
+  conv_norm_strides(out_shape, out_strides, os);
+  if (Cg >= kGrpGemmMinCg) {
+    // one b200_conv2d per group: x, w and out are read and written in place through channel slices
+    const uint64_t sx[4] = {N, H, W, Cg}, sw[4] = {Coutg, KH, KW, Cg}, so[4] = {N, OH, OW, Coutg};
+    for (uint64_t g = 0; g < groups && !rc; ++g) {
+      b200_epilogue eg{};
+      if (ep) {
+        eg = *ep;
+        if (eg.bias) eg.bias += g * Coutg * 4;
+      }
+      rc = b200_conv2d(c, s, in_dtype, out_dtype, x + g * Cg * xs[3] * 2, sx, xs, w + g * Coutg * ws[0] * 2, sw, ws,
+                       out + g * Coutg * os[3] * osz, so, os, args, ep ? &eg : nullptr);
+    }
+    return rc;
+  }
+  if ((rc = grp_limits(what, a, KH, KW))) return rc;
+  if (N * OH * OW >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * OH * OW = %llu must be < 2^31", what, (unsigned long long)(N * OH * OW));
+  if (os[3] != 1 || os[2] < Cout || os[1] != OW * os[2] || os[0] != OH * os[1])
+    return fail(B200_ERR_UNSUPPORTED, "%s: out must have unit channel stride and one pixel pitch >= Cout for N, OH, OW", what);
+  const uint64_t tiles_h = (OH + kGrpTileH - 1) / kGrpTileH, tiles_w = (OW + kGrpTileW - 1) / kGrpTileW;
+  const uint64_t chunks = (Cout + kGrpChunk - 1) / kGrpChunk;
+  if (N * tiles_h * tiles_w >= lim || chunks > 65535)
+    return fail(B200_ERR_UNSUPPORTED, "%s: too many output tiles (N * ceil(OH / 8) * ceil(OW / 8) < 2^31, Cout <= 2^21)", what);
+  CUstream st = resolve_stream(c, s);
+  CUdeviceptr tmp[2] = {0, 0};
+  ConvGroupedParams p;
+  memset(&p, 0, sizeof(p));
+  uint64_t xsr[4], wsr[4];
+  rc = grp_operand(c, st, in_dtype, x, x_shape, xs, &tmp[0], &p.x, xsr);
+  if (!rc) rc = grp_operand(c, st, in_dtype, w, w_shape, ws, &tmp[1], &p.w, wsr);
+  if (!rc) {
+    p.out = out;
+    p.x_sn = xsr[0]; p.x_sh = xsr[1]; p.x_sw = xsr[2];
+    p.w_sco = wsr[0]; p.w_sky = wsr[1]; p.w_skx = wsr[2];
+    p.o_sn = os[0]; p.o_sh = os[1]; p.o_sw = os[2];
+    p.N = (uint32_t)N; p.H = (uint32_t)H; p.W = (uint32_t)W; p.C = (uint32_t)C; p.OH = (uint32_t)OH; p.OW = (uint32_t)OW;
+    p.Cout = (uint32_t)Cout; p.KH = (uint32_t)KH; p.KW = (uint32_t)KW; p.Cg = (uint32_t)Cg; p.Coutg = (uint32_t)Coutg;
+    p.sh = a.stride_h; p.sw = a.stride_w; p.ph = a.pad_h; p.pw = a.pad_w; p.dh = a.dilation_h; p.dw = a.dilation_w;
+    p.tiles_h = (uint32_t)tiles_h; p.tiles_w = (uint32_t)tiles_w;
+    p.vec_x = (p.x % 16 == 0 && xsr[0] % 8 == 0 && xsr[1] % 8 == 0 && xsr[2] % 8 == 0) ? 1u : 0u;
+    if (ep) {
+      p.alpha = ep->alpha; p.bias = ep->bias; p.epi_act = (uint32_t)ep->activation;
+    } else {
+      p.alpha = 1.0f;
+    }
+    p.epi_on = (p.alpha != 1.0f || p.bias != 0 || p.epi_act != 0) ? 1u : 0u;
+    // the input channels one chunk of kGrpChunk output channels reads, at most; the halo is staged when it fits
+    uint64_t span = 0;
+    for (uint64_t co0 = 0; co0 < Cout; co0 += kGrpChunk) {
+      const uint64_t co_end = std::min<uint64_t>(co0 + kGrpChunk, Cout);
+      span = std::max(span, std::min(C, ((co_end - 1) / Coutg + 1) * Cg) - (co0 / Coutg) * Cg);
+    }
+    const uint64_t pitch = (span + 7) / 8 * 8;
+    const uint64_t hh = (kGrpTileH - 1) * (uint64_t)a.stride_h + (KH - 1) * (uint64_t)a.dilation_h + 1;
+    const uint64_t hw = (kGrpTileW - 1) * (uint64_t)a.stride_w + (KW - 1) * (uint64_t)a.dilation_w + 1;
+    const uint64_t smem = hh * hw * pitch * 2;
+    p.staged_ci = smem <= (uint64_t)kGrpSmemMax ? (uint32_t)pitch : 0u;
+    CUfunction f;
+    rc = get_func(c, std::string("conv2d_grp_") + grp_tag(in_dtype) + "_" + grp_tag(out_dtype), &f);
+    void* kargs[] = {&p};
+    if (!rc) rc = launch(c, f, (unsigned)(N * tiles_h * tiles_w), (unsigned)chunks, 1, 256, p.staged_ci ? (unsigned)smem : 0u, 1, st, kargs);
+  }
+  for (CUdeviceptr t : tmp)
+    if (t) pool_free(c, t, st);
+  return rc;
+}
+
+extern "C" int b200_conv2d_grouped_backward_data(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr dy,
+                                                 const uint64_t* dy_shape, const uint64_t* dy_strides, b200_dptr w,
+                                                 const uint64_t* w_shape, const uint64_t* w_strides, b200_dptr dx,
+                                                 const uint64_t* dx_shape, const uint64_t* dx_strides, const b200_conv2d_args* args,
+                                                 uint32_t groups) {
+  CTX_ENTER(c);
+  const char* what = "conv2d_grouped_backward_data";
+  if (!dy_shape || !w_shape || !dx_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
+  if (groups == 1)
+    return b200_conv2d_backward_data(c, s, in_dtype, out_dtype, dy, dy_shape, dy_strides, w, w_shape, w_strides, dx, dx_shape, dx_strides, args);
+  const uint64_t N = dx_shape[0], H = dx_shape[1], W = dx_shape[2], C = dx_shape[3];
+  const uint64_t Cout = w_shape[0], KH = w_shape[1], KW = w_shape[2];
+  int rc = grp_check(what, groups, C, Cout, w_shape[3]);
+  if (rc) return rc;
+  const b200_conv2d_args& a = *args;
+  const uint64_t w_full[4] = {Cout, KH, KW, C};
+  uint64_t OH = 0, OW = 0;
+  if ((rc = conv_bwd_check(what, in_dtype, out_dtype, a, dx_shape, w_full, dy_shape, &OH, &OW))) return rc;
+  if (N == 0 || H == 0 || W == 0 || C == 0) return B200_OK;   // no dx
+  if (!dy || !w || !dx) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
+  const size_t osz = dtype_size(out_dtype);
+  if (dx % osz) return fail(B200_ERR_INVALID_ARG, "%s: dx pointer is not aligned to its element size", what);
+  const uint64_t Cg = C / groups, Coutg = Cout / groups;
+  uint64_t ys[4], ws[4], os[4];
+  conv_norm_strides(dy_shape, dy_strides, ys);
+  conv_norm_strides(w_shape, w_strides, ws);
+  conv_norm_strides(dx_shape, dx_strides, os);
+  if (Cg >= kGrpGemmMinCg) {
+    const uint64_t sy[4] = {N, OH, OW, Coutg}, sw[4] = {Coutg, KH, KW, Cg}, sx[4] = {N, H, W, Cg};
+    for (uint64_t g = 0; g < groups && !rc; ++g)
+      rc = b200_conv2d_backward_data(c, s, in_dtype, out_dtype, dy + g * Coutg * ys[3] * 2, sy, ys, w + g * Coutg * ws[0] * 2, sw, ws,
+                                     dx + g * Cg * os[3] * osz, sx, os, args);
+    return rc;
+  }
+  if (KH && KW && (rc = grp_limits(what, a, KH, KW))) return rc;
+  const uint64_t lim = 1ull << 31;
+  if (N * H * W >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * H * W = %llu must be < 2^31", what, (unsigned long long)(N * H * W));
+  if (os[3] != 1 || os[2] < C || os[1] != W * os[2] || os[0] != H * os[1])
+    return fail(B200_ERR_UNSUPPORTED, "%s: dx must have unit channel stride and one pixel pitch >= C for N, H, W", what);
+  const uint64_t chunks = (C + kGrpChunk - 1) / kGrpChunk;
+  if (chunks > 65535) return fail(B200_ERR_UNSUPPORTED, "%s: C must be <= 2^21", what);
+  CUstream st = resolve_stream(c, s);
+  CUdeviceptr tmp[2] = {0, 0};
+  ConvGroupedParams p;
+  memset(&p, 0, sizeof(p));
+  uint64_t ysr[4] = {0, 0, 0, 1}, wsr[4] = {0, 0, 0, 1};
+  // an empty dy or kernel reads nothing: dx comes out as +0 from the same launch
+  if (Cout && KH && KW) {
+    rc = grp_operand(c, st, in_dtype, dy, dy_shape, ys, &tmp[0], &p.x, ysr);
+    if (!rc) rc = grp_operand(c, st, in_dtype, w, w_shape, ws, &tmp[1], &p.w, wsr);
+  }
+  if (!rc) {
+    p.out = dx;
+    p.x_sn = ysr[0]; p.x_sh = ysr[1]; p.x_sw = ysr[2];
+    p.w_sco = wsr[0]; p.w_sky = wsr[1]; p.w_skx = wsr[2];
+    p.o_sn = os[0]; p.o_sh = os[1]; p.o_sw = os[2];
+    p.N = (uint32_t)N; p.H = (uint32_t)H; p.W = (uint32_t)W; p.C = (uint32_t)C; p.OH = (uint32_t)OH; p.OW = (uint32_t)OW;
+    p.Cout = (uint32_t)Cout; p.KH = (uint32_t)KH; p.KW = (uint32_t)KW; p.Cg = (uint32_t)Cg; p.Coutg = (uint32_t)Coutg;
+    p.sh = a.stride_h; p.sw = a.stride_w; p.ph = a.pad_h; p.pw = a.pad_w; p.dh = a.dilation_h; p.dw = a.dilation_w;
+    CUfunction f;
+    rc = get_func(c, std::string("conv2d_grp_dgrad_") + grp_tag(in_dtype) + "_" + grp_tag(out_dtype), &f);
+    void* kargs[] = {&p};
+    if (!rc) rc = launch(c, f, (unsigned)((N * H * W + 7) / 8), (unsigned)chunks, 1, 256, 0, 1, st, kargs);
+  }
+  for (CUdeviceptr t : tmp)
+    if (t) pool_free(c, t, st);
+  return rc;
+}
+
+// Segments of the weight gradient's pixel sum, a function of the shape only: enough (elements x segments) threads to fill
+// the GPU (2^18, at most 4096 segments), each segment at least 64 pixels.
+static void grp_wgrad_segments(uint64_t P, uint64_t elems, uint64_t* seg_len, uint64_t* nseg) {
+  const uint64_t want = std::min<uint64_t>(4096, std::max<uint64_t>(1, ((1ull << 18) + elems - 1) / elems));
+  *seg_len = std::max<uint64_t>(64, (P + want - 1) / want);
+  *nseg = P ? (P + *seg_len - 1) / *seg_len : 1;
+}
+
+extern "C" int b200_conv2d_grouped_backward_weight(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr x,
+                                                   const uint64_t* x_shape, const uint64_t* x_strides, b200_dptr dy,
+                                                   const uint64_t* dy_shape, const uint64_t* dy_strides, b200_dptr dw,
+                                                   const uint64_t* dw_shape, const uint64_t* dw_strides, const b200_conv2d_args* args,
+                                                   uint32_t groups) {
+  CTX_ENTER(c);
+  const char* what = "conv2d_grouped_backward_weight";
+  if (!x_shape || !dy_shape || !dw_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
+  if (groups == 1)
+    return b200_conv2d_backward_weight(c, s, in_dtype, out_dtype, x, x_shape, x_strides, dy, dy_shape, dy_strides, dw, dw_shape, dw_strides,
+                                       args);
+  const uint64_t N = x_shape[0], H = x_shape[1], W = x_shape[2], C = x_shape[3];
+  const uint64_t Cout = dw_shape[0], KH = dw_shape[1], KW = dw_shape[2];
+  int rc = grp_check(what, groups, C, Cout, dw_shape[3]);
+  if (rc) return rc;
+  const b200_conv2d_args& a = *args;
+  const uint64_t dw_full[4] = {Cout, KH, KW, C};
+  uint64_t OH = 0, OW = 0;
+  if ((rc = conv_bwd_check(what, in_dtype, out_dtype, a, x_shape, dw_full, dy_shape, &OH, &OW))) return rc;
+  if (Cout == 0 || C == 0 || KH == 0 || KW == 0) return B200_OK;   // no dw
+  if ((rc = grp_limits(what, a, KH, KW))) return rc;
+  const uint64_t P = N * OH * OW, lim = 1ull << 31;
+  if (P >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * OH * OW = %llu must be < 2^31", what, (unsigned long long)P);
+  if (!x || !dy || !dw) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
+  const size_t osz = dtype_size(out_dtype);
+  if (dw % osz) return fail(B200_ERR_INVALID_ARG, "%s: dw pointer is not aligned to its element size", what);
+  const uint64_t Cg = C / groups, Coutg = Cout / groups;
+  uint64_t xs[4], ys[4], ds[4];
+  conv_norm_strides(x_shape, x_strides, xs);
+  conv_norm_strides(dy_shape, dy_strides, ys);
+  conv_norm_strides(dw_shape, dw_strides, ds);
+  if (Cg >= kGrpGemmMinCg) {
+    const uint64_t sx[4] = {N, H, W, Cg}, sy[4] = {N, OH, OW, Coutg}, sw[4] = {Coutg, KH, KW, Cg};
+    for (uint64_t g = 0; g < groups && !rc; ++g)
+      rc = b200_conv2d_backward_weight(c, s, in_dtype, out_dtype, x + g * Cg * xs[3] * 2, sx, xs, dy + g * Coutg * ys[3] * 2, sy, ys,
+                                       dw + g * Coutg * ds[0] * osz, sw, ds, args);
+    return rc;
+  }
+  const uint64_t dw_sp = (KW == 1) ? ds[1] : (KH == 1 || ds[1] == KW * ds[2]) ? ds[2] : 0;
+  if (ds[3] != 1 || dw_sp == 0 || ds[0] * osz >= (1ull << 40) || dw_sp * osz >= (1ull << 40))
+    return fail(B200_ERR_UNSUPPORTED, "%s: dw must have unit channel stride and (KH, KW) flattening into one stride", what);
+  const uint64_t elems = Cout * KH * KW * Cg;
+  if (elems >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: Cout * KH * KW * C / groups = %llu must be < 2^31", what, (unsigned long long)elems);
+  uint64_t seg_len = 0, nseg = 0;
+  grp_wgrad_segments(P, elems, &seg_len, &nseg);
+  if (c->dry) {
+    char line[160];
+    snprintf(line, sizeof(line), "conv grouped wgrad pixels=%llu elements=%llu segments=%llu length=%llu\n", (unsigned long long)P,
+             (unsigned long long)elems, (unsigned long long)nseg, (unsigned long long)seg_len);
+    c->plan += line;
+  }
+  CUstream st = resolve_stream(c, s);
+  CUdeviceptr tmp[3] = {0, 0, 0};
+  ConvGroupedParams p;
+  memset(&p, 0, sizeof(p));
+  uint64_t xsr[4], ysr[4];
+  rc = grp_operand(c, st, in_dtype, x, x_shape, xs, &tmp[0], &p.x, xsr);
+  if (!rc) rc = grp_operand(c, st, in_dtype, dy, dy_shape, ys, &tmp[1], &p.w, ysr);
+  if (!rc && nseg > 1) rc = pool_alloc(c, nseg * elems * 4, &tmp[2], st);
+  if (!rc) {
+    p.out = dw; p.part = tmp[2];
+    p.x_sn = xsr[0]; p.x_sh = xsr[1]; p.x_sw = xsr[2];
+    p.y_sn = ysr[0]; p.y_sh = ysr[1]; p.y_sw = ysr[2];
+    p.o_sn = ds[0]; p.o_sw = dw_sp;
+    p.seg_len = seg_len; p.elems = elems; p.nseg = (uint32_t)nseg;
+    p.N = (uint32_t)N; p.H = (uint32_t)H; p.W = (uint32_t)W; p.C = (uint32_t)C; p.OH = (uint32_t)OH; p.OW = (uint32_t)OW;
+    p.Cout = (uint32_t)Cout; p.KH = (uint32_t)KH; p.KW = (uint32_t)KW; p.Cg = (uint32_t)Cg; p.Coutg = (uint32_t)Coutg;
+    p.sh = a.stride_h; p.sw = a.stride_w; p.ph = a.pad_h; p.pw = a.pad_w; p.dh = a.dilation_h; p.dw = a.dilation_w;
+    const unsigned blocks = (unsigned)((elems + 255) / 256);
+    void* kargs[] = {&p};
+    CUfunction f;
+    rc = get_func(c, std::string("conv2d_grp_wgrad_") + grp_tag(in_dtype) + "_" + grp_tag(out_dtype), &f);
+    if (!rc) rc = launch(c, f, blocks, (unsigned)nseg, 1, 256, 0, 1, st, kargs);
+    if (!rc && nseg > 1) rc = get_func(c, std::string("conv2d_grp_wgrad_combine_") + grp_tag(out_dtype), &f);
+    if (!rc && nseg > 1) rc = launch(c, f, blocks, 1, 1, 256, 0, 1, st, kargs);
+  }
+  for (CUdeviceptr t : tmp)
+    if (t) pool_free(c, t, st);
   return rc;
 }
 

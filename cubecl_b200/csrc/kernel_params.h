@@ -149,6 +149,35 @@ struct ConvDgradWeightsParams {
   uint32_t kmax_h[kDgradMaxStride], kmax_w[kDgradMaxStride], taps_h[kDgradMaxStride], taps_w[kDgradMaxStride];
 };
 
+// ================================================================================================ conv_grouped.cu
+// Direct NHWC grouped convolution (b200_conv2d_grouped*, group width Cg = C / groups < 64).  Group g owns input channels
+// [g Cg, (g+1) Cg) and output channels [g Coutg, (g+1) Coutg).  Every strided operand has a unit channel stride; strides
+// are in elements.
+//   conv2d_grp_*        x [N, H, W, C], w [Cout, KH, KW, Cg] -> out [N, OH, OW, Cout] (fused epilogue as GemmParams)
+//   conv2d_grp_dgrad_*  dy [N, OH, OW, Cout], w -> dx [N, H, W, C]
+//   conv2d_grp_wgrad_*  x, dy -> f32 partials [nseg][elems] (nseg > 1) or dw (nseg == 1); conv2d_grp_wgrad_combine_* adds the
+//                       partials in segment order into dw.  Element t = (kpos * Cout + co) * Cg + ci, kpos = ky * KW + kx.
+// Forward tile: kGrpTileH x kGrpTileW output pixels of one image x kGrpChunk output channels (one per lane); the input halo
+// of those channels is staged in shared memory when it fits (staged_ci != 0: that many channels per halo pixel).
+constexpr int kGrpChunk = 32;
+constexpr int kGrpTileH = 8;
+constexpr int kGrpTileW = 8;
+constexpr int kGrpSmemMax = 48 * 1024;
+struct ConvGroupedParams {
+  uint64_t x, w, out, bias;          // x: x, or dy (dgrad); w: w, or dy (wgrad); bias: f32[Cout] or 0 (forward only)
+  uint64_t x_sn, x_sh, x_sw;         // x (forward, wgrad) or dy (dgrad): the strided NHWC input
+  uint64_t w_sco, w_sky, w_skx;      // w (forward, dgrad)
+  uint64_t y_sn, y_sh, y_sw;         // dy (wgrad)
+  uint64_t o_sn, o_sh, o_sw;         // out / dx: one pixel pitch; dw: o_sn = Cout stride, o_sw = kernel-position stride
+  uint64_t part;                     // wgrad: f32 partials [nseg][elems]
+  uint64_t seg_len, elems;           // wgrad: pixels per segment (the last may be shorter), Cout * KH * KW * Cg
+  uint32_t N, H, W, C, OH, OW, Cout, KH, KW, Cg, Coutg, nseg;
+  int32_t sh, sw, ph, pw, dh, dw;
+  uint32_t tiles_w, tiles_h, staged_ci, vec_x;   // forward: tile grid, halo channels per pixel (0 = not staged), 16-byte loads
+  float alpha;
+  uint32_t epi_act, epi_on, pad;
+};
+
 // ================================================================================================ reduce.cu
 struct ReduceParams {
   uint64_t in;        // input view, element (o, l, i) at in + (o * s_outer + l * s_len + inner_off(i)) elements

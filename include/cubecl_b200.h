@@ -383,6 +383,50 @@ int b200_conv2d_backward_weight(b200_ctx* ctx, b200_stream s, b200_dtype in_dtyp
                                 b200_dptr dw, const uint64_t* dw_shape, const uint64_t* dw_strides,
                                 const b200_conv2d_args* args);
 
+/* ---- grouped and depthwise 2-D convolution, forward and both gradients ------------------------------------------------
+ * As b200_conv2d / _backward_data / _backward_weight with `groups` > 1 groups: x is [N, H, W, C], w and dw are
+ * [Cout, KH, KW, Cg] with Cg = C / groups (PyTorch's grouped weight [Cout, C / groups, KH, KW] permuted as for b200_conv2d),
+ * out and dy are [N, OH, OW, Cout].  Group g owns input channels [g Cg, (g+1) Cg) and output channels [g Coutg, (g+1) Coutg),
+ * Coutg = Cout / groups; any channel multiplier Coutg / Cg is allowed (groups = C is depthwise).
+ *   out[n, oh, ow, co] = act(alpha * sum_{ky, kx, ci < Cg} x[n, oh*sh - ph + ky*dh, ow*sw - pw + kx*dw, g*Cg + ci] * w[co, ky, kx, ci]
+ *                            + bias[co]),  g = co / Coutg
+ * and the gradients of that sum (f32 accumulation, no epilogue; the bias gradient is b200_reduce over axis 0 of dy).  Input
+ * outside x reads as +0 and is multiplied like any other element (an inf weight gives NaN at a padded window).  A NaN or inf
+ * in group g's input or dy channels reaches only group g's outputs.  Dtypes, stride / padding / dilation limits, the
+ * output-shape rule, the out / dx / dw view rules and the zero-extent rules are those of the groups == 1 functions.
+ * Errors: B200_ERR_INVALID_ARG for groups == 0, C or Cout not divisible by groups, or a weight channel extent != C / groups,
+ * plus the groups == 1 functions' errors; B200_ERR_UNSUPPORTED for their limits.
+ * Routing (from the shape alone):
+ *   groups == 1: the groups == 1 function itself (same plan, same bits).
+ *   Cg >= 64: one groups == 1 call per group on channel slices (x, dy, out, dx in place through their pixel pitch; w and dw
+ *     as row blocks); a slice whose base is not 16-byte aligned takes that function's gather or padding copy.
+ *   Cg < 64: direct NHWC kernels on the CUDA cores, one launch each (+1 per x / dy / w view without a unit channel stride,
+ *     which is gathered first), in a fixed order of f32 FMAs, bitwise reproducible:
+ *     forward (conv2d_grp_*): acc = +0; for ky, kx, ci ascending: acc = fma(x, w, acc); then the epilogue.
+ *     backward_data (conv2d_grp_dgrad_*): acc = +0; for ky, kx ascending over the taps with (h + ph - ky*dh) % sh == 0 and
+ *       (w + pw - kx*dw) % sw == 0, then co in the group ascending: acc = fma(dy, w, acc); dy reads as +0 outside
+ *       [0, OH) x [0, OW).
+ *     backward_weight (conv2d_grp_wgrad_*): the P = N*OH*OW pixels are cut into segments of L pixels, with
+ *       E = Cout*KH*KW*Cg, S' = min(4096, max(1, ceil(2^18 / E))), L = max(64, ceil(P / S')), S = ceil(P / L) (1 when P = 0).
+ *       Per segment, acc = +0; for pixels ascending (n, oh, ow order): acc = fma(dy, x, acc).  S == 1 writes dw directly;
+ *       otherwise the f32 partials go to a pooled S * E * 4-byte buffer and conv2d_grp_wgrad_combine_* writes
+ *       dw = ((p_0 + p_1) + p_2) + ....  The dry-run plan records "conv grouped wgrad pixels= elements= segments= length=". */
+int b200_conv2d_grouped(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype,
+                        b200_dptr x, const uint64_t* x_shape, const uint64_t* x_strides,
+                        b200_dptr w, const uint64_t* w_shape, const uint64_t* w_strides,
+                        b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides,
+                        const b200_conv2d_args* args, uint32_t groups, const b200_epilogue* epilogue);
+int b200_conv2d_grouped_backward_data(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype,
+                                      b200_dptr dy, const uint64_t* dy_shape, const uint64_t* dy_strides,
+                                      b200_dptr w, const uint64_t* w_shape, const uint64_t* w_strides,
+                                      b200_dptr dx, const uint64_t* dx_shape, const uint64_t* dx_strides,
+                                      const b200_conv2d_args* args, uint32_t groups);
+int b200_conv2d_grouped_backward_weight(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype,
+                                        b200_dptr x, const uint64_t* x_shape, const uint64_t* x_strides,
+                                        b200_dptr dy, const uint64_t* dy_shape, const uint64_t* dy_strides,
+                                        b200_dptr dw, const uint64_t* dw_shape, const uint64_t* dw_strides,
+                                        const b200_conv2d_args* args, uint32_t groups);
+
 /* ---- collectives: ServerCommunication (server/base.rs:632-739), CUDA impl cubecl-cuda/src/compute/server.rs:666-926 -- */
 #define B200_UNIQUE_ID_BYTES 128
 int b200_comm_get_unique_id(b200_ctx* ctx, void* id128);            /* ncclGetUniqueId (communication.rs:11-25 holds it per device set) */

@@ -262,6 +262,47 @@ inline void backward_weight(ComputeClient& client, const TensorHandle& x, const 
                                              dy.strides.data(), dw.handle.ptr(), dw.shape.data(), dw.strides.data(), &args);
   if (rc != B200_OK) client.defer(b200_last_error());
 }
+
+/// Grouped / depthwise convolution: w [Cout, KH, KW, C / groups].  See b200_conv2d_grouped.  Errors are deferred to client.sync().
+inline void launch_grouped(ComputeClient& client, const TensorHandle& x, const TensorHandle& w, const TensorHandle& out,
+                           const b200_conv2d_args& args, uint32_t groups, const b200_epilogue* epilogue = nullptr) {
+  if (x.shape.size() != 4 || w.shape.size() != 4 || out.shape.size() != 4 || x.dtype != w.dtype) {
+    client.defer("InvalidArgument: conv2d_grouped needs rank-4 x, w and out, and x and w of one dtype");
+    return;
+  }
+  const int rc = b200_conv2d_grouped(client.raw(), nullptr, static_cast<b200_dtype>(x.dtype), static_cast<b200_dtype>(out.dtype),
+                                     x.handle.ptr(), x.shape.data(), x.strides.data(), w.handle.ptr(), w.shape.data(), w.strides.data(),
+                                     out.handle.ptr(), out.shape.data(), out.strides.data(), &args, groups, epilogue);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+
+/// Input gradient of launch_grouped.  See b200_conv2d_grouped_backward_data.  Errors are deferred to client.sync().
+inline void backward_data_grouped(ComputeClient& client, const TensorHandle& dy, const TensorHandle& w, const TensorHandle& dx,
+                                  const b200_conv2d_args& args, uint32_t groups) {
+  if (dy.shape.size() != 4 || w.shape.size() != 4 || dx.shape.size() != 4 || dy.dtype != w.dtype) {
+    client.defer("InvalidArgument: conv2d_grouped_backward_data needs rank-4 dy, w and dx, and dy and w of one dtype");
+    return;
+  }
+  const int rc = b200_conv2d_grouped_backward_data(client.raw(), nullptr, static_cast<b200_dtype>(dy.dtype),
+                                                   static_cast<b200_dtype>(dx.dtype), dy.handle.ptr(), dy.shape.data(),
+                                                   dy.strides.data(), w.handle.ptr(), w.shape.data(), w.strides.data(), dx.handle.ptr(),
+                                                   dx.shape.data(), dx.strides.data(), &args, groups);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+
+/// Weight gradient of launch_grouped: dw [Cout, KH, KW, C / groups].  See b200_conv2d_grouped_backward_weight.
+inline void backward_weight_grouped(ComputeClient& client, const TensorHandle& x, const TensorHandle& dy, const TensorHandle& dw,
+                                    const b200_conv2d_args& args, uint32_t groups) {
+  if (x.shape.size() != 4 || dy.shape.size() != 4 || dw.shape.size() != 4 || x.dtype != dy.dtype) {
+    client.defer("InvalidArgument: conv2d_grouped_backward_weight needs rank-4 x, dy and dw, and x and dy of one dtype");
+    return;
+  }
+  const int rc = b200_conv2d_grouped_backward_weight(client.raw(), nullptr, static_cast<b200_dtype>(x.dtype),
+                                                     static_cast<b200_dtype>(dw.dtype), x.handle.ptr(), x.shape.data(),
+                                                     x.strides.data(), dy.handle.ptr(), dy.shape.data(), dy.strides.data(),
+                                                     dw.handle.ptr(), dw.shape.data(), dw.strides.data(), &args, groups);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
 }  // namespace conv
 
 namespace reduce {

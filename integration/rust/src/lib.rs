@@ -421,6 +421,66 @@ impl Context {
         ))
     }
 
+    /// Grouped / depthwise [`Context::conv2d`]: w [Cout, KH, KW, C / groups].  See b200_conv2d_grouped in cubecl_b200.h.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::conv2d`].
+    pub unsafe fn conv2d_grouped(
+        &mut self, stream: b200_stream, in_dtype: DType, out_dtype: DType, x: &TensorView, w: &TensorView, out: &TensorView,
+        args: [i32; 6], groups: u32, epilogue: Option<&Epilogue>,
+    ) -> Result<(), Error> {
+        assert!(x.shape.len() == 4 && w.shape.len() == 4 && out.shape.len() == 4);
+        assert!(x.strides.len() == 4 && w.strides.len() == 4 && out.strides.len() == 4);
+        let a = sys::b200_conv2d_args {
+            stride_h: args[0], stride_w: args[1], pad_h: args[2], pad_w: args[3], dilation_h: args[4], dilation_w: args[5],
+        };
+        let e = epilogue.map(|e| sys::b200_epilogue { alpha: e.alpha, activation: e.activation as i32, bias: e.bias });
+        check(sys::b200_conv2d_grouped(
+            self.0, stream, in_dtype as c_int, out_dtype as c_int, x.ptr, x.shape.as_ptr(), x.strides.as_ptr(), w.ptr,
+            w.shape.as_ptr(), w.strides.as_ptr(), out.ptr, out.shape.as_ptr(), out.strides.as_ptr(), &a, groups,
+            e.as_ref().map_or(std::ptr::null(), |e| e as *const sys::b200_epilogue),
+        ))
+    }
+
+    /// Input gradient of [`Context::conv2d_grouped`].  See b200_conv2d_grouped_backward_data in cubecl_b200.h.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::matmul`] for the three pointers.
+    pub unsafe fn conv2d_grouped_backward_data(
+        &mut self, stream: b200_stream, in_dtype: DType, out_dtype: DType, dy: &TensorView, w: &TensorView, dx: &TensorView,
+        args: [i32; 6], groups: u32,
+    ) -> Result<(), Error> {
+        assert!(dy.shape.len() == 4 && w.shape.len() == 4 && dx.shape.len() == 4);
+        assert!(dy.strides.len() == 4 && w.strides.len() == 4 && dx.strides.len() == 4);
+        let a = sys::b200_conv2d_args {
+            stride_h: args[0], stride_w: args[1], pad_h: args[2], pad_w: args[3], dilation_h: args[4], dilation_w: args[5],
+        };
+        check(sys::b200_conv2d_grouped_backward_data(
+            self.0, stream, in_dtype as c_int, out_dtype as c_int, dy.ptr, dy.shape.as_ptr(), dy.strides.as_ptr(), w.ptr,
+            w.shape.as_ptr(), w.strides.as_ptr(), dx.ptr, dx.shape.as_ptr(), dx.strides.as_ptr(), &a, groups,
+        ))
+    }
+
+    /// Weight gradient of [`Context::conv2d_grouped`]: dw [Cout, KH, KW, C / groups].  See
+    /// b200_conv2d_grouped_backward_weight in cubecl_b200.h.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::matmul`] for the three pointers.
+    pub unsafe fn conv2d_grouped_backward_weight(
+        &mut self, stream: b200_stream, in_dtype: DType, out_dtype: DType, x: &TensorView, dy: &TensorView, dw: &TensorView,
+        args: [i32; 6], groups: u32,
+    ) -> Result<(), Error> {
+        assert!(x.shape.len() == 4 && dy.shape.len() == 4 && dw.shape.len() == 4);
+        assert!(x.strides.len() == 4 && dy.strides.len() == 4 && dw.strides.len() == 4);
+        let a = sys::b200_conv2d_args {
+            stride_h: args[0], stride_w: args[1], pad_h: args[2], pad_w: args[3], dilation_h: args[4], dilation_w: args[5],
+        };
+        check(sys::b200_conv2d_grouped_backward_weight(
+            self.0, stream, in_dtype as c_int, out_dtype as c_int, x.ptr, x.shape.as_ptr(), x.strides.as_ptr(), dy.ptr,
+            dy.shape.as_ptr(), dy.strides.as_ptr(), dw.ptr, dw.shape.as_ptr(), dw.strides.as_ptr(), &a, groups,
+        ))
+    }
+
     /// Block-scaled (MX / NVFP4) matmul: lhs [batch, m, k], rhs [batch, n, k] K-contiguous, scales per `scale_block`
     /// (32: ue8m0, 16: e4m3) elements of K; replaces `MmaDefinition::new_scaled` / `execute_scaled` tiles
     /// (crates/cubecl-core/src/frontend/cmma.rs:438-460, 798-840) at GEMM level.
