@@ -67,32 +67,17 @@ def launch(client: ComputeClient, x: TensorHandle, w: TensorHandle, out: TensorH
     epilogue: out = activation(alpha * conv + bias[co]) with `bias` an f32 [Cout] tensor.  groups > 1: a grouped convolution
     with w [Cout, KH, KW, C / groups].  Never raises for launch problems: errors are deferred to client.sync() / read_one()
     like matmul.launch."""
-    try:
+    def epilogue():
         if activation not in ACTIVATIONS:
             raise B200Error(6, f"unknown activation {activation!r}")
-        if len(x.shape) != 4 or len(w.shape) != 4 or len(out.shape) != 4:
-            raise B200Error(6, "conv2d: x, w and out must have rank 4")
-        if x.dtype != w.dtype:
-            raise B200Error(6, f"conv2d: x dtype {x.dtype} != w dtype {w.dtype}")
         if bias is not None and (bias.dtype != "f32" or not bias.is_contiguous() or bias.size() != w.shape[0]):
             raise B200Error(6, "conv2d: bias must be a contiguous f32 tensor with Cout elements")
-        (sh, sw), (ph, pw), (dh, dw) = _pair(stride, "stride"), _pair(padding, "padding"), _pair(dilation, "dilation")
-        for t in (x, w, out) + ((bias,) if bias is not None else ()):
-            t.handle.used_on(stream)
-        args = _ffi.Conv2dArgs(sh, sw, ph, pw, dh, dw)
-        ep = None
-        if alpha != 1.0 or bias is not None or activation not in (None, "none"):
-            ep = C.byref(_ffi.Epilogue(float(alpha), ACTIVATIONS[activation], bias.handle.ptr if bias is not None else 0))
-        operands = (client._ctx, stream, DTYPES[x.dtype], DTYPES[out.dtype],
-                    C.c_uint64(x.handle.ptr), _ffi.u64_array(x.shape), _ffi.u64_array(x.strides),
-                    C.c_uint64(w.handle.ptr), _ffi.u64_array(w.shape), _ffi.u64_array(w.strides),
-                    C.c_uint64(out.handle.ptr), _ffi.u64_array(out.shape), _ffi.u64_array(out.strides), C.byref(args))
-        if groups == 1:
-            _ffi.check(client._lib.b200_conv2d(*operands, ep))
-        else:
-            _ffi.check(client._lib.b200_conv2d_grouped(*operands, _groups(groups), ep))
-    except (B200Error, ValueError) as e:
-        client._defer(e if isinstance(e, B200Error) else B200Error(6, str(e)))
+        if alpha == 1.0 and bias is None and activation in (None, "none"):
+            return None, ()
+        ep = _ffi.Epilogue(float(alpha), ACTIVATIONS[activation], bias.handle.ptr if bias is not None else 0)
+        return C.byref(ep), (() if bias is None else (bias,))
+
+    _enqueue(client, "conv2d", x, w, out, stride, padding, dilation, stream, groups, epilogue)
 
 
 def launch_alloc(client: ComputeClient, x: TensorHandle, w: TensorHandle, out_dtype: str | None = None, **kwargs) -> TensorHandle:
@@ -111,33 +96,40 @@ def _groups(groups) -> C.c_uint32:
     return C.c_uint32(groups)
 
 
-def _check_grad_operands(what: str, a: TensorHandle, b: TensorHandle, out: TensorHandle) -> None:
-    if len(a.shape) != 4 or len(b.shape) != 4 or len(out.shape) != 4:
-        raise B200Error(6, f"{what}: every operand must have rank 4")
-    if a.dtype != b.dtype:
-        raise B200Error(6, f"{what}: operand dtypes differ ({a.dtype}, {b.dtype})")
+def _enqueue(client: ComputeClient, name: str, a: TensorHandle, b: TensorHandle, out: TensorHandle, stride, padding, dilation, stream,
+             groups, epilogue=None) -> None:
+    """The body of launch, backward_data and backward_weight: check the operands, mark them used on `stream` and call
+    b200_<name>(a, b, out, args[, epilogue]), or its grouped form when groups != 1.  epilogue (launch only) checks the
+    epilogue arguments and returns (the b200_epilogue pointer or None, the extra handles it reads).  Errors are deferred to
+    client.sync() / read_one()."""
+    try:
+        if len(a.shape) != 4 or len(b.shape) != 4 or len(out.shape) != 4:
+            raise B200Error(6, f"{name}: every operand must have rank 4")
+        if a.dtype != b.dtype:
+            raise B200Error(6, f"{name}: operand dtypes differ ({a.dtype}, {b.dtype})")
+        ep, extra = epilogue() if epilogue else (None, ())
+        (sh, sw), (ph, pw), (dh, dw) = _pair(stride, "stride"), _pair(padding, "padding"), _pair(dilation, "dilation")
+        for t in (a, b, out, *extra):
+            t.handle.used_on(stream)
+        args = _ffi.Conv2dArgs(sh, sw, ph, pw, dh, dw)
+        operands = (client._ctx, stream, DTYPES[a.dtype], DTYPES[out.dtype],
+                    C.c_uint64(a.handle.ptr), _ffi.u64_array(a.shape), _ffi.u64_array(a.strides),
+                    C.c_uint64(b.handle.ptr), _ffi.u64_array(b.shape), _ffi.u64_array(b.strides),
+                    C.c_uint64(out.handle.ptr), _ffi.u64_array(out.shape), _ffi.u64_array(out.strides), C.byref(args))
+        tail = (ep,) if epilogue else ()
+        if groups == 1:
+            _ffi.check(getattr(client._lib, "b200_" + name)(*operands, *tail))
+        else:
+            _ffi.check(getattr(client._lib, "b200_" + name.replace("conv2d", "conv2d_grouped", 1))(*operands, _groups(groups), *tail))
+    except (B200Error, ValueError) as e:
+        client._defer(e if isinstance(e, B200Error) else B200Error(6, str(e)))
 
 
 def backward_data(client: ComputeClient, dy: TensorHandle, w: TensorHandle, dx: TensorHandle, stride=1, padding=0, dilation=1,
                   stream=None, groups: int = 1) -> None:
     """Enqueue dx = the gradient of conv2d with respect to its input: dy [N, OH, OW, Cout], w [Cout, KH, KW, C / groups], dx
     [N, H, W, C] (NHWC), with dy's shape the output rule of (dx, w).  Errors are deferred like launch."""
-    try:
-        _check_grad_operands("conv2d_backward_data", dy, w, dx)
-        (sh, sw), (ph, pw), (dh, dw) = _pair(stride, "stride"), _pair(padding, "padding"), _pair(dilation, "dilation")
-        for t in (dy, w, dx):
-            t.handle.used_on(stream)
-        args = _ffi.Conv2dArgs(sh, sw, ph, pw, dh, dw)
-        operands = (client._ctx, stream, DTYPES[dy.dtype], DTYPES[dx.dtype],
-                    C.c_uint64(dy.handle.ptr), _ffi.u64_array(dy.shape), _ffi.u64_array(dy.strides),
-                    C.c_uint64(w.handle.ptr), _ffi.u64_array(w.shape), _ffi.u64_array(w.strides),
-                    C.c_uint64(dx.handle.ptr), _ffi.u64_array(dx.shape), _ffi.u64_array(dx.strides), C.byref(args))
-        if groups == 1:
-            _ffi.check(client._lib.b200_conv2d_backward_data(*operands))
-        else:
-            _ffi.check(client._lib.b200_conv2d_grouped_backward_data(*operands, _groups(groups)))
-    except (B200Error, ValueError) as e:
-        client._defer(e if isinstance(e, B200Error) else B200Error(6, str(e)))
+    _enqueue(client, "conv2d_backward_data", dy, w, dx, stride, padding, dilation, stream, groups)
 
 
 def backward_data_alloc(client: ComputeClient, dy: TensorHandle, w: TensorHandle, input_hw, out_dtype: str | None = None,
@@ -155,22 +147,7 @@ def backward_weight(client: ComputeClient, x: TensorHandle, dy: TensorHandle, dw
                     stream=None, groups: int = 1) -> None:
     """Enqueue dw = the gradient of conv2d with respect to its weights: x [N, H, W, C], dy [N, OH, OW, Cout], dw
     [Cout, KH, KW, C / groups], with dy's shape the output rule of (x, dw).  Errors are deferred like launch."""
-    try:
-        _check_grad_operands("conv2d_backward_weight", x, dy, dw)
-        (sh, sw), (ph, pw), (dh, dw_) = _pair(stride, "stride"), _pair(padding, "padding"), _pair(dilation, "dilation")
-        for t in (x, dy, dw):
-            t.handle.used_on(stream)
-        args = _ffi.Conv2dArgs(sh, sw, ph, pw, dh, dw_)
-        operands = (client._ctx, stream, DTYPES[x.dtype], DTYPES[dw.dtype],
-                    C.c_uint64(x.handle.ptr), _ffi.u64_array(x.shape), _ffi.u64_array(x.strides),
-                    C.c_uint64(dy.handle.ptr), _ffi.u64_array(dy.shape), _ffi.u64_array(dy.strides),
-                    C.c_uint64(dw.handle.ptr), _ffi.u64_array(dw.shape), _ffi.u64_array(dw.strides), C.byref(args))
-        if groups == 1:
-            _ffi.check(client._lib.b200_conv2d_backward_weight(*operands))
-        else:
-            _ffi.check(client._lib.b200_conv2d_grouped_backward_weight(*operands, _groups(groups)))
-    except (B200Error, ValueError) as e:
-        client._defer(e if isinstance(e, B200Error) else B200Error(6, str(e)))
+    _enqueue(client, "conv2d_backward_weight", x, dy, dw, stride, padding, dilation, stream, groups)
 
 
 def backward_weight_alloc(client: ComputeClient, x: TensorHandle, dy: TensorHandle, kernel_hw, out_dtype: str | None = None,

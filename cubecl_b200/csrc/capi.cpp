@@ -2596,6 +2596,97 @@ static void conv_norm_strides(const uint64_t* shape, const uint64_t* strides, ui
   }
 }
 
+// A stride of `e` 16-bit elements that a tensor map can take: a 16-byte multiple below 2^40 bytes.
+static bool conv_al16(uint64_t e) { return e % 8 == 0 && e * 2 < (1ull << 40); }
+
+// Two adjacent dimensions [outer, inner] of a view as one strided dimension: its stride, or 0 when they do not flatten.
+static uint64_t conv_flat_stride(uint64_t outer, uint64_t inner, uint64_t s_outer, uint64_t s_inner) {
+  return inner == 1 ? s_outer : (outer == 1 || s_outer == inner * s_inner) ? s_inner : 0;
+}
+
+// Checks every convolution entry point shares; what: the entry point, for messages.  The dtypes, the epilogue's activation,
+// the args, and the weights' channels w_c against the input channels of one group, in_c.
+static int conv_check_args(const char* what, b200_dtype in_dtype, b200_dtype out_dtype, const b200_conv2d_args& a, const b200_epilogue* ep,
+                           uint64_t in_c, uint64_t w_c) {
+  if (in_dtype != B200_F16 && in_dtype != B200_BF16)
+    return fail(B200_ERR_UNSUPPORTED, "%s: input dtype %d unsupported (f16, bf16)", what, (int)in_dtype);
+  if (out_dtype != in_dtype && out_dtype != B200_F32)
+    return fail(B200_ERR_UNSUPPORTED, "%s: output dtype must equal the input dtype or be f32", what);
+  if (ep && (ep->activation < 0 || ep->activation > 2)) return fail(B200_ERR_INVALID_ARG, "%s: unknown activation %d", what, ep->activation);
+  if (a.stride_h < 1 || a.stride_w < 1 || a.dilation_h < 1 || a.dilation_w < 1 || a.pad_h < 0 || a.pad_w < 0)
+    return fail(B200_ERR_INVALID_ARG, "%s: strides and dilations must be >= 1 and padding >= 0", what);
+  if (w_c != in_c)
+    return fail(B200_ERR_INVALID_ARG, "%s: weights have %llu channels, the input has %llu", what, (unsigned long long)w_c, (unsigned long long)in_c);
+  return B200_OK;
+}
+
+// Extents < 2^31, then PyTorch's output rule for the input [N, H, W, C] and weights [Cout, KH, KW, *]: y (the forward's out
+// or a gradient's dy, y_name in messages) must be [N, OH, OW, Cout].  An empty kernel has no output extent to check.
+static int conv_check_shape(const char* what, const b200_conv2d_args& a, const uint64_t* in, const uint64_t* w, const uint64_t* y,
+                            const char* y_name, uint64_t* OH, uint64_t* OW) {
+  const uint64_t lim = 1ull << 31;
+  for (int d = 0; d < 4; ++d)
+    if (in[d] >= lim || w[d] >= lim || y[d] >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: extents must be < 2^31", what);
+  const int64_t KH = (int64_t)w[1], KW = (int64_t)w[2];
+  if (KH == 0 || KW == 0) return B200_OK;
+  const int64_t nh = (int64_t)in[1] + 2 * (int64_t)a.pad_h - (int64_t)a.dilation_h * (KH - 1) - 1;
+  const int64_t nw = (int64_t)in[2] + 2 * (int64_t)a.pad_w - (int64_t)a.dilation_w * (KW - 1) - 1;
+  if (nh < 0 || nw < 0)
+    return fail(B200_ERR_INVALID_ARG, "%s: the dilated kernel is larger than the padded input (output extent < 1)", what);
+  *OH = (uint64_t)(nh / a.stride_h) + 1;
+  *OW = (uint64_t)(nw / a.stride_w) + 1;
+  if (y[0] != in[0] || y[1] != *OH || y[2] != *OW || y[3] != w[0])
+    return fail(B200_ERR_INVALID_ARG, "%s: %s is [%llu,%llu,%llu,%llu], expected [%llu,%llu,%llu,%llu]", what, y_name, (unsigned long long)y[0],
+                (unsigned long long)y[1], (unsigned long long)y[2], (unsigned long long)y[3], (unsigned long long)in[0],
+                (unsigned long long)*OH, (unsigned long long)*OW, (unsigned long long)w[0]);
+  return B200_OK;
+}
+
+// The 4-D im2col limits of the tensor map (cuda.h: cuTensorMapEncodeIm2col): pixel-box corners in [-128, 127] ...
+static int conv_check_corners(const char* what, const int64_t corners[4]) {
+  for (int i = 0; i < 4; ++i)
+    if (corners[i] < -128 || corners[i] > 127)
+      return fail(B200_ERR_UNSUPPORTED, "%s: im2col pixel-box corner %lld outside [-128, 127]", what, (long long)corners[i]);
+  return B200_OK;
+}
+
+// ... with the forward's corners -pad and pad - dilation * (kernel - 1) ...
+static int conv_check_fwd_corners(const char* what, const b200_conv2d_args& a, uint64_t KH, uint64_t KW) {
+  const int64_t corners[4] = {-(int64_t)a.pad_h, -(int64_t)a.pad_w, (int64_t)a.pad_h - (int64_t)a.dilation_h * ((int64_t)KH - 1),
+                              (int64_t)a.pad_w - (int64_t)a.dilation_w * ((int64_t)KW - 1)};
+  return conv_check_corners(what, corners);
+}
+
+// ... and an element stride (the conv stride) <= 8, which also bounds the data gradient's phases per dimension.
+static int conv_check_stride(const char* what, const b200_conv2d_args& a) {
+  if (a.stride_h > kDgradMaxStride || a.stride_w > kDgradMaxStride)
+    return fail(B200_ERR_UNSUPPORTED, "%s: the conv stride must be <= %d", what, kDgradMaxStride);
+  return B200_OK;
+}
+
+// Device pointers present, and the output's (out_name in messages) aligned to its element size.
+static int conv_check_ptrs(const char* what, uint64_t a, uint64_t b, uint64_t out, const char* out_name, b200_dtype out_dtype) {
+  if (!a || !b || !out) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
+  if (out % dtype_size(out_dtype)) return fail(B200_ERR_INVALID_ARG, "%s: %s pointer is not aligned to its element size", what, out_name);
+  return B200_OK;
+}
+
+// An NHWC output (out or dx; normalised strides ns): unit channel stride, and one pixel pitch >= its channels for N, H, W.
+static int conv_check_pixels(const char* what, const char* name, const uint64_t* shape, const uint64_t* ns) {
+  if (ns[3] != 1 || ns[2] < shape[3] || ns[1] != shape[2] * ns[2] || ns[0] != shape[1] * ns[1])
+    return fail(B200_ERR_UNSUPPORTED, "%s: %s must have unit channel stride and one pixel pitch >= its channels for N, H, W", what, name);
+  return B200_OK;
+}
+
+// dw [Cout, KH, KW, C'] (normalised strides ds): unit channel stride, (KH, KW) flattening into one kernel-position stride
+// (*dw_sp), and an output-channel stride.
+static int conv_check_dw(const char* what, const uint64_t* shape, const uint64_t* ds, size_t osz, uint64_t* dw_sp) {
+  *dw_sp = conv_flat_stride(shape[1], shape[2], ds[1], ds[2]);
+  if (ds[3] != 1 || *dw_sp == 0 || ds[0] * osz >= (1ull << 40) || *dw_sp * osz >= (1ull << 40))
+    return fail(B200_ERR_UNSUPPORTED, "%s: dw must have unit channel stride and (KH, KW) flattening into one stride", what);
+  return B200_OK;
+}
+
 // Pooled copy of an operand seen as [batch, rows, C] (strides in elements) with C padded to `cp` zero channels (repitch_rows
 // writes the padding columns as zeros).
 static int conv_pad_channels(b200_ctx* c, CUstream st, uint64_t in, uint64_t batch, uint64_t rows, uint64_t C, uint64_t s_b,
@@ -2628,115 +2719,95 @@ static int conv_gather(b200_ctx* c, CUstream st, b200_dtype dt, uint64_t in, con
   return B200_OK;
 }
 
+// An operand [N, H, W, C] (normalised strides `ns`) as the convolution maps read it: unit channel stride, 16-byte aligned base
+// and strides, channels a multiple of 8.  A view that does not qualify is gathered into a compact pooled copy; channel counts
+// that are not multiples of 8 are copied with the channels padded to 8 zeros.  flat: the leading dimensions the map reads
+// as one strided dimension -- none (x, and dy in the data gradient), (H, W) (the forward's weights: one kernel-position
+// dimension, returned as s_w) or (N, H, W) (dy in the weight gradient: [pixels, Cout]).  tmp[0] / tmp[1] receive the pooled
+// copies (the caller frees them).
+struct NhwcOperand {
+  uint64_t ptr, C, s_w, s_h, s_n;
+};
+enum ConvFlat { kFlatNone, kFlatHW, kFlatNHW };
+static int conv_prep_nhwc(b200_ctx* c, CUstream st, b200_dtype dt, uint64_t ptr, const uint64_t* shape, const uint64_t* ns, ConvFlat flat,
+                          CUdeviceptr tmp[2], NhwcOperand* o) {
+  const uint64_t N = shape[0], H = shape[1], W = shape[2], C = shape[3];
+  const uint64_t spx = conv_flat_stride(H, W, ns[1], ns[2]);   // (H, W) as one pixel dimension
+  int rc = B200_OK;
+  if (C % 8 == 0) {
+    bool in_place = ptr % 16 == 0 && ns[3] == 1 && conv_al16(ns[0]);
+    if (flat == kFlatHW) in_place = in_place && spx != 0 && conv_al16(spx);
+    else in_place = in_place && conv_al16(ns[1]) && conv_al16(ns[2]) && (flat == kFlatNone || (ns[1] == W * ns[2] && ns[0] == H * ns[1]));
+    if (in_place) {
+      *o = {ptr, C, flat == kFlatHW ? spx : ns[2], ns[1], ns[0]};
+      return B200_OK;
+    }
+    rc = conv_gather(c, st, dt, ptr, shape, ns, &tmp[0]);
+    *o = {tmp[0], C, C, W * C, H * W * C};
+    return rc;
+  }
+  const uint64_t cp = (C + 7) / 8 * 8;
+  uint64_t in = ptr, sb = ns[0], sp = spx, sc = ns[3];
+  if (spx == 0) {
+    rc = conv_gather(c, st, dt, ptr, shape, ns, &tmp[0]);
+    in = tmp[0]; sb = H * W * C; sp = C; sc = 1;
+  }
+  if (!rc) rc = conv_pad_channels(c, st, in, N, H * W, C, sb, sp, sc, cp, &tmp[1]);
+  *o = {tmp[1], cp, cp, W * cp, H * W * cp};
+  return rc;
+}
+
+// The implicit GEMM of a convolution map: M pixel rows of A and N rows of B, each K elements with unit k stride (the weight
+// gradient, which reads both MN-major, sets its own operand strides); out rows o_sm apart with unit column stride.
+static GemmProblem conv_problem(b200_dtype in_dtype, b200_dtype out_dtype, uint64_t a, uint64_t b, uint64_t out, uint64_t M, uint64_t N,
+                                uint64_t K, uint64_t o_sm, ConvGeom* g) {
+  GemmProblem gp{};
+  gp.in_dtype = in_dtype; gp.out_dtype = out_dtype;
+  gp.a = a; gp.b = b; gp.out = out;
+  gp.M = M; gp.N = N; gp.K = K; gp.batch = 1;
+  gp.a_sm = K; gp.a_sk = 1; gp.b_sn = K; gp.b_sk = 1;
+  gp.o_sm = o_sm; gp.o_sn = 1; gp.o_sb = 0;
+  gp.conv = g;
+  return gp;
+}
+
 extern "C" int b200_conv2d(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr x, const uint64_t* x_shape,
                            const uint64_t* x_strides, b200_dptr w, const uint64_t* w_shape, const uint64_t* w_strides, b200_dptr out,
                            const uint64_t* out_shape, const uint64_t* out_strides, const b200_conv2d_args* args, const b200_epilogue* ep) {
   CTX_ENTER(c);
-  if (!x_shape || !w_shape || !out_shape || !args) return fail(B200_ERR_INVALID_ARG, "conv2d: null shape or args");
-  if (in_dtype != B200_F16 && in_dtype != B200_BF16)
-    return fail(B200_ERR_UNSUPPORTED, "conv2d: input dtype %d unsupported (f16, bf16)", (int)in_dtype);
-  if (out_dtype != in_dtype && out_dtype != B200_F32)
-    return fail(B200_ERR_UNSUPPORTED, "conv2d: output dtype must equal the input dtype or be f32");
-  if (ep && (ep->activation < 0 || ep->activation > 2)) return fail(B200_ERR_INVALID_ARG, "conv2d: unknown activation %d", ep->activation);
+  const char* what = "conv2d";
+  if (!x_shape || !w_shape || !out_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
   const b200_conv2d_args& a = *args;
-  if (a.stride_h < 1 || a.stride_w < 1 || a.dilation_h < 1 || a.dilation_w < 1 || a.pad_h < 0 || a.pad_w < 0)
-    return fail(B200_ERR_INVALID_ARG, "conv2d: strides and dilations must be >= 1 and padding >= 0");
   const uint64_t N = x_shape[0], H = x_shape[1], W = x_shape[2], C = x_shape[3];
   const uint64_t Cout = w_shape[0], KH = w_shape[1], KW = w_shape[2];
-  if (w_shape[3] != C)
-    return fail(B200_ERR_INVALID_ARG, "conv2d: weights have %llu channels, x has %llu", (unsigned long long)w_shape[3], (unsigned long long)C);
+  int rc = conv_check_args(what, in_dtype, out_dtype, a, ep, C, w_shape[3]);
+  if (rc) return rc;
   if (N == 0 || H == 0 || W == 0 || C == 0 || Cout == 0 || KH == 0 || KW == 0) return B200_OK;
-  const uint64_t lim = 1ull << 31;
-  if (N >= lim || H >= lim || W >= lim || C >= lim || Cout >= lim || KH >= lim || KW >= lim)
-    return fail(B200_ERR_UNSUPPORTED, "conv2d: extents must be < 2^31");
-  // PyTorch's output rule
-  const int64_t nh = (int64_t)H + 2 * (int64_t)a.pad_h - (int64_t)a.dilation_h * ((int64_t)KH - 1) - 1;
-  const int64_t nw = (int64_t)W + 2 * (int64_t)a.pad_w - (int64_t)a.dilation_w * ((int64_t)KW - 1) - 1;
-  if (nh < 0 || nw < 0) return fail(B200_ERR_INVALID_ARG, "conv2d: the dilated kernel is larger than the padded input (output extent < 1)");
-  const uint64_t OH = (uint64_t)(nh / a.stride_h) + 1, OW = (uint64_t)(nw / a.stride_w) + 1;
-  if (out_shape[0] != N || out_shape[1] != OH || out_shape[2] != OW || out_shape[3] != Cout)
-    return fail(B200_ERR_INVALID_ARG, "conv2d: out is [%llu,%llu,%llu,%llu], expected [%llu,%llu,%llu,%llu]", (unsigned long long)out_shape[0],
-                (unsigned long long)out_shape[1], (unsigned long long)out_shape[2], (unsigned long long)out_shape[3], (unsigned long long)N,
-                (unsigned long long)OH, (unsigned long long)OW, (unsigned long long)Cout);
-  // the 4-D im2col limits of the tensor map (cuda.h: cuTensorMapEncodeIm2col)
-  const int64_t corners[4] = {-(int64_t)a.pad_h, -(int64_t)a.pad_w, (int64_t)a.pad_h - (int64_t)a.dilation_h * ((int64_t)KH - 1),
-                              (int64_t)a.pad_w - (int64_t)a.dilation_w * ((int64_t)KW - 1)};
-  for (int64_t k : corners)
-    if (k < -128 || k > 127)
-      return fail(B200_ERR_UNSUPPORTED, "conv2d: im2col pixel-box corner %lld outside [-128, 127] (-pad and pad - dilation * (kernel - 1))", (long long)k);
-  if (a.stride_h > 8 || a.stride_w > 8) return fail(B200_ERR_UNSUPPORTED, "conv2d: im2col element stride (the conv stride) must be <= 8");
-  const uint64_t M = N * OH * OW;
-  if (M >= lim) return fail(B200_ERR_UNSUPPORTED, "conv2d: N * OH * OW = %llu must be < 2^31", (unsigned long long)M);
-  if (!x || !w || !out) return fail(B200_ERR_INVALID_ARG, "conv2d: null device pointer");
-  const size_t osz = dtype_size(out_dtype);
-  if (out % osz) return fail(B200_ERR_INVALID_ARG, "conv2d: output pointer is not aligned to its element size");
-  // out: unit channel stride, the three outer strides one pixel pitch >= Cout
-  uint64_t os[4];
+  uint64_t OH = 0, OW = 0;
+  if ((rc = conv_check_shape(what, a, x_shape, w_shape, out_shape, "out", &OH, &OW))) return rc;
+  if ((rc = conv_check_fwd_corners(what, a, KH, KW)) || (rc = conv_check_stride(what, a))) return rc;
+  const uint64_t M = N * OH * OW, lim = 1ull << 31;
+  if (M >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * OH * OW = %llu must be < 2^31", what, (unsigned long long)M);
+  if ((rc = conv_check_ptrs(what, x, w, out, "output", out_dtype))) return rc;
+  uint64_t os[4], xs[4], ws[4];
   conv_norm_strides(out_shape, out_strides, os);
-  if (os[3] != 1 || os[2] < Cout || os[1] != OW * os[2] || os[0] != OH * os[1])
-    return fail(B200_ERR_UNSUPPORTED, "conv2d: out must have unit channel stride and one pixel pitch >= Cout for N, OH, OW");
-  if (KH * KW * ((C + 63) / 64 * 64) >= lim) return fail(B200_ERR_UNSUPPORTED, "conv2d: KH * KW * C (C padded to 64) must be < 2^31");
+  if ((rc = conv_check_pixels(what, "out", out_shape, os))) return rc;
+  if (KH * KW * ((C + 63) / 64 * 64) >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: KH * KW * C (C padded to 64) must be < 2^31", what);
   CUstream st = resolve_stream(c, s);
-  uint64_t xs[4], ws[4];
   conv_norm_strides(x_shape, x_strides, xs);
   conv_norm_strides(w_shape, w_strides, ws);
-  // (KH, KW) as one kernel-position dimension: stride, or 0 when the view cannot be flattened
-  const uint64_t w_sp = (KW == 1) ? ws[1] : (KH == 1 || ws[1] == KW * ws[2]) ? ws[2] : 0;
-  const uint64_t x_spx = (W == 1) ? xs[1] : (H == 1 || xs[1] == W * xs[2]) ? xs[2] : 0;   // (H, W) as one pixel dimension
-  auto al = [](uint64_t e) { return e % 8 == 0 && e * 2 < (1ull << 40); };   // 16-byte multiple (16-bit elements)
-  ConvGeom g{};
-  g.N = N; g.H = H; g.W = W; g.KH = KH; g.KW = KW; g.OH = OH; g.OW = OW; g.Cout = Cout;
-  g.sh = a.stride_h; g.sw = a.stride_w; g.ph = a.pad_h; g.pw = a.pad_w; g.dh = a.dilation_h; g.dw = a.dilation_w;
   CUdeviceptr tmp[4] = {0, 0, 0, 0};
-  uint64_t xa = x, wa = w;
-  int rc = B200_OK;
-  if (C % 8 == 0) {
-    g.C = C;
-    if (x % 16 == 0 && xs[3] == 1 && al(xs[0]) && al(xs[1]) && al(xs[2])) {
-      g.x_sw = xs[2]; g.x_sh = xs[1]; g.x_sn = xs[0];
-    } else {
-      rc = conv_gather(c, st, in_dtype, x, x_shape, xs, &tmp[0]);
-      xa = tmp[0];
-      g.x_sw = C; g.x_sh = W * C; g.x_sn = H * W * C;
-    }
-    if (!rc && w % 16 == 0 && ws[3] == 1 && w_sp != 0 && al(w_sp) && al(ws[0])) {
-      g.w_sp = w_sp; g.w_sco = ws[0];
-    } else if (!rc) {
-      rc = conv_gather(c, st, in_dtype, w, w_shape, ws, &tmp[1]);
-      wa = tmp[1];
-      g.w_sp = C; g.w_sco = KH * KW * C;
-    }
-  } else {
-    // rows of C * 2 bytes are not 16-byte multiples: TMA cannot describe them.  Both operands are copied with C padded to a
-    // multiple of 8 zero channels (first gathered when their spatial dimensions do not flatten into one strided dimension)
-    const uint64_t cp = (C + 7) / 8 * 8;
-    g.C = cp;
-    uint64_t xin = x, xsb = xs[0], xsp = x_spx, xsc = xs[3];
-    if (x_spx == 0) {
-      rc = conv_gather(c, st, in_dtype, x, x_shape, xs, &tmp[0]);
-      xin = tmp[0]; xsb = H * W * C; xsp = C; xsc = 1;
-    }
-    if (!rc) rc = conv_pad_channels(c, st, xin, N, H * W, C, xsb, xsp, xsc, cp, &tmp[2]);
-    xa = tmp[2];
-    g.x_sw = cp; g.x_sh = W * cp; g.x_sn = H * W * cp;
-    uint64_t win = w, wsb = ws[0], wsp = w_sp, wsc = ws[3];
-    if (!rc && w_sp == 0) {
-      rc = conv_gather(c, st, in_dtype, w, w_shape, ws, &tmp[1]);
-      win = tmp[1]; wsb = KH * KW * C; wsp = C; wsc = 1;
-    }
-    if (!rc) rc = conv_pad_channels(c, st, win, Cout, KH * KW, C, wsb, wsp, wsc, cp, &tmp[3]);
-    wa = tmp[3];
-    g.w_sp = cp; g.w_sco = KH * KW * cp;
-  }
+  NhwcOperand xo{}, wo{};
+  rc = conv_prep_nhwc(c, st, in_dtype, x, x_shape, xs, kFlatNone, &tmp[0], &xo);
+  if (!rc) rc = conv_prep_nhwc(c, st, in_dtype, w, w_shape, ws, kFlatHW, &tmp[2], &wo);
   if (!rc) {
-    GemmProblem gp{};
-    gp.in_dtype = in_dtype; gp.out_dtype = out_dtype;
-    gp.a = xa; gp.b = wa; gp.out = out;
-    gp.M = M; gp.N = Cout; gp.K = KH * KW * ((g.C + 63) / 64 * 64); gp.batch = 1;
-    gp.a_sm = gp.K; gp.a_sk = 1; gp.b_sn = gp.K; gp.b_sk = 1;
-    gp.o_sm = os[2]; gp.o_sn = 1; gp.o_sb = 0;
+    ConvGeom g{};
+    g.N = N; g.H = H; g.W = W; g.C = xo.C; g.KH = KH; g.KW = KW; g.OH = OH; g.OW = OW; g.Cout = Cout;
+    g.sh = a.stride_h; g.sw = a.stride_w; g.ph = a.pad_h; g.pw = a.pad_w; g.dh = a.dilation_h; g.dw = a.dilation_w;
+    g.x_sw = xo.s_w; g.x_sh = xo.s_h; g.x_sn = xo.s_n;
+    g.w_sp = wo.s_w; g.w_sco = wo.s_n;
+    GemmProblem gp = conv_problem(in_dtype, out_dtype, xo.ptr, wo.ptr, out, M, Cout, KH * KW * ((g.C + 63) / 64 * 64), os[2], &g);
     if (ep) { gp.alpha = ep->alpha; gp.bias = ep->bias; gp.act = (uint32_t)ep->activation; }
-    gp.conv = &g;
     rc = launch_wgmma(c, st, gp, false, false);
   }
   for (CUdeviceptr t : tmp)
@@ -2755,74 +2826,6 @@ static int memset2d_zero(b200_ctx* c, CUstream st, CUdeviceptr dst, size_t esz, 
   }
   if (esz == 4) CU_CHECK(g_drv.cuMemsetD2D32Async_p(dst, pitch * 4, 0u, cols, rows, st));
   else CU_CHECK(g_drv.cuMemsetD2D16Async_p(dst, pitch * 2, 0, cols, rows, st));
-  return B200_OK;
-}
-
-// An NHWC operand [N, H, W, C] (normalised strides `ns`) as the convolution maps read it: unit channel stride, 16-byte
-// aligned base and pixel / row / image strides, channels a multiple of 8 -- the forward's rules.  A view that does not
-// qualify is gathered into a compact pooled copy; channel counts that are not multiples of 8 are copied with the channels
-// padded to 8 zeros.  one_pitch: the pixels must also form one strided dimension (the weight gradient reads dy as
-// [pixels, Cout]).  tmp[0] / tmp[1] receive the pooled copies (the caller frees them).
-struct NhwcOperand {
-  uint64_t ptr, C, s_w, s_h, s_n;
-};
-static int conv_prep_nhwc(b200_ctx* c, CUstream st, b200_dtype dt, uint64_t ptr, const uint64_t* shape, const uint64_t* ns, bool one_pitch,
-                          CUdeviceptr tmp[2], NhwcOperand* o) {
-  const uint64_t N = shape[0], H = shape[1], W = shape[2], C = shape[3];
-  auto al = [](uint64_t e) { return e % 8 == 0 && e * 2 < (1ull << 40); };   // 16-byte multiple (16-bit elements)
-  const bool pitch_ok = !one_pitch || (ns[1] == W * ns[2] && ns[0] == H * ns[1]);
-  int rc = B200_OK;
-  if (C % 8 == 0) {
-    if (ptr % 16 == 0 && ns[3] == 1 && al(ns[0]) && al(ns[1]) && al(ns[2]) && pitch_ok) {
-      *o = {ptr, C, ns[2], ns[1], ns[0]};
-      return B200_OK;
-    }
-    rc = conv_gather(c, st, dt, ptr, shape, ns, &tmp[0]);
-    *o = {tmp[0], C, C, W * C, H * W * C};
-    return rc;
-  }
-  const uint64_t cp = (C + 7) / 8 * 8;
-  const uint64_t spx = (W == 1) ? ns[1] : (H == 1 || ns[1] == W * ns[2]) ? ns[2] : 0;   // (H, W) as one pixel dimension
-  uint64_t in = ptr, sb = ns[0], sp = spx, sc = ns[3];
-  if (spx == 0) {
-    rc = conv_gather(c, st, dt, ptr, shape, ns, &tmp[0]);
-    in = tmp[0]; sb = H * W * C; sp = C; sc = 1;
-  }
-  if (!rc) rc = conv_pad_channels(c, st, in, N, H * W, C, sb, sp, sc, cp, &tmp[1]);
-  *o = {tmp[1], cp, cp, W * cp, H * W * cp};
-  return rc;
-}
-
-// Shared argument checks of the two gradients: dtypes, args, and dy's shape against the forward's output rule for the
-// input [N, H, W, C] and weights [Cout, KH, KW, C].  what: the entry point, for messages.
-static int conv_bwd_check(const char* what, b200_dtype in_dtype, b200_dtype out_dtype, const b200_conv2d_args& a, const uint64_t* in_shape,
-                          const uint64_t* w_shape, const uint64_t* dy_shape, uint64_t* OH, uint64_t* OW) {
-  if (in_dtype != B200_F16 && in_dtype != B200_BF16)
-    return fail(B200_ERR_UNSUPPORTED, "%s: input dtype %d unsupported (f16, bf16)", what, (int)in_dtype);
-  if (out_dtype != in_dtype && out_dtype != B200_F32)
-    return fail(B200_ERR_UNSUPPORTED, "%s: output dtype must equal the input dtype or be f32", what);
-  if (a.stride_h < 1 || a.stride_w < 1 || a.dilation_h < 1 || a.dilation_w < 1 || a.pad_h < 0 || a.pad_w < 0)
-    return fail(B200_ERR_INVALID_ARG, "%s: strides and dilations must be >= 1 and padding >= 0", what);
-  if (w_shape[3] != in_shape[3])
-    return fail(B200_ERR_INVALID_ARG, "%s: weights have %llu channels, the input has %llu", what, (unsigned long long)w_shape[3],
-                (unsigned long long)in_shape[3]);
-  const uint64_t lim = 1ull << 31;
-  for (int d = 0; d < 4; ++d)
-    if (in_shape[d] >= lim || w_shape[d] >= lim || dy_shape[d] >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: extents must be < 2^31", what);
-  const int64_t KH = (int64_t)w_shape[1], KW = (int64_t)w_shape[2];
-  if (KH == 0 || KW == 0) return B200_OK;   // an empty kernel: no output rule to check (the gradients are zero or empty)
-  const int64_t nh = (int64_t)in_shape[1] + 2 * (int64_t)a.pad_h - (int64_t)a.dilation_h * (KH - 1) - 1;
-  const int64_t nw = (int64_t)in_shape[2] + 2 * (int64_t)a.pad_w - (int64_t)a.dilation_w * (KW - 1) - 1;
-  if (nh < 0 || nw < 0)
-    return fail(B200_ERR_INVALID_ARG, "%s: the dilated kernel is larger than the padded input (output extent < 1)", what);
-  *OH = (uint64_t)(nh / a.stride_h) + 1;
-  *OW = (uint64_t)(nw / a.stride_w) + 1;
-  if (dy_shape[0] != in_shape[0] || dy_shape[1] != *OH || dy_shape[2] != *OW || dy_shape[3] != w_shape[0])
-    return fail(B200_ERR_INVALID_ARG, "%s: dy is [%llu,%llu,%llu,%llu], expected [%llu,%llu,%llu,%llu]", what, (unsigned long long)dy_shape[0],
-                (unsigned long long)dy_shape[1], (unsigned long long)dy_shape[2], (unsigned long long)dy_shape[3],
-                (unsigned long long)in_shape[0], (unsigned long long)*OH, (unsigned long long)*OW, (unsigned long long)w_shape[0]);
-  if (a.stride_h > kDgradMaxStride || a.stride_w > kDgradMaxStride)
-    return fail(B200_ERR_UNSUPPORTED, "%s: the conv stride must be <= %d", what, kDgradMaxStride);
   return B200_OK;
 }
 
@@ -2860,11 +2863,13 @@ extern "C" int b200_conv2d_backward_data(b200_ctx* c, b200_stream s, b200_dtype 
   const char* what = "conv2d_backward_data";
   if (!dy_shape || !w_shape || !dx_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
   const b200_conv2d_args& a = *args;
-  uint64_t OH = 0, OW = 0;
-  int rc = conv_bwd_check(what, in_dtype, out_dtype, a, dx_shape, w_shape, dy_shape, &OH, &OW);
-  if (rc) return rc;
   const uint64_t N = dx_shape[0], H = dx_shape[1], W = dx_shape[2], C = dx_shape[3];
   const uint64_t Cout = w_shape[0], KH = w_shape[1], KW = w_shape[2];
+  uint64_t OH = 0, OW = 0;
+  int rc = conv_check_args(what, in_dtype, out_dtype, a, nullptr, C, w_shape[3]);
+  if (!rc) rc = conv_check_shape(what, a, dx_shape, w_shape, dy_shape, "dy", &OH, &OW);
+  if (!rc && KH && KW) rc = conv_check_stride(what, a);
+  if (rc) return rc;
   if (N == 0 || H == 0 || W == 0 || C == 0) return B200_OK;   // no dx
   const uint64_t lim = 1ull << 31;
   if (N * H * W >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * H * W = %llu must be < 2^31", what, (unsigned long long)(N * H * W));
@@ -2879,17 +2884,13 @@ extern "C" int b200_conv2d_backward_data(b200_ctx* c, b200_stream s, b200_dtype 
       if (!ph.extent || !pw.extent) continue;
       if (!ph.taps || !pw.taps || Cout == 0) { zero_phase = true; continue; }
       const int64_t corners[4] = {ph.e0, pw.e0, ph.e0 + (int64_t)ph.extent - (int64_t)OH, pw.e0 + (int64_t)pw.extent - (int64_t)OW};
-      for (int64_t k : corners)
-        if (k < -128 || k > 127)
-          return fail(B200_ERR_UNSUPPORTED, "%s: im2col pixel-box corner %lld of phase (%u, %u) outside [-128, 127]", what, (long long)k, ph.r, pw.r);
+      if ((rc = conv_check_corners(what, corners))) return rc;
     }
-  if (!dy || !w || !dx) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
+  if ((rc = conv_check_ptrs(what, dy, w, dx, "dx", out_dtype))) return rc;
   const size_t osz = dtype_size(out_dtype);
-  if (dx % osz) return fail(B200_ERR_INVALID_ARG, "%s: dx pointer is not aligned to its element size", what);
   uint64_t os[4], ys[4], ws[4];
   conv_norm_strides(dx_shape, dx_strides, os);
-  if (os[3] != 1 || os[2] < C || os[1] != W * os[2] || os[0] != H * os[1])
-    return fail(B200_ERR_UNSUPPORTED, "%s: dx must have unit channel stride and one pixel pitch >= C for N, H, W", what);
+  if ((rc = conv_check_pixels(what, "dx", dx_shape, os))) return rc;
   CUstream st = resolve_stream(c, s);
   // dx pixels that no tap reaches are exact zeros: one memset of dx, before the phases that overwrite the rest
   if (zero_phase) {
@@ -2901,7 +2902,7 @@ extern "C" int b200_conv2d_backward_data(b200_ctx* c, b200_stream s, b200_dtype 
   conv_norm_strides(w_shape, w_strides, ws);
   CUdeviceptr tmp[3] = {0, 0, 0};
   NhwcOperand y{};
-  rc = conv_prep_nhwc(c, st, in_dtype, dy, dy_shape, ys, false, tmp, &y);
+  rc = conv_prep_nhwc(c, st, in_dtype, dy, dy_shape, ys, kFlatNone, tmp, &y);
   // every phase's flipped, channel-transposed weights [C][Th][Tw][cp] in one pooled buffer of KH * KW * C * cp elements
   const uint64_t cp = y.C;
   ConvDgradWeightsParams wp;
@@ -2952,14 +2953,9 @@ extern "C" int b200_conv2d_backward_data(b200_ctx* c, b200_stream s, b200_dtype 
                 std::to_string(pw.extent) + ")\n";
         c->plan += line;
       }
-      GemmProblem gp{};
-      gp.in_dtype = in_dtype; gp.out_dtype = out_dtype;
-      gp.a = y.ptr; gp.b = tmp[2] + wp.off[ph.r * a.stride_w + pw.r] * 2;
-      gp.out = dx + ((uint64_t)ph.r * os[1] + (uint64_t)pw.r * os[2]) * osz;
-      gp.M = N * ph.extent * pw.extent; gp.N = C; gp.K = (uint64_t)ph.taps * pw.taps * ((cp + 63) / 64 * 64); gp.batch = 1;
-      gp.a_sm = gp.K; gp.a_sk = 1; gp.b_sn = gp.K; gp.b_sk = 1;
-      gp.o_sm = os[2]; gp.o_sn = 1; gp.o_sb = 0;
-      gp.conv = &g;
+      const GemmProblem gp = conv_problem(in_dtype, out_dtype, y.ptr, tmp[2] + wp.off[ph.r * a.stride_w + pw.r] * 2,
+                                          dx + ((uint64_t)ph.r * os[1] + (uint64_t)pw.r * os[2]) * osz, N * ph.extent * pw.extent, C,
+                                          (uint64_t)ph.taps * pw.taps * ((cp + 63) / 64 * 64), os[2], &g);
       rc = launch_wgmma(c, st, gp, false, false);
     }
   for (CUdeviceptr t : tmp)
@@ -2975,32 +2971,24 @@ extern "C" int b200_conv2d_backward_weight(b200_ctx* c, b200_stream s, b200_dtyp
   const char* what = "conv2d_backward_weight";
   if (!x_shape || !dy_shape || !dw_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
   const b200_conv2d_args& a = *args;
-  uint64_t OH = 0, OW = 0;
-  int rc = conv_bwd_check(what, in_dtype, out_dtype, a, x_shape, dw_shape, dy_shape, &OH, &OW);
-  if (rc) return rc;
   const uint64_t N = x_shape[0], H = x_shape[1], W = x_shape[2], C = x_shape[3];
   const uint64_t Cout = dw_shape[0], KH = dw_shape[1], KW = dw_shape[2];
+  uint64_t OH = 0, OW = 0;
+  int rc = conv_check_args(what, in_dtype, out_dtype, a, nullptr, C, dw_shape[3]);
+  if (!rc) rc = conv_check_shape(what, a, x_shape, dw_shape, dy_shape, "dy", &OH, &OW);
+  if (!rc && KH && KW) rc = conv_check_stride(what, a);
+  if (rc) return rc;
   if (Cout == 0 || C == 0 || KH == 0 || KW == 0) return B200_OK;   // no dw
-  // the forward's 4-D im2col limits: x is read through the same map
-  const int64_t corners[4] = {-(int64_t)a.pad_h, -(int64_t)a.pad_w, (int64_t)a.pad_h - (int64_t)a.dilation_h * ((int64_t)KH - 1),
-                              (int64_t)a.pad_w - (int64_t)a.dilation_w * ((int64_t)KW - 1)};
-  for (int64_t k : corners)
-    if (k < -128 || k > 127)
-      return fail(B200_ERR_UNSUPPORTED, "%s: im2col pixel-box corner %lld outside [-128, 127] (-pad and pad - dilation * (kernel - 1))", what,
-                  (long long)k);
+  if ((rc = conv_check_fwd_corners(what, a, KH, KW))) return rc;   // x is read through the forward's map
   const uint64_t P = N * OH * OW, lim = 1ull << 31;
   if (P >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * OH * OW = %llu must be < 2^31", what, (unsigned long long)P);
   const uint64_t cx = (C + 7) / 8 * 8;
   if (KH * KW * ((cx + 63) / 64 * 64) >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: KH * KW * C (C padded to 64) must be < 2^31", what);
-  if (!x || !dy || !dw) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
+  if ((rc = conv_check_ptrs(what, x, dy, dw, "dw", out_dtype))) return rc;
   const size_t osz = dtype_size(out_dtype);
-  if (dw % osz) return fail(B200_ERR_INVALID_ARG, "%s: dw pointer is not aligned to its element size", what);
-  // dw: unit channel stride, (KH, KW) flattening into one kernel-position stride, and an output-channel stride
-  uint64_t ds[4], xs[4], ys[4];
+  uint64_t ds[4], xs[4], ys[4], dw_sp = 0;
   conv_norm_strides(dw_shape, dw_strides, ds);
-  const uint64_t dw_sp = (KW == 1) ? ds[1] : (KH == 1 || ds[1] == KW * ds[2]) ? ds[2] : 0;
-  if (ds[3] != 1 || dw_sp == 0 || ds[0] * osz >= (1ull << 40) || dw_sp * osz >= (1ull << 40))
-    return fail(B200_ERR_UNSUPPORTED, "%s: dw must have unit channel stride and (KH, KW) flattening into one stride", what);
+  if ((rc = conv_check_dw(what, dw_shape, ds, osz, &dw_sp))) return rc;
   CUstream st = resolve_stream(c, s);
   if (P == 0) {
     // no pixels: dw is exactly zero
@@ -3012,21 +3000,16 @@ extern "C" int b200_conv2d_backward_weight(b200_ctx* c, b200_stream s, b200_dtyp
   conv_norm_strides(dy_shape, dy_strides, ys);
   CUdeviceptr tmp[4] = {0, 0, 0, 0};
   NhwcOperand xo{}, yo{};
-  rc = conv_prep_nhwc(c, st, in_dtype, x, x_shape, xs, false, &tmp[0], &xo);
-  if (!rc) rc = conv_prep_nhwc(c, st, in_dtype, dy, dy_shape, ys, true, &tmp[2], &yo);
+  rc = conv_prep_nhwc(c, st, in_dtype, x, x_shape, xs, kFlatNone, &tmp[0], &xo);
+  if (!rc) rc = conv_prep_nhwc(c, st, in_dtype, dy, dy_shape, ys, kFlatNHW, &tmp[2], &yo);
   if (!rc) {
     ConvGeom g{};
     g.N = N; g.H = H; g.W = W; g.C = xo.C; g.KH = KH; g.KW = KW; g.OH = OH; g.OW = OW; g.Cout = Cout;
     g.sh = a.stride_h; g.sw = a.stride_w; g.ph = a.pad_h; g.pw = a.pad_w; g.dh = a.dilation_h; g.dw = a.dilation_w;
     g.x_sw = xo.s_w; g.x_sh = xo.s_h; g.x_sn = xo.s_n;
     g.mode = 2; g.dw_sp = dw_sp; g.dw_c = C;
-    GemmProblem gp{};
-    gp.in_dtype = in_dtype; gp.out_dtype = out_dtype;
-    gp.a = yo.ptr; gp.b = xo.ptr; gp.out = dw;
-    gp.M = Cout; gp.N = KH * KW * ((xo.C + 63) / 64 * 64); gp.K = P; gp.batch = 1;
-    gp.a_sm = 1; gp.a_sk = yo.s_w; gp.b_sn = 1; gp.b_sk = xo.s_w;
-    gp.o_sm = ds[0]; gp.o_sn = 1; gp.o_sb = 0;
-    gp.conv = &g;
+    GemmProblem gp = conv_problem(in_dtype, out_dtype, yo.ptr, xo.ptr, dw, Cout, KH * KW * ((xo.C + 63) / 64 * 64), P, ds[0], &g);
+    gp.a_sm = 1; gp.a_sk = yo.s_w; gp.b_sn = 1; gp.b_sk = xo.s_w;   // both operands MN-major
     // few tiles, a long K: the stream-K head may cut a tile into as many ranges as fill the SMs, each >= 8 k-blocks
     gp.sk_max_parts = std::max<uint64_t>(8, (P + 63) / 64 / 8);
     rc = launch_wgmma(c, st, gp, true, true);
@@ -3039,7 +3022,8 @@ extern "C" int b200_conv2d_backward_weight(b200_ctx* c, b200_stream s, b200_dtyp
 // ------------------------------------------------------------------------------------------------ grouped convolution
 // Routing, from the shape alone: groups == 1 is the plain entry point; a group width Cg = C / groups of at least one
 // k-block (64 channels) runs one implicit GEMM per group on channel slices; narrower groups run the direct kernels of
-// conv_grouped.cu, for which the GEMM route would multiply mostly zero-padded k-blocks.
+// conv_grouped.cu, for which the GEMM route would multiply mostly zero-padded k-blocks.  The direct route applies the same
+// checks as the GEMM route, so both accept the same shapes.
 constexpr uint64_t kGrpGemmMinCg = 64;
 
 static int grp_check(const char* what, uint32_t groups, uint64_t C, uint64_t Cout, uint64_t w_c) {
@@ -3053,16 +3037,15 @@ static int grp_check(const char* what, uint32_t groups, uint64_t C, uint64_t Cou
   return B200_OK;
 }
 
-// The forward's limits on (args, kernel extent), applied to every direct-route kernel so both routes accept the same shapes.
-static int grp_limits(const char* what, const b200_conv2d_args& a, uint64_t KH, uint64_t KW) {
-  const int64_t corners[4] = {-(int64_t)a.pad_h, -(int64_t)a.pad_w, (int64_t)a.pad_h - (int64_t)a.dilation_h * ((int64_t)KH - 1),
-                              (int64_t)a.pad_w - (int64_t)a.dilation_w * ((int64_t)KW - 1)};
-  for (int64_t k : corners)
-    if (k < -128 || k > 127)
-      return fail(B200_ERR_UNSUPPORTED, "%s: pixel-box corner %lld outside [-128, 127] (-pad and pad - dilation * (kernel - 1))", what,
-                  (long long)k);
-  if (a.stride_h > 8 || a.stride_w > 8) return fail(B200_ERR_UNSUPPORTED, "%s: the conv stride must be <= 8", what);
-  return B200_OK;
+// The parameter fields every direct kernel reads: the input [N, H, W, C], the output extents, the weights [Cout, KH, KW, *],
+// groups and args; the rest is zero.
+static ConvGroupedParams grp_params(const uint64_t* in, uint64_t OH, uint64_t OW, const uint64_t* w, uint32_t groups, const b200_conv2d_args& a) {
+  ConvGroupedParams p;
+  memset(&p, 0, sizeof(p));
+  p.N = (uint32_t)in[0]; p.H = (uint32_t)in[1]; p.W = (uint32_t)in[2]; p.C = (uint32_t)in[3]; p.OH = (uint32_t)OH; p.OW = (uint32_t)OW;
+  p.Cout = (uint32_t)w[0]; p.KH = (uint32_t)w[1]; p.KW = (uint32_t)w[2]; p.Cg = (uint32_t)(in[3] / groups); p.Coutg = (uint32_t)(w[0] / groups);
+  p.sh = a.stride_h; p.sw = a.stride_w; p.ph = a.pad_h; p.pw = a.pad_w; p.dh = a.dilation_h; p.dw = a.dilation_w;
+  return p;
 }
 
 // A rank-4 operand the direct kernels read through its strides: kept in place with a unit channel stride, else gathered
@@ -3091,34 +3074,17 @@ extern "C" int b200_conv2d_grouped(b200_ctx* c, b200_stream s, b200_dtype in_dty
   if (!x_shape || !w_shape || !out_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
   if (groups == 1)
     return b200_conv2d(c, s, in_dtype, out_dtype, x, x_shape, x_strides, w, w_shape, w_strides, out, out_shape, out_strides, args, ep);
+  const b200_conv2d_args& a = *args;
   const uint64_t N = x_shape[0], H = x_shape[1], W = x_shape[2], C = x_shape[3];
   const uint64_t Cout = w_shape[0], KH = w_shape[1], KW = w_shape[2];
   int rc = grp_check(what, groups, C, Cout, w_shape[3]);
+  if (!rc) rc = conv_check_args(what, in_dtype, out_dtype, a, ep, C / groups, w_shape[3]);
   if (rc) return rc;
-  if (in_dtype != B200_F16 && in_dtype != B200_BF16)
-    return fail(B200_ERR_UNSUPPORTED, "%s: input dtype %d unsupported (f16, bf16)", what, (int)in_dtype);
-  if (out_dtype != in_dtype && out_dtype != B200_F32)
-    return fail(B200_ERR_UNSUPPORTED, "%s: output dtype must equal the input dtype or be f32", what);
-  if (ep && (ep->activation < 0 || ep->activation > 2)) return fail(B200_ERR_INVALID_ARG, "%s: unknown activation %d", what, ep->activation);
-  const b200_conv2d_args& a = *args;
-  if (a.stride_h < 1 || a.stride_w < 1 || a.dilation_h < 1 || a.dilation_w < 1 || a.pad_h < 0 || a.pad_w < 0)
-    return fail(B200_ERR_INVALID_ARG, "%s: strides and dilations must be >= 1 and padding >= 0", what);
   if (N == 0 || H == 0 || W == 0 || C == 0 || Cout == 0 || KH == 0 || KW == 0) return B200_OK;
-  const uint64_t lim = 1ull << 31;
-  if (N >= lim || H >= lim || W >= lim || C >= lim || Cout >= lim || KH >= lim || KW >= lim)
-    return fail(B200_ERR_UNSUPPORTED, "%s: extents must be < 2^31", what);
-  const int64_t nh = (int64_t)H + 2 * (int64_t)a.pad_h - (int64_t)a.dilation_h * ((int64_t)KH - 1) - 1;
-  const int64_t nw = (int64_t)W + 2 * (int64_t)a.pad_w - (int64_t)a.dilation_w * ((int64_t)KW - 1) - 1;
-  if (nh < 0 || nw < 0) return fail(B200_ERR_INVALID_ARG, "%s: the dilated kernel is larger than the padded input (output extent < 1)", what);
-  const uint64_t OH = (uint64_t)(nh / a.stride_h) + 1, OW = (uint64_t)(nw / a.stride_w) + 1;
-  if (out_shape[0] != N || out_shape[1] != OH || out_shape[2] != OW || out_shape[3] != Cout)
-    return fail(B200_ERR_INVALID_ARG, "%s: out is [%llu,%llu,%llu,%llu], expected [%llu,%llu,%llu,%llu]", what,
-                (unsigned long long)out_shape[0], (unsigned long long)out_shape[1], (unsigned long long)out_shape[2],
-                (unsigned long long)out_shape[3], (unsigned long long)N, (unsigned long long)OH, (unsigned long long)OW,
-                (unsigned long long)Cout);
-  if (!x || !w || !out) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
+  uint64_t OH = 0, OW = 0;
+  if ((rc = conv_check_shape(what, a, x_shape, w_shape, out_shape, "out", &OH, &OW))) return rc;
+  if ((rc = conv_check_ptrs(what, x, w, out, "output", out_dtype))) return rc;
   const size_t osz = dtype_size(out_dtype);
-  if (out % osz) return fail(B200_ERR_INVALID_ARG, "%s: output pointer is not aligned to its element size", what);
   const uint64_t Cg = C / groups, Coutg = Cout / groups;
   uint64_t xs[4], ws[4], os[4];
   conv_norm_strides(x_shape, x_strides, xs);
@@ -3138,18 +3104,17 @@ extern "C" int b200_conv2d_grouped(b200_ctx* c, b200_stream s, b200_dtype in_dty
     }
     return rc;
   }
-  if ((rc = grp_limits(what, a, KH, KW))) return rc;
+  if ((rc = conv_check_fwd_corners(what, a, KH, KW)) || (rc = conv_check_stride(what, a))) return rc;
+  const uint64_t lim = 1ull << 31;
   if (N * OH * OW >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * OH * OW = %llu must be < 2^31", what, (unsigned long long)(N * OH * OW));
-  if (os[3] != 1 || os[2] < Cout || os[1] != OW * os[2] || os[0] != OH * os[1])
-    return fail(B200_ERR_UNSUPPORTED, "%s: out must have unit channel stride and one pixel pitch >= Cout for N, OH, OW", what);
+  if ((rc = conv_check_pixels(what, "out", out_shape, os))) return rc;
   const uint64_t tiles_h = (OH + kGrpTileH - 1) / kGrpTileH, tiles_w = (OW + kGrpTileW - 1) / kGrpTileW;
   const uint64_t chunks = (Cout + kGrpChunk - 1) / kGrpChunk;
   if (N * tiles_h * tiles_w >= lim || chunks > 65535)
     return fail(B200_ERR_UNSUPPORTED, "%s: too many output tiles (N * ceil(OH / 8) * ceil(OW / 8) < 2^31, Cout <= 2^21)", what);
   CUstream st = resolve_stream(c, s);
   CUdeviceptr tmp[2] = {0, 0};
-  ConvGroupedParams p;
-  memset(&p, 0, sizeof(p));
+  ConvGroupedParams p = grp_params(x_shape, OH, OW, w_shape, groups, a);
   uint64_t xsr[4], wsr[4];
   rc = grp_operand(c, st, in_dtype, x, x_shape, xs, &tmp[0], &p.x, xsr);
   if (!rc) rc = grp_operand(c, st, in_dtype, w, w_shape, ws, &tmp[1], &p.w, wsr);
@@ -3158,9 +3123,6 @@ extern "C" int b200_conv2d_grouped(b200_ctx* c, b200_stream s, b200_dtype in_dty
     p.x_sn = xsr[0]; p.x_sh = xsr[1]; p.x_sw = xsr[2];
     p.w_sco = wsr[0]; p.w_sky = wsr[1]; p.w_skx = wsr[2];
     p.o_sn = os[0]; p.o_sh = os[1]; p.o_sw = os[2];
-    p.N = (uint32_t)N; p.H = (uint32_t)H; p.W = (uint32_t)W; p.C = (uint32_t)C; p.OH = (uint32_t)OH; p.OW = (uint32_t)OW;
-    p.Cout = (uint32_t)Cout; p.KH = (uint32_t)KH; p.KW = (uint32_t)KW; p.Cg = (uint32_t)Cg; p.Coutg = (uint32_t)Coutg;
-    p.sh = a.stride_h; p.sw = a.stride_w; p.ph = a.pad_h; p.pw = a.pad_w; p.dh = a.dilation_h; p.dw = a.dilation_w;
     p.tiles_h = (uint32_t)tiles_h; p.tiles_w = (uint32_t)tiles_w;
     p.vec_x = (p.x % 16 == 0 && xsr[0] % 8 == 0 && xsr[1] % 8 == 0 && xsr[2] % 8 == 0) ? 1u : 0u;
     if (ep) {
@@ -3200,18 +3162,18 @@ extern "C" int b200_conv2d_grouped_backward_data(b200_ctx* c, b200_stream s, b20
   if (!dy_shape || !w_shape || !dx_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
   if (groups == 1)
     return b200_conv2d_backward_data(c, s, in_dtype, out_dtype, dy, dy_shape, dy_strides, w, w_shape, w_strides, dx, dx_shape, dx_strides, args);
+  const b200_conv2d_args& a = *args;
   const uint64_t N = dx_shape[0], H = dx_shape[1], W = dx_shape[2], C = dx_shape[3];
   const uint64_t Cout = w_shape[0], KH = w_shape[1], KW = w_shape[2];
-  int rc = grp_check(what, groups, C, Cout, w_shape[3]);
-  if (rc) return rc;
-  const b200_conv2d_args& a = *args;
-  const uint64_t w_full[4] = {Cout, KH, KW, C};
   uint64_t OH = 0, OW = 0;
-  if ((rc = conv_bwd_check(what, in_dtype, out_dtype, a, dx_shape, w_full, dy_shape, &OH, &OW))) return rc;
+  int rc = grp_check(what, groups, C, Cout, w_shape[3]);
+  if (!rc) rc = conv_check_args(what, in_dtype, out_dtype, a, nullptr, C / groups, w_shape[3]);
+  if (!rc) rc = conv_check_shape(what, a, dx_shape, w_shape, dy_shape, "dy", &OH, &OW);
+  if (!rc && KH && KW) rc = conv_check_stride(what, a);
+  if (rc) return rc;
   if (N == 0 || H == 0 || W == 0 || C == 0) return B200_OK;   // no dx
-  if (!dy || !w || !dx) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
+  if ((rc = conv_check_ptrs(what, dy, w, dx, "dx", out_dtype))) return rc;
   const size_t osz = dtype_size(out_dtype);
-  if (dx % osz) return fail(B200_ERR_INVALID_ARG, "%s: dx pointer is not aligned to its element size", what);
   const uint64_t Cg = C / groups, Coutg = Cout / groups;
   uint64_t ys[4], ws[4], os[4];
   conv_norm_strides(dy_shape, dy_strides, ys);
@@ -3224,17 +3186,15 @@ extern "C" int b200_conv2d_grouped_backward_data(b200_ctx* c, b200_stream s, b20
                                      dx + g * Cg * os[3] * osz, sx, os, args);
     return rc;
   }
-  if (KH && KW && (rc = grp_limits(what, a, KH, KW))) return rc;
+  if (KH && KW && (rc = conv_check_fwd_corners(what, a, KH, KW))) return rc;
   const uint64_t lim = 1ull << 31;
   if (N * H * W >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * H * W = %llu must be < 2^31", what, (unsigned long long)(N * H * W));
-  if (os[3] != 1 || os[2] < C || os[1] != W * os[2] || os[0] != H * os[1])
-    return fail(B200_ERR_UNSUPPORTED, "%s: dx must have unit channel stride and one pixel pitch >= C for N, H, W", what);
+  if ((rc = conv_check_pixels(what, "dx", dx_shape, os))) return rc;
   const uint64_t chunks = (C + kGrpChunk - 1) / kGrpChunk;
   if (chunks > 65535) return fail(B200_ERR_UNSUPPORTED, "%s: C must be <= 2^21", what);
   CUstream st = resolve_stream(c, s);
   CUdeviceptr tmp[2] = {0, 0};
-  ConvGroupedParams p;
-  memset(&p, 0, sizeof(p));
+  ConvGroupedParams p = grp_params(dx_shape, OH, OW, w_shape, groups, a);
   uint64_t ysr[4] = {0, 0, 0, 1}, wsr[4] = {0, 0, 0, 1};
   // an empty dy or kernel reads nothing: dx comes out as +0 from the same launch
   if (Cout && KH && KW) {
@@ -3246,9 +3206,6 @@ extern "C" int b200_conv2d_grouped_backward_data(b200_ctx* c, b200_stream s, b20
     p.x_sn = ysr[0]; p.x_sh = ysr[1]; p.x_sw = ysr[2];
     p.w_sco = wsr[0]; p.w_sky = wsr[1]; p.w_skx = wsr[2];
     p.o_sn = os[0]; p.o_sh = os[1]; p.o_sw = os[2];
-    p.N = (uint32_t)N; p.H = (uint32_t)H; p.W = (uint32_t)W; p.C = (uint32_t)C; p.OH = (uint32_t)OH; p.OW = (uint32_t)OW;
-    p.Cout = (uint32_t)Cout; p.KH = (uint32_t)KH; p.KW = (uint32_t)KW; p.Cg = (uint32_t)Cg; p.Coutg = (uint32_t)Coutg;
-    p.sh = a.stride_h; p.sw = a.stride_w; p.ph = a.pad_h; p.pw = a.pad_w; p.dh = a.dilation_h; p.dw = a.dilation_w;
     CUfunction f;
     rc = get_func(c, std::string("conv2d_grp_dgrad_") + grp_tag(in_dtype) + "_" + grp_tag(out_dtype), &f);
     void* kargs[] = {&p};
@@ -3278,21 +3235,21 @@ extern "C" int b200_conv2d_grouped_backward_weight(b200_ctx* c, b200_stream s, b
   if (groups == 1)
     return b200_conv2d_backward_weight(c, s, in_dtype, out_dtype, x, x_shape, x_strides, dy, dy_shape, dy_strides, dw, dw_shape, dw_strides,
                                        args);
+  const b200_conv2d_args& a = *args;
   const uint64_t N = x_shape[0], H = x_shape[1], W = x_shape[2], C = x_shape[3];
   const uint64_t Cout = dw_shape[0], KH = dw_shape[1], KW = dw_shape[2];
-  int rc = grp_check(what, groups, C, Cout, dw_shape[3]);
-  if (rc) return rc;
-  const b200_conv2d_args& a = *args;
-  const uint64_t dw_full[4] = {Cout, KH, KW, C};
   uint64_t OH = 0, OW = 0;
-  if ((rc = conv_bwd_check(what, in_dtype, out_dtype, a, x_shape, dw_full, dy_shape, &OH, &OW))) return rc;
+  int rc = grp_check(what, groups, C, Cout, dw_shape[3]);
+  if (!rc) rc = conv_check_args(what, in_dtype, out_dtype, a, nullptr, C / groups, dw_shape[3]);
+  if (!rc) rc = conv_check_shape(what, a, x_shape, dw_shape, dy_shape, "dy", &OH, &OW);
+  if (!rc && KH && KW) rc = conv_check_stride(what, a);
+  if (rc) return rc;
   if (Cout == 0 || C == 0 || KH == 0 || KW == 0) return B200_OK;   // no dw
-  if ((rc = grp_limits(what, a, KH, KW))) return rc;
+  if ((rc = conv_check_fwd_corners(what, a, KH, KW))) return rc;
   const uint64_t P = N * OH * OW, lim = 1ull << 31;
   if (P >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * OH * OW = %llu must be < 2^31", what, (unsigned long long)P);
-  if (!x || !dy || !dw) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
+  if ((rc = conv_check_ptrs(what, x, dy, dw, "dw", out_dtype))) return rc;
   const size_t osz = dtype_size(out_dtype);
-  if (dw % osz) return fail(B200_ERR_INVALID_ARG, "%s: dw pointer is not aligned to its element size", what);
   const uint64_t Cg = C / groups, Coutg = Cout / groups;
   uint64_t xs[4], ys[4], ds[4];
   conv_norm_strides(x_shape, x_strides, xs);
@@ -3305,9 +3262,8 @@ extern "C" int b200_conv2d_grouped_backward_weight(b200_ctx* c, b200_stream s, b
                                        dw + g * Coutg * ds[0] * osz, sw, ds, args);
     return rc;
   }
-  const uint64_t dw_sp = (KW == 1) ? ds[1] : (KH == 1 || ds[1] == KW * ds[2]) ? ds[2] : 0;
-  if (ds[3] != 1 || dw_sp == 0 || ds[0] * osz >= (1ull << 40) || dw_sp * osz >= (1ull << 40))
-    return fail(B200_ERR_UNSUPPORTED, "%s: dw must have unit channel stride and (KH, KW) flattening into one stride", what);
+  uint64_t dw_sp = 0;
+  if ((rc = conv_check_dw(what, dw_shape, ds, osz, &dw_sp))) return rc;
   const uint64_t elems = Cout * KH * KW * Cg;
   if (elems >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: Cout * KH * KW * C / groups = %llu must be < 2^31", what, (unsigned long long)elems);
   uint64_t seg_len = 0, nseg = 0;
@@ -3320,8 +3276,7 @@ extern "C" int b200_conv2d_grouped_backward_weight(b200_ctx* c, b200_stream s, b
   }
   CUstream st = resolve_stream(c, s);
   CUdeviceptr tmp[3] = {0, 0, 0};
-  ConvGroupedParams p;
-  memset(&p, 0, sizeof(p));
+  ConvGroupedParams p = grp_params(x_shape, OH, OW, dw_shape, groups, a);
   uint64_t xsr[4], ysr[4];
   rc = grp_operand(c, st, in_dtype, x, x_shape, xs, &tmp[0], &p.x, xsr);
   if (!rc) rc = grp_operand(c, st, in_dtype, dy, dy_shape, ys, &tmp[1], &p.w, ysr);
@@ -3332,9 +3287,6 @@ extern "C" int b200_conv2d_grouped_backward_weight(b200_ctx* c, b200_stream s, b
     p.y_sn = ysr[0]; p.y_sh = ysr[1]; p.y_sw = ysr[2];
     p.o_sn = ds[0]; p.o_sw = dw_sp;
     p.seg_len = seg_len; p.elems = elems; p.nseg = (uint32_t)nseg;
-    p.N = (uint32_t)N; p.H = (uint32_t)H; p.W = (uint32_t)W; p.C = (uint32_t)C; p.OH = (uint32_t)OH; p.OW = (uint32_t)OW;
-    p.Cout = (uint32_t)Cout; p.KH = (uint32_t)KH; p.KW = (uint32_t)KW; p.Cg = (uint32_t)Cg; p.Coutg = (uint32_t)Coutg;
-    p.sh = a.stride_h; p.sw = a.stride_w; p.ph = a.pad_h; p.pw = a.pad_w; p.dh = a.dilation_h; p.dw = a.dilation_w;
     const unsigned blocks = (unsigned)((elems + 255) / 256);
     void* kargs[] = {&p};
     CUfunction f;
