@@ -47,6 +47,13 @@ class Conv2dArgs(C.Structure):
                 ("dilation_h", C.c_int32), ("dilation_w", C.c_int32)]
 
 
+class Conv3dArgs(C.Structure):
+    """b200_conv3d_args: stride, padding and dilation per spatial axis (d, h, w)."""
+    _fields_ = [("stride_d", C.c_int32), ("stride_h", C.c_int32), ("stride_w", C.c_int32), ("pad_d", C.c_int32),
+                ("pad_h", C.c_int32), ("pad_w", C.c_int32), ("dilation_d", C.c_int32), ("dilation_h", C.c_int32),
+                ("dilation_w", C.c_int32)]
+
+
 class QuantScheme(C.Structure):
     """b200_quant_scheme: value (b200_quant_value), block, block_scale (b200_dtype), tensor_scale (0 / 1)."""
     _fields_ = [("value", C.c_int32), ("block", C.c_int32), ("block_scale", C.c_int32), ("tensor_scale", C.c_int32)]
@@ -123,6 +130,12 @@ SIGNATURES = {
                                                     C.c_uint64, _u64p, _u64p, C.POINTER(Conv2dArgs), C.c_uint32]),
     "b200_conv2d_grouped_backward_weight": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, _u64p, _u64p, C.c_uint64, _u64p, _u64p,
                                                       C.c_uint64, _u64p, _u64p, C.POINTER(Conv2dArgs), C.c_uint32]),
+    "b200_conv3d": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, _u64p, _u64p, C.c_uint64, _u64p, _u64p, C.c_uint64, _u64p,
+                              _u64p, C.POINTER(Conv3dArgs), C.POINTER(Epilogue)]),
+    "b200_conv3d_backward_data": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, _u64p, _u64p, C.c_uint64, _u64p, _u64p,
+                                            C.c_uint64, _u64p, _u64p, C.POINTER(Conv3dArgs)]),
+    "b200_conv3d_backward_weight": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, _u64p, _u64p, C.c_uint64, _u64p, _u64p,
+                                              C.c_uint64, _u64p, _u64p, C.POINTER(Conv3dArgs)]),
     "b200_reduce": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, C.c_uint64, C.c_int, _u64p, C.c_int]),
     "b200_reduce_strided": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, C.c_uint64, C.c_int, _u64p, _u64p, C.c_int]),
     "b200_reduce_debug": (C.c_int, [_vp, _vp, _u64p]),

@@ -31,12 +31,13 @@ class ConvShapeError(ValueError):
     """The output-shape rule does not hold: channel mismatch, rank, or an output extent < 1."""
 
 
-def _pair(v, what: str) -> tuple[int, int]:
+def _pair(v, what: str, n: int = 2) -> tuple[int, ...]:
+    """v as n ints: an int repeats, a sequence must have n entries."""
     if isinstance(v, int):
-        return int(v), int(v)
+        return (int(v),) * n
     v = tuple(int(e) for e in v)
-    if len(v) != 2:
-        raise ValueError(f"{what} must be an int or a pair, got {v!r}")
+    if len(v) != n:
+        raise ValueError(f"{what} must be an int or {'a pair' if n == 2 else f'{n} ints'}, got {v!r}")
     return v
 
 
@@ -67,17 +68,22 @@ def launch(client: ComputeClient, x: TensorHandle, w: TensorHandle, out: TensorH
     epilogue: out = activation(alpha * conv + bias[co]) with `bias` an f32 [Cout] tensor.  groups > 1: a grouped convolution
     with w [Cout, KH, KW, C / groups].  Never raises for launch problems: errors are deferred to client.sync() / read_one()
     like matmul.launch."""
+    _enqueue(client, "conv2d", x, w, out, stride, padding, dilation, stream, groups, _epilogue_check("conv2d", w, alpha, bias, activation))
+
+
+def _epilogue_check(what: str, w: TensorHandle, alpha: float, bias: TensorHandle | None, activation: str | None):
+    """launch's epilogue callback for _enqueue: checks the epilogue arguments, returns (b200_epilogue pointer or None,
+    the extra handles it reads)."""
     def epilogue():
         if activation not in ACTIVATIONS:
             raise B200Error(6, f"unknown activation {activation!r}")
         if bias is not None and (bias.dtype != "f32" or not bias.is_contiguous() or bias.size() != w.shape[0]):
-            raise B200Error(6, "conv2d: bias must be a contiguous f32 tensor with Cout elements")
+            raise B200Error(6, f"{what}: bias must be a contiguous f32 tensor with Cout elements")
         if alpha == 1.0 and bias is None and activation in (None, "none"):
             return None, ()
         ep = _ffi.Epilogue(float(alpha), ACTIVATIONS[activation], bias.handle.ptr if bias is not None else 0)
         return C.byref(ep), (() if bias is None else (bias,))
-
-    _enqueue(client, "conv2d", x, w, out, stride, padding, dilation, stream, groups, epilogue)
+    return epilogue
 
 
 def launch_alloc(client: ComputeClient, x: TensorHandle, w: TensorHandle, out_dtype: str | None = None, **kwargs) -> TensorHandle:
@@ -97,21 +103,22 @@ def _groups(groups) -> C.c_uint32:
 
 
 def _enqueue(client: ComputeClient, name: str, a: TensorHandle, b: TensorHandle, out: TensorHandle, stride, padding, dilation, stream,
-             groups, epilogue=None) -> None:
-    """The body of launch, backward_data and backward_weight: check the operands, mark them used on `stream` and call
-    b200_<name>(a, b, out, args[, epilogue]), or its grouped form when groups != 1.  epilogue (launch only) checks the
-    epilogue arguments and returns (the b200_epilogue pointer or None, the extra handles it reads).  Errors are deferred to
-    client.sync() / read_one()."""
+             groups, epilogue=None, spatial: int = 2) -> None:
+    """The body of launch, backward_data and backward_weight (and of conv3d's, spatial = 3): check the operands, mark them
+    used on `stream` and call b200_<name>(a, b, out, args[, epilogue]), or its grouped form when groups != 1.  epilogue
+    (launch only) checks the epilogue arguments and returns (the b200_epilogue pointer or None, the extra handles it reads).
+    Errors are deferred to client.sync() / read_one()."""
     try:
-        if len(a.shape) != 4 or len(b.shape) != 4 or len(out.shape) != 4:
-            raise B200Error(6, f"{name}: every operand must have rank 4")
+        rank = spatial + 2
+        if len(a.shape) != rank or len(b.shape) != rank or len(out.shape) != rank:
+            raise B200Error(6, f"{name}: every operand must have rank {rank}")
         if a.dtype != b.dtype:
             raise B200Error(6, f"{name}: operand dtypes differ ({a.dtype}, {b.dtype})")
         ep, extra = epilogue() if epilogue else (None, ())
-        (sh, sw), (ph, pw), (dh, dw) = _pair(stride, "stride"), _pair(padding, "padding"), _pair(dilation, "dilation")
+        s, p, d = _pair(stride, "stride", spatial), _pair(padding, "padding", spatial), _pair(dilation, "dilation", spatial)
         for t in (a, b, out, *extra):
             t.handle.used_on(stream)
-        args = _ffi.Conv2dArgs(sh, sw, ph, pw, dh, dw)
+        args = _ffi.Conv2dArgs(*s, *p, *d) if spatial == 2 else _ffi.Conv3dArgs(*s, *p, *d)
         operands = (client._ctx, stream, DTYPES[a.dtype], DTYPES[out.dtype],
                     C.c_uint64(a.handle.ptr), _ffi.u64_array(a.shape), _ffi.u64_array(a.strides),
                     C.c_uint64(b.handle.ptr), _ffi.u64_array(b.shape), _ffi.u64_array(b.strides),

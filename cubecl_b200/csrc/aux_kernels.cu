@@ -470,3 +470,38 @@ extern "C" __global__ void __launch_bounds__(256) conv_dgrad_weights(const __gri
     if (c < p.C && co < p.cp) out[base + c * c_pitch + co] = tile[tx][r];
   }
 }
+
+// Conv3dDgradWeightsParams: one block per (32 input channels x 32 output channels, kernel position (kz, ky, kx)).
+extern "C" __global__ void __launch_bounds__(256) conv3d_dgrad_weights(const __grid_constant__ Conv3dDgradWeightsParams p) {
+  __shared__ uint16_t tile[32][33];
+  const uint32_t khw = p.k[1] * p.k[2], kpos = blockIdx.y;
+  const uint32_t kk[3] = {kpos / khw, (kpos % khw) / p.k[2], kpos % p.k[2]};
+  const uint64_t c_tiles = (p.C + 31) / 32;
+  const uint64_t c0 = (blockIdx.x % c_tiles) * 32, co0 = (blockIdx.x / c_tiles) * 32;
+  const uint32_t tx = threadIdx.x & 31u, ty = threadIdx.x >> 5;
+  const uint16_t* w = reinterpret_cast<const uint16_t*>(p.w);
+  for (uint32_t r = ty; r < 32; r += 8) {
+    const uint64_t co = co0 + r, c = c0 + tx;
+    tile[r][tx] = (co < p.Cout && c < p.C) ? w[co * p.s_co + kk[0] * p.s_kz + kk[1] * p.s_ky + kk[2] * p.s_kx + c * p.s_c]
+                                           : static_cast<uint16_t>(0);
+  }
+  __syncthreads();
+  // per dimension: this position's phase, its tap index inside the phase, the phase's tap count and the taps before it
+  uint32_t t[3], n[3], pre[3];
+  for (int i = 0; i < 3; ++i) {
+    const uint32_t r = (kk[i] * p.d[i] + p.s[i] * p.p[i] - p.p[i]) % p.s[i];
+    t[i] = (p.kmax[i][r] - kk[i]) / p.q[i];
+    n[i] = p.taps[i][r];
+    pre[i] = 0;
+    for (uint32_t j = 0; j < r; ++j) pre[i] += p.taps[i][j];
+  }
+  const uint64_t blk = p.C * p.cp *
+      (static_cast<uint64_t>(pre[0]) * khw + static_cast<uint64_t>(n[0]) * (static_cast<uint64_t>(pre[1]) * p.k[2] + static_cast<uint64_t>(n[1]) * pre[2]));
+  const uint64_t base = blk + ((static_cast<uint64_t>(t[0]) * n[1] + t[1]) * n[2] + t[2]) * p.cp;
+  const uint64_t c_pitch = static_cast<uint64_t>(n[0]) * n[1] * n[2] * p.cp;
+  uint16_t* out = reinterpret_cast<uint16_t*>(p.out);
+  for (uint32_t r = ty; r < 32; r += 8) {
+    const uint64_t c = c0 + r, co = co0 + tx;
+    if (c < p.C && co < p.cp) out[base + c * c_pitch + co] = tile[tx][r];
+  }
+}

@@ -51,6 +51,8 @@ extern const unsigned char b200_cubin_gemm_convbwd[];
 extern const unsigned char b200_cubin_gemm_convbwd_end[];
 extern const unsigned char b200_cubin_conv_grouped[];
 extern const unsigned char b200_cubin_conv_grouped_end[];
+extern const unsigned char b200_cubin_gemm_conv3d[];
+extern const unsigned char b200_cubin_gemm_conv3d_end[];
 }
 
 // ================================================================================================ errors
@@ -322,13 +324,15 @@ static int get_func(b200_ctx* c, const std::string& name, CUfunction* out) {
   auto it = c->funcs.find(name);
   if (it != c->funcs.end()) { *out = it->second; return B200_OK; }
   // modules are loaded in the order gemm, reduce, aux, gemm_b, gemm_c, quant, gemm_q, quant_mm, gemm_conv, gemm_convbwd,
-  // conv_grouped; the kernel
+  // conv_grouped, gemm_conv3d; the kernel
   // name says where a
   // kernel lives (no failing lookups, which API-level tools such as compute-sanitizer would report)
   auto starts = [&](const char* pfx) { return name.rfind(pfx, 0) == 0; };
   auto has = [&](const char* part) { return name.find(part) != std::string::npos; };
   const bool tc_gemm = starts("gemm_") && name != "gemm_simt_strided" && name != "gemm_scaled_simt";
-  const size_t home = starts("conv2d_grp_") ? 10
+  const size_t home = name == "conv3d_dgrad_weights" ? 2
+                      : starts("conv3d_") ? 11
+                      : starts("conv2d_grp_") ? 10
                       : starts("conv2d_dgrad_") || starts("conv2d_wgrad_") ? 9
                       : starts("conv2d_") ? 8
                       : starts("gemm_q8") ? 6
@@ -363,7 +367,8 @@ extern "C" int b200_get_cubin(const char* name, const void** image, size_t* size
   else if (!strcmp(name, "gemm_conv")) { b = b200_cubin_gemm_conv; e = b200_cubin_gemm_conv_end; }
   else if (!strcmp(name, "gemm_convbwd")) { b = b200_cubin_gemm_convbwd; e = b200_cubin_gemm_convbwd_end; }
   else if (!strcmp(name, "conv_grouped")) { b = b200_cubin_conv_grouped; e = b200_cubin_conv_grouped_end; }
-  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd|conv_grouped)", name);
+  else if (!strcmp(name, "gemm_conv3d")) { b = b200_cubin_gemm_conv3d; e = b200_cubin_gemm_conv3d_end; }
+  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd|conv_grouped|gemm_conv3d)", name);
   *image = b;
   *size = static_cast<size_t>(e - b);
   return B200_OK;
@@ -421,7 +426,8 @@ extern "C" int b200_init(int device, b200_ctx** out) {
       (rc = load_module(c, b200_cubin_quant_mm, b200_cubin_quant_mm_end, "quant_mm")) ||
       (rc = load_module(c, b200_cubin_gemm_conv, b200_cubin_gemm_conv_end, "gemm_conv")) ||
       (rc = load_module(c, b200_cubin_gemm_convbwd, b200_cubin_gemm_convbwd_end, "gemm_convbwd")) ||
-      (rc = load_module(c, b200_cubin_conv_grouped, b200_cubin_conv_grouped_end, "conv_grouped"))) {
+      (rc = load_module(c, b200_cubin_conv_grouped, b200_cubin_conv_grouped_end, "conv_grouped")) ||
+      (rc = load_module(c, b200_cubin_gemm_conv3d, b200_cubin_gemm_conv3d_end, "gemm_conv3d"))) {
     for (CUmodule m : c->modules) g_drv.cuModuleUnload_p(m);
     g_drv.cuDevicePrimaryCtxRelease_p(c->dev);
     return bail(rc);
@@ -911,6 +917,50 @@ static int encode_im2col(b200_ctx* c, CUtensorMap* out, CUtensorMapDataType dt, 
   return B200_OK;
 }
 
+// 5-D im2col map of an NDHWC tensor (dims innermost first: C, W, H, D, N; strides of W, H, D, N in elements): as
+// encode_im2col with a depth dimension.  Corners (w, h, d) must lie in [-16, 15] (cuda.h, rank 5); estr_* are the conv strides.
+static int encode_im2col5(b200_ctx* c, CUtensorMap* out, CUtensorMapDataType dt, size_t esz, uint64_t base, const uint64_t dims[5],
+                          const uint64_t strides[4], const int lower[3], const int upper[3], uint32_t channels, uint32_t pixels,
+                          const uint32_t estr_whd[3]) {
+  const int promo_bytes = atoi(opt(c, "gemm.l2_promotion", "256").c_str());
+  const CUtensorMapL2promotion promo = promo_bytes >= 256 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B
+                                       : promo_bytes >= 128 ? CU_TENSOR_MAP_L2_PROMOTION_L2_128B
+                                       : promo_bytes >= 64 ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B : CU_TENSOR_MAP_L2_PROMOTION_NONE;
+  std::string key = "im2col5d|" + std::to_string((int)dt) + "|" + std::to_string(base);
+  for (int i = 0; i < 5; ++i) key += "|" + std::to_string(dims[i]);
+  for (int i = 0; i < 4; ++i) key += "|" + std::to_string(strides[i]);
+  for (int i = 0; i < 3; ++i) key += "|" + std::to_string(lower[i]) + "|" + std::to_string(upper[i]) + "|" + std::to_string(estr_whd[i]);
+  key += "|" + std::to_string(channels) + "|" + std::to_string(pixels) + "|" + std::to_string((int)promo);
+  if (c->dry) {
+    char line[400];
+    snprintf(line, sizeof(line),
+             "tmap im2col5d esz=%zu dims=(%llu,%llu,%llu,%llu,%llu) strides=(%llu,%llu,%llu,%llu) lower=(%d,%d,%d) upper=(%d,%d,%d) "
+             "channels=%u pixels=%u estrides=(1,%u,%u,%u,1) swizzle=%d\n",
+             esz, (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)dims[2], (unsigned long long)dims[3],
+             (unsigned long long)dims[4], (unsigned long long)(strides[0] * esz), (unsigned long long)(strides[1] * esz),
+             (unsigned long long)(strides[2] * esz), (unsigned long long)(strides[3] * esz), lower[0], lower[1], lower[2], upper[0],
+             upper[1], upper[2], channels, pixels, estr_whd[0], estr_whd[1], estr_whd[2], (int)CU_TENSOR_MAP_SWIZZLE_128B);
+    c->plan += line;
+    memset(out, 0, sizeof(*out));
+    return B200_OK;
+  }
+  auto it = c->tmap_cache.find(key);
+  if (it != c->tmap_cache.end()) { *out = it->second; return B200_OK; }
+  cuuint64_t gdim[5] = {dims[0], dims[1], dims[2], dims[3], dims[4]};
+  cuuint64_t gstr[4] = {strides[0] * esz, strides[1] * esz, strides[2] * esz, strides[3] * esz};
+  cuuint32_t estr[5] = {1, estr_whd[0], estr_whd[1], estr_whd[2], 1};
+  CUresult r = g_drv.cuTensorMapEncodeIm2col_p(out, dt, 5, reinterpret_cast<void*>(base), gdim, gstr, lower, upper, channels, pixels, estr,
+                                               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, promo,
+                                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS)
+    return fail(B200_ERR_INVALID_ARG, "cuTensorMapEncodeIm2col (rank 5) failed: %s (dims %llu,%llu,%llu,%llu,%llu corners (%d,%d,%d)..(%d,%d,%d))",
+                cu_err(r), (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)dims[2], (unsigned long long)dims[3],
+                (unsigned long long)dims[4], lower[0], lower[1], lower[2], upper[0], upper[1], upper[2]);
+  if (c->tmap_cache.size() > 512) c->tmap_cache.clear();
+  c->tmap_cache[key] = *out;
+  return B200_OK;
+}
+
 // Geometry of a 2-D convolution run as an implicit GEMM (b200_conv2d): x is NHWC with unit channel stride, w is
 // [Cout, KH * KW, C] with unit channel stride; strides in elements.
 struct ConvGeom {
@@ -927,6 +977,12 @@ struct ConvGeom {
   int mode = 0;
   uint64_t dx_sn = 0, dx_si = 0, dx_sj = 0;
   uint64_t dw_sp = 0, dw_c = 0;
+  // 3-D convolution (b200_conv3d*): dims = 3 adds a depth dimension to everything above (x strides x_sd, a pixel box corner
+  // lo_d, dx stride dx_sd per phase row).  The defaults leave every 2-D path as it is.
+  int dims = 2;
+  uint64_t D = 1, KD = 1, OD = 1;
+  int32_t sd = 1, pd = 0, dd = 1, lo_d = 0;
+  uint64_t x_sd = 0, dx_sd = 0;
 };
 
 // One batched problem with LINEAR batch strides (0 = broadcast).  Strides in elements.
@@ -1125,7 +1181,9 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
   const GemmVariant& v = *best;
 
   const int cmode = g.conv ? g.conv->mode : 0;
-  const std::string name = g.conv ? std::string(cmode == 1 ? "conv2d_dgrad_" : cmode == 2 ? "conv2d_wgrad_" : "conv2d_") + in_tag + "_" + out_tag + "_" + v.tag
+  const bool cv3 = g.conv && g.conv->dims == 3;
+  const std::string cpfx = cv3 ? "conv3d_" : "conv2d_";
+  const std::string name = g.conv ? cpfx + (cmode == 1 ? "dgrad_" : cmode == 2 ? "wgrad_" : "") + in_tag + "_" + out_tag + "_" + v.tag
                                   : std::string("gemm_") + in_tag + "_" + out_tag + "_" + v.tag + (a_mn ? "_m" : "_k") + (b_mn ? "n" : "k");
   CUfunction f;
   int rc = get_func(c, name, &f);
@@ -1146,6 +1204,17 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
   // grid reads at kernel position (0, 0)
   auto conv_im2col = [&](CUtensorMap* m, uint64_t base, uint32_t pixels) {
     const ConvGeom& cv = *g.conv;
+    if (cv.dims == 3) {
+      const uint64_t dims5[5] = {cv.C, cv.W, cv.H, cv.D, cv.N}, strides4[4] = {cv.x_sw, cv.x_sh, cv.x_sd, cv.x_sn};
+      int lo[3] = {-cv.pw, -cv.ph, -cv.pd};
+      int up[3] = {cv.pw - cv.dw * (int)(cv.KW - 1), cv.ph - cv.dh * (int)(cv.KH - 1), cv.pd - cv.dd * (int)(cv.KD - 1)};
+      if (cv.box) {
+        lo[0] = cv.lo_w; lo[1] = cv.lo_h; lo[2] = cv.lo_d;
+        up[0] = cv.lo_w + (int)cv.OW - (int)cv.W; up[1] = cv.lo_h + (int)cv.OH - (int)cv.H; up[2] = cv.lo_d + (int)cv.OD - (int)cv.D;
+      }
+      const uint32_t estr[3] = {(uint32_t)cv.sw, (uint32_t)cv.sh, (uint32_t)cv.sd};
+      return encode_im2col5(c, m, dt, esz, base, dims5, strides4, lo, up, 64, pixels, estr);
+    }
     const uint64_t dims[4] = {cv.C, cv.W, cv.H, cv.N}, strides[3] = {cv.x_sw, cv.x_sh, cv.x_sn};
     int lower[2] = {-cv.pw, -cv.ph};
     int upper[2] = {cv.pw - cv.dw * (int)(cv.KW - 1), cv.ph - cv.dh * (int)(cv.KH - 1)};
@@ -1171,7 +1240,7 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
   } else if (g.conv) {
     // [n_local output channels x 64 channels] of one kernel position
     const ConvGeom& cv = *g.conv;
-    rc = encode_tmap(c, &tb, dt, esz, g.b, cv.C, cv.KH * cv.KW, cv.Cout, cv.w_sp, cv.w_sco, 64, 1, CU_TENSOR_MAP_SWIZZLE_128B, n_local);
+    rc = encode_tmap(c, &tb, dt, esz, g.b, cv.C, cv.KD * cv.KH * cv.KW, cv.Cout, cv.w_sp, cv.w_sco, 64, 1, CU_TENSOR_MAP_SWIZZLE_128B, n_local);
   } else if (!b_mn) {
     const uint64_t b_sn = g.N > 1 ? g.b_sn : pad16(g.K);
     rc = encode_tmap(c, &tb, dt, esz, g.b, g.K, g.N, b_bcast ? 1 : g.batch, b_sn, b_bcast ? b_sn * g.N : g.b_sb, block_k, n_local);
@@ -1231,6 +1300,11 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
     p.cv_dil_h = (uint32_t)cv.dh; p.cv_dil_w = (uint32_t)cv.dw;
     p.dx_sn = cv.dx_sn; p.dx_si = cv.dx_si; p.dx_sj = cv.dx_sj;
     p.dw_sp = cv.dw_sp; p.dw_c = (uint32_t)cv.dw_c;
+    if (cv.dims == 3) {
+      p.cv_odhw = (uint32_t)(cv.OD * cv.OH * cv.OW); p.cv_khw = (uint32_t)(cv.KH * cv.KW);
+      p.cv_stride_d = cv.sd; p.cv_pad_d = cv.pd; p.cv_dil_d = (uint32_t)cv.dd;
+      p.dx_sd = cv.dx_sd;
+    }
   }
   p.q_ga = g.q_ga; p.q_gb = g.q_gb;
   p.alpha = g.alpha; p.bias = g.bias; p.epi_act = g.act;
@@ -1245,7 +1319,7 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
   p.a_bmul = a_bcast ? 0 : 1;
   p.b_bmul = b_bcast ? 0 : 1;
   p.vec_store = (g.out % 16 == 0 && (g.o_sm * osz) % 16 == 0 && (g.o_sb * osz) % 16 == 0) ? 1 : 0;
-  if (cmode == 1 && ((p.dx_sn * osz) % 16 || (p.dx_si * osz) % 16 || (p.dx_sj * osz) % 16)) p.vec_store = 0;
+  if (cmode == 1 && ((p.dx_sn * osz) % 16 || (p.dx_si * osz) % 16 || (p.dx_sj * osz) % 16 || (p.dx_sd * osz) % 16)) p.vec_store = 0;
   if (cmode == 2 && (p.dw_sp * osz) % 16) p.vec_store = 0;
   // whole tiles leave through swizzled staging tiles and TMA stores when `out` is describable: (N, M, batch), [128 B x 64 rows] boxes
   const std::string epi = opt(c, "gemm.epilogue", "tma");
@@ -1254,10 +1328,10 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
   memset(&tout, 0, sizeof(tout));
   const uint64_t lim40 = 1ull << 40;
   if (cmode == 2 && p.vec_store && epi == "tma" && g.o_sm * osz < lim40 && p.dw_sp * osz < lim40) {
-    // dw as (C, Cout, KH * KW): a staging tile of 64-column chunk (kpos, ch0) lands at (ch0, co, kpos), clipped at C
+    // dw as (C, Cout, KD * KH * KW): a staging tile of 64-column chunk (kpos, ch0) lands at (ch0, co, kpos), clipped at C
     const ConvGeom& cv = *g.conv;
     rc = encode_tmap(c, &tout, osz == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_UINT16, osz, g.out, cv.dw_c, g.M,
-                     cv.KH * cv.KW, g.o_sm, cv.dw_sp, static_cast<uint32_t>(128 / osz), 64);
+                     cv.KD * cv.KH * cv.KW, g.o_sm, cv.dw_sp, static_cast<uint32_t>(128 / osz), 64);
     if (rc) return rc;
     p.tma_store = 1;
   } else if (cmode == 0 && p.vec_store && epi == "tma" && g.o_sm * osz < lim40 && g.o_sb * osz < lim40 && (g.M == 1 || g.o_sm >= g.N)) {
@@ -3012,6 +3086,381 @@ extern "C" int b200_conv2d_backward_weight(b200_ctx* c, b200_stream s, b200_dtyp
     gp.a_sm = 1; gp.a_sk = yo.s_w; gp.b_sn = 1; gp.b_sk = xo.s_w;   // both operands MN-major
     // few tiles, a long K: the stream-K head may cut a tile into as many ranges as fill the SMs, each >= 8 k-blocks
     gp.sk_max_parts = std::max<uint64_t>(8, (P + 63) / 64 / 8);
+    rc = launch_wgmma(c, st, gp, true, true);
+  }
+  for (CUdeviceptr t : tmp)
+    if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMM has drained
+  return rc;
+}
+
+// ------------------------------------------------------------------------------------------------ 3-D convolution
+// b200_conv3d*: the 2-D machinery with a depth dimension.  Arrays over the spatial dimensions are ordered (D, H, W).
+// Rank-5 tensor maps take pixel-box corners in [-16, 15] (cuda.h: cuTensorMapEncodeIm2col) and the load's im2col offsets
+// in [0, 31] (5 bits each; PTX ISA, cp.async.bulk.tensor im2col mode).
+static constexpr int64_t kIm2col5Lo = -16, kIm2col5Hi = 15, kIm2col5MaxOffset = 31;
+
+// Strides of a rank-5 view with extent-1 dimensions normalised (see conv_norm_strides).
+static void conv3_norm_strides(const uint64_t* shape, const uint64_t* strides, uint64_t* out) {
+  uint64_t inner = 1;
+  for (int d = 4; d >= 0; --d) {
+    out[d] = strides ? strides[d] : inner;
+    if (shape[d] == 1) out[d] = inner;
+    inner = out[d] * shape[d];
+  }
+}
+
+// (D, H, W) = dimensions 1..3 of a rank-5 view as one strided dimension: its stride, or 0.
+static uint64_t conv3_flat_dhw(const uint64_t* shape, const uint64_t* ns) {
+  const uint64_t s_hw = conv_flat_stride(shape[2], shape[3], ns[2], ns[3]);
+  return s_hw == 0 ? 0 : conv_flat_stride(shape[1], shape[2] * shape[3], ns[1], s_hw);
+}
+
+// conv_check_args for the 3-D args: dtypes, activation, strides / dilations >= 1, padding >= 0, channels.
+static int conv3_check_args(const char* what, b200_dtype in_dtype, b200_dtype out_dtype, const b200_conv3d_args& a, const b200_epilogue* ep,
+                            uint64_t in_c, uint64_t w_c) {
+  const b200_conv2d_args hw{a.stride_h, a.stride_w, a.pad_h, a.pad_w, a.dilation_h, a.dilation_w};
+  if (a.stride_d < 1 || a.dilation_d < 1 || a.pad_d < 0)
+    return fail(B200_ERR_INVALID_ARG, "%s: strides and dilations must be >= 1 and padding >= 0", what);
+  return conv_check_args(what, in_dtype, out_dtype, hw, ep, in_c, w_c);
+}
+
+// Extents < 2^31, then PyTorch's output rule per dimension: y must be [N, OD, OH, OW, Cout] for in [N, D, H, W, C] and
+// w [Cout, KD, KH, KW, *].  O receives (OD, OH, OW).
+static int conv3_check_shape(const char* what, const b200_conv3d_args& a, const uint64_t* in, const uint64_t* w, const uint64_t* y,
+                             const char* y_name, uint64_t O[3]) {
+  const uint64_t lim = 1ull << 31;
+  for (int d = 0; d < 5; ++d)
+    if (in[d] >= lim || w[d] >= lim || y[d] >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: extents must be < 2^31", what);
+  if (w[1] == 0 || w[2] == 0 || w[3] == 0) return B200_OK;
+  const int64_t s[3] = {a.stride_d, a.stride_h, a.stride_w}, p[3] = {a.pad_d, a.pad_h, a.pad_w};
+  const int64_t dl[3] = {a.dilation_d, a.dilation_h, a.dilation_w};
+  for (int i = 0; i < 3; ++i) {
+    const int64_t n = (int64_t)in[1 + i] + 2 * p[i] - dl[i] * ((int64_t)w[1 + i] - 1) - 1;
+    if (n < 0) return fail(B200_ERR_INVALID_ARG, "%s: the dilated kernel is larger than the padded input (output extent < 1)", what);
+    O[i] = (uint64_t)(n / s[i]) + 1;
+  }
+  if (y[0] != in[0] || y[1] != O[0] || y[2] != O[1] || y[3] != O[2] || y[4] != w[0])
+    return fail(B200_ERR_INVALID_ARG, "%s: %s is [%llu,%llu,%llu,%llu,%llu], expected [%llu,%llu,%llu,%llu,%llu]", what, y_name,
+                (unsigned long long)y[0], (unsigned long long)y[1], (unsigned long long)y[2], (unsigned long long)y[3],
+                (unsigned long long)y[4], (unsigned long long)in[0], (unsigned long long)O[0], (unsigned long long)O[1],
+                (unsigned long long)O[2], (unsigned long long)w[0]);
+  return B200_OK;
+}
+
+// The rank-5 im2col limits: pixel-box corners in [-16, 15], and the largest im2col offset (dilation * (taps - 1)) of each
+// dimension in [0, 31].
+static int conv3_check_corners(const char* what, const int64_t* corners, int n) {
+  for (int i = 0; i < n; ++i)
+    if (corners[i] < kIm2col5Lo || corners[i] > kIm2col5Hi)
+      return fail(B200_ERR_UNSUPPORTED, "%s: im2col pixel-box corner %lld outside [-16, 15] (rank-5 tensor map)", what, (long long)corners[i]);
+  return B200_OK;
+}
+static int conv3_check_offsets(const char* what, const int64_t max_off[3]) {
+  for (int i = 0; i < 3; ++i)
+    if (max_off[i] > kIm2col5MaxOffset)
+      return fail(B200_ERR_UNSUPPORTED, "%s: im2col offset dilation * (kernel - 1) = %lld exceeds 31 (5-bit rank-5 offsets)", what,
+                  (long long)max_off[i]);
+  return B200_OK;
+}
+// The forward's map (also backward_weight's x): corners -p and p - d*(K-1), offsets d*(K-1), and conv strides <= 8.
+static int conv3_check_fwd(const char* what, const b200_conv3d_args& a, const uint64_t* w) {
+  const int64_t p[3] = {a.pad_d, a.pad_h, a.pad_w}, dl[3] = {a.dilation_d, a.dilation_h, a.dilation_w};
+  int64_t corners[6], off[3];
+  for (int i = 0; i < 3; ++i) {
+    off[i] = dl[i] * ((int64_t)w[1 + i] - 1);
+    corners[2 * i] = -p[i];
+    corners[2 * i + 1] = p[i] - off[i];
+  }
+  int rc = conv3_check_corners(what, corners, 6);
+  if (!rc) rc = conv3_check_offsets(what, off);
+  return rc;
+}
+static int conv3_check_stride(const char* what, const b200_conv3d_args& a) {
+  if (a.stride_d > kDgradMaxStride || a.stride_h > kDgradMaxStride || a.stride_w > kDgradMaxStride)
+    return fail(B200_ERR_UNSUPPORTED, "%s: the conv stride must be <= %d", what, kDgradMaxStride);
+  return B200_OK;
+}
+
+// An NDHWC output (out or dx): unit channel stride, one pixel pitch >= its channels across N, D, H, W.
+static int conv3_check_pixels(const char* what, const char* name, const uint64_t* shape, const uint64_t* ns) {
+  if (ns[4] != 1 || ns[3] < shape[4] || ns[2] != shape[3] * ns[3] || ns[1] != shape[2] * ns[2] || ns[0] != shape[1] * ns[1])
+    return fail(B200_ERR_UNSUPPORTED, "%s: %s must have unit channel stride and one pixel pitch >= its channels for N, D, H, W", what, name);
+  return B200_OK;
+}
+
+// An operand [N, D, H, W, C] (normalised strides ns) as the convolution maps read it; conv_prep_nhwc with a depth dimension.
+// flat: none (x, dy in the data gradient), (D, H, W) (the weights: one kernel-position stride, returned as s_w) or
+// (N, D, H, W) (dy in the weight gradient: [pixels, Cout]).
+struct NdhwcOperand {
+  uint64_t ptr, C, s_w, s_h, s_d, s_n;
+};
+static int conv3_prep(b200_ctx* c, CUstream st, b200_dtype dt, uint64_t ptr, const uint64_t* shape, const uint64_t* ns, ConvFlat flat,
+                      CUdeviceptr tmp[2], NdhwcOperand* o) {
+  const uint64_t N = shape[0], D = shape[1], H = shape[2], W = shape[3], C = shape[4];
+  const uint64_t spx = conv3_flat_dhw(shape, ns);   // (D, H, W) as one pixel dimension
+  int rc = B200_OK;
+  auto gather = [&]() -> int {
+    CUdeviceptr buf;
+    int r = pool_alloc(c, N * D * H * W * C * 2, &buf, st);
+    if (r) return r;
+    r = b200_into_contiguous(c, static_cast<b200_stream>(st), dt, ptr, buf, 5, shape, ns);
+    if (r) { pool_free(c, buf, st); return r; }
+    tmp[0] = buf;
+    return B200_OK;
+  };
+  if (C % 8 == 0) {
+    bool in_place = ptr % 16 == 0 && ns[4] == 1 && conv_al16(ns[0]);
+    if (flat == kFlatHW) in_place = in_place && spx != 0 && conv_al16(spx);
+    else in_place = in_place && conv_al16(ns[1]) && conv_al16(ns[2]) && conv_al16(ns[3]) &&
+                    (flat == kFlatNone || (ns[2] == W * ns[3] && ns[1] == H * ns[2] && ns[0] == D * ns[1]));
+    if (in_place) {
+      *o = {ptr, C, flat == kFlatHW ? spx : ns[3], ns[2], ns[1], ns[0]};
+      return B200_OK;
+    }
+    rc = gather();
+    *o = {tmp[0], C, C, W * C, H * W * C, D * H * W * C};
+    return rc;
+  }
+  const uint64_t cp = (C + 7) / 8 * 8;
+  uint64_t in = ptr, sb = ns[0], sp = spx, sc = ns[4];
+  if (spx == 0) {
+    rc = gather();
+    in = tmp[0]; sb = D * H * W * C; sp = C; sc = 1;
+  }
+  if (!rc) rc = conv_pad_channels(c, st, in, N, D * H * W, C, sb, sp, sc, cp, &tmp[1]);
+  *o = {tmp[1], cp, cp, W * cp, H * W * cp, D * H * W * cp};
+  return rc;
+}
+
+// ConvGeom of a 3-D map: input extents I = (D, H, W), kernel K, output O, per-dimension stride / pad / dilation.
+static ConvGeom conv3_geom(uint64_t N, const uint64_t I[3], uint64_t C, const uint64_t K[3], const uint64_t O[3], uint64_t Cout,
+                           const int32_t s[3], const int32_t p[3], const int32_t d[3]) {
+  ConvGeom g{};
+  g.dims = 3;
+  g.N = N; g.D = I[0]; g.H = I[1]; g.W = I[2]; g.C = C; g.KD = K[0]; g.KH = K[1]; g.KW = K[2];
+  g.OD = O[0]; g.OH = O[1]; g.OW = O[2]; g.Cout = Cout;
+  g.sd = s[0]; g.sh = s[1]; g.sw = s[2]; g.pd = p[0]; g.ph = p[1]; g.pw = p[2]; g.dd = d[0]; g.dh = d[1]; g.dw = d[2];
+  return g;
+}
+
+extern "C" int b200_conv3d(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr x, const uint64_t* x_shape,
+                           const uint64_t* x_strides, b200_dptr w, const uint64_t* w_shape, const uint64_t* w_strides, b200_dptr out,
+                           const uint64_t* out_shape, const uint64_t* out_strides, const b200_conv3d_args* args, const b200_epilogue* ep) {
+  CTX_ENTER(c);
+  const char* what = "conv3d";
+  if (!x_shape || !w_shape || !out_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
+  const b200_conv3d_args& a = *args;
+  const uint64_t N = x_shape[0], C = x_shape[4], Cout = w_shape[0];
+  const uint64_t I[3] = {x_shape[1], x_shape[2], x_shape[3]}, K[3] = {w_shape[1], w_shape[2], w_shape[3]};
+  int rc = conv3_check_args(what, in_dtype, out_dtype, a, ep, C, w_shape[4]);
+  if (rc) return rc;
+  if (N == 0 || I[0] == 0 || I[1] == 0 || I[2] == 0 || C == 0 || Cout == 0 || K[0] == 0 || K[1] == 0 || K[2] == 0) return B200_OK;
+  uint64_t O[3] = {0, 0, 0};
+  if ((rc = conv3_check_shape(what, a, x_shape, w_shape, out_shape, "out", O))) return rc;
+  if ((rc = conv3_check_fwd(what, a, w_shape)) || (rc = conv3_check_stride(what, a))) return rc;
+  const uint64_t M = N * O[0] * O[1] * O[2], lim = 1ull << 31, KK = K[0] * K[1] * K[2];
+  if (M >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * OD * OH * OW = %llu must be < 2^31", what, (unsigned long long)M);
+  if ((rc = conv_check_ptrs(what, x, w, out, "output", out_dtype))) return rc;
+  uint64_t os[5], xs[5], ws[5];
+  conv3_norm_strides(out_shape, out_strides, os);
+  if ((rc = conv3_check_pixels(what, "out", out_shape, os))) return rc;
+  if (KK * ((C + 63) / 64 * 64) >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: KD * KH * KW * C (C padded to 64) must be < 2^31", what);
+  CUstream st = resolve_stream(c, s);
+  conv3_norm_strides(x_shape, x_strides, xs);
+  conv3_norm_strides(w_shape, w_strides, ws);
+  CUdeviceptr tmp[4] = {0, 0, 0, 0};
+  NdhwcOperand xo{}, wo{};
+  rc = conv3_prep(c, st, in_dtype, x, x_shape, xs, kFlatNone, &tmp[0], &xo);
+  if (!rc) rc = conv3_prep(c, st, in_dtype, w, w_shape, ws, kFlatHW, &tmp[2], &wo);
+  if (!rc) {
+    const int32_t sv[3] = {a.stride_d, a.stride_h, a.stride_w}, pv[3] = {a.pad_d, a.pad_h, a.pad_w};
+    const int32_t dv[3] = {a.dilation_d, a.dilation_h, a.dilation_w};
+    ConvGeom g = conv3_geom(N, I, xo.C, K, O, Cout, sv, pv, dv);
+    g.x_sw = xo.s_w; g.x_sh = xo.s_h; g.x_sd = xo.s_d; g.x_sn = xo.s_n;
+    g.w_sp = wo.s_w; g.w_sco = wo.s_n;
+    GemmProblem gp = conv_problem(in_dtype, out_dtype, xo.ptr, wo.ptr, out, M, Cout, KK * ((g.C + 63) / 64 * 64), os[3], &g);
+    if (ep) { gp.alpha = ep->alpha; gp.bias = ep->bias; gp.act = (uint32_t)ep->activation; }
+    rc = launch_wgmma(c, st, gp, false, false);
+  }
+  for (CUdeviceptr t : tmp)
+    if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMM has drained
+  return rc;
+}
+
+extern "C" int b200_conv3d_backward_data(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr dy,
+                                         const uint64_t* dy_shape, const uint64_t* dy_strides, b200_dptr w, const uint64_t* w_shape,
+                                         const uint64_t* w_strides, b200_dptr dx, const uint64_t* dx_shape, const uint64_t* dx_strides,
+                                         const b200_conv3d_args* args) {
+  CTX_ENTER(c);
+  const char* what = "conv3d_backward_data";
+  if (!dy_shape || !w_shape || !dx_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
+  const b200_conv3d_args& a = *args;
+  const uint64_t N = dx_shape[0], C = dx_shape[4], Cout = w_shape[0];
+  const uint64_t I[3] = {dx_shape[1], dx_shape[2], dx_shape[3]}, K[3] = {w_shape[1], w_shape[2], w_shape[3]};
+  const int64_t sv[3] = {a.stride_d, a.stride_h, a.stride_w}, pv[3] = {a.pad_d, a.pad_h, a.pad_w};
+  const int64_t dv[3] = {a.dilation_d, a.dilation_h, a.dilation_w};
+  uint64_t O[3] = {0, 0, 0};
+  int rc = conv3_check_args(what, in_dtype, out_dtype, a, nullptr, C, w_shape[4]);
+  if (!rc) rc = conv3_check_shape(what, a, dx_shape, w_shape, dy_shape, "dy", O);
+  if (!rc && K[0] && K[1] && K[2]) rc = conv3_check_stride(what, a);
+  if (rc) return rc;
+  if (N == 0 || I[0] == 0 || I[1] == 0 || I[2] == 0 || C == 0) return B200_OK;   // no dx
+  const uint64_t lim = 1ull << 31, P = N * I[0] * I[1] * I[2], KK = K[0] * K[1] * K[2];
+  if (P >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * D * H * W = %llu must be < 2^31", what, (unsigned long long)P);
+  if (KK * ((Cout + 63) / 64 * 64) >= lim)
+    return fail(B200_ERR_UNSUPPORTED, "%s: KD * KH * KW * Cout (Cout padded to 64) must be < 2^31", what);
+  // phases of each dimension, and the im2col limits of every phase that runs
+  std::vector<DgradPhase1D> ph[3];
+  for (int i = 0; i < 3; ++i)
+    for (int64_t r = 0; r < sv[i]; ++r) ph[i].push_back(dgrad_phase(I[i], K[i], sv[i], pv[i], dv[i], (uint32_t)r));
+  bool zero_phase = false;
+  for (const DgradPhase1D& pd : ph[0])
+    for (const DgradPhase1D& phh : ph[1])
+      for (const DgradPhase1D& pw : ph[2]) {
+        const DgradPhase1D* q[3] = {&pd, &phh, &pw};
+        if (!pd.extent || !phh.extent || !pw.extent) continue;
+        if (!pd.taps || !phh.taps || !pw.taps || Cout == 0) { zero_phase = true; continue; }
+        int64_t corners[6], off[3];
+        for (int i = 0; i < 3; ++i) {
+          corners[2 * i] = q[i]->e0;
+          corners[2 * i + 1] = q[i]->e0 + (int64_t)q[i]->extent - (int64_t)O[i];
+          off[i] = (int64_t)(q[i]->taps - 1) * q[i]->dil;
+        }
+        if ((rc = conv3_check_corners(what, corners, 6)) || (rc = conv3_check_offsets(what, off))) return rc;
+      }
+  if ((rc = conv_check_ptrs(what, dy, w, dx, "dx", out_dtype))) return rc;
+  const size_t osz = dtype_size(out_dtype);
+  uint64_t os[5], ys[5], ws[5];
+  conv3_norm_strides(dx_shape, dx_strides, os);
+  if ((rc = conv3_check_pixels(what, "dx", dx_shape, os))) return rc;
+  CUstream st = resolve_stream(c, s);
+  // dx pixels that no tap reaches are exact zeros: one memset of dx, before the phases that overwrite the rest
+  if (zero_phase) {
+    rc = memset2d_zero(c, st, dx, osz, os[3], C, P);
+    if (rc) return rc;
+  }
+  if (Cout == 0 || KK == 0) return B200_OK;
+  conv3_norm_strides(dy_shape, dy_strides, ys);
+  conv3_norm_strides(w_shape, w_strides, ws);
+  CUdeviceptr tmp[3] = {0, 0, 0};
+  NdhwcOperand y{};
+  rc = conv3_prep(c, st, in_dtype, dy, dy_shape, ys, kFlatNone, tmp, &y);
+  // every phase's flipped, channel-transposed weights [C][Td][Th][Tw][cp] in one pooled buffer of |w| * cp / Cout elements, in
+  // (rd, rh, rw) order (Conv3dDgradWeightsParams)
+  const uint64_t cp = y.C;
+  Conv3dDgradWeightsParams wp;
+  memset(&wp, 0, sizeof(wp));
+  uint64_t pre[3][kDgradMaxStride];
+  for (int i = 0; i < 3; ++i) {
+    uint64_t acc = 0;
+    for (const DgradPhase1D& q : ph[i]) { pre[i][q.r] = acc; acc += q.taps; wp.kmax[i][q.r] = q.kmax; wp.taps[i][q.r] = q.taps; }
+    wp.k[i] = (uint32_t)K[i]; wp.s[i] = (uint32_t)sv[i]; wp.d[i] = (uint32_t)dv[i]; wp.p[i] = (uint32_t)pv[i]; wp.q[i] = ph[i][0].step;
+  }
+  auto phase_off = [&](uint32_t rd, uint32_t rh, uint32_t rw) {
+    return C * cp * (pre[0][rd] * K[1] * K[2] + (uint64_t)wp.taps[0][rd] * (pre[1][rh] * K[2] + (uint64_t)wp.taps[1][rh] * pre[2][rw]));
+  };
+  if (!rc) rc = pool_alloc(c, KK * C * cp * 2, &tmp[2], st);
+  if (!rc) {
+    wp.w = w; wp.out = tmp[2];
+    wp.s_co = ws[0]; wp.s_kz = ws[1]; wp.s_ky = ws[2]; wp.s_kx = ws[3]; wp.s_c = ws[4];
+    wp.C = C; wp.Cout = Cout; wp.cp = cp;
+    CUfunction f;
+    rc = get_func(c, "conv3d_dgrad_weights", &f);
+    void* kargs[] = {&wp};
+    if (!rc) rc = launch(c, f, (unsigned)(((C + 31) / 32) * ((cp + 31) / 32)), (unsigned)KK, 1, 256, 0, 1, st, kargs);
+  }
+  // one stride-1 convolution of dy per phase that has taps and pixels
+  const bool stride1 = sv[0] == 1 && sv[1] == 1 && sv[2] == 1;
+  for (const DgradPhase1D& pd : ph[0])
+    for (const DgradPhase1D& phh : ph[1])
+      for (const DgradPhase1D& pw : ph[2]) {
+        if (rc) break;
+        const DgradPhase1D* q[3] = {&pd, &phh, &pw};
+        if (!pd.extent || !phh.extent || !pw.extent || !pd.taps || !phh.taps || !pw.taps) continue;
+        const uint64_t T[3] = {pd.taps, phh.taps, pw.taps}, E[3] = {pd.extent, phh.extent, pw.extent};
+        const int32_t one[3] = {1, 1, 1}, pp[3] = {(int32_t)-pd.e0, (int32_t)-phh.e0, (int32_t)-pw.e0};
+        const int32_t dil[3] = {(int32_t)pd.dil, (int32_t)phh.dil, (int32_t)pw.dil};
+        ConvGeom g = conv3_geom(N, O, cp, T, E, C, one, pp, dil);
+        g.x_sw = y.s_w; g.x_sh = y.s_h; g.x_sd = y.s_d; g.x_sn = y.s_n;
+        g.w_sp = cp; g.w_sco = T[0] * T[1] * T[2] * cp;
+        g.box = true; g.lo_d = (int32_t)pd.e0; g.lo_h = (int32_t)phh.e0; g.lo_w = (int32_t)pw.e0;
+        g.mode = stride1 ? 0 : 1;
+        g.dx_sn = os[0]; g.dx_sd = (uint64_t)sv[0] * os[1]; g.dx_si = (uint64_t)sv[1] * os[2]; g.dx_sj = (uint64_t)sv[2] * os[3];
+        if (c->dry) {
+          std::string line = "conv3d dgrad phase r=(" + std::to_string(pd.r) + "," + std::to_string(phh.r) + "," + std::to_string(pw.r) + ")";
+          const char* tn[3] = {" taps_d=", " taps_h=", " taps_w="};
+          for (int i = 0; i < 3; ++i) {
+            line += tn[i];
+            for (uint32_t t = 0; t < q[i]->taps; ++t) line += (t ? "," : "") + std::to_string(q[i]->kmax - t * q[i]->step);
+          }
+          auto triple = [&](auto f) { return "(" + std::to_string(f(0)) + "," + std::to_string(f(1)) + "," + std::to_string(f(2)) + ")"; };
+          line += " dil=" + triple([&](int i) { return (int64_t)q[i]->dil; });
+          line += " lower=" + triple([&](int i) { return q[i]->e0; });
+          line += " upper=" + triple([&](int i) { return q[i]->e0 + (int64_t)q[i]->extent - (int64_t)O[i]; });
+          line += " extent=" + triple([&](int i) { return (int64_t)q[i]->extent; }) + "\n";
+          c->plan += line;
+        }
+        const GemmProblem gp = conv_problem(in_dtype, out_dtype, y.ptr, tmp[2] + phase_off(pd.r, phh.r, pw.r) * 2,
+                                            dx + ((uint64_t)pd.r * os[1] + (uint64_t)phh.r * os[2] + (uint64_t)pw.r * os[3]) * osz,
+                                            N * E[0] * E[1] * E[2], C, T[0] * T[1] * T[2] * ((cp + 63) / 64 * 64), os[3], &g);
+        rc = launch_wgmma(c, st, gp, false, false);
+      }
+  for (CUdeviceptr t : tmp)
+    if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMMs have drained
+  return rc;
+}
+
+extern "C" int b200_conv3d_backward_weight(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr x,
+                                           const uint64_t* x_shape, const uint64_t* x_strides, b200_dptr dy, const uint64_t* dy_shape,
+                                           const uint64_t* dy_strides, b200_dptr dw, const uint64_t* dw_shape, const uint64_t* dw_strides,
+                                           const b200_conv3d_args* args) {
+  CTX_ENTER(c);
+  const char* what = "conv3d_backward_weight";
+  if (!x_shape || !dy_shape || !dw_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
+  const b200_conv3d_args& a = *args;
+  const uint64_t N = x_shape[0], C = x_shape[4], Cout = dw_shape[0];
+  const uint64_t I[3] = {x_shape[1], x_shape[2], x_shape[3]}, K[3] = {dw_shape[1], dw_shape[2], dw_shape[3]};
+  uint64_t O[3] = {0, 0, 0};
+  int rc = conv3_check_args(what, in_dtype, out_dtype, a, nullptr, C, dw_shape[4]);
+  if (!rc) rc = conv3_check_shape(what, a, x_shape, dw_shape, dy_shape, "dy", O);
+  if (!rc && K[0] && K[1] && K[2]) rc = conv3_check_stride(what, a);
+  if (rc) return rc;
+  const uint64_t KK = K[0] * K[1] * K[2];
+  if (Cout == 0 || C == 0 || KK == 0) return B200_OK;   // no dw
+  if ((rc = conv3_check_fwd(what, a, dw_shape))) return rc;   // x is read through the forward's map
+  const uint64_t P = N * O[0] * O[1] * O[2], lim = 1ull << 31;
+  if (P >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * OD * OH * OW = %llu must be < 2^31", what, (unsigned long long)P);
+  const uint64_t cx = (C + 7) / 8 * 8;
+  if (KK * ((cx + 63) / 64 * 64) >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: KD * KH * KW * C (C padded to 64) must be < 2^31", what);
+  if ((rc = conv_check_ptrs(what, x, dy, dw, "dw", out_dtype))) return rc;
+  const size_t osz = dtype_size(out_dtype);
+  uint64_t ds[5], xs[5], ys[5];
+  conv3_norm_strides(dw_shape, dw_strides, ds);
+  const uint64_t dw_sp = conv3_flat_dhw(dw_shape, ds);
+  if (ds[4] != 1 || dw_sp == 0 || ds[0] * osz >= (1ull << 40) || dw_sp * osz >= (1ull << 40))
+    return fail(B200_ERR_UNSUPPORTED, "%s: dw must have unit channel stride and (KD, KH, KW) flattening into one stride", what);
+  CUstream st = resolve_stream(c, s);
+  if (P == 0) {
+    // no pixels: dw is exactly zero
+    if (ds[0] == KK * dw_sp) return memset2d_zero(c, st, dw, osz, dw_sp, C, Cout * KK);
+    for (uint64_t co = 0; co < Cout && !rc; ++co) rc = memset2d_zero(c, st, dw + co * ds[0] * osz, osz, dw_sp, C, KK);
+    return rc;
+  }
+  conv3_norm_strides(x_shape, x_strides, xs);
+  conv3_norm_strides(dy_shape, dy_strides, ys);
+  CUdeviceptr tmp[4] = {0, 0, 0, 0};
+  NdhwcOperand xo{}, yo{};
+  rc = conv3_prep(c, st, in_dtype, x, x_shape, xs, kFlatNone, &tmp[0], &xo);
+  if (!rc) rc = conv3_prep(c, st, in_dtype, dy, dy_shape, ys, kFlatNHW, &tmp[2], &yo);
+  if (!rc) {
+    const int32_t sv[3] = {a.stride_d, a.stride_h, a.stride_w}, pv[3] = {a.pad_d, a.pad_h, a.pad_w};
+    const int32_t dv[3] = {a.dilation_d, a.dilation_h, a.dilation_w};
+    ConvGeom g = conv3_geom(N, I, xo.C, K, O, Cout, sv, pv, dv);
+    g.x_sw = xo.s_w; g.x_sh = xo.s_h; g.x_sd = xo.s_d; g.x_sn = xo.s_n;
+    g.mode = 2; g.dw_sp = dw_sp; g.dw_c = C;
+    GemmProblem gp = conv_problem(in_dtype, out_dtype, yo.ptr, xo.ptr, dw, Cout, KK * ((xo.C + 63) / 64 * 64), P, ds[0], &g);
+    gp.a_sm = 1; gp.a_sk = yo.s_w; gp.b_sn = 1; gp.b_sk = xo.s_w;   // both operands MN-major
+    gp.sk_max_parts = std::max<uint64_t>(8, (P + 63) / 64 / 8);      // as b200_conv2d_backward_weight
     rc = launch_wgmma(c, st, gp, true, true);
   }
   for (CUdeviceptr t : tmp)

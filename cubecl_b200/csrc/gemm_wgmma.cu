@@ -153,9 +153,12 @@ enum : int { QM_NONE = 0, QM_BLOCK = 1, QM_TENSOR = 2 };
 //             [64 pixel rows x 128 B], exactly an MN-major B chunk.  Pixels past N * OH * OW read as zero on both sides (tiled
 //             out-of-bounds fill for dy; the im2col walk runs into image N for x).  The epilogue maps virtual column
 //             (kpos, ch) to dw's column and drops ch >= C, in the direct stores and in the TMA-store coordinate.
+// CONV_DIMS (capi.cpp: b200_conv3d*): 3 runs the CONV producer, CB_DGRAD epilogue and CB_WGRAD producer over a 3-D convolution
+// -- 5-D im2col loads (C, W, H, D, N) with offsets (kx dw, ky dh, kz dd), pixels and kernel positions decoded with the depth
+// term (GemmParams cv_odhw, cv_khw, dx_sd).  2 is the 2-D convolution; every other stage of the kernel is the same.
 enum : int { CB_NONE = 0, CB_DGRAD = 1, CB_WGRAD = 2 };
 template <int CG, int BLOCK_N, bool A_MN, bool B_MN, int KIND, int OUT, int STAGES, bool PROMOTE = false, int MT = 1, int QM = QM_NONE,
-          bool CONV = false, int CB = CB_NONE>
+          bool CONV = false, int CB = CB_NONE, int CONV_DIMS = 2>
 __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUtensorMap* tma_b_hi, const CUtensorMap* tma_a_lo,
                                           const CUtensorMap* tma_b_lo, const CUtensorMap* tma_out, const GemmParams& p) {
   constexpr bool INT_ACC = (KIND == KIND_U8 || KIND == KIND_S8) && QM != QM_BLOCK;
@@ -163,6 +166,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
   static_assert(!CONV || ((KIND == KIND_BF16 || KIND == KIND_F16) && !A_MN && !B_MN && !PROMOTE && MT == 1 && QM == QM_NONE),
                 "convolution: 16-bit kinds, K-major operands");
   static_assert(CB != CB_DGRAD || CONV, "data gradient: the convolution producer");
+  static_assert(CONV_DIMS == 2 || (CONV_DIMS == 3 && (CONV || CB == CB_WGRAD)), "3-D: the convolution kernels");
   static_assert(CB != CB_WGRAD || (!CONV && A_MN && B_MN && (KIND == KIND_BF16 || KIND == KIND_F16) && !PROMOTE && MT == 1 && QM == QM_NONE),
                 "weight gradient: 16-bit kinds, MN-major operands");
   // per-block scale tiles of one stage, sized for the finest block (Bk = 32: four blocks per 128-element stage)
@@ -246,12 +250,36 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
         uint32_t seg, kk;  // segment (0 unless k_segments == 3), k-block within it
         seg_of(wu.kb0, seg, kk);
         // convolution: input pixel of the tile's first row (output pixel (n, oh, ow) at kernel position (0, 0)), once per tile
-        int cv_w = 0, cv_h = 0, cv_n = 0;
-        if constexpr (CONV) {
+        int cv_w = 0, cv_h = 0, cv_d = 0, cv_n = 0;
+        if constexpr (CONV && CONV_DIMS == 3) {
+          const uint32_t mu = static_cast<uint32_t>(m0), n = mu / p.cv_odhw, r0 = mu - n * p.cv_odhw, od = r0 / p.cv_ohw;
+          const uint32_t r = r0 - od * p.cv_ohw, oh = r / p.cv_ow;
+          cv_n = static_cast<int>(n);
+          cv_d = static_cast<int>(od) * p.cv_stride_d - p.cv_pad_d;
+          cv_h = static_cast<int>(oh) * p.cv_stride_h - p.cv_pad_h;
+          cv_w = static_cast<int>(r - oh * p.cv_ow) * p.cv_stride_w - p.cv_pad_w;
+        } else if constexpr (CONV) {
           const uint32_t mu = static_cast<uint32_t>(m0), n = mu / p.cv_ohw, r = mu - n * p.cv_ohw, oh = r / p.cv_ow;
           cv_n = static_cast<int>(n);
           cv_h = static_cast<int>(oh) * p.cv_stride_h - p.cv_pad_h;
           cv_w = static_cast<int>(r - oh * p.cv_ow) * p.cv_stride_w - p.cv_pad_w;
+        }
+        // 3-D weight gradient: each B chunk's (channel block, kernel position) is fixed for the tile, decoded here once to its
+        // first channel and its im2col offsets (kx dw, ky dh, kz dd; each <= 31, packed 5 bits apart) -- decoding it per k-block
+        // needs more than the producer's 40 registers
+        int wg3_c0[NUM_CHUNKS > 0 ? NUM_CHUNKS : 1];
+        uint32_t wg3_off[NUM_CHUNKS > 0 ? NUM_CHUNKS : 1];
+        if constexpr (CB == CB_WGRAD && CONV_DIMS == 3) {
+#pragma unroll
+          for (int c = 0; c < NUM_CHUNKS; ++c) {
+            const int ci = static_cast<int>(rank) * NUM_CHUNKS + c;
+            // a chunk past N (odd chunk count) loads the last chunk again: its columns are never stored
+            const uint32_t col = min(static_cast<uint32_t>(nb0 + ci * CHUNK_N), p.N - CHUNK_N) / CHUNK_N;
+            const uint32_t kpos = col / p.cv_cblk, cb = col - kpos * p.cv_cblk;
+            const uint32_t kz = kpos / p.cv_khw, kr = kpos - kz * p.cv_khw, ky = kr / p.cv_kw, kx = kr - ky * p.cv_kw;
+            wg3_c0[c] = static_cast<int>(cb * 64u);
+            wg3_off[c] = kx * p.cv_dil_w | (ky * p.cv_dil_h) << 5 | (kz * p.cv_dil_d) << 10;
+          }
         }
         for (uint32_t kb = wu.kb0; kb < wu.kb1; ++kb) {
           mbar_wait(empty_bar(s), ph ^ 1);   // every consumer of the pair has released the stage
@@ -261,10 +289,16 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
           if constexpr (CONV) {
             mbar_arrive_expect_tx(fb, STAGE_BYTES);
             const uint32_t kpos = kb / p.cv_cblk, cb = kb - kpos * p.cv_cblk;
-            const uint32_t ky = kpos / p.cv_kw, kx = kpos - ky * p.cv_kw;
             const int c0 = static_cast<int>(cb * 64u);
-            tma_load_im2col_4d(sa, tma_a_hi, fb, c0, cv_w, cv_h, cv_n, static_cast<uint16_t>(kx * p.cv_dil_w),
-                               static_cast<uint16_t>(ky * p.cv_dil_h));
+            if constexpr (CONV_DIMS == 3) {
+              const uint32_t kz = kpos / p.cv_khw, kr = kpos - kz * p.cv_khw, ky = kr / p.cv_kw, kx = kr - ky * p.cv_kw;
+              tma_load_im2col_5d(sa, tma_a_hi, fb, c0, cv_w, cv_h, cv_d, cv_n, static_cast<uint16_t>(kx * p.cv_dil_w),
+                                 static_cast<uint16_t>(ky * p.cv_dil_h), static_cast<uint16_t>(kz * p.cv_dil_d));
+            } else {
+              const uint32_t ky = kpos / p.cv_kw, kx = kpos - ky * p.cv_kw;
+              tma_load_im2col_4d(sa, tma_a_hi, fb, c0, cv_w, cv_h, cv_n, static_cast<uint16_t>(kx * p.cv_dil_w),
+                                 static_cast<uint16_t>(ky * p.cv_dil_h));
+            }
             const int n_row = nb0 + static_cast<int>(rank * N_LOCAL);
             if constexpr (CG == 2) tma_load_3d_mc(sb + rank * N_LOCAL * 128u, tma_b_hi, fb, static_cast<uint16_t>(3), c0, static_cast<int>(kpos), n_row);
             else tma_load_3d(sb, tma_b_hi, fb, c0, static_cast<int>(kpos), n_row);
@@ -306,7 +340,25 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
 #pragma unroll
               for (int mt = 0; mt < MT; ++mt) tma_load_3d(sa + mt * A_SUB_BYTES, tma_a, fb, k0, m0 + mt * 128, ba);
             }
-            if constexpr (CB == CB_WGRAD) {
+            if constexpr (CB == CB_WGRAD && CONV_DIMS == 3) {
+              // input pixel of output pixel k0 = (n, od, oh, ow) at kernel position (0, 0, 0)
+              const uint32_t px = static_cast<uint32_t>(k0), n = px / p.cv_odhw, r0 = px - n * p.cv_odhw, od = r0 / p.cv_ohw;
+              const uint32_t r = r0 - od * p.cv_ohw, oh = r / p.cv_ow;
+              const int d = static_cast<int>(od) * p.cv_stride_d - p.cv_pad_d;
+              const int h = static_cast<int>(oh) * p.cv_stride_h - p.cv_pad_h;
+              const int w = static_cast<int>(r - oh * p.cv_ow) * p.cv_stride_w - p.cv_pad_w;
+#pragma unroll
+              for (int c = 0; c < NUM_CHUNKS; ++c) {
+                const int ci = static_cast<int>(rank) * NUM_CHUNKS + c;
+                const uint32_t o = wg3_off[c];
+                const uint16_t ow_ = static_cast<uint16_t>(o & 31u), oh_ = static_cast<uint16_t>((o >> 5) & 31u), od_ = static_cast<uint16_t>(o >> 10);
+                if constexpr (CG == 2)
+                  tma_load_im2col_5d_mc(sb + ci * CHUNK_BYTES, tma_b, fb, static_cast<uint16_t>(3), wg3_c0[c], w, h, d,
+                                        static_cast<int>(n), ow_, oh_, od_);
+                else
+                  tma_load_im2col_5d(sb + ci * CHUNK_BYTES, tma_b, fb, wg3_c0[c], w, h, d, static_cast<int>(n), ow_, oh_, od_);
+              }
+            } else if constexpr (CB == CB_WGRAD) {
               // input pixel of output pixel k0 = (n, oh, ow) at kernel position (0, 0)
               const uint32_t px = static_cast<uint32_t>(k0), n = px / p.cv_ohw, r = px - n * p.cv_ohw, oh = r / p.cv_ow;
               const int h = static_cast<int>(oh) * p.cv_stride_h - p.cv_pad_h;
@@ -518,7 +570,14 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
       };
       // data gradient: the dx addresses of this thread's two fragment rows, once per tile
       uint64_t dg_row[2] = {0, 0};
-      if constexpr (CB == CB_DGRAD) {
+      if constexpr (CB == CB_DGRAD && CONV_DIMS == 3) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const uint32_t r = m_cta + cw * 64u + wq * 16u + (lane >> 2) + 8u * h;
+          const uint32_t n = r / p.cv_odhw, r0 = r - n * p.cv_odhw, a = r0 / p.cv_ohw, rr = r0 - a * p.cv_ohw, i = rr / p.cv_ow, j = rr - i * p.cv_ow;
+          dg_row[h] = p.out + (n * p.dx_sn + a * p.dx_sd + i * p.dx_si + j * p.dx_sj) * osz;
+        }
+      } else if constexpr (CB == CB_DGRAD) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const uint32_t r = m_cta + cw * 64u + wq * 16u + (lane >> 2) + 8u * h;
@@ -748,6 +807,24 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
            const __grid_constant__ CUtensorMap tma_out, const __grid_constant__ GemmParams p) {                    \
     gemm_body<CG, BN, false, false, KIND, OUT, STAGES, false, 1, QM_NONE, true>(&tma_a, &tma_b, &tma_a_lo, &tma_b_lo, &tma_out, p); \
   }
+// 3-D convolution (CONV_DIMS = 3): 5-D im2col maps of x (forward, weight gradient) or dy (data gradient); names conv3d_*
+#define CONV3D_KERNEL(NAME, CG, BN, AMN, KIND, OUT, STAGES, CONV, CB)                                               \
+  extern "C" __global__ void __launch_bounds__(kNumThreads, 1)                                                     \
+      NAME(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,                  \
+           const __grid_constant__ CUtensorMap tma_a_lo, const __grid_constant__ CUtensorMap tma_b_lo,            \
+           const __grid_constant__ CUtensorMap tma_out, const __grid_constant__ GemmParams p) {                    \
+    gemm_body<CG, BN, AMN, AMN, KIND, OUT, STAGES, false, 1, QM_NONE, CONV, CB, 3>(&tma_a, &tma_b, &tma_a_lo, &tma_b_lo, &tma_out, p); \
+  }
+#define CONV3D_ONE(TILE, CG, BN, STAGES, IN, OUTT, KIND, OUT)                                                   \
+  CONV3D_KERNEL(conv3d_##IN##_##OUTT##_##TILE, CG, BN, false, KIND, OUT, STAGES, true, CB_NONE)                 \
+  CONV3D_KERNEL(conv3d_dgrad_##IN##_##OUTT##_##TILE, CG, BN, false, KIND, OUT, STAGES, true, CB_DGRAD)          \
+  CONV3D_KERNEL(conv3d_wgrad_##IN##_##OUTT##_##TILE, CG, BN, true, KIND, OUT, STAGES, false, CB_WGRAD)
+#define CONV3D_DTYPES(TILE, CG, BN, STAGES)                                 \
+  CONV3D_ONE(TILE, CG, BN, STAGES, bf16, bf16, KIND_BF16, OUT_BF16)          \
+  CONV3D_ONE(TILE, CG, BN, STAGES, bf16, f32, KIND_BF16, OUT_F32)            \
+  CONV3D_ONE(TILE, CG, BN, STAGES, f16, f16, KIND_F16, OUT_F16)              \
+  CONV3D_ONE(TILE, CG, BN, STAGES, f16, f32, KIND_F16, OUT_F32)
+
 #define CONV_DTYPES(TILE, CG, BN, STAGES)                                  \
   CONV_KERNEL(conv2d_bf16_bf16_##TILE, CG, BN, KIND_BF16, OUT_BF16, STAGES) \
   CONV_KERNEL(conv2d_bf16_f32_##TILE, CG, BN, KIND_BF16, OUT_F32, STAGES)   \
@@ -773,13 +850,14 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
   CONV_BWD_KERNEL(conv2d_wgrad_f16_f16_##TILE, CG, BN, true, KIND_F16, OUT_F16, STAGES, false, CB_WGRAD)       \
   CONV_BWD_KERNEL(conv2d_wgrad_f16_f32_##TILE, CG, BN, true, KIND_F16, OUT_F32, STAGES, false, CB_WGRAD)
 
-// The kernels are built as six cubins from this one source (cubecl_b200/build.py compiles them in parallel):
+// The kernels are built as seven cubins from this one source (cubecl_b200/build.py compiles them in parallel):
 //   GEMM_PART 0 ("gemm")       256 x 256 pair tiles (2-CTA cluster, 128 x 256 per CTA) and the bf16 peak probe
 //   GEMM_PART 1 ("gemm_b")     256 x 128 pair tiles, 256 x 224 block-scaled pair tiles
 //   GEMM_PART 2 ("gemm_c")     128 x 128 single-CTA tiles, 512 x 128 pair tiles
 //   GEMM_PART 3 ("gemm_q")     the quantized-operand kernels of every tile
 //   GEMM_PART 4 ("gemm_conv")  the 2-D convolution kernels of the 2sm_n128 and 1sm_n128 tiles
 //   GEMM_PART 5 ("gemm_convbwd")  the convolution backward kernels (data and weight gradients) of the same two tiles
+//   GEMM_PART 6 ("gemm_conv3d")   the 3-D convolution kernels (forward, data and weight gradients) of the same two tiles
 #ifndef GEMM_PART
 #define GEMM_PART 0
 #endif
@@ -832,6 +910,10 @@ CONV_DTYPES(1sm_n128, 1, 128, 6)
 #if GEMM_PART == 5
 CONV_BWD_DTYPES(2sm_n128, 2, 128, 6)
 CONV_BWD_DTYPES(1sm_n128, 1, 128, 6)
+#endif
+#if GEMM_PART == 6
+CONV3D_DTYPES(2sm_n128, 2, 128, 6)
+CONV3D_DTYPES(1sm_n128, 1, 128, 6)
 #endif
 
 #if GEMM_PART == 0

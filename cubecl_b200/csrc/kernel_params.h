@@ -67,6 +67,14 @@ struct GemmParams {
   // kpos = n / (cv_cblk * 64) is dw's element kpos * dw_sp + ch of row co; columns with ch >= dw_c are dropped.
   uint64_t dw_sp;
   uint32_t dw_c, dw_pad;
+  // 3-D convolution (conv3d_* kernels; capi.cpp: b200_conv3d*): GEMM row / wgrad pixel m is output pixel (n, od, oh, ow)
+  // with n = m / cv_odhw, od = (m % cv_odhw) / cv_ohw and (oh, ow) from the remainder as above; kernel position kpos is
+  // (kz, ky, kx) = (kpos / cv_khw, (kpos % cv_khw) / cv_kw, kpos % cv_kw).  The im2col maps are 5-D (C, W, H, D, N).  The
+  // data gradient's phase row (n, a, i, j) is stored at out + n * dx_sn + a * dx_sd + i * dx_si + j * dx_sj elements.
+  uint32_t cv_odhw, cv_khw;
+  int32_t cv_stride_d, cv_pad_d;
+  uint32_t cv_dil_d, cv_pad2;
+  uint64_t dx_sd;
 };
 
 // ================================================================================================ aux_kernels.cu
@@ -147,6 +155,20 @@ struct ConvDgradWeightsParams {
   uint64_t off[kDgradMaxStride * kDgradMaxStride];
   uint32_t KH, KW, sh, sw, dh, dw, ph, pw, qh, qw;
   uint32_t kmax_h[kDgradMaxStride], kmax_w[kDgradMaxStride], taps_h[kDgradMaxStride], taps_w[kDgradMaxStride];
+};
+
+// 3-D convolution data gradient (conv3d_dgrad_weights): as ConvDgradWeightsParams with a depth dimension.  Arrays are
+// indexed by dimension (0 = D, 1 = H, 2 = W) and phase.  Phase (rd, rh, rw) owns taps (kz, ky, kx) of its per-dimension
+// progressions and its block is [C][Td][Th][Tw][cp].  Blocks are laid out in (rd, rh, rw) order; as the phases of each
+// dimension partition its taps, block (rd, rh, rw) starts at element
+//   C * cp * (pre[0][rd] * KH * KW + taps[0][rd] * (pre[1][rh] * KW + taps[1][rh] * pre[2][rw])),
+// pre[i][r] = taps[i][0] + ... + taps[i][r - 1] (no per-phase offset table: up to 8^3 phases).
+struct Conv3dDgradWeightsParams {
+  uint64_t w, out;
+  uint64_t s_co, s_kz, s_ky, s_kx, s_c;   // w [Cout, KD, KH, KW, C] strides in elements
+  uint64_t C, Cout, cp;
+  uint32_t k[3], s[3], d[3], p[3], q[3], pad;
+  uint32_t kmax[3][kDgradMaxStride], taps[3][kDgradMaxStride];
 };
 
 // ================================================================================================ conv_grouped.cu

@@ -166,6 +166,31 @@ __device__ __forceinline__ void tma_load_im2col_4d_mc(uint32_t dst, const CUtens
       : "memory");
 }
 
+// 5-D im2col load of an NDHWC tensor: as tma_load_im2col_4d with one more spatial dimension, walking W, then H, then D,
+// then N; every pixel is read at (d + off_d, h + off_h, w + off_w).  The PTX ISA gives rank-5 offsets 5 bits ([0, 31]).
+__device__ __forceinline__ void tma_load_im2col_5d(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c, int w, int h, int d, int n,
+                                                   uint16_t off_w, uint16_t off_h, uint16_t off_d) {
+  asm volatile(
+      "cp.async.bulk.tensor.5d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes"
+      " [%0], [%1, {%3, %4, %5, %6, %7}], [%2], {%8, %9, %10};"
+      :
+      : "r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c), "r"(w), "r"(h), "r"(d), "r"(n), "h"(off_w), "h"(off_h),
+        "h"(off_d)
+      : "memory");
+}
+
+// Multicast 5-D im2col load (see tma_load_im2col_4d_mc).
+__device__ __forceinline__ void tma_load_im2col_5d_mc(uint32_t dst, const CUtensorMap* m, uint32_t bar, uint16_t mask, int c, int w,
+                                                      int h, int d, int n, uint16_t off_w, uint16_t off_h, uint16_t off_d) {
+  asm volatile(
+      "cp.async.bulk.tensor.5d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%4, %5, %6, %7, %8}], [%2], {%9, %10, %11}, %3;"
+      :
+      : "r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "h"(mask), "r"(c), "r"(w), "r"(h), "r"(d), "r"(n), "h"(off_w),
+        "h"(off_h), "h"(off_d)
+      : "memory");
+}
+
 // Multicast 3-D load: the box lands at the same smem offset in every CTA of `mask`, each CTA's own barrier
 // (same offset) receives the complete_tx.
 __device__ __forceinline__ void tma_load_3d_mc(uint32_t dst, const CUtensorMap* m, uint32_t bar, uint16_t mask, int c0,

@@ -427,6 +427,50 @@ int b200_conv2d_grouped_backward_weight(b200_ctx* ctx, b200_stream s, b200_dtype
                                         b200_dptr dw, const uint64_t* dw_shape, const uint64_t* dw_strides,
                                         const b200_conv2d_args* args, uint32_t groups);
 
+/* ---- 3-D convolution, forward and both gradients, an implicit GEMM on the wgmma kernel -----------------------------------
+ * out[n, od, oh, ow, co] = act(alpha * sum_{kz, ky, kx, c} x[n, od*sd - pd + kz*dd, oh*sh - ph + ky*dh, ow*sw - pw + kx*dw, c]
+ *                              * w[co, kz, ky, kx, c] + bias[co])
+ * x is [N, D, H, W, C] (NDHWC), w is [Cout, KD, KH, KW, C] (PyTorch's OIDHW weight permuted as for b200_conv2d), out and dy
+ * are [N, OD, OH, OW, Cout] with PyTorch's output rule in each dimension.  The gradients are b200_conv2d's with the depth term
+ * added; the bias gradient is b200_reduce (sum) over axis 0 of dy viewed as [N * OD * OH * OW, Cout].  No groups argument.
+ * Every rule that is not specific to 3-D is b200_conv2d's (and its gradients'): F16 / BF16 in, out the input dtype or F32,
+ * anything else B200_ERR_UNSUPPORTED; zero extents are no-ops (the gradients' zero-fill rules apply); INVALID_ARG versus
+ * UNSUPPORTED as for 2-D; bitwise reproducible for a fixed shape, dtypes and SM count; "gemm.variant" (2sm_n128 | 1sm_n128),
+ * "gemm.split_k" and "gemm.epilogue" apply.  Inputs with unit channel stride and 16-byte aligned base and strides are read in
+ * place (w and dw need (KD, KH, KW) to flatten into one stride); any other view is gathered at rank 5, and C * 2 % 16 != 0
+ * is copied with the channels padded to 8.  out and dx need a unit channel stride and one pixel pitch >= their channels
+ * across N, D, H and W.
+ * Limits of the 5-D im2col map, B200_ERR_UNSUPPORTED, each named in the message:
+ *   corners: pixel-box corners in [-16, 15] (cuTensorMapEncodeIm2col, rank 5): -p and p - d*(K-1) per dimension for the
+ *     forward and backward_weight, each phase's lower and upper corner for backward_data;
+ *   offsets: the load's im2col offsets kx*dw, ky*dh, kz*dd are 5-bit for rank 5 (PTX ISA), so d*(K-1) <= 31 per dimension
+ *     (backward_data: the phase's (taps - 1) * dilation);
+ *   stride: <= 8 per dimension;
+ *   size: N*OD*OH*OW < 2^31 (backward_data also N*D*H*W), KD*KH*KW*pad64(C) < 2^31.
+ * backward_data: dx splits into sd*sh*sw phases (d = rd + sd*a, h = rh + sh*i, w = rw + sw*j); one conv3d_dgrad_weights launch
+ * writes every phase's flipped, channel-transposed weights into one buffer of |w| elements, then stride 1 runs one conv3d GEMM
+ * and stride > 1 one conv3d_dgrad GEMM per phase with taps and pixels, plus one memset of dx when some phase receives no tap.
+ * The dry-run plan records each phase as "conv3d dgrad phase r=(rd,rh,rw) taps_d= taps_h= taps_w= dil= lower= upper= extent=".
+ * backward_weight: one conv3d_wgrad GEMM with M = Cout, N = KD*KH*KW*pad64(C), K = N*OD*OH*OW (stream-K head as 2-D). */
+typedef struct b200_conv3d_args {
+  int32_t stride_d, stride_h, stride_w, pad_d, pad_h, pad_w, dilation_d, dilation_h, dilation_w;
+} b200_conv3d_args;
+int b200_conv3d(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype,
+                b200_dptr x, const uint64_t* x_shape, const uint64_t* x_strides,
+                b200_dptr w, const uint64_t* w_shape, const uint64_t* w_strides,
+                b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides,
+                const b200_conv3d_args* args, const b200_epilogue* epilogue);
+int b200_conv3d_backward_data(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype,
+                              b200_dptr dy, const uint64_t* dy_shape, const uint64_t* dy_strides,
+                              b200_dptr w, const uint64_t* w_shape, const uint64_t* w_strides,
+                              b200_dptr dx, const uint64_t* dx_shape, const uint64_t* dx_strides,
+                              const b200_conv3d_args* args);
+int b200_conv3d_backward_weight(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype,
+                                b200_dptr x, const uint64_t* x_shape, const uint64_t* x_strides,
+                                b200_dptr dy, const uint64_t* dy_shape, const uint64_t* dy_strides,
+                                b200_dptr dw, const uint64_t* dw_shape, const uint64_t* dw_strides,
+                                const b200_conv3d_args* args);
+
 /* ---- collectives: ServerCommunication (server/base.rs:632-739), CUDA impl cubecl-cuda/src/compute/server.rs:666-926 -- */
 #define B200_UNIQUE_ID_BYTES 128
 int b200_comm_get_unique_id(b200_ctx* ctx, void* id128);            /* ncclGetUniqueId (communication.rs:11-25 holds it per device set) */

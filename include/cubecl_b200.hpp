@@ -305,6 +305,50 @@ inline void backward_weight_grouped(ComputeClient& client, const TensorHandle& x
 }
 }  // namespace conv
 
+namespace conv3d {
+/// 3-D convolution: x [N, D, H, W, C] (NDHWC), w [Cout, KD, KH, KW, C], out [N, OD, OH, OW, Cout]; f32 accumulation, optional
+/// fused epilogue (nullptr = none).  See b200_conv3d in cubecl_b200.h.  Errors are deferred to client.sync().
+inline void launch(ComputeClient& client, const TensorHandle& x, const TensorHandle& w, const TensorHandle& out,
+                   const b200_conv3d_args& args, const b200_epilogue* epilogue = nullptr) {
+  if (x.shape.size() != 5 || w.shape.size() != 5 || out.shape.size() != 5 || x.dtype != w.dtype) {
+    client.defer("InvalidArgument: conv3d needs rank-5 x, w and out, and x and w of one dtype");
+    return;
+  }
+  const int rc = b200_conv3d(client.raw(), nullptr, static_cast<b200_dtype>(x.dtype), static_cast<b200_dtype>(out.dtype),
+                             x.handle.ptr(), x.shape.data(), x.strides.data(), w.handle.ptr(), w.shape.data(), w.strides.data(),
+                             out.handle.ptr(), out.shape.data(), out.strides.data(), &args, epilogue);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+
+/// Input gradient: dy [N, OD, OH, OW, Cout], w [Cout, KD, KH, KW, C] -> dx [N, D, H, W, C].  See b200_conv3d_backward_data.
+/// Errors are deferred to client.sync().
+inline void backward_data(ComputeClient& client, const TensorHandle& dy, const TensorHandle& w, const TensorHandle& dx,
+                          const b200_conv3d_args& args) {
+  if (dy.shape.size() != 5 || w.shape.size() != 5 || dx.shape.size() != 5 || dy.dtype != w.dtype) {
+    client.defer("InvalidArgument: conv3d_backward_data needs rank-5 dy, w and dx, and dy and w of one dtype");
+    return;
+  }
+  const int rc = b200_conv3d_backward_data(client.raw(), nullptr, static_cast<b200_dtype>(dy.dtype), static_cast<b200_dtype>(dx.dtype),
+                                           dy.handle.ptr(), dy.shape.data(), dy.strides.data(), w.handle.ptr(), w.shape.data(),
+                                           w.strides.data(), dx.handle.ptr(), dx.shape.data(), dx.strides.data(), &args);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+
+/// Weight gradient: x [N, D, H, W, C], dy [N, OD, OH, OW, Cout] -> dw [Cout, KD, KH, KW, C].  The bias gradient is reduce (sum)
+/// over axis 0 of dy viewed as [N * OD * OH * OW, Cout].  See b200_conv3d_backward_weight.  Errors are deferred to client.sync().
+inline void backward_weight(ComputeClient& client, const TensorHandle& x, const TensorHandle& dy, const TensorHandle& dw,
+                            const b200_conv3d_args& args) {
+  if (x.shape.size() != 5 || dy.shape.size() != 5 || dw.shape.size() != 5 || x.dtype != dy.dtype) {
+    client.defer("InvalidArgument: conv3d_backward_weight needs rank-5 x, dy and dw, and x and dy of one dtype");
+    return;
+  }
+  const int rc = b200_conv3d_backward_weight(client.raw(), nullptr, static_cast<b200_dtype>(x.dtype), static_cast<b200_dtype>(dw.dtype),
+                                             x.handle.ptr(), x.shape.data(), x.strides.data(), dy.handle.ptr(), dy.shape.data(),
+                                             dy.strides.data(), dw.handle.ptr(), dw.shape.data(), dw.strides.data(), &args);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+}  // namespace conv3d
+
 namespace reduce {
 enum class Op : int { Sum = B200_REDUCE_SUM, Prod = B200_REDUCE_PROD, Max = B200_REDUCE_MAX, Min = B200_REDUCE_MIN,
                       ArgMax = B200_REDUCE_ARGMAX, ArgMin = B200_REDUCE_ARGMIN, Mean = B200_REDUCE_MEAN };

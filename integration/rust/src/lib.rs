@@ -148,6 +148,14 @@ pub struct Error {
     pub message: String,
 }
 
+/// b200_conv3d_args from (stride_d, stride_h, stride_w, pad_d, pad_h, pad_w, dilation_d, dilation_h, dilation_w).
+fn conv3d_args(a: [i32; 9]) -> sys::b200_conv3d_args {
+    sys::b200_conv3d_args {
+        stride_d: a[0], stride_h: a[1], stride_w: a[2], pad_d: a[3], pad_h: a[4], pad_w: a[5], dilation_d: a[6], dilation_h: a[7],
+        dilation_w: a[8],
+    }
+}
+
 fn check(rc: c_int) -> Result<(), Error> {
     if rc == 0 {
         return Ok(());
@@ -416,6 +424,64 @@ impl Context {
             stride_h: args[0], stride_w: args[1], pad_h: args[2], pad_w: args[3], dilation_h: args[4], dilation_w: args[5],
         };
         check(sys::b200_conv2d_backward_weight(
+            self.0, stream, in_dtype as c_int, out_dtype as c_int, x.ptr, x.shape.as_ptr(), x.strides.as_ptr(), dy.ptr,
+            dy.shape.as_ptr(), dy.strides.as_ptr(), dw.ptr, dw.shape.as_ptr(), dw.strides.as_ptr(), &a,
+        ))
+    }
+
+    /// 3-D convolution: x [N, D, H, W, C] (NDHWC), w [Cout, KD, KH, KW, C], out [N, OD, OH, OW, Cout], f32 accumulation,
+    /// optional fused epilogue; `args` = (stride_d, stride_h, stride_w, pad_d, pad_h, pad_w, dilation_d, dilation_h,
+    /// dilation_w).  See b200_conv3d in cubecl_b200.h.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::conv2d`].
+    pub unsafe fn conv3d(
+        &mut self, stream: b200_stream, in_dtype: DType, out_dtype: DType, x: &TensorView, w: &TensorView, out: &TensorView,
+        args: [i32; 9], epilogue: Option<&Epilogue>,
+    ) -> Result<(), Error> {
+        assert!(x.shape.len() == 5 && w.shape.len() == 5 && out.shape.len() == 5);
+        assert!(x.strides.len() == 5 && w.strides.len() == 5 && out.strides.len() == 5);
+        let a = conv3d_args(args);
+        let e = epilogue.map(|e| sys::b200_epilogue { alpha: e.alpha, activation: e.activation as i32, bias: e.bias });
+        check(sys::b200_conv3d(
+            self.0, stream, in_dtype as c_int, out_dtype as c_int, x.ptr, x.shape.as_ptr(), x.strides.as_ptr(), w.ptr,
+            w.shape.as_ptr(), w.strides.as_ptr(), out.ptr, out.shape.as_ptr(), out.strides.as_ptr(), &a,
+            e.as_ref().map_or(std::ptr::null(), |e| e as *const sys::b200_epilogue),
+        ))
+    }
+
+    /// Input gradient of [`Context::conv3d`]: dy [N, OD, OH, OW, Cout], w [Cout, KD, KH, KW, C] -> dx [N, D, H, W, C].  See
+    /// b200_conv3d_backward_data in cubecl_b200.h.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::matmul`] for the three pointers.
+    pub unsafe fn conv3d_backward_data(
+        &mut self, stream: b200_stream, in_dtype: DType, out_dtype: DType, dy: &TensorView, w: &TensorView, dx: &TensorView,
+        args: [i32; 9],
+    ) -> Result<(), Error> {
+        assert!(dy.shape.len() == 5 && w.shape.len() == 5 && dx.shape.len() == 5);
+        assert!(dy.strides.len() == 5 && w.strides.len() == 5 && dx.strides.len() == 5);
+        let a = conv3d_args(args);
+        check(sys::b200_conv3d_backward_data(
+            self.0, stream, in_dtype as c_int, out_dtype as c_int, dy.ptr, dy.shape.as_ptr(), dy.strides.as_ptr(), w.ptr,
+            w.shape.as_ptr(), w.strides.as_ptr(), dx.ptr, dx.shape.as_ptr(), dx.strides.as_ptr(), &a,
+        ))
+    }
+
+    /// Weight gradient of [`Context::conv3d`]: x [N, D, H, W, C], dy [N, OD, OH, OW, Cout] -> dw [Cout, KD, KH, KW, C].  The
+    /// bias gradient is [`Context::reduce`] (sum) over axis 0 of dy viewed as [N * OD * OH * OW, Cout].  See
+    /// b200_conv3d_backward_weight in cubecl_b200.h.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::matmul`] for the three pointers.
+    pub unsafe fn conv3d_backward_weight(
+        &mut self, stream: b200_stream, in_dtype: DType, out_dtype: DType, x: &TensorView, dy: &TensorView, dw: &TensorView,
+        args: [i32; 9],
+    ) -> Result<(), Error> {
+        assert!(x.shape.len() == 5 && dy.shape.len() == 5 && dw.shape.len() == 5);
+        assert!(x.strides.len() == 5 && dy.strides.len() == 5 && dw.strides.len() == 5);
+        let a = conv3d_args(args);
+        check(sys::b200_conv3d_backward_weight(
             self.0, stream, in_dtype as c_int, out_dtype as c_int, x.ptr, x.shape.as_ptr(), x.strides.as_ptr(), dy.ptr,
             dy.shape.as_ptr(), dy.strides.as_ptr(), dw.ptr, dw.shape.as_ptr(), dw.strides.as_ptr(), &a,
         ))
