@@ -136,6 +136,10 @@ SIGNATURES = {
                                             C.c_uint64, _u64p, _u64p, C.POINTER(Conv3dArgs)]),
     "b200_conv3d_backward_weight": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, _u64p, _u64p, C.c_uint64, _u64p, _u64p,
                                               C.c_uint64, _u64p, _u64p, C.POINTER(Conv3dArgs)]),
+    "b200_conv_transpose2d": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, _u64p, _u64p, C.c_uint64, _u64p, _u64p, C.c_uint64,
+                                        _u64p, _u64p, C.POINTER(Conv2dArgs), C.POINTER(Epilogue)]),
+    "b200_conv_transpose3d": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, _u64p, _u64p, C.c_uint64, _u64p, _u64p, C.c_uint64,
+                                        _u64p, _u64p, C.POINTER(Conv3dArgs), C.POINTER(Epilogue)]),
     "b200_reduce": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, C.c_uint64, C.c_int, _u64p, C.c_int]),
     "b200_reduce_strided": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, C.c_uint64, C.c_int, _u64p, _u64p, C.c_int]),
     "b200_reduce_debug": (C.c_int, [_vp, _vp, _u64p]),

@@ -71,13 +71,14 @@ def launch(client: ComputeClient, x: TensorHandle, w: TensorHandle, out: TensorH
     _enqueue(client, "conv2d", x, w, out, stride, padding, dilation, stream, groups, _epilogue_check("conv2d", w, alpha, bias, activation))
 
 
-def _epilogue_check(what: str, w: TensorHandle, alpha: float, bias: TensorHandle | None, activation: str | None):
+def _epilogue_check(what: str, w: TensorHandle, alpha: float, bias: TensorHandle | None, activation: str | None,
+                    cout: int | None = None):
     """launch's epilogue callback for _enqueue: checks the epilogue arguments, returns (b200_epilogue pointer or None,
-    the extra handles it reads)."""
+    the extra handles it reads).  cout: the output channels (default w.shape[0])."""
     def epilogue():
         if activation not in ACTIVATIONS:
             raise B200Error(6, f"unknown activation {activation!r}")
-        if bias is not None and (bias.dtype != "f32" or not bias.is_contiguous() or bias.size() != w.shape[0]):
+        if bias is not None and (bias.dtype != "f32" or not bias.is_contiguous() or bias.size() != (w.shape[0] if cout is None else cout)):
             raise B200Error(6, f"{what}: bias must be a contiguous f32 tensor with Cout elements")
         if alpha == 1.0 and bias is None and activation in (None, "none"):
             return None, ()

@@ -16,6 +16,7 @@
 #include <unistd.h>
 
 #include <algorithm>
+#include <memory>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -53,6 +54,8 @@ extern const unsigned char b200_cubin_conv_grouped[];
 extern const unsigned char b200_cubin_conv_grouped_end[];
 extern const unsigned char b200_cubin_gemm_conv3d[];
 extern const unsigned char b200_cubin_gemm_conv3d_end[];
+extern const unsigned char b200_cubin_gemm_convt[];
+extern const unsigned char b200_cubin_gemm_convt_end[];
 }
 
 // ================================================================================================ errors
@@ -324,13 +327,14 @@ static int get_func(b200_ctx* c, const std::string& name, CUfunction* out) {
   auto it = c->funcs.find(name);
   if (it != c->funcs.end()) { *out = it->second; return B200_OK; }
   // modules are loaded in the order gemm, reduce, aux, gemm_b, gemm_c, quant, gemm_q, quant_mm, gemm_conv, gemm_convbwd,
-  // conv_grouped, gemm_conv3d; the kernel
+  // conv_grouped, gemm_conv3d, gemm_convt; the kernel
   // name says where a
   // kernel lives (no failing lookups, which API-level tools such as compute-sanitizer would report)
   auto starts = [&](const char* pfx) { return name.rfind(pfx, 0) == 0; };
   auto has = [&](const char* part) { return name.find(part) != std::string::npos; };
   const bool tc_gemm = starts("gemm_") && name != "gemm_simt_strided" && name != "gemm_scaled_simt";
   const size_t home = name == "conv3d_dgrad_weights" ? 2
+                      : starts("conv2d_tconv_") || starts("conv3d_tconv_") ? 12
                       : starts("conv3d_") ? 11
                       : starts("conv2d_grp_") ? 10
                       : starts("conv2d_dgrad_") || starts("conv2d_wgrad_") ? 9
@@ -368,7 +372,8 @@ extern "C" int b200_get_cubin(const char* name, const void** image, size_t* size
   else if (!strcmp(name, "gemm_convbwd")) { b = b200_cubin_gemm_convbwd; e = b200_cubin_gemm_convbwd_end; }
   else if (!strcmp(name, "conv_grouped")) { b = b200_cubin_conv_grouped; e = b200_cubin_conv_grouped_end; }
   else if (!strcmp(name, "gemm_conv3d")) { b = b200_cubin_gemm_conv3d; e = b200_cubin_gemm_conv3d_end; }
-  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd|conv_grouped|gemm_conv3d)", name);
+  else if (!strcmp(name, "gemm_convt")) { b = b200_cubin_gemm_convt; e = b200_cubin_gemm_convt_end; }
+  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd|conv_grouped|gemm_conv3d|gemm_convt)", name);
   *image = b;
   *size = static_cast<size_t>(e - b);
   return B200_OK;
@@ -427,7 +432,8 @@ extern "C" int b200_init(int device, b200_ctx** out) {
       (rc = load_module(c, b200_cubin_gemm_conv, b200_cubin_gemm_conv_end, "gemm_conv")) ||
       (rc = load_module(c, b200_cubin_gemm_convbwd, b200_cubin_gemm_convbwd_end, "gemm_convbwd")) ||
       (rc = load_module(c, b200_cubin_conv_grouped, b200_cubin_conv_grouped_end, "conv_grouped")) ||
-      (rc = load_module(c, b200_cubin_gemm_conv3d, b200_cubin_gemm_conv3d_end, "gemm_conv3d"))) {
+      (rc = load_module(c, b200_cubin_gemm_conv3d, b200_cubin_gemm_conv3d_end, "gemm_conv3d")) ||
+      (rc = load_module(c, b200_cubin_gemm_convt, b200_cubin_gemm_convt_end, "gemm_convt"))) {
     for (CUmodule m : c->modules) g_drv.cuModuleUnload_p(m);
     g_drv.cuDevicePrimaryCtxRelease_p(c->dev);
     return bail(rc);
@@ -1139,7 +1145,8 @@ static uint64_t gemm_num_kb(const GemmProblem& g, uint32_t block_k) {
 
 // Tile variant by modelled time (ties -> larger tile, less L2 traffic): waves of tiles, with the last partial wave replaced by a
 // stream-K head where that pays (sk_plan).  nullptr: gemm.variant names no variant this dtype / kind has.
-static const GemmVariant* pick_variant(b200_ctx* c, const GemmProblem& g, SkPlan* sk_out) {
+// stream_k = false: a launch that plans no stream-K head (whole tiles only) is costed by its waves alone.
+static const GemmVariant* pick_variant(b200_ctx* c, const GemmProblem& g, SkPlan* sk_out, bool stream_k = true) {
   const size_t esz = dtype_size(g.in_dtype);
   const uint32_t block_k = static_cast<uint32_t>(128 / esz);
   const std::string forced = opt(c, "gemm.variant", "auto");
@@ -1158,7 +1165,7 @@ static const GemmVariant* pick_variant(b200_ctx* c, const GemmProblem& g, SkPlan
     const uint64_t tiles = tm * tn * g.batch;
     const uint64_t clusters = std::max(1, c->props.num_sms / v.cg);
     // the slab exchange is a per-128-row-CTA-tile protocol with f32 accumulators: not for the 512-row tile, not for integers
-    const SkPlan sk = sk_plan(tiles, clusters, num_kb, split_opt, float_acc && v.mt == 1, g.sk_max_parts);
+    const SkPlan sk = sk_plan(tiles, clusters, num_kb, split_opt, float_acc && v.mt == 1 && stream_k, g.sk_max_parts);
     const double eff = v.eff > 0 ? v.eff : 1.0;
     const double cost = sk.time * (128.0 * v.mt * v.block_n) / eff;  // per-SM MMA time
     if (!best || cost < best_cost * 0.999) { best = &v; best_cost = cost; *sk_out = sk; }
@@ -2929,6 +2936,86 @@ static DgradPhase1D dgrad_phase(uint64_t H, uint64_t K, int64_t s, int64_t p, in
   return ph;
 }
 
+// The taps of a phase in walk order (ascending dy offset), comma-separated, for the plan lines.
+static std::string dgrad_taps(const DgradPhase1D& q) {
+  std::string s;
+  for (uint32_t t = 0; t < q.taps; ++t) s += (t ? "," : "") + std::to_string(q.kmax - t * q.step);
+  return s;
+}
+
+// The 2-D data gradient's phases (also b200_conv_transpose2d's, x in dy's role): per dimension, and the im2col corner
+// limits of every phase that runs.  dx is [N, H, W, *] from dy [N, OH, OW, Cout]; *zero_phase: a phase with pixels receives
+// no tap (or Cout == 0).
+static int dgrad2_plan(const char* what, const b200_conv2d_args& a, uint64_t H, uint64_t W, uint64_t KH, uint64_t KW, uint64_t OH,
+                       uint64_t OW, uint64_t Cout, std::vector<DgradPhase1D>* phs, std::vector<DgradPhase1D>* pws, bool* zero_phase) {
+  for (int r = 0; r < a.stride_h; ++r) phs->push_back(dgrad_phase(H, KH, a.stride_h, a.pad_h, a.dilation_h, (uint32_t)r));
+  for (int r = 0; r < a.stride_w; ++r) pws->push_back(dgrad_phase(W, KW, a.stride_w, a.pad_w, a.dilation_w, (uint32_t)r));
+  *zero_phase = false;
+  for (const DgradPhase1D& ph : *phs)
+    for (const DgradPhase1D& pw : *pws) {
+      if (!ph.extent || !pw.extent) continue;
+      if (!ph.taps || !pw.taps || Cout == 0) { *zero_phase = true; continue; }
+      const int64_t corners[4] = {ph.e0, pw.e0, ph.e0 + (int64_t)ph.extent - (int64_t)OH, pw.e0 + (int64_t)pw.extent - (int64_t)OW};
+      int rc = conv_check_corners(what, corners);
+      if (rc) return rc;
+    }
+  return B200_OK;
+}
+
+// Every phase's flipped, channel-transposed weights [C][Th][Tw][cp] in one pooled buffer (*buf) of KH * KW * C * cp
+// elements, written by conv_dgrad_weights from w [Cout, KH, KW, C] (strides ws); wp->off holds each phase's block.
+static int dgrad2_prep(b200_ctx* c, CUstream st, uint64_t w, const uint64_t ws[4], const b200_conv2d_args& a, uint64_t C, uint64_t Cout,
+                       uint64_t cp, uint64_t KH, uint64_t KW, const std::vector<DgradPhase1D>& phs, const std::vector<DgradPhase1D>& pws,
+                       CUdeviceptr* buf, ConvDgradWeightsParams* wp_out) {
+  ConvDgradWeightsParams& wp = *wp_out;
+  memset(&wp, 0, sizeof(wp));
+  int rc = pool_alloc(c, KH * KW * C * cp * 2, buf, st);
+  if (rc) return rc;
+  wp.w = w; wp.out = *buf;
+  wp.s_co = ws[0]; wp.s_ky = ws[1]; wp.s_kx = ws[2]; wp.s_c = ws[3];
+  wp.C = C; wp.Cout = Cout; wp.cp = cp;
+  wp.KH = (uint32_t)KH; wp.KW = (uint32_t)KW; wp.sh = (uint32_t)a.stride_h; wp.sw = (uint32_t)a.stride_w;
+  wp.dh = (uint32_t)a.dilation_h; wp.dw = (uint32_t)a.dilation_w; wp.ph = (uint32_t)a.pad_h; wp.pw = (uint32_t)a.pad_w;
+  wp.qh = phs[0].step; wp.qw = pws[0].step;
+  uint64_t off = 0;
+  for (const DgradPhase1D& ph : phs)
+    for (const DgradPhase1D& pw : pws) {
+      wp.off[ph.r * a.stride_w + pw.r] = off;
+      off += (uint64_t)ph.taps * pw.taps * C * cp;
+    }
+  for (const DgradPhase1D& ph : phs) { wp.kmax_h[ph.r] = ph.kmax; wp.taps_h[ph.r] = ph.taps; }
+  for (const DgradPhase1D& pw : pws) { wp.kmax_w[pw.r] = pw.kmax; wp.taps_w[pw.r] = pw.taps; }
+  CUfunction f;
+  rc = get_func(c, "conv_dgrad_weights", &f);
+  void* kargs[] = {&wp};
+  if (!rc) rc = launch(c, f, (unsigned)(((C + 31) / 32) * ((cp + 31) / 32)), (unsigned)(KH * KW), 1, 256, 0, 1, st, kargs);
+  return rc;
+}
+
+// One phase (ph, pw) as a stride-1 convolution of dy (read through y) into C channels: its geometry, with the phase-addressed
+// epilogue of dx (normalised strides os) unless the conv stride is 1.
+static ConvGeom dgrad2_geom(uint64_t N, uint64_t OH, uint64_t OW, uint64_t cp, uint64_t C, const DgradPhase1D& ph, const DgradPhase1D& pw,
+                            const NhwcOperand& y, const uint64_t os[4], const b200_conv2d_args& a) {
+  ConvGeom g{};
+  g.N = N; g.H = OH; g.W = OW; g.C = cp; g.KH = ph.taps; g.KW = pw.taps; g.OH = ph.extent; g.OW = pw.extent; g.Cout = C;
+  g.sh = 1; g.sw = 1; g.ph = (int32_t)-ph.e0; g.pw = (int32_t)-pw.e0; g.dh = (int32_t)ph.dil; g.dw = (int32_t)pw.dil;
+  g.x_sw = y.s_w; g.x_sh = y.s_h; g.x_sn = y.s_n;
+  g.w_sp = cp; g.w_sco = (uint64_t)ph.taps * pw.taps * cp;
+  g.box = true; g.lo_h = (int32_t)ph.e0; g.lo_w = (int32_t)pw.e0;
+  g.mode = a.stride_h == 1 && a.stride_w == 1 ? 0 : 1;
+  g.dx_sn = os[0]; g.dx_si = (uint64_t)a.stride_h * os[1]; g.dx_sj = (uint64_t)a.stride_w * os[2];
+  return g;
+}
+
+// The plan line of phase (ph, pw): `head` r=(rh,rw) taps_h= taps_w= dil= lower= upper= extent=, no newline.
+static std::string dgrad2_phase_line(const char* head, const DgradPhase1D& ph, const DgradPhase1D& pw, uint64_t OH, uint64_t OW) {
+  return std::string(head) + " r=(" + std::to_string(ph.r) + "," + std::to_string(pw.r) + ") taps_h=" + dgrad_taps(ph) +
+         " taps_w=" + dgrad_taps(pw) + " dil=(" + std::to_string(ph.dil) + "," + std::to_string(pw.dil) + ") lower=(" +
+         std::to_string(ph.e0) + "," + std::to_string(pw.e0) + ") upper=(" + std::to_string(ph.e0 + (int64_t)ph.extent - (int64_t)OH) +
+         "," + std::to_string(pw.e0 + (int64_t)pw.extent - (int64_t)OW) + ") extent=(" + std::to_string(ph.extent) + "," +
+         std::to_string(pw.extent) + ")";
+}
+
 extern "C" int b200_conv2d_backward_data(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr dy,
                                          const uint64_t* dy_shape, const uint64_t* dy_strides, b200_dptr w, const uint64_t* w_shape,
                                          const uint64_t* w_strides, b200_dptr dx, const uint64_t* dx_shape, const uint64_t* dx_strides,
@@ -2950,16 +3037,8 @@ extern "C" int b200_conv2d_backward_data(b200_ctx* c, b200_stream s, b200_dtype 
   if (KH * KW * ((Cout + 63) / 64 * 64) >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: KH * KW * Cout (Cout padded to 64) must be < 2^31", what);
   // phases of each dimension, and the im2col limits of every phase that runs
   std::vector<DgradPhase1D> phs, pws;
-  for (int r = 0; r < a.stride_h; ++r) phs.push_back(dgrad_phase(H, KH, a.stride_h, a.pad_h, a.dilation_h, (uint32_t)r));
-  for (int r = 0; r < a.stride_w; ++r) pws.push_back(dgrad_phase(W, KW, a.stride_w, a.pad_w, a.dilation_w, (uint32_t)r));
   bool zero_phase = false;
-  for (const DgradPhase1D& ph : phs)
-    for (const DgradPhase1D& pw : pws) {
-      if (!ph.extent || !pw.extent) continue;
-      if (!ph.taps || !pw.taps || Cout == 0) { zero_phase = true; continue; }
-      const int64_t corners[4] = {ph.e0, pw.e0, ph.e0 + (int64_t)ph.extent - (int64_t)OH, pw.e0 + (int64_t)pw.extent - (int64_t)OW};
-      if ((rc = conv_check_corners(what, corners))) return rc;
-    }
+  if ((rc = dgrad2_plan(what, a, H, W, KH, KW, OH, OW, Cout, &phs, &pws, &zero_phase))) return rc;
   if ((rc = conv_check_ptrs(what, dy, w, dx, "dx", out_dtype))) return rc;
   const size_t osz = dtype_size(out_dtype);
   uint64_t os[4], ys[4], ws[4];
@@ -2981,52 +3060,14 @@ extern "C" int b200_conv2d_backward_data(b200_ctx* c, b200_stream s, b200_dtype 
   const uint64_t cp = y.C;
   ConvDgradWeightsParams wp;
   memset(&wp, 0, sizeof(wp));
-  if (!rc) rc = pool_alloc(c, KH * KW * C * cp * 2, &tmp[2], st);
-  if (!rc) {
-    wp.w = w; wp.out = tmp[2];
-    wp.s_co = ws[0]; wp.s_ky = ws[1]; wp.s_kx = ws[2]; wp.s_c = ws[3];
-    wp.C = C; wp.Cout = Cout; wp.cp = cp;
-    wp.KH = (uint32_t)KH; wp.KW = (uint32_t)KW; wp.sh = (uint32_t)a.stride_h; wp.sw = (uint32_t)a.stride_w;
-    wp.dh = (uint32_t)a.dilation_h; wp.dw = (uint32_t)a.dilation_w; wp.ph = (uint32_t)a.pad_h; wp.pw = (uint32_t)a.pad_w;
-    wp.qh = phs[0].step; wp.qw = pws[0].step;
-    uint64_t off = 0;
-    for (const DgradPhase1D& ph : phs)
-      for (const DgradPhase1D& pw : pws) {
-        wp.off[ph.r * a.stride_w + pw.r] = off;
-        off += (uint64_t)ph.taps * pw.taps * C * cp;
-      }
-    for (const DgradPhase1D& ph : phs) { wp.kmax_h[ph.r] = ph.kmax; wp.taps_h[ph.r] = ph.taps; }
-    for (const DgradPhase1D& pw : pws) { wp.kmax_w[pw.r] = pw.kmax; wp.taps_w[pw.r] = pw.taps; }
-    CUfunction f;
-    rc = get_func(c, "conv_dgrad_weights", &f);
-    void* kargs[] = {&wp};
-    if (!rc) rc = launch(c, f, (unsigned)(((C + 31) / 32) * ((cp + 31) / 32)), (unsigned)(KH * KW), 1, 256, 0, 1, st, kargs);
-  }
+  if (!rc) rc = dgrad2_prep(c, st, w, ws, a, C, Cout, cp, KH, KW, phs, pws, &tmp[2], &wp);
   // one stride-1 convolution of dy per phase that has taps and pixels
-  const bool stride1 = a.stride_h == 1 && a.stride_w == 1;
   for (const DgradPhase1D& ph : phs)
     for (const DgradPhase1D& pw : pws) {
       if (rc) break;
       if (!ph.extent || !pw.extent || !ph.taps || !pw.taps) continue;
-      ConvGeom g{};
-      g.N = N; g.H = OH; g.W = OW; g.C = cp; g.KH = ph.taps; g.KW = pw.taps; g.OH = ph.extent; g.OW = pw.extent; g.Cout = C;
-      g.sh = 1; g.sw = 1; g.ph = (int32_t)-ph.e0; g.pw = (int32_t)-pw.e0; g.dh = (int32_t)ph.dil; g.dw = (int32_t)pw.dil;
-      g.x_sw = y.s_w; g.x_sh = y.s_h; g.x_sn = y.s_n;
-      g.w_sp = cp; g.w_sco = (uint64_t)ph.taps * pw.taps * cp;
-      g.box = true; g.lo_h = (int32_t)ph.e0; g.lo_w = (int32_t)pw.e0;
-      g.mode = stride1 ? 0 : 1;
-      g.dx_sn = os[0]; g.dx_si = (uint64_t)a.stride_h * os[1]; g.dx_sj = (uint64_t)a.stride_w * os[2];
-      if (c->dry) {
-        std::string line = "conv dgrad phase r=(" + std::to_string(ph.r) + "," + std::to_string(pw.r) + ") taps_h=";
-        for (uint32_t t = 0; t < ph.taps; ++t) line += (t ? "," : "") + std::to_string(ph.kmax - t * ph.step);
-        line += " taps_w=";
-        for (uint32_t t = 0; t < pw.taps; ++t) line += (t ? "," : "") + std::to_string(pw.kmax - t * pw.step);
-        line += " dil=(" + std::to_string(ph.dil) + "," + std::to_string(pw.dil) + ") lower=(" + std::to_string(ph.e0) + "," +
-                std::to_string(pw.e0) + ") upper=(" + std::to_string(ph.e0 + (int64_t)ph.extent - (int64_t)OH) + "," +
-                std::to_string(pw.e0 + (int64_t)pw.extent - (int64_t)OW) + ") extent=(" + std::to_string(ph.extent) + "," +
-                std::to_string(pw.extent) + ")\n";
-        c->plan += line;
-      }
+      ConvGeom g = dgrad2_geom(N, OH, OW, cp, C, ph, pw, y, os, a);
+      if (c->dry) c->plan += dgrad2_phase_line("conv dgrad phase", ph, pw, OH, OW) + "\n";
       const GemmProblem gp = conv_problem(in_dtype, out_dtype, y.ptr, tmp[2] + wp.off[ph.r * a.stride_w + pw.r] * 2,
                                           dx + ((uint64_t)ph.r * os[1] + (uint64_t)pw.r * os[2]) * osz, N * ph.extent * pw.extent, C,
                                           (uint64_t)ph.taps * pw.taps * ((cp + 63) / 64 * 64), os[2], &g);
@@ -3287,6 +3328,96 @@ extern "C" int b200_conv3d(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200
   return rc;
 }
 
+// The 3-D data gradient's phases (also b200_conv_transpose3d's): per dimension (D, H, W) of dx extents I from dy extents
+// O, and the rank-5 im2col limits (corners, offsets) of every phase that runs.  *zero_phase as dgrad2_plan.
+static int dgrad3_plan(const char* what, const int64_t sv[3], const int64_t pv[3], const int64_t dv[3], const uint64_t I[3],
+                       const uint64_t K[3], const uint64_t O[3], uint64_t Cout, std::vector<DgradPhase1D> ph[3], bool* zero_phase) {
+  for (int i = 0; i < 3; ++i)
+    for (int64_t r = 0; r < sv[i]; ++r) ph[i].push_back(dgrad_phase(I[i], K[i], sv[i], pv[i], dv[i], (uint32_t)r));
+  *zero_phase = false;
+  for (const DgradPhase1D& pd : ph[0])
+    for (const DgradPhase1D& phh : ph[1])
+      for (const DgradPhase1D& pw : ph[2]) {
+        const DgradPhase1D* q[3] = {&pd, &phh, &pw};
+        if (!pd.extent || !phh.extent || !pw.extent) continue;
+        if (!pd.taps || !phh.taps || !pw.taps || Cout == 0) { *zero_phase = true; continue; }
+        int64_t corners[6], off[3];
+        for (int i = 0; i < 3; ++i) {
+          corners[2 * i] = q[i]->e0;
+          corners[2 * i + 1] = q[i]->e0 + (int64_t)q[i]->extent - (int64_t)O[i];
+          off[i] = (int64_t)(q[i]->taps - 1) * q[i]->dil;
+        }
+        int rc = conv3_check_corners(what, corners, 6);
+        if (!rc) rc = conv3_check_offsets(what, off);
+        if (rc) return rc;
+      }
+  return B200_OK;
+}
+
+// conv3d_dgrad_weights' parameters for the phases ph of w [Cout, KD, KH, KW, C], and where each phase's block starts.
+struct Dgrad3Prep {
+  Conv3dDgradWeightsParams wp;
+  uint64_t pre[3][kDgradMaxStride];
+  uint64_t k1, k2, ccp;
+  Dgrad3Prep(const std::vector<DgradPhase1D> ph[3], const uint64_t K[3], const int64_t sv[3], const int64_t pv[3], const int64_t dv[3],
+             uint64_t C, uint64_t cp) : k1(K[1]), k2(K[2]), ccp(C * cp) {
+    memset(&wp, 0, sizeof(wp));
+    for (int i = 0; i < 3; ++i) {
+      uint64_t acc = 0;
+      for (const DgradPhase1D& q : ph[i]) { pre[i][q.r] = acc; acc += q.taps; wp.kmax[i][q.r] = q.kmax; wp.taps[i][q.r] = q.taps; }
+      wp.k[i] = (uint32_t)K[i]; wp.s[i] = (uint32_t)sv[i]; wp.d[i] = (uint32_t)dv[i]; wp.p[i] = (uint32_t)pv[i]; wp.q[i] = ph[i][0].step;
+    }
+    wp.C = C; wp.cp = cp;
+  }
+  // first element of phase (rd, rh, rw)'s block
+  uint64_t off(uint32_t rd, uint32_t rh, uint32_t rw) const {
+    return ccp * (pre[0][rd] * k1 * k2 + (uint64_t)wp.taps[0][rd] * (pre[1][rh] * k2 + (uint64_t)wp.taps[1][rh] * pre[2][rw]));
+  }
+};
+
+// Every phase's flipped, channel-transposed weights in one pooled buffer (*buf) of KK * C * cp elements (conv3d_dgrad_weights).
+static int dgrad3_prep(b200_ctx* c, CUstream st, uint64_t w, const uint64_t ws[5], uint64_t Cout, uint64_t KK, Dgrad3Prep* pr, CUdeviceptr* buf) {
+  Conv3dDgradWeightsParams& wp = pr->wp;
+  int rc = pool_alloc(c, KK * wp.C * wp.cp * 2, buf, st);
+  if (rc) return rc;
+  wp.w = w; wp.out = *buf;
+  wp.s_co = ws[0]; wp.s_kz = ws[1]; wp.s_ky = ws[2]; wp.s_kx = ws[3]; wp.s_c = ws[4];
+  wp.Cout = Cout;
+  CUfunction f;
+  rc = get_func(c, "conv3d_dgrad_weights", &f);
+  void* kargs[] = {&wp};
+  if (!rc) rc = launch(c, f, (unsigned)(((wp.C + 31) / 32) * ((wp.cp + 31) / 32)), (unsigned)KK, 1, 256, 0, 1, st, kargs);
+  return rc;
+}
+
+// Phase q = (D, H, W) phases as a stride-1 3-D convolution of dy (y, extents O) into C channels; dgrad2_geom with depth.
+static ConvGeom dgrad3_geom(uint64_t N, const uint64_t O[3], uint64_t cp, uint64_t C, const DgradPhase1D* const q[3], const NdhwcOperand& y,
+                            const uint64_t os[5], const int64_t sv[3]) {
+  const uint64_t T[3] = {q[0]->taps, q[1]->taps, q[2]->taps}, E[3] = {q[0]->extent, q[1]->extent, q[2]->extent};
+  const int32_t one[3] = {1, 1, 1}, pp[3] = {(int32_t)-q[0]->e0, (int32_t)-q[1]->e0, (int32_t)-q[2]->e0};
+  const int32_t dil[3] = {(int32_t)q[0]->dil, (int32_t)q[1]->dil, (int32_t)q[2]->dil};
+  ConvGeom g = conv3_geom(N, O, cp, T, E, C, one, pp, dil);
+  g.x_sw = y.s_w; g.x_sh = y.s_h; g.x_sd = y.s_d; g.x_sn = y.s_n;
+  g.w_sp = cp; g.w_sco = T[0] * T[1] * T[2] * cp;
+  g.box = true; g.lo_d = (int32_t)q[0]->e0; g.lo_h = (int32_t)q[1]->e0; g.lo_w = (int32_t)q[2]->e0;
+  g.mode = sv[0] == 1 && sv[1] == 1 && sv[2] == 1 ? 0 : 1;
+  g.dx_sn = os[0]; g.dx_sd = (uint64_t)sv[0] * os[1]; g.dx_si = (uint64_t)sv[1] * os[2]; g.dx_sj = (uint64_t)sv[2] * os[3];
+  return g;
+}
+
+// The plan line of phase q: `head` r=(rd,rh,rw) taps_d= taps_h= taps_w= dil= lower= upper= extent=, no newline.
+static std::string dgrad3_phase_line(const char* head, const DgradPhase1D* const q[3], const uint64_t O[3]) {
+  std::string line = std::string(head) + " r=(" + std::to_string(q[0]->r) + "," + std::to_string(q[1]->r) + "," + std::to_string(q[2]->r) + ")";
+  const char* tn[3] = {" taps_d=", " taps_h=", " taps_w="};
+  for (int i = 0; i < 3; ++i) line += tn[i] + dgrad_taps(*q[i]);
+  auto triple = [&](auto f) { return "(" + std::to_string(f(0)) + "," + std::to_string(f(1)) + "," + std::to_string(f(2)) + ")"; };
+  line += " dil=" + triple([&](int i) { return (int64_t)q[i]->dil; });
+  line += " lower=" + triple([&](int i) { return q[i]->e0; });
+  line += " upper=" + triple([&](int i) { return q[i]->e0 + (int64_t)q[i]->extent - (int64_t)O[i]; });
+  line += " extent=" + triple([&](int i) { return (int64_t)q[i]->extent; });
+  return line;
+}
+
 extern "C" int b200_conv3d_backward_data(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr dy,
                                          const uint64_t* dy_shape, const uint64_t* dy_strides, b200_dptr w, const uint64_t* w_shape,
                                          const uint64_t* w_strides, b200_dptr dx, const uint64_t* dx_shape, const uint64_t* dx_strides,
@@ -3311,23 +3442,8 @@ extern "C" int b200_conv3d_backward_data(b200_ctx* c, b200_stream s, b200_dtype 
     return fail(B200_ERR_UNSUPPORTED, "%s: KD * KH * KW * Cout (Cout padded to 64) must be < 2^31", what);
   // phases of each dimension, and the im2col limits of every phase that runs
   std::vector<DgradPhase1D> ph[3];
-  for (int i = 0; i < 3; ++i)
-    for (int64_t r = 0; r < sv[i]; ++r) ph[i].push_back(dgrad_phase(I[i], K[i], sv[i], pv[i], dv[i], (uint32_t)r));
   bool zero_phase = false;
-  for (const DgradPhase1D& pd : ph[0])
-    for (const DgradPhase1D& phh : ph[1])
-      for (const DgradPhase1D& pw : ph[2]) {
-        const DgradPhase1D* q[3] = {&pd, &phh, &pw};
-        if (!pd.extent || !phh.extent || !pw.extent) continue;
-        if (!pd.taps || !phh.taps || !pw.taps || Cout == 0) { zero_phase = true; continue; }
-        int64_t corners[6], off[3];
-        for (int i = 0; i < 3; ++i) {
-          corners[2 * i] = q[i]->e0;
-          corners[2 * i + 1] = q[i]->e0 + (int64_t)q[i]->extent - (int64_t)O[i];
-          off[i] = (int64_t)(q[i]->taps - 1) * q[i]->dil;
-        }
-        if ((rc = conv3_check_corners(what, corners, 6)) || (rc = conv3_check_offsets(what, off))) return rc;
-      }
+  if ((rc = dgrad3_plan(what, sv, pv, dv, I, K, O, Cout, ph, &zero_phase))) return rc;
   if ((rc = conv_check_ptrs(what, dy, w, dx, "dx", out_dtype))) return rc;
   const size_t osz = dtype_size(out_dtype);
   uint64_t os[5], ys[5], ws[5];
@@ -3348,61 +3464,20 @@ extern "C" int b200_conv3d_backward_data(b200_ctx* c, b200_stream s, b200_dtype 
   // every phase's flipped, channel-transposed weights [C][Td][Th][Tw][cp] in one pooled buffer of |w| * cp / Cout elements, in
   // (rd, rh, rw) order (Conv3dDgradWeightsParams)
   const uint64_t cp = y.C;
-  Conv3dDgradWeightsParams wp;
-  memset(&wp, 0, sizeof(wp));
-  uint64_t pre[3][kDgradMaxStride];
-  for (int i = 0; i < 3; ++i) {
-    uint64_t acc = 0;
-    for (const DgradPhase1D& q : ph[i]) { pre[i][q.r] = acc; acc += q.taps; wp.kmax[i][q.r] = q.kmax; wp.taps[i][q.r] = q.taps; }
-    wp.k[i] = (uint32_t)K[i]; wp.s[i] = (uint32_t)sv[i]; wp.d[i] = (uint32_t)dv[i]; wp.p[i] = (uint32_t)pv[i]; wp.q[i] = ph[i][0].step;
-  }
-  auto phase_off = [&](uint32_t rd, uint32_t rh, uint32_t rw) {
-    return C * cp * (pre[0][rd] * K[1] * K[2] + (uint64_t)wp.taps[0][rd] * (pre[1][rh] * K[2] + (uint64_t)wp.taps[1][rh] * pre[2][rw]));
-  };
-  if (!rc) rc = pool_alloc(c, KK * C * cp * 2, &tmp[2], st);
-  if (!rc) {
-    wp.w = w; wp.out = tmp[2];
-    wp.s_co = ws[0]; wp.s_kz = ws[1]; wp.s_ky = ws[2]; wp.s_kx = ws[3]; wp.s_c = ws[4];
-    wp.C = C; wp.Cout = Cout; wp.cp = cp;
-    CUfunction f;
-    rc = get_func(c, "conv3d_dgrad_weights", &f);
-    void* kargs[] = {&wp};
-    if (!rc) rc = launch(c, f, (unsigned)(((C + 31) / 32) * ((cp + 31) / 32)), (unsigned)KK, 1, 256, 0, 1, st, kargs);
-  }
+  Dgrad3Prep prep(ph, K, sv, pv, dv, C, cp);
+  if (!rc) rc = dgrad3_prep(c, st, w, ws, Cout, KK, &prep, &tmp[2]);
   // one stride-1 convolution of dy per phase that has taps and pixels
-  const bool stride1 = sv[0] == 1 && sv[1] == 1 && sv[2] == 1;
   for (const DgradPhase1D& pd : ph[0])
     for (const DgradPhase1D& phh : ph[1])
       for (const DgradPhase1D& pw : ph[2]) {
         if (rc) break;
         const DgradPhase1D* q[3] = {&pd, &phh, &pw};
         if (!pd.extent || !phh.extent || !pw.extent || !pd.taps || !phh.taps || !pw.taps) continue;
-        const uint64_t T[3] = {pd.taps, phh.taps, pw.taps}, E[3] = {pd.extent, phh.extent, pw.extent};
-        const int32_t one[3] = {1, 1, 1}, pp[3] = {(int32_t)-pd.e0, (int32_t)-phh.e0, (int32_t)-pw.e0};
-        const int32_t dil[3] = {(int32_t)pd.dil, (int32_t)phh.dil, (int32_t)pw.dil};
-        ConvGeom g = conv3_geom(N, O, cp, T, E, C, one, pp, dil);
-        g.x_sw = y.s_w; g.x_sh = y.s_h; g.x_sd = y.s_d; g.x_sn = y.s_n;
-        g.w_sp = cp; g.w_sco = T[0] * T[1] * T[2] * cp;
-        g.box = true; g.lo_d = (int32_t)pd.e0; g.lo_h = (int32_t)phh.e0; g.lo_w = (int32_t)pw.e0;
-        g.mode = stride1 ? 0 : 1;
-        g.dx_sn = os[0]; g.dx_sd = (uint64_t)sv[0] * os[1]; g.dx_si = (uint64_t)sv[1] * os[2]; g.dx_sj = (uint64_t)sv[2] * os[3];
-        if (c->dry) {
-          std::string line = "conv3d dgrad phase r=(" + std::to_string(pd.r) + "," + std::to_string(phh.r) + "," + std::to_string(pw.r) + ")";
-          const char* tn[3] = {" taps_d=", " taps_h=", " taps_w="};
-          for (int i = 0; i < 3; ++i) {
-            line += tn[i];
-            for (uint32_t t = 0; t < q[i]->taps; ++t) line += (t ? "," : "") + std::to_string(q[i]->kmax - t * q[i]->step);
-          }
-          auto triple = [&](auto f) { return "(" + std::to_string(f(0)) + "," + std::to_string(f(1)) + "," + std::to_string(f(2)) + ")"; };
-          line += " dil=" + triple([&](int i) { return (int64_t)q[i]->dil; });
-          line += " lower=" + triple([&](int i) { return q[i]->e0; });
-          line += " upper=" + triple([&](int i) { return q[i]->e0 + (int64_t)q[i]->extent - (int64_t)O[i]; });
-          line += " extent=" + triple([&](int i) { return (int64_t)q[i]->extent; }) + "\n";
-          c->plan += line;
-        }
-        const GemmProblem gp = conv_problem(in_dtype, out_dtype, y.ptr, tmp[2] + phase_off(pd.r, phh.r, pw.r) * 2,
+        ConvGeom g = dgrad3_geom(N, O, cp, C, q, y, os, sv);
+        if (c->dry) c->plan += dgrad3_phase_line("conv3d dgrad phase", q, O) + "\n";
+        const GemmProblem gp = conv_problem(in_dtype, out_dtype, y.ptr, tmp[2] + prep.off(pd.r, phh.r, pw.r) * 2,
                                             dx + ((uint64_t)pd.r * os[1] + (uint64_t)phh.r * os[2] + (uint64_t)pw.r * os[3]) * osz,
-                                            N * E[0] * E[1] * E[2], C, T[0] * T[1] * T[2] * ((cp + 63) / 64 * 64), os[3], &g);
+                                            N * g.OD * g.OH * g.OW, C, g.KD * g.KH * g.KW * ((cp + 63) / 64 * 64), os[3], &g);
         rc = launch_wgmma(c, st, gp, false, false);
       }
   for (CUdeviceptr t : tmp)
@@ -3465,6 +3540,303 @@ extern "C" int b200_conv3d_backward_weight(b200_ctx* c, b200_stream s, b200_dtyp
   }
   for (CUdeviceptr t : tmp)
     if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMM has drained
+  return rc;
+}
+
+// ------------------------------------------------------------------------------------------------ transposed convolution
+// b200_conv_transpose2d / 3d: the transpose of b200_conv2d / 3d, which is the data gradient's computation with x in dy's
+// role and the output in dx's.  The data gradient's phase plan, limits and weight prep are reused as they are; what differs
+// is the fused epilogue, that a phase no tap reaches stores act(bias) instead of a memset's zeros, and the strided launch:
+// every phase of the layer in one conv2d_tconv_* / conv3d_tconv_* launch (gemm_wgmma.cu: CB_TCONV).
+
+// One output phase: its per-dimension phases (D, H, W; a 2-D layer has a unit depth phase), pixels, k-blocks, the element
+// offset of its weight block and the address of its first output pixel.
+struct TconvRun {
+  const DgradPhase1D* q[3];
+  uint64_t M, num_kb, woff, out;
+};
+
+// The phase-batched launches of a strided transposed convolution: the runs sorted by k-blocks (most first, ties in phase
+// order), kTconvMaxPhases per launch.  x is read through xo (extents X = (D, H, W), 2-D: D = 1), the weight blocks from wbuf
+// ([Cout][taps][cp] per phase); dx_s = output strides (n, d, h, w) of one phase's pixel grid, pitch = the output pixel pitch.
+static int launch_tconv(b200_ctx* c, CUstream st, int dims, b200_dtype in_dtype, b200_dtype out_dtype, const NdhwcOperand& xo, uint64_t N,
+                        const uint64_t X[3], uint64_t Cout, CUdeviceptr wbuf, std::vector<TconvRun> runs, const uint64_t dx_s[4], uint64_t pitch,
+                        const b200_epilogue* ep) {
+  const size_t osz = dtype_size(out_dtype);
+  const uint64_t cp = xo.C, cblk = (cp + 63) / 64;
+  std::stable_sort(runs.begin(), runs.end(), [](const TconvRun& a, const TconvRun& b) { return a.num_kb > b.num_kb; });
+  // the tile: the GEMM's wave model (whole tiles, no stream-K head) over the layer's pixels and its longest phase
+  ConvGeom cg_probe{};
+  GemmProblem gp = conv_problem(in_dtype, out_dtype, 0, 0, 0, 0, Cout, std::max<uint64_t>(1, runs[0].num_kb) * 64, pitch, &cg_probe);
+  for (const TconvRun& r : runs) gp.M += r.M;
+  // gemm.split_k is validated as for every GEMM, though these launches plan no stream-K head (their tiles differ in k-blocks)
+  const std::string split_opt = opt(c, "gemm.split_k", "auto");
+  const int split_n = atoi(split_opt.c_str());
+  if (split_opt != "auto" && split_opt != "off" && split_opt != "on" && (split_n < 1 || split_n > 8))
+    return fail(B200_ERR_INVALID_ARG, "gemm.split_k must be auto, off, on or 1..8");
+  SkPlan no_sk;
+  const GemmVariant* vp = pick_variant(c, gp, &no_sk, false);
+  if (!vp) return fail(B200_ERR_INVALID_ARG, "gemm.variant '%s' is not a wgmma variant", opt(c, "gemm.variant", "auto").c_str());
+  const GemmVariant& v = *vp;
+  const char* io = in_dtype == B200_BF16 ? (out_dtype == B200_F32 ? "bf16_f32_" : "bf16_bf16_") : (out_dtype == B200_F32 ? "f16_f32_" : "f16_f16_");
+  CUfunction f;
+  int rc = get_func(c, std::string(dims == 3 ? "conv3d_tconv_" : "conv2d_tconv_") + io + v.tag, &f);
+  if (rc) return rc;
+  const unsigned smem = gemm_smem_bytes(v);
+  if (!c->dry) CU_CHECK(g_drv.cuFuncSetAttribute_p(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem));
+  const CUtensorMapDataType dt = in_dtype == B200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  const uint64_t tiles_n = (Cout + v.block_n - 1) / v.block_n, rows = 128ull * v.cg;
+  static_assert(sizeof(CUtensorMap) == sizeof(TmapBytes), "TmapBytes holds one CUtensorMap");
+  for (size_t g0 = 0; g0 < runs.size() && !rc; g0 += kTconvMaxPhases) {
+    const size_t nq = std::min<size_t>(kTconvMaxPhases, runs.size() - g0);
+    TconvParams tp;
+    memset(&tp, 0, sizeof(tp));
+    GemmParams p;
+    memset(&p, 0, sizeof(p));
+    bool vec = (pitch * osz) % 16 == 0;
+    for (int i = 0; i < 4; ++i) vec = vec && (dx_s[i] * osz) % 16 == 0;
+    uint64_t tiles = 0, pixels = 0;
+    for (size_t k = 0; k < nq && !rc; ++k) {
+      const TconvRun& r = runs[g0 + k];
+      const DgradPhase1D* const* q = r.q;
+      TconvPhase& P = tp.ph[k];
+      P.out = r.out;
+      vec = vec && r.out % 16 == 0;
+      P.tile0 = (uint32_t)tiles;
+      P.tiles_m = (uint32_t)((r.M + rows - 1) / rows);
+      tiles += P.tiles_m * tiles_n;
+      pixels += r.M;
+      P.M = (uint32_t)r.M; P.num_kb = (uint32_t)r.num_kb;
+      P.e_dhw = (uint32_t)(q[0]->extent * q[1]->extent * q[2]->extent); P.e_hw = (uint32_t)(q[1]->extent * q[2]->extent); P.e_w = (uint32_t)q[2]->extent;
+      P.t_hw = q[1]->taps * q[2]->taps; P.t_w = q[2]->taps;
+      P.lo_d = (int32_t)q[0]->e0; P.lo_h = (int32_t)q[1]->e0; P.lo_w = (int32_t)q[2]->e0;
+      P.dil_d = q[0]->dil; P.dil_h = q[1]->dil; P.dil_w = q[2]->dil;
+      if (c->dry) {
+        const std::string head = dims == 3 ? dgrad3_phase_line("conv3d tconv phase", q, X) : dgrad2_phase_line("conv tconv phase", *q[1], *q[2], X[1], X[2]);
+        c->plan += head + " kblocks=" + std::to_string(r.num_kb) + "\n";
+      }
+      if (!r.num_kb) continue;   // no loads: the maps stay empty
+      // x through im2col over the phase's pixel box; the phase's weights as (cp, taps, Cout) in [n_local x 64 channel] boxes
+      CUtensorMap am, bm;
+      int lo[3], up[3];
+      for (int i = 0; i < 3; ++i) {
+        lo[2 - i] = (int)q[i]->e0;
+        up[2 - i] = (int)(q[i]->e0 + (int64_t)q[i]->extent - (int64_t)X[i]);
+      }
+      if (dims == 3) {
+        const uint64_t d5[5] = {cp, X[2], X[1], X[0], N}, s4[4] = {xo.s_w, xo.s_h, xo.s_d, xo.s_n};
+        const uint32_t one[3] = {1, 1, 1};
+        rc = encode_im2col5(c, &am, dt, 2, xo.ptr, d5, s4, lo, up, 64, 128, one);
+      } else {
+        const uint64_t d4[4] = {cp, X[2], X[1], N}, s3[3] = {xo.s_w, xo.s_h, xo.s_n};
+        rc = encode_im2col(c, &am, dt, 2, xo.ptr, d4, s3, lo, up, 64, 128, 1, 1);
+      }
+      const uint64_t taps = (uint64_t)q[0]->taps * q[1]->taps * q[2]->taps;
+      if (!rc) rc = encode_tmap(c, &bm, dt, 2, wbuf + r.woff * 2, cp, taps, Cout, cp, taps * cp, 64, 1, CU_TENSOR_MAP_SWIZZLE_128B, (uint32_t)(v.block_n / v.cg));
+      memcpy(&tp.a[k], &am, sizeof(am));
+      memcpy(&tp.b[k], &bm, sizeof(bm));
+    }
+    if (rc) break;
+    if (tiles >= (1ull << 32)) return fail(B200_ERR_UNSUPPORTED, "too many tiles");
+    tp.phases = (uint32_t)nq;
+    p.out = runs[g0].out;
+    p.out_row_stride = pitch;
+    p.M = (uint32_t)pixels; p.N = (uint32_t)Cout; p.K = 0; p.batch = 1;
+    p.tiles_n = (uint32_t)tiles_n;
+    p.group_m = (uint32_t)std::max(1, atoi(opt(c, "gemm.group_m", "8").c_str()));
+    p.k_segments = 1;
+    p.vec_store = vec ? 1 : 0;
+    p.cv_cblk = (uint32_t)cblk;
+    p.dx_sn = dx_s[0]; p.dx_sd = dx_s[1]; p.dx_si = dx_s[2]; p.dx_sj = dx_s[3];
+    if (ep) { p.alpha = ep->alpha; p.bias = ep->bias; p.epi_act = (uint32_t)ep->activation; }
+    else p.alpha = 1.0f;
+    p.epi_on = (p.alpha != 1.0f || p.bias != 0 || p.epi_act != 0) ? 1u : 0u;
+    p.full_tiles = (uint32_t)tiles;   // whole tiles only: no stream-K head
+    const unsigned clusters = (unsigned)std::min<uint64_t>(tiles, (uint64_t)std::max(1, c->props.num_sms / v.cg));
+    void* args[] = {&tp, &p};
+    rc = launch(c, f, clusters * v.cg, 1, 1, 384, smem, v.cg, st, args);
+  }
+  return rc;
+}
+
+// output_padding = the output extent past the one the conv rule maps back to x's extent; PyTorch also accepts
+// stride <= op < dilation, which this entry point refuses (the conv rule cannot map such an output back to x).
+static int tconv_check_output_padding(const char* what, uint64_t xi, uint64_t oi, int64_t s, int64_t p, int64_t d, uint64_t k) {
+  if (k == 0 || xi == 0) return B200_OK;
+  const int64_t op = (int64_t)oi - (((int64_t)xi - 1) * s - 2 * p + d * ((int64_t)k - 1) + 1);
+  if (op >= s && op < std::max(s, d))
+    return fail(B200_ERR_UNSUPPORTED, "%s: output_padding %lld >= stride %lld is not supported", what, (long long)op, (long long)s);
+  return B200_OK;
+}
+
+// An empty kernel (some extent 0), which the convolution's output rule does not cover: x [N, *X, Cin] and out [N, *O, C] with
+// w [Cin, *K, C], and per dimension O = (X - 1) * s - 2 * p + d * (K - 1) + op + 1 with 0 <= op < s.  The sum is empty, so
+// out is act(bias).  rank 4 or 5.
+static int tconv_check_empty_kernel(const char* what, int rank, const uint64_t* x, const uint64_t* w, const uint64_t* out,
+                                    const int64_t* s, const int64_t* p, const int64_t* d) {
+  const int n = rank - 2;
+  bool ok = x[0] == out[0] && x[rank - 1] == w[0] && w[rank - 1] == out[rank - 1];
+  for (int i = 0; i < n && ok; ++i) {
+    const int64_t op = (int64_t)out[1 + i] - (((int64_t)x[1 + i] - 1) * s[i] - 2 * p[i] + d[i] * ((int64_t)w[1 + i] - 1) + 1);
+    ok = op >= 0 && op < s[i];
+  }
+  if (!ok) return fail(B200_ERR_INVALID_ARG, "%s: with an empty kernel, out must be x's batch and the transposed output rule's extents", what);
+  return B200_OK;
+}
+
+extern "C" int b200_conv_transpose2d(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr x,
+                                     const uint64_t* x_shape, const uint64_t* x_strides, b200_dptr w, const uint64_t* w_shape,
+                                     const uint64_t* w_strides, b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides,
+                                     const b200_conv2d_args* args, const b200_epilogue* ep) {
+  CTX_ENTER(c);
+  const char* what = "conv_transpose2d";
+  if (!x_shape || !w_shape || !out_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
+  const b200_conv2d_args& a = *args;
+  // the data gradient's names: dy = x [N, OH, OW, Cin], w [Cin, KH, KW, C], dx = out [N, H, W, C]
+  const uint64_t N = out_shape[0], H = out_shape[1], W = out_shape[2], C = out_shape[3];
+  const uint64_t Cin = w_shape[0], KH = w_shape[1], KW = w_shape[2];
+  uint64_t OH = 0, OW = 0;
+  int rc = conv_check_args(what, in_dtype, out_dtype, a, ep, C, w_shape[3]);
+  if (!rc) rc = tconv_check_output_padding(what, x_shape[1], H, a.stride_h, a.pad_h, a.dilation_h, KH);
+  if (!rc) rc = tconv_check_output_padding(what, x_shape[2], W, a.stride_w, a.pad_w, a.dilation_w, KW);
+  if (!rc) rc = conv_check_shape(what, a, out_shape, w_shape, x_shape, "x", &OH, &OW);
+  if (!rc && (KH == 0 || KW == 0)) {
+    const int64_t sv[2] = {a.stride_h, a.stride_w}, pv[2] = {a.pad_h, a.pad_w}, dv[2] = {a.dilation_h, a.dilation_w};
+    rc = tconv_check_empty_kernel(what, 4, x_shape, w_shape, out_shape, sv, pv, dv);
+    OH = x_shape[1]; OW = x_shape[2];
+  }
+  if (!rc) rc = conv_check_stride(what, a);   // whatever the kernel: it also bounds the phases per dimension
+  if (rc) return rc;
+  if (N == 0 || H == 0 || W == 0 || C == 0) return B200_OK;   // no output
+  const uint64_t lim = 1ull << 31;
+  if (N * H * W >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * OH * OW = %llu must be < 2^31", what, (unsigned long long)(N * H * W));
+  if (KH * KW * ((Cin + 63) / 64 * 64) >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: KH * KW * Cin (Cin padded to 64) must be < 2^31", what);
+  std::vector<DgradPhase1D> phs, pws;
+  bool zero_phase = false;
+  if ((rc = dgrad2_plan(what, a, H, W, KH, KW, OH, OW, Cin, &phs, &pws, &zero_phase))) return rc;
+  if ((rc = conv_check_ptrs(what, x, w, out, "output", out_dtype))) return rc;
+  const size_t osz = dtype_size(out_dtype);
+  uint64_t os[4], xs[4], ws[4];
+  conv_norm_strides(out_shape, out_strides, os);
+  if ((rc = conv_check_pixels(what, "out", out_shape, os))) return rc;
+  CUstream st = resolve_stream(c, s);
+  const bool taps = Cin != 0 && KH != 0 && KW != 0;
+  conv_norm_strides(x_shape, x_strides, xs);
+  conv_norm_strides(w_shape, w_strides, ws);
+  CUdeviceptr tmp[3] = {0, 0, 0};
+  NhwcOperand y{};
+  ConvDgradWeightsParams wp;
+  memset(&wp, 0, sizeof(wp));
+  if (taps) {
+    rc = conv_prep_nhwc(c, st, in_dtype, x, x_shape, xs, kFlatNone, tmp, &y);
+    if (!rc) rc = dgrad2_prep(c, st, w, ws, a, C, Cin, y.C, KH, KW, phs, pws, &tmp[2], &wp);
+  }
+  if (!rc && taps && a.stride_h == 1 && a.stride_w == 1) {
+    // one phase with every tap: the forward convolution kernel with the epilogue
+    const DgradPhase1D &ph = phs[0], &pw = pws[0];
+    ConvGeom g = dgrad2_geom(N, OH, OW, y.C, C, ph, pw, y, os, a);
+    if (c->dry) c->plan += dgrad2_phase_line("conv tconv phase", ph, pw, OH, OW) + " kblocks=" +
+                           std::to_string((uint64_t)ph.taps * pw.taps * ((y.C + 63) / 64)) + "\n";
+    GemmProblem gp = conv_problem(in_dtype, out_dtype, y.ptr, tmp[2], out, N * H * W, C, KH * KW * ((y.C + 63) / 64 * 64), os[2], &g);
+    if (ep) { gp.alpha = ep->alpha; gp.bias = ep->bias; gp.act = (uint32_t)ep->activation; }
+    rc = launch_wgmma(c, st, gp, false, false);
+  } else if (!rc) {
+    // every phase with pixels, those no tap reaches included, in phase-batched launches
+    static const DgradPhase1D unit = {0, 1, 0, 0, 1, 1, 1};
+    std::vector<TconvRun> runs;
+    const uint64_t cblk = taps ? (y.C + 63) / 64 : 0;
+    for (const DgradPhase1D& ph : phs)
+      for (const DgradPhase1D& pw : pws) {
+        if (!ph.extent || !pw.extent) continue;
+        TconvRun r{{&unit, &ph, &pw}, N * ph.extent * pw.extent, (uint64_t)ph.taps * pw.taps * cblk,
+                   taps ? wp.off[ph.r * a.stride_w + pw.r] : 0, out + ((uint64_t)ph.r * os[1] + (uint64_t)pw.r * os[2]) * osz};
+        runs.push_back(r);
+      }
+    if (!taps) y = NhwcOperand{0, 8, 8, 8, 8};
+    const uint64_t X[3] = {1, OH, OW};
+    const uint64_t dx_s[4] = {os[0], 0, (uint64_t)a.stride_h * os[1], (uint64_t)a.stride_w * os[2]};
+    const NdhwcOperand xo{y.ptr, y.C, y.s_w, y.s_h, 0, y.s_n};
+    rc = launch_tconv(c, st, 2, in_dtype, out_dtype, xo, N, X, C, tmp[2], runs, dx_s, os[2], ep);
+  }
+  for (CUdeviceptr t : tmp)
+    if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMMs have drained
+  return rc;
+}
+
+extern "C" int b200_conv_transpose3d(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr x,
+                                     const uint64_t* x_shape, const uint64_t* x_strides, b200_dptr w, const uint64_t* w_shape,
+                                     const uint64_t* w_strides, b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides,
+                                     const b200_conv3d_args* args, const b200_epilogue* ep) {
+  CTX_ENTER(c);
+  const char* what = "conv_transpose3d";
+  if (!x_shape || !w_shape || !out_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
+  const b200_conv3d_args& a = *args;
+  // the data gradient's names: dy = x [N, OD, OH, OW, Cin], w [Cin, KD, KH, KW, C], dx = out [N, D, H, W, C]
+  const uint64_t N = out_shape[0], C = out_shape[4], Cin = w_shape[0];
+  const uint64_t I[3] = {out_shape[1], out_shape[2], out_shape[3]}, K[3] = {w_shape[1], w_shape[2], w_shape[3]};
+  const int64_t sv[3] = {a.stride_d, a.stride_h, a.stride_w}, pv[3] = {a.pad_d, a.pad_h, a.pad_w};
+  const int64_t dv[3] = {a.dilation_d, a.dilation_h, a.dilation_w};
+  uint64_t O[3] = {0, 0, 0};
+  int rc = conv3_check_args(what, in_dtype, out_dtype, a, ep, C, w_shape[4]);
+  for (int i = 0; i < 3 && !rc; ++i) rc = tconv_check_output_padding(what, x_shape[1 + i], I[i], sv[i], pv[i], dv[i], K[i]);
+  if (!rc) rc = conv3_check_shape(what, a, out_shape, w_shape, x_shape, "x", O);
+  if (!rc && (K[0] == 0 || K[1] == 0 || K[2] == 0)) {
+    rc = tconv_check_empty_kernel(what, 5, x_shape, w_shape, out_shape, sv, pv, dv);
+    for (int i = 0; i < 3; ++i) O[i] = x_shape[1 + i];
+  }
+  if (!rc) rc = conv3_check_stride(what, a);   // whatever the kernel: it also bounds the phases per dimension (Dgrad3Prep)
+  if (rc) return rc;
+  if (N == 0 || I[0] == 0 || I[1] == 0 || I[2] == 0 || C == 0) return B200_OK;   // no output
+  const uint64_t lim = 1ull << 31, P = N * I[0] * I[1] * I[2], KK = K[0] * K[1] * K[2];
+  if (P >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * OD * OH * OW = %llu must be < 2^31", what, (unsigned long long)P);
+  if (KK * ((Cin + 63) / 64 * 64) >= lim)
+    return fail(B200_ERR_UNSUPPORTED, "%s: KD * KH * KW * Cin (Cin padded to 64) must be < 2^31", what);
+  std::vector<DgradPhase1D> ph[3];
+  bool zero_phase = false;
+  if ((rc = dgrad3_plan(what, sv, pv, dv, I, K, O, Cin, ph, &zero_phase))) return rc;
+  if ((rc = conv_check_ptrs(what, x, w, out, "output", out_dtype))) return rc;
+  const size_t osz = dtype_size(out_dtype);
+  uint64_t os[5], xs[5], ws[5];
+  conv3_norm_strides(out_shape, out_strides, os);
+  if ((rc = conv3_check_pixels(what, "out", out_shape, os))) return rc;
+  CUstream st = resolve_stream(c, s);
+  const bool taps = Cin != 0 && KK != 0;
+  conv3_norm_strides(x_shape, x_strides, xs);
+  conv3_norm_strides(w_shape, w_strides, ws);
+  CUdeviceptr tmp[3] = {0, 0, 0};
+  NdhwcOperand y{};
+  // the weight prep (and its per-phase offsets) only when some phase has taps
+  std::unique_ptr<Dgrad3Prep> prep;
+  if (taps) {
+    rc = conv3_prep(c, st, in_dtype, x, x_shape, xs, kFlatNone, tmp, &y);
+    prep.reset(new Dgrad3Prep(ph, K, sv, pv, dv, C, y.C));
+    if (!rc) rc = dgrad3_prep(c, st, w, ws, Cin, KK, prep.get(), &tmp[2]);
+  }
+  if (!rc && taps && sv[0] == 1 && sv[1] == 1 && sv[2] == 1) {
+    const DgradPhase1D* q[3] = {&ph[0][0], &ph[1][0], &ph[2][0]};
+    ConvGeom g = dgrad3_geom(N, O, y.C, C, q, y, os, sv);
+    if (c->dry) c->plan += dgrad3_phase_line("conv3d tconv phase", q, O) + " kblocks=" + std::to_string(KK * ((y.C + 63) / 64)) + "\n";
+    GemmProblem gp = conv_problem(in_dtype, out_dtype, y.ptr, tmp[2], out, P, C, KK * ((y.C + 63) / 64 * 64), os[3], &g);
+    if (ep) { gp.alpha = ep->alpha; gp.bias = ep->bias; gp.act = (uint32_t)ep->activation; }
+    rc = launch_wgmma(c, st, gp, false, false);
+  } else if (!rc) {
+    std::vector<TconvRun> runs;
+    const uint64_t cblk = taps ? (y.C + 63) / 64 : 0;
+    for (const DgradPhase1D& pd : ph[0])
+      for (const DgradPhase1D& phh : ph[1])
+        for (const DgradPhase1D& pw : ph[2]) {
+          if (!pd.extent || !phh.extent || !pw.extent) continue;
+          TconvRun r{{&pd, &phh, &pw}, N * pd.extent * phh.extent * pw.extent, (uint64_t)pd.taps * phh.taps * pw.taps * cblk,
+                     taps ? prep->off(pd.r, phh.r, pw.r) : 0,
+                     out + ((uint64_t)pd.r * os[1] + (uint64_t)phh.r * os[2] + (uint64_t)pw.r * os[3]) * osz};
+          runs.push_back(r);
+        }
+    if (!taps) y = NdhwcOperand{0, 8, 8, 8, 8, 8};
+    const uint64_t dx_s[4] = {os[0], (uint64_t)sv[0] * os[1], (uint64_t)sv[1] * os[2], (uint64_t)sv[2] * os[3]};
+    rc = launch_tconv(c, st, 3, in_dtype, out_dtype, y, N, O, C, tmp[2], runs, dx_s, os[3], ep);
+  }
+  for (CUdeviceptr t : tmp)
+    if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMMs have drained
   return rc;
 }
 

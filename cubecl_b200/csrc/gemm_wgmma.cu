@@ -156,16 +156,46 @@ enum : int { QM_NONE = 0, QM_BLOCK = 1, QM_TENSOR = 2 };
 // CONV_DIMS (capi.cpp: b200_conv3d*): 3 runs the CONV producer, CB_DGRAD epilogue and CB_WGRAD producer over a 3-D convolution
 // -- 5-D im2col loads (C, W, H, D, N) with offsets (kx dw, ky dh, kz dd), pixels and kernel positions decoded with the depth
 // term (GemmParams cv_odhw, cv_khw, dx_sd).  2 is the 2-D convolution; every other stage of the kernel is the same.
-enum : int { CB_NONE = 0, CB_DGRAD = 1, CB_WGRAD = 2 };
+//   CB_TCONV  transposed convolution, every stride phase of a layer in one launch (TconvParams, kernel_params.h): per tile
+//             the producer finds the tile's phase and loads through that phase's im2col and weight maps; the consumers run
+//             the phase's own k-block count from zeroed accumulators (a phase no tap reaches runs none and stores
+//             act(bias)), then store as CB_DGRAD at the phase's rows.
+enum : int { CB_NONE = 0, CB_DGRAD = 1, CB_WGRAD = 2, CB_TCONV = 3 };
+
+// phase of tile t in a transposed-convolution launch (phases in table order, tiles in one list)
+__device__ __forceinline__ uint32_t tconv_phase(uint32_t t, const TconvParams& tp) {
+  uint32_t q = 0;
+  while (q + 1 < tp.phases && t >= tp.ph[q + 1].tile0) ++q;
+  return q;
+}
+// tile_coord inside one phase's grid of tiles_m x p.tiles_n tiles
+__device__ __forceinline__ TileCoord tconv_coord(uint32_t loc, uint32_t tiles_m, const GemmParams& p) {
+  const uint32_t strip = p.group_m * p.tiles_n, g = loc / strip, first_m = g * p.group_m;
+  const uint32_t gsize = min(p.group_m, tiles_m - first_m), in = loc - g * strip;
+  TileCoord c;
+  c.b = 0;
+  c.m_blk = first_m + in % gsize;
+  c.n_blk = in / gsize;
+  return c;
+}
+// tile t's coordinate: in phase q's grid for a transposed convolution, tile_coord otherwise
+template <int CB>
+__device__ __forceinline__ TileCoord unit_coord(uint32_t t, const GemmParams& p, const TconvParams* tcp, uint32_t q) {
+  if constexpr (CB == CB_TCONV) return tconv_coord(t - tcp->ph[q].tile0, tcp->ph[q].tiles_m, p);
+  else return tile_coord(t, p);
+}
+
 template <int CG, int BLOCK_N, bool A_MN, bool B_MN, int KIND, int OUT, int STAGES, bool PROMOTE = false, int MT = 1, int QM = QM_NONE,
           bool CONV = false, int CB = CB_NONE, int CONV_DIMS = 2>
 __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUtensorMap* tma_b_hi, const CUtensorMap* tma_a_lo,
-                                          const CUtensorMap* tma_b_lo, const CUtensorMap* tma_out, const GemmParams& p) {
+                                          const CUtensorMap* tma_b_lo, const CUtensorMap* tma_out, const GemmParams& p,
+                                          const TconvParams* tcp = nullptr) {
   constexpr bool INT_ACC = (KIND == KIND_U8 || KIND == KIND_S8) && QM != QM_BLOCK;
   static_assert(QM == QM_NONE || (KIND == KIND_S8 && !A_MN && !B_MN && !PROMOTE && MT == 1), "quantized operands: s8, K-major");
   static_assert(!CONV || ((KIND == KIND_BF16 || KIND == KIND_F16) && !A_MN && !B_MN && !PROMOTE && MT == 1 && QM == QM_NONE),
                 "convolution: 16-bit kinds, K-major operands");
   static_assert(CB != CB_DGRAD || CONV, "data gradient: the convolution producer");
+  static_assert(CB != CB_TCONV || CONV, "transposed convolution: the convolution producer");
   static_assert(CONV_DIMS == 2 || (CONV_DIMS == 3 && (CONV || CB == CB_WGRAD)), "3-D: the convolution kernels");
   static_assert(CB != CB_WGRAD || (!CONV && A_MN && B_MN && (KIND == KIND_BF16 || KIND == KIND_F16) && !PROMOTE && MT == 1 && QM == QM_NONE),
                 "weight gradient: 16-bit kinds, MN-major operands");
@@ -208,8 +238,10 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
   const uint32_t n_clusters = (CG == 2) ? num_clusters_x() : gridDim.x;
 
   if (threadIdx.x == 0) {
-    tma_prefetch_desc(tma_a_hi);
-    tma_prefetch_desc(tma_b_hi);
+    if (CB != CB_TCONV || tcp->ph[0].num_kb != 0) {   // a transposed-convolution phase without taps has no maps
+      tma_prefetch_desc(tma_a_hi);
+      tma_prefetch_desc(tma_b_hi);
+    }
     if (p.k_segments > 1) { tma_prefetch_desc(tma_a_lo); tma_prefetch_desc(tma_b_lo); }
     if constexpr (QM == QM_BLOCK) { tma_prefetch_desc(tma_a_lo); tma_prefetch_desc(tma_b_lo); }
     if (p.tma_store) tma_prefetch_desc(tma_out);
@@ -243,6 +275,51 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
       UnitIter it = unit_iter(cluster_id, n_clusters, num_kb);
       WorkUnit wu;
       while (next_unit(it, p, wu)) {
+        if constexpr (CB == CB_TCONV) {
+          // transposed convolution: the tile's phase, and its first pixel decoded with the phase's extents, once per tile;
+          // per k-block the phase's im2col load at offsets (tap * dilation) and its weight load, as the data gradient
+          const uint32_t q = tconv_phase(wu.tile, *tcp);
+          const TconvPhase& P = tcp->ph[q];
+          const TileCoord tc = tconv_coord(wu.tile - P.tile0, P.tiles_m, p);
+          const uint32_t mu = (tc.m_blk * CG + rank) * 128u;
+          const int n_row = static_cast<int>(tc.n_blk * BLOCK_N + rank * N_LOCAL);
+          const CUtensorMap* am = reinterpret_cast<const CUtensorMap*>(&tcp->a[q]);
+          const CUtensorMap* bm = reinterpret_cast<const CUtensorMap*>(&tcp->b[q]);
+          int cv_w, cv_h, cv_d = 0, cv_n;
+          if constexpr (CONV_DIMS == 3) {
+            const uint32_t n = mu / P.e_dhw, r0 = mu - n * P.e_dhw, a = r0 / P.e_hw, r = r0 - a * P.e_hw, i = r / P.e_w;
+            cv_n = static_cast<int>(n);
+            cv_d = static_cast<int>(a) + P.lo_d;
+            cv_h = static_cast<int>(i) + P.lo_h;
+            cv_w = static_cast<int>(r - i * P.e_w) + P.lo_w;
+          } else {
+            const uint32_t n = mu / P.e_hw, r = mu - n * P.e_hw, i = r / P.e_w;
+            cv_n = static_cast<int>(n);
+            cv_h = static_cast<int>(i) + P.lo_h;
+            cv_w = static_cast<int>(r - i * P.e_w) + P.lo_w;
+          }
+          for (uint32_t kb = 0; kb < P.num_kb; ++kb) {
+            mbar_wait(empty_bar(s), ph ^ 1);
+            const uint32_t sa = smem_base + s * STAGE_BYTES;
+            const uint32_t sb = sa + A_BYTES;
+            const uint32_t fb = full_bar(s);
+            mbar_arrive_expect_tx(fb, STAGE_BYTES);
+            const uint32_t kpos = kb / p.cv_cblk, cb = kb - kpos * p.cv_cblk;
+            const int c0 = static_cast<int>(cb * 64u);
+            if constexpr (CONV_DIMS == 3) {
+              const uint32_t tz = kpos / P.t_hw, tr = kpos - tz * P.t_hw, ty = tr / P.t_w, tx = tr - ty * P.t_w;
+              tma_load_im2col_5d(sa, am, fb, c0, cv_w, cv_h, cv_d, cv_n, static_cast<uint16_t>(tx * P.dil_w),
+                                 static_cast<uint16_t>(ty * P.dil_h), static_cast<uint16_t>(tz * P.dil_d));
+            } else {
+              const uint32_t ty = kpos / P.t_w, tx = kpos - ty * P.t_w;
+              tma_load_im2col_4d(sa, am, fb, c0, cv_w, cv_h, cv_n, static_cast<uint16_t>(tx * P.dil_w), static_cast<uint16_t>(ty * P.dil_h));
+            }
+            if constexpr (CG == 2) tma_load_3d_mc(sb + rank * N_LOCAL * 128u, bm, fb, static_cast<uint16_t>(3), c0, static_cast<int>(kpos), n_row);
+            else tma_load_3d(sb, bm, fb, c0, static_cast<int>(kpos), n_row);
+            if (++s == STAGES) { s = 0; ph ^= 1; }
+          }
+          continue;
+        }
         const TileCoord tc = tile_coord(wu.tile, p);
         const int m0 = static_cast<int>((tc.m_blk * CG + rank) * (128 * MT));
         const int nb0 = static_cast<int>(tc.n_blk * BLOCK_N);
@@ -419,7 +496,17 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
     UnitIter it = unit_iter(cluster_id, n_clusters, num_kb);
     WorkUnit wu;
     while (next_unit(it, p, wu)) {
-      const TileCoord tc = tile_coord(wu.tile, p);
+      // transposed convolution: the tile's phase, its k-blocks and its pixel count; tq_keep masks the accumulators of a tile
+      // without k-blocks to +0
+      uint32_t tq = 0, tq_m = 0, tq_keep = 0;
+      if constexpr (CB == CB_TCONV) {
+        tq = tconv_phase(wu.tile, *tcp);
+        wu.kb0 = 0;
+        wu.kb1 = tcp->ph[tq].num_kb;
+        tq_m = tcp->ph[tq].M;
+        tq_keep = wu.kb1 != 0 ? 0xFFFFFFFFu : 0u;
+      }
+      const TileCoord tc = unit_coord<CB>(wu.tile, p, tcp, tq);
       uint32_t seg = 0, kk = 0;
       if constexpr (KIND == KIND_TF32) seg_of(wu.kb0, seg, kk);
       uint32_t prev = 0;
@@ -547,7 +634,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
         wgmma_wait<0>();
 #pragma unroll
         for (int mt = 0; mt < MT; ++mt) wgmma_fence_operands(acc[mt]);
-        release(prev);
+        if (CB != CB_TCONV || wu.kb1 != wu.kb0) release(prev);   // a tile without k-blocks holds no stage
       }
 
       // fragment of m64nNk*: thread (warp wq, lane) holds rows 16 wq + lane / 4 (+8) and column pairs 8 j + 2 (lane % 4)
@@ -584,6 +671,19 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
           const uint32_t n = r / p.cv_ohw, rr = r - n * p.cv_ohw, i = rr / p.cv_ow, j = rr - i * p.cv_ow;
           dg_row[h] = p.out + (n * p.dx_sn + i * p.dx_si + j * p.dx_sj) * osz;
         }
+      } else if constexpr (CB == CB_TCONV) {
+        const TconvPhase& P = tcp->ph[tq];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const uint32_t r = m_cta + cw * 64u + wq * 16u + (lane >> 2) + 8u * h;
+          if constexpr (CONV_DIMS == 3) {
+            const uint32_t n = r / P.e_dhw, r0 = r - n * P.e_dhw, a = r0 / P.e_hw, rr = r0 - a * P.e_hw, i = rr / P.e_w, j = rr - i * P.e_w;
+            dg_row[h] = P.out + (n * p.dx_sn + a * p.dx_sd + i * p.dx_si + j * p.dx_sj) * osz;
+          } else {
+            const uint32_t n = r / P.e_hw, rr = r - n * P.e_hw, i = rr / P.e_w, j = rr - i * P.e_w;
+            dg_row[h] = P.out + (n * p.dx_sn + i * p.dx_si + j * p.dx_sj) * osz;
+          }
+        }
       }
       // direct stores of fragment group j of sub-tile mt
       auto store_group = [&](int mt, int j, uint32_t (&v)[4]) {
@@ -594,6 +694,9 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
         if constexpr (CB == CB_DGRAD) {
           if (r0 < p.M) store_pair<OUT>(dg_row[0], n, p.N, p.vec_store != 0, v[0], v[1]);
           if (r0 + 8 < p.M) store_pair<OUT>(dg_row[1], n, p.N, p.vec_store != 0, v[2], v[3]);
+        } else if constexpr (CB == CB_TCONV) {
+          if (r0 < tq_m) store_pair<OUT>(dg_row[0], n, p.N, p.vec_store != 0, v[0], v[1]);
+          if (r0 + 8 < tq_m) store_pair<OUT>(dg_row[1], n, p.N, p.vec_store != 0, v[2], v[3]);
         } else if constexpr (CB == CB_WGRAD) {
           // virtual column n = (kpos, ch): dw row r0, element kpos * dw_sp + ch; channels ch >= C are dropped (a pair never
           // straddles two kernel positions)
@@ -611,12 +714,18 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
           if constexpr (QM == QM_TENSOR) v[e] = __float_as_uint(__fmul_rn(__int2float_rn(static_cast<int>(acc[mt][4 * j + e])), gab));
+          // transposed convolution: a tile without k-blocks (a phase no tap reaches) sums to +0 -- read as such through a
+          // mask, as no wgmma has cleared the accumulators (writing them on this data-dependent path would serialise every
+          // wgmma; a select here is hoisted out of the store loop, which then no longer unrolls)
+          else if constexpr (CB == CB_TCONV) v[e] = acc_bits(acc[mt][4 * j + e]) & tq_keep;
           else v[e] = acc_bits(acc[mt][4 * j + e]);
         }
       };
-      const bool partial = (MT == 1) && !INT_ACC && QM == QM_NONE && wu.partial;   // the host plans no stream-K head for these
+      // the host plans no stream-K head for these (nor for CB_TCONV, whose units are all whole tiles: the path stays compiled
+      // there all the same, as without it the direct-store loop below is not unrolled and the accumulators move to local memory)
+      const bool partial = (MT == 1) && !INT_ACC && QM == QM_NONE && wu.partial;
 
-      if (CB != CB_DGRAD && !partial && p.tma_store) {
+      if (CB != CB_DGRAD && CB != CB_TCONV && !partial && p.tma_store) {
         // fragments -> (epilogue, convert) -> 128B-swizzled [64 rows x 128 B] staging tile -> one TMA store per 128-byte column
         // group; the TMA unit clips ragged edges.  A direct store writes 16 bytes per row per instruction, 8 rows apart.
         const uint32_t stage_smem = epi_base + cw * 8192u;
@@ -850,7 +959,22 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
   CONV_BWD_KERNEL(conv2d_wgrad_f16_f16_##TILE, CG, BN, true, KIND_F16, OUT_F16, STAGES, false, CB_WGRAD)       \
   CONV_BWD_KERNEL(conv2d_wgrad_f16_f32_##TILE, CG, BN, true, KIND_F16, OUT_F32, STAGES, false, CB_WGRAD)
 
-// The kernels are built as seven cubins from this one source (cubecl_b200/build.py compiles them in parallel):
+// Transposed convolution, stride > 1: every phase of a layer in one launch.  The im2col and weight maps of each phase are
+// in the TconvParams parameter; names conv2d_tconv_<in>_<out>_<tile> (4-D im2col) and conv3d_tconv_* (5-D)
+#define TCONV_KERNEL(NAME, CG, BN, KIND, OUT, STAGES, DIMS)                                                        \
+  extern "C" __global__ void __launch_bounds__(kNumThreads, 1)                                                     \
+      NAME(const __grid_constant__ TconvParams tp, const __grid_constant__ GemmParams p) {                         \
+    const CUtensorMap* a0 = reinterpret_cast<const CUtensorMap*>(&tp.a[0]);                                        \
+    const CUtensorMap* b0 = reinterpret_cast<const CUtensorMap*>(&tp.b[0]);                                        \
+    gemm_body<CG, BN, false, false, KIND, OUT, STAGES, false, 1, QM_NONE, true, CB_TCONV, DIMS>(a0, b0, a0, b0, a0, p, &tp); \
+  }
+#define TCONV_DTYPES(TILE, CG, BN, STAGES, DIMS, PFX)                                        \
+  TCONV_KERNEL(PFX##_tconv_bf16_bf16_##TILE, CG, BN, KIND_BF16, OUT_BF16, STAGES, DIMS)      \
+  TCONV_KERNEL(PFX##_tconv_bf16_f32_##TILE, CG, BN, KIND_BF16, OUT_F32, STAGES, DIMS)        \
+  TCONV_KERNEL(PFX##_tconv_f16_f16_##TILE, CG, BN, KIND_F16, OUT_F16, STAGES, DIMS)          \
+  TCONV_KERNEL(PFX##_tconv_f16_f32_##TILE, CG, BN, KIND_F16, OUT_F32, STAGES, DIMS)
+
+// The kernels are built as eight cubins from this one source (cubecl_b200/build.py compiles them in parallel):
 //   GEMM_PART 0 ("gemm")       256 x 256 pair tiles (2-CTA cluster, 128 x 256 per CTA) and the bf16 peak probe
 //   GEMM_PART 1 ("gemm_b")     256 x 128 pair tiles, 256 x 224 block-scaled pair tiles
 //   GEMM_PART 2 ("gemm_c")     128 x 128 single-CTA tiles, 512 x 128 pair tiles
@@ -858,6 +982,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
 //   GEMM_PART 4 ("gemm_conv")  the 2-D convolution kernels of the 2sm_n128 and 1sm_n128 tiles
 //   GEMM_PART 5 ("gemm_convbwd")  the convolution backward kernels (data and weight gradients) of the same two tiles
 //   GEMM_PART 6 ("gemm_conv3d")   the 3-D convolution kernels (forward, data and weight gradients) of the same two tiles
+//   GEMM_PART 7 ("gemm_convt")    the phase-batched transposed-convolution kernels, 2-D and 3-D, of the same two tiles
 #ifndef GEMM_PART
 #define GEMM_PART 0
 #endif
@@ -914,6 +1039,12 @@ CONV_BWD_DTYPES(1sm_n128, 1, 128, 6)
 #if GEMM_PART == 6
 CONV3D_DTYPES(2sm_n128, 2, 128, 6)
 CONV3D_DTYPES(1sm_n128, 1, 128, 6)
+#endif
+#if GEMM_PART == 7
+TCONV_DTYPES(2sm_n128, 2, 128, 6, 2, conv2d)
+TCONV_DTYPES(1sm_n128, 1, 128, 6, 2, conv2d)
+TCONV_DTYPES(2sm_n128, 2, 128, 6, 3, conv3d)
+TCONV_DTYPES(1sm_n128, 1, 128, 6, 3, conv3d)
 #endif
 
 #if GEMM_PART == 0

@@ -171,6 +171,36 @@ struct Conv3dDgradWeightsParams {
   uint32_t kmax[3][kDgradMaxStride], taps[3][kDgradMaxStride];
 };
 
+// Transposed convolution with stride > 1 (conv2d_tconv_* / conv3d_tconv_*; capi.cpp: b200_conv_transpose2d / 3d): up to
+// kTconvMaxPhases output phases of one layer in one launch.  Each phase is the stride-1 convolution a data-gradient phase
+// runs (x in dy's role, the conv_dgrad_weights / conv3d_dgrad_weights block of the phase as its weights).  The tiles of all
+// phases form one list, phase after phase in table order (most k-blocks first, so the longest tiles start first); a tile
+// of phase q has local index t - tile0 inside the phase's (tiles_m x GemmParams::tiles_n) grid and runs num_kb k-blocks
+// (0: no tap reaches the phase, the tile stores act(bias)).  GEMM row m of a phase is pixel (n, a, i, j) of its
+// (e_d, e_h, e_w) grid, stored at out + n * dx_sn + a * dx_sd + i * dx_si + j * dx_sj elements (GemmParams strides).
+// The maps live in the launch's parameter space beside GemmParams: 16 maps (2 KB) and the table fit its 4 KB, and a
+// parameter needs no pooled buffer written ahead of the launch.
+constexpr int kTconvMaxPhases = 8;
+struct alignas(64) TmapBytes {   // one CUtensorMap (cuda.h: 128 bytes, 64-byte aligned), filled on the host
+  uint64_t opaque[16];
+};
+struct TconvPhase {
+  uint64_t out;                  // device address of the phase's first pixel (0, rd, rh, rw)
+  uint32_t tile0, tiles_m;       // first tile in the launch's list, tile rows of 128 * CG pixels
+  uint32_t M, num_kb;            // pixels N * e_d * e_h * e_w; k-blocks = taps * GemmParams::cv_cblk
+  uint32_t e_dhw, e_hw, e_w;     // pixel grid: e_d * e_h * e_w, e_h * e_w, e_w
+  uint32_t t_hw, t_w;            // taps: t_h * t_w, t_w (tap index = (tz * t_h + ty) * t_w + tx)
+  int32_t lo_d, lo_h, lo_w;      // x offset of the first tap: the im2col map's lower corner
+  uint32_t dil_d, dil_h, dil_w;  // x offset between consecutive taps
+  uint32_t pad;
+};
+struct TconvParams {
+  TmapBytes a[kTconvMaxPhases];  // im2col map of x per phase (4-D or 5-D)
+  TmapBytes b[kTconvMaxPhases];  // the phase's weights (cp, taps, Cout), [n_local x 64 channels] boxes
+  TconvPhase ph[kTconvMaxPhases];
+  uint32_t phases, pad[3];
+};
+
 // ================================================================================================ conv_grouped.cu
 // Direct NHWC grouped convolution (b200_conv2d_grouped*, group width Cg = C / groups < 64).  Group g owns input channels
 // [g Cg, (g+1) Cg) and output channels [g Coutg, (g+1) Coutg).  Every strided operand has a unit channel stride; strides

@@ -471,6 +471,42 @@ int b200_conv3d_backward_weight(b200_ctx* ctx, b200_stream s, b200_dtype in_dtyp
                                 b200_dptr dw, const uint64_t* dw_shape, const uint64_t* dw_strides,
                                 const b200_conv3d_args* args);
 
+/* ---- transposed convolution, 2-D and 3-D (PyTorch's ConvTranspose2d / 3d), with the fused epilogue -----------------------
+ * out[n, oh, ow, co] = act(alpha * sum_{ih, iw, ky, kx, ci : oh = ih*sh - ph + ky*dh, ow = iw*sw - pw + kx*dw}
+ *                                  x[n, ih, iw, ci] * w[ci, ky, kx, co] + bias[co])
+ * x is [N, H, W, Cin] (NHWC), w is [Cin, KH, KW, Cout] (PyTorch's [Cin, Cout, KH, KW] permuted), out is [N, OH, OW, Cout]
+ * with OH = (H-1)*sh - 2*ph + dh*(KH-1) + oph + 1, 0 <= oph < sh (likewise OW; 3-D adds D / KD / sd / pd / dd / opd with
+ * the NDHWC layouts of b200_conv3d).  output_padding is no argument: out_shape implies it, and exactly the output extents
+ * that b200_conv2d's output rule maps back to x's extents are accepted (PyTorch's stride <= oph < dilation is refused with
+ * B200_ERR_UNSUPPORTED).  A position the sum does not reach is act(bias[co]) (act(0) without a bias).  No groups argument.
+ * This is b200_conv2d_backward_data / b200_conv3d_backward_data with x in dy's role (w has exactly their w layout:
+ * [Cin, KH, KW, Cout] is [Cout_conv, KH, KW, C_conv]) plus the epilogue, and every rule is theirs: dtypes, views, channel
+ * padding, the out pixel-pitch rule, the corner / offset / stride <= 8 / pixel-count limits (each phase's corners), the
+ * error codes; zero extents of out are no-ops.  Unlike there, the stride <= 8 limit holds for every kernel shape, and an
+ * empty kernel (some kernel extent 0, Cin = 0 alike: out is act(bias)) needs x's batch, Cin = w's first extent, C = w's
+ * last, and per dimension the output rule above with 0 <= op < s (B200_ERR_INVALID_ARG otherwise).
+ * Launches: stride 1 in every dimension is one phase: the weight prep (conv_dgrad_weights / conv3d_dgrad_weights) and one
+ *   conv2d_* / conv3d_* forward GEMM with the epilogue.  Stride > 1: the prep and then every phase with pixels, those no tap
+ *   reaches included, in conv2d_tconv_* / conv3d_tconv_* launches of up to 8 phases each (one launch for any stride-2
+ *   layer), phases with the most k-blocks first; no memset.
+ * The dry-run plan records each phase, in walk order, as "conv tconv phase r=(rh,rw) taps_h= taps_w= dil= lower= upper=
+ * extent= kblocks=" (3-D: "conv3d tconv phase r=(rd,rh,rw) taps_d= ...").
+ * Gradients are existing entry points with roles swapped (same args):
+ *   dx    = b200_conv2d(dy, w) -- w read as conv weights with Cout := Cin, no flip;
+ *   dw    = b200_conv2d_backward_weight(x := dy, dy := x);
+ *   dbias = b200_reduce (sum) over axis 0 of dy viewed as [N * OH * OW, Cout].
+ * (3-D: b200_conv3d, b200_conv3d_backward_weight.) */
+int b200_conv_transpose2d(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype,
+                          b200_dptr x, const uint64_t* x_shape, const uint64_t* x_strides,
+                          b200_dptr w, const uint64_t* w_shape, const uint64_t* w_strides,
+                          b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides,
+                          const b200_conv2d_args* args, const b200_epilogue* epilogue);
+int b200_conv_transpose3d(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype,
+                          b200_dptr x, const uint64_t* x_shape, const uint64_t* x_strides,
+                          b200_dptr w, const uint64_t* w_shape, const uint64_t* w_strides,
+                          b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides,
+                          const b200_conv3d_args* args, const b200_epilogue* epilogue);
+
 /* ---- collectives: ServerCommunication (server/base.rs:632-739), CUDA impl cubecl-cuda/src/compute/server.rs:666-926 -- */
 #define B200_UNIQUE_ID_BYTES 128
 int b200_comm_get_unique_id(b200_ctx* ctx, void* id128);            /* ncclGetUniqueId (communication.rs:11-25 holds it per device set) */

@@ -349,6 +349,34 @@ inline void backward_weight(ComputeClient& client, const TensorHandle& x, const 
 }
 }  // namespace conv3d
 
+namespace conv_transpose {
+/// Transposed convolution, 2-D or 3-D by rank: x [N, (D,) H, W, Cin], w [Cin, (KD,) KH, KW, Cout], out [N, (OD,) OH, OW, Cout]
+/// (out's shape gives the output padding); f32 accumulation, optional fused epilogue.  args: b200_conv2d_args (rank 4) or
+/// b200_conv3d_args (rank 5).  See b200_conv_transpose2d in cubecl_b200.h.  Errors are deferred to client.sync().
+inline void launch(ComputeClient& client, const TensorHandle& x, const TensorHandle& w, const TensorHandle& out,
+                   const b200_conv2d_args& args, const b200_epilogue* epilogue = nullptr) {
+  if (x.shape.size() != 4 || w.shape.size() != 4 || out.shape.size() != 4 || x.dtype != w.dtype) {
+    client.defer("InvalidArgument: conv_transpose2d needs rank-4 x, w and out, and x and w of one dtype");
+    return;
+  }
+  const int rc = b200_conv_transpose2d(client.raw(), nullptr, static_cast<b200_dtype>(x.dtype), static_cast<b200_dtype>(out.dtype),
+                                       x.handle.ptr(), x.shape.data(), x.strides.data(), w.handle.ptr(), w.shape.data(),
+                                       w.strides.data(), out.handle.ptr(), out.shape.data(), out.strides.data(), &args, epilogue);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+inline void launch(ComputeClient& client, const TensorHandle& x, const TensorHandle& w, const TensorHandle& out,
+                   const b200_conv3d_args& args, const b200_epilogue* epilogue = nullptr) {
+  if (x.shape.size() != 5 || w.shape.size() != 5 || out.shape.size() != 5 || x.dtype != w.dtype) {
+    client.defer("InvalidArgument: conv_transpose3d needs rank-5 x, w and out, and x and w of one dtype");
+    return;
+  }
+  const int rc = b200_conv_transpose3d(client.raw(), nullptr, static_cast<b200_dtype>(x.dtype), static_cast<b200_dtype>(out.dtype),
+                                       x.handle.ptr(), x.shape.data(), x.strides.data(), w.handle.ptr(), w.shape.data(),
+                                       w.strides.data(), out.handle.ptr(), out.shape.data(), out.strides.data(), &args, epilogue);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+}  // namespace conv_transpose
+
 namespace reduce {
 enum class Op : int { Sum = B200_REDUCE_SUM, Prod = B200_REDUCE_PROD, Max = B200_REDUCE_MAX, Min = B200_REDUCE_MIN,
                       ArgMax = B200_REDUCE_ARGMAX, ArgMin = B200_REDUCE_ARGMIN, Mean = B200_REDUCE_MEAN };

@@ -487,6 +487,50 @@ impl Context {
         ))
     }
 
+    /// Transposed convolution: x [N, H, W, Cin], w [Cin, KH, KW, Cout] -> out [N, OH, OW, Cout] (out's shape gives the output
+    /// padding), f32 accumulation, optional fused epilogue; `args` as [`Context::conv2d`].  Gradients: dx =
+    /// [`Context::conv2d`] (dy, w), dw = [`Context::conv2d_backward_weight`] (x := dy, dy := x).  See b200_conv_transpose2d
+    /// in cubecl_b200.h.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::conv2d`].
+    pub unsafe fn conv_transpose2d(
+        &mut self, stream: b200_stream, in_dtype: DType, out_dtype: DType, x: &TensorView, w: &TensorView, out: &TensorView,
+        args: [i32; 6], epilogue: Option<&Epilogue>,
+    ) -> Result<(), Error> {
+        assert!(x.shape.len() == 4 && w.shape.len() == 4 && out.shape.len() == 4);
+        assert!(x.strides.len() == 4 && w.strides.len() == 4 && out.strides.len() == 4);
+        let a = sys::b200_conv2d_args {
+            stride_h: args[0], stride_w: args[1], pad_h: args[2], pad_w: args[3], dilation_h: args[4], dilation_w: args[5],
+        };
+        let e = epilogue.map(|e| sys::b200_epilogue { alpha: e.alpha, activation: e.activation as i32, bias: e.bias });
+        check(sys::b200_conv_transpose2d(
+            self.0, stream, in_dtype as c_int, out_dtype as c_int, x.ptr, x.shape.as_ptr(), x.strides.as_ptr(), w.ptr,
+            w.shape.as_ptr(), w.strides.as_ptr(), out.ptr, out.shape.as_ptr(), out.strides.as_ptr(), &a,
+            e.as_ref().map_or(std::ptr::null(), |e| e as *const sys::b200_epilogue),
+        ))
+    }
+
+    /// 3-D [`Context::conv_transpose2d`]: x [N, D, H, W, Cin], w [Cin, KD, KH, KW, Cout] -> out [N, OD, OH, OW, Cout]; `args`
+    /// as [`Context::conv3d`].  See b200_conv_transpose3d in cubecl_b200.h.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::conv2d`].
+    pub unsafe fn conv_transpose3d(
+        &mut self, stream: b200_stream, in_dtype: DType, out_dtype: DType, x: &TensorView, w: &TensorView, out: &TensorView,
+        args: [i32; 9], epilogue: Option<&Epilogue>,
+    ) -> Result<(), Error> {
+        assert!(x.shape.len() == 5 && w.shape.len() == 5 && out.shape.len() == 5);
+        assert!(x.strides.len() == 5 && w.strides.len() == 5 && out.strides.len() == 5);
+        let a = conv3d_args(args);
+        let e = epilogue.map(|e| sys::b200_epilogue { alpha: e.alpha, activation: e.activation as i32, bias: e.bias });
+        check(sys::b200_conv_transpose3d(
+            self.0, stream, in_dtype as c_int, out_dtype as c_int, x.ptr, x.shape.as_ptr(), x.strides.as_ptr(), w.ptr,
+            w.shape.as_ptr(), w.strides.as_ptr(), out.ptr, out.shape.as_ptr(), out.strides.as_ptr(), &a,
+            e.as_ref().map_or(std::ptr::null(), |e| e as *const sys::b200_epilogue),
+        ))
+    }
+
     /// Grouped / depthwise [`Context::conv2d`]: w [Cout, KH, KW, C / groups].  See b200_conv2d_grouped in cubecl_b200.h.
     ///
     /// # Safety
