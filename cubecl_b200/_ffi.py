@@ -54,6 +54,11 @@ class Conv3dArgs(C.Structure):
                 ("dilation_w", C.c_int32)]
 
 
+class AttentionArgs(C.Structure):
+    """b200_attention_args: the score scale and the causal flag (1: key j visible to query i iff j <= i)."""
+    _fields_ = [("scale", C.c_float), ("causal", C.c_int32)]
+
+
 class QuantScheme(C.Structure):
     """b200_quant_scheme: value (b200_quant_value), block, block_scale (b200_dtype), tensor_scale (0 / 1)."""
     _fields_ = [("value", C.c_int32), ("block", C.c_int32), ("block_scale", C.c_int32), ("tensor_scale", C.c_int32)]
@@ -140,6 +145,8 @@ SIGNATURES = {
                                         _u64p, _u64p, C.POINTER(Conv2dArgs), C.POINTER(Epilogue)]),
     "b200_conv_transpose3d": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, _u64p, _u64p, C.c_uint64, _u64p, _u64p, C.c_uint64,
                                         _u64p, _u64p, C.POINTER(Conv3dArgs), C.POINTER(Epilogue)]),
+    "b200_attention": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, _u64p, _u64p, C.c_uint64, _u64p, _u64p, C.c_uint64, _u64p,
+                                 _u64p, C.c_uint64, _u64p, _u64p, C.c_uint64, C.POINTER(AttentionArgs)]),
     "b200_reduce": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, C.c_uint64, C.c_int, _u64p, C.c_int]),
     "b200_reduce_strided": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, C.c_uint64, C.c_int, _u64p, _u64p, C.c_int]),
     "b200_reduce_debug": (C.c_int, [_vp, _vp, _u64p]),

@@ -56,6 +56,8 @@ extern const unsigned char b200_cubin_gemm_conv3d[];
 extern const unsigned char b200_cubin_gemm_conv3d_end[];
 extern const unsigned char b200_cubin_gemm_convt[];
 extern const unsigned char b200_cubin_gemm_convt_end[];
+extern const unsigned char b200_cubin_attention[];
+extern const unsigned char b200_cubin_attention_end[];
 }
 
 // ================================================================================================ errors
@@ -327,13 +329,14 @@ static int get_func(b200_ctx* c, const std::string& name, CUfunction* out) {
   auto it = c->funcs.find(name);
   if (it != c->funcs.end()) { *out = it->second; return B200_OK; }
   // modules are loaded in the order gemm, reduce, aux, gemm_b, gemm_c, quant, gemm_q, quant_mm, gemm_conv, gemm_convbwd,
-  // conv_grouped, gemm_conv3d, gemm_convt; the kernel
+  // conv_grouped, gemm_conv3d, gemm_convt, attention; the kernel
   // name says where a
   // kernel lives (no failing lookups, which API-level tools such as compute-sanitizer would report)
   auto starts = [&](const char* pfx) { return name.rfind(pfx, 0) == 0; };
   auto has = [&](const char* part) { return name.find(part) != std::string::npos; };
   const bool tc_gemm = starts("gemm_") && name != "gemm_simt_strided" && name != "gemm_scaled_simt";
   const size_t home = name == "conv3d_dgrad_weights" ? 2
+                      : starts("attn_") ? 13
                       : starts("conv2d_tconv_") || starts("conv3d_tconv_") ? 12
                       : starts("conv3d_") ? 11
                       : starts("conv2d_grp_") ? 10
@@ -373,7 +376,8 @@ extern "C" int b200_get_cubin(const char* name, const void** image, size_t* size
   else if (!strcmp(name, "conv_grouped")) { b = b200_cubin_conv_grouped; e = b200_cubin_conv_grouped_end; }
   else if (!strcmp(name, "gemm_conv3d")) { b = b200_cubin_gemm_conv3d; e = b200_cubin_gemm_conv3d_end; }
   else if (!strcmp(name, "gemm_convt")) { b = b200_cubin_gemm_convt; e = b200_cubin_gemm_convt_end; }
-  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd|conv_grouped|gemm_conv3d|gemm_convt)", name);
+  else if (!strcmp(name, "attention")) { b = b200_cubin_attention; e = b200_cubin_attention_end; }
+  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd|conv_grouped|gemm_conv3d|gemm_convt|attention)", name);
   *image = b;
   *size = static_cast<size_t>(e - b);
   return B200_OK;
@@ -433,7 +437,8 @@ extern "C" int b200_init(int device, b200_ctx** out) {
       (rc = load_module(c, b200_cubin_gemm_convbwd, b200_cubin_gemm_convbwd_end, "gemm_convbwd")) ||
       (rc = load_module(c, b200_cubin_conv_grouped, b200_cubin_conv_grouped_end, "conv_grouped")) ||
       (rc = load_module(c, b200_cubin_gemm_conv3d, b200_cubin_gemm_conv3d_end, "gemm_conv3d")) ||
-      (rc = load_module(c, b200_cubin_gemm_convt, b200_cubin_gemm_convt_end, "gemm_convt"))) {
+      (rc = load_module(c, b200_cubin_gemm_convt, b200_cubin_gemm_convt_end, "gemm_convt")) ||
+      (rc = load_module(c, b200_cubin_attention, b200_cubin_attention_end, "attention"))) {
     for (CUmodule m : c->modules) g_drv.cuModuleUnload_p(m);
     g_drv.cuDevicePrimaryCtxRelease_p(c->dev);
     return bail(rc);
@@ -4123,6 +4128,159 @@ extern "C" int b200_conv2d_grouped_backward_weight(b200_ctx* c, b200_stream s, b
 
 // Stage timings (ns) of the most recent fused reduce + exchange launched with option reduce.debug=1 on stream `s`:
 // words[0] = exchange (publish -> all peers seen), words[1] = partials + f64 tree of the last block.  Synchronises the stream.
+// ================================================================================================ attention
+// 4-D tiled map (dims innermost first; strides of dims 1..3 in elements), zero out-of-bounds fill.  Its own plan line and
+// cache key; encode_tmap's are unchanged.
+static int encode_tmap4(b200_ctx* c, CUtensorMap* out, CUtensorMapDataType dt, size_t esz, uint64_t base, const uint64_t dims[4],
+                        const uint64_t strides[3], const uint32_t box[4], CUtensorMapSwizzle swz) {
+  const int promo_bytes = atoi(opt(c, "gemm.l2_promotion", "256").c_str());
+  const CUtensorMapL2promotion promo = promo_bytes >= 256 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B
+                                       : promo_bytes >= 128 ? CU_TENSOR_MAP_L2_PROMOTION_L2_128B
+                                       : promo_bytes >= 64 ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B : CU_TENSOR_MAP_L2_PROMOTION_NONE;
+  std::string key = "tiled4d|" + std::to_string((int)dt) + "|" + std::to_string((int)swz) + "|" + std::to_string(base);
+  for (int i = 0; i < 4; ++i) key += "|" + std::to_string(dims[i]) + "|" + std::to_string(box[i]);
+  for (int i = 0; i < 3; ++i) key += "|" + std::to_string(strides[i]);
+  key += "|" + std::to_string((int)promo);
+  if (c->dry) {
+    char line[320];
+    snprintf(line, sizeof(line), "tmap4d esz=%zu dims=(%llu,%llu,%llu,%llu) strides=(%llu,%llu,%llu) box=(%u,%u,%u,%u) swizzle=%d\n", esz,
+             (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)dims[2], (unsigned long long)dims[3],
+             (unsigned long long)(strides[0] * esz), (unsigned long long)(strides[1] * esz), (unsigned long long)(strides[2] * esz), box[0],
+             box[1], box[2], box[3], (int)swz);
+    c->plan += line;
+    memset(out, 0, sizeof(*out));
+    return B200_OK;
+  }
+  auto it = c->tmap_cache.find(key);
+  if (it != c->tmap_cache.end()) { *out = it->second; return B200_OK; }
+  cuuint64_t gdim[4] = {dims[0], dims[1], dims[2], dims[3]};
+  cuuint64_t gstr[3] = {strides[0] * esz, strides[1] * esz, strides[2] * esz};
+  cuuint32_t bx[4] = {box[0], box[1], box[2], box[3]};
+  cuuint32_t estr[4] = {1, 1, 1, 1};
+  CUresult r = g_drv.cuTensorMapEncodeTiled_p(out, dt, 4, reinterpret_cast<void*>(base), gdim, gstr, bx, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                                              swz, promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS)
+    return fail(B200_ERR_INVALID_ARG, "cuTensorMapEncodeTiled (rank 4) failed: %s (dims %llu,%llu,%llu,%llu strides %llu,%llu,%llu)", cu_err(r),
+                (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)dims[2], (unsigned long long)dims[3],
+                (unsigned long long)gstr[0], (unsigned long long)gstr[1], (unsigned long long)gstr[2]);
+  if (c->tmap_cache.size() > 512) c->tmap_cache.clear();
+  c->tmap_cache[key] = *out;
+  return B200_OK;
+}
+
+// A [B, H, S, D] view (normalised strides ns, in elements) a tensor map reads in place: unit D stride, 16-byte aligned base and
+// S, H, B strides below 2^40 bytes.
+static bool attn_view_ok(uint64_t ptr, size_t esz, const uint64_t* ns) {
+  if (ptr % 16 || ns[3] != 1) return false;
+  for (int d = 0; d < 3; ++d)
+    if ((ns[d] * esz) % 16 || ns[d] * esz >= (1ull << 40)) return false;
+  return true;
+}
+
+extern "C" int b200_attention(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr q, const uint64_t* q_shape,
+                              const uint64_t* q_strides, b200_dptr k, const uint64_t* k_shape, const uint64_t* k_strides, b200_dptr v,
+                              const uint64_t* v_shape, const uint64_t* v_strides, b200_dptr out, const uint64_t* out_shape,
+                              const uint64_t* out_strides, b200_dptr lse, const b200_attention_args* args) {
+  CTX_ENTER(c);
+  const char* what = "attention";
+  if (!q_shape || !k_shape || !v_shape || !out_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
+  if (in_dtype != B200_F16 && in_dtype != B200_BF16)
+    return fail(B200_ERR_UNSUPPORTED, "%s: input dtype %d unsupported (f16, bf16)", what, (int)in_dtype);
+  if (out_dtype != in_dtype && out_dtype != B200_F32)
+    return fail(B200_ERR_UNSUPPORTED, "%s: output dtype must equal the input dtype or be f32", what);
+  const uint64_t B = q_shape[0], Hq = q_shape[1], Sq = q_shape[2], D = q_shape[3];
+  const uint64_t Hkv = k_shape[1], Sk = k_shape[2];
+  if (k_shape[0] != B || k_shape[3] != D)
+    return fail(B200_ERR_INVALID_ARG, "%s: k [%llu,%llu,%llu,%llu] differs from q [%llu,%llu,%llu,%llu] in batch or head dim", what,
+                (unsigned long long)k_shape[0], (unsigned long long)Hkv, (unsigned long long)Sk, (unsigned long long)k_shape[3],
+                (unsigned long long)B, (unsigned long long)Hq, (unsigned long long)Sq, (unsigned long long)D);
+  if (v_shape[0] != B || v_shape[1] != Hkv || v_shape[2] != Sk)
+    return fail(B200_ERR_INVALID_ARG, "%s: v [%llu,%llu,%llu,%llu] does not match k [%llu,%llu,%llu,%llu]", what, (unsigned long long)v_shape[0],
+                (unsigned long long)v_shape[1], (unsigned long long)v_shape[2], (unsigned long long)v_shape[3], (unsigned long long)B,
+                (unsigned long long)Hkv, (unsigned long long)Sk, (unsigned long long)D);
+  if (v_shape[3] != D) return fail(B200_ERR_UNSUPPORTED, "%s: v's head dim %llu differs from D = %llu", what, (unsigned long long)v_shape[3], (unsigned long long)D);
+  if (Hkv == 0 || Hq % Hkv)
+    return fail(B200_ERR_INVALID_ARG, "%s: Hq = %llu must be a multiple of Hkv = %llu", what, (unsigned long long)Hq, (unsigned long long)Hkv);
+  if (out_shape[0] != B || out_shape[1] != Hq || out_shape[2] != Sq || out_shape[3] != D)
+    return fail(B200_ERR_INVALID_ARG, "%s: out is [%llu,%llu,%llu,%llu], expected [%llu,%llu,%llu,%llu]", what, (unsigned long long)out_shape[0],
+                (unsigned long long)out_shape[1], (unsigned long long)out_shape[2], (unsigned long long)out_shape[3], (unsigned long long)B,
+                (unsigned long long)Hq, (unsigned long long)Sq, (unsigned long long)D);
+  if (Sk == 0 && Sq > 0) return fail(B200_ERR_INVALID_ARG, "%s: Sk = 0 leaves every query row without keys", what);
+  if (!std::isfinite(args->scale)) return fail(B200_ERR_INVALID_ARG, "%s: scale must be finite", what);
+  if (D == 0 || D > 128 || D % 8)
+    return fail(B200_ERR_UNSUPPORTED, "%s: head dim D = %llu unsupported (a multiple of 8 in [8, 128])", what, (unsigned long long)D);
+  const uint64_t lim = 1ull << 31;
+  if (B >= lim || Hq >= lim || Sq >= lim || Hkv >= lim || Sk >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: extents must be < 2^31", what);
+  if (B == 0 || Hq == 0 || Sq == 0) return B200_OK;
+  const uint64_t nqb = (Sq + kAttnBlock - 1) / kAttnBlock, ctas = nqb * Hq * B;
+  if (ctas >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: ceil(Sq / %d) * Hq * B = %llu CTAs must be < 2^31", what, kAttnBlock, (unsigned long long)ctas);
+  if (!q || !k || !v || !out) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
+  if (lse % 4) return fail(B200_ERR_INVALID_ARG, "%s: lse pointer is not 4-byte aligned", what);
+  const size_t osz = dtype_size(out_dtype);
+  uint64_t qs[4], ks[4], vs[4], os[4];
+  conv_norm_strides(out_shape, out_strides, os);
+  if (!attn_view_ok(out, osz, os))
+    return fail(B200_ERR_UNSUPPORTED, "%s: out needs a unit D stride and a 16-byte aligned base and S, H, B strides", what);
+  conv_norm_strides(q_shape, q_strides, qs);
+  conv_norm_strides(k_shape, k_strides, ks);
+  conv_norm_strides(v_shape, v_strides, vs);
+
+  CUstream st = resolve_stream(c, s);
+  CUdeviceptr tmp[3] = {0, 0, 0};
+  // each operand in place, or gathered into a compact [B, H, S, D] copy
+  auto prep = [&](int i, uint64_t ptr, const uint64_t* shape, uint64_t* ns, uint64_t* use) -> int {
+    *use = ptr;
+    if (attn_view_ok(ptr, 2, ns)) return B200_OK;
+    int rc = conv_gather(c, st, in_dtype, ptr, shape, ns, &tmp[i]);
+    *use = tmp[i];
+    ns[3] = 1; ns[2] = shape[3]; ns[1] = shape[2] * shape[3]; ns[0] = shape[1] * shape[2] * shape[3];
+    return rc;
+  };
+  uint64_t qp = 0, kp = 0, vp = 0;
+  int rc = prep(0, q, q_shape, qs, &qp);
+  if (!rc) rc = prep(1, k, k_shape, ks, &kp);
+  if (!rc) rc = prep(2, v, v_shape, vs, &vp);
+  if (!rc) {
+    const uint32_t DB = D <= 64 ? 64 : 128;
+    const CUtensorMapDataType dt = in_dtype == B200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+    CUtensorMap mq, mk, mv, mo;
+    const uint32_t box_in[4] = {64, (uint32_t)kAttnBlock, 1, 1};
+    const uint32_t box_out[4] = {(uint32_t)(128 / osz), 64, 1, 1};
+    const uint64_t dq[4] = {D, Sq, Hq, B}, dk[4] = {D, Sk, Hkv, B};
+    const uint64_t sq[3] = {qs[2], qs[1], qs[0]}, sk[3] = {ks[2], ks[1], ks[0]}, sv[3] = {vs[2], vs[1], vs[0]}, so[3] = {os[2], os[1], os[0]};
+    rc = encode_tmap4(c, &mq, dt, 2, qp, dq, sq, box_in, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (!rc) rc = encode_tmap4(c, &mk, dt, 2, kp, dk, sk, box_in, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (!rc) rc = encode_tmap4(c, &mv, dt, 2, vp, dk, sv, box_in, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (!rc)
+      rc = encode_tmap4(c, &mo, osz == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_UINT16, osz, out, dq, so, box_out,
+                        CU_TENSOR_MAP_SWIZZLE_128B);
+    CUfunction f = nullptr;
+    const char* in_tag = dt_tag(in_dtype);
+    const std::string name = std::string("attn_fwd_") + in_tag + "_d" + std::to_string(DB) + "_" + dt_tag(out_dtype);
+    if (!rc) rc = get_func(c, name, &f);
+    const unsigned smem = 1024 + (1 + 2 * kAttnStages) * kAttnBlock * DB * 2 + 1024;
+    if (!rc && !c->dry) {
+      CUresult r = g_drv.cuFuncSetAttribute_p(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem);
+      if (r != CUDA_SUCCESS) rc = fail(map_cu(r), "cuFuncSetAttribute: %s", cu_err(r));
+    }
+    if (!rc) {
+      AttnParams p{};
+      p.lse = lse;
+      p.B = (uint32_t)B; p.Hq = (uint32_t)Hq; p.Sq = (uint32_t)Sq; p.Sk = (uint32_t)Sk;
+      p.group = (uint32_t)(Hq / Hkv);
+      p.nqb = (uint32_t)nqb;
+      p.causal = args->causal != 0 ? 1u : 0u;
+      p.D = (uint32_t)D;
+      p.scale_log2 = (float)((double)args->scale * 1.4426950408889634074);
+      void* kargs[] = {&mq, &mk, &mv, &mo, &p};
+      rc = launch(c, f, (unsigned)ctas, 1, 1, 384, smem, 1, st, kargs);
+    }
+  }
+  for (CUdeviceptr t : tmp)
+    if (t) pool_free(c, t, st);   // stream-ordered: reusable once the kernel has drained
+  return rc;
+}
+
 extern "C" int b200_reduce_debug(b200_ctx* c, b200_stream s, uint64_t* words4) {
   CTX_ENTER_DEVICE(c);
   if (!words4) return fail(B200_ERR_INVALID_ARG, "reduce_debug: null output");

@@ -201,6 +201,24 @@ struct TconvParams {
   uint32_t phases, pad[3];
 };
 
+// ================================================================================================ attention.cu
+// Fused attention forward (attn_fwd_*; capi.cpp: b200_attention).  One CTA per (b, h, kAttnBlock-query block), grid
+// nqb * Hq * B with block x = ((nqb - 1 - qb) * B + b) * Hq + h; K and V stream in blocks of kAttnBlock keys through
+// kAttnStages stages.  Shared memory: 1024 (alignment slack) + (1 + 2 * kAttnStages) tiles of kAttnBlock rows x DB 16-bit
+// elements (DB = 64 or 128: Q, then K and V per stage) + 1024 (barriers).  The tensor maps are 4-D (D, S, H, B).
+constexpr int kAttnBlock = 128;
+constexpr int kAttnStages = 2;
+struct AttnParams {
+  uint64_t lse;          // f32 [B, Hq, Sq] compact, or 0
+  uint32_t B, Hq, Sq, Sk;
+  uint32_t group;        // Hq / Hkv: query head h reads kv head h / group
+  uint32_t nqb;          // query blocks: ceil(Sq / kAttnBlock)
+  uint32_t causal;       // 1: key j visible to query i iff j <= i
+  uint32_t D;            // head dim (the store clips columns >= D)
+  float scale_log2;      // scale * log2(e)
+  uint32_t pad;
+};
+
 // ================================================================================================ conv_grouped.cu
 // Direct NHWC grouped convolution (b200_conv2d_grouped*, group width Cg = C / groups < 64).  Group g owns input channels
 // [g Cg, (g+1) Cg) and output channels [g Coutg, (g+1) Coutg).  Every strided operand has a unit channel stride; strides

@@ -211,6 +211,23 @@ __device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, uint32_t src,
                : "memory");
 }
 
+// 4-D tiled load, signalling an mbarrier in this CTA (coordinates innermost first).
+__device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1, int c2, int c3) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
+      :
+      : "r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      : "memory");
+}
+
+// 4-D tiled store smem -> global (bulk async-group completion); the box is clipped at the tensor's edges.
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, uint32_t src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+               :
+               : "l"(reinterpret_cast<uint64_t>(m)), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
+
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 
 template <int N>
@@ -336,6 +353,39 @@ __device__ __forceinline__ void wgmma_ss(Acc (&d)[N / 2], uint64_t da, uint64_t 
   static_assert(N == 112 || N == 128 || N == 256 || (N == 64 && KA == 6 && KB == 6), "m64n112 / m64n128 / m64n256, m64n64 s8 only");
   if constexpr (N == 64) B200_WGMMA(64, R, 32, "s32.s8.s8", "");
   else if constexpr (N == 112) { B200_WGMMA_ALL(112) } else if constexpr (N == 128) { B200_WGMMA_ALL(128) } else { B200_WGMMA_ALL(256) }
+}
+
+// m64n64 f32 accumulators (the register list is B200_WG_REGS_64)
+#define B200_WG_OPS_F64 "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+// Register-A operand of m64nNk16 (16-bit kinds): four registers of two values each, after the N / 2 accumulators.  Thread
+// (warp w, lane) holds rows 16 w + lane / 4 (+8) and k = 2 (lane % 4) (+1, +8, +9): a0 (r, k), a1 (r + 8, k), a2 (r, k + 8),
+// a3 (r + 8, k + 8) -- the layout of columns 16 kk .. 16 kk + 15 of an m64nN f32 accumulator fragment, packed in pairs.
+#define B200_WG_A_64 "{%32, %33, %34, %35}"
+#define B200_WG_DB_RS_64 "%36"
+#define B200_WG_SC_RS_64 "%37"
+#define B200_WG_A_128 "{%64, %65, %66, %67}"
+#define B200_WG_DB_RS_128 "%68"
+#define B200_WG_SC_RS_128 "%69"
+#define B200_WGMMA_RS(N, T, TB)                                                                                         \
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, " B200_WG_SC_RS_##N ", 0;\n\t"                                    \
+               "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32." T "." T " " B200_WG_REGS_##N ", " B200_WG_A_##N ", "    \
+               B200_WG_DB_RS_##N ", p, 1, 1, " #TB ";\n\t}"                                                             \
+               : B200_WG_OPS_F##N                                                                                       \
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d))
+
+// D (+)= A[registers] * B[smem] for one warpgroup, m64 x N x k16, f32 accumulators, f16 (KIND 0) or bf16 (KIND 1).  TB: 1 = B
+// is an MN-major operand.  scale_d == 0: D = A * B.
+template <int N, int KIND, int TB>
+__device__ __forceinline__ void wgmma_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  static_assert((N == 64 || N == 128) && (KIND == 0 || KIND == 1) && (TB == 0 || TB == 1), "m64n64 / m64n128, f16 / bf16");
+  if constexpr (N == 64 && KIND == 0 && TB == 0) B200_WGMMA_RS(64, "f16", 0);
+  else if constexpr (N == 64 && KIND == 0) B200_WGMMA_RS(64, "f16", 1);
+  else if constexpr (N == 64 && TB == 0) B200_WGMMA_RS(64, "bf16", 0);
+  else if constexpr (N == 64) B200_WGMMA_RS(64, "bf16", 1);
+  else if constexpr (KIND == 0 && TB == 0) B200_WGMMA_RS(128, "f16", 0);
+  else if constexpr (KIND == 0) B200_WGMMA_RS(128, "f16", 1);
+  else if constexpr (TB == 0) B200_WGMMA_RS(128, "bf16", 0);
+  else B200_WGMMA_RS(128, "bf16", 1);
 }
 
 }  // namespace b200

@@ -507,6 +507,45 @@ int b200_conv_transpose3d(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b20
                           b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides,
                           const b200_conv3d_args* args, const b200_epilogue* epilogue);
 
+/* ---- fused scaled-dot-product attention, forward (PyTorch's scaled_dot_product_attention) ---------------------------------
+ * out[b, h, i, :] = sum_j softmax_j(scale * q[b, h, i, :] . k[b, h / G, j, :]) * v[b, h / G, j, :]      G = Hq / Hkv
+ * lse[b, h, i]    = log sum_j exp(scale * q[b, h, i, :] . k[b, h / G, j, :])                         (natural log, f32)
+ * q is [B, Hq, Sq, D], k and v are [B, Hkv, Sk, D], out is [B, Hq, Sq, D]: shapes and strides in elements, so [B, S, H, D]
+ * tensors and the q / k / v slices of a fused [B, S, 3, H, D] projection are stride-permuted views read with no copy.
+ * Hq % Hkv == 0 (GQA / MQA, torch's enable_gqa=True).  causal != 0: key j is visible to query i only when j <= i (top-left
+ * alignment, torch's is_causal=True); every row then sees key 0, so no row is empty.  scale: any finite float.
+ * Dtypes: in_dtype B200_F16 or B200_BF16 for q, k and v; out_dtype the input dtype or B200_F32.  D <= 128, D % 8 == 0, v's
+ * head dim equal to D.  A D that is not a multiple of 64 is read with the tensor-map box past D zero-filled (exact for both
+ * products) and the store is clipped to D.
+ * Numerics: scores are f32 sums of exact 16-bit products.  The softmax runs in base 2 with a running row maximum: t = s *
+ * (scale * log2 e) is formed once per score and p = exp2(t - m), so the row's maximal score contributes exp2(0) = 1 exactly
+ * (an argument below -126 gives +0).  P is rounded (RNE) to the input dtype before the P.V product; the row sum l adds the
+ * f32 p values.  out = O / l (f32 division) rounded once (RNE) to out_dtype; lse = (m + log2 l) * ln 2.  Bitwise
+ * reproducible for fixed shapes, dtypes and views: every output row is produced by one CTA in increasing key order (no
+ * atomics, no split over keys).
+ * Views: q, k and v are read in place when their D stride is 1 and the base and the S, H and B strides are 16-byte aligned;
+ * any other view is first gathered into a compact [B, H, S, D] pooled temporary with b200_into_contiguous (one extra launch
+ * per operand).  out needs a unit D stride and a 16-byte aligned base and strides, else B200_ERR_UNSUPPORTED naming out.
+ * lse: 0 (not written) or an f32 [B, Hq, Sq] compact buffer, 4-byte aligned.
+ * Errors: B200_ERR_INVALID_ARG for mismatched B or D, Hkv == 0 or Hq % Hkv != 0, a k / v shape mismatch, a wrong out shape,
+ * Sk == 0 with Sq > 0, a non-finite scale, or a null pointer (rank 4 is implied by the shape arrays; the wrappers refuse
+ * other ranks with B200_ERR_INVALID_ARG); B200_ERR_UNSUPPORTED for the dtypes, D > 128, D % 8 != 0, Dv != D, extents >= 2^31
+ * or more than 2^31 - 1 CTAs.  Zero extents: B, Hq or Sq = 0 is a no-op with no launch.
+ * Launches: the gathers, then one attn_fwd_<in>_d<64|128>_<out> launch (D <= 64: the d64 kernel) of ceil(Sq / 128) * Hq * B
+ * CTAs, queued on `s` with no host synchronisation; temporaries come from the pool in stream order (as the convolution
+ * entries).  The dry-run plan records each 4-D tensor map as "tmap4d esz= dims=(D,S,H,B) strides=(S,H,B bytes) box=(..)
+ * swizzle=" in the order q, k, v, out.  b200_last_kernel names the kernel. */
+typedef struct b200_attention_args {
+  float scale;       /* multiplies q.k before the softmax */
+  int32_t causal;    /* 1: key j visible to query i iff j <= i (top-left) */
+} b200_attention_args;
+int b200_attention(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype,
+                   b200_dptr q, const uint64_t* q_shape, const uint64_t* q_strides,
+                   b200_dptr k, const uint64_t* k_shape, const uint64_t* k_strides,
+                   b200_dptr v, const uint64_t* v_shape, const uint64_t* v_strides,
+                   b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides,
+                   b200_dptr lse, const b200_attention_args* args);
+
 /* ---- collectives: ServerCommunication (server/base.rs:632-739), CUDA impl cubecl-cuda/src/compute/server.rs:666-926 -- */
 #define B200_UNIQUE_ID_BYTES 128
 int b200_comm_get_unique_id(b200_ctx* ctx, void* id128);            /* ncclGetUniqueId (communication.rs:11-25 holds it per device set) */

@@ -377,6 +377,25 @@ inline void launch(ComputeClient& client, const TensorHandle& x, const TensorHan
 }
 }  // namespace conv_transpose
 
+namespace attention {
+/// Fused scaled-dot-product attention, forward: q [B, Hq, Sq, D], k and v [B, Hkv, Sk, D], out [B, Hq, Sq, D] (views by
+/// strides); lse: nullptr or a compact f32 [B, Hq, Sq] tensor receiving the row log-sum-exp.  See b200_attention in
+/// cubecl_b200.h.  Errors are deferred to client.sync().
+inline void launch(ComputeClient& client, const TensorHandle& q, const TensorHandle& k, const TensorHandle& v, const TensorHandle& out,
+                   float scale, bool causal = false, const TensorHandle* lse = nullptr) {
+  if (q.shape.size() != 4 || k.shape.size() != 4 || v.shape.size() != 4 || out.shape.size() != 4 || q.dtype != k.dtype || q.dtype != v.dtype) {
+    client.defer("InvalidArgument: attention needs rank-4 q, k, v and out, and q, k and v of one dtype");
+    return;
+  }
+  const b200_attention_args args{scale, causal ? 1 : 0};
+  const int rc = b200_attention(client.raw(), nullptr, static_cast<b200_dtype>(q.dtype), static_cast<b200_dtype>(out.dtype), q.handle.ptr(),
+                                q.shape.data(), q.strides.data(), k.handle.ptr(), k.shape.data(), k.strides.data(), v.handle.ptr(),
+                                v.shape.data(), v.strides.data(), out.handle.ptr(), out.shape.data(), out.strides.data(),
+                                lse ? lse->handle.ptr() : 0, &args);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+}  // namespace attention
+
 namespace reduce {
 enum class Op : int { Sum = B200_REDUCE_SUM, Prod = B200_REDUCE_PROD, Max = B200_REDUCE_MAX, Min = B200_REDUCE_MIN,
                       ArgMax = B200_REDUCE_ARGMAX, ArgMin = B200_REDUCE_ARGMIN, Mean = B200_REDUCE_MEAN };

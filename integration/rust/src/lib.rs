@@ -531,6 +531,27 @@ impl Context {
         ))
     }
 
+    /// Fused scaled-dot-product attention, forward: q [B, Hq, Sq, D], k and v [B, Hkv, Sk, D] -> out [B, Hq, Sq, D] (views by
+    /// strides), f16 / bf16 in, out in the input dtype or f32; `lse`: 0 or an f32 [B, Hq, Sq] compact buffer for the row
+    /// log-sum-exp; `causal`: key j visible to query i iff j <= i.  See b200_attention in cubecl_b200.h.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::conv2d`]; `lse`, when non-zero, must hold B * Hq * Sq f32 values.
+    pub unsafe fn attention(
+        &mut self, stream: b200_stream, in_dtype: DType, out_dtype: DType, q: &TensorView, k: &TensorView, v: &TensorView,
+        out: &TensorView, lse: b200_dptr, scale: f32, causal: bool,
+    ) -> Result<(), Error> {
+        for t in [q, k, v, out] {
+            assert!(t.shape.len() == 4 && t.strides.len() == 4);
+        }
+        let a = sys::b200_attention_args { scale, causal: causal as i32 };
+        check(sys::b200_attention(
+            self.0, stream, in_dtype as c_int, out_dtype as c_int, q.ptr, q.shape.as_ptr(), q.strides.as_ptr(), k.ptr,
+            k.shape.as_ptr(), k.strides.as_ptr(), v.ptr, v.shape.as_ptr(), v.strides.as_ptr(), out.ptr, out.shape.as_ptr(),
+            out.strides.as_ptr(), lse, &a,
+        ))
+    }
+
     /// Grouped / depthwise [`Context::conv2d`]: w [Cout, KH, KW, C / groups].  See b200_conv2d_grouped in cubecl_b200.h.
     ///
     /// # Safety
