@@ -30,7 +30,7 @@ CUBINS = {"gemm": ("gemm_wgmma.cu", ["-DGEMM_PART=0"]), "gemm_b": ("gemm_wgmma.c
           "quant_mm": ("quant.cu", ["-DQUANT_PART=1"]), "gemm_conv": ("gemm_wgmma.cu", ["-DGEMM_PART=4"]),
           "gemm_convbwd": ("gemm_wgmma.cu", ["-DGEMM_PART=5"]), "conv_grouped": ("conv_grouped.cu", []),
           "gemm_conv3d": ("gemm_wgmma.cu", ["-DGEMM_PART=6"]), "gemm_convt": ("gemm_wgmma.cu", ["-DGEMM_PART=7"]),
-          "attention": ("attention.cu", [])}
+          "attention": ("attention.cu", []), "attention_bwd": ("attention_bwd.cu", [])}
 NVCC_FLAGS = ["-cubin", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17"]
 
 
@@ -79,7 +79,8 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     # cost the five minutes of ptxas the GEMM instantiations take
     def inputs_digest(src, extra):
         h = hashlib.sha256(" ".join(NVCC_FLAGS + list(extra)).encode())
-        for f in (CSRC / src, CSRC / "ptx.cuh", CSRC / "epilogue.cuh", CSRC / "kernel_params.h", ROOT / "include" / "cubecl_b200.h"):
+        for f in (CSRC / src, CSRC / "ptx.cuh", CSRC / "epilogue.cuh", CSRC / "attention.cuh", CSRC / "kernel_params.h",
+                  ROOT / "include" / "cubecl_b200.h"):
             h.update(f.read_bytes())
         return h.hexdigest()
 

@@ -58,6 +58,8 @@ extern const unsigned char b200_cubin_gemm_convt[];
 extern const unsigned char b200_cubin_gemm_convt_end[];
 extern const unsigned char b200_cubin_attention[];
 extern const unsigned char b200_cubin_attention_end[];
+extern const unsigned char b200_cubin_attention_bwd[];
+extern const unsigned char b200_cubin_attention_bwd_end[];
 }
 
 // ================================================================================================ errors
@@ -329,13 +331,14 @@ static int get_func(b200_ctx* c, const std::string& name, CUfunction* out) {
   auto it = c->funcs.find(name);
   if (it != c->funcs.end()) { *out = it->second; return B200_OK; }
   // modules are loaded in the order gemm, reduce, aux, gemm_b, gemm_c, quant, gemm_q, quant_mm, gemm_conv, gemm_convbwd,
-  // conv_grouped, gemm_conv3d, gemm_convt, attention; the kernel
+  // conv_grouped, gemm_conv3d, gemm_convt, attention, attention_bwd; the kernel
   // name says where a
   // kernel lives (no failing lookups, which API-level tools such as compute-sanitizer would report)
   auto starts = [&](const char* pfx) { return name.rfind(pfx, 0) == 0; };
   auto has = [&](const char* part) { return name.find(part) != std::string::npos; };
   const bool tc_gemm = starts("gemm_") && name != "gemm_simt_strided" && name != "gemm_scaled_simt";
   const size_t home = name == "conv3d_dgrad_weights" ? 2
+                      : starts("attn_bwd_") ? 14
                       : starts("attn_") ? 13
                       : starts("conv2d_tconv_") || starts("conv3d_tconv_") ? 12
                       : starts("conv3d_") ? 11
@@ -377,7 +380,8 @@ extern "C" int b200_get_cubin(const char* name, const void** image, size_t* size
   else if (!strcmp(name, "gemm_conv3d")) { b = b200_cubin_gemm_conv3d; e = b200_cubin_gemm_conv3d_end; }
   else if (!strcmp(name, "gemm_convt")) { b = b200_cubin_gemm_convt; e = b200_cubin_gemm_convt_end; }
   else if (!strcmp(name, "attention")) { b = b200_cubin_attention; e = b200_cubin_attention_end; }
-  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd|conv_grouped|gemm_conv3d|gemm_convt|attention)", name);
+  else if (!strcmp(name, "attention_bwd")) { b = b200_cubin_attention_bwd; e = b200_cubin_attention_bwd_end; }
+  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd|conv_grouped|gemm_conv3d|gemm_convt|attention|attention_bwd)", name);
   *image = b;
   *size = static_cast<size_t>(e - b);
   return B200_OK;
@@ -438,7 +442,8 @@ extern "C" int b200_init(int device, b200_ctx** out) {
       (rc = load_module(c, b200_cubin_conv_grouped, b200_cubin_conv_grouped_end, "conv_grouped")) ||
       (rc = load_module(c, b200_cubin_gemm_conv3d, b200_cubin_gemm_conv3d_end, "gemm_conv3d")) ||
       (rc = load_module(c, b200_cubin_gemm_convt, b200_cubin_gemm_convt_end, "gemm_convt")) ||
-      (rc = load_module(c, b200_cubin_attention, b200_cubin_attention_end, "attention"))) {
+      (rc = load_module(c, b200_cubin_attention, b200_cubin_attention_end, "attention")) ||
+      (rc = load_module(c, b200_cubin_attention_bwd, b200_cubin_attention_bwd_end, "attention_bwd"))) {
     for (CUmodule m : c->modules) g_drv.cuModuleUnload_p(m);
     g_drv.cuDevicePrimaryCtxRelease_p(c->dev);
     return bail(rc);
@@ -4278,6 +4283,176 @@ extern "C" int b200_attention(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b
   }
   for (CUdeviceptr t : tmp)
     if (t) pool_free(c, t, st);   // stream-ordered: reusable once the kernel has drained
+  return rc;
+}
+
+// Backward of b200_attention (see cubecl_b200.h): the delta / L pass, then the dq and the dk / dv kernels.
+extern "C" int b200_attention_backward(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dtype grad_dtype,
+                                       b200_dptr q, const uint64_t* q_shape, const uint64_t* q_strides, b200_dptr k,
+                                       const uint64_t* k_shape, const uint64_t* k_strides, b200_dptr v, const uint64_t* v_shape,
+                                       const uint64_t* v_strides, b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides,
+                                       b200_dptr dout, const uint64_t* dout_shape, const uint64_t* dout_strides, b200_dptr lse,
+                                       b200_dptr dq, const uint64_t* dq_shape, const uint64_t* dq_strides, b200_dptr dk,
+                                       const uint64_t* dk_shape, const uint64_t* dk_strides, b200_dptr dv, const uint64_t* dv_shape,
+                                       const uint64_t* dv_strides, const b200_attention_args* args) {
+  CTX_ENTER(c);
+  const char* what = "attention_backward";
+  if (!q_shape || !k_shape || !v_shape || !out_shape || !dout_shape || !dq_shape || !dk_shape || !dv_shape || !args)
+    return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
+  if (in_dtype != B200_F16 && in_dtype != B200_BF16)
+    return fail(B200_ERR_UNSUPPORTED, "%s: input dtype %d unsupported (f16, bf16)", what, (int)in_dtype);
+  if (out_dtype != in_dtype && out_dtype != B200_F32)
+    return fail(B200_ERR_UNSUPPORTED, "%s: output dtype must equal the input dtype or be f32", what);
+  if (grad_dtype != in_dtype && grad_dtype != B200_F32)
+    return fail(B200_ERR_UNSUPPORTED, "%s: grad dtype must equal the input dtype or be f32", what);
+  const uint64_t B = q_shape[0], Hq = q_shape[1], Sq = q_shape[2], D = q_shape[3];
+  const uint64_t Hkv = k_shape[1], Sk = k_shape[2];
+  auto ull = [](uint64_t x) { return (unsigned long long)x; };
+  if (k_shape[0] != B || k_shape[3] != D)
+    return fail(B200_ERR_INVALID_ARG, "%s: k [%llu,%llu,%llu,%llu] differs from q [%llu,%llu,%llu,%llu] in batch or head dim", what,
+                ull(k_shape[0]), ull(Hkv), ull(Sk), ull(k_shape[3]), ull(B), ull(Hq), ull(Sq), ull(D));
+  if (v_shape[0] != B || v_shape[1] != Hkv || v_shape[2] != Sk)
+    return fail(B200_ERR_INVALID_ARG, "%s: v [%llu,%llu,%llu,%llu] does not match k [%llu,%llu,%llu,%llu]", what, ull(v_shape[0]),
+                ull(v_shape[1]), ull(v_shape[2]), ull(v_shape[3]), ull(B), ull(Hkv), ull(Sk), ull(D));
+  if (v_shape[3] != D) return fail(B200_ERR_UNSUPPORTED, "%s: v's head dim %llu differs from D = %llu", what, ull(v_shape[3]), ull(D));
+  if (Hkv == 0 || Hq % Hkv) return fail(B200_ERR_INVALID_ARG, "%s: Hq = %llu must be a multiple of Hkv = %llu", what, ull(Hq), ull(Hkv));
+  const struct { const char* name; const uint64_t* shape; const uint64_t* want; } same[] = {
+      {"out", out_shape, q_shape}, {"dout", dout_shape, q_shape}, {"dq", dq_shape, q_shape}, {"dk", dk_shape, k_shape}, {"dv", dv_shape, k_shape}};
+  for (const auto& t : same)
+    if (memcmp(t.shape, t.want, 4 * sizeof(uint64_t)))
+      return fail(B200_ERR_INVALID_ARG, "%s: %s is [%llu,%llu,%llu,%llu], expected [%llu,%llu,%llu,%llu]", what, t.name, ull(t.shape[0]),
+                  ull(t.shape[1]), ull(t.shape[2]), ull(t.shape[3]), ull(t.want[0]), ull(t.want[1]), ull(t.want[2]), ull(t.want[3]));
+  if (Sk == 0 && Sq > 0) return fail(B200_ERR_INVALID_ARG, "%s: Sk = 0 leaves every query row without keys", what);
+  if (!std::isfinite(args->scale)) return fail(B200_ERR_INVALID_ARG, "%s: scale must be finite", what);
+  if (D == 0 || D > 128 || D % 8) return fail(B200_ERR_UNSUPPORTED, "%s: head dim D = %llu unsupported (a multiple of 8 in [8, 128])", what, ull(D));
+  const uint64_t lim = 1ull << 31;
+  if (B >= lim || Hq >= lim || Sq >= lim || Hkv >= lim || Sk >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: extents must be < 2^31", what);
+  // B = 0, or no queries and no keys: nothing to write.  Sq = 0 or Hq = 0 with keys still writes zero dk and dv.
+  if (B == 0 || (Sk == 0 && Sq == 0)) return B200_OK;
+  const uint64_t nqb = (Sq + kAttnBlock - 1) / kAttnBlock, nkb = (Sk + kAttnBlock - 1) / kAttnBlock;
+  const uint64_t rows = B * Hq * nqb * kAttnBlock;   // workspace rows, padded per (b, h) to whole query blocks
+  const bool has_q = rows > 0;
+  if (nqb * Hq * B >= lim || nkb * Hkv * B >= lim || rows / 16 >= lim)
+    return fail(B200_ERR_UNSUPPORTED, "%s: more than 2^31 - 1 CTAs", what);
+  if (!k || !v || !dk || !dv || (has_q && (!q || !out || !dout || !dq || !lse))) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
+  if (lse % 4) return fail(B200_ERR_INVALID_ARG, "%s: lse pointer is not 4-byte aligned", what);
+  const size_t gsz = dtype_size(grad_dtype), osz = dtype_size(out_dtype);
+  uint64_t qs[4], ks[4], vs[4], os[4], dos[4], dqs[4], dks[4], dvs[4];
+  conv_norm_strides(dq_shape, dq_strides, dqs);
+  conv_norm_strides(dk_shape, dk_strides, dks);
+  conv_norm_strides(dv_shape, dv_strides, dvs);
+  const struct { const char* name; uint64_t ptr; const uint64_t* ns; bool used; } grads[] = {
+      {"dq", dq, dqs, has_q}, {"dk", dk, dks, true}, {"dv", dv, dvs, true}};
+  for (const auto& g : grads)
+    if (g.used && !attn_view_ok(g.ptr, gsz, g.ns))
+      return fail(B200_ERR_UNSUPPORTED, "%s: %s needs a unit D stride and a 16-byte aligned base and S, H, B strides", what, g.name);
+  conv_norm_strides(q_shape, q_strides, qs);
+  conv_norm_strides(k_shape, k_strides, ks);
+  conv_norm_strides(v_shape, v_strides, vs);
+  conv_norm_strides(out_shape, out_strides, os);
+  conv_norm_strides(dout_shape, dout_strides, dos);
+
+  CUstream st = resolve_stream(c, s);
+  CUdeviceptr tmp[6] = {0, 0, 0, 0, 0, 0};   // gathers of q, k, v, out, dout; the workspace
+  // each operand in place, or gathered into a compact [B, H, S, D] pooled copy (as b200_attention)
+  auto prep = [&](int i, b200_dtype dt, uint64_t ptr, const uint64_t* shape, uint64_t* ns, uint64_t* use) -> int {
+    *use = ptr;
+    const size_t esz = dtype_size(dt);
+    if (attn_view_ok(ptr, esz, ns)) return B200_OK;
+    int rc = pool_alloc(c, shape[0] * shape[1] * shape[2] * shape[3] * esz, &tmp[i], st);
+    if (rc) return rc;
+    *use = tmp[i];
+    rc = b200_into_contiguous(c, static_cast<b200_stream>(st), dt, ptr, tmp[i], 4, shape, ns);
+    ns[3] = 1; ns[2] = shape[3]; ns[1] = shape[2] * shape[3]; ns[0] = shape[1] * shape[2] * shape[3];
+    return rc;
+  };
+  uint64_t qp = 0, kp = 0, vp = 0, op = 0, dop = 0;
+  int rc = B200_OK;
+  if (has_q) rc = prep(0, in_dtype, q, q_shape, qs, &qp);
+  if (!rc) rc = prep(1, in_dtype, k, k_shape, ks, &kp);
+  if (!rc) rc = prep(2, in_dtype, v, v_shape, vs, &vp);
+  if (!rc && has_q) rc = prep(3, out_dtype, out, out_shape, os, &op);
+  if (!rc && has_q) rc = prep(4, in_dtype, dout, dout_shape, dos, &dop);
+  if (!has_q) {   // no query block is loaded: the q and dout maps of the dk / dv kernel describe k
+    qp = dop = kp;
+    memcpy(qs, ks, sizeof(qs));
+    memcpy(dos, ks, sizeof(dos));
+  }
+  if (!rc && has_q) rc = pool_alloc(c, 2 * rows * 4, &tmp[5], st);
+
+  AttnBwdParams p{};
+  p.ws = tmp[5];
+  p.lse = lse;
+  p.out = op; p.dout = dop;
+  p.o_sb = os[0]; p.o_sh = os[1]; p.o_ss = os[2];
+  p.d_sb = dos[0]; p.d_sh = dos[1]; p.d_ss = dos[2];
+  p.B = (uint32_t)B; p.Hq = (uint32_t)Hq; p.Sq = (uint32_t)Sq; p.Sk = (uint32_t)Sk; p.Hkv = (uint32_t)Hkv;
+  p.group = (uint32_t)(Hq / Hkv);
+  p.nqb = (uint32_t)nqb; p.nkb = (uint32_t)nkb;
+  p.nqd = (uint32_t)((Sq + kAttnBwdDkdvQueries - 1) / kAttnBwdDkdvQueries);
+  p.Sqp = (uint32_t)(nqb * kAttnBlock);
+  p.causal = args->causal != 0 ? 1u : 0u;
+  p.D = (uint32_t)D;
+  p.scale_log2 = (float)((double)args->scale * 1.4426950408889634074);
+  p.scale = args->scale;
+  const uint32_t DB = D <= 64 ? 64 : 128;
+  const std::string in_tag = dt_tag(in_dtype), g_tag = dt_tag(grad_dtype);
+  const CUtensorMapDataType dt = in_dtype == B200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  const CUtensorMapDataType gdt = gsz == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_UINT16;
+  const uint64_t dimq[4] = {D, has_q ? Sq : Sk, has_q ? Hq : Hkv, B}, dimk[4] = {D, Sk, Hkv, B};
+  const uint64_t sq[3] = {qs[2], qs[1], qs[0]}, sk[3] = {ks[2], ks[1], ks[0]}, sv[3] = {vs[2], vs[1], vs[0]}, sdo[3] = {dos[2], dos[1], dos[0]};
+  const uint32_t box128[4] = {64, (uint32_t)kAttnBlock, 1, 1}, box_g[4] = {(uint32_t)(128 / gsz), 64, 1, 1};
+  auto set_smem = [&](CUfunction f, unsigned smem) -> int {
+    if (c->dry) return B200_OK;
+    CUresult r = g_drv.cuFuncSetAttribute_p(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem);
+    return r != CUDA_SUCCESS ? fail(map_cu(r), "cuFuncSetAttribute: %s", cu_err(r)) : B200_OK;
+  };
+
+  // 1. delta and L into the workspace
+  if (!rc && has_q) {
+    CUfunction f = nullptr;
+    rc = get_func(c, "attn_bwd_delta_" + in_tag + "_" + dt_tag(out_dtype), &f);
+    void* kargs[] = {&p};
+    if (!rc) rc = launch(c, f, (unsigned)((rows + 15) / 16), 1, 1, 256, 0, 1, st, kargs);
+  }
+  // 2. dq: maps q, k, v, dout (query tiles of kAttnBlock rows, key tiles of kAttnBwdDqKeys), dq
+  if (!rc && has_q) {
+    const uint32_t box_k[4] = {64, (uint32_t)kAttnBwdDqKeys, 1, 1};
+    CUtensorMap mq, mk, mv, mdo, mdq;
+    const uint64_t sdq[3] = {dqs[2], dqs[1], dqs[0]};
+    rc = encode_tmap4(c, &mq, dt, 2, qp, dimq, sq, box128, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (!rc) rc = encode_tmap4(c, &mk, dt, 2, kp, dimk, sk, box_k, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (!rc) rc = encode_tmap4(c, &mv, dt, 2, vp, dimk, sv, box_k, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (!rc) rc = encode_tmap4(c, &mdo, dt, 2, dop, dimq, sdo, box128, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (!rc) rc = encode_tmap4(c, &mdq, gdt, gsz, dq, dimq, sdq, box_g, CU_TENSOR_MAP_SWIZZLE_128B);
+    CUfunction f = nullptr;
+    if (!rc) rc = get_func(c, "attn_bwd_dq_" + in_tag + "_d" + std::to_string(DB) + "_" + g_tag, &f);
+    const unsigned smem = 1024 + 2 * kAttnBlock * DB * 2 + 2 * kAttnBwdStages * kAttnBwdDqKeys * DB * 2 + 1024;
+    if (!rc) rc = set_smem(f, smem);
+    void* kargs[] = {&mq, &mk, &mv, &mdo, &mdq, &p};
+    if (!rc) rc = launch(c, f, (unsigned)(nqb * Hq * B), 1, 1, 384, smem, 1, st, kargs);
+  }
+  // 3. dk and dv: maps q, k, v, dout (query tiles of kAttnBwdDkdvQueries rows, key tiles of kAttnBlock), dk, dv
+  if (!rc) {
+    const uint32_t box_q[4] = {64, (uint32_t)kAttnBwdDkdvQueries, 1, 1};
+    CUtensorMap mq, mk, mv, mdo, mdk, mdv;
+    const uint64_t sdk[3] = {dks[2], dks[1], dks[0]}, sdv[3] = {dvs[2], dvs[1], dvs[0]};
+    rc = encode_tmap4(c, &mq, dt, 2, qp, dimq, sq, box_q, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (!rc) rc = encode_tmap4(c, &mk, dt, 2, kp, dimk, sk, box128, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (!rc) rc = encode_tmap4(c, &mv, dt, 2, vp, dimk, sv, box128, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (!rc) rc = encode_tmap4(c, &mdo, dt, 2, dop, dimq, sdo, box_q, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (!rc) rc = encode_tmap4(c, &mdk, gdt, gsz, dk, dimk, sdk, box_g, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (!rc) rc = encode_tmap4(c, &mdv, gdt, gsz, dv, dimk, sdv, box_g, CU_TENSOR_MAP_SWIZZLE_128B);
+    CUfunction f = nullptr;
+    if (!rc) rc = get_func(c, "attn_bwd_dkdv_" + in_tag + "_d" + std::to_string(DB) + "_" + g_tag, &f);
+    const unsigned smem = 1024 + 2 * kAttnBlock * DB * 2 + 2 * kAttnBwdStages * kAttnBwdDkdvQueries * DB * 2 +
+                          kAttnBwdStages * 2 * kAttnBwdDkdvQueries * 4 + 1024;
+    if (!rc) rc = set_smem(f, smem);
+    void* kargs[] = {&mq, &mk, &mv, &mdo, &mdk, &mdv, &p};
+    if (!rc) rc = launch(c, f, (unsigned)(nkb * Hkv * B), 1, 1, 384, smem, 1, st, kargs);
+  }
+  for (CUdeviceptr t : tmp)
+    if (t) pool_free(c, t, st);   // stream-ordered: reusable once the kernels have drained
   return rc;
 }
 

@@ -219,6 +219,44 @@ struct AttnParams {
   uint32_t pad;
 };
 
+// Fused attention backward (attn_bwd_*; capi.cpp: b200_attention_backward), three launches on one stream:
+//   attn_bwd_delta_<in>_<out>  16 threads per workspace row, 16 rows per 256-thread block, grid ceil(B * Hq * Sqp / 16).
+//   attn_bwd_dq_*              one CTA per (b, h, kAttnBlock-query block), grid nqb * Hq * B ordered as the forward's; K and V
+//                              stream in blocks of kAttnBwdDqKeys keys.  Shared memory: 1024 + 2 tiles of kAttnBlock rows (Q,
+//                              dO) + 2 * kAttnBwdStages tiles of kAttnBwdDqKeys rows (K, V) + 1024, tiles of DB 16-bit columns.
+//   attn_bwd_dkdv_*            one CTA per (b, hkv, kAttnBlock-key block), grid nkb * Hkv * B: block x = (kb * B + b) * Hkv + hk
+//                              when causal (key blocks with the most visible queries first), x = (b * Hkv + hk) * nkb + kb
+//                              otherwise (the CTAs of one kv head run together and share Q and dO in L2).  K and V stay
+//                              resident; Q, dO and the workspace slices stream per (group head, query block of
+//                              kAttnBwdDkdvQueries).  Shared memory: 1024 + 2 tiles of kAttnBlock rows + 2 * kAttnBwdStages
+//                              tiles of kAttnBwdDkdvQueries rows + kAttnBwdStages * 2 * kAttnBwdDkdvQueries f32 + 1024.
+// The score tiles are 64 wide in both kernels: at DB = 128 the dq consumer holds dQ (64 registers) plus S and dP (32 each),
+// the dkdv consumer dK and dV (64 each) plus S^T and dP^T (32 each); 128-wide score tiles would not fit setmaxnreg's 232.
+// Workspace ws: f32 [2][B * Hq][Sqp], Sqp = nqb * kAttnBlock.  Plane 0 holds L = lse * log2 e for rows < Sq and +inf past Sq
+// (so p = exp2(t - L) is +0 for the zero-filled query rows past Sq), plane 1 delta = rowsum(dout * out) and 0 past Sq.  Rows
+// are padded so every query block's slice is a 16-byte aligned bulk copy.
+constexpr int kAttnBwdDqKeys = 64;
+constexpr int kAttnBwdDkdvQueries = 64;
+constexpr int kAttnBwdStages = 2;
+struct AttnBwdParams {
+  uint64_t ws;                    // workspace (above)
+  uint64_t lse;                   // delta kernel: the forward's compact f32 [B, Hq, Sq] log-sum-exp
+  uint64_t out, dout;             // delta kernel: views with a unit D stride, 16-byte aligned base and strides
+  uint64_t o_sb, o_sh, o_ss;      // out strides in elements (B, H, S)
+  uint64_t d_sb, d_sh, d_ss;      // dout strides in elements
+  uint32_t B, Hq, Sq, Sk;
+  uint32_t group;                 // Hq / Hkv
+  uint32_t nqb;                   // ceil(Sq / kAttnBlock)
+  uint32_t nkb;                   // ceil(Sk / kAttnBlock)
+  uint32_t nqd;                   // ceil(Sq / kAttnBwdDkdvQueries)
+  uint32_t Sqp;                   // nqb * kAttnBlock
+  uint32_t causal;                // 1: key j visible to query i iff j <= i
+  uint32_t D;
+  float scale_log2;               // scale * log2(e), the forward's value
+  float scale;                    // multiplies dQ and dK in the epilogue
+  uint32_t Hkv;
+};
+
 // ================================================================================================ conv_grouped.cu
 // Direct NHWC grouped convolution (b200_conv2d_grouped*, group width Cg = C / groups < 64).  Group g owns input channels
 // [g Cg, (g+1) Cg) and output channels [g Coutg, (g+1) Coutg).  Every strided operand has a unit channel stride; strides

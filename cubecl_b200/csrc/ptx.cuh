@@ -348,15 +348,21 @@ __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.
   else if constexpr (KA == 6 && KB == 5) B200_WGMMA(N, R, 32, "s32.s8.u8", "");                               \
   else B200_WGMMA(N, R, 32, "s32.s8.s8", "");
 
+// m64n64 f32 accumulators (the register list is B200_WG_REGS_64)
+#define B200_WG_OPS_F64 "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+
+// m64n64: s8 x s8 into s32, or f16 / bf16 with both operands K-major into f32 (the attention backward's 64-wide score tiles).
 template <int N, int KA, int KB, int TA, int TB, typename Acc>
 __device__ __forceinline__ void wgmma_ss(Acc (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d) {
-  static_assert(N == 112 || N == 128 || N == 256 || (N == 64 && KA == 6 && KB == 6), "m64n112 / m64n128 / m64n256, m64n64 s8 only");
-  if constexpr (N == 64) B200_WGMMA(64, R, 32, "s32.s8.s8", "");
+  static_assert(N == 112 || N == 128 || N == 256 || (N == 64 && KA == 6 && KB == 6) ||
+                    (N == 64 && KA == KB && KA <= 1 && TA == 0 && TB == 0),
+                "m64n112 / m64n128 / m64n256; m64n64 s8, or f16 / bf16 K-major");
+  if constexpr (N == 64 && KA == 6) B200_WGMMA(64, R, 32, "s32.s8.s8", "");
+  else if constexpr (N == 64 && KA == 0) B200_WGMMA(64, F, 16, "f32.f16.f16", ", 1, 1, 0, 0");
+  else if constexpr (N == 64) B200_WGMMA(64, F, 16, "f32.bf16.bf16", ", 1, 1, 0, 0");
   else if constexpr (N == 112) { B200_WGMMA_ALL(112) } else if constexpr (N == 128) { B200_WGMMA_ALL(128) } else { B200_WGMMA_ALL(256) }
 }
 
-// m64n64 f32 accumulators (the register list is B200_WG_REGS_64)
-#define B200_WG_OPS_F64 "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
 // Register-A operand of m64nNk16 (16-bit kinds): four registers of two values each, after the N / 2 accumulators.  Thread
 // (warp w, lane) holds rows 16 w + lane / 4 (+8) and k = 2 (lane % 4) (+1, +8, +9): a0 (r, k), a1 (r + 8, k), a2 (r, k + 8),
 // a3 (r + 8, k + 8) -- the layout of columns 16 kk .. 16 kk + 15 of an m64nN f32 accumulator fragment, packed in pairs.

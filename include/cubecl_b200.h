@@ -546,6 +546,46 @@ int b200_attention(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b200_dtype
                    b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides,
                    b200_dptr lse, const b200_attention_args* args);
 
+/* ---- fused scaled-dot-product attention, backward (PyTorch's SDPA backward, given the forward's out and lse) --------------
+ * With P_ij = exp(scale * q_i . k_j - lse_i) (0 for keys hidden by causal), delta_i = sum_d dout_id * out_id and
+ * dS_ij = P_ij * (dout_i . v_j - delta_i):
+ *   dq_i = scale * sum_j dS_ij k_j      dk_j = scale * sum_{h in group, i} dS_ij q_i      dv_j = sum_{h in group, i} P_ij dout_i
+ * (with GQA / MQA, dk and dv of kv head hk sum over the G = Hq / Hkv query heads that read it).  q, out, dout and dq are
+ * [B, Hq, Sq, D]; k, v, dk and dv are [B, Hkv, Sk, D]; lse is the forward's compact f32 [B, Hq, Sq] (b200_attention's lse
+ * output, natural log).  args, dtypes of q / k / v, views, causal rule and D limits are b200_attention's; out is in the input
+ * dtype or f32 (out_dtype), dout in the input dtype, dq, dk and dv all in grad_dtype (the input dtype or B200_F32).
+ * Numerics: t = s * (scale * log2 e) with the forward's f32 factor, so the recomputed scores are the forward's bit for bit;
+ * L_i = lse_i * log2 e is formed once per row in f32 and p = exp2(t - L) (ex2.approx.ftz).  dS is formed in f32 from the f32
+ * p; P and dS are rounded (RNE) to the input dtype for the products dV += P^T dO, dK += dS^T Q and dQ += dS K.  delta is an
+ * f32 sum.  dq, dk and dv are f32 sums, multiplied by scale (dq, dk) in f32 and rounded once (RNE) to grad_dtype.  Bitwise
+ * reproducible for fixed shapes, dtypes and views: every dq row comes from one CTA in increasing key order, every dk / dv row
+ * from one CTA in (group head, query block) order; no atomics.  Q.K^T and dO.V^T are computed by both the dq and the dk / dv
+ * kernel (7 GEMM-sized products where an atomic dq needs 5).
+ * Views: q, k, v, out and dout are read in place under b200_attention's rule for its inputs, else gathered into a compact
+ * pooled copy (one b200_into_contiguous launch each).  dq, dk and dv need a unit D stride and a 16-byte aligned base and
+ * strides (so they can be the slices of one fused [B, S, 3, H, D] gradient buffer), else B200_ERR_UNSUPPORTED naming the
+ * tensor.  lse must be non-null and 4-byte aligned.
+ * dk and dv are always written in full: a key no query sees gets +0 (causal with j >= Sq, and every key when Sq = 0 or
+ * Hq = 0).  Only B = 0, or Sk = 0 together with Sq = 0, launches nothing.
+ * Errors: as b200_attention, plus B200_ERR_INVALID_ARG when out, dout or dq differ from q's shape or dk or dv from k's, a
+ * null or misaligned lse; B200_ERR_UNSUPPORTED for an out_dtype or grad_dtype other than the input dtype or f32.
+ * Launches, all on `s` with no host synchronisation: the gathers; a pooled f32 workspace of 2 * B * Hq * ceil(Sq / 128) * 128
+ * values ("alloc"); attn_bwd_delta_<in>_<out> (ceil(rows / 16) blocks of 256 threads); attn_bwd_dq_<in>_d<64|128>_<grad>
+ * (ceil(Sq / 128) * Hq * B CTAs) after its maps q, k, v, dout, dq; attn_bwd_dkdv_<in>_d<64|128>_<grad> (ceil(Sk / 128) *
+ * Hkv * B CTAs) after its maps q, k, v, dout, dk, dv.  With Sq = 0 or Hq = 0 only the dk / dv kernel runs (its q and dout
+ * maps then describe k and are never read).  The maps are "tmap4d" plan lines as b200_attention's. */
+int b200_attention_backward(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dtype grad_dtype,
+                            b200_dptr q, const uint64_t* q_shape, const uint64_t* q_strides,
+                            b200_dptr k, const uint64_t* k_shape, const uint64_t* k_strides,
+                            b200_dptr v, const uint64_t* v_shape, const uint64_t* v_strides,
+                            b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides,
+                            b200_dptr dout, const uint64_t* dout_shape, const uint64_t* dout_strides,
+                            b200_dptr lse,
+                            b200_dptr dq, const uint64_t* dq_shape, const uint64_t* dq_strides,
+                            b200_dptr dk, const uint64_t* dk_shape, const uint64_t* dk_strides,
+                            b200_dptr dv, const uint64_t* dv_shape, const uint64_t* dv_strides,
+                            const b200_attention_args* args);
+
 /* ---- collectives: ServerCommunication (server/base.rs:632-739), CUDA impl cubecl-cuda/src/compute/server.rs:666-926 -- */
 #define B200_UNIQUE_ID_BYTES 128
 int b200_comm_get_unique_id(b200_ctx* ctx, void* id128);            /* ncclGetUniqueId (communication.rs:11-25 holds it per device set) */

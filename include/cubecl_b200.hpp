@@ -394,6 +394,32 @@ inline void launch(ComputeClient& client, const TensorHandle& q, const TensorHan
                                 lse ? lse->handle.ptr() : 0, &args);
   if (rc != B200_OK) client.defer(b200_last_error());
 }
+
+/// Fused scaled-dot-product attention, backward: dq [B, Hq, Sq, D], dk and dv [B, Hkv, Sk, D] (one grad dtype) from q, k, v,
+/// the forward's out and lse (compact f32 [B, Hq, Sq]) and dout.  See b200_attention_backward in cubecl_b200.h.  Errors are
+/// deferred to client.sync().
+inline void launch_backward(ComputeClient& client, const TensorHandle& q, const TensorHandle& k, const TensorHandle& v, const TensorHandle& out,
+                            const TensorHandle& dout, const TensorHandle& lse, const TensorHandle& dq, const TensorHandle& dk,
+                            const TensorHandle& dv, float scale, bool causal = false) {
+  for (const TensorHandle* t : {&q, &k, &v, &out, &dout, &dq, &dk, &dv}) {
+    if (t->shape.size() != 4) {
+      client.defer("InvalidArgument: attention backward needs rank-4 q, k, v, out, dout, dq, dk and dv");
+      return;
+    }
+  }
+  if (q.dtype != k.dtype || q.dtype != v.dtype || q.dtype != dout.dtype || dq.dtype != dk.dtype || dq.dtype != dv.dtype) {
+    client.defer("InvalidArgument: attention backward needs q, k, v and dout of one dtype and dq, dk and dv of one dtype");
+    return;
+  }
+  const b200_attention_args args{scale, causal ? 1 : 0};
+  const int rc = b200_attention_backward(
+      client.raw(), nullptr, static_cast<b200_dtype>(q.dtype), static_cast<b200_dtype>(out.dtype), static_cast<b200_dtype>(dq.dtype),
+      q.handle.ptr(), q.shape.data(), q.strides.data(), k.handle.ptr(), k.shape.data(), k.strides.data(), v.handle.ptr(), v.shape.data(),
+      v.strides.data(), out.handle.ptr(), out.shape.data(), out.strides.data(), dout.handle.ptr(), dout.shape.data(), dout.strides.data(),
+      lse.handle.ptr(), dq.handle.ptr(), dq.shape.data(), dq.strides.data(), dk.handle.ptr(), dk.shape.data(), dk.strides.data(),
+      dv.handle.ptr(), dv.shape.data(), dv.strides.data(), &args);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
 }  // namespace attention
 
 namespace reduce {

@@ -552,6 +552,29 @@ impl Context {
         ))
     }
 
+    /// Fused scaled-dot-product attention, backward: dq [B, Hq, Sq, D], dk and dv [B, Hkv, Sk, D] in `grad_dtype` (the input
+    /// dtype or f32) from q, k, v, the forward's `out` (in `out_dtype`) and `lse` (its compact f32 [B, Hq, Sq] buffer) and
+    /// `dout` (in the input dtype).  See b200_attention_backward in cubecl_b200.h.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::conv2d`]; `lse` must hold B * Hq * Sq f32 values.
+    pub unsafe fn attention_backward(
+        &mut self, stream: b200_stream, in_dtype: DType, out_dtype: DType, grad_dtype: DType, q: &TensorView, k: &TensorView,
+        v: &TensorView, out: &TensorView, dout: &TensorView, lse: b200_dptr, dq: &TensorView, dk: &TensorView, dv: &TensorView,
+        scale: f32, causal: bool,
+    ) -> Result<(), Error> {
+        for t in [q, k, v, out, dout, dq, dk, dv] {
+            assert!(t.shape.len() == 4 && t.strides.len() == 4);
+        }
+        let a = sys::b200_attention_args { scale, causal: causal as i32 };
+        check(sys::b200_attention_backward(
+            self.0, stream, in_dtype as c_int, out_dtype as c_int, grad_dtype as c_int, q.ptr, q.shape.as_ptr(), q.strides.as_ptr(),
+            k.ptr, k.shape.as_ptr(), k.strides.as_ptr(), v.ptr, v.shape.as_ptr(), v.strides.as_ptr(), out.ptr, out.shape.as_ptr(),
+            out.strides.as_ptr(), dout.ptr, dout.shape.as_ptr(), dout.strides.as_ptr(), lse, dq.ptr, dq.shape.as_ptr(),
+            dq.strides.as_ptr(), dk.ptr, dk.shape.as_ptr(), dk.strides.as_ptr(), dv.ptr, dv.shape.as_ptr(), dv.strides.as_ptr(), &a,
+        ))
+    }
+
     /// Grouped / depthwise [`Context::conv2d`]: w [Cout, KH, KW, C / groups].  See b200_conv2d_grouped in cubecl_b200.h.
     ///
     /// # Safety
