@@ -1,7 +1,8 @@
 """cubecl_b200: H100-native (sm_90a) implementation of CubeCL's dense linear-algebra hot path.
 
-  matmul.launch / conv.launch / conv3d.launch / conv_transpose.launch / attention.launch / reduce.launch / scan.launch / quant.quantize over ComputeClient + TensorHandle  ->  C ABI (include/cubecl_b200.h)
-  ->  prebuilt sm_90a cubins: wgmma/TMA GEMM (csrc/gemm_wgmma.cu), fused attention (csrc/attention.cu, attention_bwd.cu), HBM-bound reductions
+  matmul.launch / conv.launch / conv3d.launch / conv_transpose.launch / attention.launch / attention.launch_kvcache / reduce.launch / scan.launch / quant.quantize over ComputeClient + TensorHandle  ->  C ABI (include/cubecl_b200.h)
+  ->  prebuilt sm_90a cubins: wgmma/TMA GEMM (csrc/gemm_wgmma.cu), fused attention (csrc/attention.cu, attention_bwd.cu), split-KV decoding
+      against a paged KV cache (csrc/attention_kv.cu), HBM-bound reductions
       (csrc/reduce.cu), quantization (csrc/quant.cu).
 
 There is no CPU implementation in this package; the CPU oracle lives in /oracle and is test infrastructure only.

@@ -13,6 +13,12 @@ memory.  See include/cubecl_b200.h (b200_attention) for the numerics and the vie
 The backward (launch_backward) takes the forward's out and lse with dout and writes dq [B, Hq, Sq, D] and dk, dv [B, Hkv, Sk, D]
 (with GQA, dk and dv sum over the query heads of each kv head); three kernels (csrc/attention_bwd.cu), no atomics, bitwise
 reproducible.  See b200_attention_backward for its numerics.
+
+Against a KV cache (launch_kvcache, for decoding): q [B, Hq, Sq, D] attends to the first L_b = cache_seqlens[b] keys of
+sequence b in a paged cache k_cache, v_cache [P, page, Hkv, D] reached through an i32 block_table [B, max_pages] (None: page b
+is sequence b).  causal is bottom-right there: query i also needs j <= L_b - Sq + i.  kvcache_write scatters new tokens
+[B, Snew, Hkv, D] into cache slots (slot_mapping, i32 [B * Snew]; negative slots are skipped).  One split-KV kernel with a
+fixed-order combine (csrc/attention_kv.cu); see b200_attention_kvcache and b200_kvcache_write.
 """
 from __future__ import annotations
 
@@ -122,3 +128,79 @@ def launch_backward_alloc(client: ComputeClient, q: TensorHandle, k: TensorHandl
     dv = TensorHandle.empty_contiguous(client, list(k.shape), gd)
     launch_backward(client, q, k, v, out, dout, lse, dq, dk, dv, scale=scale, causal=causal, stream=stream)
     return dq, dk, dv
+
+
+def _view_args(tensors):
+    ops = []
+    for t in tensors:
+        ops += [C.c_uint64(t.handle.ptr), _ffi.u64_array(t.shape), _ffi.u64_array(t.strides)]
+    return ops
+
+
+def launch_kvcache(client: ComputeClient, q: TensorHandle, k_cache: TensorHandle, v_cache: TensorHandle, cache_seqlens: TensorHandle,
+                   out: TensorHandle, block_table: TensorHandle | None = None, scale: float | None = None, causal: bool = False,
+                   lse: TensorHandle | None = None, stream=None) -> None:
+    """Enqueue attention of q [B, Hq, Sq, D] against a KV cache k_cache, v_cache [P, page, Hkv, D] (views by strides): sequence b
+    sees its first cache_seqlens[b] keys (compact i32 [B], read on the device), key j at row j % page of page
+    block_table[b, j / page] (i32 [B, max_pages]; None: page b).  causal: bottom-right (query i sees j <= L_b - Sq + i).  scale
+    defaults to 1 / sqrt(D); lse: an optional compact f32 [B, Hq, Sq] tensor.  Never raises for launch problems: errors are
+    deferred to client.sync()."""
+    try:
+        for name, t in (("q", q), ("k_cache", k_cache), ("v_cache", v_cache), ("out", out)):
+            if len(t.shape) != 4:
+                raise B200Error(6, f"attention_kvcache: {name} must have rank 4, got rank {len(t.shape)}")
+        if not (q.dtype == k_cache.dtype == v_cache.dtype):
+            raise B200Error(6, f"attention_kvcache: q, k_cache and v_cache dtypes differ ({q.dtype}, {k_cache.dtype}, {v_cache.dtype})")
+        if cache_seqlens.dtype != "i32" or not cache_seqlens.is_contiguous() or list(cache_seqlens.shape) != [q.shape[0]]:
+            raise B200Error(6, f"attention_kvcache: cache_seqlens must be a compact i32 [B] = [{q.shape[0]}] tensor")
+        if block_table is not None and (block_table.dtype != "i32" or len(block_table.shape) != 2):
+            raise B200Error(6, "attention_kvcache: block_table must be an i32 [B, max_pages] tensor")
+        if lse is not None and (lse.dtype != "f32" or not lse.is_contiguous() or list(lse.shape) != list(q.shape[:3])):
+            raise B200Error(6, f"attention_kvcache: lse must be a compact f32 [B, Hq, Sq] = {list(q.shape[:3])} tensor")
+        sc = 1.0 / math.sqrt(q.shape[3]) if scale is None else float(scale)
+        extra = tuple(t for t in (block_table, lse) if t is not None)
+        for t in (q, k_cache, v_cache, cache_seqlens, out) + extra:
+            t.handle.used_on(stream)
+        args = _ffi.AttentionArgs(sc, 1 if causal else 0)
+        bt = ([C.c_uint64(block_table.handle.ptr), _ffi.u64_array(block_table.shape), _ffi.u64_array(block_table.strides)]
+              if block_table is not None else [C.c_uint64(0), None, None])
+        _ffi.check(client._lib.b200_attention_kvcache(
+            client._ctx, stream, DTYPES[q.dtype], DTYPES[out.dtype], *_view_args((q, k_cache, v_cache)), *bt,
+            C.c_uint64(cache_seqlens.handle.ptr), *_view_args((out,)), C.c_uint64(lse.handle.ptr if lse is not None else 0),
+            C.byref(args)))
+    except (B200Error, ValueError) as e:
+        client._defer(e if isinstance(e, B200Error) else B200Error(6, str(e)))
+
+
+def launch_kvcache_alloc(client: ComputeClient, q: TensorHandle, k_cache: TensorHandle, v_cache: TensorHandle,
+                         cache_seqlens: TensorHandle, block_table: TensorHandle | None = None, scale: float | None = None,
+                         causal: bool = False, out_dtype: str | None = None, return_lse: bool = False, stream=None):
+    """Convenience: allocate a compact out [B, Hq, Sq, D] (and, with return_lse, a compact f32 lse [B, Hq, Sq]), then
+    launch_kvcache.  Returns out, or (out, lse)."""
+    out = TensorHandle.empty_contiguous(client, list(q.shape), out_dtype or q.dtype)
+    lse = TensorHandle.empty_contiguous(client, list(q.shape[:3]), "f32") if return_lse else None
+    launch_kvcache(client, q, k_cache, v_cache, cache_seqlens, out, block_table=block_table, scale=scale, causal=causal, lse=lse,
+                   stream=stream)
+    return (out, lse) if return_lse else out
+
+
+def kvcache_write(client: ComputeClient, k_new: TensorHandle, v_new: TensorHandle, k_cache: TensorHandle, v_cache: TensorHandle,
+                  slot_mapping: TensorHandle, stream=None) -> None:
+    """Enqueue the scatter of k_new, v_new [B, Snew, Hkv, D] into k_cache, v_cache [P, page, Hkv, D]: token t of sequence b goes
+    to flat slot slot_mapping[b * Snew + t] (compact i32; page slot / page, row slot % page); negative slots are skipped.  Lengths
+    stay with the caller.  Errors are deferred to client.sync()."""
+    try:
+        for name, t in (("k_new", k_new), ("v_new", v_new), ("k_cache", k_cache), ("v_cache", v_cache)):
+            if len(t.shape) != 4:
+                raise B200Error(6, f"kvcache_write: {name} must have rank 4, got rank {len(t.shape)}")
+        if not (k_new.dtype == v_new.dtype == k_cache.dtype == v_cache.dtype):
+            raise B200Error(6, "kvcache_write: k_new, v_new, k_cache and v_cache dtypes differ")
+        n = k_new.shape[0] * k_new.shape[1]
+        if slot_mapping.dtype != "i32" or not slot_mapping.is_contiguous() or math.prod(slot_mapping.shape) != n:
+            raise B200Error(6, f"kvcache_write: slot_mapping must be a compact i32 tensor of B * Snew = {n} slots")
+        for t in (k_new, v_new, k_cache, v_cache, slot_mapping):
+            t.handle.used_on(stream)
+        _ffi.check(client._lib.b200_kvcache_write(client._ctx, stream, DTYPES[k_cache.dtype], *_view_args((k_new, v_new, k_cache, v_cache)),
+                                                  C.c_uint64(slot_mapping.handle.ptr)))
+    except (B200Error, ValueError) as e:
+        client._defer(e if isinstance(e, B200Error) else B200Error(6, str(e)))

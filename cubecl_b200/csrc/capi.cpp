@@ -60,6 +60,8 @@ extern const unsigned char b200_cubin_attention[];
 extern const unsigned char b200_cubin_attention_end[];
 extern const unsigned char b200_cubin_attention_bwd[];
 extern const unsigned char b200_cubin_attention_bwd_end[];
+extern const unsigned char b200_cubin_attention_kv[];
+extern const unsigned char b200_cubin_attention_kv_end[];
 }
 
 // ================================================================================================ errors
@@ -331,13 +333,14 @@ static int get_func(b200_ctx* c, const std::string& name, CUfunction* out) {
   auto it = c->funcs.find(name);
   if (it != c->funcs.end()) { *out = it->second; return B200_OK; }
   // modules are loaded in the order gemm, reduce, aux, gemm_b, gemm_c, quant, gemm_q, quant_mm, gemm_conv, gemm_convbwd,
-  // conv_grouped, gemm_conv3d, gemm_convt, attention, attention_bwd; the kernel
+  // conv_grouped, gemm_conv3d, gemm_convt, attention, attention_bwd, attention_kv; the kernel
   // name says where a
   // kernel lives (no failing lookups, which API-level tools such as compute-sanitizer would report)
   auto starts = [&](const char* pfx) { return name.rfind(pfx, 0) == 0; };
   auto has = [&](const char* part) { return name.find(part) != std::string::npos; };
   const bool tc_gemm = starts("gemm_") && name != "gemm_simt_strided" && name != "gemm_scaled_simt";
   const size_t home = name == "conv3d_dgrad_weights" ? 2
+                      : starts("attn_kv_") ? 15
                       : starts("attn_bwd_") ? 14
                       : starts("attn_") ? 13
                       : starts("conv2d_tconv_") || starts("conv3d_tconv_") ? 12
@@ -381,7 +384,8 @@ extern "C" int b200_get_cubin(const char* name, const void** image, size_t* size
   else if (!strcmp(name, "gemm_convt")) { b = b200_cubin_gemm_convt; e = b200_cubin_gemm_convt_end; }
   else if (!strcmp(name, "attention")) { b = b200_cubin_attention; e = b200_cubin_attention_end; }
   else if (!strcmp(name, "attention_bwd")) { b = b200_cubin_attention_bwd; e = b200_cubin_attention_bwd_end; }
-  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd|conv_grouped|gemm_conv3d|gemm_convt|attention|attention_bwd)", name);
+  else if (!strcmp(name, "attention_kv")) { b = b200_cubin_attention_kv; e = b200_cubin_attention_kv_end; }
+  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd|conv_grouped|gemm_conv3d|gemm_convt|attention|attention_bwd|attention_kv)", name);
   *image = b;
   *size = static_cast<size_t>(e - b);
   return B200_OK;
@@ -443,7 +447,8 @@ extern "C" int b200_init(int device, b200_ctx** out) {
       (rc = load_module(c, b200_cubin_gemm_conv3d, b200_cubin_gemm_conv3d_end, "gemm_conv3d")) ||
       (rc = load_module(c, b200_cubin_gemm_convt, b200_cubin_gemm_convt_end, "gemm_convt")) ||
       (rc = load_module(c, b200_cubin_attention, b200_cubin_attention_end, "attention")) ||
-      (rc = load_module(c, b200_cubin_attention_bwd, b200_cubin_attention_bwd_end, "attention_bwd"))) {
+      (rc = load_module(c, b200_cubin_attention_bwd, b200_cubin_attention_bwd_end, "attention_bwd")) ||
+      (rc = load_module(c, b200_cubin_attention_kv, b200_cubin_attention_kv_end, "attention_kv"))) {
     for (CUmodule m : c->modules) g_drv.cuModuleUnload_p(m);
     g_drv.cuDevicePrimaryCtxRelease_p(c->dev);
     return bail(rc);
@@ -4453,6 +4458,226 @@ extern "C" int b200_attention_backward(b200_ctx* c, b200_stream s, b200_dtype in
   }
   for (CUdeviceptr t : tmp)
     if (t) pool_free(c, t, st);   // stream-ordered: reusable once the kernels have drained
+  return rc;
+}
+
+// The m-tile of b200_attention_kvcache: st queries of gt heads of one kv head's G (gt * st <= kAttnKvRows), the pair with the
+// fewest m-tiles ceil(G / gt) * ceil(Sq / st); among equals the largest st.
+static void kv_tile(uint64_t G, uint64_t Sq, uint32_t* gt, uint32_t* st) {
+  uint64_t best = UINT64_MAX;
+  for (uint64_t s = std::min<uint64_t>(Sq, kAttnKvRows); s >= 1; --s) {
+    const uint64_t g = std::min<uint64_t>(G, kAttnKvRows / s);
+    const uint64_t n = ((G + g - 1) / g) * ((Sq + s - 1) / s);
+    if (n < best) { best = n; *gt = (uint32_t)g; *st = (uint32_t)s; }
+  }
+}
+
+// The split count of b200_attention_kvcache from shapes only: `units` = B * Hkv * m-tiles CTAs per split, nkb key blocks of
+// capacity, one CTA per SM.  The count n minimising ceil(units * n / sms) * (ceil(nkb / n) + kAttnKvSplitCost), over the n
+// whose equal ranges of ceil(nkb / n) blocks are all non-empty; ties keep the smaller n.
+static uint32_t kv_splits(uint64_t units, uint64_t nkb, int sms) {
+  uint64_t best_n = 1, best = UINT64_MAX;
+  for (uint64_t n = 1; n <= std::min<uint64_t>(nkb, kAttnKvMaxSplits); ++n) {
+    const uint64_t bps = (nkb + n - 1) / n;
+    if ((nkb + bps - 1) / bps != n) continue;
+    const uint64_t cost = (units * n + sms - 1) / sms * (bps + kAttnKvSplitCost);
+    if (cost < best) { best = cost; best_n = n; }
+  }
+  return (uint32_t)best_n;
+}
+
+// Attention of q against a paged KV cache (see cubecl_b200.h): one attn_kv_* launch, plus attn_kv_combine_* when the keys
+// are split.
+extern "C" int b200_attention_kvcache(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr q,
+                                      const uint64_t* q_shape, const uint64_t* q_strides, b200_dptr k_cache, const uint64_t* kc_shape,
+                                      const uint64_t* kc_strides, b200_dptr v_cache, const uint64_t* vc_shape, const uint64_t* vc_strides,
+                                      b200_dptr block_table, const uint64_t* bt_shape, const uint64_t* bt_strides, b200_dptr cache_seqlens,
+                                      b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides, b200_dptr lse,
+                                      const b200_attention_args* args) {
+  CTX_ENTER(c);
+  const char* what = "attention_kvcache";
+  auto ull = [](uint64_t x) { return (unsigned long long)x; };
+  if (!q_shape || !kc_shape || !vc_shape || !out_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
+  if (block_table && !bt_shape) return fail(B200_ERR_INVALID_ARG, "%s: null block-table shape", what);
+  if (in_dtype != B200_F16 && in_dtype != B200_BF16)
+    return fail(B200_ERR_UNSUPPORTED, "%s: input dtype %d unsupported (f16, bf16)", what, (int)in_dtype);
+  if (out_dtype != in_dtype && out_dtype != B200_F32)
+    return fail(B200_ERR_UNSUPPORTED, "%s: output dtype must equal the input dtype or be f32", what);
+  const uint64_t B = q_shape[0], Hq = q_shape[1], Sq = q_shape[2], D = q_shape[3];
+  const uint64_t P = kc_shape[0], page = kc_shape[1], Hkv = kc_shape[2];
+  if (kc_shape[3] != D)
+    return fail(B200_ERR_INVALID_ARG, "%s: k_cache head dim %llu differs from q's D = %llu", what, ull(kc_shape[3]), ull(D));
+  if (vc_shape[0] != P || vc_shape[1] != page || vc_shape[2] != Hkv)
+    return fail(B200_ERR_INVALID_ARG, "%s: v_cache [%llu,%llu,%llu,%llu] does not match k_cache [%llu,%llu,%llu,%llu]", what, ull(vc_shape[0]),
+                ull(vc_shape[1]), ull(vc_shape[2]), ull(vc_shape[3]), ull(P), ull(page), ull(Hkv), ull(D));
+  if (vc_shape[3] != D) return fail(B200_ERR_UNSUPPORTED, "%s: v_cache's head dim %llu differs from D = %llu", what, ull(vc_shape[3]), ull(D));
+  if (Hkv == 0 || Hq % Hkv) return fail(B200_ERR_INVALID_ARG, "%s: Hq = %llu must be a multiple of Hkv = %llu", what, ull(Hq), ull(Hkv));
+  if (memcmp(out_shape, q_shape, 4 * sizeof(uint64_t)))
+    return fail(B200_ERR_INVALID_ARG, "%s: out is [%llu,%llu,%llu,%llu], expected [%llu,%llu,%llu,%llu]", what, ull(out_shape[0]),
+                ull(out_shape[1]), ull(out_shape[2]), ull(out_shape[3]), ull(B), ull(Hq), ull(Sq), ull(D));
+  if (page == 0 || P == 0) return fail(B200_ERR_INVALID_ARG, "%s: empty cache (P = %llu pages of %llu keys)", what, ull(P), ull(page));
+  const uint64_t max_pages = block_table ? bt_shape[1] : 1;
+  if (block_table && (bt_shape[0] != B || max_pages == 0))
+    return fail(B200_ERR_INVALID_ARG, "%s: block_table is [%llu,%llu], expected [%llu, max_pages >= 1]", what, ull(bt_shape[0]),
+                ull(bt_shape[1]), ull(B));
+  if (!block_table && P != B)
+    return fail(B200_ERR_INVALID_ARG, "%s: without a block table the cache holds one page per sequence (P = %llu, B = %llu)", what, ull(P), ull(B));
+  if (max_pages > 1 && (page % 16 || (kAttnKvBlock % page && page % kAttnKvBlock)))
+    return fail(B200_ERR_UNSUPPORTED, "%s: a page of %llu keys must be a multiple of 16 that divides %d or is a multiple of it", what,
+                ull(page), kAttnKvBlock);
+  if (!std::isfinite(args->scale)) return fail(B200_ERR_INVALID_ARG, "%s: scale must be finite", what);
+  if (D == 0 || D > 128 || D % 8) return fail(B200_ERR_UNSUPPORTED, "%s: head dim D = %llu unsupported (a multiple of 8 in [8, 128])", what, ull(D));
+  const uint64_t lim = 1ull << 31, cap = max_pages * page;
+  if (B >= lim || Hq >= lim || Sq >= lim || P >= lim || page >= lim || max_pages >= lim || cap >= lim)
+    return fail(B200_ERR_UNSUPPORTED, "%s: extents and the capacity max_pages * page must be < 2^31", what);
+  if (B == 0 || Hq == 0 || Sq == 0) return B200_OK;
+  if (!q || !k_cache || !v_cache || !cache_seqlens || !out) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
+  if (lse % 4 || cache_seqlens % 4 || block_table % 4)
+    return fail(B200_ERR_INVALID_ARG, "%s: lse, cache_seqlens and block_table must be 4-byte aligned", what);
+  const size_t osz = dtype_size(out_dtype);
+  uint64_t qs[4], ks[4], vs[4], os[4];
+  conv_norm_strides(out_shape, out_strides, os);
+  if (!attn_view_ok(out, osz, os))
+    return fail(B200_ERR_UNSUPPORTED, "%s: out needs a unit D stride and a 16-byte aligned base and S, H, B strides", what);
+  conv_norm_strides(kc_shape, kc_strides, ks);
+  conv_norm_strides(vc_shape, vc_strides, vs);
+  if (!attn_view_ok(k_cache, 2, ks) || !attn_view_ok(v_cache, 2, vs))
+    return fail(B200_ERR_UNSUPPORTED, "%s: a cache needs a unit D stride and a 16-byte aligned base and page, row and head strides "
+                "(it is read in place, never gathered)", what);
+  conv_norm_strides(q_shape, q_strides, qs);
+
+  const uint64_t G = Hq / Hkv;
+  uint32_t gt = 1, stq = 1;
+  kv_tile(G, Sq, &gt, &stq);
+  const uint64_t mtg = (G + gt - 1) / gt, mts = (Sq + stq - 1) / stq;
+  const uint64_t nkb = (cap + kAttnKvBlock - 1) / kAttnKvBlock;
+  const uint64_t units = B * Hkv * mtg * mts;
+  const uint32_t nsplit = kv_splits(units, nkb, c->props.num_sms);
+  const uint64_t bps = (nkb + nsplit - 1) / nsplit, ctas = units * nsplit, rows = B * Hq * Sq;
+  if (ctas >= lim || rows * (D / 4) / kAttnKvCombineThreads >= lim)
+    return fail(B200_ERR_UNSUPPORTED, "%s: more than 2^31 - 1 CTAs", what);
+
+  CUstream st = resolve_stream(c, s);
+  CUdeviceptr tmp[2] = {0, 0};   // the gather of q; the split workspace
+  uint64_t qp = q;
+  int rc = B200_OK;
+  if (!attn_view_ok(q, 2, qs)) {
+    rc = conv_gather(c, st, in_dtype, q, q_shape, qs, &tmp[0]);
+    qp = tmp[0];
+    qs[3] = 1; qs[2] = D; qs[1] = Sq * D; qs[0] = Hq * Sq * D;
+  }
+  if (!rc && nsplit > 1) rc = pool_alloc(c, (size_t)nsplit * rows * (D + 2) * 4, &tmp[1], st);
+  if (!rc) {
+    const uint32_t DB = D <= 64 ? 64 : 128;
+    const uint32_t R = max_pages == 1 ? kAttnKvBlock : (uint32_t)std::min<uint64_t>(page, kAttnKvBlock);
+    const CUtensorMapDataType dt = in_dtype == B200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+    CUtensorMap mq, mk, mv;
+    const uint32_t box_q[4] = {64, stq, gt, 1}, box_kv[4] = {64, R, 1, 1};
+    const uint64_t dq[4] = {D, Sq, Hq, B}, dkv[4] = {D, page, Hkv, P};
+    const uint64_t sq[3] = {qs[2], qs[1], qs[0]}, sk[3] = {ks[1], ks[2], ks[0]}, sv[3] = {vs[1], vs[2], vs[0]};
+    rc = encode_tmap4(c, &mq, dt, 2, qp, dq, sq, box_q, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (!rc) rc = encode_tmap4(c, &mk, dt, 2, k_cache, dkv, sk, box_kv, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (!rc) rc = encode_tmap4(c, &mv, dt, 2, v_cache, dkv, sv, box_kv, CU_TENSOR_MAP_SWIZZLE_128B);
+    AttnKvParams p{};
+    p.out = out; p.o_sb = os[0]; p.o_sh = os[1]; p.o_ss = os[2];
+    p.lse = lse;
+    p.ws = tmp[1];
+    p.table = block_table;
+    if (block_table) {
+      p.t_sb = bt_strides ? bt_strides[0] : max_pages;
+      p.t_sp = bt_strides ? bt_strides[1] : 1;
+    }
+    p.seqlens = cache_seqlens;
+    p.B = (uint32_t)B; p.Hq = (uint32_t)Hq; p.Hkv = (uint32_t)Hkv; p.Sq = (uint32_t)Sq; p.D = (uint32_t)D;
+    p.group = (uint32_t)G;
+    p.gt = gt; p.st = stq; p.mtg = (uint32_t)mtg; p.mts = (uint32_t)mts;
+    p.page = (uint32_t)page; p.rows = R;
+    p.cap = (uint32_t)cap; p.nkb = (uint32_t)nkb;
+    p.nsplit = nsplit; p.bps = (uint32_t)bps;
+    p.causal = args->causal != 0 ? 1u : 0u;
+    p.scale_log2 = (float)((double)args->scale * 1.4426950408889634074);
+    CUfunction f = nullptr;
+    const std::string in_tag = dt_tag(in_dtype), out_tag = dt_tag(out_dtype);
+    if (!rc) rc = get_func(c, "attn_kv_" + in_tag + "_d" + std::to_string(DB) + "_" + out_tag, &f);
+    const unsigned smem = 1024 + (DB / 64) * (kAttnKvRows + 2 * kAttnKvStages * kAttnKvBlock) * 128 + kAttnKvBarBytes;
+    if (!rc && !c->dry) {
+      CUresult r = g_drv.cuFuncSetAttribute_p(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem);
+      if (r != CUDA_SUCCESS) rc = fail(map_cu(r), "cuFuncSetAttribute: %s", cu_err(r));
+    }
+    void* kargs[] = {&mq, &mk, &mv, &p};
+    if (!rc) rc = launch(c, f, (unsigned)ctas, 1, 1, kAttnKvThreads, smem, 1, st, kargs);
+    if (!rc && nsplit > 1) {
+      rc = get_func(c, "attn_kv_combine_" + out_tag, &f);
+      void* cargs[] = {&p};
+      if (!rc) rc = launch(c, f, (unsigned)((rows * (D / 4) + kAttnKvCombineThreads - 1) / kAttnKvCombineThreads), 1, 1,
+                           kAttnKvCombineThreads, 0, 1, st, cargs);
+    }
+  }
+  for (CUdeviceptr t : tmp)
+    if (t) pool_free(c, t, st);   // stream-ordered: reusable once the kernels have drained
+  return rc;
+}
+
+// Scatter of new tokens into a paged KV cache (see cubecl_b200.h): one attn_kv_write launch.
+extern "C" int b200_kvcache_write(b200_ctx* c, b200_stream s, b200_dtype dtype, b200_dptr k_new, const uint64_t* kn_shape,
+                                  const uint64_t* kn_strides, b200_dptr v_new, const uint64_t* vn_shape, const uint64_t* vn_strides,
+                                  b200_dptr k_cache, const uint64_t* kc_shape, const uint64_t* kc_strides, b200_dptr v_cache,
+                                  const uint64_t* vc_shape, const uint64_t* vc_strides, b200_dptr slot_mapping) {
+  CTX_ENTER(c);
+  const char* what = "kvcache_write";
+  auto ull = [](uint64_t x) { return (unsigned long long)x; };
+  if (!kn_shape || !vn_shape || !kc_shape || !vc_shape) return fail(B200_ERR_INVALID_ARG, "%s: null shape", what);
+  if (dtype != B200_F16 && dtype != B200_BF16) return fail(B200_ERR_UNSUPPORTED, "%s: dtype %d unsupported (f16, bf16)", what, (int)dtype);
+  const uint64_t B = kn_shape[0], Snew = kn_shape[1], Hkv = kn_shape[2], D = kn_shape[3];
+  const uint64_t P = kc_shape[0], page = kc_shape[1];
+  if (memcmp(vn_shape, kn_shape, 4 * sizeof(uint64_t)))
+    return fail(B200_ERR_INVALID_ARG, "%s: v_new [%llu,%llu,%llu,%llu] does not match k_new [%llu,%llu,%llu,%llu]", what, ull(vn_shape[0]),
+                ull(vn_shape[1]), ull(vn_shape[2]), ull(vn_shape[3]), ull(B), ull(Snew), ull(Hkv), ull(D));
+  if (memcmp(vc_shape, kc_shape, 4 * sizeof(uint64_t))) return fail(B200_ERR_INVALID_ARG, "%s: v_cache does not match k_cache", what);
+  if (kc_shape[2] != Hkv || kc_shape[3] != D)
+    return fail(B200_ERR_INVALID_ARG, "%s: k_cache [%llu,%llu,%llu,%llu] differs from k_new [%llu,%llu,%llu,%llu] in heads or head dim", what,
+                ull(P), ull(page), ull(kc_shape[2]), ull(kc_shape[3]), ull(B), ull(Snew), ull(Hkv), ull(D));
+  if (D % 8) return fail(B200_ERR_UNSUPPORTED, "%s: head dim D = %llu must be a multiple of 8", what, ull(D));
+  const uint64_t units = B * Snew * Hkv * (D / 8);
+  if (units == 0) return B200_OK;
+  if (!k_new || !v_new || !k_cache || !v_cache || !slot_mapping) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
+  if (slot_mapping % 4) return fail(B200_ERR_INVALID_ARG, "%s: slot_mapping must be 4-byte aligned", what);
+  uint64_t kns[4], vns[4], kcs[4], vcs[4];
+  conv_norm_strides(kc_shape, kc_strides, kcs);
+  conv_norm_strides(vc_shape, vc_strides, vcs);
+  if (!attn_view_ok(k_cache, 2, kcs) || !attn_view_ok(v_cache, 2, vcs))
+    return fail(B200_ERR_UNSUPPORTED, "%s: a cache needs a unit D stride and a 16-byte aligned base and page, row and head strides", what);
+  conv_norm_strides(kn_shape, kn_strides, kns);
+  conv_norm_strides(vn_shape, vn_strides, vns);
+  CUstream st = resolve_stream(c, s);
+  CUdeviceptr tmp[2] = {0, 0};
+  uint64_t ptr[2] = {k_new, v_new};
+  uint64_t* ns[2] = {kns, vns};
+  int rc = B200_OK;
+  for (int i = 0; i < 2 && !rc; ++i) {   // the kernel moves 16-byte units: other views are gathered into a compact copy first
+    if (attn_view_ok(ptr[i], 2, ns[i])) continue;
+    rc = conv_gather(c, st, dtype, ptr[i], kn_shape, ns[i], &tmp[i]);
+    ptr[i] = tmp[i];
+    ns[i][3] = 1; ns[i][2] = D; ns[i][1] = Hkv * D; ns[i][0] = Snew * Hkv * D;
+  }
+  if (!rc) {
+    AttnKvWriteParams p{};
+    p.kn = ptr[0]; p.vn = ptr[1]; p.kc = k_cache; p.vc = v_cache; p.slots = slot_mapping;
+    p.kn_sb = kns[0]; p.kn_st = kns[1]; p.kn_sh = kns[2];
+    p.vn_sb = vns[0]; p.vn_st = vns[1]; p.vn_sh = vns[2];
+    p.kc_sp = kcs[0]; p.kc_sr = kcs[1]; p.kc_sh = kcs[2];
+    p.vc_sp = vcs[0]; p.vc_sr = vcs[1]; p.vc_sh = vcs[2];
+    p.units = units;
+    p.Snew = (uint32_t)Snew; p.Hkv = (uint32_t)Hkv; p.D = (uint32_t)D; p.page = (uint32_t)page;
+    p.slot_end = P * page;
+    CUfunction f = nullptr;
+    rc = get_func(c, "attn_kv_write", &f);
+    void* kargs[] = {&p};
+    const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((units + 255) / 256, (uint64_t)c->props.num_sms * 32));
+    if (!rc) rc = launch(c, f, grid, 1, 1, 256, 0, 1, st, kargs);
+  }
+  for (CUdeviceptr t : tmp)
+    if (t) pool_free(c, t, st);
   return rc;
 }
 

@@ -257,6 +257,56 @@ struct AttnBwdParams {
   uint32_t Hkv;
 };
 
+// ================================================================================================ attention_kv.cu
+// Attention against a KV cache (attn_kv_*; capi.cpp: b200_attention_kvcache).  One CTA per (b, hk, m-tile, split), grid
+// B * Hkv * nsplit * mtiles with block x = ((b * Hkv + hk) * nsplit + split) * mtiles + mt (the m-tiles that share a key range
+// run side by side).  kAttnKvThreads threads: warps 0-3 are the consumer warpgroup, warp 4 the producer.  An m-tile packs gt
+// heads of one kv head's group with st queries, gt * st <= kAttnKvRows, row r = g * st + i; m-tile mt covers group heads
+// [(mt / mts) * gt, +gt) and queries [(mt % mts) * st, +st).  Keys stream in blocks of kAttnKvBlock through kAttnKvStages
+// stages; a block arrives as kAttnKvBlock / rows TMA loads of `rows` keys (one page, or one block inside a larger page).
+// Split s covers key blocks [s * bps, min((s + 1) * bps, nkb)) of the capacity; nkb = ceil(cap / kAttnKvBlock).
+// Shared memory: 1024 (alignment slack) + DB / 64 chunks x (kAttnKvRows Q rows + 2 * kAttnKvStages * kAttnKvBlock K / V rows)
+// of 128 bytes + kAttnKvBarBytes.
+// Workspace (nsplit > 1, ws != 0): f32 O [nsplit][rows][D], then f32 (m, l) [nsplit][rows][2], rows = B * Hq * Sq in
+// (b, h, i) order.  O is un-normalised, m is the split's row maximum of t = s * scale_log2 (-inf when the split saw no key) and
+// l its row sum of exp2(t - m).  attn_kv_combine_<out> (kAttnKvCombineThreads threads, one per 4 columns of a row) reads it.
+constexpr int kAttnKvBlock = 64;
+constexpr int kAttnKvStages = 4;
+constexpr int kAttnKvRows = 64;
+constexpr int kAttnKvThreads = 160;
+constexpr int kAttnKvBarBytes = 128;
+constexpr int kAttnKvMaxSplits = 128;
+constexpr int kAttnKvSplitCost = 2;   // the split plan's fixed cost of one CTA, in key blocks (prologue and epilogue)
+constexpr int kAttnKvCombineThreads = 256;
+struct AttnKvParams {
+  uint64_t out;               // [B, Hq, Sq, D] view, unit D stride (direct path and combine)
+  uint64_t o_sb, o_sh, o_ss;  // out strides in elements
+  uint64_t lse;               // f32 [B, Hq, Sq] compact, or 0
+  uint64_t ws;                // 0: the attention kernel writes out and lse itself (nsplit == 1); else the workspace above
+  uint64_t table;             // i32 block table, element (b, p) at table + b * t_sb + p * t_sp; 0: page b is sequence b
+  uint64_t t_sb, t_sp;
+  uint64_t seqlens;           // i32 [B] cache lengths, clamped to [0, cap] on read
+  uint32_t B, Hq, Hkv, Sq, D;
+  uint32_t group;             // G = Hq / Hkv
+  uint32_t gt, st, mtg, mts;  // tile: gt heads x st queries; m-tiles mtg * mts
+  uint32_t page, rows;        // keys per page, keys per TMA load
+  uint32_t cap, nkb;          // capacity max_pages * page, its key blocks
+  uint32_t nsplit, bps;       // splits, key blocks per split
+  uint32_t causal;            // 1: query i also needs j <= L - Sq + i (bottom-right)
+  float scale_log2;           // scale * log2(e)
+};
+
+// b200_kvcache_write (attn_kv_write): one thread per 16-byte unit of a (token, kv head) row, for k and v.  Token n = b * Snew + t
+// goes to flat slot slots[n] (page slot / page, row slot % page); a slot < 0 or >= P * page is skipped.  Strides in elements.
+struct AttnKvWriteParams {
+  uint64_t kn, vn, kc, vc, slots;
+  uint64_t kn_sb, kn_st, kn_sh, vn_sb, vn_st, vn_sh;   // new tokens [B, Snew, Hkv, D]
+  uint64_t kc_sp, kc_sr, kc_sh, vc_sp, vc_sr, vc_sh;   // caches [P, page, Hkv, D]
+  uint64_t units;                                      // B * Snew * Hkv * D / 8
+  uint32_t Snew, Hkv, D, page;
+  uint64_t slot_end;                                   // P * page
+};
+
 // ================================================================================================ conv_grouped.cu
 // Direct NHWC grouped convolution (b200_conv2d_grouped*, group width Cg = C / groups < 64).  Group g owns input channels
 // [g Cg, (g+1) Cg) and output channels [g Coutg, (g+1) Coutg).  Every strided operand has a unit channel stride; strides

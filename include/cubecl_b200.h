@@ -586,6 +586,73 @@ int b200_attention_backward(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b
                             b200_dptr dv, const uint64_t* dv_shape, const uint64_t* dv_strides,
                             const b200_attention_args* args);
 
+/* ---- attention against a KV cache (decoding, speculative decoding, chunked prefill; forward only) ------------------------
+ * Sequence b of the batch has L_b = cache_seqlens[b] keys in the cache.  With G = Hq / Hkv and hk = h / G:
+ *   out[b, h, i, :] = sum_{j visible} softmax_j(scale * q[b, h, i, :] . K_b[j, hk, :]) * V_b[j, hk, :]
+ *   lse[b, h, i]    = log sum_{j visible} exp(scale * q[b, h, i, :] . K_b[j, hk, :])                      (natural log, f32)
+ * q and out are [B, Hq, Sq, D] (the Sq new queries of each sequence, usually 1); k_cache and v_cache are [P, page, Hkv, D]:
+ * P pages of `page` keys.  Shapes and strides in elements, so a [P, Hkv, page, D] (head-major) cache is the same call with
+ * permuted strides, and a [B, Sq, Hq, D] q is a stride-permuted view.
+ * Lengths: cache_seqlens is a compact i32 [B] device array, read by the kernels only (the host never reads it, so the call
+ * does not synchronise).  Each value is clamped to [0, max_pages * page].
+ * Visibility: query i of sequence b sees key j iff j < L_b and, when args->causal != 0, j <= L_b - Sq + i (bottom-right
+ * alignment: flash_attn_with_kvcache's rule, torch's causal_lower_right; the new queries are the last Sq keys).  This is the
+ * only difference from b200_attention's args.  A row with no visible key (L_b = 0, or causal with L_b < Sq - i) gets out = +0
+ * and lse = -inf.
+ * Paging: key j of sequence b is row j % page of page block_table[b, j / page], kv head hk.  block_table is an i32 [B, max_pages]
+ * array with any strides (4-byte aligned).  Entries at or past ceil(L_b / page) are never read; an out-of-range page id
+ * reads zeros and cannot fault.  block_table = 0: sequence b is page b (P must equal B, max_pages = 1), the plain contiguous
+ * [B, Smax, Hkv, D] cache.  With one page per sequence (no table, or max_pages == 1) the page may have any size; otherwise
+ * page must be a multiple of 16 that divides 64 (the kernel's key block) or is a multiple of 64.
+ * Stale slots: cache slots at or past L_b may hold anything, NaN and inf included (serving caches reuse freed pages); they
+ * never reach out.  Scores are masked with a select, and the V rows of keys >= L_b are zeroed on chip before the P.V product.
+ * Dtypes and limits: as b200_attention (f16 / bf16 in, out in the input dtype or f32, D <= 128, D % 8 == 0, the caches' head
+ * dim equal to D).  out and both caches need a unit D stride and a 16-byte aligned base and strides, else
+ * B200_ERR_UNSUPPORTED: a cache is read in place through a 4-D tensor map over (D, page, Hkv, P), never gathered (a copy of the
+ * whole cache per step would cost more than the attention).  q is read in place or gathered like b200_attention's inputs.
+ * lse: 0 or a compact f32 [B, Hq, Sq] buffer.
+ * Work: one CTA per (b, hk, m-tile, split).  An m-tile holds gt heads of one kv head's group times st queries (gt * st <= 64),
+ * so each K / V byte is read once per kv head; gt and st minimise the m-tile count ceil(G / gt) * ceil(Sq / st) (ties: the
+ * larger st).  The split count depends on shapes only (B, Hkv, the m-tiles, the capacity max_pages * page and the SM count),
+ * never on the lengths: split s takes an equal range of the capacity's 64-key blocks; a split past L_b writes an empty partial.
+ * Numerics: b200_attention's (f32 scores, base-2 online softmax with t = s * (scale * log2 e), ex2.approx.ftz, P rounded RNE to
+ * the input dtype).  One split: out = O / l rounded once.  Several: each split keeps un-normalised f32 O_s with its maximum
+ * m_s and sum l_s, and the combine forms m = max m_s, w_s = exp2(m_s - m), out = sum_s w_s O_s / sum_s w_s l_s in f32 in split
+ * order, rounded once; lse = (m + log2 l) * ln 2.  No atomics: bitwise reproducible for fixed shapes and SM count, and equal
+ * bits for the same keys in any page layout of equal capacity.
+ * Errors: B200_ERR_INVALID_ARG for a k_cache head dim other than D, a v_cache shape mismatch, Hkv == 0 or Hq % Hkv != 0, a wrong
+ * out shape, an empty cache (P or page 0), a block table that is not [B, >= 1] (or no table with P != B), a non-finite scale,
+ * a null pointer or a misaligned lse / cache_seqlens / block_table; B200_ERR_UNSUPPORTED for the dtypes, D, Dv != D, the page
+ * rule above, caches or out a tensor map cannot read, extents or capacity >= 2^31.  B, Hq or Sq = 0: no launch.
+ * Launches, on `s` with no host synchronisation: the gather of q if needed; one split: one attn_kv_<in>_d<64|128>_<out> launch of
+ * B * Hkv * m-tiles CTAs that writes out and lse.  Several: a pooled f32 workspace of nsplit * B * Hq * Sq * (D + 2) values
+ * ("alloc"), the attn_kv launch of B * Hkv * m-tiles * nsplit CTAs, then attn_kv_combine_<out>.  The dry-run plan records the
+ * maps as "tmap4d" lines in the order q (box (64, st, gt, 1)), k_cache, v_cache (box (64, rows, 1, 1), rows = 64 or the page). */
+int b200_attention_kvcache(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype,
+                           b200_dptr q, const uint64_t* q_shape, const uint64_t* q_strides,
+                           b200_dptr k_cache, const uint64_t* kc_shape, const uint64_t* kc_strides,
+                           b200_dptr v_cache, const uint64_t* vc_shape, const uint64_t* vc_strides,
+                           b200_dptr block_table, const uint64_t* bt_shape, const uint64_t* bt_strides,
+                           b200_dptr cache_seqlens,
+                           b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides,
+                           b200_dptr lse, const b200_attention_args* args);
+
+/* Scatter of new keys and values into a paged KV cache (vLLM's reshape_and_cache).  k_new and v_new are [B, Snew, Hkv, D] views,
+ * k_cache and v_cache [P, page, Hkv, D] as in b200_attention_kvcache; slot_mapping is a compact i32 [B * Snew] device array.
+ * Token t of sequence b goes to flat slot s = slot_mapping[b * Snew + t], that is row s % page of page s / page, for every kv
+ * head.  A negative slot, or one >= P * page, is skipped.  No length is updated on the device: the caller keeps the lengths
+ * (cache_seqlens) itself, as a serving scheduler already does, and uploads them for the attention call.  Two tokens mapped to
+ * one slot leave one of them there, unspecified which.
+ * dtype: B200_F16 or B200_BF16; D % 8 == 0.  The caches need a unit D stride and a 16-byte aligned base and strides (else
+ * B200_ERR_UNSUPPORTED); k_new / v_new views that do not are gathered first.  Errors: B200_ERR_INVALID_ARG for shape
+ * mismatches, a null pointer or a misaligned slot_mapping.  One attn_kv_write launch (16-byte loads and stores) on `s`. */
+int b200_kvcache_write(b200_ctx* ctx, b200_stream s, b200_dtype dtype,
+                       b200_dptr k_new, const uint64_t* kn_shape, const uint64_t* kn_strides,
+                       b200_dptr v_new, const uint64_t* vn_shape, const uint64_t* vn_strides,
+                       b200_dptr k_cache, const uint64_t* kc_shape, const uint64_t* kc_strides,
+                       b200_dptr v_cache, const uint64_t* vc_shape, const uint64_t* vc_strides,
+                       b200_dptr slot_mapping);
+
 /* ---- collectives: ServerCommunication (server/base.rs:632-739), CUDA impl cubecl-cuda/src/compute/server.rs:666-926 -- */
 #define B200_UNIQUE_ID_BYTES 128
 int b200_comm_get_unique_id(b200_ctx* ctx, void* id128);            /* ncclGetUniqueId (communication.rs:11-25 holds it per device set) */

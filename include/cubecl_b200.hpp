@@ -420,6 +420,44 @@ inline void launch_backward(ComputeClient& client, const TensorHandle& q, const 
       dv.handle.ptr(), dv.shape.data(), dv.strides.data(), &args);
   if (rc != B200_OK) client.defer(b200_last_error());
 }
+
+/// Attention against a KV cache: q [B, Hq, Sq, D] against k_cache, v_cache [P, page, Hkv, D] (views by strides); sequence b
+/// sees its first cache_seqlens[b] keys (compact i32 [B] on the device), key j in page block_table[b, j / page] (i32
+/// [B, max_pages]; nullptr: page b); causal is bottom-right.  lse: nullptr or a compact f32 [B, Hq, Sq] tensor.  See
+/// b200_attention_kvcache in cubecl_b200.h.  Errors are deferred to client.sync().
+inline void launch_kvcache(ComputeClient& client, const TensorHandle& q, const TensorHandle& k_cache, const TensorHandle& v_cache,
+                           const TensorHandle& cache_seqlens, const TensorHandle& out, const TensorHandle* block_table, float scale,
+                           bool causal = false, const TensorHandle* lse = nullptr) {
+  if (q.shape.size() != 4 || k_cache.shape.size() != 4 || v_cache.shape.size() != 4 || out.shape.size() != 4 ||
+      (block_table && block_table->shape.size() != 2) || q.dtype != k_cache.dtype || q.dtype != v_cache.dtype) {
+    client.defer("InvalidArgument: attention_kvcache needs rank-4 q, caches and out of one input dtype and a rank-2 block table");
+    return;
+  }
+  const b200_attention_args args{scale, causal ? 1 : 0};
+  const int rc = b200_attention_kvcache(
+      client.raw(), nullptr, static_cast<b200_dtype>(q.dtype), static_cast<b200_dtype>(out.dtype), q.handle.ptr(), q.shape.data(),
+      q.strides.data(), k_cache.handle.ptr(), k_cache.shape.data(), k_cache.strides.data(), v_cache.handle.ptr(), v_cache.shape.data(),
+      v_cache.strides.data(), block_table ? block_table->handle.ptr() : 0, block_table ? block_table->shape.data() : nullptr,
+      block_table ? block_table->strides.data() : nullptr, cache_seqlens.handle.ptr(), out.handle.ptr(), out.shape.data(),
+      out.strides.data(), lse ? lse->handle.ptr() : 0, &args);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+
+/// Scatter of k_new, v_new [B, Snew, Hkv, D] into k_cache, v_cache [P, page, Hkv, D]: token n = b * Snew + t goes to flat slot
+/// slot_mapping[n] (compact i32; negative slots are skipped).  See b200_kvcache_write in cubecl_b200.h.  Errors are deferred to
+/// client.sync().
+inline void kvcache_write(ComputeClient& client, const TensorHandle& k_new, const TensorHandle& v_new, const TensorHandle& k_cache,
+                          const TensorHandle& v_cache, const TensorHandle& slot_mapping) {
+  if (k_new.shape.size() != 4 || v_new.shape.size() != 4 || k_cache.shape.size() != 4 || v_cache.shape.size() != 4) {
+    client.defer("InvalidArgument: kvcache_write needs rank-4 new tokens and caches");
+    return;
+  }
+  const int rc = b200_kvcache_write(client.raw(), nullptr, static_cast<b200_dtype>(k_cache.dtype), k_new.handle.ptr(), k_new.shape.data(),
+                                    k_new.strides.data(), v_new.handle.ptr(), v_new.shape.data(), v_new.strides.data(), k_cache.handle.ptr(),
+                                    k_cache.shape.data(), k_cache.strides.data(), v_cache.handle.ptr(), v_cache.shape.data(),
+                                    v_cache.strides.data(), slot_mapping.handle.ptr());
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
 }  // namespace attention
 
 namespace reduce {

@@ -575,6 +575,54 @@ impl Context {
         ))
     }
 
+    /// Attention of q [B, Hq, Sq, D] against a KV cache `k_cache`, `v_cache` [P, page, Hkv, D] (views by strides): sequence b
+    /// sees its first `cache_seqlens`[b] keys (a compact i32 [B] device buffer), key j in page `block_table`[b, j / page] (an
+    /// i32 [B, max_pages] view; `None`: page b); `causal` is bottom-right.  See b200_attention_kvcache in cubecl_b200.h.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::conv2d`]; `cache_seqlens` must hold B i32 values and `lse`, when non-zero, B * Hq * Sq f32
+    /// values.
+    pub unsafe fn attention_kvcache(
+        &mut self, stream: b200_stream, in_dtype: DType, out_dtype: DType, q: &TensorView, k_cache: &TensorView, v_cache: &TensorView,
+        block_table: Option<&TensorView>, cache_seqlens: b200_dptr, out: &TensorView, lse: b200_dptr, scale: f32, causal: bool,
+    ) -> Result<(), Error> {
+        for t in [q, k_cache, v_cache, out] {
+            assert!(t.shape.len() == 4 && t.strides.len() == 4);
+        }
+        if let Some(t) = block_table {
+            assert!(t.shape.len() == 2 && t.strides.len() == 2);
+        }
+        let a = sys::b200_attention_args { scale, causal: causal as i32 };
+        let (bt, bt_shape, bt_strides) = match block_table {
+            Some(t) => (t.ptr, t.shape.as_ptr(), t.strides.as_ptr()),
+            None => (0, std::ptr::null(), std::ptr::null()),
+        };
+        check(sys::b200_attention_kvcache(
+            self.0, stream, in_dtype as c_int, out_dtype as c_int, q.ptr, q.shape.as_ptr(), q.strides.as_ptr(), k_cache.ptr,
+            k_cache.shape.as_ptr(), k_cache.strides.as_ptr(), v_cache.ptr, v_cache.shape.as_ptr(), v_cache.strides.as_ptr(), bt,
+            bt_shape, bt_strides, cache_seqlens, out.ptr, out.shape.as_ptr(), out.strides.as_ptr(), lse, &a,
+        ))
+    }
+
+    /// Scatter of `k_new`, `v_new` [B, Snew, Hkv, D] into `k_cache`, `v_cache` [P, page, Hkv, D]: token b * Snew + t goes to flat
+    /// slot `slot_mapping`[b * Snew + t] (a compact i32 device buffer; negative slots are skipped).  See b200_kvcache_write.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::conv2d`]; `slot_mapping` must hold B * Snew i32 values.
+    pub unsafe fn kvcache_write(
+        &mut self, stream: b200_stream, dtype: DType, k_new: &TensorView, v_new: &TensorView, k_cache: &TensorView, v_cache: &TensorView,
+        slot_mapping: b200_dptr,
+    ) -> Result<(), Error> {
+        for t in [k_new, v_new, k_cache, v_cache] {
+            assert!(t.shape.len() == 4 && t.strides.len() == 4);
+        }
+        check(sys::b200_kvcache_write(
+            self.0, stream, dtype as c_int, k_new.ptr, k_new.shape.as_ptr(), k_new.strides.as_ptr(), v_new.ptr, v_new.shape.as_ptr(),
+            v_new.strides.as_ptr(), k_cache.ptr, k_cache.shape.as_ptr(), k_cache.strides.as_ptr(), v_cache.ptr, v_cache.shape.as_ptr(),
+            v_cache.strides.as_ptr(), slot_mapping,
+        ))
+    }
+
     /// Grouped / depthwise [`Context::conv2d`]: w [Cout, KH, KW, C / groups].  See b200_conv2d_grouped in cubecl_b200.h.
     ///
     /// # Safety
