@@ -59,6 +59,13 @@ class AttentionArgs(C.Structure):
     _fields_ = [("scale", C.c_float), ("causal", C.c_int32)]
 
 
+class AttentionVarlenArgs(C.Structure):
+    """b200_attention_varlen_args: the score scale, the window (-1: unbounded on that side; (-1, 0) is bottom-right causal)
+    and the host bounds on the sequence lengths."""
+    _fields_ = [("scale", C.c_float), ("window_left", C.c_int32), ("window_right", C.c_int32), ("max_seqlen_q", C.c_int32),
+                ("max_seqlen_k", C.c_int32)]
+
+
 class QuantScheme(C.Structure):
     """b200_quant_scheme: value (b200_quant_value), block, block_scale (b200_dtype), tensor_scale (0 / 1)."""
     _fields_ = [("value", C.c_int32), ("block", C.c_int32), ("block_scale", C.c_int32), ("tensor_scale", C.c_int32)]
@@ -149,6 +156,10 @@ SIGNATURES = {
                                  _u64p, C.c_uint64, _u64p, _u64p, C.c_uint64, C.POINTER(AttentionArgs)]),
     "b200_attention_backward": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int] + [C.c_uint64, _u64p, _u64p] * 5 + [C.c_uint64]
                                 + [C.c_uint64, _u64p, _u64p] * 3 + [C.POINTER(AttentionArgs)]),
+    "b200_attention_varlen": (C.c_int, [_vp, _vp, C.c_int, C.c_int] + [C.c_uint64, _u64p, _u64p] * 3 + [C.c_uint64] * 3
+                              + [C.c_uint64, _u64p, _u64p] + [C.c_uint64, C.POINTER(AttentionVarlenArgs)]),
+    "b200_attention_varlen_backward": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int] + [C.c_uint64, _u64p, _u64p] * 5
+                                       + [C.c_uint64] * 4 + [C.c_uint64, _u64p, _u64p] * 3 + [C.POINTER(AttentionVarlenArgs)]),
     "b200_attention_kvcache": (C.c_int, [_vp, _vp, C.c_int, C.c_int] + [C.c_uint64, _u64p, _u64p] * 4 + [C.c_uint64]
                                + [C.c_uint64, _u64p, _u64p] + [C.c_uint64, C.POINTER(AttentionArgs)]),
     "b200_kvcache_write": (C.c_int, [_vp, _vp, C.c_int] + [C.c_uint64, _u64p, _u64p] * 4 + [C.c_uint64]),

@@ -19,6 +19,13 @@ sequence b in a paged cache k_cache, v_cache [P, page, Hkv, D] reached through a
 is sequence b).  causal is bottom-right there: query i also needs j <= L_b - Sq + i.  kvcache_write scatters new tokens
 [B, Snew, Hkv, D] into cache slots (slot_mapping, i32 [B * Snew]; negative slots are skipped).  One split-KV kernel with a
 fixed-order combine (csrc/attention_kv.cu); see b200_attention_kvcache and b200_kvcache_write.
+
+Variable-length (packed) sequences (launch_varlen, torch's varlen_attn / flash_attn_varlen_func): q [Tq, Hq, D] and k, v
+[Tk, Hkv, D] hold B sequences back to back; sequence b owns rows [cu_seqlens_q[b], cu_seqlens_q[b + 1]) of q and the matching
+rows of k and v (compact i32 [B + 1] device arrays, never read by the host).  window_size = (left, right) as torch's: key j is
+visible to query i iff j < Lk and i + off - left <= j <= i + off + right with off = Lk - Lq (-1: unbounded), so (-1, 0) is
+bottom-right causal.  lse is a compact f32 [Hq, Tq].  The dense kernels with per-sequence addressing (-DATTN_VARLEN builds of
+csrc/attention.cu and attention_bwd.cu); see b200_attention_varlen and b200_attention_varlen_backward.
 """
 from __future__ import annotations
 
@@ -204,3 +211,96 @@ def kvcache_write(client: ComputeClient, k_new: TensorHandle, v_new: TensorHandl
                                                   C.c_uint64(slot_mapping.handle.ptr)))
     except (B200Error, ValueError) as e:
         client._defer(e if isinstance(e, B200Error) else B200Error(6, str(e)))
+
+
+def _varlen_args(q, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, scale, window_size, what):
+    if not (cu_seqlens_q.dtype == cu_seqlens_k.dtype == "i32") or not cu_seqlens_q.is_contiguous() or not cu_seqlens_k.is_contiguous() \
+            or len(cu_seqlens_q.shape) != 1 or list(cu_seqlens_k.shape) != list(cu_seqlens_q.shape) or cu_seqlens_q.shape[0] < 1:
+        raise B200Error(6, f"{what}: cu_seqlens_q and cu_seqlens_k must be compact i32 [B + 1] tensors of one length")
+    left, right = (int(w) for w in window_size)
+    sc = 1.0 / math.sqrt(q.shape[2]) if scale is None else float(scale)
+    return _ffi.AttentionVarlenArgs(sc, left, right, int(max_seqlen_q), int(max_seqlen_k)), cu_seqlens_q.shape[0] - 1
+
+
+def launch_varlen(client: ComputeClient, q: TensorHandle, k: TensorHandle, v: TensorHandle, cu_seqlens_q: TensorHandle,
+                  cu_seqlens_k: TensorHandle, max_seqlen_q: int, max_seqlen_k: int, out: TensorHandle, scale: float | None = None,
+                  window_size=(-1, -1), lse: TensorHandle | None = None, stream=None) -> None:
+    """Enqueue attention over packed sequences: q [Tq, Hq, D], k and v [Tk, Hkv, D], out [Tq, Hq, D] (views by strides);
+    cu_seqlens_q / cu_seqlens_k compact i32 [B + 1] offsets, max_seqlen_q / max_seqlen_k host bounds on the lengths.
+    window_size (left, right), -1 unbounded: (-1, 0) is bottom-right causal.  scale defaults to 1 / sqrt(D); lse: an optional
+    compact f32 [Hq, Tq] tensor.  Rows outside every sequence are not written.  Never raises for launch problems: errors are
+    deferred to client.sync()."""
+    try:
+        for name, t in (("q", q), ("k", k), ("v", v), ("out", out)):
+            if len(t.shape) != 3:
+                raise B200Error(6, f"attention_varlen: {name} must have rank 3 [T, H, D], got rank {len(t.shape)}")
+        if not (q.dtype == k.dtype == v.dtype):
+            raise B200Error(6, f"attention_varlen: q, k and v dtypes differ ({q.dtype}, {k.dtype}, {v.dtype})")
+        if lse is not None and (lse.dtype != "f32" or not lse.is_contiguous() or list(lse.shape) != [q.shape[1], q.shape[0]]):
+            raise B200Error(6, f"attention_varlen: lse must be a compact f32 [Hq, Tq] = {[q.shape[1], q.shape[0]]} tensor")
+        args, B = _varlen_args(q, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, scale, window_size, "attention_varlen")
+        for t in (q, k, v, cu_seqlens_q, cu_seqlens_k, out) + ((lse,) if lse is not None else ()):
+            t.handle.used_on(stream)
+        _ffi.check(client._lib.b200_attention_varlen(
+            client._ctx, stream, DTYPES[q.dtype], DTYPES[out.dtype], *_view_args((q, k, v)), C.c_uint64(cu_seqlens_q.handle.ptr),
+            C.c_uint64(cu_seqlens_k.handle.ptr), C.c_uint64(B), *_view_args((out,)),
+            C.c_uint64(lse.handle.ptr if lse is not None else 0), C.byref(args)))
+    except (B200Error, ValueError) as e:
+        client._defer(e if isinstance(e, B200Error) else B200Error(6, str(e)))
+
+
+def launch_varlen_alloc(client: ComputeClient, q: TensorHandle, k: TensorHandle, v: TensorHandle, cu_seqlens_q: TensorHandle,
+                        cu_seqlens_k: TensorHandle, max_seqlen_q: int, max_seqlen_k: int, scale: float | None = None,
+                        window_size=(-1, -1), out_dtype: str | None = None, return_lse: bool = False, stream=None):
+    """Convenience: allocate a compact out [Tq, Hq, D] (and, with return_lse, a compact f32 lse [Hq, Tq]), then launch_varlen.
+    Rows outside every sequence are left as allocated.  Returns out, or (out, lse)."""
+    out = TensorHandle.empty_contiguous(client, list(q.shape), out_dtype or q.dtype)
+    lse = TensorHandle.empty_contiguous(client, [q.shape[1], q.shape[0]], "f32") if return_lse else None
+    launch_varlen(client, q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, out, scale=scale, window_size=window_size,
+                  lse=lse, stream=stream)
+    return (out, lse) if return_lse else out
+
+
+def launch_varlen_backward(client: ComputeClient, q: TensorHandle, k: TensorHandle, v: TensorHandle, out: TensorHandle,
+                           dout: TensorHandle, lse: TensorHandle, cu_seqlens_q: TensorHandle, cu_seqlens_k: TensorHandle,
+                           max_seqlen_q: int, max_seqlen_k: int, dq: TensorHandle, dk: TensorHandle, dv: TensorHandle,
+                           scale: float | None = None, window_size=(-1, -1), stream=None) -> None:
+    """Enqueue the varlen backward: dq [Tq, Hq, D], dk and dv [Tk, Hkv, D] (one grad dtype: the input dtype or f32) from q, k, v,
+    the forward's out and lse (compact f32 [Hq, Tq]) and dout.  Offsets, scale and window_size must be the forward's.  Rows
+    outside every sequence are not written.  Never raises for launch problems: errors are deferred to client.sync()."""
+    try:
+        named = (("q", q), ("k", k), ("v", v), ("out", out), ("dout", dout), ("dq", dq), ("dk", dk), ("dv", dv))
+        for name, t in named:
+            if len(t.shape) != 3:
+                raise B200Error(6, f"attention_varlen_backward: {name} must have rank 3 [T, H, D], got rank {len(t.shape)}")
+        if not (q.dtype == k.dtype == v.dtype == dout.dtype):
+            raise B200Error(6, f"attention_varlen_backward: q, k, v and dout dtypes differ ({q.dtype}, {k.dtype}, {v.dtype}, {dout.dtype})")
+        if not (dq.dtype == dk.dtype == dv.dtype):
+            raise B200Error(6, f"attention_varlen_backward: dq, dk and dv dtypes differ ({dq.dtype}, {dk.dtype}, {dv.dtype})")
+        if lse.dtype != "f32" or not lse.is_contiguous() or list(lse.shape) != [q.shape[1], q.shape[0]]:
+            raise B200Error(6, f"attention_varlen_backward: lse must be a compact f32 [Hq, Tq] = {[q.shape[1], q.shape[0]]} tensor")
+        args, B = _varlen_args(q, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, scale, window_size,
+                               "attention_varlen_backward")
+        for _, t in named + (("lse", lse), ("cu_seqlens_q", cu_seqlens_q), ("cu_seqlens_k", cu_seqlens_k)):
+            t.handle.used_on(stream)
+        _ffi.check(client._lib.b200_attention_varlen_backward(
+            client._ctx, stream, DTYPES[q.dtype], DTYPES[out.dtype], DTYPES[dq.dtype], *_view_args((q, k, v, out, dout)),
+            C.c_uint64(lse.handle.ptr), C.c_uint64(cu_seqlens_q.handle.ptr), C.c_uint64(cu_seqlens_k.handle.ptr), C.c_uint64(B),
+            *_view_args((dq, dk, dv)), C.byref(args)))
+    except (B200Error, ValueError) as e:
+        client._defer(e if isinstance(e, B200Error) else B200Error(6, str(e)))
+
+
+def launch_varlen_backward_alloc(client: ComputeClient, q: TensorHandle, k: TensorHandle, v: TensorHandle, out: TensorHandle,
+                                 dout: TensorHandle, lse: TensorHandle, cu_seqlens_q: TensorHandle, cu_seqlens_k: TensorHandle,
+                                 max_seqlen_q: int, max_seqlen_k: int, scale: float | None = None, window_size=(-1, -1),
+                                 grad_dtype: str | None = None, stream=None):
+    """Convenience: allocate compact dq [Tq, Hq, D] and dk, dv [Tk, Hkv, D] in grad_dtype (default: q's dtype), then
+    launch_varlen_backward.  Returns (dq, dk, dv)."""
+    gd = grad_dtype or q.dtype
+    dq = TensorHandle.empty_contiguous(client, list(q.shape), gd)
+    dk = TensorHandle.empty_contiguous(client, list(k.shape), gd)
+    dv = TensorHandle.empty_contiguous(client, list(k.shape), gd)
+    launch_varlen_backward(client, q, k, v, out, dout, lse, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, dq, dk, dv,
+                           scale=scale, window_size=window_size, stream=stream)
+    return dq, dk, dv

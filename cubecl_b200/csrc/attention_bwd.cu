@@ -103,13 +103,76 @@ __device__ __forceinline__ void delta_body(const AttnBwdParams& p) {
   }
 }
 
+// the first workspace row of varlen sequence b (kernel_params.h: AttnVarlenParams)
+__device__ __forceinline__ uint64_t varlen_ws_start(int qs, uint32_t b) {
+  return (static_cast<uint64_t>(qs) + static_cast<uint64_t>(kAttnBlock) * b) / kAttnBlock * kAttnBlock;
+}
+
+// varlen: blocks of 16 rows over (b, h, row group), nqb * 8 groups per (b, h); rows past the sequence's padded blocks leave
+// at once, padded rows get L = +inf and delta = 0, and so do rows whose lse is -inf (no visible key: exp2(t - L) would be +inf)
+template <int KIND, int OUT>
+__device__ __forceinline__ void delta_varlen_body(const AttnVarlenParams& p) {
+  const uint32_t groups = p.nqb * (kAttnBlock / 16u);
+  const uint32_t bh = blockIdx.x / groups, b = bh / p.Hq, h = bh - b * p.Hq;
+  const int i = static_cast<int>((blockIdx.x - bh * groups) * 16u + (threadIdx.x >> 4));
+  const uint32_t c = threadIdx.x & 15u;
+  const unsigned mask = 0xFFFFu << (threadIdx.x & 16u);
+  int qs, Lq;
+  varlen_seq(p.cu_q, b, p.Tq, p.max_q, qs, Lq);
+  if (i >= (Lq + kAttnBlock - 1) / kAttnBlock * kAttnBlock) return;   // whole half warps leave
+  const uint64_t start = varlen_ws_start(qs, b);
+  float* L = reinterpret_cast<float*>(p.ws) + static_cast<uint64_t>(h) * p.Tqp + start + i;
+  float* dl = L + static_cast<uint64_t>(p.Hq) * p.Tqp;
+  if (i >= Lq) {
+    if (c == 0) { *L = INFINITY; *dl = 0.f; }
+    return;
+  }
+  const uint64_t tok = static_cast<uint64_t>(qs) + i;
+  float acc = 0.f;
+  if (c * 8u < p.D) {
+    const uint4 dv = *reinterpret_cast<const uint4*>(p.dout + 2u * (tok * p.d_st + h * p.d_sh + c * 8u));
+    const uint32_t dw[4] = {dv.x, dv.y, dv.z, dv.w};
+    float o[8];
+    const uint64_t oe = tok * p.o_st + h * p.o_sh + c * 8u;
+    if constexpr (OUT == OUT_F32) {
+      const float4 a = *reinterpret_cast<const float4*>(p.out + 4u * oe), z = *reinterpret_cast<const float4*>(p.out + 4u * oe + 16u);
+      o[0] = a.x; o[1] = a.y; o[2] = a.z; o[3] = a.w; o[4] = z.x; o[5] = z.y; o[6] = z.z; o[7] = z.w;
+    } else {
+      const uint4 ov = *reinterpret_cast<const uint4*>(p.out + 2u * oe);
+      const uint32_t ow[4] = {ov.x, ov.y, ov.z, ov.w};
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float2 f = unpack16<KIND>(ow[e]);
+        o[2 * e] = f.x;
+        o[2 * e + 1] = f.y;
+      }
+    }
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const float2 f = unpack16<KIND>(dw[e]);
+      acc = fmaf(f.x, o[2 * e], acc);
+      acc = fmaf(f.y, o[2 * e + 1], acc);
+    }
+  }
+#pragma unroll
+  for (int off = 8; off > 0; off >>= 1) acc += __shfl_xor_sync(mask, acc, off);
+  if (c == 0) {
+    const float lse = reinterpret_cast<const float*>(p.lse)[static_cast<uint64_t>(h) * p.Tq + tok];
+    *dl = lse == -INFINITY ? 0.f : acc;
+    *L = lse == -INFINITY ? INFINITY : lse * kLog2e;
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ shared epilogue
 // acc (one consumer's m64 x DB f32 fragment) times mul, rounded to the grad dtype, staged in the consumer's 64 rows of a
 // SWIZZLE_128B tile (chunks of `chunk` bytes, the consumer's rows `rows_off` bytes in) and stored through 4-D TMA stores
 // that the unit clips at the tensor's S and D.  The staging rows are read by no other warpgroup.
-template <int DB, int OUT>
+// VL with rows_left < 64 (a varlen block the sequence ends inside; a TMA box would write the next sequence's rows): the
+// staged rows < rows_left are copied out with 16-byte stores to gbase + row * gst (bytes) instead.
+template <int DB, int OUT, bool VL = false>
 __device__ __forceinline__ void store_rows(const float (&acc)[DB / 2], float mul, uint32_t tile, uint32_t chunk, uint32_t rows_off,
-                                           const CUtensorMap* tm, int row0, uint32_t rows, int h, int b, uint32_t D, uint32_t cw) {
+                                           const CUtensorMap* tm, int row0, uint32_t rows, int h, int b, uint32_t D, uint32_t cw,
+                                           int rows_left = 64, uint64_t gbase = 0, uint64_t gst = 0) {
   constexpr int NCH = DB / 64;
   constexpr uint32_t OSZ = (OUT == OUT_F32) ? 4u : 2u;
   constexpr int CW = 128 / OSZ;        // output columns per 128-byte staging row
@@ -141,6 +204,20 @@ __device__ __forceinline__ void store_rows(const float (&acc)[DB / 2], float mul
     }
     fence_proxy_async_smem();   // generic-proxy writes -> visible to the TMA unit
     asm volatile("bar.sync %0, 128;" ::"r"(1u + cw) : "memory");
+    if constexpr (VL) {
+      if (rows_left < 64) {
+        for (int u = static_cast<int>(t); u < rows_left * 8; u += 128) {
+          const uint32_t rr = static_cast<uint32_t>(u) >> 3, k = static_cast<uint32_t>(u) & 7u;
+          const uint32_t cc = c * CW + k * (16u / OSZ);
+          if (cc >= D) continue;
+          uint4 x;
+          asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(x.x), "=r"(x.y), "=r"(x.z), "=r"(x.w)
+                       : "r"(buf + rr * 128u + ((k ^ (rr & 7u)) << 4)));
+          *reinterpret_cast<uint4*>(gbase + rr * gst + cc * OSZ) = x;
+        }
+        continue;
+      }
+    }
     if (t == 0 && row0 < static_cast<int>(rows) && c * CW < static_cast<int>(D)) {
       tma_store_4d(tm, buf, c * CW, row0, h, b);
       tma_store_commit();
@@ -149,9 +226,10 @@ __device__ __forceinline__ void store_rows(const float (&acc)[DB / 2], float mul
 }
 
 // ------------------------------------------------------------------------------------------------ dq
-template <int KIND, int DB, int OUT>
+// VL: the varlen kernels (P = AttnVarlenParams); the dense kernels have VL = false and P = AttnBwdParams
+template <int KIND, int DB, int OUT, bool VL, class P>
 __device__ __forceinline__ void dq_body(const CUtensorMap* tq, const CUtensorMap* tk, const CUtensorMap* tv, const CUtensorMap* tdo,
-                                        const CUtensorMap* tdq, const AttnBwdParams& p) {
+                                        const CUtensorMap* tdq, const P& p) {
   constexpr int NCH = DB / 64;
   constexpr int KB = kAttnBwdDqKeys;
   static_assert(KB == 64 && kAttnBlock == 128, "two consumers of 64 query rows, 64-key blocks");
@@ -177,9 +255,28 @@ __device__ __forceinline__ void dq_body(const CUtensorMap* tq, const CUtensorMap
   const uint32_t qb = p.nqb - 1u - blockIdx.x / per;
   const uint32_t rem = blockIdx.x % per;
   const uint32_t b = rem / p.Hq, h = rem - b * p.Hq, hk = h / p.group;
-  const uint32_t nkb_all = (p.Sk + KB - 1) / KB;
-  const uint32_t nkb = p.causal ? min(nkb_all, 2u * qb + 2u) : nkb_all;
   const int q0 = static_cast<int>(qb * kAttnBlock);
+  // key blocks [kb_lo, nkb); rows and keys are addressed at (qrow, krow) + block offsets in head h / hk of batch bb
+  uint32_t kb_lo = 0, nkb, nkb_all = 0;
+  int qrow = q0, krow = 0, bb = static_cast<int>(b), qs = 0;
+  int Lq = 0, Lk = 0, off = 0;   // varlen: the sequence's lengths, off = Lk - Lq
+  if constexpr (VL) {
+    int ks;
+    varlen_seq(p.cu_q, b, p.Tq, p.max_q, qs, Lq);
+    varlen_seq(p.cu_k, b, p.Tk, p.max_k, ks, Lk);
+    if (q0 >= Lq) return;   // past the sequence: no load, no store
+    off = Lk - Lq;
+    int lo, hi;
+    band_blocks(q0, min(q0 + kAttnBlock, Lq) - 1, off, p.left, p.right, Lk, KB, lo, hi);
+    kb_lo = static_cast<uint32_t>(lo);
+    nkb = static_cast<uint32_t>(hi);
+    qrow = qs + q0;
+    krow = ks;
+    bb = 0;
+  } else {
+    nkb_all = (p.Sk + KB - 1) / KB;
+    nkb = p.causal ? min(nkb_all, 2u * qb + 2u) : nkb_all;
+  }
 
   const uint32_t wg = threadIdx.x >> 7;
   if (threadIdx.x == 0) {
@@ -205,19 +302,19 @@ __device__ __forceinline__ void dq_body(const CUtensorMap* tq, const CUtensorMap
       mbar_arrive_expect_tx(q_bar, 2u * QTILE);
 #pragma unroll
       for (int c = 0; c < NCH; ++c) {
-        tma_load_4d(sq + c * QCHUNK, tq, q_bar, c * 64, q0, static_cast<int>(h), static_cast<int>(b));
-        tma_load_4d(sdo + c * QCHUNK, tdo, q_bar, c * 64, q0, static_cast<int>(h), static_cast<int>(b));
+        tma_load_4d(sq + c * QCHUNK, tq, q_bar, c * 64, qrow, static_cast<int>(h), bb);
+        tma_load_4d(sdo + c * QCHUNK, tdo, q_bar, c * 64, qrow, static_cast<int>(h), bb);
       }
       uint32_t s = 0, ph = 0;
-      for (uint32_t kb = 0; kb < nkb; ++kb) {
+      for (uint32_t kb = kb_lo; kb < nkb; ++kb) {
         mbar_wait(empty(s), ph ^ 1u);
-        const int k0 = static_cast<int>(kb * KB);
+        const int k0 = krow + static_cast<int>(kb * KB);
         mbar_arrive_expect_tx(full_k(s), KTILE);
 #pragma unroll
-        for (int c = 0; c < NCH; ++c) tma_load_4d(sk(s) + c * KCHUNK, tk, full_k(s), c * 64, k0, static_cast<int>(hk), static_cast<int>(b));
+        for (int c = 0; c < NCH; ++c) tma_load_4d(sk(s) + c * KCHUNK, tk, full_k(s), c * 64, k0, static_cast<int>(hk), bb);
         mbar_arrive_expect_tx(full_v(s), KTILE);
 #pragma unroll
-        for (int c = 0; c < NCH; ++c) tma_load_4d(sv(s) + c * KCHUNK, tv, full_v(s), c * 64, k0, static_cast<int>(hk), static_cast<int>(b));
+        for (int c = 0; c < NCH; ++c) tma_load_4d(sv(s) + c * KCHUNK, tv, full_v(s), c * 64, k0, static_cast<int>(hk), bb);
         if (++s == ST) { s = 0; ph ^= 1u; }
       }
     }
@@ -233,10 +330,24 @@ __device__ __forceinline__ void dq_body(const CUtensorMap* tq, const CUtensorMap
   const uint32_t i0 = qb * kAttnBlock + cw * 64u + r, i1 = i0 + 8u;
   const uint32_t col = 2u * (lane & 3u);
   const float c2 = p.scale_log2;
-  // a causal consumer stops at its own diagonal block: keys < q0 + 64 (cw + 1)
-  const uint32_t nkb_c = p.causal ? min(nkb_all, 2u * qb + cw + 1u) : nkb_all;
+  // a causal consumer stops at its own diagonal block: keys < q0 + 64 (cw + 1).  varlen: the consumer's rows reach key
+  // blocks [kbc_lo, kbc_hi); blocks inside keys [lo of its last row, hi of its first] need no mask
+  uint32_t nkb_c = 0;
+  int kbc_lo = 0, kbc_hi = 0, lo_c = 0, hi_c = 0;
+  uint64_t plane, rb;
+  if constexpr (VL) {
+    const int c0 = q0 + static_cast<int>(cw * 64u);
+    if (c0 < Lq) band_blocks(c0, min(c0 + 64, Lq) - 1, off, p.left, p.right, Lk, KB, kbc_lo, kbc_hi);
+    lo_c = band_lo(c0 + 63, off, p.left, Lk);
+    hi_c = band_hi(c0, off, p.right, Lk);
+    plane = static_cast<uint64_t>(p.Hq) * p.Tqp;
+    rb = static_cast<uint64_t>(h) * p.Tqp + varlen_ws_start(qs, b);
+  } else {
+    nkb_c = p.causal ? min(nkb_all, 2u * qb + cw + 1u) : nkb_all;
+    plane = static_cast<uint64_t>(p.B) * p.Hq * p.Sqp;
+    rb = (static_cast<uint64_t>(b) * p.Hq + h) * p.Sqp;
+  }
   const float* ws = reinterpret_cast<const float*>(p.ws);
-  const uint64_t plane = static_cast<uint64_t>(p.B) * p.Hq * p.Sqp, rb = (static_cast<uint64_t>(b) * p.Hq + h) * p.Sqp;
   const float L0 = ws[rb + i0], L1 = ws[rb + i1];
   const float dl0 = ws[plane + rb + i0], dl1 = ws[plane + rb + i1];
 
@@ -246,8 +357,11 @@ __device__ __forceinline__ void dq_body(const CUtensorMap* tq, const CUtensorMap
 
   mbar_wait(q_bar, 0);
   uint32_t s = 0, ph = 0;
-  for (uint32_t kb = 0; kb < nkb; ++kb) {
-    if (kb >= nkb_c) {   // past this consumer's diagonal: release the stage once it has landed
+  for (uint32_t kb = kb_lo; kb < nkb; ++kb) {
+    bool skip;
+    if constexpr (VL) skip = static_cast<int>(kb) < kbc_lo || static_cast<int>(kb) >= kbc_hi;
+    else skip = kb >= nkb_c;
+    if (skip) {   // past this consumer's diagonal (varlen: outside its rows' band): release the stage once it has landed
       mbar_wait(full_k(s), ph);
       mbar_wait(full_v(s), ph);
       if (t == 0) mbar_arrive(empty(s));
@@ -280,9 +394,21 @@ __device__ __forceinline__ void dq_body(const CUtensorMap* tq, const CUtensorMap
     wgmma_fence_operands(sc);
     wgmma_fence_operands(dp);
 
-    // ---- p = exp2(t - L) (masked on the consumer's last block), dS = p (dP - delta), both to 16 bits in the A layout
-    const bool last = kb + 1u == nkb_c;
+    // ---- p = exp2(t - L) (masked on the consumer's last block; varlen: on every block the band or Lk cuts, with dS a select
+    // too, since dP of keys past Lk reads the next sequence's V), dS = p (dP - delta), both to 16 bits in the A layout
+    bool last;
+    if constexpr (VL) last = static_cast<int>(kb * KB) < lo_c || static_cast<int>(kb * KB) + KB - 1 > hi_c;
+    else last = kb + 1u == nkb_c;
     const uint32_t key0 = kb * KB + col;
+    int lo0 = 0, hi0 = 0, lo1 = 0, hi1 = 0;   // varlen: this thread's rows see keys [lo, hi]
+    if constexpr (VL) {
+      if (last) {
+        lo0 = band_lo(static_cast<int>(i0), off, p.left, Lk);
+        hi0 = band_hi(static_cast<int>(i0), off, p.right, Lk);
+        lo1 = band_lo(static_cast<int>(i1), off, p.left, Lk);
+        hi1 = band_hi(static_cast<int>(i1), off, p.right, Lk);
+      }
+    }
     uint32_t ds[NS / 2];
 #pragma unroll
     for (int j = 0; j < KB / 8; ++j) {
@@ -290,18 +416,29 @@ __device__ __forceinline__ void dq_body(const CUtensorMap* tq, const CUtensorMap
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         float pv = ex2(__fmul_rn(sc[4 * j + e], c2) - (e < 2 ? L0 : L1));
-        if (last) {
-          const uint32_t key = key0 + 8u * j + (e & 1);
-          const uint32_t row = (e < 2) ? i0 : i1;
-          if (key >= p.Sk || (p.causal && key > row)) pv = 0.f;
+        if constexpr (VL) {
+          const int kk = static_cast<int>(key0 + 8u * j + (e & 1));
+          const bool hide = last && ((e < 2) ? (kk < lo0 || kk > hi0) : (kk < lo1 || kk > hi1));
+          if (hide) pv = 0.f;
+          v[e] = hide ? 0.f : pv * (dp[4 * j + e] - (e < 2 ? dl0 : dl1));
+        } else {
+          if (last) {
+            const uint32_t key = key0 + 8u * j + (e & 1);
+            const uint32_t row = (e < 2) ? i0 : i1;
+            if (key >= p.Sk || (p.causal && key > row)) pv = 0.f;
+          }
+          v[e] = pv * (dp[4 * j + e] - (e < 2 ? dl0 : dl1));
         }
-        v[e] = pv * (dp[4 * j + e] - (e < 2 ? dl0 : dl1));
       }
       ds[2 * j] = pack16<KIND>(v[0], v[1]);
       ds[2 * j + 1] = pack16<KIND>(v[2], v[3]);
     }
 
     // ---- dQ += dS K: K [keys, D] is an MN-major B operand, 16 keys (2048 bytes of rows) per instruction
+    if constexpr (VL) {   // K rows past Lk are the next sequence's (0 * NaN = NaN in the product): zero them
+      const int valid = Lk - static_cast<int>(kb * KB);
+      if (valid < KB) zero_rows(sk(s), NCH, KCHUNK, valid, KB, 1u + cw);
+    }
     wgmma_fence_operands(dq);
     wgmma_fence();
 #pragma unroll
@@ -318,15 +455,28 @@ __device__ __forceinline__ void dq_body(const CUtensorMap* tq, const CUtensorMap
   }
 
   // ---- epilogue: scale * dQ through the consumer's rows of the Q tile
-  store_rows<DB, OUT>(dq, p.scale, sq, QCHUNK, cw * 64u * 128u, tdq, q0 + static_cast<int>(cw * 64u), p.Sq, static_cast<int>(h),
-                      static_cast<int>(b), p.D, cw);
+  if constexpr (VL) {
+    const int row0 = q0 + static_cast<int>(cw * 64u);
+    constexpr uint32_t GSZ = OUT == OUT_F32 ? 4u : 2u;
+    // rows past Lq belong to the next sequence: a block the sequence ends inside is copied out row by row (none when the
+    // consumer's rows all lie past Lq)
+    store_rows<DB, OUT, true>(dq, p.scale, sq, QCHUNK, cw * 64u * 128u, tdq, qrow + static_cast<int>(cw * 64u), p.Tq, static_cast<int>(h),
+                              0, p.D, cw, min(Lq - row0, 64), p.dq + GSZ * ((qrow + cw * 64u) * p.dq_st + h * p.dq_sh), GSZ * p.dq_st);
+  } else {
+    store_rows<DB, OUT>(dq, p.scale, sq, QCHUNK, cw * 64u * 128u, tdq, q0 + static_cast<int>(cw * 64u), p.Sq, static_cast<int>(h),
+                        static_cast<int>(b), p.D, cw);
+  }
   if (t == 0) tma_store_wait<0>();   // outstanding stores read this CTA's shared memory: finish before exit
 }
 
 // ------------------------------------------------------------------------------------------------ dk, dv
-template <int KIND, int DB, int OUT>
+// the dk / dv kernel's block order: key-block major when causal (varlen: never)
+[[maybe_unused]] __device__ __forceinline__ uint32_t causal_order(const AttnBwdParams& p) { return p.causal; }
+[[maybe_unused]] __device__ __forceinline__ uint32_t causal_order(const AttnVarlenParams&) { return 0u; }
+
+template <int KIND, int DB, int OUT, bool VL, class P>
 __device__ __forceinline__ void dkdv_body(const CUtensorMap* tq, const CUtensorMap* tk, const CUtensorMap* tv, const CUtensorMap* tdo,
-                                          const CUtensorMap* tdk, const CUtensorMap* tdv, const AttnBwdParams& p) {
+                                          const CUtensorMap* tdk, const CUtensorMap* tdv, const P& p) {
   constexpr int NCH = DB / 64;
   constexpr int QB = kAttnBwdDkdvQueries;
   static_assert(QB == 64 && kAttnBlock == 128, "two consumers of 64 keys, 64-query blocks");
@@ -350,15 +500,34 @@ __device__ __forceinline__ void dkdv_body(const CUtensorMap* tq, const CUtensorM
   auto full_do = [&](uint32_t s) { return bars + 8u * (1u + ST + s); };
   auto empty = [&](uint32_t s) { return bars + 8u * (1u + 2u * ST + s); };
 
-  // work: see AttnBwdParams
+  // work: see AttnBwdParams (varlen: the non-causal order)
   const uint32_t Hkv = p.Hkv;
   const uint32_t per = p.B * Hkv;
-  const uint32_t kb = p.causal ? blockIdx.x / per : blockIdx.x % p.nkb;
-  const uint32_t rem = p.causal ? blockIdx.x % per : blockIdx.x / p.nkb;
+  const uint32_t kb = causal_order(p) ? blockIdx.x / per : blockIdx.x % p.nkb;
+  const uint32_t rem = causal_order(p) ? blockIdx.x % per : blockIdx.x / p.nkb;
   const uint32_t b = rem / Hkv, hk = rem - b * Hkv;
   const uint32_t k0 = kb * kAttnBlock;
-  const uint32_t qb0 = p.causal ? k0 / QB : 0u;                       // the diagonal query block
-  const uint32_t per_head = p.nqd > qb0 ? p.nqd - qb0 : 0u;
+  // query blocks [qb0, qb0 + per_head) of every group head; rows and keys at (qrow, krow) + block offsets in batch bb
+  uint32_t qb0, per_head;
+  int qrow = 0, krow = 0, bb = static_cast<int>(b), qs = 0;
+  int Lq = 0, Lk = 0, off = 0;   // varlen: the sequence's lengths, off = Lk - Lq
+  if constexpr (VL) {
+    int ks;
+    varlen_seq(p.cu_q, b, p.Tq, p.max_q, qs, Lq);
+    varlen_seq(p.cu_k, b, p.Tk, p.max_k, ks, Lk);
+    if (static_cast<int>(k0) >= Lk) return;   // past the sequence: no load, no store
+    off = Lk - Lq;
+    int lo, hi;
+    band_blocks(static_cast<int>(k0), min(static_cast<int>(k0) + kAttnBlock, Lk) - 1, -off, p.right, p.left, Lq, QB, lo, hi);
+    qb0 = static_cast<uint32_t>(lo);
+    per_head = static_cast<uint32_t>(hi - lo);
+    qrow = qs;
+    krow = ks;
+    bb = 0;
+  } else {
+    qb0 = p.causal ? k0 / QB : 0u;                                    // the diagonal query block
+    per_head = p.nqd > qb0 ? p.nqd - qb0 : 0u;
+  }
   const uint32_t steps = p.group * per_head;                          // group == 0 when Hq == 0
 
   const uint32_t wg = threadIdx.x >> 7;
@@ -379,7 +548,14 @@ __device__ __forceinline__ void dkdv_body(const CUtensorMap* tq, const CUtensorM
   }
   __syncthreads();
 
-  const uint64_t plane = static_cast<uint64_t>(p.B) * p.Hq * p.Sqp;
+  uint64_t plane, wsb;   // the workspace's delta plane; the sequence's first row (dense: the batch's, per head Sqp rows)
+  if constexpr (VL) {
+    plane = static_cast<uint64_t>(p.Hq) * p.Tqp;
+    wsb = varlen_ws_start(qs, b);
+  } else {
+    plane = static_cast<uint64_t>(p.B) * p.Hq * p.Sqp;
+    wsb = 0;
+  }
   if (wg == 0) {
     // ===================================================================== TMA producer (one thread)
     setmaxnreg_dec<40>();
@@ -387,8 +563,8 @@ __device__ __forceinline__ void dkdv_body(const CUtensorMap* tq, const CUtensorM
       mbar_arrive_expect_tx(kv_bar, 2u * KTILE);
 #pragma unroll
       for (int c = 0; c < NCH; ++c) {
-        tma_load_4d(sk + c * KCHUNK, tk, kv_bar, c * 64, static_cast<int>(k0), static_cast<int>(hk), static_cast<int>(b));
-        tma_load_4d(sv + c * KCHUNK, tv, kv_bar, c * 64, static_cast<int>(k0), static_cast<int>(hk), static_cast<int>(b));
+        tma_load_4d(sk + c * KCHUNK, tk, kv_bar, c * 64, krow + static_cast<int>(k0), static_cast<int>(hk), bb);
+        tma_load_4d(sv + c * KCHUNK, tv, kv_bar, c * 64, krow + static_cast<int>(k0), static_cast<int>(hk), bb);
       }
       const uint64_t pol = l2_policy_evict_last();   // every key block of the head reads these slices
       const uint8_t* ws = reinterpret_cast<const uint8_t*>(p.ws);
@@ -397,15 +573,17 @@ __device__ __forceinline__ void dkdv_body(const CUtensorMap* tq, const CUtensorM
         const uint32_t g = step / per_head, qb = qb0 + step % per_head;
         const uint32_t h = hk * p.group + g;
         const int q0 = static_cast<int>(qb * QB);
-        const uint64_t row = (static_cast<uint64_t>(b) * p.Hq + h) * p.Sqp + static_cast<uint64_t>(q0);
+        uint64_t row;
+        if constexpr (VL) row = static_cast<uint64_t>(h) * p.Tqp + wsb + static_cast<uint64_t>(q0);
+        else row = (static_cast<uint64_t>(b) * p.Hq + h) * p.Sqp + static_cast<uint64_t>(q0);
         mbar_wait(empty(s), ph ^ 1u);
         mbar_arrive_expect_tx(full_q(s), QTILE + QB * 4u);
 #pragma unroll
-        for (int c = 0; c < NCH; ++c) tma_load_4d(sq(s) + c * QCHUNK, tq, full_q(s), c * 64, q0, static_cast<int>(h), static_cast<int>(b));
+        for (int c = 0; c < NCH; ++c) tma_load_4d(sq(s) + c * QCHUNK, tq, full_q(s), c * 64, qrow + q0, static_cast<int>(h), bb);
         bulk_load_1d(sl(s), ws + 4u * row, QB * 4u, full_q(s), pol);
         mbar_arrive_expect_tx(full_do(s), QTILE + QB * 4u);
 #pragma unroll
-        for (int c = 0; c < NCH; ++c) tma_load_4d(sdo(s) + c * QCHUNK, tdo, full_do(s), c * 64, q0, static_cast<int>(h), static_cast<int>(b));
+        for (int c = 0; c < NCH; ++c) tma_load_4d(sdo(s) + c * QCHUNK, tdo, full_do(s), c * 64, qrow + q0, static_cast<int>(h), bb);
         bulk_load_1d(sd(s), ws + 4u * (plane + row), QB * 4u, full_do(s), pol);
         if (++s == ST) { s = 0; ph ^= 1u; }
       }
@@ -422,7 +600,9 @@ __device__ __forceinline__ void dkdv_body(const CUtensorMap* tq, const CUtensorM
   const uint32_t j0 = k0 + cw * 64u + r, j1 = j0 + 8u;   // this thread's two key rows
   const uint32_t col = 2u * (lane & 3u);
   const float c2 = p.scale_log2;
-  const uint32_t qb_c = p.causal ? (k0 + cw * 64u) / QB : 0u;   // this consumer's diagonal query block
+  // this consumer's diagonal query block (varlen: every block of the CTA's range runs, masked where the band or Lq cuts it)
+  uint32_t qb_c = 0;
+  if constexpr (!VL) qb_c = p.causal ? (k0 + cw * 64u) / QB : 0u;
 
   float dk[NA], dv[NA];
 #pragma unroll
@@ -432,7 +612,9 @@ __device__ __forceinline__ void dkdv_body(const CUtensorMap* tq, const CUtensorM
   uint32_t s = 0, ph = 0;
   for (uint32_t step = 0; step < steps; ++step) {
     const uint32_t qb = qb0 + step % per_head;
-    if (qb < qb_c) {   // every query of the block is above this consumer's keys: release the stage once it has landed
+    bool skip = false;
+    if constexpr (!VL) skip = qb < qb_c;
+    if (skip) {   // every query of the block is above this consumer's keys: release the stage once it has landed
       mbar_wait(full_q(s), ph);
       mbar_wait(full_do(s), ph);
       if (t == 0) mbar_arrive(empty(s));
@@ -465,9 +647,19 @@ __device__ __forceinline__ void dkdv_body(const CUtensorMap* tq, const CUtensorM
     wgmma_fence_operands(st);
     wgmma_fence_operands(dpt);
 
-    // ---- P^T and dS^T (columns are queries: L and delta from the stage), the causal mask on the diagonal block only
-    const bool diag = p.causal && qb == qb_c;
+    // ---- P^T and dS^T (columns are queries: L and delta from the stage), the causal mask on the diagonal block only (varlen:
+    // on every block the band or Lq cuts, dS^T a select too)
+    bool diag;
+    if constexpr (VL) {   // some (key, query) pair of the consumer's 64 keys and this block is hidden
+      const int c0 = static_cast<int>(k0 + cw * 64u), i0 = static_cast<int>(qb * QB);
+      diag = i0 < band_lo(c0 + 63, -off, p.right, Lq) || i0 + QB - 1 > band_hi(c0, -off, p.left, Lq);
+    } else {
+      diag = p.causal && qb == qb_c;
+    }
     const uint32_t qcol0 = qb * QB + col;
+    // varlen: query i sees key j iff i < Lq and -right <= i - j + off <= left (host: |i - j + off| < 2^31); d0 is that
+    // difference for this thread's first key and column pair
+    const int d0 = static_cast<int>(qcol0) - static_cast<int>(j0) + off;
     uint32_t pa[NS / 2], da[NS / 2];
 #pragma unroll
     for (int j = 0; j < QB / 8; ++j) {
@@ -477,9 +669,16 @@ __device__ __forceinline__ void dkdv_body(const CUtensorMap* tq, const CUtensorM
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         float x = ex2(__fmul_rn(st[4 * j + e], c2) - ((e & 1) ? lv.y : lv.x));
-        if (diag && ((e < 2) ? j0 : j1) > qcol0 + 8u * j + (e & 1)) x = 0.f;
-        pv[e] = x;
-        v[e] = x * (dpt[4 * j + e] - ((e & 1) ? dl.y : dl.x));
+        if constexpr (VL) {
+          const int qi = static_cast<int>(qcol0 + 8u * j + (e & 1)), d = d0 + 8 * j + (e & 1) - ((e < 2) ? 0 : 8);
+          const bool hide = diag && (qi >= Lq || (p.right >= 0 && d < -p.right) || (p.left >= 0 && d > p.left));
+          pv[e] = hide ? 0.f : x;
+          v[e] = hide ? 0.f : x * (dpt[4 * j + e] - ((e & 1) ? dl.y : dl.x));
+        } else {
+          if (diag && ((e < 2) ? j0 : j1) > qcol0 + 8u * j + (e & 1)) x = 0.f;
+          pv[e] = x;
+          v[e] = x * (dpt[4 * j + e] - ((e & 1) ? dl.y : dl.x));
+        }
       }
       pa[2 * j] = pack16<KIND>(pv[0], pv[1]);
       pa[2 * j + 1] = pack16<KIND>(pv[2], pv[3]);
@@ -488,6 +687,13 @@ __device__ __forceinline__ void dkdv_body(const CUtensorMap* tq, const CUtensorM
     }
 
     // ---- dV += P^T dO and dK += dS^T Q: dO and Q [queries, D] are MN-major B operands
+    if constexpr (VL) {   // Q and dO rows past Lq are the next sequence's (0 * NaN = NaN in the products): zero them
+      const int valid = Lq - static_cast<int>(qb * QB);
+      if (valid < QB) {
+        zero_rows(sq(s), NCH, QCHUNK, valid, QB, 1u + cw);
+        zero_rows(sdo(s), NCH, QCHUNK, valid, QB, 1u + cw);
+      }
+    }
     wgmma_fence_operands(dv);
     wgmma_fence_operands(dk);
     wgmma_fence();
@@ -513,45 +719,69 @@ __device__ __forceinline__ void dkdv_body(const CUtensorMap* tq, const CUtensorM
 
   // ---- epilogue: scale * dK through the consumer's rows of the K tile, dV through its rows of the V tile
   const int row0 = static_cast<int>(k0 + cw * 64u);
-  store_rows<DB, OUT>(dk, p.scale, sk, KCHUNK, cw * 64u * 128u, tdk, row0, p.Sk, static_cast<int>(hk), static_cast<int>(b), p.D, cw);
-  store_rows<DB, OUT>(dv, 1.0f, sv, KCHUNK, cw * 64u * 128u, tdv, row0, p.Sk, static_cast<int>(hk), static_cast<int>(b), p.D, cw);
+  if constexpr (VL) {
+    constexpr uint32_t GSZ = OUT == OUT_F32 ? 4u : 2u;
+    // rows past Lk belong to the next sequence: a block the sequence ends inside is copied out row by row (none when the
+    // consumer's rows all lie past Lk)
+    const int left = min(Lk - row0, 64);
+    const uint64_t r = static_cast<uint64_t>(krow + row0);
+    store_rows<DB, OUT, true>(dk, p.scale, sk, KCHUNK, cw * 64u * 128u, tdk, krow + row0, p.Tk, static_cast<int>(hk), 0, p.D, cw, left,
+                              p.dk + GSZ * (r * p.dk_st + hk * p.dk_sh), GSZ * p.dk_st);
+    store_rows<DB, OUT, true>(dv, 1.0f, sv, KCHUNK, cw * 64u * 128u, tdv, krow + row0, p.Tk, static_cast<int>(hk), 0, p.D, cw, left,
+                              p.dv + GSZ * (r * p.dv_st + hk * p.dv_sh), GSZ * p.dv_st);
+  } else {
+    store_rows<DB, OUT>(dk, p.scale, sk, KCHUNK, cw * 64u * 128u, tdk, row0, p.Sk, static_cast<int>(hk), static_cast<int>(b), p.D, cw);
+    store_rows<DB, OUT>(dv, 1.0f, sv, KCHUNK, cw * 64u * 128u, tdv, row0, p.Sk, static_cast<int>(hk), static_cast<int>(b), p.D, cw);
+  }
   if (t == 0) tma_store_wait<0>();
 }
 
 }  // namespace
 
-// attn_bwd_delta_<in>_<out>: out in the input dtype or f32
+// attn_bwd_delta_<in>_<out>: out in the input dtype or f32; varlen (compiled with -DATTN_VARLEN into its own cubin):
+// attn_bwd_varlen_{delta,dq,dkdv}_...
+#ifdef ATTN_VARLEN
+#define BWD_VL true
+#define BWD_P AttnVarlenParams
+#define BWD_NAME(K, REST) attn_bwd_varlen_##K##_##REST
+#define DELTA_KERNEL(NAME, KIND, OUT) \
+  extern "C" __global__ void __launch_bounds__(256) NAME(const __grid_constant__ AttnVarlenParams p) { delta_varlen_body<KIND, OUT>(p); }
+#else
+#define BWD_VL false
+#define BWD_P AttnBwdParams
+#define BWD_NAME(K, REST) attn_bwd_##K##_##REST
 #define DELTA_KERNEL(NAME, KIND, OUT) \
   extern "C" __global__ void __launch_bounds__(256) NAME(const __grid_constant__ AttnBwdParams p) { delta_body<KIND, OUT>(p); }
-DELTA_KERNEL(attn_bwd_delta_f16_f16, KIND_F16, OUT_F16)
-DELTA_KERNEL(attn_bwd_delta_f16_f32, KIND_F16, OUT_F32)
-DELTA_KERNEL(attn_bwd_delta_bf16_bf16, KIND_BF16, OUT_BF16)
-DELTA_KERNEL(attn_bwd_delta_bf16_f32, KIND_BF16, OUT_F32)
+#endif
+DELTA_KERNEL(BWD_NAME(delta, f16_f16), KIND_F16, OUT_F16)
+DELTA_KERNEL(BWD_NAME(delta, f16_f32), KIND_F16, OUT_F32)
+DELTA_KERNEL(BWD_NAME(delta, bf16_bf16), KIND_BF16, OUT_BF16)
+DELTA_KERNEL(BWD_NAME(delta, bf16_f32), KIND_BF16, OUT_F32)
 
 // attn_bwd_dq_<in>_d<64|128>_<grad> and attn_bwd_dkdv_<in>_d<64|128>_<grad>; D <= 64 runs the d64 kernels
 #define DQ_KERNEL(NAME, KIND, DB, OUT)                                                                               \
   extern "C" __global__ void __launch_bounds__(384, 1)                                                               \
       NAME(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,                         \
            const __grid_constant__ CUtensorMap tv, const __grid_constant__ CUtensorMap tdo,                        \
-           const __grid_constant__ CUtensorMap tdq, const __grid_constant__ AttnBwdParams p) {                      \
-    dq_body<KIND, DB, OUT>(&tq, &tk, &tv, &tdo, &tdq, p);                                                           \
+           const __grid_constant__ CUtensorMap tdq, const __grid_constant__ BWD_P p) {                              \
+    dq_body<KIND, DB, OUT, BWD_VL>(&tq, &tk, &tv, &tdo, &tdq, p);                                                   \
   }
 #define DKDV_KERNEL(NAME, KIND, DB, OUT)                                                                             \
   extern "C" __global__ void __launch_bounds__(384, 1)                                                               \
       NAME(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,                         \
            const __grid_constant__ CUtensorMap tv, const __grid_constant__ CUtensorMap tdo,                        \
            const __grid_constant__ CUtensorMap tdk, const __grid_constant__ CUtensorMap tdv,                       \
-           const __grid_constant__ AttnBwdParams p) {                                                               \
-    dkdv_body<KIND, DB, OUT>(&tq, &tk, &tv, &tdo, &tdk, &tdv, p);                                                   \
+           const __grid_constant__ BWD_P p) {                                                                       \
+    dkdv_body<KIND, DB, OUT, BWD_VL>(&tq, &tk, &tv, &tdo, &tdk, &tdv, p);                                           \
   }
 #define BWD_D(IN, KIND, OUT16)                                         \
-  DQ_KERNEL(attn_bwd_dq_##IN##_d64_##IN, KIND, 64, OUT16)              \
-  DQ_KERNEL(attn_bwd_dq_##IN##_d64_f32, KIND, 64, OUT_F32)             \
-  DQ_KERNEL(attn_bwd_dq_##IN##_d128_##IN, KIND, 128, OUT16)            \
-  DQ_KERNEL(attn_bwd_dq_##IN##_d128_f32, KIND, 128, OUT_F32)           \
-  DKDV_KERNEL(attn_bwd_dkdv_##IN##_d64_##IN, KIND, 64, OUT16)          \
-  DKDV_KERNEL(attn_bwd_dkdv_##IN##_d64_f32, KIND, 64, OUT_F32)         \
-  DKDV_KERNEL(attn_bwd_dkdv_##IN##_d128_##IN, KIND, 128, OUT16)        \
-  DKDV_KERNEL(attn_bwd_dkdv_##IN##_d128_f32, KIND, 128, OUT_F32)
+  DQ_KERNEL(BWD_NAME(dq, IN##_d64_##IN), KIND, 64, OUT16)              \
+  DQ_KERNEL(BWD_NAME(dq, IN##_d64_f32), KIND, 64, OUT_F32)             \
+  DQ_KERNEL(BWD_NAME(dq, IN##_d128_##IN), KIND, 128, OUT16)            \
+  DQ_KERNEL(BWD_NAME(dq, IN##_d128_f32), KIND, 128, OUT_F32)           \
+  DKDV_KERNEL(BWD_NAME(dkdv, IN##_d64_##IN), KIND, 64, OUT16)          \
+  DKDV_KERNEL(BWD_NAME(dkdv, IN##_d64_f32), KIND, 64, OUT_F32)         \
+  DKDV_KERNEL(BWD_NAME(dkdv, IN##_d128_##IN), KIND, 128, OUT16)        \
+  DKDV_KERNEL(BWD_NAME(dkdv, IN##_d128_f32), KIND, 128, OUT_F32)
 BWD_D(f16, KIND_F16, OUT_F16)
 BWD_D(bf16, KIND_BF16, OUT_BF16)

@@ -62,6 +62,10 @@ extern const unsigned char b200_cubin_attention_bwd[];
 extern const unsigned char b200_cubin_attention_bwd_end[];
 extern const unsigned char b200_cubin_attention_kv[];
 extern const unsigned char b200_cubin_attention_kv_end[];
+extern const unsigned char b200_cubin_attention_varlen[];
+extern const unsigned char b200_cubin_attention_varlen_end[];
+extern const unsigned char b200_cubin_attention_varlen_bwd[];
+extern const unsigned char b200_cubin_attention_varlen_bwd_end[];
 }
 
 // ================================================================================================ errors
@@ -333,13 +337,15 @@ static int get_func(b200_ctx* c, const std::string& name, CUfunction* out) {
   auto it = c->funcs.find(name);
   if (it != c->funcs.end()) { *out = it->second; return B200_OK; }
   // modules are loaded in the order gemm, reduce, aux, gemm_b, gemm_c, quant, gemm_q, quant_mm, gemm_conv, gemm_convbwd,
-  // conv_grouped, gemm_conv3d, gemm_convt, attention, attention_bwd, attention_kv; the kernel
+  // conv_grouped, gemm_conv3d, gemm_convt, attention, attention_bwd, attention_kv, attention_varlen, attention_varlen_bwd; the kernel
   // name says where a
   // kernel lives (no failing lookups, which API-level tools such as compute-sanitizer would report)
   auto starts = [&](const char* pfx) { return name.rfind(pfx, 0) == 0; };
   auto has = [&](const char* part) { return name.find(part) != std::string::npos; };
   const bool tc_gemm = starts("gemm_") && name != "gemm_simt_strided" && name != "gemm_scaled_simt";
   const size_t home = name == "conv3d_dgrad_weights" ? 2
+                      : starts("attn_bwd_varlen_") ? 17
+                      : starts("attn_fwd_varlen_") ? 16
                       : starts("attn_kv_") ? 15
                       : starts("attn_bwd_") ? 14
                       : starts("attn_") ? 13
@@ -385,7 +391,9 @@ extern "C" int b200_get_cubin(const char* name, const void** image, size_t* size
   else if (!strcmp(name, "attention")) { b = b200_cubin_attention; e = b200_cubin_attention_end; }
   else if (!strcmp(name, "attention_bwd")) { b = b200_cubin_attention_bwd; e = b200_cubin_attention_bwd_end; }
   else if (!strcmp(name, "attention_kv")) { b = b200_cubin_attention_kv; e = b200_cubin_attention_kv_end; }
-  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd|conv_grouped|gemm_conv3d|gemm_convt|attention|attention_bwd|attention_kv)", name);
+  else if (!strcmp(name, "attention_varlen")) { b = b200_cubin_attention_varlen; e = b200_cubin_attention_varlen_end; }
+  else if (!strcmp(name, "attention_varlen_bwd")) { b = b200_cubin_attention_varlen_bwd; e = b200_cubin_attention_varlen_bwd_end; }
+  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd|conv_grouped|gemm_conv3d|gemm_convt|attention|attention_bwd|attention_kv|attention_varlen|attention_varlen_bwd)", name);
   *image = b;
   *size = static_cast<size_t>(e - b);
   return B200_OK;
@@ -448,7 +456,9 @@ extern "C" int b200_init(int device, b200_ctx** out) {
       (rc = load_module(c, b200_cubin_gemm_convt, b200_cubin_gemm_convt_end, "gemm_convt")) ||
       (rc = load_module(c, b200_cubin_attention, b200_cubin_attention_end, "attention")) ||
       (rc = load_module(c, b200_cubin_attention_bwd, b200_cubin_attention_bwd_end, "attention_bwd")) ||
-      (rc = load_module(c, b200_cubin_attention_kv, b200_cubin_attention_kv_end, "attention_kv"))) {
+      (rc = load_module(c, b200_cubin_attention_kv, b200_cubin_attention_kv_end, "attention_kv")) ||
+      (rc = load_module(c, b200_cubin_attention_varlen, b200_cubin_attention_varlen_end, "attention_varlen")) ||
+      (rc = load_module(c, b200_cubin_attention_varlen_bwd, b200_cubin_attention_varlen_bwd_end, "attention_varlen_bwd"))) {
     for (CUmodule m : c->modules) g_drv.cuModuleUnload_p(m);
     g_drv.cuDevicePrimaryCtxRelease_p(c->dev);
     return bail(rc);
@@ -4450,6 +4460,298 @@ extern "C" int b200_attention_backward(b200_ctx* c, b200_stream s, b200_dtype in
     if (!rc) rc = encode_tmap4(c, &mdv, gdt, gsz, dv, dimk, sdv, box_g, CU_TENSOR_MAP_SWIZZLE_128B);
     CUfunction f = nullptr;
     if (!rc) rc = get_func(c, "attn_bwd_dkdv_" + in_tag + "_d" + std::to_string(DB) + "_" + g_tag, &f);
+    const unsigned smem = 1024 + 2 * kAttnBlock * DB * 2 + 2 * kAttnBwdStages * kAttnBwdDkdvQueries * DB * 2 +
+                          kAttnBwdStages * 2 * kAttnBwdDkdvQueries * 4 + 1024;
+    if (!rc) rc = set_smem(f, smem);
+    void* kargs[] = {&mq, &mk, &mv, &mdo, &mdk, &mdv, &p};
+    if (!rc) rc = launch(c, f, (unsigned)(nkb * Hkv * B), 1, 1, 384, smem, 1, st, kargs);
+  }
+  for (CUdeviceptr t : tmp)
+    if (t) pool_free(c, t, st);   // stream-ordered: reusable once the kernels have drained
+  return rc;
+}
+
+// ------------------------------------------------------------------------------------------------ varlen attention
+// A [T, H, D] varlen operand (shape and strides in elements, strides 0 = compact) as the 4-D shape [1, T, H, D] with its
+// normalised strides ns (ns[0]: the unit batch dimension's, any valid value).
+static void vl_view(const uint64_t* shape3, const uint64_t* strides3, uint64_t* shape4, uint64_t* ns) {
+  shape4[0] = 1; shape4[1] = shape3[0]; shape4[2] = shape3[1]; shape4[3] = shape3[2];
+  const uint64_t st4[4] = {0, strides3 ? strides3[0] : 0, strides3 ? strides3[1] : 0, strides3 ? strides3[2] : 0};
+  conv_norm_strides(shape4, strides3 ? st4 : nullptr, ns);
+}
+
+// The checks both varlen entries share (see cubecl_b200.h); 0 or the failure status.
+static int vl_check(const char* what, b200_dtype in_dtype, const uint64_t* q_shape, const uint64_t* k_shape, const uint64_t* v_shape,
+                    uint64_t batch, const b200_attention_varlen_args* args) {
+  auto ull = [](uint64_t x) { return (unsigned long long)x; };
+  if (in_dtype != B200_F16 && in_dtype != B200_BF16)
+    return fail(B200_ERR_UNSUPPORTED, "%s: input dtype %d unsupported (f16, bf16)", what, (int)in_dtype);
+  const uint64_t Tq = q_shape[0], Hq = q_shape[1], D = q_shape[2], Tk = k_shape[0], Hkv = k_shape[1];
+  if (k_shape[2] != D) return fail(B200_ERR_INVALID_ARG, "%s: k's head dim %llu differs from q's D = %llu", what, ull(k_shape[2]), ull(D));
+  if (v_shape[0] != Tk || v_shape[1] != Hkv)
+    return fail(B200_ERR_INVALID_ARG, "%s: v [%llu,%llu,%llu] does not match k [%llu,%llu,%llu]", what, ull(v_shape[0]), ull(v_shape[1]),
+                ull(v_shape[2]), ull(Tk), ull(Hkv), ull(D));
+  if (v_shape[2] != D) return fail(B200_ERR_UNSUPPORTED, "%s: v's head dim %llu differs from D = %llu", what, ull(v_shape[2]), ull(D));
+  if (Hkv == 0 || Hq % Hkv) return fail(B200_ERR_INVALID_ARG, "%s: Hq = %llu must be a multiple of Hkv = %llu", what, ull(Hq), ull(Hkv));
+  if (args->window_left < -1 || args->window_right < -1)
+    return fail(B200_ERR_INVALID_ARG, "%s: window (%d, %d): each side must be >= 0, or -1 for unbounded", what, args->window_left,
+                args->window_right);
+  if (args->max_seqlen_q < 0 || args->max_seqlen_k < 0)
+    return fail(B200_ERR_INVALID_ARG, "%s: max_seqlen_q = %d and max_seqlen_k = %d must be >= 0", what, args->max_seqlen_q, args->max_seqlen_k);
+  if (!std::isfinite(args->scale)) return fail(B200_ERR_INVALID_ARG, "%s: scale must be finite", what);
+  if (D == 0 || D > 128 || D % 8) return fail(B200_ERR_UNSUPPORTED, "%s: head dim D = %llu unsupported (a multiple of 8 in [8, 128])", what, ull(D));
+  const uint64_t lim = 1ull << 31;
+  if (batch >= lim || Tq >= lim || Hq >= lim || Tk >= lim || Hkv >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: extents must be < 2^31", what);
+  if (args->max_seqlen_q >= (1 << 30) || args->max_seqlen_k >= (1 << 30))
+    return fail(B200_ERR_UNSUPPORTED, "%s: max_seqlen_q and max_seqlen_k must be < 2^30", what);
+  return B200_OK;
+}
+
+// Variable-length attention, forward (see cubecl_b200.h): one attn_fwd_varlen_* launch.
+extern "C" int b200_attention_varlen(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr q,
+                                     const uint64_t* q_shape, const uint64_t* q_strides, b200_dptr k, const uint64_t* k_shape,
+                                     const uint64_t* k_strides, b200_dptr v, const uint64_t* v_shape, const uint64_t* v_strides,
+                                     b200_dptr cu_seqlens_q, b200_dptr cu_seqlens_k, uint64_t batch, b200_dptr out,
+                                     const uint64_t* out_shape, const uint64_t* out_strides, b200_dptr lse,
+                                     const b200_attention_varlen_args* args) {
+  CTX_ENTER(c);
+  const char* what = "attention_varlen";
+  auto ull = [](uint64_t x) { return (unsigned long long)x; };
+  if (!q_shape || !k_shape || !v_shape || !out_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
+  int rc = vl_check(what, in_dtype, q_shape, k_shape, v_shape, batch, args);
+  if (rc) return rc;
+  if (out_dtype != in_dtype && out_dtype != B200_F32)
+    return fail(B200_ERR_UNSUPPORTED, "%s: output dtype must equal the input dtype or be f32", what);
+  if (memcmp(out_shape, q_shape, 3 * sizeof(uint64_t)))
+    return fail(B200_ERR_INVALID_ARG, "%s: out is [%llu,%llu,%llu], expected q's [%llu,%llu,%llu]", what, ull(out_shape[0]), ull(out_shape[1]),
+                ull(out_shape[2]), ull(q_shape[0]), ull(q_shape[1]), ull(q_shape[2]));
+  const uint64_t Tq = q_shape[0], Hq = q_shape[1], D = q_shape[2], Tk = k_shape[0], Hkv = k_shape[1], B = batch;
+  const uint64_t max_q = (uint64_t)args->max_seqlen_q, max_k = (uint64_t)args->max_seqlen_k;
+  if (B == 0 || Tq == 0 || Hq == 0 || max_q == 0) return B200_OK;   // no query row
+  const uint64_t nqb = (max_q + kAttnBlock - 1) / kAttnBlock, ctas = nqb * Hq * B;
+  if (ctas >= (1ull << 31)) return fail(B200_ERR_UNSUPPORTED, "%s: ceil(max_seqlen_q / %d) * Hq * B = %llu CTAs must be < 2^31", what, kAttnBlock, ull(ctas));
+  if (!q || !k || !v || !out || !cu_seqlens_q || !cu_seqlens_k) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
+  if (lse % 4 || cu_seqlens_q % 4 || cu_seqlens_k % 4)
+    return fail(B200_ERR_INVALID_ARG, "%s: lse, cu_seqlens_q and cu_seqlens_k must be 4-byte aligned", what);
+  const size_t osz = dtype_size(out_dtype);
+  uint64_t qsh[4], ksh[4], vsh[4], osh[4], qs[4], ks[4], vs[4], os[4];
+  vl_view(out_shape, out_strides, osh, os);
+  if (!attn_view_ok(out, osz, os))
+    return fail(B200_ERR_UNSUPPORTED, "%s: out needs a unit D stride and a 16-byte aligned base and T, H strides", what);
+  vl_view(q_shape, q_strides, qsh, qs);
+  vl_view(k_shape, k_strides, ksh, ks);
+  vl_view(v_shape, v_strides, vsh, vs);
+
+  CUstream st = resolve_stream(c, s);
+  CUdeviceptr tmp[3] = {0, 0, 0};
+  // each operand in place, or gathered into a compact [T, H, D] copy
+  auto prep = [&](int i, uint64_t ptr, const uint64_t* shape, uint64_t* ns, uint64_t* use) -> int {
+    *use = ptr;
+    if (attn_view_ok(ptr, 2, ns)) return B200_OK;
+    int r = conv_gather(c, st, in_dtype, ptr, shape, ns, &tmp[i]);
+    *use = tmp[i];
+    ns[3] = 1; ns[2] = shape[3]; ns[1] = shape[2] * shape[3]; ns[0] = shape[1] * shape[2] * shape[3];
+    return r;
+  };
+  uint64_t qp = 0, kp = 0, vp = 0;
+  rc = prep(0, q, qsh, qs, &qp);
+  if (!rc) rc = prep(1, k, ksh, ks, &kp);
+  if (!rc) rc = prep(2, v, vsh, vs, &vp);
+  if (!rc) {
+    const uint32_t DB = D <= 64 ? 64 : 128;
+    const CUtensorMapDataType dt = in_dtype == B200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+    CUtensorMap mq, mk, mv, mo;
+    const uint32_t box_in[4] = {64, (uint32_t)kAttnBlock, 1, 1};
+    const uint32_t box_out[4] = {(uint32_t)(128 / osz), 64, 1, 1};
+    const uint64_t dq[4] = {D, Tq, Hq, 1}, dk[4] = {D, Tk, Hkv, 1};
+    const uint64_t sq[3] = {qs[1], qs[2], qs[0]}, sk[3] = {ks[1], ks[2], ks[0]}, sv[3] = {vs[1], vs[2], vs[0]}, so[3] = {os[1], os[2], os[0]};
+    rc = encode_tmap4(c, &mq, dt, 2, qp, dq, sq, box_in, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (!rc) rc = encode_tmap4(c, &mk, dt, 2, kp, dk, sk, box_in, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (!rc) rc = encode_tmap4(c, &mv, dt, 2, vp, dk, sv, box_in, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (!rc)
+      rc = encode_tmap4(c, &mo, osz == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_UINT16, osz, out, dq, so, box_out,
+                        CU_TENSOR_MAP_SWIZZLE_128B);
+    CUfunction f = nullptr;
+    const std::string name = std::string("attn_fwd_varlen_") + dt_tag(in_dtype) + "_d" + std::to_string(DB) + "_" + dt_tag(out_dtype);
+    if (!rc) rc = get_func(c, name, &f);
+    const unsigned smem = 1024 + (1 + 2 * kAttnStages) * kAttnBlock * DB * 2 + 1024;
+    if (!rc && !c->dry) {
+      CUresult r = g_drv.cuFuncSetAttribute_p(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem);
+      if (r != CUDA_SUCCESS) rc = fail(map_cu(r), "cuFuncSetAttribute: %s", cu_err(r));
+    }
+    if (!rc) {
+      AttnVarlenParams p{};
+      p.lse = lse;
+      p.cu_q = cu_seqlens_q; p.cu_k = cu_seqlens_k;
+      p.out = out; p.o_st = os[1]; p.o_sh = os[2];
+      p.B = (uint32_t)B; p.Hq = (uint32_t)Hq; p.Hkv = (uint32_t)Hkv; p.Tq = (uint32_t)Tq; p.Tk = (uint32_t)Tk;
+      p.group = (uint32_t)(Hq / Hkv);
+      p.max_q = (uint32_t)max_q; p.max_k = (uint32_t)max_k;
+      p.nqb = (uint32_t)nqb; p.nkb = (uint32_t)((max_k + kAttnBlock - 1) / kAttnBlock);
+      p.D = (uint32_t)D;
+      p.left = args->window_left; p.right = args->window_right;
+      p.scale_log2 = (float)((double)args->scale * 1.4426950408889634074);
+      p.scale = args->scale;
+      void* kargs[] = {&mq, &mk, &mv, &mo, &p};
+      rc = launch(c, f, (unsigned)ctas, 1, 1, 384, smem, 1, st, kargs);
+    }
+  }
+  for (CUdeviceptr t : tmp)
+    if (t) pool_free(c, t, st);   // stream-ordered: reusable once the kernel has drained
+  return rc;
+}
+
+// Backward of b200_attention_varlen (see cubecl_b200.h): the delta / L pass, then the dq and the dk / dv kernels.
+extern "C" int b200_attention_varlen_backward(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dtype grad_dtype,
+                                              b200_dptr q, const uint64_t* q_shape, const uint64_t* q_strides, b200_dptr k,
+                                              const uint64_t* k_shape, const uint64_t* k_strides, b200_dptr v, const uint64_t* v_shape,
+                                              const uint64_t* v_strides, b200_dptr out, const uint64_t* out_shape,
+                                              const uint64_t* out_strides, b200_dptr dout, const uint64_t* dout_shape,
+                                              const uint64_t* dout_strides, b200_dptr lse, b200_dptr cu_seqlens_q,
+                                              b200_dptr cu_seqlens_k, uint64_t batch, b200_dptr dq, const uint64_t* dq_shape,
+                                              const uint64_t* dq_strides, b200_dptr dk, const uint64_t* dk_shape,
+                                              const uint64_t* dk_strides, b200_dptr dv, const uint64_t* dv_shape,
+                                              const uint64_t* dv_strides, const b200_attention_varlen_args* args) {
+  CTX_ENTER(c);
+  const char* what = "attention_varlen_backward";
+  auto ull = [](uint64_t x) { return (unsigned long long)x; };
+  if (!q_shape || !k_shape || !v_shape || !out_shape || !dout_shape || !dq_shape || !dk_shape || !dv_shape || !args)
+    return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
+  int rc = vl_check(what, in_dtype, q_shape, k_shape, v_shape, batch, args);
+  if (rc) return rc;
+  if (out_dtype != in_dtype && out_dtype != B200_F32)
+    return fail(B200_ERR_UNSUPPORTED, "%s: output dtype must equal the input dtype or be f32", what);
+  if (grad_dtype != in_dtype && grad_dtype != B200_F32)
+    return fail(B200_ERR_UNSUPPORTED, "%s: grad dtype must equal the input dtype or be f32", what);
+  const struct { const char* name; const uint64_t* shape; const uint64_t* want; } same[] = {
+      {"out", out_shape, q_shape}, {"dout", dout_shape, q_shape}, {"dq", dq_shape, q_shape}, {"dk", dk_shape, k_shape}, {"dv", dv_shape, k_shape}};
+  for (const auto& t : same)
+    if (memcmp(t.shape, t.want, 3 * sizeof(uint64_t)))
+      return fail(B200_ERR_INVALID_ARG, "%s: %s is [%llu,%llu,%llu], expected [%llu,%llu,%llu]", what, t.name, ull(t.shape[0]), ull(t.shape[1]),
+                  ull(t.shape[2]), ull(t.want[0]), ull(t.want[1]), ull(t.want[2]));
+  const uint64_t Tq = q_shape[0], Hq = q_shape[1], D = q_shape[2], Tk = k_shape[0], Hkv = k_shape[1], B = batch;
+  const uint64_t max_q = (uint64_t)args->max_seqlen_q, max_k = (uint64_t)args->max_seqlen_k;
+  // query rows to differentiate (delta and dq); key rows to differentiate (dk and dv: +0 where no query sees them)
+  const bool has_q = B > 0 && Tq > 0 && Hq > 0 && max_q > 0, has_k = B > 0 && Tk > 0 && max_k > 0;
+  if (!has_q && !has_k) return B200_OK;
+  const uint64_t nqb = (max_q + kAttnBlock - 1) / kAttnBlock, nkb = (max_k + kAttnBlock - 1) / kAttnBlock;
+  const uint64_t Tqp = ((Tq + kAttnBlock - 1) / kAttnBlock + B) * kAttnBlock;   // workspace rows per head
+  if (nqb * Hq * B >= (1ull << 31) || nkb * Hkv * B >= (1ull << 31) || nqb * 8 * Hq * B >= (1ull << 31))
+    return fail(B200_ERR_UNSUPPORTED, "%s: more than 2^31 - 1 CTAs", what);
+  if (!cu_seqlens_q || !cu_seqlens_k || !k || !v || !dk || !dv || (has_q && (!q || !out || !dout || !dq || !lse)))
+    return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
+  if (lse % 4 || cu_seqlens_q % 4 || cu_seqlens_k % 4)
+    return fail(B200_ERR_INVALID_ARG, "%s: lse, cu_seqlens_q and cu_seqlens_k must be 4-byte aligned", what);
+  const size_t gsz = dtype_size(grad_dtype);
+  uint64_t qsh[4], ksh[4], vsh[4], osh[4], dosh[4], gsh[4], qs[4], ks[4], vs[4], os[4], dos[4], dqs[4], dks[4], dvs[4];
+  vl_view(dq_shape, dq_strides, gsh, dqs);
+  vl_view(dk_shape, dk_strides, gsh, dks);
+  vl_view(dv_shape, dv_strides, gsh, dvs);
+  const struct { const char* name; uint64_t ptr; const uint64_t* ns; bool used; } grads[] = {
+      {"dq", dq, dqs, has_q}, {"dk", dk, dks, has_k}, {"dv", dv, dvs, has_k}};
+  for (const auto& g : grads)
+    if (g.used && !attn_view_ok(g.ptr, gsz, g.ns))
+      return fail(B200_ERR_UNSUPPORTED, "%s: %s needs a unit D stride and a 16-byte aligned base and T, H strides", what, g.name);
+  vl_view(q_shape, q_strides, qsh, qs);
+  vl_view(k_shape, k_strides, ksh, ks);
+  vl_view(v_shape, v_strides, vsh, vs);
+  vl_view(out_shape, out_strides, osh, os);
+  vl_view(dout_shape, dout_strides, dosh, dos);
+
+  CUstream st = resolve_stream(c, s);
+  CUdeviceptr tmp[6] = {0, 0, 0, 0, 0, 0};   // gathers of q, k, v, out, dout; the workspace
+  // each operand in place, or gathered into a compact [T, H, D] pooled copy (as b200_attention_varlen); out and dout are read
+  // by the delta kernel with 16-byte loads, so they follow the same rule
+  auto prep = [&](int i, b200_dtype dt, uint64_t ptr, const uint64_t* shape, uint64_t* ns, uint64_t* use) -> int {
+    *use = ptr;
+    const size_t esz = dtype_size(dt);
+    if (attn_view_ok(ptr, esz, ns)) return B200_OK;
+    int r = pool_alloc(c, shape[1] * shape[2] * shape[3] * esz, &tmp[i], st);
+    if (r) return r;
+    *use = tmp[i];
+    r = b200_into_contiguous(c, static_cast<b200_stream>(st), dt, ptr, tmp[i], 4, shape, ns);
+    ns[3] = 1; ns[2] = shape[3]; ns[1] = shape[2] * shape[3]; ns[0] = shape[1] * shape[2] * shape[3];
+    return r;
+  };
+  uint64_t qp = 0, kp = 0, vp = 0, op = 0, dop = 0;
+  if (has_q) rc = prep(0, in_dtype, q, qsh, qs, &qp);
+  if (!rc && has_k) rc = prep(1, in_dtype, k, ksh, ks, &kp);
+  if (!rc && has_k) rc = prep(2, in_dtype, v, vsh, vs, &vp);
+  if (!rc && has_q) rc = prep(3, out_dtype, out, osh, os, &op);
+  if (!rc && has_q) rc = prep(4, in_dtype, dout, dosh, dos, &dop);
+  if (!rc && has_q) rc = pool_alloc(c, 2 * Hq * Tqp * 4, &tmp[5], st);
+
+  AttnVarlenParams p{};
+  p.lse = lse;
+  p.cu_q = cu_seqlens_q; p.cu_k = cu_seqlens_k;
+  p.ws = tmp[5];
+  p.out = op; p.dout = dop;
+  p.o_st = os[1]; p.o_sh = os[2]; p.d_st = dos[1]; p.d_sh = dos[2];
+  p.dq = dq; p.dk = dk; p.dv = dv;
+  p.dq_st = dqs[1]; p.dq_sh = dqs[2]; p.dk_st = dks[1]; p.dk_sh = dks[2]; p.dv_st = dvs[1]; p.dv_sh = dvs[2];
+  p.B = (uint32_t)B; p.Hq = (uint32_t)Hq; p.Hkv = (uint32_t)Hkv; p.Tq = (uint32_t)Tq; p.Tk = (uint32_t)Tk;
+  p.group = (uint32_t)(Hq / Hkv);
+  p.max_q = (uint32_t)max_q; p.max_k = (uint32_t)max_k;
+  p.nqb = (uint32_t)nqb; p.nkb = (uint32_t)nkb;
+  p.Tqp = (uint32_t)Tqp;
+  p.D = (uint32_t)D;
+  p.left = args->window_left; p.right = args->window_right;
+  p.scale_log2 = (float)((double)args->scale * 1.4426950408889634074);
+  p.scale = args->scale;
+  const uint32_t DB = D <= 64 ? 64 : 128;
+  const std::string in_tag = dt_tag(in_dtype), g_tag = dt_tag(grad_dtype);
+  const CUtensorMapDataType dt = in_dtype == B200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  const CUtensorMapDataType gdt = gsz == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_UINT16;
+  const uint64_t dimq[4] = {D, Tq, Hq, 1}, dimk[4] = {D, Tk, Hkv, 1};
+  const uint64_t sq[3] = {qs[1], qs[2], qs[0]}, sk[3] = {ks[1], ks[2], ks[0]}, sv[3] = {vs[1], vs[2], vs[0]}, sdo[3] = {dos[1], dos[2], dos[0]};
+  const uint32_t box128[4] = {64, (uint32_t)kAttnBlock, 1, 1}, box_g[4] = {(uint32_t)(128 / gsz), 64, 1, 1};
+  auto set_smem = [&](CUfunction f, unsigned smem) -> int {
+    if (c->dry) return B200_OK;
+    CUresult r = g_drv.cuFuncSetAttribute_p(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem);
+    return r != CUDA_SUCCESS ? fail(map_cu(r), "cuFuncSetAttribute: %s", cu_err(r)) : B200_OK;
+  };
+
+  // 1. delta and L into the workspace
+  if (!rc && has_q) {
+    CUfunction f = nullptr;
+    rc = get_func(c, "attn_bwd_varlen_delta_" + in_tag + "_" + dt_tag(out_dtype), &f);
+    void* kargs[] = {&p};
+    if (!rc) rc = launch(c, f, (unsigned)(nqb * 8 * Hq * B), 1, 1, 256, 0, 1, st, kargs);
+  }
+  // 2. dq: maps q, k, v, dout (query tiles of kAttnBlock rows, key tiles of kAttnBwdDqKeys), dq.  No keys: k's map stands in
+  // for k and v (never read: every dq row is +0)
+  if (!rc && has_q) {
+    const uint32_t box_k[4] = {64, (uint32_t)kAttnBwdDqKeys, 1, 1};
+    CUtensorMap mq, mk, mv, mdo, mdq;
+    const uint64_t sdq[3] = {dqs[1], dqs[2], dqs[0]};
+    const uint64_t kd[4] = {D, has_k ? Tk : Tq, has_k ? Hkv : Hq, 1};
+    rc = encode_tmap4(c, &mq, dt, 2, qp, dimq, sq, box128, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (!rc) rc = encode_tmap4(c, &mk, dt, 2, has_k ? kp : qp, kd, has_k ? sk : sq, box_k, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (!rc) rc = encode_tmap4(c, &mv, dt, 2, has_k ? vp : qp, kd, has_k ? sv : sq, box_k, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (!rc) rc = encode_tmap4(c, &mdo, dt, 2, dop, dimq, sdo, box128, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (!rc) rc = encode_tmap4(c, &mdq, gdt, gsz, dq, dimq, sdq, box_g, CU_TENSOR_MAP_SWIZZLE_128B);
+    CUfunction f = nullptr;
+    if (!rc) rc = get_func(c, "attn_bwd_varlen_dq_" + in_tag + "_d" + std::to_string(DB) + "_" + g_tag, &f);
+    const unsigned smem = 1024 + 2 * kAttnBlock * DB * 2 + 2 * kAttnBwdStages * kAttnBwdDqKeys * DB * 2 + 1024;
+    if (!rc) rc = set_smem(f, smem);
+    void* kargs[] = {&mq, &mk, &mv, &mdo, &mdq, &p};
+    if (!rc) rc = launch(c, f, (unsigned)(nqb * Hq * B), 1, 1, 384, smem, 1, st, kargs);
+  }
+  // 3. dk and dv: maps q, k, v, dout (query tiles of kAttnBwdDkdvQueries rows, key tiles of kAttnBlock), dk, dv.  No queries:
+  // k's map stands in for q and dout (never read: every dk / dv row is +0)
+  if (!rc && has_k) {
+    const uint32_t box_q[4] = {64, (uint32_t)kAttnBwdDkdvQueries, 1, 1};
+    CUtensorMap mq, mk, mv, mdo, mdk, mdv;
+    const uint64_t sdk[3] = {dks[1], dks[2], dks[0]}, sdv[3] = {dvs[1], dvs[2], dvs[0]};
+    const uint64_t qd[4] = {D, has_q ? Tq : Tk, has_q ? Hq : Hkv, 1};
+    rc = encode_tmap4(c, &mq, dt, 2, has_q ? qp : kp, qd, has_q ? sq : sk, box_q, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (!rc) rc = encode_tmap4(c, &mk, dt, 2, kp, dimk, sk, box128, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (!rc) rc = encode_tmap4(c, &mv, dt, 2, vp, dimk, sv, box128, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (!rc) rc = encode_tmap4(c, &mdo, dt, 2, has_q ? dop : kp, qd, has_q ? sdo : sk, box_q, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (!rc) rc = encode_tmap4(c, &mdk, gdt, gsz, dk, dimk, sdk, box_g, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (!rc) rc = encode_tmap4(c, &mdv, gdt, gsz, dv, dimk, sdv, box_g, CU_TENSOR_MAP_SWIZZLE_128B);
+    CUfunction f = nullptr;
+    if (!rc) rc = get_func(c, "attn_bwd_varlen_dkdv_" + in_tag + "_d" + std::to_string(DB) + "_" + g_tag, &f);
     const unsigned smem = 1024 + 2 * kAttnBlock * DB * 2 + 2 * kAttnBwdStages * kAttnBwdDkdvQueries * DB * 2 +
                           kAttnBwdStages * 2 * kAttnBwdDkdvQueries * 4 + 1024;
     if (!rc) rc = set_smem(f, smem);

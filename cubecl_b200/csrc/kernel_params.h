@@ -257,6 +257,38 @@ struct AttnBwdParams {
   uint32_t Hkv;
 };
 
+// Variable-length (packed) attention: attention.cu and attention_bwd.cu compiled with -DATTN_VARLEN (attn_fwd_varlen_*,
+// attn_bwd_varlen_*; capi.cpp: b200_attention_varlen, b200_attention_varlen_backward).  The dense bodies with per-sequence
+// addressing: q, out, dout, dq are [Tq, Hq, D] and k, v, dk, dv [Tk, Hkv, D], read through 4-D maps (D, T, H, 1).  Sequence b
+// owns rows [cu_q[b], cu_q[b + 1]) and [cu_k[b], cu_k[b + 1]); on read each cu value is clamped to [0, T] and each length to
+// [0, max_seqlen], so no access leaves the tensors.  With positions i, j inside the sequence and off = Lk - Lq, key j is
+// visible to query i iff j < Lk, (left < 0 or j >= i + off - left) and (right < 0 or j <= i + off + right).
+// Grids from host extents only: forward and dq nqb * Hq * B, dkdv nkb * Hkv * B (nqb = ceil(max_q / kAttnBlock), nkb =
+// ceil(max_k / kAttnBlock)) in the dense kernels' orders, with the delta kernel's nqb * 8 * Hq * B blocks of 16 rows; a CTA
+// whose block starts at or past its sequence's length exits at once.
+// Workspace ws (backward): f32 [2][Hq][Tqp], Tqp = (ceil(Tq / kAttnBlock) + B) * kAttnBlock.  Sequence b's rows start at
+// floor((cu_q[b] + kAttnBlock * b) / kAttnBlock) * kAttnBlock (a 16-byte aligned start that never reaches the previous
+// sequence's padded rows) and span ceil(Lq / kAttnBlock) whole blocks: L = +inf and delta = 0 past Lq and for rows whose lse is
+// -inf (no visible key).
+struct AttnVarlenParams {
+  uint64_t lse;                   // f32 [Hq, Tq] compact (forward: 0 = not written)
+  uint64_t cu_q, cu_k;            // i32 [B + 1]
+  uint64_t ws;                    // backward workspace (above)
+  uint64_t out, dout;             // forward: out (direct stores of partial blocks); delta kernel: out and dout views
+  uint64_t o_st, o_sh, d_st, d_sh;  // out / dout strides in elements (T, H)
+  uint64_t dq, dk, dv;            // backward: direct stores of partial blocks
+  uint64_t dq_st, dq_sh, dk_st, dk_sh, dv_st, dv_sh;
+  uint32_t B, Hq, Hkv, Tq, Tk;
+  uint32_t group;                 // Hq / Hkv
+  uint32_t max_q, max_k;          // max_seqlen_q, max_seqlen_k
+  uint32_t nqb, nkb;              // ceil(max_q / kAttnBlock), ceil(max_k / kAttnBlock)
+  uint32_t Tqp;                   // workspace rows per head
+  uint32_t D;
+  int32_t left, right;            // window; -1: unbounded
+  float scale_log2;               // scale * log2(e)
+  float scale;                    // backward: multiplies dQ and dK in the epilogue
+};
+
 // ================================================================================================ attention_kv.cu
 // Attention against a KV cache (attn_kv_*; capi.cpp: b200_attention_kvcache).  One CTA per (b, hk, m-tile, split), grid
 // B * Hkv * nsplit * mtiles with block x = ((b * Hkv + hk) * nsplit + split) * mtiles + mt (the m-tiles that share a key range

@@ -586,6 +586,89 @@ int b200_attention_backward(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b
                             b200_dptr dv, const uint64_t* dv_shape, const uint64_t* dv_strides,
                             const b200_attention_args* args);
 
+/* ---- variable-length (packed) attention, forward (flash_attn_varlen_func, torch.nn.attention.varlen.varlen_attn) -----------
+ * B sequences packed along one token axis.  q and out are [Tq, Hq, D], k and v [Tk, Hkv, D] (shapes and strides in elements,
+ * so the q / k / v slices of a fused [T, 3, H, D] projection are views read with no copy); Hq % Hkv == 0 (GQA / MQA, hk = h /
+ * (Hq / Hkv)).  Sequence b owns query rows [cu_q[b], cu_q[b + 1]) and key rows [cu_k[b], cu_k[b + 1]), lengths Lq_b and Lk_b:
+ *   out[cu_q[b] + i, h, :] = sum_{j visible} softmax_j(scale * q_i . k_j) * v_j          (k_j, v_j: row cu_k[b] + j, head hk)
+ *   lse[h, cu_q[b] + i]    = log sum_{j visible} exp(scale * q_i . k_j)                   (natural log, f32)
+ * Offsets: cu_seqlens_q and cu_seqlens_k are compact i32 [batch + 1] device arrays, read by the kernels only: the host never
+ * reads them, so the call does not synchronise and can be captured in a CUDA graph.  args->max_seqlen_q / max_seqlen_k are
+ * host bounds on the lengths (torch's max_q / max_k), and size the grid.  On the device each cu value is clamped to [0, T] and
+ * each length to [0, max_seqlen]: malformed offsets give unspecified values, but no access leaves q, k, v, out or lse.
+ * Visibility (torch's window_size, flash-attn >= 2.1): with off = Lk_b - Lq_b, key j is visible to query i iff j < Lk_b,
+ * (window_left < 0 or j >= i + off - window_left) and (window_right < 0 or j <= i + off + window_right).  (-1, -1) is full
+ * attention; (-1, 0) is causal aligned bottom-right (b200_attention_kvcache's rule; with Lq == Lk it is b200_attention's
+ * top-left causal); (W, 0) a causal sliding window.  A row with no visible key gets out = +0 and lse = -inf.
+ * Rows outside every sequence (at or past cu_q[batch], and any row no sequence owns) are not written, in out or lse.
+ * Numerics: b200_attention's (f32 scores, base-2 online softmax with t = s * (scale * log2 e), ex2.approx.ftz, P rounded RNE
+ * to the input dtype, out = O / l rounded once).  A sequence with Lq == Lk and window (-1, -1) or (-1, 0) gives the bits of a
+ * b200_attention call on that sequence alone (causal = 0 or 1).  Every row comes from one CTA in increasing key order: no
+ * atomics, bitwise reproducible.  Neighbouring sequences never meet: scores of keys past Lk_b are masked with a select and
+ * their V rows are zeroed on chip before the P.V product, and a block the sequence ends inside is stored row by row.
+ * Dtypes and limits: b200_attention's (f16 / bf16 in, out in the input dtype or f32, D <= 128, D % 8 == 0, v's head dim equal
+ * to D); max_seqlen_q and max_seqlen_k below 2^30.  Views: q, k and v are read in place under b200_attention's rule (unit D
+ * stride, 16-byte aligned base and T, H strides), else gathered into a compact [T, H, D] pooled copy.  out needs a unit D
+ * stride and a 16-byte aligned base and strides.  lse: 0 (not written) or a compact f32 [Hq, Tq] buffer, 4-byte aligned.
+ * Errors: B200_ERR_INVALID_ARG for a k head dim other than D, a v shape mismatch, Hkv == 0 or Hq % Hkv != 0, a wrong out shape,
+ * a window side below -1, a negative max_seqlen, a non-finite scale, a null pointer or a misaligned lse / cu array (the
+ * wrappers also refuse cu arrays that are not compact i32 [batch + 1]); B200_ERR_UNSUPPORTED for the dtypes, D, Dv != D, out a
+ * tensor map cannot write, extents >= 2^31, max_seqlen >= 2^30 or more than 2^31 - 1 CTAs.  batch, Tq, Hq or max_seqlen_q = 0:
+ * no launch.
+ * Launches: the gathers, then one attn_fwd_varlen_<in>_d<64|128>_<out> launch of ceil(max_seqlen_q / 128) * Hq * batch CTAs
+ * (a CTA whose block starts at or past its sequence's Lq exits at once; key blocks that no row of the CTA sees are skipped, not
+ * loaded), on `s` with no host synchronisation.  The dry-run plan records "tmap4d" lines in the order q, k, v, out with dims
+ * (D, T, H, 1). */
+typedef struct b200_attention_varlen_args {
+  float scale;            /* multiplies q.k before the softmax */
+  int32_t window_left;    /* keys before the aligned diagonal a query sees; -1: unbounded */
+  int32_t window_right;   /* keys after the aligned diagonal a query sees; -1: unbounded (0: causal) */
+  int32_t max_seqlen_q;   /* >= every Lq_b */
+  int32_t max_seqlen_k;   /* >= every Lk_b */
+} b200_attention_varlen_args;
+int b200_attention_varlen(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype,
+                          b200_dptr q, const uint64_t* q_shape, const uint64_t* q_strides,
+                          b200_dptr k, const uint64_t* k_shape, const uint64_t* k_strides,
+                          b200_dptr v, const uint64_t* v_shape, const uint64_t* v_strides,
+                          b200_dptr cu_seqlens_q, b200_dptr cu_seqlens_k, uint64_t batch,
+                          b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides,
+                          b200_dptr lse, const b200_attention_varlen_args* args);
+
+/* ---- variable-length (packed) attention, backward --------------------------------------------------------------------------
+ * b200_attention_backward's formulas per sequence of b200_attention_varlen (its layout, offsets, args and visibility): dq
+ * [Tq, Hq, D], dk and dv [Tk, Hkv, D] from q, k, v, the forward's out and lse (compact f32 [Hq, Tq], non-null) and dout; dk
+ * and dv of kv head hk sum over its G query heads.  A row without visible keys (lse = -inf) gives dq = +0 and adds nothing to
+ * dk or dv; a key no query sees gets dk = dv = +0.  Rows outside every sequence are not written, in dq, dk or dv.
+ * Numerics: b200_attention_backward's (the forward's scores bit for bit, p = exp2(t - lse * log2 e), P and dS rounded RNE,
+ * f32 sums, dq and dk multiplied by scale and rounded once).  A sequence with Lq == Lk and window (-1, -1) or (-1, 0) gives the
+ * bits of a b200_attention_backward call on that sequence alone.  Every dq row comes from one CTA in key order and every dk /
+ * dv row from one CTA in (group head, query block) order: no atomics, bitwise reproducible.  Q and dO rows past Lq_b (and K
+ * rows past Lk_b in the dq kernel) are zeroed on chip before they enter a product.
+ * Dtypes, views and limits: b200_attention_varlen's; out in the input dtype or f32 (out_dtype), dout in the input dtype; dq, dk
+ * and dv in grad_dtype (the input dtype or B200_F32) with a unit D stride and a 16-byte aligned base and strides (so they can
+ * be slices of one fused [T, 3, H, D] gradient buffer), else B200_ERR_UNSUPPORTED naming the tensor.  out and dout are read in
+ * place under the input rule, else gathered.
+ * Errors: b200_attention_varlen's, plus B200_ERR_INVALID_ARG when out, dout or dq differ from q's shape or dk or dv from k's,
+ * and B200_ERR_UNSUPPORTED for an out_dtype or grad_dtype other than the input dtype or f32.  batch = 0, or no query rows (Tq,
+ * Hq or max_seqlen_q = 0) together with no key rows (Tk or max_seqlen_k = 0), launches nothing.
+ * Launches, on `s` with no host synchronisation: the gathers; with query rows, a pooled f32 workspace of 2 * Hq * Tqp values,
+ * Tqp = (ceil(Tq / 128) + batch) * 128 ("alloc"; each sequence gets its own 128-row aligned slices), then
+ * attn_bwd_varlen_delta_<in>_<out> (ceil(max_seqlen_q / 128) * 8 * Hq * batch blocks of 256 threads) and
+ * attn_bwd_varlen_dq_<in>_d<64|128>_<grad> (ceil(max_seqlen_q / 128) * Hq * batch CTAs) after its maps q, k, v, dout, dq; with
+ * key rows, attn_bwd_varlen_dkdv_<in>_d<64|128>_<grad> (ceil(max_seqlen_k / 128) * Hkv * batch CTAs) after its maps q, k, v,
+ * dout, dk, dv.  The maps are "tmap4d" plan lines with dims (D, T, H, 1). */
+int b200_attention_varlen_backward(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dtype grad_dtype,
+                                   b200_dptr q, const uint64_t* q_shape, const uint64_t* q_strides,
+                                   b200_dptr k, const uint64_t* k_shape, const uint64_t* k_strides,
+                                   b200_dptr v, const uint64_t* v_shape, const uint64_t* v_strides,
+                                   b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides,
+                                   b200_dptr dout, const uint64_t* dout_shape, const uint64_t* dout_strides,
+                                   b200_dptr lse, b200_dptr cu_seqlens_q, b200_dptr cu_seqlens_k, uint64_t batch,
+                                   b200_dptr dq, const uint64_t* dq_shape, const uint64_t* dq_strides,
+                                   b200_dptr dk, const uint64_t* dk_shape, const uint64_t* dk_strides,
+                                   b200_dptr dv, const uint64_t* dv_shape, const uint64_t* dv_strides,
+                                   const b200_attention_varlen_args* args);
+
 /* ---- attention against a KV cache (decoding, speculative decoding, chunked prefill; forward only) ------------------------
  * Sequence b of the batch has L_b = cache_seqlens[b] keys in the cache.  With G = Hq / Hkv and hk = h / G:
  *   out[b, h, i, :] = sum_{j visible} softmax_j(scale * q[b, h, i, :] . K_b[j, hk, :]) * V_b[j, hk, :]

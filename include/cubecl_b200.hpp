@@ -421,6 +421,58 @@ inline void launch_backward(ComputeClient& client, const TensorHandle& q, const 
   if (rc != B200_OK) client.defer(b200_last_error());
 }
 
+/// Variable-length (packed) attention, forward: q [Tq, Hq, D], k and v [Tk, Hkv, D], out [Tq, Hq, D] (views by strides);
+/// sequence b owns rows [cu_q[b], cu_q[b + 1]) of q and [cu_k[b], cu_k[b + 1]) of k and v (compact i32 [B + 1] tensors read on
+/// the device); window (left, right), -1 unbounded, (-1, 0) bottom-right causal.  lse: nullptr or a compact f32 [Hq, Tq]
+/// tensor.  See b200_attention_varlen in cubecl_b200.h.  Errors are deferred to client.sync().
+inline void launch_varlen(ComputeClient& client, const TensorHandle& q, const TensorHandle& k, const TensorHandle& v,
+                          const TensorHandle& cu_seqlens_q, const TensorHandle& cu_seqlens_k, int32_t max_seqlen_q, int32_t max_seqlen_k,
+                          const TensorHandle& out, float scale, int32_t window_left = -1, int32_t window_right = -1,
+                          const TensorHandle* lse = nullptr) {
+  if (q.shape.size() != 3 || k.shape.size() != 3 || v.shape.size() != 3 || out.shape.size() != 3 || q.dtype != k.dtype ||
+      q.dtype != v.dtype || cu_seqlens_q.shape.size() != 1 || cu_seqlens_q.shape != cu_seqlens_k.shape || cu_seqlens_q.shape[0] < 1) {
+    client.defer("InvalidArgument: attention_varlen needs rank-3 q, k, v and out of one input dtype and cu arrays [B + 1] of one length");
+    return;
+  }
+  const b200_attention_varlen_args args{scale, window_left, window_right, max_seqlen_q, max_seqlen_k};
+  const int rc = b200_attention_varlen(
+      client.raw(), nullptr, static_cast<b200_dtype>(q.dtype), static_cast<b200_dtype>(out.dtype), q.handle.ptr(), q.shape.data(),
+      q.strides.data(), k.handle.ptr(), k.shape.data(), k.strides.data(), v.handle.ptr(), v.shape.data(), v.strides.data(),
+      cu_seqlens_q.handle.ptr(), cu_seqlens_k.handle.ptr(), cu_seqlens_q.shape[0] - 1, out.handle.ptr(), out.shape.data(),
+      out.strides.data(), lse ? lse->handle.ptr() : 0, &args);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+
+/// Variable-length (packed) attention, backward: dq [Tq, Hq, D], dk and dv [Tk, Hkv, D] (one grad dtype) from q, k, v, the
+/// forward's out and lse (compact f32 [Hq, Tq]) and dout, with the forward's offsets, window and scale.  See
+/// b200_attention_varlen_backward in cubecl_b200.h.  Errors are deferred to client.sync().
+inline void launch_varlen_backward(ComputeClient& client, const TensorHandle& q, const TensorHandle& k, const TensorHandle& v,
+                                   const TensorHandle& out, const TensorHandle& dout, const TensorHandle& lse,
+                                   const TensorHandle& cu_seqlens_q, const TensorHandle& cu_seqlens_k, int32_t max_seqlen_q,
+                                   int32_t max_seqlen_k, const TensorHandle& dq, const TensorHandle& dk, const TensorHandle& dv, float scale,
+                                   int32_t window_left = -1, int32_t window_right = -1) {
+  for (const TensorHandle* t : {&q, &k, &v, &out, &dout, &dq, &dk, &dv}) {
+    if (t->shape.size() != 3) {
+      client.defer("InvalidArgument: attention_varlen backward needs rank-3 q, k, v, out, dout, dq, dk and dv");
+      return;
+    }
+  }
+  if (q.dtype != k.dtype || q.dtype != v.dtype || q.dtype != dout.dtype || dq.dtype != dk.dtype || dq.dtype != dv.dtype ||
+      cu_seqlens_q.shape.size() != 1 || cu_seqlens_q.shape != cu_seqlens_k.shape || cu_seqlens_q.shape[0] < 1) {
+    client.defer("InvalidArgument: attention_varlen backward needs q, k, v and dout of one dtype, dq, dk and dv of one dtype and cu "
+                 "arrays [B + 1] of one length");
+    return;
+  }
+  const b200_attention_varlen_args args{scale, window_left, window_right, max_seqlen_q, max_seqlen_k};
+  const int rc = b200_attention_varlen_backward(
+      client.raw(), nullptr, static_cast<b200_dtype>(q.dtype), static_cast<b200_dtype>(out.dtype), static_cast<b200_dtype>(dq.dtype),
+      q.handle.ptr(), q.shape.data(), q.strides.data(), k.handle.ptr(), k.shape.data(), k.strides.data(), v.handle.ptr(), v.shape.data(),
+      v.strides.data(), out.handle.ptr(), out.shape.data(), out.strides.data(), dout.handle.ptr(), dout.shape.data(), dout.strides.data(),
+      lse.handle.ptr(), cu_seqlens_q.handle.ptr(), cu_seqlens_k.handle.ptr(), cu_seqlens_q.shape[0] - 1, dq.handle.ptr(), dq.shape.data(),
+      dq.strides.data(), dk.handle.ptr(), dk.shape.data(), dk.strides.data(), dv.handle.ptr(), dv.shape.data(), dv.strides.data(), &args);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+
 /// Attention against a KV cache: q [B, Hq, Sq, D] against k_cache, v_cache [P, page, Hkv, D] (views by strides); sequence b
 /// sees its first cache_seqlens[b] keys (compact i32 [B] on the device), key j in page block_table[b, j / page] (i32
 /// [B, max_pages]; nullptr: page b); causal is bottom-right.  lse: nullptr or a compact f32 [B, Hq, Sq] tensor.  See

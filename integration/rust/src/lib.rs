@@ -575,6 +575,57 @@ impl Context {
         ))
     }
 
+    /// Variable-length (packed) attention, forward: q [Tq, Hq, D], k and v [Tk, Hkv, D] -> out [Tq, Hq, D] (views by strides);
+    /// sequence b owns rows [cu_q[b], cu_q[b + 1]) of q and [cu_k[b], cu_k[b + 1]) of k and v (compact i32 [batch + 1] device
+    /// buffers); `window` (left, right), -1 unbounded, (-1, 0) bottom-right causal; `lse`: 0 or a compact f32 [Hq, Tq] buffer.
+    /// See b200_attention_varlen in cubecl_b200.h.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::conv2d`]; the cu buffers must hold batch + 1 i32 values, `lse`, when non-zero, Hq * Tq f32.
+    pub unsafe fn attention_varlen(
+        &mut self, stream: b200_stream, in_dtype: DType, out_dtype: DType, q: &TensorView, k: &TensorView, v: &TensorView,
+        cu_seqlens_q: b200_dptr, cu_seqlens_k: b200_dptr, batch: u64, max_seqlen: (i32, i32), out: &TensorView, lse: b200_dptr,
+        scale: f32, window: (i32, i32),
+    ) -> Result<(), Error> {
+        for t in [q, k, v, out] {
+            assert!(t.shape.len() == 3 && t.strides.len() == 3);
+        }
+        let a = sys::b200_attention_varlen_args {
+            scale, window_left: window.0, window_right: window.1, max_seqlen_q: max_seqlen.0, max_seqlen_k: max_seqlen.1,
+        };
+        check(sys::b200_attention_varlen(
+            self.0, stream, in_dtype as c_int, out_dtype as c_int, q.ptr, q.shape.as_ptr(), q.strides.as_ptr(), k.ptr,
+            k.shape.as_ptr(), k.strides.as_ptr(), v.ptr, v.shape.as_ptr(), v.strides.as_ptr(), cu_seqlens_q, cu_seqlens_k, batch,
+            out.ptr, out.shape.as_ptr(), out.strides.as_ptr(), lse, &a,
+        ))
+    }
+
+    /// Variable-length (packed) attention, backward: dq [Tq, Hq, D], dk and dv [Tk, Hkv, D] in `grad_dtype` from q, k, v, the
+    /// forward's `out` and `lse` (compact f32 [Hq, Tq]) and `dout`, with the forward's offsets, window and scale.  See
+    /// b200_attention_varlen_backward in cubecl_b200.h.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::attention_varlen`]; `lse` must hold Hq * Tq f32 values.
+    pub unsafe fn attention_varlen_backward(
+        &mut self, stream: b200_stream, in_dtype: DType, out_dtype: DType, grad_dtype: DType, q: &TensorView, k: &TensorView,
+        v: &TensorView, out: &TensorView, dout: &TensorView, lse: b200_dptr, cu_seqlens_q: b200_dptr, cu_seqlens_k: b200_dptr,
+        batch: u64, max_seqlen: (i32, i32), dq: &TensorView, dk: &TensorView, dv: &TensorView, scale: f32, window: (i32, i32),
+    ) -> Result<(), Error> {
+        for t in [q, k, v, out, dout, dq, dk, dv] {
+            assert!(t.shape.len() == 3 && t.strides.len() == 3);
+        }
+        let a = sys::b200_attention_varlen_args {
+            scale, window_left: window.0, window_right: window.1, max_seqlen_q: max_seqlen.0, max_seqlen_k: max_seqlen.1,
+        };
+        check(sys::b200_attention_varlen_backward(
+            self.0, stream, in_dtype as c_int, out_dtype as c_int, grad_dtype as c_int, q.ptr, q.shape.as_ptr(), q.strides.as_ptr(),
+            k.ptr, k.shape.as_ptr(), k.strides.as_ptr(), v.ptr, v.shape.as_ptr(), v.strides.as_ptr(), out.ptr, out.shape.as_ptr(),
+            out.strides.as_ptr(), dout.ptr, dout.shape.as_ptr(), dout.strides.as_ptr(), lse, cu_seqlens_q, cu_seqlens_k, batch,
+            dq.ptr, dq.shape.as_ptr(), dq.strides.as_ptr(), dk.ptr, dk.shape.as_ptr(), dk.strides.as_ptr(), dv.ptr, dv.shape.as_ptr(),
+            dv.strides.as_ptr(), &a,
+        ))
+    }
+
     /// Attention of q [B, Hq, Sq, D] against a KV cache `k_cache`, `v_cache` [P, page, Hkv, D] (views by strides): sequence b
     /// sees its first `cache_seqlens`[b] keys (a compact i32 [B] device buffer), key j in page `block_table`[b, j / page] (an
     /// i32 [B, max_pages] view; `None`: page b); `causal` is bottom-right.  See b200_attention_kvcache in cubecl_b200.h.
