@@ -30,6 +30,7 @@ csrc/attention.cu and attention_bwd.cu); see b200_attention_varlen and b200_atte
 from __future__ import annotations
 
 import ctypes as C
+import functools
 import math
 
 from . import _ffi
@@ -55,30 +56,71 @@ def calculate_attention_output(q_shape, k_shape, v_shape) -> list[int]:
     return list(q)
 
 
+def _defers_errors(fn):
+    """The launch never raises for launch problems: they are deferred to client.sync() / read_one() like matmul.launch."""
+    @functools.wraps(fn)
+    def wrapper(client, *args, **kwargs):
+        try:
+            fn(client, *args, **kwargs)
+        except (B200Error, ValueError) as e:
+            client._defer(e if isinstance(e, B200Error) else B200Error(6, str(e)))
+    return wrapper
+
+
+def _check_rank(what, rank, named, layout=""):
+    for name, t in named:
+        if len(t.shape) != rank:
+            raise B200Error(6, f"{what}: {name} must have rank {rank}{layout}, got rank {len(t.shape)}")
+
+
+def _check_same_dtype(what, named, listed=True):
+    if len({t.dtype for _, t in named}) > 1:
+        names = [n for n, _ in named]
+        got = f" ({', '.join(t.dtype for _, t in named)})" if listed else ""
+        raise B200Error(6, f"{what}: {', '.join(names[:-1])} and {names[-1]} dtypes differ{got}")
+
+
+def _check_lse(what, lse, dims, want):
+    """lse (None: not requested) must be a compact f32 tensor of shape `want`, named `dims` in the message."""
+    if lse is not None and (lse.dtype != "f32" or not lse.is_contiguous() or list(lse.shape) != list(want)):
+        raise B200Error(6, f"{what}: lse must be a compact f32 {dims} = {list(want)} tensor")
+
+
+def _scale(scale, D):
+    return 1.0 / math.sqrt(D) if scale is None else float(scale)
+
+
+def _used_on(stream, *tensors):
+    for t in tensors:
+        if t is not None:
+            t.handle.used_on(stream)
+
+
+def _view_args(tensors):
+    ops = []
+    for t in tensors:
+        ops += [C.c_uint64(t.handle.ptr), _ffi.u64_array(t.shape), _ffi.u64_array(t.strides)]
+    return ops
+
+
+def _ptr(t):
+    return C.c_uint64(t.handle.ptr if t is not None else 0)
+
+
+@_defers_errors
 def launch(client: ComputeClient, q: TensorHandle, k: TensorHandle, v: TensorHandle, out: TensorHandle, scale: float | None = None,
            causal: bool = False, lse: TensorHandle | None = None, stream=None) -> None:
     """Enqueue out = softmax(scale * q k^T) v on the client's stream (scale defaults to 1 / sqrt(D)).  lse: an optional compact
     f32 [B, Hq, Sq] tensor that receives the natural-log log-sum-exp of every row.  Never raises for launch problems: errors
     are deferred to client.sync() / read_one() like matmul.launch."""
-    try:
-        for name, t in (("q", q), ("k", k), ("v", v), ("out", out)):
-            if len(t.shape) != 4:
-                raise B200Error(6, f"attention: {name} must have rank 4 [B, H, S, D], got rank {len(t.shape)}")
-        if not (q.dtype == k.dtype == v.dtype):
-            raise B200Error(6, f"attention: q, k and v dtypes differ ({q.dtype}, {k.dtype}, {v.dtype})")
-        if lse is not None and (lse.dtype != "f32" or not lse.is_contiguous() or lse.shape != q.shape[:3]):
-            raise B200Error(6, f"attention: lse must be a compact f32 [B, Hq, Sq] = {q.shape[:3]} tensor")
-        sc = 1.0 / math.sqrt(q.shape[3]) if scale is None else float(scale)
-        for t in (q, k, v, out) + ((lse,) if lse is not None else ()):
-            t.handle.used_on(stream)
-        args = _ffi.AttentionArgs(sc, 1 if causal else 0)
-        ops = []
-        for t in (q, k, v, out):
-            ops += [C.c_uint64(t.handle.ptr), _ffi.u64_array(t.shape), _ffi.u64_array(t.strides)]
-        _ffi.check(client._lib.b200_attention(client._ctx, stream, DTYPES[q.dtype], DTYPES[out.dtype], *ops,
-                                              C.c_uint64(lse.handle.ptr if lse is not None else 0), C.byref(args)))
-    except (B200Error, ValueError) as e:
-        client._defer(e if isinstance(e, B200Error) else B200Error(6, str(e)))
+    what = "attention"
+    _check_rank(what, 4, (("q", q), ("k", k), ("v", v), ("out", out)), " [B, H, S, D]")
+    _check_same_dtype(what, (("q", q), ("k", k), ("v", v)))
+    _check_lse(what, lse, "[B, Hq, Sq]", q.shape[:3])
+    args = _ffi.AttentionArgs(_scale(scale, q.shape[3]), 1 if causal else 0)
+    _used_on(stream, q, k, v, out, lse)
+    _ffi.check(client._lib.b200_attention(client._ctx, stream, DTYPES[q.dtype], DTYPES[out.dtype], *_view_args((q, k, v, out)), _ptr(lse),
+                                          C.byref(args)))
 
 
 def launch_alloc(client: ComputeClient, q: TensorHandle, k: TensorHandle, v: TensorHandle, scale: float | None = None,
@@ -91,37 +133,24 @@ def launch_alloc(client: ComputeClient, q: TensorHandle, k: TensorHandle, v: Ten
     return (out, lse) if return_lse else out
 
 
+@_defers_errors
 def launch_backward(client: ComputeClient, q: TensorHandle, k: TensorHandle, v: TensorHandle, out: TensorHandle, dout: TensorHandle,
                     lse: TensorHandle, dq: TensorHandle, dk: TensorHandle, dv: TensorHandle, scale: float | None = None,
                     causal: bool = False, stream=None) -> None:
     """Enqueue the attention backward: dq, dk and dv (one grad dtype: the input dtype or f32) from q, k, v, the forward's out
     (input dtype or f32) and lse (its compact f32 [B, Hq, Sq] output) and dout (input dtype).  scale and causal must be the
     forward's (scale defaults to 1 / sqrt(D)).  Never raises for launch problems: errors are deferred to client.sync()."""
-    try:
-        named = (("q", q), ("k", k), ("v", v), ("out", out), ("dout", dout), ("dq", dq), ("dk", dk), ("dv", dv))
-        for name, t in named:
-            if len(t.shape) != 4:
-                raise B200Error(6, f"attention_backward: {name} must have rank 4 [B, H, S, D], got rank {len(t.shape)}")
-        if not (q.dtype == k.dtype == v.dtype == dout.dtype):
-            raise B200Error(6, f"attention_backward: q, k, v and dout dtypes differ ({q.dtype}, {k.dtype}, {v.dtype}, {dout.dtype})")
-        if not (dq.dtype == dk.dtype == dv.dtype):
-            raise B200Error(6, f"attention_backward: dq, dk and dv dtypes differ ({dq.dtype}, {dk.dtype}, {dv.dtype})")
-        if lse.dtype != "f32" or not lse.is_contiguous() or list(lse.shape) != list(q.shape[:3]):
-            raise B200Error(6, f"attention_backward: lse must be a compact f32 [B, Hq, Sq] = {list(q.shape[:3])} tensor")
-        sc = 1.0 / math.sqrt(q.shape[3]) if scale is None else float(scale)
-        for _, t in named + (("lse", lse),):
-            t.handle.used_on(stream)
-        args = _ffi.AttentionArgs(sc, 1 if causal else 0)
-        ops = []
-        for t in (q, k, v, out, dout):
-            ops += [C.c_uint64(t.handle.ptr), _ffi.u64_array(t.shape), _ffi.u64_array(t.strides)]
-        ops.append(C.c_uint64(lse.handle.ptr))
-        for t in (dq, dk, dv):
-            ops += [C.c_uint64(t.handle.ptr), _ffi.u64_array(t.shape), _ffi.u64_array(t.strides)]
-        _ffi.check(client._lib.b200_attention_backward(client._ctx, stream, DTYPES[q.dtype], DTYPES[out.dtype], DTYPES[dq.dtype], *ops,
-                                                       C.byref(args)))
-    except (B200Error, ValueError) as e:
-        client._defer(e if isinstance(e, B200Error) else B200Error(6, str(e)))
+    what = "attention_backward"
+    _check_rank(what, 4, (("q", q), ("k", k), ("v", v), ("out", out), ("dout", dout), ("dq", dq), ("dk", dk), ("dv", dv)),
+                " [B, H, S, D]")
+    _check_same_dtype(what, (("q", q), ("k", k), ("v", v), ("dout", dout)))
+    _check_same_dtype(what, (("dq", dq), ("dk", dk), ("dv", dv)))
+    _check_lse(what, lse, "[B, Hq, Sq]", q.shape[:3])
+    args = _ffi.AttentionArgs(_scale(scale, q.shape[3]), 1 if causal else 0)
+    _used_on(stream, q, k, v, out, dout, dq, dk, dv, lse)
+    _ffi.check(client._lib.b200_attention_backward(client._ctx, stream, DTYPES[q.dtype], DTYPES[out.dtype], DTYPES[dq.dtype],
+                                                   *_view_args((q, k, v, out, dout)), _ptr(lse), *_view_args((dq, dk, dv)),
+                                                   C.byref(args)))
 
 
 def launch_backward_alloc(client: ComputeClient, q: TensorHandle, k: TensorHandle, v: TensorHandle, out: TensorHandle,
@@ -137,13 +166,7 @@ def launch_backward_alloc(client: ComputeClient, q: TensorHandle, k: TensorHandl
     return dq, dk, dv
 
 
-def _view_args(tensors):
-    ops = []
-    for t in tensors:
-        ops += [C.c_uint64(t.handle.ptr), _ffi.u64_array(t.shape), _ffi.u64_array(t.strides)]
-    return ops
-
-
+@_defers_errors
 def launch_kvcache(client: ComputeClient, q: TensorHandle, k_cache: TensorHandle, v_cache: TensorHandle, cache_seqlens: TensorHandle,
                    out: TensorHandle, block_table: TensorHandle | None = None, scale: float | None = None, causal: bool = False,
                    lse: TensorHandle | None = None, stream=None) -> None:
@@ -152,31 +175,20 @@ def launch_kvcache(client: ComputeClient, q: TensorHandle, k_cache: TensorHandle
     block_table[b, j / page] (i32 [B, max_pages]; None: page b).  causal: bottom-right (query i sees j <= L_b - Sq + i).  scale
     defaults to 1 / sqrt(D); lse: an optional compact f32 [B, Hq, Sq] tensor.  Never raises for launch problems: errors are
     deferred to client.sync()."""
-    try:
-        for name, t in (("q", q), ("k_cache", k_cache), ("v_cache", v_cache), ("out", out)):
-            if len(t.shape) != 4:
-                raise B200Error(6, f"attention_kvcache: {name} must have rank 4, got rank {len(t.shape)}")
-        if not (q.dtype == k_cache.dtype == v_cache.dtype):
-            raise B200Error(6, f"attention_kvcache: q, k_cache and v_cache dtypes differ ({q.dtype}, {k_cache.dtype}, {v_cache.dtype})")
-        if cache_seqlens.dtype != "i32" or not cache_seqlens.is_contiguous() or list(cache_seqlens.shape) != [q.shape[0]]:
-            raise B200Error(6, f"attention_kvcache: cache_seqlens must be a compact i32 [B] = [{q.shape[0]}] tensor")
-        if block_table is not None and (block_table.dtype != "i32" or len(block_table.shape) != 2):
-            raise B200Error(6, "attention_kvcache: block_table must be an i32 [B, max_pages] tensor")
-        if lse is not None and (lse.dtype != "f32" or not lse.is_contiguous() or list(lse.shape) != list(q.shape[:3])):
-            raise B200Error(6, f"attention_kvcache: lse must be a compact f32 [B, Hq, Sq] = {list(q.shape[:3])} tensor")
-        sc = 1.0 / math.sqrt(q.shape[3]) if scale is None else float(scale)
-        extra = tuple(t for t in (block_table, lse) if t is not None)
-        for t in (q, k_cache, v_cache, cache_seqlens, out) + extra:
-            t.handle.used_on(stream)
-        args = _ffi.AttentionArgs(sc, 1 if causal else 0)
-        bt = ([C.c_uint64(block_table.handle.ptr), _ffi.u64_array(block_table.shape), _ffi.u64_array(block_table.strides)]
-              if block_table is not None else [C.c_uint64(0), None, None])
-        _ffi.check(client._lib.b200_attention_kvcache(
-            client._ctx, stream, DTYPES[q.dtype], DTYPES[out.dtype], *_view_args((q, k_cache, v_cache)), *bt,
-            C.c_uint64(cache_seqlens.handle.ptr), *_view_args((out,)), C.c_uint64(lse.handle.ptr if lse is not None else 0),
-            C.byref(args)))
-    except (B200Error, ValueError) as e:
-        client._defer(e if isinstance(e, B200Error) else B200Error(6, str(e)))
+    what = "attention_kvcache"
+    _check_rank(what, 4, (("q", q), ("k_cache", k_cache), ("v_cache", v_cache), ("out", out)))
+    _check_same_dtype(what, (("q", q), ("k_cache", k_cache), ("v_cache", v_cache)))
+    if cache_seqlens.dtype != "i32" or not cache_seqlens.is_contiguous() or list(cache_seqlens.shape) != [q.shape[0]]:
+        raise B200Error(6, f"{what}: cache_seqlens must be a compact i32 [B] = [{q.shape[0]}] tensor")
+    if block_table is not None and (block_table.dtype != "i32" or len(block_table.shape) != 2):
+        raise B200Error(6, f"{what}: block_table must be an i32 [B, max_pages] tensor")
+    _check_lse(what, lse, "[B, Hq, Sq]", q.shape[:3])
+    args = _ffi.AttentionArgs(_scale(scale, q.shape[3]), 1 if causal else 0)
+    _used_on(stream, q, k_cache, v_cache, cache_seqlens, out, block_table, lse)
+    bt = _view_args((block_table,)) if block_table is not None else [C.c_uint64(0), None, None]
+    _ffi.check(client._lib.b200_attention_kvcache(
+        client._ctx, stream, DTYPES[q.dtype], DTYPES[out.dtype], *_view_args((q, k_cache, v_cache)), *bt, _ptr(cache_seqlens),
+        *_view_args((out,)), _ptr(lse), C.byref(args)))
 
 
 def launch_kvcache_alloc(client: ComputeClient, q: TensorHandle, k_cache: TensorHandle, v_cache: TensorHandle,
@@ -191,26 +203,22 @@ def launch_kvcache_alloc(client: ComputeClient, q: TensorHandle, k_cache: Tensor
     return (out, lse) if return_lse else out
 
 
+@_defers_errors
 def kvcache_write(client: ComputeClient, k_new: TensorHandle, v_new: TensorHandle, k_cache: TensorHandle, v_cache: TensorHandle,
                   slot_mapping: TensorHandle, stream=None) -> None:
     """Enqueue the scatter of k_new, v_new [B, Snew, Hkv, D] into k_cache, v_cache [P, page, Hkv, D]: token t of sequence b goes
     to flat slot slot_mapping[b * Snew + t] (compact i32; page slot / page, row slot % page); negative slots are skipped.  Lengths
     stay with the caller.  Errors are deferred to client.sync()."""
-    try:
-        for name, t in (("k_new", k_new), ("v_new", v_new), ("k_cache", k_cache), ("v_cache", v_cache)):
-            if len(t.shape) != 4:
-                raise B200Error(6, f"kvcache_write: {name} must have rank 4, got rank {len(t.shape)}")
-        if not (k_new.dtype == v_new.dtype == k_cache.dtype == v_cache.dtype):
-            raise B200Error(6, "kvcache_write: k_new, v_new, k_cache and v_cache dtypes differ")
-        n = k_new.shape[0] * k_new.shape[1]
-        if slot_mapping.dtype != "i32" or not slot_mapping.is_contiguous() or math.prod(slot_mapping.shape) != n:
-            raise B200Error(6, f"kvcache_write: slot_mapping must be a compact i32 tensor of B * Snew = {n} slots")
-        for t in (k_new, v_new, k_cache, v_cache, slot_mapping):
-            t.handle.used_on(stream)
-        _ffi.check(client._lib.b200_kvcache_write(client._ctx, stream, DTYPES[k_cache.dtype], *_view_args((k_new, v_new, k_cache, v_cache)),
-                                                  C.c_uint64(slot_mapping.handle.ptr)))
-    except (B200Error, ValueError) as e:
-        client._defer(e if isinstance(e, B200Error) else B200Error(6, str(e)))
+    what = "kvcache_write"
+    named = (("k_new", k_new), ("v_new", v_new), ("k_cache", k_cache), ("v_cache", v_cache))
+    _check_rank(what, 4, named)
+    _check_same_dtype(what, named, listed=False)
+    n = k_new.shape[0] * k_new.shape[1]
+    if slot_mapping.dtype != "i32" or not slot_mapping.is_contiguous() or math.prod(slot_mapping.shape) != n:
+        raise B200Error(6, f"{what}: slot_mapping must be a compact i32 tensor of B * Snew = {n} slots")
+    _used_on(stream, k_new, v_new, k_cache, v_cache, slot_mapping)
+    _ffi.check(client._lib.b200_kvcache_write(client._ctx, stream, DTYPES[k_cache.dtype], *_view_args((k_new, v_new, k_cache, v_cache)),
+                                              _ptr(slot_mapping)))
 
 
 def _varlen_args(q, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, scale, window_size, what):
@@ -218,10 +226,10 @@ def _varlen_args(q, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, scal
             or len(cu_seqlens_q.shape) != 1 or list(cu_seqlens_k.shape) != list(cu_seqlens_q.shape) or cu_seqlens_q.shape[0] < 1:
         raise B200Error(6, f"{what}: cu_seqlens_q and cu_seqlens_k must be compact i32 [B + 1] tensors of one length")
     left, right = (int(w) for w in window_size)
-    sc = 1.0 / math.sqrt(q.shape[2]) if scale is None else float(scale)
-    return _ffi.AttentionVarlenArgs(sc, left, right, int(max_seqlen_q), int(max_seqlen_k)), cu_seqlens_q.shape[0] - 1
+    return _ffi.AttentionVarlenArgs(_scale(scale, q.shape[2]), left, right, int(max_seqlen_q), int(max_seqlen_k)), cu_seqlens_q.shape[0] - 1
 
 
+@_defers_errors
 def launch_varlen(client: ComputeClient, q: TensorHandle, k: TensorHandle, v: TensorHandle, cu_seqlens_q: TensorHandle,
                   cu_seqlens_k: TensorHandle, max_seqlen_q: int, max_seqlen_k: int, out: TensorHandle, scale: float | None = None,
                   window_size=(-1, -1), lse: TensorHandle | None = None, stream=None) -> None:
@@ -230,23 +238,15 @@ def launch_varlen(client: ComputeClient, q: TensorHandle, k: TensorHandle, v: Te
     window_size (left, right), -1 unbounded: (-1, 0) is bottom-right causal.  scale defaults to 1 / sqrt(D); lse: an optional
     compact f32 [Hq, Tq] tensor.  Rows outside every sequence are not written.  Never raises for launch problems: errors are
     deferred to client.sync()."""
-    try:
-        for name, t in (("q", q), ("k", k), ("v", v), ("out", out)):
-            if len(t.shape) != 3:
-                raise B200Error(6, f"attention_varlen: {name} must have rank 3 [T, H, D], got rank {len(t.shape)}")
-        if not (q.dtype == k.dtype == v.dtype):
-            raise B200Error(6, f"attention_varlen: q, k and v dtypes differ ({q.dtype}, {k.dtype}, {v.dtype})")
-        if lse is not None and (lse.dtype != "f32" or not lse.is_contiguous() or list(lse.shape) != [q.shape[1], q.shape[0]]):
-            raise B200Error(6, f"attention_varlen: lse must be a compact f32 [Hq, Tq] = {[q.shape[1], q.shape[0]]} tensor")
-        args, B = _varlen_args(q, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, scale, window_size, "attention_varlen")
-        for t in (q, k, v, cu_seqlens_q, cu_seqlens_k, out) + ((lse,) if lse is not None else ()):
-            t.handle.used_on(stream)
-        _ffi.check(client._lib.b200_attention_varlen(
-            client._ctx, stream, DTYPES[q.dtype], DTYPES[out.dtype], *_view_args((q, k, v)), C.c_uint64(cu_seqlens_q.handle.ptr),
-            C.c_uint64(cu_seqlens_k.handle.ptr), C.c_uint64(B), *_view_args((out,)),
-            C.c_uint64(lse.handle.ptr if lse is not None else 0), C.byref(args)))
-    except (B200Error, ValueError) as e:
-        client._defer(e if isinstance(e, B200Error) else B200Error(6, str(e)))
+    what = "attention_varlen"
+    _check_rank(what, 3, (("q", q), ("k", k), ("v", v), ("out", out)), " [T, H, D]")
+    _check_same_dtype(what, (("q", q), ("k", k), ("v", v)))
+    _check_lse(what, lse, "[Hq, Tq]", [q.shape[1], q.shape[0]])
+    args, B = _varlen_args(q, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, scale, window_size, what)
+    _used_on(stream, q, k, v, cu_seqlens_q, cu_seqlens_k, out, lse)
+    _ffi.check(client._lib.b200_attention_varlen(
+        client._ctx, stream, DTYPES[q.dtype], DTYPES[out.dtype], *_view_args((q, k, v)), _ptr(cu_seqlens_q), _ptr(cu_seqlens_k),
+        C.c_uint64(B), *_view_args((out,)), _ptr(lse), C.byref(args)))
 
 
 def launch_varlen_alloc(client: ComputeClient, q: TensorHandle, k: TensorHandle, v: TensorHandle, cu_seqlens_q: TensorHandle,
@@ -261,6 +261,7 @@ def launch_varlen_alloc(client: ComputeClient, q: TensorHandle, k: TensorHandle,
     return (out, lse) if return_lse else out
 
 
+@_defers_errors
 def launch_varlen_backward(client: ComputeClient, q: TensorHandle, k: TensorHandle, v: TensorHandle, out: TensorHandle,
                            dout: TensorHandle, lse: TensorHandle, cu_seqlens_q: TensorHandle, cu_seqlens_k: TensorHandle,
                            max_seqlen_q: int, max_seqlen_k: int, dq: TensorHandle, dk: TensorHandle, dv: TensorHandle,
@@ -268,27 +269,16 @@ def launch_varlen_backward(client: ComputeClient, q: TensorHandle, k: TensorHand
     """Enqueue the varlen backward: dq [Tq, Hq, D], dk and dv [Tk, Hkv, D] (one grad dtype: the input dtype or f32) from q, k, v,
     the forward's out and lse (compact f32 [Hq, Tq]) and dout.  Offsets, scale and window_size must be the forward's.  Rows
     outside every sequence are not written.  Never raises for launch problems: errors are deferred to client.sync()."""
-    try:
-        named = (("q", q), ("k", k), ("v", v), ("out", out), ("dout", dout), ("dq", dq), ("dk", dk), ("dv", dv))
-        for name, t in named:
-            if len(t.shape) != 3:
-                raise B200Error(6, f"attention_varlen_backward: {name} must have rank 3 [T, H, D], got rank {len(t.shape)}")
-        if not (q.dtype == k.dtype == v.dtype == dout.dtype):
-            raise B200Error(6, f"attention_varlen_backward: q, k, v and dout dtypes differ ({q.dtype}, {k.dtype}, {v.dtype}, {dout.dtype})")
-        if not (dq.dtype == dk.dtype == dv.dtype):
-            raise B200Error(6, f"attention_varlen_backward: dq, dk and dv dtypes differ ({dq.dtype}, {dk.dtype}, {dv.dtype})")
-        if lse.dtype != "f32" or not lse.is_contiguous() or list(lse.shape) != [q.shape[1], q.shape[0]]:
-            raise B200Error(6, f"attention_varlen_backward: lse must be a compact f32 [Hq, Tq] = {[q.shape[1], q.shape[0]]} tensor")
-        args, B = _varlen_args(q, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, scale, window_size,
-                               "attention_varlen_backward")
-        for _, t in named + (("lse", lse), ("cu_seqlens_q", cu_seqlens_q), ("cu_seqlens_k", cu_seqlens_k)):
-            t.handle.used_on(stream)
-        _ffi.check(client._lib.b200_attention_varlen_backward(
-            client._ctx, stream, DTYPES[q.dtype], DTYPES[out.dtype], DTYPES[dq.dtype], *_view_args((q, k, v, out, dout)),
-            C.c_uint64(lse.handle.ptr), C.c_uint64(cu_seqlens_q.handle.ptr), C.c_uint64(cu_seqlens_k.handle.ptr), C.c_uint64(B),
-            *_view_args((dq, dk, dv)), C.byref(args)))
-    except (B200Error, ValueError) as e:
-        client._defer(e if isinstance(e, B200Error) else B200Error(6, str(e)))
+    what = "attention_varlen_backward"
+    _check_rank(what, 3, (("q", q), ("k", k), ("v", v), ("out", out), ("dout", dout), ("dq", dq), ("dk", dk), ("dv", dv)), " [T, H, D]")
+    _check_same_dtype(what, (("q", q), ("k", k), ("v", v), ("dout", dout)))
+    _check_same_dtype(what, (("dq", dq), ("dk", dk), ("dv", dv)))
+    _check_lse(what, lse, "[Hq, Tq]", [q.shape[1], q.shape[0]])
+    args, B = _varlen_args(q, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, scale, window_size, what)
+    _used_on(stream, q, k, v, out, dout, dq, dk, dv, lse, cu_seqlens_q, cu_seqlens_k)
+    _ffi.check(client._lib.b200_attention_varlen_backward(
+        client._ctx, stream, DTYPES[q.dtype], DTYPES[out.dtype], DTYPES[dq.dtype], *_view_args((q, k, v, out, dout)), _ptr(lse),
+        _ptr(cu_seqlens_q), _ptr(cu_seqlens_k), C.c_uint64(B), *_view_args((dq, dk, dv)), C.byref(args)))
 
 
 def launch_varlen_backward_alloc(client: ComputeClient, q: TensorHandle, k: TensorHandle, v: TensorHandle, out: TensorHandle,

@@ -4188,15 +4188,243 @@ static int encode_tmap4(b200_ctx* c, CUtensorMap* out, CUtensorMapDataType dt, s
   return B200_OK;
 }
 
-// A [B, H, S, D] view (normalised strides ns, in elements) a tensor map reads in place: unit D stride, 16-byte aligned base and
-// S, H, B strides below 2^40 bytes.
-static bool attn_view_ok(uint64_t ptr, size_t esz, const uint64_t* ns) {
-  if (ptr % 16 || ns[3] != 1) return false;
+// An attention operand: the device pointer and dtype, the 4-D shape and normalised strides (elements) as the caller passed
+// them, and which axes a tensor map reads as rows (S, T or a page's keys) and as heads.  Axis 3 is D, the map's innermost
+// dimension, and axis 0 (B, a varlen tensor's unit batch, or the page) its outermost.
+struct AttnView {
+  uint64_t ptr;
+  b200_dtype dt;
+  size_t esz;
+  uint64_t shape[4], ns[4];
+  int row, head;
+  uint64_t rows() const { return shape[row]; }
+  uint64_t heads() const { return shape[head]; }
+  uint64_t s_row() const { return ns[row]; }
+  uint64_t s_head() const { return ns[head]; }
+  uint64_t s_batch() const { return ns[0]; }
+};
+
+// [B, H, S, D] (dense q, k, v, out and grads); [B or P, S or page, H, D] (KV caches and new tokens); a varlen [T, H, D] (strides
+// null: compact), seen as [1, T, H, D].
+enum AttnLayout { kAttnBHSD, kAttnBSHD, kAttnTHD };
+
+static AttnView attn_view(uint64_t ptr, b200_dtype dt, const uint64_t* shape, const uint64_t* strides, AttnLayout layout) {
+  AttnView v{};
+  v.ptr = ptr; v.dt = dt; v.esz = dtype_size(dt);
+  const bool thd = layout == kAttnTHD;
+  uint64_t st3[4] = {0, 0, 0, 0};
+  if (thd && strides) memcpy(st3 + 1, strides, 3 * sizeof(uint64_t));
+  for (int d = 0; d < 4; ++d) v.shape[d] = !thd ? shape[d] : d ? shape[d - 1] : 1;
+  conv_norm_strides(v.shape, thd && strides ? st3 : strides, v.ns);
+  v.row = layout == kAttnBHSD ? 2 : 1;
+  v.head = layout == kAttnBHSD ? 1 : 2;
+  return v;
+}
+
+// A view a tensor map (or the 16-byte loads of the delta and cache-write kernels) reads in place: unit D stride, 16-byte
+// aligned base, and the other strides 16-byte multiples below 2^40 bytes.
+static bool attn_view_ok(const AttnView& v) {
+  if (v.ptr % 16 || v.ns[3] != 1) return false;
   for (int d = 0; d < 3; ++d)
-    if ((ns[d] * esz) % 16 || ns[d] * esz >= (1ull << 40)) return false;
+    if ((v.ns[d] * v.esz) % 16 || v.ns[d] * v.esz >= (1ull << 40)) return false;
   return true;
 }
 
+// v in place when attn_view_ok, else gathered into a compact pooled copy *tmp (the caller frees it) that v then describes.
+static int attn_stage(b200_ctx* c, CUstream st, AttnView* v, CUdeviceptr* tmp) {
+  if (attn_view_ok(*v)) return B200_OK;
+  const uint64_t* sh = v->shape;
+  int rc = pool_alloc(c, sh[0] * sh[1] * sh[2] * sh[3] * v->esz, tmp, st);
+  if (rc) return rc;
+  rc = b200_into_contiguous(c, static_cast<b200_stream>(st), v->dt, v->ptr, *tmp, 4, sh, v->ns);
+  v->ptr = *tmp;
+  v->ns[3] = 1; v->ns[2] = sh[3]; v->ns[1] = sh[2] * sh[3]; v->ns[0] = sh[1] * sh[2] * sh[3];
+  return rc;
+}
+
+// The 128-byte swizzled map of v with dims (D, rows, heads, axis 0).  A load (box 64 x rows x heads) reads the input dtype; a
+// store (out and the grads: 128-byte x 64-row boxes) moves raw 16- or 32-bit words.
+static int attn_map(b200_ctx* c, CUtensorMap* m, const AttnView& v, bool store, uint32_t rows = 64, uint32_t heads = 1) {
+  const CUtensorMapDataType dt = v.esz == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                 : store    ? CU_TENSOR_MAP_DATA_TYPE_UINT16
+                                 : v.dt == B200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  const uint32_t box[4] = {store ? (uint32_t)(128 / v.esz) : 64u, rows, heads, 1};
+  const uint64_t dims[4] = {v.shape[3], v.rows(), v.heads(), v.shape[0]}, strides[3] = {v.s_row(), v.s_head(), v.s_batch()};
+  return encode_tmap4(c, m, dt, v.esz, v.ptr, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
+}
+
+static int attn_set_smem(b200_ctx* c, CUfunction f, unsigned smem) {
+  if (c->dry) return B200_OK;
+  CUresult r = g_drv.cuFuncSetAttribute_p(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem);
+  return r != CUDA_SUCCESS ? fail(map_cu(r), "cuFuncSetAttribute: %s", cu_err(r)) : B200_OK;
+}
+
+// The head-dim bucket the kernels are instantiated for, and the kernels' f32 scale * log2(e).
+static uint32_t attn_db(uint64_t D) { return D <= 64 ? 64 : 128; }
+static float attn_scale_log2(float scale) { return (float)((double)scale * 1.4426950408889634074); }
+
+static std::string attn_dims(const uint64_t* s, int rank) {
+  std::string r = "[";
+  for (int d = 0; d < rank; ++d) r += (d ? "," : "") + std::to_string(s[d]);
+  return r + "]";
+}
+
+// ---- checks the attention entry points share; what: the entry point, for messages
+static int attn_check_in_dtype(const char* what, b200_dtype in) {
+  if (in != B200_F16 && in != B200_BF16) return fail(B200_ERR_UNSUPPORTED, "%s: input dtype %d unsupported (f16, bf16)", what, (int)in);
+  return B200_OK;
+}
+
+// out ("output") or the grads ("grad"): the input dtype or f32.
+static int attn_check_out_dtype(const char* what, const char* name, b200_dtype in, b200_dtype dt) {
+  if (dt != in && dt != B200_F32) return fail(B200_ERR_UNSUPPORTED, "%s: %s dtype must equal the input dtype or be f32", what, name);
+  return B200_OK;
+}
+
+// v equals k but for the head dim, which must be k's.
+static int attn_check_v(const char* what, const char* k_name, const char* v_name, const uint64_t* k, const uint64_t* v, int rank) {
+  if (memcmp(v, k, (rank - 1) * sizeof(uint64_t)))
+    return fail(B200_ERR_INVALID_ARG, "%s: %s %s does not match %s %s", what, v_name, attn_dims(v, rank).c_str(), k_name,
+                attn_dims(k, rank).c_str());
+  if (v[rank - 1] != k[rank - 1])
+    return fail(B200_ERR_UNSUPPORTED, "%s: %s's head dim %llu differs from D = %llu", what, v_name, (unsigned long long)v[rank - 1],
+                (unsigned long long)k[rank - 1]);
+  return B200_OK;
+}
+
+static int attn_check_gqa(const char* what, uint64_t Hq, uint64_t Hkv) {
+  if (Hkv == 0 || Hq % Hkv)
+    return fail(B200_ERR_INVALID_ARG, "%s: Hq = %llu must be a multiple of Hkv = %llu", what, (unsigned long long)Hq, (unsigned long long)Hkv);
+  return B200_OK;
+}
+
+// Each named shape must equal its `want`.
+struct AttnSame {
+  const char* name;
+  const uint64_t *shape, *want;
+};
+static int attn_check_same(const char* what, int rank, std::initializer_list<AttnSame> same) {
+  for (const AttnSame& t : same)
+    if (memcmp(t.shape, t.want, rank * sizeof(uint64_t)))
+      return fail(B200_ERR_INVALID_ARG, "%s: %s is %s, expected %s", what, t.name, attn_dims(t.shape, rank).c_str(), attn_dims(t.want, rank).c_str());
+  return B200_OK;
+}
+
+static int attn_check_scale_d(const char* what, float scale, uint64_t D) {
+  if (!std::isfinite(scale)) return fail(B200_ERR_INVALID_ARG, "%s: scale must be finite", what);
+  if (D == 0 || D > 128 || D % 8)
+    return fail(B200_ERR_UNSUPPORTED, "%s: head dim D = %llu unsupported (a multiple of 8 in [8, 128])", what, (unsigned long long)D);
+  return B200_OK;
+}
+
+static int attn_check_extents(const char* what, std::initializer_list<uint64_t> extents) {
+  for (uint64_t e : extents)
+    if (e >= (1ull << 31)) return fail(B200_ERR_UNSUPPORTED, "%s: extents must be < 2^31", what);
+  return B200_OK;
+}
+
+// out or a grad (name), written in place.
+static int attn_check_out_view(const char* what, const char* name, const AttnView& v) {
+  if (attn_view_ok(v)) return B200_OK;
+  return fail(B200_ERR_UNSUPPORTED, "%s: %s needs a unit D stride and a 16-byte aligned base and %s strides", what, name,
+              v.row == 2 ? "S, H, B" : "T, H");
+}
+
+static int attn_check_caches(const char* what, const AttnView& kc, const AttnView& vc) {
+  if (attn_view_ok(kc) && attn_view_ok(vc)) return B200_OK;
+  return fail(B200_ERR_UNSUPPORTED, "%s: a cache needs a unit D stride and a 16-byte aligned base and page, row and head strides "
+              "(it is read in place, never gathered)", what);
+}
+
+// ---- launch sequences the dense and varlen entry points share
+// Stages q, k and v, maps them (loads of kAttnBlock rows) and out, then launches `<prefix><in>_d<DB>_<out>` on `ctas` CTAs
+// with the filled parameter block p.
+static int attn_fwd_launch(b200_ctx* c, CUstream st, const std::string& prefix, AttnView q, AttnView k, AttnView v, const AttnView& o,
+                           uint64_t ctas, void* p) {
+  CUdeviceptr tmp[3] = {0, 0, 0};
+  int rc = attn_stage(c, st, &q, &tmp[0]);
+  if (!rc) rc = attn_stage(c, st, &k, &tmp[1]);
+  if (!rc) rc = attn_stage(c, st, &v, &tmp[2]);
+  CUtensorMap mq, mk, mv, mo;
+  if (!rc) rc = attn_map(c, &mq, q, false, kAttnBlock);
+  if (!rc) rc = attn_map(c, &mk, k, false, kAttnBlock);
+  if (!rc) rc = attn_map(c, &mv, v, false, kAttnBlock);
+  if (!rc) rc = attn_map(c, &mo, o, true);
+  const uint32_t DB = attn_db(q.shape[3]);
+  CUfunction f = nullptr;
+  if (!rc) rc = get_func(c, prefix + dt_tag(q.dt) + "_d" + std::to_string(DB) + "_" + dt_tag(o.dt), &f);
+  const unsigned smem = 1024 + (1 + 2 * kAttnStages) * kAttnBlock * DB * 2 + 1024;
+  if (!rc) rc = attn_set_smem(c, f, smem);
+  void* kargs[] = {&mq, &mk, &mv, &mo, p};
+  if (!rc) rc = launch(c, f, (unsigned)ctas, 1, 1, 384, smem, 1, st, kargs);
+  for (CUdeviceptr t : tmp)
+    if (t) pool_free(c, t, st);   // stream-ordered: reusable once the kernel has drained
+  return rc;
+}
+
+struct AttnBwdOps {
+  AttnView q, k, v, out, dout, dq, dk, dv;
+};
+
+// Stages what the present sides read: q, out and dout with query rows (has_q), k and v with keys (has_k); tmp[0..4] receive
+// the copies (the caller frees them).
+static int attn_bwd_stage(b200_ctx* c, CUstream st, AttnBwdOps* o, bool has_q, bool has_k, CUdeviceptr tmp[5]) {
+  int rc = has_q ? attn_stage(c, st, &o->q, &tmp[0]) : B200_OK;
+  if (!rc && has_k) rc = attn_stage(c, st, &o->k, &tmp[1]);
+  if (!rc && has_k) rc = attn_stage(c, st, &o->v, &tmp[2]);
+  if (!rc && has_q) rc = attn_stage(c, st, &o->out, &tmp[3]);
+  if (!rc && has_q) rc = attn_stage(c, st, &o->dout, &tmp[4]);
+  return rc;
+}
+
+// With query rows: `<prefix>delta_*` (delta and L into the workspace) and `<prefix>dq_*` on q_ctas CTAs; with keys:
+// `<prefix>dkdv_*` on k_ctas CTAs.  A side that is absent is never read, so its maps take the other side's views.  p: the
+// kernels' filled parameter block, workspace included.
+static int attn_bwd_launch(b200_ctx* c, CUstream st, const std::string& prefix, AttnBwdOps o, bool has_q, bool has_k, uint64_t q_ctas,
+                           uint64_t k_ctas, void* p) {
+  if (!has_k) o.k = o.v = o.q;
+  if (!has_q) o.q = o.dout = o.k;
+  const uint32_t DB = attn_db(o.q.shape[3]);
+  const std::string in = dt_tag(o.q.dt), tail = "_d" + std::to_string(DB) + "_" + dt_tag(o.dq.dt);
+  CUfunction f = nullptr;
+  int rc = B200_OK;
+  if (has_q) {   // one 256-thread block per 16 workspace rows
+    rc = get_func(c, prefix + "delta_" + in + "_" + dt_tag(o.out.dt), &f);
+    void* kargs[] = {p};
+    if (!rc) rc = launch(c, f, (unsigned)(q_ctas * (kAttnBlock / 16)), 1, 1, 256, 0, 1, st, kargs);
+  }
+  if (!rc && has_q) {   // dq: query tiles of kAttnBlock rows, key tiles of kAttnBwdDqKeys
+    CUtensorMap mq, mk, mv, mdo, mdq;
+    rc = attn_map(c, &mq, o.q, false, kAttnBlock);
+    if (!rc) rc = attn_map(c, &mk, o.k, false, kAttnBwdDqKeys);
+    if (!rc) rc = attn_map(c, &mv, o.v, false, kAttnBwdDqKeys);
+    if (!rc) rc = attn_map(c, &mdo, o.dout, false, kAttnBlock);
+    if (!rc) rc = attn_map(c, &mdq, o.dq, true);
+    if (!rc) rc = get_func(c, prefix + "dq_" + in + tail, &f);
+    const unsigned smem = 1024 + 2 * kAttnBlock * DB * 2 + 2 * kAttnBwdStages * kAttnBwdDqKeys * DB * 2 + 1024;
+    if (!rc) rc = attn_set_smem(c, f, smem);
+    void* kargs[] = {&mq, &mk, &mv, &mdo, &mdq, p};
+    if (!rc) rc = launch(c, f, (unsigned)q_ctas, 1, 1, 384, smem, 1, st, kargs);
+  }
+  if (!rc && has_k) {   // dk and dv: query tiles of kAttnBwdDkdvQueries rows, key tiles of kAttnBlock
+    CUtensorMap mq, mk, mv, mdo, mdk, mdv;
+    rc = attn_map(c, &mq, o.q, false, kAttnBwdDkdvQueries);
+    if (!rc) rc = attn_map(c, &mk, o.k, false, kAttnBlock);
+    if (!rc) rc = attn_map(c, &mv, o.v, false, kAttnBlock);
+    if (!rc) rc = attn_map(c, &mdo, o.dout, false, kAttnBwdDkdvQueries);
+    if (!rc) rc = attn_map(c, &mdk, o.dk, true);
+    if (!rc) rc = attn_map(c, &mdv, o.dv, true);
+    if (!rc) rc = get_func(c, prefix + "dkdv_" + in + tail, &f);
+    const unsigned smem = 1024 + 2 * kAttnBlock * DB * 2 + 2 * kAttnBwdStages * kAttnBwdDkdvQueries * DB * 2 +
+                          kAttnBwdStages * 2 * kAttnBwdDkdvQueries * 4 + 1024;
+    if (!rc) rc = attn_set_smem(c, f, smem);
+    void* kargs[] = {&mq, &mk, &mv, &mdo, &mdk, &mdv, p};
+    if (!rc) rc = launch(c, f, (unsigned)k_ctas, 1, 1, 384, smem, 1, st, kargs);
+  }
+  return rc;
+}
+
+// ------------------------------------------------------------------------------------------------ dense attention
 extern "C" int b200_attention(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr q, const uint64_t* q_shape,
                               const uint64_t* q_strides, b200_dptr k, const uint64_t* k_shape, const uint64_t* k_strides, b200_dptr v,
                               const uint64_t* v_shape, const uint64_t* v_strides, b200_dptr out, const uint64_t* out_shape,
@@ -4204,101 +4432,41 @@ extern "C" int b200_attention(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b
   CTX_ENTER(c);
   const char* what = "attention";
   if (!q_shape || !k_shape || !v_shape || !out_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
-  if (in_dtype != B200_F16 && in_dtype != B200_BF16)
-    return fail(B200_ERR_UNSUPPORTED, "%s: input dtype %d unsupported (f16, bf16)", what, (int)in_dtype);
-  if (out_dtype != in_dtype && out_dtype != B200_F32)
-    return fail(B200_ERR_UNSUPPORTED, "%s: output dtype must equal the input dtype or be f32", what);
+  int rc = attn_check_in_dtype(what, in_dtype);
+  if (!rc) rc = attn_check_out_dtype(what, "output", in_dtype, out_dtype);
+  if (rc) return rc;
   const uint64_t B = q_shape[0], Hq = q_shape[1], Sq = q_shape[2], D = q_shape[3];
   const uint64_t Hkv = k_shape[1], Sk = k_shape[2];
   if (k_shape[0] != B || k_shape[3] != D)
-    return fail(B200_ERR_INVALID_ARG, "%s: k [%llu,%llu,%llu,%llu] differs from q [%llu,%llu,%llu,%llu] in batch or head dim", what,
-                (unsigned long long)k_shape[0], (unsigned long long)Hkv, (unsigned long long)Sk, (unsigned long long)k_shape[3],
-                (unsigned long long)B, (unsigned long long)Hq, (unsigned long long)Sq, (unsigned long long)D);
-  if (v_shape[0] != B || v_shape[1] != Hkv || v_shape[2] != Sk)
-    return fail(B200_ERR_INVALID_ARG, "%s: v [%llu,%llu,%llu,%llu] does not match k [%llu,%llu,%llu,%llu]", what, (unsigned long long)v_shape[0],
-                (unsigned long long)v_shape[1], (unsigned long long)v_shape[2], (unsigned long long)v_shape[3], (unsigned long long)B,
-                (unsigned long long)Hkv, (unsigned long long)Sk, (unsigned long long)D);
-  if (v_shape[3] != D) return fail(B200_ERR_UNSUPPORTED, "%s: v's head dim %llu differs from D = %llu", what, (unsigned long long)v_shape[3], (unsigned long long)D);
-  if (Hkv == 0 || Hq % Hkv)
-    return fail(B200_ERR_INVALID_ARG, "%s: Hq = %llu must be a multiple of Hkv = %llu", what, (unsigned long long)Hq, (unsigned long long)Hkv);
-  if (out_shape[0] != B || out_shape[1] != Hq || out_shape[2] != Sq || out_shape[3] != D)
-    return fail(B200_ERR_INVALID_ARG, "%s: out is [%llu,%llu,%llu,%llu], expected [%llu,%llu,%llu,%llu]", what, (unsigned long long)out_shape[0],
-                (unsigned long long)out_shape[1], (unsigned long long)out_shape[2], (unsigned long long)out_shape[3], (unsigned long long)B,
-                (unsigned long long)Hq, (unsigned long long)Sq, (unsigned long long)D);
-  if (Sk == 0 && Sq > 0) return fail(B200_ERR_INVALID_ARG, "%s: Sk = 0 leaves every query row without keys", what);
-  if (!std::isfinite(args->scale)) return fail(B200_ERR_INVALID_ARG, "%s: scale must be finite", what);
-  if (D == 0 || D > 128 || D % 8)
-    return fail(B200_ERR_UNSUPPORTED, "%s: head dim D = %llu unsupported (a multiple of 8 in [8, 128])", what, (unsigned long long)D);
-  const uint64_t lim = 1ull << 31;
-  if (B >= lim || Hq >= lim || Sq >= lim || Hkv >= lim || Sk >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: extents must be < 2^31", what);
+    return fail(B200_ERR_INVALID_ARG, "%s: k %s differs from q %s in batch or head dim", what, attn_dims(k_shape, 4).c_str(),
+                attn_dims(q_shape, 4).c_str());
+  rc = attn_check_v(what, "k", "v", k_shape, v_shape, 4);
+  if (!rc) rc = attn_check_gqa(what, Hq, Hkv);
+  if (!rc) rc = attn_check_same(what, 4, {{"out", out_shape, q_shape}});
+  if (!rc && Sk == 0 && Sq > 0) rc = fail(B200_ERR_INVALID_ARG, "%s: Sk = 0 leaves every query row without keys", what);
+  if (!rc) rc = attn_check_scale_d(what, args->scale, D);
+  if (!rc) rc = attn_check_extents(what, {B, Hq, Sq, Hkv, Sk});
+  if (rc) return rc;
   if (B == 0 || Hq == 0 || Sq == 0) return B200_OK;
   const uint64_t nqb = (Sq + kAttnBlock - 1) / kAttnBlock, ctas = nqb * Hq * B;
-  if (ctas >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: ceil(Sq / %d) * Hq * B = %llu CTAs must be < 2^31", what, kAttnBlock, (unsigned long long)ctas);
+  if (ctas >= (1ull << 31))
+    return fail(B200_ERR_UNSUPPORTED, "%s: ceil(Sq / %d) * Hq * B = %llu CTAs must be < 2^31", what, kAttnBlock, (unsigned long long)ctas);
   if (!q || !k || !v || !out) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
   if (lse % 4) return fail(B200_ERR_INVALID_ARG, "%s: lse pointer is not 4-byte aligned", what);
-  const size_t osz = dtype_size(out_dtype);
-  uint64_t qs[4], ks[4], vs[4], os[4];
-  conv_norm_strides(out_shape, out_strides, os);
-  if (!attn_view_ok(out, osz, os))
-    return fail(B200_ERR_UNSUPPORTED, "%s: out needs a unit D stride and a 16-byte aligned base and S, H, B strides", what);
-  conv_norm_strides(q_shape, q_strides, qs);
-  conv_norm_strides(k_shape, k_strides, ks);
-  conv_norm_strides(v_shape, v_strides, vs);
+  const AttnView ov = attn_view(out, out_dtype, out_shape, out_strides, kAttnBHSD);
+  if ((rc = attn_check_out_view(what, "out", ov))) return rc;
 
-  CUstream st = resolve_stream(c, s);
-  CUdeviceptr tmp[3] = {0, 0, 0};
-  // each operand in place, or gathered into a compact [B, H, S, D] copy
-  auto prep = [&](int i, uint64_t ptr, const uint64_t* shape, uint64_t* ns, uint64_t* use) -> int {
-    *use = ptr;
-    if (attn_view_ok(ptr, 2, ns)) return B200_OK;
-    int rc = conv_gather(c, st, in_dtype, ptr, shape, ns, &tmp[i]);
-    *use = tmp[i];
-    ns[3] = 1; ns[2] = shape[3]; ns[1] = shape[2] * shape[3]; ns[0] = shape[1] * shape[2] * shape[3];
-    return rc;
-  };
-  uint64_t qp = 0, kp = 0, vp = 0;
-  int rc = prep(0, q, q_shape, qs, &qp);
-  if (!rc) rc = prep(1, k, k_shape, ks, &kp);
-  if (!rc) rc = prep(2, v, v_shape, vs, &vp);
-  if (!rc) {
-    const uint32_t DB = D <= 64 ? 64 : 128;
-    const CUtensorMapDataType dt = in_dtype == B200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-    CUtensorMap mq, mk, mv, mo;
-    const uint32_t box_in[4] = {64, (uint32_t)kAttnBlock, 1, 1};
-    const uint32_t box_out[4] = {(uint32_t)(128 / osz), 64, 1, 1};
-    const uint64_t dq[4] = {D, Sq, Hq, B}, dk[4] = {D, Sk, Hkv, B};
-    const uint64_t sq[3] = {qs[2], qs[1], qs[0]}, sk[3] = {ks[2], ks[1], ks[0]}, sv[3] = {vs[2], vs[1], vs[0]}, so[3] = {os[2], os[1], os[0]};
-    rc = encode_tmap4(c, &mq, dt, 2, qp, dq, sq, box_in, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (!rc) rc = encode_tmap4(c, &mk, dt, 2, kp, dk, sk, box_in, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (!rc) rc = encode_tmap4(c, &mv, dt, 2, vp, dk, sv, box_in, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (!rc)
-      rc = encode_tmap4(c, &mo, osz == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_UINT16, osz, out, dq, so, box_out,
-                        CU_TENSOR_MAP_SWIZZLE_128B);
-    CUfunction f = nullptr;
-    const char* in_tag = dt_tag(in_dtype);
-    const std::string name = std::string("attn_fwd_") + in_tag + "_d" + std::to_string(DB) + "_" + dt_tag(out_dtype);
-    if (!rc) rc = get_func(c, name, &f);
-    const unsigned smem = 1024 + (1 + 2 * kAttnStages) * kAttnBlock * DB * 2 + 1024;
-    if (!rc && !c->dry) {
-      CUresult r = g_drv.cuFuncSetAttribute_p(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem);
-      if (r != CUDA_SUCCESS) rc = fail(map_cu(r), "cuFuncSetAttribute: %s", cu_err(r));
-    }
-    if (!rc) {
-      AttnParams p{};
-      p.lse = lse;
-      p.B = (uint32_t)B; p.Hq = (uint32_t)Hq; p.Sq = (uint32_t)Sq; p.Sk = (uint32_t)Sk;
-      p.group = (uint32_t)(Hq / Hkv);
-      p.nqb = (uint32_t)nqb;
-      p.causal = args->causal != 0 ? 1u : 0u;
-      p.D = (uint32_t)D;
-      p.scale_log2 = (float)((double)args->scale * 1.4426950408889634074);
-      void* kargs[] = {&mq, &mk, &mv, &mo, &p};
-      rc = launch(c, f, (unsigned)ctas, 1, 1, 384, smem, 1, st, kargs);
-    }
-  }
-  for (CUdeviceptr t : tmp)
-    if (t) pool_free(c, t, st);   // stream-ordered: reusable once the kernel has drained
-  return rc;
+  AttnParams p{};
+  p.lse = lse;
+  p.B = (uint32_t)B; p.Hq = (uint32_t)Hq; p.Sq = (uint32_t)Sq; p.Sk = (uint32_t)Sk;
+  p.group = (uint32_t)(Hq / Hkv);
+  p.nqb = (uint32_t)nqb;
+  p.causal = args->causal != 0 ? 1u : 0u;
+  p.D = (uint32_t)D;
+  p.scale_log2 = attn_scale_log2(args->scale);
+  return attn_fwd_launch(c, resolve_stream(c, s), "attn_fwd_", attn_view(q, in_dtype, q_shape, q_strides, kAttnBHSD),
+                         attn_view(k, in_dtype, k_shape, k_strides, kAttnBHSD), attn_view(v, in_dtype, v_shape, v_strides, kAttnBHSD), ov,
+                         ctas, &p);
 }
 
 // Backward of b200_attention (see cubecl_b200.h): the delta / L pass, then the dq and the dk / dv kernels.
@@ -4314,93 +4482,52 @@ extern "C" int b200_attention_backward(b200_ctx* c, b200_stream s, b200_dtype in
   const char* what = "attention_backward";
   if (!q_shape || !k_shape || !v_shape || !out_shape || !dout_shape || !dq_shape || !dk_shape || !dv_shape || !args)
     return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
-  if (in_dtype != B200_F16 && in_dtype != B200_BF16)
-    return fail(B200_ERR_UNSUPPORTED, "%s: input dtype %d unsupported (f16, bf16)", what, (int)in_dtype);
-  if (out_dtype != in_dtype && out_dtype != B200_F32)
-    return fail(B200_ERR_UNSUPPORTED, "%s: output dtype must equal the input dtype or be f32", what);
-  if (grad_dtype != in_dtype && grad_dtype != B200_F32)
-    return fail(B200_ERR_UNSUPPORTED, "%s: grad dtype must equal the input dtype or be f32", what);
+  int rc = attn_check_in_dtype(what, in_dtype);
+  if (!rc) rc = attn_check_out_dtype(what, "output", in_dtype, out_dtype);
+  if (!rc) rc = attn_check_out_dtype(what, "grad", in_dtype, grad_dtype);
+  if (rc) return rc;
   const uint64_t B = q_shape[0], Hq = q_shape[1], Sq = q_shape[2], D = q_shape[3];
   const uint64_t Hkv = k_shape[1], Sk = k_shape[2];
-  auto ull = [](uint64_t x) { return (unsigned long long)x; };
   if (k_shape[0] != B || k_shape[3] != D)
-    return fail(B200_ERR_INVALID_ARG, "%s: k [%llu,%llu,%llu,%llu] differs from q [%llu,%llu,%llu,%llu] in batch or head dim", what,
-                ull(k_shape[0]), ull(Hkv), ull(Sk), ull(k_shape[3]), ull(B), ull(Hq), ull(Sq), ull(D));
-  if (v_shape[0] != B || v_shape[1] != Hkv || v_shape[2] != Sk)
-    return fail(B200_ERR_INVALID_ARG, "%s: v [%llu,%llu,%llu,%llu] does not match k [%llu,%llu,%llu,%llu]", what, ull(v_shape[0]),
-                ull(v_shape[1]), ull(v_shape[2]), ull(v_shape[3]), ull(B), ull(Hkv), ull(Sk), ull(D));
-  if (v_shape[3] != D) return fail(B200_ERR_UNSUPPORTED, "%s: v's head dim %llu differs from D = %llu", what, ull(v_shape[3]), ull(D));
-  if (Hkv == 0 || Hq % Hkv) return fail(B200_ERR_INVALID_ARG, "%s: Hq = %llu must be a multiple of Hkv = %llu", what, ull(Hq), ull(Hkv));
-  const struct { const char* name; const uint64_t* shape; const uint64_t* want; } same[] = {
-      {"out", out_shape, q_shape}, {"dout", dout_shape, q_shape}, {"dq", dq_shape, q_shape}, {"dk", dk_shape, k_shape}, {"dv", dv_shape, k_shape}};
-  for (const auto& t : same)
-    if (memcmp(t.shape, t.want, 4 * sizeof(uint64_t)))
-      return fail(B200_ERR_INVALID_ARG, "%s: %s is [%llu,%llu,%llu,%llu], expected [%llu,%llu,%llu,%llu]", what, t.name, ull(t.shape[0]),
-                  ull(t.shape[1]), ull(t.shape[2]), ull(t.shape[3]), ull(t.want[0]), ull(t.want[1]), ull(t.want[2]), ull(t.want[3]));
-  if (Sk == 0 && Sq > 0) return fail(B200_ERR_INVALID_ARG, "%s: Sk = 0 leaves every query row without keys", what);
-  if (!std::isfinite(args->scale)) return fail(B200_ERR_INVALID_ARG, "%s: scale must be finite", what);
-  if (D == 0 || D > 128 || D % 8) return fail(B200_ERR_UNSUPPORTED, "%s: head dim D = %llu unsupported (a multiple of 8 in [8, 128])", what, ull(D));
-  const uint64_t lim = 1ull << 31;
-  if (B >= lim || Hq >= lim || Sq >= lim || Hkv >= lim || Sk >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: extents must be < 2^31", what);
+    return fail(B200_ERR_INVALID_ARG, "%s: k %s differs from q %s in batch or head dim", what, attn_dims(k_shape, 4).c_str(),
+                attn_dims(q_shape, 4).c_str());
+  rc = attn_check_v(what, "k", "v", k_shape, v_shape, 4);
+  if (!rc) rc = attn_check_gqa(what, Hq, Hkv);
+  if (!rc)
+    rc = attn_check_same(what, 4, {{"out", out_shape, q_shape}, {"dout", dout_shape, q_shape}, {"dq", dq_shape, q_shape},
+                                   {"dk", dk_shape, k_shape}, {"dv", dv_shape, k_shape}});
+  if (!rc && Sk == 0 && Sq > 0) rc = fail(B200_ERR_INVALID_ARG, "%s: Sk = 0 leaves every query row without keys", what);
+  if (!rc) rc = attn_check_scale_d(what, args->scale, D);
+  if (!rc) rc = attn_check_extents(what, {B, Hq, Sq, Hkv, Sk});
+  if (rc) return rc;
   // B = 0, or no queries and no keys: nothing to write.  Sq = 0 or Hq = 0 with keys still writes zero dk and dv.
   if (B == 0 || (Sk == 0 && Sq == 0)) return B200_OK;
   const uint64_t nqb = (Sq + kAttnBlock - 1) / kAttnBlock, nkb = (Sk + kAttnBlock - 1) / kAttnBlock;
   const uint64_t rows = B * Hq * nqb * kAttnBlock;   // workspace rows, padded per (b, h) to whole query blocks
   const bool has_q = rows > 0;
-  if (nqb * Hq * B >= lim || nkb * Hkv * B >= lim || rows / 16 >= lim)
-    return fail(B200_ERR_UNSUPPORTED, "%s: more than 2^31 - 1 CTAs", what);
+  const uint64_t lim = 1ull << 31;
+  if (nqb * Hq * B >= lim || nkb * Hkv * B >= lim || rows / 16 >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: more than 2^31 - 1 CTAs", what);
   if (!k || !v || !dk || !dv || (has_q && (!q || !out || !dout || !dq || !lse))) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
   if (lse % 4) return fail(B200_ERR_INVALID_ARG, "%s: lse pointer is not 4-byte aligned", what);
-  const size_t gsz = dtype_size(grad_dtype), osz = dtype_size(out_dtype);
-  uint64_t qs[4], ks[4], vs[4], os[4], dos[4], dqs[4], dks[4], dvs[4];
-  conv_norm_strides(dq_shape, dq_strides, dqs);
-  conv_norm_strides(dk_shape, dk_strides, dks);
-  conv_norm_strides(dv_shape, dv_strides, dvs);
-  const struct { const char* name; uint64_t ptr; const uint64_t* ns; bool used; } grads[] = {
-      {"dq", dq, dqs, has_q}, {"dk", dk, dks, true}, {"dv", dv, dvs, true}};
-  for (const auto& g : grads)
-    if (g.used && !attn_view_ok(g.ptr, gsz, g.ns))
-      return fail(B200_ERR_UNSUPPORTED, "%s: %s needs a unit D stride and a 16-byte aligned base and S, H, B strides", what, g.name);
-  conv_norm_strides(q_shape, q_strides, qs);
-  conv_norm_strides(k_shape, k_strides, ks);
-  conv_norm_strides(v_shape, v_strides, vs);
-  conv_norm_strides(out_shape, out_strides, os);
-  conv_norm_strides(dout_shape, dout_strides, dos);
+  AttnBwdOps o{attn_view(q, in_dtype, q_shape, q_strides, kAttnBHSD),          attn_view(k, in_dtype, k_shape, k_strides, kAttnBHSD),
+               attn_view(v, in_dtype, v_shape, v_strides, kAttnBHSD),          attn_view(out, out_dtype, out_shape, out_strides, kAttnBHSD),
+               attn_view(dout, in_dtype, dout_shape, dout_strides, kAttnBHSD), attn_view(dq, grad_dtype, dq_shape, dq_strides, kAttnBHSD),
+               attn_view(dk, grad_dtype, dk_shape, dk_strides, kAttnBHSD),     attn_view(dv, grad_dtype, dv_shape, dv_strides, kAttnBHSD)};
+  if (has_q) rc = attn_check_out_view(what, "dq", o.dq);
+  if (!rc) rc = attn_check_out_view(what, "dk", o.dk);
+  if (!rc) rc = attn_check_out_view(what, "dv", o.dv);
+  if (rc) return rc;
 
   CUstream st = resolve_stream(c, s);
   CUdeviceptr tmp[6] = {0, 0, 0, 0, 0, 0};   // gathers of q, k, v, out, dout; the workspace
-  // each operand in place, or gathered into a compact [B, H, S, D] pooled copy (as b200_attention)
-  auto prep = [&](int i, b200_dtype dt, uint64_t ptr, const uint64_t* shape, uint64_t* ns, uint64_t* use) -> int {
-    *use = ptr;
-    const size_t esz = dtype_size(dt);
-    if (attn_view_ok(ptr, esz, ns)) return B200_OK;
-    int rc = pool_alloc(c, shape[0] * shape[1] * shape[2] * shape[3] * esz, &tmp[i], st);
-    if (rc) return rc;
-    *use = tmp[i];
-    rc = b200_into_contiguous(c, static_cast<b200_stream>(st), dt, ptr, tmp[i], 4, shape, ns);
-    ns[3] = 1; ns[2] = shape[3]; ns[1] = shape[2] * shape[3]; ns[0] = shape[1] * shape[2] * shape[3];
-    return rc;
-  };
-  uint64_t qp = 0, kp = 0, vp = 0, op = 0, dop = 0;
-  int rc = B200_OK;
-  if (has_q) rc = prep(0, in_dtype, q, q_shape, qs, &qp);
-  if (!rc) rc = prep(1, in_dtype, k, k_shape, ks, &kp);
-  if (!rc) rc = prep(2, in_dtype, v, v_shape, vs, &vp);
-  if (!rc && has_q) rc = prep(3, out_dtype, out, out_shape, os, &op);
-  if (!rc && has_q) rc = prep(4, in_dtype, dout, dout_shape, dos, &dop);
-  if (!has_q) {   // no query block is loaded: the q and dout maps of the dk / dv kernel describe k
-    qp = dop = kp;
-    memcpy(qs, ks, sizeof(qs));
-    memcpy(dos, ks, sizeof(dos));
-  }
+  rc = attn_bwd_stage(c, st, &o, has_q, true, tmp);
   if (!rc && has_q) rc = pool_alloc(c, 2 * rows * 4, &tmp[5], st);
-
   AttnBwdParams p{};
   p.ws = tmp[5];
   p.lse = lse;
-  p.out = op; p.dout = dop;
-  p.o_sb = os[0]; p.o_sh = os[1]; p.o_ss = os[2];
-  p.d_sb = dos[0]; p.d_sh = dos[1]; p.d_ss = dos[2];
+  p.out = o.out.ptr; p.dout = o.dout.ptr;
+  p.o_sb = o.out.s_batch(); p.o_sh = o.out.s_head(); p.o_ss = o.out.s_row();
+  p.d_sb = o.dout.s_batch(); p.d_sh = o.dout.s_head(); p.d_ss = o.dout.s_row();
   p.B = (uint32_t)B; p.Hq = (uint32_t)Hq; p.Sq = (uint32_t)Sq; p.Sk = (uint32_t)Sk; p.Hkv = (uint32_t)Hkv;
   p.group = (uint32_t)(Hq / Hkv);
   p.nqb = (uint32_t)nqb; p.nkb = (uint32_t)nkb;
@@ -4408,103 +4535,35 @@ extern "C" int b200_attention_backward(b200_ctx* c, b200_stream s, b200_dtype in
   p.Sqp = (uint32_t)(nqb * kAttnBlock);
   p.causal = args->causal != 0 ? 1u : 0u;
   p.D = (uint32_t)D;
-  p.scale_log2 = (float)((double)args->scale * 1.4426950408889634074);
+  p.scale_log2 = attn_scale_log2(args->scale);
   p.scale = args->scale;
-  const uint32_t DB = D <= 64 ? 64 : 128;
-  const std::string in_tag = dt_tag(in_dtype), g_tag = dt_tag(grad_dtype);
-  const CUtensorMapDataType dt = in_dtype == B200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  const CUtensorMapDataType gdt = gsz == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_UINT16;
-  const uint64_t dimq[4] = {D, has_q ? Sq : Sk, has_q ? Hq : Hkv, B}, dimk[4] = {D, Sk, Hkv, B};
-  const uint64_t sq[3] = {qs[2], qs[1], qs[0]}, sk[3] = {ks[2], ks[1], ks[0]}, sv[3] = {vs[2], vs[1], vs[0]}, sdo[3] = {dos[2], dos[1], dos[0]};
-  const uint32_t box128[4] = {64, (uint32_t)kAttnBlock, 1, 1}, box_g[4] = {(uint32_t)(128 / gsz), 64, 1, 1};
-  auto set_smem = [&](CUfunction f, unsigned smem) -> int {
-    if (c->dry) return B200_OK;
-    CUresult r = g_drv.cuFuncSetAttribute_p(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem);
-    return r != CUDA_SUCCESS ? fail(map_cu(r), "cuFuncSetAttribute: %s", cu_err(r)) : B200_OK;
-  };
-
-  // 1. delta and L into the workspace
-  if (!rc && has_q) {
-    CUfunction f = nullptr;
-    rc = get_func(c, "attn_bwd_delta_" + in_tag + "_" + dt_tag(out_dtype), &f);
-    void* kargs[] = {&p};
-    if (!rc) rc = launch(c, f, (unsigned)((rows + 15) / 16), 1, 1, 256, 0, 1, st, kargs);
-  }
-  // 2. dq: maps q, k, v, dout (query tiles of kAttnBlock rows, key tiles of kAttnBwdDqKeys), dq
-  if (!rc && has_q) {
-    const uint32_t box_k[4] = {64, (uint32_t)kAttnBwdDqKeys, 1, 1};
-    CUtensorMap mq, mk, mv, mdo, mdq;
-    const uint64_t sdq[3] = {dqs[2], dqs[1], dqs[0]};
-    rc = encode_tmap4(c, &mq, dt, 2, qp, dimq, sq, box128, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (!rc) rc = encode_tmap4(c, &mk, dt, 2, kp, dimk, sk, box_k, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (!rc) rc = encode_tmap4(c, &mv, dt, 2, vp, dimk, sv, box_k, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (!rc) rc = encode_tmap4(c, &mdo, dt, 2, dop, dimq, sdo, box128, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (!rc) rc = encode_tmap4(c, &mdq, gdt, gsz, dq, dimq, sdq, box_g, CU_TENSOR_MAP_SWIZZLE_128B);
-    CUfunction f = nullptr;
-    if (!rc) rc = get_func(c, "attn_bwd_dq_" + in_tag + "_d" + std::to_string(DB) + "_" + g_tag, &f);
-    const unsigned smem = 1024 + 2 * kAttnBlock * DB * 2 + 2 * kAttnBwdStages * kAttnBwdDqKeys * DB * 2 + 1024;
-    if (!rc) rc = set_smem(f, smem);
-    void* kargs[] = {&mq, &mk, &mv, &mdo, &mdq, &p};
-    if (!rc) rc = launch(c, f, (unsigned)(nqb * Hq * B), 1, 1, 384, smem, 1, st, kargs);
-  }
-  // 3. dk and dv: maps q, k, v, dout (query tiles of kAttnBwdDkdvQueries rows, key tiles of kAttnBlock), dk, dv
-  if (!rc) {
-    const uint32_t box_q[4] = {64, (uint32_t)kAttnBwdDkdvQueries, 1, 1};
-    CUtensorMap mq, mk, mv, mdo, mdk, mdv;
-    const uint64_t sdk[3] = {dks[2], dks[1], dks[0]}, sdv[3] = {dvs[2], dvs[1], dvs[0]};
-    rc = encode_tmap4(c, &mq, dt, 2, qp, dimq, sq, box_q, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (!rc) rc = encode_tmap4(c, &mk, dt, 2, kp, dimk, sk, box128, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (!rc) rc = encode_tmap4(c, &mv, dt, 2, vp, dimk, sv, box128, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (!rc) rc = encode_tmap4(c, &mdo, dt, 2, dop, dimq, sdo, box_q, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (!rc) rc = encode_tmap4(c, &mdk, gdt, gsz, dk, dimk, sdk, box_g, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (!rc) rc = encode_tmap4(c, &mdv, gdt, gsz, dv, dimk, sdv, box_g, CU_TENSOR_MAP_SWIZZLE_128B);
-    CUfunction f = nullptr;
-    if (!rc) rc = get_func(c, "attn_bwd_dkdv_" + in_tag + "_d" + std::to_string(DB) + "_" + g_tag, &f);
-    const unsigned smem = 1024 + 2 * kAttnBlock * DB * 2 + 2 * kAttnBwdStages * kAttnBwdDkdvQueries * DB * 2 +
-                          kAttnBwdStages * 2 * kAttnBwdDkdvQueries * 4 + 1024;
-    if (!rc) rc = set_smem(f, smem);
-    void* kargs[] = {&mq, &mk, &mv, &mdo, &mdk, &mdv, &p};
-    if (!rc) rc = launch(c, f, (unsigned)(nkb * Hkv * B), 1, 1, 384, smem, 1, st, kargs);
-  }
+  if (!rc) rc = attn_bwd_launch(c, st, "attn_bwd_", o, has_q, true, nqb * Hq * B, nkb * Hkv * B, &p);
   for (CUdeviceptr t : tmp)
     if (t) pool_free(c, t, st);   // stream-ordered: reusable once the kernels have drained
   return rc;
 }
 
 // ------------------------------------------------------------------------------------------------ varlen attention
-// A [T, H, D] varlen operand (shape and strides in elements, strides 0 = compact) as the 4-D shape [1, T, H, D] with its
-// normalised strides ns (ns[0]: the unit batch dimension's, any valid value).
-static void vl_view(const uint64_t* shape3, const uint64_t* strides3, uint64_t* shape4, uint64_t* ns) {
-  shape4[0] = 1; shape4[1] = shape3[0]; shape4[2] = shape3[1]; shape4[3] = shape3[2];
-  const uint64_t st4[4] = {0, strides3 ? strides3[0] : 0, strides3 ? strides3[1] : 0, strides3 ? strides3[2] : 0};
-  conv_norm_strides(shape4, strides3 ? st4 : nullptr, ns);
-}
-
 // The checks both varlen entries share (see cubecl_b200.h); 0 or the failure status.
 static int vl_check(const char* what, b200_dtype in_dtype, const uint64_t* q_shape, const uint64_t* k_shape, const uint64_t* v_shape,
                     uint64_t batch, const b200_attention_varlen_args* args) {
-  auto ull = [](uint64_t x) { return (unsigned long long)x; };
-  if (in_dtype != B200_F16 && in_dtype != B200_BF16)
-    return fail(B200_ERR_UNSUPPORTED, "%s: input dtype %d unsupported (f16, bf16)", what, (int)in_dtype);
+  int rc = attn_check_in_dtype(what, in_dtype);
+  if (rc) return rc;
   const uint64_t Tq = q_shape[0], Hq = q_shape[1], D = q_shape[2], Tk = k_shape[0], Hkv = k_shape[1];
-  if (k_shape[2] != D) return fail(B200_ERR_INVALID_ARG, "%s: k's head dim %llu differs from q's D = %llu", what, ull(k_shape[2]), ull(D));
-  if (v_shape[0] != Tk || v_shape[1] != Hkv)
-    return fail(B200_ERR_INVALID_ARG, "%s: v [%llu,%llu,%llu] does not match k [%llu,%llu,%llu]", what, ull(v_shape[0]), ull(v_shape[1]),
-                ull(v_shape[2]), ull(Tk), ull(Hkv), ull(D));
-  if (v_shape[2] != D) return fail(B200_ERR_UNSUPPORTED, "%s: v's head dim %llu differs from D = %llu", what, ull(v_shape[2]), ull(D));
-  if (Hkv == 0 || Hq % Hkv) return fail(B200_ERR_INVALID_ARG, "%s: Hq = %llu must be a multiple of Hkv = %llu", what, ull(Hq), ull(Hkv));
-  if (args->window_left < -1 || args->window_right < -1)
-    return fail(B200_ERR_INVALID_ARG, "%s: window (%d, %d): each side must be >= 0, or -1 for unbounded", what, args->window_left,
-                args->window_right);
-  if (args->max_seqlen_q < 0 || args->max_seqlen_k < 0)
-    return fail(B200_ERR_INVALID_ARG, "%s: max_seqlen_q = %d and max_seqlen_k = %d must be >= 0", what, args->max_seqlen_q, args->max_seqlen_k);
-  if (!std::isfinite(args->scale)) return fail(B200_ERR_INVALID_ARG, "%s: scale must be finite", what);
-  if (D == 0 || D > 128 || D % 8) return fail(B200_ERR_UNSUPPORTED, "%s: head dim D = %llu unsupported (a multiple of 8 in [8, 128])", what, ull(D));
-  const uint64_t lim = 1ull << 31;
-  if (batch >= lim || Tq >= lim || Hq >= lim || Tk >= lim || Hkv >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: extents must be < 2^31", what);
-  if (args->max_seqlen_q >= (1 << 30) || args->max_seqlen_k >= (1 << 30))
-    return fail(B200_ERR_UNSUPPORTED, "%s: max_seqlen_q and max_seqlen_k must be < 2^30", what);
-  return B200_OK;
+  if (k_shape[2] != D)
+    return fail(B200_ERR_INVALID_ARG, "%s: k's head dim %llu differs from q's D = %llu", what, (unsigned long long)k_shape[2], (unsigned long long)D);
+  rc = attn_check_v(what, "k", "v", k_shape, v_shape, 3);
+  if (!rc) rc = attn_check_gqa(what, Hq, Hkv);
+  if (!rc && (args->window_left < -1 || args->window_right < -1))
+    rc = fail(B200_ERR_INVALID_ARG, "%s: window (%d, %d): each side must be >= 0, or -1 for unbounded", what, args->window_left,
+              args->window_right);
+  if (!rc && (args->max_seqlen_q < 0 || args->max_seqlen_k < 0))
+    rc = fail(B200_ERR_INVALID_ARG, "%s: max_seqlen_q = %d and max_seqlen_k = %d must be >= 0", what, args->max_seqlen_q, args->max_seqlen_k);
+  if (!rc) rc = attn_check_scale_d(what, args->scale, D);
+  if (!rc) rc = attn_check_extents(what, {batch, Tq, Hq, Tk, Hkv});
+  if (!rc && (args->max_seqlen_q >= (1 << 30) || args->max_seqlen_k >= (1 << 30)))
+    rc = fail(B200_ERR_UNSUPPORTED, "%s: max_seqlen_q and max_seqlen_k must be < 2^30", what);
+  return rc;
 }
 
 // Variable-length attention, forward (see cubecl_b200.h): one attn_fwd_varlen_* launch.
@@ -4516,89 +4575,39 @@ extern "C" int b200_attention_varlen(b200_ctx* c, b200_stream s, b200_dtype in_d
                                      const b200_attention_varlen_args* args) {
   CTX_ENTER(c);
   const char* what = "attention_varlen";
-  auto ull = [](uint64_t x) { return (unsigned long long)x; };
   if (!q_shape || !k_shape || !v_shape || !out_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
   int rc = vl_check(what, in_dtype, q_shape, k_shape, v_shape, batch, args);
+  if (!rc) rc = attn_check_out_dtype(what, "output", in_dtype, out_dtype);
+  if (!rc) rc = attn_check_same(what, 3, {{"out", out_shape, q_shape}});
   if (rc) return rc;
-  if (out_dtype != in_dtype && out_dtype != B200_F32)
-    return fail(B200_ERR_UNSUPPORTED, "%s: output dtype must equal the input dtype or be f32", what);
-  if (memcmp(out_shape, q_shape, 3 * sizeof(uint64_t)))
-    return fail(B200_ERR_INVALID_ARG, "%s: out is [%llu,%llu,%llu], expected q's [%llu,%llu,%llu]", what, ull(out_shape[0]), ull(out_shape[1]),
-                ull(out_shape[2]), ull(q_shape[0]), ull(q_shape[1]), ull(q_shape[2]));
   const uint64_t Tq = q_shape[0], Hq = q_shape[1], D = q_shape[2], Tk = k_shape[0], Hkv = k_shape[1], B = batch;
   const uint64_t max_q = (uint64_t)args->max_seqlen_q, max_k = (uint64_t)args->max_seqlen_k;
   if (B == 0 || Tq == 0 || Hq == 0 || max_q == 0) return B200_OK;   // no query row
   const uint64_t nqb = (max_q + kAttnBlock - 1) / kAttnBlock, ctas = nqb * Hq * B;
-  if (ctas >= (1ull << 31)) return fail(B200_ERR_UNSUPPORTED, "%s: ceil(max_seqlen_q / %d) * Hq * B = %llu CTAs must be < 2^31", what, kAttnBlock, ull(ctas));
+  if (ctas >= (1ull << 31))
+    return fail(B200_ERR_UNSUPPORTED, "%s: ceil(max_seqlen_q / %d) * Hq * B = %llu CTAs must be < 2^31", what, kAttnBlock,
+                (unsigned long long)ctas);
   if (!q || !k || !v || !out || !cu_seqlens_q || !cu_seqlens_k) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
   if (lse % 4 || cu_seqlens_q % 4 || cu_seqlens_k % 4)
     return fail(B200_ERR_INVALID_ARG, "%s: lse, cu_seqlens_q and cu_seqlens_k must be 4-byte aligned", what);
-  const size_t osz = dtype_size(out_dtype);
-  uint64_t qsh[4], ksh[4], vsh[4], osh[4], qs[4], ks[4], vs[4], os[4];
-  vl_view(out_shape, out_strides, osh, os);
-  if (!attn_view_ok(out, osz, os))
-    return fail(B200_ERR_UNSUPPORTED, "%s: out needs a unit D stride and a 16-byte aligned base and T, H strides", what);
-  vl_view(q_shape, q_strides, qsh, qs);
-  vl_view(k_shape, k_strides, ksh, ks);
-  vl_view(v_shape, v_strides, vsh, vs);
+  const AttnView ov = attn_view(out, out_dtype, out_shape, out_strides, kAttnTHD);
+  if ((rc = attn_check_out_view(what, "out", ov))) return rc;
 
-  CUstream st = resolve_stream(c, s);
-  CUdeviceptr tmp[3] = {0, 0, 0};
-  // each operand in place, or gathered into a compact [T, H, D] copy
-  auto prep = [&](int i, uint64_t ptr, const uint64_t* shape, uint64_t* ns, uint64_t* use) -> int {
-    *use = ptr;
-    if (attn_view_ok(ptr, 2, ns)) return B200_OK;
-    int r = conv_gather(c, st, in_dtype, ptr, shape, ns, &tmp[i]);
-    *use = tmp[i];
-    ns[3] = 1; ns[2] = shape[3]; ns[1] = shape[2] * shape[3]; ns[0] = shape[1] * shape[2] * shape[3];
-    return r;
-  };
-  uint64_t qp = 0, kp = 0, vp = 0;
-  rc = prep(0, q, qsh, qs, &qp);
-  if (!rc) rc = prep(1, k, ksh, ks, &kp);
-  if (!rc) rc = prep(2, v, vsh, vs, &vp);
-  if (!rc) {
-    const uint32_t DB = D <= 64 ? 64 : 128;
-    const CUtensorMapDataType dt = in_dtype == B200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-    CUtensorMap mq, mk, mv, mo;
-    const uint32_t box_in[4] = {64, (uint32_t)kAttnBlock, 1, 1};
-    const uint32_t box_out[4] = {(uint32_t)(128 / osz), 64, 1, 1};
-    const uint64_t dq[4] = {D, Tq, Hq, 1}, dk[4] = {D, Tk, Hkv, 1};
-    const uint64_t sq[3] = {qs[1], qs[2], qs[0]}, sk[3] = {ks[1], ks[2], ks[0]}, sv[3] = {vs[1], vs[2], vs[0]}, so[3] = {os[1], os[2], os[0]};
-    rc = encode_tmap4(c, &mq, dt, 2, qp, dq, sq, box_in, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (!rc) rc = encode_tmap4(c, &mk, dt, 2, kp, dk, sk, box_in, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (!rc) rc = encode_tmap4(c, &mv, dt, 2, vp, dk, sv, box_in, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (!rc)
-      rc = encode_tmap4(c, &mo, osz == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_UINT16, osz, out, dq, so, box_out,
-                        CU_TENSOR_MAP_SWIZZLE_128B);
-    CUfunction f = nullptr;
-    const std::string name = std::string("attn_fwd_varlen_") + dt_tag(in_dtype) + "_d" + std::to_string(DB) + "_" + dt_tag(out_dtype);
-    if (!rc) rc = get_func(c, name, &f);
-    const unsigned smem = 1024 + (1 + 2 * kAttnStages) * kAttnBlock * DB * 2 + 1024;
-    if (!rc && !c->dry) {
-      CUresult r = g_drv.cuFuncSetAttribute_p(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem);
-      if (r != CUDA_SUCCESS) rc = fail(map_cu(r), "cuFuncSetAttribute: %s", cu_err(r));
-    }
-    if (!rc) {
-      AttnVarlenParams p{};
-      p.lse = lse;
-      p.cu_q = cu_seqlens_q; p.cu_k = cu_seqlens_k;
-      p.out = out; p.o_st = os[1]; p.o_sh = os[2];
-      p.B = (uint32_t)B; p.Hq = (uint32_t)Hq; p.Hkv = (uint32_t)Hkv; p.Tq = (uint32_t)Tq; p.Tk = (uint32_t)Tk;
-      p.group = (uint32_t)(Hq / Hkv);
-      p.max_q = (uint32_t)max_q; p.max_k = (uint32_t)max_k;
-      p.nqb = (uint32_t)nqb; p.nkb = (uint32_t)((max_k + kAttnBlock - 1) / kAttnBlock);
-      p.D = (uint32_t)D;
-      p.left = args->window_left; p.right = args->window_right;
-      p.scale_log2 = (float)((double)args->scale * 1.4426950408889634074);
-      p.scale = args->scale;
-      void* kargs[] = {&mq, &mk, &mv, &mo, &p};
-      rc = launch(c, f, (unsigned)ctas, 1, 1, 384, smem, 1, st, kargs);
-    }
-  }
-  for (CUdeviceptr t : tmp)
-    if (t) pool_free(c, t, st);   // stream-ordered: reusable once the kernel has drained
-  return rc;
+  AttnVarlenParams p{};
+  p.lse = lse;
+  p.cu_q = cu_seqlens_q; p.cu_k = cu_seqlens_k;
+  p.out = out; p.o_st = ov.s_row(); p.o_sh = ov.s_head();
+  p.B = (uint32_t)B; p.Hq = (uint32_t)Hq; p.Hkv = (uint32_t)Hkv; p.Tq = (uint32_t)Tq; p.Tk = (uint32_t)Tk;
+  p.group = (uint32_t)(Hq / Hkv);
+  p.max_q = (uint32_t)max_q; p.max_k = (uint32_t)max_k;
+  p.nqb = (uint32_t)nqb; p.nkb = (uint32_t)((max_k + kAttnBlock - 1) / kAttnBlock);
+  p.D = (uint32_t)D;
+  p.left = args->window_left; p.right = args->window_right;
+  p.scale_log2 = attn_scale_log2(args->scale);
+  p.scale = args->scale;
+  return attn_fwd_launch(c, resolve_stream(c, s), "attn_fwd_varlen_", attn_view(q, in_dtype, q_shape, q_strides, kAttnTHD),
+                         attn_view(k, in_dtype, k_shape, k_strides, kAttnTHD), attn_view(v, in_dtype, v_shape, v_strides, kAttnTHD), ov,
+                         ctas, &p);
 }
 
 // Backward of b200_attention_varlen (see cubecl_b200.h): the delta / L pass, then the dq and the dk / dv kernels.
@@ -4614,21 +4623,15 @@ extern "C" int b200_attention_varlen_backward(b200_ctx* c, b200_stream s, b200_d
                                               const uint64_t* dv_strides, const b200_attention_varlen_args* args) {
   CTX_ENTER(c);
   const char* what = "attention_varlen_backward";
-  auto ull = [](uint64_t x) { return (unsigned long long)x; };
   if (!q_shape || !k_shape || !v_shape || !out_shape || !dout_shape || !dq_shape || !dk_shape || !dv_shape || !args)
     return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
   int rc = vl_check(what, in_dtype, q_shape, k_shape, v_shape, batch, args);
+  if (!rc) rc = attn_check_out_dtype(what, "output", in_dtype, out_dtype);
+  if (!rc) rc = attn_check_out_dtype(what, "grad", in_dtype, grad_dtype);
+  if (!rc)
+    rc = attn_check_same(what, 3, {{"out", out_shape, q_shape}, {"dout", dout_shape, q_shape}, {"dq", dq_shape, q_shape},
+                                   {"dk", dk_shape, k_shape}, {"dv", dv_shape, k_shape}});
   if (rc) return rc;
-  if (out_dtype != in_dtype && out_dtype != B200_F32)
-    return fail(B200_ERR_UNSUPPORTED, "%s: output dtype must equal the input dtype or be f32", what);
-  if (grad_dtype != in_dtype && grad_dtype != B200_F32)
-    return fail(B200_ERR_UNSUPPORTED, "%s: grad dtype must equal the input dtype or be f32", what);
-  const struct { const char* name; const uint64_t* shape; const uint64_t* want; } same[] = {
-      {"out", out_shape, q_shape}, {"dout", dout_shape, q_shape}, {"dq", dq_shape, q_shape}, {"dk", dk_shape, k_shape}, {"dv", dv_shape, k_shape}};
-  for (const auto& t : same)
-    if (memcmp(t.shape, t.want, 3 * sizeof(uint64_t)))
-      return fail(B200_ERR_INVALID_ARG, "%s: %s is [%llu,%llu,%llu], expected [%llu,%llu,%llu]", what, t.name, ull(t.shape[0]), ull(t.shape[1]),
-                  ull(t.shape[2]), ull(t.want[0]), ull(t.want[1]), ull(t.want[2]));
   const uint64_t Tq = q_shape[0], Hq = q_shape[1], D = q_shape[2], Tk = k_shape[0], Hkv = k_shape[1], B = batch;
   const uint64_t max_q = (uint64_t)args->max_seqlen_q, max_k = (uint64_t)args->max_seqlen_k;
   // query rows to differentiate (delta and dq); key rows to differentiate (dk and dv: +0 where no query sees them)
@@ -4642,53 +4645,28 @@ extern "C" int b200_attention_varlen_backward(b200_ctx* c, b200_stream s, b200_d
     return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
   if (lse % 4 || cu_seqlens_q % 4 || cu_seqlens_k % 4)
     return fail(B200_ERR_INVALID_ARG, "%s: lse, cu_seqlens_q and cu_seqlens_k must be 4-byte aligned", what);
-  const size_t gsz = dtype_size(grad_dtype);
-  uint64_t qsh[4], ksh[4], vsh[4], osh[4], dosh[4], gsh[4], qs[4], ks[4], vs[4], os[4], dos[4], dqs[4], dks[4], dvs[4];
-  vl_view(dq_shape, dq_strides, gsh, dqs);
-  vl_view(dk_shape, dk_strides, gsh, dks);
-  vl_view(dv_shape, dv_strides, gsh, dvs);
-  const struct { const char* name; uint64_t ptr; const uint64_t* ns; bool used; } grads[] = {
-      {"dq", dq, dqs, has_q}, {"dk", dk, dks, has_k}, {"dv", dv, dvs, has_k}};
-  for (const auto& g : grads)
-    if (g.used && !attn_view_ok(g.ptr, gsz, g.ns))
-      return fail(B200_ERR_UNSUPPORTED, "%s: %s needs a unit D stride and a 16-byte aligned base and T, H strides", what, g.name);
-  vl_view(q_shape, q_strides, qsh, qs);
-  vl_view(k_shape, k_strides, ksh, ks);
-  vl_view(v_shape, v_strides, vsh, vs);
-  vl_view(out_shape, out_strides, osh, os);
-  vl_view(dout_shape, dout_strides, dosh, dos);
+  AttnBwdOps o{attn_view(q, in_dtype, q_shape, q_strides, kAttnTHD),          attn_view(k, in_dtype, k_shape, k_strides, kAttnTHD),
+               attn_view(v, in_dtype, v_shape, v_strides, kAttnTHD),          attn_view(out, out_dtype, out_shape, out_strides, kAttnTHD),
+               attn_view(dout, in_dtype, dout_shape, dout_strides, kAttnTHD), attn_view(dq, grad_dtype, dq_shape, dq_strides, kAttnTHD),
+               attn_view(dk, grad_dtype, dk_shape, dk_strides, kAttnTHD),     attn_view(dv, grad_dtype, dv_shape, dv_strides, kAttnTHD)};
+  if (has_q) rc = attn_check_out_view(what, "dq", o.dq);
+  if (!rc && has_k) rc = attn_check_out_view(what, "dk", o.dk);
+  if (!rc && has_k) rc = attn_check_out_view(what, "dv", o.dv);
+  if (rc) return rc;
 
   CUstream st = resolve_stream(c, s);
   CUdeviceptr tmp[6] = {0, 0, 0, 0, 0, 0};   // gathers of q, k, v, out, dout; the workspace
-  // each operand in place, or gathered into a compact [T, H, D] pooled copy (as b200_attention_varlen); out and dout are read
-  // by the delta kernel with 16-byte loads, so they follow the same rule
-  auto prep = [&](int i, b200_dtype dt, uint64_t ptr, const uint64_t* shape, uint64_t* ns, uint64_t* use) -> int {
-    *use = ptr;
-    const size_t esz = dtype_size(dt);
-    if (attn_view_ok(ptr, esz, ns)) return B200_OK;
-    int r = pool_alloc(c, shape[1] * shape[2] * shape[3] * esz, &tmp[i], st);
-    if (r) return r;
-    *use = tmp[i];
-    r = b200_into_contiguous(c, static_cast<b200_stream>(st), dt, ptr, tmp[i], 4, shape, ns);
-    ns[3] = 1; ns[2] = shape[3]; ns[1] = shape[2] * shape[3]; ns[0] = shape[1] * shape[2] * shape[3];
-    return r;
-  };
-  uint64_t qp = 0, kp = 0, vp = 0, op = 0, dop = 0;
-  if (has_q) rc = prep(0, in_dtype, q, qsh, qs, &qp);
-  if (!rc && has_k) rc = prep(1, in_dtype, k, ksh, ks, &kp);
-  if (!rc && has_k) rc = prep(2, in_dtype, v, vsh, vs, &vp);
-  if (!rc && has_q) rc = prep(3, out_dtype, out, osh, os, &op);
-  if (!rc && has_q) rc = prep(4, in_dtype, dout, dosh, dos, &dop);
+  // out and dout are read by the delta kernel with 16-byte loads, so they follow the maps' rule
+  rc = attn_bwd_stage(c, st, &o, has_q, has_k, tmp);
   if (!rc && has_q) rc = pool_alloc(c, 2 * Hq * Tqp * 4, &tmp[5], st);
-
   AttnVarlenParams p{};
   p.lse = lse;
   p.cu_q = cu_seqlens_q; p.cu_k = cu_seqlens_k;
   p.ws = tmp[5];
-  p.out = op; p.dout = dop;
-  p.o_st = os[1]; p.o_sh = os[2]; p.d_st = dos[1]; p.d_sh = dos[2];
+  p.out = o.out.ptr; p.dout = o.dout.ptr;
+  p.o_st = o.out.s_row(); p.o_sh = o.out.s_head(); p.d_st = o.dout.s_row(); p.d_sh = o.dout.s_head();
   p.dq = dq; p.dk = dk; p.dv = dv;
-  p.dq_st = dqs[1]; p.dq_sh = dqs[2]; p.dk_st = dks[1]; p.dk_sh = dks[2]; p.dv_st = dvs[1]; p.dv_sh = dvs[2];
+  p.dq_st = o.dq.s_row(); p.dq_sh = o.dq.s_head(); p.dk_st = o.dk.s_row(); p.dk_sh = o.dk.s_head(); p.dv_st = o.dv.s_row(); p.dv_sh = o.dv.s_head();
   p.B = (uint32_t)B; p.Hq = (uint32_t)Hq; p.Hkv = (uint32_t)Hkv; p.Tq = (uint32_t)Tq; p.Tk = (uint32_t)Tk;
   p.group = (uint32_t)(Hq / Hkv);
   p.max_q = (uint32_t)max_q; p.max_k = (uint32_t)max_k;
@@ -4696,73 +4674,15 @@ extern "C" int b200_attention_varlen_backward(b200_ctx* c, b200_stream s, b200_d
   p.Tqp = (uint32_t)Tqp;
   p.D = (uint32_t)D;
   p.left = args->window_left; p.right = args->window_right;
-  p.scale_log2 = (float)((double)args->scale * 1.4426950408889634074);
+  p.scale_log2 = attn_scale_log2(args->scale);
   p.scale = args->scale;
-  const uint32_t DB = D <= 64 ? 64 : 128;
-  const std::string in_tag = dt_tag(in_dtype), g_tag = dt_tag(grad_dtype);
-  const CUtensorMapDataType dt = in_dtype == B200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  const CUtensorMapDataType gdt = gsz == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_UINT16;
-  const uint64_t dimq[4] = {D, Tq, Hq, 1}, dimk[4] = {D, Tk, Hkv, 1};
-  const uint64_t sq[3] = {qs[1], qs[2], qs[0]}, sk[3] = {ks[1], ks[2], ks[0]}, sv[3] = {vs[1], vs[2], vs[0]}, sdo[3] = {dos[1], dos[2], dos[0]};
-  const uint32_t box128[4] = {64, (uint32_t)kAttnBlock, 1, 1}, box_g[4] = {(uint32_t)(128 / gsz), 64, 1, 1};
-  auto set_smem = [&](CUfunction f, unsigned smem) -> int {
-    if (c->dry) return B200_OK;
-    CUresult r = g_drv.cuFuncSetAttribute_p(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem);
-    return r != CUDA_SUCCESS ? fail(map_cu(r), "cuFuncSetAttribute: %s", cu_err(r)) : B200_OK;
-  };
-
-  // 1. delta and L into the workspace
-  if (!rc && has_q) {
-    CUfunction f = nullptr;
-    rc = get_func(c, "attn_bwd_varlen_delta_" + in_tag + "_" + dt_tag(out_dtype), &f);
-    void* kargs[] = {&p};
-    if (!rc) rc = launch(c, f, (unsigned)(nqb * 8 * Hq * B), 1, 1, 256, 0, 1, st, kargs);
-  }
-  // 2. dq: maps q, k, v, dout (query tiles of kAttnBlock rows, key tiles of kAttnBwdDqKeys), dq.  No keys: k's map stands in
-  // for k and v (never read: every dq row is +0)
-  if (!rc && has_q) {
-    const uint32_t box_k[4] = {64, (uint32_t)kAttnBwdDqKeys, 1, 1};
-    CUtensorMap mq, mk, mv, mdo, mdq;
-    const uint64_t sdq[3] = {dqs[1], dqs[2], dqs[0]};
-    const uint64_t kd[4] = {D, has_k ? Tk : Tq, has_k ? Hkv : Hq, 1};
-    rc = encode_tmap4(c, &mq, dt, 2, qp, dimq, sq, box128, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (!rc) rc = encode_tmap4(c, &mk, dt, 2, has_k ? kp : qp, kd, has_k ? sk : sq, box_k, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (!rc) rc = encode_tmap4(c, &mv, dt, 2, has_k ? vp : qp, kd, has_k ? sv : sq, box_k, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (!rc) rc = encode_tmap4(c, &mdo, dt, 2, dop, dimq, sdo, box128, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (!rc) rc = encode_tmap4(c, &mdq, gdt, gsz, dq, dimq, sdq, box_g, CU_TENSOR_MAP_SWIZZLE_128B);
-    CUfunction f = nullptr;
-    if (!rc) rc = get_func(c, "attn_bwd_varlen_dq_" + in_tag + "_d" + std::to_string(DB) + "_" + g_tag, &f);
-    const unsigned smem = 1024 + 2 * kAttnBlock * DB * 2 + 2 * kAttnBwdStages * kAttnBwdDqKeys * DB * 2 + 1024;
-    if (!rc) rc = set_smem(f, smem);
-    void* kargs[] = {&mq, &mk, &mv, &mdo, &mdq, &p};
-    if (!rc) rc = launch(c, f, (unsigned)(nqb * Hq * B), 1, 1, 384, smem, 1, st, kargs);
-  }
-  // 3. dk and dv: maps q, k, v, dout (query tiles of kAttnBwdDkdvQueries rows, key tiles of kAttnBlock), dk, dv.  No queries:
-  // k's map stands in for q and dout (never read: every dk / dv row is +0)
-  if (!rc && has_k) {
-    const uint32_t box_q[4] = {64, (uint32_t)kAttnBwdDkdvQueries, 1, 1};
-    CUtensorMap mq, mk, mv, mdo, mdk, mdv;
-    const uint64_t sdk[3] = {dks[1], dks[2], dks[0]}, sdv[3] = {dvs[1], dvs[2], dvs[0]};
-    const uint64_t qd[4] = {D, has_q ? Tq : Tk, has_q ? Hq : Hkv, 1};
-    rc = encode_tmap4(c, &mq, dt, 2, has_q ? qp : kp, qd, has_q ? sq : sk, box_q, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (!rc) rc = encode_tmap4(c, &mk, dt, 2, kp, dimk, sk, box128, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (!rc) rc = encode_tmap4(c, &mv, dt, 2, vp, dimk, sv, box128, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (!rc) rc = encode_tmap4(c, &mdo, dt, 2, has_q ? dop : kp, qd, has_q ? sdo : sk, box_q, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (!rc) rc = encode_tmap4(c, &mdk, gdt, gsz, dk, dimk, sdk, box_g, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (!rc) rc = encode_tmap4(c, &mdv, gdt, gsz, dv, dimk, sdv, box_g, CU_TENSOR_MAP_SWIZZLE_128B);
-    CUfunction f = nullptr;
-    if (!rc) rc = get_func(c, "attn_bwd_varlen_dkdv_" + in_tag + "_d" + std::to_string(DB) + "_" + g_tag, &f);
-    const unsigned smem = 1024 + 2 * kAttnBlock * DB * 2 + 2 * kAttnBwdStages * kAttnBwdDkdvQueries * DB * 2 +
-                          kAttnBwdStages * 2 * kAttnBwdDkdvQueries * 4 + 1024;
-    if (!rc) rc = set_smem(f, smem);
-    void* kargs[] = {&mq, &mk, &mv, &mdo, &mdk, &mdv, &p};
-    if (!rc) rc = launch(c, f, (unsigned)(nkb * Hkv * B), 1, 1, 384, smem, 1, st, kargs);
-  }
+  if (!rc) rc = attn_bwd_launch(c, st, "attn_bwd_varlen_", o, has_q, has_k, nqb * Hq * B, nkb * Hkv * B, &p);
   for (CUdeviceptr t : tmp)
     if (t) pool_free(c, t, st);   // stream-ordered: reusable once the kernels have drained
   return rc;
 }
 
+// ------------------------------------------------------------------------------------------------ KV-cache attention
 // The m-tile of b200_attention_kvcache: st queries of gt heads of one kv head's G (gt * st <= kAttnKvRows), the pair with the
 // fewest m-tiles ceil(G / gt) * ceil(Sq / st); among equals the largest st.
 static void kv_tile(uint64_t G, uint64_t Sq, uint32_t* gt, uint32_t* st) {
@@ -4801,22 +4721,17 @@ extern "C" int b200_attention_kvcache(b200_ctx* c, b200_stream s, b200_dtype in_
   auto ull = [](uint64_t x) { return (unsigned long long)x; };
   if (!q_shape || !kc_shape || !vc_shape || !out_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
   if (block_table && !bt_shape) return fail(B200_ERR_INVALID_ARG, "%s: null block-table shape", what);
-  if (in_dtype != B200_F16 && in_dtype != B200_BF16)
-    return fail(B200_ERR_UNSUPPORTED, "%s: input dtype %d unsupported (f16, bf16)", what, (int)in_dtype);
-  if (out_dtype != in_dtype && out_dtype != B200_F32)
-    return fail(B200_ERR_UNSUPPORTED, "%s: output dtype must equal the input dtype or be f32", what);
+  int rc = attn_check_in_dtype(what, in_dtype);
+  if (!rc) rc = attn_check_out_dtype(what, "output", in_dtype, out_dtype);
+  if (rc) return rc;
   const uint64_t B = q_shape[0], Hq = q_shape[1], Sq = q_shape[2], D = q_shape[3];
   const uint64_t P = kc_shape[0], page = kc_shape[1], Hkv = kc_shape[2];
   if (kc_shape[3] != D)
     return fail(B200_ERR_INVALID_ARG, "%s: k_cache head dim %llu differs from q's D = %llu", what, ull(kc_shape[3]), ull(D));
-  if (vc_shape[0] != P || vc_shape[1] != page || vc_shape[2] != Hkv)
-    return fail(B200_ERR_INVALID_ARG, "%s: v_cache [%llu,%llu,%llu,%llu] does not match k_cache [%llu,%llu,%llu,%llu]", what, ull(vc_shape[0]),
-                ull(vc_shape[1]), ull(vc_shape[2]), ull(vc_shape[3]), ull(P), ull(page), ull(Hkv), ull(D));
-  if (vc_shape[3] != D) return fail(B200_ERR_UNSUPPORTED, "%s: v_cache's head dim %llu differs from D = %llu", what, ull(vc_shape[3]), ull(D));
-  if (Hkv == 0 || Hq % Hkv) return fail(B200_ERR_INVALID_ARG, "%s: Hq = %llu must be a multiple of Hkv = %llu", what, ull(Hq), ull(Hkv));
-  if (memcmp(out_shape, q_shape, 4 * sizeof(uint64_t)))
-    return fail(B200_ERR_INVALID_ARG, "%s: out is [%llu,%llu,%llu,%llu], expected [%llu,%llu,%llu,%llu]", what, ull(out_shape[0]),
-                ull(out_shape[1]), ull(out_shape[2]), ull(out_shape[3]), ull(B), ull(Hq), ull(Sq), ull(D));
+  rc = attn_check_v(what, "k_cache", "v_cache", kc_shape, vc_shape, 4);
+  if (!rc) rc = attn_check_gqa(what, Hq, Hkv);
+  if (!rc) rc = attn_check_same(what, 4, {{"out", out_shape, q_shape}});
+  if (rc) return rc;
   if (page == 0 || P == 0) return fail(B200_ERR_INVALID_ARG, "%s: empty cache (P = %llu pages of %llu keys)", what, ull(P), ull(page));
   const uint64_t max_pages = block_table ? bt_shape[1] : 1;
   if (block_table && (bt_shape[0] != B || max_pages == 0))
@@ -4827,8 +4742,7 @@ extern "C" int b200_attention_kvcache(b200_ctx* c, b200_stream s, b200_dtype in_
   if (max_pages > 1 && (page % 16 || (kAttnKvBlock % page && page % kAttnKvBlock)))
     return fail(B200_ERR_UNSUPPORTED, "%s: a page of %llu keys must be a multiple of 16 that divides %d or is a multiple of it", what,
                 ull(page), kAttnKvBlock);
-  if (!std::isfinite(args->scale)) return fail(B200_ERR_INVALID_ARG, "%s: scale must be finite", what);
-  if (D == 0 || D > 128 || D % 8) return fail(B200_ERR_UNSUPPORTED, "%s: head dim D = %llu unsupported (a multiple of 8 in [8, 128])", what, ull(D));
+  if ((rc = attn_check_scale_d(what, args->scale, D))) return rc;
   const uint64_t lim = 1ull << 31, cap = max_pages * page;
   if (B >= lim || Hq >= lim || Sq >= lim || P >= lim || page >= lim || max_pages >= lim || cap >= lim)
     return fail(B200_ERR_UNSUPPORTED, "%s: extents and the capacity max_pages * page must be < 2^31", what);
@@ -4836,17 +4750,9 @@ extern "C" int b200_attention_kvcache(b200_ctx* c, b200_stream s, b200_dtype in_
   if (!q || !k_cache || !v_cache || !cache_seqlens || !out) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
   if (lse % 4 || cache_seqlens % 4 || block_table % 4)
     return fail(B200_ERR_INVALID_ARG, "%s: lse, cache_seqlens and block_table must be 4-byte aligned", what);
-  const size_t osz = dtype_size(out_dtype);
-  uint64_t qs[4], ks[4], vs[4], os[4];
-  conv_norm_strides(out_shape, out_strides, os);
-  if (!attn_view_ok(out, osz, os))
-    return fail(B200_ERR_UNSUPPORTED, "%s: out needs a unit D stride and a 16-byte aligned base and S, H, B strides", what);
-  conv_norm_strides(kc_shape, kc_strides, ks);
-  conv_norm_strides(vc_shape, vc_strides, vs);
-  if (!attn_view_ok(k_cache, 2, ks) || !attn_view_ok(v_cache, 2, vs))
-    return fail(B200_ERR_UNSUPPORTED, "%s: a cache needs a unit D stride and a 16-byte aligned base and page, row and head strides "
-                "(it is read in place, never gathered)", what);
-  conv_norm_strides(q_shape, q_strides, qs);
+  AttnView qv = attn_view(q, in_dtype, q_shape, q_strides, kAttnBHSD), ov = attn_view(out, out_dtype, out_shape, out_strides, kAttnBHSD);
+  const AttnView kv = attn_view(k_cache, in_dtype, kc_shape, kc_strides, kAttnBSHD), vv = attn_view(v_cache, in_dtype, vc_shape, vc_strides, kAttnBSHD);
+  if ((rc = attn_check_out_view(what, "out", ov)) || (rc = attn_check_caches(what, kv, vv))) return rc;
 
   const uint64_t G = Hq / Hkv;
   uint32_t gt = 1, stq = 1;
@@ -4861,27 +4767,17 @@ extern "C" int b200_attention_kvcache(b200_ctx* c, b200_stream s, b200_dtype in_
 
   CUstream st = resolve_stream(c, s);
   CUdeviceptr tmp[2] = {0, 0};   // the gather of q; the split workspace
-  uint64_t qp = q;
-  int rc = B200_OK;
-  if (!attn_view_ok(q, 2, qs)) {
-    rc = conv_gather(c, st, in_dtype, q, q_shape, qs, &tmp[0]);
-    qp = tmp[0];
-    qs[3] = 1; qs[2] = D; qs[1] = Sq * D; qs[0] = Hq * Sq * D;
-  }
+  rc = attn_stage(c, st, &qv, &tmp[0]);
   if (!rc && nsplit > 1) rc = pool_alloc(c, (size_t)nsplit * rows * (D + 2) * 4, &tmp[1], st);
   if (!rc) {
-    const uint32_t DB = D <= 64 ? 64 : 128;
+    const uint32_t DB = attn_db(D);
     const uint32_t R = max_pages == 1 ? kAttnKvBlock : (uint32_t)std::min<uint64_t>(page, kAttnKvBlock);
-    const CUtensorMapDataType dt = in_dtype == B200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
     CUtensorMap mq, mk, mv;
-    const uint32_t box_q[4] = {64, stq, gt, 1}, box_kv[4] = {64, R, 1, 1};
-    const uint64_t dq[4] = {D, Sq, Hq, B}, dkv[4] = {D, page, Hkv, P};
-    const uint64_t sq[3] = {qs[2], qs[1], qs[0]}, sk[3] = {ks[1], ks[2], ks[0]}, sv[3] = {vs[1], vs[2], vs[0]};
-    rc = encode_tmap4(c, &mq, dt, 2, qp, dq, sq, box_q, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (!rc) rc = encode_tmap4(c, &mk, dt, 2, k_cache, dkv, sk, box_kv, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (!rc) rc = encode_tmap4(c, &mv, dt, 2, v_cache, dkv, sv, box_kv, CU_TENSOR_MAP_SWIZZLE_128B);
+    rc = attn_map(c, &mq, qv, false, stq, gt);
+    if (!rc) rc = attn_map(c, &mk, kv, false, R);
+    if (!rc) rc = attn_map(c, &mv, vv, false, R);
     AttnKvParams p{};
-    p.out = out; p.o_sb = os[0]; p.o_sh = os[1]; p.o_ss = os[2];
+    p.out = out; p.o_sb = ov.s_batch(); p.o_sh = ov.s_head(); p.o_ss = ov.s_row();
     p.lse = lse;
     p.ws = tmp[1];
     p.table = block_table;
@@ -4897,15 +4793,12 @@ extern "C" int b200_attention_kvcache(b200_ctx* c, b200_stream s, b200_dtype in_
     p.cap = (uint32_t)cap; p.nkb = (uint32_t)nkb;
     p.nsplit = nsplit; p.bps = (uint32_t)bps;
     p.causal = args->causal != 0 ? 1u : 0u;
-    p.scale_log2 = (float)((double)args->scale * 1.4426950408889634074);
+    p.scale_log2 = attn_scale_log2(args->scale);
     CUfunction f = nullptr;
     const std::string in_tag = dt_tag(in_dtype), out_tag = dt_tag(out_dtype);
     if (!rc) rc = get_func(c, "attn_kv_" + in_tag + "_d" + std::to_string(DB) + "_" + out_tag, &f);
     const unsigned smem = 1024 + (DB / 64) * (kAttnKvRows + 2 * kAttnKvStages * kAttnKvBlock) * 128 + kAttnKvBarBytes;
-    if (!rc && !c->dry) {
-      CUresult r = g_drv.cuFuncSetAttribute_p(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem);
-      if (r != CUDA_SUCCESS) rc = fail(map_cu(r), "cuFuncSetAttribute: %s", cu_err(r));
-    }
+    if (!rc) rc = attn_set_smem(c, f, smem);
     void* kargs[] = {&mq, &mk, &mv, &p};
     if (!rc) rc = launch(c, f, (unsigned)ctas, 1, 1, kAttnKvThreads, smem, 1, st, kargs);
     if (!rc && nsplit > 1) {
@@ -4927,48 +4820,37 @@ extern "C" int b200_kvcache_write(b200_ctx* c, b200_stream s, b200_dtype dtype, 
                                   const uint64_t* vc_shape, const uint64_t* vc_strides, b200_dptr slot_mapping) {
   CTX_ENTER(c);
   const char* what = "kvcache_write";
-  auto ull = [](uint64_t x) { return (unsigned long long)x; };
   if (!kn_shape || !vn_shape || !kc_shape || !vc_shape) return fail(B200_ERR_INVALID_ARG, "%s: null shape", what);
   if (dtype != B200_F16 && dtype != B200_BF16) return fail(B200_ERR_UNSUPPORTED, "%s: dtype %d unsupported (f16, bf16)", what, (int)dtype);
   const uint64_t B = kn_shape[0], Snew = kn_shape[1], Hkv = kn_shape[2], D = kn_shape[3];
   const uint64_t P = kc_shape[0], page = kc_shape[1];
   if (memcmp(vn_shape, kn_shape, 4 * sizeof(uint64_t)))
-    return fail(B200_ERR_INVALID_ARG, "%s: v_new [%llu,%llu,%llu,%llu] does not match k_new [%llu,%llu,%llu,%llu]", what, ull(vn_shape[0]),
-                ull(vn_shape[1]), ull(vn_shape[2]), ull(vn_shape[3]), ull(B), ull(Snew), ull(Hkv), ull(D));
+    return fail(B200_ERR_INVALID_ARG, "%s: v_new %s does not match k_new %s", what, attn_dims(vn_shape, 4).c_str(), attn_dims(kn_shape, 4).c_str());
   if (memcmp(vc_shape, kc_shape, 4 * sizeof(uint64_t))) return fail(B200_ERR_INVALID_ARG, "%s: v_cache does not match k_cache", what);
   if (kc_shape[2] != Hkv || kc_shape[3] != D)
-    return fail(B200_ERR_INVALID_ARG, "%s: k_cache [%llu,%llu,%llu,%llu] differs from k_new [%llu,%llu,%llu,%llu] in heads or head dim", what,
-                ull(P), ull(page), ull(kc_shape[2]), ull(kc_shape[3]), ull(B), ull(Snew), ull(Hkv), ull(D));
-  if (D % 8) return fail(B200_ERR_UNSUPPORTED, "%s: head dim D = %llu must be a multiple of 8", what, ull(D));
+    return fail(B200_ERR_INVALID_ARG, "%s: k_cache %s differs from k_new %s in heads or head dim", what, attn_dims(kc_shape, 4).c_str(),
+                attn_dims(kn_shape, 4).c_str());
+  if (D % 8) return fail(B200_ERR_UNSUPPORTED, "%s: head dim D = %llu must be a multiple of 8", what, (unsigned long long)D);
   const uint64_t units = B * Snew * Hkv * (D / 8);
   if (units == 0) return B200_OK;
   if (!k_new || !v_new || !k_cache || !v_cache || !slot_mapping) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
   if (slot_mapping % 4) return fail(B200_ERR_INVALID_ARG, "%s: slot_mapping must be 4-byte aligned", what);
-  uint64_t kns[4], vns[4], kcs[4], vcs[4];
-  conv_norm_strides(kc_shape, kc_strides, kcs);
-  conv_norm_strides(vc_shape, vc_strides, vcs);
-  if (!attn_view_ok(k_cache, 2, kcs) || !attn_view_ok(v_cache, 2, vcs))
-    return fail(B200_ERR_UNSUPPORTED, "%s: a cache needs a unit D stride and a 16-byte aligned base and page, row and head strides", what);
-  conv_norm_strides(kn_shape, kn_strides, kns);
-  conv_norm_strides(vn_shape, vn_strides, vns);
+  const AttnView kc = attn_view(k_cache, dtype, kc_shape, kc_strides, kAttnBSHD), vc = attn_view(v_cache, dtype, vc_shape, vc_strides, kAttnBSHD);
+  int rc = attn_check_caches(what, kc, vc);
+  if (rc) return rc;
+  // the kernel moves 16-byte units: other views of the new tokens are gathered into a compact copy first
+  AttnView kn = attn_view(k_new, dtype, kn_shape, kn_strides, kAttnBSHD), vn = attn_view(v_new, dtype, vn_shape, vn_strides, kAttnBSHD);
   CUstream st = resolve_stream(c, s);
   CUdeviceptr tmp[2] = {0, 0};
-  uint64_t ptr[2] = {k_new, v_new};
-  uint64_t* ns[2] = {kns, vns};
-  int rc = B200_OK;
-  for (int i = 0; i < 2 && !rc; ++i) {   // the kernel moves 16-byte units: other views are gathered into a compact copy first
-    if (attn_view_ok(ptr[i], 2, ns[i])) continue;
-    rc = conv_gather(c, st, dtype, ptr[i], kn_shape, ns[i], &tmp[i]);
-    ptr[i] = tmp[i];
-    ns[i][3] = 1; ns[i][2] = D; ns[i][1] = Hkv * D; ns[i][0] = Snew * Hkv * D;
-  }
+  rc = attn_stage(c, st, &kn, &tmp[0]);
+  if (!rc) rc = attn_stage(c, st, &vn, &tmp[1]);
   if (!rc) {
     AttnKvWriteParams p{};
-    p.kn = ptr[0]; p.vn = ptr[1]; p.kc = k_cache; p.vc = v_cache; p.slots = slot_mapping;
-    p.kn_sb = kns[0]; p.kn_st = kns[1]; p.kn_sh = kns[2];
-    p.vn_sb = vns[0]; p.vn_st = vns[1]; p.vn_sh = vns[2];
-    p.kc_sp = kcs[0]; p.kc_sr = kcs[1]; p.kc_sh = kcs[2];
-    p.vc_sp = vcs[0]; p.vc_sr = vcs[1]; p.vc_sh = vcs[2];
+    p.kn = kn.ptr; p.vn = vn.ptr; p.kc = k_cache; p.vc = v_cache; p.slots = slot_mapping;
+    p.kn_sb = kn.s_batch(); p.kn_st = kn.s_row(); p.kn_sh = kn.s_head();
+    p.vn_sb = vn.s_batch(); p.vn_st = vn.s_row(); p.vn_sh = vn.s_head();
+    p.kc_sp = kc.s_batch(); p.kc_sr = kc.s_row(); p.kc_sh = kc.s_head();
+    p.vc_sp = vc.s_batch(); p.vc_sr = vc.s_row(); p.vc_sh = vc.s_head();
     p.units = units;
     p.Snew = (uint32_t)Snew; p.Hkv = (uint32_t)Hkv; p.D = (uint32_t)D; p.page = (uint32_t)page;
     p.slot_end = P * page;

@@ -7,7 +7,9 @@
 - Against torch's varlen attention (or, where it refuses the call, torch's SDPA per sequence with an explicit mask) on the GPU.
 - Sequences are independent: NaN in one sequence's rows and outside every sequence changes no bit of the others, and rows
   outside every sequence of out, lse, dq, dk and dv keep their sentinel bytes.
-- Reproducible across repeats and two streams."""
+- Reproducible across repeats and two streams.
+- Views read in place (fused-QKV slices, pitched outputs and gradients) or gathered (a misaligned q) give the bits of compact
+  operands."""
 
 import numpy as np
 import pytest
@@ -238,3 +240,42 @@ def test_repeats_and_two_streams_give_the_same_bits(client):
     finally:
         for st in streams:
             client.destroy_stream(st)
+
+
+@pytest.mark.parametrize("f32", [False, True])
+def test_views_give_identical_bits(client, f32):
+    """q, k and v as slices of one [T, 3, H, D] projection with pitched out, dout, dq, dk and dv, and a misaligned q (gathered),
+    give the bits of compact operands, forward and backward"""
+    rng = np.random.default_rng(14)
+    lens = [100, 0, 190, 7]
+    T, H, D, P = sum(lens), 4, 64, 72
+    cuq = cu(lens)
+    qkv, dout = rng.standard_normal((T, 3, H, D)), rng.standard_normal((T, H, D))
+    dt = "f32" if f32 else "bf16"
+    ref = [bits(client, t) for t in varlen(client, qkv[:, 0], qkv[:, 1], qkv[:, 2], dout, cuq, cuq, 190, 190, "bf16", dt, dt, (-1, 0))]
+    cq = up(client, cuq, "i32")
+
+    def pitched(dtype, vals=None):   # [T, H, D] rows of P elements per head: a view, and the buffer behind it
+        buf = up(client, np.pad(vals, ((0, 0), (0, 0), (0, P - D))), dtype) if vals is not None else \
+            TensorHandle.empty_contiguous(client, [T, H, P], dtype)
+        return TensorHandle(buf.handle, [T, H, D], [H * P, P, 1], dtype), buf
+
+    fused = up(client, qkv, "bf16")
+    q, k, v = (TensorHandle(fused.handle.offset(i * H * D * 2), [T, H, D], [3 * H * D, D, 1], "bf16") for i in range(3))
+    (out, ob), (do, _), (dq, dqb), (dk, dkb), (dv, dvb) = (pitched(dt), pitched("bf16", dout), pitched(dt), pitched(dt), pitched(dt))
+    lse = TensorHandle.empty_contiguous(client, [H, T], "f32")
+    attention.launch_varlen(client, q, k, v, cq, cq, 190, 190, out, window_size=(-1, 0), lse=lse)
+    attention.launch_varlen_backward(client, q, k, v, out, do, lse, cq, cq, 190, 190, dq, dk, dv, window_size=(-1, 0))
+    client.sync()
+    for name, want, got in zip(("out", "lse", "dq", "dk", "dv"), ref, (ob, lse, dqb, dkb, dvb)):
+        g = bits(client, got)
+        np.testing.assert_array_equal(g[..., :D] if name != "lse" else g, want, err_msg=name)
+    # a q one element into its buffer: the base is not 16-byte aligned, so both calls read a gathered copy
+    qbuf = up(client, np.concatenate([[0.0], qkv[:, 0].reshape(-1)]), "bf16")
+    qm = TensorHandle(qbuf.handle.offset(2), [T, H, D], [H * D, D, 1], "bf16")
+    kc, vc, doc = (up(client, t, "bf16") for t in (qkv[:, 1], qkv[:, 2], dout))
+    out, lse = attention.launch_varlen_alloc(client, qm, kc, vc, cq, cq, 190, 190, window_size=(-1, 0), out_dtype=dt, return_lse=True)
+    grads = attention.launch_varlen_backward_alloc(client, qm, kc, vc, out, doc, lse, cq, cq, 190, 190, window_size=(-1, 0), grad_dtype=dt)
+    client.sync()
+    for name, want, got in zip(("out", "lse", "dq", "dk", "dv"), ref, (out, lse) + tuple(grads)):
+        np.testing.assert_array_equal(bits(client, got), want, err_msg=f"misaligned q: {name}")
