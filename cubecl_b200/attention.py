@@ -18,7 +18,9 @@ Against a KV cache (launch_kvcache, for decoding): q [B, Hq, Sq, D] attends to t
 sequence b in a paged cache k_cache, v_cache [P, page, Hkv, D] reached through an i32 block_table [B, max_pages] (None: page b
 is sequence b).  causal is bottom-right there: query i also needs j <= L_b - Sq + i.  kvcache_write scatters new tokens
 [B, Snew, Hkv, D] into cache slots (slot_mapping, i32 [B * Snew]; negative slots are skipped).  One split-KV kernel with a
-fixed-order combine (csrc/attention_kv.cu); see b200_attention_kvcache and b200_kvcache_write.
+fixed-order combine (csrc/attention_kv.cu); see b200_attention_kvcache and b200_kvcache_write.  fp8 caches (f8e4m3 / f8e5m2 with
+f32 [Hkv] per-head k_scale and v_scale): launch_kvcache_fp8 widens K and V to q's dtype on chip, kvcache_write_fp8 quantizes new
+tokens into them; see b200_attention_kvcache_fp8 and b200_kvcache_write_fp8.
 
 Variable-length (packed) sequences (launch_varlen, torch's varlen_attn / flash_attn_varlen_func): q [Tq, Hq, D] and k, v
 [Tk, Hkv, D] hold B sequences back to back; sequence b owns rows [cu_seqlens_q[b], cu_seqlens_q[b + 1]) of q and the matching
@@ -219,6 +221,77 @@ def kvcache_write(client: ComputeClient, k_new: TensorHandle, v_new: TensorHandl
     _used_on(stream, k_new, v_new, k_cache, v_cache, slot_mapping)
     _ffi.check(client._lib.b200_kvcache_write(client._ctx, stream, DTYPES[k_cache.dtype], *_view_args((k_new, v_new, k_cache, v_cache)),
                                               _ptr(slot_mapping)))
+
+
+_FP8 = ("f8e4m3", "f8e5m2")
+
+
+def _check_fp8(what, k_cache, v_cache, k_scale, v_scale, Hkv):
+    if k_cache.dtype != v_cache.dtype:
+        raise B200Error(7, f"{what}: k_cache and v_cache dtypes differ ({k_cache.dtype}, {v_cache.dtype})")
+    if k_cache.dtype not in _FP8:
+        raise B200Error(7, f"{what}: cache dtype {k_cache.dtype} unsupported (f8e4m3, f8e5m2)")
+    for name, t in (("k_scale", k_scale), ("v_scale", v_scale)):
+        if t.dtype != "f32" or not t.is_contiguous() or list(t.shape) != [Hkv]:
+            raise B200Error(6, f"{what}: {name} must be a compact f32 [Hkv] = [{Hkv}] tensor")
+
+
+@_defers_errors
+def launch_kvcache_fp8(client: ComputeClient, q: TensorHandle, k_cache: TensorHandle, v_cache: TensorHandle,
+                       cache_seqlens: TensorHandle, k_scale: TensorHandle, v_scale: TensorHandle, out: TensorHandle,
+                       block_table: TensorHandle | None = None, scale: float | None = None, causal: bool = False,
+                       lse: TensorHandle | None = None, stream=None) -> None:
+    """launch_kvcache against an fp8 cache: k_cache and v_cache f8e4m3 or f8e5m2 [P, page, Hkv, D] holding K = k_scale[hk] * k8
+    and V = v_scale[hk] * v8, with k_scale and v_scale compact f32 [Hkv] tensors (read on the device).  K and V are widened
+    exactly to q's dtype on chip; scores are scaled by scale * k_scale[hk] and out = (v_scale[hk] * O) / l.  Power-of-two
+    scales give the bits of launch_kvcache on the dequantized cache.  Never raises for launch problems: errors are deferred to
+    client.sync()."""
+    what = "attention_kvcache_fp8"
+    _check_rank(what, 4, (("q", q), ("k_cache", k_cache), ("v_cache", v_cache), ("out", out)))
+    _check_fp8(what, k_cache, v_cache, k_scale, v_scale, k_cache.shape[2])
+    if cache_seqlens.dtype != "i32" or not cache_seqlens.is_contiguous() or list(cache_seqlens.shape) != [q.shape[0]]:
+        raise B200Error(6, f"{what}: cache_seqlens must be a compact i32 [B] = [{q.shape[0]}] tensor")
+    if block_table is not None and (block_table.dtype != "i32" or len(block_table.shape) != 2):
+        raise B200Error(6, f"{what}: block_table must be an i32 [B, max_pages] tensor")
+    _check_lse(what, lse, "[B, Hq, Sq]", q.shape[:3])
+    args = _ffi.AttentionArgs(_scale(scale, q.shape[3]), 1 if causal else 0)
+    _used_on(stream, q, k_cache, v_cache, cache_seqlens, k_scale, v_scale, out, block_table, lse)
+    bt = _view_args((block_table,)) if block_table is not None else [C.c_uint64(0), None, None]
+    _ffi.check(client._lib.b200_attention_kvcache_fp8(
+        client._ctx, stream, DTYPES[q.dtype], DTYPES[k_cache.dtype], DTYPES[out.dtype], *_view_args((q, k_cache, v_cache)), *bt,
+        _ptr(cache_seqlens), _ptr(k_scale), _ptr(v_scale), *_view_args((out,)), _ptr(lse), C.byref(args)))
+
+
+def launch_kvcache_fp8_alloc(client: ComputeClient, q: TensorHandle, k_cache: TensorHandle, v_cache: TensorHandle,
+                             cache_seqlens: TensorHandle, k_scale: TensorHandle, v_scale: TensorHandle,
+                             block_table: TensorHandle | None = None, scale: float | None = None, causal: bool = False,
+                             out_dtype: str | None = None, return_lse: bool = False, stream=None):
+    """Convenience: allocate a compact out [B, Hq, Sq, D] (and, with return_lse, a compact f32 lse [B, Hq, Sq]), then
+    launch_kvcache_fp8.  Returns out, or (out, lse)."""
+    out = TensorHandle.empty_contiguous(client, list(q.shape), out_dtype or q.dtype)
+    lse = TensorHandle.empty_contiguous(client, list(q.shape[:3]), "f32") if return_lse else None
+    launch_kvcache_fp8(client, q, k_cache, v_cache, cache_seqlens, k_scale, v_scale, out, block_table=block_table, scale=scale,
+                       causal=causal, lse=lse, stream=stream)
+    return (out, lse) if return_lse else out
+
+
+@_defers_errors
+def kvcache_write_fp8(client: ComputeClient, k_new: TensorHandle, v_new: TensorHandle, k_cache: TensorHandle, v_cache: TensorHandle,
+                      slot_mapping: TensorHandle, k_scale: TensorHandle, v_scale: TensorHandle, stream=None) -> None:
+    """kvcache_write into fp8 caches: k_new, v_new f16 or bf16 [B, Snew, Hkv, D]; each value x of kv head hk is stored as
+    sat_rn(x / scale[hk]) in the cache format (saturating to +-448 for e4m3, +-57344 for e5m2; NaN stays NaN), with k_scale /
+    v_scale compact f32 [Hkv] tensors.  Slots as kvcache_write.  Errors are deferred to client.sync()."""
+    what = "kvcache_write_fp8"
+    _check_rank(what, 4, (("k_new", k_new), ("v_new", v_new), ("k_cache", k_cache), ("v_cache", v_cache)))
+    _check_same_dtype(what, (("k_new", k_new), ("v_new", v_new)))
+    _check_fp8(what, k_cache, v_cache, k_scale, v_scale, k_cache.shape[2])
+    n = k_new.shape[0] * k_new.shape[1]
+    if slot_mapping.dtype != "i32" or not slot_mapping.is_contiguous() or math.prod(slot_mapping.shape) != n:
+        raise B200Error(6, f"{what}: slot_mapping must be a compact i32 tensor of B * Snew = {n} slots")
+    _used_on(stream, k_new, v_new, k_cache, v_cache, slot_mapping, k_scale, v_scale)
+    _ffi.check(client._lib.b200_kvcache_write_fp8(client._ctx, stream, DTYPES[k_new.dtype], DTYPES[k_cache.dtype],
+                                                  *_view_args((k_new, v_new, k_cache, v_cache)), _ptr(slot_mapping), _ptr(k_scale),
+                                                  _ptr(v_scale)))
 
 
 def _varlen_args(q, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, scale, window_size, what):

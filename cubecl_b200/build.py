@@ -32,7 +32,8 @@ CUBINS = {"gemm": ("gemm_wgmma.cu", ["-DGEMM_PART=0"]), "gemm_b": ("gemm_wgmma.c
           "gemm_conv3d": ("gemm_wgmma.cu", ["-DGEMM_PART=6"]), "gemm_convt": ("gemm_wgmma.cu", ["-DGEMM_PART=7"]),
           "attention": ("attention.cu", []), "attention_bwd": ("attention_bwd.cu", []),
           "attention_kv": ("attention_kv.cu", []), "attention_varlen": ("attention.cu", ["-DATTN_VARLEN"]),
-          "attention_varlen_bwd": ("attention_bwd.cu", ["-DATTN_VARLEN"])}
+          "attention_varlen_bwd": ("attention_bwd.cu", ["-DATTN_VARLEN"]),
+          "attention_kv_fp8": ("attention_kv.cu", ["-DATTN_KV_FP8"])}
 NVCC_FLAGS = ["-cubin", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17"]
 
 

@@ -66,6 +66,8 @@ extern const unsigned char b200_cubin_attention_varlen[];
 extern const unsigned char b200_cubin_attention_varlen_end[];
 extern const unsigned char b200_cubin_attention_varlen_bwd[];
 extern const unsigned char b200_cubin_attention_varlen_bwd_end[];
+extern const unsigned char b200_cubin_attention_kv_fp8[];
+extern const unsigned char b200_cubin_attention_kv_fp8_end[];
 }
 
 // ================================================================================================ errors
@@ -337,13 +339,14 @@ static int get_func(b200_ctx* c, const std::string& name, CUfunction* out) {
   auto it = c->funcs.find(name);
   if (it != c->funcs.end()) { *out = it->second; return B200_OK; }
   // modules are loaded in the order gemm, reduce, aux, gemm_b, gemm_c, quant, gemm_q, quant_mm, gemm_conv, gemm_convbwd,
-  // conv_grouped, gemm_conv3d, gemm_convt, attention, attention_bwd, attention_kv, attention_varlen, attention_varlen_bwd; the kernel
-  // name says where a
+  // conv_grouped, gemm_conv3d, gemm_convt, attention, attention_bwd, attention_kv, attention_varlen, attention_varlen_bwd,
+  // attention_kv_fp8; the kernel name says where a
   // kernel lives (no failing lookups, which API-level tools such as compute-sanitizer would report)
   auto starts = [&](const char* pfx) { return name.rfind(pfx, 0) == 0; };
   auto has = [&](const char* part) { return name.find(part) != std::string::npos; };
   const bool tc_gemm = starts("gemm_") && name != "gemm_simt_strided" && name != "gemm_scaled_simt";
   const size_t home = name == "conv3d_dgrad_weights" ? 2
+                      : starts("attn_kv_") && (has("_e4m3_") || has("_e5m2_") || has("_fp8")) ? 18
                       : starts("attn_bwd_varlen_") ? 17
                       : starts("attn_fwd_varlen_") ? 16
                       : starts("attn_kv_") ? 15
@@ -393,7 +396,8 @@ extern "C" int b200_get_cubin(const char* name, const void** image, size_t* size
   else if (!strcmp(name, "attention_kv")) { b = b200_cubin_attention_kv; e = b200_cubin_attention_kv_end; }
   else if (!strcmp(name, "attention_varlen")) { b = b200_cubin_attention_varlen; e = b200_cubin_attention_varlen_end; }
   else if (!strcmp(name, "attention_varlen_bwd")) { b = b200_cubin_attention_varlen_bwd; e = b200_cubin_attention_varlen_bwd_end; }
-  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd|conv_grouped|gemm_conv3d|gemm_convt|attention|attention_bwd|attention_kv|attention_varlen|attention_varlen_bwd)", name);
+  else if (!strcmp(name, "attention_kv_fp8")) { b = b200_cubin_attention_kv_fp8; e = b200_cubin_attention_kv_fp8_end; }
+  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd|conv_grouped|gemm_conv3d|gemm_convt|attention|attention_bwd|attention_kv|attention_varlen|attention_varlen_bwd|attention_kv_fp8)", name);
   *image = b;
   *size = static_cast<size_t>(e - b);
   return B200_OK;
@@ -458,7 +462,8 @@ extern "C" int b200_init(int device, b200_ctx** out) {
       (rc = load_module(c, b200_cubin_attention_bwd, b200_cubin_attention_bwd_end, "attention_bwd")) ||
       (rc = load_module(c, b200_cubin_attention_kv, b200_cubin_attention_kv_end, "attention_kv")) ||
       (rc = load_module(c, b200_cubin_attention_varlen, b200_cubin_attention_varlen_end, "attention_varlen")) ||
-      (rc = load_module(c, b200_cubin_attention_varlen_bwd, b200_cubin_attention_varlen_bwd_end, "attention_varlen_bwd"))) {
+      (rc = load_module(c, b200_cubin_attention_varlen_bwd, b200_cubin_attention_varlen_bwd_end, "attention_varlen_bwd")) ||
+      (rc = load_module(c, b200_cubin_attention_kv_fp8, b200_cubin_attention_kv_fp8_end, "attention_kv_fp8"))) {
     for (CUmodule m : c->modules) g_drv.cuModuleUnload_p(m);
     g_drv.cuDevicePrimaryCtxRelease_p(c->dev);
     return bail(rc);
@@ -4243,12 +4248,14 @@ static int attn_stage(b200_ctx* c, CUstream st, AttnView* v, CUdeviceptr* tmp) {
 }
 
 // The 128-byte swizzled map of v with dims (D, rows, heads, axis 0).  A load (box 64 x rows x heads) reads the input dtype; a
-// store (out and the grads: 128-byte x 64-row boxes) moves raw 16- or 32-bit words.
+// store (out and the grads: 128-byte x 64-row boxes) moves raw 16- or 32-bit words.  An fp8 cache moves raw bytes, 128 (a
+// whole head, D <= 128) per box row.
 static int attn_map(b200_ctx* c, CUtensorMap* m, const AttnView& v, bool store, uint32_t rows = 64, uint32_t heads = 1) {
   const CUtensorMapDataType dt = v.esz == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                 : v.esz == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8
                                  : store    ? CU_TENSOR_MAP_DATA_TYPE_UINT16
                                  : v.dt == B200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  const uint32_t box[4] = {store ? (uint32_t)(128 / v.esz) : 64u, rows, heads, 1};
+  const uint32_t box[4] = {store || v.esz == 1 ? (uint32_t)(128 / v.esz) : 64u, rows, heads, 1};
   const uint64_t dims[4] = {v.shape[3], v.rows(), v.heads(), v.shape[0]}, strides[3] = {v.s_row(), v.s_head(), v.s_batch()};
   return encode_tmap4(c, m, dt, v.esz, v.ptr, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
@@ -4708,22 +4715,41 @@ static uint32_t kv_splits(uint64_t units, uint64_t nkb, int sms) {
   return (uint32_t)best_n;
 }
 
+// An fp8 KV cache: its format and the f32 [Hkv] per-head scales (device pointers, read by the kernels only).
+struct KvFp8 {
+  b200_dtype cache;
+  b200_dptr k_scale, v_scale;
+};
+
+static int kv_check_fp8(const char* what, const KvFp8* f8) {
+  if (f8 && f8->cache != B200_F8E4M3 && f8->cache != B200_F8E5M2)
+    return fail(B200_ERR_UNSUPPORTED, "%s: cache dtype %d unsupported (f8e4m3, f8e5m2)", what, (int)f8->cache);
+  return B200_OK;
+}
+
+static int kv_check_scales(const char* what, const KvFp8* f8) {
+  if (!f8) return B200_OK;
+  if (!f8->k_scale || !f8->v_scale) return fail(B200_ERR_INVALID_ARG, "%s: null k_scale or v_scale", what);
+  if (f8->k_scale % 4 || f8->v_scale % 4) return fail(B200_ERR_INVALID_ARG, "%s: k_scale and v_scale must be 4-byte aligned", what);
+  return B200_OK;
+}
+
 // Attention of q against a paged KV cache (see cubecl_b200.h): one attn_kv_* launch, plus attn_kv_combine_* when the keys
-// are split.
-extern "C" int b200_attention_kvcache(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr q,
-                                      const uint64_t* q_shape, const uint64_t* q_strides, b200_dptr k_cache, const uint64_t* kc_shape,
-                                      const uint64_t* kc_strides, b200_dptr v_cache, const uint64_t* vc_shape, const uint64_t* vc_strides,
-                                      b200_dptr block_table, const uint64_t* bt_shape, const uint64_t* bt_strides, b200_dptr cache_seqlens,
-                                      b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides, b200_dptr lse,
-                                      const b200_attention_args* args) {
-  CTX_ENTER(c);
-  const char* what = "attention_kvcache";
+// are split.  f8: an fp8 cache (b200_attention_kvcache_fp8), else the caches hold the input dtype.
+static int kv_attend(b200_ctx* c, b200_stream s, const char* what, b200_dtype in_dtype, const KvFp8* f8, b200_dtype out_dtype, b200_dptr q,
+                     const uint64_t* q_shape, const uint64_t* q_strides, b200_dptr k_cache, const uint64_t* kc_shape,
+                     const uint64_t* kc_strides, b200_dptr v_cache, const uint64_t* vc_shape, const uint64_t* vc_strides,
+                     b200_dptr block_table, const uint64_t* bt_shape, const uint64_t* bt_strides, b200_dptr cache_seqlens,
+                     b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides, b200_dptr lse,
+                     const b200_attention_args* args) {
   auto ull = [](uint64_t x) { return (unsigned long long)x; };
   if (!q_shape || !kc_shape || !vc_shape || !out_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
   if (block_table && !bt_shape) return fail(B200_ERR_INVALID_ARG, "%s: null block-table shape", what);
   int rc = attn_check_in_dtype(what, in_dtype);
   if (!rc) rc = attn_check_out_dtype(what, "output", in_dtype, out_dtype);
+  if (!rc) rc = kv_check_fp8(what, f8);
   if (rc) return rc;
+  const b200_dtype cache_dtype = f8 ? f8->cache : in_dtype;
   const uint64_t B = q_shape[0], Hq = q_shape[1], Sq = q_shape[2], D = q_shape[3];
   const uint64_t P = kc_shape[0], page = kc_shape[1], Hkv = kc_shape[2];
   if (kc_shape[3] != D)
@@ -4750,8 +4776,9 @@ extern "C" int b200_attention_kvcache(b200_ctx* c, b200_stream s, b200_dtype in_
   if (!q || !k_cache || !v_cache || !cache_seqlens || !out) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
   if (lse % 4 || cache_seqlens % 4 || block_table % 4)
     return fail(B200_ERR_INVALID_ARG, "%s: lse, cache_seqlens and block_table must be 4-byte aligned", what);
+  if ((rc = kv_check_scales(what, f8))) return rc;
   AttnView qv = attn_view(q, in_dtype, q_shape, q_strides, kAttnBHSD), ov = attn_view(out, out_dtype, out_shape, out_strides, kAttnBHSD);
-  const AttnView kv = attn_view(k_cache, in_dtype, kc_shape, kc_strides, kAttnBSHD), vv = attn_view(v_cache, in_dtype, vc_shape, vc_strides, kAttnBSHD);
+  const AttnView kv = attn_view(k_cache, cache_dtype, kc_shape, kc_strides, kAttnBSHD), vv = attn_view(v_cache, cache_dtype, vc_shape, vc_strides, kAttnBSHD);
   if ((rc = attn_check_out_view(what, "out", ov)) || (rc = attn_check_caches(what, kv, vv))) return rc;
 
   const uint64_t G = Hq / Hkv;
@@ -4794,15 +4821,19 @@ extern "C" int b200_attention_kvcache(b200_ctx* c, b200_stream s, b200_dtype in_
     p.nsplit = nsplit; p.bps = (uint32_t)bps;
     p.causal = args->causal != 0 ? 1u : 0u;
     p.scale_log2 = attn_scale_log2(args->scale);
+    if (f8) { p.k_scale = f8->k_scale; p.v_scale = f8->v_scale; }
     CUfunction f = nullptr;
     const std::string in_tag = dt_tag(in_dtype), out_tag = dt_tag(out_dtype);
-    if (!rc) rc = get_func(c, "attn_kv_" + in_tag + "_d" + std::to_string(DB) + "_" + out_tag, &f);
-    const unsigned smem = 1024 + (DB / 64) * (kAttnKvRows + 2 * kAttnKvStages * kAttnKvBlock) * 128 + kAttnKvBarBytes;
+    const std::string fmt = !f8 ? "" : f8->cache == B200_F8E5M2 ? "_e5m2" : "_e4m3";
+    if (!rc) rc = get_func(c, "attn_kv_" + in_tag + fmt + "_d" + std::to_string(DB) + "_" + out_tag, &f);
+    const unsigned smem = !f8 ? 1024 + (DB / 64) * (kAttnKvRows + 2 * kAttnKvStages * kAttnKvBlock) * 128 + kAttnKvBarBytes
+                              : 1024 + (DB / 64) * (kAttnKvRows + 3 * kAttnKvBlock) * 128 + kAttnKvF8Stages * 2 * kAttnKvBlock * 128 +
+                                    kAttnKvF8BarBytes;
     if (!rc) rc = attn_set_smem(c, f, smem);
     void* kargs[] = {&mq, &mk, &mv, &p};
     if (!rc) rc = launch(c, f, (unsigned)ctas, 1, 1, kAttnKvThreads, smem, 1, st, kargs);
     if (!rc && nsplit > 1) {
-      rc = get_func(c, "attn_kv_combine_" + out_tag, &f);
+      rc = get_func(c, std::string(f8 ? "attn_kv_combine_fp8_" : "attn_kv_combine_") + out_tag, &f);
       void* cargs[] = {&p};
       if (!rc) rc = launch(c, f, (unsigned)((rows * (D / 4) + kAttnKvCombineThreads - 1) / kAttnKvCombineThreads), 1, 1,
                            kAttnKvCombineThreads, 0, 1, st, cargs);
@@ -4813,15 +4844,40 @@ extern "C" int b200_attention_kvcache(b200_ctx* c, b200_stream s, b200_dtype in_
   return rc;
 }
 
-// Scatter of new tokens into a paged KV cache (see cubecl_b200.h): one attn_kv_write launch.
-extern "C" int b200_kvcache_write(b200_ctx* c, b200_stream s, b200_dtype dtype, b200_dptr k_new, const uint64_t* kn_shape,
-                                  const uint64_t* kn_strides, b200_dptr v_new, const uint64_t* vn_shape, const uint64_t* vn_strides,
-                                  b200_dptr k_cache, const uint64_t* kc_shape, const uint64_t* kc_strides, b200_dptr v_cache,
-                                  const uint64_t* vc_shape, const uint64_t* vc_strides, b200_dptr slot_mapping) {
+extern "C" int b200_attention_kvcache(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr q,
+                                      const uint64_t* q_shape, const uint64_t* q_strides, b200_dptr k_cache, const uint64_t* kc_shape,
+                                      const uint64_t* kc_strides, b200_dptr v_cache, const uint64_t* vc_shape, const uint64_t* vc_strides,
+                                      b200_dptr block_table, const uint64_t* bt_shape, const uint64_t* bt_strides, b200_dptr cache_seqlens,
+                                      b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides, b200_dptr lse,
+                                      const b200_attention_args* args) {
   CTX_ENTER(c);
-  const char* what = "kvcache_write";
+  return kv_attend(c, s, "attention_kvcache", in_dtype, nullptr, out_dtype, q, q_shape, q_strides, k_cache, kc_shape, kc_strides, v_cache,
+                   vc_shape, vc_strides, block_table, bt_shape, bt_strides, cache_seqlens, out, out_shape, out_strides, lse, args);
+}
+
+extern "C" int b200_attention_kvcache_fp8(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype cache_dtype, b200_dtype out_dtype,
+                                          b200_dptr q, const uint64_t* q_shape, const uint64_t* q_strides, b200_dptr k_cache,
+                                          const uint64_t* kc_shape, const uint64_t* kc_strides, b200_dptr v_cache, const uint64_t* vc_shape,
+                                          const uint64_t* vc_strides, b200_dptr block_table, const uint64_t* bt_shape,
+                                          const uint64_t* bt_strides, b200_dptr cache_seqlens, b200_dptr k_scale, b200_dptr v_scale,
+                                          b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides, b200_dptr lse,
+                                          const b200_attention_args* args) {
+  CTX_ENTER(c);
+  const KvFp8 f8{cache_dtype, k_scale, v_scale};
+  return kv_attend(c, s, "attention_kvcache_fp8", in_dtype, &f8, out_dtype, q, q_shape, q_strides, k_cache, kc_shape, kc_strides, v_cache,
+                   vc_shape, vc_strides, block_table, bt_shape, bt_strides, cache_seqlens, out, out_shape, out_strides, lse, args);
+}
+
+// Scatter of new tokens into a paged KV cache (see cubecl_b200.h): one attn_kv_write launch, or attn_kv_write_fp8 (f8: an
+// fp8 cache, quantized with its per-head scales).
+static int kv_write(b200_ctx* c, b200_stream s, const char* what, b200_dtype dtype, const KvFp8* f8, b200_dptr k_new, const uint64_t* kn_shape,
+                    const uint64_t* kn_strides, b200_dptr v_new, const uint64_t* vn_shape, const uint64_t* vn_strides,
+                    b200_dptr k_cache, const uint64_t* kc_shape, const uint64_t* kc_strides, b200_dptr v_cache,
+                    const uint64_t* vc_shape, const uint64_t* vc_strides, b200_dptr slot_mapping) {
   if (!kn_shape || !vn_shape || !kc_shape || !vc_shape) return fail(B200_ERR_INVALID_ARG, "%s: null shape", what);
   if (dtype != B200_F16 && dtype != B200_BF16) return fail(B200_ERR_UNSUPPORTED, "%s: dtype %d unsupported (f16, bf16)", what, (int)dtype);
+  if (int rc0 = kv_check_fp8(what, f8)) return rc0;
+  const b200_dtype cache_dtype = f8 ? f8->cache : dtype;
   const uint64_t B = kn_shape[0], Snew = kn_shape[1], Hkv = kn_shape[2], D = kn_shape[3];
   const uint64_t P = kc_shape[0], page = kc_shape[1];
   if (memcmp(vn_shape, kn_shape, 4 * sizeof(uint64_t)))
@@ -4835,7 +4891,8 @@ extern "C" int b200_kvcache_write(b200_ctx* c, b200_stream s, b200_dtype dtype, 
   if (units == 0) return B200_OK;
   if (!k_new || !v_new || !k_cache || !v_cache || !slot_mapping) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
   if (slot_mapping % 4) return fail(B200_ERR_INVALID_ARG, "%s: slot_mapping must be 4-byte aligned", what);
-  const AttnView kc = attn_view(k_cache, dtype, kc_shape, kc_strides, kAttnBSHD), vc = attn_view(v_cache, dtype, vc_shape, vc_strides, kAttnBSHD);
+  if (int rc0 = kv_check_scales(what, f8)) return rc0;
+  const AttnView kc = attn_view(k_cache, cache_dtype, kc_shape, kc_strides, kAttnBSHD), vc = attn_view(v_cache, cache_dtype, vc_shape, vc_strides, kAttnBSHD);
   int rc = attn_check_caches(what, kc, vc);
   if (rc) return rc;
   // the kernel moves 16-byte units: other views of the new tokens are gathered into a compact copy first
@@ -4854,8 +4911,13 @@ extern "C" int b200_kvcache_write(b200_ctx* c, b200_stream s, b200_dtype dtype, 
     p.units = units;
     p.Snew = (uint32_t)Snew; p.Hkv = (uint32_t)Hkv; p.D = (uint32_t)D; p.page = (uint32_t)page;
     p.slot_end = P * page;
+    if (f8) {
+      p.k_scale = f8->k_scale; p.v_scale = f8->v_scale;
+      p.in_bf16 = dtype == B200_BF16 ? 1u : 0u;
+      p.e5m2 = f8->cache == B200_F8E5M2 ? 1u : 0u;
+    }
     CUfunction f = nullptr;
-    rc = get_func(c, "attn_kv_write", &f);
+    rc = get_func(c, f8 ? "attn_kv_write_fp8" : "attn_kv_write", &f);
     void* kargs[] = {&p};
     const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((units + 255) / 256, (uint64_t)c->props.num_sms * 32));
     if (!rc) rc = launch(c, f, grid, 1, 1, 256, 0, 1, st, kargs);
@@ -4863,6 +4925,26 @@ extern "C" int b200_kvcache_write(b200_ctx* c, b200_stream s, b200_dtype dtype, 
   for (CUdeviceptr t : tmp)
     if (t) pool_free(c, t, st);
   return rc;
+}
+
+extern "C" int b200_kvcache_write(b200_ctx* c, b200_stream s, b200_dtype dtype, b200_dptr k_new, const uint64_t* kn_shape,
+                                  const uint64_t* kn_strides, b200_dptr v_new, const uint64_t* vn_shape, const uint64_t* vn_strides,
+                                  b200_dptr k_cache, const uint64_t* kc_shape, const uint64_t* kc_strides, b200_dptr v_cache,
+                                  const uint64_t* vc_shape, const uint64_t* vc_strides, b200_dptr slot_mapping) {
+  CTX_ENTER(c);
+  return kv_write(c, s, "kvcache_write", dtype, nullptr, k_new, kn_shape, kn_strides, v_new, vn_shape, vn_strides, k_cache, kc_shape,
+                  kc_strides, v_cache, vc_shape, vc_strides, slot_mapping);
+}
+
+extern "C" int b200_kvcache_write_fp8(b200_ctx* c, b200_stream s, b200_dtype dtype, b200_dtype cache_dtype, b200_dptr k_new,
+                                      const uint64_t* kn_shape, const uint64_t* kn_strides, b200_dptr v_new, const uint64_t* vn_shape,
+                                      const uint64_t* vn_strides, b200_dptr k_cache, const uint64_t* kc_shape, const uint64_t* kc_strides,
+                                      b200_dptr v_cache, const uint64_t* vc_shape, const uint64_t* vc_strides, b200_dptr slot_mapping,
+                                      b200_dptr k_scale, b200_dptr v_scale) {
+  CTX_ENTER(c);
+  const KvFp8 f8{cache_dtype, k_scale, v_scale};
+  return kv_write(c, s, "kvcache_write_fp8", dtype, &f8, k_new, kn_shape, kn_strides, v_new, vn_shape, vn_strides, k_cache, kc_shape,
+                  kc_strides, v_cache, vc_shape, vc_strides, slot_mapping);
 }
 
 extern "C" int b200_reduce_debug(b200_ctx* c, b200_stream s, uint64_t* words4) {

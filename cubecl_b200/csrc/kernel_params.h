@@ -302,6 +302,12 @@ struct AttnVarlenParams {
 // Workspace (nsplit > 1, ws != 0): f32 O [nsplit][rows][D], then f32 (m, l) [nsplit][rows][2], rows = B * Hq * Sq in
 // (b, h, i) order.  O is un-normalised, m is the split's row maximum of t = s * scale_log2 (-inf when the split saw no key) and
 // l its row sum of exp2(t - m).  attn_kv_combine_<out> (kAttnKvCombineThreads threads, one per 4 columns of a row) reads it.
+// fp8 caches (attn_kv_<in>_<e4m3|e5m2>_d<64|128>_<out>, cubin attention_kv_fp8): a K or V block arrives as 128-byte rows (one
+// box of 128 bytes x rows keys per load, columns >= D zero-filled) through kAttnKvF8Stages stages, and the consumer widens
+// it into 16-bit swizzled buffers: two K buffers (alternating blocks) and one V buffer.  Shared memory: 1024 + DB / 64 x
+// kAttnKvRows Q rows of 128 bytes + kAttnKvF8Stages x 2 x kAttnKvBlock x 128 + 3 x DB / 64 x kAttnKvBlock x 128 +
+// kAttnKvF8BarBytes.  k_scale and v_scale are f32 [Hkv]: t = s * (scale_log2 * k_scale[hk]), and v_scale[hk] multiplies the
+// un-normalised O (or, with splits, the combined sum) just before the division by l.  The workspace holds the unscaled O.
 constexpr int kAttnKvBlock = 64;
 constexpr int kAttnKvStages = 4;
 constexpr int kAttnKvRows = 64;
@@ -310,6 +316,8 @@ constexpr int kAttnKvBarBytes = 128;
 constexpr int kAttnKvMaxSplits = 128;
 constexpr int kAttnKvSplitCost = 2;   // the split plan's fixed cost of one CTA, in key blocks (prologue and epilogue)
 constexpr int kAttnKvCombineThreads = 256;
+constexpr int kAttnKvF8Stages = 8;
+constexpr int kAttnKvF8BarBytes = 256;
 struct AttnKvParams {
   uint64_t out;               // [B, Hq, Sq, D] view, unit D stride (direct path and combine)
   uint64_t o_sb, o_sh, o_ss;  // out strides in elements
@@ -326,6 +334,7 @@ struct AttnKvParams {
   uint32_t nsplit, bps;       // splits, key blocks per split
   uint32_t causal;            // 1: query i also needs j <= L - Sq + i (bottom-right)
   float scale_log2;           // scale * log2(e)
+  uint64_t k_scale, v_scale;  // fp8 caches: f32 [Hkv] scales (the 16-bit kernels do not read them)
 };
 
 // b200_kvcache_write (attn_kv_write): one thread per 16-byte unit of a (token, kv head) row, for k and v.  Token n = b * Snew + t
@@ -337,6 +346,10 @@ struct AttnKvWriteParams {
   uint64_t units;                                      // B * Snew * Hkv * D / 8
   uint32_t Snew, Hkv, D, page;
   uint64_t slot_end;                                   // P * page
+  // b200_kvcache_write_fp8 (attn_kv_write_fp8): one thread per 8 elements; element x of kv head hk is stored as
+  // sat_rn(x / scale[hk]) in the cache format.  The 16-bit attn_kv_write does not read these.
+  uint64_t k_scale, v_scale;                           // f32 [Hkv]
+  uint32_t in_bf16, e5m2;                              // new tokens bf16 (else f16); cache e5m2 (else e4m3)
 };
 
 // ================================================================================================ conv_grouped.cu

@@ -736,6 +736,45 @@ int b200_kvcache_write(b200_ctx* ctx, b200_stream s, b200_dtype dtype,
                        b200_dptr v_cache, const uint64_t* vc_shape, const uint64_t* vc_strides,
                        b200_dptr slot_mapping);
 
+/* ---- fp8 KV caches (vLLM's kv_cache_dtype="fp8", FlashAttention-3's k_descale / v_descale) ------------------------------
+ * b200_attention_kvcache with the caches in B200_F8E4M3 or B200_F8E5M2 (cache_dtype, both caches) and two compact f32 [Hkv]
+ * device arrays k_scale and v_scale (read by the kernels only: no synchronisation, graph-capturable; a per-tensor scale is the
+ * same value in every entry).  The cache holds K = k_scale[hk] * k8 and V = v_scale[hk] * v8.  q is f16 or bf16, out q's dtype
+ * or f32; shapes, paging, block_table, cache_seqlens, bottom-right causal, stale slots, lse and the errors are those of
+ * b200_attention_kvcache.
+ * Numerics: K and V are widened on chip to q's dtype (exact: every e4m3 and e5m2 value is an f16 and a bf16 value); t = s * c
+ * with s the f32 score of q against the widened K and c = (scale * log2 e) * k_scale[hk], one f32 product per CTA; the online
+ * softmax and P rounding of b200_attention_kvcache; v_scale is applied once to the un-normalised f32 sum just before the
+ * division: out = (v_scale * O) / l rounded once, and with several splits out = (v_scale * sum_s w_s O_s) / sum_s w_s l_s.
+ * lse does not depend on v_scale.  So power-of-two scales (and scales of 1) give bit for bit the output of
+ * b200_attention_kvcache on the dequantized 16-bit cache.
+ * Views: a cache is read in place with a unit D stride and a 16-byte aligned base and strides, in bytes: a compact fp8 cache
+ * needs D % 16 == 0.  Errors beyond b200_attention_kvcache's: B200_ERR_UNSUPPORTED for a cache dtype that is not fp8;
+ * B200_ERR_INVALID_ARG for a null or not 4-byte aligned k_scale or v_scale.
+ * Launches: one attn_kv_<in>_<e4m3|e5m2>_d<64|128>_<out> launch (split count and m-tile as b200_attention_kvcache), plus
+ * attn_kv_combine_fp8_<out> when the keys are split.  The plan's k_cache and v_cache maps have esz=1 and box (128, rows, 1, 1). */
+int b200_attention_kvcache_fp8(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b200_dtype cache_dtype, b200_dtype out_dtype,
+                               b200_dptr q, const uint64_t* q_shape, const uint64_t* q_strides,
+                               b200_dptr k_cache, const uint64_t* kc_shape, const uint64_t* kc_strides,
+                               b200_dptr v_cache, const uint64_t* vc_shape, const uint64_t* vc_strides,
+                               b200_dptr block_table, const uint64_t* bt_shape, const uint64_t* bt_strides,
+                               b200_dptr cache_seqlens, b200_dptr k_scale, b200_dptr v_scale,
+                               b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides,
+                               b200_dptr lse, const b200_attention_args* args);
+
+/* b200_kvcache_write into fp8 caches (vLLM's reshape_and_cache with an fp8 cache): k_new and v_new are f16 or bf16 (dtype),
+ * the caches cache_dtype (B200_F8E4M3 or B200_F8E5M2), k_scale and v_scale compact f32 [Hkv] device arrays.  Each stored value
+ * is sat_rn(x / scale[hk]): an f32 division rounded to nearest, then RNE to the cache format with saturation to +-448 (e4m3)
+ * or +-57344 (e5m2); NaN stays NaN.  In torch: (x.float() / s).clamp(-max, max).to(float8).  Slots, views and errors as
+ * b200_kvcache_write, plus b200_attention_kvcache_fp8's cache-dtype and scale errors.  One attn_kv_write_fp8 launch (16-byte
+ * loads, 8-byte stores). */
+int b200_kvcache_write_fp8(b200_ctx* ctx, b200_stream s, b200_dtype dtype, b200_dtype cache_dtype,
+                           b200_dptr k_new, const uint64_t* kn_shape, const uint64_t* kn_strides,
+                           b200_dptr v_new, const uint64_t* vn_shape, const uint64_t* vn_strides,
+                           b200_dptr k_cache, const uint64_t* kc_shape, const uint64_t* kc_strides,
+                           b200_dptr v_cache, const uint64_t* vc_shape, const uint64_t* vc_strides,
+                           b200_dptr slot_mapping, b200_dptr k_scale, b200_dptr v_scale);
+
 /* ---- collectives: ServerCommunication (server/base.rs:632-739), CUDA impl cubecl-cuda/src/compute/server.rs:666-926 -- */
 #define B200_UNIQUE_ID_BYTES 128
 int b200_comm_get_unique_id(b200_ctx* ctx, void* id128);            /* ncclGetUniqueId (communication.rs:11-25 holds it per device set) */

@@ -510,6 +510,47 @@ inline void kvcache_write(ComputeClient& client, const TensorHandle& k_new, cons
                                     v_cache.strides.data(), slot_mapping.handle.ptr());
   if (rc != B200_OK) client.defer(b200_last_error());
 }
+
+/// launch_kvcache against an fp8 cache: k_cache, v_cache F8E4M3 or F8E5M2 (one dtype) hold K = k_scale[hk] * k8 and
+/// V = v_scale[hk] * v8, with k_scale, v_scale compact f32 [Hkv] tensors.  See b200_attention_kvcache_fp8 in cubecl_b200.h.
+/// Errors are deferred to client.sync().
+inline void launch_kvcache_fp8(ComputeClient& client, const TensorHandle& q, const TensorHandle& k_cache, const TensorHandle& v_cache,
+                               const TensorHandle& cache_seqlens, const TensorHandle& k_scale, const TensorHandle& v_scale,
+                               const TensorHandle& out, const TensorHandle* block_table, float scale, bool causal = false,
+                               const TensorHandle* lse = nullptr) {
+  if (q.shape.size() != 4 || k_cache.shape.size() != 4 || v_cache.shape.size() != 4 || out.shape.size() != 4 ||
+      (block_table && block_table->shape.size() != 2) || k_cache.dtype != v_cache.dtype) {
+    client.defer("InvalidArgument: attention_kvcache_fp8 needs rank-4 q, caches and out, caches of one dtype and a rank-2 block table");
+    return;
+  }
+  const b200_attention_args args{scale, causal ? 1 : 0};
+  const int rc = b200_attention_kvcache_fp8(
+      client.raw(), nullptr, static_cast<b200_dtype>(q.dtype), static_cast<b200_dtype>(k_cache.dtype), static_cast<b200_dtype>(out.dtype),
+      q.handle.ptr(), q.shape.data(), q.strides.data(), k_cache.handle.ptr(), k_cache.shape.data(), k_cache.strides.data(),
+      v_cache.handle.ptr(), v_cache.shape.data(), v_cache.strides.data(), block_table ? block_table->handle.ptr() : 0,
+      block_table ? block_table->shape.data() : nullptr, block_table ? block_table->strides.data() : nullptr, cache_seqlens.handle.ptr(),
+      k_scale.handle.ptr(), v_scale.handle.ptr(), out.handle.ptr(), out.shape.data(), out.strides.data(), lse ? lse->handle.ptr() : 0,
+      &args);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+
+/// kvcache_write into fp8 caches: each value x of kv head hk is stored as sat_rn(x / scale[hk]).  See b200_kvcache_write_fp8 in
+/// cubecl_b200.h.  Errors are deferred to client.sync().
+inline void kvcache_write_fp8(ComputeClient& client, const TensorHandle& k_new, const TensorHandle& v_new, const TensorHandle& k_cache,
+                              const TensorHandle& v_cache, const TensorHandle& slot_mapping, const TensorHandle& k_scale,
+                              const TensorHandle& v_scale) {
+  if (k_new.shape.size() != 4 || v_new.shape.size() != 4 || k_cache.shape.size() != 4 || v_cache.shape.size() != 4 ||
+      k_cache.dtype != v_cache.dtype) {
+    client.defer("InvalidArgument: kvcache_write_fp8 needs rank-4 new tokens and caches of one dtype");
+    return;
+  }
+  const int rc = b200_kvcache_write_fp8(client.raw(), nullptr, static_cast<b200_dtype>(k_new.dtype), static_cast<b200_dtype>(k_cache.dtype),
+                                        k_new.handle.ptr(), k_new.shape.data(), k_new.strides.data(), v_new.handle.ptr(), v_new.shape.data(),
+                                        v_new.strides.data(), k_cache.handle.ptr(), k_cache.shape.data(), k_cache.strides.data(),
+                                        v_cache.handle.ptr(), v_cache.shape.data(), v_cache.strides.data(), slot_mapping.handle.ptr(),
+                                        k_scale.handle.ptr(), v_scale.handle.ptr());
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
 }  // namespace attention
 
 namespace reduce {

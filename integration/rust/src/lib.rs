@@ -674,6 +674,54 @@ impl Context {
         ))
     }
 
+    /// [`Context::attention_kvcache`] against an fp8 cache: `k_cache`, `v_cache` in `cache_dtype` (F8E4M3 or F8E5M2) hold
+    /// K = k_scale[hk] * k8 and V = v_scale[hk] * v8, with `k_scale`, `v_scale` compact f32 [Hkv] device buffers.  See
+    /// b200_attention_kvcache_fp8 in cubecl_b200.h.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::attention_kvcache`]; `k_scale` and `v_scale` must hold Hkv f32 values.
+    pub unsafe fn attention_kvcache_fp8(
+        &mut self, stream: b200_stream, in_dtype: DType, cache_dtype: DType, out_dtype: DType, q: &TensorView, k_cache: &TensorView,
+        v_cache: &TensorView, block_table: Option<&TensorView>, cache_seqlens: b200_dptr, k_scale: b200_dptr, v_scale: b200_dptr,
+        out: &TensorView, lse: b200_dptr, scale: f32, causal: bool,
+    ) -> Result<(), Error> {
+        for t in [q, k_cache, v_cache, out] {
+            assert!(t.shape.len() == 4 && t.strides.len() == 4);
+        }
+        if let Some(t) = block_table {
+            assert!(t.shape.len() == 2 && t.strides.len() == 2);
+        }
+        let a = sys::b200_attention_args { scale, causal: causal as i32 };
+        let (bt, bt_shape, bt_strides) = match block_table {
+            Some(t) => (t.ptr, t.shape.as_ptr(), t.strides.as_ptr()),
+            None => (0, std::ptr::null(), std::ptr::null()),
+        };
+        check(sys::b200_attention_kvcache_fp8(
+            self.0, stream, in_dtype as c_int, cache_dtype as c_int, out_dtype as c_int, q.ptr, q.shape.as_ptr(), q.strides.as_ptr(),
+            k_cache.ptr, k_cache.shape.as_ptr(), k_cache.strides.as_ptr(), v_cache.ptr, v_cache.shape.as_ptr(), v_cache.strides.as_ptr(),
+            bt, bt_shape, bt_strides, cache_seqlens, k_scale, v_scale, out.ptr, out.shape.as_ptr(), out.strides.as_ptr(), lse, &a,
+        ))
+    }
+
+    /// [`Context::kvcache_write`] into fp8 caches (`cache_dtype` F8E4M3 or F8E5M2): each value x of kv head hk is stored as
+    /// sat_rn(x / scale[hk]).  See b200_kvcache_write_fp8.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::kvcache_write`]; `k_scale` and `v_scale` must hold Hkv f32 values.
+    pub unsafe fn kvcache_write_fp8(
+        &mut self, stream: b200_stream, dtype: DType, cache_dtype: DType, k_new: &TensorView, v_new: &TensorView, k_cache: &TensorView,
+        v_cache: &TensorView, slot_mapping: b200_dptr, k_scale: b200_dptr, v_scale: b200_dptr,
+    ) -> Result<(), Error> {
+        for t in [k_new, v_new, k_cache, v_cache] {
+            assert!(t.shape.len() == 4 && t.strides.len() == 4);
+        }
+        check(sys::b200_kvcache_write_fp8(
+            self.0, stream, dtype as c_int, cache_dtype as c_int, k_new.ptr, k_new.shape.as_ptr(), k_new.strides.as_ptr(), v_new.ptr,
+            v_new.shape.as_ptr(), v_new.strides.as_ptr(), k_cache.ptr, k_cache.shape.as_ptr(), k_cache.strides.as_ptr(), v_cache.ptr,
+            v_cache.shape.as_ptr(), v_cache.strides.as_ptr(), slot_mapping, k_scale, v_scale,
+        ))
+    }
+
     /// Grouped / depthwise [`Context::conv2d`]: w [Cout, KH, KW, C / groups].  See b200_conv2d_grouped in cubecl_b200.h.
     ///
     /// # Safety
