@@ -28,6 +28,12 @@ rows of k and v (compact i32 [B + 1] device arrays, never read by the host).  wi
 visible to query i iff j < Lk and i + off - left <= j <= i + off + right with off = Lk - Lq (-1: unbounded), so (-1, 0) is
 bottom-right causal.  lse is a compact f32 [Hq, Tq].  The dense kernels with per-sequence addressing (-DATTN_VARLEN builds of
 csrc/attention.cu and attention_bwd.cu); see b200_attention_varlen and b200_attention_varlen_backward.
+
+Paged variable-length attention (launch_varlen_paged, for chunked prefill and prefix caching; flash_attn_varlen_func with a
+block_table): packed q [Tq, Hq, D] as launch_varlen's against a paged cache as launch_kvcache's.  Sequence b's Lq_b new queries
+are the last of its cache_seqlens[b] cached keys (write the chunk's keys with kvcache_write first), under launch_varlen's window
+rule.  Out and lse are bit for bit those of launch_varlen on each sequence's cached keys packed contiguously.  The varlen
+forward kernel with paged K / V addressing (-DATTN_VARLEN -DATTN_PAGED); see b200_attention_varlen_paged.
 """
 from __future__ import annotations
 
@@ -367,3 +373,50 @@ def launch_varlen_backward_alloc(client: ComputeClient, q: TensorHandle, k: Tens
     launch_varlen_backward(client, q, k, v, out, dout, lse, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, dq, dk, dv,
                            scale=scale, window_size=window_size, stream=stream)
     return dq, dk, dv
+
+
+@_defers_errors
+def launch_varlen_paged(client: ComputeClient, q: TensorHandle, k_cache: TensorHandle, v_cache: TensorHandle, cu_seqlens_q: TensorHandle,
+                        cache_seqlens: TensorHandle, max_seqlen_q: int, max_seqlen_k: int, out: TensorHandle,
+                        block_table: TensorHandle | None = None, scale: float | None = None, window_size=(-1, -1),
+                        lse: TensorHandle | None = None, stream=None) -> None:
+    """Enqueue packed queries q [Tq, Hq, D] (rows [cu_seqlens_q[b], cu_seqlens_q[b + 1]) of sequence b; compact i32 [B + 1])
+    against a paged cache k_cache, v_cache [P, page, Hkv, D] in q's dtype (views by strides): sequence b has its first
+    cache_seqlens[b] keys (compact i32 [B], read on the device, clamped to max_seqlen_k), key j at row j % page of page
+    block_table[b, j / page] (i32 [B, max_pages]; None: page b).  window_size as launch_varlen's with off = Lk - Lq: the new
+    queries are the last keys, (-1, 0) is bottom-right causal.  out [Tq, Hq, D]; lse: an optional compact f32 [Hq, Tq] tensor.
+    Rows outside every sequence are not written.  Never raises for launch problems: errors are deferred to client.sync()."""
+    what = "attention_varlen_paged"
+    _check_rank(what, 3, (("q", q), ("out", out)), " [T, H, D]")
+    _check_rank(what, 4, (("k_cache", k_cache), ("v_cache", v_cache)), " [P, page, Hkv, D]")
+    if k_cache.dtype in _FP8 or v_cache.dtype in _FP8:
+        raise B200Error(7, f"{what}: fp8 caches unsupported (the caches hold q's dtype)")
+    _check_same_dtype(what, (("q", q), ("k_cache", k_cache), ("v_cache", v_cache)))
+    if cu_seqlens_q.dtype != "i32" or not cu_seqlens_q.is_contiguous() or len(cu_seqlens_q.shape) != 1 or cu_seqlens_q.shape[0] < 1:
+        raise B200Error(6, f"{what}: cu_seqlens_q must be a compact i32 [B + 1] tensor")
+    B = cu_seqlens_q.shape[0] - 1
+    if cache_seqlens.dtype != "i32" or not cache_seqlens.is_contiguous() or list(cache_seqlens.shape) != [B]:
+        raise B200Error(6, f"{what}: cache_seqlens must be a compact i32 [B] = [{B}] tensor")
+    if block_table is not None and (block_table.dtype != "i32" or len(block_table.shape) != 2):
+        raise B200Error(6, f"{what}: block_table must be an i32 [B, max_pages] tensor")
+    _check_lse(what, lse, "[Hq, Tq]", [q.shape[1], q.shape[0]])
+    left, right = (int(w) for w in window_size)
+    args = _ffi.AttentionVarlenArgs(_scale(scale, q.shape[2]), left, right, int(max_seqlen_q), int(max_seqlen_k))
+    _used_on(stream, q, k_cache, v_cache, cu_seqlens_q, cache_seqlens, out, block_table, lse)
+    bt = _view_args((block_table,)) if block_table is not None else [C.c_uint64(0), None, None]
+    _ffi.check(client._lib.b200_attention_varlen_paged(
+        client._ctx, stream, DTYPES[q.dtype], DTYPES[out.dtype], *_view_args((q, k_cache, v_cache)), *bt, _ptr(cu_seqlens_q),
+        _ptr(cache_seqlens), C.c_uint64(B), *_view_args((out,)), _ptr(lse), C.byref(args)))
+
+
+def launch_varlen_paged_alloc(client: ComputeClient, q: TensorHandle, k_cache: TensorHandle, v_cache: TensorHandle,
+                              cu_seqlens_q: TensorHandle, cache_seqlens: TensorHandle, max_seqlen_q: int, max_seqlen_k: int,
+                              block_table: TensorHandle | None = None, scale: float | None = None, window_size=(-1, -1),
+                              out_dtype: str | None = None, return_lse: bool = False, stream=None):
+    """Convenience: allocate a compact out [Tq, Hq, D] (and, with return_lse, a compact f32 lse [Hq, Tq]), then
+    launch_varlen_paged.  Rows outside every sequence are left as allocated.  Returns out, or (out, lse)."""
+    out = TensorHandle.empty_contiguous(client, list(q.shape), out_dtype or q.dtype)
+    lse = TensorHandle.empty_contiguous(client, [q.shape[1], q.shape[0]], "f32") if return_lse else None
+    launch_varlen_paged(client, q, k_cache, v_cache, cu_seqlens_q, cache_seqlens, max_seqlen_q, max_seqlen_k, out,
+                        block_table=block_table, scale=scale, window_size=window_size, lse=lse, stream=stream)
+    return (out, lse) if return_lse else out

@@ -21,6 +21,10 @@
 // The epilogue stages O / l in the consumer's own rows of the Q tile (SWIZZLE_128B, 128-byte column groups) and leaves
 // through 4-D TMA stores that the unit clips at Sq and D; lse is written for rows < Sq.
 //
+// Paged varlen (-DATTN_VARLEN -DATTN_PAGED; capi.cpp: b200_attention_varlen_paged): the varlen body with K and V read from a
+// paged KV cache through a block table (warp 0 of the producer warpgroup resolves page ids; lane 0 issues one load per chunk of
+// `rows` keys that starts below the sequence's cache length).  The consumers are varlen's, so are the numerics.
+//
 // Compiled to a cubin (no host code here): nvcc -cubin -gencode arch=compute_90a,code=sm_90a
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -33,8 +37,9 @@ using namespace b200;
 
 namespace {
 
-// VL: the varlen kernels (P = AttnVarlenParams; kernel_params.h); the dense kernels have VL = false and P = AttnParams
-template <int KIND, int DB, int OUT, bool VL, class P>
+// VL: the varlen kernels (P = AttnVarlenParams; kernel_params.h); the dense kernels have VL = false and P = AttnParams.
+// PG (with VL): the paged varlen kernels (P = AttnVarlenPagedParams): K and V come from a paged cache, the rest is varlen's
+template <int KIND, int DB, int OUT, bool VL, bool PG, class P>
 __device__ __forceinline__ void attn_body(const CUtensorMap* tq, const CUtensorMap* tk, const CUtensorMap* tv, const CUtensorMap* to,
                                           const P& p) {
   constexpr int NCH = DB / 64;                                // 128-byte (64-element) column chunks of a head
@@ -67,9 +72,10 @@ __device__ __forceinline__ void attn_body(const CUtensorMap* tq, const CUtensorM
   int qrow = q0, krow = 0, bb = static_cast<int>(b);
   int Lq = 0, Lk = 0, off = 0;   // varlen: the sequence's lengths, off = Lk - Lq
   if constexpr (VL) {
-    int qs, ks;
+    int qs, ks = 0;
     varlen_seq(p.cu_q, b, p.Tq, p.max_q, qs, Lq);
-    varlen_seq(p.cu_k, b, p.Tk, p.max_k, ks, Lk);
+    if constexpr (PG) Lk = min(max(__ldg(reinterpret_cast<const int*>(p.seqlens) + b), 0), static_cast<int>(min(p.max_k, p.cap)));
+    else varlen_seq(p.cu_k, b, p.Tk, p.max_k, ks, Lk);
     if (q0 >= Lq) return;   // past the sequence: no load, no store
     off = Lk - Lq;
     int lo, hi;
@@ -103,7 +109,64 @@ __device__ __forceinline__ void attn_body(const CUtensorMap* tq, const CUtensorM
   if (wg == 0) {
     // ===================================================================== TMA producer (one thread)
     setmaxnreg_dec<40>();
-    if (threadIdx.x == 0) {
+    if constexpr (PG) {
+      // paged: warp 0 reads the block table 32 chunks of `rows` keys at a time, one batch ahead (chunk indices from the CTA's
+      // first band block); lane 0 issues one load per chunk that starts below Lk.  Stages keep stale rows where a chunk is not
+      // loaded: the consumers mask those keys and zero their V rows, as for the keys past Lk of a contiguous sequence.
+      if (threadIdx.x < 32) {
+        const uint32_t lane = threadIdx.x, R = p.rows, per = kAttnBlock / R;   // keys per load, loads per block (1 to 8)
+        if (lane == 0) {
+          mbar_arrive_expect_tx(q_bar, TILE);
+#pragma unroll
+          for (int c = 0; c < NCH; ++c) tma_load_4d(sq + c * CHUNK, tq, q_bar, c * 64, qrow, static_cast<int>(h), 0);
+        }
+        const int* tbl = reinterpret_cast<const int*>(p.table);
+        // page id of chunk c (keys c R .. c R + R - 1); never reads a table entry at or past ceil(Lk / page)
+        auto page_of = [&](uint32_t c) -> int {
+          const uint32_t j0 = c * R;
+          if (j0 >= static_cast<uint32_t>(Lk)) return 0;
+          return tbl ? tbl[b * p.t_sb + (j0 / p.page) * p.t_sp] : static_cast<int>(b);
+        };
+        uint32_t cbase = kb_lo * per;
+        int cur = page_of(cbase + lane), nxt = page_of(cbase + 32u + lane);
+        uint32_t s = 0, ph = 0;
+        for (uint32_t kb = kb_lo; kb < nkb; ++kb) {
+          const uint32_t c = kb * per;
+          if (c - cbase == 32u) {   // 32 % per == 0: batches start on block boundaries
+            cbase += 32u;
+            cur = nxt;
+            nxt = page_of(cbase + 32u + lane);
+          }
+          const int k0 = static_cast<int>(kb * kAttnBlock);
+          const uint32_t nload = min(per, static_cast<uint32_t>(Lk - k0 + static_cast<int>(R) - 1) / R);   // chunks below Lk
+          mbar_wait(empty(s), ph ^ 1u);
+          if (lane == 0) {
+            mbar_arrive_expect_tx(full_k(s), nload * NCH * R * 128u);
+            mbar_arrive_expect_tx(full_v(s), nload * NCH * R * 128u);
+          }
+          for (uint32_t i = 0; i < per; ++i) {
+            const int pg = __shfl_sync(0xFFFFFFFFu, cur, (c - cbase + i) & 31u);
+            const int row = static_cast<int>((static_cast<uint32_t>(k0) + i * R) % p.page);
+            if (lane == 0 && i < nload) {
+#pragma unroll
+              for (int cc = 0; cc < NCH; ++cc)
+                tma_load_4d(sk(s) + cc * CHUNK + i * R * 128u, tk, full_k(s), cc * 64, row, static_cast<int>(hk), pg);
+            }
+          }
+          for (uint32_t i = 0; i < per; ++i) {
+            const int pg = __shfl_sync(0xFFFFFFFFu, cur, (c - cbase + i) & 31u);
+            const int row = static_cast<int>((static_cast<uint32_t>(k0) + i * R) % p.page);
+            if (lane == 0 && i < nload) {
+#pragma unroll
+              for (int cc = 0; cc < NCH; ++cc)
+                tma_load_4d(sv(s) + cc * CHUNK + i * R * 128u, tv, full_v(s), cc * 64, row, static_cast<int>(hk), pg);
+            }
+          }
+          __syncwarp();
+          if (++s == kAttnStages) { s = 0; ph ^= 1u; }
+        }
+      }
+    } else if (threadIdx.x == 0) {
       mbar_arrive_expect_tx(q_bar, TILE);
 #pragma unroll
       for (int c = 0; c < NCH; ++c) tma_load_4d(sq + c * CHUNK, tq, q_bar, c * 64, qrow, static_cast<int>(h), bb);
@@ -337,12 +400,20 @@ __device__ __forceinline__ void attn_body(const CUtensorMap* tq, const CUtensorM
 
 // name: attn_fwd_<in>_d<64|128>_<out>; D <= 64 runs the d64 kernel, 64 < D <= 128 the d128 kernel
 // varlen (compiled with -DATTN_VARLEN into its own cubin): attn_fwd_varlen_<in>_d<64|128>_<out>
-#ifdef ATTN_VARLEN
+// paged varlen (-DATTN_VARLEN -DATTN_PAGED, cubin attention_paged): attn_fwd_paged_<in>_d<64|128>_<out>
+#if defined(ATTN_VARLEN) && defined(ATTN_PAGED)
 #define ATTN_VL true
+#define ATTN_PG true
+#define ATTN_P AttnVarlenPagedParams
+#define ATTN_NAME(IN, D, OUT) attn_fwd_paged_##IN##_d##D##_##OUT
+#elif defined(ATTN_VARLEN)
+#define ATTN_VL true
+#define ATTN_PG false
 #define ATTN_P AttnVarlenParams
 #define ATTN_NAME(IN, D, OUT) attn_fwd_varlen_##IN##_d##D##_##OUT
 #else
 #define ATTN_VL false
+#define ATTN_PG false
 #define ATTN_P AttnParams
 #define ATTN_NAME(IN, D, OUT) attn_fwd_##IN##_d##D##_##OUT
 #endif
@@ -351,7 +422,7 @@ __device__ __forceinline__ void attn_body(const CUtensorMap* tq, const CUtensorM
       NAME(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,                         \
            const __grid_constant__ CUtensorMap tv, const __grid_constant__ CUtensorMap to,                         \
            const __grid_constant__ ATTN_P p) {                                                                      \
-    attn_body<KIND, DB, OUT, ATTN_VL>(&tq, &tk, &tv, &to, p);                                                       \
+    attn_body<KIND, DB, OUT, ATTN_VL, ATTN_PG>(&tq, &tk, &tv, &to, p);                                              \
   }
 #define ATTN_D(IN, KIND, OUT16)                                  \
   ATTN_KERNEL(ATTN_NAME(IN, 64, IN), KIND, 64, OUT16)            \

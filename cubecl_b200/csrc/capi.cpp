@@ -24,6 +24,7 @@
 #include <cstring>
 #include <map>
 #include <mutex>
+#include <numeric>
 #include <string>
 #include <unordered_map>
 #include <vector>
@@ -68,6 +69,8 @@ extern const unsigned char b200_cubin_attention_varlen_bwd[];
 extern const unsigned char b200_cubin_attention_varlen_bwd_end[];
 extern const unsigned char b200_cubin_attention_kv_fp8[];
 extern const unsigned char b200_cubin_attention_kv_fp8_end[];
+extern const unsigned char b200_cubin_attention_paged[];
+extern const unsigned char b200_cubin_attention_paged_end[];
 }
 
 // ================================================================================================ errors
@@ -340,12 +343,13 @@ static int get_func(b200_ctx* c, const std::string& name, CUfunction* out) {
   if (it != c->funcs.end()) { *out = it->second; return B200_OK; }
   // modules are loaded in the order gemm, reduce, aux, gemm_b, gemm_c, quant, gemm_q, quant_mm, gemm_conv, gemm_convbwd,
   // conv_grouped, gemm_conv3d, gemm_convt, attention, attention_bwd, attention_kv, attention_varlen, attention_varlen_bwd,
-  // attention_kv_fp8; the kernel name says where a
+  // attention_kv_fp8, attention_paged; the kernel name says where a
   // kernel lives (no failing lookups, which API-level tools such as compute-sanitizer would report)
   auto starts = [&](const char* pfx) { return name.rfind(pfx, 0) == 0; };
   auto has = [&](const char* part) { return name.find(part) != std::string::npos; };
   const bool tc_gemm = starts("gemm_") && name != "gemm_simt_strided" && name != "gemm_scaled_simt";
   const size_t home = name == "conv3d_dgrad_weights" ? 2
+                      : starts("attn_fwd_paged_") ? 19
                       : starts("attn_kv_") && (has("_e4m3_") || has("_e5m2_") || has("_fp8")) ? 18
                       : starts("attn_bwd_varlen_") ? 17
                       : starts("attn_fwd_varlen_") ? 16
@@ -397,7 +401,8 @@ extern "C" int b200_get_cubin(const char* name, const void** image, size_t* size
   else if (!strcmp(name, "attention_varlen")) { b = b200_cubin_attention_varlen; e = b200_cubin_attention_varlen_end; }
   else if (!strcmp(name, "attention_varlen_bwd")) { b = b200_cubin_attention_varlen_bwd; e = b200_cubin_attention_varlen_bwd_end; }
   else if (!strcmp(name, "attention_kv_fp8")) { b = b200_cubin_attention_kv_fp8; e = b200_cubin_attention_kv_fp8_end; }
-  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd|conv_grouped|gemm_conv3d|gemm_convt|attention|attention_bwd|attention_kv|attention_varlen|attention_varlen_bwd|attention_kv_fp8)", name);
+  else if (!strcmp(name, "attention_paged")) { b = b200_cubin_attention_paged; e = b200_cubin_attention_paged_end; }
+  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd|conv_grouped|gemm_conv3d|gemm_convt|attention|attention_bwd|attention_kv|attention_varlen|attention_varlen_bwd|attention_kv_fp8|attention_paged)", name);
   *image = b;
   *size = static_cast<size_t>(e - b);
   return B200_OK;
@@ -463,7 +468,8 @@ extern "C" int b200_init(int device, b200_ctx** out) {
       (rc = load_module(c, b200_cubin_attention_kv, b200_cubin_attention_kv_end, "attention_kv")) ||
       (rc = load_module(c, b200_cubin_attention_varlen, b200_cubin_attention_varlen_end, "attention_varlen")) ||
       (rc = load_module(c, b200_cubin_attention_varlen_bwd, b200_cubin_attention_varlen_bwd_end, "attention_varlen_bwd")) ||
-      (rc = load_module(c, b200_cubin_attention_kv_fp8, b200_cubin_attention_kv_fp8_end, "attention_kv_fp8"))) {
+      (rc = load_module(c, b200_cubin_attention_kv_fp8, b200_cubin_attention_kv_fp8_end, "attention_kv_fp8")) ||
+      (rc = load_module(c, b200_cubin_attention_paged, b200_cubin_attention_paged_end, "attention_paged"))) {
     for (CUmodule m : c->modules) g_drv.cuModuleUnload_p(m);
     g_drv.cuDevicePrimaryCtxRelease_p(c->dev);
     return bail(rc);
@@ -4343,19 +4349,20 @@ static int attn_check_caches(const char* what, const AttnView& kc, const AttnVie
               "(it is read in place, never gathered)", what);
 }
 
-// ---- launch sequences the dense and varlen entry points share
-// Stages q, k and v, maps them (loads of kAttnBlock rows) and out, then launches `<prefix><in>_d<DB>_<out>` on `ctas` CTAs
-// with the filled parameter block p.
+// ---- launch sequences the dense, varlen and paged varlen entry points share
+// Stages q, k and v (k and v only with stage_kv: a paged cache is read in place, never gathered), maps them (q in loads of
+// kAttnBlock rows, k and v of kv_rows) and out, then launches `<prefix><in>_d<DB>_<out>` on `ctas` CTAs with the filled
+// parameter block p.
 static int attn_fwd_launch(b200_ctx* c, CUstream st, const std::string& prefix, AttnView q, AttnView k, AttnView v, const AttnView& o,
-                           uint64_t ctas, void* p) {
+                           uint64_t ctas, void* p, uint32_t kv_rows = kAttnBlock, bool stage_kv = true) {
   CUdeviceptr tmp[3] = {0, 0, 0};
   int rc = attn_stage(c, st, &q, &tmp[0]);
-  if (!rc) rc = attn_stage(c, st, &k, &tmp[1]);
-  if (!rc) rc = attn_stage(c, st, &v, &tmp[2]);
+  if (!rc && stage_kv) rc = attn_stage(c, st, &k, &tmp[1]);
+  if (!rc && stage_kv) rc = attn_stage(c, st, &v, &tmp[2]);
   CUtensorMap mq, mk, mv, mo;
   if (!rc) rc = attn_map(c, &mq, q, false, kAttnBlock);
-  if (!rc) rc = attn_map(c, &mk, k, false, kAttnBlock);
-  if (!rc) rc = attn_map(c, &mv, v, false, kAttnBlock);
+  if (!rc) rc = attn_map(c, &mk, k, false, kv_rows);
+  if (!rc) rc = attn_map(c, &mv, v, false, kv_rows);
   if (!rc) rc = attn_map(c, &mo, o, true);
   const uint32_t DB = attn_db(q.shape[3]);
   CUfunction f = nullptr;
@@ -4551,6 +4558,22 @@ extern "C" int b200_attention_backward(b200_ctx* c, b200_stream s, b200_dtype in
 }
 
 // ------------------------------------------------------------------------------------------------ varlen attention
+// The window and the max_seqlen signs, then (after the scale and extent checks) the max_seqlen bounds, of every varlen entry.
+static int vl_check_window(const char* what, const b200_attention_varlen_args* args) {
+  if (args->window_left < -1 || args->window_right < -1)
+    return fail(B200_ERR_INVALID_ARG, "%s: window (%d, %d): each side must be >= 0, or -1 for unbounded", what, args->window_left,
+                args->window_right);
+  if (args->max_seqlen_q < 0 || args->max_seqlen_k < 0)
+    return fail(B200_ERR_INVALID_ARG, "%s: max_seqlen_q = %d and max_seqlen_k = %d must be >= 0", what, args->max_seqlen_q, args->max_seqlen_k);
+  return B200_OK;
+}
+
+static int vl_check_max_seqlen(const char* what, const b200_attention_varlen_args* args) {
+  if (args->max_seqlen_q >= (1 << 30) || args->max_seqlen_k >= (1 << 30))
+    return fail(B200_ERR_UNSUPPORTED, "%s: max_seqlen_q and max_seqlen_k must be < 2^30", what);
+  return B200_OK;
+}
+
 // The checks both varlen entries share (see cubecl_b200.h); 0 or the failure status.
 static int vl_check(const char* what, b200_dtype in_dtype, const uint64_t* q_shape, const uint64_t* k_shape, const uint64_t* v_shape,
                     uint64_t batch, const b200_attention_varlen_args* args) {
@@ -4561,15 +4584,10 @@ static int vl_check(const char* what, b200_dtype in_dtype, const uint64_t* q_sha
     return fail(B200_ERR_INVALID_ARG, "%s: k's head dim %llu differs from q's D = %llu", what, (unsigned long long)k_shape[2], (unsigned long long)D);
   rc = attn_check_v(what, "k", "v", k_shape, v_shape, 3);
   if (!rc) rc = attn_check_gqa(what, Hq, Hkv);
-  if (!rc && (args->window_left < -1 || args->window_right < -1))
-    rc = fail(B200_ERR_INVALID_ARG, "%s: window (%d, %d): each side must be >= 0, or -1 for unbounded", what, args->window_left,
-              args->window_right);
-  if (!rc && (args->max_seqlen_q < 0 || args->max_seqlen_k < 0))
-    rc = fail(B200_ERR_INVALID_ARG, "%s: max_seqlen_q = %d and max_seqlen_k = %d must be >= 0", what, args->max_seqlen_q, args->max_seqlen_k);
+  if (!rc) rc = vl_check_window(what, args);
   if (!rc) rc = attn_check_scale_d(what, args->scale, D);
   if (!rc) rc = attn_check_extents(what, {batch, Tq, Hq, Tk, Hkv});
-  if (!rc && (args->max_seqlen_q >= (1 << 30) || args->max_seqlen_k >= (1 << 30)))
-    rc = fail(B200_ERR_UNSUPPORTED, "%s: max_seqlen_q and max_seqlen_k must be < 2^30", what);
+  if (!rc) rc = vl_check_max_seqlen(what, args);
   return rc;
 }
 
@@ -4734,6 +4752,32 @@ static int kv_check_scales(const char* what, const KvFp8* f8) {
   return B200_OK;
 }
 
+// The paging of a KV cache of P pages of `page` keys for B sequences (see b200_attention_kvcache): the cache is not empty, a
+// block table is [B, max_pages >= 1] (none: P == B), and with several pages per sequence the page rule holds.  *max_pages:
+// the table's width, or 1.
+static int kv_check_pages(const char* what, uint64_t B, uint64_t P, uint64_t page, b200_dptr block_table, const uint64_t* bt_shape,
+                          uint64_t* max_pages) {
+  auto ull = [](uint64_t x) { return (unsigned long long)x; };
+  if (page == 0 || P == 0) return fail(B200_ERR_INVALID_ARG, "%s: empty cache (P = %llu pages of %llu keys)", what, ull(P), ull(page));
+  *max_pages = block_table ? bt_shape[1] : 1;
+  if (block_table && (bt_shape[0] != B || *max_pages == 0))
+    return fail(B200_ERR_INVALID_ARG, "%s: block_table is [%llu,%llu], expected [%llu, max_pages >= 1]", what, ull(bt_shape[0]),
+                ull(bt_shape[1]), ull(B));
+  if (!block_table && P != B)
+    return fail(B200_ERR_INVALID_ARG, "%s: without a block table the cache holds one page per sequence (P = %llu, B = %llu)", what, ull(P), ull(B));
+  if (*max_pages > 1 && (page % 16 || (kAttnKvBlock % page && page % kAttnKvBlock)))
+    return fail(B200_ERR_UNSUPPORTED, "%s: a page of %llu keys must be a multiple of 16 that divides %d or is a multiple of it", what,
+                ull(page), kAttnKvBlock);
+  return B200_OK;
+}
+
+// The extents of a call against a paged cache, its capacity max_pages * page among them.
+static int kv_check_capacity(const char* what, std::initializer_list<uint64_t> extents) {
+  for (uint64_t e : extents)
+    if (e >= (1ull << 31)) return fail(B200_ERR_UNSUPPORTED, "%s: extents and the capacity max_pages * page must be < 2^31", what);
+  return B200_OK;
+}
+
 // Attention of q against a paged KV cache (see cubecl_b200.h): one attn_kv_* launch, plus attn_kv_combine_* when the keys
 // are split.  f8: an fp8 cache (b200_attention_kvcache_fp8), else the caches hold the input dtype.
 static int kv_attend(b200_ctx* c, b200_stream s, const char* what, b200_dtype in_dtype, const KvFp8* f8, b200_dtype out_dtype, b200_dptr q,
@@ -4757,21 +4801,12 @@ static int kv_attend(b200_ctx* c, b200_stream s, const char* what, b200_dtype in
   rc = attn_check_v(what, "k_cache", "v_cache", kc_shape, vc_shape, 4);
   if (!rc) rc = attn_check_gqa(what, Hq, Hkv);
   if (!rc) rc = attn_check_same(what, 4, {{"out", out_shape, q_shape}});
-  if (rc) return rc;
-  if (page == 0 || P == 0) return fail(B200_ERR_INVALID_ARG, "%s: empty cache (P = %llu pages of %llu keys)", what, ull(P), ull(page));
-  const uint64_t max_pages = block_table ? bt_shape[1] : 1;
-  if (block_table && (bt_shape[0] != B || max_pages == 0))
-    return fail(B200_ERR_INVALID_ARG, "%s: block_table is [%llu,%llu], expected [%llu, max_pages >= 1]", what, ull(bt_shape[0]),
-                ull(bt_shape[1]), ull(B));
-  if (!block_table && P != B)
-    return fail(B200_ERR_INVALID_ARG, "%s: without a block table the cache holds one page per sequence (P = %llu, B = %llu)", what, ull(P), ull(B));
-  if (max_pages > 1 && (page % 16 || (kAttnKvBlock % page && page % kAttnKvBlock)))
-    return fail(B200_ERR_UNSUPPORTED, "%s: a page of %llu keys must be a multiple of 16 that divides %d or is a multiple of it", what,
-                ull(page), kAttnKvBlock);
-  if ((rc = attn_check_scale_d(what, args->scale, D))) return rc;
+  uint64_t max_pages = 1;
+  if (!rc) rc = kv_check_pages(what, B, P, page, block_table, bt_shape, &max_pages);
+  if (!rc) rc = attn_check_scale_d(what, args->scale, D);
   const uint64_t lim = 1ull << 31, cap = max_pages * page;
-  if (B >= lim || Hq >= lim || Sq >= lim || P >= lim || page >= lim || max_pages >= lim || cap >= lim)
-    return fail(B200_ERR_UNSUPPORTED, "%s: extents and the capacity max_pages * page must be < 2^31", what);
+  if (!rc) rc = kv_check_capacity(what, {B, Hq, Sq, P, page, max_pages, cap});
+  if (rc) return rc;
   if (B == 0 || Hq == 0 || Sq == 0) return B200_OK;
   if (!q || !k_cache || !v_cache || !cache_seqlens || !out) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
   if (lse % 4 || cache_seqlens % 4 || block_table % 4)
@@ -4866,6 +4901,78 @@ extern "C" int b200_attention_kvcache_fp8(b200_ctx* c, b200_stream s, b200_dtype
   const KvFp8 f8{cache_dtype, k_scale, v_scale};
   return kv_attend(c, s, "attention_kvcache_fp8", in_dtype, &f8, out_dtype, q, q_shape, q_strides, k_cache, kc_shape, kc_strides, v_cache,
                    vc_shape, vc_strides, block_table, bt_shape, bt_strides, cache_seqlens, out, out_shape, out_strides, lse, args);
+}
+
+// ------------------------------------------------------------------------------------------------ paged varlen attention
+// Packed queries against a paged KV cache (see cubecl_b200.h): the gather of q if needed, then one attn_fwd_paged_* launch.
+extern "C" int b200_attention_varlen_paged(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr q,
+                                           const uint64_t* q_shape, const uint64_t* q_strides, b200_dptr k_cache, const uint64_t* kc_shape,
+                                           const uint64_t* kc_strides, b200_dptr v_cache, const uint64_t* vc_shape,
+                                           const uint64_t* vc_strides, b200_dptr block_table, const uint64_t* bt_shape,
+                                           const uint64_t* bt_strides, b200_dptr cu_seqlens_q, b200_dptr cache_seqlens, uint64_t batch,
+                                           b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides, b200_dptr lse,
+                                           const b200_attention_varlen_args* args) {
+  CTX_ENTER(c);
+  const char* what = "attention_varlen_paged";
+  if (!q_shape || !kc_shape || !vc_shape || !out_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
+  if (block_table && !bt_shape) return fail(B200_ERR_INVALID_ARG, "%s: null block-table shape", what);
+  int rc = attn_check_in_dtype(what, in_dtype);
+  if (!rc) rc = attn_check_out_dtype(what, "output", in_dtype, out_dtype);
+  if (rc) return rc;
+  const uint64_t Tq = q_shape[0], Hq = q_shape[1], D = q_shape[2], B = batch;
+  const uint64_t P = kc_shape[0], page = kc_shape[1], Hkv = kc_shape[2];
+  if (kc_shape[3] != D)
+    return fail(B200_ERR_INVALID_ARG, "%s: k_cache head dim %llu differs from q's D = %llu", what, (unsigned long long)kc_shape[3],
+                (unsigned long long)D);
+  rc = attn_check_v(what, "k_cache", "v_cache", kc_shape, vc_shape, 4);
+  if (!rc) rc = attn_check_gqa(what, Hq, Hkv);
+  if (!rc) rc = attn_check_same(what, 3, {{"out", out_shape, q_shape}});
+  if (!rc) rc = vl_check_window(what, args);
+  uint64_t max_pages = 1;
+  if (!rc) rc = kv_check_pages(what, B, P, page, block_table, bt_shape, &max_pages);
+  if (!rc) rc = attn_check_scale_d(what, args->scale, D);
+  const uint64_t cap = max_pages * page;
+  if (!rc) rc = kv_check_capacity(what, {B, Tq, Hq, P, page, max_pages, cap});
+  if (!rc) rc = vl_check_max_seqlen(what, args);
+  if (rc) return rc;
+  const uint64_t max_q = (uint64_t)args->max_seqlen_q, max_k = (uint64_t)args->max_seqlen_k;
+  if (B == 0 || Tq == 0 || Hq == 0 || max_q == 0) return B200_OK;   // no query row
+  const uint64_t nqb = (max_q + kAttnBlock - 1) / kAttnBlock, ctas = nqb * Hq * B;
+  if (ctas >= (1ull << 31))
+    return fail(B200_ERR_UNSUPPORTED, "%s: ceil(max_seqlen_q / %d) * Hq * B = %llu CTAs must be < 2^31", what, kAttnBlock,
+                (unsigned long long)ctas);
+  if (!q || !k_cache || !v_cache || !out || !cu_seqlens_q || !cache_seqlens) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
+  if (lse % 4 || cu_seqlens_q % 4 || cache_seqlens % 4 || block_table % 4)
+    return fail(B200_ERR_INVALID_ARG, "%s: lse, cu_seqlens_q, cache_seqlens and block_table must be 4-byte aligned", what);
+  const AttnView ov = attn_view(out, out_dtype, out_shape, out_strides, kAttnTHD);
+  const AttnView kv = attn_view(k_cache, in_dtype, kc_shape, kc_strides, kAttnBSHD), vv = attn_view(v_cache, in_dtype, vc_shape, vc_strides, kAttnBSHD);
+  if ((rc = attn_check_out_view(what, "out", ov)) || (rc = attn_check_caches(what, kv, vv))) return rc;
+
+  // keys per TMA load: a chunk of a 128-key block never crosses a page; one page per sequence is read in 128-row boxes, the
+  // rows past the page zero-filled
+  const uint32_t R = max_pages == 1 ? kAttnBlock : (uint32_t)std::gcd<uint64_t>(page, kAttnBlock);
+  AttnVarlenPagedParams p{};
+  p.lse = lse;
+  p.cu_q = cu_seqlens_q;
+  p.out = out; p.o_st = ov.s_row(); p.o_sh = ov.s_head();
+  p.B = (uint32_t)B; p.Hq = (uint32_t)Hq; p.Hkv = (uint32_t)Hkv; p.Tq = (uint32_t)Tq;
+  p.group = (uint32_t)(Hq / Hkv);
+  p.max_q = (uint32_t)max_q; p.max_k = (uint32_t)max_k;
+  p.nqb = (uint32_t)nqb; p.nkb = (uint32_t)((max_k + kAttnBlock - 1) / kAttnBlock);
+  p.D = (uint32_t)D;
+  p.left = args->window_left; p.right = args->window_right;
+  p.scale_log2 = attn_scale_log2(args->scale);
+  p.scale = args->scale;
+  p.table = block_table;
+  if (block_table) {
+    p.t_sb = bt_strides ? bt_strides[0] : max_pages;
+    p.t_sp = bt_strides ? bt_strides[1] : 1;
+  }
+  p.seqlens = cache_seqlens;
+  p.page = (uint32_t)page; p.rows = R;
+  p.cap = (uint32_t)cap;
+  return attn_fwd_launch(c, resolve_stream(c, s), "attn_fwd_paged_", attn_view(q, in_dtype, q_shape, q_strides, kAttnTHD), kv, vv, ov,
+                         ctas, &p, R, false);
 }
 
 // Scatter of new tokens into a paged KV cache (see cubecl_b200.h): one attn_kv_write launch, or attn_kv_write_fp8 (f8: an

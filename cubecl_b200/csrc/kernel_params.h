@@ -289,6 +289,21 @@ struct AttnVarlenParams {
   float scale;                    // backward: multiplies dQ and dK in the epilogue
 };
 
+// Paged varlen attention: attention.cu compiled with -DATTN_VARLEN -DATTN_PAGED (attn_fwd_paged_*; capi.cpp:
+// b200_attention_varlen_paged).  The varlen forward with its queries (cu_q, Tq, max_q, window, out, lse) and K / V read from a
+// paged cache [P, page, Hkv, D] through 4-D maps (D, page, Hkv, P): sequence b has Lk = clamp(seqlens[b], 0, min(max_k, cap))
+// keys, key j at row j % page of page table[b * t_sb + (j / page) * t_sp] (table 0: page b).  A 128-key block arrives as
+// kAttnBlock / rows loads of `rows` keys (rows divides the page, or rows = kAttnBlock with one page per sequence); loads of
+// chunks at or past Lk are not issued.  The cu_k, Tk and backward fields of the base are unused.
+struct AttnVarlenPagedParams : AttnVarlenParams {
+  uint64_t table;                 // i32 block table, or 0
+  uint64_t t_sb, t_sp;            // its strides in elements
+  uint64_t seqlens;               // i32 [B] cache lengths
+  uint32_t page, rows;            // keys per page, keys per TMA load
+  uint32_t cap;                   // capacity max_pages * page
+  uint32_t pad;
+};
+
 // ================================================================================================ attention_kv.cu
 // Attention against a KV cache (attn_kv_*; capi.cpp: b200_attention_kvcache).  One CTA per (b, hk, m-tile, split), grid
 // B * Hkv * nsplit * mtiles with block x = ((b * Hkv + hk) * nsplit + split) * mtiles + mt (the m-tiles that share a key range

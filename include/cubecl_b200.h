@@ -736,6 +736,47 @@ int b200_kvcache_write(b200_ctx* ctx, b200_stream s, b200_dtype dtype,
                        b200_dptr v_cache, const uint64_t* vc_shape, const uint64_t* vc_strides,
                        b200_dptr slot_mapping);
 
+/* ---- paged variable-length attention (chunked prefill, prefix caching; flash_attn_varlen_func with block_table) -----------
+ * Packed queries (b200_attention_varlen's layout) against a paged KV cache (b200_attention_kvcache's layout): q and out are
+ * [Tq, Hq, D], k_cache and v_cache [P, page, Hkv, D] in q's dtype, Hq % Hkv == 0, hk = h / (Hq / Hkv).
+ *   out[cu_q[b] + i, h, :] = sum_{j visible} softmax_j(scale * q_i . K_b[j, hk, :]) * V_b[j, hk, :]
+ *   lse[h, cu_q[b] + i]    = log sum_{j visible} exp(scale * q_i . K_b[j, hk, :])                      (natural log, f32)
+ * Queries: sequence b owns rows [cu_q[b], cu_q[b + 1]) (Lq_b rows) of the compact i32 [batch + 1] device array cu_seqlens_q,
+ * clamped on the device as in b200_attention_varlen; the host never reads it, so the call does not synchronise and can be
+ * captured in a CUDA graph.  Rows outside every sequence are not written, in out or lse.
+ * Keys: sequence b has Lk_b = clamp(cache_seqlens[b], 0, min(args->max_seqlen_k, max_pages * page)) keys (cache_seqlens: a
+ * compact i32 [batch] device array); key j is row j % page of page block_table[b, j / page] (i32 [batch, max_pages], any
+ * strides).  block_table = 0: sequence b is page b (P == batch, any page size).  Table entries at or past ceil(Lk_b / page)
+ * are never read, an out-of-range page id reads zeros, and stale slots (NaN or inf included) never reach out.  The page rule
+ * is b200_attention_kvcache's, so one cache serves both calls.
+ * Visibility: b200_attention_varlen's band with off = Lk_b - Lq_b: the new queries are the last Lq_b of the Lk_b cached keys,
+ * (-1, 0) is bottom-right causal and (W, 0) a causal sliding window.  A row with no visible key gets out = +0 and lse = -inf.
+ * Chunked prefill: write the chunk's own keys and values first (b200_kvcache_write) and count them in cache_seqlens.
+ * Numerics: b200_attention_varlen's exactly: for every sequence, out and lse equal bit for bit those of a b200_attention_varlen
+ * call whose k and v are that sequence's Lk_b cached rows packed contiguously, with the same args.  No atomics: bitwise
+ * reproducible.
+ * Dtypes and limits: b200_attention_varlen's (f16 / bf16 in, out in the input dtype or f32, D <= 128, D % 8 == 0).  Views: q is
+ * read in place or gathered like b200_attention_varlen's; the caches and out are never gathered: a view a tensor map cannot
+ * read is refused (B200_ERR_UNSUPPORTED).  lse: 0 or a compact f32 [Hq, Tq] buffer.
+ * Errors: b200_attention_varlen's window, max_seqlen and scale errors and b200_attention_kvcache's cache, table and page
+ * errors (B200_ERR_INVALID_ARG for a k_cache head dim other than D, a v_cache shape mismatch, Hkv == 0 or Hq % Hkv != 0, a
+ * wrong out shape, an empty cache, a block table that is not [batch, >= 1] or no table with P != batch, a null pointer or a
+ * misaligned lse / cu_seqlens_q / cache_seqlens / block_table; B200_ERR_UNSUPPORTED for the dtypes, D, Dv != D, the page rule,
+ * caches or out a tensor map cannot read, extents or capacity >= 2^31, max_seqlen >= 2^30 or more than 2^31 - 1 CTAs).
+ * batch, Tq, Hq or max_seqlen_q = 0: no launch.
+ * Launches, on `s` with no host synchronisation: the gather of q if needed, then one attn_fwd_paged_<in>_d<64|128>_<out>
+ * launch of ceil(max_seqlen_q / 128) * Hq * batch CTAs with the shared memory of b200_attention_varlen (no workspace, no
+ * combine).  The dry-run plan records "tmap4d" lines in the order q (D, Tq, Hq, 1), k_cache, v_cache (D, page, Hkv, P), out;
+ * the cache maps have box (64, R, 1, 1), R = gcd(page, 128), or R = 128 with one page per sequence (max_pages == 1). */
+int b200_attention_varlen_paged(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype,
+                                b200_dptr q, const uint64_t* q_shape, const uint64_t* q_strides,
+                                b200_dptr k_cache, const uint64_t* kc_shape, const uint64_t* kc_strides,
+                                b200_dptr v_cache, const uint64_t* vc_shape, const uint64_t* vc_strides,
+                                b200_dptr block_table, const uint64_t* bt_shape, const uint64_t* bt_strides,
+                                b200_dptr cu_seqlens_q, b200_dptr cache_seqlens, uint64_t batch,
+                                b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides,
+                                b200_dptr lse, const b200_attention_varlen_args* args);
+
 /* ---- fp8 KV caches (vLLM's kv_cache_dtype="fp8", FlashAttention-3's k_descale / v_descale) ------------------------------
  * b200_attention_kvcache with the caches in B200_F8E4M3 or B200_F8E5M2 (cache_dtype, both caches) and two compact f32 [Hkv]
  * device arrays k_scale and v_scale (read by the kernels only: no synchronisation, graph-capturable; a per-tensor scale is the

@@ -655,6 +655,43 @@ impl Context {
         ))
     }
 
+    /// Paged variable-length attention: packed q [Tq, Hq, D] -> out [Tq, Hq, D] (sequence b owns rows [cu_q[b], cu_q[b + 1]),
+    /// a compact i32 [batch + 1] device buffer) against `k_cache`, `v_cache` [P, page, Hkv, D] in q's dtype: sequence b sees its
+    /// first `cache_seqlens`[b] keys (a compact i32 [batch] device buffer), key j in page `block_table`[b, j / page] (an i32
+    /// [batch, max_pages] view; `None`: page b); `window` as [`Context::attention_varlen`]'s with the queries aligned to the last
+    /// keys.  See b200_attention_varlen_paged in cubecl_b200.h.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::conv2d`]; `cu_seqlens_q` must hold batch + 1 i32 values, `cache_seqlens` batch, and `lse`,
+    /// when non-zero, Hq * Tq f32 values.
+    pub unsafe fn attention_varlen_paged(
+        &mut self, stream: b200_stream, in_dtype: DType, out_dtype: DType, q: &TensorView, k_cache: &TensorView, v_cache: &TensorView,
+        block_table: Option<&TensorView>, cu_seqlens_q: b200_dptr, cache_seqlens: b200_dptr, batch: u64, max_seqlen: (i32, i32),
+        out: &TensorView, lse: b200_dptr, scale: f32, window: (i32, i32),
+    ) -> Result<(), Error> {
+        for t in [q, out] {
+            assert!(t.shape.len() == 3 && t.strides.len() == 3);
+        }
+        for t in [k_cache, v_cache] {
+            assert!(t.shape.len() == 4 && t.strides.len() == 4);
+        }
+        if let Some(t) = block_table {
+            assert!(t.shape.len() == 2 && t.strides.len() == 2);
+        }
+        let a = sys::b200_attention_varlen_args {
+            scale, window_left: window.0, window_right: window.1, max_seqlen_q: max_seqlen.0, max_seqlen_k: max_seqlen.1,
+        };
+        let (bt, bt_shape, bt_strides) = match block_table {
+            Some(t) => (t.ptr, t.shape.as_ptr(), t.strides.as_ptr()),
+            None => (0, std::ptr::null(), std::ptr::null()),
+        };
+        check(sys::b200_attention_varlen_paged(
+            self.0, stream, in_dtype as c_int, out_dtype as c_int, q.ptr, q.shape.as_ptr(), q.strides.as_ptr(), k_cache.ptr,
+            k_cache.shape.as_ptr(), k_cache.strides.as_ptr(), v_cache.ptr, v_cache.shape.as_ptr(), v_cache.strides.as_ptr(), bt,
+            bt_shape, bt_strides, cu_seqlens_q, cache_seqlens, batch, out.ptr, out.shape.as_ptr(), out.strides.as_ptr(), lse, &a,
+        ))
+    }
+
     /// Scatter of `k_new`, `v_new` [B, Snew, Hkv, D] into `k_cache`, `v_cache` [P, page, Hkv, D]: token b * Snew + t goes to flat
     /// slot `slot_mapping`[b * Snew + t] (a compact i32 device buffer; negative slots are skipped).  See b200_kvcache_write.
     ///
