@@ -168,6 +168,8 @@ SIGNATURES = {
     "b200_kvcache_write_fp8": (C.c_int, [_vp, _vp, C.c_int, C.c_int] + [C.c_uint64, _u64p, _u64p] * 4 + [C.c_uint64] * 3),
     "b200_attention_varlen_paged": (C.c_int, [_vp, _vp, C.c_int, C.c_int] + [C.c_uint64, _u64p, _u64p] * 4 + [C.c_uint64] * 3
                                     + [C.c_uint64, _u64p, _u64p] + [C.c_uint64, C.POINTER(AttentionVarlenArgs)]),
+    "b200_attention_varlen_paged_fp8": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int] + [C.c_uint64, _u64p, _u64p] * 4
+                                        + [C.c_uint64] * 5 + [C.c_uint64, _u64p, _u64p] + [C.c_uint64, C.POINTER(AttentionVarlenArgs)]),
     "b200_reduce": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, C.c_uint64, C.c_int, _u64p, C.c_int]),
     "b200_reduce_strided": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, C.c_uint64, C.c_int, _u64p, _u64p, C.c_int]),
     "b200_reduce_debug": (C.c_int, [_vp, _vp, _u64p]),

@@ -34,6 +34,9 @@ block_table): packed q [Tq, Hq, D] as launch_varlen's against a paged cache as l
 are the last of its cache_seqlens[b] cached keys (write the chunk's keys with kvcache_write first), under launch_varlen's window
 rule.  Out and lse are bit for bit those of launch_varlen on each sequence's cached keys packed contiguously.  The varlen
 forward kernel with paged K / V addressing (-DATTN_VARLEN -DATTN_PAGED); see b200_attention_varlen_paged.
+launch_varlen_paged_fp8 does the same against fp8 caches written by kvcache_write_fp8 (chunked prefill and prefix caching with
+kv_cache_dtype="fp8"): idle producer warps widen K and V to q's dtype on chip, and power-of-two scales give the bits of
+launch_varlen_paged on the dequantized cache; see b200_attention_varlen_paged_fp8.
 """
 from __future__ import annotations
 
@@ -419,4 +422,50 @@ def launch_varlen_paged_alloc(client: ComputeClient, q: TensorHandle, k_cache: T
     lse = TensorHandle.empty_contiguous(client, [q.shape[1], q.shape[0]], "f32") if return_lse else None
     launch_varlen_paged(client, q, k_cache, v_cache, cu_seqlens_q, cache_seqlens, max_seqlen_q, max_seqlen_k, out,
                         block_table=block_table, scale=scale, window_size=window_size, lse=lse, stream=stream)
+    return (out, lse) if return_lse else out
+
+
+@_defers_errors
+def launch_varlen_paged_fp8(client: ComputeClient, q: TensorHandle, k_cache: TensorHandle, v_cache: TensorHandle,
+                            cu_seqlens_q: TensorHandle, cache_seqlens: TensorHandle, k_scale: TensorHandle, v_scale: TensorHandle,
+                            max_seqlen_q: int, max_seqlen_k: int, out: TensorHandle, block_table: TensorHandle | None = None,
+                            scale: float | None = None, window_size=(-1, -1), lse: TensorHandle | None = None, stream=None) -> None:
+    """launch_varlen_paged against an fp8 cache: k_cache and v_cache f8e4m3 or f8e5m2 [P, page, Hkv, D] holding
+    K = k_scale[hk] * k8 and V = v_scale[hk] * v8, with k_scale and v_scale compact f32 [Hkv] tensors (read on the device).
+    K and V are widened exactly to q's dtype on chip; scores are scaled by scale * k_scale[hk] and out = (v_scale[hk] * O) / l.
+    Power-of-two scales give the bits of launch_varlen_paged on the dequantized cache.  Never raises for launch problems:
+    errors are deferred to client.sync()."""
+    what = "attention_varlen_paged_fp8"
+    _check_rank(what, 3, (("q", q), ("out", out)), " [T, H, D]")
+    _check_rank(what, 4, (("k_cache", k_cache), ("v_cache", v_cache)), " [P, page, Hkv, D]")
+    _check_fp8(what, k_cache, v_cache, k_scale, v_scale, k_cache.shape[2])
+    if cu_seqlens_q.dtype != "i32" or not cu_seqlens_q.is_contiguous() or len(cu_seqlens_q.shape) != 1 or cu_seqlens_q.shape[0] < 1:
+        raise B200Error(6, f"{what}: cu_seqlens_q must be a compact i32 [B + 1] tensor")
+    B = cu_seqlens_q.shape[0] - 1
+    if cache_seqlens.dtype != "i32" or not cache_seqlens.is_contiguous() or list(cache_seqlens.shape) != [B]:
+        raise B200Error(6, f"{what}: cache_seqlens must be a compact i32 [B] = [{B}] tensor")
+    if block_table is not None and (block_table.dtype != "i32" or len(block_table.shape) != 2):
+        raise B200Error(6, f"{what}: block_table must be an i32 [B, max_pages] tensor")
+    _check_lse(what, lse, "[Hq, Tq]", [q.shape[1], q.shape[0]])
+    left, right = (int(w) for w in window_size)
+    args = _ffi.AttentionVarlenArgs(_scale(scale, q.shape[2]), left, right, int(max_seqlen_q), int(max_seqlen_k))
+    _used_on(stream, q, k_cache, v_cache, cu_seqlens_q, cache_seqlens, k_scale, v_scale, out, block_table, lse)
+    bt = _view_args((block_table,)) if block_table is not None else [C.c_uint64(0), None, None]
+    _ffi.check(client._lib.b200_attention_varlen_paged_fp8(
+        client._ctx, stream, DTYPES[q.dtype], DTYPES[k_cache.dtype], DTYPES[out.dtype], *_view_args((q, k_cache, v_cache)), *bt,
+        _ptr(cu_seqlens_q), _ptr(cache_seqlens), C.c_uint64(B), _ptr(k_scale), _ptr(v_scale), *_view_args((out,)), _ptr(lse),
+        C.byref(args)))
+
+
+def launch_varlen_paged_fp8_alloc(client: ComputeClient, q: TensorHandle, k_cache: TensorHandle, v_cache: TensorHandle,
+                                  cu_seqlens_q: TensorHandle, cache_seqlens: TensorHandle, k_scale: TensorHandle, v_scale: TensorHandle,
+                                  max_seqlen_q: int, max_seqlen_k: int, block_table: TensorHandle | None = None,
+                                  scale: float | None = None, window_size=(-1, -1), out_dtype: str | None = None,
+                                  return_lse: bool = False, stream=None):
+    """Convenience: allocate a compact out [Tq, Hq, D] (and, with return_lse, a compact f32 lse [Hq, Tq]), then
+    launch_varlen_paged_fp8.  Rows outside every sequence are left as allocated.  Returns out, or (out, lse)."""
+    out = TensorHandle.empty_contiguous(client, list(q.shape), out_dtype or q.dtype)
+    lse = TensorHandle.empty_contiguous(client, [q.shape[1], q.shape[0]], "f32") if return_lse else None
+    launch_varlen_paged_fp8(client, q, k_cache, v_cache, cu_seqlens_q, cache_seqlens, k_scale, v_scale, max_seqlen_q, max_seqlen_k,
+                            out, block_table=block_table, scale=scale, window_size=window_size, lse=lse, stream=stream)
     return (out, lse) if return_lse else out

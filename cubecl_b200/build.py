@@ -34,7 +34,8 @@ CUBINS = {"gemm": ("gemm_wgmma.cu", ["-DGEMM_PART=0"]), "gemm_b": ("gemm_wgmma.c
           "attention_kv": ("attention_kv.cu", []), "attention_varlen": ("attention.cu", ["-DATTN_VARLEN"]),
           "attention_varlen_bwd": ("attention_bwd.cu", ["-DATTN_VARLEN"]),
           "attention_kv_fp8": ("attention_kv.cu", ["-DATTN_KV_FP8"]),
-          "attention_paged": ("attention.cu", ["-DATTN_VARLEN", "-DATTN_PAGED"])}
+          "attention_paged": ("attention.cu", ["-DATTN_VARLEN", "-DATTN_PAGED"]),
+          "attention_paged_fp8": ("attention.cu", ["-DATTN_VARLEN", "-DATTN_PAGED", "-DATTN_PAGED_FP8"])}
 NVCC_FLAGS = ["-cubin", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17"]
 
 

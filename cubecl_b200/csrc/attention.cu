@@ -24,6 +24,11 @@
 // Paged varlen (-DATTN_VARLEN -DATTN_PAGED; capi.cpp: b200_attention_varlen_paged): the varlen body with K and V read from a
 // paged KV cache through a block table (warp 0 of the producer warpgroup resolves page ids; lane 0 issues one load per chunk of
 // `rows` keys that starts below the sequence's cache length).  The consumers are varlen's, so are the numerics.
+// Paged fp8 caches (-DATTN_PAGED_FP8 as well; capi.cpp: b200_attention_varlen_paged_fp8): warp 0 loads 128-byte fp8 rows
+// (one box of 128 bytes x rows keys per chunk) into kAttnStages fp8 stages, and warps 1-3 of the producer warpgroup widen
+// each block exactly into the 16-bit ring (the layout the 16-bit TMA loads produce), K and V rows of keys >= Lk as zeros, then
+// arrive on the ring's full barriers (arrive counts instead of TMA byte counts).  The consumers are varlen's but for the
+// scales: t = s * scale_log2 * k_scale[hk], out = (v_scale[hk] O) / l rounded once; lse does not depend on v_scale.
 //
 // Compiled to a cubin (no host code here): nvcc -cubin -gencode arch=compute_90a,code=sm_90a
 #include <cuda_bf16.h>
@@ -37,9 +42,12 @@ using namespace b200;
 
 namespace {
 
+constexpr uint32_t F8T = kAttnBlock * 128u;   // an fp8 K or V stage (paged fp8 caches): one 128-byte row per key
+
 // VL: the varlen kernels (P = AttnVarlenParams; kernel_params.h); the dense kernels have VL = false and P = AttnParams.
 // PG (with VL): the paged varlen kernels (P = AttnVarlenPagedParams): K and V come from a paged cache, the rest is varlen's
-template <int KIND, int DB, int OUT, bool VL, bool PG, class P>
+// CF (with PG): the cache format; CF_E4M3 / CF_E5M2 (P = AttnVarlenPagedFp8Params) widen fp8 pages on the producer warpgroup
+template <int KIND, int DB, int OUT, bool VL, bool PG, int CF, class P>
 __device__ __forceinline__ void attn_body(const CUtensorMap* tq, const CUtensorMap* tk, const CUtensorMap* tv, const CUtensorMap* to,
                                           const P& p) {
   constexpr int NCH = DB / 64;                                // 128-byte (64-element) column chunks of a head
@@ -49,17 +57,25 @@ __device__ __forceinline__ void attn_body(const CUtensorMap* tq, const CUtensorM
   constexpr uint32_t OSZ = (OUT == OUT_F32) ? 4u : 2u;
   constexpr int CW = 128 / OSZ;                               // output columns per 128-byte staging row
   constexpr int NST = DB / CW;                                // TMA stores per consumer
+  constexpr bool F8 = CF != CF_16;                            // fp8 pages, widened by producer warps 1-3
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t sq = base;
   auto sk = [&](uint32_t s) { return base + TILE * (1u + 2u * s); };
   auto sv = [&](uint32_t s) { return base + TILE * (2u + 2u * s); };
-  const uint32_t bars = base + TILE * (1u + 2u * kAttnStages);
+  // fp8: the fp8 K and V stages follow the 16-bit ring
+  auto sk8 = [&](uint32_t s) { return base + TILE * (1u + 2u * kAttnStages) + 2u * F8T * s; };
+  auto sv8 = [&](uint32_t s) { return base + TILE * (1u + 2u * kAttnStages) + 2u * F8T * s + F8T; };
+  const uint32_t bars = base + TILE * (1u + 2u * kAttnStages) + (F8 ? 2u * F8T * kAttnStages : 0u);
   const uint32_t q_bar = bars;
   auto full_k = [&](uint32_t s) { return bars + 8u * (1u + s); };
   auto full_v = [&](uint32_t s) { return bars + 8u * (1u + kAttnStages + s); };
   auto empty = [&](uint32_t s) { return bars + 8u * (1u + 2u * kAttnStages + s); };
+  // fp8: TMA barriers of the fp8 stages, and their release by the widening warps
+  auto full_k8 = [&](uint32_t s) { return bars + 8u * (1u + 3u * kAttnStages + s); };
+  auto full_v8 = [&](uint32_t s) { return bars + 8u * (1u + 4u * kAttnStages + s); };
+  auto empty8 = [&](uint32_t s) { return bars + 8u * (1u + 5u * kAttnStages + s); };
 
   // work: query block (last first), head, batch
   const uint32_t per = p.Hq * p.B;
@@ -98,9 +114,14 @@ __device__ __forceinline__ void attn_body(const CUtensorMap* tq, const CUtensorM
     tma_prefetch_desc(to);
     mbar_init(q_bar, 1);
     for (uint32_t s = 0; s < kAttnStages; ++s) {
-      mbar_init(full_k(s), 1);
-      mbar_init(full_v(s), 1);
+      mbar_init(full_k(s), F8 ? kAttnF8WidenWarps : 1);   // fp8: one arrive per widening warp
+      mbar_init(full_v(s), F8 ? kAttnF8WidenWarps : 1);
       mbar_init(empty(s), 2);   // one arrive per consumer warpgroup
+      if constexpr (F8) {
+        mbar_init(full_k8(s), 1);
+        mbar_init(full_v8(s), 1);
+        mbar_init(empty8(s), kAttnF8WidenWarps);
+      }
     }
     fence_mbar_init();
   }
@@ -108,7 +129,7 @@ __device__ __forceinline__ void attn_body(const CUtensorMap* tq, const CUtensorM
 
   if (wg == 0) {
     // ===================================================================== TMA producer (one thread)
-    setmaxnreg_dec<40>();
+    setmaxnreg_dec<F8 ? 64 : 40>();   // fp8: the widening warps need 64 registers
     if constexpr (PG) {
       // paged: warp 0 reads the block table 32 chunks of `rows` keys at a time, one batch ahead (chunk indices from the CTA's
       // first band block); lane 0 issues one load per chunk that starts below Lk.  Stages keep stale rows where a chunk is not
@@ -139,30 +160,71 @@ __device__ __forceinline__ void attn_body(const CUtensorMap* tq, const CUtensorM
           }
           const int k0 = static_cast<int>(kb * kAttnBlock);
           const uint32_t nload = min(per, static_cast<uint32_t>(Lk - k0 + static_cast<int>(R) - 1) / R);   // chunks below Lk
-          mbar_wait(empty(s), ph ^ 1u);
-          if (lane == 0) {
-            mbar_arrive_expect_tx(full_k(s), nload * NCH * R * 128u);
-            mbar_arrive_expect_tx(full_v(s), nload * NCH * R * 128u);
-          }
-          for (uint32_t i = 0; i < per; ++i) {
-            const int pg = __shfl_sync(0xFFFFFFFFu, cur, (c - cbase + i) & 31u);
-            const int row = static_cast<int>((static_cast<uint32_t>(k0) + i * R) % p.page);
-            if (lane == 0 && i < nload) {
-#pragma unroll
-              for (int cc = 0; cc < NCH; ++cc)
-                tma_load_4d(sk(s) + cc * CHUNK + i * R * 128u, tk, full_k(s), cc * 64, row, static_cast<int>(hk), pg);
+          if constexpr (F8) {
+            // fp8: one 128-byte box per chunk covers the whole head (columns >= D read as zeros)
+            mbar_wait(empty8(s), ph ^ 1u);
+            if (lane == 0) {
+              mbar_arrive_expect_tx(full_k8(s), nload * R * 128u);
+              mbar_arrive_expect_tx(full_v8(s), nload * R * 128u);
             }
-          }
-          for (uint32_t i = 0; i < per; ++i) {
-            const int pg = __shfl_sync(0xFFFFFFFFu, cur, (c - cbase + i) & 31u);
-            const int row = static_cast<int>((static_cast<uint32_t>(k0) + i * R) % p.page);
-            if (lane == 0 && i < nload) {
+            for (uint32_t i = 0; i < per; ++i) {
+              const int pg = __shfl_sync(0xFFFFFFFFu, cur, (c - cbase + i) & 31u);
+              const int row = static_cast<int>((static_cast<uint32_t>(k0) + i * R) % p.page);
+              if (lane == 0 && i < nload) {
+                tma_load_4d(sk8(s) + i * R * 128u, tk, full_k8(s), 0, row, static_cast<int>(hk), pg);
+                tma_load_4d(sv8(s) + i * R * 128u, tv, full_v8(s), 0, row, static_cast<int>(hk), pg);
+              }
+            }
+          } else {
+            mbar_wait(empty(s), ph ^ 1u);
+            if (lane == 0) {
+              mbar_arrive_expect_tx(full_k(s), nload * NCH * R * 128u);
+              mbar_arrive_expect_tx(full_v(s), nload * NCH * R * 128u);
+            }
+            for (uint32_t i = 0; i < per; ++i) {
+              const int pg = __shfl_sync(0xFFFFFFFFu, cur, (c - cbase + i) & 31u);
+              const int row = static_cast<int>((static_cast<uint32_t>(k0) + i * R) % p.page);
+              if (lane == 0 && i < nload) {
 #pragma unroll
-              for (int cc = 0; cc < NCH; ++cc)
-                tma_load_4d(sv(s) + cc * CHUNK + i * R * 128u, tv, full_v(s), cc * 64, row, static_cast<int>(hk), pg);
+                for (int cc = 0; cc < NCH; ++cc)
+                  tma_load_4d(sk(s) + cc * CHUNK + i * R * 128u, tk, full_k(s), cc * 64, row, static_cast<int>(hk), pg);
+              }
+            }
+            for (uint32_t i = 0; i < per; ++i) {
+              const int pg = __shfl_sync(0xFFFFFFFFu, cur, (c - cbase + i) & 31u);
+              const int row = static_cast<int>((static_cast<uint32_t>(k0) + i * R) % p.page);
+              if (lane == 0 && i < nload) {
+#pragma unroll
+                for (int cc = 0; cc < NCH; ++cc)
+                  tma_load_4d(sv(s) + cc * CHUNK + i * R * 128u, tv, full_v(s), cc * 64, row, static_cast<int>(hk), pg);
+              }
             }
           }
           __syncwarp();
+          if (++s == kAttnStages) { s = 0; ph ^= 1u; }
+        }
+      } else if constexpr (F8) {
+        // fp8: warps 1-3 widen block kb from fp8 stage s into 16-bit stage s once the consumers have released it; rows of
+        // keys >= Lk (stale slots, or chunks never loaded) become zeros.  Each warp makes its writes visible to wgmma and
+        // arrives once on the stage's full barrier, then releases the fp8 stage to warp 0.
+        const uint32_t t = threadIdx.x - 32u, wl = threadIdx.x & 31u;
+        uint32_t s = 0, ph = 0;
+        for (uint32_t kb = kb_lo; kb < nkb; ++kb) {
+          const uint32_t z = static_cast<uint32_t>(min(max(Lk - static_cast<int>(kb * kAttnBlock), 0), kAttnBlock));
+          mbar_wait(empty(s), ph ^ 1u);
+          mbar_wait(full_k8(s), ph);
+          widen_block<KIND, CF, DB, kAttnBlock, 32 * kAttnF8WidenWarps>(sk8(s), sk(s), z, t);
+          fence_proxy_async_smem();   // generic-proxy writes -> visible to wgmma
+          __syncwarp();
+          if (wl == 0) mbar_arrive(full_k(s));
+          mbar_wait(full_v8(s), ph);
+          widen_block<KIND, CF, DB, kAttnBlock, 32 * kAttnF8WidenWarps>(sv8(s), sv(s), z, t);
+          fence_proxy_async_smem();
+          __syncwarp();
+          if (wl == 0) {
+            mbar_arrive(full_v(s));
+            mbar_arrive(empty8(s));   // the warp has read both fp8 blocks
+          }
           if (++s == kAttnStages) { s = 0; ph ^= 1u; }
         }
       }
@@ -187,7 +249,7 @@ __device__ __forceinline__ void attn_body(const CUtensorMap* tq, const CUtensorM
   }
 
   // ======================================================================= consumers: 64 query rows each
-  setmaxnreg_inc<232>();
+  setmaxnreg_inc<F8 ? 216 : 232>();   // fp8: 128 x 64 + 256 x 216 <= the 384 x 168 the CTA launched with
   const uint32_t cw = wg - 1u;
   const uint32_t t = threadIdx.x & 127u;
   const uint32_t lane = t & 31u, wq = t >> 5;
@@ -195,7 +257,8 @@ __device__ __forceinline__ void attn_body(const CUtensorMap* tq, const CUtensorM
   const uint32_t r = wq * 16u + (lane >> 2);
   const uint32_t i0 = qb * kAttnBlock + cw * 64u + r, i1 = i0 + 8u;
   const uint32_t col = 2u * (lane & 3u);
-  const float c2 = p.scale_log2;
+  float c2 = p.scale_log2;
+  if constexpr (F8) c2 = p.scale_log2 * reinterpret_cast<const float*>(p.k_scale)[hk];   // one f32 product per CTA
 
   float o[NO];
 #pragma unroll
@@ -302,7 +365,7 @@ __device__ __forceinline__ void attn_body(const CUtensorMap* tq, const CUtensorM
 
     // ---- O += P V: V [keys, D] is an MN-major B operand, 16 keys (2048 bytes of rows) per instruction
     mbar_wait(full_v(s), ph);
-    if constexpr (VL) {   // V rows past Lk are the next sequence's (maybe NaN or inf; 0 * NaN = NaN in the product): zero them
+    if constexpr (VL && !F8) {   // V rows past Lk are the next sequence's (maybe NaN or inf; 0 * NaN = NaN in the product): zero them
       const int valid = Lk - static_cast<int>(kb * kAttnBlock);
       if (valid < kAttnBlock) zero_rows(sv(s), NCH, CHUNK, valid, kAttnBlock, 1u + cw);
     }
@@ -322,6 +385,11 @@ __device__ __forceinline__ void attn_body(const CUtensorMap* tq, const CUtensorM
   }
 
   // ---- epilogue: l over the quad, O / l through the consumer's rows of the Q tile, TMA stores clipped at Sq and D
+  if constexpr (F8) {   // out = (v_scale O) / l
+    const float vs = reinterpret_cast<const float*>(p.v_scale)[hk];
+#pragma unroll
+    for (int i = 0; i < NO; ++i) o[i] = __fmul_rn(vs, o[i]);
+  }
   l0 += __shfl_xor_sync(0xFFFFFFFFu, l0, 1);
   l0 += __shfl_xor_sync(0xFFFFFFFFu, l0, 2);
   l1 += __shfl_xor_sync(0xFFFFFFFFu, l1, 1);
@@ -401,7 +469,13 @@ __device__ __forceinline__ void attn_body(const CUtensorMap* tq, const CUtensorM
 // name: attn_fwd_<in>_d<64|128>_<out>; D <= 64 runs the d64 kernel, 64 < D <= 128 the d128 kernel
 // varlen (compiled with -DATTN_VARLEN into its own cubin): attn_fwd_varlen_<in>_d<64|128>_<out>
 // paged varlen (-DATTN_VARLEN -DATTN_PAGED, cubin attention_paged): attn_fwd_paged_<in>_d<64|128>_<out>
-#if defined(ATTN_VARLEN) && defined(ATTN_PAGED)
+// paged varlen, fp8 caches (-DATTN_VARLEN -DATTN_PAGED -DATTN_PAGED_FP8, cubin attention_paged_fp8):
+// attn_fwd_paged_<in>_<e4m3|e5m2>_d<64|128>_<out>
+#if defined(ATTN_VARLEN) && defined(ATTN_PAGED) && defined(ATTN_PAGED_FP8)
+#define ATTN_VL true
+#define ATTN_PG true
+#define ATTN_P AttnVarlenPagedFp8Params
+#elif defined(ATTN_VARLEN) && defined(ATTN_PAGED)
 #define ATTN_VL true
 #define ATTN_PG true
 #define ATTN_P AttnVarlenPagedParams
@@ -417,13 +491,25 @@ __device__ __forceinline__ void attn_body(const CUtensorMap* tq, const CUtensorM
 #define ATTN_P AttnParams
 #define ATTN_NAME(IN, D, OUT) attn_fwd_##IN##_d##D##_##OUT
 #endif
-#define ATTN_KERNEL(NAME, KIND, DB, OUT)                                                                             \
+#define ATTN_KERNEL_CF(NAME, KIND, DB, OUT, CF)                                                                      \
   extern "C" __global__ void __launch_bounds__(384, 1)                                                               \
       NAME(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,                         \
            const __grid_constant__ CUtensorMap tv, const __grid_constant__ CUtensorMap to,                         \
            const __grid_constant__ ATTN_P p) {                                                                      \
-    attn_body<KIND, DB, OUT, ATTN_VL, ATTN_PG>(&tq, &tk, &tv, &to, p);                                              \
+    attn_body<KIND, DB, OUT, ATTN_VL, ATTN_PG, CF>(&tq, &tk, &tv, &to, p);                                          \
   }
+#ifdef ATTN_PAGED_FP8
+#define ATTN_F8_D(IN, KIND, OUT16, F, CF)                                                    \
+  ATTN_KERNEL_CF(attn_fwd_paged_##IN##_##F##_d64_##IN, KIND, 64, OUT16, CF)                \
+  ATTN_KERNEL_CF(attn_fwd_paged_##IN##_##F##_d64_f32, KIND, 64, OUT_F32, CF)               \
+  ATTN_KERNEL_CF(attn_fwd_paged_##IN##_##F##_d128_##IN, KIND, 128, OUT16, CF)              \
+  ATTN_KERNEL_CF(attn_fwd_paged_##IN##_##F##_d128_f32, KIND, 128, OUT_F32, CF)
+ATTN_F8_D(f16, KIND_F16, OUT_F16, e4m3, CF_E4M3)
+ATTN_F8_D(f16, KIND_F16, OUT_F16, e5m2, CF_E5M2)
+ATTN_F8_D(bf16, KIND_BF16, OUT_BF16, e4m3, CF_E4M3)
+ATTN_F8_D(bf16, KIND_BF16, OUT_BF16, e5m2, CF_E5M2)
+#else
+#define ATTN_KERNEL(NAME, KIND, DB, OUT) ATTN_KERNEL_CF(NAME, KIND, DB, OUT, CF_16)
 #define ATTN_D(IN, KIND, OUT16)                                  \
   ATTN_KERNEL(ATTN_NAME(IN, 64, IN), KIND, 64, OUT16)            \
   ATTN_KERNEL(ATTN_NAME(IN, 64, f32), KIND, 64, OUT_F32)         \
@@ -431,3 +517,4 @@ __device__ __forceinline__ void attn_body(const CUtensorMap* tq, const CUtensorM
   ATTN_KERNEL(ATTN_NAME(IN, 128, f32), KIND, 128, OUT_F32)
 ATTN_D(f16, KIND_F16, OUT_F16)
 ATTN_D(bf16, KIND_BF16, OUT_BF16)
+#endif

@@ -47,58 +47,6 @@ __device__ __forceinline__ void store_pair(uint64_t addr, float x0, float x1) {
   }
 }
 
-// Cache formats: the 16-bit input dtype itself, or fp8 widened on chip.
-enum : int { CF_16 = 0, CF_E4M3 = 1, CF_E5M2 = 2 };
-
-// Four fp8 values (memory order) -> two pairs of the 16-bit KIND, exactly: every e4m3 and e5m2 value is an f16 and a bf16
-// value.  bf16 goes through f32 (f16 -> f32 -> bf16, each step exact).
-template <int KIND, int CF>
-__device__ __forceinline__ void widen4(uint32_t w, uint32_t& lo, uint32_t& hi) {
-  const unsigned short w0 = static_cast<unsigned short>(w), w1 = static_cast<unsigned short>(w >> 16);
-  if constexpr (CF == CF_E4M3) {
-    asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(lo) : "h"(w0));
-    asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(hi) : "h"(w1));
-  } else {
-    asm("cvt.rn.f16x2.e5m2x2 %0, %1;" : "=r"(lo) : "h"(w0));
-    asm("cvt.rn.f16x2.e5m2x2 %0, %1;" : "=r"(hi) : "h"(w1));
-  }
-  if constexpr (KIND == KIND_BF16) {
-    asm("{.reg .b16 a, b; .reg .f32 x, y;\n\t"
-        "mov.b32 {a, b}, %0; cvt.f32.f16 x, a; cvt.f32.f16 y, b; cvt.rn.bf16x2.f32 %0, y, x;}" : "+r"(lo));
-    asm("{.reg .b16 a, b; .reg .f32 x, y;\n\t"
-        "mov.b32 {a, b}, %0; cvt.f32.f16 x, a; cvt.f32.f16 y, b; cvt.rn.bf16x2.f32 %0, y, x;}" : "+r"(hi));
-  }
-}
-
-// Widen one fp8 block (kAttnKvBlock rows of 128 swizzled bytes at src, as the 128-byte TMA box wrote it) into the 16-bit
-// 128-byte-swizzled layout at dst that the 16-bit kernels' TMA loads produce (DB / 64 chunks of kAttnKvBlock rows x 128
-// bytes).  Rows >= z are written as zeros (the V rows of keys past L: stale bytes may be NaN or inf).  One 16-byte unit of 16
-// values per thread and step; the two 16-byte stores of a unit go out in an order that keeps a quarter warp on distinct banks.
-template <int KIND, int CF, int DB>
-__device__ __forceinline__ void widen_block(uint32_t src, uint32_t dst, uint32_t z, uint32_t t) {
-  constexpr uint32_t UPR = DB / 16;   // 16-byte fp8 units per row
-#pragma unroll
-  for (uint32_t i = 0; i < kAttnKvBlock * UPR / 128u; ++i) {
-    const uint32_t u = t + 128u * i, j = u / UPR, g = u % UPR, sw = j & 7u;
-    uint32_t w0, w1, w2, w3;
-    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(w0), "=r"(w1), "=r"(w2), "=r"(w3) : "r"(src + j * 128u + ((g ^ sw) << 4)));
-    uint32_t h[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
-    if (j < z) {
-      widen4<KIND, CF>(w0, h[0], h[1]);
-      widen4<KIND, CF>(w1, h[2], h[3]);
-      widen4<KIND, CF>(w2, h[4], h[5]);
-      widen4<KIND, CF>(w3, h[6], h[7]);
-    }
-    const uint32_t row = dst + (g >> 2) * (kAttnKvBlock * 128u) + j * 128u;
-    const uint32_t c0 = 2u * (g & 3u), f = (g >> 2) & 1u;   // 16-byte groups c0, c0 + 1; f: store c0 + 1 first
-    const uint32_t a0 = row + (((c0 + f) ^ sw) << 4), a1 = row + (((c0 + 1u - f) ^ sw) << 4);
-    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a0), "r"(f ? h[4] : h[0]), "r"(f ? h[5] : h[1]), "r"(f ? h[6] : h[2]),
-                 "r"(f ? h[7] : h[3]) : "memory");
-    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a1), "r"(f ? h[0] : h[4]), "r"(f ? h[1] : h[5]), "r"(f ? h[2] : h[6]),
-                 "r"(f ? h[3] : h[7]) : "memory");
-  }
-}
-
 template <int KIND, int DB, int OUT, int CF = CF_16>
 __device__ __forceinline__ void kv_body(const CUtensorMap* tq, const CUtensorMap* tk, const CUtensorMap* tv, const AttnKvParams& p) {
   constexpr int NCH = DB / 64;                          // 128-byte (64-element) column chunks of a head
@@ -270,7 +218,7 @@ __device__ __forceinline__ void kv_body(const CUtensorMap* tq, const CUtensorMap
     // wgmma in a slower warp; every warp has passed that wgmma's wait before the barrier after this block's V widening)
     const uint32_t kbuf = kw + (kb & 1u) * KT;
     if constexpr (CF != CF_16) {
-      widen_block<KIND, CF, DB>(sk(s), kbuf, KB, t);
+      widen_block<KIND, CF, DB, KB, 128>(sk(s), kbuf, KB, t);
       fence_proxy_async_smem();   // generic-proxy writes -> visible to wgmma
       asm volatile("bar.sync 1, 128;" ::: "memory");
     }
@@ -286,7 +234,7 @@ __device__ __forceinline__ void kv_body(const CUtensorMap* tq, const CUtensorMap
     if constexpr (CF != CF_16) {
       // widen V while S = Q K^T runs; the V rows of keys >= L become zeros here (stale slots, or chunks never loaded)
       mbar_wait(full_v(s), ph);
-      widen_block<KIND, CF, DB>(sv(s), vw, static_cast<uint32_t>(min(max(L - static_cast<int>(kb) * KB, 0), KB)), t);
+      widen_block<KIND, CF, DB, KB, 128>(sv(s), vw, static_cast<uint32_t>(min(max(L - static_cast<int>(kb) * KB, 0), KB)), t);
       fence_proxy_async_smem();
       asm volatile("bar.sync 1, 128;" ::: "memory");
       if (t == 0) mbar_arrive(empty(s));   // every consumer thread is done with the fp8 stage

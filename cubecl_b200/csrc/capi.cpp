@@ -71,6 +71,8 @@ extern const unsigned char b200_cubin_attention_kv_fp8[];
 extern const unsigned char b200_cubin_attention_kv_fp8_end[];
 extern const unsigned char b200_cubin_attention_paged[];
 extern const unsigned char b200_cubin_attention_paged_end[];
+extern const unsigned char b200_cubin_attention_paged_fp8[];
+extern const unsigned char b200_cubin_attention_paged_fp8_end[];
 }
 
 // ================================================================================================ errors
@@ -343,12 +345,13 @@ static int get_func(b200_ctx* c, const std::string& name, CUfunction* out) {
   if (it != c->funcs.end()) { *out = it->second; return B200_OK; }
   // modules are loaded in the order gemm, reduce, aux, gemm_b, gemm_c, quant, gemm_q, quant_mm, gemm_conv, gemm_convbwd,
   // conv_grouped, gemm_conv3d, gemm_convt, attention, attention_bwd, attention_kv, attention_varlen, attention_varlen_bwd,
-  // attention_kv_fp8, attention_paged; the kernel name says where a
+  // attention_kv_fp8, attention_paged, attention_paged_fp8; the kernel name says where a
   // kernel lives (no failing lookups, which API-level tools such as compute-sanitizer would report)
   auto starts = [&](const char* pfx) { return name.rfind(pfx, 0) == 0; };
   auto has = [&](const char* part) { return name.find(part) != std::string::npos; };
   const bool tc_gemm = starts("gemm_") && name != "gemm_simt_strided" && name != "gemm_scaled_simt";
   const size_t home = name == "conv3d_dgrad_weights" ? 2
+                      : starts("attn_fwd_paged_") && (has("_e4m3_") || has("_e5m2_")) ? 20
                       : starts("attn_fwd_paged_") ? 19
                       : starts("attn_kv_") && (has("_e4m3_") || has("_e5m2_") || has("_fp8")) ? 18
                       : starts("attn_bwd_varlen_") ? 17
@@ -402,7 +405,8 @@ extern "C" int b200_get_cubin(const char* name, const void** image, size_t* size
   else if (!strcmp(name, "attention_varlen_bwd")) { b = b200_cubin_attention_varlen_bwd; e = b200_cubin_attention_varlen_bwd_end; }
   else if (!strcmp(name, "attention_kv_fp8")) { b = b200_cubin_attention_kv_fp8; e = b200_cubin_attention_kv_fp8_end; }
   else if (!strcmp(name, "attention_paged")) { b = b200_cubin_attention_paged; e = b200_cubin_attention_paged_end; }
-  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd|conv_grouped|gemm_conv3d|gemm_convt|attention|attention_bwd|attention_kv|attention_varlen|attention_varlen_bwd|attention_kv_fp8|attention_paged)", name);
+  else if (!strcmp(name, "attention_paged_fp8")) { b = b200_cubin_attention_paged_fp8; e = b200_cubin_attention_paged_fp8_end; }
+  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd|conv_grouped|gemm_conv3d|gemm_convt|attention|attention_bwd|attention_kv|attention_varlen|attention_varlen_bwd|attention_kv_fp8|attention_paged|attention_paged_fp8)", name);
   *image = b;
   *size = static_cast<size_t>(e - b);
   return B200_OK;
@@ -469,7 +473,8 @@ extern "C" int b200_init(int device, b200_ctx** out) {
       (rc = load_module(c, b200_cubin_attention_varlen, b200_cubin_attention_varlen_end, "attention_varlen")) ||
       (rc = load_module(c, b200_cubin_attention_varlen_bwd, b200_cubin_attention_varlen_bwd_end, "attention_varlen_bwd")) ||
       (rc = load_module(c, b200_cubin_attention_kv_fp8, b200_cubin_attention_kv_fp8_end, "attention_kv_fp8")) ||
-      (rc = load_module(c, b200_cubin_attention_paged, b200_cubin_attention_paged_end, "attention_paged"))) {
+      (rc = load_module(c, b200_cubin_attention_paged, b200_cubin_attention_paged_end, "attention_paged")) ||
+      (rc = load_module(c, b200_cubin_attention_paged_fp8, b200_cubin_attention_paged_fp8_end, "attention_paged_fp8"))) {
     for (CUmodule m : c->modules) g_drv.cuModuleUnload_p(m);
     g_drv.cuDevicePrimaryCtxRelease_p(c->dev);
     return bail(rc);
@@ -4352,7 +4357,8 @@ static int attn_check_caches(const char* what, const AttnView& kc, const AttnVie
 // ---- launch sequences the dense, varlen and paged varlen entry points share
 // Stages q, k and v (k and v only with stage_kv: a paged cache is read in place, never gathered), maps them (q in loads of
 // kAttnBlock rows, k and v of kv_rows) and out, then launches `<prefix><in>_d<DB>_<out>` on `ctas` CTAs with the filled
-// parameter block p.
+// parameter block p.  fp8 k and v (paged fp8 caches) launch `<prefix><in>_<e4m3|e5m2>_d<DB>_<out>` with kAttnStages fp8 K and
+// V stages of kAttnBlock 128-byte rows more shared memory.
 static int attn_fwd_launch(b200_ctx* c, CUstream st, const std::string& prefix, AttnView q, AttnView k, AttnView v, const AttnView& o,
                            uint64_t ctas, void* p, uint32_t kv_rows = kAttnBlock, bool stage_kv = true) {
   CUdeviceptr tmp[3] = {0, 0, 0};
@@ -4365,9 +4371,11 @@ static int attn_fwd_launch(b200_ctx* c, CUstream st, const std::string& prefix, 
   if (!rc) rc = attn_map(c, &mv, v, false, kv_rows);
   if (!rc) rc = attn_map(c, &mo, o, true);
   const uint32_t DB = attn_db(q.shape[3]);
+  const bool f8 = k.esz == 1;
+  const std::string fmt = !f8 ? "" : k.dt == B200_F8E5M2 ? "_e5m2" : "_e4m3";
   CUfunction f = nullptr;
-  if (!rc) rc = get_func(c, prefix + dt_tag(q.dt) + "_d" + std::to_string(DB) + "_" + dt_tag(o.dt), &f);
-  const unsigned smem = 1024 + (1 + 2 * kAttnStages) * kAttnBlock * DB * 2 + 1024;
+  if (!rc) rc = get_func(c, prefix + dt_tag(q.dt) + fmt + "_d" + std::to_string(DB) + "_" + dt_tag(o.dt), &f);
+  const unsigned smem = 1024 + (1 + 2 * kAttnStages) * kAttnBlock * DB * 2 + (f8 ? kAttnStages * 2 * kAttnBlock * 128 : 0) + 1024;
   if (!rc) rc = attn_set_smem(c, f, smem);
   void* kargs[] = {&mq, &mk, &mv, &mo, p};
   if (!rc) rc = launch(c, f, (unsigned)ctas, 1, 1, 384, smem, 1, st, kargs);
@@ -4905,20 +4913,20 @@ extern "C" int b200_attention_kvcache_fp8(b200_ctx* c, b200_stream s, b200_dtype
 
 // ------------------------------------------------------------------------------------------------ paged varlen attention
 // Packed queries against a paged KV cache (see cubecl_b200.h): the gather of q if needed, then one attn_fwd_paged_* launch.
-extern "C" int b200_attention_varlen_paged(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr q,
-                                           const uint64_t* q_shape, const uint64_t* q_strides, b200_dptr k_cache, const uint64_t* kc_shape,
-                                           const uint64_t* kc_strides, b200_dptr v_cache, const uint64_t* vc_shape,
-                                           const uint64_t* vc_strides, b200_dptr block_table, const uint64_t* bt_shape,
-                                           const uint64_t* bt_strides, b200_dptr cu_seqlens_q, b200_dptr cache_seqlens, uint64_t batch,
-                                           b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides, b200_dptr lse,
-                                           const b200_attention_varlen_args* args) {
-  CTX_ENTER(c);
-  const char* what = "attention_varlen_paged";
+// f8: an fp8 cache (b200_attention_varlen_paged_fp8), else the caches hold the input dtype.
+static int vl_paged_attend(b200_ctx* c, b200_stream s, const char* what, b200_dtype in_dtype, const KvFp8* f8, b200_dtype out_dtype,
+                           b200_dptr q, const uint64_t* q_shape, const uint64_t* q_strides, b200_dptr k_cache, const uint64_t* kc_shape,
+                           const uint64_t* kc_strides, b200_dptr v_cache, const uint64_t* vc_shape, const uint64_t* vc_strides,
+                           b200_dptr block_table, const uint64_t* bt_shape, const uint64_t* bt_strides, b200_dptr cu_seqlens_q,
+                           b200_dptr cache_seqlens, uint64_t batch, b200_dptr out, const uint64_t* out_shape,
+                           const uint64_t* out_strides, b200_dptr lse, const b200_attention_varlen_args* args) {
   if (!q_shape || !kc_shape || !vc_shape || !out_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
   if (block_table && !bt_shape) return fail(B200_ERR_INVALID_ARG, "%s: null block-table shape", what);
   int rc = attn_check_in_dtype(what, in_dtype);
   if (!rc) rc = attn_check_out_dtype(what, "output", in_dtype, out_dtype);
+  if (!rc) rc = kv_check_fp8(what, f8);
   if (rc) return rc;
+  const b200_dtype cache_dtype = f8 ? f8->cache : in_dtype;
   const uint64_t Tq = q_shape[0], Hq = q_shape[1], D = q_shape[2], B = batch;
   const uint64_t P = kc_shape[0], page = kc_shape[1], Hkv = kc_shape[2];
   if (kc_shape[3] != D)
@@ -4944,14 +4952,15 @@ extern "C" int b200_attention_varlen_paged(b200_ctx* c, b200_stream s, b200_dtyp
   if (!q || !k_cache || !v_cache || !out || !cu_seqlens_q || !cache_seqlens) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
   if (lse % 4 || cu_seqlens_q % 4 || cache_seqlens % 4 || block_table % 4)
     return fail(B200_ERR_INVALID_ARG, "%s: lse, cu_seqlens_q, cache_seqlens and block_table must be 4-byte aligned", what);
+  if ((rc = kv_check_scales(what, f8))) return rc;
   const AttnView ov = attn_view(out, out_dtype, out_shape, out_strides, kAttnTHD);
-  const AttnView kv = attn_view(k_cache, in_dtype, kc_shape, kc_strides, kAttnBSHD), vv = attn_view(v_cache, in_dtype, vc_shape, vc_strides, kAttnBSHD);
+  const AttnView kv = attn_view(k_cache, cache_dtype, kc_shape, kc_strides, kAttnBSHD), vv = attn_view(v_cache, cache_dtype, vc_shape, vc_strides, kAttnBSHD);
   if ((rc = attn_check_out_view(what, "out", ov)) || (rc = attn_check_caches(what, kv, vv))) return rc;
 
   // keys per TMA load: a chunk of a 128-key block never crosses a page; one page per sequence is read in 128-row boxes, the
   // rows past the page zero-filled
   const uint32_t R = max_pages == 1 ? kAttnBlock : (uint32_t)std::gcd<uint64_t>(page, kAttnBlock);
-  AttnVarlenPagedParams p{};
+  AttnVarlenPagedFp8Params p{};   // the 16-bit kernels take its AttnVarlenPagedParams base
   p.lse = lse;
   p.cu_q = cu_seqlens_q;
   p.out = out; p.o_st = ov.s_row(); p.o_sh = ov.s_head();
@@ -4971,8 +4980,38 @@ extern "C" int b200_attention_varlen_paged(b200_ctx* c, b200_stream s, b200_dtyp
   p.seqlens = cache_seqlens;
   p.page = (uint32_t)page; p.rows = R;
   p.cap = (uint32_t)cap;
+  if (f8) { p.k_scale = f8->k_scale; p.v_scale = f8->v_scale; }
+  void* pp = f8 ? static_cast<void*>(&p) : static_cast<void*>(static_cast<AttnVarlenPagedParams*>(&p));
   return attn_fwd_launch(c, resolve_stream(c, s), "attn_fwd_paged_", attn_view(q, in_dtype, q_shape, q_strides, kAttnTHD), kv, vv, ov,
-                         ctas, &p, R, false);
+                         ctas, pp, R, false);
+}
+
+extern "C" int b200_attention_varlen_paged(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr q,
+                                           const uint64_t* q_shape, const uint64_t* q_strides, b200_dptr k_cache, const uint64_t* kc_shape,
+                                           const uint64_t* kc_strides, b200_dptr v_cache, const uint64_t* vc_shape,
+                                           const uint64_t* vc_strides, b200_dptr block_table, const uint64_t* bt_shape,
+                                           const uint64_t* bt_strides, b200_dptr cu_seqlens_q, b200_dptr cache_seqlens, uint64_t batch,
+                                           b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides, b200_dptr lse,
+                                           const b200_attention_varlen_args* args) {
+  CTX_ENTER(c);
+  return vl_paged_attend(c, s, "attention_varlen_paged", in_dtype, nullptr, out_dtype, q, q_shape, q_strides, k_cache, kc_shape,
+                         kc_strides, v_cache, vc_shape, vc_strides, block_table, bt_shape, bt_strides, cu_seqlens_q, cache_seqlens,
+                         batch, out, out_shape, out_strides, lse, args);
+}
+
+extern "C" int b200_attention_varlen_paged_fp8(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype cache_dtype,
+                                               b200_dtype out_dtype, b200_dptr q, const uint64_t* q_shape, const uint64_t* q_strides,
+                                               b200_dptr k_cache, const uint64_t* kc_shape, const uint64_t* kc_strides,
+                                               b200_dptr v_cache, const uint64_t* vc_shape, const uint64_t* vc_strides,
+                                               b200_dptr block_table, const uint64_t* bt_shape, const uint64_t* bt_strides,
+                                               b200_dptr cu_seqlens_q, b200_dptr cache_seqlens, uint64_t batch, b200_dptr k_scale,
+                                               b200_dptr v_scale, b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides,
+                                               b200_dptr lse, const b200_attention_varlen_args* args) {
+  CTX_ENTER(c);
+  const KvFp8 f8{cache_dtype, k_scale, v_scale};
+  return vl_paged_attend(c, s, "attention_varlen_paged_fp8", in_dtype, &f8, out_dtype, q, q_shape, q_strides, k_cache, kc_shape,
+                         kc_strides, v_cache, vc_shape, vc_strides, block_table, bt_shape, bt_strides, cu_seqlens_q, cache_seqlens,
+                         batch, out, out_shape, out_strides, lse, args);
 }
 
 // Scatter of new tokens into a paged KV cache (see cubecl_b200.h): one attn_kv_write launch, or attn_kv_write_fp8 (f8: an

@@ -304,6 +304,23 @@ struct AttnVarlenPagedParams : AttnVarlenParams {
   uint32_t pad;
 };
 
+// Paged varlen attention against fp8 caches: attention.cu compiled with -DATTN_VARLEN -DATTN_PAGED -DATTN_PAGED_FP8
+// (attn_fwd_paged_<in>_<e4m3|e5m2>_d<64|128>_<out>, cubin attention_paged_fp8; capi.cpp: b200_attention_varlen_paged_fp8).
+// The paged varlen kernel with e4m3 / e5m2 caches read through UINT8 maps: a chunk of `rows` keys arrives as one box of
+// 128 bytes x rows (the whole head, columns >= D zero-filled) in an fp8 stage of kAttnBlock 128-byte rows, and the
+// kAttnF8WidenWarps idle warps of the producer warpgroup widen it into the 16-bit ring of the 16-bit kernel (K and V rows of
+// keys >= Lk as zeros).  Their full barriers count one arrive per widening warp instead of TMA bytes.
+// Shared memory: 1024 (alignment slack) + (1 + 2 * kAttnStages) tiles of kAttnBlock rows x DB 16-bit (Q and the 16-bit
+// ring) + kAttnStages x 2 fp8 stages of kAttnBlock x 128 bytes + 1024 (13 barriers: q, full K / V and empty of the ring,
+// full K / V and empty of the fp8 stages).  At DB = 128: 1024 + 5 x 32768 + 65536 + 1024 = 231424 bytes, under the 232448-byte
+// opt-in limit; at DB = 64: 148480.  Both fp8 stages fit, so there is no one-stage variant.  Registers: the producer
+// warpgroup runs at 64 (the widening spills at 40 and 56), the consumers at 216.  k_scale and v_scale are f32 [Hkv]:
+// t = s * (scale_log2 * k_scale[hk]) and out = (v_scale[hk] O) / l.
+constexpr int kAttnF8WidenWarps = 3;
+struct AttnVarlenPagedFp8Params : AttnVarlenPagedParams {
+  uint64_t k_scale, v_scale;      // f32 [Hkv] per-head scales
+};
+
 // ================================================================================================ attention_kv.cu
 // Attention against a KV cache (attn_kv_*; capi.cpp: b200_attention_kvcache).  One CTA per (b, hk, m-tile, split), grid
 // B * Hkv * nsplit * mtiles with block x = ((b * Hkv + hk) * nsplit + split) * mtiles + mt (the m-tiles that share a key range

@@ -816,6 +816,36 @@ int b200_kvcache_write_fp8(b200_ctx* ctx, b200_stream s, b200_dtype dtype, b200_
                            b200_dptr v_cache, const uint64_t* vc_shape, const uint64_t* vc_strides,
                            b200_dptr slot_mapping, b200_dptr k_scale, b200_dptr v_scale);
 
+/* ---- paged variable-length attention against fp8 caches (chunked prefill and prefix caching with kv_cache_dtype="fp8";
+ * flash_attn_varlen_func with block_table, seqused_k and k_descale / v_descale) ------------------------------------------
+ * b200_attention_varlen_paged with the caches in B200_F8E4M3 or B200_F8E5M2 (cache_dtype, both caches) and two compact f32
+ * [Hkv] device arrays k_scale and v_scale as b200_attention_kvcache_fp8's: the cache holds K = k_scale[hk] * k8 and
+ * V = v_scale[hk] * v8.  Write the cache with b200_kvcache_write_fp8.  Queries, keys, paging, visibility, stale slots, rows
+ * outside every sequence, lse and the launch grid are those of b200_attention_varlen_paged.
+ * Numerics: K and V are widened on chip to q's dtype, exactly (every e4m3 and e5m2 value is an f16 and a bf16 value); t = s * c
+ * with s the f32 score of q against the widened K and c = (scale * log2 e) * k_scale[hk], one f32 product per CTA; the online
+ * softmax and P rounding of b200_attention_varlen; out = (v_scale[hk] * O) / l rounded once; lse does not depend on v_scale.
+ * So with power-of-two scales (and scales of 1), every sequence's out and lse equal bit for bit those of a
+ * b200_attention_varlen_paged call with the same arguments on the dequantized 16-bit cache (scale * code in q's dtype).  A row
+ * with no visible key gets out = +0 and lse = -inf.  No atomics: bitwise reproducible.
+ * Views: q is read in place or gathered as in b200_attention_varlen_paged; a cache is read in place with a unit D stride and a
+ * 16-byte aligned base and strides, in bytes: a compact fp8 cache needs D % 16 == 0.
+ * Errors: b200_attention_varlen_paged's, plus B200_ERR_UNSUPPORTED for a cache dtype that is not fp8 and B200_ERR_INVALID_ARG
+ * for a null or not 4-byte aligned k_scale or v_scale.  batch, Tq, Hq or max_seqlen_q = 0: no launch.
+ * Launches, on `s` with no host synchronisation: the gather of q if needed, then one
+ * attn_fwd_paged_<in>_<e4m3|e5m2>_d<64|128>_<out> launch of ceil(max_seqlen_q / 128) * Hq * batch CTAs with 64 KiB more
+ * shared memory than b200_attention_varlen_paged's (two fp8 K and V stages).  The plan's k_cache and v_cache maps have esz=1
+ * and box (128, R, 1, 1), R as in b200_attention_varlen_paged. */
+int b200_attention_varlen_paged_fp8(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b200_dtype cache_dtype, b200_dtype out_dtype,
+                                    b200_dptr q, const uint64_t* q_shape, const uint64_t* q_strides,
+                                    b200_dptr k_cache, const uint64_t* kc_shape, const uint64_t* kc_strides,
+                                    b200_dptr v_cache, const uint64_t* vc_shape, const uint64_t* vc_strides,
+                                    b200_dptr block_table, const uint64_t* bt_shape, const uint64_t* bt_strides,
+                                    b200_dptr cu_seqlens_q, b200_dptr cache_seqlens, uint64_t batch,
+                                    b200_dptr k_scale, b200_dptr v_scale,
+                                    b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides,
+                                    b200_dptr lse, const b200_attention_varlen_args* args);
+
 /* ---- collectives: ServerCommunication (server/base.rs:632-739), CUDA impl cubecl-cuda/src/compute/server.rs:666-926 -- */
 #define B200_UNIQUE_ID_BYTES 128
 int b200_comm_get_unique_id(b200_ctx* ctx, void* id128);            /* ncclGetUniqueId (communication.rs:11-25 holds it per device set) */

@@ -522,6 +522,32 @@ inline void launch_varlen_paged(ComputeClient& client, const TensorHandle& q, co
   if (rc != B200_OK) client.defer(b200_last_error());
 }
 
+/// launch_varlen_paged against an fp8 cache: k_cache, v_cache F8E4M3 or F8E5M2 (one dtype) hold K = k_scale[hk] * k8 and
+/// V = v_scale[hk] * v8, with k_scale, v_scale compact f32 [Hkv] tensors.  See b200_attention_varlen_paged_fp8 in
+/// cubecl_b200.h.  Errors are deferred to client.sync().
+inline void launch_varlen_paged_fp8(ComputeClient& client, const TensorHandle& q, const TensorHandle& k_cache, const TensorHandle& v_cache,
+                                    const TensorHandle& cu_seqlens_q, const TensorHandle& cache_seqlens, const TensorHandle& k_scale,
+                                    const TensorHandle& v_scale, int32_t max_seqlen_q, int32_t max_seqlen_k, const TensorHandle& out,
+                                    const TensorHandle* block_table, float scale, int32_t window_left = -1, int32_t window_right = -1,
+                                    const TensorHandle* lse = nullptr) {
+  if (q.shape.size() != 3 || k_cache.shape.size() != 4 || v_cache.shape.size() != 4 || out.shape.size() != 3 ||
+      (block_table && block_table->shape.size() != 2) || k_cache.dtype != v_cache.dtype || cu_seqlens_q.shape.size() != 1 ||
+      cu_seqlens_q.shape[0] < 1 || cache_seqlens.shape.size() != 1 || cache_seqlens.shape[0] + 1 != cu_seqlens_q.shape[0]) {
+    client.defer("InvalidArgument: attention_varlen_paged_fp8 needs rank-3 q and out, rank-4 caches of one dtype, a rank-2 block "
+                 "table, cu_seqlens_q [B + 1] and cache_seqlens [B]");
+    return;
+  }
+  const b200_attention_varlen_args args{scale, window_left, window_right, max_seqlen_q, max_seqlen_k};
+  const int rc = b200_attention_varlen_paged_fp8(
+      client.raw(), nullptr, static_cast<b200_dtype>(q.dtype), static_cast<b200_dtype>(k_cache.dtype), static_cast<b200_dtype>(out.dtype),
+      q.handle.ptr(), q.shape.data(), q.strides.data(), k_cache.handle.ptr(), k_cache.shape.data(), k_cache.strides.data(),
+      v_cache.handle.ptr(), v_cache.shape.data(), v_cache.strides.data(), block_table ? block_table->handle.ptr() : 0,
+      block_table ? block_table->shape.data() : nullptr, block_table ? block_table->strides.data() : nullptr, cu_seqlens_q.handle.ptr(),
+      cache_seqlens.handle.ptr(), cu_seqlens_q.shape[0] - 1, k_scale.handle.ptr(), v_scale.handle.ptr(), out.handle.ptr(),
+      out.shape.data(), out.strides.data(), lse ? lse->handle.ptr() : 0, &args);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+
 /// Scatter of k_new, v_new [B, Snew, Hkv, D] into k_cache, v_cache [P, page, Hkv, D]: token n = b * Snew + t goes to flat slot
 /// slot_mapping[n] (compact i32; negative slots are skipped).  See b200_kvcache_write in cubecl_b200.h.  Errors are deferred to
 /// client.sync().

@@ -759,6 +759,41 @@ impl Context {
         ))
     }
 
+    /// [`Context::attention_varlen_paged`] against an fp8 cache: `k_cache`, `v_cache` in `cache_dtype` (F8E4M3 or F8E5M2) hold
+    /// K = k_scale[hk] * k8 and V = v_scale[hk] * v8, with `k_scale`, `v_scale` compact f32 [Hkv] device buffers.  See
+    /// b200_attention_varlen_paged_fp8 in cubecl_b200.h.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::attention_varlen_paged`]; `k_scale` and `v_scale` must hold Hkv f32 values.
+    pub unsafe fn attention_varlen_paged_fp8(
+        &mut self, stream: b200_stream, in_dtype: DType, cache_dtype: DType, out_dtype: DType, q: &TensorView, k_cache: &TensorView,
+        v_cache: &TensorView, block_table: Option<&TensorView>, cu_seqlens_q: b200_dptr, cache_seqlens: b200_dptr, batch: u64,
+        k_scale: b200_dptr, v_scale: b200_dptr, max_seqlen: (i32, i32), out: &TensorView, lse: b200_dptr, scale: f32, window: (i32, i32),
+    ) -> Result<(), Error> {
+        for t in [q, out] {
+            assert!(t.shape.len() == 3 && t.strides.len() == 3);
+        }
+        for t in [k_cache, v_cache] {
+            assert!(t.shape.len() == 4 && t.strides.len() == 4);
+        }
+        if let Some(t) = block_table {
+            assert!(t.shape.len() == 2 && t.strides.len() == 2);
+        }
+        let a = sys::b200_attention_varlen_args {
+            scale, window_left: window.0, window_right: window.1, max_seqlen_q: max_seqlen.0, max_seqlen_k: max_seqlen.1,
+        };
+        let (bt, bt_shape, bt_strides) = match block_table {
+            Some(t) => (t.ptr, t.shape.as_ptr(), t.strides.as_ptr()),
+            None => (0, std::ptr::null(), std::ptr::null()),
+        };
+        check(sys::b200_attention_varlen_paged_fp8(
+            self.0, stream, in_dtype as c_int, cache_dtype as c_int, out_dtype as c_int, q.ptr, q.shape.as_ptr(), q.strides.as_ptr(),
+            k_cache.ptr, k_cache.shape.as_ptr(), k_cache.strides.as_ptr(), v_cache.ptr, v_cache.shape.as_ptr(), v_cache.strides.as_ptr(),
+            bt, bt_shape, bt_strides, cu_seqlens_q, cache_seqlens, batch, k_scale, v_scale, out.ptr, out.shape.as_ptr(),
+            out.strides.as_ptr(), lse, &a,
+        ))
+    }
+
     /// Grouped / depthwise [`Context::conv2d`]: w [Cout, KH, KW, C / groups].  See b200_conv2d_grouped in cubecl_b200.h.
     ///
     /// # Safety
