@@ -128,6 +128,8 @@ SIGNATURES = {
                                     _u64p, _u64p, _u64p, _u64p, _u64p, _u64p, C.POINTER(Epilogue)]),
     "b200_matmul_scaled": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64,
                                      C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64, C.c_int, C.c_int]),
+    "b200_matmul_grouped": (C.c_int, [_vp, _vp, C.c_int, C.c_int] + [C.c_uint64, C.c_int, _u64p, _u64p] * 2
+                            + [C.c_uint64, C.c_uint64] + [C.c_uint64, C.c_int, _u64p, _u64p] + [C.POINTER(Epilogue)]),
     "b200_matmul_quantized": (C.c_int, [_vp, _vp, C.POINTER(QuantOperand), C.POINTER(QuantOperand), C.c_int, C.c_uint64,
                                         C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64]),
     "b200_conv2d": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, _u64p, _u64p, C.c_uint64, _u64p, _u64p, C.c_uint64, _u64p,

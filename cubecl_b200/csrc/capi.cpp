@@ -73,6 +73,8 @@ extern const unsigned char b200_cubin_attention_paged[];
 extern const unsigned char b200_cubin_attention_paged_end[];
 extern const unsigned char b200_cubin_attention_paged_fp8[];
 extern const unsigned char b200_cubin_attention_paged_fp8_end[];
+extern const unsigned char b200_cubin_gemm_grouped[];
+extern const unsigned char b200_cubin_gemm_grouped_end[];
 }
 
 // ================================================================================================ errors
@@ -345,12 +347,13 @@ static int get_func(b200_ctx* c, const std::string& name, CUfunction* out) {
   if (it != c->funcs.end()) { *out = it->second; return B200_OK; }
   // modules are loaded in the order gemm, reduce, aux, gemm_b, gemm_c, quant, gemm_q, quant_mm, gemm_conv, gemm_convbwd,
   // conv_grouped, gemm_conv3d, gemm_convt, attention, attention_bwd, attention_kv, attention_varlen, attention_varlen_bwd,
-  // attention_kv_fp8, attention_paged, attention_paged_fp8; the kernel name says where a
+  // attention_kv_fp8, attention_paged, attention_paged_fp8, gemm_grouped; the kernel name says where a
   // kernel lives (no failing lookups, which API-level tools such as compute-sanitizer would report)
   auto starts = [&](const char* pfx) { return name.rfind(pfx, 0) == 0; };
   auto has = [&](const char* part) { return name.find(part) != std::string::npos; };
   const bool tc_gemm = starts("gemm_") && name != "gemm_simt_strided" && name != "gemm_scaled_simt";
   const size_t home = name == "conv3d_dgrad_weights" ? 2
+                      : starts("gemm_grouped_") ? 21
                       : starts("attn_fwd_paged_") && (has("_e4m3_") || has("_e5m2_")) ? 20
                       : starts("attn_fwd_paged_") ? 19
                       : starts("attn_kv_") && (has("_e4m3_") || has("_e5m2_") || has("_fp8")) ? 18
@@ -406,7 +409,8 @@ extern "C" int b200_get_cubin(const char* name, const void** image, size_t* size
   else if (!strcmp(name, "attention_kv_fp8")) { b = b200_cubin_attention_kv_fp8; e = b200_cubin_attention_kv_fp8_end; }
   else if (!strcmp(name, "attention_paged")) { b = b200_cubin_attention_paged; e = b200_cubin_attention_paged_end; }
   else if (!strcmp(name, "attention_paged_fp8")) { b = b200_cubin_attention_paged_fp8; e = b200_cubin_attention_paged_fp8_end; }
-  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd|conv_grouped|gemm_conv3d|gemm_convt|attention|attention_bwd|attention_kv|attention_varlen|attention_varlen_bwd|attention_kv_fp8|attention_paged|attention_paged_fp8)", name);
+  else if (!strcmp(name, "gemm_grouped")) { b = b200_cubin_gemm_grouped; e = b200_cubin_gemm_grouped_end; }
+  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd|conv_grouped|gemm_conv3d|gemm_convt|attention|attention_bwd|attention_kv|attention_varlen|attention_varlen_bwd|attention_kv_fp8|attention_paged|attention_paged_fp8|gemm_grouped)", name);
   *image = b;
   *size = static_cast<size_t>(e - b);
   return B200_OK;
@@ -474,7 +478,8 @@ extern "C" int b200_init(int device, b200_ctx** out) {
       (rc = load_module(c, b200_cubin_attention_varlen_bwd, b200_cubin_attention_varlen_bwd_end, "attention_varlen_bwd")) ||
       (rc = load_module(c, b200_cubin_attention_kv_fp8, b200_cubin_attention_kv_fp8_end, "attention_kv_fp8")) ||
       (rc = load_module(c, b200_cubin_attention_paged, b200_cubin_attention_paged_end, "attention_paged")) ||
-      (rc = load_module(c, b200_cubin_attention_paged_fp8, b200_cubin_attention_paged_fp8_end, "attention_paged_fp8"))) {
+      (rc = load_module(c, b200_cubin_attention_paged_fp8, b200_cubin_attention_paged_fp8_end, "attention_paged_fp8")) ||
+      (rc = load_module(c, b200_cubin_gemm_grouped, b200_cubin_gemm_grouped_end, "gemm_grouped"))) {
     for (CUmodule m : c->modules) g_drv.cuModuleUnload_p(m);
     g_drv.cuDevicePrimaryCtxRelease_p(c->dev);
     return bail(rc);
@@ -1835,6 +1840,252 @@ static int matmul_impl(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dty
   for (int i = 0; i < nb; ++i)
     if (shape_out[i] == 0) return B200_OK;
   return matmul_rec(c, st, g, nb, shape_out, shape_lhs, strides_lhs, shape_rhs, strides_rhs, strides_out);
+}
+
+// ------------------------------------------------------------------------------------------------ grouped matmul
+// b200_matmul_grouped: one launch of a gemm_grouped_* kernel (GroupedParams, kernel_params.h).  The offsets stay on the
+// device: the grid is sized from an upper bound on the tiles, and the kernel skips the units past its own count.
+
+// The tile from the rows per group: the 256-row pair tile reads B from L2 once per pair but wastes twice the rows at each
+// group's end (on average 128 against 64).  Under the variants' assumed efficiencies (0.9 and 0.85, kVariants) the two
+// break even at 1024 rows per group: fewer take 1sm_n128.  Ragged K with M <= 128 would idle half of a pair: 1sm_n128.
+constexpr uint64_t kGroupedPairRowsPerGroup = 1024;
+static const GemmVariant* grouped_variant(b200_ctx* c, bool ragged_k, uint64_t T, uint64_t G, uint64_t M) {
+  const std::string forced = opt(c, "gemm.variant", "auto");
+  std::string tag = forced;
+  if (forced == "auto") tag = (T >= kGroupedPairRowsPerGroup * G && (!ragged_k || M > 128)) ? "2sm_n128" : "1sm_n128";
+  if (tag != "2sm_n128" && tag != "1sm_n128") return nullptr;
+  for (const GemmVariant& v : kVariants)
+    if (tag == v.tag) return &v;
+  return nullptr;
+}
+
+// Can TMA read an MN-major operand (mn contiguous, rows of K) in place?  Strides in elements.
+static bool mn_major_tma_ok(uint64_t ptr, size_t esz, uint64_t mn, uint64_t K, uint64_t s_mn, uint64_t s_k) {
+  return ptr % 16 == 0 && (s_mn == 1 || mn == 1) && (K == 1 || ((s_k * esz) % 16 == 0 && s_k >= mn)) && s_k * esz < (1ull << 40);
+}
+
+extern "C" int b200_matmul_grouped(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr lhs, int lhs_rank,
+                                   const uint64_t* lhs_shape, const uint64_t* lhs_strides, b200_dptr rhs, int rhs_rank,
+                                   const uint64_t* rhs_shape, const uint64_t* rhs_strides, b200_dptr offs, uint64_t groups, b200_dptr out,
+                                   int out_rank, const uint64_t* out_shape, const uint64_t* out_strides, const b200_epilogue* ep) {
+  CTX_ENTER(c);
+  typedef unsigned long long ull;
+  if (!lhs_shape || !rhs_shape || !out_shape) return fail(B200_ERR_INVALID_ARG, "matmul_grouped: null shape array");
+  if (lhs_rank == 3 && rhs_rank == 3)
+    return fail(B200_ERR_UNSUPPORTED, "matmul_grouped: 3-D x 3-D is a batched matmul without offsets: use b200_matmul");
+  if (lhs_rank == 3 && rhs_rank == 2) return fail(B200_ERR_UNSUPPORTED, "matmul_grouped: 3-D x 2-D (ragged N) is not supported");
+  const bool rk = (lhs_rank == 2 && rhs_rank == 2);
+  if (lhs_rank != 2 || (rhs_rank != 2 && rhs_rank != 3) || out_rank != (rk ? 3 : 2))
+    return fail(B200_ERR_INVALID_ARG, "matmul_grouped: ranks lhs %d, rhs %d, out %d (need 2 x 3 -> 2, ragged M, or 2 x 2 -> 3, ragged K)",
+                lhs_rank, rhs_rank, out_rank);
+  if (in_dtype != B200_BF16 && in_dtype != B200_F16)
+    return fail(B200_ERR_UNSUPPORTED, "matmul_grouped: input dtype %d unsupported (bf16, f16)", (int)in_dtype);
+  if (out_dtype != in_dtype && out_dtype != B200_F32)
+    return fail(B200_ERR_UNSUPPORTED, "matmul_grouped: output dtype must equal the input dtype or be f32");
+  // strides in elements; NULL = compact row-major
+  uint64_t lst[2], rst[3], ost[3];
+  auto strides_of = [](int rank, const uint64_t* shape, const uint64_t* st, uint64_t* o) {
+    uint64_t acc = 1;
+    for (int i = rank - 1; i >= 0; --i) { o[i] = st ? st[i] : acc; acc *= shape[i]; }
+  };
+  strides_of(2, lhs_shape, lhs_strides, lst);
+  strides_of(rhs_rank, rhs_shape, rhs_strides, rst);
+  strides_of(out_rank, out_shape, out_strides, ost);
+  uint64_t T, M, N, K;
+  if (!rk) {   // lhs [T, K] x rhs [G, K, N] -> out [T, N]
+    T = lhs_shape[0]; K = lhs_shape[1]; N = rhs_shape[2]; M = T;
+    if (rhs_shape[1] != K)
+      return fail(B200_ERR_INVALID_ARG, "matmul_grouped: inner dimensions differ (lhs k=%llu, rhs k=%llu)", (ull)K, (ull)rhs_shape[1]);
+    if (rhs_shape[0] != groups)
+      return fail(B200_ERR_INVALID_ARG, "matmul_grouped: %llu groups in offs, but rhs has %llu (shape[0])", (ull)groups, (ull)rhs_shape[0]);
+    if (out_shape[0] != T || out_shape[1] != N)
+      return fail(B200_ERR_INVALID_ARG, "matmul_grouped: output is [%llu,%llu], expected [%llu,%llu]", (ull)out_shape[0], (ull)out_shape[1],
+                  (ull)T, (ull)N);
+  } else {     // lhs [M, T] x rhs [T, N] -> out [G, M, N]
+    M = lhs_shape[0]; T = lhs_shape[1]; N = rhs_shape[1]; K = T;
+    if (rhs_shape[0] != T)
+      return fail(B200_ERR_INVALID_ARG, "matmul_grouped: inner dimensions differ (lhs k=%llu, rhs k=%llu)", (ull)T, (ull)rhs_shape[0]);
+    if (out_shape[0] != groups)
+      return fail(B200_ERR_INVALID_ARG, "matmul_grouped: %llu groups in offs, but out has %llu (shape[0])", (ull)groups, (ull)out_shape[0]);
+    if (out_shape[1] != M || out_shape[2] != N)
+      return fail(B200_ERR_INVALID_ARG, "matmul_grouped: output is [%llu,%llu,%llu], expected [%llu,%llu,%llu]", (ull)out_shape[0],
+                  (ull)out_shape[1], (ull)out_shape[2], (ull)groups, (ull)M, (ull)N);
+  }
+  if (ep && rk) return fail(B200_ERR_UNSUPPORTED, "matmul_grouped: the ragged-K mode (weight gradient) takes no epilogue");
+  if (ep && (ep->activation < 0 || ep->activation > 2))
+    return fail(B200_ERR_INVALID_ARG, "matmul_grouped: unknown activation %d", ep->activation);
+  if (groups > (uint64_t)kGroupedMaxGroups)
+    return fail(B200_ERR_UNSUPPORTED, "matmul_grouped: %llu groups exceed the limit of %d", (ull)groups, kGroupedMaxGroups);
+  if (T >= (1ull << 31) || M >= (1ull << 31) || N >= (1ull << 31) || K >= (1ull << 31))
+    return fail(B200_ERR_UNSUPPORTED, "matmul_grouped: extents must be below 2^31");
+  if (groups == 0 || M == 0 || N == 0) return B200_OK;   // nothing is written (ragged M: no row lies in a group)
+  const size_t esz = 2, osz = dtype_size(out_dtype);
+  if (!offs) return fail(B200_ERR_INVALID_ARG, "matmul_grouped: null offs");
+  if (offs % 4) return fail(B200_ERR_INVALID_ARG, "matmul_grouped: offs is misaligned (a compact i32 [groups] array)");
+  const bool reads = (rk ? T : K) != 0;   // without k-blocks no operand is read
+  if (!out || (reads && (!lhs || !rhs))) return fail(B200_ERR_INVALID_ARG, "matmul_grouped: null device pointer");
+  if (lhs % esz || rhs % esz || out % osz) return fail(B200_ERR_INVALID_ARG, "matmul_grouped: misaligned lhs, rhs or out");
+  if (ep && ep->bias % 4) return fail(B200_ERR_INVALID_ARG, "matmul_grouped: misaligned bias (f32 [groups, N])");
+  // out: one unit column stride, stored in place (outputs are never gathered)
+  const uint64_t o_sm = ost[rk ? 1 : 0], o_sb = rk ? ost[0] : 0;
+  if (ost[rk ? 2 : 1] != 1 && N != 1) return fail(B200_ERR_UNSUPPORTED, "matmul_grouped: out needs a unit column stride");
+  if (o_sm * osz >= (1ull << 40) || o_sb * osz >= (1ull << 40)) return fail(B200_ERR_UNSUPPORTED, "matmul_grouped: out strides too large");
+
+  // operands: read in place where TMA can describe them, else staged once into an aligned pooled copy
+  uint64_t a = lhs, b = rhs;
+  uint64_t a_mn_s, a_k_s, b_mn_s, b_k_s, b_sb = 0;
+  bool a_mn = false, b_mn = false;
+  if (!rk) {
+    a_mn_s = lst[0]; a_k_s = lst[1];
+    b_mn_s = rst[2]; b_k_s = rst[1]; b_sb = groups > 1 ? rst[0] : 0;
+  } else {
+    a_mn_s = lst[0]; a_k_s = lst[1];
+    b_mn_s = rst[1]; b_k_s = rst[0];
+    if ((a_mn_s != 1 && M != 1) || (b_mn_s != 1 && N != 1))
+      return fail(B200_ERR_UNSUPPORTED, "matmul_grouped: the ragged-K mode reads an M-contiguous lhs [M, T] (x.t() of x [T, M]) and an "
+                                        "N-contiguous rhs [T, N]; K-major operands are not supported");
+    a_mn = b_mn = true;
+  }
+  CUstream st = resolve_stream(c, s);
+  CUdeviceptr sa = 0, sb = 0;
+  auto release = [&](int rc) {
+    if (sa) pool_free(c, sa, st);
+    if (sb) pool_free(c, sb, st);
+    return rc;
+  };
+  int rc = B200_OK;
+  if (reads) {
+    uint64_t o_sb_unused = 0;
+    if (!rk) {
+      if (!operand_tma_ok(a, esz, T, K, a_mn_s, a_k_s, 0, &a_mn)) {
+        if ((rc = stage_operand(c, st, esz, a, 1, T, K, a_mn_s, a_k_s, 0, &sa, &a_mn_s, &a_k_s, &o_sb_unused))) return release(rc);
+        a = sa;
+        if (!operand_tma_ok(a, esz, T, K, a_mn_s, a_k_s, 0, &a_mn)) return release(fail(B200_ERR_UNSUPPORTED, "matmul_grouped: lhs cannot be staged"));
+      }
+      if (!operand_tma_ok(b, esz, N, K, b_mn_s, b_k_s, b_sb, &b_mn)) {
+        if ((rc = stage_operand(c, st, esz, b, groups, N, K, b_mn_s, b_k_s, b_sb, &sb, &b_mn_s, &b_k_s, &b_sb))) return release(rc);
+        b = sb;
+        if (!operand_tma_ok(b, esz, N, K, b_mn_s, b_k_s, b_sb, &b_mn)) return release(fail(B200_ERR_UNSUPPORTED, "matmul_grouped: rhs cannot be staged"));
+      }
+    } else {
+      if (!mn_major_tma_ok(a, esz, M, T, a_mn_s, a_k_s)) {
+        if ((rc = stage_operand(c, st, esz, a, 1, M, T, 1, a_k_s, 0, &sa, &a_mn_s, &a_k_s, &o_sb_unused))) return release(rc);
+        a = sa;
+        if (!mn_major_tma_ok(a, esz, M, T, a_mn_s, a_k_s))
+          return release(fail(B200_ERR_UNSUPPORTED, "matmul_grouped: lhs cannot be staged M-contiguous"));
+      }
+      if (!mn_major_tma_ok(b, esz, N, T, b_mn_s, b_k_s)) {
+        if ((rc = stage_operand(c, st, esz, b, 1, N, T, 1, b_k_s, 0, &sb, &b_mn_s, &b_k_s, &o_sb_unused))) return release(rc);
+        b = sb;
+        if (!mn_major_tma_ok(b, esz, N, T, b_mn_s, b_k_s))
+          return release(fail(B200_ERR_UNSUPPORTED, "matmul_grouped: rhs cannot be staged N-contiguous"));
+      }
+    }
+  }
+
+  const GemmVariant* vp = grouped_variant(c, rk, T, groups, M);
+  if (!vp)
+    return release(fail(B200_ERR_INVALID_ARG, "gemm.variant '%s' is not a grouped matmul tile (2sm_n128, 1sm_n128)",
+                        opt(c, "gemm.variant", "auto").c_str()));
+  const GemmVariant& v = *vp;
+  const std::string epi = opt(c, "gemm.epilogue", "tma");
+  if (epi != "tma" && epi != "direct") return release(fail(B200_ERR_INVALID_ARG, "gemm.epilogue must be tma or direct"));
+  // the grid's bound on the tiles: every group may add one partial tile-row (ragged M; with an M-contiguous lhs a group's
+  // tile-rows start up to 63 rows early, GroupedParams); G whole grids (ragged K)
+  const uint64_t rows = 128ull * v.cg, tiles_n = (N + v.block_n - 1) / v.block_n, tiles_m = (M + rows - 1) / rows;
+  const uint64_t span = T + (a_mn && !rk ? 63 * groups : 0);
+  const uint64_t tile_rows = rk ? groups * tiles_m : (span + rows - 1) / rows + groups, bound = tile_rows * tiles_n;
+  if (bound >= (1ull << 32)) return release(fail(B200_ERR_UNSUPPORTED, "matmul_grouped: too many tiles (bound %llu)", (ull)bound));
+  const char* in_tag = in_dtype == B200_BF16 ? "bf16" : "f16";
+  const char* out_tag = out_dtype == B200_F32 ? "f32" : in_tag;
+  const std::string name = std::string(rk ? "gemm_grouped_k_" : "gemm_grouped_m_") + in_tag + "_" + out_tag + "_" + v.tag +
+                           (rk ? "" : std::string("_") + (a_mn ? "m" : "k") + (b_mn ? "n" : "k"));
+  if (c->dry) {
+    char line[200];
+    snprintf(line, sizeof(line), "gemm grouped %s groups=%llu T=%llu tile_rows<=%llu tiles<=%llu\n", rk ? "ragged_k" : "ragged_m",
+             (ull)groups, (ull)T, (ull)tile_rows, (ull)bound);
+    c->plan += line;
+  }
+  CUfunction f;
+  if ((rc = get_func(c, name, &f))) return release(rc);
+  const unsigned smem = gemm_smem_bytes(v) + kGroupedTableBytes;
+  if (!c->dry) {
+    CUresult r = g_drv.cuFuncSetAttribute_p(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem);
+    if (r != CUDA_SUCCESS) return release(fail(map_cu(r), "cuFuncSetAttribute: %s", cu_err(r)));
+  }
+
+  const CUtensorMapDataType dt = in_dtype == B200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  auto pad8 = [](uint64_t e) { return (e + 7) / 8 * 8; };
+  const uint32_t n_local = (uint32_t)(v.block_n / v.cg);
+  const uint64_t gb = b_sb != 0 ? groups : 1;   // a broadcast rhs (batch stride 0) is one map batch
+  CUtensorMap ta, tb, tout;
+  memset(&ta, 0, sizeof(ta));
+  memset(&tb, 0, sizeof(tb));
+  memset(&tout, 0, sizeof(tout));
+  if (reads && !rk) {
+    // lhs [T, K]: K-major rows of 128 B x 128 rows, or MN-major [64 rows x 64 K] chunks
+    if (!a_mn) {
+      const uint64_t s = T > 1 ? a_mn_s : pad8(K);
+      rc = encode_tmap(c, &ta, dt, esz, a, K, T, 1, s, s * T, 64, 128);
+    } else {
+      const uint64_t s = K > 1 ? a_k_s : pad8(T);
+      rc = encode_tmap(c, &ta, dt, esz, a, T, K, 1, s, s * K, 64, 64);
+    }
+    // rhs [G, K, N] with the group as the batch: [n_local x 64 K] K-major boxes or [64 N x 64 K] MN-major chunks
+    if (!rc && !b_mn) {
+      const uint64_t s = N > 1 ? b_mn_s : pad8(K);
+      rc = encode_tmap(c, &tb, dt, esz, b, K, N, gb, s, gb > 1 ? b_sb : s * N, 64, n_local);
+    } else if (!rc) {
+      const uint64_t s = K > 1 ? b_k_s : pad8(N);
+      rc = encode_tmap(c, &tb, dt, esz, b, N, K, gb, s, gb > 1 ? b_sb : s * K, 64, 64);
+    }
+  } else if (reads) {
+    // lhs [M, T] and rhs [T, N], both MN-major: [64 rows x 64 positions] chunks
+    const uint64_t sa_k = T > 1 ? a_k_s : pad8(M), sb_k = T > 1 ? b_k_s : pad8(N);
+    rc = encode_tmap(c, &ta, dt, esz, a, M, T, 1, sa_k, sa_k * T, 64, 64);
+    if (!rc) rc = encode_tmap(c, &tb, dt, esz, b, N, T, 1, sb_k, sb_k * T, 64, 64);
+  }
+  if (rc) return release(rc);
+
+  GemmParams p;
+  memset(&p, 0, sizeof(p));
+  p.out = out;
+  p.out_row_stride = o_sm;
+  p.out_batch_stride = o_sb;
+  p.M = (uint32_t)M; p.N = (uint32_t)N; p.K = (uint32_t)K; p.batch = rk ? (uint32_t)groups : 1u;
+  p.tiles_m = (uint32_t)(rk ? tiles_m : tile_rows);
+  p.tiles_n = (uint32_t)tiles_n;
+  p.group_m = (uint32_t)std::max(1, atoi(opt(c, "gemm.group_m", "8").c_str()));
+  p.a_bmul = 0;
+  p.b_bmul = (!rk && gb > 1) ? 1u : 0u;
+  p.k_segments = 1;
+  if (ep) { p.alpha = ep->alpha; p.bias = ep->bias; p.epi_act = (uint32_t)ep->activation; }
+  else p.alpha = 1.0f;
+  p.epi_on = (p.alpha != 1.0f || p.bias != 0 || p.epi_act != 0) ? 1u : 0u;
+  p.vec_store = (out % 16 == 0 && (o_sm * osz) % 16 == 0 && (o_sb * osz) % 16 == 0) ? 1u : 0u;
+  p.full_tiles = (uint32_t)bound;   // whole tiles only: no stream-K head (the host does not know the tile count)
+  // whole CTA tiles leave through swizzled staging and TMA stores when out is describable: (N, rows, G) in [128 B x 64 rows]
+  // boxes; ragged M's tiles that a group's end cuts store directly
+  const uint64_t o_rows = rk ? M : T, o_b = rk ? groups : 1;
+  if (p.vec_store && epi == "tma" && (o_rows == 1 || o_sm >= N)) {
+    const uint64_t os = o_rows > 1 ? o_sm : (N + 15) / 16 * 16;
+    rc = encode_tmap(c, &tout, osz == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_UINT16, osz, out, N, o_rows, o_b, os,
+                     o_b > 1 ? o_sb : os * o_rows, (uint32_t)(128 / osz), 64);
+    if (rc) return release(rc);
+    p.tma_store = 1;
+  }
+  GroupedParams gp;
+  memset(&gp, 0, sizeof(gp));
+  gp.offs = offs;
+  gp.bias_stride = N;
+  gp.groups = (uint32_t)groups;
+  gp.T = (uint32_t)T;
+  gp.mode = rk ? 1u : 0u;
+  const unsigned clusters = (unsigned)std::min<uint64_t>(bound, (uint64_t)std::max(1, c->props.num_sms / v.cg));
+  void* args[] = {&ta, &tb, &tout, &gp, &p};
+  rc = launch(c, f, clusters * v.cg, 1, 1, 384, smem, v.cg, st, args);
+  return release(rc);   // stream-ordered: staged copies are reused only by later work
 }
 
 // ================================================================================================ reduce

@@ -160,7 +160,14 @@ enum : int { QM_NONE = 0, QM_BLOCK = 1, QM_TENSOR = 2 };
 //             the producer finds the tile's phase and loads through that phase's im2col and weight maps; the consumers run
 //             the phase's own k-block count from zeroed accumulators (a phase no tap reaches runs none and stores
 //             act(bias)), then store as CB_DGRAD at the phase's rows.
-enum : int { CB_NONE = 0, CB_DGRAD = 1, CB_WGRAD = 2, CB_TCONV = 3 };
+//   CB_GRP_M  grouped matmul, ragged M (GroupedParams, kernel_params.h): each CTA reads the group offsets once into a table
+//             in shared memory and maps every tile to (group, m-block, n-block) from it; A rows start at the group's first
+//             row, B is the group's batch of the 3-D rhs map.  A tile that the group's end cuts leaves through direct
+//             stores of the group's rows only.
+//   CB_GRP_K  grouped matmul, ragged K (the weight gradient; MN-major operands as CB_WGRAD): tile t belongs to group
+//             t / (tiles_m * tiles_n) and runs that group's k-blocks from its first position; in the last one the rows of
+//             positions past the group are zeroed in shared memory before the MMAs.  A group without k-blocks stores +0.
+enum : int { CB_NONE = 0, CB_DGRAD = 1, CB_WGRAD = 2, CB_TCONV = 3, CB_GRP_M = 4, CB_GRP_K = 5 };
 
 // phase of tile t in a transposed-convolution launch (phases in table order, tiles in one list)
 __device__ __forceinline__ uint32_t tconv_phase(uint32_t t, const TconvParams& tp) {
@@ -185,12 +192,118 @@ __device__ __forceinline__ TileCoord unit_coord(uint32_t t, const GemmParams& p,
   else return tile_coord(t, p);
 }
 
+// Grouped matmul: the shared-memory table of one CTA (GroupedParams), built by one warp.  Lane l takes groups
+// [l S, (l + 1) S), S = ceil(G / 32): a running maximum of offs (o_{-1} = 0) clamped to T gives the ends o[g], and a
+// prefix sum of the groups' tile-rows of `rows` rows gives pre[g] (pre[G] = all of them).  A non-empty group's tile-rows
+// start at its first row rounded down to a multiple of mask + 1.
+__device__ __forceinline__ void grp_tables(const GroupedParams& gp, uint32_t* o, uint32_t* pre, uint32_t rows, uint32_t mask,
+                                           uint32_t lane) {
+  const uint32_t G = gp.groups, S = (G + 31u) / 32u, b = min(lane * S, G), e = min(b + S, G);
+  const int32_t* offs = reinterpret_cast<const int32_t*>(gp.offs);
+  int32_t mx = 0;
+  for (uint32_t i = b; i < e; ++i) {
+    const int32_t v = __ldg(offs + i);
+    o[i] = static_cast<uint32_t>(v);
+    mx = max(mx, v);
+  }
+  int32_t run = mx;   // inclusive running maximum over the lanes
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const int32_t y = __shfl_up_sync(0xFFFFFFFFu, run, d);
+    if (static_cast<int>(lane) >= d) run = max(run, y);
+  }
+  int32_t m = __shfl_up_sync(0xFFFFFFFFu, run, 1);
+  if (lane == 0) m = 0;
+  uint32_t prev = min(static_cast<uint32_t>(m), gp.T), cnt = 0;
+  for (uint32_t i = b; i < e; ++i) {
+    m = max(m, static_cast<int32_t>(o[i]));
+    const uint32_t end = min(static_cast<uint32_t>(m), gp.T), tr = end > prev ? (end - (prev & ~mask) + rows - 1u) / rows : 0u;
+    o[i] = end;
+    pre[i] = tr;
+    cnt += tr;
+    prev = end;
+  }
+  uint32_t sum = cnt;   // inclusive prefix sum over the lanes
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, sum, d);
+    if (static_cast<int>(lane) >= d) sum += y;
+  }
+  uint32_t acc = sum - cnt;
+  for (uint32_t i = b; i < e; ++i) {
+    const uint32_t tr = pre[i];
+    pre[i] = acc;
+    acc += tr;
+  }
+  if (lane == 31) pre[G] = sum;
+}
+
+struct GrpUnit {
+  TileCoord tc;       // b = the group
+  uint32_t g;
+  uint32_t lo, hi;    // the group's rows (ragged M) or positions (ragged K): [o_{g-1}, o_g)
+  uint32_t row0;      // ragged M: first row of the group's tile-rows (lo rounded down to a multiple of MASK + 1)
+  uint32_t nkb;       // k-blocks of the tile
+};
+// tile t of a grouped launch: its group (ragged M: the last g with pre[g] <= t / tiles_n, by bisection), and its coordinate
+// inside the group's grid of tile-rows x tiles_n in group_m strips
+template <int CB, uint32_t MASK>
+__device__ __forceinline__ GrpUnit grp_unit(uint32_t t, const GemmParams& p, const GroupedParams& gp, const uint32_t* o, const uint32_t* pre) {
+  uint32_t g, loc, tiles_m;
+  if constexpr (CB == CB_GRP_M) {
+    const uint32_t q = t / p.tiles_n;
+    uint32_t lo = 0, hi = gp.groups;
+    while (hi - lo > 1u) {
+      const uint32_t mid = (lo + hi) >> 1;
+      if (pre[mid] <= q) lo = mid; else hi = mid;
+    }
+    g = lo;
+    loc = t - pre[g] * p.tiles_n;
+    tiles_m = pre[g + 1] - pre[g];
+  } else {
+    const uint32_t per = p.tiles_m * p.tiles_n;
+    g = t / per;
+    loc = t - g * per;
+    tiles_m = p.tiles_m;
+  }
+  GrpUnit u;
+  u.tc = tconv_coord(loc, tiles_m, p);
+  u.tc.b = g;
+  u.g = g;
+  u.lo = g ? o[g - 1] : 0u;
+  u.hi = o[g];
+  u.row0 = u.lo & ~MASK;
+  u.nkb = (CB == CB_GRP_M) ? (p.K + 63u) / 64u : (u.hi - u.lo + 63u) / 64u;
+  return u;
+}
+
+// Ragged K, the last k-block of a group: rows of positions >= o_g (the next group's, or zeros past T) are cleared in the four
+// [64 positions x 128 B] MN-major chunks of the stage (A's two, then B's two) -- 0 * NaN is NaN inside an MMA.  A position is
+// one whole 128-byte row of a chunk whatever the swizzle.  Both consumer warpgroups (thread ct of 256), then one barrier.
+__device__ __forceinline__ void grp_zero_rows(uint32_t stage, uint32_t keep, uint32_t ct) {
+  const uint32_t per = (64u - keep) * 8u;   // 16-byte units per chunk
+  for (uint32_t u = ct; u < 4u * per; u += 256u) {
+    const uint32_t c = u / per, r = u - c * per;
+    asm volatile("st.shared.v4.b32 [%0], {%1, %1, %1, %1};" ::"r"(stage + c * 8192u + keep * 128u + r * 16u), "r"(0u) : "memory");
+  }
+  fence_proxy_async_smem();   // generic-proxy writes -> visible to wgmma's async-proxy reads
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+}
+
 template <int CG, int BLOCK_N, bool A_MN, bool B_MN, int KIND, int OUT, int STAGES, bool PROMOTE = false, int MT = 1, int QM = QM_NONE,
           bool CONV = false, int CB = CB_NONE, int CONV_DIMS = 2>
 __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUtensorMap* tma_b_hi, const CUtensorMap* tma_a_lo,
                                           const CUtensorMap* tma_b_lo, const CUtensorMap* tma_out, const GemmParams& p,
-                                          const TconvParams* tcp = nullptr) {
+                                          const TconvParams* tcp = nullptr, const GroupedParams* gpp = nullptr) {
   constexpr bool INT_ACC = (KIND == KIND_U8 || KIND == KIND_S8) && QM != QM_BLOCK;
+  constexpr bool GRP = (CB == CB_GRP_M || CB == CB_GRP_K);
+  static_assert(!GRP || (!CONV && (KIND == KIND_BF16 || KIND == KIND_F16) && !PROMOTE && MT == 1 && QM == QM_NONE && CONV_DIMS == 2),
+                "grouped matmul: 16-bit kinds, one M sub-tile");
+  static_assert(CB != CB_GRP_K || (A_MN && B_MN), "ragged K: MN-major operands");
+  // ragged M with an M-contiguous lhs: the group's first row is the innermost coordinate of the A loads, and such loads at
+  // coordinates that are not a multiple of 16 bytes faulted (illegal instruction) on an H100 -- the group's tile-rows start
+  // at a multiple of 64 rows instead, and the rows before the group are not stored
+  constexpr uint32_t GRP_MASK = (CB == CB_GRP_M && A_MN) ? 63u : 0u;
   static_assert(QM == QM_NONE || (KIND == KIND_S8 && !A_MN && !B_MN && !PROMOTE && MT == 1), "quantized operands: s8, K-major");
   static_assert(!CONV || ((KIND == KIND_BF16 || KIND == KIND_F16) && !A_MN && !B_MN && !PROMOTE && MT == 1 && QM == QM_NONE),
                 "convolution: 16-bit kinds, K-major operands");
@@ -237,8 +350,12 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
   const uint32_t cluster_id = (CG == 2) ? cluster_id_x() : blockIdx.x;
   const uint32_t n_clusters = (CG == 2) ? num_clusters_x() : gridDim.x;
 
+  // grouped matmul: the offset table after the TMA-store staging (GroupedParams)
+  uint32_t* const grp_o = reinterpret_cast<uint32_t*>(smem_raw + (epi_base + 16384u - smem_u32(smem_raw)));
+  uint32_t* const grp_pre = grp_o + kGroupedMaxGroups;
   if (threadIdx.x == 0) {
-    if (CB != CB_TCONV || tcp->ph[0].num_kb != 0) {   // a transposed-convolution phase without taps has no maps
+    // a transposed-convolution phase without taps has no maps, nor has a grouped launch without k-blocks
+    if ((CB != CB_TCONV || tcp->ph[0].num_kb != 0) && (!GRP || p.K != 0)) {
       tma_prefetch_desc(tma_a_hi);
       tma_prefetch_desc(tma_b_hi);
     }
@@ -251,7 +368,14 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
     }
     fence_mbar_init();
   }
+  if constexpr (GRP) {
+    if (threadIdx.x < 32) grp_tables(*gpp, grp_o, grp_pre, 128u * CG, GRP_MASK, threadIdx.x);
+  }
   if constexpr (CG == 2) cluster_sync_all(); else __syncthreads();
+  // grouped matmul: units past the device's tile count are skipped by every role alike
+  uint32_t grp_total = 0;
+  if constexpr (CB == CB_GRP_M) grp_total = grp_pre[gpp->groups] * p.tiles_n;
+  else if constexpr (CB == CB_GRP_K) grp_total = p.full_tiles;
 
   // 3xTF32: x = hi + lo with hi = the top 19 bits of x (exactly what the tf32 datapath reads from an f32 operand, so the
   // ORIGINAL tensors serve as "hi") and lo = x - hi materialised once.  A*B ~= hi*hi + hi*lo + lo*hi is accumulated by
@@ -320,8 +444,17 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
           }
           continue;
         }
-        const TileCoord tc = tile_coord(wu.tile, p);
-        const int m0 = static_cast<int>((tc.m_blk * CG + rank) * (128 * MT));
+        GrpUnit gu;
+        if constexpr (GRP) {
+          if (wu.tile >= grp_total) break;
+          gu = grp_unit<CB, GRP_MASK>(wu.tile, p, *gpp, grp_o, grp_pre);
+          wu.kb0 = 0;
+          wu.kb1 = gu.nkb;
+        }
+        TileCoord tc = tile_coord(wu.tile, p);
+        if constexpr (GRP) tc = gu.tc;
+        int m0 = static_cast<int>((tc.m_blk * CG + rank) * (128 * MT));
+        if constexpr (CB == CB_GRP_M) m0 += static_cast<int>(gu.row0);   // the group's first tile-row
         const int nb0 = static_cast<int>(tc.n_blk * BLOCK_N);
         const int ba = static_cast<int>(tc.b * p.a_bmul), bb = static_cast<int>(tc.b * p.b_bmul);
         uint32_t seg, kk;  // segment (0 unless k_segments == 3), k-block within it
@@ -407,7 +540,8 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
             tma_load_3d(sa, tma_a_lo, fb, k0, m0, ea);
             load_b(sb + rank * N_LOCAL * 128u, tma_b_lo, k0, nb0 + static_cast<int>(rank * N_LOCAL), eb);
           } else {
-            const int k0 = static_cast<int>(kk * BLOCK_K);
+            int k0 = static_cast<int>(kk * BLOCK_K);
+            if constexpr (CB == CB_GRP_K) k0 += static_cast<int>(gu.lo);   // the group's first position
             const CUtensorMap* tma_a = (seg == 2) ? tma_a_lo : tma_a_hi;
             const CUtensorMap* tma_b = (seg == 1) ? tma_b_lo : tma_b_hi;
             if constexpr (A_MN) {
@@ -506,7 +640,18 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
         tq_m = tcp->ph[tq].M;
         tq_keep = wu.kb1 != 0 ? 0xFFFFFFFFu : 0u;
       }
-      const TileCoord tc = unit_coord<CB>(wu.tile, p, tcp, tq);
+      // grouped matmul: the tile's group and k-blocks; a tile without k-blocks reads its accumulators as +0 (tq_keep)
+      GrpUnit gu;
+      if constexpr (GRP) {
+        if (wu.tile >= grp_total) break;
+        gu = grp_unit<CB, GRP_MASK>(wu.tile, p, *gpp, grp_o, grp_pre);
+        wu.kb0 = 0;
+        wu.kb1 = gu.nkb;
+        tq_keep = gu.nkb != 0 ? 0xFFFFFFFFu : 0u;
+        if constexpr (CB == CB_GRP_M) gu.tc.b = 0;   // out is 2-D: the group picks rows, not a batch
+      }
+      TileCoord tc = unit_coord<CB>(wu.tile, p, tcp, tq);
+      if constexpr (GRP) tc = gu.tc;
       uint32_t seg = 0, kk = 0;
       if constexpr (KIND == KIND_TF32) seg_of(wu.kb0, seg, kk);
       uint32_t prev = 0;
@@ -518,6 +663,10 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
         mbar_wait(full_bar(s), ph);
         const uint32_t sa = smem_base + s * STAGE_BYTES;
         const uint32_t sb = sa + A_BYTES;
+        if constexpr (CB == CB_GRP_K) {
+          const uint32_t keep = (gu.hi - gu.lo) & 63u;
+          if (kb + 1u == wu.kb1 && keep != 0) grp_zero_rows(sa, keep, ct);
+        }
         // A rows of (sub-tile mt, half cw): K-major 128-byte rows, or the (2 mt + cw)-th 64-element MN-major chunk
         auto a_desc_of = [&](int mt) {
           return A_MN ? make_smem_desc_sw128(sa + (2u * mt + cw) * CHUNK_BYTES, CHUNK_BYTES, 1024)
@@ -634,16 +783,24 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
         wgmma_wait<0>();
 #pragma unroll
         for (int mt = 0; mt < MT; ++mt) wgmma_fence_operands(acc[mt]);
-        if (CB != CB_TCONV || wu.kb1 != wu.kb0) release(prev);   // a tile without k-blocks holds no stage
+        if constexpr (GRP) {
+          if (wu.kb1 != wu.kb0) release(prev);
+        } else if (CB != CB_TCONV || wu.kb1 != wu.kb0) {
+          release(prev);   // a tile without k-blocks holds no stage
+        }
       }
 
       // fragment of m64nNk*: thread (warp wq, lane) holds rows 16 wq + lane / 4 (+8) and column pairs 8 j + 2 (lane % 4)
-      const uint32_t m_cta = (tc.m_blk * CG + rank) * (128u * MT);
+      uint32_t m_cta = (tc.m_blk * CG + rank) * (128u * MT);
+      if constexpr (CB == CB_GRP_M) m_cta += gu.row0;
       const uint32_t c0 = tc.n_blk * BLOCK_N + 2u * (lane & 3u);
       // fused epilogue of fragment group j: v = {(r, n), (r, n + 1), (r + 8, n), (r + 8, n + 1)}
       auto epilogue = [&](uint32_t n, uint32_t (&v)[4]) {
         if (!INT_ACC && QM == QM_NONE && p.epi_on) {
           const float* bias = reinterpret_cast<const float*>(p.bias);
+          if constexpr (CB == CB_GRP_M) {
+            if (bias != nullptr) bias += gu.g * gpp->bias_stride;   // the group's row of the [G, N] bias
+          }
 #pragma unroll
           for (int e = 0; e < 4; ++e) {
             const uint32_t col = n + (e & 1);
@@ -704,6 +861,11 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
           const uint64_t row0 = p.out + (static_cast<uint64_t>(r0) * p.out_row_stride + kpos * p.dw_sp) * osz;
           if (r0 < p.M) store_pair<OUT>(row0, ch, p.dw_c, p.vec_store != 0, v[0], v[1]);
           if (r0 + 8 < p.M) store_pair<OUT>(row0 + static_cast<uint64_t>(8) * p.out_row_stride * osz, ch, p.dw_c, p.vec_store != 0, v[2], v[3]);
+        } else if constexpr (CB == CB_GRP_M) {
+          // rows of the group only: the rows around it belong to other groups (or to none)
+          const uint64_t row0 = p.out + static_cast<uint64_t>(r0) * p.out_row_stride * osz;
+          if (r0 >= gu.lo && r0 < gu.hi) store_pair<OUT>(row0, n, p.N, p.vec_store != 0, v[0], v[1]);
+          if (r0 + 8 >= gu.lo && r0 + 8 < gu.hi) store_pair<OUT>(row0 + static_cast<uint64_t>(8) * p.out_row_stride * osz, n, p.N, p.vec_store != 0, v[2], v[3]);
         } else {
           const uint64_t row0 = p.out + (static_cast<uint64_t>(tc.b) * p.out_batch_stride + static_cast<uint64_t>(r0) * p.out_row_stride) * osz;
           if (r0 < p.M) store_pair<OUT>(row0, n, p.N, p.vec_store != 0, v[0], v[1]);
@@ -717,7 +879,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
           // transposed convolution: a tile without k-blocks (a phase no tap reaches) sums to +0 -- read as such through a
           // mask, as no wgmma has cleared the accumulators (writing them on this data-dependent path would serialise every
           // wgmma; a select here is hoisted out of the store loop, which then no longer unrolls)
-          else if constexpr (CB == CB_TCONV) v[e] = acc_bits(acc[mt][4 * j + e]) & tq_keep;
+          else if constexpr (CB == CB_TCONV || GRP) v[e] = acc_bits(acc[mt][4 * j + e]) & tq_keep;
           else v[e] = acc_bits(acc[mt][4 * j + e]);
         }
       };
@@ -725,7 +887,10 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
       // there all the same, as without it the direct-store loop below is not unrolled and the accumulators move to local memory)
       const bool partial = (MT == 1) && !INT_ACC && QM == QM_NONE && wu.partial;
 
-      if (CB != CB_DGRAD && CB != CB_TCONV && !partial && p.tma_store) {
+      // grouped, ragged M: only a CTA tile that lies inside its group leaves through the TMA store (it cannot clip at o_g)
+      bool grp_full = true;
+      if constexpr (CB == CB_GRP_M) grp_full = m_cta >= gu.lo && m_cta + 128u <= gu.hi;
+      if (CB != CB_DGRAD && CB != CB_TCONV && !partial && (CB == CB_GRP_M ? (p.tma_store && grp_full) : p.tma_store != 0)) {
         // fragments -> (epilogue, convert) -> 128B-swizzled [64 rows x 128 B] staging tile -> one TMA store per 128-byte column
         // group; the TMA unit clips ragged edges.  A direct store writes 16 bytes per row per instruction, 8 rows apart.
         const uint32_t stage_smem = epi_base + cw * 8192u;
@@ -974,7 +1139,29 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
   TCONV_KERNEL(PFX##_tconv_f16_f16_##TILE, CG, BN, KIND_F16, OUT_F16, STAGES, DIMS)          \
   TCONV_KERNEL(PFX##_tconv_f16_f32_##TILE, CG, BN, KIND_F16, OUT_F32, STAGES, DIMS)
 
-// The kernels are built as eight cubins from this one source (cubecl_b200/build.py compiles them in parallel):
+// Grouped matmul (GroupedParams; capi.cpp: b200_matmul_grouped): tma_a = lhs, tma_b = rhs (ragged M: 3-D with the group as
+// batch), tma_out = out for the TMA-store path.  Names gemm_grouped_m_<in>_<out>_<tile>_<a><b> (ragged M, the four operand
+// layouts of gemm_*) and gemm_grouped_k_<in>_<out>_<tile> (ragged K: M-contiguous lhs, N-contiguous rhs)
+#define GRP_KERNEL(NAME, CG, BN, AMN, BMN, KIND, OUT, CB)                                                         \
+  extern "C" __global__ void __launch_bounds__(kNumThreads, 1)                                                     \
+      NAME(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,                  \
+           const __grid_constant__ CUtensorMap tma_out, const __grid_constant__ GroupedParams gp,                 \
+           const __grid_constant__ GemmParams p) {                                                                \
+    gemm_body<CG, BN, AMN, BMN, KIND, OUT, 6, false, 1, QM_NONE, false, CB>(&tma_a, &tma_b, &tma_a, &tma_b, &tma_out, p, nullptr, &gp); \
+  }
+#define GRP_ONE(TILE, CG, BN, IN, OUTT, KIND, OUT)                                                     \
+  GRP_KERNEL(gemm_grouped_m_##IN##_##OUTT##_##TILE##_kn, CG, BN, false, true, KIND, OUT, CB_GRP_M)   \
+  GRP_KERNEL(gemm_grouped_m_##IN##_##OUTT##_##TILE##_kk, CG, BN, false, false, KIND, OUT, CB_GRP_M)  \
+  GRP_KERNEL(gemm_grouped_m_##IN##_##OUTT##_##TILE##_mn, CG, BN, true, true, KIND, OUT, CB_GRP_M)    \
+  GRP_KERNEL(gemm_grouped_m_##IN##_##OUTT##_##TILE##_mk, CG, BN, true, false, KIND, OUT, CB_GRP_M)   \
+  GRP_KERNEL(gemm_grouped_k_##IN##_##OUTT##_##TILE, CG, BN, true, true, KIND, OUT, CB_GRP_K)
+#define GRP_DTYPES(TILE, CG, BN)                                 \
+  GRP_ONE(TILE, CG, BN, bf16, bf16, KIND_BF16, OUT_BF16)          \
+  GRP_ONE(TILE, CG, BN, bf16, f32, KIND_BF16, OUT_F32)            \
+  GRP_ONE(TILE, CG, BN, f16, f16, KIND_F16, OUT_F16)              \
+  GRP_ONE(TILE, CG, BN, f16, f32, KIND_F16, OUT_F32)
+
+// The kernels are built as nine cubins from this one source (cubecl_b200/build.py compiles them in parallel):
 //   GEMM_PART 0 ("gemm")       256 x 256 pair tiles (2-CTA cluster, 128 x 256 per CTA) and the bf16 peak probe
 //   GEMM_PART 1 ("gemm_b")     256 x 128 pair tiles, 256 x 224 block-scaled pair tiles
 //   GEMM_PART 2 ("gemm_c")     128 x 128 single-CTA tiles, 512 x 128 pair tiles
@@ -983,6 +1170,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
 //   GEMM_PART 5 ("gemm_convbwd")  the convolution backward kernels (data and weight gradients) of the same two tiles
 //   GEMM_PART 6 ("gemm_conv3d")   the 3-D convolution kernels (forward, data and weight gradients) of the same two tiles
 //   GEMM_PART 7 ("gemm_convt")    the phase-batched transposed-convolution kernels, 2-D and 3-D, of the same two tiles
+//   GEMM_PART 8 ("gemm_grouped")  the grouped-matmul kernels (ragged M and ragged K) of the same two tiles
 #ifndef GEMM_PART
 #define GEMM_PART 0
 #endif
@@ -1045,6 +1233,10 @@ TCONV_DTYPES(2sm_n128, 2, 128, 6, 2, conv2d)
 TCONV_DTYPES(1sm_n128, 1, 128, 6, 2, conv2d)
 TCONV_DTYPES(2sm_n128, 2, 128, 6, 3, conv3d)
 TCONV_DTYPES(1sm_n128, 1, 128, 6, 3, conv3d)
+#endif
+#if GEMM_PART == 8
+GRP_DTYPES(2sm_n128, 2, 128)
+GRP_DTYPES(1sm_n128, 1, 128)
 #endif
 
 #if GEMM_PART == 0

@@ -201,6 +201,33 @@ struct TconvParams {
   uint32_t phases, pad[3];
 };
 
+// Grouped matmul for mixture-of-experts layers (gemm_grouped_m_* / gemm_grouped_k_*, cubin gemm_grouped; capi.cpp:
+// b200_matmul_grouped).  offs: i32 [groups] cumulative ends on the device, read only by the kernel; on read
+// o_g = min(max(offs[g], o_{g-1}), T) with o_{-1} = 0, so group g owns positions [o_{g-1}, o_g) and a malformed table only makes
+// groups empty or short.  Every CTA reads offs once into a table at the end of its shared memory (after the TMA-store staging):
+// u32 o[kGroupedMaxGroups] (the clamped ends), then u32 pre[kGroupedMaxGroups + 1] (pre[g] = tile-rows of the groups before g,
+// a tile-row being 128 * CG rows of a group; pre[groups] = every group's).
+//   mode 0, ragged M (gemm_grouped_m_*): lhs [T, K] x rhs [G, K, N] -> out [T, N].  Tiles are listed group after group, each
+//        group's pre[g + 1] - pre[g] tile-rows x GemmParams::tiles_n in GemmParams::group_m strips; units past pre[groups] *
+//        tiles_n are skipped.  A rows come from r_g + m_blk * 128 * CG of the 2-D lhs map, B from the 3-D rhs map at batch g;
+//        r_g = o_{g-1}, or with an M-contiguous lhs o_{g-1} rounded down to a multiple of 64 (the group's first row is then the
+//        innermost coordinate of the A loads; loads there at a coordinate that is not a multiple of 16 bytes faulted).  A CTA tile inside its group leaves through
+//        the TMA store, any other through direct stores of rows in [o_{g-1}, o_g); rows >= o_{G-1} are never written.  bias (GemmParams::bias) is f32 [G, N], row g at bias + g * bias_stride.
+//   mode 1, ragged K (gemm_grouped_k_*, the weight gradient): lhs [M, T] (M-contiguous) x rhs [T, N] (N-contiguous) ->
+//        out [G, M, N], out[g] = lhs[:, o_{g-1}:o_g] @ rhs[o_{g-1}:o_g, :].  Tile t is group t / (tiles_m * tiles_n); it runs
+//        ceil(n_g / 64) k-blocks from position o_{g-1}, and zeroes the rows of positions >= o_g in both operands of its last
+//        k-block before the MMAs read them.  A group without positions stores +0.
+// The host sizes the grid from an upper bound on the tiles (GemmParams::full_tiles): (ceil(T / (128 CG)) + G) * tiles_n in
+// mode 0 (ceil((T + 63 G) / (128 CG)) + G tile-rows with an M-contiguous lhs), G * tiles_m * tiles_n in mode 1.  Shared memory: gemm_smem_bytes(variant) + kGroupedTableBytes.
+constexpr int kGroupedMaxGroups = 1024;
+constexpr uint32_t kGroupedTableBytes = (2 * kGroupedMaxGroups + 4) * 4;
+struct GroupedParams {
+  uint64_t offs;          // i32 [groups] cumulative ends, 4-byte aligned
+  uint64_t bias_stride;   // mode 0: elements between the bias rows of consecutive groups
+  uint32_t groups, T;     // G (1 .. kGroupedMaxGroups); T = the ragged extent (lhs rows, or positions)
+  uint32_t mode, pad;     // 0 ragged M, 1 ragged K
+};
+
 // ================================================================================================ attention.cu
 // Fused attention forward (attn_fwd_*; capi.cpp: b200_attention).  One CTA per (b, h, kAttnBlock-query block), grid
 // nqb * Hq * B with block x = ((nqb - 1 - qb) * B + b) * Hq + h; K and V stream in blocks of kAttnBlock keys through

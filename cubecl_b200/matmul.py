@@ -163,6 +163,68 @@ def launch_quantized(client: ComputeClient, lhs, rhs, out: TensorHandle, stream=
         client._defer(e)
 
 
+def calculate_grouped_output(shape_lhs, shape_rhs, groups: int) -> list[int]:
+    """Output shape of a grouped matmul (torch.nn.functional.grouped_mm with offs): lhs [T, K] x rhs [G, K, N] -> [T, N]
+    (ragged M), or lhs [M, T] x rhs [T, N] -> [G, M, N] (ragged K); `groups` is the length of offs."""
+    shape_lhs, shape_rhs = list(shape_lhs), list(shape_rhs)
+    if len(shape_lhs) == 2 and len(shape_rhs) == 3:
+        if shape_lhs[1] != shape_rhs[1]:
+            raise MatmulShapeError(f"inner dims differ: lhs k={shape_lhs[1]}, rhs k={shape_rhs[1]}")
+        if shape_rhs[0] != groups:
+            raise MatmulShapeError(f"{groups} groups in offs, but rhs has {shape_rhs[0]}")
+        return [shape_lhs[0], shape_rhs[2]]
+    if len(shape_lhs) == 2 and len(shape_rhs) == 2:
+        if shape_lhs[1] != shape_rhs[0]:
+            raise MatmulShapeError(f"inner dims differ: lhs k={shape_lhs[1]}, rhs k={shape_rhs[0]}")
+        return [groups, shape_lhs[0], shape_rhs[1]]
+    raise MatmulShapeError(f"grouped matmul takes 2-D x 3-D (ragged M) or 2-D x 2-D (ragged K), not {len(shape_lhs)}-D x "
+                           f"{len(shape_rhs)}-D")
+
+
+def launch_grouped(client: ComputeClient, lhs: TensorHandle, rhs: TensorHandle, offs: TensorHandle, out: TensorHandle,
+                   bias: TensorHandle | None = None, alpha: float = 1.0, activation: str | None = None, stream=None) -> None:
+    """Grouped matmul for mixture-of-experts layers, the interface of torch.nn.functional.grouped_mm(lhs, rhs, offs=offs):
+      ragged M: lhs [T, K] x rhs [G, K, N] -> out [T, N]; rows of group g use rhs[g]; rows >= offs[-1] are not written.
+      ragged K: lhs [M, T] (M-contiguous, x.t()) x rhs [T, N] (N-contiguous) -> out [G, M, N], out[g] sums group g's positions.
+    offs is a compact i32 [G] device tensor of cumulative ends, read on the device only (no host sync); see b200_matmul_grouped
+    in include/cubecl_b200.h for the clamping rule.  Ragged M takes the fused epilogue out = act(alpha * acc + bias[g, n]) with
+    an f32 [G, N] bias.  Errors are deferred to client.sync() like every launch."""
+    try:
+        if activation not in ACTIVATIONS:
+            raise B200Error(6, f"unknown activation {activation!r}")
+        if lhs.dtype != rhs.dtype:
+            raise B200Error(6, f"matmul_grouped: lhs dtype {lhs.dtype} != rhs dtype {rhs.dtype}")
+        if offs.dtype != "i32" or len(offs.shape) != 1 or not offs.is_contiguous():
+            raise B200Error(6, "matmul_grouped: offs must be a compact i32 [groups] tensor")
+        groups = offs.shape[0]
+        if bias is not None:
+            if bias.dtype != "f32" or not bias.is_contiguous() or list(bias.shape) != [groups, out.shape[-1]]:
+                raise B200Error(6, "matmul_grouped: bias must be a contiguous f32 [groups, N] tensor")
+        fused = alpha != 1.0 or bias is not None or activation not in (None, "none")
+        ep = _ffi.Epilogue(float(alpha), ACTIVATIONS[activation], bias.handle.ptr if bias is not None else 0) if fused else None
+        for th in (lhs, rhs, offs, out) + ((bias,) if bias is not None else ()):
+            th.handle.used_on(stream)
+        _ffi.check(client._lib.b200_matmul_grouped(
+            client._ctx, stream, DTYPES[lhs.dtype], DTYPES[out.dtype],
+            C.c_uint64(lhs.handle.ptr), len(lhs.shape), _ffi.u64_array(lhs.shape), _ffi.u64_array(lhs.strides),
+            C.c_uint64(rhs.handle.ptr), len(rhs.shape), _ffi.u64_array(rhs.shape), _ffi.u64_array(rhs.strides),
+            C.c_uint64(offs.handle.ptr), groups,
+            C.c_uint64(out.handle.ptr), len(out.shape), _ffi.u64_array(out.shape), _ffi.u64_array(out.strides),
+            C.byref(ep) if ep is not None else None))
+    except B200Error as e:
+        client._defer(e)
+
+
+def launch_grouped_alloc(client: ComputeClient, lhs: TensorHandle, rhs: TensorHandle, offs: TensorHandle,
+                         out_dtype: str | None = None, **kw) -> TensorHandle:
+    """Convenience: allocate a contiguous `out` by calculate_grouped_output, then launch_grouped (ragged M leaves the rows
+    past the last group uninitialised, as torch does)."""
+    shape = calculate_grouped_output(lhs.shape, rhs.shape, offs.shape[0] if len(offs.shape) == 1 else 0)
+    out = TensorHandle.empty_contiguous(client, shape, out_dtype or lhs.dtype)
+    launch_grouped(client, lhs, rhs, offs, out, **kw)
+    return out
+
+
 def launch_alloc(client: ComputeClient, lhs: TensorHandle, rhs: TensorHandle, out_dtype: str | None = None) -> TensorHandle:
     """Convenience: allocate `out` with the reference's shape rule, then launch."""
     shape = calculate_matmul_output(lhs.shape, rhs.shape)

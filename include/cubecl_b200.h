@@ -184,6 +184,34 @@ int b200_matmul_fused(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b200_dt
                       const uint64_t* shape_rhs, const uint64_t* strides_rhs,
                       const uint64_t* shape_out, const uint64_t* strides_out, const b200_epilogue* epilogue);
 
+/* Grouped matmul for mixture-of-experts layers: the interface of torch.nn.functional.grouped_mm(mat_a, mat_b, offs=...) for
+ * its two offset modes, in one launch with the offsets read on the device only (no host sync; the call can be captured in a
+ * graph).  offs: a compact, 4-byte aligned i32 [groups] device array of cumulative ends; on read each is clamped,
+ * o_g = min(max(offs[g], o_{g-1}), T) with o_{-1} = 0, so group g owns positions [o_{g-1}, o_g) and a malformed table makes
+ * groups empty or short but never reads or writes out of bounds.  The mode comes from the ranks (shapes and strides in
+ * elements; NULL strides = compact row-major):
+ *   ragged M (forward, data gradient): lhs [T, K] x rhs [G, K, N] -> out [T, N]; rows of group g use rhs[g].  Rows >= o_{G-1}
+ *     of out are NOT written (torch leaves them undefined).  All four operand-major layouts are read in place, as by
+ *     b200_matmul: the forward x @ W_g^T passes rhs as the transposed view of [G, N, K] weights.  epilogue (NULL = none):
+ *     out = act(alpha * acc + bias[g, n]) with bias a compact f32 [G, N] array (row g for group g) or 0.
+ *   ragged K (weight gradient, grouped_mm(x.t(), dy, offs)): lhs [M, T] x rhs [T, N] -> out [G, M, N],
+ *     out[g] = lhs[:, o_{g-1}:o_g] @ rhs[o_{g-1}:o_g, :]; a group without positions gets out[g] = +0 (written).  lhs must be
+ *     M-contiguous (x.t() of x [T, M]) and rhs N-contiguous; other layouts and a non-NULL epilogue: B200_ERR_UNSUPPORTED.
+ * in_dtype BF16 or F16 (both operands); out_dtype the input dtype or F32.  f32 accumulation over increasing k, one rounding per
+ * output.  No atomics and no stream-K: bitwise reproducible for fixed shapes, offsets and SM count.  groups = G must equal
+ * rhs shape[0] (ragged M) or out shape[0] (ragged K) and be at most 1024 (more: B200_ERR_UNSUPPORTED).  Input views TMA cannot
+ * describe are staged once; out needs a unit column stride and is written in place.  Options "gemm.variant" (auto, 2sm_n128,
+ * 1sm_n128) and "gemm.epilogue" apply; "gemm.split_k" does not.
+ * Errors: B200_ERR_INVALID_ARG for ranks other than the two modes, mismatched K / N / out shapes, a groups count that does not
+ * match, a null or misaligned pointer, an unknown activation; B200_ERR_UNSUPPORTED for 3-D x 3-D (a batched b200_matmul),
+ * 3-D x 2-D (ragged N), other dtypes, extents >= 2^31 and a tile bound >= 2^32.  groups = 0, M = 0 or N = 0 is a no-op. */
+int b200_matmul_grouped(b200_ctx* ctx, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype,
+                        b200_dptr lhs, int lhs_rank, const uint64_t* lhs_shape, const uint64_t* lhs_strides,
+                        b200_dptr rhs, int rhs_rank, const uint64_t* rhs_shape, const uint64_t* rhs_strides,
+                        b200_dptr offs, uint64_t groups,
+                        b200_dptr out, int out_rank, const uint64_t* out_shape, const uint64_t* out_strides,
+                        const b200_epilogue* epilogue);
+
 /* Block-scaled (MX) matmul: out[b,m,n] = sum_k (lhs[b,m,k] * lhs_scales[b,m,k/32]) * (rhs[b,n,k] * rhs_scales[b,n,k/32]),
  * f32 accumulation.  Replaces MmaDefinition::new_scaled / execute_scaled (crates/cubecl-core/src/frontend/cmma.rs:438-460,
  * 798-840), the ScaledMmaConfig feature rows (crates/cubecl-ir/src/features.rs:190-211; on CUDA the reference offers them

@@ -32,14 +32,14 @@ struct MatmulShapeError : std::invalid_argument {
   using std::invalid_argument::invalid_argument;
 };
 
-enum class DType : int { F32 = B200_F32, F16 = B200_F16, BF16 = B200_BF16, U32 = B200_U32, U8 = B200_U8, I8 = B200_I8,
+enum class DType : int { F32 = B200_F32, F16 = B200_F16, BF16 = B200_BF16, U32 = B200_U32, I32 = B200_I32, U8 = B200_U8, I8 = B200_I8,
                          F8E4M3 = B200_F8E4M3, F8E5M2 = B200_F8E5M2,
                          F4E2M1X2 = B200_F4E2M1X2,  // one element = one byte holding two e2m1 values
                          UE8M0 = B200_UE8M0 };
 inline size_t dtype_size(DType d) {
   switch (d) {
     case DType::F16: case DType::BF16: return 2;
-    case DType::F32: case DType::U32: return 4;
+    case DType::F32: case DType::U32: case DType::I32: return 4;
     default: return 1;
   }
 }
@@ -216,6 +216,22 @@ inline void launch_quantized(ComputeClient& client, const b200_quant_operand& lh
                              uint64_t batch, uint64_t m, uint64_t n, uint64_t k) {
   const int rc = b200_matmul_quantized(client.raw(), nullptr, &lhs, &rhs, static_cast<b200_dtype>(out.dtype), out.handle.ptr(),
                                        batch, m, n, k);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+/// Grouped matmul for mixture-of-experts layers (torch's grouped_mm with offs): lhs [T, K] x rhs [G, K, N] -> out [T, N]
+/// (ragged M), or lhs [M, T] x rhs [T, N] -> out [G, M, N] (ragged K); offs is a compact i32 [G] tensor of cumulative ends
+/// read on the device only.  See b200_matmul_grouped in cubecl_b200.h for the contract.  Errors are deferred to client.sync().
+inline void launch_grouped(ComputeClient& client, const TensorHandle& lhs, const TensorHandle& rhs, const TensorHandle& offs,
+                           const TensorHandle& out, const b200_epilogue* epilogue = nullptr) {
+  if (lhs.dtype != rhs.dtype || offs.dtype != DType::I32 || offs.shape.size() != 1 || (offs.shape[0] > 1 && offs.strides[0] != 1)) {
+    client.defer("InvalidArgument: matmul_grouped needs lhs and rhs of one dtype and a compact i32 [groups] offs");
+    return;
+  }
+  const int rc = b200_matmul_grouped(client.raw(), nullptr, static_cast<b200_dtype>(lhs.dtype), static_cast<b200_dtype>(out.dtype),
+                                     lhs.handle.ptr(), static_cast<int>(lhs.shape.size()), lhs.shape.data(), lhs.strides.data(),
+                                     rhs.handle.ptr(), static_cast<int>(rhs.shape.size()), rhs.shape.data(), rhs.strides.data(),
+                                     offs.handle.ptr(), offs.shape[0], out.handle.ptr(), static_cast<int>(out.shape.size()),
+                                     out.shape.data(), out.strides.data(), epilogue);
   if (rc != B200_OK) client.defer(b200_last_error());
 }
 }  // namespace matmul
