@@ -925,117 +925,93 @@ static int encode_tmap(b200_ctx* c, CUtensorMap* out, CUtensorMapDataType dt, si
   return B200_OK;
 }
 
-// 4-D im2col map of an NHWC tensor (dims innermost first: C, W, H, N; strides of W, H, N in elements), SWIZZLE_128B, zero
-// out-of-bounds fill.  Corners (w, h) bound the pixels a load walks; estr_w / estr_h are the conv strides.  Same cache as
-// encode_tmap.
-static int encode_im2col(b200_ctx* c, CUtensorMap* out, CUtensorMapDataType dt, size_t esz, uint64_t base, const uint64_t dims[4],
-                         const uint64_t strides[3], const int lower[2], const int upper[2], uint32_t channels, uint32_t pixels,
-                         uint32_t estr_w, uint32_t estr_h) {
+// im2col map of an NHWC (rank 4) or NDHWC (rank 5) tensor, dims innermost first (C, W, H, (D,) N; strides of all but C in
+// elements), SWIZZLE_128B, zero out-of-bounds fill.  Per spatial dimension, innermost first: corners lower / upper bound the
+// pixels a load walks and estr are the conv strides.  cuda.h (cuTensorMapEncodeIm2col) limits the corners to [-128, 127] at
+// rank 4 and [-16, 15] at rank 5.  Same cache as encode_tmap.
+static int encode_im2col(b200_ctx* c, CUtensorMap* out, CUtensorMapDataType dt, size_t esz, uint64_t base, int rank, const uint64_t* dims,
+                         const uint64_t* strides, const int* lower, const int* upper, uint32_t channels, uint32_t pixels, const uint32_t* estr) {
   const int promo_bytes = atoi(opt(c, "gemm.l2_promotion", "256").c_str());
   const CUtensorMapL2promotion promo = promo_bytes >= 256 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B
                                        : promo_bytes >= 128 ? CU_TENSOR_MAP_L2_PROMOTION_L2_128B
                                        : promo_bytes >= 64 ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B : CU_TENSOR_MAP_L2_PROMOTION_NONE;
-  char key[320];
-  snprintf(key, sizeof(key), "im2col|%d|%llx|%llu|%llu|%llu|%llu|%llu|%llu|%llu|%d|%d|%d|%d|%u|%u|%u|%u|%d", (int)dt,
-           (unsigned long long)base, (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)dims[2],
-           (unsigned long long)dims[3], (unsigned long long)strides[0], (unsigned long long)strides[1], (unsigned long long)strides[2],
-           lower[0], lower[1], upper[0], upper[1], channels, pixels, estr_w, estr_h, (int)promo);
+  const int sp = rank - 2;
+  auto join = [](int n, auto f) {
+    std::string t;
+    for (int i = 0; i < n; ++i) t += (i ? "," : "") + std::to_string(f(i));
+    return t;
+  };
+  const std::string dims_j = join(rank, [&](int i) { return dims[i]; }), estr_j = join(sp, [&](int i) { return estr[i]; });
+  const std::string lower_t = "(" + join(sp, [&](int i) { return lower[i]; }) + ")", upper_t = "(" + join(sp, [&](int i) { return upper[i]; }) + ")";
+  const std::string key = "im2col|" + std::to_string(rank) + "|" + std::to_string((int)dt) + "|" + std::to_string(base) + "|" + dims_j + "|" +
+                          join(rank - 1, [&](int i) { return strides[i]; }) + "|" + lower_t + upper_t + estr_j + "|" + std::to_string(channels) +
+                          "|" + std::to_string(pixels) + "|" + std::to_string((int)promo);
   if (c->dry) {
-    char line[320];
-    snprintf(line, sizeof(line),
-             "tmap im2col esz=%zu dims=(%llu,%llu,%llu,%llu) strides=(%llu,%llu,%llu) lower=(%d,%d) upper=(%d,%d) channels=%u pixels=%u "
-             "estrides=(1,%u,%u,1) swizzle=%d\n",
-             esz, (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)dims[2], (unsigned long long)dims[3],
-             (unsigned long long)(strides[0] * esz), (unsigned long long)(strides[1] * esz), (unsigned long long)(strides[2] * esz),
-             lower[0], lower[1], upper[0], upper[1], channels, pixels, estr_w, estr_h, (int)CU_TENSOR_MAP_SWIZZLE_128B);
-    c->plan += line;
+    c->plan += std::string(rank == 5 ? "tmap im2col5d" : "tmap im2col") + " esz=" + std::to_string(esz) + " dims=(" + dims_j + ") strides=(" +
+               join(rank - 1, [&](int i) { return strides[i] * esz; }) + ") lower=" + lower_t + " upper=" + upper_t + " channels=" +
+               std::to_string(channels) + " pixels=" + std::to_string(pixels) + " estrides=(1," + estr_j + ",1) swizzle=" +
+               std::to_string((int)CU_TENSOR_MAP_SWIZZLE_128B) + "\n";
     memset(out, 0, sizeof(*out));
     return B200_OK;
   }
   auto it = c->tmap_cache.find(key);
   if (it != c->tmap_cache.end()) { *out = it->second; return B200_OK; }
-  cuuint64_t gdim[4] = {dims[0], dims[1], dims[2], dims[3]};
-  cuuint64_t gstr[3] = {strides[0] * esz, strides[1] * esz, strides[2] * esz};
-  cuuint32_t estr[4] = {1, estr_w, estr_h, 1};
-  CUresult r = g_drv.cuTensorMapEncodeIm2col_p(out, dt, 4, reinterpret_cast<void*>(base), gdim, gstr, lower, upper, channels, pixels, estr,
+  cuuint64_t gdim[5], gstr[4];
+  cuuint32_t es[5] = {1, 1, 1, 1, 1};
+  for (int i = 0; i < rank; ++i) gdim[i] = dims[i];
+  for (int i = 0; i < rank - 1; ++i) gstr[i] = strides[i] * esz;
+  for (int i = 0; i < sp; ++i) es[1 + i] = estr[i];
+  CUresult r = g_drv.cuTensorMapEncodeIm2col_p(out, dt, rank, reinterpret_cast<void*>(base), gdim, gstr, lower, upper, channels, pixels, es,
                                                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, promo,
                                                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)
-    return fail(B200_ERR_INVALID_ARG, "cuTensorMapEncodeIm2col failed: %s (dims %llu,%llu,%llu,%llu corners (%d,%d)..(%d,%d))", cu_err(r),
-                (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)dims[2], (unsigned long long)dims[3],
-                lower[0], lower[1], upper[0], upper[1]);
+    return fail(B200_ERR_INVALID_ARG, "cuTensorMapEncodeIm2col%s failed: %s (dims %s corners %s..%s)", rank == 5 ? " (rank 5)" : "", cu_err(r),
+                dims_j.c_str(), lower_t.c_str(), upper_t.c_str());
   if (c->tmap_cache.size() > 512) c->tmap_cache.clear();
   c->tmap_cache[key] = *out;
   return B200_OK;
 }
 
-// 5-D im2col map of an NDHWC tensor (dims innermost first: C, W, H, D, N; strides of W, H, D, N in elements): as
-// encode_im2col with a depth dimension.  Corners (w, h, d) must lie in [-16, 15] (cuda.h, rank 5); estr_* are the conv strides.
-static int encode_im2col5(b200_ctx* c, CUtensorMap* out, CUtensorMapDataType dt, size_t esz, uint64_t base, const uint64_t dims[5],
-                          const uint64_t strides[4], const int lower[3], const int upper[3], uint32_t channels, uint32_t pixels,
-                          const uint32_t estr_whd[3]) {
-  const int promo_bytes = atoi(opt(c, "gemm.l2_promotion", "256").c_str());
-  const CUtensorMapL2promotion promo = promo_bytes >= 256 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B
-                                       : promo_bytes >= 128 ? CU_TENSOR_MAP_L2_PROMOTION_L2_128B
-                                       : promo_bytes >= 64 ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B : CU_TENSOR_MAP_L2_PROMOTION_NONE;
-  std::string key = "im2col5d|" + std::to_string((int)dt) + "|" + std::to_string(base);
-  for (int i = 0; i < 5; ++i) key += "|" + std::to_string(dims[i]);
-  for (int i = 0; i < 4; ++i) key += "|" + std::to_string(strides[i]);
-  for (int i = 0; i < 3; ++i) key += "|" + std::to_string(lower[i]) + "|" + std::to_string(upper[i]) + "|" + std::to_string(estr_whd[i]);
-  key += "|" + std::to_string(channels) + "|" + std::to_string(pixels) + "|" + std::to_string((int)promo);
-  if (c->dry) {
-    char line[400];
-    snprintf(line, sizeof(line),
-             "tmap im2col5d esz=%zu dims=(%llu,%llu,%llu,%llu,%llu) strides=(%llu,%llu,%llu,%llu) lower=(%d,%d,%d) upper=(%d,%d,%d) "
-             "channels=%u pixels=%u estrides=(1,%u,%u,%u,1) swizzle=%d\n",
-             esz, (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)dims[2], (unsigned long long)dims[3],
-             (unsigned long long)dims[4], (unsigned long long)(strides[0] * esz), (unsigned long long)(strides[1] * esz),
-             (unsigned long long)(strides[2] * esz), (unsigned long long)(strides[3] * esz), lower[0], lower[1], lower[2], upper[0],
-             upper[1], upper[2], channels, pixels, estr_whd[0], estr_whd[1], estr_whd[2], (int)CU_TENSOR_MAP_SWIZZLE_128B);
-    c->plan += line;
-    memset(out, 0, sizeof(*out));
-    return B200_OK;
-  }
-  auto it = c->tmap_cache.find(key);
-  if (it != c->tmap_cache.end()) { *out = it->second; return B200_OK; }
-  cuuint64_t gdim[5] = {dims[0], dims[1], dims[2], dims[3], dims[4]};
-  cuuint64_t gstr[4] = {strides[0] * esz, strides[1] * esz, strides[2] * esz, strides[3] * esz};
-  cuuint32_t estr[5] = {1, estr_whd[0], estr_whd[1], estr_whd[2], 1};
-  CUresult r = g_drv.cuTensorMapEncodeIm2col_p(out, dt, 5, reinterpret_cast<void*>(base), gdim, gstr, lower, upper, channels, pixels, estr,
-                                               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, promo,
-                                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS)
-    return fail(B200_ERR_INVALID_ARG, "cuTensorMapEncodeIm2col (rank 5) failed: %s (dims %llu,%llu,%llu,%llu,%llu corners (%d,%d,%d)..(%d,%d,%d))",
-                cu_err(r), (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)dims[2], (unsigned long long)dims[3],
-                (unsigned long long)dims[4], lower[0], lower[1], lower[2], upper[0], upper[1], upper[2]);
-  if (c->tmap_cache.size() > 512) c->tmap_cache.clear();
-  c->tmap_cache[key] = *out;
-  return B200_OK;
-}
-
-// Geometry of a 2-D convolution run as an implicit GEMM (b200_conv2d): x is NHWC with unit channel stride, w is
-// [Cout, KH * KW, C] with unit channel stride; strides in elements.
+// Geometry of a 2-D or 3-D convolution run as an implicit GEMM: x is N(D)HWC with unit channel stride, w is
+// [Cout, kernel positions, C] with unit channel stride; strides in elements.  Per-dimension arrays are ordered (D, H, W); a
+// 2-D convolution (n = 2) has a unit depth (extents 1, stride 1, pad 0, dilation 1, strides 0).
 struct ConvGeom {
-  uint64_t N, H, W, C, KH, KW, OH, OW, Cout;
-  int32_t sh, sw, ph, pw, dh, dw;
-  uint64_t x_sw, x_sh, x_sn;   // x: pixel (w), row (h) and image (n) strides
-  uint64_t w_sp, w_sco;        // w: kernel-position and output-channel strides
-  // An explicit, asymmetric pixel box (stride 1 only): the im2col walk covers OW x OH pixels from the lower corner
-  // (lo_w, lo_h) instead of the forward's (-pw, -ph) .. (pw - dw (KW - 1), ph - dh (KH - 1)).  A data-gradient phase.
+  int n = 2;
+  uint64_t N = 0, C = 0, Cout = 0;
+  uint64_t I[3] = {1, 1, 1}, K[3] = {1, 1, 1}, O[3] = {1, 1, 1};   // input, kernel and output extents
+  int32_t s[3] = {1, 1, 1}, p[3] = {0, 0, 0}, d[3] = {1, 1, 1};
+  uint64_t x_s[3] = {0, 0, 0}, x_sn = 0;   // x: pixel strides per dimension, image stride
+  uint64_t w_sp = 0, w_sco = 0;            // w: kernel-position and output-channel strides
+  // An explicit, asymmetric pixel box (stride 1 only): the im2col walk covers the O pixels from the lower corner lo instead of
+  // the forward's -p .. p - d (K - 1).  A data-gradient phase.
   bool box = false;
-  int32_t lo_h = 0, lo_w = 0;
-  // 0: the forward (conv2d_*); 1: a data-gradient phase with the phase-addressed epilogue (conv2d_dgrad_*, dx_* strides);
-  // 2: the weight gradient (conv2d_wgrad_*): A = dy [Cout x pixels], B = x through im2col, out = dw (dw_sp, dw_c)
+  int32_t lo[3] = {0, 0, 0};
+  // 0: the forward (conv2d_* / conv3d_*); 1: a data-gradient phase with the phase-addressed epilogue (*_dgrad_*, dx_* strides);
+  // 2: the weight gradient (*_wgrad_*): A = dy [Cout x pixels], B = x through im2col, out = dw (dw_sp, dw_c)
   int mode = 0;
-  uint64_t dx_sn = 0, dx_si = 0, dx_sj = 0;
+  uint64_t dx_sn = 0, dx_s[3] = {0, 0, 0};
   uint64_t dw_sp = 0, dw_c = 0;
-  // 3-D convolution (b200_conv3d*): dims = 3 adds a depth dimension to everything above (x strides x_sd, a pixel box corner
-  // lo_d, dx stride dx_sd per phase row).  The defaults leave every 2-D path as it is.
-  int dims = 2;
-  uint64_t D = 1, KD = 1, OD = 1;
-  int32_t sd = 1, pd = 0, dd = 1, lo_d = 0;
-  uint64_t x_sd = 0, dx_sd = 0;
 };
+
+// The im2col map of the convolution input: `pixels` output pixels x 64 channels per load, walking the input pixels the
+// output grid reads at kernel position 0.
+static int encode_conv_im2col(b200_ctx* c, CUtensorMap* m, CUtensorMapDataType dt, size_t esz, const ConvGeom& cv, uint64_t base, uint32_t pixels) {
+  uint64_t dims[5], strides[4];
+  int lo[3], up[3];
+  uint32_t estr[3];
+  dims[0] = cv.C;
+  for (int j = 0; j < cv.n; ++j) {   // innermost first: W, H, (D)
+    const int i = 2 - j;
+    dims[1 + j] = cv.I[i];
+    strides[j] = cv.x_s[i];
+    lo[j] = cv.box ? cv.lo[i] : -cv.p[i];
+    up[j] = cv.box ? cv.lo[i] + (int)cv.O[i] - (int)cv.I[i] : cv.p[i] - cv.d[i] * (int)(cv.K[i] - 1);
+    estr[j] = (uint32_t)cv.s[i];
+  }
+  dims[cv.n + 1] = cv.N;
+  strides[cv.n] = cv.x_sn;
+  return encode_im2col(c, m, dt, esz, base, cv.n + 2, dims, strides, lo, up, 64, pixels, estr);
+}
 
 // One batched problem with LINEAR batch strides (0 = broadcast).  Strides in elements.
 struct GemmProblem {
@@ -1058,7 +1034,7 @@ struct GemmProblem {
   int q = 0;
   uint32_t q_bk = 0;
   uint64_t q_sa = 0, q_sb = 0, q_ga = 0, q_gb = 0;
-  // 2-D convolution (b200_conv2d): a = x, b = w, M = N * OH * OW, N = Cout, K = KH * KW * (C padded to 64), batch 1
+  // convolution (b200_conv2d / 3d): a = x, b = w, M = output pixels, N = Cout, K = kernel positions * (C padded to 64), batch 1
   const ConvGeom* conv = nullptr;
   uint64_t sk_max_parts = 8;    // stream-K head: at most this many ranges per tile (sk_plan)
 };
@@ -1234,8 +1210,7 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
   const GemmVariant& v = *best;
 
   const int cmode = g.conv ? g.conv->mode : 0;
-  const bool cv3 = g.conv && g.conv->dims == 3;
-  const std::string cpfx = cv3 ? "conv3d_" : "conv2d_";
+  const std::string cpfx = g.conv && g.conv->n == 3 ? "conv3d_" : "conv2d_";
   const std::string name = g.conv ? cpfx + (cmode == 1 ? "dgrad_" : cmode == 2 ? "wgrad_" : "") + in_tag + "_" + out_tag + "_" + v.tag
                                   : std::string("gemm_") + in_tag + "_" + out_tag + "_" + v.tag + (a_mn ? "_m" : "_k") + (b_mn ? "n" : "k");
   CUfunction f;
@@ -1253,32 +1228,8 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
   auto pad16 = [&](uint64_t elems) { const uint64_t q = 16 / esz; return (elems + q - 1) / q * q; };
   const uint32_t chunk = static_cast<uint32_t>(128 / esz);  // MN-major operands (16-bit): elements per 128-byte row
   const uint32_t n_local = v.block_n / v.cg;   // B rows each CTA of a pair loads (multicast to both)
-  // im2col map of the convolution input: `pixels` output pixels x 64 channels per load, walking the input pixels the output
-  // grid reads at kernel position (0, 0)
-  auto conv_im2col = [&](CUtensorMap* m, uint64_t base, uint32_t pixels) {
-    const ConvGeom& cv = *g.conv;
-    if (cv.dims == 3) {
-      const uint64_t dims5[5] = {cv.C, cv.W, cv.H, cv.D, cv.N}, strides4[4] = {cv.x_sw, cv.x_sh, cv.x_sd, cv.x_sn};
-      int lo[3] = {-cv.pw, -cv.ph, -cv.pd};
-      int up[3] = {cv.pw - cv.dw * (int)(cv.KW - 1), cv.ph - cv.dh * (int)(cv.KH - 1), cv.pd - cv.dd * (int)(cv.KD - 1)};
-      if (cv.box) {
-        lo[0] = cv.lo_w; lo[1] = cv.lo_h; lo[2] = cv.lo_d;
-        up[0] = cv.lo_w + (int)cv.OW - (int)cv.W; up[1] = cv.lo_h + (int)cv.OH - (int)cv.H; up[2] = cv.lo_d + (int)cv.OD - (int)cv.D;
-      }
-      const uint32_t estr[3] = {(uint32_t)cv.sw, (uint32_t)cv.sh, (uint32_t)cv.sd};
-      return encode_im2col5(c, m, dt, esz, base, dims5, strides4, lo, up, 64, pixels, estr);
-    }
-    const uint64_t dims[4] = {cv.C, cv.W, cv.H, cv.N}, strides[3] = {cv.x_sw, cv.x_sh, cv.x_sn};
-    int lower[2] = {-cv.pw, -cv.ph};
-    int upper[2] = {cv.pw - cv.dw * (int)(cv.KW - 1), cv.ph - cv.dh * (int)(cv.KH - 1)};
-    if (cv.box) {
-      lower[0] = cv.lo_w; lower[1] = cv.lo_h;
-      upper[0] = cv.lo_w + (int)cv.OW - (int)cv.W; upper[1] = cv.lo_h + (int)cv.OH - (int)cv.H;
-    }
-    return encode_im2col(c, m, dt, esz, base, dims, strides, lower, upper, 64, pixels, (uint32_t)cv.sw, (uint32_t)cv.sh);
-  };
   if (g.conv && cmode != 2) {
-    rc = conv_im2col(&ta, g.a, 128);
+    rc = encode_conv_im2col(c, &ta, dt, esz, *g.conv, g.a, 128);
   } else if (!a_mn) {
     const uint64_t a_sm = g.M > 1 ? g.a_sm : pad16(g.K);
     rc = encode_tmap(c, &ta, dt, esz, g.a, g.K, g.M, a_bcast ? 1 : g.batch, a_sm, a_bcast ? a_sm * g.M : g.a_sb, block_k, 128);
@@ -1289,11 +1240,11 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
   if (rc) return rc;
   if (cmode == 2) {
     // weight gradient: 64 pixels x 64 channels of x per MN-major B chunk
-    rc = conv_im2col(&tb, g.b, 64);
+    rc = encode_conv_im2col(c, &tb, dt, esz, *g.conv, g.b, 64);
   } else if (g.conv) {
     // [n_local output channels x 64 channels] of one kernel position
     const ConvGeom& cv = *g.conv;
-    rc = encode_tmap(c, &tb, dt, esz, g.b, cv.C, cv.KD * cv.KH * cv.KW, cv.Cout, cv.w_sp, cv.w_sco, 64, 1, CU_TENSOR_MAP_SWIZZLE_128B, n_local);
+    rc = encode_tmap(c, &tb, dt, esz, g.b, cv.C, cv.K[0] * cv.K[1] * cv.K[2], cv.Cout, cv.w_sp, cv.w_sco, 64, 1, CU_TENSOR_MAP_SWIZZLE_128B, n_local);
   } else if (!b_mn) {
     const uint64_t b_sn = g.N > 1 ? g.b_sn : pad16(g.K);
     rc = encode_tmap(c, &tb, dt, esz, g.b, g.K, g.N, b_bcast ? 1 : g.batch, b_sn, b_bcast ? b_sn * g.N : g.b_sb, block_k, n_local);
@@ -1347,16 +1298,16 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
   if (g.q == 1) p.q_nsub = 128u / g.q_bk;
   if (g.conv) {
     const ConvGeom& cv = *g.conv;
-    p.cv_ohw = (uint32_t)(cv.OH * cv.OW); p.cv_ow = (uint32_t)cv.OW;
-    p.cv_cblk = (uint32_t)((cv.C + 63) / 64); p.cv_kw = (uint32_t)cv.KW;
-    p.cv_stride_h = cv.sh; p.cv_stride_w = cv.sw; p.cv_pad_h = cv.ph; p.cv_pad_w = cv.pw;
-    p.cv_dil_h = (uint32_t)cv.dh; p.cv_dil_w = (uint32_t)cv.dw;
-    p.dx_sn = cv.dx_sn; p.dx_si = cv.dx_si; p.dx_sj = cv.dx_sj;
+    p.cv_ohw = (uint32_t)(cv.O[1] * cv.O[2]); p.cv_ow = (uint32_t)cv.O[2];
+    p.cv_cblk = (uint32_t)((cv.C + 63) / 64); p.cv_kw = (uint32_t)cv.K[2];
+    p.cv_stride_h = cv.s[1]; p.cv_stride_w = cv.s[2]; p.cv_pad_h = cv.p[1]; p.cv_pad_w = cv.p[2];
+    p.cv_dil_h = (uint32_t)cv.d[1]; p.cv_dil_w = (uint32_t)cv.d[2];
+    p.dx_sn = cv.dx_sn; p.dx_si = cv.dx_s[1]; p.dx_sj = cv.dx_s[2];
     p.dw_sp = cv.dw_sp; p.dw_c = (uint32_t)cv.dw_c;
-    if (cv.dims == 3) {
-      p.cv_odhw = (uint32_t)(cv.OD * cv.OH * cv.OW); p.cv_khw = (uint32_t)(cv.KH * cv.KW);
-      p.cv_stride_d = cv.sd; p.cv_pad_d = cv.pd; p.cv_dil_d = (uint32_t)cv.dd;
-      p.dx_sd = cv.dx_sd;
+    if (cv.n == 3) {   // the depth fields stay zero for 2-D
+      p.cv_odhw = (uint32_t)(cv.O[0] * cv.O[1] * cv.O[2]); p.cv_khw = (uint32_t)(cv.K[1] * cv.K[2]);
+      p.cv_stride_d = cv.s[0]; p.cv_pad_d = cv.p[0]; p.cv_dil_d = (uint32_t)cv.d[0];
+      p.dx_sd = cv.dx_s[0];
     }
   }
   p.q_ga = g.q_ga; p.q_gb = g.q_gb;
@@ -1384,7 +1335,7 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
     // dw as (C, Cout, KD * KH * KW): a staging tile of 64-column chunk (kpos, ch0) lands at (ch0, co, kpos), clipped at C
     const ConvGeom& cv = *g.conv;
     rc = encode_tmap(c, &tout, osz == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_UINT16, osz, g.out, cv.dw_c, g.M,
-                     cv.KD * cv.KH * cv.KW, g.o_sm, cv.dw_sp, static_cast<uint32_t>(128 / osz), 64);
+                     cv.K[0] * cv.K[1] * cv.K[2], g.o_sm, cv.dw_sp, static_cast<uint32_t>(128 / osz), 64);
     if (rc) return rc;
     p.tma_store = 1;
   } else if (cmode == 0 && p.vec_store && epi == "tma" && g.o_sm * osz < lim40 && g.o_sb * osz < lim40 && (g.M == 1 || g.o_sm >= g.N)) {
@@ -2957,12 +2908,55 @@ extern "C" int b200_matmul_quantized(b200_ctx* c, b200_stream s, const b200_quan
   return rc;
 }
 
-// ------------------------------------------------------------------------------------------------ 2-D convolution
-// Strides of a rank-4 view with every extent-1 dimension given the stride a compact tensor would have there (the address of
+// ------------------------------------------------------------------------------------------------ convolution
+// b200_conv2d* and b200_conv3d* (and the transposed b200_conv_transpose2d / 3d) run one host path for n = 2 or 3 spatial
+// dimensions.  Tensors keep their rank n + 2 ([N, (D,) H, W, C] and [Cout, (KD,) KH, KW, C]); per-dimension arrays are
+// ordered (D, H, W), and a 2-D convolution has a unit depth there (extent 1, stride 1, pad 0, dilation 1), so products over
+// the three dimensions need no rank test.  What stays rank-specific: the kernels and their parameter blocks, and the tensor
+// map's im2col limits -- rank 4 takes pixel-box corners in [-128, 127]; rank 5 takes corners in [-16, 15] (cuda.h:
+// cuTensorMapEncodeIm2col) and im2col offsets in [0, 31] (5 bits each; PTX ISA, cp.async.bulk.tensor im2col mode).
+struct ConvNd {
+  int n;              // spatial dimensions: 2 or 3
+  const char* what;   // the entry point, for messages
+  int64_t s[3], p[3], d[3];    // stride, padding and dilation
+  uint64_t I[3], K[3], O[3];   // extents of the input (x, dx, or the transposed convolution's out), the kernel and the output
+  int first() const { return 3 - n; }          // the first dimension that exists
+  int dim(int i) const { return i + n - 2; }   // the tensor index of dimension i
+};
+
+// The description of a call from its args and the input and kernel extents of `in` / `w`; conv_check_shape fills O.
+static ConvNd conv_nd(const char* what, int n, const int64_t s[3], const int64_t p[3], const int64_t d[3], const uint64_t* in, const uint64_t* w) {
+  ConvNd cv{n, what, {s[0], s[1], s[2]}, {p[0], p[1], p[2]}, {d[0], d[1], d[2]}, {1, 1, 1}, {1, 1, 1}, {1, 0, 0}};
+  if (n == 3) cv.O[0] = 0;
+  for (int i = cv.first(); i < 3; ++i) { cv.I[i] = in[cv.dim(i)]; cv.K[i] = w[cv.dim(i)]; }
+  return cv;
+}
+static ConvNd conv_nd(const char* what, const b200_conv2d_args& a, const uint64_t* in, const uint64_t* w) {
+  const int64_t s[3] = {1, a.stride_h, a.stride_w}, p[3] = {0, a.pad_h, a.pad_w}, d[3] = {1, a.dilation_h, a.dilation_w};
+  return conv_nd(what, 2, s, p, d, in, w);
+}
+static ConvNd conv_nd(const char* what, const b200_conv3d_args& a, const uint64_t* in, const uint64_t* w) {
+  const int64_t s[3] = {a.stride_d, a.stride_h, a.stride_w}, p[3] = {a.pad_d, a.pad_h, a.pad_w};
+  const int64_t d[3] = {a.dilation_d, a.dilation_h, a.dilation_w};
+  return conv_nd(what, 3, s, p, d, in, w);
+}
+
+// The names of the dimensions that exist, each after `prefix`, joined by `sep`: ("O", " * ") gives "OH * OW" or "OD * OH * OW".
+static std::string conv_names(const ConvNd& cv, const char* prefix, const char* sep) {
+  static const char* const dhw[3] = {"D", "H", "W"};
+  std::string t;
+  for (int i = cv.first(); i < 3; ++i) t += (i > cv.first() ? sep : "") + std::string(prefix) + dhw[i];
+  return t;
+}
+
+static uint64_t conv_prod(const uint64_t e[3]) { return e[0] * e[1] * e[2]; }
+static bool conv_any0(const uint64_t e[3]) { return e[0] == 0 || e[1] == 0 || e[2] == 0; }
+
+// Strides of a rank-r view with every extent-1 dimension given the stride a compact tensor would have there (the address of
 // its only index is unchanged), so layout tests do not trip over strides that are never used.
-static void conv_norm_strides(const uint64_t* shape, const uint64_t* strides, uint64_t* out) {
+static void conv_norm_strides(int r, const uint64_t* shape, const uint64_t* strides, uint64_t* out) {
   uint64_t inner = 1;
-  for (int d = 3; d >= 0; --d) {
+  for (int d = r - 1; d >= 0; --d) {
     out[d] = strides ? strides[d] : inner;
     if (shape[d] == 1) out[d] = inner;
     inner = out[d] * shape[d];
@@ -2977,63 +2971,105 @@ static uint64_t conv_flat_stride(uint64_t outer, uint64_t inner, uint64_t s_oute
   return inner == 1 ? s_outer : (outer == 1 || s_outer == inner * s_inner) ? s_inner : 0;
 }
 
-// Checks every convolution entry point shares; what: the entry point, for messages.  The dtypes, the epilogue's activation,
-// the args, and the weights' channels w_c against the input channels of one group, in_c.
-static int conv_check_args(const char* what, b200_dtype in_dtype, b200_dtype out_dtype, const b200_conv2d_args& a, const b200_epilogue* ep,
-                           uint64_t in_c, uint64_t w_c) {
+// The spatial dimensions 1..n of a rank n + 2 view (normalised strides ns) as one strided dimension: its stride, or 0.
+static uint64_t conv_flat_spatial(int n, const uint64_t* shape, const uint64_t* ns) {
+  uint64_t st = ns[n], inner = shape[n];
+  for (int j = n - 1; j >= 1 && st; --j) {
+    st = conv_flat_stride(shape[j], inner, ns[j], st);
+    inner *= shape[j];
+  }
+  return st;
+}
+
+// Checks every convolution entry point shares: the dtypes, the epilogue's activation, strides / dilations >= 1 and padding
+// >= 0, and the weights' channels w_c against the input channels of one group, in_c.  The depth args come first (a 2-D
+// call's unit depth passes), so a 3-D call with a bad depth arg and a bad dtype reports the arg.
+static int conv_check_args(const ConvNd& cv, b200_dtype in_dtype, b200_dtype out_dtype, const b200_epilogue* ep, uint64_t in_c, uint64_t w_c) {
+  const char* what = cv.what;
+  auto bad_args = [&](int i0, int i1) {
+    for (int i = i0; i < i1; ++i)
+      if (cv.s[i] < 1 || cv.d[i] < 1 || cv.p[i] < 0) return true;
+    return false;
+  };
+  const char* args_msg = "%s: strides and dilations must be >= 1 and padding >= 0";
+  if (bad_args(0, 1)) return fail(B200_ERR_INVALID_ARG, args_msg, what);
   if (in_dtype != B200_F16 && in_dtype != B200_BF16)
     return fail(B200_ERR_UNSUPPORTED, "%s: input dtype %d unsupported (f16, bf16)", what, (int)in_dtype);
   if (out_dtype != in_dtype && out_dtype != B200_F32)
     return fail(B200_ERR_UNSUPPORTED, "%s: output dtype must equal the input dtype or be f32", what);
   if (ep && (ep->activation < 0 || ep->activation > 2)) return fail(B200_ERR_INVALID_ARG, "%s: unknown activation %d", what, ep->activation);
-  if (a.stride_h < 1 || a.stride_w < 1 || a.dilation_h < 1 || a.dilation_w < 1 || a.pad_h < 0 || a.pad_w < 0)
-    return fail(B200_ERR_INVALID_ARG, "%s: strides and dilations must be >= 1 and padding >= 0", what);
+  if (bad_args(1, 3)) return fail(B200_ERR_INVALID_ARG, args_msg, what);
   if (w_c != in_c)
     return fail(B200_ERR_INVALID_ARG, "%s: weights have %llu channels, the input has %llu", what, (unsigned long long)w_c, (unsigned long long)in_c);
   return B200_OK;
 }
 
-// Extents < 2^31, then PyTorch's output rule for the input [N, H, W, C] and weights [Cout, KH, KW, *]: y (the forward's out
-// or a gradient's dy, y_name in messages) must be [N, OH, OW, Cout].  An empty kernel has no output extent to check.
-static int conv_check_shape(const char* what, const b200_conv2d_args& a, const uint64_t* in, const uint64_t* w, const uint64_t* y,
-                            const char* y_name, uint64_t* OH, uint64_t* OW) {
+// Extents < 2^31, then PyTorch's output rule per dimension for the input `in` and weights w [Cout, *K, *]: y (the forward's
+// out or a gradient's dy, y_name in messages) must be [N, *O, Cout]; cv->O receives O.  An empty kernel has no output extent
+// to check.
+static int conv_check_shape(ConvNd* cv, const uint64_t* in, const uint64_t* w, const uint64_t* y, const char* y_name) {
+  const char* what = cv->what;
+  const int r = cv->n + 2;
   const uint64_t lim = 1ull << 31;
-  for (int d = 0; d < 4; ++d)
+  for (int d = 0; d < r; ++d)
     if (in[d] >= lim || w[d] >= lim || y[d] >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: extents must be < 2^31", what);
-  const int64_t KH = (int64_t)w[1], KW = (int64_t)w[2];
-  if (KH == 0 || KW == 0) return B200_OK;
-  const int64_t nh = (int64_t)in[1] + 2 * (int64_t)a.pad_h - (int64_t)a.dilation_h * (KH - 1) - 1;
-  const int64_t nw = (int64_t)in[2] + 2 * (int64_t)a.pad_w - (int64_t)a.dilation_w * (KW - 1) - 1;
-  if (nh < 0 || nw < 0)
-    return fail(B200_ERR_INVALID_ARG, "%s: the dilated kernel is larger than the padded input (output extent < 1)", what);
-  *OH = (uint64_t)(nh / a.stride_h) + 1;
-  *OW = (uint64_t)(nw / a.stride_w) + 1;
-  if (y[0] != in[0] || y[1] != *OH || y[2] != *OW || y[3] != w[0])
-    return fail(B200_ERR_INVALID_ARG, "%s: %s is [%llu,%llu,%llu,%llu], expected [%llu,%llu,%llu,%llu]", what, y_name, (unsigned long long)y[0],
-                (unsigned long long)y[1], (unsigned long long)y[2], (unsigned long long)y[3], (unsigned long long)in[0],
-                (unsigned long long)*OH, (unsigned long long)*OW, (unsigned long long)w[0]);
+  if (conv_any0(cv->K)) return B200_OK;
+  for (int i = cv->first(); i < 3; ++i) {
+    const int64_t e = (int64_t)cv->I[i] + 2 * cv->p[i] - cv->d[i] * ((int64_t)cv->K[i] - 1) - 1;
+    if (e < 0) return fail(B200_ERR_INVALID_ARG, "%s: the dilated kernel is larger than the padded input (output extent < 1)", what);
+    cv->O[i] = (uint64_t)(e / cv->s[i]) + 1;
+  }
+  bool ok = y[0] == in[0] && y[r - 1] == w[0];
+  for (int i = cv->first(); i < 3; ++i) ok = ok && y[cv->dim(i)] == cv->O[i];
+  if (ok) return B200_OK;
+  std::string got, want = std::to_string(in[0]);
+  for (int d = 0; d < r; ++d) got += (d ? "," : "") + std::to_string(y[d]);
+  for (int i = cv->first(); i < 3; ++i) want += "," + std::to_string(cv->O[i]);
+  want += "," + std::to_string(w[0]);
+  return fail(B200_ERR_INVALID_ARG, "%s: %s is [%s], expected [%s]", what, y_name, got.c_str(), want.c_str());
+}
+
+// The im2col limits of the map's rank for a pixel box with corners lo / up and largest im2col offsets off (dilation *
+// (taps - 1)) per dimension.  Rank 4 checks the corners in the order (lo_h, lo_w, up_h, up_w); rank 5 per dimension
+// (lo, up), then the offsets.
+static int conv_check_box(const ConvNd& cv, const int64_t lo[3], const int64_t up[3], const int64_t off[3]) {
+  const char* what = cv.what;
+  int64_t corners[6];
+  int k = 0;
+  if (cv.n == 2) {
+    for (int i = 1; i < 3; ++i) corners[k++] = lo[i];
+    for (int i = 1; i < 3; ++i) corners[k++] = up[i];
+  } else {
+    for (int i = 0; i < 3; ++i) { corners[k++] = lo[i]; corners[k++] = up[i]; }
+  }
+  const int64_t cmin = cv.n == 2 ? -128 : -16, cmax = cv.n == 2 ? 127 : 15;
+  for (int j = 0; j < k; ++j)
+    if (corners[j] < cmin || corners[j] > cmax)
+      return fail(B200_ERR_UNSUPPORTED, "%s: im2col pixel-box corner %lld outside [%lld, %lld]%s", what, (long long)corners[j], (long long)cmin,
+                  (long long)cmax, cv.n == 3 ? " (rank-5 tensor map)" : "");
+  if (cv.n == 3)
+    for (int i = 0; i < 3; ++i)
+      if (off[i] > 31)
+        return fail(B200_ERR_UNSUPPORTED, "%s: im2col offset dilation * (kernel - 1) = %lld exceeds 31 (5-bit rank-5 offsets)", what,
+                    (long long)off[i]);
   return B200_OK;
 }
 
-// The 4-D im2col limits of the tensor map (cuda.h: cuTensorMapEncodeIm2col): pixel-box corners in [-128, 127] ...
-static int conv_check_corners(const char* what, const int64_t corners[4]) {
-  for (int i = 0; i < 4; ++i)
-    if (corners[i] < -128 || corners[i] > 127)
-      return fail(B200_ERR_UNSUPPORTED, "%s: im2col pixel-box corner %lld outside [-128, 127]", what, (long long)corners[i]);
-  return B200_OK;
+// The forward's map (also the weight gradient's x): corners -pad and pad - dilation * (kernel - 1).
+static int conv_check_fwd(const ConvNd& cv) {
+  int64_t lo[3], up[3], off[3];
+  for (int i = 0; i < 3; ++i) {
+    off[i] = cv.d[i] * ((int64_t)cv.K[i] - 1);
+    lo[i] = -cv.p[i];
+    up[i] = cv.p[i] - off[i];
+  }
+  return conv_check_box(cv, lo, up, off);
 }
 
-// ... with the forward's corners -pad and pad - dilation * (kernel - 1) ...
-static int conv_check_fwd_corners(const char* what, const b200_conv2d_args& a, uint64_t KH, uint64_t KW) {
-  const int64_t corners[4] = {-(int64_t)a.pad_h, -(int64_t)a.pad_w, (int64_t)a.pad_h - (int64_t)a.dilation_h * ((int64_t)KH - 1),
-                              (int64_t)a.pad_w - (int64_t)a.dilation_w * ((int64_t)KW - 1)};
-  return conv_check_corners(what, corners);
-}
-
-// ... and an element stride (the conv stride) <= 8, which also bounds the data gradient's phases per dimension.
-static int conv_check_stride(const char* what, const b200_conv2d_args& a) {
-  if (a.stride_h > kDgradMaxStride || a.stride_w > kDgradMaxStride)
-    return fail(B200_ERR_UNSUPPORTED, "%s: the conv stride must be <= %d", what, kDgradMaxStride);
+// An element stride (the conv stride) <= 8, which also bounds the data gradient's phases per dimension.
+static int conv_check_stride(const ConvNd& cv) {
+  if (cv.s[0] > kDgradMaxStride || cv.s[1] > kDgradMaxStride || cv.s[2] > kDgradMaxStride)
+    return fail(B200_ERR_UNSUPPORTED, "%s: the conv stride must be <= %d", cv.what, kDgradMaxStride);
   return B200_OK;
 }
 
@@ -3044,19 +3080,25 @@ static int conv_check_ptrs(const char* what, uint64_t a, uint64_t b, uint64_t ou
   return B200_OK;
 }
 
-// An NHWC output (out or dx; normalised strides ns): unit channel stride, and one pixel pitch >= its channels for N, H, W.
-static int conv_check_pixels(const char* what, const char* name, const uint64_t* shape, const uint64_t* ns) {
-  if (ns[3] != 1 || ns[2] < shape[3] || ns[1] != shape[2] * ns[2] || ns[0] != shape[1] * ns[1])
-    return fail(B200_ERR_UNSUPPORTED, "%s: %s must have unit channel stride and one pixel pitch >= its channels for N, H, W", what, name);
+// An N(D)HWC output (out or dx; normalised strides ns): unit channel stride, and one pixel pitch >= its channels for N and
+// every spatial dimension.
+static int conv_check_pixels(const ConvNd& cv, const char* name, const uint64_t* shape, const uint64_t* ns) {
+  const int n = cv.n;
+  bool ok = ns[n + 1] == 1 && ns[n] >= shape[n + 1];
+  for (int j = 0; j < n; ++j) ok = ok && ns[j] == shape[j + 1] * ns[j + 1];
+  if (!ok)
+    return fail(B200_ERR_UNSUPPORTED, "%s: %s must have unit channel stride and one pixel pitch >= its channels for N, %s", cv.what, name,
+                conv_names(cv, "", ", ").c_str());
   return B200_OK;
 }
 
-// dw [Cout, KH, KW, C'] (normalised strides ds): unit channel stride, (KH, KW) flattening into one kernel-position stride
-// (*dw_sp), and an output-channel stride.
-static int conv_check_dw(const char* what, const uint64_t* shape, const uint64_t* ds, size_t osz, uint64_t* dw_sp) {
-  *dw_sp = conv_flat_stride(shape[1], shape[2], ds[1], ds[2]);
-  if (ds[3] != 1 || *dw_sp == 0 || ds[0] * osz >= (1ull << 40) || *dw_sp * osz >= (1ull << 40))
-    return fail(B200_ERR_UNSUPPORTED, "%s: dw must have unit channel stride and (KH, KW) flattening into one stride", what);
+// dw [Cout, *K, C'] (normalised strides ds): unit channel stride, the kernel dimensions flattening into one kernel-position
+// stride (*dw_sp), and an output-channel stride.
+static int conv_check_dw(const ConvNd& cv, const uint64_t* shape, const uint64_t* ds, size_t osz, uint64_t* dw_sp) {
+  *dw_sp = conv_flat_spatial(cv.n, shape, ds);
+  if (ds[cv.n + 1] != 1 || *dw_sp == 0 || ds[0] * osz >= (1ull << 40) || *dw_sp * osz >= (1ull << 40))
+    return fail(B200_ERR_UNSUPPORTED, "%s: dw must have unit channel stride and (%s) flattening into one stride", cv.what,
+                conv_names(cv, "K", ", ").c_str());
   return B200_OK;
 }
 
@@ -3080,53 +3122,62 @@ static int conv_pad_channels(b200_ctx* c, CUstream st, uint64_t in, uint64_t bat
   return B200_OK;
 }
 
-// A compact pooled copy of a rank-4 view (b200_into_contiguous).
-static int conv_gather(b200_ctx* c, CUstream st, b200_dtype dt, uint64_t in, const uint64_t* shape, const uint64_t* strides,
+// A compact pooled copy of a rank-r view (b200_into_contiguous).
+static int conv_gather(b200_ctx* c, CUstream st, b200_dtype dt, uint64_t in, int r, const uint64_t* shape, const uint64_t* strides,
                        CUdeviceptr* out) {
   CUdeviceptr buf;
-  int rc = pool_alloc(c, shape[0] * shape[1] * shape[2] * shape[3] * 2, &buf, st);
+  uint64_t elems = 1;
+  for (int d = 0; d < r; ++d) elems *= shape[d];
+  int rc = pool_alloc(c, elems * 2, &buf, st);
   if (rc) return rc;
-  rc = b200_into_contiguous(c, static_cast<b200_stream>(st), dt, in, buf, 4, shape, strides);
+  rc = b200_into_contiguous(c, static_cast<b200_stream>(st), dt, in, buf, r, shape, strides);
   if (rc) { pool_free(c, buf, st); return rc; }
   *out = buf;
   return B200_OK;
 }
 
-// An operand [N, H, W, C] (normalised strides `ns`) as the convolution maps read it: unit channel stride, 16-byte aligned base
-// and strides, channels a multiple of 8.  A view that does not qualify is gathered into a compact pooled copy; channel counts
-// that are not multiples of 8 are copied with the channels padded to 8 zeros.  flat: the leading dimensions the map reads
-// as one strided dimension -- none (x, and dy in the data gradient), (H, W) (the forward's weights: one kernel-position
-// dimension, returned as s_w) or (N, H, W) (dy in the weight gradient: [pixels, Cout]).  tmp[0] / tmp[1] receive the pooled
-// copies (the caller frees them).
-struct NhwcOperand {
-  uint64_t ptr, C, s_w, s_h, s_n;
+// An operand [N, (D,) H, W, C] (normalised strides `ns`) as the convolution maps read it: unit channel stride, 16-byte aligned
+// base and strides, channels a multiple of 8.  A view that does not qualify is gathered into a compact pooled copy; channel
+// counts that are not multiples of 8 are copied with the channels padded to 8 zeros.  flat: the leading dimensions the map
+// reads as one strided dimension -- none (x, and dy in the data gradient), the spatial ones (the forward's weights: one
+// kernel-position dimension, returned as s_w) or N and the spatial ones (dy in the weight gradient: [pixels, Cout]).  s_d is
+// 0 for 2-D.  tmp[0] / tmp[1] receive the pooled copies (the caller frees them).
+struct ConvOperand {
+  uint64_t ptr, C, s_w, s_h, s_d, s_n;
 };
-enum ConvFlat { kFlatNone, kFlatHW, kFlatNHW };
-static int conv_prep_nhwc(b200_ctx* c, CUstream st, b200_dtype dt, uint64_t ptr, const uint64_t* shape, const uint64_t* ns, ConvFlat flat,
-                          CUdeviceptr tmp[2], NhwcOperand* o) {
-  const uint64_t N = shape[0], H = shape[1], W = shape[2], C = shape[3];
-  const uint64_t spx = conv_flat_stride(H, W, ns[1], ns[2]);   // (H, W) as one pixel dimension
+enum ConvFlat { kFlatNone, kFlatSpatial, kFlatAll };
+static int conv_prep(b200_ctx* c, CUstream st, b200_dtype dt, int n, uint64_t ptr, const uint64_t* shape, const uint64_t* ns, ConvFlat flat,
+                     CUdeviceptr tmp[2], ConvOperand* o) {
+  const uint64_t N = shape[0], H = shape[n - 1], W = shape[n], C = shape[n + 1];
+  uint64_t px = 1;
+  for (int j = 1; j <= n; ++j) px *= shape[j];
+  auto compact = [&](uint64_t base, uint64_t cc) { return ConvOperand{base, cc, cc, W * cc, n == 3 ? H * W * cc : 0, px * cc}; };
+  const uint64_t spx = conv_flat_spatial(n, shape, ns);   // the spatial dimensions as one pixel dimension
   int rc = B200_OK;
   if (C % 8 == 0) {
-    bool in_place = ptr % 16 == 0 && ns[3] == 1 && conv_al16(ns[0]);
-    if (flat == kFlatHW) in_place = in_place && spx != 0 && conv_al16(spx);
-    else in_place = in_place && conv_al16(ns[1]) && conv_al16(ns[2]) && (flat == kFlatNone || (ns[1] == W * ns[2] && ns[0] == H * ns[1]));
+    bool in_place = ptr % 16 == 0 && ns[n + 1] == 1 && conv_al16(ns[0]);
+    if (flat == kFlatSpatial) {
+      in_place = in_place && spx != 0 && conv_al16(spx);
+    } else {
+      for (int j = 1; j <= n; ++j) in_place = in_place && conv_al16(ns[j]);
+      for (int j = 0; j < n && flat == kFlatAll; ++j) in_place = in_place && ns[j] == shape[j + 1] * ns[j + 1];
+    }
     if (in_place) {
-      *o = {ptr, C, flat == kFlatHW ? spx : ns[2], ns[1], ns[0]};
+      *o = {ptr, C, flat == kFlatSpatial ? spx : ns[n], ns[n - 1], n == 3 ? ns[1] : 0, ns[0]};
       return B200_OK;
     }
-    rc = conv_gather(c, st, dt, ptr, shape, ns, &tmp[0]);
-    *o = {tmp[0], C, C, W * C, H * W * C};
+    rc = conv_gather(c, st, dt, ptr, n + 2, shape, ns, &tmp[0]);
+    *o = compact(tmp[0], C);
     return rc;
   }
   const uint64_t cp = (C + 7) / 8 * 8;
-  uint64_t in = ptr, sb = ns[0], sp = spx, sc = ns[3];
+  uint64_t in = ptr, sb = ns[0], sp = spx, sc = ns[n + 1];
   if (spx == 0) {
-    rc = conv_gather(c, st, dt, ptr, shape, ns, &tmp[0]);
-    in = tmp[0]; sb = H * W * C; sp = C; sc = 1;
+    rc = conv_gather(c, st, dt, ptr, n + 2, shape, ns, &tmp[0]);
+    in = tmp[0]; sb = px * C; sp = C; sc = 1;
   }
-  if (!rc) rc = conv_pad_channels(c, st, in, N, H * W, C, sb, sp, sc, cp, &tmp[1]);
-  *o = {tmp[1], cp, cp, W * cp, H * W * cp};
+  if (!rc) rc = conv_pad_channels(c, st, in, N, px, C, sb, sp, sc, cp, &tmp[1]);
+  *o = compact(tmp[1], cp);
   return rc;
 }
 
@@ -3144,43 +3195,55 @@ static GemmProblem conv_problem(b200_dtype in_dtype, b200_dtype out_dtype, uint6
   return gp;
 }
 
-extern "C" int b200_conv2d(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr x, const uint64_t* x_shape,
-                           const uint64_t* x_strides, b200_dptr w, const uint64_t* w_shape, const uint64_t* w_strides, b200_dptr out,
-                           const uint64_t* out_shape, const uint64_t* out_strides, const b200_conv2d_args* args, const b200_epilogue* ep) {
-  CTX_ENTER(c);
-  const char* what = "conv2d";
-  if (!x_shape || !w_shape || !out_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
-  const b200_conv2d_args& a = *args;
-  const uint64_t N = x_shape[0], H = x_shape[1], W = x_shape[2], C = x_shape[3];
-  const uint64_t Cout = w_shape[0], KH = w_shape[1], KW = w_shape[2];
-  int rc = conv_check_args(what, in_dtype, out_dtype, a, ep, C, w_shape[3]);
+// ConvGeom of the map that reads x (operand xo, extents I) with kernel K into the output extents O.
+static ConvGeom conv_geom(int n, uint64_t N, const uint64_t I[3], const ConvOperand& xo, const uint64_t K[3], const uint64_t O[3], uint64_t Cout) {
+  ConvGeom g{};
+  g.n = n; g.N = N; g.C = xo.C; g.Cout = Cout;
+  for (int i = 0; i < 3; ++i) { g.I[i] = I[i]; g.K[i] = K[i]; g.O[i] = O[i]; }
+  g.x_s[0] = xo.s_d; g.x_s[1] = xo.s_h; g.x_s[2] = xo.s_w; g.x_sn = xo.s_n;
+  return g;
+}
+static void conv_geom_args(const ConvNd& cv, ConvGeom* g) {
+  for (int i = 0; i < 3; ++i) { g->s[i] = (int32_t)cv.s[i]; g->p[i] = (int32_t)cv.p[i]; g->d[i] = (int32_t)cv.d[i]; }
+}
+
+static void conv_set_epilogue(GemmProblem* gp, const b200_epilogue* ep) {
+  if (ep) { gp->alpha = ep->alpha; gp->bias = ep->bias; gp->act = (uint32_t)ep->activation; }
+}
+
+// b200_conv2d / b200_conv3d: x [N, *I, C], w [Cout, *K, C], out [N, *O, Cout].
+static int conv_forward(b200_ctx* c, b200_stream s, ConvNd cv, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr x, const uint64_t* x_shape,
+                        const uint64_t* x_strides, b200_dptr w, const uint64_t* w_shape, const uint64_t* w_strides, b200_dptr out,
+                        const uint64_t* out_shape, const uint64_t* out_strides, const b200_epilogue* ep) {
+  const char* what = cv.what;
+  const int n = cv.n, r = n + 2;
+  const uint64_t N = x_shape[0], C = x_shape[r - 1], Cout = w_shape[0];
+  int rc = conv_check_args(cv, in_dtype, out_dtype, ep, C, w_shape[r - 1]);
   if (rc) return rc;
-  if (N == 0 || H == 0 || W == 0 || C == 0 || Cout == 0 || KH == 0 || KW == 0) return B200_OK;
-  uint64_t OH = 0, OW = 0;
-  if ((rc = conv_check_shape(what, a, x_shape, w_shape, out_shape, "out", &OH, &OW))) return rc;
-  if ((rc = conv_check_fwd_corners(what, a, KH, KW)) || (rc = conv_check_stride(what, a))) return rc;
-  const uint64_t M = N * OH * OW, lim = 1ull << 31;
-  if (M >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * OH * OW = %llu must be < 2^31", what, (unsigned long long)M);
+  if (N == 0 || conv_any0(cv.I) || C == 0 || Cout == 0 || conv_any0(cv.K)) return B200_OK;
+  if ((rc = conv_check_shape(&cv, x_shape, w_shape, out_shape, "out"))) return rc;
+  if ((rc = conv_check_fwd(cv)) || (rc = conv_check_stride(cv))) return rc;
+  const uint64_t M = N * conv_prod(cv.O), lim = 1ull << 31, KK = conv_prod(cv.K);
+  if (M >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * %s = %llu must be < 2^31", what, conv_names(cv, "O", " * ").c_str(), (unsigned long long)M);
   if ((rc = conv_check_ptrs(what, x, w, out, "output", out_dtype))) return rc;
-  uint64_t os[4], xs[4], ws[4];
-  conv_norm_strides(out_shape, out_strides, os);
-  if ((rc = conv_check_pixels(what, "out", out_shape, os))) return rc;
-  if (KH * KW * ((C + 63) / 64 * 64) >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: KH * KW * C (C padded to 64) must be < 2^31", what);
+  uint64_t os[5], xs[5], ws[5];
+  conv_norm_strides(r, out_shape, out_strides, os);
+  if ((rc = conv_check_pixels(cv, "out", out_shape, os))) return rc;
+  if (KK * ((C + 63) / 64 * 64) >= lim)
+    return fail(B200_ERR_UNSUPPORTED, "%s: %s * C (C padded to 64) must be < 2^31", what, conv_names(cv, "K", " * ").c_str());
   CUstream st = resolve_stream(c, s);
-  conv_norm_strides(x_shape, x_strides, xs);
-  conv_norm_strides(w_shape, w_strides, ws);
+  conv_norm_strides(r, x_shape, x_strides, xs);
+  conv_norm_strides(r, w_shape, w_strides, ws);
   CUdeviceptr tmp[4] = {0, 0, 0, 0};
-  NhwcOperand xo{}, wo{};
-  rc = conv_prep_nhwc(c, st, in_dtype, x, x_shape, xs, kFlatNone, &tmp[0], &xo);
-  if (!rc) rc = conv_prep_nhwc(c, st, in_dtype, w, w_shape, ws, kFlatHW, &tmp[2], &wo);
+  ConvOperand xo{}, wo{};
+  rc = conv_prep(c, st, in_dtype, n, x, x_shape, xs, kFlatNone, &tmp[0], &xo);
+  if (!rc) rc = conv_prep(c, st, in_dtype, n, w, w_shape, ws, kFlatSpatial, &tmp[2], &wo);
   if (!rc) {
-    ConvGeom g{};
-    g.N = N; g.H = H; g.W = W; g.C = xo.C; g.KH = KH; g.KW = KW; g.OH = OH; g.OW = OW; g.Cout = Cout;
-    g.sh = a.stride_h; g.sw = a.stride_w; g.ph = a.pad_h; g.pw = a.pad_w; g.dh = a.dilation_h; g.dw = a.dilation_w;
-    g.x_sw = xo.s_w; g.x_sh = xo.s_h; g.x_sn = xo.s_n;
+    ConvGeom g = conv_geom(n, N, cv.I, xo, cv.K, cv.O, Cout);
+    conv_geom_args(cv, &g);
     g.w_sp = wo.s_w; g.w_sco = wo.s_n;
-    GemmProblem gp = conv_problem(in_dtype, out_dtype, xo.ptr, wo.ptr, out, M, Cout, KH * KW * ((g.C + 63) / 64 * 64), os[2], &g);
-    if (ep) { gp.alpha = ep->alpha; gp.bias = ep->bias; gp.act = (uint32_t)ep->activation; }
+    GemmProblem gp = conv_problem(in_dtype, out_dtype, xo.ptr, wo.ptr, out, M, Cout, KK * ((g.C + 63) / 64 * 64), os[n], &g);
+    conv_set_epilogue(&gp, ep);
     rc = launch_wgmma(c, st, gp, false, false);
   }
   for (CUdeviceptr t : tmp)
@@ -3235,187 +3298,231 @@ static std::string dgrad_taps(const DgradPhase1D& q) {
   return s;
 }
 
-// The 2-D data gradient's phases (also b200_conv_transpose2d's, x in dy's role): per dimension, and the im2col corner
-// limits of every phase that runs.  dx is [N, H, W, *] from dy [N, OH, OW, Cout]; *zero_phase: a phase with pixels receives
-// no tap (or Cout == 0).
-static int dgrad2_plan(const char* what, const b200_conv2d_args& a, uint64_t H, uint64_t W, uint64_t KH, uint64_t KW, uint64_t OH,
-                       uint64_t OW, uint64_t Cout, std::vector<DgradPhase1D>* phs, std::vector<DgradPhase1D>* pws, bool* zero_phase) {
-  for (int r = 0; r < a.stride_h; ++r) phs->push_back(dgrad_phase(H, KH, a.stride_h, a.pad_h, a.dilation_h, (uint32_t)r));
-  for (int r = 0; r < a.stride_w; ++r) pws->push_back(dgrad_phase(W, KW, a.stride_w, a.pad_w, a.dilation_w, (uint32_t)r));
-  *zero_phase = false;
-  for (const DgradPhase1D& ph : *phs)
-    for (const DgradPhase1D& pw : *pws) {
-      if (!ph.extent || !pw.extent) continue;
-      if (!ph.taps || !pw.taps || Cout == 0) { *zero_phase = true; continue; }
-      const int64_t corners[4] = {ph.e0, pw.e0, ph.e0 + (int64_t)ph.extent - (int64_t)OH, pw.e0 + (int64_t)pw.extent - (int64_t)OW};
-      int rc = conv_check_corners(what, corners);
-      if (rc) return rc;
+// The data gradient's phases (also the transposed convolution's, x in dy's role): per dimension (D, H, W) of dx (extents
+// cv.I) from dy (extents cv.O); a 2-D plan has one unit depth phase.  A phase of the layer is one phase per dimension,
+// q[0..2], taken in (D, H, W) order.
+struct ConvPhases {
+  std::vector<DgradPhase1D> q[3];
+  bool zero_phase = false;   // a phase with pixels receives no tap (or there are no output channels)
+  uint64_t pre[3][kDgradMaxStride];   // the taps of the phases before r, per dimension
+  uint64_t KH, KW;
+  // The prep kernels write every phase's flipped, channel-transposed weights [C][Td][Th][Tw][cp] into one buffer, blocks in
+  // (rd, rh, rw) order.  As the phases of a dimension partition its taps, block q starts at this element times C * cp.
+  uint64_t off(const DgradPhase1D* const q3[3]) const {
+    return pre[0][q3[0]->r] * KH * KW + (uint64_t)q3[0]->taps * (pre[1][q3[1]->r] * KW + (uint64_t)q3[1]->taps * pre[2][q3[2]->r]);
+  }
+  // f(q) for every phase of the layer, in order, until f returns non-zero
+  template <class F> int each(F f) const {
+    for (const DgradPhase1D& a : q[0])
+      for (const DgradPhase1D& b : q[1])
+        for (const DgradPhase1D& c : q[2]) {
+          const DgradPhase1D* q3[3] = {&a, &b, &c};
+          if (int rc = f(q3)) return rc;
+        }
+    return B200_OK;
+  }
+};
+
+// The phase plan, and the im2col limits of every phase that runs.
+static int conv_phase_plan(const ConvNd& cv, uint64_t Cout, ConvPhases* ph) {
+  for (int i = 0; i < 3; ++i) {
+    uint64_t acc = 0;
+    for (int64_t r = 0; r < cv.s[i]; ++r) {
+      ph->q[i].push_back(dgrad_phase(cv.I[i], cv.K[i], cv.s[i], cv.p[i], cv.d[i], (uint32_t)r));
+      ph->pre[i][r] = acc;
+      acc += ph->q[i].back().taps;
     }
-  return B200_OK;
+  }
+  ph->KH = cv.K[1]; ph->KW = cv.K[2];
+  return ph->each([&](const DgradPhase1D* const* q) -> int {
+    if (!q[0]->extent || !q[1]->extent || !q[2]->extent) return B200_OK;
+    if (!q[0]->taps || !q[1]->taps || !q[2]->taps || Cout == 0) { ph->zero_phase = true; return B200_OK; }
+    int64_t lo[3], up[3], off[3];
+    for (int i = 0; i < 3; ++i) {
+      lo[i] = q[i]->e0;
+      up[i] = q[i]->e0 + (int64_t)q[i]->extent - (int64_t)cv.O[i];
+      off[i] = (int64_t)(q[i]->taps - 1) * q[i]->dil;
+    }
+    return conv_check_box(cv, lo, up, off);
+  });
 }
 
-// Every phase's flipped, channel-transposed weights [C][Th][Tw][cp] in one pooled buffer (*buf) of KH * KW * C * cp
-// elements, written by conv_dgrad_weights from w [Cout, KH, KW, C] (strides ws); wp->off holds each phase's block.
-static int dgrad2_prep(b200_ctx* c, CUstream st, uint64_t w, const uint64_t ws[4], const b200_conv2d_args& a, uint64_t C, uint64_t Cout,
-                       uint64_t cp, uint64_t KH, uint64_t KW, const std::vector<DgradPhase1D>& phs, const std::vector<DgradPhase1D>& pws,
-                       CUdeviceptr* buf, ConvDgradWeightsParams* wp_out) {
-  ConvDgradWeightsParams& wp = *wp_out;
-  memset(&wp, 0, sizeof(wp));
-  int rc = pool_alloc(c, KH * KW * C * cp * 2, buf, st);
+// Every phase's weights from w [Cout, *K, C] (strides ws) into one pooled buffer (*buf) of |K| * C * cp elements, by
+// conv_dgrad_weights (2-D) or conv3d_dgrad_weights (3-D).
+static int conv_dgrad_weights(b200_ctx* c, CUstream st, const ConvNd& cv, const ConvPhases& ph, uint64_t w, const uint64_t* ws, uint64_t C,
+                              uint64_t Cout, uint64_t cp, CUdeviceptr* buf) {
+  const uint64_t KK = conv_prod(cv.K);
+  int rc = pool_alloc(c, KK * C * cp * 2, buf, st);
   if (rc) return rc;
-  wp.w = w; wp.out = *buf;
-  wp.s_co = ws[0]; wp.s_ky = ws[1]; wp.s_kx = ws[2]; wp.s_c = ws[3];
-  wp.C = C; wp.Cout = Cout; wp.cp = cp;
-  wp.KH = (uint32_t)KH; wp.KW = (uint32_t)KW; wp.sh = (uint32_t)a.stride_h; wp.sw = (uint32_t)a.stride_w;
-  wp.dh = (uint32_t)a.dilation_h; wp.dw = (uint32_t)a.dilation_w; wp.ph = (uint32_t)a.pad_h; wp.pw = (uint32_t)a.pad_w;
-  wp.qh = phs[0].step; wp.qw = pws[0].step;
-  uint64_t off = 0;
-  for (const DgradPhase1D& ph : phs)
-    for (const DgradPhase1D& pw : pws) {
-      wp.off[ph.r * a.stride_w + pw.r] = off;
-      off += (uint64_t)ph.taps * pw.taps * C * cp;
+  ConvDgradWeightsParams wp2;
+  Conv3dDgradWeightsParams wp3;
+  memset(&wp2, 0, sizeof(wp2));
+  memset(&wp3, 0, sizeof(wp3));
+  if (cv.n == 2) {
+    ConvDgradWeightsParams& wp = wp2;
+    wp.w = w; wp.out = *buf;
+    wp.s_co = ws[0]; wp.s_ky = ws[1]; wp.s_kx = ws[2]; wp.s_c = ws[3];
+    wp.C = C; wp.Cout = Cout; wp.cp = cp;
+    wp.KH = (uint32_t)cv.K[1]; wp.KW = (uint32_t)cv.K[2]; wp.sh = (uint32_t)cv.s[1]; wp.sw = (uint32_t)cv.s[2];
+    wp.dh = (uint32_t)cv.d[1]; wp.dw = (uint32_t)cv.d[2]; wp.ph = (uint32_t)cv.p[1]; wp.pw = (uint32_t)cv.p[2];
+    wp.qh = ph.q[1][0].step; wp.qw = ph.q[2][0].step;
+    ph.each([&](const DgradPhase1D* const* q) {
+      wp.off[q[1]->r * cv.s[2] + q[2]->r] = ph.off(q) * C * cp;
+      return B200_OK;
+    });
+    for (const DgradPhase1D& q : ph.q[1]) { wp.kmax_h[q.r] = q.kmax; wp.taps_h[q.r] = q.taps; }
+    for (const DgradPhase1D& q : ph.q[2]) { wp.kmax_w[q.r] = q.kmax; wp.taps_w[q.r] = q.taps; }
+  } else {
+    Conv3dDgradWeightsParams& wp = wp3;
+    wp.w = w; wp.out = *buf;
+    wp.s_co = ws[0]; wp.s_kz = ws[1]; wp.s_ky = ws[2]; wp.s_kx = ws[3]; wp.s_c = ws[4];
+    wp.C = C; wp.Cout = Cout; wp.cp = cp;
+    for (int i = 0; i < 3; ++i) {
+      for (const DgradPhase1D& q : ph.q[i]) { wp.kmax[i][q.r] = q.kmax; wp.taps[i][q.r] = q.taps; }
+      wp.k[i] = (uint32_t)cv.K[i]; wp.s[i] = (uint32_t)cv.s[i]; wp.d[i] = (uint32_t)cv.d[i]; wp.p[i] = (uint32_t)cv.p[i]; wp.q[i] = ph.q[i][0].step;
     }
-  for (const DgradPhase1D& ph : phs) { wp.kmax_h[ph.r] = ph.kmax; wp.taps_h[ph.r] = ph.taps; }
-  for (const DgradPhase1D& pw : pws) { wp.kmax_w[pw.r] = pw.kmax; wp.taps_w[pw.r] = pw.taps; }
+  }
   CUfunction f;
-  rc = get_func(c, "conv_dgrad_weights", &f);
-  void* kargs[] = {&wp};
-  if (!rc) rc = launch(c, f, (unsigned)(((C + 31) / 32) * ((cp + 31) / 32)), (unsigned)(KH * KW), 1, 256, 0, 1, st, kargs);
+  rc = get_func(c, cv.n == 3 ? "conv3d_dgrad_weights" : "conv_dgrad_weights", &f);
+  void* kargs[] = {cv.n == 3 ? (void*)&wp3 : (void*)&wp2};
+  if (!rc) rc = launch(c, f, (unsigned)(((C + 31) / 32) * ((cp + 31) / 32)), (unsigned)KK, 1, 256, 0, 1, st, kargs);
   return rc;
 }
 
-// One phase (ph, pw) as a stride-1 convolution of dy (read through y) into C channels: its geometry, with the phase-addressed
-// epilogue of dx (normalised strides os) unless the conv stride is 1.
-static ConvGeom dgrad2_geom(uint64_t N, uint64_t OH, uint64_t OW, uint64_t cp, uint64_t C, const DgradPhase1D& ph, const DgradPhase1D& pw,
-                            const NhwcOperand& y, const uint64_t os[4], const b200_conv2d_args& a) {
-  ConvGeom g{};
-  g.N = N; g.H = OH; g.W = OW; g.C = cp; g.KH = ph.taps; g.KW = pw.taps; g.OH = ph.extent; g.OW = pw.extent; g.Cout = C;
-  g.sh = 1; g.sw = 1; g.ph = (int32_t)-ph.e0; g.pw = (int32_t)-pw.e0; g.dh = (int32_t)ph.dil; g.dw = (int32_t)pw.dil;
-  g.x_sw = y.s_w; g.x_sh = y.s_h; g.x_sn = y.s_n;
-  g.w_sp = cp; g.w_sco = (uint64_t)ph.taps * pw.taps * cp;
-  g.box = true; g.lo_h = (int32_t)ph.e0; g.lo_w = (int32_t)pw.e0;
-  g.mode = a.stride_h == 1 && a.stride_w == 1 ? 0 : 1;
-  g.dx_sn = os[0]; g.dx_si = (uint64_t)a.stride_h * os[1]; g.dx_sj = (uint64_t)a.stride_w * os[2];
+// Phase q as a stride-1 convolution of dy (read through y, extents cv.O) into C channels: its geometry, with the
+// phase-addressed epilogue of dx (normalised strides os, rank n + 2) unless every conv stride is 1.
+static ConvGeom conv_phase_geom(const ConvNd& cv, uint64_t N, uint64_t C, const DgradPhase1D* const q[3], const ConvOperand& y, const uint64_t* os) {
+  const uint64_t T[3] = {q[0]->taps, q[1]->taps, q[2]->taps}, E[3] = {q[0]->extent, q[1]->extent, q[2]->extent};
+  ConvGeom g = conv_geom(cv.n, N, cv.O, y, T, E, C);
+  g.w_sp = y.C; g.w_sco = conv_prod(T) * y.C;
+  g.box = true;
+  g.mode = cv.s[0] == 1 && cv.s[1] == 1 && cv.s[2] == 1 ? 0 : 1;
+  g.dx_sn = os[0];
+  for (int i = 0; i < 3; ++i) {
+    g.p[i] = (int32_t)-q[i]->e0; g.d[i] = (int32_t)q[i]->dil; g.lo[i] = (int32_t)q[i]->e0;
+    g.dx_s[i] = i < cv.first() ? 0 : (uint64_t)cv.s[i] * os[cv.dim(i)];
+  }
   return g;
 }
 
-// The plan line of phase (ph, pw): `head` r=(rh,rw) taps_h= taps_w= dil= lower= upper= extent=, no newline.
-static std::string dgrad2_phase_line(const char* head, const DgradPhase1D& ph, const DgradPhase1D& pw, uint64_t OH, uint64_t OW) {
-  return std::string(head) + " r=(" + std::to_string(ph.r) + "," + std::to_string(pw.r) + ") taps_h=" + dgrad_taps(ph) +
-         " taps_w=" + dgrad_taps(pw) + " dil=(" + std::to_string(ph.dil) + "," + std::to_string(pw.dil) + ") lower=(" +
-         std::to_string(ph.e0) + "," + std::to_string(pw.e0) + ") upper=(" + std::to_string(ph.e0 + (int64_t)ph.extent - (int64_t)OH) +
-         "," + std::to_string(pw.e0 + (int64_t)pw.extent - (int64_t)OW) + ") extent=(" + std::to_string(ph.extent) + "," +
-         std::to_string(pw.extent) + ")";
+// The element offset of phase q's first dx pixel (normalised strides os).
+static uint64_t conv_phase_dx(const ConvNd& cv, const DgradPhase1D* const q[3], const uint64_t* os) {
+  uint64_t e = 0;
+  for (int i = cv.first(); i < 3; ++i) e += (uint64_t)q[i]->r * os[cv.dim(i)];
+  return e;
 }
 
-extern "C" int b200_conv2d_backward_data(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr dy,
-                                         const uint64_t* dy_shape, const uint64_t* dy_strides, b200_dptr w, const uint64_t* w_shape,
-                                         const uint64_t* w_strides, b200_dptr dx, const uint64_t* dx_shape, const uint64_t* dx_strides,
-                                         const b200_conv2d_args* args) {
-  CTX_ENTER(c);
-  const char* what = "conv2d_backward_data";
-  if (!dy_shape || !w_shape || !dx_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
-  const b200_conv2d_args& a = *args;
-  const uint64_t N = dx_shape[0], H = dx_shape[1], W = dx_shape[2], C = dx_shape[3];
-  const uint64_t Cout = w_shape[0], KH = w_shape[1], KW = w_shape[2];
-  uint64_t OH = 0, OW = 0;
-  int rc = conv_check_args(what, in_dtype, out_dtype, a, nullptr, C, w_shape[3]);
-  if (!rc) rc = conv_check_shape(what, a, dx_shape, w_shape, dy_shape, "dy", &OH, &OW);
-  if (!rc && KH && KW) rc = conv_check_stride(what, a);
+// The plan line of phase q (dy extents O): `conv[3d] <kind> phase r=(...) taps_h= taps_w= dil= lower= upper= extent=`, one
+// entry per dimension that exists, no newline.
+static std::string conv_phase_line(const ConvNd& cv, const char* kind, const DgradPhase1D* const q[3], const uint64_t O[3]) {
+  static const char* const tn[3] = {" taps_d=", " taps_h=", " taps_w="};
+  auto tuple = [&](auto f) {
+    std::string t = "(";
+    for (int i = cv.first(); i < 3; ++i) t += (i > cv.first() ? "," : "") + std::to_string(f(i));
+    return t + ")";
+  };
+  std::string line = std::string(cv.n == 3 ? "conv3d " : "conv ") + kind + " phase r=" + tuple([&](int i) { return q[i]->r; });
+  for (int i = cv.first(); i < 3; ++i) line += tn[i] + dgrad_taps(*q[i]);
+  line += " dil=" + tuple([&](int i) { return q[i]->dil; });
+  line += " lower=" + tuple([&](int i) { return q[i]->e0; });
+  line += " upper=" + tuple([&](int i) { return q[i]->e0 + (int64_t)q[i]->extent - (int64_t)O[i]; });
+  line += " extent=" + tuple([&](int i) { return q[i]->extent; });
+  return line;
+}
+
+// b200_conv2d_backward_data / b200_conv3d_backward_data: dy [N, *O, Cout], w [Cout, *K, C], dx [N, *I, C].
+static int conv_backward_data(b200_ctx* c, b200_stream s, ConvNd cv, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr dy,
+                              const uint64_t* dy_shape, const uint64_t* dy_strides, b200_dptr w, const uint64_t* w_shape,
+                              const uint64_t* w_strides, b200_dptr dx, const uint64_t* dx_shape, const uint64_t* dx_strides) {
+  const char* what = cv.what;
+  const int n = cv.n, r = n + 2;
+  const uint64_t N = dx_shape[0], C = dx_shape[r - 1], Cout = w_shape[0], KK = conv_prod(cv.K);
+  int rc = conv_check_args(cv, in_dtype, out_dtype, nullptr, C, w_shape[r - 1]);
+  if (!rc) rc = conv_check_shape(&cv, dx_shape, w_shape, dy_shape, "dy");
+  if (!rc && !conv_any0(cv.K)) rc = conv_check_stride(cv);
   if (rc) return rc;
-  if (N == 0 || H == 0 || W == 0 || C == 0) return B200_OK;   // no dx
-  const uint64_t lim = 1ull << 31;
-  if (N * H * W >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * H * W = %llu must be < 2^31", what, (unsigned long long)(N * H * W));
-  if (KH * KW * ((Cout + 63) / 64 * 64) >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: KH * KW * Cout (Cout padded to 64) must be < 2^31", what);
-  // phases of each dimension, and the im2col limits of every phase that runs
-  std::vector<DgradPhase1D> phs, pws;
-  bool zero_phase = false;
-  if ((rc = dgrad2_plan(what, a, H, W, KH, KW, OH, OW, Cout, &phs, &pws, &zero_phase))) return rc;
+  if (N == 0 || conv_any0(cv.I) || C == 0) return B200_OK;   // no dx
+  const uint64_t lim = 1ull << 31, P = N * conv_prod(cv.I);
+  if (P >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * %s = %llu must be < 2^31", what, conv_names(cv, "", " * ").c_str(), (unsigned long long)P);
+  if (KK * ((Cout + 63) / 64 * 64) >= lim)
+    return fail(B200_ERR_UNSUPPORTED, "%s: %s * Cout (Cout padded to 64) must be < 2^31", what, conv_names(cv, "K", " * ").c_str());
+  ConvPhases ph;
+  if ((rc = conv_phase_plan(cv, Cout, &ph))) return rc;
   if ((rc = conv_check_ptrs(what, dy, w, dx, "dx", out_dtype))) return rc;
   const size_t osz = dtype_size(out_dtype);
-  uint64_t os[4], ys[4], ws[4];
-  conv_norm_strides(dx_shape, dx_strides, os);
-  if ((rc = conv_check_pixels(what, "dx", dx_shape, os))) return rc;
+  uint64_t os[5], ys[5], ws[5];
+  conv_norm_strides(r, dx_shape, dx_strides, os);
+  if ((rc = conv_check_pixels(cv, "dx", dx_shape, os))) return rc;
   CUstream st = resolve_stream(c, s);
   // dx pixels that no tap reaches are exact zeros: one memset of dx, before the phases that overwrite the rest
-  if (zero_phase) {
-    rc = memset2d_zero(c, st, dx, osz, os[2], C, N * H * W);
+  if (ph.zero_phase) {
+    rc = memset2d_zero(c, st, dx, osz, os[n], C, P);
     if (rc) return rc;
   }
-  if (Cout == 0 || KH == 0 || KW == 0) return B200_OK;
-  conv_norm_strides(dy_shape, dy_strides, ys);
-  conv_norm_strides(w_shape, w_strides, ws);
+  if (Cout == 0 || KK == 0) return B200_OK;
+  conv_norm_strides(r, dy_shape, dy_strides, ys);
+  conv_norm_strides(r, w_shape, w_strides, ws);
   CUdeviceptr tmp[3] = {0, 0, 0};
-  NhwcOperand y{};
-  rc = conv_prep_nhwc(c, st, in_dtype, dy, dy_shape, ys, kFlatNone, tmp, &y);
-  // every phase's flipped, channel-transposed weights [C][Th][Tw][cp] in one pooled buffer of KH * KW * C * cp elements
+  ConvOperand y{};
+  rc = conv_prep(c, st, in_dtype, n, dy, dy_shape, ys, kFlatNone, tmp, &y);
   const uint64_t cp = y.C;
-  ConvDgradWeightsParams wp;
-  memset(&wp, 0, sizeof(wp));
-  if (!rc) rc = dgrad2_prep(c, st, w, ws, a, C, Cout, cp, KH, KW, phs, pws, &tmp[2], &wp);
+  if (!rc) rc = conv_dgrad_weights(c, st, cv, ph, w, ws, C, Cout, cp, &tmp[2]);
   // one stride-1 convolution of dy per phase that has taps and pixels
-  for (const DgradPhase1D& ph : phs)
-    for (const DgradPhase1D& pw : pws) {
-      if (rc) break;
-      if (!ph.extent || !pw.extent || !ph.taps || !pw.taps) continue;
-      ConvGeom g = dgrad2_geom(N, OH, OW, cp, C, ph, pw, y, os, a);
-      if (c->dry) c->plan += dgrad2_phase_line("conv dgrad phase", ph, pw, OH, OW) + "\n";
-      const GemmProblem gp = conv_problem(in_dtype, out_dtype, y.ptr, tmp[2] + wp.off[ph.r * a.stride_w + pw.r] * 2,
-                                          dx + ((uint64_t)ph.r * os[1] + (uint64_t)pw.r * os[2]) * osz, N * ph.extent * pw.extent, C,
-                                          (uint64_t)ph.taps * pw.taps * ((cp + 63) / 64 * 64), os[2], &g);
-      rc = launch_wgmma(c, st, gp, false, false);
-    }
+  if (!rc) rc = ph.each([&](const DgradPhase1D* const* q) -> int {
+    for (int i = 0; i < 3; ++i)
+      if (!q[i]->extent || !q[i]->taps) return B200_OK;
+    ConvGeom g = conv_phase_geom(cv, N, C, q, y, os);
+    if (c->dry) c->plan += conv_phase_line(cv, "dgrad", q, cv.O) + "\n";
+    const GemmProblem gp = conv_problem(in_dtype, out_dtype, y.ptr, tmp[2] + ph.off(q) * C * cp * 2, dx + conv_phase_dx(cv, q, os) * osz,
+                                        N * conv_prod(g.O), C, conv_prod(g.K) * ((cp + 63) / 64 * 64), os[n], &g);
+    return launch_wgmma(c, st, gp, false, false);
+  });
   for (CUdeviceptr t : tmp)
     if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMMs have drained
   return rc;
 }
 
-extern "C" int b200_conv2d_backward_weight(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr x,
-                                           const uint64_t* x_shape, const uint64_t* x_strides, b200_dptr dy, const uint64_t* dy_shape,
-                                           const uint64_t* dy_strides, b200_dptr dw, const uint64_t* dw_shape, const uint64_t* dw_strides,
-                                           const b200_conv2d_args* args) {
-  CTX_ENTER(c);
-  const char* what = "conv2d_backward_weight";
-  if (!x_shape || !dy_shape || !dw_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
-  const b200_conv2d_args& a = *args;
-  const uint64_t N = x_shape[0], H = x_shape[1], W = x_shape[2], C = x_shape[3];
-  const uint64_t Cout = dw_shape[0], KH = dw_shape[1], KW = dw_shape[2];
-  uint64_t OH = 0, OW = 0;
-  int rc = conv_check_args(what, in_dtype, out_dtype, a, nullptr, C, dw_shape[3]);
-  if (!rc) rc = conv_check_shape(what, a, x_shape, dw_shape, dy_shape, "dy", &OH, &OW);
-  if (!rc && KH && KW) rc = conv_check_stride(what, a);
+// b200_conv2d_backward_weight / b200_conv3d_backward_weight: x [N, *I, C], dy [N, *O, Cout], dw [Cout, *K, C].
+static int conv_backward_weight(b200_ctx* c, b200_stream s, ConvNd cv, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr x,
+                                const uint64_t* x_shape, const uint64_t* x_strides, b200_dptr dy, const uint64_t* dy_shape,
+                                const uint64_t* dy_strides, b200_dptr dw, const uint64_t* dw_shape, const uint64_t* dw_strides) {
+  const char* what = cv.what;
+  const int n = cv.n, r = n + 2;
+  const uint64_t N = x_shape[0], C = x_shape[r - 1], Cout = dw_shape[0], KK = conv_prod(cv.K);
+  int rc = conv_check_args(cv, in_dtype, out_dtype, nullptr, C, dw_shape[r - 1]);
+  if (!rc) rc = conv_check_shape(&cv, x_shape, dw_shape, dy_shape, "dy");
+  if (!rc && !conv_any0(cv.K)) rc = conv_check_stride(cv);
   if (rc) return rc;
-  if (Cout == 0 || C == 0 || KH == 0 || KW == 0) return B200_OK;   // no dw
-  if ((rc = conv_check_fwd_corners(what, a, KH, KW))) return rc;   // x is read through the forward's map
-  const uint64_t P = N * OH * OW, lim = 1ull << 31;
-  if (P >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * OH * OW = %llu must be < 2^31", what, (unsigned long long)P);
+  if (Cout == 0 || C == 0 || KK == 0) return B200_OK;   // no dw
+  if ((rc = conv_check_fwd(cv))) return rc;   // x is read through the forward's map
+  const uint64_t P = N * conv_prod(cv.O), lim = 1ull << 31;
+  if (P >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * %s = %llu must be < 2^31", what, conv_names(cv, "O", " * ").c_str(), (unsigned long long)P);
   const uint64_t cx = (C + 7) / 8 * 8;
-  if (KH * KW * ((cx + 63) / 64 * 64) >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: KH * KW * C (C padded to 64) must be < 2^31", what);
+  if (KK * ((cx + 63) / 64 * 64) >= lim)
+    return fail(B200_ERR_UNSUPPORTED, "%s: %s * C (C padded to 64) must be < 2^31", what, conv_names(cv, "K", " * ").c_str());
   if ((rc = conv_check_ptrs(what, x, dy, dw, "dw", out_dtype))) return rc;
   const size_t osz = dtype_size(out_dtype);
-  uint64_t ds[4], xs[4], ys[4], dw_sp = 0;
-  conv_norm_strides(dw_shape, dw_strides, ds);
-  if ((rc = conv_check_dw(what, dw_shape, ds, osz, &dw_sp))) return rc;
+  uint64_t ds[5], xs[5], ys[5], dw_sp = 0;
+  conv_norm_strides(r, dw_shape, dw_strides, ds);
+  if ((rc = conv_check_dw(cv, dw_shape, ds, osz, &dw_sp))) return rc;
   CUstream st = resolve_stream(c, s);
   if (P == 0) {
     // no pixels: dw is exactly zero
-    if (ds[0] == KH * KW * dw_sp) return memset2d_zero(c, st, dw, osz, dw_sp, C, Cout * KH * KW);
-    for (uint64_t co = 0; co < Cout && !rc; ++co) rc = memset2d_zero(c, st, dw + co * ds[0] * osz, osz, dw_sp, C, KH * KW);
+    if (ds[0] == KK * dw_sp) return memset2d_zero(c, st, dw, osz, dw_sp, C, Cout * KK);
+    for (uint64_t co = 0; co < Cout && !rc; ++co) rc = memset2d_zero(c, st, dw + co * ds[0] * osz, osz, dw_sp, C, KK);
     return rc;
   }
-  conv_norm_strides(x_shape, x_strides, xs);
-  conv_norm_strides(dy_shape, dy_strides, ys);
+  conv_norm_strides(r, x_shape, x_strides, xs);
+  conv_norm_strides(r, dy_shape, dy_strides, ys);
   CUdeviceptr tmp[4] = {0, 0, 0, 0};
-  NhwcOperand xo{}, yo{};
-  rc = conv_prep_nhwc(c, st, in_dtype, x, x_shape, xs, kFlatNone, &tmp[0], &xo);
-  if (!rc) rc = conv_prep_nhwc(c, st, in_dtype, dy, dy_shape, ys, kFlatNHW, &tmp[2], &yo);
+  ConvOperand xo{}, yo{};
+  rc = conv_prep(c, st, in_dtype, n, x, x_shape, xs, kFlatNone, &tmp[0], &xo);
+  if (!rc) rc = conv_prep(c, st, in_dtype, n, dy, dy_shape, ys, kFlatAll, &tmp[2], &yo);
   if (!rc) {
-    ConvGeom g{};
-    g.N = N; g.H = H; g.W = W; g.C = xo.C; g.KH = KH; g.KW = KW; g.OH = OH; g.OW = OW; g.Cout = Cout;
-    g.sh = a.stride_h; g.sw = a.stride_w; g.ph = a.pad_h; g.pw = a.pad_w; g.dh = a.dilation_h; g.dw = a.dilation_w;
-    g.x_sw = xo.s_w; g.x_sh = xo.s_h; g.x_sn = xo.s_n;
+    ConvGeom g = conv_geom(n, N, cv.I, xo, cv.K, cv.O, Cout);
+    conv_geom_args(cv, &g);
     g.mode = 2; g.dw_sp = dw_sp; g.dw_c = C;
-    GemmProblem gp = conv_problem(in_dtype, out_dtype, yo.ptr, xo.ptr, dw, Cout, KH * KW * ((xo.C + 63) / 64 * 64), P, ds[0], &g);
+    GemmProblem gp = conv_problem(in_dtype, out_dtype, yo.ptr, xo.ptr, dw, Cout, KK * ((xo.C + 63) / 64 * 64), P, ds[0], &g);
     gp.a_sm = 1; gp.a_sk = yo.s_w; gp.b_sn = 1; gp.b_sk = xo.s_w;   // both operands MN-major
     // few tiles, a long K: the stream-K head may cut a tile into as many ranges as fill the SMs, each >= 8 k-blocks
     gp.sk_max_parts = std::max<uint64_t>(8, (P + 63) / 64 / 8);
@@ -3426,288 +3533,32 @@ extern "C" int b200_conv2d_backward_weight(b200_ctx* c, b200_stream s, b200_dtyp
   return rc;
 }
 
-// ------------------------------------------------------------------------------------------------ 3-D convolution
-// b200_conv3d*: the 2-D machinery with a depth dimension.  Arrays over the spatial dimensions are ordered (D, H, W).
-// Rank-5 tensor maps take pixel-box corners in [-16, 15] (cuda.h: cuTensorMapEncodeIm2col) and the load's im2col offsets
-// in [0, 31] (5 bits each; PTX ISA, cp.async.bulk.tensor im2col mode).
-static constexpr int64_t kIm2col5Lo = -16, kIm2col5Hi = 15, kIm2col5MaxOffset = 31;
-
-// Strides of a rank-5 view with extent-1 dimensions normalised (see conv_norm_strides).
-static void conv3_norm_strides(const uint64_t* shape, const uint64_t* strides, uint64_t* out) {
-  uint64_t inner = 1;
-  for (int d = 4; d >= 0; --d) {
-    out[d] = strides ? strides[d] : inner;
-    if (shape[d] == 1) out[d] = inner;
-    inner = out[d] * shape[d];
-  }
-}
-
-// (D, H, W) = dimensions 1..3 of a rank-5 view as one strided dimension: its stride, or 0.
-static uint64_t conv3_flat_dhw(const uint64_t* shape, const uint64_t* ns) {
-  const uint64_t s_hw = conv_flat_stride(shape[2], shape[3], ns[2], ns[3]);
-  return s_hw == 0 ? 0 : conv_flat_stride(shape[1], shape[2] * shape[3], ns[1], s_hw);
-}
-
-// conv_check_args for the 3-D args: dtypes, activation, strides / dilations >= 1, padding >= 0, channels.
-static int conv3_check_args(const char* what, b200_dtype in_dtype, b200_dtype out_dtype, const b200_conv3d_args& a, const b200_epilogue* ep,
-                            uint64_t in_c, uint64_t w_c) {
-  const b200_conv2d_args hw{a.stride_h, a.stride_w, a.pad_h, a.pad_w, a.dilation_h, a.dilation_w};
-  if (a.stride_d < 1 || a.dilation_d < 1 || a.pad_d < 0)
-    return fail(B200_ERR_INVALID_ARG, "%s: strides and dilations must be >= 1 and padding >= 0", what);
-  return conv_check_args(what, in_dtype, out_dtype, hw, ep, in_c, w_c);
-}
-
-// Extents < 2^31, then PyTorch's output rule per dimension: y must be [N, OD, OH, OW, Cout] for in [N, D, H, W, C] and
-// w [Cout, KD, KH, KW, *].  O receives (OD, OH, OW).
-static int conv3_check_shape(const char* what, const b200_conv3d_args& a, const uint64_t* in, const uint64_t* w, const uint64_t* y,
-                             const char* y_name, uint64_t O[3]) {
-  const uint64_t lim = 1ull << 31;
-  for (int d = 0; d < 5; ++d)
-    if (in[d] >= lim || w[d] >= lim || y[d] >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: extents must be < 2^31", what);
-  if (w[1] == 0 || w[2] == 0 || w[3] == 0) return B200_OK;
-  const int64_t s[3] = {a.stride_d, a.stride_h, a.stride_w}, p[3] = {a.pad_d, a.pad_h, a.pad_w};
-  const int64_t dl[3] = {a.dilation_d, a.dilation_h, a.dilation_w};
-  for (int i = 0; i < 3; ++i) {
-    const int64_t n = (int64_t)in[1 + i] + 2 * p[i] - dl[i] * ((int64_t)w[1 + i] - 1) - 1;
-    if (n < 0) return fail(B200_ERR_INVALID_ARG, "%s: the dilated kernel is larger than the padded input (output extent < 1)", what);
-    O[i] = (uint64_t)(n / s[i]) + 1;
-  }
-  if (y[0] != in[0] || y[1] != O[0] || y[2] != O[1] || y[3] != O[2] || y[4] != w[0])
-    return fail(B200_ERR_INVALID_ARG, "%s: %s is [%llu,%llu,%llu,%llu,%llu], expected [%llu,%llu,%llu,%llu,%llu]", what, y_name,
-                (unsigned long long)y[0], (unsigned long long)y[1], (unsigned long long)y[2], (unsigned long long)y[3],
-                (unsigned long long)y[4], (unsigned long long)in[0], (unsigned long long)O[0], (unsigned long long)O[1],
-                (unsigned long long)O[2], (unsigned long long)w[0]);
-  return B200_OK;
-}
-
-// The rank-5 im2col limits: pixel-box corners in [-16, 15], and the largest im2col offset (dilation * (taps - 1)) of each
-// dimension in [0, 31].
-static int conv3_check_corners(const char* what, const int64_t* corners, int n) {
-  for (int i = 0; i < n; ++i)
-    if (corners[i] < kIm2col5Lo || corners[i] > kIm2col5Hi)
-      return fail(B200_ERR_UNSUPPORTED, "%s: im2col pixel-box corner %lld outside [-16, 15] (rank-5 tensor map)", what, (long long)corners[i]);
-  return B200_OK;
-}
-static int conv3_check_offsets(const char* what, const int64_t max_off[3]) {
-  for (int i = 0; i < 3; ++i)
-    if (max_off[i] > kIm2col5MaxOffset)
-      return fail(B200_ERR_UNSUPPORTED, "%s: im2col offset dilation * (kernel - 1) = %lld exceeds 31 (5-bit rank-5 offsets)", what,
-                  (long long)max_off[i]);
-  return B200_OK;
-}
-// The forward's map (also backward_weight's x): corners -p and p - d*(K-1), offsets d*(K-1), and conv strides <= 8.
-static int conv3_check_fwd(const char* what, const b200_conv3d_args& a, const uint64_t* w) {
-  const int64_t p[3] = {a.pad_d, a.pad_h, a.pad_w}, dl[3] = {a.dilation_d, a.dilation_h, a.dilation_w};
-  int64_t corners[6], off[3];
-  for (int i = 0; i < 3; ++i) {
-    off[i] = dl[i] * ((int64_t)w[1 + i] - 1);
-    corners[2 * i] = -p[i];
-    corners[2 * i + 1] = p[i] - off[i];
-  }
-  int rc = conv3_check_corners(what, corners, 6);
-  if (!rc) rc = conv3_check_offsets(what, off);
-  return rc;
-}
-static int conv3_check_stride(const char* what, const b200_conv3d_args& a) {
-  if (a.stride_d > kDgradMaxStride || a.stride_h > kDgradMaxStride || a.stride_w > kDgradMaxStride)
-    return fail(B200_ERR_UNSUPPORTED, "%s: the conv stride must be <= %d", what, kDgradMaxStride);
-  return B200_OK;
-}
-
-// An NDHWC output (out or dx): unit channel stride, one pixel pitch >= its channels across N, D, H, W.
-static int conv3_check_pixels(const char* what, const char* name, const uint64_t* shape, const uint64_t* ns) {
-  if (ns[4] != 1 || ns[3] < shape[4] || ns[2] != shape[3] * ns[3] || ns[1] != shape[2] * ns[2] || ns[0] != shape[1] * ns[1])
-    return fail(B200_ERR_UNSUPPORTED, "%s: %s must have unit channel stride and one pixel pitch >= its channels for N, D, H, W", what, name);
-  return B200_OK;
-}
-
-// An operand [N, D, H, W, C] (normalised strides ns) as the convolution maps read it; conv_prep_nhwc with a depth dimension.
-// flat: none (x, dy in the data gradient), (D, H, W) (the weights: one kernel-position stride, returned as s_w) or
-// (N, D, H, W) (dy in the weight gradient: [pixels, Cout]).
-struct NdhwcOperand {
-  uint64_t ptr, C, s_w, s_h, s_d, s_n;
-};
-static int conv3_prep(b200_ctx* c, CUstream st, b200_dtype dt, uint64_t ptr, const uint64_t* shape, const uint64_t* ns, ConvFlat flat,
-                      CUdeviceptr tmp[2], NdhwcOperand* o) {
-  const uint64_t N = shape[0], D = shape[1], H = shape[2], W = shape[3], C = shape[4];
-  const uint64_t spx = conv3_flat_dhw(shape, ns);   // (D, H, W) as one pixel dimension
-  int rc = B200_OK;
-  auto gather = [&]() -> int {
-    CUdeviceptr buf;
-    int r = pool_alloc(c, N * D * H * W * C * 2, &buf, st);
-    if (r) return r;
-    r = b200_into_contiguous(c, static_cast<b200_stream>(st), dt, ptr, buf, 5, shape, ns);
-    if (r) { pool_free(c, buf, st); return r; }
-    tmp[0] = buf;
-    return B200_OK;
-  };
-  if (C % 8 == 0) {
-    bool in_place = ptr % 16 == 0 && ns[4] == 1 && conv_al16(ns[0]);
-    if (flat == kFlatHW) in_place = in_place && spx != 0 && conv_al16(spx);
-    else in_place = in_place && conv_al16(ns[1]) && conv_al16(ns[2]) && conv_al16(ns[3]) &&
-                    (flat == kFlatNone || (ns[2] == W * ns[3] && ns[1] == H * ns[2] && ns[0] == D * ns[1]));
-    if (in_place) {
-      *o = {ptr, C, flat == kFlatHW ? spx : ns[3], ns[2], ns[1], ns[0]};
-      return B200_OK;
-    }
-    rc = gather();
-    *o = {tmp[0], C, C, W * C, H * W * C, D * H * W * C};
-    return rc;
-  }
-  const uint64_t cp = (C + 7) / 8 * 8;
-  uint64_t in = ptr, sb = ns[0], sp = spx, sc = ns[4];
-  if (spx == 0) {
-    rc = gather();
-    in = tmp[0]; sb = D * H * W * C; sp = C; sc = 1;
-  }
-  if (!rc) rc = conv_pad_channels(c, st, in, N, D * H * W, C, sb, sp, sc, cp, &tmp[1]);
-  *o = {tmp[1], cp, cp, W * cp, H * W * cp, D * H * W * cp};
-  return rc;
-}
-
-// ConvGeom of a 3-D map: input extents I = (D, H, W), kernel K, output O, per-dimension stride / pad / dilation.
-static ConvGeom conv3_geom(uint64_t N, const uint64_t I[3], uint64_t C, const uint64_t K[3], const uint64_t O[3], uint64_t Cout,
-                           const int32_t s[3], const int32_t p[3], const int32_t d[3]) {
-  ConvGeom g{};
-  g.dims = 3;
-  g.N = N; g.D = I[0]; g.H = I[1]; g.W = I[2]; g.C = C; g.KD = K[0]; g.KH = K[1]; g.KW = K[2];
-  g.OD = O[0]; g.OH = O[1]; g.OW = O[2]; g.Cout = Cout;
-  g.sd = s[0]; g.sh = s[1]; g.sw = s[2]; g.pd = p[0]; g.ph = p[1]; g.pw = p[2]; g.dd = d[0]; g.dh = d[1]; g.dw = d[2];
-  return g;
+extern "C" int b200_conv2d(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr x, const uint64_t* x_shape,
+                           const uint64_t* x_strides, b200_dptr w, const uint64_t* w_shape, const uint64_t* w_strides, b200_dptr out,
+                           const uint64_t* out_shape, const uint64_t* out_strides, const b200_conv2d_args* args, const b200_epilogue* ep) {
+  CTX_ENTER(c);
+  if (!x_shape || !w_shape || !out_shape || !args) return fail(B200_ERR_INVALID_ARG, "conv2d: null shape or args");
+  return conv_forward(c, s, conv_nd("conv2d", *args, x_shape, w_shape), in_dtype, out_dtype, x, x_shape, x_strides, w, w_shape, w_strides, out,
+                      out_shape, out_strides, ep);
 }
 
 extern "C" int b200_conv3d(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr x, const uint64_t* x_shape,
                            const uint64_t* x_strides, b200_dptr w, const uint64_t* w_shape, const uint64_t* w_strides, b200_dptr out,
                            const uint64_t* out_shape, const uint64_t* out_strides, const b200_conv3d_args* args, const b200_epilogue* ep) {
   CTX_ENTER(c);
-  const char* what = "conv3d";
-  if (!x_shape || !w_shape || !out_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
-  const b200_conv3d_args& a = *args;
-  const uint64_t N = x_shape[0], C = x_shape[4], Cout = w_shape[0];
-  const uint64_t I[3] = {x_shape[1], x_shape[2], x_shape[3]}, K[3] = {w_shape[1], w_shape[2], w_shape[3]};
-  int rc = conv3_check_args(what, in_dtype, out_dtype, a, ep, C, w_shape[4]);
-  if (rc) return rc;
-  if (N == 0 || I[0] == 0 || I[1] == 0 || I[2] == 0 || C == 0 || Cout == 0 || K[0] == 0 || K[1] == 0 || K[2] == 0) return B200_OK;
-  uint64_t O[3] = {0, 0, 0};
-  if ((rc = conv3_check_shape(what, a, x_shape, w_shape, out_shape, "out", O))) return rc;
-  if ((rc = conv3_check_fwd(what, a, w_shape)) || (rc = conv3_check_stride(what, a))) return rc;
-  const uint64_t M = N * O[0] * O[1] * O[2], lim = 1ull << 31, KK = K[0] * K[1] * K[2];
-  if (M >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * OD * OH * OW = %llu must be < 2^31", what, (unsigned long long)M);
-  if ((rc = conv_check_ptrs(what, x, w, out, "output", out_dtype))) return rc;
-  uint64_t os[5], xs[5], ws[5];
-  conv3_norm_strides(out_shape, out_strides, os);
-  if ((rc = conv3_check_pixels(what, "out", out_shape, os))) return rc;
-  if (KK * ((C + 63) / 64 * 64) >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: KD * KH * KW * C (C padded to 64) must be < 2^31", what);
-  CUstream st = resolve_stream(c, s);
-  conv3_norm_strides(x_shape, x_strides, xs);
-  conv3_norm_strides(w_shape, w_strides, ws);
-  CUdeviceptr tmp[4] = {0, 0, 0, 0};
-  NdhwcOperand xo{}, wo{};
-  rc = conv3_prep(c, st, in_dtype, x, x_shape, xs, kFlatNone, &tmp[0], &xo);
-  if (!rc) rc = conv3_prep(c, st, in_dtype, w, w_shape, ws, kFlatHW, &tmp[2], &wo);
-  if (!rc) {
-    const int32_t sv[3] = {a.stride_d, a.stride_h, a.stride_w}, pv[3] = {a.pad_d, a.pad_h, a.pad_w};
-    const int32_t dv[3] = {a.dilation_d, a.dilation_h, a.dilation_w};
-    ConvGeom g = conv3_geom(N, I, xo.C, K, O, Cout, sv, pv, dv);
-    g.x_sw = xo.s_w; g.x_sh = xo.s_h; g.x_sd = xo.s_d; g.x_sn = xo.s_n;
-    g.w_sp = wo.s_w; g.w_sco = wo.s_n;
-    GemmProblem gp = conv_problem(in_dtype, out_dtype, xo.ptr, wo.ptr, out, M, Cout, KK * ((g.C + 63) / 64 * 64), os[3], &g);
-    if (ep) { gp.alpha = ep->alpha; gp.bias = ep->bias; gp.act = (uint32_t)ep->activation; }
-    rc = launch_wgmma(c, st, gp, false, false);
-  }
-  for (CUdeviceptr t : tmp)
-    if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMM has drained
-  return rc;
+  if (!x_shape || !w_shape || !out_shape || !args) return fail(B200_ERR_INVALID_ARG, "conv3d: null shape or args");
+  return conv_forward(c, s, conv_nd("conv3d", *args, x_shape, w_shape), in_dtype, out_dtype, x, x_shape, x_strides, w, w_shape, w_strides, out,
+                      out_shape, out_strides, ep);
 }
 
-// The 3-D data gradient's phases (also b200_conv_transpose3d's): per dimension (D, H, W) of dx extents I from dy extents
-// O, and the rank-5 im2col limits (corners, offsets) of every phase that runs.  *zero_phase as dgrad2_plan.
-static int dgrad3_plan(const char* what, const int64_t sv[3], const int64_t pv[3], const int64_t dv[3], const uint64_t I[3],
-                       const uint64_t K[3], const uint64_t O[3], uint64_t Cout, std::vector<DgradPhase1D> ph[3], bool* zero_phase) {
-  for (int i = 0; i < 3; ++i)
-    for (int64_t r = 0; r < sv[i]; ++r) ph[i].push_back(dgrad_phase(I[i], K[i], sv[i], pv[i], dv[i], (uint32_t)r));
-  *zero_phase = false;
-  for (const DgradPhase1D& pd : ph[0])
-    for (const DgradPhase1D& phh : ph[1])
-      for (const DgradPhase1D& pw : ph[2]) {
-        const DgradPhase1D* q[3] = {&pd, &phh, &pw};
-        if (!pd.extent || !phh.extent || !pw.extent) continue;
-        if (!pd.taps || !phh.taps || !pw.taps || Cout == 0) { *zero_phase = true; continue; }
-        int64_t corners[6], off[3];
-        for (int i = 0; i < 3; ++i) {
-          corners[2 * i] = q[i]->e0;
-          corners[2 * i + 1] = q[i]->e0 + (int64_t)q[i]->extent - (int64_t)O[i];
-          off[i] = (int64_t)(q[i]->taps - 1) * q[i]->dil;
-        }
-        int rc = conv3_check_corners(what, corners, 6);
-        if (!rc) rc = conv3_check_offsets(what, off);
-        if (rc) return rc;
-      }
-  return B200_OK;
-}
-
-// conv3d_dgrad_weights' parameters for the phases ph of w [Cout, KD, KH, KW, C], and where each phase's block starts.
-struct Dgrad3Prep {
-  Conv3dDgradWeightsParams wp;
-  uint64_t pre[3][kDgradMaxStride];
-  uint64_t k1, k2, ccp;
-  Dgrad3Prep(const std::vector<DgradPhase1D> ph[3], const uint64_t K[3], const int64_t sv[3], const int64_t pv[3], const int64_t dv[3],
-             uint64_t C, uint64_t cp) : k1(K[1]), k2(K[2]), ccp(C * cp) {
-    memset(&wp, 0, sizeof(wp));
-    for (int i = 0; i < 3; ++i) {
-      uint64_t acc = 0;
-      for (const DgradPhase1D& q : ph[i]) { pre[i][q.r] = acc; acc += q.taps; wp.kmax[i][q.r] = q.kmax; wp.taps[i][q.r] = q.taps; }
-      wp.k[i] = (uint32_t)K[i]; wp.s[i] = (uint32_t)sv[i]; wp.d[i] = (uint32_t)dv[i]; wp.p[i] = (uint32_t)pv[i]; wp.q[i] = ph[i][0].step;
-    }
-    wp.C = C; wp.cp = cp;
-  }
-  // first element of phase (rd, rh, rw)'s block
-  uint64_t off(uint32_t rd, uint32_t rh, uint32_t rw) const {
-    return ccp * (pre[0][rd] * k1 * k2 + (uint64_t)wp.taps[0][rd] * (pre[1][rh] * k2 + (uint64_t)wp.taps[1][rh] * pre[2][rw]));
-  }
-};
-
-// Every phase's flipped, channel-transposed weights in one pooled buffer (*buf) of KK * C * cp elements (conv3d_dgrad_weights).
-static int dgrad3_prep(b200_ctx* c, CUstream st, uint64_t w, const uint64_t ws[5], uint64_t Cout, uint64_t KK, Dgrad3Prep* pr, CUdeviceptr* buf) {
-  Conv3dDgradWeightsParams& wp = pr->wp;
-  int rc = pool_alloc(c, KK * wp.C * wp.cp * 2, buf, st);
-  if (rc) return rc;
-  wp.w = w; wp.out = *buf;
-  wp.s_co = ws[0]; wp.s_kz = ws[1]; wp.s_ky = ws[2]; wp.s_kx = ws[3]; wp.s_c = ws[4];
-  wp.Cout = Cout;
-  CUfunction f;
-  rc = get_func(c, "conv3d_dgrad_weights", &f);
-  void* kargs[] = {&wp};
-  if (!rc) rc = launch(c, f, (unsigned)(((wp.C + 31) / 32) * ((wp.cp + 31) / 32)), (unsigned)KK, 1, 256, 0, 1, st, kargs);
-  return rc;
-}
-
-// Phase q = (D, H, W) phases as a stride-1 3-D convolution of dy (y, extents O) into C channels; dgrad2_geom with depth.
-static ConvGeom dgrad3_geom(uint64_t N, const uint64_t O[3], uint64_t cp, uint64_t C, const DgradPhase1D* const q[3], const NdhwcOperand& y,
-                            const uint64_t os[5], const int64_t sv[3]) {
-  const uint64_t T[3] = {q[0]->taps, q[1]->taps, q[2]->taps}, E[3] = {q[0]->extent, q[1]->extent, q[2]->extent};
-  const int32_t one[3] = {1, 1, 1}, pp[3] = {(int32_t)-q[0]->e0, (int32_t)-q[1]->e0, (int32_t)-q[2]->e0};
-  const int32_t dil[3] = {(int32_t)q[0]->dil, (int32_t)q[1]->dil, (int32_t)q[2]->dil};
-  ConvGeom g = conv3_geom(N, O, cp, T, E, C, one, pp, dil);
-  g.x_sw = y.s_w; g.x_sh = y.s_h; g.x_sd = y.s_d; g.x_sn = y.s_n;
-  g.w_sp = cp; g.w_sco = T[0] * T[1] * T[2] * cp;
-  g.box = true; g.lo_d = (int32_t)q[0]->e0; g.lo_h = (int32_t)q[1]->e0; g.lo_w = (int32_t)q[2]->e0;
-  g.mode = sv[0] == 1 && sv[1] == 1 && sv[2] == 1 ? 0 : 1;
-  g.dx_sn = os[0]; g.dx_sd = (uint64_t)sv[0] * os[1]; g.dx_si = (uint64_t)sv[1] * os[2]; g.dx_sj = (uint64_t)sv[2] * os[3];
-  return g;
-}
-
-// The plan line of phase q: `head` r=(rd,rh,rw) taps_d= taps_h= taps_w= dil= lower= upper= extent=, no newline.
-static std::string dgrad3_phase_line(const char* head, const DgradPhase1D* const q[3], const uint64_t O[3]) {
-  std::string line = std::string(head) + " r=(" + std::to_string(q[0]->r) + "," + std::to_string(q[1]->r) + "," + std::to_string(q[2]->r) + ")";
-  const char* tn[3] = {" taps_d=", " taps_h=", " taps_w="};
-  for (int i = 0; i < 3; ++i) line += tn[i] + dgrad_taps(*q[i]);
-  auto triple = [&](auto f) { return "(" + std::to_string(f(0)) + "," + std::to_string(f(1)) + "," + std::to_string(f(2)) + ")"; };
-  line += " dil=" + triple([&](int i) { return (int64_t)q[i]->dil; });
-  line += " lower=" + triple([&](int i) { return q[i]->e0; });
-  line += " upper=" + triple([&](int i) { return q[i]->e0 + (int64_t)q[i]->extent - (int64_t)O[i]; });
-  line += " extent=" + triple([&](int i) { return (int64_t)q[i]->extent; });
-  return line;
+extern "C" int b200_conv2d_backward_data(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr dy,
+                                         const uint64_t* dy_shape, const uint64_t* dy_strides, b200_dptr w, const uint64_t* w_shape,
+                                         const uint64_t* w_strides, b200_dptr dx, const uint64_t* dx_shape, const uint64_t* dx_strides,
+                                         const b200_conv2d_args* args) {
+  CTX_ENTER(c);
+  if (!dy_shape || !w_shape || !dx_shape || !args) return fail(B200_ERR_INVALID_ARG, "conv2d_backward_data: null shape or args");
+  return conv_backward_data(c, s, conv_nd("conv2d_backward_data", *args, dx_shape, w_shape), in_dtype, out_dtype, dy, dy_shape, dy_strides, w,
+                            w_shape, w_strides, dx, dx_shape, dx_strides);
 }
 
 extern "C" int b200_conv3d_backward_data(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr dy,
@@ -3715,66 +3566,19 @@ extern "C" int b200_conv3d_backward_data(b200_ctx* c, b200_stream s, b200_dtype 
                                          const uint64_t* w_strides, b200_dptr dx, const uint64_t* dx_shape, const uint64_t* dx_strides,
                                          const b200_conv3d_args* args) {
   CTX_ENTER(c);
-  const char* what = "conv3d_backward_data";
-  if (!dy_shape || !w_shape || !dx_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
-  const b200_conv3d_args& a = *args;
-  const uint64_t N = dx_shape[0], C = dx_shape[4], Cout = w_shape[0];
-  const uint64_t I[3] = {dx_shape[1], dx_shape[2], dx_shape[3]}, K[3] = {w_shape[1], w_shape[2], w_shape[3]};
-  const int64_t sv[3] = {a.stride_d, a.stride_h, a.stride_w}, pv[3] = {a.pad_d, a.pad_h, a.pad_w};
-  const int64_t dv[3] = {a.dilation_d, a.dilation_h, a.dilation_w};
-  uint64_t O[3] = {0, 0, 0};
-  int rc = conv3_check_args(what, in_dtype, out_dtype, a, nullptr, C, w_shape[4]);
-  if (!rc) rc = conv3_check_shape(what, a, dx_shape, w_shape, dy_shape, "dy", O);
-  if (!rc && K[0] && K[1] && K[2]) rc = conv3_check_stride(what, a);
-  if (rc) return rc;
-  if (N == 0 || I[0] == 0 || I[1] == 0 || I[2] == 0 || C == 0) return B200_OK;   // no dx
-  const uint64_t lim = 1ull << 31, P = N * I[0] * I[1] * I[2], KK = K[0] * K[1] * K[2];
-  if (P >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * D * H * W = %llu must be < 2^31", what, (unsigned long long)P);
-  if (KK * ((Cout + 63) / 64 * 64) >= lim)
-    return fail(B200_ERR_UNSUPPORTED, "%s: KD * KH * KW * Cout (Cout padded to 64) must be < 2^31", what);
-  // phases of each dimension, and the im2col limits of every phase that runs
-  std::vector<DgradPhase1D> ph[3];
-  bool zero_phase = false;
-  if ((rc = dgrad3_plan(what, sv, pv, dv, I, K, O, Cout, ph, &zero_phase))) return rc;
-  if ((rc = conv_check_ptrs(what, dy, w, dx, "dx", out_dtype))) return rc;
-  const size_t osz = dtype_size(out_dtype);
-  uint64_t os[5], ys[5], ws[5];
-  conv3_norm_strides(dx_shape, dx_strides, os);
-  if ((rc = conv3_check_pixels(what, "dx", dx_shape, os))) return rc;
-  CUstream st = resolve_stream(c, s);
-  // dx pixels that no tap reaches are exact zeros: one memset of dx, before the phases that overwrite the rest
-  if (zero_phase) {
-    rc = memset2d_zero(c, st, dx, osz, os[3], C, P);
-    if (rc) return rc;
-  }
-  if (Cout == 0 || KK == 0) return B200_OK;
-  conv3_norm_strides(dy_shape, dy_strides, ys);
-  conv3_norm_strides(w_shape, w_strides, ws);
-  CUdeviceptr tmp[3] = {0, 0, 0};
-  NdhwcOperand y{};
-  rc = conv3_prep(c, st, in_dtype, dy, dy_shape, ys, kFlatNone, tmp, &y);
-  // every phase's flipped, channel-transposed weights [C][Td][Th][Tw][cp] in one pooled buffer of |w| * cp / Cout elements, in
-  // (rd, rh, rw) order (Conv3dDgradWeightsParams)
-  const uint64_t cp = y.C;
-  Dgrad3Prep prep(ph, K, sv, pv, dv, C, cp);
-  if (!rc) rc = dgrad3_prep(c, st, w, ws, Cout, KK, &prep, &tmp[2]);
-  // one stride-1 convolution of dy per phase that has taps and pixels
-  for (const DgradPhase1D& pd : ph[0])
-    for (const DgradPhase1D& phh : ph[1])
-      for (const DgradPhase1D& pw : ph[2]) {
-        if (rc) break;
-        const DgradPhase1D* q[3] = {&pd, &phh, &pw};
-        if (!pd.extent || !phh.extent || !pw.extent || !pd.taps || !phh.taps || !pw.taps) continue;
-        ConvGeom g = dgrad3_geom(N, O, cp, C, q, y, os, sv);
-        if (c->dry) c->plan += dgrad3_phase_line("conv3d dgrad phase", q, O) + "\n";
-        const GemmProblem gp = conv_problem(in_dtype, out_dtype, y.ptr, tmp[2] + prep.off(pd.r, phh.r, pw.r) * 2,
-                                            dx + ((uint64_t)pd.r * os[1] + (uint64_t)phh.r * os[2] + (uint64_t)pw.r * os[3]) * osz,
-                                            N * g.OD * g.OH * g.OW, C, g.KD * g.KH * g.KW * ((cp + 63) / 64 * 64), os[3], &g);
-        rc = launch_wgmma(c, st, gp, false, false);
-      }
-  for (CUdeviceptr t : tmp)
-    if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMMs have drained
-  return rc;
+  if (!dy_shape || !w_shape || !dx_shape || !args) return fail(B200_ERR_INVALID_ARG, "conv3d_backward_data: null shape or args");
+  return conv_backward_data(c, s, conv_nd("conv3d_backward_data", *args, dx_shape, w_shape), in_dtype, out_dtype, dy, dy_shape, dy_strides, w,
+                            w_shape, w_strides, dx, dx_shape, dx_strides);
+}
+
+extern "C" int b200_conv2d_backward_weight(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr x,
+                                           const uint64_t* x_shape, const uint64_t* x_strides, b200_dptr dy, const uint64_t* dy_shape,
+                                           const uint64_t* dy_strides, b200_dptr dw, const uint64_t* dw_shape, const uint64_t* dw_strides,
+                                           const b200_conv2d_args* args) {
+  CTX_ENTER(c);
+  if (!x_shape || !dy_shape || !dw_shape || !args) return fail(B200_ERR_INVALID_ARG, "conv2d_backward_weight: null shape or args");
+  return conv_backward_weight(c, s, conv_nd("conv2d_backward_weight", *args, x_shape, dw_shape), in_dtype, out_dtype, x, x_shape, x_strides, dy,
+                              dy_shape, dy_strides, dw, dw_shape, dw_strides);
 }
 
 extern "C" int b200_conv3d_backward_weight(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr x,
@@ -3782,57 +3586,9 @@ extern "C" int b200_conv3d_backward_weight(b200_ctx* c, b200_stream s, b200_dtyp
                                            const uint64_t* dy_strides, b200_dptr dw, const uint64_t* dw_shape, const uint64_t* dw_strides,
                                            const b200_conv3d_args* args) {
   CTX_ENTER(c);
-  const char* what = "conv3d_backward_weight";
-  if (!x_shape || !dy_shape || !dw_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
-  const b200_conv3d_args& a = *args;
-  const uint64_t N = x_shape[0], C = x_shape[4], Cout = dw_shape[0];
-  const uint64_t I[3] = {x_shape[1], x_shape[2], x_shape[3]}, K[3] = {dw_shape[1], dw_shape[2], dw_shape[3]};
-  uint64_t O[3] = {0, 0, 0};
-  int rc = conv3_check_args(what, in_dtype, out_dtype, a, nullptr, C, dw_shape[4]);
-  if (!rc) rc = conv3_check_shape(what, a, x_shape, dw_shape, dy_shape, "dy", O);
-  if (!rc && K[0] && K[1] && K[2]) rc = conv3_check_stride(what, a);
-  if (rc) return rc;
-  const uint64_t KK = K[0] * K[1] * K[2];
-  if (Cout == 0 || C == 0 || KK == 0) return B200_OK;   // no dw
-  if ((rc = conv3_check_fwd(what, a, dw_shape))) return rc;   // x is read through the forward's map
-  const uint64_t P = N * O[0] * O[1] * O[2], lim = 1ull << 31;
-  if (P >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * OD * OH * OW = %llu must be < 2^31", what, (unsigned long long)P);
-  const uint64_t cx = (C + 7) / 8 * 8;
-  if (KK * ((cx + 63) / 64 * 64) >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: KD * KH * KW * C (C padded to 64) must be < 2^31", what);
-  if ((rc = conv_check_ptrs(what, x, dy, dw, "dw", out_dtype))) return rc;
-  const size_t osz = dtype_size(out_dtype);
-  uint64_t ds[5], xs[5], ys[5];
-  conv3_norm_strides(dw_shape, dw_strides, ds);
-  const uint64_t dw_sp = conv3_flat_dhw(dw_shape, ds);
-  if (ds[4] != 1 || dw_sp == 0 || ds[0] * osz >= (1ull << 40) || dw_sp * osz >= (1ull << 40))
-    return fail(B200_ERR_UNSUPPORTED, "%s: dw must have unit channel stride and (KD, KH, KW) flattening into one stride", what);
-  CUstream st = resolve_stream(c, s);
-  if (P == 0) {
-    // no pixels: dw is exactly zero
-    if (ds[0] == KK * dw_sp) return memset2d_zero(c, st, dw, osz, dw_sp, C, Cout * KK);
-    for (uint64_t co = 0; co < Cout && !rc; ++co) rc = memset2d_zero(c, st, dw + co * ds[0] * osz, osz, dw_sp, C, KK);
-    return rc;
-  }
-  conv3_norm_strides(x_shape, x_strides, xs);
-  conv3_norm_strides(dy_shape, dy_strides, ys);
-  CUdeviceptr tmp[4] = {0, 0, 0, 0};
-  NdhwcOperand xo{}, yo{};
-  rc = conv3_prep(c, st, in_dtype, x, x_shape, xs, kFlatNone, &tmp[0], &xo);
-  if (!rc) rc = conv3_prep(c, st, in_dtype, dy, dy_shape, ys, kFlatNHW, &tmp[2], &yo);
-  if (!rc) {
-    const int32_t sv[3] = {a.stride_d, a.stride_h, a.stride_w}, pv[3] = {a.pad_d, a.pad_h, a.pad_w};
-    const int32_t dv[3] = {a.dilation_d, a.dilation_h, a.dilation_w};
-    ConvGeom g = conv3_geom(N, I, xo.C, K, O, Cout, sv, pv, dv);
-    g.x_sw = xo.s_w; g.x_sh = xo.s_h; g.x_sd = xo.s_d; g.x_sn = xo.s_n;
-    g.mode = 2; g.dw_sp = dw_sp; g.dw_c = C;
-    GemmProblem gp = conv_problem(in_dtype, out_dtype, yo.ptr, xo.ptr, dw, Cout, KK * ((xo.C + 63) / 64 * 64), P, ds[0], &g);
-    gp.a_sm = 1; gp.a_sk = yo.s_w; gp.b_sn = 1; gp.b_sk = xo.s_w;   // both operands MN-major
-    gp.sk_max_parts = std::max<uint64_t>(8, (P + 63) / 64 / 8);      // as b200_conv2d_backward_weight
-    rc = launch_wgmma(c, st, gp, true, true);
-  }
-  for (CUdeviceptr t : tmp)
-    if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMM has drained
-  return rc;
+  if (!x_shape || !dy_shape || !dw_shape || !args) return fail(B200_ERR_INVALID_ARG, "conv3d_backward_weight: null shape or args");
+  return conv_backward_weight(c, s, conv_nd("conv3d_backward_weight", *args, x_shape, dw_shape), in_dtype, out_dtype, x, x_shape, x_strides, dy,
+                              dy_shape, dy_strides, dw, dw_shape, dw_strides);
 }
 
 // ------------------------------------------------------------------------------------------------ transposed convolution
@@ -3841,18 +3597,18 @@ extern "C" int b200_conv3d_backward_weight(b200_ctx* c, b200_stream s, b200_dtyp
 // is the fused epilogue, that a phase no tap reaches stores act(bias) instead of a memset's zeros, and the strided launch:
 // every phase of the layer in one conv2d_tconv_* / conv3d_tconv_* launch (gemm_wgmma.cu: CB_TCONV).
 
-// One output phase: its per-dimension phases (D, H, W; a 2-D layer has a unit depth phase), pixels, k-blocks, the element
-// offset of its weight block and the address of its first output pixel.
+// One output phase: its per-dimension phases, pixels, k-blocks, the element offset of its weight block and the address of
+// its first output pixel.
 struct TconvRun {
   const DgradPhase1D* q[3];
   uint64_t M, num_kb, woff, out;
 };
 
 // The phase-batched launches of a strided transposed convolution: the runs sorted by k-blocks (most first, ties in phase
-// order), kTconvMaxPhases per launch.  x is read through xo (extents X = (D, H, W), 2-D: D = 1), the weight blocks from wbuf
-// ([Cout][taps][cp] per phase); dx_s = output strides (n, d, h, w) of one phase's pixel grid, pitch = the output pixel pitch.
-static int launch_tconv(b200_ctx* c, CUstream st, int dims, b200_dtype in_dtype, b200_dtype out_dtype, const NdhwcOperand& xo, uint64_t N,
-                        const uint64_t X[3], uint64_t Cout, CUdeviceptr wbuf, std::vector<TconvRun> runs, const uint64_t dx_s[4], uint64_t pitch,
+// order), kTconvMaxPhases per launch.  x is read through xo (extents cv.O), the weight blocks from wbuf ([Cout][taps][cp]
+// per phase); dx_s = output strides (n, d, h, w) of one phase's pixel grid, pitch = the output pixel pitch.
+static int launch_tconv(b200_ctx* c, CUstream st, const ConvNd& cv, b200_dtype in_dtype, b200_dtype out_dtype, const ConvOperand& xo, uint64_t N,
+                        uint64_t Cout, CUdeviceptr wbuf, std::vector<TconvRun> runs, const uint64_t dx_s[4], uint64_t pitch,
                         const b200_epilogue* ep) {
   const size_t osz = dtype_size(out_dtype);
   const uint64_t cp = xo.C, cblk = (cp + 63) / 64;
@@ -3872,7 +3628,7 @@ static int launch_tconv(b200_ctx* c, CUstream st, int dims, b200_dtype in_dtype,
   const GemmVariant& v = *vp;
   const char* io = in_dtype == B200_BF16 ? (out_dtype == B200_F32 ? "bf16_f32_" : "bf16_bf16_") : (out_dtype == B200_F32 ? "f16_f32_" : "f16_f16_");
   CUfunction f;
-  int rc = get_func(c, std::string(dims == 3 ? "conv3d_tconv_" : "conv2d_tconv_") + io + v.tag, &f);
+  int rc = get_func(c, std::string(cv.n == 3 ? "conv3d_tconv_" : "conv2d_tconv_") + io + v.tag, &f);
   if (rc) return rc;
   const unsigned smem = gemm_smem_bytes(v);
   if (!c->dry) CU_CHECK(g_drv.cuFuncSetAttribute_p(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem));
@@ -3903,27 +3659,16 @@ static int launch_tconv(b200_ctx* c, CUstream st, int dims, b200_dtype in_dtype,
       P.t_hw = q[1]->taps * q[2]->taps; P.t_w = q[2]->taps;
       P.lo_d = (int32_t)q[0]->e0; P.lo_h = (int32_t)q[1]->e0; P.lo_w = (int32_t)q[2]->e0;
       P.dil_d = q[0]->dil; P.dil_h = q[1]->dil; P.dil_w = q[2]->dil;
-      if (c->dry) {
-        const std::string head = dims == 3 ? dgrad3_phase_line("conv3d tconv phase", q, X) : dgrad2_phase_line("conv tconv phase", *q[1], *q[2], X[1], X[2]);
-        c->plan += head + " kblocks=" + std::to_string(r.num_kb) + "\n";
-      }
+      if (c->dry) c->plan += conv_phase_line(cv, "tconv", q, cv.O) + " kblocks=" + std::to_string(r.num_kb) + "\n";
       if (!r.num_kb) continue;   // no loads: the maps stay empty
       // x through im2col over the phase's pixel box; the phase's weights as (cp, taps, Cout) in [n_local x 64 channel] boxes
       CUtensorMap am, bm;
-      int lo[3], up[3];
-      for (int i = 0; i < 3; ++i) {
-        lo[2 - i] = (int)q[i]->e0;
-        up[2 - i] = (int)(q[i]->e0 + (int64_t)q[i]->extent - (int64_t)X[i]);
-      }
-      if (dims == 3) {
-        const uint64_t d5[5] = {cp, X[2], X[1], X[0], N}, s4[4] = {xo.s_w, xo.s_h, xo.s_d, xo.s_n};
-        const uint32_t one[3] = {1, 1, 1};
-        rc = encode_im2col5(c, &am, dt, 2, xo.ptr, d5, s4, lo, up, 64, 128, one);
-      } else {
-        const uint64_t d4[4] = {cp, X[2], X[1], N}, s3[3] = {xo.s_w, xo.s_h, xo.s_n};
-        rc = encode_im2col(c, &am, dt, 2, xo.ptr, d4, s3, lo, up, 64, 128, 1, 1);
-      }
-      const uint64_t taps = (uint64_t)q[0]->taps * q[1]->taps * q[2]->taps;
+      const uint64_t T[3] = {q[0]->taps, q[1]->taps, q[2]->taps}, E[3] = {q[0]->extent, q[1]->extent, q[2]->extent};
+      ConvGeom g = conv_geom(cv.n, N, cv.O, xo, T, E, Cout);
+      g.box = true;
+      for (int i = 0; i < 3; ++i) g.lo[i] = (int32_t)q[i]->e0;
+      rc = encode_conv_im2col(c, &am, dt, 2, g, xo.ptr, 128);
+      const uint64_t taps = conv_prod(T);
       if (!rc) rc = encode_tmap(c, &bm, dt, 2, wbuf + r.woff * 2, cp, taps, Cout, cp, taps * cp, 64, 1, CU_TENSOR_MAP_SWIZZLE_128B, (uint32_t)(v.block_n / v.cg));
       memcpy(&tp.a[k], &am, sizeof(am));
       memcpy(&tp.b[k], &bm, sizeof(bm));
@@ -3963,17 +3708,85 @@ static int tconv_check_output_padding(const char* what, uint64_t xi, uint64_t oi
 
 // An empty kernel (some extent 0), which the convolution's output rule does not cover: x [N, *X, Cin] and out [N, *O, C] with
 // w [Cin, *K, C], and per dimension O = (X - 1) * s - 2 * p + d * (K - 1) + op + 1 with 0 <= op < s.  The sum is empty, so
-// out is act(bias).  rank 4 or 5.
-static int tconv_check_empty_kernel(const char* what, int rank, const uint64_t* x, const uint64_t* w, const uint64_t* out,
-                                    const int64_t* s, const int64_t* p, const int64_t* d) {
-  const int n = rank - 2;
-  bool ok = x[0] == out[0] && x[rank - 1] == w[0] && w[rank - 1] == out[rank - 1];
-  for (int i = 0; i < n && ok; ++i) {
-    const int64_t op = (int64_t)out[1 + i] - (((int64_t)x[1 + i] - 1) * s[i] - 2 * p[i] + d[i] * ((int64_t)w[1 + i] - 1) + 1);
-    ok = op >= 0 && op < s[i];
+// out is act(bias).
+static int tconv_check_empty_kernel(const ConvNd& cv, const uint64_t* x, const uint64_t* w, const uint64_t* out) {
+  const int r = cv.n + 2;
+  bool ok = x[0] == out[0] && x[r - 1] == w[0] && w[r - 1] == out[r - 1];
+  for (int i = cv.first(); i < 3 && ok; ++i) {
+    const int j = cv.dim(i);
+    const int64_t op = (int64_t)out[j] - (((int64_t)x[j] - 1) * cv.s[i] - 2 * cv.p[i] + cv.d[i] * ((int64_t)w[j] - 1) + 1);
+    ok = op >= 0 && op < cv.s[i];
   }
-  if (!ok) return fail(B200_ERR_INVALID_ARG, "%s: with an empty kernel, out must be x's batch and the transposed output rule's extents", what);
+  if (!ok) return fail(B200_ERR_INVALID_ARG, "%s: with an empty kernel, out must be x's batch and the transposed output rule's extents", cv.what);
   return B200_OK;
+}
+
+// b200_conv_transpose2d / 3d in the data gradient's names: dy = x [N, *O, Cin], w [Cin, *K, C], dx = out [N, *I, C].
+static int conv_transpose(b200_ctx* c, b200_stream s, ConvNd cv, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr x, const uint64_t* x_shape,
+                          const uint64_t* x_strides, b200_dptr w, const uint64_t* w_shape, const uint64_t* w_strides, b200_dptr out,
+                          const uint64_t* out_shape, const uint64_t* out_strides, const b200_epilogue* ep) {
+  const char* what = cv.what;
+  const int n = cv.n, r = n + 2;
+  const uint64_t N = out_shape[0], C = out_shape[r - 1], Cin = w_shape[0], KK = conv_prod(cv.K);
+  int rc = conv_check_args(cv, in_dtype, out_dtype, ep, C, w_shape[r - 1]);
+  for (int i = cv.first(); i < 3 && !rc; ++i)
+    rc = tconv_check_output_padding(what, x_shape[cv.dim(i)], cv.I[i], cv.s[i], cv.p[i], cv.d[i], cv.K[i]);
+  if (!rc) rc = conv_check_shape(&cv, out_shape, w_shape, x_shape, "x");
+  if (!rc && conv_any0(cv.K)) {
+    rc = tconv_check_empty_kernel(cv, x_shape, w_shape, out_shape);
+    for (int i = cv.first(); i < 3; ++i) cv.O[i] = x_shape[cv.dim(i)];
+  }
+  if (!rc) rc = conv_check_stride(cv);   // whatever the kernel: it also bounds the phases per dimension
+  if (rc) return rc;
+  if (N == 0 || conv_any0(cv.I) || C == 0) return B200_OK;   // no output
+  const uint64_t lim = 1ull << 31, P = N * conv_prod(cv.I);
+  if (P >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * %s = %llu must be < 2^31", what, conv_names(cv, "O", " * ").c_str(), (unsigned long long)P);
+  if (KK * ((Cin + 63) / 64 * 64) >= lim)
+    return fail(B200_ERR_UNSUPPORTED, "%s: %s * Cin (Cin padded to 64) must be < 2^31", what, conv_names(cv, "K", " * ").c_str());
+  ConvPhases ph;
+  if ((rc = conv_phase_plan(cv, Cin, &ph))) return rc;
+  if ((rc = conv_check_ptrs(what, x, w, out, "output", out_dtype))) return rc;
+  const size_t osz = dtype_size(out_dtype);
+  uint64_t os[5], xs[5], ws[5];
+  conv_norm_strides(r, out_shape, out_strides, os);
+  if ((rc = conv_check_pixels(cv, "out", out_shape, os))) return rc;
+  CUstream st = resolve_stream(c, s);
+  const bool taps = Cin != 0 && KK != 0;
+  conv_norm_strides(r, x_shape, x_strides, xs);
+  conv_norm_strides(r, w_shape, w_strides, ws);
+  CUdeviceptr tmp[3] = {0, 0, 0};
+  ConvOperand y{};
+  // the weight prep (and its per-phase offsets) only when some phase has taps
+  if (taps) {
+    rc = conv_prep(c, st, in_dtype, n, x, x_shape, xs, kFlatNone, tmp, &y);
+    if (!rc) rc = conv_dgrad_weights(c, st, cv, ph, w, ws, C, Cin, y.C, &tmp[2]);
+  }
+  if (!rc && taps && cv.s[0] == 1 && cv.s[1] == 1 && cv.s[2] == 1) {
+    // one phase with every tap: the forward convolution kernel with the epilogue
+    const DgradPhase1D* q[3] = {&ph.q[0][0], &ph.q[1][0], &ph.q[2][0]};
+    ConvGeom g = conv_phase_geom(cv, N, C, q, y, os);
+    if (c->dry) c->plan += conv_phase_line(cv, "tconv", q, cv.O) + " kblocks=" + std::to_string(KK * ((y.C + 63) / 64)) + "\n";
+    GemmProblem gp = conv_problem(in_dtype, out_dtype, y.ptr, tmp[2], out, P, C, KK * ((y.C + 63) / 64 * 64), os[n], &g);
+    conv_set_epilogue(&gp, ep);
+    rc = launch_wgmma(c, st, gp, false, false);
+  } else if (!rc) {
+    // every phase with pixels, those no tap reaches included, in phase-batched launches
+    std::vector<TconvRun> runs;
+    const uint64_t cblk = taps ? (y.C + 63) / 64 : 0;
+    ph.each([&](const DgradPhase1D* const* q) {
+      if (!q[0]->extent || !q[1]->extent || !q[2]->extent) return B200_OK;
+      const uint64_t T[3] = {q[0]->taps, q[1]->taps, q[2]->taps}, E[3] = {q[0]->extent, q[1]->extent, q[2]->extent};
+      runs.push_back(TconvRun{{q[0], q[1], q[2]}, N * conv_prod(E), conv_prod(T) * cblk, taps ? ph.off(q) * C * y.C : 0,
+                              out + conv_phase_dx(cv, q, os) * osz});
+      return B200_OK;
+    });
+    if (!taps) y = ConvOperand{0, 8, 8, 8, 8, 8};
+    const uint64_t dx_s[4] = {os[0], n == 3 ? (uint64_t)cv.s[0] * os[1] : 0, (uint64_t)cv.s[1] * os[n - 1], (uint64_t)cv.s[2] * os[n]};
+    rc = launch_tconv(c, st, cv, in_dtype, out_dtype, y, N, C, tmp[2], runs, dx_s, os[n], ep);
+  }
+  for (CUdeviceptr t : tmp)
+    if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMMs have drained
+  return rc;
 }
 
 extern "C" int b200_conv_transpose2d(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr x,
@@ -3981,78 +3794,9 @@ extern "C" int b200_conv_transpose2d(b200_ctx* c, b200_stream s, b200_dtype in_d
                                      const uint64_t* w_strides, b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides,
                                      const b200_conv2d_args* args, const b200_epilogue* ep) {
   CTX_ENTER(c);
-  const char* what = "conv_transpose2d";
-  if (!x_shape || !w_shape || !out_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
-  const b200_conv2d_args& a = *args;
-  // the data gradient's names: dy = x [N, OH, OW, Cin], w [Cin, KH, KW, C], dx = out [N, H, W, C]
-  const uint64_t N = out_shape[0], H = out_shape[1], W = out_shape[2], C = out_shape[3];
-  const uint64_t Cin = w_shape[0], KH = w_shape[1], KW = w_shape[2];
-  uint64_t OH = 0, OW = 0;
-  int rc = conv_check_args(what, in_dtype, out_dtype, a, ep, C, w_shape[3]);
-  if (!rc) rc = tconv_check_output_padding(what, x_shape[1], H, a.stride_h, a.pad_h, a.dilation_h, KH);
-  if (!rc) rc = tconv_check_output_padding(what, x_shape[2], W, a.stride_w, a.pad_w, a.dilation_w, KW);
-  if (!rc) rc = conv_check_shape(what, a, out_shape, w_shape, x_shape, "x", &OH, &OW);
-  if (!rc && (KH == 0 || KW == 0)) {
-    const int64_t sv[2] = {a.stride_h, a.stride_w}, pv[2] = {a.pad_h, a.pad_w}, dv[2] = {a.dilation_h, a.dilation_w};
-    rc = tconv_check_empty_kernel(what, 4, x_shape, w_shape, out_shape, sv, pv, dv);
-    OH = x_shape[1]; OW = x_shape[2];
-  }
-  if (!rc) rc = conv_check_stride(what, a);   // whatever the kernel: it also bounds the phases per dimension
-  if (rc) return rc;
-  if (N == 0 || H == 0 || W == 0 || C == 0) return B200_OK;   // no output
-  const uint64_t lim = 1ull << 31;
-  if (N * H * W >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * OH * OW = %llu must be < 2^31", what, (unsigned long long)(N * H * W));
-  if (KH * KW * ((Cin + 63) / 64 * 64) >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: KH * KW * Cin (Cin padded to 64) must be < 2^31", what);
-  std::vector<DgradPhase1D> phs, pws;
-  bool zero_phase = false;
-  if ((rc = dgrad2_plan(what, a, H, W, KH, KW, OH, OW, Cin, &phs, &pws, &zero_phase))) return rc;
-  if ((rc = conv_check_ptrs(what, x, w, out, "output", out_dtype))) return rc;
-  const size_t osz = dtype_size(out_dtype);
-  uint64_t os[4], xs[4], ws[4];
-  conv_norm_strides(out_shape, out_strides, os);
-  if ((rc = conv_check_pixels(what, "out", out_shape, os))) return rc;
-  CUstream st = resolve_stream(c, s);
-  const bool taps = Cin != 0 && KH != 0 && KW != 0;
-  conv_norm_strides(x_shape, x_strides, xs);
-  conv_norm_strides(w_shape, w_strides, ws);
-  CUdeviceptr tmp[3] = {0, 0, 0};
-  NhwcOperand y{};
-  ConvDgradWeightsParams wp;
-  memset(&wp, 0, sizeof(wp));
-  if (taps) {
-    rc = conv_prep_nhwc(c, st, in_dtype, x, x_shape, xs, kFlatNone, tmp, &y);
-    if (!rc) rc = dgrad2_prep(c, st, w, ws, a, C, Cin, y.C, KH, KW, phs, pws, &tmp[2], &wp);
-  }
-  if (!rc && taps && a.stride_h == 1 && a.stride_w == 1) {
-    // one phase with every tap: the forward convolution kernel with the epilogue
-    const DgradPhase1D &ph = phs[0], &pw = pws[0];
-    ConvGeom g = dgrad2_geom(N, OH, OW, y.C, C, ph, pw, y, os, a);
-    if (c->dry) c->plan += dgrad2_phase_line("conv tconv phase", ph, pw, OH, OW) + " kblocks=" +
-                           std::to_string((uint64_t)ph.taps * pw.taps * ((y.C + 63) / 64)) + "\n";
-    GemmProblem gp = conv_problem(in_dtype, out_dtype, y.ptr, tmp[2], out, N * H * W, C, KH * KW * ((y.C + 63) / 64 * 64), os[2], &g);
-    if (ep) { gp.alpha = ep->alpha; gp.bias = ep->bias; gp.act = (uint32_t)ep->activation; }
-    rc = launch_wgmma(c, st, gp, false, false);
-  } else if (!rc) {
-    // every phase with pixels, those no tap reaches included, in phase-batched launches
-    static const DgradPhase1D unit = {0, 1, 0, 0, 1, 1, 1};
-    std::vector<TconvRun> runs;
-    const uint64_t cblk = taps ? (y.C + 63) / 64 : 0;
-    for (const DgradPhase1D& ph : phs)
-      for (const DgradPhase1D& pw : pws) {
-        if (!ph.extent || !pw.extent) continue;
-        TconvRun r{{&unit, &ph, &pw}, N * ph.extent * pw.extent, (uint64_t)ph.taps * pw.taps * cblk,
-                   taps ? wp.off[ph.r * a.stride_w + pw.r] : 0, out + ((uint64_t)ph.r * os[1] + (uint64_t)pw.r * os[2]) * osz};
-        runs.push_back(r);
-      }
-    if (!taps) y = NhwcOperand{0, 8, 8, 8, 8};
-    const uint64_t X[3] = {1, OH, OW};
-    const uint64_t dx_s[4] = {os[0], 0, (uint64_t)a.stride_h * os[1], (uint64_t)a.stride_w * os[2]};
-    const NdhwcOperand xo{y.ptr, y.C, y.s_w, y.s_h, 0, y.s_n};
-    rc = launch_tconv(c, st, 2, in_dtype, out_dtype, xo, N, X, C, tmp[2], runs, dx_s, os[2], ep);
-  }
-  for (CUdeviceptr t : tmp)
-    if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMMs have drained
-  return rc;
+  if (!x_shape || !w_shape || !out_shape || !args) return fail(B200_ERR_INVALID_ARG, "conv_transpose2d: null shape or args");
+  return conv_transpose(c, s, conv_nd("conv_transpose2d", *args, out_shape, w_shape), in_dtype, out_dtype, x, x_shape, x_strides, w, w_shape,
+                        w_strides, out, out_shape, out_strides, ep);
 }
 
 extern "C" int b200_conv_transpose3d(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr x,
@@ -4060,76 +3804,9 @@ extern "C" int b200_conv_transpose3d(b200_ctx* c, b200_stream s, b200_dtype in_d
                                      const uint64_t* w_strides, b200_dptr out, const uint64_t* out_shape, const uint64_t* out_strides,
                                      const b200_conv3d_args* args, const b200_epilogue* ep) {
   CTX_ENTER(c);
-  const char* what = "conv_transpose3d";
-  if (!x_shape || !w_shape || !out_shape || !args) return fail(B200_ERR_INVALID_ARG, "%s: null shape or args", what);
-  const b200_conv3d_args& a = *args;
-  // the data gradient's names: dy = x [N, OD, OH, OW, Cin], w [Cin, KD, KH, KW, C], dx = out [N, D, H, W, C]
-  const uint64_t N = out_shape[0], C = out_shape[4], Cin = w_shape[0];
-  const uint64_t I[3] = {out_shape[1], out_shape[2], out_shape[3]}, K[3] = {w_shape[1], w_shape[2], w_shape[3]};
-  const int64_t sv[3] = {a.stride_d, a.stride_h, a.stride_w}, pv[3] = {a.pad_d, a.pad_h, a.pad_w};
-  const int64_t dv[3] = {a.dilation_d, a.dilation_h, a.dilation_w};
-  uint64_t O[3] = {0, 0, 0};
-  int rc = conv3_check_args(what, in_dtype, out_dtype, a, ep, C, w_shape[4]);
-  for (int i = 0; i < 3 && !rc; ++i) rc = tconv_check_output_padding(what, x_shape[1 + i], I[i], sv[i], pv[i], dv[i], K[i]);
-  if (!rc) rc = conv3_check_shape(what, a, out_shape, w_shape, x_shape, "x", O);
-  if (!rc && (K[0] == 0 || K[1] == 0 || K[2] == 0)) {
-    rc = tconv_check_empty_kernel(what, 5, x_shape, w_shape, out_shape, sv, pv, dv);
-    for (int i = 0; i < 3; ++i) O[i] = x_shape[1 + i];
-  }
-  if (!rc) rc = conv3_check_stride(what, a);   // whatever the kernel: it also bounds the phases per dimension (Dgrad3Prep)
-  if (rc) return rc;
-  if (N == 0 || I[0] == 0 || I[1] == 0 || I[2] == 0 || C == 0) return B200_OK;   // no output
-  const uint64_t lim = 1ull << 31, P = N * I[0] * I[1] * I[2], KK = K[0] * K[1] * K[2];
-  if (P >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * OD * OH * OW = %llu must be < 2^31", what, (unsigned long long)P);
-  if (KK * ((Cin + 63) / 64 * 64) >= lim)
-    return fail(B200_ERR_UNSUPPORTED, "%s: KD * KH * KW * Cin (Cin padded to 64) must be < 2^31", what);
-  std::vector<DgradPhase1D> ph[3];
-  bool zero_phase = false;
-  if ((rc = dgrad3_plan(what, sv, pv, dv, I, K, O, Cin, ph, &zero_phase))) return rc;
-  if ((rc = conv_check_ptrs(what, x, w, out, "output", out_dtype))) return rc;
-  const size_t osz = dtype_size(out_dtype);
-  uint64_t os[5], xs[5], ws[5];
-  conv3_norm_strides(out_shape, out_strides, os);
-  if ((rc = conv3_check_pixels(what, "out", out_shape, os))) return rc;
-  CUstream st = resolve_stream(c, s);
-  const bool taps = Cin != 0 && KK != 0;
-  conv3_norm_strides(x_shape, x_strides, xs);
-  conv3_norm_strides(w_shape, w_strides, ws);
-  CUdeviceptr tmp[3] = {0, 0, 0};
-  NdhwcOperand y{};
-  // the weight prep (and its per-phase offsets) only when some phase has taps
-  std::unique_ptr<Dgrad3Prep> prep;
-  if (taps) {
-    rc = conv3_prep(c, st, in_dtype, x, x_shape, xs, kFlatNone, tmp, &y);
-    prep.reset(new Dgrad3Prep(ph, K, sv, pv, dv, C, y.C));
-    if (!rc) rc = dgrad3_prep(c, st, w, ws, Cin, KK, prep.get(), &tmp[2]);
-  }
-  if (!rc && taps && sv[0] == 1 && sv[1] == 1 && sv[2] == 1) {
-    const DgradPhase1D* q[3] = {&ph[0][0], &ph[1][0], &ph[2][0]};
-    ConvGeom g = dgrad3_geom(N, O, y.C, C, q, y, os, sv);
-    if (c->dry) c->plan += dgrad3_phase_line("conv3d tconv phase", q, O) + " kblocks=" + std::to_string(KK * ((y.C + 63) / 64)) + "\n";
-    GemmProblem gp = conv_problem(in_dtype, out_dtype, y.ptr, tmp[2], out, P, C, KK * ((y.C + 63) / 64 * 64), os[3], &g);
-    if (ep) { gp.alpha = ep->alpha; gp.bias = ep->bias; gp.act = (uint32_t)ep->activation; }
-    rc = launch_wgmma(c, st, gp, false, false);
-  } else if (!rc) {
-    std::vector<TconvRun> runs;
-    const uint64_t cblk = taps ? (y.C + 63) / 64 : 0;
-    for (const DgradPhase1D& pd : ph[0])
-      for (const DgradPhase1D& phh : ph[1])
-        for (const DgradPhase1D& pw : ph[2]) {
-          if (!pd.extent || !phh.extent || !pw.extent) continue;
-          TconvRun r{{&pd, &phh, &pw}, N * pd.extent * phh.extent * pw.extent, (uint64_t)pd.taps * phh.taps * pw.taps * cblk,
-                     taps ? prep->off(pd.r, phh.r, pw.r) : 0,
-                     out + ((uint64_t)pd.r * os[1] + (uint64_t)phh.r * os[2] + (uint64_t)pw.r * os[3]) * osz};
-          runs.push_back(r);
-        }
-    if (!taps) y = NdhwcOperand{0, 8, 8, 8, 8, 8};
-    const uint64_t dx_s[4] = {os[0], (uint64_t)sv[0] * os[1], (uint64_t)sv[1] * os[2], (uint64_t)sv[2] * os[3]};
-    rc = launch_tconv(c, st, 3, in_dtype, out_dtype, y, N, O, C, tmp[2], runs, dx_s, os[3], ep);
-  }
-  for (CUdeviceptr t : tmp)
-    if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMMs have drained
-  return rc;
+  if (!x_shape || !w_shape || !out_shape || !args) return fail(B200_ERR_INVALID_ARG, "conv_transpose3d: null shape or args");
+  return conv_transpose(c, s, conv_nd("conv_transpose3d", *args, out_shape, w_shape), in_dtype, out_dtype, x, x_shape, x_strides, w, w_shape,
+                        w_strides, out, out_shape, out_strides, ep);
 }
 
 // ------------------------------------------------------------------------------------------------ grouped convolution
@@ -4170,7 +3847,7 @@ static int grp_operand(b200_ctx* c, CUstream st, b200_dtype dt, uint64_t ptr, co
     for (int d = 0; d < 4; ++d) s[d] = ns[d];
     return B200_OK;
   }
-  int rc = conv_gather(c, st, dt, ptr, shape, ns, tmp);
+  int rc = conv_gather(c, st, dt, ptr, 4, shape, ns, tmp);
   *out = *tmp;
   s[3] = 1; s[2] = shape[3]; s[1] = shape[2] * shape[3]; s[0] = shape[1] * shape[2] * shape[3];
   return rc;
@@ -4190,19 +3867,20 @@ extern "C" int b200_conv2d_grouped(b200_ctx* c, b200_stream s, b200_dtype in_dty
   const b200_conv2d_args& a = *args;
   const uint64_t N = x_shape[0], H = x_shape[1], W = x_shape[2], C = x_shape[3];
   const uint64_t Cout = w_shape[0], KH = w_shape[1], KW = w_shape[2];
+  ConvNd cv = conv_nd(what, a, x_shape, w_shape);
   int rc = grp_check(what, groups, C, Cout, w_shape[3]);
-  if (!rc) rc = conv_check_args(what, in_dtype, out_dtype, a, ep, C / groups, w_shape[3]);
+  if (!rc) rc = conv_check_args(cv, in_dtype, out_dtype, ep, C / groups, w_shape[3]);
   if (rc) return rc;
   if (N == 0 || H == 0 || W == 0 || C == 0 || Cout == 0 || KH == 0 || KW == 0) return B200_OK;
-  uint64_t OH = 0, OW = 0;
-  if ((rc = conv_check_shape(what, a, x_shape, w_shape, out_shape, "out", &OH, &OW))) return rc;
+  if ((rc = conv_check_shape(&cv, x_shape, w_shape, out_shape, "out"))) return rc;
+  const uint64_t OH = cv.O[1], OW = cv.O[2];
   if ((rc = conv_check_ptrs(what, x, w, out, "output", out_dtype))) return rc;
   const size_t osz = dtype_size(out_dtype);
   const uint64_t Cg = C / groups, Coutg = Cout / groups;
   uint64_t xs[4], ws[4], os[4];
-  conv_norm_strides(x_shape, x_strides, xs);
-  conv_norm_strides(w_shape, w_strides, ws);
-  conv_norm_strides(out_shape, out_strides, os);
+  conv_norm_strides(4, x_shape, x_strides, xs);
+  conv_norm_strides(4, w_shape, w_strides, ws);
+  conv_norm_strides(4, out_shape, out_strides, os);
   if (Cg >= kGrpGemmMinCg) {
     // one b200_conv2d per group: x, w and out are read and written in place through channel slices
     const uint64_t sx[4] = {N, H, W, Cg}, sw[4] = {Coutg, KH, KW, Cg}, so[4] = {N, OH, OW, Coutg};
@@ -4217,10 +3895,10 @@ extern "C" int b200_conv2d_grouped(b200_ctx* c, b200_stream s, b200_dtype in_dty
     }
     return rc;
   }
-  if ((rc = conv_check_fwd_corners(what, a, KH, KW)) || (rc = conv_check_stride(what, a))) return rc;
+  if ((rc = conv_check_fwd(cv)) || (rc = conv_check_stride(cv))) return rc;
   const uint64_t lim = 1ull << 31;
   if (N * OH * OW >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * OH * OW = %llu must be < 2^31", what, (unsigned long long)(N * OH * OW));
-  if ((rc = conv_check_pixels(what, "out", out_shape, os))) return rc;
+  if ((rc = conv_check_pixels(cv, "out", out_shape, os))) return rc;
   const uint64_t tiles_h = (OH + kGrpTileH - 1) / kGrpTileH, tiles_w = (OW + kGrpTileW - 1) / kGrpTileW;
   const uint64_t chunks = (Cout + kGrpChunk - 1) / kGrpChunk;
   if (N * tiles_h * tiles_w >= lim || chunks > 65535)
@@ -4278,20 +3956,21 @@ extern "C" int b200_conv2d_grouped_backward_data(b200_ctx* c, b200_stream s, b20
   const b200_conv2d_args& a = *args;
   const uint64_t N = dx_shape[0], H = dx_shape[1], W = dx_shape[2], C = dx_shape[3];
   const uint64_t Cout = w_shape[0], KH = w_shape[1], KW = w_shape[2];
-  uint64_t OH = 0, OW = 0;
+  ConvNd cv = conv_nd(what, a, dx_shape, w_shape);
   int rc = grp_check(what, groups, C, Cout, w_shape[3]);
-  if (!rc) rc = conv_check_args(what, in_dtype, out_dtype, a, nullptr, C / groups, w_shape[3]);
-  if (!rc) rc = conv_check_shape(what, a, dx_shape, w_shape, dy_shape, "dy", &OH, &OW);
-  if (!rc && KH && KW) rc = conv_check_stride(what, a);
+  if (!rc) rc = conv_check_args(cv, in_dtype, out_dtype, nullptr, C / groups, w_shape[3]);
+  if (!rc) rc = conv_check_shape(&cv, dx_shape, w_shape, dy_shape, "dy");
+  if (!rc && KH && KW) rc = conv_check_stride(cv);
   if (rc) return rc;
+  const uint64_t OH = cv.O[1], OW = cv.O[2];
   if (N == 0 || H == 0 || W == 0 || C == 0) return B200_OK;   // no dx
   if ((rc = conv_check_ptrs(what, dy, w, dx, "dx", out_dtype))) return rc;
   const size_t osz = dtype_size(out_dtype);
   const uint64_t Cg = C / groups, Coutg = Cout / groups;
   uint64_t ys[4], ws[4], os[4];
-  conv_norm_strides(dy_shape, dy_strides, ys);
-  conv_norm_strides(w_shape, w_strides, ws);
-  conv_norm_strides(dx_shape, dx_strides, os);
+  conv_norm_strides(4, dy_shape, dy_strides, ys);
+  conv_norm_strides(4, w_shape, w_strides, ws);
+  conv_norm_strides(4, dx_shape, dx_strides, os);
   if (Cg >= kGrpGemmMinCg) {
     const uint64_t sy[4] = {N, OH, OW, Coutg}, sw[4] = {Coutg, KH, KW, Cg}, sx[4] = {N, H, W, Cg};
     for (uint64_t g = 0; g < groups && !rc; ++g)
@@ -4299,10 +3978,10 @@ extern "C" int b200_conv2d_grouped_backward_data(b200_ctx* c, b200_stream s, b20
                                      dx + g * Cg * os[3] * osz, sx, os, args);
     return rc;
   }
-  if (KH && KW && (rc = conv_check_fwd_corners(what, a, KH, KW))) return rc;
+  if (KH && KW && (rc = conv_check_fwd(cv))) return rc;
   const uint64_t lim = 1ull << 31;
   if (N * H * W >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * H * W = %llu must be < 2^31", what, (unsigned long long)(N * H * W));
-  if ((rc = conv_check_pixels(what, "dx", dx_shape, os))) return rc;
+  if ((rc = conv_check_pixels(cv, "dx", dx_shape, os))) return rc;
   const uint64_t chunks = (C + kGrpChunk - 1) / kGrpChunk;
   if (chunks > 65535) return fail(B200_ERR_UNSUPPORTED, "%s: C must be <= 2^21", what);
   CUstream st = resolve_stream(c, s);
@@ -4351,23 +4030,24 @@ extern "C" int b200_conv2d_grouped_backward_weight(b200_ctx* c, b200_stream s, b
   const b200_conv2d_args& a = *args;
   const uint64_t N = x_shape[0], H = x_shape[1], W = x_shape[2], C = x_shape[3];
   const uint64_t Cout = dw_shape[0], KH = dw_shape[1], KW = dw_shape[2];
-  uint64_t OH = 0, OW = 0;
+  ConvNd cv = conv_nd(what, a, x_shape, dw_shape);
   int rc = grp_check(what, groups, C, Cout, dw_shape[3]);
-  if (!rc) rc = conv_check_args(what, in_dtype, out_dtype, a, nullptr, C / groups, dw_shape[3]);
-  if (!rc) rc = conv_check_shape(what, a, x_shape, dw_shape, dy_shape, "dy", &OH, &OW);
-  if (!rc && KH && KW) rc = conv_check_stride(what, a);
+  if (!rc) rc = conv_check_args(cv, in_dtype, out_dtype, nullptr, C / groups, dw_shape[3]);
+  if (!rc) rc = conv_check_shape(&cv, x_shape, dw_shape, dy_shape, "dy");
+  if (!rc && KH && KW) rc = conv_check_stride(cv);
   if (rc) return rc;
   if (Cout == 0 || C == 0 || KH == 0 || KW == 0) return B200_OK;   // no dw
-  if ((rc = conv_check_fwd_corners(what, a, KH, KW))) return rc;
+  if ((rc = conv_check_fwd(cv))) return rc;
+  const uint64_t OH = cv.O[1], OW = cv.O[2];
   const uint64_t P = N * OH * OW, lim = 1ull << 31;
   if (P >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: N * OH * OW = %llu must be < 2^31", what, (unsigned long long)P);
   if ((rc = conv_check_ptrs(what, x, dy, dw, "dw", out_dtype))) return rc;
   const size_t osz = dtype_size(out_dtype);
   const uint64_t Cg = C / groups, Coutg = Cout / groups;
   uint64_t xs[4], ys[4], ds[4];
-  conv_norm_strides(x_shape, x_strides, xs);
-  conv_norm_strides(dy_shape, dy_strides, ys);
-  conv_norm_strides(dw_shape, dw_strides, ds);
+  conv_norm_strides(4, x_shape, x_strides, xs);
+  conv_norm_strides(4, dy_shape, dy_strides, ys);
+  conv_norm_strides(4, dw_shape, dw_strides, ds);
   if (Cg >= kGrpGemmMinCg) {
     const uint64_t sx[4] = {N, H, W, Cg}, sy[4] = {N, OH, OW, Coutg}, sw[4] = {Coutg, KH, KW, Cg};
     for (uint64_t g = 0; g < groups && !rc; ++g)
@@ -4376,7 +4056,7 @@ extern "C" int b200_conv2d_grouped_backward_weight(b200_ctx* c, b200_stream s, b
     return rc;
   }
   uint64_t dw_sp = 0;
-  if ((rc = conv_check_dw(what, dw_shape, ds, osz, &dw_sp))) return rc;
+  if ((rc = conv_check_dw(cv, dw_shape, ds, osz, &dw_sp))) return rc;
   const uint64_t elems = Cout * KH * KW * Cg;
   if (elems >= lim) return fail(B200_ERR_UNSUPPORTED, "%s: Cout * KH * KW * C / groups = %llu must be < 2^31", what, (unsigned long long)elems);
   uint64_t seg_len = 0, nseg = 0;
@@ -4482,7 +4162,7 @@ static AttnView attn_view(uint64_t ptr, b200_dtype dt, const uint64_t* shape, co
   uint64_t st3[4] = {0, 0, 0, 0};
   if (thd && strides) memcpy(st3 + 1, strides, 3 * sizeof(uint64_t));
   for (int d = 0; d < 4; ++d) v.shape[d] = !thd ? shape[d] : d ? shape[d - 1] : 1;
-  conv_norm_strides(v.shape, thd && strides ? st3 : strides, v.ns);
+  conv_norm_strides(4, v.shape, thd && strides ? st3 : strides, v.ns);
   v.row = layout == kAttnBHSD ? 2 : 1;
   v.head = layout == kAttnBHSD ? 1 : 2;
   return v;
