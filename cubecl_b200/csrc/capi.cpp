@@ -882,47 +882,62 @@ static unsigned gemm_q8_smem_bytes(const GemmVariant& v) {
   return 1024 + gemm_q8_stages(v) * (16384 + v.block_n * 128 + (128 + v.block_n) * 16) + 1024 + 16384;
 }
 
-static int encode_tmap(b200_ctx* c, CUtensorMap* out, CUtensorMapDataType dt, size_t esz, uint64_t base, uint64_t d0,
-                       uint64_t d1, uint64_t d2, uint64_t s1_elems, uint64_t s2_elems, uint32_t b0, uint32_t b1,
-                       CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B, uint32_t b2 = 1) {
+// What every tensor-map encoder shares: a dry run appends line() to the plan and leaves the map zero; otherwise the map is
+// looked up by key (with the L2 promotion appended) or made by encode(promotion) and cached.
+template <class Line, class Encode>
+static int encode_cached(b200_ctx* c, CUtensorMap* out, std::string key, Line line, Encode encode) {
+  if (c->dry) {
+    c->plan += line();
+    memset(out, 0, sizeof(*out));
+    return B200_OK;
+  }
   // L2 promotion: how much of a line's neighbourhood a TMA load pulls into L2 (tuning knob; 256 B measured best so far)
   const int promo_bytes = atoi(opt(c, "gemm.l2_promotion", "256").c_str());
   const CUtensorMapL2promotion promo = promo_bytes >= 256 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B
                                        : promo_bytes >= 128 ? CU_TENSOR_MAP_L2_PROMOTION_L2_128B
                                        : promo_bytes >= 64 ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B : CU_TENSOR_MAP_L2_PROMOTION_NONE;
-  char key[256];
-  snprintf(key, sizeof(key), "%d|%d|%llx|%llu|%llu|%llu|%llu|%llu|%u|%u|%u|%d", (int)dt, (int)swz, (unsigned long long)base,
-           (unsigned long long)d0, (unsigned long long)d1, (unsigned long long)d2, (unsigned long long)s1_elems,
-           (unsigned long long)s2_elems, b0, b1, b2, (int)promo);
-  if (c->dry) {
-    char line[256];
-    if (b2 == 1)
-      snprintf(line, sizeof(line), "tmap esz=%zu dims=(%llu,%llu,%llu) strides=(%llu,%llu) box=(%u,%u) swizzle=%d\n", esz,
-               (unsigned long long)d0, (unsigned long long)d1, (unsigned long long)d2, (unsigned long long)(s1_elems * esz),
-               (unsigned long long)(s2_elems * esz), b0, b1, (int)swz);
-    else
-      snprintf(line, sizeof(line), "tmap esz=%zu dims=(%llu,%llu,%llu) strides=(%llu,%llu) box=(%u,%u,%u) swizzle=%d\n", esz,
-               (unsigned long long)d0, (unsigned long long)d1, (unsigned long long)d2, (unsigned long long)(s1_elems * esz),
-               (unsigned long long)(s2_elems * esz), b0, b1, b2, (int)swz);
-    c->plan += line;
-    memset(out, 0, sizeof(*out));
-    return B200_OK;
-  }
+  key += "|" + std::to_string((int)promo);
   auto it = c->tmap_cache.find(key);
   if (it != c->tmap_cache.end()) { *out = it->second; return B200_OK; }
-  cuuint64_t dims[3] = {d0, d1, d2};
-  cuuint64_t strides[2] = {s1_elems * esz, s2_elems * esz};
-  cuuint32_t box[3] = {b0, b1, b2};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = g_drv.cuTensorMapEncodeTiled_p(out, dt, 3, reinterpret_cast<void*>(base), dims, strides, box, estr,
-                                              CU_TENSOR_MAP_INTERLEAVE_NONE, swz, promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS)
-    return fail(B200_ERR_INVALID_ARG, "cuTensorMapEncodeTiled failed: %s (dims %llu,%llu,%llu strides %llu,%llu box %u,%u)",
-                cu_err(r), (unsigned long long)d0, (unsigned long long)d1, (unsigned long long)d2,
-                (unsigned long long)strides[0], (unsigned long long)strides[1], b0, b1);
+  const int rc = encode(promo);
+  if (rc) return rc;
   if (c->tmap_cache.size() > 512) c->tmap_cache.clear();
   c->tmap_cache[key] = *out;
   return B200_OK;
+}
+
+static int encode_tmap(b200_ctx* c, CUtensorMap* out, CUtensorMapDataType dt, size_t esz, uint64_t base, uint64_t d0,
+                       uint64_t d1, uint64_t d2, uint64_t s1_elems, uint64_t s2_elems, uint32_t b0, uint32_t b1,
+                       CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B, uint32_t b2 = 1) {
+  char key[256];
+  snprintf(key, sizeof(key), "%d|%d|%llx|%llu|%llu|%llu|%llu|%llu|%u|%u|%u", (int)dt, (int)swz, (unsigned long long)base,
+           (unsigned long long)d0, (unsigned long long)d1, (unsigned long long)d2, (unsigned long long)s1_elems,
+           (unsigned long long)s2_elems, b0, b1, b2);
+  auto line = [&] {
+    char l[256];
+    if (b2 == 1)
+      snprintf(l, sizeof(l), "tmap esz=%zu dims=(%llu,%llu,%llu) strides=(%llu,%llu) box=(%u,%u) swizzle=%d\n", esz,
+               (unsigned long long)d0, (unsigned long long)d1, (unsigned long long)d2, (unsigned long long)(s1_elems * esz),
+               (unsigned long long)(s2_elems * esz), b0, b1, (int)swz);
+    else
+      snprintf(l, sizeof(l), "tmap esz=%zu dims=(%llu,%llu,%llu) strides=(%llu,%llu) box=(%u,%u,%u) swizzle=%d\n", esz,
+               (unsigned long long)d0, (unsigned long long)d1, (unsigned long long)d2, (unsigned long long)(s1_elems * esz),
+               (unsigned long long)(s2_elems * esz), b0, b1, b2, (int)swz);
+    return std::string(l);
+  };
+  return encode_cached(c, out, key, line, [&](CUtensorMapL2promotion promo) -> int {
+    cuuint64_t dims[3] = {d0, d1, d2};
+    cuuint64_t strides[2] = {s1_elems * esz, s2_elems * esz};
+    cuuint32_t box[3] = {b0, b1, b2};
+    cuuint32_t estr[3] = {1, 1, 1};
+    CUresult r = g_drv.cuTensorMapEncodeTiled_p(out, dt, 3, reinterpret_cast<void*>(base), dims, strides, box, estr,
+                                                CU_TENSOR_MAP_INTERLEAVE_NONE, swz, promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS)
+      return fail(B200_ERR_INVALID_ARG, "cuTensorMapEncodeTiled failed: %s (dims %llu,%llu,%llu strides %llu,%llu box %u,%u)",
+                  cu_err(r), (unsigned long long)d0, (unsigned long long)d1, (unsigned long long)d2,
+                  (unsigned long long)strides[0], (unsigned long long)strides[1], b0, b1);
+    return B200_OK;
+  });
 }
 
 // im2col map of an NHWC (rank 4) or NDHWC (rank 5) tensor, dims innermost first (C, W, H, (D,) N; strides of all but C in
@@ -931,10 +946,6 @@ static int encode_tmap(b200_ctx* c, CUtensorMap* out, CUtensorMapDataType dt, si
 // rank 4 and [-16, 15] at rank 5.  Same cache as encode_tmap.
 static int encode_im2col(b200_ctx* c, CUtensorMap* out, CUtensorMapDataType dt, size_t esz, uint64_t base, int rank, const uint64_t* dims,
                          const uint64_t* strides, const int* lower, const int* upper, uint32_t channels, uint32_t pixels, const uint32_t* estr) {
-  const int promo_bytes = atoi(opt(c, "gemm.l2_promotion", "256").c_str());
-  const CUtensorMapL2promotion promo = promo_bytes >= 256 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B
-                                       : promo_bytes >= 128 ? CU_TENSOR_MAP_L2_PROMOTION_L2_128B
-                                       : promo_bytes >= 64 ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B : CU_TENSOR_MAP_L2_PROMOTION_NONE;
   const int sp = rank - 2;
   auto join = [](int n, auto f) {
     std::string t;
@@ -945,31 +956,27 @@ static int encode_im2col(b200_ctx* c, CUtensorMap* out, CUtensorMapDataType dt, 
   const std::string lower_t = "(" + join(sp, [&](int i) { return lower[i]; }) + ")", upper_t = "(" + join(sp, [&](int i) { return upper[i]; }) + ")";
   const std::string key = "im2col|" + std::to_string(rank) + "|" + std::to_string((int)dt) + "|" + std::to_string(base) + "|" + dims_j + "|" +
                           join(rank - 1, [&](int i) { return strides[i]; }) + "|" + lower_t + upper_t + estr_j + "|" + std::to_string(channels) +
-                          "|" + std::to_string(pixels) + "|" + std::to_string((int)promo);
-  if (c->dry) {
-    c->plan += std::string(rank == 5 ? "tmap im2col5d" : "tmap im2col") + " esz=" + std::to_string(esz) + " dims=(" + dims_j + ") strides=(" +
-               join(rank - 1, [&](int i) { return strides[i] * esz; }) + ") lower=" + lower_t + " upper=" + upper_t + " channels=" +
-               std::to_string(channels) + " pixels=" + std::to_string(pixels) + " estrides=(1," + estr_j + ",1) swizzle=" +
-               std::to_string((int)CU_TENSOR_MAP_SWIZZLE_128B) + "\n";
-    memset(out, 0, sizeof(*out));
+                          "|" + std::to_string(pixels);
+  auto line = [&] {
+    return std::string(rank == 5 ? "tmap im2col5d" : "tmap im2col") + " esz=" + std::to_string(esz) + " dims=(" + dims_j + ") strides=(" +
+           join(rank - 1, [&](int i) { return strides[i] * esz; }) + ") lower=" + lower_t + " upper=" + upper_t + " channels=" +
+           std::to_string(channels) + " pixels=" + std::to_string(pixels) + " estrides=(1," + estr_j + ",1) swizzle=" +
+           std::to_string((int)CU_TENSOR_MAP_SWIZZLE_128B) + "\n";
+  };
+  return encode_cached(c, out, key, line, [&](CUtensorMapL2promotion promo) -> int {
+    cuuint64_t gdim[5], gstr[4];
+    cuuint32_t es[5] = {1, 1, 1, 1, 1};
+    for (int i = 0; i < rank; ++i) gdim[i] = dims[i];
+    for (int i = 0; i < rank - 1; ++i) gstr[i] = strides[i] * esz;
+    for (int i = 0; i < sp; ++i) es[1 + i] = estr[i];
+    CUresult r = g_drv.cuTensorMapEncodeIm2col_p(out, dt, rank, reinterpret_cast<void*>(base), gdim, gstr, lower, upper, channels, pixels, es,
+                                                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, promo,
+                                                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS)
+      return fail(B200_ERR_INVALID_ARG, "cuTensorMapEncodeIm2col%s failed: %s (dims %s corners %s..%s)", rank == 5 ? " (rank 5)" : "", cu_err(r),
+                  dims_j.c_str(), lower_t.c_str(), upper_t.c_str());
     return B200_OK;
-  }
-  auto it = c->tmap_cache.find(key);
-  if (it != c->tmap_cache.end()) { *out = it->second; return B200_OK; }
-  cuuint64_t gdim[5], gstr[4];
-  cuuint32_t es[5] = {1, 1, 1, 1, 1};
-  for (int i = 0; i < rank; ++i) gdim[i] = dims[i];
-  for (int i = 0; i < rank - 1; ++i) gstr[i] = strides[i] * esz;
-  for (int i = 0; i < sp; ++i) es[1 + i] = estr[i];
-  CUresult r = g_drv.cuTensorMapEncodeIm2col_p(out, dt, rank, reinterpret_cast<void*>(base), gdim, gstr, lower, upper, channels, pixels, es,
-                                               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, promo,
-                                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS)
-    return fail(B200_ERR_INVALID_ARG, "cuTensorMapEncodeIm2col%s failed: %s (dims %s corners %s..%s)", rank == 5 ? " (rank 5)" : "", cu_err(r),
-                dims_j.c_str(), lower_t.c_str(), upper_t.c_str());
-  if (c->tmap_cache.size() > 512) c->tmap_cache.clear();
-  c->tmap_cache[key] = *out;
-  return B200_OK;
+  });
 }
 
 // Geometry of a 2-D or 3-D convolution run as an implicit GEMM: x is N(D)HWC with unit channel stride, w is
@@ -1195,17 +1202,82 @@ static const GemmVariant* pick_variant(b200_ctx* c, const GemmProblem& g, SkPlan
   return best;
 }
 
+// The shared host path of every wgmma GEMM launch (launch_wgmma, b200_matmul_grouped, launch_tconv): kernel lookup, operand
+// and output maps, the common GemmParams fields, and the clustered launch.  What a family picks itself stays with it: the
+// variant policy, the kernel name and its own parameter fields.
+
+// The kernel `name`, allowed `smem` bytes of dynamic shared memory.
+static int gemm_kernel(b200_ctx* c, const std::string& name, unsigned smem, CUfunction* f) {
+  int rc = get_func(c, name, f);
+  if (rc) return rc;
+  if (!c->dry) CU_CHECK(g_drv.cuFuncSetAttribute_p(*f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem));
+  return B200_OK;
+}
+
+// The map of one A / B operand, `mn` x K elements of `batch` entries (strides in elements): K-major (rows of K) in [128 B of K x
+// `rows`] boxes, or MN-major (rows of the M / N extent) in [128 B x 128 B of K] chunks.  A single row's degenerate stride is
+// replaced by the 16-byte padded row, and a broadcast operand (batch stride 0, or one entry) is one map batch.
+static int encode_operand(b200_ctx* c, CUtensorMap* m, CUtensorMapDataType dt, size_t esz, uint64_t ptr, uint64_t mn, uint64_t K,
+                          uint64_t batch, uint64_t s_mn, uint64_t s_k, uint64_t s_b, bool mn_major, uint32_t rows) {
+  const uint64_t q = 16 / esz;
+  const uint32_t chunk = static_cast<uint32_t>(128 / esz);
+  const bool bcast = s_b == 0 || batch == 1;
+  if (!mn_major) {
+    const uint64_t s = mn > 1 ? s_mn : (K + q - 1) / q * q;
+    return encode_tmap(c, m, dt, esz, ptr, K, mn, bcast ? 1 : batch, s, bcast ? s * mn : s_b, chunk, rows);
+  }
+  const uint64_t s = K > 1 ? s_k : (mn + q - 1) / q * q;
+  return encode_tmap(c, m, dt, esz, ptr, mn, K, bcast ? 1 : batch, s, bcast ? s * K : s_b, chunk, chunk);
+}
+
+// The GemmParams fields every wgmma GEMM launch fills (the rest zero): out [batch, M, N] and its strides, the extents, the tile
+// grid (tiles_m as given, tiles_n from the variant), gemm.group_m, the K segments, the fused epilogue, and 16-byte stores when
+// every output row starts 16-byte aligned.
+static void gemm_params(b200_ctx* c, GemmParams* p, const GemmVariant& v, size_t osz, uint64_t out, uint64_t o_sm, uint64_t o_sb,
+                        uint64_t M, uint64_t N, uint64_t K, uint64_t batch, uint64_t tiles_m, const b200_epilogue* ep, uint32_t k_segments = 1) {
+  memset(p, 0, sizeof(*p));
+  p->out = out;
+  p->out_row_stride = o_sm;
+  p->out_batch_stride = o_sb;
+  p->M = (uint32_t)M; p->N = (uint32_t)N; p->K = (uint32_t)K; p->batch = (uint32_t)batch;
+  p->tiles_m = (uint32_t)tiles_m;
+  p->tiles_n = (uint32_t)((N + v.block_n - 1) / v.block_n);
+  p->group_m = (uint32_t)std::max(1, atoi(opt(c, "gemm.group_m", "8").c_str()));
+  p->k_segments = k_segments;
+  p->alpha = ep ? ep->alpha : 1.0f;
+  p->bias = ep ? ep->bias : 0;
+  p->epi_act = ep ? (uint32_t)ep->activation : 0u;
+  p->epi_on = (p->alpha != 1.0f || p->bias != 0 || p->epi_act != 0) ? 1u : 0u;
+  p->vec_store = (out % 16 == 0 && (o_sm * osz) % 16 == 0 && (o_sb * osz) % 16 == 0) ? 1u : 0u;
+}
+
+// Whole tiles leave through swizzled staging tiles and TMA stores when gemm.epilogue is tma and p's out is describable: the map
+// (N, M, batch) in [128 B x 64 rows] boxes, and p->tma_store = 1.  Otherwise the map stays zero and tiles store directly.
+static int encode_out_map(b200_ctx* c, CUtensorMap* m, size_t osz, const std::string& epi, GemmParams* p) {
+  memset(m, 0, sizeof(*m));
+  const uint64_t lim40 = 1ull << 40, M = p->M, N = p->N, o_sm = p->out_row_stride, o_sb = p->out_batch_stride;
+  if (!p->vec_store || epi != "tma" || o_sm * osz >= lim40 || o_sb * osz >= lim40 || (M != 1 && o_sm < N)) return B200_OK;
+  const uint64_t s = M > 1 ? o_sm : (N + 15) / 16 * 16;
+  const int rc = encode_tmap(c, m, osz == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_UINT16, osz, p->out, N, M, p->batch, s,
+                             p->batch > 1 ? o_sb : s * M, static_cast<uint32_t>(128 / osz), 64);
+  if (!rc) p->tma_store = 1;
+  return rc;
+}
+
+// One launch of 384-thread CTAs in clusters of v.cg: one cluster per work unit, at most one per SM (pair).
+static int gemm_launch(b200_ctx* c, CUstream st, CUfunction f, const GemmVariant& v, uint64_t units, unsigned smem, void** args) {
+  const unsigned clusters = (unsigned)std::min<uint64_t>(units, (uint64_t)std::max(1, c->props.num_sms / v.cg));
+  return launch(c, f, clusters * v.cg, 1, 1, 384, smem, v.cg, st, args);
+}
+
 static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_mn, bool b_mn) {
   const size_t esz = dtype_size(g.in_dtype), osz = dtype_size(g.out_dtype);
   const char* in_tag = g.q == 1 ? "q8" : g.q == 2 ? "q8t" : g.mx ? "mx" : g.in_dtype == B200_BF16 ? "bf16" : g.in_dtype == B200_F16 ? "f16" : g.in_dtype == B200_F8E4M3 ? "e4m3"
                        : g.in_dtype == B200_F8E5M2 ? "e5m2" : g.in_dtype == B200_U8 ? "u8" : g.in_dtype == B200_I8 ? "s8" : "tf32";
   const char* out_tag = g.out_dtype == B200_BF16 ? "bf16" : g.out_dtype == B200_F16 ? "f16" : g.out_dtype == B200_I32 ? "i32" : "f32";
-  const uint32_t block_k = static_cast<uint32_t>(128 / esz);
-  const std::string forced = opt(c, "gemm.variant", "auto");
-  const uint64_t k_segments = (g.a_lo != 0 && g.b_lo != 0) ? 3 : 1;
   SkPlan best_sk;
   const GemmVariant* best = pick_variant(c, g, &best_sk);
-  if (!best) return fail(B200_ERR_INVALID_ARG, "gemm.variant '%s' is not a wgmma variant", forced.c_str());
+  if (!best) return fail(B200_ERR_INVALID_ARG, "gemm.variant '%s' is not a wgmma variant", opt(c, "gemm.variant", "auto").c_str());
   if (best_sk.bad_option) return fail(B200_ERR_INVALID_ARG, "gemm.split_k must be auto, off, on or 1..8");
   const GemmVariant& v = *best;
 
@@ -1213,11 +1285,10 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
   const std::string cpfx = g.conv && g.conv->n == 3 ? "conv3d_" : "conv2d_";
   const std::string name = g.conv ? cpfx + (cmode == 1 ? "dgrad_" : cmode == 2 ? "wgrad_" : "") + in_tag + "_" + out_tag + "_" + v.tag
                                   : std::string("gemm_") + in_tag + "_" + out_tag + "_" + v.tag + (a_mn ? "_m" : "_k") + (b_mn ? "n" : "k");
-  CUfunction f;
-  int rc = get_func(c, name, &f);
-  if (rc) return rc;
   const unsigned smem = g.q == 1 ? gemm_q8_smem_bytes(v) : gemm_smem_bytes(v);
-  if (!c->dry) CU_CHECK(g_drv.cuFuncSetAttribute_p(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem));
+  CUfunction f;
+  int rc = gemm_kernel(c, name, smem, &f);
+  if (rc) return rc;
 
   const CUtensorMapDataType dt = g.in_dtype == B200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
                                  : g.in_dtype == B200_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
@@ -1226,17 +1297,9 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
   const bool a_bcast = (g.a_sb == 0 || g.batch == 1), b_bcast = (g.b_sb == 0 || g.batch == 1);
   CUtensorMap ta, tb;
   auto pad16 = [&](uint64_t elems) { const uint64_t q = 16 / esz; return (elems + q - 1) / q * q; };
-  const uint32_t chunk = static_cast<uint32_t>(128 / esz);  // MN-major operands (16-bit): elements per 128-byte row
   const uint32_t n_local = v.block_n / v.cg;   // B rows each CTA of a pair loads (multicast to both)
-  if (g.conv && cmode != 2) {
-    rc = encode_conv_im2col(c, &ta, dt, esz, *g.conv, g.a, 128);
-  } else if (!a_mn) {
-    const uint64_t a_sm = g.M > 1 ? g.a_sm : pad16(g.K);
-    rc = encode_tmap(c, &ta, dt, esz, g.a, g.K, g.M, a_bcast ? 1 : g.batch, a_sm, a_bcast ? a_sm * g.M : g.a_sb, block_k, 128);
-  } else {
-    const uint64_t a_sk = g.K > 1 ? g.a_sk : pad16(g.M);
-    rc = encode_tmap(c, &ta, dt, esz, g.a, g.M, g.K, a_bcast ? 1 : g.batch, a_sk, a_bcast ? a_sk * g.K : g.a_sb, chunk, block_k);
-  }
+  if (g.conv && cmode != 2) rc = encode_conv_im2col(c, &ta, dt, esz, *g.conv, g.a, 128);
+  else rc = encode_operand(c, &ta, dt, esz, g.a, g.M, g.K, g.batch, g.a_sm, g.a_sk, g.a_sb, a_mn, 128);
   if (rc) return rc;
   if (cmode == 2) {
     // weight gradient: 64 pixels x 64 channels of x per MN-major B chunk
@@ -1245,31 +1308,21 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
     // [n_local output channels x 64 channels] of one kernel position
     const ConvGeom& cv = *g.conv;
     rc = encode_tmap(c, &tb, dt, esz, g.b, cv.C, cv.K[0] * cv.K[1] * cv.K[2], cv.Cout, cv.w_sp, cv.w_sco, 64, 1, CU_TENSOR_MAP_SWIZZLE_128B, n_local);
-  } else if (!b_mn) {
-    const uint64_t b_sn = g.N > 1 ? g.b_sn : pad16(g.K);
-    rc = encode_tmap(c, &tb, dt, esz, g.b, g.K, g.N, b_bcast ? 1 : g.batch, b_sn, b_bcast ? b_sn * g.N : g.b_sb, block_k, n_local);
   } else {
-    const uint64_t b_sk = g.K > 1 ? g.b_sk : pad16(g.N);
-    rc = encode_tmap(c, &tb, dt, esz, g.b, g.N, g.K, b_bcast ? 1 : g.batch, b_sk, b_bcast ? b_sk * g.K : g.b_sb, chunk, block_k);
+    rc = encode_operand(c, &tb, dt, esz, g.b, g.N, g.K, g.batch, g.b_sn, g.b_sk, g.b_sb, b_mn, n_local);
   }
   if (rc) return rc;
-  // 3xTF32: compact low parts (K-major: [rows, K]); hybrid: bf16 pair buffers
+  // K-major low parts, one compact [rows, K padded to 16 bytes] matrix per entry: 3xTF32's f32 lo, or the hybrid schedule's
+  // bf16 pair buffers, planes [0, entries) = bf16(x) then [entries, 2 entries) = bf16(lo), 64 elements of K per stage
   CUtensorMap ta_lo = ta, tb_lo = tb;
   const bool split = (g.a_lo != 0 && g.b_lo != 0);
-  if (split && g.hybrid) {
-    // bf16 pair buffers: planes [0, entries) = bf16(x), [entries, 2 entries) = bf16(lo); 64 elements of K per stage
-    const uint64_t ab = a_bcast ? 1 : g.batch, bb = b_bcast ? 1 : g.batch;
-    auto pad8 = [](uint64_t e) { return (e + 7) / 8 * 8; };
-    const CUtensorMapDataType d16 = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-    rc = encode_tmap(c, &ta_lo, d16, 2, g.a_lo, g.K, g.M, 2 * ab, pad8(g.K), pad8(g.K) * g.M, 64, 128);
+  if (split) {
+    const CUtensorMapDataType ldt = g.hybrid ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : dt;
+    const size_t lsz = g.hybrid ? 2 : esz;
+    const uint64_t planes = g.hybrid ? 2 : 1, kp = g.hybrid ? (g.K + 7) / 8 * 8 : pad16(g.K);
+    rc = encode_operand(c, &ta_lo, ldt, lsz, g.a_lo, g.M, g.K, planes * (a_bcast ? 1 : g.batch), kp, 1, kp * g.M, false, 128);
     if (rc) return rc;
-    rc = encode_tmap(c, &tb_lo, d16, 2, g.b_lo, g.K, g.N, 2 * bb, pad8(g.K), pad8(g.K) * g.N, 64, n_local);
-    if (rc) return rc;
-  } else if (split) {
-    const uint64_t ab = a_bcast ? 1 : g.batch, bb = b_bcast ? 1 : g.batch;
-    rc = encode_tmap(c, &ta_lo, dt, esz, g.a_lo, g.K, g.M, ab, pad16(g.K), pad16(g.K) * g.M, block_k, 128);
-    if (rc) return rc;
-    rc = encode_tmap(c, &tb_lo, dt, esz, g.b_lo, g.K, g.N, bb, pad16(g.K), pad16(g.K) * g.N, block_k, n_local);
+    rc = encode_operand(c, &tb_lo, ldt, lsz, g.b_lo, g.N, g.K, planes * (b_bcast ? 1 : g.batch), kp, 1, kp * g.N, false, n_local);
     if (rc) return rc;
   } else if (g.q == 1) {
     // effective-scale tiles of one stage: [128 / Bk blocks][128 rows] of A, [128 / Bk][block_n] of B (no swizzle)
@@ -1284,12 +1337,14 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
   }
 
   GemmParams p;
-  memset(&p, 0, sizeof(p));
+  b200_epilogue ep{};
+  ep.alpha = g.alpha; ep.activation = (int32_t)g.act; ep.bias = g.bias;
+  const uint64_t tile_m = 128ull * v.cg * v.mt;
+  gemm_params(c, &p, v, osz, g.out, g.o_sm, g.o_sb, g.M, g.N, g.K, g.batch, (g.M + tile_m - 1) / tile_m, &ep, split ? 3 : 1);
   if (g.rhs_dtype >= 0 && g.rhs_dtype != g.in_dtype) {
     p.fmt_b = (g.rhs_dtype == B200_F8E5M2 || g.rhs_dtype == B200_I8) ? 1u : 0u;   // 0 = e4m3 / u8, 1 = e5m2 / s8
     p.fmt_mixed = 1;
   }
-  p.k_segments = (uint32_t)k_segments;
   if (split && g.hybrid) {
     p.hyb = 1;
     p.hyb_nba = a_bcast ? 1u : (uint32_t)g.batch;
@@ -1311,49 +1366,31 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
     }
   }
   p.q_ga = g.q_ga; p.q_gb = g.q_gb;
-  p.alpha = g.alpha; p.bias = g.bias; p.epi_act = g.act;
-  p.epi_on = (g.alpha != 1.0f || g.bias != 0 || g.act != 0) ? 1u : 0u;
-  p.out = g.out;
-  p.out_row_stride = g.o_sm;
-  p.out_batch_stride = g.o_sb;
-  p.M = (uint32_t)g.M; p.N = (uint32_t)g.N; p.K = (uint32_t)g.K; p.batch = (uint32_t)g.batch;
-  p.tiles_m = (uint32_t)((g.M + 128 * v.cg * v.mt - 1) / (128 * v.cg * v.mt));
-  p.tiles_n = (uint32_t)((g.N + v.block_n - 1) / v.block_n);
-  p.group_m = (uint32_t)std::max(1, atoi(opt(c, "gemm.group_m", "8").c_str()));
   p.a_bmul = a_bcast ? 0 : 1;
   p.b_bmul = b_bcast ? 0 : 1;
-  p.vec_store = (g.out % 16 == 0 && (g.o_sm * osz) % 16 == 0 && (g.o_sb * osz) % 16 == 0) ? 1 : 0;
   if (cmode == 1 && ((p.dx_sn * osz) % 16 || (p.dx_si * osz) % 16 || (p.dx_sj * osz) % 16 || (p.dx_sd * osz) % 16)) p.vec_store = 0;
   if (cmode == 2 && (p.dw_sp * osz) % 16) p.vec_store = 0;
-  // whole tiles leave through swizzled staging tiles and TMA stores when `out` is describable: (N, M, batch), [128 B x 64 rows] boxes
   const std::string epi = opt(c, "gemm.epilogue", "tma");
   if (epi != "tma" && epi != "direct") return fail(B200_ERR_INVALID_ARG, "gemm.epilogue must be tma or direct");
   CUtensorMap tout;
   memset(&tout, 0, sizeof(tout));
-  const uint64_t lim40 = 1ull << 40;
-  if (cmode == 2 && p.vec_store && epi == "tma" && g.o_sm * osz < lim40 && p.dw_sp * osz < lim40) {
+  if (cmode == 0) {
+    rc = encode_out_map(c, &tout, osz, epi, &p);
+  } else if (cmode == 2 && p.vec_store && epi == "tma" && g.o_sm * osz < (1ull << 40) && p.dw_sp * osz < (1ull << 40)) {
     // dw as (C, Cout, KD * KH * KW): a staging tile of 64-column chunk (kpos, ch0) lands at (ch0, co, kpos), clipped at C
     const ConvGeom& cv = *g.conv;
     rc = encode_tmap(c, &tout, osz == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_UINT16, osz, g.out, cv.dw_c, g.M,
                      cv.K[0] * cv.K[1] * cv.K[2], g.o_sm, cv.dw_sp, static_cast<uint32_t>(128 / osz), 64);
-    if (rc) return rc;
-    p.tma_store = 1;
-  } else if (cmode == 0 && p.vec_store && epi == "tma" && g.o_sm * osz < lim40 && g.o_sb * osz < lim40 && (g.M == 1 || g.o_sm >= g.N)) {
-    const uint64_t o_sm = g.M > 1 ? g.o_sm : (g.N + 15) / 16 * 16;
-    const uint64_t o_sb = g.batch > 1 ? g.o_sb : o_sm * g.M;
-    rc = encode_tmap(c, &tout, osz == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_UINT16, osz, g.out, g.N, g.M, g.batch,
-                     o_sm, o_sb, static_cast<uint32_t>(128 / osz), 64);
-    if (rc) return rc;
     p.tma_store = 1;
   }
+  if (rc) return rc;
 
   const uint64_t total_tiles = static_cast<uint64_t>(p.tiles_m) * p.tiles_n * p.batch;
   if (total_tiles >= (1ull << 32)) return fail(B200_ERR_UNSUPPORTED, "too many tiles");
-  const unsigned max_clusters = (unsigned)std::max(1, c->props.num_sms / v.cg);
-  unsigned clusters = (unsigned)std::min<uint64_t>(total_tiles, max_clusters);
 
   // Stream-K head (plan chosen with the variant above)
   CUdeviceptr slabs = 0;
+  uint64_t units = total_tiles;
   p.full_tiles = (uint32_t)total_tiles;
   if (best_sk.sk_tiles) {
     if (best_sk.sk_tiles * v.cg > kWsGemmTickets) return fail(B200_ERR_UNSUPPORTED, "stream-K head: %llu tiles exceed the ticket area", (unsigned long long)best_sk.sk_tiles);
@@ -1370,7 +1407,7 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
     p.split_ws = slabs;
     p.split_tickets = ws + kWsGemmTicketOffset;
     // the head's ranges are dealt to clusters 0 .. ranges-1 (mod the grid); whole tiles to every cluster
-    clusters = (unsigned)std::min<uint64_t>(std::max<uint64_t>(p.full_tiles, best_sk.ranges), max_clusters);
+    units = std::max<uint64_t>(p.full_tiles, best_sk.ranges);
     if (c->dry) {
       char line[200];
       snprintf(line, sizeof(line), "gemm stream-k head: %u whole tiles + %u tiles in %u k-ranges (<= %u slabs per range)\n", p.full_tiles, p.sk_tiles,
@@ -1379,7 +1416,7 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
     }
   }
   void* args[] = {&ta, &tb, &ta_lo, &tb_lo, &tout, &p};
-  rc = launch(c, f, clusters * v.cg, 1, 1, 384, smem, v.cg, st, args);
+  rc = gemm_launch(c, st, f, v, units, smem, args);
   if (slabs) pool_free(c, slabs, st);  // stream-ordered: reusable by later work once this launch has drained
   return rc;
 }
@@ -1958,74 +1995,27 @@ extern "C" int b200_matmul_grouped(b200_ctx* c, b200_stream s, b200_dtype in_dty
              (ull)groups, (ull)T, (ull)tile_rows, (ull)bound);
     c->plan += line;
   }
-  CUfunction f;
-  if ((rc = get_func(c, name, &f))) return release(rc);
   const unsigned smem = gemm_smem_bytes(v) + kGroupedTableBytes;
-  if (!c->dry) {
-    CUresult r = g_drv.cuFuncSetAttribute_p(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem);
-    if (r != CUDA_SUCCESS) return release(fail(map_cu(r), "cuFuncSetAttribute: %s", cu_err(r)));
-  }
+  CUfunction f;
+  if ((rc = gemm_kernel(c, name, smem, &f))) return release(rc);
 
+  // ragged M: lhs [T, K] and rhs [G, K, N] with the group as the batch; ragged K: lhs [M, T] and rhs [T, N], both MN-major
   const CUtensorMapDataType dt = in_dtype == B200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  auto pad8 = [](uint64_t e) { return (e + 7) / 8 * 8; };
-  const uint32_t n_local = (uint32_t)(v.block_n / v.cg);
-  const uint64_t gb = b_sb != 0 ? groups : 1;   // a broadcast rhs (batch stride 0) is one map batch
   CUtensorMap ta, tb, tout;
   memset(&ta, 0, sizeof(ta));
   memset(&tb, 0, sizeof(tb));
-  memset(&tout, 0, sizeof(tout));
-  if (reads && !rk) {
-    // lhs [T, K]: K-major rows of 128 B x 128 rows, or MN-major [64 rows x 64 K] chunks
-    if (!a_mn) {
-      const uint64_t s = T > 1 ? a_mn_s : pad8(K);
-      rc = encode_tmap(c, &ta, dt, esz, a, K, T, 1, s, s * T, 64, 128);
-    } else {
-      const uint64_t s = K > 1 ? a_k_s : pad8(T);
-      rc = encode_tmap(c, &ta, dt, esz, a, T, K, 1, s, s * K, 64, 64);
-    }
-    // rhs [G, K, N] with the group as the batch: [n_local x 64 K] K-major boxes or [64 N x 64 K] MN-major chunks
-    if (!rc && !b_mn) {
-      const uint64_t s = N > 1 ? b_mn_s : pad8(K);
-      rc = encode_tmap(c, &tb, dt, esz, b, K, N, gb, s, gb > 1 ? b_sb : s * N, 64, n_local);
-    } else if (!rc) {
-      const uint64_t s = K > 1 ? b_k_s : pad8(N);
-      rc = encode_tmap(c, &tb, dt, esz, b, N, K, gb, s, gb > 1 ? b_sb : s * K, 64, 64);
-    }
-  } else if (reads) {
-    // lhs [M, T] and rhs [T, N], both MN-major: [64 rows x 64 positions] chunks
-    const uint64_t sa_k = T > 1 ? a_k_s : pad8(M), sb_k = T > 1 ? b_k_s : pad8(N);
-    rc = encode_tmap(c, &ta, dt, esz, a, M, T, 1, sa_k, sa_k * T, 64, 64);
-    if (!rc) rc = encode_tmap(c, &tb, dt, esz, b, N, T, 1, sb_k, sb_k * T, 64, 64);
+  if (reads) {
+    rc = encode_operand(c, &ta, dt, esz, a, M, K, 1, a_mn_s, a_k_s, 0, a_mn, 128);
+    if (!rc) rc = encode_operand(c, &tb, dt, esz, b, N, K, rk ? 1 : groups, b_mn_s, b_k_s, b_sb, b_mn, (uint32_t)(v.block_n / v.cg));
   }
   if (rc) return release(rc);
 
   GemmParams p;
-  memset(&p, 0, sizeof(p));
-  p.out = out;
-  p.out_row_stride = o_sm;
-  p.out_batch_stride = o_sb;
-  p.M = (uint32_t)M; p.N = (uint32_t)N; p.K = (uint32_t)K; p.batch = rk ? (uint32_t)groups : 1u;
-  p.tiles_m = (uint32_t)(rk ? tiles_m : tile_rows);
-  p.tiles_n = (uint32_t)tiles_n;
-  p.group_m = (uint32_t)std::max(1, atoi(opt(c, "gemm.group_m", "8").c_str()));
-  p.a_bmul = 0;
-  p.b_bmul = (!rk && gb > 1) ? 1u : 0u;
-  p.k_segments = 1;
-  if (ep) { p.alpha = ep->alpha; p.bias = ep->bias; p.epi_act = (uint32_t)ep->activation; }
-  else p.alpha = 1.0f;
-  p.epi_on = (p.alpha != 1.0f || p.bias != 0 || p.epi_act != 0) ? 1u : 0u;
-  p.vec_store = (out % 16 == 0 && (o_sm * osz) % 16 == 0 && (o_sb * osz) % 16 == 0) ? 1u : 0u;
+  gemm_params(c, &p, v, osz, out, o_sm, o_sb, M, N, K, rk ? groups : 1, rk ? tiles_m : tile_rows, ep);
+  p.b_bmul = (!rk && b_sb != 0 && groups > 1) ? 1u : 0u;
   p.full_tiles = (uint32_t)bound;   // whole tiles only: no stream-K head (the host does not know the tile count)
-  // whole CTA tiles leave through swizzled staging and TMA stores when out is describable: (N, rows, G) in [128 B x 64 rows]
-  // boxes; ragged M's tiles that a group's end cuts store directly
-  const uint64_t o_rows = rk ? M : T, o_b = rk ? groups : 1;
-  if (p.vec_store && epi == "tma" && (o_rows == 1 || o_sm >= N)) {
-    const uint64_t os = o_rows > 1 ? o_sm : (N + 15) / 16 * 16;
-    rc = encode_tmap(c, &tout, osz == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_UINT16, osz, out, N, o_rows, o_b, os,
-                     o_b > 1 ? o_sb : os * o_rows, (uint32_t)(128 / osz), 64);
-    if (rc) return release(rc);
-    p.tma_store = 1;
-  }
+  // ragged M's tiles that a group's end cuts store directly
+  if ((rc = encode_out_map(c, &tout, osz, epi, &p))) return release(rc);
   GroupedParams gp;
   memset(&gp, 0, sizeof(gp));
   gp.offs = offs;
@@ -2033,9 +2023,8 @@ extern "C" int b200_matmul_grouped(b200_ctx* c, b200_stream s, b200_dtype in_dty
   gp.groups = (uint32_t)groups;
   gp.T = (uint32_t)T;
   gp.mode = rk ? 1u : 0u;
-  const unsigned clusters = (unsigned)std::min<uint64_t>(bound, (uint64_t)std::max(1, c->props.num_sms / v.cg));
   void* args[] = {&ta, &tb, &tout, &gp, &p};
-  rc = launch(c, f, clusters * v.cg, 1, 1, 384, smem, v.cg, st, args);
+  rc = gemm_launch(c, st, f, v, bound, smem, args);
   return release(rc);   // stream-ordered: staged copies are reused only by later work
 }
 
@@ -3627,11 +3616,10 @@ static int launch_tconv(b200_ctx* c, CUstream st, const ConvNd& cv, b200_dtype i
   if (!vp) return fail(B200_ERR_INVALID_ARG, "gemm.variant '%s' is not a wgmma variant", opt(c, "gemm.variant", "auto").c_str());
   const GemmVariant& v = *vp;
   const char* io = in_dtype == B200_BF16 ? (out_dtype == B200_F32 ? "bf16_f32_" : "bf16_bf16_") : (out_dtype == B200_F32 ? "f16_f32_" : "f16_f16_");
-  CUfunction f;
-  int rc = get_func(c, std::string(cv.n == 3 ? "conv3d_tconv_" : "conv2d_tconv_") + io + v.tag, &f);
-  if (rc) return rc;
   const unsigned smem = gemm_smem_bytes(v);
-  if (!c->dry) CU_CHECK(g_drv.cuFuncSetAttribute_p(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem));
+  CUfunction f;
+  int rc = gemm_kernel(c, std::string(cv.n == 3 ? "conv3d_tconv_" : "conv2d_tconv_") + io + v.tag, smem, &f);
+  if (rc) return rc;
   const CUtensorMapDataType dt = in_dtype == B200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   const uint64_t tiles_n = (Cout + v.block_n - 1) / v.block_n, rows = 128ull * v.cg;
   static_assert(sizeof(CUtensorMap) == sizeof(TmapBytes), "TmapBytes holds one CUtensorMap");
@@ -3639,8 +3627,6 @@ static int launch_tconv(b200_ctx* c, CUstream st, const ConvNd& cv, b200_dtype i
     const size_t nq = std::min<size_t>(kTconvMaxPhases, runs.size() - g0);
     TconvParams tp;
     memset(&tp, 0, sizeof(tp));
-    GemmParams p;
-    memset(&p, 0, sizeof(p));
     bool vec = (pitch * osz) % 16 == 0;
     for (int i = 0; i < 4; ++i) vec = vec && (dx_s[i] * osz) % 16 == 0;
     uint64_t tiles = 0, pixels = 0;
@@ -3676,22 +3662,15 @@ static int launch_tconv(b200_ctx* c, CUstream st, const ConvNd& cv, b200_dtype i
     if (rc) break;
     if (tiles >= (1ull << 32)) return fail(B200_ERR_UNSUPPORTED, "too many tiles");
     tp.phases = (uint32_t)nq;
-    p.out = runs[g0].out;
-    p.out_row_stride = pitch;
-    p.M = (uint32_t)pixels; p.N = (uint32_t)Cout; p.K = 0; p.batch = 1;
-    p.tiles_n = (uint32_t)tiles_n;
-    p.group_m = (uint32_t)std::max(1, atoi(opt(c, "gemm.group_m", "8").c_str()));
-    p.k_segments = 1;
-    p.vec_store = vec ? 1 : 0;
+    // the tile grid is per phase (TconvPhase): tiles_m stays zero
+    GemmParams p;
+    gemm_params(c, &p, v, osz, runs[g0].out, pitch, 0, pixels, Cout, 0, 1, 0, ep);
+    if (!vec) p.vec_store = 0;
     p.cv_cblk = (uint32_t)cblk;
     p.dx_sn = dx_s[0]; p.dx_sd = dx_s[1]; p.dx_si = dx_s[2]; p.dx_sj = dx_s[3];
-    if (ep) { p.alpha = ep->alpha; p.bias = ep->bias; p.epi_act = (uint32_t)ep->activation; }
-    else p.alpha = 1.0f;
-    p.epi_on = (p.alpha != 1.0f || p.bias != 0 || p.epi_act != 0) ? 1u : 0u;
     p.full_tiles = (uint32_t)tiles;   // whole tiles only: no stream-K head
-    const unsigned clusters = (unsigned)std::min<uint64_t>(tiles, (uint64_t)std::max(1, c->props.num_sms / v.cg));
     void* args[] = {&tp, &p};
-    rc = launch(c, f, clusters * v.cg, 1, 1, 384, smem, v.cg, st, args);
+    rc = gemm_launch(c, st, f, v, tiles, smem, args);
   }
   return rc;
 }
@@ -4100,39 +4079,30 @@ extern "C" int b200_conv2d_grouped_backward_weight(b200_ctx* c, b200_stream s, b
 // cache key; encode_tmap's are unchanged.
 static int encode_tmap4(b200_ctx* c, CUtensorMap* out, CUtensorMapDataType dt, size_t esz, uint64_t base, const uint64_t dims[4],
                         const uint64_t strides[3], const uint32_t box[4], CUtensorMapSwizzle swz) {
-  const int promo_bytes = atoi(opt(c, "gemm.l2_promotion", "256").c_str());
-  const CUtensorMapL2promotion promo = promo_bytes >= 256 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B
-                                       : promo_bytes >= 128 ? CU_TENSOR_MAP_L2_PROMOTION_L2_128B
-                                       : promo_bytes >= 64 ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B : CU_TENSOR_MAP_L2_PROMOTION_NONE;
   std::string key = "tiled4d|" + std::to_string((int)dt) + "|" + std::to_string((int)swz) + "|" + std::to_string(base);
   for (int i = 0; i < 4; ++i) key += "|" + std::to_string(dims[i]) + "|" + std::to_string(box[i]);
   for (int i = 0; i < 3; ++i) key += "|" + std::to_string(strides[i]);
-  key += "|" + std::to_string((int)promo);
-  if (c->dry) {
-    char line[320];
-    snprintf(line, sizeof(line), "tmap4d esz=%zu dims=(%llu,%llu,%llu,%llu) strides=(%llu,%llu,%llu) box=(%u,%u,%u,%u) swizzle=%d\n", esz,
+  auto line = [&] {
+    char l[320];
+    snprintf(l, sizeof(l), "tmap4d esz=%zu dims=(%llu,%llu,%llu,%llu) strides=(%llu,%llu,%llu) box=(%u,%u,%u,%u) swizzle=%d\n", esz,
              (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)dims[2], (unsigned long long)dims[3],
              (unsigned long long)(strides[0] * esz), (unsigned long long)(strides[1] * esz), (unsigned long long)(strides[2] * esz), box[0],
              box[1], box[2], box[3], (int)swz);
-    c->plan += line;
-    memset(out, 0, sizeof(*out));
+    return std::string(l);
+  };
+  return encode_cached(c, out, key, line, [&](CUtensorMapL2promotion promo) -> int {
+    cuuint64_t gdim[4] = {dims[0], dims[1], dims[2], dims[3]};
+    cuuint64_t gstr[3] = {strides[0] * esz, strides[1] * esz, strides[2] * esz};
+    cuuint32_t bx[4] = {box[0], box[1], box[2], box[3]};
+    cuuint32_t estr[4] = {1, 1, 1, 1};
+    CUresult r = g_drv.cuTensorMapEncodeTiled_p(out, dt, 4, reinterpret_cast<void*>(base), gdim, gstr, bx, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                                                swz, promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS)
+      return fail(B200_ERR_INVALID_ARG, "cuTensorMapEncodeTiled (rank 4) failed: %s (dims %llu,%llu,%llu,%llu strides %llu,%llu,%llu)", cu_err(r),
+                  (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)dims[2], (unsigned long long)dims[3],
+                  (unsigned long long)gstr[0], (unsigned long long)gstr[1], (unsigned long long)gstr[2]);
     return B200_OK;
-  }
-  auto it = c->tmap_cache.find(key);
-  if (it != c->tmap_cache.end()) { *out = it->second; return B200_OK; }
-  cuuint64_t gdim[4] = {dims[0], dims[1], dims[2], dims[3]};
-  cuuint64_t gstr[3] = {strides[0] * esz, strides[1] * esz, strides[2] * esz};
-  cuuint32_t bx[4] = {box[0], box[1], box[2], box[3]};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = g_drv.cuTensorMapEncodeTiled_p(out, dt, 4, reinterpret_cast<void*>(base), gdim, gstr, bx, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                              swz, promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS)
-    return fail(B200_ERR_INVALID_ARG, "cuTensorMapEncodeTiled (rank 4) failed: %s (dims %llu,%llu,%llu,%llu strides %llu,%llu,%llu)", cu_err(r),
-                (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)dims[2], (unsigned long long)dims[3],
-                (unsigned long long)gstr[0], (unsigned long long)gstr[1], (unsigned long long)gstr[2]);
-  if (c->tmap_cache.size() > 512) c->tmap_cache.clear();
-  c->tmap_cache[key] = *out;
-  return B200_OK;
+  });
 }
 
 // An attention operand: the device pointer and dtype, the 4-D shape and normalised strides (elements) as the caller passed
