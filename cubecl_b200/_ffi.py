@@ -132,6 +132,8 @@ SIGNATURES = {
                             + [C.c_uint64, C.c_uint64] + [C.c_uint64, C.c_int, _u64p, _u64p] + [C.POINTER(Epilogue)]),
     "b200_matmul_quantized": (C.c_int, [_vp, _vp, C.POINTER(QuantOperand), C.POINTER(QuantOperand), C.c_int, C.c_uint64,
                                         C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64]),
+    "b200_matmul_quantized_fp8": (C.c_int, [_vp, _vp, C.POINTER(QuantOperand), C.POINTER(QuantOperand), C.c_int, C.c_uint64,
+                                            C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64]),
     "b200_conv2d": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, _u64p, _u64p, C.c_uint64, _u64p, _u64p, C.c_uint64, _u64p,
                               _u64p, C.POINTER(Conv2dArgs), C.POINTER(Epilogue)]),
     "b200_conv2d_backward_data": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, _u64p, _u64p, C.c_uint64, _u64p, _u64p,

@@ -23,14 +23,14 @@ BUILD = PKG / "build"
 LIBDIR = PKG / "lib"
 LIB = LIBDIR / "libcubecl_b200.so"
 
-# tag -> (source, extra nvcc flags); the GEMM source is split in nine cubins so the parts compile in parallel
+# tag -> (source, extra nvcc flags); the GEMM source is split in ten cubins so the parts compile in parallel
 CUBINS = {"gemm": ("gemm_wgmma.cu", ["-DGEMM_PART=0"]), "gemm_b": ("gemm_wgmma.cu", ["-DGEMM_PART=1"]),
           "gemm_c": ("gemm_wgmma.cu", ["-DGEMM_PART=2"]), "reduce": ("reduce.cu", []), "aux": ("aux_kernels.cu", []),
           "quant": ("quant.cu", []), "gemm_q": ("gemm_wgmma.cu", ["-DGEMM_PART=3"]),
           "quant_mm": ("quant.cu", ["-DQUANT_PART=1"]), "gemm_conv": ("gemm_wgmma.cu", ["-DGEMM_PART=4"]),
           "gemm_convbwd": ("gemm_wgmma.cu", ["-DGEMM_PART=5"]), "conv_grouped": ("conv_grouped.cu", []),
           "gemm_conv3d": ("gemm_wgmma.cu", ["-DGEMM_PART=6"]), "gemm_convt": ("gemm_wgmma.cu", ["-DGEMM_PART=7"]),
-          "gemm_grouped": ("gemm_wgmma.cu", ["-DGEMM_PART=8"]),
+          "gemm_grouped": ("gemm_wgmma.cu", ["-DGEMM_PART=8"]), "gemm_qf8": ("gemm_wgmma.cu", ["-DGEMM_PART=9"]),
           "attention": ("attention.cu", []), "attention_bwd": ("attention_bwd.cu", []),
           "attention_kv": ("attention_kv.cu", []), "attention_varlen": ("attention.cu", ["-DATTN_VARLEN"]),
           "attention_varlen_bwd": ("attention_bwd.cu", ["-DATTN_VARLEN"]),

@@ -75,6 +75,8 @@ extern const unsigned char b200_cubin_attention_paged_fp8[];
 extern const unsigned char b200_cubin_attention_paged_fp8_end[];
 extern const unsigned char b200_cubin_gemm_grouped[];
 extern const unsigned char b200_cubin_gemm_grouped_end[];
+extern const unsigned char b200_cubin_gemm_qf8[];
+extern const unsigned char b200_cubin_gemm_qf8_end[];
 }
 
 // ================================================================================================ errors
@@ -347,12 +349,13 @@ static int get_func(b200_ctx* c, const std::string& name, CUfunction* out) {
   if (it != c->funcs.end()) { *out = it->second; return B200_OK; }
   // modules are loaded in the order gemm, reduce, aux, gemm_b, gemm_c, quant, gemm_q, quant_mm, gemm_conv, gemm_convbwd,
   // conv_grouped, gemm_conv3d, gemm_convt, attention, attention_bwd, attention_kv, attention_varlen, attention_varlen_bwd,
-  // attention_kv_fp8, attention_paged, attention_paged_fp8, gemm_grouped; the kernel name says where a
+  // attention_kv_fp8, attention_paged, attention_paged_fp8, gemm_grouped, gemm_qf8; the kernel name says where a
   // kernel lives (no failing lookups, which API-level tools such as compute-sanitizer would report)
   auto starts = [&](const char* pfx) { return name.rfind(pfx, 0) == 0; };
   auto has = [&](const char* part) { return name.find(part) != std::string::npos; };
   const bool tc_gemm = starts("gemm_") && name != "gemm_simt_strided" && name != "gemm_scaled_simt";
   const size_t home = name == "conv3d_dgrad_weights" ? 2
+                      : starts("gemm_qf8_") ? 22
                       : starts("gemm_grouped_") ? 21
                       : starts("attn_fwd_paged_") && (has("_e4m3_") || has("_e5m2_")) ? 20
                       : starts("attn_fwd_paged_") ? 19
@@ -410,7 +413,8 @@ extern "C" int b200_get_cubin(const char* name, const void** image, size_t* size
   else if (!strcmp(name, "attention_paged")) { b = b200_cubin_attention_paged; e = b200_cubin_attention_paged_end; }
   else if (!strcmp(name, "attention_paged_fp8")) { b = b200_cubin_attention_paged_fp8; e = b200_cubin_attention_paged_fp8_end; }
   else if (!strcmp(name, "gemm_grouped")) { b = b200_cubin_gemm_grouped; e = b200_cubin_gemm_grouped_end; }
-  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd|conv_grouped|gemm_conv3d|gemm_convt|attention|attention_bwd|attention_kv|attention_varlen|attention_varlen_bwd|attention_kv_fp8|attention_paged|attention_paged_fp8|gemm_grouped)", name);
+  else if (!strcmp(name, "gemm_qf8")) { b = b200_cubin_gemm_qf8; e = b200_cubin_gemm_qf8_end; }
+  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd|conv_grouped|gemm_conv3d|gemm_convt|attention|attention_bwd|attention_kv|attention_varlen|attention_varlen_bwd|attention_kv_fp8|attention_paged|attention_paged_fp8|gemm_grouped|gemm_qf8)", name);
   *image = b;
   *size = static_cast<size_t>(e - b);
   return B200_OK;
@@ -479,7 +483,8 @@ extern "C" int b200_init(int device, b200_ctx** out) {
       (rc = load_module(c, b200_cubin_attention_kv_fp8, b200_cubin_attention_kv_fp8_end, "attention_kv_fp8")) ||
       (rc = load_module(c, b200_cubin_attention_paged, b200_cubin_attention_paged_end, "attention_paged")) ||
       (rc = load_module(c, b200_cubin_attention_paged_fp8, b200_cubin_attention_paged_fp8_end, "attention_paged_fp8")) ||
-      (rc = load_module(c, b200_cubin_gemm_grouped, b200_cubin_gemm_grouped_end, "gemm_grouped"))) {
+      (rc = load_module(c, b200_cubin_gemm_grouped, b200_cubin_gemm_grouped_end, "gemm_grouped")) ||
+      (rc = load_module(c, b200_cubin_gemm_qf8, b200_cubin_gemm_qf8_end, "gemm_qf8"))) {
     for (CUmodule m : c->modules) g_drv.cuModuleUnload_p(m);
     g_drv.cuDevicePrimaryCtxRelease_p(c->dev);
     return bail(rc);
@@ -1037,7 +1042,8 @@ struct GemmProblem {
   uint64_t o_sm, o_sn, o_sb;
   // integer-quantized operands (b200_matmul_quantized): s8 codes, K-major.  q = 1: per-block scales folded per Bk block of K
   // from the f32 effective-scale buffers sa_q / sb_q ([batch][K / Bk][rows padded to 4]); q = 2: per-tensor scales g_a, g_b
-  // read from the device in the epilogue
+  // read from the device in the epilogue.  q = 3 (b200_matmul_quantized_fp8): fp8 codes, in_dtype / rhs_dtype the two formats,
+  // the q = 1 fold on fresh f32 partials of the fp8 tensor cores; sa_q / sb_q cover ceil(K / Bk) blocks
   int q = 0;
   uint32_t q_bk = 0;
   uint64_t q_sa = 0, q_sb = 0, q_ga = 0, q_gb = 0;
@@ -1048,6 +1054,7 @@ struct GemmProblem {
 
 static bool variant_has(const GemmVariant& v, const GemmProblem& g) {
   if (g.conv) return !strcmp(v.tag, "2sm_n128") || !strcmp(v.tag, "1sm_n128");   // gemm_wgmma.cu: GEMM_PART 4
+  if (g.q == 3) return !strcmp(v.tag, "2sm_n128") || !strcmp(v.tag, "1sm_n128");  // gemm_wgmma.cu: GEMM_PART 9
   if (g.q == 1 && v.block_n == 256) return false;   // the per-block fold has 128-wide tiles only (gemm_wgmma.cu: GEMM_Q)
   if (!strcmp(v.tag, "2sm_n224")) return g.mx;
   if (!strcmp(v.tag, "2sm_m512")) return !g.mx && (g.in_dtype == B200_BF16 || g.in_dtype == B200_F16);
@@ -1272,11 +1279,11 @@ static int gemm_launch(b200_ctx* c, CUstream st, CUfunction f, const GemmVariant
 
 static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_mn, bool b_mn) {
   const size_t esz = dtype_size(g.in_dtype), osz = dtype_size(g.out_dtype);
-  const char* in_tag = g.q == 1 ? "q8" : g.q == 2 ? "q8t" : g.mx ? "mx" : g.in_dtype == B200_BF16 ? "bf16" : g.in_dtype == B200_F16 ? "f16" : g.in_dtype == B200_F8E4M3 ? "e4m3"
+  const char* in_tag = g.q == 1 ? "q8" : g.q == 2 ? "q8t" : g.q == 3 ? (g.in_dtype == B200_F8E4M3 ? "qf8_e4m3" : "qf8_e5m2") : g.mx ? "mx" : g.in_dtype == B200_BF16 ? "bf16" : g.in_dtype == B200_F16 ? "f16" : g.in_dtype == B200_F8E4M3 ? "e4m3"
                        : g.in_dtype == B200_F8E5M2 ? "e5m2" : g.in_dtype == B200_U8 ? "u8" : g.in_dtype == B200_I8 ? "s8" : "tf32";
   const char* out_tag = g.out_dtype == B200_BF16 ? "bf16" : g.out_dtype == B200_F16 ? "f16" : g.out_dtype == B200_I32 ? "i32" : "f32";
   SkPlan best_sk;
-  const GemmVariant* best = pick_variant(c, g, &best_sk);
+  const GemmVariant* best = pick_variant(c, g, &best_sk, g.q != 3);   // the fp8 fold runs whole tiles only
   if (!best) return fail(B200_ERR_INVALID_ARG, "gemm.variant '%s' is not a wgmma variant", opt(c, "gemm.variant", "auto").c_str());
   if (best_sk.bad_option) return fail(B200_ERR_INVALID_ARG, "gemm.split_k must be auto, off, on or 1..8");
   const GemmVariant& v = *best;
@@ -1285,7 +1292,7 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
   const std::string cpfx = g.conv && g.conv->n == 3 ? "conv3d_" : "conv2d_";
   const std::string name = g.conv ? cpfx + (cmode == 1 ? "dgrad_" : cmode == 2 ? "wgrad_" : "") + in_tag + "_" + out_tag + "_" + v.tag
                                   : std::string("gemm_") + in_tag + "_" + out_tag + "_" + v.tag + (a_mn ? "_m" : "_k") + (b_mn ? "n" : "k");
-  const unsigned smem = g.q == 1 ? gemm_q8_smem_bytes(v) : gemm_smem_bytes(v);
+  const unsigned smem = g.q == 1 || g.q == 3 ? gemm_q8_smem_bytes(v) : gemm_smem_bytes(v);
   CUfunction f;
   int rc = gemm_kernel(c, name, smem, &f);
   if (rc) return rc;
@@ -1324,9 +1331,9 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
     if (rc) return rc;
     rc = encode_operand(c, &tb_lo, ldt, lsz, g.b_lo, g.N, g.K, planes * (b_bcast ? 1 : g.batch), kp, 1, kp * g.N, false, n_local);
     if (rc) return rc;
-  } else if (g.q == 1) {
+  } else if (g.q == 1 || g.q == 3) {
     // effective-scale tiles of one stage: [128 / Bk blocks][128 rows] of A, [128 / Bk][block_n] of B (no swizzle)
-    const uint64_t nblk = g.K / g.q_bk, ra = (g.M + 3) / 4 * 4, rb = (g.N + 3) / 4 * 4;
+    const uint64_t nblk = (g.K + g.q_bk - 1) / g.q_bk, ra = (g.M + 3) / 4 * 4, rb = (g.N + 3) / 4 * 4;
     const uint32_t nsub = 128u / g.q_bk;
     rc = encode_tmap(c, &ta_lo, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, g.q_sa, ra, nblk, a_bcast ? 1 : g.batch, ra, ra * nblk, 128, nsub,
                      CU_TENSOR_MAP_SWIZZLE_NONE);
@@ -1350,7 +1357,7 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
     p.hyb_nba = a_bcast ? 1u : (uint32_t)g.batch;
     p.hyb_nbb = b_bcast ? 1u : (uint32_t)g.batch;
   }
-  if (g.q == 1) p.q_nsub = 128u / g.q_bk;
+  if (g.q == 1 || g.q == 3) p.q_nsub = 128u / g.q_bk;
   if (g.conv) {
     const ConvGeom& cv = *g.conv;
     p.cv_ohw = (uint32_t)(cv.O[1] * cv.O[2]); p.cv_ow = (uint32_t)cv.O[2];
@@ -2818,10 +2825,11 @@ static int qmm_codes(b200_ctx* c, CUstream st, const b200_quant_operand* o, uint
   return launch(c, f, grid, 1, 1, kQuantThreads, 0, 1, st, args);
 }
 
-// The f32 effective scales of one operand per GEMM block of bk elements, block-major [batch][K / bk][rows padded to 4].
+// The f32 effective scales of one operand per GEMM block of bk elements, block-major [batch][ceil(K / bk)][rows padded to 4]
+// (a short last block only for per-tensor scales: a block level divides K).
 static int qmm_scales(b200_ctx* c, CUstream st, const b200_quant_operand* o, uint64_t batch, uint64_t rows, uint64_t K, uint32_t bk,
                       CUdeviceptr* out) {
-  const uint64_t rows_pad = (rows + 3) / 4 * 4, nblk = K / bk, total = batch * nblk * rows_pad;
+  const uint64_t rows_pad = (rows + 3) / 4 * 4, nblk = (K + bk - 1) / bk, total = batch * nblk * rows_pad;
   int rc = pool_alloc(c, total * 4, out, st);
   if (rc) return rc;
   const int32_t block = o->scheme.block;
@@ -2891,6 +2899,65 @@ extern "C" int b200_matmul_quantized(b200_ctx* c, b200_stream s, const b200_quan
     if (!rc) rc = qmm_scales(c, st, rhs, batch, n, k, g.q_bk, &tmp[3]);
     g.q_sa = tmp[2]; g.q_sb = tmp[3];
   }
+  if (!rc) rc = launch_wgmma(c, st, g, false, false);
+  for (CUdeviceptr t : tmp)
+    if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMM has drained
+  return rc;
+}
+
+// fp8 codes (e4m3 / e5m2 on either side) on the fp8 tensor cores: Bk / 32 wgmma k32 steps per block into a fresh f32 partial,
+// folded as b200_matmul_quantized's per-block kernels fold their exact s32 partials (gemm_qf8_*, gemm_wgmma.cu: QM_FP8)
+extern "C" int b200_matmul_quantized_fp8(b200_ctx* c, b200_stream s, const b200_quant_operand* lhs, const b200_quant_operand* rhs,
+                                         b200_dtype out_dtype, b200_dptr out, uint64_t batch, uint64_t m, uint64_t n, uint64_t k) {
+  CTX_ENTER(c);
+  if (!lhs || !rhs) return fail(B200_ERR_INVALID_ARG, "matmul_quantized_fp8: null operand");
+  const bool empty = (batch == 0 || m == 0 || n == 0);
+  const b200_quant_operand* ops[2] = {lhs, rhs};
+  const uint64_t rows[2] = {m, n};
+  for (int i = 0; i < 2; ++i) {
+    const char* what = i == 0 ? "matmul_quantized_fp8 (lhs)" : "matmul_quantized_fp8 (rhs)";
+    const uint64_t shape[2] = {empty ? 0 : batch * rows[i], k};
+    uint64_t nel = 0, K = 0;
+    int rc = quant_check(what, &ops[i]->scheme, 2, shape, ops[i]->block_scales, ops[i]->tensor_scale, &nel, &K);
+    if (rc) return rc;
+    const int32_t v = ops[i]->scheme.value;
+    if (v == B200_QV_E2M1)
+      return fail(B200_ERR_UNSUPPORTED, "%s: e2m1 values with block scales run through b200_matmul_scaled", what);
+    if (v != B200_QV_E4M3 && v != B200_QV_E5M2)
+      return fail(B200_ERR_UNSUPPORTED, "%s: integer values run through b200_matmul_quantized", what);
+    if (ops[i]->scheme.block == 8 || ops[i]->scheme.block == 16)
+      return fail(B200_ERR_UNSUPPORTED, "%s: block %d (32, 64 or 128: fp8 wgmma consumes K in steps of 32)", what, (int)ops[i]->scheme.block);
+  }
+  if (out_dtype != B200_F32 && out_dtype != B200_BF16 && out_dtype != B200_F16)
+    return fail(B200_ERR_INVALID_ARG, "matmul_quantized_fp8: output dtype %d is not F32, BF16 or F16", (int)out_dtype);
+  if (empty) return B200_OK;
+  if (k == 0) return fail(B200_ERR_INVALID_ARG, "matmul_quantized_fp8: K must be positive");
+  if (!out || !lhs->values || !rhs->values) return fail(B200_ERR_INVALID_ARG, "matmul_quantized_fp8: null device pointer");
+  const size_t osz = dtype_size(out_dtype);
+  if (out % osz) return fail(B200_ERR_INVALID_ARG, "matmul_quantized_fp8: output pointer is not aligned to its element size");
+  if (m >= (1ull << 31) || n >= (1ull << 31) || k >= (1ull << 31) || batch >= (1ull << 20))
+    return fail(B200_ERR_UNSUPPORTED, "matmul_quantized_fp8: extent too large");
+  CUstream st = resolve_stream(c, s);
+  CUdeviceptr tmp[4] = {0, 0, 0, 0};   // lhs codes, rhs codes, lhs scales, rhs scales
+  uint64_t pa = 0, pb = 0, pitch_a = 0, pitch_b = 0;
+  int rc = qmm_codes(c, st, lhs, batch, m, k, &tmp[0], &pa, &pitch_a);
+  if (!rc) rc = qmm_codes(c, st, rhs, batch, n, k, &tmp[1], &pb, &pitch_b);
+  auto fp8 = [](int32_t v) { return v == B200_QV_E4M3 ? B200_F8E4M3 : B200_F8E5M2; };
+  GemmProblem g{};
+  g.in_dtype = fp8(lhs->scheme.value); g.rhs_dtype = fp8(rhs->scheme.value); g.out_dtype = out_dtype;
+  g.a = pa; g.b = pb; g.out = out;
+  g.M = m; g.N = n; g.K = k; g.batch = batch;
+  g.a_sm = pitch_a; g.a_sk = 1; g.a_sb = batch > 1 ? m * pitch_a : 0;
+  g.b_sn = pitch_b; g.b_sk = 1; g.b_sb = batch > 1 ? n * pitch_b : 0;
+  g.o_sm = n; g.o_sn = 1; g.o_sb = batch > 1 ? m * n : 0;
+  // kernel block: the finer of the present block levels; a coarser block repeats its scale, a per-tensor side uses g; two
+  // per-tensor sides fold per 128 elements of K (the last block short when 128 does not divide K)
+  const int32_t ba = lhs->scheme.block, bb = rhs->scheme.block;
+  g.q = 3;
+  g.q_bk = (uint32_t)(ba == 0 && bb == 0 ? 128 : ba == 0 ? bb : bb == 0 ? ba : std::min(ba, bb));
+  if (!rc) rc = qmm_scales(c, st, lhs, batch, m, k, g.q_bk, &tmp[2]);
+  if (!rc) rc = qmm_scales(c, st, rhs, batch, n, k, g.q_bk, &tmp[3]);
+  g.q_sa = tmp[2]; g.q_sb = tmp[3];
   if (!rc) rc = launch_wgmma(c, st, g, false, false);
   for (CUdeviceptr t : tmp)
     if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMM has drained

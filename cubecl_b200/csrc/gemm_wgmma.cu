@@ -140,7 +140,10 @@ __device__ __forceinline__ uint32_t acc_bits(uint32_t x) { return x; }
 //              producer also loads the stage's f32 effective-scale tiles ([128/Bk][rows] boxes of a block-major buffer) through
 //              tma_a_lo / tma_b_lo into a region after the operand ring.
 //   QM_TENSOR  one f32 scale per side: the s8 mainloop into s32 accumulators; the epilogue stores rn(f32(D) * rn(g_a * g_b)).
-enum : int { QM_NONE = 0, QM_BLOCK = 1, QM_TENSOR = 2 };
+//   QM_FP8     fp8 codes (capi.cpp: b200_matmul_quantized_fp8; KIND the lhs format, the rhs format chosen at run time as for
+//              the mixed fp8 kernels): the QM_BLOCK producer and fold, each block summed by fp8 wgmma into a fresh f32 partial
+//              P_j and folded as acc = fma(P_j, rn(eff_a * eff_b), acc) -- no integer conversion.
+enum : int { QM_NONE = 0, QM_BLOCK = 1, QM_TENSOR = 2, QM_FP8 = 3 };
 // CONV (2-D convolution as an implicit GEMM; capi.cpp: b200_conv2d): the A tile of k-block kb is one im2col load -- 128
 // consecutive output pixels x 64 channels of kernel position kb / cv_cblk, channel block kb % cv_cblk -- which TMA writes in
 // exactly the 128B-swizzled [128 rows x 128 B] layout of a K-major A tile; B is the weights' [n_local x 64 channels] box of
@@ -304,7 +307,9 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
   // coordinates that are not a multiple of 16 bytes faulted (illegal instruction) on an H100 -- the group's tile-rows start
   // at a multiple of 64 rows instead, and the rows before the group are not stored
   constexpr uint32_t GRP_MASK = (CB == CB_GRP_M && A_MN) ? 63u : 0u;
-  static_assert(QM == QM_NONE || (KIND == KIND_S8 && !A_MN && !B_MN && !PROMOTE && MT == 1), "quantized operands: s8, K-major");
+  static_assert(QM == QM_NONE || ((QM == QM_FP8 ? (KIND == KIND_E4M3 || KIND == KIND_E5M2) : KIND == KIND_S8) && !A_MN && !B_MN &&
+                                  !PROMOTE && MT == 1), "quantized operands: s8 (fp8 for QM_FP8), K-major");
+  constexpr bool QBLK = (QM == QM_BLOCK || QM == QM_FP8);   // per-block scale tiles in every stage
   static_assert(!CONV || ((KIND == KIND_BF16 || KIND == KIND_F16) && !A_MN && !B_MN && !PROMOTE && MT == 1 && QM == QM_NONE),
                 "convolution: 16-bit kinds, K-major operands");
   static_assert(CB != CB_DGRAD || CONV, "data gradient: the convolution producer");
@@ -313,8 +318,8 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
   static_assert(CB != CB_WGRAD || (!CONV && A_MN && B_MN && (KIND == KIND_BF16 || KIND == KIND_F16) && !PROMOTE && MT == 1 && QM == QM_NONE),
                 "weight gradient: 16-bit kinds, MN-major operands");
   // per-block scale tiles of one stage, sized for the finest block (Bk = 32: four blocks per 128-element stage)
-  constexpr uint32_t SC_A_BYTES = (QM == QM_BLOCK) ? 128u * 4u * 4u : 0u;
-  constexpr uint32_t SC_STAGE_BYTES = (QM == QM_BLOCK) ? SC_A_BYTES + BLOCK_N * 4u * 4u : 0u;
+  constexpr uint32_t SC_A_BYTES = QBLK ? 128u * 4u * 4u : 0u;
+  constexpr uint32_t SC_STAGE_BYTES = QBLK ? SC_A_BYTES + BLOCK_N * 4u * 4u : 0u;
   constexpr int ESZ = (KIND == KIND_TF32) ? 4 : (KIND >= KIND_E4M3) ? 1 : 2;
   static_assert(ESZ == 2 || (!A_MN && !B_MN), "wgmma reads MN-major operands for 16-bit kinds only");
   constexpr int BLOCK_K = 128 / ESZ;  // one 128-byte swizzle row of K per stage
@@ -360,7 +365,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
       tma_prefetch_desc(tma_b_hi);
     }
     if (p.k_segments > 1) { tma_prefetch_desc(tma_a_lo); tma_prefetch_desc(tma_b_lo); }
-    if constexpr (QM == QM_BLOCK) { tma_prefetch_desc(tma_a_lo); tma_prefetch_desc(tma_b_lo); }
+    if constexpr (QBLK) { tma_prefetch_desc(tma_a_lo); tma_prefetch_desc(tma_b_lo); }
     if (p.tma_store) tma_prefetch_desc(tma_out);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);        // one arrive.expect_tx by this CTA's producer; the peer's multicast bytes counted too
@@ -515,7 +520,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
             if (++s == STAGES) { s = 0; ph ^= 1; }
             continue;
           }
-          if constexpr (QM == QM_BLOCK) {
+          if constexpr (QBLK) {
             // the scale tiles of this stage: A rows of this CTA, and every column of the B tile (each CTA of a pair loads
             // its own copy, no multicast)
             mbar_arrive_expect_tx(fb, STAGE_BYTES + (128u + BLOCK_N) * 4u * p.q_nsub);
@@ -655,7 +660,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
       uint32_t seg = 0, kk = 0;
       if constexpr (KIND == KIND_TF32) seg_of(wu.kb0, seg, kk);
       uint32_t prev = 0;
-      if constexpr (PROMOTE || QM == QM_BLOCK) {
+      if constexpr (PROMOTE || QBLK) {
 #pragma unroll
         for (int i = 0; i < NACC; ++i) acc[0][i] = 0.f;
       }
@@ -735,6 +740,61 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
           else if (p.q_nsub == 2) fold_stage(std::integral_constant<uint32_t, 2>{});
           else fold_stage(std::integral_constant<uint32_t, 1>{});
           release(s);
+        } else if constexpr (QM == QM_FP8) {
+          // the QM_BLOCK fold on f32 partials: per scale block j of the stage and 64-column part h (unit u = j * HP + h), 4 / nsub
+          // fp8 wgmma k32 into a fresh partial, then acc = fma(P_j, rn(eff_a * eff_b), acc).  Two partial buffers: unit u + 1's
+          // wgmma is issued before unit u is folded, so the tensor cores run under the fold.
+          const uint32_t sc = sc_base + s * SC_STAGE_BYTES;
+          const uint32_t row = cw * 64u + wq * 16u + (lane >> 2);
+          auto fold_stage = [&](auto ns, auto kb_) {
+            constexpr uint32_t NSUB = decltype(ns)::value, KPER = 4u / NSUB, HP = BLOCK_N / 64, U = NSUB * HP;
+            constexpr int KB = decltype(kb_)::value;
+            float part[2][32];
+            auto issue = [&](uint32_t u) {
+              const uint32_t j = u / HP, h = u % HP;
+              wgmma_fence();
+#pragma unroll
+              for (uint32_t k = 0; k < KPER; ++k) {
+                const uint32_t kk2 = 2u * (j * KPER + k);
+                wgmma_ss<64, KIND, KB, 0, 0>(part[u & 1u], a_desc + kk2, b_desc + ((h * 64u * 128u) >> 4) + kk2, k != 0 ? 1u : 0u);
+              }
+              wgmma_commit();
+            };
+            issue(0);
+#pragma unroll
+            for (uint32_t u = 0; u < U; ++u) {
+              const uint32_t j = u / HP, h = u % HP;
+              if (u + 1 < U) {
+                issue(u + 1);
+                wgmma_wait<1>();
+              } else {
+                wgmma_wait<0>();
+              }
+              wgmma_fence_operands(part[u & 1u]);
+              float ra0, ra1;
+              asm volatile("ld.shared.f32 %0, [%1];" : "=f"(ra0) : "r"(sc + (j * 128u + row) * 4u) : "memory");
+              asm volatile("ld.shared.f32 %0, [%1];" : "=f"(ra1) : "r"(sc + (j * 128u + row + 8u) * 4u) : "memory");
+              const uint32_t scb = sc + SC_A_BYTES + (j * BLOCK_N + 2u * (lane & 3u)) * 4u;
+#pragma unroll
+              for (int g = 0; g < 8; ++g) {
+                float cb0, cb1;
+                asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(cb0), "=f"(cb1) : "r"(scb + (h * 64u + 8u * g) * 4u) : "memory");
+                const float sc4[4] = {__fmul_rn(ra0, cb0), __fmul_rn(ra0, cb1), __fmul_rn(ra1, cb0), __fmul_rn(ra1, cb1)};
+#pragma unroll
+                for (int e = 0; e < 4; ++e)
+                  acc[0][32 * h + 4 * g + e] = __fmaf_rn(part[u & 1u][4 * g + e], sc4[e], acc[0][32 * h + 4 * g + e]);
+              }
+            }
+          };
+          // straight-line code per (block size, rhs format)
+          auto by_nsub = [&](auto kb_) {
+            if (p.q_nsub == 4) fold_stage(std::integral_constant<uint32_t, 4>{}, kb_);
+            else if (p.q_nsub == 2) fold_stage(std::integral_constant<uint32_t, 2>{}, kb_);
+            else fold_stage(std::integral_constant<uint32_t, 1>{}, kb_);
+          };
+          if (mixed) by_nsub(std::integral_constant<int, KIND_OTHER>{});
+          else by_nsub(std::integral_constant<int, KIND>{});
+          release(s);
         } else {
   #pragma unroll
           for (int mt = 0; mt < MT; ++mt) wgmma_fence_operands(acc[mt]);
@@ -779,7 +839,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
         }
         if (++s == STAGES) { s = 0; ph ^= 1; }
       }
-      if constexpr (!PROMOTE && QM != QM_BLOCK) {
+      if constexpr (!PROMOTE && !QBLK) {
         wgmma_wait<0>();
 #pragma unroll
         for (int mt = 0; mt < MT; ++mt) wgmma_fence_operands(acc[mt]);
@@ -1072,6 +1132,22 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
   GEMM_KERNEL_Q(gemm_q8_f32_##TILE##_kk, CG, BN, OUT_F32, QSTAGES, QM_BLOCK)               \
   GEMM_Q8T(TILE, CG, BN, STAGES)
 
+// fp8-quantized operands (capi.cpp: b200_matmul_quantized_fp8): gemm_qf8_<lhs format>_<out>_<tile>_kk, the QM_BLOCK stages
+#define GEMM_KERNEL_QF8(NAME, CG, BN, KIND, OUT)                                                                  \
+  extern "C" __global__ void __launch_bounds__(kNumThreads, 1)                                                     \
+      NAME(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,                  \
+           const __grid_constant__ CUtensorMap tma_a_sc, const __grid_constant__ CUtensorMap tma_b_sc,            \
+           const __grid_constant__ CUtensorMap tma_out, const __grid_constant__ GemmParams p) {                    \
+    gemm_body<CG, BN, false, false, KIND, OUT, 5, false, 1, QM_FP8>(&tma_a, &tma_b, &tma_a_sc, &tma_b_sc, &tma_out, p); \
+  }
+#define GEMM_QF8(TILE, CG, BN)                                                    \
+  GEMM_KERNEL_QF8(gemm_qf8_e4m3_bf16_##TILE##_kk, CG, BN, KIND_E4M3, OUT_BF16)     \
+  GEMM_KERNEL_QF8(gemm_qf8_e4m3_f16_##TILE##_kk, CG, BN, KIND_E4M3, OUT_F16)       \
+  GEMM_KERNEL_QF8(gemm_qf8_e4m3_f32_##TILE##_kk, CG, BN, KIND_E4M3, OUT_F32)       \
+  GEMM_KERNEL_QF8(gemm_qf8_e5m2_bf16_##TILE##_kk, CG, BN, KIND_E5M2, OUT_BF16)     \
+  GEMM_KERNEL_QF8(gemm_qf8_e5m2_f16_##TILE##_kk, CG, BN, KIND_E5M2, OUT_F16)       \
+  GEMM_KERNEL_QF8(gemm_qf8_e5m2_f32_##TILE##_kk, CG, BN, KIND_E5M2, OUT_F32)
+
 // 2-D convolution (implicit GEMM, CONV): tma_a = im2col map of x, tma_b = 3-D weight map; tma_a_lo / tma_b_lo are unused
 // name: conv2d_<in>_<out>_<tile>
 #define CONV_KERNEL(NAME, CG, BN, KIND, OUT, STAGES)                                                                \
@@ -1161,7 +1237,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
   GRP_ONE(TILE, CG, BN, f16, f16, KIND_F16, OUT_F16)              \
   GRP_ONE(TILE, CG, BN, f16, f32, KIND_F16, OUT_F32)
 
-// The kernels are built as nine cubins from this one source (cubecl_b200/build.py compiles them in parallel):
+// The kernels are built as ten cubins from this one source (cubecl_b200/build.py compiles them in parallel):
 //   GEMM_PART 0 ("gemm")       256 x 256 pair tiles (2-CTA cluster, 128 x 256 per CTA) and the bf16 peak probe
 //   GEMM_PART 1 ("gemm_b")     256 x 128 pair tiles, 256 x 224 block-scaled pair tiles
 //   GEMM_PART 2 ("gemm_c")     128 x 128 single-CTA tiles, 512 x 128 pair tiles
@@ -1171,6 +1247,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
 //   GEMM_PART 6 ("gemm_conv3d")   the 3-D convolution kernels (forward, data and weight gradients) of the same two tiles
 //   GEMM_PART 7 ("gemm_convt")    the phase-batched transposed-convolution kernels, 2-D and 3-D, of the same two tiles
 //   GEMM_PART 8 ("gemm_grouped")  the grouped-matmul kernels (ragged M and ragged K) of the same two tiles
+//   GEMM_PART 9 ("gemm_qf8")      the fp8-quantized kernels (QM_FP8) of the same two tiles
 #ifndef GEMM_PART
 #define GEMM_PART 0
 #endif
@@ -1237,6 +1314,11 @@ TCONV_DTYPES(1sm_n128, 1, 128, 6, 3, conv3d)
 #if GEMM_PART == 8
 GRP_DTYPES(2sm_n128, 2, 128)
 GRP_DTYPES(1sm_n128, 1, 128)
+#endif
+#if GEMM_PART == 9
+// the per-block stage count of gemm_q8_* (capi.cpp: gemm_q8_stages)
+GEMM_QF8(2sm_n128, 2, 128)
+GEMM_QF8(1sm_n128, 1, 128)
 #endif
 
 #if GEMM_PART == 0

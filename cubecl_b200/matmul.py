@@ -139,15 +139,29 @@ def launch_quantized(client: ComputeClient, lhs, rhs, out: TensorHandle, stream=
     dims (flattened into one batch); out [..., M, N] contiguous f32 / bf16 / f16 = sum_k deq(lhs)[.., m, k] * deq(rhs)[.., n, k].
     Values q8f / q8s / q4f / q4s / q2f / q2s; per-tensor, per-block (32, 64, 128) or two-level scales on either side.  The
     bit-exact arithmetic is stated in include/cubecl_b200.h (b200_matmul_quantized).  Errors are deferred to client.sync()."""
+    _launch_q(client, lhs, rhs, out, stream, "matmul_quantized")
+
+
+def launch_quantized_fp8(client: ComputeClient, lhs, rhs, out: TensorHandle, stream=None) -> None:
+    """Matmul of two fp8-quantized tensors (cubecl_b200.quant.QuantizedTensor, values e4m3 or e5m2 on either side) on the fp8
+    tensor cores, block scales folded in f32 inside the GEMM: lhs [..., M, K] and rhs [..., N, K] quantized along K with equal
+    leading dims (flattened into one batch); out [..., M, N] contiguous f32 / bf16 / f16.  Per-tensor, per-block (32, 64, 128)
+    or two-level scales on either side.  The arithmetic is stated in include/cubecl_b200.h (b200_matmul_quantized_fp8).
+    Errors are deferred to client.sync()."""
+    _launch_q(client, lhs, rhs, out, stream, "matmul_quantized_fp8")
+
+
+def _launch_q(client, lhs, rhs, out, stream, what: str) -> None:
+    """The shared body of launch_quantized / launch_quantized_fp8: b200_<what> on two QuantizedTensors."""
     try:
         ls, rs = list(lhs.shape), list(rhs.shape)
         if len(ls) < 2 or len(ls) != len(rs) or ls[:-2] != rs[:-2]:
-            raise B200Error(6, f"matmul_quantized: lhs {ls} and rhs {rs} need rank >= 2 and equal leading dims")
+            raise B200Error(6, f"{what}: lhs {ls} and rhs {rs} need rank >= 2 and equal leading dims")
         if ls[-1] != rs[-1]:
-            raise B200Error(6, f"matmul_quantized: K mismatch (lhs {ls[-1]}, rhs {rs[-1]})")
+            raise B200Error(6, f"{what}: K mismatch (lhs {ls[-1]}, rhs {rs[-1]})")
         M, N, K = ls[-2], rs[-2], ls[-1]
         if list(out.shape) != ls[:-2] + [M, N] or not out.is_contiguous():
-            raise B200Error(6, f"matmul_quantized: out must be contiguous with shape {ls[:-2] + [M, N]}")
+            raise B200Error(6, f"{what}: out must be contiguous with shape {ls[:-2] + [M, N]}")
         batch = int(np.prod(ls[:-2])) if len(ls) > 2 else 1
         ops = []
         for q in (lhs, rhs):
@@ -157,8 +171,9 @@ def launch_quantized(client: ComputeClient, lhs, rhs, out: TensorHandle, stream=
             ops.append(_ffi.QuantOperand(q.scheme.to_c(), *(t.handle.ptr if t is not None else 0
                                                               for t in (q.values, q.block_scales, q.tensor_scale))))
         out.handle.used_on(stream)
-        _ffi.check(client._lib.b200_matmul_quantized(client._ctx, stream, C.byref(ops[0]), C.byref(ops[1]), DTYPES[out.dtype],
-                                                     C.c_uint64(out.handle.ptr), batch, M, N, K))
+        fn = getattr(client._lib, "b200_" + what)
+        _ffi.check(fn(client._ctx, stream, C.byref(ops[0]), C.byref(ops[1]), DTYPES[out.dtype], C.c_uint64(out.handle.ptr),
+                      batch, M, N, K))
     except B200Error as e:
         client._defer(e)
 

@@ -341,6 +341,34 @@ typedef struct b200_quant_operand {
 int b200_matmul_quantized(b200_ctx* ctx, b200_stream s, const b200_quant_operand* lhs, const b200_quant_operand* rhs,
                           b200_dtype out_dtype, b200_dptr out, uint64_t batch, uint64_t m, uint64_t n, uint64_t k);
 
+/* ---- matmul of fp8-quantized operands on the fp8 tensor cores, block scales folded in f32 inside the GEMM ------------------
+ * The layout of b200_matmul_quantized: lhs codes [batch, M, K], rhs [batch, N, K], both quantized along K exactly as
+ * b200_quantize writes them; out [batch, M, N] contiguous in F32 / BF16 / F16.  Values E4M3 or E5M2, independently per side
+ * (e5m2 gradients x e4m3 weights); per-tensor, per-block (32, 64, 128) or two-level scales on either side, every block-scale
+ * dtype b200_dequantize reads.  Tensor scales are read on the device: b200_quantize and this call may be enqueued back to back.
+ * Arithmetic.  eff_x[b, r, j] is the effective scale of block j of row r as in b200_matmul_quantized.  Bk = the finer of the
+ * present block levels (a coarser block repeats its scale, a per-tensor side uses g); with no block level on either side
+ * Bk = 128 and the last block of a K that 128 does not divide is short.  P_j = the tensor core's sum over block j of the
+ * code products, computed by Bk / 32 fp8 wgmma k32 steps into a fresh f32 partial (scale-d = 0 on the first).  Blocks fold
+ * in increasing j: acc_0 = 0, acc_{j+1} = fma(P_j, rn(eff_a[m, j] * eff_b[n, j]), acc_j); out = RNE(acc_J).
+ * P_j is NOT IEEE-defined: the fp8 tensor cores accumulate with truncation, below f32 precision.  When every partial sum
+ * inside a block is an integer of magnitude <= 2^11 (integer-valued codes, e.g. |q| <= 4 with Bk = 128), P_j is expected to
+ * equal the exact dot product D_j, and the result is then b200_matmul_quantized's per-block contract bit for bit.  On real
+ * data the error of one block is a few f32 ulps of sum |a_k b_k| over the block; DESIGN.md section 3.18 gives the measured
+ * bound.  NaN / inf codes (e4m3 0x7F, e5m2 +-inf) and non-finite scales reach only their own rows and columns.  No stream-K
+ * head runs and there are no atomics: results are bitwise reproducible from run to run.
+ * DeepSeek-style 128 x 128 weight scales ([N / 128, K / 128] f32): repeat each scale row 128 times into [N, K / 128] and pass
+ * the weight as a per-block-128 F32 operand.  The effective scales are the same numbers, so the result is exact.
+ * Errors: B200_ERR_UNSUPPORTED for integer values (use b200_matmul_quantized), e2m1 (use b200_matmul_scaled) and blocks of 8
+ * or 16; B200_ERR_INVALID_ARG for everything b200_quantize's checks reject (K not divisible by a block, a null pointer for a
+ * present level or a non-null one for an absent level, an unknown value or dtype), a null code or output pointer, and K == 0
+ * with a non-empty output.  batch, M or N of 0 is a no-op.
+ * Launches: 2 effective-scale passes + 1 GEMM (gemm_qf8_<lhs>_<out>_<2sm_n128 | 1sm_n128>_kk, the rhs format chosen at run
+ * time); +1 per operand TMA cannot read in place (base not 16-byte aligned or K % 16 != 0: staging).  "gemm.variant" may force
+ * 2sm_n128 or 1sm_n128.  Temporaries come from the pool, stream-ordered. */
+int b200_matmul_quantized_fp8(b200_ctx* ctx, b200_stream s, const b200_quant_operand* lhs, const b200_quant_operand* rhs,
+                              b200_dtype out_dtype, b200_dptr out, uint64_t batch, uint64_t m, uint64_t n, uint64_t k);
+
 /* ---- 2-D convolution (cubek's convolution kernels), an implicit GEMM on the wgmma kernel --------------------------------
  * out[n, oh, ow, co] = act(alpha * sum_{ky, kx, c} x[n, oh*sh - ph + ky*dh, ow*sw - pw + kx*dw, c] * w[co, ky, kx, c] + bias[co]).
  * Input outside x reads as zero; f32 accumulation; the epilogue is b200_epilogue (NULL = none).  x is [N, H, W, C] (NHWC), w is

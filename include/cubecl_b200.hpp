@@ -218,6 +218,15 @@ inline void launch_quantized(ComputeClient& client, const b200_quant_operand& lh
                                        batch, m, n, k);
   if (rc != B200_OK) client.defer(b200_last_error());
 }
+/// out (contiguous [batch, m, n], F32 / BF16 / F16) = deq(lhs) x deq(rhs)^T of two fp8-quantized operands (e4m3 / e5m2 on
+/// either side) on the fp8 tensor cores, block scales folded in f32 inside the GEMM; see b200_matmul_quantized_fp8 in
+/// cubecl_b200.h for the contract. Errors deferred.
+inline void launch_quantized_fp8(ComputeClient& client, const b200_quant_operand& lhs, const b200_quant_operand& rhs, const TensorHandle& out,
+                                 uint64_t batch, uint64_t m, uint64_t n, uint64_t k) {
+  const int rc = b200_matmul_quantized_fp8(client.raw(), nullptr, &lhs, &rhs, static_cast<b200_dtype>(out.dtype), out.handle.ptr(),
+                                           batch, m, n, k);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
 /// Grouped matmul for mixture-of-experts layers (torch's grouped_mm with offs): lhs [T, K] x rhs [G, K, N] -> out [T, N]
 /// (ragged M), or lhs [M, T] x rhs [T, N] -> out [G, M, N] (ragged K); offs is a compact i32 [G] tensor of cumulative ends
 /// read on the device only.  See b200_matmul_grouped in cubecl_b200.h for the contract.  Errors are deferred to client.sync().

@@ -132,6 +132,26 @@ pub mod matmul {
     pub unsafe fn launch_quantized(
         ctx: &mut Context, stream: b200_stream, lhs: &QuantizedTensor, rhs: &QuantizedTensor, out: &TensorHandle, k: u64,
     ) -> Result<(), Error> {
+        let (a, b, batch, m, n) = quantized_args(lhs, rhs, out)?;
+        ctx.matmul_quantized(stream, &a, &b, out.dtype, out.ptr, batch, m, n, k)
+    }
+
+    /// `matmul::launch_quantized_fp8(client, lhs, rhs, out)`: as [`launch_quantized`] for E4M3 / E5M2 codes, on the fp8 tensor
+    /// cores (`b200_matmul_quantized_fp8`).
+    ///
+    /// # Safety
+    /// As [`launch`].
+    pub unsafe fn launch_quantized_fp8(
+        ctx: &mut Context, stream: b200_stream, lhs: &QuantizedTensor, rhs: &QuantizedTensor, out: &TensorHandle, k: u64,
+    ) -> Result<(), Error> {
+        let (a, b, batch, m, n) = quantized_args(lhs, rhs, out)?;
+        ctx.matmul_quantized_fp8(stream, &a, &b, out.dtype, out.ptr, batch, m, n, k)
+    }
+
+    // the two operands, the batch and (M, N) of a quantized matmul into `out`
+    fn quantized_args(
+        lhs: &QuantizedTensor, rhs: &QuantizedTensor, out: &TensorHandle,
+    ) -> Result<(QuantOperand, QuantOperand, u64, u64, u64), Error> {
         let r = out.shape.len();
         if r < 2 || lhs.values.shape.len() != r || rhs.values.shape.len() != r || lhs.values.shape[..r - 2] != rhs.values.shape[..r - 2] {
             return Err(invalid("lhs [.., M, K] and rhs [.., N, K] need the rank of out and equal leading dims".to_string()));
@@ -144,7 +164,7 @@ pub mod matmul {
             block_scales: q.block_scales.map_or(0, |t| t.ptr),
             tensor_scale: q.tensor_scale.map_or(0, |t| t.ptr),
         };
-        ctx.matmul_quantized(stream, &op(lhs), &op(rhs), out.dtype, out.ptr, batch, m, n, k)
+        Ok((op(lhs), op(rhs), batch, m, n))
     }
 }
 

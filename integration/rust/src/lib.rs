@@ -955,6 +955,21 @@ impl Context {
         check(sys::b200_matmul_quantized(self.0, stream, &a, &b, out_dtype as c_int, out, batch, m, n, k))
     }
 
+    /// out [batch, m, n] (contiguous, F32 / BF16 / F16) = deq(lhs) x deq(rhs)^T of two fp8-quantized operands (E4M3 / E5M2 on
+    /// either side), codes [batch, m | n, k] quantized along k, on the fp8 tensor cores with the block scales folded in f32
+    /// inside the GEMM; the contract is `b200_matmul_quantized_fp8`'s in include/cubecl_b200.h.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::matmul`].
+    #[allow(clippy::too_many_arguments)]
+    pub unsafe fn matmul_quantized_fp8(
+        &mut self, stream: b200_stream, lhs: &QuantOperand, rhs: &QuantOperand, out_dtype: DType, out: b200_dptr, batch: u64,
+        m: u64, n: u64, k: u64,
+    ) -> Result<(), Error> {
+        let (a, b) = (lhs.raw(), rhs.raw());
+        check(sys::b200_matmul_quantized_fp8(self.0, stream, &a, &b, out_dtype as c_int, out, batch, m, n, k))
+    }
+
     /// out (compact row-major) = gather of the strided tensor `input` (into_contiguous, cubecl-std/src/tensor/contiguous.rs).
     ///
     /// # Safety
