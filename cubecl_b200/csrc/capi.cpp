@@ -77,6 +77,8 @@ extern const unsigned char b200_cubin_gemm_grouped[];
 extern const unsigned char b200_cubin_gemm_grouped_end[];
 extern const unsigned char b200_cubin_gemm_qf8[];
 extern const unsigned char b200_cubin_gemm_qf8_end[];
+extern const unsigned char b200_cubin_gemm_grouped_qf8[];
+extern const unsigned char b200_cubin_gemm_grouped_qf8_end[];
 }
 
 // ================================================================================================ errors
@@ -349,12 +351,13 @@ static int get_func(b200_ctx* c, const std::string& name, CUfunction* out) {
   if (it != c->funcs.end()) { *out = it->second; return B200_OK; }
   // modules are loaded in the order gemm, reduce, aux, gemm_b, gemm_c, quant, gemm_q, quant_mm, gemm_conv, gemm_convbwd,
   // conv_grouped, gemm_conv3d, gemm_convt, attention, attention_bwd, attention_kv, attention_varlen, attention_varlen_bwd,
-  // attention_kv_fp8, attention_paged, attention_paged_fp8, gemm_grouped, gemm_qf8; the kernel name says where a
+  // attention_kv_fp8, attention_paged, attention_paged_fp8, gemm_grouped, gemm_qf8, gemm_grouped_qf8; the kernel name says where a
   // kernel lives (no failing lookups, which API-level tools such as compute-sanitizer would report)
   auto starts = [&](const char* pfx) { return name.rfind(pfx, 0) == 0; };
   auto has = [&](const char* part) { return name.find(part) != std::string::npos; };
   const bool tc_gemm = starts("gemm_") && name != "gemm_simt_strided" && name != "gemm_scaled_simt";
   const size_t home = name == "conv3d_dgrad_weights" ? 2
+                      : starts("gemm_grouped_qf8_") ? 23
                       : starts("gemm_qf8_") ? 22
                       : starts("gemm_grouped_") ? 21
                       : starts("attn_fwd_paged_") && (has("_e4m3_") || has("_e5m2_")) ? 20
@@ -414,7 +417,8 @@ extern "C" int b200_get_cubin(const char* name, const void** image, size_t* size
   else if (!strcmp(name, "attention_paged_fp8")) { b = b200_cubin_attention_paged_fp8; e = b200_cubin_attention_paged_fp8_end; }
   else if (!strcmp(name, "gemm_grouped")) { b = b200_cubin_gemm_grouped; e = b200_cubin_gemm_grouped_end; }
   else if (!strcmp(name, "gemm_qf8")) { b = b200_cubin_gemm_qf8; e = b200_cubin_gemm_qf8_end; }
-  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd|conv_grouped|gemm_conv3d|gemm_convt|attention|attention_bwd|attention_kv|attention_varlen|attention_varlen_bwd|attention_kv_fp8|attention_paged|attention_paged_fp8|gemm_grouped|gemm_qf8)", name);
+  else if (!strcmp(name, "gemm_grouped_qf8")) { b = b200_cubin_gemm_grouped_qf8; e = b200_cubin_gemm_grouped_qf8_end; }
+  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd|conv_grouped|gemm_conv3d|gemm_convt|attention|attention_bwd|attention_kv|attention_varlen|attention_varlen_bwd|attention_kv_fp8|attention_paged|attention_paged_fp8|gemm_grouped|gemm_qf8|gemm_grouped_qf8)", name);
   *image = b;
   *size = static_cast<size_t>(e - b);
   return B200_OK;
@@ -484,7 +488,8 @@ extern "C" int b200_init(int device, b200_ctx** out) {
       (rc = load_module(c, b200_cubin_attention_paged, b200_cubin_attention_paged_end, "attention_paged")) ||
       (rc = load_module(c, b200_cubin_attention_paged_fp8, b200_cubin_attention_paged_fp8_end, "attention_paged_fp8")) ||
       (rc = load_module(c, b200_cubin_gemm_grouped, b200_cubin_gemm_grouped_end, "gemm_grouped")) ||
-      (rc = load_module(c, b200_cubin_gemm_qf8, b200_cubin_gemm_qf8_end, "gemm_qf8"))) {
+      (rc = load_module(c, b200_cubin_gemm_qf8, b200_cubin_gemm_qf8_end, "gemm_qf8")) ||
+      (rc = load_module(c, b200_cubin_gemm_grouped_qf8, b200_cubin_gemm_grouped_qf8_end, "gemm_grouped_qf8"))) {
     for (CUmodule m : c->modules) g_drv.cuModuleUnload_p(m);
     g_drv.cuDevicePrimaryCtxRelease_p(c->dev);
     return bail(rc);
@@ -1277,6 +1282,28 @@ static int gemm_launch(b200_ctx* c, CUstream st, CUfunction f, const GemmVariant
   return launch(c, f, clusters * v.cg, 1, 1, 384, smem, v.cg, st, args);
 }
 
+// The GemmParams fields of 8-bit and quantized operands, after gemm_params (launch_wgmma and the grouped fp8 launch): the rhs
+// format of a mixed 8-bit pair, the per-tensor scale pointers (q = 2), and for the per-block folds (q = 1, 3) the blocks per
+// stage with the maps of the effective-scale tiles of one stage, [128 / Bk blocks][128 rows] of A and [128 / Bk][block_n] of
+// B (no swizzle), into *ta_sc / *tb_sc.
+static int gemm_quant_params(b200_ctx* c, const GemmProblem& g, const GemmVariant& v, bool a_bcast, bool b_bcast, CUtensorMap* ta_sc,
+                             CUtensorMap* tb_sc, GemmParams* p) {
+  if (g.rhs_dtype >= 0 && g.rhs_dtype != g.in_dtype) {
+    p->fmt_b = (g.rhs_dtype == B200_F8E5M2 || g.rhs_dtype == B200_I8) ? 1u : 0u;   // 0 = e4m3 / u8, 1 = e5m2 / s8
+    p->fmt_mixed = 1;
+  }
+  p->q_ga = g.q_ga; p->q_gb = g.q_gb;
+  if (g.q != 1 && g.q != 3) return B200_OK;
+  const uint64_t nblk = (g.K + g.q_bk - 1) / g.q_bk, ra = (g.M + 3) / 4 * 4, rb = (g.N + 3) / 4 * 4;
+  const uint32_t nsub = 128u / g.q_bk;
+  p->q_nsub = nsub;
+  int rc = encode_tmap(c, ta_sc, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, g.q_sa, ra, nblk, a_bcast ? 1 : g.batch, ra, ra * nblk, 128, nsub,
+                       CU_TENSOR_MAP_SWIZZLE_NONE);
+  if (!rc) rc = encode_tmap(c, tb_sc, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, g.q_sb, rb, nblk, b_bcast ? 1 : g.batch, rb, rb * nblk,
+                            (uint32_t)v.block_n, nsub, CU_TENSOR_MAP_SWIZZLE_NONE);
+  return rc;
+}
+
 static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_mn, bool b_mn) {
   const size_t esz = dtype_size(g.in_dtype), osz = dtype_size(g.out_dtype);
   const char* in_tag = g.q == 1 ? "q8" : g.q == 2 ? "q8t" : g.q == 3 ? (g.in_dtype == B200_F8E4M3 ? "qf8_e4m3" : "qf8_e5m2") : g.mx ? "mx" : g.in_dtype == B200_BF16 ? "bf16" : g.in_dtype == B200_F16 ? "f16" : g.in_dtype == B200_F8E4M3 ? "e4m3"
@@ -1331,16 +1358,6 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
     if (rc) return rc;
     rc = encode_operand(c, &tb_lo, ldt, lsz, g.b_lo, g.N, g.K, planes * (b_bcast ? 1 : g.batch), kp, 1, kp * g.N, false, n_local);
     if (rc) return rc;
-  } else if (g.q == 1 || g.q == 3) {
-    // effective-scale tiles of one stage: [128 / Bk blocks][128 rows] of A, [128 / Bk][block_n] of B (no swizzle)
-    const uint64_t nblk = (g.K + g.q_bk - 1) / g.q_bk, ra = (g.M + 3) / 4 * 4, rb = (g.N + 3) / 4 * 4;
-    const uint32_t nsub = 128u / g.q_bk;
-    rc = encode_tmap(c, &ta_lo, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, g.q_sa, ra, nblk, a_bcast ? 1 : g.batch, ra, ra * nblk, 128, nsub,
-                     CU_TENSOR_MAP_SWIZZLE_NONE);
-    if (rc) return rc;
-    rc = encode_tmap(c, &tb_lo, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, g.q_sb, rb, nblk, b_bcast ? 1 : g.batch, rb, rb * nblk,
-                     (uint32_t)v.block_n, nsub, CU_TENSOR_MAP_SWIZZLE_NONE);
-    if (rc) return rc;
   }
 
   GemmParams p;
@@ -1348,16 +1365,12 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
   ep.alpha = g.alpha; ep.activation = (int32_t)g.act; ep.bias = g.bias;
   const uint64_t tile_m = 128ull * v.cg * v.mt;
   gemm_params(c, &p, v, osz, g.out, g.o_sm, g.o_sb, g.M, g.N, g.K, g.batch, (g.M + tile_m - 1) / tile_m, &ep, split ? 3 : 1);
-  if (g.rhs_dtype >= 0 && g.rhs_dtype != g.in_dtype) {
-    p.fmt_b = (g.rhs_dtype == B200_F8E5M2 || g.rhs_dtype == B200_I8) ? 1u : 0u;   // 0 = e4m3 / u8, 1 = e5m2 / s8
-    p.fmt_mixed = 1;
-  }
+  if ((rc = gemm_quant_params(c, g, v, a_bcast, b_bcast, &ta_lo, &tb_lo, &p))) return rc;
   if (split && g.hybrid) {
     p.hyb = 1;
     p.hyb_nba = a_bcast ? 1u : (uint32_t)g.batch;
     p.hyb_nbb = b_bcast ? 1u : (uint32_t)g.batch;
   }
-  if (g.q == 1 || g.q == 3) p.q_nsub = 128u / g.q_bk;
   if (g.conv) {
     const ConvGeom& cv = *g.conv;
     p.cv_ohw = (uint32_t)(cv.O[1] * cv.O[2]); p.cv_ow = (uint32_t)cv.O[2];
@@ -1372,7 +1385,6 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
       p.dx_sd = cv.dx_s[0];
     }
   }
-  p.q_ga = g.q_ga; p.q_gb = g.q_gb;
   p.a_bmul = a_bcast ? 0 : 1;
   p.b_bmul = b_bcast ? 0 : 1;
   if (cmode == 1 && ((p.dx_sn * osz) % 16 || (p.dx_si * osz) % 16 || (p.dx_sj * osz) % 16 || (p.dx_sd * osz) % 16)) p.vec_store = 0;
@@ -1855,6 +1867,62 @@ static const GemmVariant* grouped_variant(b200_ctx* c, bool ragged_k, uint64_t T
   return nullptr;
 }
 
+// A grouped launch once its operands are checked (b200_matmul_grouped, b200_matmul_grouped_quantized_fp8): the tile, the store
+// path, and the grid's bound on the tiles.  Every group may add one partial tile-row (ragged M), and its tile-rows start up to
+// `lead` rows before its first row (63 with an M-contiguous lhs, 3 for the fp8 kernels' scale tiles; gemm_wgmma.cu:
+// GRP_MASK); ragged K runs G whole grids.
+struct GroupedPlan {
+  const GemmVariant* v = nullptr;
+  std::string epi;
+  uint64_t tiles_m = 0, tile_rows = 0, bound = 0;
+};
+static int grouped_plan(b200_ctx* c, const char* what, bool rk, uint64_t lead, uint64_t groups, uint64_t T, uint64_t M, uint64_t N, GroupedPlan* pl) {
+  typedef unsigned long long ull;
+  pl->v = grouped_variant(c, rk, T, groups, M);
+  if (!pl->v)
+    return fail(B200_ERR_INVALID_ARG, "gemm.variant '%s' is not a grouped matmul tile (2sm_n128, 1sm_n128)", opt(c, "gemm.variant", "auto").c_str());
+  const GemmVariant& v = *pl->v;
+  pl->epi = opt(c, "gemm.epilogue", "tma");
+  if (pl->epi != "tma" && pl->epi != "direct") return fail(B200_ERR_INVALID_ARG, "gemm.epilogue must be tma or direct");
+  const uint64_t rows = 128ull * v.cg, tiles_n = (N + v.block_n - 1) / v.block_n, span = T + lead * groups;
+  pl->tiles_m = (M + rows - 1) / rows;
+  pl->tile_rows = rk ? groups * pl->tiles_m : (span + rows - 1) / rows + groups;
+  pl->bound = pl->tile_rows * tiles_n;
+  if (pl->bound >= (1ull << 32)) return fail(B200_ERR_UNSUPPORTED, "%s: too many tiles (bound %llu)", what, (ull)pl->bound);
+  if (c->dry) {
+    char line[200];
+    snprintf(line, sizeof(line), "gemm grouped %s groups=%llu T=%llu tile_rows<=%llu tiles<=%llu\n", rk ? "ragged_k" : "ragged_m",
+             (ull)groups, (ull)T, (ull)pl->tile_rows, (ull)pl->bound);
+    c->plan += line;
+  }
+  return B200_OK;
+}
+
+// The end of a grouped launch, after gemm_params and the family's own fields: whole tiles only (no stream-K head: the host
+// does not know the tile count), the output map (ragged M's tiles that a group's end cuts store directly), GroupedParams and
+// one launch.  maps: the kernel's leading tensor-map parameters, in order.
+static int grouped_launch(b200_ctx* c, CUstream st, CUfunction f, const GroupedPlan& pl, unsigned smem, size_t osz, b200_dptr offs,
+                          uint64_t groups, uint64_t T, bool rk, GemmParams* p, std::initializer_list<CUtensorMap*> maps) {
+  p->full_tiles = (uint32_t)pl.bound;
+  CUtensorMap tout;
+  const int rc = encode_out_map(c, &tout, osz, pl.epi, p);
+  if (rc) return rc;
+  GroupedParams gp;
+  memset(&gp, 0, sizeof(gp));
+  gp.offs = offs;
+  gp.bias_stride = p->N;
+  gp.groups = (uint32_t)groups;
+  gp.T = (uint32_t)T;
+  gp.mode = rk ? 1u : 0u;
+  void* args[8];
+  size_t n = 0;
+  for (CUtensorMap* m : maps) args[n++] = m;
+  args[n++] = &tout;
+  args[n++] = &gp;
+  args[n++] = p;
+  return gemm_launch(c, st, f, *pl.v, pl.bound, smem, args);
+}
+
 // Can TMA read an MN-major operand (mn contiguous, rows of K) in place?  Strides in elements.
 static bool mn_major_tma_ok(uint64_t ptr, size_t esz, uint64_t mn, uint64_t K, uint64_t s_mn, uint64_t s_k) {
   return ptr % 16 == 0 && (s_mn == 1 || mn == 1) && (K == 1 || ((s_k * esz) % 16 == 0 && s_k >= mn)) && s_k * esz < (1ull << 40);
@@ -1979,36 +2047,20 @@ extern "C" int b200_matmul_grouped(b200_ctx* c, b200_stream s, b200_dtype in_dty
     }
   }
 
-  const GemmVariant* vp = grouped_variant(c, rk, T, groups, M);
-  if (!vp)
-    return release(fail(B200_ERR_INVALID_ARG, "gemm.variant '%s' is not a grouped matmul tile (2sm_n128, 1sm_n128)",
-                        opt(c, "gemm.variant", "auto").c_str()));
-  const GemmVariant& v = *vp;
-  const std::string epi = opt(c, "gemm.epilogue", "tma");
-  if (epi != "tma" && epi != "direct") return release(fail(B200_ERR_INVALID_ARG, "gemm.epilogue must be tma or direct"));
-  // the grid's bound on the tiles: every group may add one partial tile-row (ragged M; with an M-contiguous lhs a group's
-  // tile-rows start up to 63 rows early, GroupedParams); G whole grids (ragged K)
-  const uint64_t rows = 128ull * v.cg, tiles_n = (N + v.block_n - 1) / v.block_n, tiles_m = (M + rows - 1) / rows;
-  const uint64_t span = T + (a_mn && !rk ? 63 * groups : 0);
-  const uint64_t tile_rows = rk ? groups * tiles_m : (span + rows - 1) / rows + groups, bound = tile_rows * tiles_n;
-  if (bound >= (1ull << 32)) return release(fail(B200_ERR_UNSUPPORTED, "matmul_grouped: too many tiles (bound %llu)", (ull)bound));
+  GroupedPlan pl;
+  if ((rc = grouped_plan(c, "matmul_grouped", rk, a_mn && !rk ? 63 : 0, groups, T, M, N, &pl))) return release(rc);
+  const GemmVariant& v = *pl.v;
   const char* in_tag = in_dtype == B200_BF16 ? "bf16" : "f16";
   const char* out_tag = out_dtype == B200_F32 ? "f32" : in_tag;
   const std::string name = std::string(rk ? "gemm_grouped_k_" : "gemm_grouped_m_") + in_tag + "_" + out_tag + "_" + v.tag +
                            (rk ? "" : std::string("_") + (a_mn ? "m" : "k") + (b_mn ? "n" : "k"));
-  if (c->dry) {
-    char line[200];
-    snprintf(line, sizeof(line), "gemm grouped %s groups=%llu T=%llu tile_rows<=%llu tiles<=%llu\n", rk ? "ragged_k" : "ragged_m",
-             (ull)groups, (ull)T, (ull)tile_rows, (ull)bound);
-    c->plan += line;
-  }
   const unsigned smem = gemm_smem_bytes(v) + kGroupedTableBytes;
   CUfunction f;
   if ((rc = gemm_kernel(c, name, smem, &f))) return release(rc);
 
   // ragged M: lhs [T, K] and rhs [G, K, N] with the group as the batch; ragged K: lhs [M, T] and rhs [T, N], both MN-major
   const CUtensorMapDataType dt = in_dtype == B200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  CUtensorMap ta, tb, tout;
+  CUtensorMap ta, tb;
   memset(&ta, 0, sizeof(ta));
   memset(&tb, 0, sizeof(tb));
   if (reads) {
@@ -2018,20 +2070,9 @@ extern "C" int b200_matmul_grouped(b200_ctx* c, b200_stream s, b200_dtype in_dty
   if (rc) return release(rc);
 
   GemmParams p;
-  gemm_params(c, &p, v, osz, out, o_sm, o_sb, M, N, K, rk ? groups : 1, rk ? tiles_m : tile_rows, ep);
+  gemm_params(c, &p, v, osz, out, o_sm, o_sb, M, N, K, rk ? groups : 1, rk ? pl.tiles_m : pl.tile_rows, ep);
   p.b_bmul = (!rk && b_sb != 0 && groups > 1) ? 1u : 0u;
-  p.full_tiles = (uint32_t)bound;   // whole tiles only: no stream-K head (the host does not know the tile count)
-  // ragged M's tiles that a group's end cuts store directly
-  if ((rc = encode_out_map(c, &tout, osz, epi, &p))) return release(rc);
-  GroupedParams gp;
-  memset(&gp, 0, sizeof(gp));
-  gp.offs = offs;
-  gp.bias_stride = N;
-  gp.groups = (uint32_t)groups;
-  gp.T = (uint32_t)T;
-  gp.mode = rk ? 1u : 0u;
-  void* args[] = {&ta, &tb, &tout, &gp, &p};
-  rc = gemm_launch(c, st, f, v, bound, smem, args);
+  rc = grouped_launch(c, st, f, pl, smem, osz, offs, groups, T, rk, &p, {&ta, &tb});
   return release(rc);   // stream-ordered: staged copies are reused only by later work
 }
 
@@ -2905,6 +2946,36 @@ extern "C" int b200_matmul_quantized(b200_ctx* c, b200_stream s, const b200_quan
   return rc;
 }
 
+// One operand of the fp8-quantized matmuls: `rows` x K codes as b200_quantize writes them (quant_check; rows = 0 for an empty
+// call checks the scheme alone), with e4m3 or e5m2 values and blocks of 32, 64 or 128 elements.
+static int qf8_operand_check(const char* what, const b200_quant_operand* o, uint64_t rows, uint64_t k) {
+  const uint64_t shape[2] = {rows, k};
+  uint64_t nel = 0, K = 0;
+  const int rc = quant_check(what, &o->scheme, 2, shape, o->block_scales, o->tensor_scale, &nel, &K);
+  if (rc) return rc;
+  const int32_t v = o->scheme.value;
+  if (v == B200_QV_E2M1)
+    return fail(B200_ERR_UNSUPPORTED, "%s: e2m1 values with block scales run through b200_matmul_scaled", what);
+  if (v != B200_QV_E4M3 && v != B200_QV_E5M2)
+    return fail(B200_ERR_UNSUPPORTED, "%s: integer values run through b200_matmul_quantized", what);
+  if (o->scheme.block == 8 || o->scheme.block == 16)
+    return fail(B200_ERR_UNSUPPORTED, "%s: block %d (32, 64 or 128: fp8 wgmma consumes K in steps of 32)", what, (int)o->scheme.block);
+  return B200_OK;
+}
+
+// The GEMM problem of the fp8 fold (q = 3) without its operand layout: the two formats and the kernel block -- the finer of
+// the present block levels; a coarser block repeats its scale, a per-tensor side uses g; two per-tensor sides fold per 128
+// elements of K (the last block short when 128 does not divide K).
+static GemmProblem qf8_problem(const b200_quant_operand* lhs, const b200_quant_operand* rhs, b200_dtype out_dtype) {
+  auto fp8 = [](int32_t v) { return v == B200_QV_E4M3 ? B200_F8E4M3 : B200_F8E5M2; };
+  GemmProblem g{};
+  g.in_dtype = fp8(lhs->scheme.value); g.rhs_dtype = fp8(rhs->scheme.value); g.out_dtype = out_dtype;
+  const int32_t ba = lhs->scheme.block, bb = rhs->scheme.block;
+  g.q = 3;
+  g.q_bk = (uint32_t)(ba == 0 && bb == 0 ? 128 : ba == 0 ? bb : bb == 0 ? ba : std::min(ba, bb));
+  return g;
+}
+
 // fp8 codes (e4m3 / e5m2 on either side) on the fp8 tensor cores: Bk / 32 wgmma k32 steps per block into a fresh f32 partial,
 // folded as b200_matmul_quantized's per-block kernels fold their exact s32 partials (gemm_qf8_*, gemm_wgmma.cu: QM_FP8)
 extern "C" int b200_matmul_quantized_fp8(b200_ctx* c, b200_stream s, const b200_quant_operand* lhs, const b200_quant_operand* rhs,
@@ -2912,22 +2983,9 @@ extern "C" int b200_matmul_quantized_fp8(b200_ctx* c, b200_stream s, const b200_
   CTX_ENTER(c);
   if (!lhs || !rhs) return fail(B200_ERR_INVALID_ARG, "matmul_quantized_fp8: null operand");
   const bool empty = (batch == 0 || m == 0 || n == 0);
-  const b200_quant_operand* ops[2] = {lhs, rhs};
-  const uint64_t rows[2] = {m, n};
-  for (int i = 0; i < 2; ++i) {
-    const char* what = i == 0 ? "matmul_quantized_fp8 (lhs)" : "matmul_quantized_fp8 (rhs)";
-    const uint64_t shape[2] = {empty ? 0 : batch * rows[i], k};
-    uint64_t nel = 0, K = 0;
-    int rc = quant_check(what, &ops[i]->scheme, 2, shape, ops[i]->block_scales, ops[i]->tensor_scale, &nel, &K);
-    if (rc) return rc;
-    const int32_t v = ops[i]->scheme.value;
-    if (v == B200_QV_E2M1)
-      return fail(B200_ERR_UNSUPPORTED, "%s: e2m1 values with block scales run through b200_matmul_scaled", what);
-    if (v != B200_QV_E4M3 && v != B200_QV_E5M2)
-      return fail(B200_ERR_UNSUPPORTED, "%s: integer values run through b200_matmul_quantized", what);
-    if (ops[i]->scheme.block == 8 || ops[i]->scheme.block == 16)
-      return fail(B200_ERR_UNSUPPORTED, "%s: block %d (32, 64 or 128: fp8 wgmma consumes K in steps of 32)", what, (int)ops[i]->scheme.block);
-  }
+  int rc = qf8_operand_check("matmul_quantized_fp8 (lhs)", lhs, empty ? 0 : batch * m, k);
+  if (!rc) rc = qf8_operand_check("matmul_quantized_fp8 (rhs)", rhs, empty ? 0 : batch * n, k);
+  if (rc) return rc;
   if (out_dtype != B200_F32 && out_dtype != B200_BF16 && out_dtype != B200_F16)
     return fail(B200_ERR_INVALID_ARG, "matmul_quantized_fp8: output dtype %d is not F32, BF16 or F16", (int)out_dtype);
   if (empty) return B200_OK;
@@ -2940,27 +2998,78 @@ extern "C" int b200_matmul_quantized_fp8(b200_ctx* c, b200_stream s, const b200_
   CUstream st = resolve_stream(c, s);
   CUdeviceptr tmp[4] = {0, 0, 0, 0};   // lhs codes, rhs codes, lhs scales, rhs scales
   uint64_t pa = 0, pb = 0, pitch_a = 0, pitch_b = 0;
-  int rc = qmm_codes(c, st, lhs, batch, m, k, &tmp[0], &pa, &pitch_a);
+  rc = qmm_codes(c, st, lhs, batch, m, k, &tmp[0], &pa, &pitch_a);
   if (!rc) rc = qmm_codes(c, st, rhs, batch, n, k, &tmp[1], &pb, &pitch_b);
-  auto fp8 = [](int32_t v) { return v == B200_QV_E4M3 ? B200_F8E4M3 : B200_F8E5M2; };
-  GemmProblem g{};
-  g.in_dtype = fp8(lhs->scheme.value); g.rhs_dtype = fp8(rhs->scheme.value); g.out_dtype = out_dtype;
+  GemmProblem g = qf8_problem(lhs, rhs, out_dtype);
   g.a = pa; g.b = pb; g.out = out;
   g.M = m; g.N = n; g.K = k; g.batch = batch;
   g.a_sm = pitch_a; g.a_sk = 1; g.a_sb = batch > 1 ? m * pitch_a : 0;
   g.b_sn = pitch_b; g.b_sk = 1; g.b_sb = batch > 1 ? n * pitch_b : 0;
   g.o_sm = n; g.o_sn = 1; g.o_sb = batch > 1 ? m * n : 0;
-  // kernel block: the finer of the present block levels; a coarser block repeats its scale, a per-tensor side uses g; two
-  // per-tensor sides fold per 128 elements of K (the last block short when 128 does not divide K)
-  const int32_t ba = lhs->scheme.block, bb = rhs->scheme.block;
-  g.q = 3;
-  g.q_bk = (uint32_t)(ba == 0 && bb == 0 ? 128 : ba == 0 ? bb : bb == 0 ? ba : std::min(ba, bb));
   if (!rc) rc = qmm_scales(c, st, lhs, batch, m, k, g.q_bk, &tmp[2]);
   if (!rc) rc = qmm_scales(c, st, rhs, batch, n, k, g.q_bk, &tmp[3]);
   g.q_sa = tmp[2]; g.q_sb = tmp[3];
   if (!rc) rc = launch_wgmma(c, st, g, false, false);
   for (CUdeviceptr t : tmp)
     if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMM has drained
+  return rc;
+}
+
+// Grouped matmul of fp8-quantized operands (ragged M): lhs codes [T, K] against rhs codes [G, N, K], the fold of
+// b200_matmul_quantized_fp8 per row of each group (gemm_grouped_qf8_*, gemm_wgmma.cu: QM_FP8 with CB_GRP_M).  The group's
+// rhs codes and effective scales are batch g of their maps; the lhs is one batch (a_bmul = 0), read at the group's rows.
+extern "C" int b200_matmul_grouped_quantized_fp8(b200_ctx* c, b200_stream s, const b200_quant_operand* lhs, const b200_quant_operand* rhs,
+                                                 b200_dptr offs, uint64_t groups, b200_dtype out_dtype, b200_dptr out, uint64_t t,
+                                                 uint64_t n, uint64_t k) {
+  CTX_ENTER(c);
+  typedef unsigned long long ull;
+  if (!lhs || !rhs) return fail(B200_ERR_INVALID_ARG, "matmul_grouped_quantized_fp8: null operand");
+  if (groups > (uint64_t)kGroupedMaxGroups)
+    return fail(B200_ERR_UNSUPPORTED, "matmul_grouped_quantized_fp8: %llu groups exceed the limit of %d", (ull)groups, kGroupedMaxGroups);
+  if (t >= (1ull << 31) || n >= (1ull << 31) || k >= (1ull << 31))
+    return fail(B200_ERR_UNSUPPORTED, "matmul_grouped_quantized_fp8: extents must be below 2^31");
+  const bool empty = (groups == 0 || t == 0 || n == 0);   // nothing is written: no row lies in a group
+  int rc = qf8_operand_check("matmul_grouped_quantized_fp8 (lhs)", lhs, empty ? 0 : t, k);
+  if (!rc) rc = qf8_operand_check("matmul_grouped_quantized_fp8 (rhs)", rhs, empty ? 0 : groups * n, k);
+  if (rc) return rc;
+  if (out_dtype != B200_F32 && out_dtype != B200_BF16 && out_dtype != B200_F16)
+    return fail(B200_ERR_INVALID_ARG, "matmul_grouped_quantized_fp8: output dtype %d is not F32, BF16 or F16", (int)out_dtype);
+  if (empty) return B200_OK;
+  if (k == 0) return fail(B200_ERR_INVALID_ARG, "matmul_grouped_quantized_fp8: K must be positive");
+  if (!offs) return fail(B200_ERR_INVALID_ARG, "matmul_grouped_quantized_fp8: null offs");
+  if (offs % 4) return fail(B200_ERR_INVALID_ARG, "matmul_grouped_quantized_fp8: offs is misaligned (a compact i32 [groups] array)");
+  if (!out || !lhs->values || !rhs->values) return fail(B200_ERR_INVALID_ARG, "matmul_grouped_quantized_fp8: null device pointer");
+  const size_t osz = dtype_size(out_dtype);
+  if (out % osz) return fail(B200_ERR_INVALID_ARG, "matmul_grouped_quantized_fp8: output pointer is not aligned to its element size");
+  GroupedPlan pl;
+  if ((rc = grouped_plan(c, "matmul_grouped_quantized_fp8", false, 3, groups, t, t, n, &pl))) return rc;
+  const GemmVariant& v = *pl.v;
+  GemmProblem g = qf8_problem(lhs, rhs, out_dtype);
+  g.M = t; g.N = n; g.K = k; g.batch = groups;
+  const std::string name = std::string("gemm_grouped_qf8_") + (g.in_dtype == B200_F8E4M3 ? "e4m3" : "e5m2") + "_" +
+                           (out_dtype == B200_BF16 ? "bf16" : out_dtype == B200_F16 ? "f16" : "f32") + "_" + v.tag + "_kk";
+  const unsigned smem = gemm_q8_smem_bytes(v) + kGroupedTableBytes;
+  CUstream st = resolve_stream(c, s);
+  CUdeviceptr tmp[4] = {0, 0, 0, 0};   // lhs codes, rhs codes, lhs scales, rhs scales
+  uint64_t pa = 0, pb = 0, pitch_a = 0, pitch_b = 0;
+  rc = qmm_codes(c, st, lhs, 1, t, k, &tmp[0], &pa, &pitch_a);
+  if (!rc) rc = qmm_codes(c, st, rhs, groups, n, k, &tmp[1], &pb, &pitch_b);
+  if (!rc) rc = qmm_scales(c, st, lhs, 1, t, k, g.q_bk, &tmp[2]);
+  if (!rc) rc = qmm_scales(c, st, rhs, groups, n, k, g.q_bk, &tmp[3]);
+  g.q_sa = tmp[2]; g.q_sb = tmp[3];
+  CUfunction f = nullptr;
+  if (!rc) rc = gemm_kernel(c, name, smem, &f);
+  CUtensorMap ta, tb, ta_sc, tb_sc;
+  if (!rc) rc = encode_operand(c, &ta, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, pa, t, k, 1, pitch_a, 1, 0, false, 128);
+  if (!rc) rc = encode_operand(c, &tb, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, pb, n, k, groups, pitch_b, 1, n * pitch_b, false,
+                               (uint32_t)(v.block_n / v.cg));
+  GemmParams p;
+  gemm_params(c, &p, v, osz, out, n, 0, t, n, k, 1, pl.tile_rows, nullptr);
+  p.b_bmul = groups > 1 ? 1u : 0u;   // a_bmul stays 0: the lhs is one batch, whatever the group
+  if (!rc) rc = gemm_quant_params(c, g, v, true, groups == 1, &ta_sc, &tb_sc, &p);
+  if (!rc) rc = grouped_launch(c, st, f, pl, smem, osz, offs, groups, t, false, &p, {&ta, &tb, &ta_sc, &tb_sc});
+  for (CUdeviceptr x : tmp)
+    if (x) pool_free(c, x, st);   // stream-ordered: reusable by later work once the GEMM has drained
   return rc;
 }
 

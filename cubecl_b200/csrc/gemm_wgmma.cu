@@ -249,8 +249,8 @@ struct GrpUnit {
   uint32_t nkb;       // k-blocks of the tile
 };
 // tile t of a grouped launch: its group (ragged M: the last g with pre[g] <= t / tiles_n, by bisection), and its coordinate
-// inside the group's grid of tile-rows x tiles_n in group_m strips
-template <int CB, uint32_t MASK>
+// inside the group's grid of tile-rows x tiles_n in group_m strips; ragged M runs ceil(K / BLOCK_K) k-blocks per tile
+template <int CB, uint32_t MASK, uint32_t BLOCK_K>
 __device__ __forceinline__ GrpUnit grp_unit(uint32_t t, const GemmParams& p, const GroupedParams& gp, const uint32_t* o, const uint32_t* pre) {
   uint32_t g, loc, tiles_m;
   if constexpr (CB == CB_GRP_M) {
@@ -276,7 +276,7 @@ __device__ __forceinline__ GrpUnit grp_unit(uint32_t t, const GemmParams& p, con
   u.lo = g ? o[g - 1] : 0u;
   u.hi = o[g];
   u.row0 = u.lo & ~MASK;
-  u.nkb = (CB == CB_GRP_M) ? (p.K + 63u) / 64u : (u.hi - u.lo + 63u) / 64u;
+  u.nkb = (CB == CB_GRP_M) ? (p.K + BLOCK_K - 1u) / BLOCK_K : (u.hi - u.lo + 63u) / 64u;
   return u;
 }
 
@@ -300,16 +300,21 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
                                           const TconvParams* tcp = nullptr, const GroupedParams* gpp = nullptr) {
   constexpr bool INT_ACC = (KIND == KIND_U8 || KIND == KIND_S8) && QM != QM_BLOCK;
   constexpr bool GRP = (CB == CB_GRP_M || CB == CB_GRP_K);
-  static_assert(!GRP || (!CONV && (KIND == KIND_BF16 || KIND == KIND_F16) && !PROMOTE && MT == 1 && QM == QM_NONE && CONV_DIMS == 2),
-                "grouped matmul: 16-bit kinds, one M sub-tile");
+  // ragged M also takes fp8-quantized K-major operands (gemm_grouped_qf8_*): the QM_FP8 producer loads the lhs scale tile at
+  // the group's rows (m0) and the rhs one from the group's batch (bb)
+  static_assert(!GRP || (!CONV && !PROMOTE && MT == 1 && CONV_DIMS == 2 &&
+                         (((KIND == KIND_BF16 || KIND == KIND_F16) && QM == QM_NONE) ||
+                          (CB == CB_GRP_M && QM == QM_FP8 && !A_MN && !B_MN))),
+                "grouped matmul: 16-bit kinds (fp8-quantized K-major operands for ragged M), one M sub-tile");
   static_assert(CB != CB_GRP_K || (A_MN && B_MN), "ragged K: MN-major operands");
-  // ragged M with an M-contiguous lhs: the group's first row is the innermost coordinate of the A loads, and such loads at
-  // coordinates that are not a multiple of 16 bytes faulted (illegal instruction) on an H100 -- the group's tile-rows start
-  // at a multiple of 64 rows instead, and the rows before the group are not stored
-  constexpr uint32_t GRP_MASK = (CB == CB_GRP_M && A_MN) ? 63u : 0u;
   static_assert(QM == QM_NONE || ((QM == QM_FP8 ? (KIND == KIND_E4M3 || KIND == KIND_E5M2) : KIND == KIND_S8) && !A_MN && !B_MN &&
                                   !PROMOTE && MT == 1), "quantized operands: s8 (fp8 for QM_FP8), K-major");
   constexpr bool QBLK = (QM == QM_BLOCK || QM == QM_FP8);   // per-block scale tiles in every stage
+  // ragged M with an M-contiguous lhs: the group's first row is the innermost coordinate of the A loads, and such loads at
+  // coordinates that are not a multiple of 16 bytes faulted (illegal instruction) on an H100 -- the group's tile-rows start
+  // at a multiple of 64 rows instead, and the rows before the group are not stored.  With per-block scale tiles the row is
+  // the innermost coordinate of the f32 A scale load ([blocks][rows]): tile-rows start at a multiple of 4 rows.
+  constexpr uint32_t GRP_MASK = (CB == CB_GRP_M && A_MN) ? 63u : (CB == CB_GRP_M && QBLK) ? 3u : 0u;
   static_assert(!CONV || ((KIND == KIND_BF16 || KIND == KIND_F16) && !A_MN && !B_MN && !PROMOTE && MT == 1 && QM == QM_NONE),
                 "convolution: 16-bit kinds, K-major operands");
   static_assert(CB != CB_DGRAD || CONV, "data gradient: the convolution producer");
@@ -452,7 +457,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
         GrpUnit gu;
         if constexpr (GRP) {
           if (wu.tile >= grp_total) break;
-          gu = grp_unit<CB, GRP_MASK>(wu.tile, p, *gpp, grp_o, grp_pre);
+          gu = grp_unit<CB, GRP_MASK, BLOCK_K>(wu.tile, p, *gpp, grp_o, grp_pre);
           wu.kb0 = 0;
           wu.kb1 = gu.nkb;
         }
@@ -649,7 +654,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
       GrpUnit gu;
       if constexpr (GRP) {
         if (wu.tile >= grp_total) break;
-        gu = grp_unit<CB, GRP_MASK>(wu.tile, p, *gpp, grp_o, grp_pre);
+        gu = grp_unit<CB, GRP_MASK, BLOCK_K>(wu.tile, p, *gpp, grp_o, grp_pre);
         wu.kb0 = 0;
         wu.kb1 = gu.nkb;
         tq_keep = gu.nkb != 0 ? 0xFFFFFFFFu : 0u;
@@ -1237,7 +1242,27 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
   GRP_ONE(TILE, CG, BN, f16, f16, KIND_F16, OUT_F16)              \
   GRP_ONE(TILE, CG, BN, f16, f32, KIND_F16, OUT_F32)
 
-// The kernels are built as ten cubins from this one source (cubecl_b200/build.py compiles them in parallel):
+// Grouped matmul of fp8-quantized operands, ragged M (capi.cpp: b200_matmul_grouped_quantized_fp8): the maps of
+// gemm_qf8_* (lhs codes [T, K], rhs codes with the group as batch, and their effective-scale tiles), tma_out, GroupedParams.
+// Names gemm_grouped_qf8_<lhs format>_<out>_<tile>_kk; the rhs format is chosen at run time
+#define GRP_QF8_KERNEL(NAME, CG, BN, KIND, OUT)                                                                   \
+  extern "C" __global__ void __launch_bounds__(kNumThreads, 1)                                                     \
+      NAME(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,                  \
+           const __grid_constant__ CUtensorMap tma_a_sc, const __grid_constant__ CUtensorMap tma_b_sc,            \
+           const __grid_constant__ CUtensorMap tma_out, const __grid_constant__ GroupedParams gp,                 \
+           const __grid_constant__ GemmParams p) {                                                                \
+    gemm_body<CG, BN, false, false, KIND, OUT, 5, false, 1, QM_FP8, false, CB_GRP_M>(&tma_a, &tma_b, &tma_a_sc, &tma_b_sc, &tma_out, p, \
+                                                                                     nullptr, &gp);               \
+  }
+#define GRP_QF8(TILE, CG, BN)                                                          \
+  GRP_QF8_KERNEL(gemm_grouped_qf8_e4m3_bf16_##TILE##_kk, CG, BN, KIND_E4M3, OUT_BF16)   \
+  GRP_QF8_KERNEL(gemm_grouped_qf8_e4m3_f16_##TILE##_kk, CG, BN, KIND_E4M3, OUT_F16)     \
+  GRP_QF8_KERNEL(gemm_grouped_qf8_e4m3_f32_##TILE##_kk, CG, BN, KIND_E4M3, OUT_F32)     \
+  GRP_QF8_KERNEL(gemm_grouped_qf8_e5m2_bf16_##TILE##_kk, CG, BN, KIND_E5M2, OUT_BF16)   \
+  GRP_QF8_KERNEL(gemm_grouped_qf8_e5m2_f16_##TILE##_kk, CG, BN, KIND_E5M2, OUT_F16)     \
+  GRP_QF8_KERNEL(gemm_grouped_qf8_e5m2_f32_##TILE##_kk, CG, BN, KIND_E5M2, OUT_F32)
+
+// The kernels are built as eleven cubins from this one source (cubecl_b200/build.py compiles them in parallel):
 //   GEMM_PART 0 ("gemm")       256 x 256 pair tiles (2-CTA cluster, 128 x 256 per CTA) and the bf16 peak probe
 //   GEMM_PART 1 ("gemm_b")     256 x 128 pair tiles, 256 x 224 block-scaled pair tiles
 //   GEMM_PART 2 ("gemm_c")     128 x 128 single-CTA tiles, 512 x 128 pair tiles
@@ -1248,6 +1273,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tma_a_hi, const CUt
 //   GEMM_PART 7 ("gemm_convt")    the phase-batched transposed-convolution kernels, 2-D and 3-D, of the same two tiles
 //   GEMM_PART 8 ("gemm_grouped")  the grouped-matmul kernels (ragged M and ragged K) of the same two tiles
 //   GEMM_PART 9 ("gemm_qf8")      the fp8-quantized kernels (QM_FP8) of the same two tiles
+//   GEMM_PART 10 ("gemm_grouped_qf8")  the fp8-quantized grouped-matmul kernels (QM_FP8, ragged M) of the same two tiles
 #ifndef GEMM_PART
 #define GEMM_PART 0
 #endif
@@ -1319,6 +1345,10 @@ GRP_DTYPES(1sm_n128, 1, 128)
 // the per-block stage count of gemm_q8_* (capi.cpp: gemm_q8_stages)
 GEMM_QF8(2sm_n128, 2, 128)
 GEMM_QF8(1sm_n128, 1, 128)
+#endif
+#if GEMM_PART == 10
+GRP_QF8(2sm_n128, 2, 128)
+GRP_QF8(1sm_n128, 1, 128)
 #endif
 
 #if GEMM_PART == 0

@@ -240,6 +240,51 @@ def launch_grouped_alloc(client: ComputeClient, lhs: TensorHandle, rhs: TensorHa
     return out
 
 
+def launch_grouped_quantized_fp8(client: ComputeClient, qx, qw, offs: TensorHandle, out: TensorHandle, stream=None) -> None:
+    """Grouped matmul of fp8-quantized operands for mixture-of-experts layers (cubecl_b200.quant.QuantizedTensor, values e4m3
+    or e5m2 on either side): qx [T, K] (the routed tokens sorted by expert) x qw [G, N, K] (the experts' weights, nn.Linear
+    layout) -> out [T, N] contiguous f32 / bf16 / f16; rows of group g fold against qw[g] as launch_quantized_fp8 folds them.
+    offs is a compact i32 [G] device tensor of cumulative ends, read on the device only; rows >= offs[-1] are not written.  See
+    b200_matmul_grouped_quantized_fp8 in include/cubecl_b200.h for the contract.  Errors are deferred to client.sync()."""
+    what = "matmul_grouped_quantized_fp8"
+    try:
+        xs, ws = list(qx.shape), list(qw.shape)
+        if len(xs) != 2 or len(ws) != 3:
+            raise B200Error(6, f"{what}: qx [T, K] and qw [G, N, K] expected, got {xs} and {ws}")
+        if xs[1] != ws[2]:
+            raise B200Error(6, f"{what}: K mismatch (qx {xs[1]}, qw {ws[2]})")
+        if offs.dtype != "i32" or len(offs.shape) != 1 or not offs.is_contiguous():
+            raise B200Error(6, f"{what}: offs must be a compact i32 [groups] tensor")
+        if offs.shape[0] != ws[0]:
+            raise B200Error(6, f"{what}: {offs.shape[0]} groups in offs, but qw has {ws[0]}")
+        T, (G, N, K) = xs[0], ws
+        if list(out.shape) != [T, N] or not out.is_contiguous():
+            raise B200Error(6, f"{what}: out must be contiguous with shape {[T, N]}")
+        ops = []
+        for q in (qx, qw):
+            for t in (q.values, q.block_scales, q.tensor_scale):
+                if t is not None:
+                    t.handle.used_on(stream)
+            ops.append(_ffi.QuantOperand(q.scheme.to_c(), *(t.handle.ptr if t is not None else 0
+                                                              for t in (q.values, q.block_scales, q.tensor_scale))))
+        offs.handle.used_on(stream)
+        out.handle.used_on(stream)
+        _ffi.check(client._lib.b200_matmul_grouped_quantized_fp8(client._ctx, stream, C.byref(ops[0]), C.byref(ops[1]),
+                                                                 C.c_uint64(offs.handle.ptr), G, DTYPES[out.dtype],
+                                                                 C.c_uint64(out.handle.ptr), T, N, K))
+    except B200Error as e:
+        client._defer(e)
+
+
+def launch_grouped_quantized_fp8_alloc(client: ComputeClient, qx, qw, offs: TensorHandle, out_dtype: str = "bf16",
+                                       stream=None) -> TensorHandle:
+    """Convenience: allocate a contiguous out [T, N] of `out_dtype`, then launch_grouped_quantized_fp8 (the rows past the last
+    group stay uninitialised)."""
+    out = TensorHandle.empty_contiguous(client, [qx.shape[0], qw.shape[1] if len(qw.shape) == 3 else 0], out_dtype)
+    launch_grouped_quantized_fp8(client, qx, qw, offs, out, stream)
+    return out
+
+
 def launch_alloc(client: ComputeClient, lhs: TensorHandle, rhs: TensorHandle, out_dtype: str | None = None) -> TensorHandle:
     """Convenience: allocate `out` with the reference's shape rule, then launch."""
     shape = calculate_matmul_output(lhs.shape, rhs.shape)

@@ -369,6 +369,32 @@ int b200_matmul_quantized(b200_ctx* ctx, b200_stream s, const b200_quant_operand
 int b200_matmul_quantized_fp8(b200_ctx* ctx, b200_stream s, const b200_quant_operand* lhs, const b200_quant_operand* rhs,
                               b200_dtype out_dtype, b200_dptr out, uint64_t batch, uint64_t m, uint64_t n, uint64_t k);
 
+/* ---- grouped matmul of fp8-quantized operands for mixture-of-experts layers (ragged M), in one launch --------------------
+ * lhs codes [T, K]: the routed tokens sorted by expert.  rhs codes [G, N, K]: the experts' weights in nn.Linear layout,
+ * groups = G.  out [T, N] compact in F32 / BF16 / F16.  Both operands are quantized along K exactly as b200_quantize writes
+ * them: b200_quantize of a [G, N, K] tensor is one rhs operand, and its per-tensor level is one g shared by all experts.
+ * offs: a compact, 4-byte aligned i32 [G] device array of cumulative ends, read on the device only (no host sync; the call can
+ * be captured in a graph), clamped on read as for b200_matmul_grouped: o_g = min(max(offs[g], o_{g-1}), T), o_{-1} = 0.  Row
+ * r of group g (o_{g-1} <= r < o_g) is b200_matmul_quantized_fp8's fold of lhs row r against rhs[g] -- the same Bk rule
+ * (the finer present block; two per-tensor sides fold per 128 with a short last block) and the same steps
+ * acc_{j+1} = fma(P_j, rn(eff_a * eff_b), acc_j).  Rows >= o_{G-1} are not written; a malformed table makes groups empty or
+ * short but never moves an access out of bounds.  No epilogue, no stream-K head, no atomics: bitwise reproducible.
+ * Values E4M3 or E5M2, independently per side; per-tensor, per-block (32, 64, 128) or two-level scales on either side, in
+ * every block-scale dtype b200_dequantize reads.
+ * Recipes, with no extra code: DeepSeek-style 128 x 128 weight scales [G, N / 128, K / 128] -- repeat each scale row 128
+ * times into [G, N, K / 128] and pass the weights as a per-block-128 F32 operand (exact, as for the dense call).  A
+ * per-expert tensor scale s_g -- a per-block-128 F32 scale array [G, N, K / 128] filled with s_g.
+ * Errors: B200_ERR_UNSUPPORTED for integer values (use b200_matmul_quantized), e2m1, blocks of 8 or 16, groups > 1024,
+ * extents >= 2^31 and a tile bound >= 2^32; B200_ERR_INVALID_ARG for everything b200_quantize's checks reject, a null or
+ * misaligned offs, a null code or output pointer, K == 0 with a non-empty output and a "gemm.variant" that is not a grouped
+ * tile.  groups, T or N of 0 is a no-op.
+ * Launches: 2 effective-scale passes + 1 GEMM (gemm_grouped_qf8_<lhs>_<out>_<2sm_n128 | 1sm_n128>_kk, the rhs format chosen
+ * at run time); +1 per operand TMA cannot read in place (staging).  "gemm.variant" (auto, 2sm_n128, 1sm_n128) and
+ * "gemm.epilogue" apply; "gemm.split_k" does not.  Temporaries come from the pool, stream-ordered. */
+int b200_matmul_grouped_quantized_fp8(b200_ctx* ctx, b200_stream s, const b200_quant_operand* lhs, const b200_quant_operand* rhs,
+                                      b200_dptr offs, uint64_t groups, b200_dtype out_dtype, b200_dptr out, uint64_t t,
+                                      uint64_t n, uint64_t k);
+
 /* ---- 2-D convolution (cubek's convolution kernels), an implicit GEMM on the wgmma kernel --------------------------------
  * out[n, oh, ow, co] = act(alpha * sum_{ky, kx, c} x[n, oh*sh - ph + ky*dh, ow*sw - pw + kx*dw, c] * w[co, ky, kx, c] + bias[co]).
  * Input outside x reads as zero; f32 accumulation; the epilogue is b200_epilogue (NULL = none).  x is [N, H, W, C] (NHWC), w is

@@ -243,6 +243,20 @@ inline void launch_grouped(ComputeClient& client, const TensorHandle& lhs, const
                                      out.shape.data(), out.strides.data(), epilogue);
   if (rc != B200_OK) client.defer(b200_last_error());
 }
+/// Grouped matmul of fp8-quantized operands for mixture-of-experts layers: lhs codes [t, k] (tokens sorted by expert) x rhs
+/// codes [groups, n, k] (the experts' weights) -> out [t, n] (contiguous, F32 / BF16 / F16), each group's rows folded as
+/// b200_matmul_quantized_fp8 folds them; offs is a compact i32 [groups] tensor of cumulative ends read on the device only.
+/// See b200_matmul_grouped_quantized_fp8 in cubecl_b200.h for the contract.  Errors are deferred to client.sync().
+inline void launch_grouped_quantized_fp8(ComputeClient& client, const b200_quant_operand& lhs, const b200_quant_operand& rhs,
+                                         const TensorHandle& offs, const TensorHandle& out, uint64_t t, uint64_t n, uint64_t k) {
+  if (offs.dtype != DType::I32 || offs.shape.size() != 1 || (offs.shape[0] > 1 && offs.strides[0] != 1)) {
+    client.defer("InvalidArgument: matmul_grouped_quantized_fp8 needs a compact i32 [groups] offs");
+    return;
+  }
+  const int rc = b200_matmul_grouped_quantized_fp8(client.raw(), nullptr, &lhs, &rhs, offs.handle.ptr(), offs.shape[0],
+                                                   static_cast<b200_dtype>(out.dtype), out.handle.ptr(), t, n, k);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
 }  // namespace matmul
 
 namespace conv {

@@ -970,6 +970,22 @@ impl Context {
         check(sys::b200_matmul_quantized_fp8(self.0, stream, &a, &b, out_dtype as c_int, out, batch, m, n, k))
     }
 
+    /// out [t, n] (contiguous, F32 / BF16 / F16): grouped matmul of fp8-quantized operands for mixture-of-experts layers, lhs
+    /// codes [t, k] (tokens sorted by expert) against rhs codes [groups, n, k] (the experts' weights), both quantized along k;
+    /// `offs` is a compact i32 [groups] device array of cumulative ends read on the device only, and rows past the last group
+    /// are not written.  The contract is `b200_matmul_grouped_quantized_fp8`'s in include/cubecl_b200.h.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::matmul`]; `offs` must hold `groups` i32 values on this context's device.
+    #[allow(clippy::too_many_arguments)]
+    pub unsafe fn matmul_grouped_quantized_fp8(
+        &mut self, stream: b200_stream, lhs: &QuantOperand, rhs: &QuantOperand, offs: b200_dptr, groups: u64, out_dtype: DType,
+        out: b200_dptr, t: u64, n: u64, k: u64,
+    ) -> Result<(), Error> {
+        let (a, b) = (lhs.raw(), rhs.raw());
+        check(sys::b200_matmul_grouped_quantized_fp8(self.0, stream, &a, &b, offs, groups, out_dtype as c_int, out, t, n, k))
+    }
+
     /// out (compact row-major) = gather of the strided tensor `input` (into_contiguous, cubecl-std/src/tensor/contiguous.rs).
     ///
     /// # Safety
