@@ -663,6 +663,26 @@ static int pool_free(b200_ctx* c, CUdeviceptr p, CUstream used_on = nullptr) {
   return B200_OK;
 }
 
+// The pooled temporaries of one call (or of one scope of it): alloc() takes pages from the pool on the call's stream, and
+// leaving the scope returns every page handed out, in allocation order, stream-ordered -- the pool gives a page out again
+// only to later work, once the launches queued on `st` have drained.  Error returns need no cleanup of their own.
+struct Scratch {
+  b200_ctx* c;
+  CUstream st;
+  std::vector<CUdeviceptr> held;
+  Scratch(b200_ctx* c, CUstream st) : c(c), st(st) {}
+  Scratch(const Scratch&) = delete;
+  Scratch& operator=(const Scratch&) = delete;
+  ~Scratch() {
+    for (CUdeviceptr p : held) pool_free(c, p, st);
+  }
+  int alloc(size_t bytes, CUdeviceptr* out) {
+    const int rc = pool_alloc(c, bytes, out, st);
+    if (!rc) held.push_back(*out);
+    return rc;
+  }
+};
+
 extern "C" int b200_alloc(b200_ctx* c, size_t bytes, b200_dptr* out) {
   CTX_ENTER(c);
   if (!out) return fail(B200_ERR_INVALID_ARG, "null out");
@@ -1408,7 +1428,7 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
   if (total_tiles >= (1ull << 32)) return fail(B200_ERR_UNSUPPORTED, "too many tiles");
 
   // Stream-K head (plan chosen with the variant above)
-  CUdeviceptr slabs = 0;
+  Scratch scr(c, st);
   uint64_t units = total_tiles;
   p.full_tiles = (uint32_t)total_tiles;
   if (best_sk.sk_tiles) {
@@ -1417,7 +1437,8 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
     rc = reduce_workspace(c, st, &ws);
     if (rc) return rc;
     const uint64_t slab_bytes = 128ull * v.cg * v.block_n * 4;
-    rc = pool_alloc(c, best_sk.ranges * best_sk.umax * slab_bytes, &slabs, st);
+    CUdeviceptr slabs;
+    rc = scr.alloc(best_sk.ranges * best_sk.umax * slab_bytes, &slabs);
     if (rc) return rc;
     p.full_tiles = (uint32_t)(total_tiles - best_sk.sk_tiles);
     p.sk_tiles = (uint32_t)best_sk.sk_tiles;
@@ -1435,43 +1456,27 @@ static int launch_wgmma(b200_ctx* c, CUstream st, const GemmProblem& g, bool a_m
     }
   }
   void* args[] = {&ta, &tb, &ta_lo, &tb_lo, &tout, &p};
-  rc = gemm_launch(c, st, f, v, units, smem, args);
-  if (slabs) pool_free(c, slabs, st);  // stream-ordered: reusable by later work once this launch has drained
-  return rc;
+  return gemm_launch(c, st, f, v, units, smem, args);
 }
 
-static inline uint64_t pad4(uint64_t elems) { return (elems + 3) / 4 * 4; }
-
-// lo = x - trunc_tf32(x) of a logical [batch, rows, cols] view (cols innermost), written with row pitch pad4(cols)
-static int launch_split(b200_ctx* c, CUstream st, uint64_t in, uint64_t out, uint64_t batch, uint64_t rows, uint64_t cols,
-                        uint64_t in_bs, uint64_t in_rs) {
+// One split pass over a logical [batch, rows, cols] f32 view (cols innermost), `vec` elements per thread, rows written with
+// their pitch rounded up to `vec` elements.  split_tf32_lo (vec 4) writes lo = x - trunc_tf32(x); split_f32_bf16_pair (vec 8)
+// writes the bf16 pair, plane 0 = bf16(x), plane 1 = bf16(x - trunc_tf32(x)).
+static int launch_split(b200_ctx* c, CUstream st, const char* kernel, uint64_t vec, uint64_t in, uint64_t out, uint64_t batch,
+                        uint64_t rows, uint64_t cols, uint64_t in_bs, uint64_t in_rs) {
   CUfunction f;
-  int rc = get_func(c, "split_tf32_lo", &f);
+  int rc = get_func(c, kernel, &f);
   if (rc) return rc;
-  SplitParams p{in, out, batch, rows, cols, in_bs, in_rs, pad4(cols)};
+  SplitParams p{in, out, batch, rows, cols, in_bs, in_rs, (cols + vec - 1) / vec * vec};
   const uint64_t total = batch * rows * cols;
-  const unsigned grid = (unsigned)std::min<uint64_t>((total / 4 + 255) / 256 + 1, (uint64_t)c->props.num_sms * 16);
-  void* args[] = {&p};
-  return launch(c, f, std::max(1u, grid), 1, 1, 256, 0, 1, st, args);
-}
-
-// bf16 pair of a logical [batch, rows, cols] f32 view: plane 0 = bf16(x), plane 1 = bf16(x - trunc_tf32(x)), rows pitched to 8 elements
-static inline uint64_t pad8e(uint64_t elems) { return (elems + 7) / 8 * 8; }
-static int launch_split_pair(b200_ctx* c, CUstream st, uint64_t in, uint64_t out, uint64_t batch, uint64_t rows, uint64_t cols,
-                             uint64_t in_bs, uint64_t in_rs) {
-  CUfunction f;
-  int rc = get_func(c, "split_f32_bf16_pair", &f);
-  if (rc) return rc;
-  SplitParams p{in, out, batch, rows, cols, in_bs, in_rs, pad8e(cols)};
-  const uint64_t total = batch * rows * cols;
-  const unsigned grid = (unsigned)std::min<uint64_t>((total / 8 + 255) / 256 + 1, (uint64_t)c->props.num_sms * 16);
+  const unsigned grid = (unsigned)std::min<uint64_t>((total / vec + 255) / 256 + 1, (uint64_t)c->props.num_sms * 16);
   void* args[] = {&p};
   return launch(c, f, std::max(1u, grid), 1, 1, 256, 0, 1, st, args);
 }
 
 // One pass that copies an operand TMA cannot describe (row pitch or base not 16-byte aligned, no unit stride) into a pooled
 // buffer it can: [batch, rows, pitch] with the operand's own contiguous dimension innermost when it has one.
-static int stage_operand(b200_ctx* c, CUstream st, size_t esz, uint64_t ptr, uint64_t batch, uint64_t mn, uint64_t K, uint64_t s_mn, uint64_t s_k,
+static int stage_operand(Scratch& scr, size_t esz, uint64_t ptr, uint64_t batch, uint64_t mn, uint64_t K, uint64_t s_mn, uint64_t s_k,
                          uint64_t s_b, CUdeviceptr* out, uint64_t* o_smn, uint64_t* o_sk, uint64_t* o_sb) {
   // rows of the M / N extent are kept (coalesced both ways) where wgmma reads them: 16-bit operands
   const bool keep_mn_major = (s_mn == 1 && s_k != 1) && esz == 2;
@@ -1479,17 +1484,15 @@ static int stage_operand(b200_ctx* c, CUstream st, size_t esz, uint64_t ptr, uin
   const uint64_t q = 16 / esz, pitch = (cols + q - 1) / q * q;
   const uint64_t nb = (s_b == 0) ? 1 : batch;                  // a broadcast operand is staged once
   CUdeviceptr buf;
-  int rc = pool_alloc(c, nb * rows * pitch * esz, &buf, st);
-  if (rc) return rc;
   CUfunction f;
-  rc = get_func(c, "repitch_rows", &f);
-  if (rc) { pool_free(c, buf, st); return rc; }
+  int rc = scr.alloc(nb * rows * pitch * esz, &buf);
+  if (!rc) rc = get_func(scr.c, "repitch_rows", &f);
+  if (rc) return rc;
   RepitchParams p{ptr, buf, nb, rows, cols, s_b, keep_mn_major ? s_k : s_mn, keep_mn_major ? s_mn : s_k, pitch, (uint32_t)esz, 0};
   const uint64_t vecs = nb * rows * (pitch / q);               // one 16-byte output vector per thread
   const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((vecs + 255) / 256, 0x7FFFFFFFull));
   void* args[] = {&p};
-  rc = launch(c, f, grid, 1, 1, 256, 0, 1, st, args);
-  if (rc) { pool_free(c, buf, st); return rc; }
+  if ((rc = launch(scr.c, f, grid, 1, 1, 256, 0, 1, scr.st, args))) return rc;
   *out = buf;
   *o_smn = keep_mn_major ? 1 : pitch;
   *o_sk = keep_mn_major ? pitch : 1;
@@ -1502,24 +1505,22 @@ static int run_gemm(b200_ctx* c, CUstream st, const GemmProblem& g);
 
 // An fp8 operand widened to f16 (exact) in a pooled [batch, rows, pitch] buffer that keeps the operand's own contiguous
 // dimension innermost when it has one (wgmma reads 16-bit operands in either major).
-static int widen_fp8_operand(b200_ctx* c, CUstream st, int dtype, uint64_t ptr, uint64_t batch, uint64_t mn, uint64_t K, uint64_t s_mn,
+static int widen_fp8_operand(Scratch& scr, int dtype, uint64_t ptr, uint64_t batch, uint64_t mn, uint64_t K, uint64_t s_mn,
                              uint64_t s_k, uint64_t s_b, CUdeviceptr* out, uint64_t* o_smn, uint64_t* o_sk, uint64_t* o_sb) {
   const bool keep_mn_major = (s_mn == 1 && s_k != 1);
   const uint64_t rows = keep_mn_major ? K : mn, cols = keep_mn_major ? mn : K;
   const uint64_t pitch = (cols + 7) / 8 * 8;
   const uint64_t nb = (s_b == 0) ? 1 : batch;
   CUdeviceptr buf;
-  int rc = pool_alloc(c, nb * rows * pitch * 2, &buf, st);
-  if (rc) return rc;
   CUfunction f;
-  rc = get_func(c, "convert_fp8_f16", &f);
-  if (rc) { pool_free(c, buf, st); return rc; }
+  int rc = scr.alloc(nb * rows * pitch * 2, &buf);
+  if (!rc) rc = get_func(scr.c, "convert_fp8_f16", &f);
+  if (rc) return rc;
   ConvertF16Params p{ptr, buf, nb, rows, cols, s_b, keep_mn_major ? s_k : s_mn, keep_mn_major ? s_mn : s_k, pitch, (uint32_t)dtype, 0};
   const uint64_t vecs = nb * rows * (pitch / 8);
-  const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((vecs + 255) / 256, (uint64_t)c->props.num_sms * 16));
+  const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((vecs + 255) / 256, (uint64_t)scr.c->props.num_sms * 16));
   void* args[] = {&p};
-  rc = launch(c, f, grid, 1, 1, 256, 0, 1, st, args);
-  if (rc) { pool_free(c, buf, st); return rc; }
+  if ((rc = launch(scr.c, f, grid, 1, 1, 256, 0, 1, scr.st, args))) return rc;
   *out = buf;
   *o_smn = keep_mn_major ? 1 : pitch;
   *o_sk = keep_mn_major ? pitch : 1;
@@ -1534,17 +1535,14 @@ static int run_gemm_fp8_as_f16(b200_ctx* c, CUstream st, const GemmProblem& g) {
   GemmProblem h = g;
   h.in_dtype = B200_F16;
   h.rhs_dtype = -1;
+  Scratch scr(c, st);
   CUdeviceptr wa = 0, wb = 0;
-  int rc = widen_fp8_operand(c, st, g.in_dtype, g.a, g.batch, g.M, g.K, g.a_sm, g.a_sk, g.a_sb, &wa, &h.a_sm, &h.a_sk, &h.a_sb);
-  if (!rc) rc = widen_fp8_operand(c, st, rdt, g.b, g.batch, g.N, g.K, g.b_sn, g.b_sk, g.b_sb, &wb, &h.b_sn, &h.b_sk, &h.b_sb);
-  if (!rc) {
-    h.a = wa;
-    h.b = wb;
-    rc = run_gemm(c, st, h);
-  }
-  if (wa) pool_free(c, wa, st);
-  if (wb) pool_free(c, wb, st);
-  return rc;
+  int rc = widen_fp8_operand(scr, g.in_dtype, g.a, g.batch, g.M, g.K, g.a_sm, g.a_sk, g.a_sb, &wa, &h.a_sm, &h.a_sk, &h.a_sb);
+  if (!rc) rc = widen_fp8_operand(scr, rdt, g.b, g.batch, g.N, g.K, g.b_sn, g.b_sk, g.b_sb, &wb, &h.b_sn, &h.b_sk, &h.b_sb);
+  if (rc) return rc;
+  h.a = wa;
+  h.b = wb;
+  return run_gemm(c, st, h);
 }
 
 static int run_gemm(b200_ctx* c, CUstream st, const GemmProblem& g) {
@@ -1570,54 +1568,35 @@ static int run_gemm(b200_ctx* c, CUstream st, const GemmProblem& g) {
   const std::string f32_mode = g.in_dtype == B200_F32 ? opt(c, "gemm.f32", "hybrid") : std::string();
   if (g.in_dtype == B200_F32 && f32_mode != "hybrid" && f32_mode != "3xtf32" && f32_mode != "tf32")
     return fail(B200_ERR_INVALID_ARG, "gemm.f32 must be hybrid, 3xtf32 or tf32");
-  if (f32_mode == "hybrid") {
-    // f32-grade product in TWO tensor passes' worth of time, one launch: x = hi + lo with hi = the top 19 bits (what the tf32
-    // datapath reads from the original tensor).  hi*hi runs as kind::tf32 on the originals; the cross terms A*B_lo + A_lo*B run
-    // as kind::f16 on bf16 copies (bf16(A), bf16(B_lo), bf16(A_lo), bf16(B)) at twice the tf32 rate, into the same f32
-    // accumulators.  The cross terms are ~2^-11 of the product, so their bf16 rounding (2^-9) lands at ~2^-20 of it.
-    const uint64_t ab = (g.a_sb == 0) ? 1 : g.batch, bb = (g.b_sb == 0) ? 1 : g.batch;
-    const uint64_t a_elems = !a_mn ? g.M * pad8e(g.K) : g.K * pad8e(g.M), b_elems = !b_mn ? g.N * pad8e(g.K) : g.K * pad8e(g.N);
-    CUdeviceptr a_p = 0, b_p = 0;
-    int rc = pool_alloc(c, 2 * ab * a_elems * 2, &a_p, st);
-    if (rc) return rc;
-    rc = pool_alloc(c, 2 * bb * b_elems * 2, &b_p, st);
-    if (rc) { pool_free(c, a_p, st); return rc; }
-    rc = !a_mn ? launch_split_pair(c, st, g.a, a_p, ab, g.M, g.K, g.a_sb, g.a_sm) : launch_split_pair(c, st, g.a, a_p, ab, g.K, g.M, g.a_sb, g.a_sk);
-    if (!rc) rc = !b_mn ? launch_split_pair(c, st, g.b, b_p, bb, g.N, g.K, g.b_sb, g.b_sn) : launch_split_pair(c, st, g.b, b_p, bb, g.K, g.N, g.b_sb, g.b_sk);
-    if (!rc) {
-      GemmProblem h = g;
-      h.a_lo = a_p;
-      h.b_lo = b_p;
-      h.hybrid = true;
-      rc = launch_wgmma(c, st, h, a_mn, b_mn);
-    }
-    pool_free(c, a_p, st);
-    pool_free(c, b_p, st);
-    return rc;
-  }
-  if (f32_mode == "3xtf32") {
+  if (f32_mode == "hybrid" || f32_mode == "3xtf32") {
+    // hybrid: an f32-grade product in TWO tensor passes' worth of time, one launch: x = hi + lo with hi = the top 19 bits (what
+    // the tf32 datapath reads from the original tensor).  hi*hi runs as kind::tf32 on the originals; the cross terms
+    // A*B_lo + A_lo*B run as kind::f16 on bf16 copies (bf16(A), bf16(B_lo), bf16(A_lo), bf16(B)) at twice the tf32 rate, into
+    // the same f32 accumulators.  The cross terms are ~2^-11 of the product, so their bf16 rounding (2^-9) lands at ~2^-20 of it.
     // 3xTF32 in ONE GEMM launch: the tf32 datapath reads only the top 19 bits of an f32 operand, so the original tensors
     // are the "hi" parts; only lo = x - hi is materialised (compact), and the kernel runs K three times:
     // (A,B) + (A,B_lo) + (A_lo,B), f32 accumulation throughout.
+    // Either way one low-part buffer per operand, 4 bytes per element: two bf16 planes (hybrid) or one f32 plane (3xTF32).
+    const bool hybrid = f32_mode == "hybrid";
+    const char* kernel = hybrid ? "split_f32_bf16_pair" : "split_tf32_lo";
+    const uint64_t vec = hybrid ? 8 : 4;
+    auto pad = [&](uint64_t elems) { return (elems + vec - 1) / vec * vec; };
     const uint64_t ab = (g.a_sb == 0) ? 1 : g.batch, bb = (g.b_sb == 0) ? 1 : g.batch;
-    const uint64_t a_elems = !a_mn ? g.M * pad4(g.K) : g.K * pad4(g.M), b_elems = !b_mn ? g.N * pad4(g.K) : g.K * pad4(g.N);
+    const uint64_t a_elems = !a_mn ? g.M * pad(g.K) : g.K * pad(g.M), b_elems = !b_mn ? g.N * pad(g.K) : g.K * pad(g.N);
+    Scratch scr(c, st);
     CUdeviceptr a_lo = 0, b_lo = 0;
-    int rc = pool_alloc(c, ab * a_elems * 4, &a_lo, st);
+    int rc = scr.alloc(ab * a_elems * 4, &a_lo);
+    if (!rc) rc = scr.alloc(bb * b_elems * 4, &b_lo);
+    if (!rc) rc = !a_mn ? launch_split(c, st, kernel, vec, g.a, a_lo, ab, g.M, g.K, g.a_sb, g.a_sm)
+                        : launch_split(c, st, kernel, vec, g.a, a_lo, ab, g.K, g.M, g.a_sb, g.a_sk);
+    if (!rc) rc = !b_mn ? launch_split(c, st, kernel, vec, g.b, b_lo, bb, g.N, g.K, g.b_sb, g.b_sn)
+                        : launch_split(c, st, kernel, vec, g.b, b_lo, bb, g.K, g.N, g.b_sb, g.b_sk);
     if (rc) return rc;
-    rc = pool_alloc(c, bb * b_elems * 4, &b_lo, st);
-    if (rc) { pool_free(c, a_lo, st); return rc; }
-    rc = !a_mn ? launch_split(c, st, g.a, a_lo, ab, g.M, g.K, g.a_sb, g.a_sm) : launch_split(c, st, g.a, a_lo, ab, g.K, g.M, g.a_sb, g.a_sk);
-    if (!rc) rc = !b_mn ? launch_split(c, st, g.b, b_lo, bb, g.N, g.K, g.b_sb, g.b_sn) : launch_split(c, st, g.b, b_lo, bb, g.K, g.N, g.b_sb, g.b_sk);
-    if (!rc) {
-      GemmProblem h = g;
-      h.a_lo = a_lo;
-      h.b_lo = b_lo;
-      rc = launch_wgmma(c, st, h, a_mn, b_mn);
-    }
-    // stream-ordered reuse: the pool hands these pages out again only to later work on this context
-    pool_free(c, a_lo, st);
-    pool_free(c, b_lo, st);
-    return rc;
+    GemmProblem h = g;
+    h.a_lo = a_lo;
+    h.b_lo = b_lo;
+    h.hybrid = hybrid;
+    return launch_wgmma(c, st, h, a_mn, b_mn);
   }
   return launch_wgmma(c, st, g, a_mn, b_mn);
 }
@@ -1625,24 +1604,20 @@ static int run_gemm(b200_ctx* c, CUstream st, const GemmProblem& g) {
 static int run_gemm_staged(b200_ctx* c, CUstream st, const GemmProblem& g) {
   const size_t esz = dtype_size(g.in_dtype);
   GemmProblem h = g;
+  Scratch scr(c, st);
   CUdeviceptr sa = 0, sb = 0;
   bool mn = false;
   int rc = B200_OK;
   if (!operand_tma_ok(g.a, esz, g.M, g.K, g.a_sm, g.a_sk, g.a_sb, &mn) || (mn && esz != 2)) {
-    rc = stage_operand(c, st, esz, g.a, g.batch, g.M, g.K, g.a_sm, g.a_sk, g.a_sb, &sa, &h.a_sm, &h.a_sk, &h.a_sb);
-    if (!rc) h.a = sa;
+    if ((rc = stage_operand(scr, esz, g.a, g.batch, g.M, g.K, g.a_sm, g.a_sk, g.a_sb, &sa, &h.a_sm, &h.a_sk, &h.a_sb))) return rc;
+    h.a = sa;
   }
-  if (!rc && (!operand_tma_ok(g.b, esz, g.N, g.K, g.b_sn, g.b_sk, g.b_sb, &mn) || (mn && esz != 2))) {
-    rc = stage_operand(c, st, esz, g.b, g.batch, g.N, g.K, g.b_sn, g.b_sk, g.b_sb, &sb, &h.b_sn, &h.b_sk, &h.b_sb);
-    if (!rc) h.b = sb;
+  if (!operand_tma_ok(g.b, esz, g.N, g.K, g.b_sn, g.b_sk, g.b_sb, &mn) || (mn && esz != 2)) {
+    if ((rc = stage_operand(scr, esz, g.b, g.batch, g.N, g.K, g.b_sn, g.b_sk, g.b_sb, &sb, &h.b_sn, &h.b_sk, &h.b_sb))) return rc;
+    h.b = sb;
   }
-  if (!rc) {
-    bool a_mn = false, b_mn = false;
-    rc = tma_ok(h, &a_mn, &b_mn) ? run_gemm(c, st, h) : launch_simt(c, st, g);
-  }
-  if (sa) pool_free(c, sa, st);
-  if (sb) pool_free(c, sb, st);
-  return rc;
+  bool a_mn = false, b_mn = false;
+  return tma_ok(h, &a_mn, &b_mn) ? run_gemm(c, st, h) : launch_simt(c, st, g);
 }
 
 // Collapse batch dims [0, nb) of one operand into a linear stride; false if the offsets are not linear in the flat index.
@@ -1710,6 +1685,17 @@ extern "C" int b200_matmul_fused(b200_ctx* c, b200_stream s, b200_dtype in_dtype
 }
 
 // ------------------------------------------------------------------------------------------------ block-scaled matmul
+// The operand and output layout of a compact K-major problem: a [batch, M, pitch_a], b [batch, N, pitch_b] (K valid elements
+// per row) and out [batch, M, N]; one batch has zero batch strides.
+static void compact_kk_layout(GemmProblem* g, uint64_t a, uint64_t pitch_a, uint64_t b, uint64_t pitch_b, uint64_t out, uint64_t batch,
+                              uint64_t M, uint64_t N, uint64_t K) {
+  g->a = a; g->b = b; g->out = out;
+  g->M = M; g->N = N; g->K = K; g->batch = batch;
+  g->a_sm = pitch_a; g->a_sk = 1; g->a_sb = batch > 1 ? M * pitch_a : 0;
+  g->b_sn = pitch_b; g->b_sk = 1; g->b_sb = batch > 1 ? N * pitch_b : 0;
+  g->o_sm = N; g->o_sn = 1; g->o_sb = batch > 1 ? M * N : 0;
+}
+
 extern "C" int b200_matmul_scaled(b200_ctx* c, b200_stream s, b200_dtype lhs_dtype, b200_dtype rhs_dtype, b200_dtype out_dtype,
                                   b200_dptr lhs, b200_dptr rhs, b200_dptr lhs_scales, b200_dptr rhs_scales, b200_dptr out,
                                   uint64_t batch, uint64_t M, uint64_t N, uint64_t K, int scale_block, int scales_packed) {
@@ -1750,11 +1736,11 @@ extern "C" int b200_matmul_scaled(b200_ctx* c, b200_stream s, b200_dtype lhs_dty
   // Hopper's tensor cores take no scale factors: each operand is expanded once to bf16 x * scale (exact, see
   // dequant_scaled_bf16) and the bf16 wgmma GEMM accumulates the products in f32
   const uint64_t ab = batch * M, bb = batch * N;
+  Scratch scr(c, st);
   CUdeviceptr da = 0, db = 0;
-  int rc = pool_alloc(c, ab * K * 2, &da, st);
+  int rc = scr.alloc(ab * K * 2, &da);
+  if (!rc) rc = scr.alloc(bb * K * 2, &db);
   if (rc) return rc;
-  rc = pool_alloc(c, bb * K * 2, &db, st);
-  if (rc) { pool_free(c, da, st); return rc; }
   auto dequant = [&](uint64_t in, uint64_t scales, CUdeviceptr out_bf16, uint64_t rows, int dtype) {
     CUfunction f;
     int r = get_func(c, "dequant_scaled_bf16", &f);
@@ -1766,23 +1752,13 @@ extern "C" int b200_matmul_scaled(b200_ctx* c, b200_stream s, b200_dtype lhs_dty
     void* args[] = {&p};
     return launch(c, f, std::max(1u, grid), 1, 1, 256, 0, 1, st, args);
   };
-  rc = dequant(lhs, lhs_scales, da, M, lhs_dtype);
-  if (!rc) rc = dequant(rhs, rhs_scales, db, N, rhs_dtype);
-  if (!rc) {
-    GemmProblem g{};
-    g.in_dtype = B200_BF16;
-    g.out_dtype = out_dtype;
-    g.a = da; g.b = db; g.out = out;
-    g.M = M; g.N = N; g.K = K; g.batch = batch;
-    g.a_sm = K; g.a_sk = 1; g.a_sb = batch > 1 ? M * K : 0;
-    g.b_sn = K; g.b_sk = 1; g.b_sb = batch > 1 ? N * K : 0;
-    g.o_sm = N; g.o_sn = 1; g.o_sb = batch > 1 ? M * N : 0;
-    g.mx = true;
-    rc = launch_wgmma(c, st, g, false, false);
-  }
-  pool_free(c, da, st);
-  pool_free(c, db, st);
-  return rc;
+  if ((rc = dequant(lhs, lhs_scales, da, M, lhs_dtype)) || (rc = dequant(rhs, rhs_scales, db, N, rhs_dtype))) return rc;
+  GemmProblem g{};
+  g.in_dtype = B200_BF16;
+  g.out_dtype = out_dtype;
+  g.mx = true;
+  compact_kk_layout(&g, da, K, db, K, out, batch, M, N, K);
+  return launch_wgmma(c, st, g, false, false);
 }
 
 // Mixed 8-bit operand formats (the cartesian products the reference instantiates for its manual MMA,
@@ -2011,44 +1987,28 @@ extern "C" int b200_matmul_grouped(b200_ctx* c, b200_stream s, b200_dtype in_dty
     a_mn = b_mn = true;
   }
   CUstream st = resolve_stream(c, s);
-  CUdeviceptr sa = 0, sb = 0;
-  auto release = [&](int rc) {
-    if (sa) pool_free(c, sa, st);
-    if (sb) pool_free(c, sb, st);
-    return rc;
+  Scratch scr(c, st);
+  // one operand, read in place when TMA can describe it (ragged M: K-major or MN-major; ragged K: MN-major), else staged once
+  auto place = [&](uint64_t* ptr, uint64_t batch, uint64_t mn, uint64_t k, uint64_t* s_mn, uint64_t* s_k, uint64_t* s_b, bool* is_mn,
+                   const char* refusal) {
+    auto ok = [&] { return rk ? mn_major_tma_ok(*ptr, esz, mn, k, *s_mn, *s_k) : operand_tma_ok(*ptr, esz, mn, k, *s_mn, *s_k, *s_b, is_mn); };
+    if (ok()) return (int)B200_OK;
+    CUdeviceptr staged;
+    const int rc = stage_operand(scr, esz, *ptr, batch, mn, k, rk ? 1 : *s_mn, *s_k, *s_b, &staged, s_mn, s_k, s_b);
+    if (rc) return rc;
+    *ptr = staged;
+    return ok() ? (int)B200_OK : fail(B200_ERR_UNSUPPORTED, "matmul_grouped: %s", refusal);
   };
   int rc = B200_OK;
   if (reads) {
-    uint64_t o_sb_unused = 0;
-    if (!rk) {
-      if (!operand_tma_ok(a, esz, T, K, a_mn_s, a_k_s, 0, &a_mn)) {
-        if ((rc = stage_operand(c, st, esz, a, 1, T, K, a_mn_s, a_k_s, 0, &sa, &a_mn_s, &a_k_s, &o_sb_unused))) return release(rc);
-        a = sa;
-        if (!operand_tma_ok(a, esz, T, K, a_mn_s, a_k_s, 0, &a_mn)) return release(fail(B200_ERR_UNSUPPORTED, "matmul_grouped: lhs cannot be staged"));
-      }
-      if (!operand_tma_ok(b, esz, N, K, b_mn_s, b_k_s, b_sb, &b_mn)) {
-        if ((rc = stage_operand(c, st, esz, b, groups, N, K, b_mn_s, b_k_s, b_sb, &sb, &b_mn_s, &b_k_s, &b_sb))) return release(rc);
-        b = sb;
-        if (!operand_tma_ok(b, esz, N, K, b_mn_s, b_k_s, b_sb, &b_mn)) return release(fail(B200_ERR_UNSUPPORTED, "matmul_grouped: rhs cannot be staged"));
-      }
-    } else {
-      if (!mn_major_tma_ok(a, esz, M, T, a_mn_s, a_k_s)) {
-        if ((rc = stage_operand(c, st, esz, a, 1, M, T, 1, a_k_s, 0, &sa, &a_mn_s, &a_k_s, &o_sb_unused))) return release(rc);
-        a = sa;
-        if (!mn_major_tma_ok(a, esz, M, T, a_mn_s, a_k_s))
-          return release(fail(B200_ERR_UNSUPPORTED, "matmul_grouped: lhs cannot be staged M-contiguous"));
-      }
-      if (!mn_major_tma_ok(b, esz, N, T, b_mn_s, b_k_s)) {
-        if ((rc = stage_operand(c, st, esz, b, 1, N, T, 1, b_k_s, 0, &sb, &b_mn_s, &b_k_s, &o_sb_unused))) return release(rc);
-        b = sb;
-        if (!mn_major_tma_ok(b, esz, N, T, b_mn_s, b_k_s))
-          return release(fail(B200_ERR_UNSUPPORTED, "matmul_grouped: rhs cannot be staged N-contiguous"));
-      }
-    }
+    uint64_t a_sb = 0;
+    if ((rc = place(&a, 1, M, K, &a_mn_s, &a_k_s, &a_sb, &a_mn, rk ? "lhs cannot be staged M-contiguous" : "lhs cannot be staged")) ||
+        (rc = place(&b, rk ? 1 : groups, N, K, &b_mn_s, &b_k_s, &b_sb, &b_mn, rk ? "rhs cannot be staged N-contiguous" : "rhs cannot be staged")))
+      return rc;
   }
 
   GroupedPlan pl;
-  if ((rc = grouped_plan(c, "matmul_grouped", rk, a_mn && !rk ? 63 : 0, groups, T, M, N, &pl))) return release(rc);
+  if ((rc = grouped_plan(c, "matmul_grouped", rk, a_mn && !rk ? 63 : 0, groups, T, M, N, &pl))) return rc;
   const GemmVariant& v = *pl.v;
   const char* in_tag = in_dtype == B200_BF16 ? "bf16" : "f16";
   const char* out_tag = out_dtype == B200_F32 ? "f32" : in_tag;
@@ -2056,7 +2016,7 @@ extern "C" int b200_matmul_grouped(b200_ctx* c, b200_stream s, b200_dtype in_dty
                            (rk ? "" : std::string("_") + (a_mn ? "m" : "k") + (b_mn ? "n" : "k"));
   const unsigned smem = gemm_smem_bytes(v) + kGroupedTableBytes;
   CUfunction f;
-  if ((rc = gemm_kernel(c, name, smem, &f))) return release(rc);
+  if ((rc = gemm_kernel(c, name, smem, &f))) return rc;
 
   // ragged M: lhs [T, K] and rhs [G, K, N] with the group as the batch; ragged K: lhs [M, T] and rhs [T, N], both MN-major
   const CUtensorMapDataType dt = in_dtype == B200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
@@ -2067,13 +2027,12 @@ extern "C" int b200_matmul_grouped(b200_ctx* c, b200_stream s, b200_dtype in_dty
     rc = encode_operand(c, &ta, dt, esz, a, M, K, 1, a_mn_s, a_k_s, 0, a_mn, 128);
     if (!rc) rc = encode_operand(c, &tb, dt, esz, b, N, K, rk ? 1 : groups, b_mn_s, b_k_s, b_sb, b_mn, (uint32_t)(v.block_n / v.cg));
   }
-  if (rc) return release(rc);
+  if (rc) return rc;
 
   GemmParams p;
   gemm_params(c, &p, v, osz, out, o_sm, o_sb, M, N, K, rk ? groups : 1, rk ? pl.tiles_m : pl.tile_rows, ep);
   p.b_bmul = (!rk && b_sb != 0 && groups > 1) ? 1u : 0u;
-  rc = grouped_launch(c, st, f, pl, smem, osz, offs, groups, T, rk, &p, {&ta, &tb});
-  return release(rc);   // stream-ordered: staged copies are reused only by later work
+  return grouped_launch(c, st, f, pl, smem, osz, offs, groups, T, rk, &p, {&ta, &tb});
 }
 
 // ================================================================================================ reduce
@@ -2320,13 +2279,11 @@ static int reduce_axis_view(b200_ctx* c, CUstream st, int op, int dt, const RVie
   }
   // two passes: partials [outer, nseg, inner] (f32 values, or u32 keys + u32 indices), then the partials
   const uint64_t count = v.outer * nseg * v.inner;
+  Scratch scr(c, st);
   CUdeviceptr tmp = 0, tmp2 = 0;
-  int rc = pool_alloc(c, count * 4, &tmp, st);
+  int rc = scr.alloc(count * 4, &tmp);
+  if (!rc && arg) rc = scr.alloc(count * 4, &tmp2);
   if (rc) return rc;
-  if (arg) {
-    rc = pool_alloc(c, count * 4, &tmp2, st);
-    if (rc) { pool_free(c, tmp, st); return rc; }
-  }
   bool fused = false;
   rc = v.inner == 1 ? launch_rows_kernel(c, st, op, dt, v, seg_len, tmp, tmp2, 1.0f)
                     : launch_cols_kernel(c, st, op, dt, v, seg_len, tmp, tmp2, scale, out, &fused);
@@ -2344,8 +2301,6 @@ static int reduce_axis_view(b200_ctx* c, CUstream st, int op, int dt, const RVie
                         : launch_cols_kernel(c, st, op, B200_F32, t, nseg, out, 0, scale, 0, nullptr, pdl);
     }
   }
-  pool_free(c, tmp, st);
-  if (tmp2) pool_free(c, tmp2, st);
   return rc;
 }
 
@@ -2437,18 +2392,14 @@ static int reduce_impl(b200_ctx* c, b200_stream s, b200_reduce_op op, b200_dtype
     return reduce_axis_view(c, st, op, in_dtype, v, out, scale);
   }
   // not reducible in place: gather into a compact temporary first (into_contiguous), then reduce that
+  Scratch scr(c, st);
   CUdeviceptr tmp;
-  int rc = pool_alloc(c, n * dtype_size(in_dtype), &tmp, st);
+  int rc = scr.alloc(n * dtype_size(in_dtype), &tmp);
+  if (!rc) rc = b200_into_contiguous(c, s, in_dtype, in, tmp, rank, shape, strides);
   if (rc) return rc;
-  rc = b200_into_contiguous(c, s, in_dtype, in, tmp, rank, shape, strides);
-  if (!rc) {
-    RView w;
-    const bool ok = plan_view(rank, shape, nullptr, axis, arg, tmp, &w);
-    rc = !ok ? fail(B200_ERR_UNKNOWN, "reduce: contiguous plan failed")
-             : axis < 0 ? launch_reduce_all(c, st, op, in_dtype, w, out, scale) : reduce_axis_view(c, st, op, in_dtype, w, out, scale);
-  }
-  pool_free(c, tmp, st);
-  return rc;
+  RView w;
+  if (!plan_view(rank, shape, nullptr, axis, arg, tmp, &w)) return fail(B200_ERR_UNKNOWN, "reduce: contiguous plan failed");
+  return axis < 0 ? launch_reduce_all(c, st, op, in_dtype, w, out, scale) : reduce_axis_view(c, st, op, in_dtype, w, out, scale);
 }
 
 extern "C" int b200_reduce(b200_ctx* c, b200_stream s, b200_reduce_op op, b200_dtype in_dtype, b200_dptr in, b200_dptr out,
@@ -2558,11 +2509,11 @@ static int scan_axis_view(b200_ctx* c, CUstream st, int op, int dt, int odt, con
   const uint64_t nseg = ceil_div(v.len, seg_len);
   if (nseg == 1) return launch_scan(c, st, op, dt, odt, v, v.len, out, 0, exclusive, false);
   const uint64_t count = v.outer * nseg * v.inner;
+  Scratch scr(c, st);
   CUdeviceptr partials = 0, carries = 0;
-  int rc = pool_alloc(c, count * 4, &partials, st);
+  int rc = scr.alloc(count * 4, &partials);
+  if (!rc) rc = scr.alloc(count * 4, &carries);
   if (rc) return rc;
-  rc = pool_alloc(c, count * 4, &carries, st);
-  if (rc) { pool_free(c, partials, st); return rc; }
   rc = v.inner == 1 ? launch_rows_kernel(c, st, op, dt, v, seg_len, partials, 0, 1.0f)
                     : launch_cols_kernel(c, st, op, dt, v, seg_len, partials, 0, 1.0f);
   if (!rc) {
@@ -2572,8 +2523,6 @@ static int scan_axis_view(b200_ctx* c, CUstream st, int op, int dt, int odt, con
     rc = launch_scan(c, st, op, B200_F32, B200_F32, t, nseg, carries, 0, true, true);
   }
   if (!rc) rc = launch_scan(c, st, op, dt, odt, v, seg_len, out, carries, exclusive, true);
-  pool_free(c, partials, st);
-  pool_free(c, carries, st);
   return rc;
 }
 
@@ -2608,17 +2557,14 @@ static int scan_impl(b200_ctx* c, b200_stream s, b200_reduce_op op, int exclusiv
   RView v;
   if (in_order && plan_view(rank, shape, strides, axis, false, in, &v)) return scan_axis_view(c, st, op, in_dtype, out_dtype, v, out, exclusive != 0);
   // any other view: gather into a compact temporary first (into_contiguous), then scan that
+  Scratch scr(c, st);
   CUdeviceptr tmp;
-  int rc = pool_alloc(c, n * dtype_size(in_dtype), &tmp, st);
+  int rc = scr.alloc(n * dtype_size(in_dtype), &tmp);
+  if (!rc) rc = b200_into_contiguous(c, s, in_dtype, in, tmp, rank, shape, strides);
   if (rc) return rc;
-  rc = b200_into_contiguous(c, s, in_dtype, in, tmp, rank, shape, strides);
-  if (!rc) {
-    RView w;
-    rc = !plan_view(rank, shape, nullptr, axis, false, tmp, &w) ? fail(B200_ERR_UNKNOWN, "scan: contiguous plan failed")
-                                                                : scan_axis_view(c, st, op, in_dtype, out_dtype, w, out, exclusive != 0);
-  }
-  pool_free(c, tmp, st);
-  return rc;
+  RView w;
+  if (!plan_view(rank, shape, nullptr, axis, false, tmp, &w)) return fail(B200_ERR_UNKNOWN, "scan: contiguous plan failed");
+  return scan_axis_view(c, st, op, in_dtype, out_dtype, w, out, exclusive != 0);
 }
 
 extern "C" int b200_scan(b200_ctx* c, b200_stream s, b200_reduce_op op, int exclusive, b200_dtype in_dtype, b200_dtype out_dtype,
@@ -2749,13 +2695,14 @@ static int quant_impl(b200_ctx* c, b200_stream s, const b200_quant_scheme* q, b2
   p.values = values; p.block_scales = block_scales; p.tensor_scale = tensor_scale;
   p.value = (uint32_t)q->value; p.block = (uint32_t)q->block; p.scale_dt = q->block > 0 ? (uint32_t)q->block_scale : B200_F32;
   p.block_log2 = log2_u32(p.block);
+  Scratch scr(c, st);
   CUdeviceptr tmp = 0, amax = 0;
   uint64_t rows, pitch;
   if (quant_rows_view(rank, shape, strides, n, esz, q->block == 0, in, &rows, &K, &pitch)) {
     p.in = in;
   } else {
     // any other view (or an unaligned base / row): gather into a compact pooled temporary first
-    rc = pool_alloc(c, n * esz, &tmp, st);
+    rc = scr.alloc(n * esz, &tmp);
     if (rc) return rc;
     std::vector<uint64_t> cs(rank);
     uint64_t acc = 1;
@@ -2768,7 +2715,7 @@ static int quant_impl(b200_ctx* c, b200_stream s, const b200_quant_scheme* q, b2
   const uint64_t vec = 16 / esz, chunks = rows * ((K + vec - 1) / vec);
   if (!rc && q->tensor_scale) {
     // the tensor level first: the finite |x| max of the whole tensor, atomicMax'ed as u32 bits into a pooled word
-    rc = pool_alloc(c, 4, &amax, st);
+    rc = scr.alloc(4, &amax);
     if (!rc) rc = memset32_async(c, st, amax, 0, 1);
     CUfunction f;
     if (!rc) rc = get_func(c, std::string("quant_absmax_") + dt_tag(in_dtype), &f);
@@ -2790,8 +2737,6 @@ static int quant_impl(b200_ctx* c, b200_stream s, const b200_quant_scheme* q, b2
       if (!rc) rc = launch(c, f, (unsigned)grid, 1, 1, kQuantThreads, 0, 1, st, args);
     }
   }
-  if (amax) pool_free(c, amax, st);
-  if (tmp) pool_free(c, tmp, st);
   return rc;
 }
 
@@ -2840,127 +2785,131 @@ static const char* quant_scale_tag(int32_t dt) {
   }
 }
 
-// The codes of one operand as s8 rows TMA can read: Q8 codes in place (16-byte aligned base, K % 16 == 0) or through the
-// staging pass; Q4 / Q2 codes widened exactly to one s8 per element.  *tmp is the pooled buffer, if any.
-static int qmm_codes(b200_ctx* c, CUstream st, const b200_quant_operand* o, uint64_t batch, uint64_t rows, uint64_t K,
-                     CUdeviceptr* tmp, uint64_t* ptr, uint64_t* pitch) {
+// The codes of one operand as s8 rows TMA can read: Q8 (and fp8) codes in place (16-byte aligned base, K % 16 == 0) or
+// through the staging pass; Q4 / Q2 codes widened exactly to one s8 per element.
+static int qmm_codes(Scratch& scr, const b200_quant_operand* o, uint64_t batch, uint64_t rows, uint64_t K, uint64_t* ptr, uint64_t* pitch) {
   const uint32_t bits = quant_bits(o->scheme.value);
+  CUdeviceptr buf = 0;
   if (bits == 8) {
     if (o->values % 16 == 0 && K % 16 == 0) { *ptr = o->values; *pitch = K; return B200_OK; }
-    uint64_t s_mn, s_k, s_b;
-    int rc = stage_operand(c, st, 1, o->values, batch, rows, K, K, 1, rows * K, tmp, &s_mn, &s_k, &s_b);
-    *ptr = *tmp; *pitch = s_mn;
+    uint64_t s_mn = 0, s_k, s_b;
+    int rc = stage_operand(scr, 1, o->values, batch, rows, K, K, 1, rows * K, &buf, &s_mn, &s_k, &s_b);
+    *ptr = buf; *pitch = s_mn;
     return rc;
   }
   const uint64_t total_rows = batch * rows, pch = (K + 15) / 16 * 16;
-  int rc = pool_alloc(c, total_rows * pch, tmp, st);
-  if (rc) return rc;
   CUfunction f;
-  rc = get_func(c, "quant_widen_s8", &f);
+  int rc = scr.alloc(total_rows * pch, &buf);
+  if (!rc) rc = get_func(scr.c, "quant_widen_s8", &f);
   if (rc) return rc;
-  QuantWidenParams p{o->values, *tmp, total_rows, K, pch, bits, 0};
+  QuantWidenParams p{o->values, buf, total_rows, K, pch, bits, 0};
   const uint64_t vecs = total_rows * (pch / 16);
-  const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(ceil_div(vecs, (uint64_t)kQuantThreads), (uint64_t)c->props.num_sms * 16));
+  const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(ceil_div(vecs, (uint64_t)kQuantThreads), (uint64_t)scr.c->props.num_sms * 16));
   void* args[] = {&p};
-  *ptr = *tmp; *pitch = pch;
-  return launch(c, f, grid, 1, 1, kQuantThreads, 0, 1, st, args);
+  *ptr = buf; *pitch = pch;
+  return launch(scr.c, f, grid, 1, 1, kQuantThreads, 0, 1, scr.st, args);
 }
 
 // The f32 effective scales of one operand per GEMM block of bk elements, block-major [batch][ceil(K / bk)][rows padded to 4]
 // (a short last block only for per-tensor scales: a block level divides K).
-static int qmm_scales(b200_ctx* c, CUstream st, const b200_quant_operand* o, uint64_t batch, uint64_t rows, uint64_t K, uint32_t bk,
-                      CUdeviceptr* out) {
+static int qmm_scales(Scratch& scr, const b200_quant_operand* o, uint64_t batch, uint64_t rows, uint64_t K, uint32_t bk, uint64_t* out) {
   const uint64_t rows_pad = (rows + 3) / 4 * 4, nblk = (K + bk - 1) / bk, total = batch * nblk * rows_pad;
-  int rc = pool_alloc(c, total * 4, out, st);
-  if (rc) return rc;
   const int32_t block = o->scheme.block;
+  CUdeviceptr buf;
   CUfunction f;
-  rc = get_func(c, std::string("quant_scales_f32_") + (block ? quant_scale_tag(o->scheme.block_scale) : "tensor"), &f);
+  int rc = scr.alloc(total * 4, &buf);
   if (rc) return rc;
-  QuantScalesParams p{block ? o->block_scales : 0, o->tensor_scale, *out, batch, rows, rows_pad, nblk, block ? (uint32_t)block / bk : 1u, 0};
-  const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(ceil_div(total, (uint64_t)kQuantThreads), (uint64_t)c->props.num_sms * 16));
+  *out = buf;
+  if ((rc = get_func(scr.c, std::string("quant_scales_f32_") + (block ? quant_scale_tag(o->scheme.block_scale) : "tensor"), &f))) return rc;
+  QuantScalesParams p{block ? o->block_scales : 0, o->tensor_scale, buf, batch, rows, rows_pad, nblk, block ? (uint32_t)block / bk : 1u, 0};
+  const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(ceil_div(total, (uint64_t)kQuantThreads), (uint64_t)scr.c->props.num_sms * 16));
   void* args[] = {&p};
-  return launch(c, f, grid, 1, 1, kQuantThreads, 0, 1, st, args);
+  return launch(scr.c, f, grid, 1, 1, kQuantThreads, 0, 1, scr.st, args);
 }
 
-extern "C" int b200_matmul_quantized(b200_ctx* c, b200_stream s, const b200_quant_operand* lhs, const b200_quant_operand* rhs,
-                                     b200_dtype out_dtype, b200_dptr out, uint64_t batch, uint64_t m, uint64_t n, uint64_t k) {
-  CTX_ENTER(c);
-  if (!lhs || !rhs) return fail(B200_ERR_INVALID_ARG, "matmul_quantized: null operand");
-  const bool empty = (batch == 0 || m == 0 || n == 0);
-  const b200_quant_operand* ops[2] = {lhs, rhs};
-  const uint64_t rows[2] = {m, n};
-  for (int i = 0; i < 2; ++i) {
-    const char* what = i == 0 ? "matmul_quantized (lhs)" : "matmul_quantized (rhs)";
-    const uint64_t shape[2] = {empty ? 0 : batch * rows[i], k};
-    uint64_t nel = 0, K = 0;
-    int rc = quant_check(what, &ops[i]->scheme, 2, shape, ops[i]->block_scales, ops[i]->tensor_scale, &nel, &K);
-    if (rc) return rc;
-    const int32_t v = ops[i]->scheme.value;
-    if (v == B200_QV_E4M3 || v == B200_QV_E5M2 || v == B200_QV_E2M1)
-      return fail(B200_ERR_UNSUPPORTED, "%s: minifloat values (e4m3 / e5m2 / e2m1) with block scales run through b200_matmul_scaled", what);
-    if (ops[i]->scheme.block == 8 || ops[i]->scheme.block == 16)
-      return fail(B200_ERR_UNSUPPORTED, "%s: block %d (32, 64 or 128: s8 wgmma consumes K in steps of 32)", what, (int)ops[i]->scheme.block);
-  }
-  if (out_dtype != B200_F32 && out_dtype != B200_BF16 && out_dtype != B200_F16)
-    return fail(B200_ERR_INVALID_ARG, "matmul_quantized: output dtype %d is not F32, BF16 or F16", (int)out_dtype);
-  if (empty) return B200_OK;
-  if (k == 0) return fail(B200_ERR_INVALID_ARG, "matmul_quantized: K must be positive");
-  const bool per_tensor = lhs->scheme.block == 0 && rhs->scheme.block == 0;
-  // |q| <= 128 on either side: one product is at most 2^14, so the exact s32 dot product over K needs K * 2^14 < 2^31
-  if (per_tensor && k >= (1ull << 17))
-    return fail(B200_ERR_UNSUPPORTED, "matmul_quantized: per-tensor x per-tensor needs K < 131072 (exact s32 dot products), K = %llu",
-                (unsigned long long)k);
-  if (!out || !lhs->values || !rhs->values) return fail(B200_ERR_INVALID_ARG, "matmul_quantized: null device pointer");
-  const size_t osz = dtype_size(out_dtype);
-  if (out % osz) return fail(B200_ERR_INVALID_ARG, "matmul_quantized: output pointer is not aligned to its element size");
-  if (m >= (1ull << 31) || n >= (1ull << 31) || k >= (1ull << 31) || batch >= (1ull << 20))
-    return fail(B200_ERR_UNSUPPORTED, "matmul_quantized: extent too large");
-  CUstream st = resolve_stream(c, s);
-  CUdeviceptr tmp[4] = {0, 0, 0, 0};   // lhs codes, rhs codes, lhs scales, rhs scales
-  uint64_t pa = 0, pb = 0, pitch_a = 0, pitch_b = 0;
-  int rc = qmm_codes(c, st, lhs, batch, m, k, &tmp[0], &pa, &pitch_a);
-  if (!rc) rc = qmm_codes(c, st, rhs, batch, n, k, &tmp[1], &pb, &pitch_b);
-  GemmProblem g{};
-  g.in_dtype = B200_I8; g.out_dtype = out_dtype;
-  g.a = pa; g.b = pb; g.out = out;
-  g.M = m; g.N = n; g.K = k; g.batch = batch;
-  g.a_sm = pitch_a; g.a_sk = 1; g.a_sb = batch > 1 ? m * pitch_a : 0;
-  g.b_sn = pitch_b; g.b_sk = 1; g.b_sb = batch > 1 ? n * pitch_b : 0;
-  g.o_sm = n; g.o_sn = 1; g.o_sb = batch > 1 ? m * n : 0;
-  if (per_tensor) {
-    g.q = 2;
-    g.q_ga = lhs->tensor_scale; g.q_gb = rhs->tensor_scale;
-  } else {
-    // kernel block: the finer of the present block levels; a coarser block repeats its scale, a per-tensor side uses g
-    const int32_t ba = lhs->scheme.block, bb = rhs->scheme.block;
-    g.q = 1;
-    g.q_bk = (uint32_t)(ba == 0 ? bb : bb == 0 ? ba : std::min(ba, bb));
-    if (!rc) rc = qmm_scales(c, st, lhs, batch, m, k, g.q_bk, &tmp[2]);
-    if (!rc) rc = qmm_scales(c, st, rhs, batch, n, k, g.q_bk, &tmp[3]);
-    g.q_sa = tmp[2]; g.q_sb = tmp[3];
-  }
-  if (!rc) rc = launch_wgmma(c, st, g, false, false);
-  for (CUdeviceptr t : tmp)
-    if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMM has drained
+// Where the staged codes of a quantized pair are read: lhs [a_batch, m, pitch_a], rhs [b_batch, n, pitch_b].
+struct QmmCodes { uint64_t a = 0, pitch_a = 0, b = 0, pitch_b = 0; };
+
+// Stages a quantized pair into scr: both sides' codes, then -- with a kernel block g->q_bk -- both sides' effective scales,
+// whose pointers land in g->q_sa / g->q_sb.
+static int qmm_stage(Scratch& scr, const b200_quant_operand* lhs, const b200_quant_operand* rhs, uint64_t a_batch, uint64_t b_batch,
+                     uint64_t m, uint64_t n, uint64_t k, GemmProblem* g, QmmCodes* q) {
+  int rc = qmm_codes(scr, lhs, a_batch, m, k, &q->a, &q->pitch_a);
+  if (!rc) rc = qmm_codes(scr, rhs, b_batch, n, k, &q->b, &q->pitch_b);
+  if (!rc && g->q_bk) rc = qmm_scales(scr, lhs, a_batch, m, k, g->q_bk, &g->q_sa);
+  if (!rc && g->q_bk) rc = qmm_scales(scr, rhs, b_batch, n, k, g->q_bk, &g->q_sb);
   return rc;
 }
 
-// One operand of the fp8-quantized matmuls: `rows` x K codes as b200_quantize writes them (quant_check; rows = 0 for an empty
-// call checks the scheme alone), with e4m3 or e5m2 values and blocks of 32, 64 or 128 elements.
-static int qf8_operand_check(const char* what, const b200_quant_operand* o, uint64_t rows, uint64_t k) {
+// One operand of a quantized matmul: `rows` x K codes as b200_quantize writes them (quant_check; rows = 0 for an empty call
+// checks the scheme alone), with the family's values -- Q8 / Q4 / Q2 (int8) or e4m3 / e5m2 (fp8) -- and blocks of 32, 64 or
+// 128 elements.
+static int qmm_operand_check(const std::string& what, bool fp8, const b200_quant_operand* o, uint64_t rows, uint64_t k) {
   const uint64_t shape[2] = {rows, k};
   uint64_t nel = 0, K = 0;
-  const int rc = quant_check(what, &o->scheme, 2, shape, o->block_scales, o->tensor_scale, &nel, &K);
+  const int rc = quant_check(what.c_str(), &o->scheme, 2, shape, o->block_scales, o->tensor_scale, &nel, &K);
   if (rc) return rc;
   const int32_t v = o->scheme.value;
-  if (v == B200_QV_E2M1)
-    return fail(B200_ERR_UNSUPPORTED, "%s: e2m1 values with block scales run through b200_matmul_scaled", what);
-  if (v != B200_QV_E4M3 && v != B200_QV_E5M2)
-    return fail(B200_ERR_UNSUPPORTED, "%s: integer values run through b200_matmul_quantized", what);
+  const bool minifloat = (v == B200_QV_E4M3 || v == B200_QV_E5M2 || v == B200_QV_E2M1);
+  if (!fp8 && minifloat)
+    return fail(B200_ERR_UNSUPPORTED, "%s: minifloat values (e4m3 / e5m2 / e2m1) with block scales run through b200_matmul_scaled", what.c_str());
+  if (fp8 && v == B200_QV_E2M1)
+    return fail(B200_ERR_UNSUPPORTED, "%s: e2m1 values with block scales run through b200_matmul_scaled", what.c_str());
+  if (fp8 && !minifloat) return fail(B200_ERR_UNSUPPORTED, "%s: integer values run through b200_matmul_quantized", what.c_str());
   if (o->scheme.block == 8 || o->scheme.block == 16)
-    return fail(B200_ERR_UNSUPPORTED, "%s: block %d (32, 64 or 128: fp8 wgmma consumes K in steps of 32)", what, (int)o->scheme.block);
+    return fail(B200_ERR_UNSUPPORTED, "%s: block %d (32, 64 or 128: %s wgmma consumes K in steps of 32)", what.c_str(), (int)o->scheme.block,
+                fp8 ? "fp8" : "s8");
   return B200_OK;
+}
+
+// The checks of a quantized matmul of the int8 or the fp8 family.  Dense: lhs codes [batch, m, k] x rhs codes [batch, n, k]
+// -> out [batch, m, n].  Grouped: lhs [m = T, k] x rhs [batch = G, n, k] -> out [T, n] with the i32 group offsets `offs`.
+// *empty is set when the call writes nothing (B200_OK).  The entry points' orders differ, and each is kept: the int8 family
+// bounds per-tensor K before the pointers; a grouped call bounds its groups and extents first and checks offs before the
+// pointers.
+static int qmm_check(const char* what, bool fp8, bool grouped, b200_dptr offs, const b200_quant_operand* lhs, const b200_quant_operand* rhs,
+                     b200_dtype out_dtype, b200_dptr out, uint64_t batch, uint64_t m, uint64_t n, uint64_t k, bool* empty) {
+  typedef unsigned long long ull;
+  if (!lhs || !rhs) return fail(B200_ERR_INVALID_ARG, "%s: null operand", what);
+  if (grouped && batch > (uint64_t)kGroupedMaxGroups)
+    return fail(B200_ERR_UNSUPPORTED, "%s: %llu groups exceed the limit of %d", what, (ull)batch, kGroupedMaxGroups);
+  if (grouped && (m >= (1ull << 31) || n >= (1ull << 31) || k >= (1ull << 31)))
+    return fail(B200_ERR_UNSUPPORTED, "%s: extents must be below 2^31", what);
+  *empty = (batch == 0 || m == 0 || n == 0);   // grouped: no row lies in a group
+  int rc = qmm_operand_check(std::string(what) + " (lhs)", fp8, lhs, *empty ? 0 : grouped ? m : batch * m, k);
+  if (!rc) rc = qmm_operand_check(std::string(what) + " (rhs)", fp8, rhs, *empty ? 0 : batch * n, k);
+  if (rc) return rc;
+  if (out_dtype != B200_F32 && out_dtype != B200_BF16 && out_dtype != B200_F16)
+    return fail(B200_ERR_INVALID_ARG, "%s: output dtype %d is not F32, BF16 or F16", what, (int)out_dtype);
+  if (*empty) return B200_OK;
+  if (k == 0) return fail(B200_ERR_INVALID_ARG, "%s: K must be positive", what);
+  // |q| <= 128 on either side: one product is at most 2^14, so the exact s32 dot product over K needs K * 2^14 < 2^31
+  if (!fp8 && lhs->scheme.block == 0 && rhs->scheme.block == 0 && k >= (1ull << 17))
+    return fail(B200_ERR_UNSUPPORTED, "%s: per-tensor x per-tensor needs K < 131072 (exact s32 dot products), K = %llu", what, (ull)k);
+  if (grouped && !offs) return fail(B200_ERR_INVALID_ARG, "%s: null offs", what);
+  if (grouped && offs % 4) return fail(B200_ERR_INVALID_ARG, "%s: offs is misaligned (a compact i32 [groups] array)", what);
+  if (!out || !lhs->values || !rhs->values) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
+  if (out % dtype_size(out_dtype)) return fail(B200_ERR_INVALID_ARG, "%s: output pointer is not aligned to its element size", what);
+  if (!grouped && (m >= (1ull << 31) || n >= (1ull << 31) || k >= (1ull << 31) || batch >= (1ull << 20)))
+    return fail(B200_ERR_UNSUPPORTED, "%s: extent too large", what);
+  return B200_OK;
+}
+
+// The GEMM problem of int8 codes without its operand layout: two per-tensor sides fold their scales once (q = 2, gemm_q8t_*);
+// otherwise the fold is per block (q = 1, gemm_q8_*) with the kernel block the finer of the present block levels -- a coarser
+// block repeats its scale, a per-tensor side uses g.
+static GemmProblem q8_problem(const b200_quant_operand* lhs, const b200_quant_operand* rhs, b200_dtype out_dtype) {
+  GemmProblem g{};
+  g.in_dtype = B200_I8; g.out_dtype = out_dtype;
+  const int32_t ba = lhs->scheme.block, bb = rhs->scheme.block;
+  if (ba == 0 && bb == 0) {
+    g.q = 2;
+    g.q_ga = lhs->tensor_scale; g.q_gb = rhs->tensor_scale;
+  } else {
+    g.q = 1;
+    g.q_bk = (uint32_t)(ba == 0 ? bb : bb == 0 ? ba : std::min(ba, bb));
+  }
+  return g;
 }
 
 // The GEMM problem of the fp8 fold (q = 3) without its operand layout: the two formats and the kernel block -- the finer of
@@ -2976,43 +2925,32 @@ static GemmProblem qf8_problem(const b200_quant_operand* lhs, const b200_quant_o
   return g;
 }
 
-// fp8 codes (e4m3 / e5m2 on either side) on the fp8 tensor cores: Bk / 32 wgmma k32 steps per block into a fresh f32 partial,
-// folded as b200_matmul_quantized's per-block kernels fold their exact s32 partials (gemm_qf8_*, gemm_wgmma.cu: QM_FP8)
+// The dense quantized matmuls.  int8: Q8 / Q4 / Q2 codes on the s8 tensor cores with exact s32 partials.  fp8: e4m3 / e5m2
+// codes on either side on the fp8 tensor cores, Bk / 32 wgmma k32 steps per block into a fresh f32 partial, folded as the int8
+// per-block kernels fold their s32 partials (gemm_qf8_*, gemm_wgmma.cu: QM_FP8).
+static int matmul_quantized(b200_ctx* c, b200_stream s, bool fp8, const b200_quant_operand* lhs, const b200_quant_operand* rhs,
+                            b200_dtype out_dtype, b200_dptr out, uint64_t batch, uint64_t m, uint64_t n, uint64_t k) {
+  CTX_ENTER(c);
+  bool empty = false;
+  int rc = qmm_check(fp8 ? "matmul_quantized_fp8" : "matmul_quantized", fp8, false, 0, lhs, rhs, out_dtype, out, batch, m, n, k, &empty);
+  if (rc || empty) return rc;
+  CUstream st = resolve_stream(c, s);
+  GemmProblem g = fp8 ? qf8_problem(lhs, rhs, out_dtype) : q8_problem(lhs, rhs, out_dtype);
+  Scratch scr(c, st);
+  QmmCodes q;
+  if ((rc = qmm_stage(scr, lhs, rhs, batch, batch, m, n, k, &g, &q))) return rc;
+  compact_kk_layout(&g, q.a, q.pitch_a, q.b, q.pitch_b, out, batch, m, n, k);
+  return launch_wgmma(c, st, g, false, false);
+}
+
+extern "C" int b200_matmul_quantized(b200_ctx* c, b200_stream s, const b200_quant_operand* lhs, const b200_quant_operand* rhs,
+                                     b200_dtype out_dtype, b200_dptr out, uint64_t batch, uint64_t m, uint64_t n, uint64_t k) {
+  return matmul_quantized(c, s, false, lhs, rhs, out_dtype, out, batch, m, n, k);
+}
+
 extern "C" int b200_matmul_quantized_fp8(b200_ctx* c, b200_stream s, const b200_quant_operand* lhs, const b200_quant_operand* rhs,
                                          b200_dtype out_dtype, b200_dptr out, uint64_t batch, uint64_t m, uint64_t n, uint64_t k) {
-  CTX_ENTER(c);
-  if (!lhs || !rhs) return fail(B200_ERR_INVALID_ARG, "matmul_quantized_fp8: null operand");
-  const bool empty = (batch == 0 || m == 0 || n == 0);
-  int rc = qf8_operand_check("matmul_quantized_fp8 (lhs)", lhs, empty ? 0 : batch * m, k);
-  if (!rc) rc = qf8_operand_check("matmul_quantized_fp8 (rhs)", rhs, empty ? 0 : batch * n, k);
-  if (rc) return rc;
-  if (out_dtype != B200_F32 && out_dtype != B200_BF16 && out_dtype != B200_F16)
-    return fail(B200_ERR_INVALID_ARG, "matmul_quantized_fp8: output dtype %d is not F32, BF16 or F16", (int)out_dtype);
-  if (empty) return B200_OK;
-  if (k == 0) return fail(B200_ERR_INVALID_ARG, "matmul_quantized_fp8: K must be positive");
-  if (!out || !lhs->values || !rhs->values) return fail(B200_ERR_INVALID_ARG, "matmul_quantized_fp8: null device pointer");
-  const size_t osz = dtype_size(out_dtype);
-  if (out % osz) return fail(B200_ERR_INVALID_ARG, "matmul_quantized_fp8: output pointer is not aligned to its element size");
-  if (m >= (1ull << 31) || n >= (1ull << 31) || k >= (1ull << 31) || batch >= (1ull << 20))
-    return fail(B200_ERR_UNSUPPORTED, "matmul_quantized_fp8: extent too large");
-  CUstream st = resolve_stream(c, s);
-  CUdeviceptr tmp[4] = {0, 0, 0, 0};   // lhs codes, rhs codes, lhs scales, rhs scales
-  uint64_t pa = 0, pb = 0, pitch_a = 0, pitch_b = 0;
-  rc = qmm_codes(c, st, lhs, batch, m, k, &tmp[0], &pa, &pitch_a);
-  if (!rc) rc = qmm_codes(c, st, rhs, batch, n, k, &tmp[1], &pb, &pitch_b);
-  GemmProblem g = qf8_problem(lhs, rhs, out_dtype);
-  g.a = pa; g.b = pb; g.out = out;
-  g.M = m; g.N = n; g.K = k; g.batch = batch;
-  g.a_sm = pitch_a; g.a_sk = 1; g.a_sb = batch > 1 ? m * pitch_a : 0;
-  g.b_sn = pitch_b; g.b_sk = 1; g.b_sb = batch > 1 ? n * pitch_b : 0;
-  g.o_sm = n; g.o_sn = 1; g.o_sb = batch > 1 ? m * n : 0;
-  if (!rc) rc = qmm_scales(c, st, lhs, batch, m, k, g.q_bk, &tmp[2]);
-  if (!rc) rc = qmm_scales(c, st, rhs, batch, n, k, g.q_bk, &tmp[3]);
-  g.q_sa = tmp[2]; g.q_sb = tmp[3];
-  if (!rc) rc = launch_wgmma(c, st, g, false, false);
-  for (CUdeviceptr t : tmp)
-    if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMM has drained
-  return rc;
+  return matmul_quantized(c, s, true, lhs, rhs, out_dtype, out, batch, m, n, k);
 }
 
 // Grouped matmul of fp8-quantized operands (ragged M): lhs codes [T, K] against rhs codes [G, N, K], the fold of
@@ -3022,25 +2960,10 @@ extern "C" int b200_matmul_grouped_quantized_fp8(b200_ctx* c, b200_stream s, con
                                                  b200_dptr offs, uint64_t groups, b200_dtype out_dtype, b200_dptr out, uint64_t t,
                                                  uint64_t n, uint64_t k) {
   CTX_ENTER(c);
-  typedef unsigned long long ull;
-  if (!lhs || !rhs) return fail(B200_ERR_INVALID_ARG, "matmul_grouped_quantized_fp8: null operand");
-  if (groups > (uint64_t)kGroupedMaxGroups)
-    return fail(B200_ERR_UNSUPPORTED, "matmul_grouped_quantized_fp8: %llu groups exceed the limit of %d", (ull)groups, kGroupedMaxGroups);
-  if (t >= (1ull << 31) || n >= (1ull << 31) || k >= (1ull << 31))
-    return fail(B200_ERR_UNSUPPORTED, "matmul_grouped_quantized_fp8: extents must be below 2^31");
-  const bool empty = (groups == 0 || t == 0 || n == 0);   // nothing is written: no row lies in a group
-  int rc = qf8_operand_check("matmul_grouped_quantized_fp8 (lhs)", lhs, empty ? 0 : t, k);
-  if (!rc) rc = qf8_operand_check("matmul_grouped_quantized_fp8 (rhs)", rhs, empty ? 0 : groups * n, k);
-  if (rc) return rc;
-  if (out_dtype != B200_F32 && out_dtype != B200_BF16 && out_dtype != B200_F16)
-    return fail(B200_ERR_INVALID_ARG, "matmul_grouped_quantized_fp8: output dtype %d is not F32, BF16 or F16", (int)out_dtype);
-  if (empty) return B200_OK;
-  if (k == 0) return fail(B200_ERR_INVALID_ARG, "matmul_grouped_quantized_fp8: K must be positive");
-  if (!offs) return fail(B200_ERR_INVALID_ARG, "matmul_grouped_quantized_fp8: null offs");
-  if (offs % 4) return fail(B200_ERR_INVALID_ARG, "matmul_grouped_quantized_fp8: offs is misaligned (a compact i32 [groups] array)");
-  if (!out || !lhs->values || !rhs->values) return fail(B200_ERR_INVALID_ARG, "matmul_grouped_quantized_fp8: null device pointer");
+  bool empty = false;
+  int rc = qmm_check("matmul_grouped_quantized_fp8", true, true, offs, lhs, rhs, out_dtype, out, groups, t, n, k, &empty);
+  if (rc || empty) return rc;
   const size_t osz = dtype_size(out_dtype);
-  if (out % osz) return fail(B200_ERR_INVALID_ARG, "matmul_grouped_quantized_fp8: output pointer is not aligned to its element size");
   GroupedPlan pl;
   if ((rc = grouped_plan(c, "matmul_grouped_quantized_fp8", false, 3, groups, t, t, n, &pl))) return rc;
   const GemmVariant& v = *pl.v;
@@ -3050,27 +2973,20 @@ extern "C" int b200_matmul_grouped_quantized_fp8(b200_ctx* c, b200_stream s, con
                            (out_dtype == B200_BF16 ? "bf16" : out_dtype == B200_F16 ? "f16" : "f32") + "_" + v.tag + "_kk";
   const unsigned smem = gemm_q8_smem_bytes(v) + kGroupedTableBytes;
   CUstream st = resolve_stream(c, s);
-  CUdeviceptr tmp[4] = {0, 0, 0, 0};   // lhs codes, rhs codes, lhs scales, rhs scales
-  uint64_t pa = 0, pb = 0, pitch_a = 0, pitch_b = 0;
-  rc = qmm_codes(c, st, lhs, 1, t, k, &tmp[0], &pa, &pitch_a);
-  if (!rc) rc = qmm_codes(c, st, rhs, groups, n, k, &tmp[1], &pb, &pitch_b);
-  if (!rc) rc = qmm_scales(c, st, lhs, 1, t, k, g.q_bk, &tmp[2]);
-  if (!rc) rc = qmm_scales(c, st, rhs, groups, n, k, g.q_bk, &tmp[3]);
-  g.q_sa = tmp[2]; g.q_sb = tmp[3];
+  Scratch scr(c, st);
+  QmmCodes q;
   CUfunction f = nullptr;
-  if (!rc) rc = gemm_kernel(c, name, smem, &f);
   CUtensorMap ta, tb, ta_sc, tb_sc;
-  if (!rc) rc = encode_operand(c, &ta, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, pa, t, k, 1, pitch_a, 1, 0, false, 128);
-  if (!rc) rc = encode_operand(c, &tb, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, pb, n, k, groups, pitch_b, 1, n * pitch_b, false,
-                               (uint32_t)(v.block_n / v.cg));
+  if ((rc = qmm_stage(scr, lhs, rhs, 1, groups, t, n, k, &g, &q)) || (rc = gemm_kernel(c, name, smem, &f)) ||
+      (rc = encode_operand(c, &ta, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, q.a, t, k, 1, q.pitch_a, 1, 0, false, 128)) ||
+      (rc = encode_operand(c, &tb, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, q.b, n, k, groups, q.pitch_b, 1, n * q.pitch_b, false,
+                           (uint32_t)(v.block_n / v.cg))))
+    return rc;
   GemmParams p;
   gemm_params(c, &p, v, osz, out, n, 0, t, n, k, 1, pl.tile_rows, nullptr);
   p.b_bmul = groups > 1 ? 1u : 0u;   // a_bmul stays 0: the lhs is one batch, whatever the group
-  if (!rc) rc = gemm_quant_params(c, g, v, true, groups == 1, &ta_sc, &tb_sc, &p);
-  if (!rc) rc = grouped_launch(c, st, f, pl, smem, osz, offs, groups, t, false, &p, {&ta, &tb, &ta_sc, &tb_sc});
-  for (CUdeviceptr x : tmp)
-    if (x) pool_free(c, x, st);   // stream-ordered: reusable by later work once the GEMM has drained
-  return rc;
+  if ((rc = gemm_quant_params(c, g, v, true, groups == 1, &ta_sc, &tb_sc, &p))) return rc;
+  return grouped_launch(c, st, f, pl, smem, osz, offs, groups, t, false, &p, {&ta, &tb, &ta_sc, &tb_sc});
 }
 
 // ------------------------------------------------------------------------------------------------ convolution
@@ -3269,34 +3185,30 @@ static int conv_check_dw(const ConvNd& cv, const uint64_t* shape, const uint64_t
 
 // Pooled copy of an operand seen as [batch, rows, C] (strides in elements) with C padded to `cp` zero channels (repitch_rows
 // writes the padding columns as zeros).
-static int conv_pad_channels(b200_ctx* c, CUstream st, uint64_t in, uint64_t batch, uint64_t rows, uint64_t C, uint64_t s_b,
-                             uint64_t s_r, uint64_t s_c, uint64_t cp, CUdeviceptr* out) {
+static int conv_pad_channels(Scratch& scr, uint64_t in, uint64_t batch, uint64_t rows, uint64_t C, uint64_t s_b, uint64_t s_r,
+                             uint64_t s_c, uint64_t cp, CUdeviceptr* out) {
   CUdeviceptr buf;
-  int rc = pool_alloc(c, batch * rows * cp * 2, &buf, st);
-  if (rc) return rc;
   CUfunction f;
-  rc = get_func(c, "repitch_rows", &f);
-  if (rc) { pool_free(c, buf, st); return rc; }
+  int rc = scr.alloc(batch * rows * cp * 2, &buf);
+  if (!rc) rc = get_func(scr.c, "repitch_rows", &f);
+  if (rc) return rc;
   RepitchParams p{in, buf, batch, rows, C, s_b, s_r, s_c, cp, 2u, 0u};
   const uint64_t vecs = batch * rows * (cp / 8);
   const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((vecs + 255) / 256, 0x7FFFFFFFull));
   void* args[] = {&p};
-  rc = launch(c, f, grid, 1, 1, 256, 0, 1, st, args);
-  if (rc) { pool_free(c, buf, st); return rc; }
+  if ((rc = launch(scr.c, f, grid, 1, 1, 256, 0, 1, scr.st, args))) return rc;
   *out = buf;
   return B200_OK;
 }
 
 // A compact pooled copy of a rank-r view (b200_into_contiguous).
-static int conv_gather(b200_ctx* c, CUstream st, b200_dtype dt, uint64_t in, int r, const uint64_t* shape, const uint64_t* strides,
-                       CUdeviceptr* out) {
+static int conv_gather(Scratch& scr, b200_dtype dt, uint64_t in, int r, const uint64_t* shape, const uint64_t* strides, CUdeviceptr* out) {
   CUdeviceptr buf;
   uint64_t elems = 1;
   for (int d = 0; d < r; ++d) elems *= shape[d];
-  int rc = pool_alloc(c, elems * 2, &buf, st);
+  int rc = scr.alloc(elems * 2, &buf);
+  if (!rc) rc = b200_into_contiguous(scr.c, static_cast<b200_stream>(scr.st), dt, in, buf, r, shape, strides);
   if (rc) return rc;
-  rc = b200_into_contiguous(c, static_cast<b200_stream>(st), dt, in, buf, r, shape, strides);
-  if (rc) { pool_free(c, buf, st); return rc; }
   *out = buf;
   return B200_OK;
 }
@@ -3306,18 +3218,19 @@ static int conv_gather(b200_ctx* c, CUstream st, b200_dtype dt, uint64_t in, int
 // counts that are not multiples of 8 are copied with the channels padded to 8 zeros.  flat: the leading dimensions the map
 // reads as one strided dimension -- none (x, and dy in the data gradient), the spatial ones (the forward's weights: one
 // kernel-position dimension, returned as s_w) or N and the spatial ones (dy in the weight gradient: [pixels, Cout]).  s_d is
-// 0 for 2-D.  tmp[0] / tmp[1] receive the pooled copies (the caller frees them).
+// 0 for 2-D.  The copies are pooled in scr.
 struct ConvOperand {
   uint64_t ptr, C, s_w, s_h, s_d, s_n;
 };
 enum ConvFlat { kFlatNone, kFlatSpatial, kFlatAll };
-static int conv_prep(b200_ctx* c, CUstream st, b200_dtype dt, int n, uint64_t ptr, const uint64_t* shape, const uint64_t* ns, ConvFlat flat,
-                     CUdeviceptr tmp[2], ConvOperand* o) {
+static int conv_prep(Scratch& scr, b200_dtype dt, int n, uint64_t ptr, const uint64_t* shape, const uint64_t* ns, ConvFlat flat,
+                     ConvOperand* o) {
   const uint64_t N = shape[0], H = shape[n - 1], W = shape[n], C = shape[n + 1];
   uint64_t px = 1;
   for (int j = 1; j <= n; ++j) px *= shape[j];
   auto compact = [&](uint64_t base, uint64_t cc) { return ConvOperand{base, cc, cc, W * cc, n == 3 ? H * W * cc : 0, px * cc}; };
   const uint64_t spx = conv_flat_spatial(n, shape, ns);   // the spatial dimensions as one pixel dimension
+  CUdeviceptr gathered = 0, padded = 0;
   int rc = B200_OK;
   if (C % 8 == 0) {
     bool in_place = ptr % 16 == 0 && ns[n + 1] == 1 && conv_al16(ns[0]);
@@ -3331,18 +3244,18 @@ static int conv_prep(b200_ctx* c, CUstream st, b200_dtype dt, int n, uint64_t pt
       *o = {ptr, C, flat == kFlatSpatial ? spx : ns[n], ns[n - 1], n == 3 ? ns[1] : 0, ns[0]};
       return B200_OK;
     }
-    rc = conv_gather(c, st, dt, ptr, n + 2, shape, ns, &tmp[0]);
-    *o = compact(tmp[0], C);
+    rc = conv_gather(scr, dt, ptr, n + 2, shape, ns, &gathered);
+    *o = compact(gathered, C);
     return rc;
   }
   const uint64_t cp = (C + 7) / 8 * 8;
   uint64_t in = ptr, sb = ns[0], sp = spx, sc = ns[n + 1];
   if (spx == 0) {
-    rc = conv_gather(c, st, dt, ptr, n + 2, shape, ns, &tmp[0]);
-    in = tmp[0]; sb = px * C; sp = C; sc = 1;
+    rc = conv_gather(scr, dt, ptr, n + 2, shape, ns, &gathered);
+    in = gathered; sb = px * C; sp = C; sc = 1;
   }
-  if (!rc) rc = conv_pad_channels(c, st, in, N, px, C, sb, sp, sc, cp, &tmp[1]);
-  *o = compact(tmp[1], cp);
+  if (!rc) rc = conv_pad_channels(scr, in, N, px, C, sb, sp, sc, cp, &padded);
+  *o = compact(padded, cp);
   return rc;
 }
 
@@ -3399,21 +3312,16 @@ static int conv_forward(b200_ctx* c, b200_stream s, ConvNd cv, b200_dtype in_dty
   CUstream st = resolve_stream(c, s);
   conv_norm_strides(r, x_shape, x_strides, xs);
   conv_norm_strides(r, w_shape, w_strides, ws);
-  CUdeviceptr tmp[4] = {0, 0, 0, 0};
+  Scratch scr(c, st);
   ConvOperand xo{}, wo{};
-  rc = conv_prep(c, st, in_dtype, n, x, x_shape, xs, kFlatNone, &tmp[0], &xo);
-  if (!rc) rc = conv_prep(c, st, in_dtype, n, w, w_shape, ws, kFlatSpatial, &tmp[2], &wo);
-  if (!rc) {
-    ConvGeom g = conv_geom(n, N, cv.I, xo, cv.K, cv.O, Cout);
-    conv_geom_args(cv, &g);
-    g.w_sp = wo.s_w; g.w_sco = wo.s_n;
-    GemmProblem gp = conv_problem(in_dtype, out_dtype, xo.ptr, wo.ptr, out, M, Cout, KK * ((g.C + 63) / 64 * 64), os[n], &g);
-    conv_set_epilogue(&gp, ep);
-    rc = launch_wgmma(c, st, gp, false, false);
-  }
-  for (CUdeviceptr t : tmp)
-    if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMM has drained
-  return rc;
+  if ((rc = conv_prep(scr, in_dtype, n, x, x_shape, xs, kFlatNone, &xo)) || (rc = conv_prep(scr, in_dtype, n, w, w_shape, ws, kFlatSpatial, &wo)))
+    return rc;
+  ConvGeom g = conv_geom(n, N, cv.I, xo, cv.K, cv.O, Cout);
+  conv_geom_args(cv, &g);
+  g.w_sp = wo.s_w; g.w_sco = wo.s_n;
+  GemmProblem gp = conv_problem(in_dtype, out_dtype, xo.ptr, wo.ptr, out, M, Cout, KK * ((g.C + 63) / 64 * 64), os[n], &g);
+  conv_set_epilogue(&gp, ep);
+  return launch_wgmma(c, st, gp, false, false);
 }
 
 // ------------------------------------------------------------------------------------------------ convolution backward
@@ -3514,10 +3422,12 @@ static int conv_phase_plan(const ConvNd& cv, uint64_t Cout, ConvPhases* ph) {
 
 // Every phase's weights from w [Cout, *K, C] (strides ws) into one pooled buffer (*buf) of |K| * C * cp elements, by
 // conv_dgrad_weights (2-D) or conv3d_dgrad_weights (3-D).
-static int conv_dgrad_weights(b200_ctx* c, CUstream st, const ConvNd& cv, const ConvPhases& ph, uint64_t w, const uint64_t* ws, uint64_t C,
+static int conv_dgrad_weights(Scratch& scr, const ConvNd& cv, const ConvPhases& ph, uint64_t w, const uint64_t* ws, uint64_t C,
                               uint64_t Cout, uint64_t cp, CUdeviceptr* buf) {
+  b200_ctx* c = scr.c;
+  CUstream st = scr.st;
   const uint64_t KK = conv_prod(cv.K);
-  int rc = pool_alloc(c, KK * C * cp * 2, buf, st);
+  int rc = scr.alloc(KK * C * cp * 2, buf);
   if (rc) return rc;
   ConvDgradWeightsParams wp2;
   Conv3dDgradWeightsParams wp3;
@@ -3627,24 +3537,23 @@ static int conv_backward_data(b200_ctx* c, b200_stream s, ConvNd cv, b200_dtype 
   if (Cout == 0 || KK == 0) return B200_OK;
   conv_norm_strides(r, dy_shape, dy_strides, ys);
   conv_norm_strides(r, w_shape, w_strides, ws);
-  CUdeviceptr tmp[3] = {0, 0, 0};
+  Scratch scr(c, st);
+  CUdeviceptr wbuf = 0;
   ConvOperand y{};
-  rc = conv_prep(c, st, in_dtype, n, dy, dy_shape, ys, kFlatNone, tmp, &y);
+  rc = conv_prep(scr, in_dtype, n, dy, dy_shape, ys, kFlatNone, &y);
   const uint64_t cp = y.C;
-  if (!rc) rc = conv_dgrad_weights(c, st, cv, ph, w, ws, C, Cout, cp, &tmp[2]);
+  if (!rc) rc = conv_dgrad_weights(scr, cv, ph, w, ws, C, Cout, cp, &wbuf);
+  if (rc) return rc;
   // one stride-1 convolution of dy per phase that has taps and pixels
-  if (!rc) rc = ph.each([&](const DgradPhase1D* const* q) -> int {
+  return ph.each([&](const DgradPhase1D* const* q) -> int {
     for (int i = 0; i < 3; ++i)
       if (!q[i]->extent || !q[i]->taps) return B200_OK;
     ConvGeom g = conv_phase_geom(cv, N, C, q, y, os);
     if (c->dry) c->plan += conv_phase_line(cv, "dgrad", q, cv.O) + "\n";
-    const GemmProblem gp = conv_problem(in_dtype, out_dtype, y.ptr, tmp[2] + ph.off(q) * C * cp * 2, dx + conv_phase_dx(cv, q, os) * osz,
+    const GemmProblem gp = conv_problem(in_dtype, out_dtype, y.ptr, wbuf + ph.off(q) * C * cp * 2, dx + conv_phase_dx(cv, q, os) * osz,
                                         N * conv_prod(g.O), C, conv_prod(g.K) * ((cp + 63) / 64 * 64), os[n], &g);
     return launch_wgmma(c, st, gp, false, false);
   });
-  for (CUdeviceptr t : tmp)
-    if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMMs have drained
-  return rc;
 }
 
 // b200_conv2d_backward_weight / b200_conv3d_backward_weight: x [N, *I, C], dy [N, *O, Cout], dw [Cout, *K, C].
@@ -3679,23 +3588,18 @@ static int conv_backward_weight(b200_ctx* c, b200_stream s, ConvNd cv, b200_dtyp
   }
   conv_norm_strides(r, x_shape, x_strides, xs);
   conv_norm_strides(r, dy_shape, dy_strides, ys);
-  CUdeviceptr tmp[4] = {0, 0, 0, 0};
+  Scratch scr(c, st);
   ConvOperand xo{}, yo{};
-  rc = conv_prep(c, st, in_dtype, n, x, x_shape, xs, kFlatNone, &tmp[0], &xo);
-  if (!rc) rc = conv_prep(c, st, in_dtype, n, dy, dy_shape, ys, kFlatAll, &tmp[2], &yo);
-  if (!rc) {
-    ConvGeom g = conv_geom(n, N, cv.I, xo, cv.K, cv.O, Cout);
-    conv_geom_args(cv, &g);
-    g.mode = 2; g.dw_sp = dw_sp; g.dw_c = C;
-    GemmProblem gp = conv_problem(in_dtype, out_dtype, yo.ptr, xo.ptr, dw, Cout, KK * ((xo.C + 63) / 64 * 64), P, ds[0], &g);
-    gp.a_sm = 1; gp.a_sk = yo.s_w; gp.b_sn = 1; gp.b_sk = xo.s_w;   // both operands MN-major
-    // few tiles, a long K: the stream-K head may cut a tile into as many ranges as fill the SMs, each >= 8 k-blocks
-    gp.sk_max_parts = std::max<uint64_t>(8, (P + 63) / 64 / 8);
-    rc = launch_wgmma(c, st, gp, true, true);
-  }
-  for (CUdeviceptr t : tmp)
-    if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMM has drained
-  return rc;
+  if ((rc = conv_prep(scr, in_dtype, n, x, x_shape, xs, kFlatNone, &xo)) || (rc = conv_prep(scr, in_dtype, n, dy, dy_shape, ys, kFlatAll, &yo)))
+    return rc;
+  ConvGeom g = conv_geom(n, N, cv.I, xo, cv.K, cv.O, Cout);
+  conv_geom_args(cv, &g);
+  g.mode = 2; g.dw_sp = dw_sp; g.dw_c = C;
+  GemmProblem gp = conv_problem(in_dtype, out_dtype, yo.ptr, xo.ptr, dw, Cout, KK * ((xo.C + 63) / 64 * 64), P, ds[0], &g);
+  gp.a_sm = 1; gp.a_sk = yo.s_w; gp.b_sn = 1; gp.b_sk = xo.s_w;   // both operands MN-major
+  // few tiles, a long K: the stream-K head may cut a tile into as many ranges as fill the SMs, each >= 8 k-blocks
+  gp.sk_max_parts = std::max<uint64_t>(8, (P + 63) / 64 / 8);
+  return launch_wgmma(c, st, gp, true, true);
 }
 
 extern "C" int b200_conv2d(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr x, const uint64_t* x_shape,
@@ -3909,39 +3813,36 @@ static int conv_transpose(b200_ctx* c, b200_stream s, ConvNd cv, b200_dtype in_d
   const bool taps = Cin != 0 && KK != 0;
   conv_norm_strides(r, x_shape, x_strides, xs);
   conv_norm_strides(r, w_shape, w_strides, ws);
-  CUdeviceptr tmp[3] = {0, 0, 0};
+  Scratch scr(c, st);
+  CUdeviceptr wbuf = 0;
   ConvOperand y{};
   // the weight prep (and its per-phase offsets) only when some phase has taps
   if (taps) {
-    rc = conv_prep(c, st, in_dtype, n, x, x_shape, xs, kFlatNone, tmp, &y);
-    if (!rc) rc = conv_dgrad_weights(c, st, cv, ph, w, ws, C, Cin, y.C, &tmp[2]);
+    if ((rc = conv_prep(scr, in_dtype, n, x, x_shape, xs, kFlatNone, &y))) return rc;
+    if ((rc = conv_dgrad_weights(scr, cv, ph, w, ws, C, Cin, y.C, &wbuf))) return rc;
   }
-  if (!rc && taps && cv.s[0] == 1 && cv.s[1] == 1 && cv.s[2] == 1) {
+  if (taps && cv.s[0] == 1 && cv.s[1] == 1 && cv.s[2] == 1) {
     // one phase with every tap: the forward convolution kernel with the epilogue
     const DgradPhase1D* q[3] = {&ph.q[0][0], &ph.q[1][0], &ph.q[2][0]};
     ConvGeom g = conv_phase_geom(cv, N, C, q, y, os);
     if (c->dry) c->plan += conv_phase_line(cv, "tconv", q, cv.O) + " kblocks=" + std::to_string(KK * ((y.C + 63) / 64)) + "\n";
-    GemmProblem gp = conv_problem(in_dtype, out_dtype, y.ptr, tmp[2], out, P, C, KK * ((y.C + 63) / 64 * 64), os[n], &g);
+    GemmProblem gp = conv_problem(in_dtype, out_dtype, y.ptr, wbuf, out, P, C, KK * ((y.C + 63) / 64 * 64), os[n], &g);
     conv_set_epilogue(&gp, ep);
-    rc = launch_wgmma(c, st, gp, false, false);
-  } else if (!rc) {
-    // every phase with pixels, those no tap reaches included, in phase-batched launches
-    std::vector<TconvRun> runs;
-    const uint64_t cblk = taps ? (y.C + 63) / 64 : 0;
-    ph.each([&](const DgradPhase1D* const* q) {
-      if (!q[0]->extent || !q[1]->extent || !q[2]->extent) return B200_OK;
-      const uint64_t T[3] = {q[0]->taps, q[1]->taps, q[2]->taps}, E[3] = {q[0]->extent, q[1]->extent, q[2]->extent};
-      runs.push_back(TconvRun{{q[0], q[1], q[2]}, N * conv_prod(E), conv_prod(T) * cblk, taps ? ph.off(q) * C * y.C : 0,
-                              out + conv_phase_dx(cv, q, os) * osz});
-      return B200_OK;
-    });
-    if (!taps) y = ConvOperand{0, 8, 8, 8, 8, 8};
-    const uint64_t dx_s[4] = {os[0], n == 3 ? (uint64_t)cv.s[0] * os[1] : 0, (uint64_t)cv.s[1] * os[n - 1], (uint64_t)cv.s[2] * os[n]};
-    rc = launch_tconv(c, st, cv, in_dtype, out_dtype, y, N, C, tmp[2], runs, dx_s, os[n], ep);
+    return launch_wgmma(c, st, gp, false, false);
   }
-  for (CUdeviceptr t : tmp)
-    if (t) pool_free(c, t, st);   // stream-ordered: reusable by later work once the GEMMs have drained
-  return rc;
+  // every phase with pixels, those no tap reaches included, in phase-batched launches
+  std::vector<TconvRun> runs;
+  const uint64_t cblk = taps ? (y.C + 63) / 64 : 0;
+  ph.each([&](const DgradPhase1D* const* q) {
+    if (!q[0]->extent || !q[1]->extent || !q[2]->extent) return B200_OK;
+    const uint64_t T[3] = {q[0]->taps, q[1]->taps, q[2]->taps}, E[3] = {q[0]->extent, q[1]->extent, q[2]->extent};
+    runs.push_back(TconvRun{{q[0], q[1], q[2]}, N * conv_prod(E), conv_prod(T) * cblk, taps ? ph.off(q) * C * y.C : 0,
+                            out + conv_phase_dx(cv, q, os) * osz});
+    return B200_OK;
+  });
+  if (!taps) y = ConvOperand{0, 8, 8, 8, 8, 8};
+  const uint64_t dx_s[4] = {os[0], n == 3 ? (uint64_t)cv.s[0] * os[1] : 0, (uint64_t)cv.s[1] * os[n - 1], (uint64_t)cv.s[2] * os[n]};
+  return launch_tconv(c, st, cv, in_dtype, out_dtype, y, N, C, wbuf, runs, dx_s, os[n], ep);
 }
 
 extern "C" int b200_conv_transpose2d(b200_ctx* c, b200_stream s, b200_dtype in_dtype, b200_dtype out_dtype, b200_dptr x,
@@ -3994,16 +3895,16 @@ static ConvGroupedParams grp_params(const uint64_t* in, uint64_t OH, uint64_t OW
 }
 
 // A rank-4 operand the direct kernels read through its strides: kept in place with a unit channel stride, else gathered
-// into a compact pooled copy (*tmp, freed by the caller).  s: the strides to read it with.
-static int grp_operand(b200_ctx* c, CUstream st, b200_dtype dt, uint64_t ptr, const uint64_t* shape, const uint64_t* ns,
-                       CUdeviceptr* tmp, uint64_t* out, uint64_t s[4]) {
+// into a compact copy pooled in scr.  s: the strides to read it with.
+static int grp_operand(Scratch& scr, b200_dtype dt, uint64_t ptr, const uint64_t* shape, const uint64_t* ns, uint64_t* out, uint64_t s[4]) {
   if (ns[3] == 1) {
     *out = ptr;
     for (int d = 0; d < 4; ++d) s[d] = ns[d];
     return B200_OK;
   }
-  int rc = conv_gather(c, st, dt, ptr, 4, shape, ns, tmp);
-  *out = *tmp;
+  CUdeviceptr buf = 0;
+  int rc = conv_gather(scr, dt, ptr, 4, shape, ns, &buf);
+  *out = buf;
   s[3] = 1; s[2] = shape[3]; s[1] = shape[2] * shape[3]; s[0] = shape[1] * shape[2] * shape[3];
   return rc;
 }
@@ -4059,11 +3960,11 @@ extern "C" int b200_conv2d_grouped(b200_ctx* c, b200_stream s, b200_dtype in_dty
   if (N * tiles_h * tiles_w >= lim || chunks > 65535)
     return fail(B200_ERR_UNSUPPORTED, "%s: too many output tiles (N * ceil(OH / 8) * ceil(OW / 8) < 2^31, Cout <= 2^21)", what);
   CUstream st = resolve_stream(c, s);
-  CUdeviceptr tmp[2] = {0, 0};
+  Scratch scr(c, st);
   ConvGroupedParams p = grp_params(x_shape, OH, OW, w_shape, groups, a);
   uint64_t xsr[4], wsr[4];
-  rc = grp_operand(c, st, in_dtype, x, x_shape, xs, &tmp[0], &p.x, xsr);
-  if (!rc) rc = grp_operand(c, st, in_dtype, w, w_shape, ws, &tmp[1], &p.w, wsr);
+  rc = grp_operand(scr, in_dtype, x, x_shape, xs, &p.x, xsr);
+  if (!rc) rc = grp_operand(scr, in_dtype, w, w_shape, ws, &p.w, wsr);
   if (!rc) {
     p.out = out;
     p.x_sn = xsr[0]; p.x_sh = xsr[1]; p.x_sw = xsr[2];
@@ -4093,8 +3994,6 @@ extern "C" int b200_conv2d_grouped(b200_ctx* c, b200_stream s, b200_dtype in_dty
     void* kargs[] = {&p};
     if (!rc) rc = launch(c, f, (unsigned)(N * tiles_h * tiles_w), (unsigned)chunks, 1, 256, p.staged_ci ? (unsigned)smem : 0u, 1, st, kargs);
   }
-  for (CUdeviceptr t : tmp)
-    if (t) pool_free(c, t, st);
   return rc;
 }
 
@@ -4140,13 +4039,13 @@ extern "C" int b200_conv2d_grouped_backward_data(b200_ctx* c, b200_stream s, b20
   const uint64_t chunks = (C + kGrpChunk - 1) / kGrpChunk;
   if (chunks > 65535) return fail(B200_ERR_UNSUPPORTED, "%s: C must be <= 2^21", what);
   CUstream st = resolve_stream(c, s);
-  CUdeviceptr tmp[2] = {0, 0};
+  Scratch scr(c, st);
   ConvGroupedParams p = grp_params(dx_shape, OH, OW, w_shape, groups, a);
   uint64_t ysr[4] = {0, 0, 0, 1}, wsr[4] = {0, 0, 0, 1};
   // an empty dy or kernel reads nothing: dx comes out as +0 from the same launch
   if (Cout && KH && KW) {
-    rc = grp_operand(c, st, in_dtype, dy, dy_shape, ys, &tmp[0], &p.x, ysr);
-    if (!rc) rc = grp_operand(c, st, in_dtype, w, w_shape, ws, &tmp[1], &p.w, wsr);
+    rc = grp_operand(scr, in_dtype, dy, dy_shape, ys, &p.x, ysr);
+    if (!rc) rc = grp_operand(scr, in_dtype, w, w_shape, ws, &p.w, wsr);
   }
   if (!rc) {
     p.out = dx;
@@ -4158,8 +4057,6 @@ extern "C" int b200_conv2d_grouped_backward_data(b200_ctx* c, b200_stream s, b20
     void* kargs[] = {&p};
     if (!rc) rc = launch(c, f, (unsigned)((N * H * W + 7) / 8), (unsigned)chunks, 1, 256, 0, 1, st, kargs);
   }
-  for (CUdeviceptr t : tmp)
-    if (t) pool_free(c, t, st);
   return rc;
 }
 
@@ -4223,14 +4120,15 @@ extern "C" int b200_conv2d_grouped_backward_weight(b200_ctx* c, b200_stream s, b
     c->plan += line;
   }
   CUstream st = resolve_stream(c, s);
-  CUdeviceptr tmp[3] = {0, 0, 0};
+  Scratch scr(c, st);
+  CUdeviceptr part = 0;   // the per-segment partial sums
   ConvGroupedParams p = grp_params(x_shape, OH, OW, dw_shape, groups, a);
   uint64_t xsr[4], ysr[4];
-  rc = grp_operand(c, st, in_dtype, x, x_shape, xs, &tmp[0], &p.x, xsr);
-  if (!rc) rc = grp_operand(c, st, in_dtype, dy, dy_shape, ys, &tmp[1], &p.w, ysr);
-  if (!rc && nseg > 1) rc = pool_alloc(c, nseg * elems * 4, &tmp[2], st);
+  rc = grp_operand(scr, in_dtype, x, x_shape, xs, &p.x, xsr);
+  if (!rc) rc = grp_operand(scr, in_dtype, dy, dy_shape, ys, &p.w, ysr);
+  if (!rc && nseg > 1) rc = scr.alloc(nseg * elems * 4, &part);
   if (!rc) {
-    p.out = dw; p.part = tmp[2];
+    p.out = dw; p.part = part;
     p.x_sn = xsr[0]; p.x_sh = xsr[1]; p.x_sw = xsr[2];
     p.y_sn = ysr[0]; p.y_sh = ysr[1]; p.y_sw = ysr[2];
     p.o_sn = ds[0]; p.o_sw = dw_sp;
@@ -4243,8 +4141,6 @@ extern "C" int b200_conv2d_grouped_backward_weight(b200_ctx* c, b200_stream s, b
     if (!rc && nseg > 1) rc = get_func(c, std::string("conv2d_grp_wgrad_combine_") + grp_tag(out_dtype), &f);
     if (!rc && nseg > 1) rc = launch(c, f, blocks, 1, 1, 256, 0, 1, st, kargs);
   }
-  for (CUdeviceptr t : tmp)
-    if (t) pool_free(c, t, st);
   return rc;
 }
 
@@ -4323,14 +4219,15 @@ static bool attn_view_ok(const AttnView& v) {
   return true;
 }
 
-// v in place when attn_view_ok, else gathered into a compact pooled copy *tmp (the caller frees it) that v then describes.
-static int attn_stage(b200_ctx* c, CUstream st, AttnView* v, CUdeviceptr* tmp) {
+// v in place when attn_view_ok, else gathered into a compact copy pooled in scr that v then describes.
+static int attn_stage(Scratch& scr, AttnView* v) {
   if (attn_view_ok(*v)) return B200_OK;
   const uint64_t* sh = v->shape;
-  int rc = pool_alloc(c, sh[0] * sh[1] * sh[2] * sh[3] * v->esz, tmp, st);
+  CUdeviceptr buf;
+  int rc = scr.alloc(sh[0] * sh[1] * sh[2] * sh[3] * v->esz, &buf);
   if (rc) return rc;
-  rc = b200_into_contiguous(c, static_cast<b200_stream>(st), v->dt, v->ptr, *tmp, 4, sh, v->ns);
-  v->ptr = *tmp;
+  rc = b200_into_contiguous(scr.c, static_cast<b200_stream>(scr.st), v->dt, v->ptr, buf, 4, sh, v->ns);
+  v->ptr = buf;
   v->ns[3] = 1; v->ns[2] = sh[3]; v->ns[1] = sh[2] * sh[3]; v->ns[0] = sh[1] * sh[2] * sh[3];
   return rc;
 }
@@ -4438,10 +4335,10 @@ static int attn_check_caches(const char* what, const AttnView& kc, const AttnVie
 // V stages of kAttnBlock 128-byte rows more shared memory.
 static int attn_fwd_launch(b200_ctx* c, CUstream st, const std::string& prefix, AttnView q, AttnView k, AttnView v, const AttnView& o,
                            uint64_t ctas, void* p, uint32_t kv_rows = kAttnBlock, bool stage_kv = true) {
-  CUdeviceptr tmp[3] = {0, 0, 0};
-  int rc = attn_stage(c, st, &q, &tmp[0]);
-  if (!rc && stage_kv) rc = attn_stage(c, st, &k, &tmp[1]);
-  if (!rc && stage_kv) rc = attn_stage(c, st, &v, &tmp[2]);
+  Scratch scr(c, st);
+  int rc = attn_stage(scr, &q);
+  if (!rc && stage_kv) rc = attn_stage(scr, &k);
+  if (!rc && stage_kv) rc = attn_stage(scr, &v);
   CUtensorMap mq, mk, mv, mo;
   if (!rc) rc = attn_map(c, &mq, q, false, kAttnBlock);
   if (!rc) rc = attn_map(c, &mk, k, false, kv_rows);
@@ -4456,8 +4353,6 @@ static int attn_fwd_launch(b200_ctx* c, CUstream st, const std::string& prefix, 
   if (!rc) rc = attn_set_smem(c, f, smem);
   void* kargs[] = {&mq, &mk, &mv, &mo, p};
   if (!rc) rc = launch(c, f, (unsigned)ctas, 1, 1, 384, smem, 1, st, kargs);
-  for (CUdeviceptr t : tmp)
-    if (t) pool_free(c, t, st);   // stream-ordered: reusable once the kernel has drained
   return rc;
 }
 
@@ -4465,14 +4360,13 @@ struct AttnBwdOps {
   AttnView q, k, v, out, dout, dq, dk, dv;
 };
 
-// Stages what the present sides read: q, out and dout with query rows (has_q), k and v with keys (has_k); tmp[0..4] receive
-// the copies (the caller frees them).
-static int attn_bwd_stage(b200_ctx* c, CUstream st, AttnBwdOps* o, bool has_q, bool has_k, CUdeviceptr tmp[5]) {
-  int rc = has_q ? attn_stage(c, st, &o->q, &tmp[0]) : B200_OK;
-  if (!rc && has_k) rc = attn_stage(c, st, &o->k, &tmp[1]);
-  if (!rc && has_k) rc = attn_stage(c, st, &o->v, &tmp[2]);
-  if (!rc && has_q) rc = attn_stage(c, st, &o->out, &tmp[3]);
-  if (!rc && has_q) rc = attn_stage(c, st, &o->dout, &tmp[4]);
+// Stages what the present sides read into scr: q, out and dout with query rows (has_q), k and v with keys (has_k).
+static int attn_bwd_stage(Scratch& scr, AttnBwdOps* o, bool has_q, bool has_k) {
+  int rc = has_q ? attn_stage(scr, &o->q) : B200_OK;
+  if (!rc && has_k) rc = attn_stage(scr, &o->k);
+  if (!rc && has_k) rc = attn_stage(scr, &o->v);
+  if (!rc && has_q) rc = attn_stage(scr, &o->out);
+  if (!rc && has_q) rc = attn_stage(scr, &o->dout);
   return rc;
 }
 
@@ -4618,11 +4512,12 @@ extern "C" int b200_attention_backward(b200_ctx* c, b200_stream s, b200_dtype in
   if (rc) return rc;
 
   CUstream st = resolve_stream(c, s);
-  CUdeviceptr tmp[6] = {0, 0, 0, 0, 0, 0};   // gathers of q, k, v, out, dout; the workspace
-  rc = attn_bwd_stage(c, st, &o, has_q, true, tmp);
-  if (!rc && has_q) rc = pool_alloc(c, 2 * rows * 4, &tmp[5], st);
+  Scratch scr(c, st);
+  CUdeviceptr ws = 0;
+  rc = attn_bwd_stage(scr, &o, has_q, true);
+  if (!rc && has_q) rc = scr.alloc(2 * rows * 4, &ws);
   AttnBwdParams p{};
-  p.ws = tmp[5];
+  p.ws = ws;
   p.lse = lse;
   p.out = o.out.ptr; p.dout = o.dout.ptr;
   p.o_sb = o.out.s_batch(); p.o_sh = o.out.s_head(); p.o_ss = o.out.s_row();
@@ -4637,8 +4532,6 @@ extern "C" int b200_attention_backward(b200_ctx* c, b200_stream s, b200_dtype in
   p.scale_log2 = attn_scale_log2(args->scale);
   p.scale = args->scale;
   if (!rc) rc = attn_bwd_launch(c, st, "attn_bwd_", o, has_q, true, nqb * Hq * B, nkb * Hkv * B, &p);
-  for (CUdeviceptr t : tmp)
-    if (t) pool_free(c, t, st);   // stream-ordered: reusable once the kernels have drained
   return rc;
 }
 
@@ -4765,14 +4658,15 @@ extern "C" int b200_attention_varlen_backward(b200_ctx* c, b200_stream s, b200_d
   if (rc) return rc;
 
   CUstream st = resolve_stream(c, s);
-  CUdeviceptr tmp[6] = {0, 0, 0, 0, 0, 0};   // gathers of q, k, v, out, dout; the workspace
+  Scratch scr(c, st);
+  CUdeviceptr ws = 0;
   // out and dout are read by the delta kernel with 16-byte loads, so they follow the maps' rule
-  rc = attn_bwd_stage(c, st, &o, has_q, has_k, tmp);
-  if (!rc && has_q) rc = pool_alloc(c, 2 * Hq * Tqp * 4, &tmp[5], st);
+  rc = attn_bwd_stage(scr, &o, has_q, has_k);
+  if (!rc && has_q) rc = scr.alloc(2 * Hq * Tqp * 4, &ws);
   AttnVarlenParams p{};
   p.lse = lse;
   p.cu_q = cu_seqlens_q; p.cu_k = cu_seqlens_k;
-  p.ws = tmp[5];
+  p.ws = ws;
   p.out = o.out.ptr; p.dout = o.dout.ptr;
   p.o_st = o.out.s_row(); p.o_sh = o.out.s_head(); p.d_st = o.dout.s_row(); p.d_sh = o.dout.s_head();
   p.dq = dq; p.dk = dk; p.dv = dv;
@@ -4787,8 +4681,6 @@ extern "C" int b200_attention_varlen_backward(b200_ctx* c, b200_stream s, b200_d
   p.scale_log2 = attn_scale_log2(args->scale);
   p.scale = args->scale;
   if (!rc) rc = attn_bwd_launch(c, st, "attn_bwd_varlen_", o, has_q, has_k, nqb * Hq * B, nkb * Hkv * B, &p);
-  for (CUdeviceptr t : tmp)
-    if (t) pool_free(c, t, st);   // stream-ordered: reusable once the kernels have drained
   return rc;
 }
 
@@ -4913,9 +4805,10 @@ static int kv_attend(b200_ctx* c, b200_stream s, const char* what, b200_dtype in
     return fail(B200_ERR_UNSUPPORTED, "%s: more than 2^31 - 1 CTAs", what);
 
   CUstream st = resolve_stream(c, s);
-  CUdeviceptr tmp[2] = {0, 0};   // the gather of q; the split workspace
-  rc = attn_stage(c, st, &qv, &tmp[0]);
-  if (!rc && nsplit > 1) rc = pool_alloc(c, (size_t)nsplit * rows * (D + 2) * 4, &tmp[1], st);
+  Scratch scr(c, st);
+  CUdeviceptr ws = 0;   // the split workspace
+  rc = attn_stage(scr, &qv);
+  if (!rc && nsplit > 1) rc = scr.alloc((size_t)nsplit * rows * (D + 2) * 4, &ws);
   if (!rc) {
     const uint32_t DB = attn_db(D);
     const uint32_t R = max_pages == 1 ? kAttnKvBlock : (uint32_t)std::min<uint64_t>(page, kAttnKvBlock);
@@ -4926,7 +4819,7 @@ static int kv_attend(b200_ctx* c, b200_stream s, const char* what, b200_dtype in
     AttnKvParams p{};
     p.out = out; p.o_sb = ov.s_batch(); p.o_sh = ov.s_head(); p.o_ss = ov.s_row();
     p.lse = lse;
-    p.ws = tmp[1];
+    p.ws = ws;
     p.table = block_table;
     if (block_table) {
       p.t_sb = bt_strides ? bt_strides[0] : max_pages;
@@ -4959,8 +4852,6 @@ static int kv_attend(b200_ctx* c, b200_stream s, const char* what, b200_dtype in
                            kAttnKvCombineThreads, 0, 1, st, cargs);
     }
   }
-  for (CUdeviceptr t : tmp)
-    if (t) pool_free(c, t, st);   // stream-ordered: reusable once the kernels have drained
   return rc;
 }
 
@@ -5121,9 +5012,9 @@ static int kv_write(b200_ctx* c, b200_stream s, const char* what, b200_dtype dty
   // the kernel moves 16-byte units: other views of the new tokens are gathered into a compact copy first
   AttnView kn = attn_view(k_new, dtype, kn_shape, kn_strides, kAttnBSHD), vn = attn_view(v_new, dtype, vn_shape, vn_strides, kAttnBSHD);
   CUstream st = resolve_stream(c, s);
-  CUdeviceptr tmp[2] = {0, 0};
-  rc = attn_stage(c, st, &kn, &tmp[0]);
-  if (!rc) rc = attn_stage(c, st, &vn, &tmp[1]);
+  Scratch scr(c, st);
+  rc = attn_stage(scr, &kn);
+  if (!rc) rc = attn_stage(scr, &vn);
   if (!rc) {
     AttnKvWriteParams p{};
     p.kn = kn.ptr; p.vn = vn.ptr; p.kc = k_cache; p.vc = v_cache; p.slots = slot_mapping;
@@ -5145,8 +5036,6 @@ static int kv_write(b200_ctx* c, b200_stream s, const char* what, b200_dtype dty
     const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((units + 255) / 256, (uint64_t)c->props.num_sms * 32));
     if (!rc) rc = launch(c, f, grid, 1, 1, 256, 0, 1, st, kargs);
   }
-  for (CUdeviceptr t : tmp)
-    if (t) pool_free(c, t, st);
   return rc;
 }
 

@@ -151,6 +151,15 @@ def launch_quantized_fp8(client: ComputeClient, lhs, rhs, out: TensorHandle, str
     _launch_q(client, lhs, rhs, out, stream, "matmul_quantized_fp8")
 
 
+def _quant_operand(q, stream):
+    """The b200_quant_operand of a QuantizedTensor, its tensors marked as used on `stream`."""
+    ts = (q.values, q.block_scales, q.tensor_scale)
+    for t in ts:
+        if t is not None:
+            t.handle.used_on(stream)
+    return _ffi.QuantOperand(q.scheme.to_c(), *(t.handle.ptr if t is not None else 0 for t in ts))
+
+
 def _launch_q(client, lhs, rhs, out, stream, what: str) -> None:
     """The shared body of launch_quantized / launch_quantized_fp8: b200_<what> on two QuantizedTensors."""
     try:
@@ -163,13 +172,7 @@ def _launch_q(client, lhs, rhs, out, stream, what: str) -> None:
         if list(out.shape) != ls[:-2] + [M, N] or not out.is_contiguous():
             raise B200Error(6, f"{what}: out must be contiguous with shape {ls[:-2] + [M, N]}")
         batch = int(np.prod(ls[:-2])) if len(ls) > 2 else 1
-        ops = []
-        for q in (lhs, rhs):
-            for t in (q.values, q.block_scales, q.tensor_scale):
-                if t is not None:
-                    t.handle.used_on(stream)
-            ops.append(_ffi.QuantOperand(q.scheme.to_c(), *(t.handle.ptr if t is not None else 0
-                                                              for t in (q.values, q.block_scales, q.tensor_scale))))
+        ops = [_quant_operand(q, stream) for q in (lhs, rhs)]
         out.handle.used_on(stream)
         fn = getattr(client._lib, "b200_" + what)
         _ffi.check(fn(client._ctx, stream, C.byref(ops[0]), C.byref(ops[1]), DTYPES[out.dtype], C.c_uint64(out.handle.ptr),
@@ -260,13 +263,7 @@ def launch_grouped_quantized_fp8(client: ComputeClient, qx, qw, offs: TensorHand
         T, (G, N, K) = xs[0], ws
         if list(out.shape) != [T, N] or not out.is_contiguous():
             raise B200Error(6, f"{what}: out must be contiguous with shape {[T, N]}")
-        ops = []
-        for q in (qx, qw):
-            for t in (q.values, q.block_scales, q.tensor_scale):
-                if t is not None:
-                    t.handle.used_on(stream)
-            ops.append(_ffi.QuantOperand(q.scheme.to_c(), *(t.handle.ptr if t is not None else 0
-                                                              for t in (q.values, q.block_scales, q.tensor_scale))))
+        ops = [_quant_operand(q, stream) for q in (qx, qw)]
         offs.handle.used_on(stream)
         out.handle.used_on(stream)
         _ffi.check(client._lib.b200_matmul_grouped_quantized_fp8(client._ctx, stream, C.byref(ops[0]), C.byref(ops[1]),

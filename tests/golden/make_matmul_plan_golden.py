@@ -3,13 +3,15 @@ tests/test_matmul_plan_golden_cpu.py).
 
     python tests/golden/make_matmul_plan_golden.py
 
-Each case is one call of b200_matmul, b200_matmul_fused, b200_matmul_mixed, b200_matmul_scaled, b200_matmul_quantized or
-b200_matmul_grouped in a fresh planning context (b200_plan_begin, 132 SMs); the fixture stores the call, the returned status,
-the full error message and the full plan text.  The cases cover every input dtype with every output dtype, the f32 modes, all
-four operand majors, batch broadcasts that collapse and that peel, unit and empty extents, pitched and misaligned operands on
-the staging and the SIMT paths, every gemm.variant / split_k / epilogue value, output strides with and without TMA stores, the
-epilogue fields, block-scaled and integer-quantized operands, both grouped modes with all operand layouts, and one case per
-refusal, with a few calls where two checks fail at once.  Plans hold no pointer bases and no kernel parameter blocks, so those
+Each case is one call of b200_matmul, b200_matmul_fused, b200_matmul_mixed, b200_matmul_scaled, b200_matmul_quantized,
+b200_matmul_quantized_fp8, b200_matmul_grouped or b200_matmul_grouped_quantized_fp8 in a fresh planning context
+(b200_plan_begin, 132 SMs); the fixture stores the call, the returned status, the full error message and the full plan text.
+The cases cover every input dtype with every output dtype, the f32 modes, all four operand majors, batch broadcasts that
+collapse and that peel, unit and empty extents, pitched and misaligned operands on the staging and the SIMT paths, every
+gemm.variant / split_k / epilogue value, output strides with and without TMA stores, the epilogue fields, block-scaled,
+integer-quantized and fp8-quantized operands (e4m3 / e5m2 per side, every block size, block-scale dtype and level, staged
+codes), both grouped modes with all operand layouts, the fp8 grouped matmul's group counts, tile threshold and empty extents,
+and one case per refusal, with a few calls where two checks fail at once.  Plans hold no pointer bases and no kernel parameter blocks, so those
 are left to the GPU tests.
 """
 from __future__ import annotations
@@ -130,6 +132,15 @@ def qop(value="q8s", block=32, block_scale="f32", tensor=0, values=A, bs=S1, ts=
 
 def qmm(lhs, rhs, M, N, K, odt="f32", batch=1, o=O, options=None):
     return {"fn": "b200_matmul_quantized", "args": [lhs, rhs, odt, o, batch, M, N, K], "options": options or {}}
+
+
+def qf8(lhs, rhs, M, N, K, odt="bf16", batch=1, o=O, options=None):
+    return {"fn": "b200_matmul_quantized_fp8", "args": [lhs, rhs, odt, o, batch, M, N, K], "options": options or {}}
+
+
+def gqf8(lhs, rhs, G, T, N, K, odt="bf16", o=O, offs=OFFS, options=None):
+    """b200_matmul_grouped_quantized_fp8: lhs codes [T, K] x rhs codes [G, N, K] -> out [T, N]."""
+    return {"fn": "b200_matmul_grouped_quantized_fp8", "args": [lhs, rhs, offs, G, odt, o, T, N, K], "options": options or {}}
 
 
 def grouped(mode, T, G, K=None, N=64, M=None, idt="bf16", odt="bf16", a_major=None, b_major=None, a_pitch=0, b_pitch=0, o_pitch=0,
@@ -523,6 +534,158 @@ def cases():
     add("grp-err2-tiles-and-epilogue", grouped("m", (1 << 31) - 1, 1024, 64, (1 << 31) - 1, options={"gemm.epilogue": "bogus"}))
     add("grp-err2-kmajor-and-staged", grouped("k", 4096, 8, N=512, M=256, a_major="k", a=A + 2))
     add("grp-err2-col-stride-and-misaligned", grouped("m", 4096, 8, 512, 768, a=A + 1, strides=([512, 1], [512 * 768, 768, 1], [1, 4096])))
+
+    # ---- b200_matmul_quantized_fp8
+    fp8s, bsds = ("e4m3", "e5m2"), ("f32", "f16", "bf16", "ue8m0", "e4m3")
+
+    def tens(v, ts=S2):
+        return qop(v, 0, 0, 1, bs=0, ts=ts)
+
+    for lv in fp8s:
+        for rv in fp8s:
+            add(f"qf8-tensor-{lv}-{rv}", qf8(tens(lv), tens(rv, S2 + 4), 1024, 768, 512))
+            add(f"qf8-block-{lv}-{rv}", qf8(qop(lv, 128), qop(rv, 128, bs=S2), 1024, 768, 512))
+    for v in fp8s:
+        for blk in (32, 64, 128):
+            for bsd in bsds:
+                add(f"qf8-block-{v}-{blk}-{bsd}", qf8(qop(v, blk, bsd), qop(v, blk, bsd, bs=S2), 1024, 768, 512))
+            add(f"qf8-twolevel-{v}-{blk}", qf8(qop(v, blk, "f16", 1, ts=S2), qop(v, blk, "e4m3", 1, bs=S2, ts=S2 + 4), 512, 512, 512))
+    for lb, rb in ((32, 64), (128, 32), (64, 128), (0, 32), (128, 0), (0, 0)):
+        for odt in ("f32", "bf16", "f16"):
+            lq = qop("e4m3", lb, "f32", 0 if lb else 1, bs=S1 if lb else 0, ts=0 if lb else S2)
+            rq = qop("e5m2", rb, "ue8m0", 0 if rb else 1, bs=S2 if rb else 0, ts=0 if rb else S2 + 4)
+            add(f"qf8-mixed-{lb}-{rb}-{odt}", qf8(lq, rq, 1024, 768, 512, odt))
+            add(f"qf8-mixed-{lb}-{rb}-{odt}-batch", qf8(lq, rq, 256, 256, 256, odt, batch=3))
+    for opts in ({"gemm.variant": "2sm_n256"}, {"gemm.variant": "2sm_n128"}, {"gemm.variant": "1sm_n128"}, {"gemm.variant": "2sm_m512"},
+                 {"gemm.variant": "2sm_n224"}, {"gemm.variant": "simt"}, {"gemm.variant": "bogus"}, {"gemm.split_k": "on"},
+                 {"gemm.split_k": "3"}, {"gemm.split_k": "bogus"}, {"gemm.epilogue": "tma"}, {"gemm.epilogue": "direct"},
+                 {"gemm.epilogue": "bogus"}):
+        tag = "-".join(f"{k.split('.')[1]}={v}" for k, v in opts.items())
+        add(f"qf8-opt-{tag}-block", qf8(qop("e4m3", 128), qop("e4m3", 128, bs=S2), 4096, 4096, 4096, options=opts))
+        add(f"qf8-opt-{tag}-tensor", qf8(tens("e4m3"), tens("e5m2", S2 + 4), 4096, 4096, 4096, options=opts))
+    add("qf8-misaligned-lhs", qf8(qop("e4m3", 32, values=A + 8), qop("e4m3", 32, bs=S2), 1024, 768, 512))
+    add("qf8-misaligned-rhs", qf8(qop("e4m3", 32), qop("e5m2", 32, values=B + 1, bs=S2), 1024, 768, 512))
+    add("qf8-k-not-16", qf8(tens("e4m3"), tens("e4m3", S2 + 4), 256, 256, 200))
+    add("qf8-k-not-16-batch", qf8(tens("e5m2"), tens("e4m3", S2 + 4), 256, 256, 200, batch=3))
+    add("qf8-k-short-block", qf8(tens("e4m3"), tens("e4m3", S2 + 4), 256, 256, 320))
+    add("qf8-small", qf8(qop("e4m3", 32), qop("e5m2", 32, bs=S2), 16, 8, 64))
+    add("qf8-m1", qf8(qop("e4m3", 64), qop("e4m3", 64, bs=S2), 1, 4096, 4096))
+    add("qf8-n1", qf8(qop("e4m3", 64), qop("e4m3", 64, bs=S2), 4096, 1, 4096))
+    add("qf8-k-2^17", qf8(tens("e4m3"), tens("e4m3", S2 + 4), 64, 64, 1 << 17))
+    add("qf8-empty-m", qf8(qop("e4m3", 32), qop("e4m3", 32, bs=S2), 0, 64, 64))
+    add("qf8-empty-n", qf8(qop("e4m3", 32), qop("e4m3", 32, bs=S2), 64, 0, 64))
+    add("qf8-empty-batch", qf8(qop("e4m3", 32), qop("e4m3", 32, bs=S2), 64, 64, 64, batch=0))
+    add("qf8-empty-null", qf8(qop("e4m3", 32, values=0), qop("e4m3", 32, bs=S2), 0, 64, 64, o=0))
+    add("qf8-err-null-lhs", qf8(None, qop("e4m3", 32, bs=S2), 64, 64, 64))
+    add("qf8-err-null-rhs", qf8(qop("e4m3", 32), None, 64, 64, 64))
+    for v in ("q8s", "q8f", "q4s", "q2f"):
+        add(f"qf8-err-int-{v}-lhs", qf8(qop(v, 32), qop("e4m3", 32, bs=S2), 64, 64, 64))
+        add(f"qf8-err-int-{v}-rhs", qf8(qop("e4m3", 32), qop(v, 32, bs=S2), 64, 64, 64))
+    add("qf8-err-e2m1", qf8(qop("e4m3", 32), qop("e2m1", 32, "ue8m0", bs=S2), 64, 64, 64))
+    add("qf8-err-e2m1-lhs", qf8(qop("e2m1", 32, "ue8m0"), qop("e4m3", 32, bs=S2), 64, 64, 64))
+    add("qf8-err-block16", qf8(qop("e4m3", 16), qop("e4m3", 16, bs=S2), 64, 64, 64))
+    add("qf8-err-block8", qf8(qop("e4m3", 32), qop("e4m3", 8, bs=S2), 64, 64, 64))
+    add("qf8-err-block256", qf8(qop("e4m3", 256), qop("e4m3", 32, bs=S2), 64, 64, 256))
+    add("qf8-err-bad-value", qf8(qop("bogus", 32), qop("e4m3", 32, bs=S2), 64, 64, 64))
+    add("qf8-err-tensor-flag", qf8(qop("e4m3", 32, tensor=2), qop("e4m3", 32, bs=S2), 64, 64, 64))
+    add("qf8-err-no-level", qf8(qop("e4m3", 0, 0, 0, bs=0), qop("e4m3", 32, bs=S2), 64, 64, 64))
+    add("qf8-err-bad-scale-dtype", qf8(qop("e4m3", 32, "i32"), qop("e4m3", 32, bs=S2), 64, 64, 64))
+    add("qf8-err-k-block", qf8(qop("e4m3", 32), qop("e4m3", 32, bs=S2), 64, 64, 48))
+    add("qf8-err-null-block-scales", qf8(qop("e4m3", 32, bs=0), qop("e4m3", 32, bs=S2), 64, 64, 64))
+    add("qf8-err-null-tensor-scale", qf8(tens("e4m3", 0), tens("e4m3", S2 + 4), 64, 64, 64))
+    add("qf8-err-misaligned-scales", qf8(qop("e4m3", 32, bs=S1 + 1), qop("e4m3", 32, bs=S2), 64, 64, 64))
+    add("qf8-err-out-i32", qf8(qop("e4m3", 32), qop("e4m3", 32, bs=S2), 64, 64, 64, "i32"))
+    add("qf8-err-out-e4m3", qf8(qop("e4m3", 32), qop("e4m3", 32, bs=S2), 64, 64, 64, "e4m3"))
+    add("qf8-err-k0", qf8(qop("e4m3", 32), qop("e4m3", 32, bs=S2), 64, 64, 0))
+    add("qf8-err-k0-tensor", qf8(tens("e4m3"), tens("e4m3", S2 + 4), 64, 64, 0))
+    add("qf8-err-null-values", qf8(qop("e4m3", 32, values=0), qop("e4m3", 32, bs=S2), 64, 64, 64))
+    add("qf8-err-null-rhs-values", qf8(qop("e4m3", 32), qop("e4m3", 32, values=0, bs=S2), 64, 64, 64))
+    add("qf8-err-null-out", qf8(qop("e4m3", 32), qop("e4m3", 32, bs=S2), 64, 64, 64, o=0))
+    add("qf8-err-misaligned-out", qf8(qop("e4m3", 32), qop("e4m3", 32, bs=S2), 64, 64, 64, "f32", o=O + 2))
+    add("qf8-err-m-2^31", qf8(qop("e4m3", 32), qop("e4m3", 32, bs=S2), BIG, 64, 64))
+    add("qf8-err-n-2^31", qf8(qop("e4m3", 32), qop("e4m3", 32, bs=S2), 64, BIG, 64))
+    add("qf8-err-k-2^31", qf8(tens("e4m3"), tens("e4m3", S2 + 4), 64, 64, BIG))
+    add("qf8-err-batch-2^20", qf8(qop("e4m3", 32), qop("e4m3", 32, bs=S2), 64, 64, 64, batch=1 << 20))
+    add("qf8-err-tiles", qf8(qop("e4m3", 32), qop("e4m3", 32, bs=S2), (1 << 31) - 1, (1 << 31) - 1, 64, batch=(1 << 20) - 1))
+    add("qf8-err2-lhs-and-rhs", qf8(qop("q8s", 32), qop("e4m3", 16, bs=S2), 64, 64, 64))
+    add("qf8-err2-e2m1-and-block", qf8(qop("e2m1", 16, "ue8m0"), qop("e4m3", 32, bs=S2), 64, 64, 64))
+    add("qf8-err2-out-and-k0", qf8(qop("e4m3", 32), qop("e4m3", 32, bs=S2), 64, 64, 0, "i32"))
+    add("qf8-err2-null-and-misaligned", qf8(qop("e4m3", 32, values=0), qop("e4m3", 32, bs=S2), 64, 64, 64, o=O + 2))
+    add("qf8-err2-misaligned-and-extent", qf8(qop("e4m3", 32), qop("e4m3", 32, bs=S2), BIG, 64, 64, o=O + 2))
+    add("qf8-err2-staged-and-variant", qf8(qop("e4m3", 32, values=A + 8), qop("e4m3", 32, bs=S2), 1024, 768, 512,
+                                            options={"gemm.variant": "bogus"}))
+    add("qf8-err2-staged-and-epilogue", qf8(tens("e4m3"), tens("e4m3", S2 + 4), 1024, 768, 200, options={"gemm.epilogue": "bogus"}))
+    add("qf8-err2-variant-and-epilogue", qf8(qop("e4m3", 128), qop("e4m3", 128, bs=S2), 4096, 4096, 4096,
+                                             options={"gemm.variant": "bogus", "gemm.epilogue": "bogus"}))
+
+    # ---- b200_matmul_grouped_quantized_fp8
+    for lv in fp8s:
+        for rv in fp8s:
+            add(f"gqf8-tensor-{lv}-{rv}", gqf8(tens(lv), tens(rv, S2 + 4), 8, 4096, 768, 512))
+            add(f"gqf8-block-{lv}-{rv}", gqf8(qop(lv, 128), qop(rv, 128, bs=S2), 8, 4096, 768, 512))
+    for v in fp8s:
+        for blk in (32, 64, 128):
+            for bsd in bsds:
+                add(f"gqf8-block-{v}-{blk}-{bsd}", gqf8(qop(v, blk, bsd), qop(v, blk, bsd, bs=S2), 8, 4096, 768, 512))
+            add(f"gqf8-twolevel-{v}-{blk}", gqf8(qop(v, blk, "f16", 1, ts=S2), qop(v, blk, "e4m3", 1, bs=S2, ts=S2 + 4), 6, 3000, 512, 512))
+    for lb, rb in ((32, 64), (128, 32), (0, 128), (128, 0), (0, 0)):
+        for odt in ("f32", "bf16", "f16"):
+            lq = qop("e5m2", lb, "bf16", 0 if lb else 1, bs=S1 if lb else 0, ts=0 if lb else S2)
+            rq = qop("e4m3", rb, "f32", 0 if rb else 1, bs=S2 if rb else 0, ts=0 if rb else S2 + 4)
+            add(f"gqf8-mixed-{lb}-{rb}-{odt}", gqf8(lq, rq, 8, 4096, 768, 512, odt))
+    blk = (qop("e4m3", 128), qop("e4m3", 128, bs=S2))
+    for G, T, N, K in ((1, 4096, 768, 512), (128, 32768, 1536, 1024), (1024, 65536, 256, 256), (8, 8 * 1024, 256, 256),
+                       (8, 8 * 1024 - 1, 256, 256), (8, 100, 256, 256), (8, 1, 256, 256), (3, 1000, 700, 384), (32, 32768, 4096, 7168)):
+        add(f"gqf8-shape-G{G}-T{T}-N{N}-K{K}", gqf8(*blk, G, T, N, K))
+    add("gqf8-G1-tensor", gqf8(tens("e4m3"), tens("e4m3", S2 + 4), 1, 4096, 768, 512))
+    add("gqf8-G1024-tensor", gqf8(tens("e4m3"), tens("e4m3", S2 + 4), 1024, 65536, 256, 256))
+    add("gqf8-T0", gqf8(*blk, 8, 0, 768, 512))
+    add("gqf8-N0", gqf8(*blk, 8, 4096, 0, 512))
+    add("gqf8-G0", gqf8(*blk, 0, 4096, 768, 512))
+    add("gqf8-T0-null", gqf8(qop("e4m3", 128, values=0), qop("e4m3", 128, values=0, bs=S2), 8, 0, 768, 512, o=0, offs=0))
+    add("gqf8-err-K0", gqf8(*blk, 8, 4096, 768, 0))
+    add("gqf8-err-K0-tensor", gqf8(tens("e4m3"), tens("e4m3", S2 + 4), 8, 4096, 768, 0))
+    for tag in ("auto", "2sm_n256", "2sm_n128", "1sm_n128", "2sm_m512", "2sm_n224", "simt", "bogus"):
+        for epi in ("tma", "direct", "bogus"):
+            opts = {"gemm.variant": tag, "gemm.epilogue": epi}
+            add(f"gqf8-variant={tag}-epi={epi}", gqf8(*blk, 64, 32768, 768, 512, options=opts))
+    for val in ("on", "3", "bogus"):
+        add(f"gqf8-splitk={val}", gqf8(*blk, 64, 32768, 768, 512, options={"gemm.split_k": val}))
+    add("gqf8-misaligned-lhs", gqf8(qop("e4m3", 128, values=A + 8), qop("e4m3", 128, bs=S2), 8, 4096, 768, 512))
+    add("gqf8-misaligned-rhs", gqf8(qop("e4m3", 128), qop("e4m3", 128, values=B + 1, bs=S2), 8, 4096, 768, 512))
+    add("gqf8-k-not-16", gqf8(tens("e4m3"), tens("e5m2", S2 + 4), 8, 4096, 768, 200))
+    add("gqf8-k-not-16-G1", gqf8(tens("e4m3"), tens("e5m2", S2 + 4), 1, 4096, 768, 200))
+    add("gqf8-err-null-lhs", gqf8(None, qop("e4m3", 128, bs=S2), 8, 4096, 768, 512))
+    add("gqf8-err-null-rhs", gqf8(qop("e4m3", 128), None, 8, 4096, 768, 512))
+    add("gqf8-err-G1025", gqf8(*blk, 1025, 65536, 256, 256))
+    add("gqf8-err-G1025-empty", gqf8(*blk, 1025, 0, 256, 256))
+    add("gqf8-err-T-2^31", gqf8(*blk, 8, BIG, 768, 512))
+    add("gqf8-err-N-2^31", gqf8(*blk, 8, 4096, BIG, 512))
+    add("gqf8-err-K-2^31", gqf8(tens("e4m3"), tens("e4m3", S2 + 4), 8, 4096, 768, BIG))
+    for v in ("q8s", "q4f"):
+        add(f"gqf8-err-int-{v}-lhs", gqf8(qop(v, 128), qop("e4m3", 128, bs=S2), 8, 4096, 768, 512))
+        add(f"gqf8-err-int-{v}-rhs", gqf8(qop("e4m3", 128), qop(v, 128, bs=S2), 8, 4096, 768, 512))
+    add("gqf8-err-e2m1", gqf8(qop("e2m1", 32, "ue8m0"), qop("e4m3", 32, bs=S2), 8, 4096, 768, 512))
+    add("gqf8-err-e2m1-rhs", gqf8(qop("e4m3", 32), qop("e2m1", 32, "ue8m0", bs=S2), 8, 4096, 768, 512))
+    add("gqf8-err-block16", gqf8(qop("e4m3", 16), qop("e4m3", 16, bs=S2), 8, 4096, 768, 512))
+    add("gqf8-err-k-block", gqf8(qop("e4m3", 128), qop("e4m3", 128, bs=S2), 8, 4096, 768, 96))
+    add("gqf8-err-null-block-scales", gqf8(qop("e4m3", 128, bs=0), qop("e4m3", 128, bs=S2), 8, 4096, 768, 512))
+    add("gqf8-err-out-i32", gqf8(*blk, 8, 4096, 768, 512, "i32"))
+    add("gqf8-err-null-offs", gqf8(*blk, 8, 4096, 768, 512, offs=0))
+    add("gqf8-err-misaligned-offs", gqf8(*blk, 8, 4096, 768, 512, offs=OFFS + 2))
+    add("gqf8-err-null-out", gqf8(*blk, 8, 4096, 768, 512, o=0))
+    add("gqf8-err-null-values", gqf8(qop("e4m3", 128, values=0), qop("e4m3", 128, bs=S2), 8, 4096, 768, 512))
+    add("gqf8-err-misaligned-out", gqf8(*blk, 8, 4096, 768, 512, "f32", o=O + 2))
+    add("gqf8-err-tiles", gqf8(*blk, 1024, (1 << 31) - 1, (1 << 31) - 1, 128))
+    add("gqf8-err2-groups-and-dtype", gqf8(qop("q8s", 128), qop("e4m3", 128, bs=S2), 1025, 4096, 768, 512))
+    add("gqf8-err2-extent-and-dtype", gqf8(qop("q8s", 128), qop("e4m3", 128, bs=S2), 8, BIG, 768, 512))
+    add("gqf8-err2-offs-and-ptr", gqf8(*blk, 8, 4096, 768, 512, offs=0, o=0))
+    add("gqf8-err2-misaligned-offs-and-out", gqf8(*blk, 8, 4096, 768, 512, offs=OFFS + 2, o=O + 2))
+    add("gqf8-err2-out-and-k0", gqf8(*blk, 8, 4096, 768, 0, "i32"))
+    add("gqf8-err2-staged-and-variant", gqf8(qop("e4m3", 128, values=A + 8), qop("e4m3", 128, bs=S2), 8, 4096, 768, 512,
+                                             options={"gemm.variant": "bogus"}))
+    add("gqf8-err2-staged-and-epilogue", gqf8(tens("e4m3"), tens("e4m3", S2 + 4), 8, 4096, 768, 200, options={"gemm.epilogue": "bogus"}))
+    add("gqf8-err2-tiles-and-epilogue", gqf8(*blk, 1024, (1 << 31) - 1, (1 << 31) - 1, 128, options={"gemm.epilogue": "bogus"}))
     return out
 
 

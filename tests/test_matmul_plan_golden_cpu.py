@@ -1,4 +1,5 @@
-"""CPU: the matmul entry points (b200_matmul, _fused, _mixed, _scaled, _quantized and _grouped) replayed through a dry-run
+"""CPU: the matmul entry points (b200_matmul, _fused, _mixed, _scaled, _quantized, _quantized_fp8, _grouped and
+_grouped_quantized_fp8) replayed through a dry-run
 planning context against golden/matmul_plan_golden.json.gz: the returned status, the full error message and the full plan
 text must be byte-identical to the recorded ones.  It pins the host-side checks, their order, the messages, routing, operand
 staging, variant and stream-K choices, tensor maps and launches of the GEMM code; golden/make_matmul_plan_golden.py writes it
