@@ -19,6 +19,7 @@ F32, F16, BF16, U32, I32, F64, I64, U64, U8, I8, F8E4M3, F8E5M2, F4E2M1X2, UE8M0
 REDUCE_SUM, REDUCE_PROD, REDUCE_MAX, REDUCE_MIN, REDUCE_ARGMAX, REDUCE_ARGMIN, REDUCE_MEAN = range(7)
 COMM_SUM, COMM_MEAN = 0, 1
 QV_Q8F, QV_E5M2, QV_E4M3, QV_Q4F, QV_E2M1, QV_Q2F, QV_Q8S, QV_Q4S, QV_Q2S = range(9)
+MOE_SOFTMAX, MOE_SIGMOID = 0, 1
 UNIQUE_ID_BYTES = 128
 IPC_HANDLE_BYTES = 64
 
@@ -69,6 +70,13 @@ class AttentionVarlenArgs(C.Structure):
 class QuantScheme(C.Structure):
     """b200_quant_scheme: value (b200_quant_value), block, block_scale (b200_dtype), tensor_scale (0 / 1)."""
     _fields_ = [("value", C.c_int32), ("block", C.c_int32), ("block_scale", C.c_int32), ("tensor_scale", C.c_int32)]
+
+
+class MoeRouteArgs(C.Structure):
+    """b200_moe_route_args: k, score (MOE_SOFTMAX / MOE_SIGMOID), renormalize (0 / 1), n_group and topk_group (n_group <= 1: no
+    group limit), scale."""
+    _fields_ = [("k", C.c_int32), ("score", C.c_int32), ("renormalize", C.c_int32), ("n_group", C.c_int32),
+                ("topk_group", C.c_int32), ("scale", C.c_float)]
 
 
 class Props(C.Structure):
@@ -136,6 +144,12 @@ SIGNATURES = {
                                             C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64]),
     "b200_matmul_grouped_quantized_fp8": (C.c_int, [_vp, _vp, C.POINTER(QuantOperand), C.POINTER(QuantOperand), C.c_uint64,
                                                     C.c_uint64, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64]),
+    "b200_moe_route": (C.c_int, [_vp, _vp, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64,
+                                 C.POINTER(MoeRouteArgs), C.c_uint64, C.c_uint64]),
+    "b200_moe_plan": (C.c_int, [_vp, _vp] + [C.c_uint64] * 7),
+    "b200_moe_permute": (C.c_int, [_vp, _vp] + [C.c_uint64] * 8),
+    "b200_moe_combine": (C.c_int, [_vp, _vp, C.c_int, C.c_int] + [C.c_uint64] * 10),
+    "b200_moe_combine_backward": (C.c_int, [_vp, _vp, C.c_int, C.c_int] + [C.c_uint64] * 13),
     "b200_conv2d": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, _u64p, _u64p, C.c_uint64, _u64p, _u64p, C.c_uint64, _u64p,
                               _u64p, C.POINTER(Conv2dArgs), C.POINTER(Epilogue)]),
     "b200_conv2d_backward_data": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_uint64, _u64p, _u64p, C.c_uint64, _u64p, _u64p,

@@ -79,6 +79,8 @@ extern const unsigned char b200_cubin_gemm_qf8[];
 extern const unsigned char b200_cubin_gemm_qf8_end[];
 extern const unsigned char b200_cubin_gemm_grouped_qf8[];
 extern const unsigned char b200_cubin_gemm_grouped_qf8_end[];
+extern const unsigned char b200_cubin_moe[];
+extern const unsigned char b200_cubin_moe_end[];
 }
 
 // ================================================================================================ errors
@@ -351,12 +353,13 @@ static int get_func(b200_ctx* c, const std::string& name, CUfunction* out) {
   if (it != c->funcs.end()) { *out = it->second; return B200_OK; }
   // modules are loaded in the order gemm, reduce, aux, gemm_b, gemm_c, quant, gemm_q, quant_mm, gemm_conv, gemm_convbwd,
   // conv_grouped, gemm_conv3d, gemm_convt, attention, attention_bwd, attention_kv, attention_varlen, attention_varlen_bwd,
-  // attention_kv_fp8, attention_paged, attention_paged_fp8, gemm_grouped, gemm_qf8, gemm_grouped_qf8; the kernel name says where a
+  // attention_kv_fp8, attention_paged, attention_paged_fp8, gemm_grouped, gemm_qf8, gemm_grouped_qf8, moe; the kernel name says where a
   // kernel lives (no failing lookups, which API-level tools such as compute-sanitizer would report)
   auto starts = [&](const char* pfx) { return name.rfind(pfx, 0) == 0; };
   auto has = [&](const char* part) { return name.find(part) != std::string::npos; };
   const bool tc_gemm = starts("gemm_") && name != "gemm_simt_strided" && name != "gemm_scaled_simt";
   const size_t home = name == "conv3d_dgrad_weights" ? 2
+                      : starts("moe_") ? 24
                       : starts("gemm_grouped_qf8_") ? 23
                       : starts("gemm_qf8_") ? 22
                       : starts("gemm_grouped_") ? 21
@@ -418,7 +421,8 @@ extern "C" int b200_get_cubin(const char* name, const void** image, size_t* size
   else if (!strcmp(name, "gemm_grouped")) { b = b200_cubin_gemm_grouped; e = b200_cubin_gemm_grouped_end; }
   else if (!strcmp(name, "gemm_qf8")) { b = b200_cubin_gemm_qf8; e = b200_cubin_gemm_qf8_end; }
   else if (!strcmp(name, "gemm_grouped_qf8")) { b = b200_cubin_gemm_grouped_qf8; e = b200_cubin_gemm_grouped_qf8_end; }
-  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd|conv_grouped|gemm_conv3d|gemm_convt|attention|attention_bwd|attention_kv|attention_varlen|attention_varlen_bwd|attention_kv_fp8|attention_paged|attention_paged_fp8|gemm_grouped|gemm_qf8|gemm_grouped_qf8)", name);
+  else if (!strcmp(name, "moe")) { b = b200_cubin_moe; e = b200_cubin_moe_end; }
+  else return fail(B200_ERR_INVALID_ARG, "get_cubin: unknown image '%s' (gemm|gemm_b|gemm_c|reduce|aux|quant|gemm_q|quant_mm|gemm_conv|gemm_convbwd|conv_grouped|gemm_conv3d|gemm_convt|attention|attention_bwd|attention_kv|attention_varlen|attention_varlen_bwd|attention_kv_fp8|attention_paged|attention_paged_fp8|gemm_grouped|gemm_qf8|gemm_grouped_qf8|moe)", name);
   *image = b;
   *size = static_cast<size_t>(e - b);
   return B200_OK;
@@ -489,7 +493,8 @@ extern "C" int b200_init(int device, b200_ctx** out) {
       (rc = load_module(c, b200_cubin_attention_paged_fp8, b200_cubin_attention_paged_fp8_end, "attention_paged_fp8")) ||
       (rc = load_module(c, b200_cubin_gemm_grouped, b200_cubin_gemm_grouped_end, "gemm_grouped")) ||
       (rc = load_module(c, b200_cubin_gemm_qf8, b200_cubin_gemm_qf8_end, "gemm_qf8")) ||
-      (rc = load_module(c, b200_cubin_gemm_grouped_qf8, b200_cubin_gemm_grouped_qf8_end, "gemm_grouped_qf8"))) {
+      (rc = load_module(c, b200_cubin_gemm_grouped_qf8, b200_cubin_gemm_grouped_qf8_end, "gemm_grouped_qf8")) ||
+      (rc = load_module(c, b200_cubin_moe, b200_cubin_moe_end, "moe"))) {
     for (CUmodule m : c->modules) g_drv.cuModuleUnload_p(m);
     g_drv.cuDevicePrimaryCtxRelease_p(c->dev);
     return bail(rc);
@@ -2987,6 +2992,204 @@ extern "C" int b200_matmul_grouped_quantized_fp8(b200_ctx* c, b200_stream s, con
   p.b_bmul = groups > 1 ? 1u : 0u;   // a_bmul stays 0: the lhs is one batch, whatever the group
   if ((rc = gemm_quant_params(c, g, v, true, groups == 1, &ta_sc, &tb_sc, &p))) return rc;
   return grouped_launch(c, st, f, pl, smem, osz, offs, groups, t, false, &p, {&ta, &tb, &ta_sc, &tb_sc});
+}
+
+// ================================================================================================ mixture-of-experts routing
+// Kernels in csrc/moe.cu.  Each entry checks its arguments, writes one "moe ..." plan line, and launches.
+static void moe_plan_line(b200_ctx* c, const char* fmt, ...) {
+  if (!c->dry) return;
+  char line[200];
+  va_list ap;
+  va_start(ap, fmt);
+  vsnprintf(line, sizeof(line), fmt, ap);
+  va_end(ap);
+  c->plan += line;
+}
+
+extern "C" int b200_moe_route(b200_ctx* c, b200_stream s, b200_dtype logits_dtype, b200_dptr logits, uint64_t t, uint64_t e,
+                              uint64_t logits_stride, b200_dptr bias, const b200_moe_route_args* a, b200_dptr ids, b200_dptr weights) {
+  CTX_ENTER(c);
+  typedef unsigned long long ull;
+  if (!a) return fail(B200_ERR_INVALID_ARG, "moe_route: null args");
+  if (!dt_tag(logits_dtype)) return fail(B200_ERR_UNSUPPORTED, "moe_route: logits dtype %d unsupported (f32, bf16, f16)", (int)logits_dtype);
+  if (e == 0) return fail(B200_ERR_INVALID_ARG, "moe_route: no experts (e = 0)");
+  if (e > (uint64_t)kMoeMaxExperts) return fail(B200_ERR_UNSUPPORTED, "moe_route: %llu experts exceed the limit of %d", (ull)e, kMoeMaxExperts);
+  if (t >= (1ull << 31)) return fail(B200_ERR_UNSUPPORTED, "moe_route: t must be below 2^31");
+  if (a->k < 1 || (uint64_t)a->k > std::min<uint64_t>(e, kMoeMaxK))
+    return fail(B200_ERR_INVALID_ARG, "moe_route: k = %d outside [1, min(e, %d)]", a->k, kMoeMaxK);
+  if (a->score != B200_MOE_SOFTMAX && a->score != B200_MOE_SIGMOID) return fail(B200_ERR_INVALID_ARG, "moe_route: unknown score %d", a->score);
+  if (a->n_group > 1) {
+    const uint64_t g = (uint64_t)a->n_group;
+    if (e % g || e / g < 2)
+      return fail(B200_ERR_INVALID_ARG, "moe_route: %llu experts do not split into %d groups of at least 2", (ull)e, a->n_group);
+    if (a->topk_group < 1 || a->topk_group > a->n_group || (uint64_t)a->topk_group * (e / g) < (uint64_t)a->k)
+      return fail(B200_ERR_INVALID_ARG, "moe_route: topk_group %d of %d groups cannot hold k = %d experts", a->topk_group, a->n_group, a->k);
+  } else if (a->n_group < 0) {
+    return fail(B200_ERR_INVALID_ARG, "moe_route: n_group %d is negative", a->n_group);
+  }
+  if (logits_stride < e) return fail(B200_ERR_INVALID_ARG, "moe_route: logits stride %llu below e = %llu", (ull)logits_stride, (ull)e);
+  if (t == 0) return B200_OK;
+  const size_t esz = dtype_size(logits_dtype);
+  if (!logits || !ids || !weights) return fail(B200_ERR_INVALID_ARG, "moe_route: null device pointer");
+  if (logits % esz || ids % 4 || weights % 4 || bias % 4) return fail(B200_ERR_INVALID_ARG, "moe_route: misaligned logits, bias, ids or weights");
+  MoeRouteParams p;
+  memset(&p, 0, sizeof(p));
+  p.logits = logits; p.bias = bias; p.ids = ids; p.weights = weights;
+  p.T = t; p.stride = logits_stride;
+  p.E = (uint32_t)e; p.k = (uint32_t)a->k; p.score = (uint32_t)a->score; p.renorm = a->renormalize ? 1u : 0u;
+  p.n_group = a->n_group > 1 ? (uint32_t)a->n_group : 0u; p.topk_group = p.n_group ? (uint32_t)a->topk_group : 0u;
+  p.scale = a->scale;
+  moe_plan_line(c, "moe route t=%llu e=%llu k=%d score=%s bias=%d groups=%u/%u\n", (ull)t, (ull)e, a->k,
+                a->score == B200_MOE_SIGMOID ? "sigmoid" : "softmax", bias ? 1 : 0, p.topk_group, p.n_group);
+  CUfunction f;
+  int rc = get_func(c, std::string("moe_route_") + dt_tag(logits_dtype), &f);
+  if (rc) return rc;
+  void* args[] = {&p};
+  const unsigned smem = (unsigned)(kMoeRouteWarps * (e + e / 2) * 4);
+  return launch(c, f, (unsigned)((t + kMoeRouteWarps - 1) / kMoeRouteWarps), 1, 1, kMoeRouteWarps * 32, smem, 1, resolve_stream(c, s), args);
+}
+
+extern "C" int b200_moe_plan(b200_ctx* c, b200_stream s, b200_dptr ids, uint64_t t, uint64_t k, uint64_t e, b200_dptr offs,
+                             b200_dptr row_of, b200_dptr slot_of) {
+  CTX_ENTER(c);
+  typedef unsigned long long ull;
+  if (e == 0) return fail(B200_ERR_INVALID_ARG, "moe_plan: no experts (e = 0)");
+  if (e > (uint64_t)kMoeMaxExperts) return fail(B200_ERR_UNSUPPORTED, "moe_plan: %llu experts exceed the limit of %d", (ull)e, kMoeMaxExperts);
+  if (t >= (1ull << 31) || k >= (1ull << 31) || t * k >= (1ull << 31)) return fail(B200_ERR_UNSUPPORTED, "moe_plan: t * k must be below 2^31");
+  const uint64_t n = t * k;
+  if (!offs || (n && (!ids || !row_of || !slot_of))) return fail(B200_ERR_INVALID_ARG, "moe_plan: null device pointer");
+  if (offs % 4 || ids % 4 || row_of % 4 || slot_of % 4) return fail(B200_ERR_INVALID_ARG, "moe_plan: misaligned ids, offs, row_of or slot_of");
+  // 256 slots per warp, widened in steps of 256 once that would take more than kMoePlanMaxCtas CTAs: the scanned [E][CTAs]
+  // table stays within 4 MiB and the single-CTA scan within 1024 entries per thread, whatever t * k
+  const uint64_t chunk = kMoePlanWarps * kMoePlanWarpSlots, steps = std::max<uint64_t>(1, (n + chunk * kMoePlanMaxCtas - 1) / (chunk * kMoePlanMaxCtas));
+  const uint64_t ctas = (n + chunk * steps - 1) / (chunk * steps);
+  CUstream st = resolve_stream(c, s);
+  Scratch scr(c, st);
+  MoePlanParams p;
+  memset(&p, 0, sizeof(p));
+  p.ids = ids; p.offs = offs; p.row_of = row_of; p.slot_of = slot_of;
+  p.n = (uint32_t)n; p.E = (uint32_t)e; p.ctas = (uint32_t)ctas; p.warp_slots = (uint32_t)(kMoePlanWarpSlots * steps);
+  moe_plan_line(c, "moe plan slots=%llu e=%llu ctas=%llu warp_slots=%u\n", (ull)n, (ull)e, (ull)ctas, p.warp_slots);
+  int rc = B200_OK;
+  CUdeviceptr hist = 0;
+  if (ctas && (rc = scr.alloc(e * ctas * 4, &hist))) return rc;
+  p.hist = hist;
+  const unsigned smem = (unsigned)(kMoePlanWarps * e * 4);
+  void* args[] = {&p};
+  CUfunction f;
+  if (ctas && ((rc = get_func(c, "moe_plan_histogram", &f)) ||
+               (rc = launch(c, f, (unsigned)ctas, 1, 1, kMoePlanWarps * 32, smem, 1, st, args))))
+    return rc;
+  if ((rc = get_func(c, "moe_plan_scan", &f)) || (rc = launch(c, f, 1, 1, 1, kMoeScanThreads, 0, 1, st, args))) return rc;
+  if (ctas && ((rc = get_func(c, "moe_plan_scatter", &f)) ||
+               (rc = launch(c, f, (unsigned)ctas, 1, 1, kMoePlanWarps * 32, smem, 1, st, args))))
+    return rc;
+  return B200_OK;
+}
+
+extern "C" int b200_moe_permute(b200_ctx* c, b200_stream s, b200_dptr src, uint64_t src_pitch, b200_dptr slot_of, uint64_t t, uint64_t k,
+                                b200_dptr dst, uint64_t dst_pitch, uint64_t row_bytes) {
+  CTX_ENTER(c);
+  typedef unsigned long long ull;
+  if (t >= (1ull << 31) || k >= (1ull << 31) || t * k >= (1ull << 31)) return fail(B200_ERR_UNSUPPORTED, "moe_permute: t * k must be below 2^31");
+  if (row_bytes >= (1ull << 31)) return fail(B200_ERR_UNSUPPORTED, "moe_permute: row_bytes must be below 2^31");
+  if (src_pitch < row_bytes || dst_pitch < row_bytes)
+    return fail(B200_ERR_INVALID_ARG, "moe_permute: pitches (%llu, %llu) below row_bytes %llu", (ull)src_pitch, (ull)dst_pitch, (ull)row_bytes);
+  const uint64_t rows = t * k;
+  if (rows == 0 || row_bytes == 0) return B200_OK;
+  if (!src || !dst || !slot_of) return fail(B200_ERR_INVALID_ARG, "moe_permute: null device pointer");
+  if (slot_of % 4) return fail(B200_ERR_INVALID_ARG, "moe_permute: misaligned slot_of");
+  const uint64_t all = src | dst | src_pitch | dst_pitch | row_bytes;
+  const int v = all % 16 == 0 ? 16 : all % 4 == 0 ? 4 : 1;
+  MoePermuteParams p;
+  memset(&p, 0, sizeof(p));
+  p.src = src; p.dst = dst; p.slot_of = slot_of;
+  p.src_pitch = src_pitch; p.dst_pitch = dst_pitch; p.row_bytes = row_bytes;
+  p.rows = rows; p.k = (uint32_t)k;
+  moe_plan_line(c, "moe permute rows=%llu row_bytes=%llu vec=%d\n", (ull)rows, (ull)row_bytes, v);
+  CUfunction f;
+  int rc = get_func(c, "moe_permute_v" + std::to_string(v), &f);
+  if (rc) return rc;
+  void* args[] = {&p};
+  return launch(c, f, (unsigned)((rows + kMoePermuteWarps - 1) / kMoePermuteWarps), 1, 1, kMoePermuteWarps * 32, 0, 1,
+                resolve_stream(c, s), args);
+}
+
+// The checks both combine directions share: dtypes, extents, strides, pointers.  *empty: nothing to do.
+static int moe_combine_check(const char* what, b200_dtype a_dt, b200_dtype b_dt, uint64_t t, uint64_t k, uint64_t n,
+                             std::initializer_list<uint64_t> strides, std::initializer_list<b200_dptr> ptrs, bool* empty) {
+  typedef unsigned long long ull;
+  if (!dt_tag(a_dt) || !dt_tag(b_dt)) return fail(B200_ERR_UNSUPPORTED, "%s: dtypes %d, %d unsupported (f32, bf16, f16)", what, (int)a_dt, (int)b_dt);
+  if (t >= (1ull << 31) || n >= (1ull << 31) || k >= (1ull << 31) || t * k >= (1ull << 31))
+    return fail(B200_ERR_UNSUPPORTED, "%s: t, n and t * k must be below 2^31", what);
+  for (uint64_t st : strides)
+    if (st < n) return fail(B200_ERR_INVALID_ARG, "%s: row stride %llu below n = %llu", what, (ull)st, (ull)n);
+  *empty = t == 0 || n == 0;
+  if (*empty) return B200_OK;
+  for (b200_dptr p : ptrs)
+    if (!p) return fail(B200_ERR_INVALID_ARG, "%s: null device pointer", what);
+  return B200_OK;
+}
+
+static int moe_combine_launch(b200_ctx* c, CUstream st, const std::string& name, unsigned grid_x, unsigned grid_y, unsigned smem,
+                              MoeCombineParams* p) {
+  CUfunction f;
+  int rc = get_func(c, name, &f);
+  if (rc) return rc;
+  if (smem > 48 * 1024 && !c->dry) CU_CHECK(g_drv.cuFuncSetAttribute_p(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem));
+  void* args[] = {p};
+  return launch(c, f, grid_x, grid_y, 1, kMoeThreads, smem, 1, st, args);
+}
+
+extern "C" int b200_moe_combine(b200_ctx* c, b200_stream s, b200_dtype ys_dtype, b200_dtype y_dtype, b200_dptr ys, uint64_t rows,
+                                uint64_t ys_stride, b200_dptr weights, b200_dptr row_of, uint64_t t, uint64_t k, uint64_t n, b200_dptr y,
+                                uint64_t y_stride) {
+  CTX_ENTER(c);
+  typedef unsigned long long ull;
+  bool empty = false;
+  int rc = moe_combine_check("moe_combine", ys_dtype, y_dtype, t, k, n, {ys_stride, y_stride}, {y, ys, row_of}, &empty);
+  if (rc) return rc;
+  const uint64_t chunks = (n + kMoeThreads * 8 - 1) / (kMoeThreads * 8);   // grid.y
+  if (chunks > 65535) return fail(B200_ERR_UNSUPPORTED, "moe_combine: n = %llu exceeds %d", (ull)n, 65535 * kMoeThreads * 8);
+  if (empty) return B200_OK;
+  const size_t ysz = dtype_size(ys_dtype), osz = dtype_size(y_dtype);
+  if (ys % ysz || y % osz || row_of % 4 || weights % 4) return fail(B200_ERR_INVALID_ARG, "moe_combine: misaligned ys, y, row_of or weights");
+  MoeCombineParams p;
+  memset(&p, 0, sizeof(p));
+  p.ys = ys; p.weights = weights; p.row_of = row_of; p.y = y;
+  p.ys_stride = ys_stride; p.y_stride = y_stride; p.rows = rows;
+  p.T = (uint32_t)t; p.k = (uint32_t)k; p.N = (uint32_t)n;
+  p.vec = (ys % 16 == 0 && y % 16 == 0 && (ys_stride * ysz) % 16 == 0 && (y_stride * osz) % 16 == 0 && n % 8 == 0) ? 1u : 0u;
+  moe_plan_line(c, "moe combine t=%llu k=%llu n=%llu rows=%llu weights=%d vec=%u\n", (ull)t, (ull)k, (ull)n, (ull)rows, weights ? 1 : 0, p.vec);
+  return moe_combine_launch(c, resolve_stream(c, s), std::string("moe_combine_") + dt_tag(ys_dtype) + "_" + dt_tag(y_dtype), (unsigned)t,
+                            (unsigned)chunks, 0, &p);
+}
+
+extern "C" int b200_moe_combine_backward(b200_ctx* c, b200_stream s, b200_dtype grad_dtype, b200_dtype ys_dtype, b200_dptr dy,
+                                         uint64_t dy_stride, b200_dptr ys, uint64_t rows, uint64_t ys_stride, b200_dptr weights,
+                                         b200_dptr row_of, uint64_t t, uint64_t k, uint64_t n, b200_dptr d_ys, uint64_t d_ys_stride,
+                                         b200_dptr d_w) {
+  CTX_ENTER(c);
+  typedef unsigned long long ull;
+  bool empty = false;
+  int rc = moe_combine_check("moe_combine_backward", grad_dtype, ys_dtype, t, k, n, {dy_stride, ys_stride, d_ys_stride},
+                             {dy, ys, d_ys, weights, row_of, d_w}, &empty);
+  if (rc) return rc;
+  if (n > (uint64_t)kMoeBwdMaxN) return fail(B200_ERR_UNSUPPORTED, "moe_combine_backward: n = %llu exceeds %d", (ull)n, kMoeBwdMaxN);
+  if (empty || k == 0) return B200_OK;
+  const size_t gsz = dtype_size(grad_dtype), ysz = dtype_size(ys_dtype);
+  if (dy % gsz || d_ys % gsz || ys % ysz || weights % 4 || row_of % 4 || d_w % 4)
+    return fail(B200_ERR_INVALID_ARG, "moe_combine_backward: misaligned dy, ys, d_ys, weights, row_of or d_w");
+  MoeCombineParams p;
+  memset(&p, 0, sizeof(p));
+  p.ys = ys; p.weights = weights; p.row_of = row_of; p.y = dy; p.d_ys = d_ys; p.d_w = d_w;
+  p.ys_stride = ys_stride; p.y_stride = dy_stride; p.d_ys_stride = d_ys_stride; p.rows = rows;
+  p.T = (uint32_t)t; p.k = (uint32_t)k; p.N = (uint32_t)n;
+  p.vec = (dy % 16 == 0 && ys % 16 == 0 && d_ys % 16 == 0 && (dy_stride * gsz) % 16 == 0 && (ys_stride * ysz) % 16 == 0 &&
+           (d_ys_stride * gsz) % 16 == 0 && n % 8 == 0) ? 1u : 0u;
+  moe_plan_line(c, "moe combine_backward t=%llu k=%llu n=%llu rows=%llu vec=%u\n", (ull)t, (ull)k, (ull)n, (ull)rows, p.vec);
+  return moe_combine_launch(c, resolve_stream(c, s), std::string("moe_combine_bwd_") + dt_tag(grad_dtype) + "_" + dt_tag(ys_dtype),
+                            (unsigned)t, 1, (unsigned)(n * 4), &p);
 }
 
 // ------------------------------------------------------------------------------------------------ convolution

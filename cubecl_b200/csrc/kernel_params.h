@@ -552,3 +552,52 @@ struct QuantWidenParams {
   uint64_t rows, K, pitch;
   uint32_t bits, pad;
 };
+
+// ================================================================================================ moe.cu
+// Mixture-of-experts routing (capi.cpp: b200_moe_*).  Index arrays are compact i32: ids / row_of [T, k], slot_of [T * k].
+struct MoeRouteParams {
+  uint64_t logits;        // [T, E] in the logits dtype, element (t, e) at logits + t * stride + e
+  uint64_t bias;          // f32 [E] selection bias, or 0
+  uint64_t ids, weights;  // i32 / f32 [T, k]
+  uint64_t T, stride;
+  uint32_t E, k, score, renorm;  // score: b200_moe_score
+  uint32_t n_group, topk_group;  // n_group <= 1: no group limit
+  float scale;
+  uint32_t pad;
+};
+
+struct MoePlanParams {
+  uint64_t ids, offs, row_of, slot_of;
+  uint64_t hist;          // i32 [E][ctas]: each CTA's count per expert, then (moe_plan_scan) the first row of its run
+  uint32_t n;             // T * k slots
+  uint32_t E, ctas;
+  uint32_t warp_slots;    // consecutive slots per warp (a multiple of kMoePlanWarpSlots); a CTA owns 8 warps' worth
+};
+
+struct MoePermuteParams {
+  uint64_t src, dst, slot_of;
+  uint64_t src_pitch, dst_pitch, row_bytes;  // bytes
+  uint64_t rows;          // T * k
+  uint32_t k, pad;
+};
+
+// b200_moe_combine (ys -> y) and b200_moe_combine_backward (dy, ys -> d_ys, d_w); strides in elements
+struct MoeCombineParams {
+  uint64_t ys, weights, row_of, y;
+  uint64_t d_ys, d_w;
+  uint64_t ys_stride, y_stride, d_ys_stride;  // y / y_stride are dy and its stride in the backward
+  uint64_t rows;          // rows of ys (and d_ys); row_of entries outside [0, rows) are dropped slots
+  uint32_t T, k, N;
+  uint32_t vec;           // 1: every row start is 16-byte aligned and N % 8 == 0 (8-element vector access)
+};
+
+constexpr int kMoeMaxExperts = 1024;
+constexpr int kMoeMaxK = 32;
+constexpr int kMoeRouteWarps = 4;      // tokens per route CTA, one warp each
+constexpr int kMoePlanWarps = 8;       // a plan CTA: 8 warps, each owning warp_slots consecutive slots
+constexpr int kMoePlanWarpSlots = 256; // the least warp_slots; more once T * k needs over kMoePlanMaxCtas CTAs
+constexpr int kMoePlanMaxCtas = 1024;  // bounds the [E][CTAs] table: at most 4 MiB, 1024 entries per scan thread
+constexpr int kMoeScanThreads = 1024;
+constexpr int kMoePermuteWarps = 8;    // rows per permute CTA, one warp each
+constexpr int kMoeThreads = 256;       // combine / combine-backward CTA; a thread owns 8 consecutive columns per step
+constexpr int kMoeBwdMaxN = 32768;     // the backward stages dy[t] as f32 in shared memory

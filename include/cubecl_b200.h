@@ -395,6 +395,88 @@ int b200_matmul_grouped_quantized_fp8(b200_ctx* ctx, b200_stream s, const b200_q
                                       b200_dptr offs, uint64_t groups, b200_dtype out_dtype, b200_dptr out, uint64_t t,
                                       uint64_t n, uint64_t k);
 
+/* ---- mixture-of-experts routing: top-k gating, the expert-sorted dispatch plan, token permute and weighted combine ----------
+ * A layer on these calls and the grouped matmuls: ids, weights = route(logits); offs, row_of, slot_of = plan(ids);
+ * xs = permute(x, slot_of); ys = grouped matmuls(xs, offs); y = combine(ys, weights, row_of).  Index arrays are compact i32
+ * device arrays: ids and row_of [T, k] (slot t * k + j is token t's j-th choice), slot_of [T * k], offs [E].  Row strides are in
+ * elements and must be at least the row length; columns are unit-stride.  All five calls are stream-ordered, never
+ * synchronise with the host (a whole layer can be captured in a graph), take temporaries from the pool, use no atomics and
+ * are bitwise reproducible from run to run.  A zero extent (T, k or N) is a no-op, except that plan then writes offs = 0. */
+typedef enum b200_moe_score { B200_MOE_SOFTMAX = 0, B200_MOE_SIGMOID = 1 } b200_moe_score;
+typedef struct b200_moe_route_args {
+  int32_t k;             /* experts per token, 1 <= k <= min(E, 32) */
+  int32_t score;         /* b200_moe_score */
+  int32_t renormalize;   /* 1: the k weights are divided by their sum */
+  int32_t n_group;       /* 0 or 1: no group limit; > 1: group-limited routing over n_group groups of E / n_group experts */
+  int32_t topk_group;    /* groups that stay eligible (n_group > 1 only) */
+  float scale;           /* routed scaling factor applied last (1.0f: none) */
+} b200_moe_route_args;
+/* Top-k gating.  logits [t, e] (F32 / BF16 / F16, row stride logits_stride) and an optional f32 [e] selection bias (DeepSeek-V3's
+ * correction bias; 0 = none) -> ids i32 [t, k] and weights f32 [t, k].
+ *   Scores: s_e = softmax(l)_e over all E (f32, max-subtracted: expf(l_e - max) / sum, the sum in a fixed order), or
+ *   sigmoid(l_e) = 1 / (1 + expf(-l_e)).  expf is CUDA's (2 ulp).
+ *   Selection key: l_e without a bias (both scores are monotone in l, so ids are exact); with a bias rn(s_e + b_e).
+ *   Group-limited routing (n_group > 1) needs E % n_group == 0, E / n_group >= 2, 1 <= topk_group <= n_group and
+ *   topk_group * E / n_group >= k.  A group's score is rn(sum of its two largest keys); only the topk_group best groups stay
+ *   eligible.
+ *   Selection orders experts (and groups) by descending key, ties to the lower index, -0 equal to +0, NaN below -inf.
+ *   ids[t, j] is the j-th selected expert.  w_j = s_{e_j}; with renormalize w_j = w_j / (w_0 + w_1 + ... + w_{k-1}), summed in
+ *   j order; then w_j = rn(w_j * scale).  Mixtral / Qwen3-MoE: softmax, renormalize.  DeepSeek-V3: sigmoid, bias, n_group 8,
+ *   topk_group 4, k 8, scale 2.5.
+ * Errors: B200_ERR_INVALID_ARG for a null args, ids, weights or logits pointer, misaligned pointers, a logits stride below e,
+ * k outside [1, min(e, 32)], an unknown score and the group conditions above; B200_ERR_UNSUPPORTED for other logits dtypes,
+ * e > 1024 (the grouped matmul's group limit) and t >= 2^31.  e = 0 is B200_ERR_INVALID_ARG.  One moe_route_<dtype> launch. */
+int b200_moe_route(b200_ctx* ctx, b200_stream s, b200_dtype logits_dtype, b200_dptr logits, uint64_t t, uint64_t e,
+                   uint64_t logits_stride, b200_dptr bias, const b200_moe_route_args* args, b200_dptr ids, b200_dptr weights);
+/* The expert-sorted dispatch plan of ids [t, k] over e experts: a stable counting sort of the t * k slots by expert, exactly
+ * torch's argsort(ids.flatten(), stable=True) with the dropped slots removed.  Ids outside [0, e) are dropped (expert
+ * parallelism marks non-local experts that way).
+ *   offs i32 [e]: the cumulative ends b200_matmul_grouped* take unchanged (offs[e-1] = the kept count).
+ *   row_of i32 [t, k]: the sorted row of slot (t, j), or -1 when dropped.  Expert g's rows are its slots in increasing
+ *   t * k + j.
+ *   slot_of i32 [t * k]: the slot of each sorted row, -1 at and past the kept count.
+ * Errors: B200_ERR_INVALID_ARG for a null or misaligned pointer and e = 0; B200_ERR_UNSUPPORTED for e > 1024 and t * k >= 2^31.
+ * Launches: moe_plan_histogram (per-CTA counts of 2048 consecutive slots, or of a larger multiple of 2048 once t * k exceeds
+ * 2048 * 1024, so there are at most 1024 CTAs), moe_plan_scan (one CTA, a fixed-order scan over [e][CTAs]) and
+ * moe_plan_scatter (the stable re-rank); t * k = 0 launches moe_plan_scan alone.  One pooled temporary of e * CTAs * 4
+ * bytes (at most 4 MiB). */
+int b200_moe_plan(b200_ctx* ctx, b200_stream s, b200_dptr ids, uint64_t t, uint64_t k, uint64_t e, b200_dptr offs,
+                  b200_dptr row_of, b200_dptr slot_of);
+/* Gather rows into expert order: dst[r] = src[slot_of[r] / k] for every r < t * k with 0 <= slot_of[r] < t * k; other rows of
+ * dst are not written.  Rows are opaque: row_bytes bytes, src_pitch / dst_pitch bytes apart (at least row_bytes), so one call
+ * moves bf16 activations, fp8 codes or their block-scale rows.  16-byte access when both bases, both pitches and row_bytes
+ * are multiples of 16 (moe_permute_v16), else 4-byte (moe_permute_v4) or byte access (moe_permute_v1).
+ * fp8 recipe for b200_matmul_grouped_quantized_fp8: b200_quantize's per-row and per-block scales are row-local, so quantize x
+ * [t, K] once, then permute its codes (row_bytes K) and its block scales (row_bytes K / block * scale size) with the same
+ * slot_of; the result equals quantizing the permuted rows, bit for bit.  A per-tensor scale is shared and is not permuted.
+ * The permute's backward is b200_moe_combine with weights = 0: dx[t] = sum_j dxs[row_of[t, j]].
+ * Errors: B200_ERR_INVALID_ARG for a null pointer and a pitch below row_bytes; B200_ERR_UNSUPPORTED for t * k >= 2^31 and
+ * row_bytes >= 2^31.  row_bytes = 0 is a no-op.  One launch. */
+int b200_moe_permute(b200_ctx* ctx, b200_stream s, b200_dptr src, uint64_t src_pitch, b200_dptr slot_of, uint64_t t, uint64_t k,
+                     b200_dptr dst, uint64_t dst_pitch, uint64_t row_bytes);
+/* Weighted un-permute: y [t, n] from ys [rows, n] (rows: the extent of ys; slots whose row_of is outside [0, rows) are dropped).
+ * y[t, c] = RNE(acc_k) with acc_0 = +0 and acc_{j+1} = fma(weights[t, j], f32(ys[row_of[t, j], c]), acc_j) in increasing j,
+ * dropped slots skipped; weights = 0 makes each step acc_j + f32(ys[...]) (the permute's backward).  ys_dtype and y_dtype are
+ * F32 / BF16 / F16 independently.  Errors: B200_ERR_INVALID_ARG for a null or misaligned pointer and a stride below n;
+ * B200_ERR_UNSUPPORTED for other dtypes, t or t * k >= 2^31 and n > 65535 * 2048.  One moe_combine_<ys>_<y> launch (8-element
+ * vectors when every row start is 16-byte aligned and n % 8 == 0). */
+int b200_moe_combine(b200_ctx* ctx, b200_stream s, b200_dtype ys_dtype, b200_dtype y_dtype, b200_dptr ys, uint64_t rows,
+                     uint64_t ys_stride, b200_dptr weights, b200_dptr row_of, uint64_t t, uint64_t k, uint64_t n, b200_dptr y,
+                     uint64_t y_stride);
+/* Backward of b200_moe_combine with weights: dy [t, n] and d_ys [rows, n] in grad_dtype, ys [rows, n] in ys_dtype (both F32 /
+ * BF16 / F16), weights f32 and row_of i32 [t, k].
+ *   d_ys[row_of[t, j]] = RNE(rn(weights[t, j] * f32(dy[t]))) in grad_dtype; rows no slot references are not written.  row_of
+ *   must name each row at most once, as b200_moe_plan's does; a row named by two slots gets one of their values, which one
+ *   unspecified, and d_ys is then not reproducible.
+ *   d_w[t, j] (f32 [t, k]) = the f32 dot product of dy[t] and ys[row_of[t, j]] in a fixed order (each of 256 threads chains
+ *   fma over its columns in increasing order, then a fixed tree over the threads); +0 for a dropped slot.
+ * One moe_combine_bwd_<grad>_<ys> launch, one CTA per token, reading dy[t] once into shared memory.  Errors as
+ * b200_moe_combine, plus B200_ERR_UNSUPPORTED for n > 32768. */
+int b200_moe_combine_backward(b200_ctx* ctx, b200_stream s, b200_dtype grad_dtype, b200_dtype ys_dtype, b200_dptr dy,
+                              uint64_t dy_stride, b200_dptr ys, uint64_t rows, uint64_t ys_stride, b200_dptr weights,
+                              b200_dptr row_of, uint64_t t, uint64_t k, uint64_t n, b200_dptr d_ys, uint64_t d_ys_stride,
+                              b200_dptr d_w);
+
 /* ---- 2-D convolution (cubek's convolution kernels), an implicit GEMM on the wgmma kernel --------------------------------
  * out[n, oh, ow, co] = act(alpha * sum_{ky, kx, c} x[n, oh*sh - ph + ky*dh, ow*sw - pw + kx*dw, c] * w[co, ky, kx, c] + bias[co]).
  * Input outside x reads as zero; f32 accumulation; the epilogue is b200_epilogue (NULL = none).  x is [N, H, W, C] (NHWC), w is

@@ -669,6 +669,63 @@ inline void launch(ComputeClient& client, const TensorHandle& input, const Tenso
 }
 }  // namespace scan
 
+namespace moe {
+/// Mixture-of-experts routing; the contracts are those of b200_moe_* in cubecl_b200.h.  Index tensors are compact i32.
+/// Errors are deferred to client.sync().
+using RouteArgs = b200_moe_route_args;
+/// Top-k gating: logits [T, E] (unit column stride) -> ids i32 [T, k] and weights f32 [T, k]; bias: f32 [E] device pointer or 0.
+inline void route(ComputeClient& client, const TensorHandle& logits, b200_dptr bias, const RouteArgs& args, const TensorHandle& ids,
+                  const TensorHandle& weights) {
+  if (logits.shape.size() != 2) { client.defer("InvalidArgument: moe_route needs logits [T, E]"); return; }
+  const int rc = b200_moe_route(client.raw(), nullptr, static_cast<b200_dtype>(logits.dtype), logits.handle.ptr(), logits.shape[0],
+                                logits.shape[1], logits.strides[0], bias, &args, ids.handle.ptr(), weights.handle.ptr());
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+/// The expert-sorted dispatch plan of ids [T, k] over `experts`: offs [E], row_of [T, k], slot_of [T * k].
+inline void plan(ComputeClient& client, const TensorHandle& ids, uint64_t experts, const TensorHandle& offs, const TensorHandle& row_of,
+                 const TensorHandle& slot_of) {
+  if (ids.shape.size() != 2) { client.defer("InvalidArgument: moe_plan needs ids [T, k]"); return; }
+  const int rc = b200_moe_plan(client.raw(), nullptr, ids.handle.ptr(), ids.shape[0], ids.shape[1], experts, offs.handle.ptr(),
+                               row_of.handle.ptr(), slot_of.handle.ptr());
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+/// dst [T * k, C] = src [T, C] gathered into expert order by slot_of (any dtype, unit column stride).
+inline void permute(ComputeClient& client, const TensorHandle& src, const TensorHandle& slot_of, uint64_t k, const TensorHandle& dst) {
+  if (src.shape.size() != 2 || dst.shape.size() != 2 || src.dtype != dst.dtype) {
+    client.defer("InvalidArgument: moe_permute needs 2-D src and dst of one dtype");
+    return;
+  }
+  const uint64_t esz = dtype_size(src.dtype);
+  const int rc = b200_moe_permute(client.raw(), nullptr, src.handle.ptr(), src.strides[0] * esz, slot_of.handle.ptr(), src.shape[0], k,
+                                  dst.handle.ptr(), dst.strides[0] * esz, src.shape[1] * esz);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+/// y [T, N] = sum_j weights[t, j] * ys[row_of[t, j]]; weights 0 = the plain sum (the permute's backward).
+inline void combine(ComputeClient& client, const TensorHandle& ys, b200_dptr weights, const TensorHandle& row_of, const TensorHandle& y) {
+  if (ys.shape.size() != 2 || y.shape.size() != 2 || row_of.shape.size() != 2) {
+    client.defer("InvalidArgument: moe_combine needs ys [R, N], row_of [T, k] and y [T, N]");
+    return;
+  }
+  const int rc = b200_moe_combine(client.raw(), nullptr, static_cast<b200_dtype>(ys.dtype), static_cast<b200_dtype>(y.dtype),
+                                  ys.handle.ptr(), ys.shape[0], ys.strides[0], weights, row_of.handle.ptr(), row_of.shape[0],
+                                  row_of.shape[1], ys.shape[1], y.handle.ptr(), y.strides[0]);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+/// Gradients of combine: d_ys [R, N] (dy's dtype) and d_w f32 [T, k] from dy [T, N], ys, weights f32 [T, k] and row_of.
+inline void combine_backward(ComputeClient& client, const TensorHandle& dy, const TensorHandle& ys, b200_dptr weights,
+                             const TensorHandle& row_of, const TensorHandle& d_ys, b200_dptr d_w) {
+  if (dy.shape.size() != 2 || ys.shape.size() != 2 || d_ys.shape.size() != 2 || row_of.shape.size() != 2 || d_ys.dtype != dy.dtype) {
+    client.defer("InvalidArgument: moe_combine_backward needs dy [T, N], ys and d_ys [R, N] (d_ys in dy's dtype), row_of [T, k]");
+    return;
+  }
+  const int rc = b200_moe_combine_backward(client.raw(), nullptr, static_cast<b200_dtype>(dy.dtype), static_cast<b200_dtype>(ys.dtype),
+                                           dy.handle.ptr(), dy.strides[0], ys.handle.ptr(), ys.shape[0], ys.strides[0], weights,
+                                           row_of.handle.ptr(), row_of.shape[0], row_of.shape[1], ys.shape[1], d_ys.handle.ptr(),
+                                           d_ys.strides[0], d_w);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+}  // namespace moe
+
 namespace quant {
 /// QuantScheme (value, block level, per-tensor level); see b200_quantize in cubecl_b200.h for the contract.
 using Scheme = b200_quant_scheme;

@@ -905,6 +905,77 @@ impl Context {
         ))
     }
 
+    /// Mixture-of-experts top-k gating: `logits` [t, e] (F32 / BF16 / F16, row stride `logits_stride`) -> `ids` i32 [t, k] and
+    /// `weights` f32 [t, k]; `bias` is an f32 [e] selection bias or 0.  The contract is `b200_moe_route`'s in
+    /// include/cubecl_b200.h.
+    ///
+    /// # Safety
+    /// Every pointer must be a live device allocation of this context large enough for its extents.
+    #[allow(clippy::too_many_arguments)]
+    pub unsafe fn moe_route(
+        &mut self, stream: b200_stream, logits_dtype: DType, logits: b200_dptr, t: u64, e: u64, logits_stride: u64, bias: b200_dptr,
+        args: &sys::b200_moe_route_args, ids: b200_dptr, weights: b200_dptr,
+    ) -> Result<(), Error> {
+        check(sys::b200_moe_route(self.0, stream, logits_dtype as c_int, logits, t, e, logits_stride, bias, args, ids, weights))
+    }
+
+    /// The expert-sorted dispatch plan of `ids` i32 [t, k] over `e` experts: `offs` i32 [e] (what the grouped matmuls take),
+    /// `row_of` i32 [t, k] and `slot_of` i32 [t * k].  See `b200_moe_plan`.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::moe_route`].
+    #[allow(clippy::too_many_arguments)]
+    pub unsafe fn moe_plan(
+        &mut self, stream: b200_stream, ids: b200_dptr, t: u64, k: u64, e: u64, offs: b200_dptr, row_of: b200_dptr, slot_of: b200_dptr,
+    ) -> Result<(), Error> {
+        check(sys::b200_moe_plan(self.0, stream, ids, t, k, e, offs, row_of, slot_of))
+    }
+
+    /// Gather rows into expert order: dst[r] = src[slot_of[r] / k], rows of `row_bytes` bytes at byte pitches.  See
+    /// `b200_moe_permute`.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::moe_route`].
+    #[allow(clippy::too_many_arguments)]
+    pub unsafe fn moe_permute(
+        &mut self, stream: b200_stream, src: b200_dptr, src_pitch: u64, slot_of: b200_dptr, t: u64, k: u64, dst: b200_dptr,
+        dst_pitch: u64, row_bytes: u64,
+    ) -> Result<(), Error> {
+        check(sys::b200_moe_permute(self.0, stream, src, src_pitch, slot_of, t, k, dst, dst_pitch, row_bytes))
+    }
+
+    /// Weighted un-permute: y [t, n] = sum_j weights[t, j] * ys[row_of[t, j]] (`weights` 0: the plain sum).  See
+    /// `b200_moe_combine`.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::moe_route`].
+    #[allow(clippy::too_many_arguments)]
+    pub unsafe fn moe_combine(
+        &mut self, stream: b200_stream, ys_dtype: DType, y_dtype: DType, ys: b200_dptr, rows: u64, ys_stride: u64, weights: b200_dptr,
+        row_of: b200_dptr, t: u64, k: u64, n: u64, y: b200_dptr, y_stride: u64,
+    ) -> Result<(), Error> {
+        check(sys::b200_moe_combine(
+            self.0, stream, ys_dtype as c_int, y_dtype as c_int, ys, rows, ys_stride, weights, row_of, t, k, n, y, y_stride,
+        ))
+    }
+
+    /// Gradients of [`Context::moe_combine`]: d_ys [rows, n] in `grad_dtype` and d_w f32 [t, k].  See
+    /// `b200_moe_combine_backward`.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::moe_route`].
+    #[allow(clippy::too_many_arguments)]
+    pub unsafe fn moe_combine_backward(
+        &mut self, stream: b200_stream, grad_dtype: DType, ys_dtype: DType, dy: b200_dptr, dy_stride: u64, ys: b200_dptr, rows: u64,
+        ys_stride: u64, weights: b200_dptr, row_of: b200_dptr, t: u64, k: u64, n: u64, d_ys: b200_dptr, d_ys_stride: u64,
+        d_w: b200_dptr,
+    ) -> Result<(), Error> {
+        check(sys::b200_moe_combine_backward(
+            self.0, stream, grad_dtype as c_int, ys_dtype as c_int, dy, dy_stride, ys, rows, ys_stride, weights, row_of, t, k, n, d_ys,
+            d_ys_stride, d_w,
+        ))
+    }
+
     /// Quantize `input` ([..., K], F32 / F16 / BF16, any strides) along its innermost axis under `scheme` into compact
     /// codes [..., K * bits / 8], block scales [..., K / block] and the f32 tensor scale (0 for an absent level); the
     /// contract is `b200_quantize`'s in include/cubecl_b200.h.
