@@ -154,6 +154,81 @@ def block_scaled_operands(M, N, K, kind: str, seed: int, batch=()):
     return a_dev, b_dev, sa, sb, a, b
 
 
+# ------------------------------------------------------------------------------------------------ f32 operands with low parts
+# x = hi + lo with hi an integer of at most 2 bits and lo a multiple of LOW_GRAIN of the same sign and below half the tf32 ulp of
+# hi: the tf32 datapath reads hi whether it truncates or rounds, x - trunc_tf32(x) = lo exactly, bf16(x) = hi, and lo is exact in
+# tf32 and bf16.  So the 3xTF32 and hybrid schedules both compute sum(a b - a_lo b_lo) and tf32 alone sum(a_hi b_hi), and with
+# every partial sum a multiple of LOW_GRAIN below 2^24 LOW_GRAIN, each of them is exact in f32.
+LOW_GRAIN = 2.0 ** -14
+F32_SCHEDULES = ("3xtf32", "hybrid", "tf32")
+# kernels that compute the wrong low-part arithmetic, each of which the exact checks must catch
+LOWPART_MUTANTS = ("tf32_only", "lo_lo_added", "a_lo_shifted_k", "b_lo_shifted_k", "a_lo_b_hi_negated", "a_hi_b_lo_negated")
+
+
+def tf32_trunc(x) -> np.ndarray:
+    return (np.asarray(x, np.float32).view(np.uint32) & np.uint32(0xFFFFE000)).view(np.float32)
+
+
+def tf32_rn(x) -> np.ndarray:
+    u = np.asarray(x, np.float32).view(np.uint32).astype(np.uint64)
+    return (((u + 0xFFF + ((u >> 13) & 1)) >> 13) << 13).astype(np.uint32).view(np.float32)
+
+
+def lowpart_values(shape, seed: int, hi_max: int = 3, lo_max: int = 7, density: float = 1.0):
+    """(x, hi, lo) in f64: hi integers in [-hi_max, hi_max] (zero with probability 1 - density), lo = sign(hi) * j * LOW_GRAIN
+    with j in [0, lo_max].  Asserts what the schedules read from x."""
+    assert hi_max <= 3 and (lo_max + 1) * LOW_GRAIN <= 2.0 ** -11, "lo must stay below half the tf32 ulp of hi"
+    rng = np.random.default_rng(seed)
+    hi = rng.integers(1, hi_max + 1, size=shape) * rng.choice([-1.0, 1.0], size=shape)
+    hi[rng.random(size=shape) >= density] = 0.0
+    lo = np.sign(hi) * rng.integers(0, lo_max + 1, size=shape) * LOW_GRAIN
+    x = hi + lo
+    x32 = x.astype(np.float32)
+    assert np.array_equal(x32.astype(np.float64), x)
+    assert np.array_equal(tf32_trunc(x32), hi) and np.array_equal(tf32_rn(x32), hi), "the tf32 datapath must read hi"
+    assert np.array_equal((x32 - tf32_trunc(x32)).astype(np.float64), lo), "the split must leave lo"
+    assert np.array_equal(synth.bf16_bits_to_f32(synth.f32_to_bf16_bits(x32)), hi), "bf16(x) must be hi"
+    lo32 = lo.astype(np.float32)
+    assert np.array_equal(tf32_trunc(lo32), lo32) and np.array_equal(synth.bf16_bits_to_f32(synth.f32_to_bf16_bits(lo32)), lo32)
+    return x, hi, lo
+
+
+def lowpart_products(parts, schedule: str, mutant: str | None = None) -> np.ndarray:
+    """f64 result of a schedule on lowpart_values operands parts = (a_hi, a_lo, b_hi, b_lo) ([.., M, K] and [.., K, N]), or of
+    one of LOWPART_MUTANTS of it."""
+    ah, al, bh, bl = parts
+    if schedule == "tf32" or mutant == "tf32_only":
+        return np.matmul(ah, bh)
+    if mutant == "a_lo_shifted_k":     # the low plane of a read one k further on
+        al = np.concatenate([al[..., 1:], np.zeros_like(al[..., :1])], axis=-1)
+    if mutant == "b_lo_shifted_k":
+        bl = np.concatenate([bl[..., 1:, :], np.zeros_like(bl[..., :1, :])], axis=-2)
+    hl, lh = np.matmul(ah, bl), np.matmul(al, bh)
+    if mutant == "a_hi_b_lo_negated":
+        hl = -hl
+    if mutant == "a_lo_b_hi_negated":
+        lh = -lh
+    out = np.matmul(ah, bh) + hl + lh
+    if mutant == "lo_lo_added":
+        out = out + np.matmul(al, bl)
+    return out
+
+
+def lowpart_operands(lhs_shape, rhs_shape, seed: int, schedule: str, density: float = 1.0):
+    """Low-part f32 operands a [.., M, K] and b [.., K, N], the exact result of `schedule`, and the (a_hi, a_lo, b_hi, b_lo)
+    parts.  Asserts that every partial sum of every schedule's terms is exact in f32 (sum |terms| < 2^24 LOW_GRAIN) and that the
+    low parts really change the result."""
+    a, ah, al = lowpart_values(lhs_shape, seed, density=density)
+    b, bh, bl = lowpart_values(rhs_shape, seed + 1, density=density)
+    parts = (ah, al, bh, bl)
+    assert_exact_bound((np.matmul(np.abs(ah), np.abs(bh)) + np.matmul(np.abs(ah), np.abs(bl)) + np.matmul(np.abs(al), np.abs(bh)))
+                       / LOW_GRAIN)
+    exact = lowpart_products(parts, schedule)
+    if schedule != "tf32":
+        assert np.mean(exact != lowpart_products(parts, "tf32")) > 0.5, "the low parts must change most outputs"
+    return a, b, exact, parts
+
+
 def matmul_f64_ieee(a, b) -> np.ndarray:
     """a [M, K] @ b [K, N] in f64 one k at a time, so inf * 0 and inf - inf give NaN as IEEE arithmetic does (an optimised BLAS
     may skip zero terms)."""

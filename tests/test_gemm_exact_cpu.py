@@ -193,3 +193,76 @@ def test_conv_case_lists_cover_multi_phase_dgrad_and_the_wgrad_head():
     # the one-rounding list holds a multi-phase dgrad and a wgrad with a head
     rounding = [p for w, g, od, o, p in plans if (w, g) in gpu.ROUNDING_CONV and not o]
     assert any(p.phases > 1 for p in rounding) and any(p.head and "wgrad" in p.kernel for p in rounding)
+
+
+# ------------------------------------------------------------------------------------------------ f32 operands with low parts
+import test_f32_split_model as split_model  # noqa: E402
+import test_gemm_f32_lowpart_exact_gpu as lowgpu  # noqa: E402
+
+
+def test_lowpart_values_split_as_the_schedules_read_them():
+    x, hi, lo = ge.lowpart_values((64, 200), seed=5)
+    assert np.any(lo != 0) and set(np.unique(np.abs(hi))) == {1.0, 2.0, 3.0}
+    assert np.all((lo == 0) | (np.sign(lo) == np.sign(hi)))
+    assert np.max(np.abs(lo)) < 2.0 ** -11                              # below half the tf32 ulp of |hi| >= 1
+    # round-to-nearest tf32 and bf16 read hi too, even where lo is largest
+    edge = np.array([1 + 7 * ge.LOW_GRAIN, -3 - 7 * ge.LOW_GRAIN, 2 + 7 * ge.LOW_GRAIN], np.float32)
+    assert list(ge.tf32_rn(edge)) == [1.0, -3.0, 2.0] and list(ge.tf32_trunc(edge)) == [1.0, -3.0, 2.0]
+    with pytest.raises(AssertionError, match="half the tf32 ulp"):
+        ge.lowpart_values((4, 4), seed=1, lo_max=8)
+
+
+@pytest.mark.parametrize("density", [1.0, 0.35])
+def test_lowpart_schedules_match_the_split_model(density):
+    """The f64 schedules of test_f32_split_model on the f32 operands give exactly what lowpart_products predicts, and every
+    f32 partial sum of them is exact."""
+    a, b, exact, parts = ge.lowpart_operands((48, 200 if density == 1.0 else 1000), (200 if density == 1.0 else 1000, 40), 3,
+                                             "hybrid", density=density)
+    s = split_model.schedules(a.astype(np.float32), b.astype(np.float32))
+    for sched in ge.F32_SCHEDULES:
+        assert np.array_equal(s[sched], ge.lowpart_products(parts, sched)), sched
+    assert np.array_equal(exact, a @ b - parts[1] @ parts[3])
+    assert np.array_equal(exact.astype(np.float32).astype(np.float64), exact)
+
+
+def test_lowpart_generator_refuses_inexact_sums():
+    with pytest.raises(AssertionError, match="2\\^24"):
+        ge.lowpart_operands((4, 2000), (2000, 4), 1, "3xtf32")
+
+
+@pytest.fixture(scope="module")
+def lowpart_plans():
+    return [(c, ge.plan_gemm_case(c, SMS)) for c in lowgpu.LOWPART_CASES]
+
+
+def test_lowpart_cases_take_the_paths_their_names_say(lowpart_plans):
+    for c, p in lowpart_plans:
+        lowgpu.expect_lowpart_path(c, p)
+
+
+def test_lowpart_case_list_covers_every_schedule_tile_store_and_split(lowpart_plans):
+    covered = {(lowgpu.schedule(c),) + _cell(c, p)[:3] for c, p in lowpart_plans}
+    want = {(s, v, store, head) for s in ("3xtf32", "hybrid") for v in lowgpu.TILE_SHAPES for store in ("tma", "direct")
+            for head in ("head", "nohead")}
+    want |= {("tf32", v, "tma", "head") for v in lowgpu.TILE_SHAPES}
+    assert not (want - covered), sorted(want - covered)
+    # and per low-part schedule: batched, broadcast, each operand staged from MN-major, unaligned K, a pitched output window,
+    # three k-ranges per tile
+    for s in ("3xtf32", "hybrid"):
+        cs = [c for c, _ in lowpart_plans if lowgpu.schedule(c) == s]
+        assert any(c.batch and not c.bcast for c in cs) and any(c.bcast for c in cs)
+        assert any(c.lhs_t for c in cs) and any(c.rhs_t for c in cs) and any(not c.rhs_t for c in cs)
+        assert any(c.K % 4 for c in cs) and any(c.window for c in cs) and any(c.options.get("gemm.split_k") == "3" for c in cs)
+
+
+def test_every_wrong_low_part_kernel_changes_some_lowpart_case_output():
+    for case in lowgpu.LOWPART_CASES:
+        _, _, exact, parts = lowgpu.operands(case)
+        want = ge.rne(exact, "f32")
+        sched = lowgpu.schedule(case)
+        if sched == "tf32":   # the single pass must not pick up the low parts
+            assert ge.bit_mismatches(ge.rne(ge.lowpart_products(parts, "3xtf32"), "f32"), want, "f32").any(), case.name
+            continue
+        for mutant in ge.LOWPART_MUTANTS:
+            bad = ge.bit_mismatches(ge.rne(ge.lowpart_products(parts, sched, mutant), "f32"), want, "f32")
+            assert bad.mean() > 0.01, (case.name, mutant, float(bad.mean()))
