@@ -1,12 +1,13 @@
 """CPU: the C-ABI library loads and exports everything include/*.h declares; the product path has no CPU fallback."""
 import ast
 import ctypes
+import re
 import subprocess
 from pathlib import Path
 
 import pytest
 
-from cubecl_b200 import _ffi
+from cubecl_b200 import _ffi, build
 
 ROOT = Path(__file__).resolve().parent.parent
 
@@ -59,13 +60,23 @@ def test_embedded_images_are_elf_cubins_for_sm100():
     # (name kept from the Blackwell build; the images are sm_90a)
     # "driver-API load of a prebuilt sm_90a .cubin": the images inside the .so are the nvcc -cubin outputs, byte for byte
     lib = _ffi.load()
-    for name in ("gemm", "gemm_b", "gemm_c", "reduce", "aux"):
+    for name in build.CUBINS:
         img, size = ctypes.c_void_p(), ctypes.c_size_t()
         assert lib.b200_get_cubin(name.encode(), ctypes.byref(img), ctypes.byref(size)) == 0
         blob = ctypes.string_at(img.value, size.value)
         assert blob[:4] == b"\x7fELF"
         assert blob == (ROOT / "cubecl_b200" / "build" / f"{name}.cubin").read_bytes()
     assert lib.b200_get_cubin(b"nope", ctypes.byref(img), ctypes.byref(size)) == 6
+
+
+def test_cubin_table_sorts_kernels_and_rejects_ambiguous_or_empty_images():
+    table = build.cubin_table({"b": ["zeta", "alpha"], "a": ["mid"]})
+    assert table.index('{"b", b200_cubin_b, b200_cubin_b_end}') < table.index('{"a", b200_cubin_a, b200_cubin_a_end}')
+    assert re.findall(r'\{"(\w+)", (\d+)\}', table) == [("alpha", "0"), ("mid", "1"), ("zeta", "0")]
+    with pytest.raises(RuntimeError, match="'k' is exported by both cubin 'a' and 'b'"):
+        build.cubin_table({"a": ["k"], "b": ["j", "k"]})
+    with pytest.raises(RuntimeError, match="cubin 'b' exports no kernels"):
+        build.cubin_table({"a": ["k"], "b": []})
 
 
 def test_no_gpu_fails_loudly_not_silently():
