@@ -9,14 +9,14 @@ a test can assert the path it meant to exercise really ran.
 """
 from __future__ import annotations
 
-import ctypes as C
 import re
 from dataclasses import dataclass, field
 
 import numpy as np
 
-from cubecl_b200 import _ffi, synth
+from cubecl_b200 import synth
 from cubecl_b200.client import DTYPE_SIZE, Handle, TensorHandle
+from plan_context import PlanContext
 
 EXACT_LIMIT = 2.0 ** 24
 # smallest |output| at which a 16-bit result is rounded (integers above it are not all representable)
@@ -286,38 +286,22 @@ _KERNEL = re.compile(r"^launch ((?:gemm|conv2d)_\S+)", re.M)
 _HEAD = re.compile(r"gemm stream-k head: (\d+) whole tiles")
 
 
-class PlanClient:
+class PlanClient(PlanContext):
     """Stands in for a ComputeClient with a dry-run planning context (b200_plan_begin): the library's launch functions take it
     as they take a client, and launch errors raise instead of being deferred."""
 
     def __init__(self, sms: int, options: dict):
-        self._lib = _ffi.load()
-        self._ctx = C.c_void_p()
-        _ffi.check(self._lib.b200_plan_begin(int(sms), C.byref(self._ctx)))
-        for k, v in options.items():
-            _ffi.check(self._lib.b200_set_option(self._ctx, k.encode(), str(v).encode()))
+        super().__init__(sms, options)
+        self._lib, self._ctx = self.lib, self.ctx
 
     def _defer(self, err):
         raise err
 
-    def text(self) -> str:
-        need = C.c_size_t()
-        _ffi.check(self._lib.b200_plan_text(self._ctx, None, 0, C.byref(need)))
-        buf = C.create_string_buffer(need.value)
-        _ffi.check(self._lib.b200_plan_text(self._ctx, buf, need.value, None))
-        return buf.value.decode()
-
-    def close(self):
-        self._lib.b200_destroy(self._ctx)
-
 
 def _plan_text(sms, options, issue) -> str:
-    pc = PlanClient(sms, options)
-    try:
+    with PlanClient(sms, options) as pc:
         issue(pc)
         return pc.text()
-    finally:
-        pc.close()
 
 
 def probe(sms: int, options: dict, issue) -> Plan:

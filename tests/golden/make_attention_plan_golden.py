@@ -62,8 +62,7 @@ PLANNERS = {
 def replay(call: dict) -> dict:
     """One recorded call in a fresh dry-run context: {status, error (the message up to its first ':'), plan}."""
     cls, method = PLANNERS[call["fn"]]
-    p = cls(call["sms"])
-    try:
+    with cls(call["sms"]) as p:
         kw = dict(call["kw"])
         if "shapes" in kw and call["fn"] == "varlen_bwd":
             rc, text = _varlen_bwd(p, *call["args"], **kw)
@@ -77,8 +76,6 @@ def replay(call: dict) -> dict:
             msg = p.lib.b200_last_error()
             err = msg.decode().split(":")[0] if msg else ""
         return {"status": rc, "error": err, "plan": text}
-    finally:
-        p.close()
 
 
 def cases():

@@ -24,6 +24,7 @@ TESTS = Path(__file__).resolve().parent.parent
 sys.path[:0] = [str(TESTS.parent), str(TESTS)]
 
 from cubecl_b200 import _ffi  # noqa: E402
+from plan_context import PlanContext  # noqa: E402
 
 GOLDEN = Path(__file__).resolve().parent / "conv_nd_plan_golden.json.gz"
 GOLDEN_2D = Path(__file__).resolve().parent / "conv_plan_golden.json.gz"
@@ -35,22 +36,9 @@ BIG = 1 << 31
 DT = (("bf16", "bf16"), ("f16", "f32"))
 
 
-def _plan_text(lib, ctx) -> str:
-    need = C.c_size_t()
-    _ffi.check(lib.b200_plan_text(ctx, None, 0, C.byref(need)))
-    buf = C.create_string_buffer(need.value)
-    _ffi.check(lib.b200_plan_text(ctx, buf, need.value, None))
-    return buf.value.decode()
-
-
 def replay(call: dict) -> dict:
     """One recorded call in a fresh dry-run context (132 SMs): {status, error (the full message, "" on success), plan}."""
-    lib = _ffi.load()
-    ctx = C.c_void_p()
-    _ffi.check(lib.b200_plan_begin(132, C.byref(ctx)))
-    try:
-        for k, v in call["options"].items():
-            _ffi.check(lib.b200_set_option(ctx, k.encode(), v.encode()))
+    with PlanContext(132, call["options"]) as p:
         fn = call["fn"]
         arr = lambda v: _ffi.u64_array(v) if v is not None else None  # noqa: E731
         args = None
@@ -59,16 +47,14 @@ def replay(call: dict) -> dict:
         extra = (C.c_uint32(call["groups"]),) if call["groups"] is not None else ()
         if fn in WITH_EP:
             extra += (C.byref(_ffi.Epilogue(*call["ep"])) if call["ep"] is not None else None,)
-        rc = getattr(lib, fn)(ctx, None, DTYPES[call["idt"]], DTYPES[call["odt"]], call["a"], arr(call["a_shape"]), arr(call["a_strides"]),
-                              call["b"], arr(call["b_shape"]), arr(call["b_strides"]), call["o"], arr(call["o_shape"]),
-                              arr(call["o_strides"]), args, *extra)
+        rc = getattr(p.lib, fn)(p.ctx, None, DTYPES[call["idt"]], DTYPES[call["odt"]], call["a"], arr(call["a_shape"]),
+                                arr(call["a_strides"]), call["b"], arr(call["b_shape"]), arr(call["b_strides"]), call["o"],
+                                arr(call["o_shape"]), arr(call["o_strides"]), args, *extra)
         err = ""
         if rc:
-            msg = lib.b200_last_error()
+            msg = p.lib.b200_last_error()
             err = msg.decode() if msg else ""
-        return {"status": rc, "error": err, "plan": _plan_text(lib, ctx)}
-    finally:
-        lib.b200_destroy(ctx)
+        return {"status": rc, "error": err, "plan": p.text()}
 
 
 def _vec(v, n):

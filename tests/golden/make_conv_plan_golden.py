@@ -37,10 +37,7 @@ DT = (("bf16", "bf16"), ("f16", "f32"))
 
 def replay(call: dict) -> dict:
     """One recorded call in a fresh dry-run context (132 SMs): {status, error (the message up to its first ':'), plan}."""
-    p = Planner(132)
-    try:
-        for k, v in call["options"].items():
-            _ffi.check(p.lib.b200_set_option(p.ctx, k.encode(), v.encode()))
+    with Planner(132, call["options"]) as p:
         ep = _ffi.Epilogue(*call["ep"]) if call["ep"] is not None else None
         rc, text = p.call(ENTRY[call["fn"]], call["a_shape"], call["b_shape"], call["o_shape"], call["groups"],
                           idt=DTYPES[call["idt"]], odt=DTYPES[call["odt"]], stride=call["stride"], pad=call["pad"], dil=call["dil"],
@@ -51,8 +48,6 @@ def replay(call: dict) -> dict:
             msg = p.lib.b200_last_error()
             err = msg.decode().split(":")[0] if msg else ""
         return {"status": rc, "error": err, "plan": text}
-    finally:
-        p.close()
 
 
 def call(fn, xs, ws, groups=None, stride=1, pad=0, dil=1, dt=DT[0], ys=None, a_strides=None, b_strides=None, o_strides=None,

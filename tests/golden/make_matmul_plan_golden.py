@@ -26,6 +26,7 @@ TESTS = Path(__file__).resolve().parent.parent
 sys.path[:0] = [str(TESTS.parent), str(TESTS)]
 
 from cubecl_b200 import _ffi  # noqa: E402
+from plan_context import PlanContext  # noqa: E402
 
 GOLDEN = Path(__file__).resolve().parent / "matmul_plan_golden.json.gz"
 DT = {"f32": _ffi.F32, "f16": _ffi.F16, "bf16": _ffi.BF16, "i32": _ffi.I32, "u8": _ffi.U8, "i8": _ffi.I8, "e4m3": _ffi.F8E4M3,
@@ -35,14 +36,6 @@ QV = {"q8f": _ffi.QV_Q8F, "q8s": _ffi.QV_Q8S, "q4f": _ffi.QV_Q4F, "q4s": _ffi.QV
 
 A, B, O, S1, S2, OFFS, BIAS = 0x10000000, 0x20000000, 0x30000000, 0x40000000, 0x48000000, 0x50000000, 0x60000000
 BIG = 1 << 31
-
-
-def _plan_text(lib, ctx) -> str:
-    need = C.c_size_t()
-    _ffi.check(lib.b200_plan_text(ctx, None, 0, C.byref(need)))
-    buf = C.create_string_buffer(need.value)
-    _ffi.check(lib.b200_plan_text(ctx, buf, need.value, None))
-    return buf.value.decode()
 
 
 def _arg(v):
@@ -63,20 +56,13 @@ def _arg(v):
 
 def replay(call: dict) -> dict:
     """One recorded call in a fresh dry-run context (132 SMs): {status, error (the full message, "" on success), plan}."""
-    lib = _ffi.load()
-    ctx = C.c_void_p()
-    _ffi.check(lib.b200_plan_begin(132, C.byref(ctx)))
-    try:
-        for k, v in call["options"].items():
-            _ffi.check(lib.b200_set_option(ctx, k.encode(), v.encode()))
-        rc = getattr(lib, call["fn"])(ctx, None, *[_arg(a) for a in call["args"]])
+    with PlanContext(132, call["options"]) as p:
+        rc = getattr(p.lib, call["fn"])(p.ctx, None, *[_arg(a) for a in call["args"]])
         err = ""
         if rc:
-            msg = lib.b200_last_error()
+            msg = p.lib.b200_last_error()
             err = msg.decode() if msg else ""
-        return {"status": rc, "error": err, "plan": _plan_text(lib, ctx)}
-    finally:
-        lib.b200_destroy(ctx)
+        return {"status": rc, "error": err, "plan": p.text()}
 
 
 def u64(v):

@@ -14,15 +14,38 @@ ROOT = Path(__file__).resolve().parent.parent
 
 def test_library_exports_every_declared_symbol():
     lib = _ffi.load()
-    declared = _ffi.header_symbols()
+    # every b200_* name followed by '(' outside comments: a prototype parse_header does not recognise has no binding
+    declared = sorted(set(re.findall(r"\b(b200_[a-z0-9_]+)\s*\(", re.sub(r"/\*.*?\*/", "", _ffi.HEADER_PATH.read_text(), flags=re.S))))
     assert len(declared) >= 30
     for name in declared:
         assert hasattr(lib, name), f"{name} declared in cubecl_b200.h but not exported"
-    assert set(declared) == set(_ffi.SIGNATURES), "ctypes table and header disagree"
+    assert set(declared) == set(_ffi.SIGNATURES), "the header declares a function the derived bindings miss"
     out = subprocess.run(["nm", "-D", "--defined-only", str(_ffi.LIB_PATH)], capture_output=True, text=True).stdout
     exported = {line.split()[-1] for line in out.splitlines() if " T " in line}
     assert set(declared) <= exported
     assert lib.b200_abi_version() == 1
+
+
+def test_ctypes_layout_matches_the_c_compiler(tmp_path):
+    # the header is parsed once for C and Python alike, so this guards the maps from C types to ctypes: g++ lays out every
+    # struct and sizes every parameter and return type, and the derived classes and SIGNATURES must agree with it
+    _, _, structs, protos = _ffi.parse_header(_ffi.HEADER_PATH.read_text())
+    want = {}
+    for sname, fields in structs:
+        cls = _ffi.STRUCTS[sname]
+        want[f"sizeof({sname})"] = ctypes.sizeof(cls)
+        want.update((f"offsetof({sname}, {f})", getattr(cls, f).offset) for f, _ in fields)
+    for name, ret, args in protos:
+        restype, argtypes = _ffi.SIGNATURES[name]
+        for ctype, pytype in [(ret, restype), *((t, a) for (_, t), a in zip(args, argtypes, strict=True))]:
+            assert want.setdefault(f"sizeof({ctype})", ctypes.sizeof(pytype)) == ctypes.sizeof(pytype), (name, ctype)
+    assert len(structs) >= 9 and "sizeof(uint32_t)" in want and "sizeof(b200_dtype)" in want
+    src = tmp_path / "layout.cpp"
+    src.write_text('#include <cstddef>\n#include <cstdio>\n#include "cubecl_b200.h"\nint main() {\n'
+                   + "".join(f'  std::printf("%zu\\n", {e});\n' for e in want) + "}\n")
+    subprocess.run(["g++", "-std=c++17", "-I", str(_ffi.HEADER_PATH.parent), str(src), "-o", str(tmp_path / "layout")], check=True)
+    out = subprocess.run([str(tmp_path / "layout")], capture_output=True, text=True, check=True).stdout.split()
+    assert dict(zip(want, map(int, out), strict=True)) == want
 
 
 def test_cubins_are_embedded_and_sm100a():

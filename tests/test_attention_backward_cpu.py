@@ -13,6 +13,7 @@ import torch
 
 import attention_backward_oracle as abo
 from cubecl_b200 import _ffi
+from plan_context import PlanContext
 from test_conv_cpu import ROOT, _tool
 
 F32, F16, BF16, I8 = _ffi.F32, _ffi.F16, _ffi.BF16, _ffi.I8
@@ -48,19 +49,7 @@ def test_backward_oracle_writes_zero_for_keys_no_query_sees():
 
 
 # ---------------------------------------------------------------------------------------------- dry-run plans
-class Planner:
-    def __init__(self, sms=132):   # H100 SXM
-        self.lib = _ffi.load()
-        self.ctx = C.c_void_p()
-        _ffi.check(self.lib.b200_plan_begin(sms, C.byref(self.ctx)))
-
-    def text(self):
-        need = C.c_size_t()
-        _ffi.check(self.lib.b200_plan_text(self.ctx, None, 0, C.byref(need)))
-        buf = C.create_string_buffer(need.value)
-        _ffi.check(self.lib.b200_plan_text(self.ctx, buf, need.value, None))
-        return buf.value.decode()
-
+class Planner(PlanContext):
     def run(self, qs, ks, idt=BF16, odt=None, gdt=None, shapes=None, strides=None, ptrs=None, lse=LSE, scale=0.125, causal=0,
             null_args=False):
         """shapes / strides / ptrs: dicts over q, k, v, out, dout, dq, dk, dv overriding the compact defaults"""
@@ -83,15 +72,11 @@ class Planner:
         rc = self.lib.b200_attention_backward(self.ctx, None, idt, odt, gdt, *ops, None if null_args else C.byref(args))
         return rc, self.text()
 
-    def close(self):
-        self.lib.b200_destroy(self.ctx)
-
 
 @pytest.fixture
 def plan():
-    p = Planner()
-    yield p
-    p.close()
+    with Planner() as p:
+        yield p
 
 
 _LAUNCH = re.compile(r"launch (\S+) grid=\((\d+),1,1\) block=(\d+) smem=(\d+) cluster=1")

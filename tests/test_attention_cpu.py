@@ -13,6 +13,7 @@ import torch
 import attention_oracle as ao
 from cubecl_b200 import _ffi
 from cubecl_b200.attention import AttentionShapeError, calculate_attention_output
+from plan_context import PlanContext
 from test_conv_cpu import ROOT, _tool
 
 F32, F16, BF16, I8 = _ffi.F32, _ffi.F16, _ffi.BF16, _ffi.I8
@@ -57,19 +58,7 @@ def test_output_rule():
 
 
 # ---------------------------------------------------------------------------------------------- dry-run plans
-class Planner:
-    def __init__(self, sms=132):   # H100 SXM
-        self.lib = _ffi.load()
-        self.ctx = C.c_void_p()
-        _ffi.check(self.lib.b200_plan_begin(sms, C.byref(self.ctx)))
-
-    def text(self):
-        need = C.c_size_t()
-        _ffi.check(self.lib.b200_plan_text(self.ctx, None, 0, C.byref(need)))
-        buf = C.create_string_buffer(need.value)
-        _ffi.check(self.lib.b200_plan_text(self.ctx, buf, need.value, None))
-        return buf.value.decode()
-
+class Planner(PlanContext):
     def run(self, qs, ks, vs=None, outs=None, idt=BF16, odt=None, strides=(None, None, None, None), ptrs=(Q, K, V, OUT), lse=0,
             scale=0.125, causal=0, null_args=False):
         vs = ks if vs is None else vs
@@ -83,15 +72,11 @@ class Planner:
         rc = self.lib.b200_attention(self.ctx, None, idt, odt, *ops, lse, None if null_args else C.byref(args))
         return rc, self.text()
 
-    def close(self):
-        self.lib.b200_destroy(self.ctx)
-
 
 @pytest.fixture
 def plan():
-    p = Planner()
-    yield p
-    p.close()
+    with Planner() as p:
+        yield p
 
 
 def _launches(t):

@@ -14,6 +14,7 @@ import torch
 import attention_kvcache_oracle as ko
 import attention_oracle as ao
 from cubecl_b200 import _ffi
+from plan_context import PlanContext
 from test_conv_cpu import ROOT, _tool
 
 F32, F16, BF16, I8 = _ffi.F32, _ffi.F16, _ffi.BF16, _ffi.I8
@@ -79,19 +80,7 @@ def test_oracle_rows_without_keys_and_clamped_lengths():
 
 
 # ---------------------------------------------------------------------------------------------- dry-run plans
-class Planner:
-    def __init__(self, sms=132):   # H100 SXM
-        self.lib = _ffi.load()
-        self.ctx = C.c_void_p()
-        _ffi.check(self.lib.b200_plan_begin(sms, C.byref(self.ctx)))
-
-    def text(self):
-        need = C.c_size_t()
-        _ffi.check(self.lib.b200_plan_text(self.ctx, None, 0, C.byref(need)))
-        buf = C.create_string_buffer(need.value)
-        _ffi.check(self.lib.b200_plan_text(self.ctx, buf, need.value, None))
-        return buf.value.decode()
-
+class Planner(PlanContext):
     def run(self, qs, kcs, vcs=None, bts=None, outs=None, idt=BF16, odt=None, strides=(None, None, None, None, None),
             ptrs=(Q, KC, VC, BT, SL, OUT), lse=0, scale=0.125, causal=0, null_args=False):
         vcs = kcs if vcs is None else vcs
@@ -113,15 +102,11 @@ class Planner:
                                          ptrs[1], arr(kcs), arr(strides[2]), ptrs[2], arr(vcs), arr(strides[3]), ptrs[4])
         return rc, self.text()
 
-    def close(self):
-        self.lib.b200_destroy(self.ctx)
-
 
 @pytest.fixture
 def plan():
-    p = Planner()
-    yield p
-    p.close()
+    with Planner() as p:
+        yield p
 
 
 def _launches(t):

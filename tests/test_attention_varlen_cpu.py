@@ -13,6 +13,7 @@ import torch
 
 import attention_varlen_oracle as vo
 from cubecl_b200 import _ffi
+from plan_context import PlanContext
 from test_conv_cpu import ROOT, _tool
 
 F32, F16, BF16, I8 = _ffi.F32, _ffi.F16, _ffi.BF16, _ffi.I8
@@ -74,19 +75,7 @@ def test_band_mask_rules():
 
 
 # ---------------------------------------------------------------------------------------------- dry-run plans
-class Planner:
-    def __init__(self, sms=132):   # H100 SXM
-        self.lib = _ffi.load()
-        self.ctx = C.c_void_p()
-        _ffi.check(self.lib.b200_plan_begin(sms, C.byref(self.ctx)))
-
-    def text(self):
-        need = C.c_size_t()
-        _ffi.check(self.lib.b200_plan_text(self.ctx, None, 0, C.byref(need)))
-        buf = C.create_string_buffer(need.value)
-        _ffi.check(self.lib.b200_plan_text(self.ctx, buf, need.value, None))
-        return buf.value.decode()
-
+class Planner(PlanContext):
     def fwd(self, qs, ks, B, maxq, maxk, vs=None, outs=None, idt=BF16, odt=None, strides=(None, None, None, None),
             ptrs=(Q, K, V, CUQ, CUK, OUT), lse=0, scale=0.125, window=(-1, -1), null_args=False):
         vs = ks if vs is None else vs
@@ -115,15 +104,11 @@ class Planner:
         rc = self.lib.b200_attention_varlen_backward(self.ctx, None, idt, odt, gdt, *ops, C.byref(args))
         return rc, self.text()
 
-    def close(self):
-        self.lib.b200_destroy(self.ctx)
-
 
 @pytest.fixture
 def plan():
-    p = Planner()
-    yield p
-    p.close()
+    with Planner() as p:
+        yield p
 
 
 def _launches(t):

@@ -20,6 +20,7 @@ from torch.nn.attention.bias import causal_lower_right
 
 import attention_varlen_oracle as vo
 from cubecl_b200 import _ffi
+from plan_context import PlanContext
 from test_conv_cpu import ROOT, _tool
 
 F32, F16, BF16 = _ffi.F32, _ffi.F16, _ffi.BF16
@@ -143,19 +144,7 @@ def test_oracle_is_the_varlen_oracle_on_gathered_keys():
 
 
 # ---------------------------------------------------------------------------------------------- dry-run plans
-class Planner:
-    def __init__(self, sms=132):   # H100 SXM
-        self.lib = _ffi.load()
-        self.ctx = C.c_void_p()
-        _ffi.check(self.lib.b200_plan_begin(sms, C.byref(self.ctx)))
-
-    def text(self):
-        need = C.c_size_t()
-        _ffi.check(self.lib.b200_plan_text(self.ctx, None, 0, C.byref(need)))
-        buf = C.create_string_buffer(need.value)
-        _ffi.check(self.lib.b200_plan_text(self.ctx, buf, need.value, None))
-        return buf.value.decode()
-
+class Planner(PlanContext):
     def fwd(self, qs, kcs, B, maxq, maxk, bts=None, vcs=None, outs=None, idt=BF16, odt=None, strides=(None, None, None, None),
             bt_strides=None, ptrs=(Q, KC, VC, BT, CUQ, SEQ, OUT), lse=0, scale=0.125, window=(-1, -1), null_args=False, table=True):
         vcs = kcs if vcs is None else vcs
@@ -170,15 +159,11 @@ class Planner:
             arr(strides[2]), *bt, ptrs[4], ptrs[5], B, ptrs[6], arr(outs), arr(strides[3]), lse, None if null_args else C.byref(args))
         return rc, self.text()
 
-    def close(self):
-        self.lib.b200_destroy(self.ctx)
-
 
 @pytest.fixture
 def plan():
-    p = Planner()
-    yield p
-    p.close()
+    with Planner() as p:
+        yield p
 
 
 def _launches(t):

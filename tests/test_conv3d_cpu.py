@@ -12,6 +12,7 @@ import torch
 
 import conv3d_oracle as o3
 from cubecl_b200 import _ffi, conv3d
+from plan_context import PlanContext
 from test_conv_cpu import ROOT, _tool
 
 F32, F16, BF16, I8 = _ffi.F32, _ffi.F16, _ffi.BF16, _ffi.I8
@@ -64,22 +65,7 @@ def test_oracle_matches_torch(geom):
 
 
 # ---------------------------------------------------------------------------------------------- dry-run plans
-class Planner:
-    def __init__(self, sms=132):   # H100 SXM
-        self.lib = _ffi.load()
-        self.ctx = C.c_void_p()
-        _ffi.check(self.lib.b200_plan_begin(sms, C.byref(self.ctx)))
-
-    def text(self):
-        need = C.c_size_t()
-        _ffi.check(self.lib.b200_plan_text(self.ctx, None, 0, C.byref(need)))
-        buf = C.create_string_buffer(need.value)
-        _ffi.check(self.lib.b200_plan_text(self.ctx, buf, need.value, None))
-        return buf.value.decode()
-
-    def option(self, k, v):
-        _ffi.check(self.lib.b200_set_option(self.ctx, k.encode(), str(v).encode()))
-
+class Planner(PlanContext):
     def _call(self, fn, a, b, out, idt, odt, stride, pad, dil, strides, ptrs, ep=()):
         args = _ffi.Conv3dArgs(*o3.triple(stride), *o3.triple(pad), *o3.triple(dil))
         arr = lambda v: _ffi.u64_array(v) if v is not None else None  # noqa: E731
@@ -103,15 +89,11 @@ class Planner:
             dys = [xs[0], *o3.out_dhw(xs[1:4], dws[1:4], stride, pad, dil), dws[0]]
         return self._call(self.lib.b200_conv3d_backward_weight, xs, dys, dws, idt, odt, stride, pad, dil, strides, ptrs)
 
-    def close(self):
-        self.lib.b200_destroy(self.ctx)
-
 
 @pytest.fixture
 def plan():
-    p = Planner()
-    yield p
-    p.close()
+    with Planner() as p:
+        yield p
 
 
 def _names(t):

@@ -12,6 +12,7 @@ import torch
 import conv_backward_oracle as cbo
 import conv_oracle as co
 from cubecl_b200 import _ffi
+from plan_context import PlanContext
 from test_conv_cpu import ROOT, _tool
 
 F32, F16, BF16 = _ffi.F32, _ffi.F16, _ffi.BF16
@@ -62,22 +63,7 @@ def test_oracle_matches_torch_grad(geom):
 
 
 # ---------------------------------------------------------------------------------------------- dry-run plans
-class Planner:
-    def __init__(self, sms=132):   # H100 SXM
-        self.lib = _ffi.load()
-        self.ctx = C.c_void_p()
-        _ffi.check(self.lib.b200_plan_begin(sms, C.byref(self.ctx)))
-
-    def text(self):
-        need = C.c_size_t()
-        _ffi.check(self.lib.b200_plan_text(self.ctx, None, 0, C.byref(need)))
-        buf = C.create_string_buffer(need.value)
-        _ffi.check(self.lib.b200_plan_text(self.ctx, buf, need.value, None))
-        return buf.value.decode()
-
-    def option(self, k, v):
-        _ffi.check(self.lib.b200_set_option(self.ctx, k.encode(), str(v).encode()))
-
+class Planner(PlanContext):
     def _call(self, fn, a_shape, b_shape, out_shape, dy_shape, idt, odt, stride, pad, dil, a_strides, b_strides, o_strides, ptrs):
         (sh, sw), (ph, pw), (dh, dw) = co.pair(stride), co.pair(pad), co.pair(dil)
         args = _ffi.Conv2dArgs(sh, sw, ph, pw, dh, dw)
@@ -100,15 +86,11 @@ class Planner:
         return self._call(self.lib.b200_conv2d_backward_weight, xs, dys, dws, dys, idt, odt, stride, pad, dil, x_strides, dy_strides,
                           dw_strides, ptrs)
 
-    def close(self):
-        self.lib.b200_destroy(self.ctx)
-
 
 @pytest.fixture
 def plan():
-    p = Planner()
-    yield p
-    p.close()
+    with Planner() as p:
+        yield p
 
 
 def _names(t):

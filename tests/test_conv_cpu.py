@@ -13,6 +13,7 @@ import torch
 
 import conv_oracle as co
 from cubecl_b200 import _ffi, conv
+from plan_context import PlanContext
 
 ROOT = Path(__file__).resolve().parent.parent
 F32, F16, BF16, I8 = _ffi.F32, _ffi.F16, _ffi.BF16, _ffi.I8
@@ -64,22 +65,7 @@ def test_shape_rule_matches_torch(hw, k, s, p, d):
 
 
 # ---------------------------------------------------------------------------------------------- dry-run plans
-class Planner:
-    def __init__(self, sms=132):   # H100 SXM
-        self.lib = _ffi.load()
-        self.ctx = C.c_void_p()
-        _ffi.check(self.lib.b200_plan_begin(sms, C.byref(self.ctx)))
-
-    def text(self):
-        need = C.c_size_t()
-        _ffi.check(self.lib.b200_plan_text(self.ctx, None, 0, C.byref(need)))
-        buf = C.create_string_buffer(need.value)
-        _ffi.check(self.lib.b200_plan_text(self.ctx, buf, need.value, None))
-        return buf.value.decode()
-
-    def option(self, k, v):
-        _ffi.check(self.lib.b200_set_option(self.ctx, k.encode(), str(v).encode()))
-
+class Planner(PlanContext):
     def conv(self, xs, ws, os_=None, idt=BF16, odt=BF16, stride=1, pad=0, dil=1, x_strides=None, w_strides=None, o_strides=None,
              x=X, w=W, o=O, ep=None):
         (sh, sw), (ph, pw), (dh, dw) = co.pair(stride), co.pair(pad), co.pair(dil)
@@ -91,15 +77,11 @@ class Planner:
                                   arr(o_strides), C.byref(args), C.byref(ep) if ep is not None else None)
         return rc, self.text()
 
-    def close(self):
-        self.lib.b200_destroy(self.ctx)
-
 
 @pytest.fixture
 def plan():
-    p = Planner()
-    yield p
-    p.close()
+    with Planner() as p:
+        yield p
 
 
 def _launches(t):

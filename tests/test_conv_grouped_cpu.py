@@ -15,6 +15,7 @@ import torch
 import conv_grouped_oracle as go
 from conv_oracle import out_hw, pair
 from cubecl_b200 import _ffi, conv
+from plan_context import PlanContext
 
 ROOT = Path(__file__).resolve().parent.parent
 F32, F16, BF16 = _ffi.F32, _ffi.F16, _ffi.BF16
@@ -87,19 +88,7 @@ def test_wgrad_segments_formula():
 
 
 # ---------------------------------------------------------------------------------------------- dry-run plans
-class Planner:
-    def __init__(self, sms=132):   # H100 SXM
-        self.lib = _ffi.load()
-        self.ctx = C.c_void_p()
-        _ffi.check(self.lib.b200_plan_begin(sms, C.byref(self.ctx)))
-
-    def text(self):
-        need = C.c_size_t()
-        _ffi.check(self.lib.b200_plan_text(self.ctx, None, 0, C.byref(need)))
-        buf = C.create_string_buffer(need.value)
-        _ffi.check(self.lib.b200_plan_text(self.ctx, buf, need.value, None))
-        return buf.value.decode()
-
+class Planner(PlanContext):
     def call(self, fn, a_shape, b_shape, o_shape, groups, idt=BF16, odt=BF16, stride=1, pad=0, dil=1, a_strides=None, b_strides=None,
              o_strides=None, a=X, b=W, o=O, ep=None, forward=False):
         (sh, sw), (ph, pw), (dh, dw) = pair(stride), pair(pad), pair(dil)
@@ -127,9 +116,6 @@ class Planner:
         ys = [xs[0], *out_hw(xs[1], xs[2], ws[1], ws[2], stride, pad, dil), ws[0]]
         return self.call("b200_conv2d_backward_weight", xs, ys, ws, groups, stride=stride, pad=pad, dil=dil, **kw)
 
-    def close(self):
-        self.lib.b200_destroy(self.ctx)
-
 
 def _grouped(fn):
     return fn.replace("b200_conv2d", "b200_conv2d_grouped")
@@ -137,9 +123,8 @@ def _grouped(fn):
 
 @pytest.fixture
 def plan():
-    p = Planner()
-    yield p
-    p.close()
+    with Planner() as p:
+        yield p
 
 
 def _launches(t):

@@ -14,6 +14,7 @@ import torch
 import conv_transpose_oracle as cto
 from cubecl_b200 import _ffi
 from cubecl_b200.conv_transpose import calculate_conv_transpose_output
+from plan_context import PlanContext
 from test_conv_cpu import ROOT, _tool
 
 F32, F16, BF16, I8 = _ffi.F32, _ffi.F16, _ffi.BF16, _ffi.I8
@@ -69,22 +70,7 @@ def test_output_rule_matches_torch(geom):
 
 
 # ---------------------------------------------------------------------------------------------- dry-run plans
-class Planner:
-    def __init__(self, sms=132):   # H100 SXM
-        self.lib = _ffi.load()
-        self.ctx = C.c_void_p()
-        _ffi.check(self.lib.b200_plan_begin(sms, C.byref(self.ctx)))
-
-    def text(self):
-        need = C.c_size_t()
-        _ffi.check(self.lib.b200_plan_text(self.ctx, None, 0, C.byref(need)))
-        buf = C.create_string_buffer(need.value)
-        _ffi.check(self.lib.b200_plan_text(self.ctx, buf, need.value, None))
-        return buf.value.decode()
-
-    def option(self, k, v):
-        _ffi.check(self.lib.b200_set_option(self.ctx, k.encode(), str(v).encode()))
-
+class Planner(PlanContext):
     def run(self, xs, ws, s=1, p=0, op=0, d=1, outs=None, idt=BF16, odt=BF16, strides=(None, None, None), ptrs=(X, W, OUT), ep=None):
         n = len(xs) - 2
         if outs is None:
@@ -97,15 +83,11 @@ class Planner:
                 arr(strides[2]), C.byref(args), C.byref(ep) if ep is not None else None)
         return rc, self.text()
 
-    def close(self):
-        self.lib.b200_destroy(self.ctx)
-
 
 @pytest.fixture
 def plan():
-    p = Planner()
-    yield p
-    p.close()
+    with Planner() as p:
+        yield p
 
 
 def _names(t):

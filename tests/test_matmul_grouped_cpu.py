@@ -12,6 +12,7 @@ import torch
 
 import grouped_mm_oracle as gmo
 from cubecl_b200 import _ffi, matmul
+from plan_context import PlanContext
 from test_conv_cpu import ROOT, _tool
 
 F32, F16, BF16, F8E4M3 = _ffi.F32, _ffi.F16, _ffi.BF16, _ffi.F8E4M3
@@ -74,22 +75,7 @@ def test_clamping_rule():
 
 
 # ---------------------------------------------------------------------------------------------- dry-run plans
-class Planner:
-    def __init__(self, sms=SMS):
-        self.lib = _ffi.load()
-        self.ctx = C.c_void_p()
-        _ffi.check(self.lib.b200_plan_begin(sms, C.byref(self.ctx)))
-
-    def text(self):
-        need = C.c_size_t()
-        _ffi.check(self.lib.b200_plan_text(self.ctx, None, 0, C.byref(need)))
-        buf = C.create_string_buffer(need.value)
-        _ffi.check(self.lib.b200_plan_text(self.ctx, buf, need.value, None))
-        return buf.value.decode()
-
-    def option(self, k, v):
-        _ffi.check(self.lib.b200_set_option(self.ctx, k.encode(), str(v).encode()))
-
+class Planner(PlanContext):
     def run(self, ls, rs, os_, groups=None, lst=None, rst=None, ost=None, idt=BF16, odt=BF16, ptrs=(LHS, RHS, OFFS, OUT), ep=None):
         arr = lambda v: _ffi.u64_array(v) if v is not None else None  # noqa: E731
         if groups is None:
@@ -99,15 +85,11 @@ class Planner:
                                           C.byref(ep) if ep is not None else None)
         return rc, self.text()
 
-    def close(self):
-        self.lib.b200_destroy(self.ctx)
-
 
 @pytest.fixture
 def plan():
-    p = Planner()
-    yield p
-    p.close()
+    with Planner() as p:
+        yield p
 
 
 def _launches(t):

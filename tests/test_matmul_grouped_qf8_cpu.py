@@ -10,6 +10,7 @@ import pytest
 
 from cubecl_b200 import _ffi
 from cubecl_b200.quant import QuantScheme
+from plan_context import PlanContext
 
 ROOT = Path(__file__).resolve().parent.parent
 F32, F16, BF16, U32, F8E4M3, UE8M0 = _ffi.F32, _ffi.F16, _ffi.BF16, _ffi.U32, _ffi.F8E4M3, _ffi.UE8M0
@@ -19,25 +20,7 @@ QF8_SMEM = 202752                 # gemm_qf8_*: 5 stages of 32 KB codes + 4 KB s
 GRP_SMEM = QF8_SMEM + 8208        # + the group table (kGroupedTableBytes)
 
 
-class Planner:
-    def __init__(self, sms=132):   # H100 SXM
-        self.lib = _ffi.load()
-        self.ctx = C.c_void_p()
-        _ffi.check(self.lib.b200_plan_begin(sms, C.byref(self.ctx)))
-
-    def close(self):
-        self.lib.b200_destroy(self.ctx)
-
-    def text(self):
-        need = C.c_size_t()
-        _ffi.check(self.lib.b200_plan_text(self.ctx, None, 0, C.byref(need)))
-        buf = C.create_string_buffer(need.value)
-        _ffi.check(self.lib.b200_plan_text(self.ctx, buf, need.value, None))
-        return buf.value.decode()
-
-    def opt(self, key, value):
-        _ffi.check(self.lib.b200_set_option(self.ctx, key.encode(), value.encode()))
-
+class Planner(PlanContext):
     def run(self, sa, sb, groups, t, n, k, odt=BF16, va=VA, vb=VB, out=OUT, offs=OFFS, ptrs=None):
         ca = sa if isinstance(sa, _ffi.QuantScheme) else sa.to_c()
         cb = sb if isinstance(sb, _ffi.QuantScheme) else sb.to_c()
@@ -50,9 +33,8 @@ class Planner:
 
 @pytest.fixture
 def plan():
-    p = Planner()
-    yield p
-    p.close()
+    with Planner() as p:
+        yield p
 
 
 def launches(text):
@@ -85,7 +67,7 @@ def test_plan_of_a_deepseek_like_layer(plan):
 @pytest.mark.parametrize("lhs,fmt", [(E4B128, "e4m3"), (E5B128, "e5m2")])
 @pytest.mark.parametrize("odt,otag", [(BF16, "bf16"), (F16, "f16"), (F32, "f32")])
 def test_kernel_names(plan, tile, lhs, fmt, odt, otag):
-    plan.opt("gemm.variant", tile)
+    plan.option("gemm.variant", tile)
     for rhs in (E4B128, E5B128):   # the lhs format names the kernel; the rhs format is chosen at run time
         rc, t = plan.run(lhs, rhs, 4, 1000, 256, 512, odt=odt)
         assert rc == 0 and launches(t)[-1] == f"gemm_grouped_qf8_{fmt}_{otag}_{tile}_kk"
@@ -139,12 +121,12 @@ def test_one_group_reads_the_rhs_as_one_batch(plan):
 def test_store_path_and_no_stream_k(plan):
     rc, t = plan.run(E4B128, E4B128, 4, 8192, 1024, 1024)
     assert rc == 0 and "box=(64,64) swizzle=3" in t        # the TMA-store map of whole tiles
-    plan.opt("gemm.epilogue", "direct")
+    plan.option("gemm.epilogue", "direct")
     rc, t = plan.run(E4B128, E4B128, 4, 8192, 1024, 1024)
     assert rc == 0 and "box=(64,64)" not in t
-    plan.opt("gemm.epilogue", "tma")
+    plan.option("gemm.epilogue", "tma")
     for opt in ("on", "8", "auto"):
-        plan.opt("gemm.split_k", opt)
+        plan.option("gemm.split_k", opt)
         for shape in ((4, 8192 + 128, 8192, 4096), (128, 32768, 1536, 2048), (3, 300, 200, 256)):
             rc, t = plan.run(E4B128, E4B128, *shape)
             assert rc == 0 and "stream-k" not in t and "alloc" in t
@@ -190,12 +172,12 @@ def test_validation(plan):
     for t, n, k in ((1 << 31, 4, 64), (4, 1 << 31, 64), (4, 4, 1 << 31)):
         assert r(_sc(), _sc(), 2, t, n, k)[0] == UNSUPPORTED and "2^31" in err()
     assert r(_sc(), _sc(), 2, (1 << 31) - 1, (1 << 31) - 1, 64)[0] == UNSUPPORTED and "too many tiles" in err()
-    plan.opt("gemm.variant", "2sm_n256")
+    plan.option("gemm.variant", "2sm_n256")
     assert r(_sc(), _sc(), 2, 4, 4, 64)[0] == INVALID and "not a grouped matmul tile" in err()
-    plan.opt("gemm.variant", "auto")
-    plan.opt("gemm.epilogue", "stmatrix")
+    plan.option("gemm.variant", "auto")
+    plan.option("gemm.epilogue", "stmatrix")
     assert r(_sc(), _sc(), 2, 4, 4, 64)[0] == INVALID
-    plan.opt("gemm.epilogue", "tma")
+    plan.option("gemm.epilogue", "tma")
     # every block-scale dtype b200_dequantize reads, on a one- and a two-level side
     for dt in (F32, F16, BF16, UE8M0, F8E4M3):
         for tensor in (0, 1):

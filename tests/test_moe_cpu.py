@@ -11,6 +11,7 @@ import torch
 
 import moe_oracle as mo
 from cubecl_b200 import _ffi, moe
+from plan_context import PlanContext
 from qmatmul_oracle import fma_f32
 from test_conv_cpu import ROOT, _tool
 
@@ -123,19 +124,7 @@ def test_combine_backward_oracle_matches_autograd():
 
 
 # ---------------------------------------------------------------------------------------------- dry-run plans
-class Planner:
-    def __init__(self, sms=132):
-        self.lib = _ffi.load()
-        self.ctx = C.c_void_p()
-        _ffi.check(self.lib.b200_plan_begin(sms, C.byref(self.ctx)))
-
-    def text(self):
-        need = C.c_size_t()
-        _ffi.check(self.lib.b200_plan_text(self.ctx, None, 0, C.byref(need)))
-        buf = C.create_string_buffer(need.value)
-        _ffi.check(self.lib.b200_plan_text(self.ctx, buf, need.value, None))
-        return buf.value.decode()
-
+class Planner(PlanContext):
     def route(self, T, E, k, dt=F32, stride=None, bias=0, score=_ffi.MOE_SOFTMAX, renorm=1, n_group=0, topk_group=0, args=True,
               ptrs=(SRC, IDS, W)):
         a = _ffi.MoeRouteArgs(k, score, renorm, n_group, topk_group, 1.0)
@@ -163,15 +152,11 @@ class Planner:
                                                 ptrs[4], s[2], ptrs[5])
         return rc, self.text()
 
-    def close(self):
-        self.lib.b200_destroy(self.ctx)
-
 
 @pytest.fixture
 def plan():
-    p = Planner()
-    yield p
-    p.close()
+    with Planner() as p:
+        yield p
 
 
 def _launches(text):

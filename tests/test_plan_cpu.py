@@ -5,30 +5,13 @@ import ctypes as C
 import pytest
 
 from cubecl_b200 import _ffi
+from plan_context import PlanContext
 
 F32, F16, BF16, U32, I32, E4M3 = _ffi.F32, _ffi.F16, _ffi.BF16, _ffi.U32, _ffi.I32, _ffi.F8E4M3
 A, B, O = 0x10000000, 0x20000000, 0x30000000
 
 
-class Planner:
-    def __init__(self, sms=132):   # H100 SXM
-        self.lib = _ffi.load()
-        self.ctx = C.c_void_p()
-        _ffi.check(self.lib.b200_plan_begin(sms, C.byref(self.ctx)))
-
-    def close(self):
-        self.lib.b200_destroy(self.ctx)
-
-    def text(self):
-        need = C.c_size_t()
-        _ffi.check(self.lib.b200_plan_text(self.ctx, None, 0, C.byref(need)))
-        buf = C.create_string_buffer(need.value)
-        _ffi.check(self.lib.b200_plan_text(self.ctx, buf, need.value, None))
-        return buf.value.decode()
-
-    def option(self, k, v):
-        _ffi.check(self.lib.b200_set_option(self.ctx, k.encode(), str(v).encode()))
-
+class Planner(PlanContext):
     def matmul(self, idt, odt, ls, lst, rs, rst, os_, ost, a=A, b=B, o=O):
         rc = self.lib.b200_matmul(self.ctx, None, idt, odt, a, b, o, len(ls), _ffi.u64_array(ls), _ffi.u64_array(lst),
                                   _ffi.u64_array(rs), _ffi.u64_array(rst), _ffi.u64_array(os_), _ffi.u64_array(ost))
@@ -46,9 +29,8 @@ class Planner:
 
 @pytest.fixture
 def plan():
-    p = Planner()
-    yield p
-    p.close()
+    with Planner() as p:
+        yield p
 
 
 def cs(shape):

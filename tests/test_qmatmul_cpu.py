@@ -11,6 +11,7 @@ from pathlib import Path
 import numpy as np
 import pytest
 
+from plan_context import PlanContext
 import qmatmul_oracle as qmo
 import quant_oracle as qo
 from cubecl_b200 import _ffi
@@ -98,22 +99,7 @@ def test_oracle_fold_order_matches_a_scalar_loop():
 
 
 # ---------------------------------------------------------------------------------------------- dry-run plans
-class Planner:
-    def __init__(self, sms=132):   # H100 SXM
-        self.lib = _ffi.load()
-        self.ctx = C.c_void_p()
-        _ffi.check(self.lib.b200_plan_begin(sms, C.byref(self.ctx)))
-
-    def close(self):
-        self.lib.b200_destroy(self.ctx)
-
-    def text(self):
-        need = C.c_size_t()
-        _ffi.check(self.lib.b200_plan_text(self.ctx, None, 0, C.byref(need)))
-        buf = C.create_string_buffer(need.value)
-        _ffi.check(self.lib.b200_plan_text(self.ctx, buf, need.value, None))
-        return buf.value.decode()
-
+class Planner(PlanContext):
     def run(self, sa, sb, batch, m, n, k, odt=BF16, va=VA, vb=VB, out=OUT, ptrs=None):
         ca = sa if isinstance(sa, _ffi.QuantScheme) else sa.to_c()
         cb = sb if isinstance(sb, _ffi.QuantScheme) else sb.to_c()
@@ -126,9 +112,8 @@ class Planner:
 
 @pytest.fixture
 def plan():
-    p = Planner()
-    yield p
-    p.close()
+    with Planner() as p:
+        yield p
 
 
 def launches(text):
@@ -177,14 +162,14 @@ def test_plans(plan):
 
 def test_variants_and_no_stream_k(plan):
     # the per-block fold has 128-wide tiles only; a forced 2sm_n256 is refused, no stream-K head for either kind
-    plan.lib.b200_set_option(plan.ctx, b"gemm.variant", b"2sm_n256")
+    plan.option("gemm.variant", "2sm_n256")
     assert plan.run(Q8B128, Q8B128, 1, 1024, 1024, 1024)[0] == INVALID
     rc, t = plan.run(Q8T, Q8T, 1, 1024, 1024, 1024)
     assert rc == 0 and launches(t) == ["gemm_q8t_bf16_2sm_n256_kk"]
-    plan.lib.b200_set_option(plan.ctx, b"gemm.variant", b"1sm_n128")
+    plan.option("gemm.variant", "1sm_n128")
     rc, t = plan.run(Q8B128, Q8B128, 1, 1024, 1024, 1024)
     assert rc == 0 and launches(t)[-1] == "gemm_q8_bf16_1sm_n128_kk" and "smem=202752" in t
-    plan.lib.b200_set_option(plan.ctx, b"gemm.variant", b"auto")
+    plan.option("gemm.variant", "auto")
     for sa in (Q8T, Q8B128):
         rc, t = plan.run(sa, sa, 1, 8192 + 128, 8192, 4096)
         assert rc == 0 and "stream-k" not in t

@@ -11,6 +11,7 @@ from pathlib import Path
 import numpy as np
 import pytest
 
+from plan_context import PlanContext
 import quant_oracle as qo
 from cubecl_b200 import _ffi, synth
 from cubecl_b200.quant import QuantScheme
@@ -175,22 +176,7 @@ def test_quantize_oracle_round_trip():
 
 
 # ---------------------------------------------------------------------------------------------- dry-run plans
-class Planner:
-    def __init__(self, sms=132):   # H100 SXM
-        self.lib = _ffi.load()
-        self.ctx = C.c_void_p()
-        _ffi.check(self.lib.b200_plan_begin(sms, C.byref(self.ctx)))
-
-    def close(self):
-        self.lib.b200_destroy(self.ctx)
-
-    def text(self):
-        need = C.c_size_t()
-        _ffi.check(self.lib.b200_plan_text(self.ctx, None, 0, C.byref(need)))
-        buf = C.create_string_buffer(need.value)
-        _ffi.check(self.lib.b200_plan_text(self.ctx, buf, need.value, None))
-        return buf.value.decode()
-
+class Planner(PlanContext):
     def quantize(self, scheme, dt, shape, strides=None, a=A, v=V, s=S, t=T):
         sc = scheme if isinstance(scheme, _ffi.QuantScheme) else scheme.to_c()
         s = s if sc.block else 0
@@ -209,9 +195,8 @@ class Planner:
 
 @pytest.fixture
 def plan():
-    p = Planner()
-    yield p
-    p.close()
+    with Planner() as p:
+        yield p
 
 
 def launches(text):

@@ -11,6 +11,8 @@ import importlib.util
 import re
 from pathlib import Path
 
+from cubecl_b200._ffi import parse_header
+
 ROOT = Path(__file__).resolve().parent.parent
 spec = importlib.util.spec_from_file_location("gen_rust_sys", ROOT / "tools" / "gen_rust_sys.py")
 gen = importlib.util.module_from_spec(spec)
@@ -27,7 +29,7 @@ def test_sys_rs_is_what_the_header_generates():
 
 
 def test_every_header_function_is_bound_with_a_known_type():
-    _, _, _, protos = gen.parse(HEADER)
+    _, _, _, protos = parse_header(HEADER)
     names = [p[0] for p in protos]
     assert len(names) == len(set(names)) >= 51
     for name, _, args in protos:
@@ -56,7 +58,7 @@ def _call_args(text, start):
 
 
 def test_safe_layer_calls_match_the_prototypes():
-    _, _, _, protos = gen.parse(HEADER)
+    _, _, _, protos = parse_header(HEADER)
     arity = {name: len(args) for name, _, args in protos}
     calls = list(re.finditer(r"sys::(b200_\w+)\s*\(", LIB_RS))
     assert len(calls) >= 25
@@ -68,7 +70,7 @@ def test_safe_layer_calls_match_the_prototypes():
 
 
 def test_safe_layer_enums_carry_the_header_values():
-    _, enums, _, _ = gen.parse(HEADER)
+    _, enums, _, _ = parse_header(HEADER)
     header = {ename: dict(items) for ename, items in enums}
 
     def rust_enum(name):

@@ -1,6 +1,5 @@
 """CPU: the axis scans' oracle against the reference's plane-scan vectors, and the host plans of b200_scan (validation,
 view handling, single-pass vs three-pass choice, tile geometry) through a dry-run planning context."""
-import ctypes as C
 import json
 from pathlib import Path
 
@@ -8,6 +7,7 @@ import numpy as np
 import pytest
 
 from cubecl_b200 import _ffi
+from plan_context import PlanContext
 from scan_oracle import scan_axis_f32, scan_axis_f64
 
 F32, F16, BF16, U32 = _ffi.F32, _ffi.F16, _ffi.BF16, _ffi.U32
@@ -21,22 +21,7 @@ def scan_golden():
     return json.loads((Path(__file__).resolve().parent / "golden" / "scan_golden.json").read_text())
 
 
-class Planner:
-    def __init__(self, sms=132):   # H100 SXM
-        self.lib = _ffi.load()
-        self.ctx = C.c_void_p()
-        _ffi.check(self.lib.b200_plan_begin(sms, C.byref(self.ctx)))
-
-    def close(self):
-        self.lib.b200_destroy(self.ctx)
-
-    def text(self):
-        need = C.c_size_t()
-        _ffi.check(self.lib.b200_plan_text(self.ctx, None, 0, C.byref(need)))
-        buf = C.create_string_buffer(need.value)
-        _ffi.check(self.lib.b200_plan_text(self.ctx, buf, need.value, None))
-        return buf.value.decode()
-
+class Planner(PlanContext):
     def scan(self, op, dt, shape, axis, strides=None, odt=F32, exclusive=False, a=A, o=O):
         rc = self.lib.b200_scan(self.ctx, None, op, int(exclusive), dt, odt, a, o, len(shape), _ffi.u64_array(shape),
                                 _ffi.u64_array(strides) if strides else None, axis)
@@ -45,9 +30,8 @@ class Planner:
 
 @pytest.fixture
 def plan():
-    p = Planner()
-    yield p
-    p.close()
+    with Planner() as p:
+        yield p
 
 
 def launches(text):
