@@ -1138,8 +1138,6 @@ REDUCE_ALL(reduce_all_sum_f32_u4, OP_SUM, B200_F32, 4, false)
 REDUCE_ALL(reduce_all_sum_f32_u16, OP_SUM, B200_F32, 16, false)
 REDUCE_ALL(reduce_all_sum_f32_w2, OP_SUM, B200_F32, 2, true)
 REDUCE_ALL(reduce_all_sum_f32_w4, OP_SUM, B200_F32, 4, true)
-// the arg-reduction with more loads in flight (tuning variant)
-REDUCE_ALL(reduce_all_argmax_f32_u8, OP_ARGMAX, B200_F32, 8, false)
 
 // ================================================================================================ scans along an axis
 // cumsum / cumprod / cummax / cummin of the view [outer, len, inner] into a COMPACT row-major output of the same shape:

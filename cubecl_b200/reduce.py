@@ -4,6 +4,10 @@ cubecl-book/src/getting-started/src/bin/v1-cpu.rs:7-15).
 Reduces one axis (or every element with axis=None) of a tensor (any strides: pitched rows and transposed views are read in
 place, only views no stride description fits are compacted first); f32 accumulation; output f32 (values) or
 u32 (indices for argmax/argmin: ties -> lowest index, first NaN wins).  Kernels: csrc/reduce.cu.
+
+mean is rne_f32(S * f32(1 / len)) with S the f32 sum: the scale is applied once, to the whole sum, on every path (the
+all-elements grid stage, a one-pass axis kernel, the second pass of a split reduction or the end of the fused column finish).
+So on values whose partial sums are all exact (integers with sum |x| < 2^24) sum and mean are exact on every path.
 """
 from __future__ import annotations
 

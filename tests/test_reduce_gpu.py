@@ -286,7 +286,7 @@ def test_back_to_back_reductions_overlap_safely(client):
 
 def test_arg_reductions_special_values(client):
     # the integer-key form of the arg ops: -0.0 ties with +0.0, infinities order correctly, all-equal / all -inf inputs give
-    # index 0, NaN is the extreme for both ops, and two-pass (segmented) reductions agree with one-pass ones
+    # index 0, NaN is the extreme for both ops, and long rows and segmented columns agree with the oracle
     x = np.full(70001, -np.inf, dtype=np.float32)
     assert _run(client, x, None, "argmax")[0].tolist() == [0]
     assert _run(client, x, None, "argmin")[0].tolist() == [0]
@@ -296,7 +296,7 @@ def test_arg_reductions_special_values(client):
     assert _run(client, x, None, "argmax")[0].tolist() == [33]          # -0.0 == +0.0: the earlier one wins
     x[:] = 1.0; x[33] = 0.0; x[77] = -0.0
     assert _run(client, x, None, "argmin")[0].tolist() == [33]
-    x = synth.uniform_f32(3, 4 * (1 << 20), -1.0, 1.0).reshape(4, 1 << 20)     # few long rows: segmented + argcombine
+    x = synth.uniform_f32(3, 4 * (1 << 20), -1.0, 1.0).reshape(4, 1 << 20)     # few long rows (16 MB: one rows launch)
     x[1, 999999] = np.inf; x[2, 5] = -np.inf; x[3, 123456] = np.nan; x[3, 654321] = np.nan
     for op in ("argmax", "argmin"):
         got, vals = _run(client, x, 1, op)
