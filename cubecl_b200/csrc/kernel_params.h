@@ -601,3 +601,34 @@ constexpr int kMoeScanThreads = 1024;
 constexpr int kMoePermuteWarps = 8;    // rows per permute CTA, one warp each
 constexpr int kMoeThreads = 256;       // combine / combine-backward CTA; a thread owns 8 consecutive columns per step
 constexpr int kMoeBwdMaxN = 32768;     // the backward stages dy[t] as f32 in shared memory
+
+// ================================================================================================ norm.cu
+// RMSNorm / LayerNorm over the innermost axis (capi.cpp: b200_norm, b200_norm_quantized_fp8, b200_norm_backward).  Rows are
+// [t, n] with unit column stride; strides are in elements.  A row belongs to a group of nt threads in each of `ranks` CTAs;
+// it is split into 8-element chunks, chunk q going to thread q % (ranks * nt) of the group (rank q / nt % ranks) as that
+// thread's chunk q / (ranks * nt).  nt and ranks depend on n alone, and with them every sum's order:
+//   warp class (n <= kNormWarpMaxN):  nt = 32, ranks = 1: one warp per row, eight rows per CTA.
+//   CTA class (n > kNormWarpMaxN):    nt = 64, 128 or 256 (n <= 2048, 4096, larger), kNormThreads / nt rows per CTA; above
+//                                     8192 a cluster of ranks = 2 or 4 CTAs (n <= 16384, 32768) shares a row, the CTA
+//                                     totals exchanged through distributed shared memory.
+// A thread holds kNormChunks chunks (32 values) of a row in registers.  The backward gives each unit (a row group)
+// `rows_per_unit` consecutive rows; the unit sums dweight / dbias over them in row order in shared memory (its own columns
+// per thread) and writes f32 partials [units][n] (dweight) then [units][n] (dbias) to `part`, which norm_bwd_reduce adds in
+// unit order.
+struct NormParams {
+  uint64_t x, residual, h_out, weight, bias, y, mean, rstd;   // forward (backward: x = h)
+  uint64_t dy, d_h, dx, dweight, dbias, part;                 // backward
+  uint64_t block_scales;                                       // fp8 output: y = codes [t, n], block_scales [t, n / block]
+  uint64_t t, x_stride, residual_stride, h_stride, y_stride, dy_stride, d_h_stride, dx_stride;
+  uint32_t n, kind, w_f32, vec, nt, ranks, units, rows_per_unit;
+  uint32_t value, block, block_log2, scale_dt;   // fp8 output (b200_quant_scheme)
+  float eps;
+};
+constexpr int kNormThreads = 256;
+constexpr int kNormChunks = 4;         // 8-element chunks per thread: a warp covers 1024 columns, a CTA 8192
+constexpr int kNormWarpMaxN = 32 * 8 * kNormChunks;
+constexpr int kNormCtaMaxN = kNormThreads * 8 * kNormChunks;
+constexpr int kNormMaxN = 4 * kNormCtaMaxN;
+constexpr int kNormMaxGrid = 1 << 20;  // forward CTAs (clusters) beyond this loop over rows
+// backward accumulators in shared memory: dweight then dbias, [kNormChunks * 8][threads] f32 per unit; 64 KiB per CTA
+constexpr int kNormAccBytes = 2 * kNormChunks * 8 * kNormThreads * 4;

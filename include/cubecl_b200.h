@@ -477,6 +477,70 @@ int b200_moe_combine_backward(b200_ctx* ctx, b200_stream s, b200_dtype grad_dtyp
                               b200_dptr row_of, uint64_t t, uint64_t k, uint64_t n, b200_dptr d_ys, uint64_t d_ys_stride,
                               b200_dptr d_w);
 
+/* ---- RMSNorm and LayerNorm over the innermost axis, a fused residual add, an fp8 block-quantized output, and the backward ---
+ * Rows are [t, n], normalized over n; columns have unit stride, row strides are in elements and at least n.  1 <= n <= 32768
+ * (larger: B200_ERR_UNSUPPORTED), t < 2^31 (B200_ERR_UNSUPPORTED), t = 0 is a no-op.  rn() is one IEEE f32 rounding to
+ * nearest-even; nothing is contracted into an fma; sqrt and the division are IEEE (sqrt.rn, div.rn).
+ * Forward.  v = f32(h) with h = x, or with a residual h = RNE_x(f32(x) + f32(residual)), written to h_out (so the statistics
+ * come from the rounded h, and the fused call equals b200_norm on a separately computed h, bit for bit).
+ *   RMS:   ms = rn(S(rn(v * v)) / n); rstd = rn(1 / rn(sqrt(rn(ms + eps)))); x^ = rn(v * rstd).
+ *   Layer: mu = rn(S(v) / n); var = rn(S(rn(d * d)) / n) with d = rn(v - mu) (a second pass over the row, divided by n);
+ *          rstd as above; x^ = rn(rn(v - mu) * rstd).
+ *   y = RNE_y(rn(rn(x^ * w) + b)); a null weight is w = 1 and a null bias b = +0.  mean (Layer only) and rstd are optional
+ *   f32 [t] outputs (0 = not written).
+ * S() is a sum from +0 in an order fixed by n alone: the row is cut into 8-element chunks, chunk q going to thread
+ * q % (R * T) of a group of T threads in each of R CTAs (T = 32, 64, 128 for n <= 1024, 2048, 4096, else 256; R = 1, 2, 4 for
+ * n <= 8192, 16384, 32768); each thread adds its values in column order, then an xor butterfly over each warp (offsets 16, 8,
+ * 4, 2, 1), the group's warps in order, the CTAs in order.  So the result of a row does not depend on t, on the row's position, on
+ * pointer alignment (the 128-bit and the element-wise path give the same bits) or on the GPU: every row is batch-invariant,
+ * and every call is bitwise reproducible.
+ * dtypes: x_dtype F32 / BF16 / F16 for x, residual and h_out; w_dtype F32 or x_dtype for weight and bias; y F32 / BF16 / F16.
+ * Errors: B200_ERR_INVALID_ARG for a null args, x, y (values and block_scales) or rstd pointer where required, misaligned
+ * pointers (to their element size), a stride below n, n = 0, an unknown kind or dtype combination, eps < 0 or NaN, a residual
+ * without h_out (or h_out without a residual), a bias or a mean output with RMS.  Launches: one norm_fwd_<x>_<y>_<warp|cta>
+ * (128-bit access when every pointer and row is 16-byte aligned and n % 8 == 0); clusters of R CTAs for n > 8192.  Every
+ * call is stream-ordered and never synchronises with the host. */
+typedef enum b200_norm_kind { B200_NORM_RMS = 0, B200_NORM_LAYER = 1 } b200_norm_kind;
+typedef struct b200_norm_args {
+  int32_t kind;      /* b200_norm_kind */
+  int32_t x_dtype;   /* b200_dtype of x, residual and h_out (and h in the backward): F32, BF16 or F16 */
+  int32_t w_dtype;   /* b200_dtype of weight and bias: F32 or x_dtype */
+  float eps;         /* >= 0 */
+} b200_norm_args;
+int b200_norm(b200_ctx* ctx, b200_stream s, const b200_norm_args* args, b200_dtype y_dtype, uint64_t t, uint64_t n,
+              b200_dptr x, uint64_t x_stride, b200_dptr residual, uint64_t residual_stride, b200_dptr h_out, uint64_t h_stride,
+              b200_dptr weight, b200_dptr bias, b200_dptr y, uint64_t y_stride, b200_dptr mean, b200_dptr rstd);
+/* b200_norm with y stored as fp8 codes and block scales, bit for bit what b200_quantize(scheme, y_f32) writes for y_f32 =
+ * b200_norm's F32 output of the same call: values compact [t, n] bytes, block_scales compact [t, n / block].  The result
+ * feeds b200_matmul_quantized_fp8 (and, through b200_moe_permute, b200_matmul_grouped_quantized_fp8) unchanged.  It moves
+ * less memory than b200_norm + b200_quantize (no 16-bit activation is written and read back) but, as measured (README), it is
+ * not yet faster than that pair: its per-element encode costs more than the traffic it saves.  Schemes: value E4M3 or E5M2, block 32,
+ * 64 or 128 with n % block == 0, block_scale F32 or UE8M0, tensor_scale 0; other values, blocks, scale dtypes or a
+ * block-less scheme are B200_ERR_INVALID_ARG, and a tensor level, which needs the whole tensor's amax before any row can be
+ * encoded, is B200_ERR_UNSUPPORTED.  One norm_fwd_<x>_fp8_<warp|cta> launch. */
+int b200_norm_quantized_fp8(b200_ctx* ctx, b200_stream s, const b200_norm_args* args, const b200_quant_scheme* scheme,
+                            uint64_t t, uint64_t n, b200_dptr x, uint64_t x_stride, b200_dptr residual, uint64_t residual_stride,
+                            b200_dptr h_out, uint64_t h_stride, b200_dptr weight, b200_dptr bias, b200_dptr values,
+                            b200_dptr block_scales, b200_dptr mean, b200_dptr rstd);
+/* Backward.  h [t, n] (x_dtype: what the forward normalized), weight (w_dtype, or 0 for w = 1), the forward's f32 rstd [t]
+ * (and mean [t] for Layer), dy [t, n] in grad_dtype (F32 / BF16 / F16).  Per row, with x^ recomputed exactly as the forward
+ * did and g = rn(f32(dy) * w):
+ *   c1 = rn(S(rn(g * x^)) / n);  c2 = rn(S(g) / n) (Layer);  S() the forward's order;
+ *   e = rn(g - rn(x^ * c1)); Layer: e = rn(e - c2); d = rn(rstd * e); with d_h: d = rn(d + f32(d_h)); dx = RNE_grad(d).
+ * d_h [t, n] (grad_dtype, optional) is the gradient already flowing along the residual stream; with a fused residual, dx is
+ * then the gradient of both x and the residual.  dx rows are batch-invariant like the forward's.
+ * dweight = S_t(rn(f32(dy) * x^)) and dbias = S_t(f32(dy)), f32 [n], either optional: the t rows are cut into U units of
+ * ceil(t / U) consecutive rows (U = min(t, clamp(2^21 / n, 64, 1024)) recomputed as ceil(t / ceil(t / U))); a unit sums its
+ * rows in order from +0, and norm_bwd_reduce adds the units' partials in order.  U depends on t and n only, so dweight is
+ * reproducible for a shape on any GPU.  No atomics.  One pooled f32 temporary [2][U][n] when dweight or dbias is asked for.
+ * Errors: B200_ERR_INVALID_ARG for a null args, h, dy, dx, rstd (or Layer mean) pointer, misaligned pointers, a stride below
+ * n, n = 0, an unknown kind or dtype combination, eps < 0 or NaN (eps is not read), a dbias with RMS; limits as the forward.
+ * Launches: norm_bwd_<x>_<grad>_<warp|cta> (64 KiB of shared memory), then norm_bwd_reduce when dweight or dbias is given. */
+int b200_norm_backward(b200_ctx* ctx, b200_stream s, const b200_norm_args* args, b200_dtype grad_dtype, uint64_t t, uint64_t n,
+                       b200_dptr dy, uint64_t dy_stride, b200_dptr h, uint64_t h_stride, b200_dptr weight, b200_dptr mean,
+                       b200_dptr rstd, b200_dptr d_h, uint64_t d_h_stride, b200_dptr dx, uint64_t dx_stride, b200_dptr dweight,
+                       b200_dptr dbias);
+
 /* ---- 2-D convolution (cubek's convolution kernels), an implicit GEMM on the wgmma kernel --------------------------------
  * out[n, oh, ow, co] = act(alpha * sum_{ky, kx, c} x[n, oh*sh - ph + ky*dh, ow*sw - pw + kx*dw, c] * w[co, ky, kx, c] + bias[co]).
  * Input outside x reads as zero; f32 accumulation; the epilogue is b200_epilogue (NULL = none).  x is [N, H, W, C] (NHWC), w is

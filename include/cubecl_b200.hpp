@@ -15,6 +15,7 @@
 #pragma once
 #include <cstdint>
 #include <cstring>
+#include <initializer_list>
 #include <memory>
 #include <stdexcept>
 #include <string>
@@ -725,6 +726,56 @@ inline void combine_backward(ComputeClient& client, const TensorHandle& dy, cons
   if (rc != B200_OK) client.defer(b200_last_error());
 }
 }  // namespace moe
+
+namespace norm {
+/// RMSNorm / LayerNorm over the last axis; the contracts are those of b200_norm* in cubecl_b200.h.  Tensors are 2-D [T, n]
+/// with unit column stride; weight, bias, mean, rstd and the gradients of weight and bias are device pointers (0 = absent).
+/// residual and h_out are both given (the fused residual add) or both null.  Errors are deferred to client.sync().
+using Args = b200_norm_args;
+inline bool rows2d(ComputeClient& client, const char* what, std::initializer_list<const TensorHandle*> ts) {
+  for (const TensorHandle* t : ts)
+    if (t && t->shape.size() != 2) {
+      client.defer(std::string("InvalidArgument: ") + what + " needs 2-D [T, n] tensors");
+      return false;
+    }
+  return true;
+}
+/// y = norm(h) * weight (+ bias), h = x, or h = x + residual (rounded to x's dtype) written to h_out.
+inline void forward(ComputeClient& client, const Args& args, const TensorHandle& x, const TensorHandle& y, b200_dptr weight,
+                    b200_dptr bias = 0, const TensorHandle* residual = nullptr, const TensorHandle* h_out = nullptr,
+                    b200_dptr mean = 0, b200_dptr rstd = 0) {
+  if (!rows2d(client, "norm", {&x, &y, residual, h_out})) return;
+  const int rc = b200_norm(client.raw(), nullptr, &args, static_cast<b200_dtype>(y.dtype), x.shape[0], x.shape[1], x.handle.ptr(),
+                           x.strides[0], residual ? residual->handle.ptr() : 0, residual ? residual->strides[0] : x.shape[1],
+                           h_out ? h_out->handle.ptr() : 0, h_out ? h_out->strides[0] : x.shape[1], weight, bias, y.handle.ptr(),
+                           y.strides[0], mean, rstd);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+/// forward() with y stored as fp8 codes [T, n] and block scales [T, n / block], exactly as b200_quantize(scheme) writes them.
+inline void forward_quantized_fp8(ComputeClient& client, const Args& args, const b200_quant_scheme& scheme, const TensorHandle& x,
+                                  b200_dptr values, b200_dptr block_scales, b200_dptr weight, b200_dptr bias = 0,
+                                  const TensorHandle* residual = nullptr, const TensorHandle* h_out = nullptr, b200_dptr mean = 0,
+                                  b200_dptr rstd = 0) {
+  if (!rows2d(client, "norm_quantized_fp8", {&x, residual, h_out})) return;
+  const int rc = b200_norm_quantized_fp8(client.raw(), nullptr, &args, &scheme, x.shape[0], x.shape[1], x.handle.ptr(), x.strides[0],
+                                         residual ? residual->handle.ptr() : 0, residual ? residual->strides[0] : x.shape[1],
+                                         h_out ? h_out->handle.ptr() : 0, h_out ? h_out->strides[0] : x.shape[1], weight, bias,
+                                         values, block_scales, mean, rstd);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+/// dx (dy's dtype; plus d_h when given), dweight and dbias (f32 [n], 0 = not computed) from dy, the forward's h, weight, rstd
+/// (and mean for LayerNorm).
+inline void backward(ComputeClient& client, const Args& args, const TensorHandle& dy, const TensorHandle& h, b200_dptr weight,
+                     b200_dptr mean, b200_dptr rstd, const TensorHandle& dx, const TensorHandle* d_h = nullptr, b200_dptr dweight = 0,
+                     b200_dptr dbias = 0) {
+  if (!rows2d(client, "norm_backward", {&dy, &h, &dx, d_h})) return;
+  const int rc = b200_norm_backward(client.raw(), nullptr, &args, static_cast<b200_dtype>(dy.dtype), h.shape[0], h.shape[1],
+                                    dy.handle.ptr(), dy.strides[0], h.handle.ptr(), h.strides[0], weight, mean, rstd,
+                                    d_h ? d_h->handle.ptr() : 0, d_h ? d_h->strides[0] : h.shape[1], dx.handle.ptr(), dx.strides[0],
+                                    dweight, dbias);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+}  // namespace norm
 
 namespace quant {
 /// QuantScheme (value, block level, per-tensor level); see b200_quantize in cubecl_b200.h for the contract.

@@ -976,6 +976,61 @@ impl Context {
         ))
     }
 
+    /// RMSNorm / LayerNorm of rows `x` [t, n] (x_stride elements apart) into `y` (`y_dtype`), with an optional fused residual
+    /// (`residual` and `h_out` both non-zero: h = x + residual rounded to x's dtype, written to `h_out`); `weight`, `bias`,
+    /// `mean` and `rstd` may be 0.  The contract is `b200_norm`'s in include/cubecl_b200.h.
+    ///
+    /// # Safety
+    /// Every pointer must be 0 where the contract allows it, or a live device allocation of this context large enough for
+    /// its extents and strides.
+    #[allow(clippy::too_many_arguments)]
+    pub unsafe fn norm(
+        &mut self, stream: b200_stream, args: &sys::b200_norm_args, y_dtype: DType, t: u64, n: u64, x: b200_dptr, x_stride: u64,
+        residual: b200_dptr, residual_stride: u64, h_out: b200_dptr, h_stride: u64, weight: b200_dptr, bias: b200_dptr,
+        y: b200_dptr, y_stride: u64, mean: b200_dptr, rstd: b200_dptr,
+    ) -> Result<(), Error> {
+        check(sys::b200_norm(
+            self.0, stream, args, y_dtype as c_int, t, n, x, x_stride, residual, residual_stride, h_out, h_stride, weight, bias, y,
+            y_stride, mean, rstd,
+        ))
+    }
+
+    /// [`Context::norm`] with y stored as fp8 codes `values` [t, n] and `block_scales` [t, n / block], bit for bit what
+    /// `b200_quantize(scheme)` writes for the f32 output.  See `b200_norm_quantized_fp8`.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::norm`].
+    #[allow(clippy::too_many_arguments)]
+    pub unsafe fn norm_quantized_fp8(
+        &mut self, stream: b200_stream, args: &sys::b200_norm_args, scheme: &QuantScheme, t: u64, n: u64, x: b200_dptr,
+        x_stride: u64, residual: b200_dptr, residual_stride: u64, h_out: b200_dptr, h_stride: u64, weight: b200_dptr,
+        bias: b200_dptr, values: b200_dptr, block_scales: b200_dptr, mean: b200_dptr, rstd: b200_dptr,
+    ) -> Result<(), Error> {
+        let raw = scheme.raw();
+        check(sys::b200_norm_quantized_fp8(
+            self.0, stream, args, &raw, t, n, x, x_stride, residual, residual_stride, h_out, h_stride, weight, bias, values,
+            block_scales, mean, rstd,
+        ))
+    }
+
+    /// Gradients of [`Context::norm`]: `dx` [t, n] in `grad_dtype` (plus `d_h`, the residual stream's gradient, when
+    /// non-zero), `dweight` and `dbias` f32 [n] (0 = not computed), from `dy`, the forward's `h`, `weight`, `rstd` and, for
+    /// LayerNorm, `mean`.  See `b200_norm_backward`.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::norm`].
+    #[allow(clippy::too_many_arguments)]
+    pub unsafe fn norm_backward(
+        &mut self, stream: b200_stream, args: &sys::b200_norm_args, grad_dtype: DType, t: u64, n: u64, dy: b200_dptr,
+        dy_stride: u64, h: b200_dptr, h_stride: u64, weight: b200_dptr, mean: b200_dptr, rstd: b200_dptr, d_h: b200_dptr,
+        d_h_stride: u64, dx: b200_dptr, dx_stride: u64, dweight: b200_dptr, dbias: b200_dptr,
+    ) -> Result<(), Error> {
+        check(sys::b200_norm_backward(
+            self.0, stream, args, grad_dtype as c_int, t, n, dy, dy_stride, h, h_stride, weight, mean, rstd, d_h, d_h_stride, dx,
+            dx_stride, dweight, dbias,
+        ))
+    }
+
     /// Quantize `input` ([..., K], F32 / F16 / BF16, any strides) along its innermost axis under `scheme` into compact
     /// codes [..., K * bits / 8], block scales [..., K / block] and the f32 tensor scale (0 for an absent level); the
     /// contract is `b200_quantize`'s in include/cubecl_b200.h.
