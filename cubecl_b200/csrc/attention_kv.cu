@@ -30,6 +30,7 @@
 
 #include "attention.cuh"
 #include "kernel_params.h"
+#include "kv_quant.cuh"
 #include "ptx.cuh"
 
 using namespace b200;
@@ -479,27 +480,6 @@ ATTN_KV_F8_D(bf16, KIND_BF16, OUT_BF16, e5m2, CF_E5M2)
 ATTN_KV_F8_COMBINE(attn_kv_combine_fp8_f16, OUT_F16)
 ATTN_KV_F8_COMBINE(attn_kv_combine_fp8_bf16, OUT_BF16)
 ATTN_KV_F8_COMBINE(attn_kv_combine_fp8_f32, OUT_F32)
-
-// One 16-bit value -> f32, exactly.
-__device__ __forceinline__ float kv_in_f32(uint32_t h, bool bf16) {
-  return bf16 ? __uint_as_float(h << 16) : __half2float(__ushort_as_half(static_cast<unsigned short>(h)));
-}
-
-// Eight 16-bit values (16 bytes) -> eight fp8 bytes: sat_rn(x / s) per value (f32 division rounded to nearest, then RNE to
-// the cache format with satfinite: +-448 (e4m3) or +-57344 (e5m2) for larger magnitudes, NaN stays NaN).
-__device__ __forceinline__ uint2 kv_quant8(uint4 x, float s, bool bf16, bool e5m2) {
-  const uint32_t w[4] = {x.x, x.y, x.z, x.w};
-  uint32_t q[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const float lo = __fdiv_rn(kv_in_f32(w[i] & 0xFFFFu, bf16), s), hi = __fdiv_rn(kv_in_f32(w[i] >> 16, bf16), s);
-    unsigned short r;
-    if (e5m2) asm("cvt.rn.satfinite.e5m2x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
-    else asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
-    q[i] = r;
-  }
-  return make_uint2(q[0] | (q[1] << 16), q[2] | (q[3] << 16));
-}
 
 // Scatter of new tokens into an fp8 cache, quantized with per-head scales: 16-byte loads and 8-byte stores, grid-stride.
 extern "C" __global__ void __launch_bounds__(256) attn_kv_write_fp8(const __grid_constant__ AttnKvWriteParams p) {

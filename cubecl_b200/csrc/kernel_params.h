@@ -632,3 +632,40 @@ constexpr int kNormMaxN = 4 * kNormCtaMaxN;
 constexpr int kNormMaxGrid = 1 << 20;  // forward CTAs (clusters) beyond this loop over rows
 // backward accumulators in shared memory: dweight then dbias, [kNormChunks * 8][threads] f32 per unit; 64 KiB per CTA
 constexpr int kNormAccBytes = 2 * kNormChunks * 8 * kNormThreads * 4;
+
+// ================================================================================================ rope.cu
+// Rotary position embeddings (capi.cpp: b200_rope, b200_rope_kvcache_write, b200_rope_cos_sin).  q is [B, S, Hq, D] and k
+// [B, S, Hk, D] with unit D stride; strides are in elements.  Token n = b * S + s has position positions[n] (s when null) and
+// reads row p of the f32 table cos_sin [P, rot] (cos in columns [0, rot/2), sin in [rot/2, rot)).  A token is worked on by
+// `groups` threads, each looping over the q heads, then the k heads (then, writing a cache, the v heads) of that token:
+//   [0, gr)            gr = ceil(rot/2 / 8): 8 pair-columns each; its 8 cos and 8 sin stay in registers for every head
+//   [gr, gr + gp)      gp = ceil((D - rot) / 8) when some output is out of place (else 0): 8 pass-through columns each
+//   [gr + gp, groups)  writing a cache: D / 8 columns of v each
+// Units are n * groups + group, walked grid-stride by at most kRopeCtasPerSm (kRopeKvCtasPerSm) * SMs CTAs of kRopeThreads:
+// one wave of resident CTAs.
+struct RopeParams {
+  uint64_t q, k, qo, ko, positions, cos_sin;
+  uint64_t q_sb, q_ss, q_sh, k_sb, k_ss, k_sh, qo_sb, qo_ss, qo_sh, ko_sb, ko_ss, ko_sh;
+  uint64_t tokens, units;                      // B * S, tokens * groups
+  uint32_t S, Hq, Hk, D, rot, half, P, inverse;
+  uint32_t gr, gp, groups, vec;                // vec: 16-byte access of q, k, their outputs, v and the table
+  uint32_t pass_q, pass_k;                     // q / k go out of place (k into a cache always): pass-through columns and
+                                               // out-of-range rows are copied; in place they are not touched
+  // b200_rope_kvcache_write: k goes to the caches, not to ko.  Caches [P, page, Hkv, D]; slot rules of AttnKvWriteParams.
+  uint64_t vn, vn_sb, vn_ss, vn_sh, kc, vc, slots, k_scale, v_scale;
+  uint64_t kc_sp, kc_sr, kc_sh, vc_sp, vc_sr, vc_sh, slot_end;
+  uint32_t page, in_bf16, e5m2, vvec;          // vvec: 16-byte loads of v_new
+};
+constexpr int kRopeThreads = 256;
+constexpr int kRopeCtasPerSm = 4;     // b200_rope: 64 registers per thread, four 256-thread CTAs fill an SM's register file
+constexpr int kRopeKvCtasPerSm = 3;   // b200_rope_kvcache_write: up to 85 registers (the cache addressing and the fp8 encode)
+constexpr int kRopeMaxD = 512;
+
+// b200_rope_cos_sin: cos_sin[p, i] = rn_f32(af * cos(p * inv_freq_i)), cos_sin[p, half + i] = rn_f32(af * sin(...)), every
+// step in f64; one thread per (p, i), grid-stride.  The host works out the per-call scalars in f64: the attention factor af
+// and YaRN's ramp [ramp_lo, ramp_hi] (after truncation and clamping).
+struct RopeTableParams {
+  uint64_t out, inv_freq, n;                   // n = P * half
+  uint32_t half, kind;
+  double base, factor, low_ff, high_ff, orig, ramp_lo, ramp_hi, af;
+};

@@ -541,6 +541,111 @@ int b200_norm_backward(b200_ctx* ctx, b200_stream s, const b200_norm_args* args,
                        b200_dptr rstd, b200_dptr d_h, uint64_t d_h_stride, b200_dptr dx, uint64_t dx_stride, b200_dptr dweight,
                        b200_dptr dbias);
 
+/* ---- rotary position embeddings (RoPE): rotate q and k, the backward, a fused rotate-and-cache-write, and the tables ---
+ * q is [B, S, Hq, D] and k [B, S, Hk, D] (shapes and strides in elements, NULL strides = compact; Hq and Hk independent, so
+ * GQA and MQA); any view with a unit D stride works in place: [B, H, S, D] head-major tensors, packed [T, H, D] as B = 1,
+ * and the q / k slices of a fused [T, 3, H, D] or [T, Hq + 2 Hk, D] projection.  dtype F32, BF16 or F16, shared by q, k and
+ * the outputs.  Token (b, s) has position p = positions[b * S + s] (a compact i32 [B, S] device array, read by the kernel
+ * only: no host synchronisation, graph-capturable; NULL: p = s).  Decoding passes cache_seqlens before the step; chunked
+ * prefill passes each token's absolute position.
+ * Table: cos_sin is a compact f32 [P, rot_dim] device array, cos in columns [0, rot_dim/2) and sin in [rot_dim/2, rot_dim)
+ * (vLLM's cos_sin_cache layout).  Any table is accepted; b200_rope_cos_sin builds the standard ones.
+ * Style: B200_ROPE_NEOX pairs columns (i, i + rot_dim/2) (HF's rotate_half); B200_ROPE_GPTJ pairs (2i, 2i + 1) (flash-attn's
+ * interleaved=True).  Columns [rot_dim, D) pass through (partial rotary: GPT-NeoX-20B's 24 of 96, Phi's 32 of 80).
+ * Numerics, for each pair (a, b) widened exactly to f32, c = cos_sin[p, i] and s = cos_sin[p, rot_dim/2 + i]:
+ *   a' = rn(rn(a * c) - rn(b * s)),   b' = rn(rn(b * c) + rn(a * s)),
+ * every product and sum a separately rounded f32 operation (nothing is contracted into an fma), then rounded to nearest-even
+ * once to the dtype.  inverse = 1 is the same with s negated, bit for bit: the rotation by -theta, which is the backward (dq,
+ * dk from the gradients of the rotated q, k).  So each element's bits depend only on (a, b, c, s): results are batch-invariant,
+ * independent of the view, the alignment (the 16-byte and the element-wise path give the same bits) and the GPU.  They are
+ * not HF's bits: HF rounds cos and sin to bf16 and rounds each bf16 operation; this contract rounds once.  A rotated pair
+ * holding a NaN gives NaN, its payload the GPU's.
+ * Out-of-range positions: a token with p < 0 or p >= P keeps its rows bit for bit (copied out of place, untouched in place);
+ * it is not rotated by angle 0, which would flip -0 and turn inf * 0 into NaN.
+ * Outputs: q_out / k_out NULL rotate in place (pass-through columns untouched); otherwise they are views of the same shape
+ * with their own strides (pass-through columns copied).  An output that shares memory with an input other than its own
+ * identical view gives unspecified values.
+ * Limits: D <= 512, extents < 2^31.
+ * Errors: B200_ERR_INVALID_ARG for a null args pointer, q and k both NULL, a null shape, a mismatch in B, S or D between q and
+ * k or between an input and its output, an odd rot_dim or one outside [2, D], an unknown style, P = 0 when there are tokens,
+ * a null or misaligned (4-byte) cos_sin, a misaligned positions, a view not aligned to its element size;
+ * B200_ERR_UNSUPPORTED for the dtype, a non-unit D stride, D > 512, an extent >= 2^31.  No token or no head: no launch.
+ * Launch: one rope_<f32|bf16|f16>_<neox|gptj> of at most 4 * SMs CTAs of 256 threads, grid-stride.  A token belongs to
+ * ceil(rot_dim/2 / 8) threads that own 8 pair-columns each (plus ceil((D - rot_dim) / 8) pass-through threads when an output
+ * is out of place); a thread keeps its 8 cos and 8 sin in registers and loops over all Hq + Hk heads of the token.  16-byte
+ * access when every base and stride is 16-byte aligned and rot_dim/2 % 8 == 0, else element-wise.  The dry-run plan records
+ * one "rope" line (groups, vec) before the launch. */
+typedef enum b200_rope_style { B200_ROPE_NEOX = 0, B200_ROPE_GPTJ = 1 } b200_rope_style;
+typedef struct b200_rope_args {
+  int32_t style;     /* b200_rope_style */
+  int32_t rot_dim;   /* even, 2 <= rot_dim <= D */
+  int32_t inverse;   /* 1: rotate by -theta (the backward) */
+} b200_rope_args;
+int b200_rope(b200_ctx* ctx, b200_stream s, const b200_rope_args* args, b200_dtype dtype,
+              b200_dptr q, const uint64_t* q_shape, const uint64_t* q_strides,
+              b200_dptr k, const uint64_t* k_shape, const uint64_t* k_strides,
+              b200_dptr q_out, const uint64_t* qo_shape, const uint64_t* qo_strides,
+              b200_dptr k_out, const uint64_t* ko_shape, const uint64_t* ko_strides,
+              b200_dptr positions, b200_dptr cos_sin, uint64_t P);
+/* The decode and prefill step in one launch (vLLM's rotary_embedding + reshape_and_cache): q [B, Snew, Hq, D] is rotated in
+ * place or into q_out (q may be NULL), k_new is rotated and written to k_cache, v_new is written to v_cache unrotated;
+ * k_new and v_new [B, Snew, Hkv, D] are only read.  Caches [P_pages, page, Hkv, D], slot_mapping, the skipped slots (< 0 or
+ * >= P_pages * page), the cache views and errors are b200_kvcache_write's (dtype F16 or BF16, D % 8 == 0, caches read in
+ * place); k_new and v_new are read in place too, never gathered, so they need a unit D stride (B200_ERR_UNSUPPORTED);
+ * args, positions, the table and their errors are b200_rope's.  cache_dtype is dtype (a 16-bit cache) or B200_F8E4M3 /
+ * B200_F8E5M2 with k_scale / v_scale compact f32 [Hkv] (b200_kvcache_write_fp8's rules and errors).
+ * Contract: bit for bit equal to b200_rope(q, k_new) followed by b200_kvcache_write (or b200_kvcache_write_fp8) of the
+ * rotated k_new.  So with an fp8 cache K is rounded to dtype first and then stored as sat_rn(x / k_scale[hk]).
+ * Launch: one rope_kv_<bf16|f16>_<neox|gptj> (16-bit cache) or rope_kv_fp8_<bf16|f16>_<neox|gptj>; b200_rope's threads per
+ * token (pass-through threads whenever rot_dim < D, since k always goes out of place) plus D / 8 threads for v, at most
+ * 3 * SMs CTAs.  As measured (README) it beats the unfused pair when decoding, where it saves a launch, but not yet on a
+ * prefill chunk, although it moves fewer bytes. */
+int b200_rope_kvcache_write(b200_ctx* ctx, b200_stream s, const b200_rope_args* args, b200_dtype dtype, b200_dtype cache_dtype,
+                            b200_dptr q, const uint64_t* q_shape, const uint64_t* q_strides,
+                            b200_dptr q_out, const uint64_t* qo_shape, const uint64_t* qo_strides,
+                            b200_dptr k_new, const uint64_t* kn_shape, const uint64_t* kn_strides,
+                            b200_dptr v_new, const uint64_t* vn_shape, const uint64_t* vn_strides,
+                            b200_dptr k_cache, const uint64_t* kc_shape, const uint64_t* kc_strides,
+                            b200_dptr v_cache, const uint64_t* vc_shape, const uint64_t* vc_strides,
+                            b200_dptr slot_mapping, b200_dptr positions, b200_dptr cos_sin, uint64_t P,
+                            b200_dptr k_scale, b200_dptr v_scale);
+/* Build the table on the device: cos_sin[p, i] = rn_f32(af * cos(p * inv_freq_i)) and cos_sin[p, rot_dim/2 + i] =
+ * rn_f32(af * sin(p * inv_freq_i)) for p < P, i < rot_dim/2, with the angle, cos, sin and the product by the attention
+ * factor af all in f64, rounded once to f32.  (HF forms the angle in f32, which at position 10^5 is off by about 4e-3 rad;
+ * a caller who wants HF's table passes their own.)  inv_freq_i by kind, in f64 (transformers' rope_parameters rules):
+ *   DEFAULT   base^(-2i / rot_dim);
+ *   LINEAR    DEFAULT / factor;
+ *   LLAMA3    wavelength w = 2 pi / DEFAULT: w < orig / high_freq_factor keeps DEFAULT, w > orig / low_freq_factor takes
+ *             DEFAULT / factor, between: (1 - m) DEFAULT / factor + m DEFAULT with m = (orig / w - low) / (high - low);
+ *   YARN      ramp r_i = clamp((i - lo) / (hi - lo), 0, 1) with lo, hi = dim(beta_fast), dim(beta_slow), dim(x) =
+ *             rot_dim ln(orig / (2 pi x)) / (2 ln base), floored / ceiled when truncate, clamped to [0, rot_dim - 1], hi +=
+ *             0.001 when equal; inv = DEFAULT / factor * r_i + DEFAULT * (1 - r_i); beta_fast 0 means 32, beta_slow 0 means 1;
+ *   INV_FREQ  the caller's f32 [rot_dim/2] device array inv_freq (longrope, dynamic NTK, anything else).
+ * (orig = original_max_position_embeddings.)  attention_factor <= 0 means the rule's default: 1, or for YARN
+ * g(factor, mscale) / g(factor, mscale_all_dim) when both are nonzero (DeepSeek), else g(factor, 1), with g(f, m) = 1 for
+ * f <= 1 and 0.1 m ln f + 1 otherwise.
+ * Errors: B200_ERR_INVALID_ARG for a null args or cos_sin (P > 0), a misaligned cos_sin or inv_freq, an odd rot_dim or one
+ * outside [2, 512], a non-finite or non-positive base (not read by INV_FREQ), factor < 1 (LINEAR, LLAMA3, YARN), LLAMA3
+ * without 0 < low_freq_factor < high_freq_factor, LLAMA3 / YARN without original_max_position_embeddings > 0, an unknown
+ * kind, a null inv_freq for INV_FREQ; B200_ERR_UNSUPPORTED for P >= 2^31.  P = 0: no launch.  One rope_cos_sin launch. */
+typedef enum b200_rope_scaling {
+  B200_ROPE_DEFAULT = 0, B200_ROPE_LINEAR = 1, B200_ROPE_LLAMA3 = 2, B200_ROPE_YARN = 3, B200_ROPE_INV_FREQ = 4
+} b200_rope_scaling;
+typedef struct b200_rope_table_args {
+  b200_dptr inv_freq;                          /* INV_FREQ: f32 [rot_dim / 2] */
+  int32_t kind;                                /* b200_rope_scaling */
+  int32_t rot_dim;
+  float base;                                  /* rope_theta */
+  float factor;                                /* LINEAR, LLAMA3, YARN */
+  float low_freq_factor, high_freq_factor;     /* LLAMA3 */
+  float beta_fast, beta_slow;                  /* YARN (0: 32 and 1) */
+  float mscale, mscale_all_dim;                /* YARN's attention factor (0: absent) */
+  float attention_factor;                      /* <= 0: the rule's default */
+  int32_t original_max_position_embeddings;    /* LLAMA3, YARN */
+  int32_t truncate;                            /* YARN: 1 floors / ceils the ramp bounds (HF's default) */
+} b200_rope_table_args;
+int b200_rope_cos_sin(b200_ctx* ctx, b200_stream s, const b200_rope_table_args* args, uint64_t P, b200_dptr cos_sin);
+
 /* ---- 2-D convolution (cubek's convolution kernels), an implicit GEMM on the wgmma kernel --------------------------------
  * out[n, oh, ow, co] = act(alpha * sum_{ky, kx, c} x[n, oh*sh - ph + ky*dh, ow*sw - pw + kx*dw, c] * w[co, ky, kx, c] + bias[co]).
  * Input outside x reads as zero; f32 accumulation; the epilogue is b200_epilogue (NULL = none).  x is [N, H, W, C] (NHWC), w is

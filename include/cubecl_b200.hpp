@@ -727,6 +727,56 @@ inline void combine_backward(ComputeClient& client, const TensorHandle& dy, cons
 }
 }  // namespace moe
 
+namespace rope {
+/// Rotary position embeddings; the contracts are those of b200_rope* in cubecl_b200.h.  q, k and the outputs are 4-D
+/// [B, S, H, D] views (null: absent; null outputs rotate in place), positions a compact i32 [B, S] and cos_sin a compact f32
+/// [P, rot_dim] device array (0 = positions s).  Errors are deferred to client.sync().
+using Args = b200_rope_args;
+using TableArgs = b200_rope_table_args;
+inline const uint64_t* shape_of(const TensorHandle* t) { return t ? t->shape.data() : nullptr; }
+inline const uint64_t* strides_of(const TensorHandle* t) { return t ? t->strides.data() : nullptr; }
+inline b200_dptr ptr_of(const TensorHandle* t) { return t ? t->handle.ptr() : 0; }
+inline bool rank4(ComputeClient& client, const char* what, std::initializer_list<const TensorHandle*> ts) {
+  for (const TensorHandle* t : ts)
+    if (t && t->shape.size() != 4) {
+      client.defer(std::string("InvalidArgument: ") + what + " needs 4-D [B, S, H, D] views");
+      return false;
+    }
+  return true;
+}
+/// Rotate q and / or k by the table rows at `positions` (inverse in args: the backward).
+inline void apply(ComputeClient& client, const Args& args, const TensorHandle& cos_sin, const TensorHandle* q, const TensorHandle* k,
+                  b200_dptr positions = 0, const TensorHandle* q_out = nullptr, const TensorHandle* k_out = nullptr) {
+  if (!rank4(client, "rope", {q, k, q_out, k_out})) return;
+  const TensorHandle* ref = q ? q : k;
+  const int rc = b200_rope(client.raw(), nullptr, &args, static_cast<b200_dtype>(ref ? ref->dtype : DType::F32), ptr_of(q), shape_of(q),
+                           strides_of(q), ptr_of(k), shape_of(k), strides_of(k), ptr_of(q_out), shape_of(q_out), strides_of(q_out),
+                           ptr_of(k_out), shape_of(k_out), strides_of(k_out), positions, cos_sin.handle.ptr(),
+                           cos_sin.shape.empty() ? 0 : cos_sin.shape[0]);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+/// One launch: q rotated (in place or into q_out), k_new rotated and v_new written to their cache slots; bit for bit apply()
+/// then kvcache_write (or the fp8 write with k_scale / v_scale, when the caches are fp8).
+inline void kvcache_write(ComputeClient& client, const Args& args, const TensorHandle& cos_sin, const TensorHandle* q,
+                          const TensorHandle& k_new, const TensorHandle& v_new, const TensorHandle& k_cache, const TensorHandle& v_cache,
+                          const TensorHandle& slot_mapping, b200_dptr positions, const TensorHandle* q_out = nullptr,
+                          b200_dptr k_scale = 0, b200_dptr v_scale = 0) {
+  if (!rank4(client, "rope_kvcache_write", {q, q_out, &k_new, &v_new, &k_cache, &v_cache})) return;
+  const int rc = b200_rope_kvcache_write(
+      client.raw(), nullptr, &args, static_cast<b200_dtype>(k_new.dtype), static_cast<b200_dtype>(k_cache.dtype), ptr_of(q), shape_of(q),
+      strides_of(q), ptr_of(q_out), shape_of(q_out), strides_of(q_out), k_new.handle.ptr(), k_new.shape.data(), k_new.strides.data(),
+      v_new.handle.ptr(), v_new.shape.data(), v_new.strides.data(), k_cache.handle.ptr(), k_cache.shape.data(), k_cache.strides.data(),
+      v_cache.handle.ptr(), v_cache.shape.data(), v_cache.strides.data(), slot_mapping.handle.ptr(), positions, cos_sin.handle.ptr(),
+      cos_sin.shape.empty() ? 0 : cos_sin.shape[0], k_scale, v_scale);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+/// Fill cos_sin (compact f32 [P, rot_dim]) with the table of args' rule, in f64.
+inline void cos_sin(ComputeClient& client, const TableArgs& args, const TensorHandle& out) {
+  const int rc = b200_rope_cos_sin(client.raw(), nullptr, &args, out.shape.empty() ? 0 : out.shape[0], out.handle.ptr());
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+}  // namespace rope
+
 namespace norm {
 /// RMSNorm / LayerNorm over the last axis; the contracts are those of b200_norm* in cubecl_b200.h.  Tensors are 2-D [T, n]
 /// with unit column stride; weight, bias, mean, rstd and the gradients of weight and bias are device pointers (0 = absent).

@@ -1031,6 +1031,57 @@ impl Context {
         ))
     }
 
+    /// Rotate `q` [B, S, Hq, D] and / or `k` [B, S, Hk, D] (0 = absent; shapes and strides in elements, null strides =
+    /// compact) by the rows of the f32 table `cos_sin` [p, rot_dim] at `positions` (i32 [B, S], 0 = s), in place or into
+    /// `q_out` / `k_out`.  The contract is `b200_rope`'s in include/cubecl_b200.h.
+    ///
+    /// # Safety
+    /// Every pointer must be 0 where the contract allows it, or a live device allocation of this context large enough for
+    /// its extents and strides; every shape and stride pointer must point at 4 values (or be null where allowed).
+    #[allow(clippy::too_many_arguments)]
+    pub unsafe fn rope(
+        &mut self, stream: b200_stream, args: &sys::b200_rope_args, dtype: DType, q: b200_dptr, q_shape: *const u64,
+        q_strides: *const u64, k: b200_dptr, k_shape: *const u64, k_strides: *const u64, q_out: b200_dptr, qo_shape: *const u64,
+        qo_strides: *const u64, k_out: b200_dptr, ko_shape: *const u64, ko_strides: *const u64, positions: b200_dptr,
+        cos_sin: b200_dptr, p: u64,
+    ) -> Result<(), Error> {
+        check(sys::b200_rope(
+            self.0, stream, args, dtype as c_int, q, q_shape, q_strides, k, k_shape, k_strides, q_out, qo_shape, qo_strides, k_out,
+            ko_shape, ko_strides, positions, cos_sin, p,
+        ))
+    }
+
+    /// The decode / prefill step in one launch: [`Context::rope`] of `q` and `k_new`, with the rotated k and `v_new` written to
+    /// their cache slots, bit for bit `b200_rope` then `b200_kvcache_write(_fp8)`.  See `b200_rope_kvcache_write`.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::rope`].
+    #[allow(clippy::too_many_arguments)]
+    pub unsafe fn rope_kvcache_write(
+        &mut self, stream: b200_stream, args: &sys::b200_rope_args, dtype: DType, cache_dtype: DType, q: b200_dptr,
+        q_shape: *const u64, q_strides: *const u64, q_out: b200_dptr, qo_shape: *const u64, qo_strides: *const u64, k_new: b200_dptr,
+        kn_shape: *const u64, kn_strides: *const u64, v_new: b200_dptr, vn_shape: *const u64, vn_strides: *const u64,
+        k_cache: b200_dptr, kc_shape: *const u64, kc_strides: *const u64, v_cache: b200_dptr, vc_shape: *const u64,
+        vc_strides: *const u64, slot_mapping: b200_dptr, positions: b200_dptr, cos_sin: b200_dptr, p: u64, k_scale: b200_dptr,
+        v_scale: b200_dptr,
+    ) -> Result<(), Error> {
+        check(sys::b200_rope_kvcache_write(
+            self.0, stream, args, dtype as c_int, cache_dtype as c_int, q, q_shape, q_strides, q_out, qo_shape, qo_strides, k_new,
+            kn_shape, kn_strides, v_new, vn_shape, vn_strides, k_cache, kc_shape, kc_strides, v_cache, vc_shape, vc_strides,
+            slot_mapping, positions, cos_sin, p, k_scale, v_scale,
+        ))
+    }
+
+    /// Fill `cos_sin` (compact f32 [p, rot_dim]) with the table of `args`' rule, computed in f64.  See `b200_rope_cos_sin`.
+    ///
+    /// # Safety
+    /// `cos_sin` (and `args.inv_freq` when used) must be live device allocations of this context of the stated sizes.
+    pub unsafe fn rope_cos_sin(
+        &mut self, stream: b200_stream, args: &sys::b200_rope_table_args, p: u64, cos_sin: b200_dptr,
+    ) -> Result<(), Error> {
+        check(sys::b200_rope_cos_sin(self.0, stream, args, p, cos_sin))
+    }
+
     /// Quantize `input` ([..., K], F32 / F16 / BF16, any strides) along its innermost axis under `scheme` into compact
     /// codes [..., K * bits / 8], block scales [..., K / block] and the f32 tensor scale (0 for an absent level); the
     /// contract is `b200_quantize`'s in include/cubecl_b200.h.
