@@ -669,3 +669,30 @@ struct RopeTableParams {
   uint32_t half, kind;
   double base, factor, low_ff, high_ff, orig, ramp_lo, ramp_hi, af;
 };
+
+// ================================================================================================ cross_entropy.cu
+// Softmax cross-entropy over the vocabulary (capi.cpp: b200_cross_entropy, b200_cross_entropy_backward).  Logits are [t, v]
+// with unit column stride; strides are in elements.  A row belongs to a group of nt threads in each of `ranks` CTAs (a
+// cluster in the forward, which merges the row's statistics through distributed shared memory); chunk q of 8 elements goes
+// to thread q % (ranks * nt), rank q / nt % ranks.  nt and ranks depend on v alone:
+//   warp class (v <= kXentWarpMaxV):  nt = 32, ranks = 1, eight rows per CTA;
+//   CTA class:                        nt = 64, 128 or 256 (v <= 2048, 4096, larger), kXentThreads / nt rows per CTA, and
+//                                     ranks = min(kXentMaxRanks, ceil(v / kXentRankV)) CTAs per row (nt = 256 when > 1).
+// Rows are walked grid-stride by at most kXentMaxGrid clusters.  xent_count and xent_total are one CTA of kXentTotalThreads.
+struct XentParams {
+  uint64_t logits, targets, loss, lse, dloss, dlogits;
+  uint64_t count, partials;                    // pooled: the counted rows (u32, MEAN) and a SUM / MEAN forward's row losses
+  uint64_t t, ls, gs;                          // rows; logits and dlogits row strides
+  uint32_t v, nt, ranks, vec, t64, reduction;  // vec: 16-byte access of logits and dlogits; t64: i64 targets
+  int32_t ignore_index;
+  float omega, eps_v, z, z2;                   // rn(1 - eps), rn(eps / v), z, rn(2 z)
+};
+constexpr int kXentThreads = 256;
+constexpr int kXentCtasPerSm = 3;      // forward and backward: at most 80 registers per thread
+constexpr int kXentFusedCtasPerSm = 2; // forward with gradient: at most 128 (it holds the row's statistics through the second pass)
+constexpr int kXentWarpMaxV = 1024;
+constexpr int kXentRankV = 16384;
+constexpr int kXentMaxRanks = 8;
+constexpr int kXentMaxV = 1 << 20;
+constexpr int kXentMaxGrid = 1 << 20;
+constexpr int kXentTotalThreads = 1024;

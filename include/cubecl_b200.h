@@ -646,6 +646,69 @@ typedef struct b200_rope_table_args {
 } b200_rope_table_args;
 int b200_rope_cos_sin(b200_ctx* ctx, b200_stream s, const b200_rope_table_args* args, uint64_t P, b200_dptr cos_sin);
 
+/* ---- softmax cross-entropy over the vocabulary: per-row loss and lse, the logits gradient, and both in one launch -------
+ * logits [t, v] (logits_dtype F32 / BF16 / F16) with unit column stride and a row stride >= v in elements; targets a compact
+ * [t] in target_dtype I32 or I64.  1 <= v <= 2^20 (larger: B200_ERR_UNSUPPORTED), t < 2^31 (B200_ERR_UNSUPPORTED), t = 0 is
+ * a no-op.  rn() is one IEEE f32 rounding to nearest-even; nothing is contracted into an fma; ex2() is ex2.approx.ftz.f32 and
+ * lg2() lg2.approx.ftz.f32, as attention uses them; log2e and ln2 are the f32 roundings of log2(e) and ln(2).
+ * Per row, with x = f32(logits):
+ *   m = max x;  s = S(ex2(rn(rn(x_v - m') * log2e)));  lse = rn(m + rn(lg2(s) * ln2)), the natural-log logsumexp, where the
+ *   terms of s are taken relative to the running max m' of S()'s order (the max of the values summed so far, 0 while it is
+ *   -inf): when a chunk of 8 raises it from m0 to m1, the sum so far is first multiplied once, s = rn(s * ex2(rn(rn(m0 - m1)
+ *   * log2e))); two partial states merge as (max, rn(s_a' + s_b'), rn(sx_a + sx_b)), each s rescaled to the common max the
+ *   same way (not at all when its max is the common max).  sx = S(x) from the same read.
+ *   omega = rn(1 - eps), e = rn(eps / v), z2 = rn(2 * z) (eps = label_smoothing, z = z_loss, all f32);
+ *   loss = rn(lse - rn(omega * x_y)); when e != 0: loss = rn(loss - rn(e * sx)); when z != 0: loss = rn(loss + rn(z *
+ *   rn(lse * lse))).  That is torch's F.cross_entropy(label_smoothing = eps), lse - (1 - eps) x_y - (eps / v) sum x, plus the
+ *   z-loss z lse^2 of PaLM / OLMo.
+ * S() has an order fixed by v alone: the row is cut into 8-element chunks, chunk q going to thread q % (R * T) of a group of T
+ * threads in each of R CTAs (T = 32, 64, 128 for v <= 1024, 2048, 4096, else 256; R = min(8, ceil(v / 16384))); each thread
+ * takes its chunks in order (the values of a chunk in column order), then an xor butterfly over each warp (offsets 16, 8, 4,
+ * 2, 1), the group's warps in order, the CTAs in order (exchanged through distributed shared memory).  So a row's results do
+ * not depend on t, on the row's position, on pointer alignment (the 128-bit and the element-wise path give the same bits) or
+ * on the GPU: every row is batch-invariant and every call bitwise reproducible.  No atomics.
+ * Targets.  A row whose target equals ignore_index gets loss +0 and a dlogits row of +0 and is not counted; its lse is still
+ * written.  A target outside [0, v) that is not ignore_index gives that row a NaN loss and a NaN dlogits row (torch asserts
+ * on the device; the library makes the row loudly wrong instead).
+ * Reductions.  NONE: loss is f32 [t].  SUM: loss is one f32, the row losses added in an order fixed by t alone (thread i of
+ * 1024 adds rows i, i + 1024, ... from +0, then an xor butterfly over each warp, then the warps in order), in a second
+ * one-CTA launch (xent_total) over pooled per-row partials.  MEAN: that sum divided once, rn(sum / f32(count)), by the count
+ * of counted rows, which a one-CTA pre-launch (xent_count) forms on the device (an integer sum, exact in any order); a count
+ * of 0 gives NaN, as in torch.
+ * lse is an optional f32 [t] output of the forward.
+ * Gradient, dloss f32 [t] for NONE and one f32 for SUM and MEAN: g = dloss_r (NONE), dloss (SUM), rn(dloss / f32(count))
+ * (MEAN, the count by the pre-launch).  Per element, with p = ex2(rn(rn(x_v - lse) * log2e)):
+ *   d = p; when z != 0: d = rn(d * rn(1 + rn(z2 * lse))); at v = y: d = rn(d - omega); when e != 0: d = rn(d - e);
+ *   dlogits_v = RNE_grad(rn(g * d)), grad_dtype F32 / BF16 / F16.
+ * Each logit is read once and each gradient written once.  dlogits may be exactly logits (same base, row stride and dtype):
+ * the gradient then overwrites the logits in place and needs no second [t, v] buffer.  Any other overlap is
+ * B200_ERR_INVALID_ARG.
+ * b200_cross_entropy with dlogits (and dloss) writes the gradient in the same launch, bit for bit b200_cross_entropy followed
+ * by b200_cross_entropy_backward: a CTA re-reads its own slice of the row (from L2) once the row's statistics are merged.
+ * It reads the logits from HBM once instead of twice but, as measured (README), it is not yet faster than that pair: the
+ * forward half is not HBM-bound.  b200_cross_entropy_backward also serves callers whose dloss is not known at forward time.
+ * Errors: B200_ERR_INVALID_ARG for a null args, logits, targets or loss pointer (and in the backward lse, dloss or dlogits),
+ * dloss without dlogits or dlogits without dloss, misaligned pointers (to their element size), a stride below v, v = 0, an
+ * unknown dtype or reduction, eps outside [0, 1] or NaN, z < 0, NaN or infinite, a partial overlap of dlogits with logits.
+ * Launches: xent_count (MEAN), then xent_fwd_<x>_<warp|cta> or, with a gradient, xent_fused_<x>_<grad>_<warp|cta>
+ * (clusters of R CTAs for v > 16384; 128-bit access when every base and row is 16-byte aligned and v % 8 == 0), then
+ * xent_total (SUM, MEAN); the backward runs xent_count (MEAN) and xent_bwd_<x>_<grad>_<warp|cta>.  Temporaries come from the
+ * pool; every call is stream-ordered and never synchronises with the host. */
+typedef enum b200_xent_reduction { B200_XENT_NONE = 0, B200_XENT_SUM = 1, B200_XENT_MEAN = 2 } b200_xent_reduction;
+typedef struct b200_xent_args {
+  int32_t reduction;       /* b200_xent_reduction */
+  int32_t ignore_index;    /* rows whose target equals it contribute nothing (torch's default -100) */
+  float label_smoothing;   /* 0 <= eps <= 1, torch's definition */
+  float z_loss;            /* >= 0: adds z_loss * lse^2 per counted row */
+} b200_xent_args;
+int b200_cross_entropy(b200_ctx* ctx, b200_stream s, const b200_xent_args* args, b200_dtype logits_dtype, b200_dtype target_dtype,
+                       uint64_t t, uint64_t v, b200_dptr logits, uint64_t logits_stride, b200_dptr targets, b200_dptr loss,
+                       b200_dptr lse, b200_dptr dloss, b200_dtype grad_dtype, b200_dptr dlogits, uint64_t dlogits_stride);
+int b200_cross_entropy_backward(b200_ctx* ctx, b200_stream s, const b200_xent_args* args, b200_dtype logits_dtype,
+                                b200_dtype target_dtype, b200_dtype grad_dtype, uint64_t t, uint64_t v, b200_dptr logits,
+                                uint64_t logits_stride, b200_dptr targets, b200_dptr lse, b200_dptr dloss, b200_dptr dlogits,
+                                uint64_t dlogits_stride);
+
 /* ---- 2-D convolution (cubek's convolution kernels), an implicit GEMM on the wgmma kernel --------------------------------
  * out[n, oh, ow, co] = act(alpha * sum_{ky, kx, c} x[n, oh*sh - ph + ky*dh, ow*sw - pw + kx*dw, c] * w[co, ky, kx, c] + bias[co]).
  * Input outside x reads as zero; f32 accumulation; the epilogue is b200_epilogue (NULL = none).  x is [N, H, W, C] (NHWC), w is

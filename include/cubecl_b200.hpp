@@ -727,6 +727,32 @@ inline void combine_backward(ComputeClient& client, const TensorHandle& dy, cons
 }
 }  // namespace moe
 
+namespace cross_entropy {
+/// Softmax cross-entropy over the vocabulary; the contracts are those of b200_cross_entropy* in cubecl_b200.h.  logits and
+/// dlogits are 2-D [t, v] with unit column stride (dlogits may be logits itself: in place), targets a compact i32 / i64 [t];
+/// loss (f32 [t] for NONE, one f32 otherwise), lse (f32 [t]) and dloss are device pointers (0 = absent).  Errors are
+/// deferred to client.sync().
+using Args = b200_xent_args;
+/// loss and lse; with dloss and dlogits also the gradient, in the same launch.
+inline void forward(ComputeClient& client, const Args& args, const TensorHandle& logits, const TensorHandle& targets, b200_dptr loss,
+                    b200_dptr lse = 0, b200_dptr dloss = 0, const TensorHandle* dlogits = nullptr) {
+  const int rc = b200_cross_entropy(client.raw(), nullptr, &args, static_cast<b200_dtype>(logits.dtype), static_cast<b200_dtype>(targets.dtype),
+                                    logits.shape[0], logits.shape[1], logits.handle.ptr(), logits.strides[0], targets.handle.ptr(), loss,
+                                    lse, dloss, static_cast<b200_dtype>(dlogits ? dlogits->dtype : logits.dtype),
+                                    dlogits ? dlogits->handle.ptr() : 0, dlogits ? dlogits->strides[0] : logits.shape[1]);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+/// dlogits from the forward's lse and dloss.
+inline void backward(ComputeClient& client, const Args& args, const TensorHandle& logits, const TensorHandle& targets, b200_dptr lse,
+                     b200_dptr dloss, const TensorHandle& dlogits) {
+  const int rc = b200_cross_entropy_backward(client.raw(), nullptr, &args, static_cast<b200_dtype>(logits.dtype),
+                                             static_cast<b200_dtype>(targets.dtype), static_cast<b200_dtype>(dlogits.dtype), logits.shape[0],
+                                             logits.shape[1], logits.handle.ptr(), logits.strides[0], targets.handle.ptr(), lse, dloss,
+                                             dlogits.handle.ptr(), dlogits.strides[0]);
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+}  // namespace cross_entropy
+
 namespace rope {
 /// Rotary position embeddings; the contracts are those of b200_rope* in cubecl_b200.h.  q, k and the outputs are 4-D
 /// [B, S, H, D] views (null: absent; null outputs rotate in place), positions a compact i32 [B, S] and cos_sin a compact f32

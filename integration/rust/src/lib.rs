@@ -1082,6 +1082,42 @@ impl Context {
         check(sys::b200_rope_cos_sin(self.0, stream, args, p, cos_sin))
     }
 
+    /// Softmax cross-entropy of `logits` [t, v] (unit column stride, row stride `logits_stride` in elements) against
+    /// `targets` (i32 / i64 [t]): `loss` (f32 [t] for NONE, one f32 otherwise) and `lse` (f32 [t], 0 = absent); with `dloss`
+    /// and `dlogits` (0 = absent; may be `logits` itself) also the gradient in the same launch.  The contract is
+    /// `b200_cross_entropy`'s in include/cubecl_b200.h.
+    ///
+    /// # Safety
+    /// Every pointer must be 0 where the contract allows it, or a live device allocation of this context large enough for its
+    /// extents and strides.
+    #[allow(clippy::too_many_arguments)]
+    pub unsafe fn cross_entropy(
+        &mut self, stream: b200_stream, args: &sys::b200_xent_args, logits_dtype: DType, target_dtype: DType, t: u64, v: u64,
+        logits: b200_dptr, logits_stride: u64, targets: b200_dptr, loss: b200_dptr, lse: b200_dptr, dloss: b200_dptr,
+        grad_dtype: DType, dlogits: b200_dptr, dlogits_stride: u64,
+    ) -> Result<(), Error> {
+        check(sys::b200_cross_entropy(
+            self.0, stream, args, logits_dtype as c_int, target_dtype as c_int, t, v, logits, logits_stride, targets, loss, lse,
+            dloss, grad_dtype as c_int, dlogits, dlogits_stride,
+        ))
+    }
+
+    /// The logits' gradient from the forward's `lse` and `dloss`; see `b200_cross_entropy_backward`.
+    ///
+    /// # Safety
+    /// Same contract as [`Context::cross_entropy`].
+    #[allow(clippy::too_many_arguments)]
+    pub unsafe fn cross_entropy_backward(
+        &mut self, stream: b200_stream, args: &sys::b200_xent_args, logits_dtype: DType, target_dtype: DType, grad_dtype: DType,
+        t: u64, v: u64, logits: b200_dptr, logits_stride: u64, targets: b200_dptr, lse: b200_dptr, dloss: b200_dptr,
+        dlogits: b200_dptr, dlogits_stride: u64,
+    ) -> Result<(), Error> {
+        check(sys::b200_cross_entropy_backward(
+            self.0, stream, args, logits_dtype as c_int, target_dtype as c_int, grad_dtype as c_int, t, v, logits, logits_stride,
+            targets, lse, dloss, dlogits, dlogits_stride,
+        ))
+    }
+
     /// Quantize `input` ([..., K], F32 / F16 / BF16, any strides) along its innermost axis under `scheme` into compact
     /// codes [..., K * bits / 8], block scales [..., K / block] and the f32 tensor scale (0 for an absent level); the
     /// contract is `b200_quantize`'s in include/cubecl_b200.h.
