@@ -696,3 +696,29 @@ constexpr int kXentMaxRanks = 8;
 constexpr int kXentMaxV = 1 << 20;
 constexpr int kXentMaxGrid = 1 << 20;
 constexpr int kXentTotalThreads = 1024;
+
+// ================================================================================================ sample.cu
+// Token sampling from logits (capi.cpp: b200_sample).  Logits are [b, v] with unit column stride; strides are in elements.
+// A row runs on a cluster of `ranks` CTAs of kSampleThreads (one plain CTA when ranks = 1), ranks = min(kSampleMaxRanks,
+// ceil(v / kSampleRankV)).  Rank r holds the columns [r * slice, min(v, (r + 1) * slice)), slice = ceil(v / ranks) rounded up
+// to a multiple of 8, in dynamic shared memory as f32 (z, then the kept masses), followed by two histogram buffers of
+// kSampleHistWords u32; 8-element chunk c of the slice is loaded by thread c % kSampleThreads.  The radix selects merge their
+// kSampleBins-bin histograms through distributed shared memory.
+// Rows are walked grid-stride by at most kSampleMaxGrid clusters.  The per-row arrays are 0 when the scalar applies.
+struct SampleParams {
+  uint64_t logits, ids;
+  uint64_t temperatures, top_ks, top_ps, min_ps, seeds, offsets;
+  uint64_t seed, offset;
+  uint64_t b, ls;                                   // rows; logits row stride
+  uint32_t v, ranks, slice, vec, ids64, advance;    // vec: 16-byte loads; ids64: i64 ids; advance: offsets[r] += 1
+  float temperature, top_p, min_p;
+  int32_t top_k;
+};
+constexpr int kSampleThreads = 256;
+constexpr int kSampleRankV = 16384;
+constexpr int kSampleMaxRanks = 8;
+constexpr int kSampleMaxV = 1 << 18;
+constexpr int kSampleMaxSlice = kSampleMaxV / kSampleMaxRanks;   // 32768 f32: 128 KB of dynamic shared memory
+constexpr int kSampleBins = 2048;                                // 11-bit radix digits
+constexpr int kSampleHistWords = 3 * kSampleBins;                // one histogram buffer: u32 counts, or a mass in 3 parts
+constexpr int kSampleMaxGrid = 1 << 20;

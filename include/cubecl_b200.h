@@ -709,6 +709,66 @@ int b200_cross_entropy_backward(b200_ctx* ctx, b200_stream s, const b200_xent_ar
                                 uint64_t logits_stride, b200_dptr targets, b200_dptr lse, b200_dptr dloss, b200_dptr dlogits,
                                 uint64_t dlogits_stride);
 
+/* ---- token sampling from logits: temperature, top-k, min-p, top-p and a seeded draw, one launch -------------------------
+ * logits [b, v] (logits_dtype F32 / BF16 / F16) with unit column stride and a row stride >= v in elements; ids a compact [b]
+ * in ids_dtype I32 or I64.  1 <= v <= 2^18 (larger: B200_ERR_UNSUPPORTED), b < 2^31 (B200_ERR_UNSUPPORTED), b = 0 is a
+ * no-op.  Each parameter is the args scalar, or row r's entry of its per-row device array when that pointer is not 0:
+ * temperatures f32 [b], top_ks i32 [b], top_ps f32 [b], min_ps f32 [b], seeds u64 [b], offsets u64 [b].  rn() is one IEEE
+ * f32 rounding to nearest-even, ex2() is ex2.approx.ftz.f32 as attention and cross-entropy use it, log2e the f32 rounding of
+ * log2(e).  Per row r, with x = f32(logits[r]) and T, k, top_p, min_p, seed, offset its parameters:
+ *   1. T = 0 (either sign) is greedy: id = the lowest i with x_i = max x.  Otherwise z_i = rn(x_i / T).
+ *   2. The row is invalid, and id = -1, when T < 0, T is NaN or +inf, top_p is not in (0, 1], min_p is not in [0, 1], any z
+ *      (greedy: any x) is NaN or +inf, or every value is -inf.  The host refuses the same values in the scalars with
+ *      B200_ERR_INVALID_ARG; per-row arrays can only be checked on the device, so a bad entry makes its row loudly wrong.
+ *   3. Top-k, when 1 <= k < v: keep i with z_i >= the k-th largest z, counted with multiplicity; ties at the threshold are all
+ *      kept, and -0 equals +0 (the value threshold of HF's TopKLogitsWarper and vLLM).  k <= 0 or k >= v keeps every i.
+ *   4. m = max z; w_i = ex2(rn(rn(z_i - m) * log2e)); the mass q_i = floor(w_i * 2^40), an exact u64.  Tokens top-k or min-p
+ *      drop have q = 0.  S = the sum of q over the kept set, at most 2^58, so every sum is exact in u64 in any order.  A token
+ *      with w < 2^-40 has q = 0 and is never drawn: at most v * 2^-40 of the mass is lost.
+ *   5. Min-p: keep i with w_i >= min_p (an f32 compare), min_p relative to the most likely token (vLLM, HF's
+ *      MinPLogitsWarper).  It commutes with top-k: both are filters of the same row.
+ *   6. Top-p, over what top-k and min-p kept: P = ceil(top_p * S), exactly (top_p is a 24-bit dyadic number); tau = the
+ *      largest kept mass value with (the kept mass of q_i >= tau) >= P; keep every kept i with q_i >= tau, ties included.
+ *      This is the minimal nucleus; on tie-free rows it is HF's TopPLogitsWarper.  top_p = 1 keeps every q > 0.
+ *   7. Draw: (r0, r1, ., .) = Philox4x32-10 (Random123) with key (lo(seed), hi(seed)) and counter (lo(offset), hi(offset), 0,
+ *      0); R = r0 + 2^32 r1; t = floor(R * S' / 2^64) with S' the mass that survived 6; id = the surviving i whose interval
+ *      [C_i, C_i + q_i) holds t, C_i the surviving mass at indices below i.
+ * The row index is not part of the counter, so a request's token does not depend on its position in the batch: give each
+ * request its own seed (and step its offset).  With advance_offsets != 0 (offsets required), the kernel writes offsets[r] + 1
+ * back after row r, invalid and greedy rows included, so a CUDA-graph decode loop needs no host work per step.
+ * Every decision is an exact integer comparison or one exactly rounded f32 operation, so any reduction order gives the same
+ * id: rows are batch-invariant, view- and alignment-invariant (the 128-bit and the element-wise path give the same ids) and
+ * every call is bitwise reproducible.  Histograms use 32-bit shared-memory integer atomics (order-independent); there are
+ * no global atomics.
+ * Compositions: the logprob of the sampled token under the raw logits is b200_cross_entropy with targets = ids and reduction
+ * NONE (logprob = -loss; -1 ids are rejected there as out-of-range NaN rows).  Greedy decoding agrees with b200_reduce's argmax
+ * on rows with no NaN or +inf.
+ * Kernel: a row is read from HBM once into shared memory, split over a cluster of R = min(8, ceil(v / 16384)) CTAs of 256
+ * threads (one CTA for v <= 16384), z as f32 (128 KB per CTA at v = 2^18) beside two 24 KB histograms; top-k is a
+ * three-pass 11 / 11 / 10-bit radix select over order-preserving keys of z, top-p a four-pass radix select over the masses
+ * (each bin's mass summed exactly in three 32-bit parts), the cluster's histograms merged through distributed shared memory;
+ * the draw takes a rank-order prefix of the CTAs' masses and the CTA holding t scans its slice.  A launch whose temperature
+ * is the scalar 0 runs sample_greedy_<x> (one argmax pass, no shared row); otherwise sample_<x>.  128-bit loads when the
+ * base and every row are 16-byte aligned and v % 8 == 0.  The plan depends on v, the dtype and the alignment, never on b.
+ * One launch, no temporaries, no host synchronisation.
+ * Speed (README): the filtered path is not yet fast.  Each radix pass costs about 16 us per row, because every CTA reads
+ * every rank's whole histogram through distributed shared memory, so top-k 50 + top-p 0.9 takes about 118 us for one
+ * row at v = 128256 (H100 80GB HBM3, 700 W).  That misses the goals of 2x the greedy time and 10x torch's sort-based
+ * pipeline, and FlashInfer's sampler is faster.  Greedy and plain temperature sampling are a single pass.
+ * Errors: B200_ERR_INVALID_ARG for a null args, logits or ids pointer, misaligned pointers (to their element size), a stride
+ * below v, v = 0, an unknown dtype, a bad scalar (above), advance_offsets without offsets. */
+typedef struct b200_sample_args {
+  float temperature;        /* 0: greedy */
+  int32_t top_k;            /* <= 0 or >= v: off */
+  float top_p;              /* in (0, 1]; 1: off */
+  float min_p;              /* in [0, 1]; 0: off */
+  uint64_t seed, offset;    /* Philox key and counter */
+  b200_dptr temperatures, top_ks, top_ps, min_ps, seeds, offsets;   /* per-row arrays; 0: the scalar for every row */
+  int32_t advance_offsets;  /* != 0: offsets[r] += 1 after row r (needs offsets) */
+} b200_sample_args;
+int b200_sample(b200_ctx* ctx, b200_stream s, const b200_sample_args* args, b200_dtype logits_dtype, b200_dtype ids_dtype,
+                uint64_t b, uint64_t v, b200_dptr logits, uint64_t logits_stride, b200_dptr ids);
+
 /* ---- 2-D convolution (cubek's convolution kernels), an implicit GEMM on the wgmma kernel --------------------------------
  * out[n, oh, ow, co] = act(alpha * sum_{ky, kx, c} x[n, oh*sh - ph + ky*dh, ow*sw - pw + kx*dw, c] * w[co, ky, kx, c] + bias[co]).
  * Input outside x reads as zero; f32 accumulation; the epilogue is b200_epilogue (NULL = none).  x is [N, H, W, C] (NHWC), w is

@@ -753,6 +753,18 @@ inline void backward(ComputeClient& client, const Args& args, const TensorHandle
 }
 }  // namespace cross_entropy
 
+namespace sample {
+/// Token sampling from logits; the contract is b200_sample's in cubecl_b200.h.  logits is 2-D [b, v] with unit column
+/// stride, ids a compact i32 / i64 [b]; the per-row arrays of args (0 = the scalar) are device pointers.  Errors are
+/// deferred to client.sync().
+using Args = b200_sample_args;
+inline void sample(ComputeClient& client, const Args& args, const TensorHandle& logits, const TensorHandle& ids) {
+  const int rc = b200_sample(client.raw(), nullptr, &args, static_cast<b200_dtype>(logits.dtype), static_cast<b200_dtype>(ids.dtype),
+                             logits.shape[0], logits.shape[1], logits.handle.ptr(), logits.strides[0], ids.handle.ptr());
+  if (rc != B200_OK) client.defer(b200_last_error());
+}
+}  // namespace sample
+
 namespace rope {
 /// Rotary position embeddings; the contracts are those of b200_rope* in cubecl_b200.h.  q, k and the outputs are 4-D
 /// [B, S, H, D] views (null: absent; null outputs rotate in place), positions a compact i32 [B, S] and cos_sin a compact f32

@@ -1118,6 +1118,21 @@ impl Context {
         ))
     }
 
+    /// Token sampling: `ids` (i32 / i64 [b]) drawn from `logits` [b, v] (unit column stride, row stride `logits_stride` in
+    /// elements) under temperature, top-k, min-p and top-p, from per-row Philox seeds and offsets; -1 for an invalid row.  The
+    /// contract is `b200_sample`'s in include/cubecl_b200.h.
+    ///
+    /// # Safety
+    /// `logits`, `ids` and every non-zero per-row array of `args` must be live device allocations of this context large
+    /// enough for `b` rows.
+    #[allow(clippy::too_many_arguments)]
+    pub unsafe fn sample(
+        &mut self, stream: b200_stream, args: &sys::b200_sample_args, logits_dtype: DType, ids_dtype: DType, b: u64, v: u64,
+        logits: b200_dptr, logits_stride: u64, ids: b200_dptr,
+    ) -> Result<(), Error> {
+        check(sys::b200_sample(self.0, stream, args, logits_dtype as c_int, ids_dtype as c_int, b, v, logits, logits_stride, ids))
+    }
+
     /// Quantize `input` ([..., K], F32 / F16 / BF16, any strides) along its innermost axis under `scheme` into compact
     /// codes [..., K * bits / 8], block scales [..., K / block] and the f32 tensor scale (0 for an absent level); the
     /// contract is `b200_quantize`'s in include/cubecl_b200.h.
